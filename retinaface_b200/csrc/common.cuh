@@ -58,22 +58,52 @@ inline uint32_t fast_div_mul(uint32_t d) { return d <= 1 ? 0u : (uint32_t)((((ui
 __device__ __forceinline__ int fast_div(int n, uint32_t mul) { return mul ? (int)__umulhi((uint32_t)n, mul) : n; }
 __device__ __forceinline__ int fast_floor_div(int n, int d, uint32_t mul) { return n >= 0 ? fast_div(n, mul) : -fast_div(-n + d - 1, mul); }
 
-// ---- depthwise inner product on packed FP16 pairs: acc[i] += x[i] * w[i] with FP16 multiplicands, FP32 addend and result.
-// Both conversions to FP32 are exact and so is the product of two 11-bit significands, so the FFMA rounds once, like a fused
-// FP16 x FP16 + FP32 multiply-add.  The depthwise weights are FP16-rounded, like every other weight of the FP16 engine; the
-// bias stays FP32.
-__device__ __forceinline__ void fhfma2(float &a0, float &a1, uint32_t x2, uint32_t w2) {
-    const float2 x = __half22float2(*reinterpret_cast<const __half2 *>(&x2)), w = __half22float2(*reinterpret_cast<const __half2 *>(&w2));
-    a0 = fmaf(x.x, w.x, a0);
-    a1 = fmaf(x.y, w.y, a1);
+// ---- depthwise 3x3 stencil of the FP16 tensor-core kernels, 8 channels per thread, on an NY x NX block of outputs whose
+// windows overlap (output (oy, ox) reads window row S*oy + ky, column S*ox + kx).  Each FP16 activation of the block's window
+// is converted to FP32 once and feeds every output that reads it; the weights are FP32 values equal to the FP16-rounded
+// depthwise weights (dw_weight_f16), so acc = fmaf(x, w, acc) rounds once, like a fused FP16 x FP16 + FP32 multiply-add.
+// Every output starts from its FP32 bias and takes its taps in the order ky, kx ascending, whatever the block shape: the
+// results do not depend on NY and NX.
+//   base: window pixel (0, 0) of this thread's channel group; row / pix: bytes between window rows / pixels;
+//   w: [9 taps][wstride] FP32 weights, at this thread's channel group
+__device__ __forceinline__ float dw_weight_f16(float w) { return __half2float(__float2half_rn(w)); }
+template <int S, int NY, int NX>
+__device__ __forceinline__ void dw_stencil_block(float (&acc)[NY][NX][8], const unsigned char *base, int row, int pix, const float *w, int wstride) {
+#pragma unroll 1                     // one window row at a time: unrolled, the loads of every row are hoisted and spill
+    for (int ry = 0; ry < S * (NY - 1) + 3; ry++) {
+#pragma unroll
+        for (int cx = 0; cx < S * (NX - 1) + 3; cx++) {
+            const uint4 raw = *reinterpret_cast<const uint4 *>(base + ry * row + cx * pix);
+            const __half2 *h = reinterpret_cast<const __half2 *>(&raw);
+            float x[8];
+#pragma unroll
+            for (int i = 0; i < 4; i++) { const float2 t = __half22float2(h[i]); x[2 * i] = t.x; x[2 * i + 1] = t.y; }
+#pragma unroll
+            for (int oy = 0; oy < NY; oy++) {
+#pragma unroll
+                for (int ox = 0; ox < NX; ox++) {
+                    const int ky = ry - S * oy, kx = cx - S * ox;
+                    if (ky < 0 || ky > 2 || kx < 0 || kx > 2) continue;
+                    const float4 w0 = *reinterpret_cast<const float4 *>(w + (ky * 3 + kx) * wstride), w1 = *reinterpret_cast<const float4 *>(w + (ky * 3 + kx) * wstride + 4);
+                    float *a = acc[oy][ox];
+                    a[0] = fmaf(x[0], w0.x, a[0]); a[1] = fmaf(x[1], w0.y, a[1]); a[2] = fmaf(x[2], w0.z, a[2]); a[3] = fmaf(x[3], w0.w, a[3]);
+                    a[4] = fmaf(x[4], w1.x, a[4]); a[5] = fmaf(x[5], w1.y, a[5]); a[6] = fmaf(x[6], w1.z, a[6]); a[7] = fmaf(x[7], w1.w, a[7]);
+                }
+            }
+        }
+    }
 }
-__device__ __forceinline__ void fhfma8(float (&acc)[8], const uint4 &x, const uint4 &w) {
-    fhfma2(acc[0], acc[1], x.x, w.x); fhfma2(acc[2], acc[3], x.y, w.y); fhfma2(acc[4], acc[5], x.z, w.z); fhfma2(acc[6], acc[7], x.w, w.w);
+// bias in, ReLU and FP16 rounding out (the A operand of the pointwise GEMM)
+__device__ __forceinline__ void dw_bias8(float (&acc)[8], const float *b) {
+    const float4 b0 = *reinterpret_cast<const float4 *>(b), b1 = *reinterpret_cast<const float4 *>(b + 4);
+    acc[0] = b0.x; acc[1] = b0.y; acc[2] = b0.z; acc[3] = b0.w; acc[4] = b1.x; acc[5] = b1.y; acc[6] = b1.z; acc[7] = b1.w;
 }
-__device__ __forceinline__ uint4 pack_half8(const float4 &a, const float4 &b) {
-    const __half2 h0 = __floats2half2_rn(a.x, a.y), h1 = __floats2half2_rn(a.z, a.w), h2 = __floats2half2_rn(b.x, b.y), h3 = __floats2half2_rn(b.z, b.w);
-    return make_uint4(*reinterpret_cast<const uint32_t *>(&h0), *reinterpret_cast<const uint32_t *>(&h1), *reinterpret_cast<const uint32_t *>(&h2),
-                      *reinterpret_cast<const uint32_t *>(&h3));
+__device__ __forceinline__ uint4 dw_relu_h8(float (&acc)[8]) {
+    uint4 v;
+    __half2 *h = reinterpret_cast<__half2 *>(&v);
+#pragma unroll
+    for (int i = 0; i < 4; i++) h[i] = __floats2half2_rn(fmaxf(acc[2 * i], 0.f), fmaxf(acc[2 * i + 1], 0.f));
+    return v;
 }
 
 // ---- programmatic dependent launch (PDL) ------------------------------------------------------

@@ -94,10 +94,10 @@ void launch_tc_dwpw(const TcDwArgs &a_in, int nsplit, cudaStream_t s) {
     dim3 grid((unsigned)((M + a.rows - 1) / a.rows), nsplit);
     const size_t smem = tc_dw_smem_bytes(a);
     switch (tc_n_bucket(a.N)) {
-        case 32: if (a.C >= 64) CK_L(k_tc_dwpw_staged<32, true>, grid, dim3(TC_THREADS), smem, s, a); else CK_L(k_tc_dwpw_staged<32, false>, grid, dim3(TC_THREADS), smem, s, a); break;
-        case 64: if (a.C >= 64) CK_L(k_tc_dwpw_staged<64, true>, grid, dim3(TC_THREADS), smem, s, a); else CK_L(k_tc_dwpw_staged<64, false>, grid, dim3(TC_THREADS), smem, s, a); break;
-        case 128: if (a.C >= 64) CK_L(k_tc_dwpw_staged<128, true>, grid, dim3(TC_THREADS), smem, s, a); else CK_L(k_tc_dwpw_staged<128, false>, grid, dim3(TC_THREADS), smem, s, a); break;
-        default: if (a.C >= 64) CK_L(k_tc_dwpw_staged<256, true>, grid, dim3(TC_THREADS), smem, s, a); else CK_L(k_tc_dwpw_staged<256, false>, grid, dim3(TC_THREADS), smem, s, a); break;
+        case 32: CK_L(k_tc_dwpw_staged<32>, grid, dim3(TC_THREADS), smem, s, a); break;
+        case 64: CK_L(k_tc_dwpw_staged<64>, grid, dim3(TC_THREADS), smem, s, a); break;
+        case 128: CK_L(k_tc_dwpw_staged<128>, grid, dim3(TC_THREADS), smem, s, a); break;
+        default: CK_L(k_tc_dwpw_staged<256>, grid, dim3(TC_THREADS), smem, s, a); break;
     }
 }
 void launch_tc_dwpw_2d(const TcDw2dArgs &a, cudaStream_t s) {
@@ -116,8 +116,7 @@ cudaError_t tc_init() {
 #define RF_TC_ATTR(K_) if ((e = cudaFuncSetAttribute(K_, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT))) return e
     RF_TC_ATTR((k_tc_conv_staged<32, false>)); RF_TC_ATTR((k_tc_conv_staged<64, false>)); RF_TC_ATTR((k_tc_conv_staged<128, false>)); RF_TC_ATTR((k_tc_conv_staged<256, false>));
     RF_TC_ATTR((k_tc_conv_staged<32, true>)); RF_TC_ATTR((k_tc_conv_staged<64, true>)); RF_TC_ATTR((k_tc_conv_staged<128, true>)); RF_TC_ATTR((k_tc_conv_staged<256, true>));
-    RF_TC_ATTR((k_tc_dwpw_staged<32, true>)); RF_TC_ATTR((k_tc_dwpw_staged<64, true>)); RF_TC_ATTR((k_tc_dwpw_staged<128, true>)); RF_TC_ATTR((k_tc_dwpw_staged<256, true>));
-    RF_TC_ATTR((k_tc_dwpw_staged<32, false>)); RF_TC_ATTR((k_tc_dwpw_staged<64, false>)); RF_TC_ATTR((k_tc_dwpw_staged<128, false>)); RF_TC_ATTR((k_tc_dwpw_staged<256, false>));
+    RF_TC_ATTR(k_tc_dwpw_staged<32>); RF_TC_ATTR(k_tc_dwpw_staged<64>); RF_TC_ATTR(k_tc_dwpw_staged<128>); RF_TC_ATTR(k_tc_dwpw_staged<256>);
     RF_TC_ATTR(k_tc_dwpw_2d<32>); RF_TC_ATTR(k_tc_dwpw_2d<64>); RF_TC_ATTR(k_tc_dwpw_2d<128>); RF_TC_ATTR(k_tc_dwpw_2d<256>);
 #undef RF_TC_ATTR
     return cudaSuccess;

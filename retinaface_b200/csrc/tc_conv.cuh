@@ -309,9 +309,7 @@ __global__ void __launch_bounds__(TC_THREADS) k_tc_conv_staged(const TcConvArgs 
     const uint32_t lbo_b = (uint32_t)a.N * 16;
     wg::for_chunks<(NT < 64 ? NT : 64)>(a.N, [&](auto nc, int n0) {
         constexpr int NC = decltype(nc)::value;
-        float d[NC / 2];
-#pragma unroll
-        for (int i = 0; i < NC / 2; i++) d[i] = 0.f;
+        float d[NC / 2];                 // not zeroed: the first MMA runs with scale-d = 0 (see wg::fence)
         wg::fence();
         int acc = 0;
         for (int t = 0; t < a.taps; t++) {
@@ -358,20 +356,17 @@ struct TcDwArgs {
 __host__ __device__ inline uint32_t tc_dw_lbo_a(int rows) { return (uint32_t)rows * 16 + 16; }
 inline size_t tc_dw_smem_bytes(const TcDwArgs &a) {
     return (size_t)((a.C + 7) / 8) * a.Rmax * 16 + (size_t)(a.Kpad / 8) * tc_dw_lbo_a(a.rows) + (size_t)a.Kpad * a.N * 2 +
-           (size_t)a.Rmax * 4 + 128;
+           (size_t)10 * a.C * 4 + (size_t)a.Rmax * 4 + 128;
 }
 
-// WREG: depthwise weights in registers (C >= 64: few threads share a channel group) or in shared memory
-// (small C, thousands of CTAs: registers are better spent on occupancy; all lanes of a warp read the same
-// few addresses, so the shared reads are broadcasts).
-template <int NT, bool WREG>
-__global__ void __launch_bounds__(TC_THREADS, WREG ? 3 : 4) k_tc_dwpw_staged(const TcDwArgs a) {
+// The depthwise weights and biases sit in shared memory as FP32 (all lanes of a warp read the same few addresses, so the reads
+// are broadcasts); a thread computes up to 4 consecutive outputs of one output row (dw_stencil_block).
+template <int NT>
+__global__ void __launch_bounds__(TC_THREADS, 3) k_tc_dwpw_staged(const TcDwArgs a) {
     extern __shared__ __align__(128) unsigned char smem[];
     __shared__ __align__(8) uint64_t bar_b;
     __shared__ int s_cpos[128];          // GEMM row -> staged index of its stencil centre, -1 = no output
     __shared__ float s_bias[256];
-    __shared__ __align__(16) __half s_dwh[WREG ? 8 : 9 * 64];  // !WREG: [tap][C] FP16 weights (C <= 64)
-    __shared__ __align__(16) float s_dwb[WREG ? 4 : 64];       // !WREG: [C] bias
 
     const int tid = threadIdx.x, warp = tid >> 5;
     const int G = a.C >> 3;
@@ -385,7 +380,9 @@ __global__ void __launch_bounds__(TC_THREADS, WREG ? 3 : 4) k_tc_dwpw_staged(con
     unsigned char *sA = smem + (size_t)a.Rmax * pix;
     const uint32_t lbo_a = tc_dw_lbo_a(a.rows);
     unsigned char *sB = sA + (size_t)(a.Kpad / 8) * lbo_a;
-    int *s_off = reinterpret_cast<int *>(sB + (size_t)a.Kpad * a.N * 2);      // staged position -> element offset, -1 = padding
+    float *s_dww = reinterpret_cast<float *>(sB + (size_t)a.Kpad * a.N * 2);  // [tap][C] FP16-rounded depthwise weights as FP32
+    float *s_dwb = s_dww + 9 * a.C;                                             // [C] depthwise bias
+    int *s_off = reinterpret_cast<int *>(s_dwb + a.C);                          // staged position -> element offset, -1 = padding
     const int M = a.nimg * a.OH * a.OW;
     const int m0 = blockIdx.x * a.rows;
     const int mlast = min(m0 + a.rows, M) - 1;
@@ -406,20 +403,8 @@ __global__ void __launch_bounds__(TC_THREADS, WREG ? 3 : 4) k_tc_dwpw_staged(con
     }
     pdl_trigger();
     if (tid < a.N) s_bias[tid] = a.bias[blockIdx.y * a.N + tid];
-    uint4 wreg[WREG ? 9 : 1];            // [tap] 8 packed FP16 depthwise weights of this thread's channel group (fhfma8)
-    float breg[8];                       // its 8 biases
-    if (!WREG) {
-        for (int i = tid; i < 9 * a.C; i += TC_THREADS) s_dwh[i] = __float2half_rn(a.dw_w[i]);
-        for (int i = tid; i < a.C; i += TC_THREADS) s_dwb[i] = a.dw_b[i];
-    } else if (g_own < G) {
-#pragma unroll
-        for (int t = 0; t < (WREG ? 9 : 1); t++) {
-            const float *src = a.dw_w + t * a.C + g_own * 8;
-            wreg[t] = pack_half8(__ldg(reinterpret_cast<const float4 *>(src)), __ldg(reinterpret_cast<const float4 *>(src) + 1));
-        }
-        const float4 b0 = __ldg(reinterpret_cast<const float4 *>(a.dw_b + g_own * 8)), b1 = __ldg(reinterpret_cast<const float4 *>(a.dw_b + g_own * 8) + 1);
-        breg[0] = b0.x; breg[1] = b0.y; breg[2] = b0.z; breg[3] = b0.w; breg[4] = b1.x; breg[5] = b1.y; breg[6] = b1.z; breg[7] = b1.w;
-    }
+    for (int i = tid; i < 9 * a.C; i += TC_THREADS) s_dww[i] = dw_weight_f16(a.dw_w[i]);
+    for (int i = tid; i < a.C; i += TC_THREADS) s_dwb[i] = a.dw_b[i];
     {
         const int lane = tid & 31;
         const int prow0 = fast_floor_div(lo, a.Wp, a.mul_Wp);          // floor
@@ -454,34 +439,41 @@ __global__ void __launch_bounds__(TC_THREADS, WREG ? 3 : 4) k_tc_dwpw_staged(con
     cp_async_wait_all();
     __syncthreads();
     // ---- depthwise stencil from shared memory -> A operand (canonical K-major layout) -------------------
-    // Each thread owns ONE 8-channel group (TC_THREADS % GA == 0) and walks the tile's rows, so its 72
-    // folded depthwise weights + 8 biases live in registers (loaded before pdl_wait, above).
+    // Each thread owns ONE 8-channel group (TC_THREADS % GA == 0) and walks the tile's rows four at a time.  Four consecutive
+    // outputs of one output row have their stencil centres S staged positions apart and share window columns: 3 x (3S + 3)
+    // loads and conversions for 36 taps.  A quad that crosses the end of an output row, of an image or of M takes its rows
+    // one by one (within an output row the centres step by exactly S, across one by more).
     if (g_own < G) {
-        for (int r = tid >> lgGA; r < a.rows; r += TC_THREADS >> lgGA) {
-            const int cp = s_cpos[r];
-            if (cp < 0) continue;            // rows beyond M (last tile): never read back
-            float acc[8];
-            if (WREG) {
+        auto stencil = [&](auto s_) {
+            constexpr int S = decltype(s_)::value;
+            const float *w = s_dww + g_own * 8;
+            const int win = g_own * 16 - (a.Wp + 1) * pix;     // sS + win + centre * pix: window pixel (0, 0)
+            for (int r0 = 4 * (tid >> lgGA); r0 < a.rows; r0 += 4 * (TC_THREADS >> lgGA)) {
+                const int cp0 = s_cpos[r0];
+                if (cp0 < 0) continue;       // rows beyond M (last tile): never read back
+                unsigned char *dst = sA + (size_t)g_own * lbo_a + (size_t)r0 * 16;
+                if (s_cpos[r0 + 3] == cp0 + 3 * S) {
+                    float acc[1][4][8];
+                    dw_bias8(acc[0][0], s_dwb + g_own * 8);
 #pragma unroll
-                for (int i = 0; i < 8; i++) acc[i] = breg[i];
-            } else {
-                const float4 b0 = *reinterpret_cast<const float4 *>(&s_dwb[g_own * 8]), b1 = *reinterpret_cast<const float4 *>(&s_dwb[g_own * 8 + 4]);
-                acc[0] = b0.x; acc[1] = b0.y; acc[2] = b0.z; acc[3] = b0.w; acc[4] = b1.x; acc[5] = b1.y; acc[6] = b1.z; acc[7] = b1.w;
+                    for (int i = 0; i < 8; i++) { acc[0][1][i] = acc[0][0][i]; acc[0][2][i] = acc[0][0][i]; acc[0][3][i] = acc[0][0][i]; }
+                    dw_stencil_block<S, 1, 4>(acc, sS + win + cp0 * pix, a.Wp * pix, pix, w, a.C);
+#pragma unroll
+                    for (int q = 0; q < 4; q++) *reinterpret_cast<uint4 *>(dst + q * 16) = dw_relu_h8(acc[0][q]);
+                } else {
+                    for (int q = 0; q < 4; q++) {
+                        const int cp = s_cpos[r0 + q];
+                        if (cp < 0) continue;
+                        float acc[1][1][8];
+                        dw_bias8(acc[0][0], s_dwb + g_own * 8);
+                        dw_stencil_block<S, 1, 1>(acc, sS + win + cp * pix, a.Wp * pix, pix, w, a.C);
+                        *reinterpret_cast<uint4 *>(dst + q * 16) = dw_relu_h8(acc[0][0]);
+                    }
+                }
             }
-            const unsigned char *base = sS + cp * pix + g_own * 16;
-#pragma unroll
-            for (int t = 0; t < 9; t++) {
-                const int shift = (t / 3 - 1) * a.Wp + (t % 3 - 1);
-                const uint4 x = *reinterpret_cast<const uint4 *>(base + shift * pix);
-                if (WREG) fhfma8(acc, x, wreg[WREG ? t : 0]);
-                else fhfma8(acc, x, *reinterpret_cast<const uint4 *>(&s_dwh[t * a.C + g_own * 8]));
-            }
-#pragma unroll
-            for (int i = 0; i < 8; i++) acc[i] = fmaxf(acc[i], 0.f);
-            Vec8<__half> o;
-            o.from_float(acc);
-            *reinterpret_cast<uint4 *>(sA + (size_t)g_own * lbo_a + (size_t)r * 16) = o.v;
-        }
+        };
+        if (a.S == 1) stencil(std::integral_constant<int, 1>{});
+        else stencil(std::integral_constant<int, 2>{});
     } else {                                  // K padding group of the Cin = 8 layer: zeros
         for (int r = tid >> lgGA; r < a.rows; r += TC_THREADS >> lgGA)
             *reinterpret_cast<uint4 *>(sA + (size_t)g_own * lbo_a + (size_t)r * 16) = make_uint4(0, 0, 0, 0);
@@ -501,14 +493,13 @@ __global__ void __launch_bounds__(TC_THREADS, WREG ? 3 : 4) k_tc_dwpw_staged(con
     const TcOut o{a.out, a.Ntotal, a.Ntotal, 1, nullptr, 0, 0};
     wg::for_chunks<(NT < 64 ? NT : 64)>(a.N, [&](auto nc, int n0) {
         constexpr int NC = decltype(nc)::value;
-        float d[NC / 2];
-#pragma unroll
-        for (int i = 0; i < NC / 2; i++) d[i] = 0.f;
+        float d[NC / 2];                 // not zeroed: the first MMA runs with scale-d = 0 (see wg::fence)
         wg::fence();
-        for (int ks = 0; ks < (a.Kpad >> 4); ks++) {
+        wg::mma_ss<NC>(d, wg::desc(a_addr, lbo_a, 128), wg::desc(b_addr + (uint32_t)n0 * 16u, lbo_b, 128), 0);
+        for (int ks = 1; ks < (a.Kpad >> 4); ks++) {
             const uint64_t ad = wg::desc(a_addr + (uint32_t)(2 * ks) * lbo_a, lbo_a, 128);
             const uint64_t bd = wg::desc(b_addr + (uint32_t)(2 * ks) * lbo_b + (uint32_t)n0 * 16u, lbo_b, 128);
-            wg::mma_ss<NC>(d, ad, bd, ks > 0);
+            wg::mma_ss<NC>(d, ad, bd, 1);
         }
         wg::commit();
         wg::wait<0>();

@@ -242,9 +242,7 @@ __global__ void __launch_bounds__(TC_THREADS) k_tc_conv_staged_i8(const TcConvAr
     const uint32_t lbo_b = (uint32_t)a.N * 16;
     wg::for_chunks<(NT < 64 ? NT : 64)>(a.N, [&](auto nc, int n0) {
         constexpr int NC = decltype(nc)::value;
-        int d[NC / 2];
-#pragma unroll
-        for (int i = 0; i < NC / 2; i++) d[i] = 0;
+        int d[NC / 2];                   // not zeroed: the first MMA runs with scale-d = 0 (see wg::fence)
         wg::fence();
         int acc = 0;
         for (int t = 0; t < a.taps; t++) {
@@ -436,9 +434,7 @@ __global__ void __launch_bounds__(TC_THREADS, 2) k_tc_dwpw_staged_i8(const TcDwA
     const TcOutI8 o{a.out, a.Ntotal, a.Ntotal, 1, nullptr, 0, 0};
     wg::for_chunks<(NT < 64 ? NT : 64)>(a.N, [&](auto nc, int n0) {
         constexpr int NC = decltype(nc)::value;
-        int d[NC / 2];
-#pragma unroll
-        for (int i = 0; i < NC / 2; i++) d[i] = 0;
+        int d[NC / 2];                   // not zeroed: the first MMA runs with scale-d = 0 (see wg::fence)
         wg::fence();
         for (int ks = 0; ks < (GA >> 1); ks++) {
             const uint64_t ad = wg::desc(a_addr + (uint32_t)(2 * ks) * lbo_a, lbo_a, 128);

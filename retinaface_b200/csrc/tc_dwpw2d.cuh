@@ -6,9 +6,8 @@
 // with the accumulator in registers.  What differs is the tile: TH x TW output pixels of ONE image (TH*TW <= 128) instead of
 // 128 consecutive pixels of the linearised map.  On a wide map the 1-D tile stages 128 + 2*(W+3) input positions for 128
 // outputs (2.8x at W = 112); the 2-D tile stages ((TH-1)*S+3) x ((TW-1)*S+3) (1.4x), needs no position table (a staged
-// row is a contiguous run of the NHWC input: the cp.async addresses are affine in the lane), and vertically adjacent
-// outputs sit in one thread: at stride 1 a thread computes two output rows of one column from 4 input rows (12 loads +
-// conversions instead of 18, one set of weight reads).
+// row is a contiguous run of the NHWC input: the cp.async addresses are affine in the lane), and a 2x2 block of adjacent
+// outputs sits in one thread: each staged activation it reads is converted once for all four (dw_stencil_block).
 #pragma once
 #include "tc_conv.cuh"
 
@@ -49,17 +48,17 @@ inline size_t tc_dw2d_smem_bytes(const TcDw2dArgs &a) {
     return (size_t)a.PH * a.PW * a.C * 2 + (size_t)(a.C / 8) * a.lbo_a + (size_t)a.C * a.N * 2 + 128;
 }
 
-// resident CTAs per SM the register allocation aims at (64 registers at 4; wgmma needs more than the 40 of 6); the driver
-// sizes the shared-memory carve-out to match.  The pointwise accumulator is taken in chunks of at most 32 columns.
+// resident CTAs per SM the register allocation aims at (80 registers at 3: the 2x2 output block of the stencil holds 32
+// accumulators, and at 4 -- 64 registers -- it spills).  The pointwise accumulator is taken in chunks of at most 32 columns.
 #ifndef RF_DW2D_OCC
-#define RF_DW2D_OCC 4
+#define RF_DW2D_OCC 3
 #endif
 template <int NT>
 __global__ void __launch_bounds__(TC_THREADS, RF_DW2D_OCC) k_tc_dwpw_2d(const TcDw2dArgs a) {
     extern __shared__ __align__(128) unsigned char smem[];
     __shared__ __align__(8) uint64_t bar_b;
     __shared__ float s_bias[256];
-    __shared__ __align__(16) __half s_dwh[9 * 64];    // [tap][C] folded depthwise weights, FP16 (fhfma8)
+    __shared__ __align__(16) float s_dww[9 * 64];     // [tap][C] folded depthwise weights, FP16-rounded, as FP32 (dw_stencil_block)
     __shared__ __align__(16) float s_dwb[64];         // [C] bias
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -85,7 +84,7 @@ __global__ void __launch_bounds__(TC_THREADS, RF_DW2D_OCC) k_tc_dwpw_2d(const Tc
     }
     pdl_trigger();
     if (tid < a.N) s_bias[tid] = a.bias[tid];
-    for (int i = tid; i < 9 * a.C; i += TC_THREADS) s_dwh[i] = __float2half_rn(a.dw_w[i]);
+    for (int i = tid; i < 9 * a.C; i += TC_THREADS) s_dww[i] = dw_weight_f16(a.dw_w[i]);
     if (tid < a.C) s_dwb[tid] = a.dw_b[tid];
     pdl_wait();
     // ---- stage the (PH x PW) input window: one warp per staged row, lanes over (column, channel group) -- a staged row
@@ -111,62 +110,30 @@ __global__ void __launch_bounds__(TC_THREADS, RF_DW2D_OCC) k_tc_dwpw_2d(const Tc
     cp_async_wait_all();
     __syncthreads();
     // ---- depthwise stencil -> A operand.  GEMM row r = ty * TW + tx ------------------------------------------------------
+    // item = (channel group, 2x2 block of outputs): at stride 1 a 4x4 window feeds 4 outputs (16 conversions for 36 taps), at
+    // stride 2 a 5x5 window (25 for 36).  TH and TW are even.
     const int rows = a.TH * a.TW;
-    if (a.S == 1) {
-        // item = (channel group, column, PAIR of output rows): 4 staged rows feed 2 outputs
-        const int items = (a.TH >> 1) * a.TW << lg;
+    auto stencil = [&](auto s_) {
+        constexpr int S = decltype(s_)::value;
+        const int items = (a.TH >> 1) * (a.TW >> 1) << lg;
         for (int it = tid; it < items; it += TC_THREADS) {
             const int g = it & (G - 1), rest = it >> lg;
-            const int typ = fast_div(rest, a.mul_TW), tx = rest - typ * a.TW;
-            const int ty = typ * 2;
-            float acc0[8], acc1[8];
-            {
-                const float4 b0 = *reinterpret_cast<const float4 *>(&s_dwb[g * 8]), b1 = *reinterpret_cast<const float4 *>(&s_dwb[g * 8 + 4]);
-                acc0[0] = b0.x; acc0[1] = b0.y; acc0[2] = b0.z; acc0[3] = b0.w; acc0[4] = b1.x; acc0[5] = b1.y; acc0[6] = b1.z; acc0[7] = b1.w;
+            const int typ = fast_div(2 * rest, a.mul_TW), ty = 2 * typ, tx = 2 * rest - typ * a.TW;
+            float acc[2][2][8];
+            dw_bias8(acc[0][0], &s_dwb[g * 8]);
 #pragma unroll
-                for (int i = 0; i < 8; i++) acc1[i] = acc0[i];
-            }
-            const unsigned char *base = sS + (ty * PW + tx) * pix + g * 16;
-#pragma unroll 1                     // (uniform branches on ry; keeps the 12 window loads from being hoisted into 48 registers)
-            for (int ry = 0; ry < 4; ry++) {
-#pragma unroll
-                for (int kx = 0; kx < 3; kx++) {
-                    const uint4 x = *reinterpret_cast<const uint4 *>(base + (ry * PW + kx) * pix);
-                    if (ry < 3) fhfma8(acc0, x, *reinterpret_cast<const uint4 *>(&s_dwh[(ry * 3 + kx) * a.C + g * 8]));         // output row ty: kernel row ry
-                    if (ry > 0) fhfma8(acc1, x, *reinterpret_cast<const uint4 *>(&s_dwh[((ry - 1) * 3 + kx) * a.C + g * 8]));   // output row ty + 1: kernel row ry - 1
-                }
-            }
-#pragma unroll
-            for (int i = 0; i < 8; i++) { acc0[i] = fmaxf(acc0[i], 0.f); acc1[i] = fmaxf(acc1[i], 0.f); }
-            Vec8<__half> o0, o1;
-            o0.from_float(acc0);
-            o1.from_float(acc1);
+            for (int i = 0; i < 8; i++) { acc[0][1][i] = acc[0][0][i]; acc[1][0][i] = acc[0][0][i]; acc[1][1][i] = acc[0][0][i]; }
+            dw_stencil_block<S, 2, 2>(acc, sS + (ty * S * PW + tx * S) * pix + g * 16, PW * pix, pix, &s_dww[g * 8], a.C);
             const int r = ty * a.TW + tx;
-            *reinterpret_cast<uint4 *>(sA + (size_t)g * lbo_a + (size_t)r * 16) = o0.v;
-            *reinterpret_cast<uint4 *>(sA + (size_t)g * lbo_a + (size_t)(r + a.TW) * 16) = o1.v;
+            unsigned char *dst = sA + (size_t)g * lbo_a + (size_t)r * 16;
+            *reinterpret_cast<uint4 *>(dst) = dw_relu_h8(acc[0][0]);
+            *reinterpret_cast<uint4 *>(dst + 16) = dw_relu_h8(acc[0][1]);
+            *reinterpret_cast<uint4 *>(dst + a.TW * 16) = dw_relu_h8(acc[1][0]);
+            *reinterpret_cast<uint4 *>(dst + a.TW * 16 + 16) = dw_relu_h8(acc[1][1]);
         }
-    } else {
-        const int items = rows << lg;
-        for (int it = tid; it < items; it += TC_THREADS) {
-            const int g = it & (G - 1), r = it >> lg;
-            const int ty = fast_div(r, a.mul_TW), tx = r - ty * a.TW;
-            float acc[8];
-            {
-                const float4 b0 = *reinterpret_cast<const float4 *>(&s_dwb[g * 8]), b1 = *reinterpret_cast<const float4 *>(&s_dwb[g * 8 + 4]);
-                acc[0] = b0.x; acc[1] = b0.y; acc[2] = b0.z; acc[3] = b0.w; acc[4] = b1.x; acc[5] = b1.y; acc[6] = b1.z; acc[7] = b1.w;
-            }
-            const unsigned char *base = sS + (ty * a.S * PW + tx * a.S) * pix + g * 16;
-#pragma unroll
-            for (int t = 0; t < 9; t++) {
-                fhfma8(acc, *reinterpret_cast<const uint4 *>(base + ((t / 3) * PW + (t % 3)) * pix), *reinterpret_cast<const uint4 *>(&s_dwh[t * a.C + g * 8]));
-            }
-#pragma unroll
-            for (int i = 0; i < 8; i++) acc[i] = fmaxf(acc[i], 0.f);
-            Vec8<__half> o;
-            o.from_float(acc);
-            *reinterpret_cast<uint4 *>(sA + (size_t)g * lbo_a + (size_t)r * 16) = o.v;
-        }
-    }
+    };
+    if (a.S == 1) stencil(std::integral_constant<int, 1>{});
+    else stencil(std::integral_constant<int, 2>{});
     tc::fence_async_smem();
     __syncthreads();
     if (64 * (warp >> 2) >= rows) return;         // the second warpgroup has no GEMM rows
@@ -184,14 +151,13 @@ __global__ void __launch_bounds__(TC_THREADS, RF_DW2D_OCC) k_tc_dwpw_2d(const Tc
     const TcOut o{a.out, a.N, a.N, 1, nullptr, 0, 0};
     wg::for_chunks<(NT < 32 ? NT : 32)>(a.N, [&](auto nc, int n0) {
         constexpr int NC = decltype(nc)::value;
-        float d[NC / 2];
-#pragma unroll
-        for (int i = 0; i < NC / 2; i++) d[i] = 0.f;
+        float d[NC / 2];                 // not zeroed: the first MMA runs with scale-d = 0 (see wg::fence)
         wg::fence();
-        for (int ks = 0; ks < (a.C >> 4); ks++) {
+        wg::mma_ss<NC>(d, wg::desc(a_addr, lbo_a, 128), wg::desc(b_addr + (uint32_t)n0 * 16u, lbo_b, 128), 0);
+        for (int ks = 1; ks < (a.C >> 4); ks++) {
             const uint64_t ad = wg::desc(a_addr + (uint32_t)(2 * ks) * lbo_a, lbo_a, 128);
             const uint64_t bd = wg::desc(b_addr + (uint32_t)(2 * ks) * lbo_b + (uint32_t)n0 * 16u, lbo_b, 128);
-            wg::mma_ss<NC>(d, ad, bd, ks > 0);
+            wg::mma_ss<NC>(d, ad, bd, 1);
         }
         wg::commit();
         wg::wait<0>();

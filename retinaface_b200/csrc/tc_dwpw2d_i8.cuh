@@ -171,9 +171,7 @@ __global__ void __launch_bounds__(TC_THREADS, 3) k_tc_dwpw_2d_i8(const TcDw2dArg
     const TcOutI8 o{a.out, a.N, a.N, 1, nullptr, 0, 0};
     wg::for_chunks<(NT < 64 ? NT : 64)>(a.N, [&](auto nc, int n0) {
         constexpr int NC = decltype(nc)::value;
-        int d[NC / 2];
-#pragma unroll
-        for (int i = 0; i < NC / 2; i++) d[i] = 0;
+        int d[NC / 2];                   // not zeroed: the first MMA runs with scale-d = 0 (see wg::fence)
         wg::fence();
         for (int ks = 0; ks < (GA >> 1); ks++) {
             const uint64_t ad = wg::desc(a_addr + (uint32_t)(2 * ks) * lbo_a, lbo_a, 128);

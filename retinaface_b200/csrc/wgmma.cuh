@@ -26,6 +26,8 @@ __device__ __forceinline__ uint64_t desc_sw(uint32_t addr, uint32_t row) {
     return (uint64_t)((addr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(((8 * row) >> 4) & 0x3FFF) << 32) | (layout << 62);
 }
 
+// Between fence() and wait() nothing but wgmma may write an accumulator register: a zero fill there makes ptxas serialise
+// every MMA of the sequence (C7515).  The first MMA of a sequence runs with scale-d = 0 (acc == 0) instead.
 __device__ __forceinline__ void fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }

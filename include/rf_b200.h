@@ -227,6 +227,43 @@ int rf_detect_views(rf_handle h, const uint8_t *bgr, int width, int height, int 
                     float score_threshold, float nms_threshold, rf_face *out_faces, int *out_count, int32_t *out_view_of,
                     float *out_view_scales);
 
+/* f5 face alignment: detect, then cut one recognition-ready crop per kept face out of the ORIGINAL image, on the GPU.
+ * For each face the least-squares similarity transform M (image -> crop; rotation, uniform scale, translation) from its five
+ * landmarks to `template_xy` is fitted in FP64 (the minimiser of skimage's SimilarityTransform.estimate, which insightface's
+ * norm_crop uses), and the image is warped into the crop bit for bit as
+ * cv2.warpAffine(img, M, (crop_w, crop_h), INTER_LINEAR, BORDER_CONSTANT, 0) does.  Landmarks whose spread is zero give an
+ * all-zero u8 crop and an all-zero M.  Crop layouts:
+ *   RF_CROP_BGR_U8   crop_h x crop_w x 3 u8, HWC BGR (the warpAffine bytes)
+ *   RF_CROP_RGB_F32  3 x crop_h x crop_w float32, planar RGB, (u8 - mean) * (1 / std)  (cv2.dnn.blobFromImages(crops, 1 / std,
+ *                    size, (mean, mean, mean), swapRB = true): the input of an ArcFace recogniser)
+ *   RF_CROP_RGB_F16  the same rounded to float16 */
+#define RF_CROP_BGR_U8  0
+#define RF_CROP_RGB_F32 1
+#define RF_CROP_RGB_F16 2
+typedef struct rf_align_params {
+    int crop_w, crop_h;      /* 0, 0 -> 112 x 112; otherwise each in [8, 512] */
+    float template_xy[10];   /* crop-pixel targets of the 5 landmarks (x0, y0 .. x4, y4); all 0 -> ArcFace 112x112 template */
+    int max_faces;           /* crops per image, best score first; 0 -> every kept face (<= the handle's max_faces) */
+    int format;              /* RF_CROP_BGR_U8 | RF_CROP_RGB_F32 | RF_CROP_RGB_F16 */
+    float mean, std;         /* float formats; 0, 0 -> 127.5, 127.5 */
+} rf_align_params;
+/* Inputs as rf_detect_batch (any size up to max_image, row strides, pinned or pageable).  out_faces [n][max_faces] are in
+ * ORIGINAL IMAGE pixels: every coordinate is rf_detect_batch's times the image's map-back scale, rounded to float.
+ * With A = params->max_faces (or the handle's max_faces when 0): image i has crops j < min(out_counts[i], A) at
+ * out_crops + (i * A + j) * crop bytes (host); later slots are not written.  out_mats (optional, host double [n][A][6]):
+ * each crop's M, row-major 2 x 3.  Every image that is not network-sized needs its own raw device buffer while the crops
+ * are cut: more of them in one call than the handle has (max_batch, capped at 2 GiB of max_image buffers) is
+ * RF_ERR_CAPACITY.  Bad params: RF_ERR_INVALID_ARG.  Blocking. */
+int rf_detect_align_batch(rf_handle h, const uint8_t *const *bgr_images, const int *widths, const int *heights,
+                          const int *row_strides, int n, float score_threshold, float nms_threshold, const rf_align_params *params,
+                          rf_face *out_faces, int *out_counts, void *out_crops, double *out_mats);
+/* rf_detect_batch_device (network-sized device images, the same context rotation and outputs) followed by the crops of every
+ * kept face, written into the caller's DEVICE buffer dev_crops [n][A][crop bytes] (e.g. a recogniser's input tensor) and,
+ * optionally, dev_mats (device double [n][A][6]).  Asynchronous on rf_last_stream(). */
+int rf_detect_align_batch_device(rf_handle h, const uint8_t *dev_bgr, int n, float score_threshold, float nms_threshold,
+                                 const rf_align_params *params, void *dev_crops, double *dev_mats, const rf_det **dev_dets,
+                                 const int32_t **dev_counts);
+
 /* Preprocess parity: replaces imageROIResize8U3C + the OpenCV branch (RetinaFace.cpp:593-647):
  * letter-boxes one host image into a host net_h*net_w*3 u8 BGR buffer using the GPU kernel. */
 int rf_preprocess(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, uint8_t *out_net_sized);

@@ -24,6 +24,7 @@ SOURCES = [
     ("jpeg.cu", []),
     ("postproc.cu", ["-fmad=false"]),
     ("preprocess.cu", ["-fmad=false"]),
+    ("align.cu", ["-fmad=false"]),      # cv::warpAffine's coordinates and the similarity fit: multiply and add, never fused
     ("calibrate.cu", []),
     ("model.cpp", []),
     ("frontend.cpp", []),

@@ -26,12 +26,40 @@ EXPORTS = [
     "rf_submit_batch_allgather", "rf_collect_batch_allgather", "rf_detect_batch_allgather",
     "rf_model_load", "rf_network_config", "rf_cache_status",
     "rf_detect_jpeg_batch", "rf_decode_jpeg", "rf_jpeg_backend",
+    "rf_detect_align_batch", "rf_detect_align_batch_device",
 ]
 COMM_BLOB_BYTES = 128
 
 
 class _View(C.Structure):       # rf_view
     _fields_ = [("shrink", C.c_float), ("flip", C.c_int32)]
+
+
+RF_CROP_BGR_U8, RF_CROP_RGB_F32, RF_CROP_RGB_F16 = 0, 1, 2
+# crop format name -> (RF_CROP_*, element type, channels-last)
+CROP_FORMATS = {"bgr_u8": (RF_CROP_BGR_U8, np.uint8, True), "rgb_f32": (RF_CROP_RGB_F32, np.float32, False),
+                "rgb_f16": (RF_CROP_RGB_F16, np.float16, False)}
+
+
+class AlignParams(C.Structure):  # rf_align_params
+    _fields_ = [("crop_w", C.c_int), ("crop_h", C.c_int), ("template_xy", C.c_float * 10), ("max_faces", C.c_int),
+                ("format", C.c_int), ("mean", C.c_float), ("std", C.c_float)]
+
+
+def align_params(crop=(112, 112), template=None, fmt: str = "bgr_u8", max_faces: int = 0, mean: float = 0.0, std: float = 0.0) -> AlignParams:
+    """rf_align_params.  crop = (width, height); template: 5 (x, y) crop-pixel targets, None -> the ArcFace 112x112 template;
+    mean = std = 0 -> 127.5."""
+    if fmt not in CROP_FORMATS:
+        raise ValueError(f"crop format {fmt!r}: one of {sorted(CROP_FORMATS)}")
+    t = np.zeros(10, np.float32) if template is None else np.asarray(template, np.float32).reshape(10)
+    return AlignParams(int(crop[0]), int(crop[1]), (C.c_float * 10)(*t.tolist()), int(max_faces), CROP_FORMATS[fmt][0], float(mean), float(std))
+
+
+def crop_shape(fmt: str, crop) -> Tuple[tuple, type]:
+    """(shape, dtype) of one crop: (h, w, 3) u8 BGR or (3, h, w) planar RGB."""
+    _, dt, hwc = CROP_FORMATS[fmt]
+    w, h = int(crop[0]) or 112, int(crop[1]) or 112
+    return ((h, w, 3) if hwc else (3, h, w)), dt
 
 
 class RfError(RuntimeError):
@@ -116,6 +144,10 @@ def load_library() -> C.CDLL:
     lib.rf_decode_jpeg.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
     lib.rf_jpeg_backend.restype = C.c_char_p
     lib.rf_jpeg_backend.argtypes = [C.c_void_p]
+    lib.rf_detect_align_batch.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int,
+                                          C.c_float, C.c_float, C.POINTER(AlignParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.rf_detect_align_batch_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_float, C.POINTER(AlignParams), C.c_void_p,
+                                                 C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
     _lib = lib
     return lib
 
@@ -298,6 +330,48 @@ class Engine:
         if want_index:
             return out, [idx[i, :counts[i]].copy() for i in range(n)]
         return out
+
+    def detect_align(self, images: Sequence[np.ndarray], thr: float, nms_thr: float, crop=(112, 112), template=None, fmt: str = "bgr_u8",
+                     max_faces: int = 0, want_mats: bool = False, mean: float = 0.0, std: float = 0.0):
+        """rf_detect_align_batch: u8 BGR HWC images (any size <= max_image; rows may be strided, e.g. a slice of a larger array)
+        -> (faces: list of (k, 15) float32 arrays in ORIGINAL IMAGE pixels, crops: list of (min(k, A), *crop_shape) arrays
+        [, mats: list of (min(k, A), 2, 3) float64 image -> crop matrices]), A = max_faces or the engine's max_faces."""
+        n = len(images)
+        keep = []
+        for im in images:
+            if im.ndim != 3 or im.shape[2] != 3:
+                raise ValueError(f"u8 BGR HWC images expected, got shape {im.shape}")
+            if not (im.dtype == np.uint8 and im.strides[1:] == (3, 1) and im.strides[0] >= 3 * im.shape[1]):
+                im = np.ascontiguousarray(im, dtype=np.uint8)
+            keep.append(im)
+        p = align_params(crop, template, fmt, max_faces, mean, std)
+        A = max_faces or self.max_faces
+        shape, dt = crop_shape(fmt, (p.crop_w, p.crop_h))
+        ptrs = (C.c_void_p * max(n, 1))(*[im.ctypes.data for im in keep])
+        ws = (C.c_int * max(n, 1))(*[im.shape[1] for im in keep])
+        hs = (C.c_int * max(n, 1))(*[im.shape[0] for im in keep])
+        rs = (C.c_int * max(n, 1))(*[im.strides[0] for im in keep])
+        faces = np.empty((n, self.max_faces, FACE_FLOATS), dtype=np.float32)
+        counts = np.zeros(n, dtype=np.int32)
+        crops = np.empty((n, A) + shape, dtype=dt)
+        mats = np.empty((n, A, 2, 3), dtype=np.float64) if want_mats else None
+        self._check(self.lib.rf_detect_align_batch(self.h, ptrs, ws, hs, rs, n, thr, nms_thr, C.byref(p), faces.ctypes.data, counts.ctypes.data,
+                                                   crops.ctypes.data, mats.ctypes.data if want_mats else None))
+        out = ([faces[i, :counts[i]].copy() for i in range(n)], [crops[i, :min(counts[i], A)].copy() for i in range(n)])
+        if want_mats:
+            out += ([mats[i, :min(counts[i], A)].copy() for i in range(n)],)
+        return out
+
+    def detect_align_device(self, n: int, thr: float, nms_thr: float, dev_crops_ptr: int, crop=(112, 112), template=None, fmt: str = "bgr_u8",
+                            max_faces: int = 0, mean: float = 0.0, std: float = 0.0, dev_mats_ptr: Optional[int] = None,
+                            dev_ptr: Optional[int] = None):
+        """rf_detect_align_batch_device: asynchronous; the crops of image i, face j land at dev_crops_ptr + (i * A + j) * crop bytes
+        (device).  Returns the (dets_ptr, counts_ptr) device addresses of rf_detect_batch_device."""
+        p = align_params(crop, template, fmt, max_faces, mean, std)
+        d, c = C.c_void_p(), C.c_void_p()
+        self._check(self.lib.rf_detect_align_batch_device(self.h, dev_ptr if dev_ptr is not None else self.device_input_ptr(), n, thr, nms_thr,
+                                                          C.byref(p), dev_crops_ptr, dev_mats_ptr, C.byref(d), C.byref(c)))
+        return int(d.value), int(c.value)
 
     def detect_jpeg(self, streams: Sequence[bytes], thr: float, nms_thr: float):
         """JPEG bitstreams (bytes) -> decoded on the GPU (nvJPEG), letter-boxed, detected.  Returns (list of (k,15) arrays in

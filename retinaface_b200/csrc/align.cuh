@@ -1,0 +1,43 @@
+// align.cuh -- f5 face alignment: the crops a face recogniser takes, cut from the original images on the GPU.
+//
+// For every kept face of a batch, k_align_faces fits the least-squares similarity transform from the face's five landmarks
+// (in original image pixels) to a template of crop-pixel targets (the ArcFace 112x112 template by default), and warps the
+// ORIGINAL image into the crop exactly the way cv2.warpAffine(img, M, (cw, ch), INTER_LINEAR, BORDER_CONSTANT, 0) does
+// (OpenCV's fixed point: 1/1024-pixel coordinates, 1/32-pixel bilinear phases, integer weights).  The crop is stored as
+// u8 BGR HWC, or as planar RGB float32 / float16 (u8 - mean) * (1 / std), the input of an ArcFace-style recogniser.
+#pragma once
+#include "common.cuh"
+#include "postproc.cuh"
+
+namespace rf {
+
+// One source image of the batch: u8 BGR HWC rows of row_bytes, and the factor that maps network-input coordinates to its
+// pixels (the float letterbox_fill returns; 1 for network-sized images).
+struct AlignImage {
+    const uint8_t *src;
+    int w, h, row_bytes;
+    float scale;
+};
+
+struct AlignArgs {
+    const AlignImage *images;   // device [n]; NULL: image i is uniform_base + i * uniform_bytes, net-sized, packed, scale 1
+    const uint8_t *uniform_base;
+    size_t uniform_bytes;
+    int uniform_w, uniform_h;
+    int n, max_align;           // slots per image: crop j of image i is slot i * max_align + j, j < min(count_i, max_align)
+    int crop_w, crop_h, format; // RF_CROP_*
+    float mean, inv_std;
+    double tmpl[10];            // template points (x0, y0 .. x4, y4), crop pixels
+    size_t crop_bytes;          // align_crop_bytes(crop_w, crop_h, format)
+    void *crops;                // [n][max_align][crop bytes]
+    double *mats;               // optional [n][max_align][6]: M, image -> crop
+};
+
+constexpr int ALIGN_MIN_SIDE = 8, ALIGN_MAX_SIDE = 512;
+
+size_t align_crop_bytes(int crop_w, int crop_h, int format);
+// One launch, the grid sized from the SM count: kept counts and landmarks are read from pb on the device, and only the crops
+// that exist are cut.  n <= max_batch (<= 4096: the per-image scan lives in 4 n bytes of shared memory).
+cudaError_t launch_align_faces(const AlignArgs &a, const PostBuffers &pb, int num_sms, cudaStream_t s);
+
+}  // namespace rf

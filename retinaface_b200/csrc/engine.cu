@@ -4,6 +4,8 @@
 // Replaces the reference's engine slot: TrtNetBase / TrtRetinaFaceNet
 // (retinaface/tensorrt/trtnetbase.cpp:199-330, trtretinafacenet.cpp:48-210) and the detect
 // orchestration of RetinaFace::detect / detectBatchImages (retinaface/RetinaFace.cpp:576-940).
+#include <cmath>
+
 #include "engine_internal.cuh"
 #include "calibrate.cuh"
 #include "preprocess.cuh"
@@ -176,6 +178,7 @@ void destroy(rf_handle h) {
     for (auto p : h->d_blobs) cudaFree(p);
     h->copy_pool.reset();
     for (auto e : h->raw_ev) if (e) cudaEventDestroy(e);
+    cudaFree(h->d_align_images); cudaFreeHost(h->h_align_images); cudaFree(h->d_align_crops); cudaFree(h->d_align_mats);
     cudaFreeHost(h->h_input); cudaFreeHost(h->h_raw); cudaFreeHost(h->h_dets); cudaFreeHost(h->h_counts); cudaFreeHost(h->tile_dbg);
     for (auto &sl : h->slots) {
         cudaFree(sl.d_in); cudaFreeHost(sl.h_in); cudaFreeHost(sl.h_dets); cudaFreeHost(sl.h_counts);
@@ -525,74 +528,204 @@ static uint8_t *upload_raw(rf_handle h, const uint8_t *src, int width, int heigh
     return d_dst;
 }
 
+// The n caller images of rf_detect_batch -> the input tensor, on the handle's stream.  With `originals`
+// (rf_detect_align_batch, which has checked that every image that is not network-sized gets a raw buffer of its own),
+// originals[i] records where image i's own pixels stay resident and its map-back scale.
+static int stage_images(rf_handle h, const char *who, const uint8_t *const *imgs, const int *widths, const int *heights,
+                        const int *row_strides, int n, AlignImage *originals) {
+    const int Hn = h->cfg.net_h, Wn = h->cfg.net_w;
+    const size_t img_bytes = (size_t)Hn * Wn * 3;
+    // Network-sized packed images are copied H2D straight from the caller's memory when it is
+    // pinned (cudaHostAlloc / cudaHostRegister / the library's own rf_pinned_input), otherwise via the
+    // library's pinned mirror; runs of adjacent sources collapse into one copy.  Other sizes are
+    // letter-boxed on the GPU one by one (preprocess.cuh).
+    const uint8_t *run_src = nullptr;
+    int run_start = -1, run_len = 0;
+    auto flush = [&]() {
+        if (run_start < 0) return;
+        CK(cudaMemcpyAsync(h->d_input + (size_t)run_start * img_bytes, run_src, (size_t)run_len * img_bytes,
+                           cudaMemcpyHostToDevice, h->stream));
+        run_start = -1;
+    };
+    bool staging_dirty = false;
+    // other sizes: uploaded into per-image raw buffers, then ONE letter-box launch for all of them (RF_FLAG_NPP_RESIZE: the
+    // reference's NPP super-sampling definition instead of its OpenCV bilinear one)
+    const int area = (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0;
+    std::vector<LbItem> lb;
+    auto flush_lb = [&]() {
+        if (lb.empty()) return;
+        CK(launch_letterbox_batch(lb.data(), (int)lb.size(), Wn, Hn, h->stream));
+        lb.clear();
+    };
+    for (int i = 0; i < n; i++) {
+        if (!imgs[i] || widths[i] <= 0 || heights[i] <= 0) { return fail(h, RF_ERR_INVALID_ARG, fmt("%s: image %d is empty", who, i)); }
+        const int rs = row_strides && row_strides[i] ? row_strides[i] : widths[i] * 3;
+        if (widths[i] == Wn && heights[i] == Hn && rs == Wn * 3) {
+            const uint8_t *src = imgs[i];
+            const bool in_mirror = src >= h->h_input && src < h->h_input + (size_t)h->cfg.max_batch * img_bytes;
+            if (!in_mirror) {
+                cudaPointerAttributes at{};
+                bool pinned = cudaPointerGetAttributes(&at, src) == cudaSuccess && at.type == cudaMemoryTypeHost;
+                if (!pinned) {
+                    cudaGetLastError();
+                    if (!staging_dirty) { CK(cudaStreamSynchronize(h->stream)); staging_dirty = true; }
+                    uint8_t *slot = h->h_input + (size_t)i * img_bytes;
+                    memcpy(slot, src, img_bytes);
+                    src = slot;
+                }
+            }
+            if (run_start >= 0 && src == run_src + (size_t)run_len * img_bytes) { run_len++; }
+            else { flush(); run_start = i; run_src = src; run_len = 1; }
+            if (originals) originals[i] = AlignImage{h->d_input + (size_t)i * img_bytes, Wn, Hn, Wn * 3, 1.f};
+        } else {
+            flush();
+            if (widths[i] > h->cfg.max_image_w || heights[i] > h->cfg.max_image_h)
+                return fail(h, RF_ERR_CAPACITY, fmt("image %d is %dx%d, larger than max_image %dx%d", i, widths[i], heights[i],
+                                                    h->cfg.max_image_w, h->cfg.max_image_h));
+            if ((int)lb.size() == h->raw_slots) flush_lb();
+            const uint8_t *d_src = upload_raw(h, imgs[i], widths[i], heights[i], rs, (int)lb.size());
+            lb.emplace_back();
+            const float scale = letterbox_fill(lb.back(), d_src, widths[i], heights[i], h->d_input + (size_t)i * img_bytes, Wn, Hn, 0, area);
+            if (originals) originals[i] = AlignImage{d_src, widths[i], heights[i], widths[i] * 3, scale};
+        }
+    }
+    flush();
+    flush_lb();
+    return RF_OK;
+}
+
 int rf_detect_batch(rf_handle h, const uint8_t *const *imgs, const int *widths, const int *heights, const int *row_strides,
                     int n, float thr, float nms, rf_face *out_faces, int *out_counts, int32_t *out_idx) {
     int rc = check_n(h, n);
     if (rc) return rc;
     if (n == 0) return RF_OK;
     if (!imgs || !widths || !heights) return fail(h, RF_ERR_INVALID_ARG, "rf_detect_batch: NULL image arrays");
-    const int Hn = h->cfg.net_h, Wn = h->cfg.net_w;
-    const size_t img_bytes = (size_t)Hn * Wn * 3;
     try {
         CK(cudaSetDevice(h->device));
         switch_ctx(h, 0);
-        // Network-sized packed images are copied H2D straight from the caller's memory when it is
-        // pinned (cudaHostAlloc / cudaHostRegister / the library's own rf_pinned_input), otherwise via the
-        // library's pinned mirror; runs of adjacent sources collapse into one copy.  Other sizes are
-        // letter-boxed on the GPU one by one (preprocess.cuh).
-        const uint8_t *run_src = nullptr;
-        int run_start = -1, run_len = 0;
-        auto flush = [&]() {
-            if (run_start < 0) return;
-            CK(cudaMemcpyAsync(h->d_input + (size_t)run_start * img_bytes, run_src, (size_t)run_len * img_bytes,
-                               cudaMemcpyHostToDevice, h->stream));
-            run_start = -1;
-        };
-        bool staging_dirty = false;
-        // other sizes: uploaded into per-image raw buffers, then ONE letter-box launch for all of them (RF_FLAG_NPP_RESIZE: the
-        // reference's NPP super-sampling definition instead of its OpenCV bilinear one)
-        const int area = (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0;
-        std::vector<LbItem> lb;
-        auto flush_lb = [&]() {
-            if (lb.empty()) return;
-            CK(launch_letterbox_batch(lb.data(), (int)lb.size(), Wn, Hn, h->stream));
-            lb.clear();
-        };
-        for (int i = 0; i < n; i++) {
-            if (!imgs[i] || widths[i] <= 0 || heights[i] <= 0) { return fail(h, RF_ERR_INVALID_ARG, fmt("rf_detect_batch: image %d is empty", i)); }
-            const int rs = row_strides && row_strides[i] ? row_strides[i] : widths[i] * 3;
-            if (widths[i] == Wn && heights[i] == Hn && rs == Wn * 3) {
-                const uint8_t *src = imgs[i];
-                const bool in_mirror = src >= h->h_input && src < h->h_input + (size_t)h->cfg.max_batch * img_bytes;
-                if (!in_mirror) {
-                    cudaPointerAttributes at{};
-                    bool pinned = cudaPointerGetAttributes(&at, src) == cudaSuccess && at.type == cudaMemoryTypeHost;
-                    if (!pinned) {
-                        cudaGetLastError();
-                        if (!staging_dirty) { CK(cudaStreamSynchronize(h->stream)); staging_dirty = true; }
-                        uint8_t *slot = h->h_input + (size_t)i * img_bytes;
-                        memcpy(slot, src, img_bytes);
-                        src = slot;
-                    }
-                }
-                if (run_start >= 0 && src == run_src + (size_t)run_len * img_bytes) { run_len++; }
-                else { flush(); run_start = i; run_src = src; run_len = 1; }
-            } else {
-                flush();
-                if (widths[i] > h->cfg.max_image_w || heights[i] > h->cfg.max_image_h)
-                    return fail(h, RF_ERR_CAPACITY, fmt("image %d is %dx%d, larger than max_image %dx%d", i, widths[i], heights[i],
-                                                        h->cfg.max_image_w, h->cfg.max_image_h));
-                if ((int)lb.size() == h->raw_slots) flush_lb();
-                const uint8_t *d_src = upload_raw(h, imgs[i], widths[i], heights[i], rs, (int)lb.size());
-                lb.emplace_back();
-                letterbox_fill(lb.back(), d_src, widths[i], heights[i], h->d_input + (size_t)i * img_bytes, Wn, Hn, 0, area);
-            }
-        }
-        flush();
-        flush_lb();
+        if ((rc = stage_images(h, "rf_detect_batch", imgs, widths, heights, row_strides, n, nullptr))) return rc;
         set_params(h, thr, nms);
         forward_graph(h, n);
         fetch_results(h, n, out_faces, out_counts, out_idx, nullptr);
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
+}
+
+// ---- f5 face alignment (align.cuh) ----------------------------------------------------------------------------------------------
+// Checks the caller's rf_align_params and fills the image-independent kernel arguments (defaults applied).
+static int align_setup(rf_handle h, const char *who, const rf_align_params *p, AlignArgs &a) {
+    if (!p) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: params is NULL", who));
+    a = AlignArgs{};
+    a.crop_w = p->crop_w; a.crop_h = p->crop_h;
+    if (a.crop_w == 0 && a.crop_h == 0) a.crop_w = a.crop_h = 112;
+    if (a.crop_w < ALIGN_MIN_SIDE || a.crop_w > ALIGN_MAX_SIDE || a.crop_h < ALIGN_MIN_SIDE || a.crop_h > ALIGN_MAX_SIDE)
+        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: crop %dx%d, each side must be in [%d, %d]", who, p->crop_w, p->crop_h, ALIGN_MIN_SIDE, ALIGN_MAX_SIDE));
+    if (p->format != RF_CROP_BGR_U8 && p->format != RF_CROP_RGB_F32 && p->format != RF_CROP_RGB_F16)
+        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: unknown crop format %d", who, p->format));
+    if (p->max_faces < 0 || p->max_faces > h->cfg.max_faces)
+        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: max_faces %d, must be in [0, %d] (the handle's max_faces)", who, p->max_faces, h->cfg.max_faces));
+    float mean = p->mean, sd = p->std;
+    if (mean == 0.f && sd == 0.f) mean = sd = 127.5f;
+    if (sd == 0.f || !std::isfinite(sd) || !std::isfinite(mean)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: std must be finite and non-zero", who));
+    // insightface's arcface_dst: left eye, right eye, nose, left and right mouth corner in a 112 x 112 crop
+    static const float arcface[10] = {38.2946f, 51.6963f, 73.5318f, 51.5014f, 56.0252f, 71.7366f, 41.5493f, 92.3655f, 70.7299f, 92.2041f};
+    bool given = false;
+    for (int k = 0; k < 10; k++) given |= p->template_xy[k] != 0.f;
+    for (int k = 0; k < 10; k++) a.tmpl[k] = (double)(given ? p->template_xy[k] : arcface[k]);
+    a.max_align = p->max_faces ? p->max_faces : h->cfg.max_faces;
+    a.format = p->format;
+    a.mean = mean;
+    a.inv_std = (float)(1.0 / (double)sd);
+    a.crop_bytes = align_crop_bytes(a.crop_w, a.crop_h, a.format);
+    return RF_OK;
+}
+
+int rf_detect_align_batch(rf_handle h, const uint8_t *const *imgs, const int *widths, const int *heights, const int *row_strides,
+                          int n, float thr, float nms, const rf_align_params *params, rf_face *out_faces, int *out_counts,
+                          void *out_crops, double *out_mats) {
+    int rc = check_n(h, n);
+    if (rc) return rc;
+    AlignArgs a;
+    if ((rc = align_setup(h, "rf_detect_align_batch", params, a))) return rc;
+    if (n == 0) return RF_OK;
+    if (!imgs || !widths || !heights || !out_crops) return fail(h, RF_ERR_INVALID_ARG, "rf_detect_align_batch: NULL image arrays or out_crops");
+    const int Hn = h->cfg.net_h, Wn = h->cfg.net_w, mf = h->cfg.max_faces;
+    // the kernel samples every original after the forward: no raw buffer may be recycled within the call
+    int raw = 0;
+    for (int i = 0; i < n; i++) {
+        const int rs = row_strides && row_strides[i] ? row_strides[i] : widths[i] * 3;
+        raw += !(widths[i] == Wn && heights[i] == Hn && rs == Wn * 3);
+    }
+    if (raw > h->raw_slots)
+        return fail(h, RF_ERR_CAPACITY, fmt("rf_detect_align_batch: %d images are not %dx%d packed, but the handle keeps at most %d such originals "
+                                            "resident (one %dx%d raw buffer each); split the batch", raw, Wn, Hn, h->raw_slots,
+                                            h->cfg.max_image_w, h->cfg.max_image_h));
+    try {
+        CK(cudaSetDevice(h->device));
+        switch_ctx(h, 0);
+        if (!h->d_align_images) {
+            CK(cudaMalloc(&h->d_align_images, sizeof(AlignImage) * h->cfg.max_batch));
+            CK(cudaHostAlloc(&h->h_align_images, sizeof(AlignImage) * h->cfg.max_batch, cudaHostAllocDefault));
+            CK(cudaMalloc(&h->d_align_mats, sizeof(double) * 6 * h->cfg.max_batch * mf));
+        }
+        const size_t need = (size_t)n * a.max_align * a.crop_bytes;
+        if (need > h->align_crops_bytes) {
+            CK(cudaFree(h->d_align_crops));
+            h->d_align_crops = nullptr;
+            h->align_crops_bytes = 0;
+            CK(cudaMalloc(&h->d_align_crops, need));
+            h->align_crops_bytes = need;
+        }
+        if ((rc = stage_images(h, "rf_detect_align_batch", imgs, widths, heights, row_strides, n, h->h_align_images))) return rc;
+        CK(cudaMemcpyAsync(h->d_align_images, h->h_align_images, sizeof(AlignImage) * n, cudaMemcpyHostToDevice, h->stream));
+        set_params(h, thr, nms);
+        forward_graph(h, n);
+        a.images = h->d_align_images;
+        a.n = n;
+        a.crops = h->d_align_crops;
+        a.mats = out_mats ? h->d_align_mats : nullptr;
+        CK(launch_align_faces(a, h->pb, h->num_sms, h->stream));
+        fetch_results(h, n, nullptr, out_counts, nullptr, nullptr);
+        for (int i = 0; i < n; i++) {
+            const int k = h->h_counts[i];
+            const float s = h->h_align_images[i].scale;
+            for (int j = 0; out_faces && j < k; j++) {
+                rf_face f = h->h_dets[(size_t)i * mf + j].face;      // network-input pixels -> image pixels (k_merge_views' map-back)
+                f.x1 *= s; f.y1 *= s; f.x2 *= s; f.y2 *= s;
+                for (int l = 0; l < 5; l++) { f.lx[l] *= s; f.ly[l] *= s; }
+                out_faces[(size_t)i * mf + j] = f;
+            }
+            const size_t first = (size_t)i * a.max_align, m = (size_t)std::min(k, a.max_align);
+            if (!m) continue;
+            CK(cudaMemcpyAsync(static_cast<uint8_t *>(out_crops) + first * a.crop_bytes, static_cast<uint8_t *>(h->d_align_crops) + first * a.crop_bytes,
+                               m * a.crop_bytes, cudaMemcpyDeviceToHost, h->stream));
+            if (out_mats)
+                CK(cudaMemcpyAsync(out_mats + first * 6, h->d_align_mats + first * 6, m * 6 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+        }
+        CK(cudaStreamSynchronize(h->stream));
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
+}
+
+int rf_detect_align_batch_device(rf_handle h, const uint8_t *dev_bgr, int n, float thr, float nms, const rf_align_params *params,
+                                 void *dev_crops, double *dev_mats, const rf_det **dev_dets, const int32_t **dev_counts) {
+    if (!h) return RF_ERR_INVALID_ARG;
+    AlignArgs a;
+    int rc = align_setup(h, "rf_detect_align_batch_device", params, a);
+    if (rc) return rc;
+    if (n > 0 && !dev_crops) return fail(h, RF_ERR_INVALID_ARG, "rf_detect_align_batch_device: dev_crops is NULL");
+    if ((rc = detect_device_impl(h, dev_bgr, n, thr, nms, dev_dets, dev_counts, false))) return rc;
+    if (n == 0) return RF_OK;
+    // detect_device_impl left the context it ran on active: its stream, its results
+    a.uniform_base = dev_bgr ? dev_bgr : h->d_input;
+    a.uniform_bytes = (size_t)h->cfg.net_h * h->cfg.net_w * 3;
+    a.uniform_w = h->cfg.net_w;
+    a.uniform_h = h->cfg.net_h;
+    a.n = n;
+    a.crops = dev_crops;
+    a.mats = dev_mats;
+    try {
+        CK(launch_align_faces(a, h->pb, h->num_sms, h->stream));
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }

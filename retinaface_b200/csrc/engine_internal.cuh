@@ -15,6 +15,7 @@
 #include <type_traits>
 #include <vector>
 
+#include "align.cuh"
 #include "common.cuh"
 #include "host_copy.h"
 #include "model.h"
@@ -137,6 +138,12 @@ struct rf_handle_s {
     cudaEvent_t raw_ev[2] = {nullptr, nullptr};   // H2D out of staging buffer i has completed
     unsigned raw_seq = 0;
     std::unique_ptr<HostCopyPool> copy_pool;      // row-band parallel host copy into the staging buffers (lazily created)
+    // rf_detect_align_batch (lazily allocated): where each image's original pixels are resident, the crops (grown on
+    // demand) and the matrices [max_batch][max_faces][6]
+    AlignImage *d_align_images = nullptr, *h_align_images = nullptr;
+    void *d_align_crops = nullptr;
+    size_t align_crops_bytes = 0;
+    double *d_align_mats = nullptr;
     PostParams *d_params = nullptr, *h_params = nullptr;
     PostBuffers pb{};
     LevelDesc lv[3];

@@ -52,6 +52,14 @@ class RetinaFace:
         rows = self.engine.detect_batch(list(imgs), threshold, self.nms_threshold)
         return [[FaceDetectInfo.from_row(r) for r in per] for per in rows]
 
+    def detectAndAlign(self, imgs: Sequence[np.ndarray], threshold: float = 0.5, **align) -> List[List[tuple]]:
+        """Face alignment on the GPU (f5): per image, a list of ``(FaceDetectInfo, crop)`` -- the face in ORIGINAL IMAGE pixels and
+        its crop warped from the original image onto a landmark template (``Engine.detect_align``'s keyword arguments: crop,
+        template, fmt, max_faces, mean, std; by default 112x112 u8 BGR on the ArcFace template).  With ``max_faces`` only the
+        best-scoring faces of each image are returned."""
+        faces, crops = self.engine.detect_align(list(imgs), threshold, self.nms_threshold, **align)
+        return [[(FaceDetectInfo.from_row(r), c) for r, c in zip(f, cs)] for f, cs in zip(faces, crops)]
+
     def detectInImage(self, img: np.ndarray, threshold: float = 0.5, scales: Sequence[float] = (1.0,), flip: bool = False
                       ) -> List[FaceDetectInfo]:
         """SURVEY.md 8f-2: what the reference leaves commented out / unused (RetinaFace.cpp:730-746, the `scales` argument of

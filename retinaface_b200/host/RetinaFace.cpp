@@ -2,6 +2,7 @@
 #include "RetinaFace.h"
 
 #include <cmath>
+#include <cstring>
 
 #include <stdexcept>
 
@@ -92,6 +93,47 @@ void RetinaFace::detectBatchImages(vector<cv::Mat> imgs, float threshold) {
         for (int i = 0; i < n; i++) {
             const FaceDetectInfo *f = reinterpret_cast<const FaceDetectInfo *>(out_faces_.data() + (size_t)i * opt_.max_faces);
             last_[start + i].assign(f, f + out_counts_[i]);
+        }
+    }
+}
+
+void RetinaFace::detectAndAlign(vector<cv::Mat> imgs, float threshold, const AlignOptions &align) {
+    last_.assign(imgs.size(), vector<FaceDetectInfo>());
+    scales_.assign(imgs.size(), 1.f);
+    crops_.assign(imgs.size(), vector<Mat>());
+    rf_align_params p{};
+    p.crop_w = align.crop_w;
+    p.crop_h = align.crop_h;
+    for (int k = 0; k < 10; k++) p.template_xy[k] = align.template_xy[k];
+    p.max_faces = align.max_faces;
+    p.format = RF_CROP_BGR_U8;
+    const int per = align.max_faces > 0 ? align.max_faces : opt_.max_faces;
+    const bool dflt = align.crop_w == 0 && align.crop_h == 0;    // rf_align_params: 0 x 0 -> 112 x 112
+    const int cw = dflt ? 112 : align.crop_w, ch = dflt ? 112 : align.crop_h;
+    const size_t crop_bytes = (size_t)cw * ch * 3;
+    const size_t mb = (size_t)opt_.max_batch;
+    vector<unsigned char> crops(mb * per * crop_bytes);
+    for (size_t start = 0; start < imgs.size(); start += mb) {
+        const int n = (int)std::min(mb, imgs.size() - start);
+        vector<const uint8_t *> ptrs(n);
+        vector<int> ws(n), hs(n), strides(n);
+        for (int i = 0; i < n; i++) {
+            const cv::Mat &m = imgs[start + i];
+            if (m.empty()) throw std::runtime_error("detectAndAlign: empty image");
+            ptrs[i] = m.data; ws[i] = m.cols; hs[i] = m.rows; strides[i] = (int)m.step;
+        }
+        int rc = rf_detect_align_batch(h_, ptrs.data(), ws.data(), hs.data(), strides.data(), n, threshold, nms_threshold, &p,
+                                       out_faces_.data(), out_counts_.data(), crops.data(), nullptr);
+        if (rc != RF_OK) throw std::runtime_error(string("rf_detect_align_batch: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+        for (int i = 0; i < n; i++) {
+            const FaceDetectInfo *f = reinterpret_cast<const FaceDetectInfo *>(out_faces_.data() + (size_t)i * opt_.max_faces);
+            last_[start + i].assign(f, f + out_counts_[i]);
+            for (int j = 0; j < std::min(out_counts_[i], per); j++) {
+                Mat c(ch, cw, CV_8UC3);
+                const unsigned char *src = crops.data() + ((size_t)i * per + j) * crop_bytes;
+                for (int y = 0; y < ch; y++) std::memcpy(c.data + (size_t)y * c.step, src + (size_t)y * cw * 3, (size_t)cw * 3);
+                crops_[start + i].push_back(c);
+            }
         }
     }
 }

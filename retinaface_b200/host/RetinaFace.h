@@ -42,6 +42,14 @@ struct RetinaFaceOptions {
                                          // staleness check).  Empty: none
 };
 
+// f5 face alignment (rf_detect_align_batch): one u8 BGR crop per kept face, warped from the original image so that the five
+// landmarks land on a template (cv::warpAffine INTER_LINEAR bit for bit, on the GPU)
+struct AlignOptions {
+    int crop_w = 112, crop_h = 112;
+    float template_xy[10] = {0};         // crop-pixel targets (x0, y0 .. x4, y4); all 0: the ArcFace 112x112 template
+    int max_faces = 0;                   // crops per image, best score first; 0: every kept face
+};
+
 class RetinaFace {
    public:
     RetinaFace(string &model, string network = "net3", float nms = 0.4, const RetinaFaceOptions &opt = RetinaFaceOptions());
@@ -66,6 +74,10 @@ class RetinaFace {
     // runs mirrored.  All views run as one batch and are merged by NMS on the GPU (rf_detect_views).
     vector<FaceDetectInfo> detectInImage(const Mat &img, float threshold = 0.5, const vector<float> &scales = vector<float>(1, 1.0f),
                                          bool flip = false);
+    // detect + align: afterwards lastBatchFaces() holds the faces in ORIGINAL IMAGE pixels (lastScale() is 1) and lastCrops()[i]
+    // the crops of image i's first min(faces, max_faces) faces, crop_h x crop_w 8UC3 Mats
+    void detectAndAlign(vector<cv::Mat> imgs, float threshold, const AlignOptions &align = AlignOptions());
+    const vector<vector<Mat>> &lastCrops() const { return crops_; }
     // the reference's visualisation (RetinaFace.cpp:730-741): red box outline (thickness 2), green landmark dots, on a clone
     static Mat draw(const Mat &img, const vector<FaceDetectInfo> &faces);
     int netWidth() const { return opt_.net_w; }
@@ -79,6 +91,7 @@ class RetinaFace {
     vector<vector<FaceDetectInfo>> last_;
     vector<FaceDetectInfo> empty_;
     vector<float> scales_;
+    vector<vector<Mat>> crops_;
     vector<rf_face> out_faces_;
     vector<int> out_counts_;
 };

@@ -68,11 +68,11 @@ void comm_release(rf_handle h) {
 }
 
 // Orders `s` behind the arrival of every rank's records of the step the run parameters name.
-void comm_wait_in_graph(rf_handle h, int n, cudaStream_t s) {
+void comm_wait_in_graph(rf_handle h, const Ctx &x, int n, cudaStream_t s) {
     Comm &c = h->comm;
     const unsigned *flags = reinterpret_cast<const unsigned *>(c.window + dets_bytes(h, c.world) + words(h, c.world) * 4);
     const int threads = std::min(1024, std::max(32, c.world * n));
-    k_comm_wait_p<<<1, threads, 0, s>>>(flags, h->d_params, c.world, h->cfg.max_batch, n, c.d_err);
+    k_comm_wait_p<<<1, threads, 0, s>>>(flags, x.d_params, c.world, h->cfg.max_batch, n, c.d_err);
     CK(cudaGetLastError());
 }
 
@@ -143,15 +143,12 @@ int rf_comm_init(rf_handle h, const void *blobs) {
             v.flags[p] = reinterpret_cast<unsigned *>(c.peer[p] + dets_bytes(h, c.world) + words(h, c.world) * 4);
         }
         // every context's NMS gets the peer view; graphs captured before carry the old (empty) one
-        const int keep = h->active;
-        for (int x = 0; x < h->nctx; x++) {
-            switch_ctx(h, x);
-            CK(cudaStreamSynchronize(h->stream));
-            h->pb.comm = v;
-            for (auto &g : h->graphs) cudaGraphExecDestroy(g.second);
-            h->graphs.clear();
+        for (Ctx &x : h->ctx) {
+            CK(cudaStreamSynchronize(x.stream));
+            x.pb.comm = v;
+            for (auto &g : x.graphs) cudaGraphExecDestroy(g.second);
+            x.graphs.clear();
         }
-        switch_ctx(h, keep);
         c.ready = true;
         c.seq = 0;
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
@@ -215,12 +212,12 @@ int rf_comm_init_nccl(rf_handle h, const void *nccl_unique_id, int rank, int wor
         if (nrc) return fail(h, RF_ERR_CUDA, fmt("ncclCommInitRank failed: %s", api->GetErrorString ? api->GetErrorString(nrc) : "?"));
         CK(cudaMalloc(&d_send, sizeof(CommBlob)));
         CK(cudaMalloc(&d_recv, sizeof(CommBlob) * world));
-        switch_ctx(h, 0);
-        CK(cudaMemcpyAsync(d_send, &mine, sizeof mine, cudaMemcpyHostToDevice, h->stream));
-        nrc = api->AllGather(d_send, d_recv, sizeof(CommBlob), /* ncclChar */ 0, comm, h->stream);
+        cudaStream_t s = h->ctx[0].stream;
+        CK(cudaMemcpyAsync(d_send, &mine, sizeof mine, cudaMemcpyHostToDevice, s));
+        nrc = api->AllGather(d_send, d_recv, sizeof(CommBlob), /* ncclChar */ 0, comm, s);
         if (nrc) { api->CommDestroy(comm); cudaFree(d_send); cudaFree(d_recv); return fail(h, RF_ERR_CUDA, fmt("ncclAllGather failed: %s", api->GetErrorString ? api->GetErrorString(nrc) : "?")); }
-        CK(cudaMemcpyAsync(all.data(), d_recv, sizeof(CommBlob) * world, cudaMemcpyDeviceToHost, h->stream));
-        CK(cudaStreamSynchronize(h->stream));
+        CK(cudaMemcpyAsync(all.data(), d_recv, sizeof(CommBlob) * world, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
         api->CommDestroy(comm);
         cudaFree(d_send); cudaFree(d_recv);
     } catch (const CudaFail &f) {

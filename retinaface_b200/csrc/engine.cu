@@ -95,85 +95,148 @@ void place_tensors(rf_handle h, bool keep_all) {
     h->arena_bytes = top;
 }
 
-// Issue the forward pass: lane 0 on `s`, side lanes on their own streams, joined by events.  Works both
-// under stream capture (the side streams fork from / join into the capturing stream) and eagerly.
-void run_steps(rf_handle h, int n, cudaStream_t s, bool use_lanes = true) {
+// The layer plan of h->cfg (INT8, FP32, FP16 tile chains or FP16 per-layer kernels), linked across lanes and placed in the
+// arena.  `init`: also set the kernels' launch attributes up on the current device (rf_plan_describe needs no GPU).
+void make_plan(rf_handle h, bool init) {
+    const rf_config &cfg = h->cfg;
+    h->use_tc = cfg.precision == RF_PREC_INT8 || (cfg.precision == RF_PREC_FP16 && !(cfg.flags & RF_FLAG_NO_TENSORCORE));
+    if (init && h->use_tc) CK(tc_init());
+    if (cfg.precision == RF_PREC_INT8) { if (init) CK(tc_init_i8()); build_plan_i8(h); }
+    else if (cfg.precision == RF_PREC_FP32) build_plan<float>(h);
+    else if (h->use_tc && !(cfg.flags & RF_FLAG_LEGACY_TC)) { if (init) CK(tile_init()); build_plan_tiles(h); }
+    else build_plan<__half>(h);
+    link_steps(h);
+    place_tensors(h, false);
+}
+
+// Candidate and output buffers of the NMS for `batch` images of up to `anchors` candidates each.
+void alloc_post_buffers(PostBuffers &pb, int anchors, int batch, int max_faces) {
+    int ap2 = 1;
+    while (ap2 < anchors) ap2 <<= 1;
+    pb.anchors_per_image = anchors; pb.anchors_pow2 = ap2; pb.max_faces = max_faces; pb.max_batch = batch;
+    const size_t B = batch;
+    CK(cudaMalloc(&pb.cand_keys, sizeof(unsigned long long) * B * anchors));
+    CK(cudaMalloc(&pb.cand_recs, sizeof(rf_det) * B * anchors));
+    CK(cudaMalloc(&pb.cand_count, sizeof(int) * B));
+    CK(cudaMemset(pb.cand_count, 0, sizeof(int) * B));
+    CK(cudaMalloc(&pb.sort_scratch, sizeof(unsigned long long) * B * ap2));
+    CK(cudaMalloc(&pb.flag_scratch, B * ap2));
+    CK(cudaMalloc(&pb.out_dets, sizeof(rf_det) * B * max_faces));
+    CK(cudaMalloc(&pb.out_counts, sizeof(int) * B));
+    CK(cudaMalloc(&pb.out_total_kept, sizeof(int) * B));
+    CK(cudaMemset(pb.out_counts, 0, sizeof(int) * B));
+    CK(cudaMalloc(&pb.tile_done, sizeof(int) * B));
+    CK(cudaMemset(pb.tile_done, 0, sizeof(int) * B));
+}
+void free_post_buffers(PostBuffers &pb) {
+    cudaFree(pb.cand_keys); cudaFree(pb.cand_recs); cudaFree(pb.cand_count); cudaFree(pb.sort_scratch); cudaFree(pb.flag_scratch);
+    cudaFree(pb.out_dets); cudaFree(pb.out_counts); cudaFree(pb.out_total_kept); cudaFree(pb.tile_done);
+    pb = PostBuffers{};
+}
+
+// Allocates context c's arena (h->arena_bytes); with `all`, everything else the context owns too.
+void create_ctx(rf_handle h, Ctx &c, bool all) {
+    if (all) {
+        CK(cudaStreamCreateWithFlags(&c.stream, cudaStreamNonBlocking));
+        for (int l = 1; l < 3; l++) CK(cudaStreamCreateWithFlags(&c.lane_stream[l], cudaStreamNonBlocking));
+        c.step_event.assign(h->steps.size(), nullptr);
+        for (size_t i = 0; i < h->steps.size(); i++)
+            if (h->steps[i].signals) CK(cudaEventCreateWithFlags(&c.step_event[i], cudaEventDisableTiming));
+        CK(cudaEventCreateWithFlags(&c.fence, cudaEventDisableTiming));
+    }
+    CK(cudaMalloc(&c.arena, h->arena_bytes));
+    if (!all) return;
+    CK(cudaMalloc(&c.d_params, sizeof(PostParams)));
+    CK(cudaHostAlloc(&c.h_params, sizeof(PostParams) * Ctx::kParamSlots, cudaHostAllocDefault));
+    int anchors = 0;
+    for (const LevelDesc &lv : h->lv) anchors += 2 * lv.h * lv.w;
+    alloc_post_buffers(c.pb, anchors, h->cfg.max_batch, h->cfg.max_faces);
+}
+
+// Waits for context c, drops its captured graphs (they hold arena addresses) and frees its arena; with `all`, everything else
+// the context owns too.
+void release_ctx(Ctx &c, bool all) {
+    if (c.stream) cudaStreamSynchronize(c.stream);
+    for (auto &g : c.graphs) cudaGraphExecDestroy(g.second);
+    c.graphs.clear();
+    cudaFree(c.arena);
+    c.arena = nullptr;
+    if (!all) return;
+    cudaFree(c.d_params); cudaFreeHost(c.h_params);
+    free_post_buffers(c.pb);
+    for (auto e : c.step_event) if (e) cudaEventDestroy(e);
+    for (int l = 1; l < 3; l++) if (c.lane_stream[l]) cudaStreamDestroy(c.lane_stream[l]);
+    if (c.fence) cudaEventDestroy(c.fence);
+    if (c.stream) cudaStreamDestroy(c.stream);
+    c = Ctx{};
+}
+
+// Issue the forward pass into r.ctx: lane 0 on r.stream, side lanes on the context's lane streams, joined by events.  Works
+// both under stream capture (the side streams fork from / join into the capturing stream) and eagerly.
+void run_steps(rf_handle h, const Run &r, bool use_lanes = true) {
     static const bool one_lane = [] { const char *e = getenv("RF_ONE_LANE"); return e && e[0] == '1'; }();   // A/B measurements
     if (one_lane) use_lanes = false;
+    const Ctx &c = r.ctx;
     for (size_t i = 0; i < h->steps.size(); i++) {
         Step &st = h->steps[i];
-        cudaStream_t cs = (use_lanes && st.lane) ? h->lane_stream[st.lane] : s;
+        cudaStream_t cs = (use_lanes && st.lane) ? c.lane_stream[st.lane] : r.stream;
         if (use_lanes)
-            for (int d : st.deps) CK(cudaStreamWaitEvent(cs, h->step_event[d], 0));
-        st.launch(n, cs);
-        if (use_lanes && st.signals) CK(cudaEventRecord(h->step_event[i], cs));
+            for (int d : st.deps) CK(cudaStreamWaitEvent(cs, c.step_event[d], 0));
+        st.launch(Run{c, r.n, cs, r.blobs});
+        if (use_lanes && st.signals) CK(cudaEventRecord(c.step_event[i], cs));
     }
     if (use_lanes)
         for (int l = 1; l < 3; l++)
-            if (h->lane_last[l] >= 0) CK(cudaStreamWaitEvent(s, h->step_event[h->lane_last[l]], 0));
+            if (h->lane_last[l] >= 0) CK(cudaStreamWaitEvent(r.stream, c.step_event[h->lane_last[l]], 0));
     // multi-GPU handles: the wait for every rank's records of this step is the forward's last node (a no-op kernel for runs
     // without an exchange), not a separate launch behind the graph
-    if (h->comm.ready && !h->profiling) comm_wait_in_graph(h, n, s);
+    if (h->comm.ready) comm_wait_in_graph(h, c, r.n, r.stream);
 }
 
-void forward_graph(rf_handle h, int n) {
+void forward_graph(rf_handle h, Ctx &c, int n) {
     if (h->cfg.flags & RF_FLAG_NO_GRAPH) {
-        run_steps(h, n, h->stream);
+        run_steps(h, Run{c, n, c.stream});
         CK(cudaGetLastError());
         return;
     }
-    auto it = h->graphs.find(n);
-    if (it == h->graphs.end()) {
+    auto it = c.graphs.find(n);
+    if (it == c.graphs.end()) {
         cudaGraph_t g = nullptr;
-        CK(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
-        run_steps(h, n, h->stream);
-        cudaError_t e = cudaStreamEndCapture(h->stream, &g);
+        CK(cudaStreamBeginCapture(c.stream, cudaStreamCaptureModeThreadLocal));
+        run_steps(h, Run{c, n, c.stream});
+        cudaError_t e = cudaStreamEndCapture(c.stream, &g);
         if (e != cudaSuccess) throw CudaFail{e, "cudaStreamEndCapture", __FILE__, __LINE__};
         cudaGraphExec_t ge = nullptr;
         e = cudaGraphInstantiate(&ge, g, 0);
         cudaGraphDestroy(g);
         if (e != cudaSuccess) throw CudaFail{e, "cudaGraphInstantiate", __FILE__, __LINE__};
-        it = h->graphs.emplace(n, ge).first;
+        it = c.graphs.emplace(n, ge).first;
     }
-    CK(cudaGraphLaunch(it->second, h->stream));
+    CK(cudaGraphLaunch(it->second, c.stream));
 }
 
 // Run parameters travel through a small ring of pinned slots so that an asynchronous caller
 // (rf_detect_batch_device) can queue several runs without overwriting a copy still in flight.
-void set_params(rf_handle h, float thr, float nms, const uint8_t *input = nullptr, unsigned comm_seq = 0) {
-    PostParams *slot = h->h_params + (h->param_seq++ % rf_handle_s::kParamSlots);
+void set_params(rf_handle h, Ctx &c, float thr, float nms, const uint8_t *input = nullptr, unsigned comm_seq = 0) {
+    PostParams *slot = c.h_params + (c.param_seq++ % Ctx::kParamSlots);
     slot->score_thr = thr;
     slot->nms_thr = nms;
     slot->input = input ? input : h->d_input;
     slot->comm_seq = comm_seq;
     slot->comm_slot = comm_seq ? comm_seq % (unsigned)h->comm.ring : 0u;
-    h->cur_thr = thr;
-    h->cur_nms = nms;
-    CK(cudaMemcpyAsync(h->d_params, slot, sizeof(PostParams), cudaMemcpyHostToDevice, h->stream));
+    c.cur_thr = thr;
+    c.cur_nms = nms;
+    CK(cudaMemcpyAsync(c.d_params, slot, sizeof(PostParams), cudaMemcpyHostToDevice, c.stream));
 }
 
 void destroy(rf_handle h) {
     if (!h) return;
     cudaSetDevice(h->device);
-    if (h->saved.empty()) h->saved.resize(1);
-    for (int c = 0; c < (int)h->saved.size(); c++) { switch_ctx(h, c); if (h->stream) cudaStreamSynchronize(h->stream); }
+    for (Ctx &c : h->ctx) if (c.stream) cudaStreamSynchronize(c.stream);
     comm_release(h);
     jpeg_release(h);
-    for (int c = 0; c < (int)h->saved.size(); c++) {
-        switch_ctx(h, c);
-        if (h->stream) cudaStreamSynchronize(h->stream);
-        for (auto &g : h->graphs) cudaGraphExecDestroy(g.second);
-        h->graphs.clear();
-        cudaFree(h->arena); cudaFree(h->d_params); cudaFreeHost(h->h_params);
-        cudaFree(h->pb.cand_keys); cudaFree(h->pb.cand_recs); cudaFree(h->pb.cand_count); cudaFree(h->pb.sort_scratch);
-        cudaFree(h->pb.flag_scratch); cudaFree(h->pb.out_dets); cudaFree(h->pb.out_counts); cudaFree(h->pb.out_total_kept); cudaFree(h->pb.tile_done);
-        for (auto e : h->step_event) if (e) cudaEventDestroy(e);
-        for (int l = 1; l < 3; l++) if (h->lane_stream[l]) cudaStreamDestroy(h->lane_stream[l]);
-        if (h->fence) cudaEventDestroy(h->fence);
-        if (h->stream) cudaStreamDestroy(h->stream);
-    }
-    cudaFree(h->pb_merge.cand_keys); cudaFree(h->pb_merge.cand_recs); cudaFree(h->pb_merge.cand_count); cudaFree(h->pb_merge.sort_scratch);
-    cudaFree(h->pb_merge.flag_scratch); cudaFree(h->pb_merge.out_dets); cudaFree(h->pb_merge.out_counts); cudaFree(h->pb_merge.out_total_kept);
+    for (Ctx &c : h->ctx) release_ctx(c, true);
+    free_post_buffers(h->pb_merge);
     cudaFree(h->d_weights); cudaFree(h->d_weights_h); cudaFree(h->d_weights_q); cudaFree(h->d_input); cudaFree(h->d_raw);
     for (auto p : h->d_blobs) cudaFree(p);
     h->copy_pool.reset();
@@ -302,7 +365,6 @@ int rf_create(const rf_config *cfg, rf_handle *out) {
         if (prop.major != 9 || prop.minor != 0)
             return fail(nullptr, RF_ERR_NO_DEVICE, fmt("device %d is sm_%d%d; librf_b200 is built for sm_90a only", h->device, prop.major, prop.minor));
         h->num_sms = prop.multiProcessorCount;
-        CK(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
         CK(cudaEventCreate(&h->ev0));
         CK(cudaEventCreate(&h->ev1));
         CK(postproc_init());
@@ -318,18 +380,7 @@ int rf_create(const rf_config *cfg, rf_handle *out) {
             base_anchors_net3(strides[l], lv.base);
             abase += 2 * lv.h * lv.w; pbase += lv.h * lv.w;
         }
-        const int A = abase;
-        int ap2 = 1;
-        while (ap2 < A) ap2 <<= 1;
-
-        h->use_tc = h->cfg.precision == RF_PREC_INT8 || (h->cfg.precision == RF_PREC_FP16 && !(h->cfg.flags & RF_FLAG_NO_TENSORCORE));
-        if (h->use_tc) CK(tc_init());
-        if (h->cfg.precision == RF_PREC_INT8) { CK(tc_init_i8()); build_plan_i8(h); }
-        else if (h->cfg.precision == RF_PREC_FP32) build_plan<float>(h);
-        else if (h->use_tc && !(h->cfg.flags & RF_FLAG_LEGACY_TC)) { CK(tile_init()); build_plan_tiles(h); }
-        else build_plan<__half>(h);
-        link_steps(h);
-        place_tensors(h, false);
+        make_plan(h, true);
         CK(cudaMalloc(&h->d_weights, h->wstage.size() * sizeof(float)));
         CK(cudaMemcpy(h->d_weights, h->wstage.data(), h->wstage.size() * sizeof(float), cudaMemcpyHostToDevice));
         if (!h->wstage_h.empty()) {
@@ -355,36 +406,8 @@ int rf_create(const rf_config *cfg, rf_handle *out) {
         CK(cudaHostAlloc(&h->tile_dbg, 64, cudaHostAllocMapped));
         memset(h->tile_dbg, 0, 64);
         CK(cudaHostGetDevicePointer(&h->tile_dbg_dev, h->tile_dbg, 0));
-        // ---- per-context resources ----
-        h->nctx = h->cfg.streams <= 0 ? RF_MAX_STREAMS : std::min(h->cfg.streams, RF_MAX_STREAMS);
-        h->saved.resize(h->nctx);
-        for (int c = 0; c < h->nctx; c++) {
-            switch_ctx(h, c);
-            if (c > 0) CK(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));   // context 0 keeps the stream created above
-            for (int l = 1; l < 3; l++) CK(cudaStreamCreateWithFlags(&h->lane_stream[l], cudaStreamNonBlocking));
-            h->step_event.assign(h->steps.size(), nullptr);
-            for (size_t i = 0; i < h->steps.size(); i++)
-                if (h->steps[i].signals) CK(cudaEventCreateWithFlags(&h->step_event[i], cudaEventDisableTiming));
-            CK(cudaEventCreateWithFlags(&h->fence, cudaEventDisableTiming));
-            CK(cudaMalloc(&h->arena, h->arena_bytes));
-            CK(cudaMalloc(&h->d_params, sizeof(PostParams)));
-            CK(cudaHostAlloc(&h->h_params, sizeof(PostParams) * rf_handle_s::kParamSlots, cudaHostAllocDefault));
-            PostBuffers &pb = h->pb;
-            pb.anchors_per_image = A; pb.anchors_pow2 = ap2; pb.max_faces = h->cfg.max_faces; pb.max_batch = Bm;
-            CK(cudaMalloc(&pb.cand_keys, sizeof(unsigned long long) * (size_t)Bm * A));
-            CK(cudaMalloc(&pb.cand_recs, sizeof(rf_det) * (size_t)Bm * A));
-            CK(cudaMalloc(&pb.cand_count, sizeof(int) * Bm));
-            CK(cudaMemset(pb.cand_count, 0, sizeof(int) * Bm));
-            CK(cudaMalloc(&pb.sort_scratch, sizeof(unsigned long long) * (size_t)Bm * ap2));
-            CK(cudaMalloc(&pb.flag_scratch, (size_t)Bm * ap2));
-            CK(cudaMalloc(&pb.out_dets, sizeof(rf_det) * (size_t)Bm * pb.max_faces));
-            CK(cudaMalloc(&pb.out_counts, sizeof(int) * Bm));
-            CK(cudaMalloc(&pb.out_total_kept, sizeof(int) * Bm));
-            CK(cudaMemset(pb.out_counts, 0, sizeof(int) * Bm));
-            CK(cudaMalloc(&pb.tile_done, sizeof(int) * Bm));
-            CK(cudaMemset(pb.tile_done, 0, sizeof(int) * Bm));
-        }
-        switch_ctx(h, 0);
+        h->ctx.resize(h->cfg.streams <= 0 ? RF_MAX_STREAMS : std::min(h->cfg.streams, RF_MAX_STREAMS));
+        for (Ctx &c : h->ctx) create_ctx(h, c, true);
         for (int l = 0; l < 3; l++) {
             const int ch[3] = {4, 8, 20};
             for (int k = 0; k < 3; k++) h->blob_elems[3 * l + k] = (size_t)ch[k] * h->lv[l].h * h->lv[l].w;
@@ -412,16 +435,14 @@ int rf_get_net_size(rf_handle h, int *net_w, int *net_h, int *max_batch, int *ma
     if (max_faces) *max_faces = h->cfg.max_faces;
     return RF_OK;
 }
-int rf_num_anchors(rf_handle h) { return h ? h->pb.anchors_per_image : RF_ERR_INVALID_ARG; }
-void *rf_stream(rf_handle h) { if (!h) return nullptr; switch_ctx(h, 0); return (void *)h->stream; }
+int rf_num_anchors(rf_handle h) { return h ? h->ctx[0].pb.anchors_per_image : RF_ERR_INVALID_ARG; }
+void *rf_stream(rf_handle h) { return h ? (void *)h->ctx[0].stream : nullptr; }
 
 int rf_synchronize(rf_handle h) {
     if (!h) return RF_ERR_INVALID_ARG;
     try {
         CK(cudaSetDevice(h->device));
-        const int keep = h->active;
-        for (int c = 0; c < h->nctx; c++) { switch_ctx(h, c); CK(cudaStreamSynchronize(h->stream)); }
-        switch_ctx(h, keep);
+        for (Ctx &c : h->ctx) CK(cudaStreamSynchronize(c.stream));
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }
@@ -431,49 +452,48 @@ int rf_fence(rf_handle h) {
     if (!h) return RF_ERR_INVALID_ARG;
     try {
         CK(cudaSetDevice(h->device));
-        switch_ctx(h, 0);
-        cudaStream_t s0 = h->stream;
-        for (int c = 1; c < h->nctx; c++) {
-            switch_ctx(h, c);
-            CK(cudaEventRecord(h->fence, h->stream));
-            CK(cudaStreamWaitEvent(s0, h->fence, 0));
+        for (size_t c = 1; c < h->ctx.size(); c++) {
+            CK(cudaEventRecord(h->ctx[c].fence, h->ctx[c].stream));
+            CK(cudaStreamWaitEvent(h->ctx[0].stream, h->ctx[c].fence, 0));
         }
-        switch_ctx(h, 0);
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }
 
-void *rf_last_stream(rf_handle h) { return h ? (void *)(h->last_stream ? h->last_stream : h->stream) : nullptr; }
+void *rf_last_stream(rf_handle h) { return h ? (void *)(h->last_stream ? h->last_stream : h->ctx[0].stream) : nullptr; }
 
 int rf_launches_per_batch(rf_handle h, int n) {
     (void)n;
     return h ? (int)h->steps.size() : RF_ERR_INVALID_ARG;
 }
 
+// `ran_on` (optional) receives the context the forward was issued on.
 static int detect_device_impl(rf_handle h, const uint8_t *dev_bgr, int n, float thr, float nms, const rf_det **dev_dets, const int32_t **dev_counts,
-                              bool gather) {
+                              bool gather, Ctx **ran_on = nullptr) {
     int rc = check_n(h, n);
     if (rc) return rc;
     if (gather && (!h->comm.ready || n == 0)) return fail(h, RF_ERR_INVALID_ARG, "rf_detect_batch_device_allgather: call rf_comm_init first (and n > 0)");
     try {
         CK(cudaSetDevice(h->device));
-        switch_ctx(h, (int)(h->next_dev_ctx++ % (unsigned)h->nctx));   // consecutive batches overlap on different contexts
-        h->last_stream = h->stream;
+        Ctx &c = h->ctx[h->next_dev_ctx++ % h->ctx.size()];   // consecutive batches overlap on different contexts
+        if (ran_on) *ran_on = &c;
+        h->last_stream = c.stream;
         // the caller's device images are read in place (conv0 takes the pointer from the run parameters)
-        if (h->param_seq && h->param_seq % rf_handle_s::kParamSlots == 0) CK(cudaStreamSynchronize(h->stream));
+        if (c.param_seq && c.param_seq % Ctx::kParamSlots == 0) CK(cudaStreamSynchronize(c.stream));
         const unsigned seq = gather ? ++h->comm.seq : 0u;
-        set_params(h, thr, nms, dev_bgr, seq);
-        if (n > 0) forward_graph(h, n);
+        set_params(h, c, thr, nms, dev_bgr, seq);
+        if (n > 0) forward_graph(h, c, n);
+        const rf_det *dets = c.pb.out_dets;
+        const int32_t *counts = c.pb.out_counts;
         if (gather) {
             const unsigned slot = seq % (unsigned)h->comm.ring;
             const size_t img0 = (size_t)slot * h->comm.world * h->cfg.max_batch;
-            if (dev_dets) *dev_dets = h->pb.comm.dets[h->comm.rank] + img0 * h->cfg.max_faces;
-            if (dev_counts) *dev_counts = h->pb.comm.counts[h->comm.rank] + img0;
-            return RF_OK;
+            dets = c.pb.comm.dets[h->comm.rank] + img0 * h->cfg.max_faces;
+            counts = c.pb.comm.counts[h->comm.rank] + img0;
         }
+        if (dev_dets) *dev_dets = dets;
+        if (dev_counts) *dev_counts = counts;
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    if (dev_dets) *dev_dets = h->pb.out_dets;
-    if (dev_counts) *dev_counts = h->pb.out_counts;
     return RF_OK;
 }
 
@@ -486,52 +506,82 @@ int rf_detect_batch_device_allgather(rf_handle h, const uint8_t *dev_bgr, int n,
     return detect_device_impl(h, dev_bgr, n, thr, nms, all_dets, all_counts, true);
 }
 
-static int fetch_results(rf_handle h, int n, rf_face *out_faces, int *out_counts, int32_t *out_idx, int *out_ncand) {
+// Kept records of images [first, first + n) -> the caller's arrays, image g at the same place on both sides (max_faces
+// records per image).  Counts are clamped to max_faces: those of other ranks come from peer memory.
+static void put_results(rf_handle h, const rf_det *dets, const int *counts, size_t first, int n, rf_face *out_faces, int *out_counts,
+                        int32_t *out_idx) {
     const int mf = h->cfg.max_faces;
-    CK(cudaMemcpyAsync(h->h_counts, h->pb.out_counts, sizeof(int) * n, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaMemcpyAsync(h->h_dets, h->pb.out_dets, sizeof(rf_det) * (size_t)n * mf, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    for (int i = 0; i < n; i++) {
-        int k = h->h_counts[i];
-        if (out_counts) out_counts[i] = k;
+    for (size_t g = first; g < first + n; g++) {
+        const int k = std::min(counts[g], mf);
+        if (out_counts) out_counts[g] = k;
         for (int j = 0; j < k; j++) {
-            const rf_det &d = h->h_dets[(size_t)i * mf + j];
-            if (out_faces) out_faces[(size_t)i * mf + j] = d.face;
-            if (out_idx) out_idx[(size_t)i * mf + j] = d.anchor_index;
+            const rf_det &d = dets[g * mf + j];
+            if (out_faces) out_faces[g * mf + j] = d.face;
+            if (out_idx) out_idx[g * mf + j] = d.anchor_index;
         }
     }
-    (void)out_ncand;
-    return RF_OK;
 }
 
-// One caller image of arbitrary size -> d_raw (packed rows) on the handle's stream.  Pinned sources (cudaHostAlloc /
+// Waits for context c's results of n images and copies them out (through the pinned h_counts / h_dets).
+static void fetch_results(rf_handle h, Ctx &c, int n, rf_face *out_faces, int *out_counts, int32_t *out_idx) {
+    CK(cudaMemcpyAsync(h->h_counts, c.pb.out_counts, sizeof(int) * n, cudaMemcpyDeviceToHost, c.stream));
+    CK(cudaMemcpyAsync(h->h_dets, c.pb.out_dets, sizeof(rf_det) * (size_t)n * h->cfg.max_faces, cudaMemcpyDeviceToHost, c.stream));
+    CK(cudaStreamSynchronize(c.stream));
+    put_results(h, h->h_dets, h->h_counts, 0, n, out_faces, out_counts, out_idx);
+}
+
+// Whether `p` is page-locked host memory (cudaHostAlloc / cudaHostRegister), which an H2D copy may read in place.
+static bool is_pinned(const void *p) {
+    cudaPointerAttributes at{};
+    if (cudaPointerGetAttributes(&at, p) == cudaSuccess && at.type == cudaMemoryTypeHost) return true;
+    cudaGetLastError();
+    return false;
+}
+
+// H2D copies of network-sized images i -> dst + i * img_bytes, issued on `s` in runs: consecutive images whose sources are
+// adjacent in host memory go as one copy.
+struct H2DRuns {
+    uint8_t *dst;
+    size_t img_bytes;
+    cudaStream_t s;
+    const uint8_t *src = nullptr;
+    int start = -1, len = 0;
+    void add(int i, const uint8_t *p) {
+        if (start >= 0 && i == start + len && p == src + (size_t)len * img_bytes) { len++; return; }
+        flush();
+        start = i; src = p; len = 1;
+    }
+    void flush() {
+        if (start >= 0) CK(cudaMemcpyAsync(dst + (size_t)start * img_bytes, src, (size_t)len * img_bytes, cudaMemcpyHostToDevice, s));
+        start = -1;
+    }
+};
+
+// One caller image of arbitrary size -> d_raw (packed rows) on `s`.  Pinned sources (cudaHostAlloc /
 // cudaHostRegister) are copied straight from the caller's memory, row stride and all.  Pageable sources are staged through
 // two pinned buffers: a row-band parallel host copy (host_copy.h) into one buffer overlaps the DMA out of the other; the
 // only host wait is for the DMA that last read the buffer about to be overwritten.  In both cases the stream orders the
 // copy into d_raw behind the letter-box kernel that still reads the previous image.
-static uint8_t *upload_raw(rf_handle h, const uint8_t *src, int width, int height, int row_stride, int raw_slot = 0) {
+static uint8_t *upload_raw(rf_handle h, cudaStream_t s, const uint8_t *src, int width, int height, int row_stride, int raw_slot = 0) {
     uint8_t *d_dst = h->d_raw + (size_t)raw_slot * h->raw_bytes;
-    cudaPointerAttributes at{};
-    const bool pinned = cudaPointerGetAttributes(&at, src) == cudaSuccess && at.type == cudaMemoryTypeHost;
-    if (pinned) {
-        CK(cudaMemcpy2DAsync(d_dst, (size_t)width * 3, src, (size_t)row_stride, (size_t)width * 3, (size_t)height, cudaMemcpyHostToDevice, h->stream));
+    if (is_pinned(src)) {
+        CK(cudaMemcpy2DAsync(d_dst, (size_t)width * 3, src, (size_t)row_stride, (size_t)width * 3, (size_t)height, cudaMemcpyHostToDevice, s));
         return d_dst;
     }
-    cudaGetLastError();
     if (!h->copy_pool) h->copy_pool.reset(new HostCopyPool((int)std::min(3u, std::max(1u, std::thread::hardware_concurrency()) - 1u)));
     const int slot = (int)(h->raw_seq++ & 1u);
     uint8_t *buf = h->h_raw + (size_t)slot * h->raw_bytes;
     CK(cudaEventSynchronize(h->raw_ev[slot]));      // (returns at once for an event never recorded)
     h->copy_pool->copy_rows(buf, src, (size_t)width * 3, (size_t)row_stride, height);
-    CK(cudaMemcpyAsync(d_dst, buf, (size_t)width * height * 3, cudaMemcpyHostToDevice, h->stream));
-    CK(cudaEventRecord(h->raw_ev[slot], h->stream));
+    CK(cudaMemcpyAsync(d_dst, buf, (size_t)width * height * 3, cudaMemcpyHostToDevice, s));
+    CK(cudaEventRecord(h->raw_ev[slot], s));
     return d_dst;
 }
 
-// The n caller images of rf_detect_batch -> the input tensor, on the handle's stream.  With `originals`
+// The n caller images of rf_detect_batch -> the input tensor, on `s`.  With `originals`
 // (rf_detect_align_batch, which has checked that every image that is not network-sized gets a raw buffer of its own),
 // originals[i] records where image i's own pixels stay resident and its map-back scale.
-static int stage_images(rf_handle h, const char *who, const uint8_t *const *imgs, const int *widths, const int *heights,
+static int stage_images(rf_handle h, cudaStream_t s, const char *who, const uint8_t *const *imgs, const int *widths, const int *heights,
                         const int *row_strides, int n, AlignImage *originals) {
     const int Hn = h->cfg.net_h, Wn = h->cfg.net_w;
     const size_t img_bytes = (size_t)Hn * Wn * 3;
@@ -539,14 +589,7 @@ static int stage_images(rf_handle h, const char *who, const uint8_t *const *imgs
     // pinned (cudaHostAlloc / cudaHostRegister / the library's own rf_pinned_input), otherwise via the
     // library's pinned mirror; runs of adjacent sources collapse into one copy.  Other sizes are
     // letter-boxed on the GPU one by one (preprocess.cuh).
-    const uint8_t *run_src = nullptr;
-    int run_start = -1, run_len = 0;
-    auto flush = [&]() {
-        if (run_start < 0) return;
-        CK(cudaMemcpyAsync(h->d_input + (size_t)run_start * img_bytes, run_src, (size_t)run_len * img_bytes,
-                           cudaMemcpyHostToDevice, h->stream));
-        run_start = -1;
-    };
+    H2DRuns runs{h->d_input, img_bytes, s};
     bool staging_dirty = false;
     // other sizes: uploaded into per-image raw buffers, then ONE letter-box launch for all of them (RF_FLAG_NPP_RESIZE: the
     // reference's NPP super-sampling definition instead of its OpenCV bilinear one)
@@ -554,7 +597,7 @@ static int stage_images(rf_handle h, const char *who, const uint8_t *const *imgs
     std::vector<LbItem> lb;
     auto flush_lb = [&]() {
         if (lb.empty()) return;
-        CK(launch_letterbox_batch(lb.data(), (int)lb.size(), Wn, Hn, h->stream));
+        CK(launch_letterbox_batch(lb.data(), (int)lb.size(), Wn, Hn, s));
         lb.clear();
     };
     for (int i = 0; i < n; i++) {
@@ -563,33 +606,27 @@ static int stage_images(rf_handle h, const char *who, const uint8_t *const *imgs
         if (widths[i] == Wn && heights[i] == Hn && rs == Wn * 3) {
             const uint8_t *src = imgs[i];
             const bool in_mirror = src >= h->h_input && src < h->h_input + (size_t)h->cfg.max_batch * img_bytes;
-            if (!in_mirror) {
-                cudaPointerAttributes at{};
-                bool pinned = cudaPointerGetAttributes(&at, src) == cudaSuccess && at.type == cudaMemoryTypeHost;
-                if (!pinned) {
-                    cudaGetLastError();
-                    if (!staging_dirty) { CK(cudaStreamSynchronize(h->stream)); staging_dirty = true; }
-                    uint8_t *slot = h->h_input + (size_t)i * img_bytes;
-                    memcpy(slot, src, img_bytes);
-                    src = slot;
-                }
+            if (!in_mirror && !is_pinned(src)) {
+                if (!staging_dirty) { CK(cudaStreamSynchronize(s)); staging_dirty = true; }
+                uint8_t *slot = h->h_input + (size_t)i * img_bytes;
+                memcpy(slot, src, img_bytes);
+                src = slot;
             }
-            if (run_start >= 0 && src == run_src + (size_t)run_len * img_bytes) { run_len++; }
-            else { flush(); run_start = i; run_src = src; run_len = 1; }
+            runs.add(i, src);
             if (originals) originals[i] = AlignImage{h->d_input + (size_t)i * img_bytes, Wn, Hn, Wn * 3, 1.f};
         } else {
-            flush();
+            runs.flush();
             if (widths[i] > h->cfg.max_image_w || heights[i] > h->cfg.max_image_h)
                 return fail(h, RF_ERR_CAPACITY, fmt("image %d is %dx%d, larger than max_image %dx%d", i, widths[i], heights[i],
                                                     h->cfg.max_image_w, h->cfg.max_image_h));
             if ((int)lb.size() == h->raw_slots) flush_lb();
-            const uint8_t *d_src = upload_raw(h, imgs[i], widths[i], heights[i], rs, (int)lb.size());
+            const uint8_t *d_src = upload_raw(h, s, imgs[i], widths[i], heights[i], rs, (int)lb.size());
             lb.emplace_back();
             const float scale = letterbox_fill(lb.back(), d_src, widths[i], heights[i], h->d_input + (size_t)i * img_bytes, Wn, Hn, 0, area);
             if (originals) originals[i] = AlignImage{d_src, widths[i], heights[i], widths[i] * 3, scale};
         }
     }
-    flush();
+    runs.flush();
     flush_lb();
     return RF_OK;
 }
@@ -602,11 +639,11 @@ int rf_detect_batch(rf_handle h, const uint8_t *const *imgs, const int *widths, 
     if (!imgs || !widths || !heights) return fail(h, RF_ERR_INVALID_ARG, "rf_detect_batch: NULL image arrays");
     try {
         CK(cudaSetDevice(h->device));
-        switch_ctx(h, 0);
-        if ((rc = stage_images(h, "rf_detect_batch", imgs, widths, heights, row_strides, n, nullptr))) return rc;
-        set_params(h, thr, nms);
-        forward_graph(h, n);
-        fetch_results(h, n, out_faces, out_counts, out_idx, nullptr);
+        Ctx &c = h->ctx[0];
+        if ((rc = stage_images(h, c.stream, "rf_detect_batch", imgs, widths, heights, row_strides, n, nullptr))) return rc;
+        set_params(h, c, thr, nms);
+        forward_graph(h, c, n);
+        fetch_results(h, c, n, out_faces, out_counts, out_idx);
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }
@@ -662,7 +699,7 @@ int rf_detect_align_batch(rf_handle h, const uint8_t *const *imgs, const int *wi
                                             h->cfg.max_image_w, h->cfg.max_image_h));
     try {
         CK(cudaSetDevice(h->device));
-        switch_ctx(h, 0);
+        Ctx &c = h->ctx[0];
         if (!h->d_align_images) {
             CK(cudaMalloc(&h->d_align_images, sizeof(AlignImage) * h->cfg.max_batch));
             CK(cudaHostAlloc(&h->h_align_images, sizeof(AlignImage) * h->cfg.max_batch, cudaHostAllocDefault));
@@ -676,16 +713,16 @@ int rf_detect_align_batch(rf_handle h, const uint8_t *const *imgs, const int *wi
             CK(cudaMalloc(&h->d_align_crops, need));
             h->align_crops_bytes = need;
         }
-        if ((rc = stage_images(h, "rf_detect_align_batch", imgs, widths, heights, row_strides, n, h->h_align_images))) return rc;
-        CK(cudaMemcpyAsync(h->d_align_images, h->h_align_images, sizeof(AlignImage) * n, cudaMemcpyHostToDevice, h->stream));
-        set_params(h, thr, nms);
-        forward_graph(h, n);
+        if ((rc = stage_images(h, c.stream, "rf_detect_align_batch", imgs, widths, heights, row_strides, n, h->h_align_images))) return rc;
+        CK(cudaMemcpyAsync(h->d_align_images, h->h_align_images, sizeof(AlignImage) * n, cudaMemcpyHostToDevice, c.stream));
+        set_params(h, c, thr, nms);
+        forward_graph(h, c, n);
         a.images = h->d_align_images;
         a.n = n;
         a.crops = h->d_align_crops;
         a.mats = out_mats ? h->d_align_mats : nullptr;
-        CK(launch_align_faces(a, h->pb, h->num_sms, h->stream));
-        fetch_results(h, n, nullptr, out_counts, nullptr, nullptr);
+        CK(launch_align_faces(a, c.pb, h->num_sms, c.stream));
+        fetch_results(h, c, n, nullptr, out_counts, nullptr);
         for (int i = 0; i < n; i++) {
             const int k = h->h_counts[i];
             const float s = h->h_align_images[i].scale;
@@ -698,11 +735,11 @@ int rf_detect_align_batch(rf_handle h, const uint8_t *const *imgs, const int *wi
             const size_t first = (size_t)i * a.max_align, m = (size_t)std::min(k, a.max_align);
             if (!m) continue;
             CK(cudaMemcpyAsync(static_cast<uint8_t *>(out_crops) + first * a.crop_bytes, static_cast<uint8_t *>(h->d_align_crops) + first * a.crop_bytes,
-                               m * a.crop_bytes, cudaMemcpyDeviceToHost, h->stream));
+                               m * a.crop_bytes, cudaMemcpyDeviceToHost, c.stream));
             if (out_mats)
-                CK(cudaMemcpyAsync(out_mats + first * 6, h->d_align_mats + first * 6, m * 6 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+                CK(cudaMemcpyAsync(out_mats + first * 6, h->d_align_mats + first * 6, m * 6 * sizeof(double), cudaMemcpyDeviceToHost, c.stream));
         }
-        CK(cudaStreamSynchronize(h->stream));
+        CK(cudaStreamSynchronize(c.stream));
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }
@@ -714,9 +751,9 @@ int rf_detect_align_batch_device(rf_handle h, const uint8_t *dev_bgr, int n, flo
     int rc = align_setup(h, "rf_detect_align_batch_device", params, a);
     if (rc) return rc;
     if (n > 0 && !dev_crops) return fail(h, RF_ERR_INVALID_ARG, "rf_detect_align_batch_device: dev_crops is NULL");
-    if ((rc = detect_device_impl(h, dev_bgr, n, thr, nms, dev_dets, dev_counts, false))) return rc;
+    Ctx *c = nullptr;
+    if ((rc = detect_device_impl(h, dev_bgr, n, thr, nms, dev_dets, dev_counts, false, &c))) return rc;
     if (n == 0) return RF_OK;
-    // detect_device_impl left the context it ran on active: its stream, its results
     a.uniform_base = dev_bgr ? dev_bgr : h->d_input;
     a.uniform_bytes = (size_t)h->cfg.net_h * h->cfg.net_w * 3;
     a.uniform_w = h->cfg.net_w;
@@ -725,7 +762,7 @@ int rf_detect_align_batch_device(rf_handle h, const uint8_t *dev_bgr, int n, flo
     a.crops = dev_crops;
     a.mats = dev_mats;
     try {
-        CK(launch_align_faces(a, h->pb, h->num_sms, h->stream));
+        CK(launch_align_faces(a, c->pb, h->num_sms, c->stream));
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }
@@ -741,7 +778,7 @@ int rf_detect_jpeg_batch(rf_handle h, const uint8_t *const *jpegs, const size_t 
     const size_t img_bytes = (size_t)Hn * Wn * 3;
     try {
         CK(cudaSetDevice(h->device));
-        switch_ctx(h, 0);
+        Ctx &c = h->ctx[0];
         std::vector<int> w(n), hg(n);
         for (int i = 0; i < n; i++) {
             if (!jpegs[i] || !jpeg_bytes[i]) return fail(h, RF_ERR_INVALID_ARG, fmt("rf_detect_jpeg_batch: stream %d is empty", i));
@@ -768,13 +805,13 @@ int rf_detect_jpeg_batch(rf_handle h, const uint8_t *const *jpegs, const size_t 
                     used++;
                 }
             }
-            if ((rc = jpeg_decode(h, jpegs + i0, jpeg_bytes + i0, i1 - i0, dst.data(), w.data() + i0, hg.data() + i0, h->stream))) return rc;
-            if (!lb.empty()) CK(launch_letterbox_batch(lb.data(), (int)lb.size(), Wn, Hn, h->stream));
+            if ((rc = jpeg_decode(h, jpegs + i0, jpeg_bytes + i0, i1 - i0, dst.data(), w.data() + i0, hg.data() + i0, c.stream))) return rc;
+            if (!lb.empty()) CK(launch_letterbox_batch(lb.data(), (int)lb.size(), Wn, Hn, c.stream));
             i0 = i1;
         }
-        set_params(h, thr, nms);
-        forward_graph(h, n);
-        fetch_results(h, n, out_faces, out_counts, out_idx, nullptr);
+        set_params(h, c, thr, nms);
+        forward_graph(h, c, n);
+        fetch_results(h, c, n, out_faces, out_counts, out_idx);
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }
@@ -784,7 +821,7 @@ int rf_decode_jpeg(rf_handle h, const uint8_t *jpeg, size_t bytes, uint8_t *out_
     if (!jpeg || !bytes || !width || !height) return fail(h, RF_ERR_INVALID_ARG, "rf_decode_jpeg: NULL argument");
     try {
         CK(cudaSetDevice(h->device));
-        switch_ctx(h, 0);
+        cudaStream_t s = h->ctx[0].stream;
         int rc = jpeg_info(h, jpeg, bytes, width, height);
         if (rc) return rc;
         if (!out_bgr) return RF_OK;                                    // size query
@@ -793,9 +830,9 @@ int rf_decode_jpeg(rf_handle h, const uint8_t *jpeg, size_t bytes, uint8_t *out_
         if (*width > h->cfg.max_image_w || *height > h->cfg.max_image_h)
             return fail(h, RF_ERR_CAPACITY, fmt("JPEG is %dx%d, larger than max_image %dx%d", *width, *height, h->cfg.max_image_w, h->cfg.max_image_h));
         uint8_t *dst = h->d_raw;
-        if ((rc = jpeg_decode(h, &jpeg, &bytes, 1, &dst, width, height, h->stream))) return rc;
-        CK(cudaMemcpyAsync(out_bgr, h->d_raw, need, cudaMemcpyDeviceToHost, h->stream));
-        CK(cudaStreamSynchronize(h->stream));
+        if ((rc = jpeg_decode(h, &jpeg, &bytes, 1, &dst, width, height, s))) return rc;
+        CK(cudaMemcpyAsync(out_bgr, h->d_raw, need, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }
@@ -825,38 +862,26 @@ static int submit_impl(rf_handle h, const uint8_t *const *imgs, int n, float thr
     try {
         CK(cudaSetDevice(h->device));
         ensure_slots(h);
-        switch_ctx(h, (int)(h->submit_seq % (unsigned)h->nctx));
+        Ctx &c = h->ctx[h->submit_seq % h->ctx.size()];
         rf_handle_s::Slot &sl = h->slots[h->submit_seq % RF_PIPELINE_DEPTH];
         if (sl.busy) return fail(h, RF_ERR_CAPACITY, "rf_submit_batch: RF_PIPELINE_DEPTH batches already in flight; collect one first");
-        // H2D on the copy stream: adjacent sources collapse into one copy
-        const uint8_t *run_src = nullptr;
-        int run_start = -1, run_len = 0;
-        auto flush = [&]() {
-            if (run_start < 0) return;
-            CK(cudaMemcpyAsync(sl.d_in + (size_t)run_start * img_bytes, run_src, (size_t)run_len * img_bytes, cudaMemcpyHostToDevice,
-                               h->copy_stream));
-            run_start = -1;
-        };
+        H2DRuns runs{sl.d_in, img_bytes, h->copy_stream};     // H2D on the copy stream
         for (int i = 0; i < n; i++) {
             if (!imgs[i]) return fail(h, RF_ERR_INVALID_ARG, fmt("rf_submit_batch: image %d is NULL", i));
             const uint8_t *src = imgs[i];
-            cudaPointerAttributes at{};
-            bool pinned = cudaPointerGetAttributes(&at, src) == cudaSuccess && at.type == cudaMemoryTypeHost;
-            if (!pinned) {
-                cudaGetLastError();
+            if (!is_pinned(src)) {
                 memcpy(sl.h_in + (size_t)i * img_bytes, src, img_bytes);   // slot is free: its previous H2D completed before collect
                 src = sl.h_in + (size_t)i * img_bytes;
             }
-            if (run_start >= 0 && src == run_src + (size_t)run_len * img_bytes) run_len++;
-            else { flush(); run_start = i; run_src = src; run_len = 1; }
+            runs.add(i, src);
         }
-        flush();
+        runs.flush();
         CK(cudaEventRecord(sl.ev_h2d, h->copy_stream));
-        CK(cudaStreamWaitEvent(h->stream, sl.ev_h2d, 0));
-        if (h->param_seq && h->param_seq % rf_handle_s::kParamSlots == 0) CK(cudaStreamSynchronize(h->stream));
+        CK(cudaStreamWaitEvent(c.stream, sl.ev_h2d, 0));
+        if (c.param_seq && c.param_seq % Ctx::kParamSlots == 0) CK(cudaStreamSynchronize(c.stream));
         const unsigned seq = gather ? ++h->comm.seq : 0u;
-        set_params(h, thr, nms, sl.d_in, seq);
-        forward_graph(h, n);
+        set_params(h, c, thr, nms, sl.d_in, seq);
+        forward_graph(h, c, n);
         if (gather) {
             // results of ALL ranks: wait for every rank's flags of this step, then read this rank's window slot
             Comm::Slot &cs = h->comm.slots[h->submit_seq % RF_PIPELINE_DEPTH];
@@ -867,15 +892,15 @@ static int submit_impl(rf_handle h, const uint8_t *const *imgs, int n, float thr
             }
             const unsigned slot = seq % (unsigned)h->comm.ring;
             const size_t img0 = (size_t)slot * nimg;
-            CK(cudaMemcpyAsync(cs.h_counts, h->pb.comm.counts[h->comm.rank] + img0, sizeof(int) * nimg, cudaMemcpyDeviceToHost, h->stream));
-            CK(cudaMemcpyAsync(cs.h_dets, h->pb.comm.dets[h->comm.rank] + img0 * h->cfg.max_faces, sizeof(rf_det) * nimg * h->cfg.max_faces, cudaMemcpyDeviceToHost,
-                               h->stream));
-            CK(cudaMemcpyAsync(h->comm.h_err, h->comm.d_err, 4, cudaMemcpyDeviceToHost, h->stream));
+            CK(cudaMemcpyAsync(cs.h_counts, c.pb.comm.counts[h->comm.rank] + img0, sizeof(int) * nimg, cudaMemcpyDeviceToHost, c.stream));
+            CK(cudaMemcpyAsync(cs.h_dets, c.pb.comm.dets[h->comm.rank] + img0 * h->cfg.max_faces, sizeof(rf_det) * nimg * h->cfg.max_faces, cudaMemcpyDeviceToHost,
+                               c.stream));
+            CK(cudaMemcpyAsync(h->comm.h_err, h->comm.d_err, 4, cudaMemcpyDeviceToHost, c.stream));
         } else {
-            CK(cudaMemcpyAsync(sl.h_counts, h->pb.out_counts, sizeof(int) * n, cudaMemcpyDeviceToHost, h->stream));
-            CK(cudaMemcpyAsync(sl.h_dets, h->pb.out_dets, sizeof(rf_det) * (size_t)n * h->cfg.max_faces, cudaMemcpyDeviceToHost, h->stream));
+            CK(cudaMemcpyAsync(sl.h_counts, c.pb.out_counts, sizeof(int) * n, cudaMemcpyDeviceToHost, c.stream));
+            CK(cudaMemcpyAsync(sl.h_dets, c.pb.out_dets, sizeof(rf_det) * (size_t)n * h->cfg.max_faces, cudaMemcpyDeviceToHost, c.stream));
         }
-        CK(cudaEventRecord(sl.ev_done, h->stream));
+        CK(cudaEventRecord(sl.ev_done, c.stream));
         sl.n = n;
         sl.busy = true;
         sl.gather = gather;
@@ -901,48 +926,20 @@ static int collect_impl(rf_handle h, int ticket, rf_face *out_faces, int *out_co
         CK(cudaSetDevice(h->device));
         CK(cudaEventSynchronize(sl.ev_done));
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    const int mf = h->cfg.max_faces;
-    const rf_det *dets = sl.h_dets;
-    const int *counts = sl.h_counts;
-    int nimg = sl.n;
-    if (gather) {
-        Comm::Slot &cs = h->comm.slots[h->collect_seq % RF_PIPELINE_DEPTH];
-        dets = cs.h_dets; counts = cs.h_counts;
-        if (*h->comm.h_err) {
-            sl.busy = false;
-            h->collect_seq++;
-            return fail(h, RF_ERR_CUDA, fmt("multi-GPU exchange: rank %u never delivered its records of this step", *h->comm.h_err - 1));
-        }
-        // rank r's image i at r * max_batch + i; images beyond a rank's n are reported empty
-        for (int r = 0; r < h->comm.world; r++)
-            for (int i = sl.n; i < h->cfg.max_batch; i++)
-                if (out_counts) out_counts[r * h->cfg.max_batch + i] = 0;
-        for (int r = 0; r < h->comm.world; r++)
-            for (int i = 0; i < sl.n; i++) {
-                const size_t g = (size_t)r * h->cfg.max_batch + i;
-                const int k = std::min(counts[g], mf);
-                if (out_counts) out_counts[g] = k;
-                for (int j = 0; j < k; j++) {
-                    const rf_det &d = dets[g * mf + j];
-                    if (out_faces) out_faces[g * mf + j] = d.face;
-                    if (out_idx) out_idx[g * mf + j] = d.anchor_index;
-                }
-            }
-        sl.busy = false;
-        h->collect_seq++;
-        return RF_OK;
-    }
-    for (int i = 0; i < nimg; i++) {
-        const int k = counts[i];
-        if (out_counts) out_counts[i] = k;
-        for (int j = 0; j < k; j++) {
-            const rf_det &d = dets[(size_t)i * mf + j];
-            if (out_faces) out_faces[(size_t)i * mf + j] = d.face;
-            if (out_idx) out_idx[(size_t)i * mf + j] = d.anchor_index;
-        }
-    }
     sl.busy = false;
     h->collect_seq++;
+    if (!gather) {
+        put_results(h, sl.h_dets, sl.h_counts, 0, sl.n, out_faces, out_counts, out_idx);
+        return RF_OK;
+    }
+    const Comm::Slot &cs = h->comm.slots[(unsigned)ticket % RF_PIPELINE_DEPTH];
+    if (*h->comm.h_err) return fail(h, RF_ERR_CUDA, fmt("multi-GPU exchange: rank %u never delivered its records of this step", *h->comm.h_err - 1));
+    // rank r's image i at r * max_batch + i; images beyond a rank's n are reported empty
+    const size_t mb = h->cfg.max_batch;
+    for (int r = 0; r < h->comm.world; r++) {
+        put_results(h, cs.h_dets, cs.h_counts, r * mb, sl.n, out_faces, out_counts, out_idx);
+        if (out_counts) std::fill(out_counts + r * mb + sl.n, out_counts + (r + 1) * mb, 0);
+    }
     return RF_OK;
 }
 
@@ -959,25 +956,6 @@ int rf_detect_batch_allgather(rf_handle h, const uint8_t *const *imgs, int n, fl
     return rf_collect_batch_allgather(h, t, out_faces, out_counts, out_idx);
 }
 
-static void ensure_merge_buffers(rf_handle h) {
-    PostBuffers &pb = h->pb_merge;
-    if (pb.cand_keys) return;
-    const int A = h->cfg.max_batch * h->cfg.max_faces;       // every view may contribute max_faces candidates
-    int ap2 = 1;
-    while (ap2 < A) ap2 <<= 1;
-    pb.anchors_per_image = A; pb.anchors_pow2 = ap2; pb.max_faces = h->cfg.max_faces; pb.max_batch = 1;
-    CK(cudaMalloc(&pb.cand_keys, sizeof(unsigned long long) * (size_t)A));
-    CK(cudaMalloc(&pb.cand_recs, sizeof(rf_det) * (size_t)A));
-    CK(cudaMalloc(&pb.cand_count, sizeof(int)));
-    CK(cudaMemset(pb.cand_count, 0, sizeof(int)));
-    CK(cudaMalloc(&pb.sort_scratch, sizeof(unsigned long long) * (size_t)ap2));
-    CK(cudaMalloc(&pb.flag_scratch, (size_t)ap2));
-    CK(cudaMalloc(&pb.out_dets, sizeof(rf_det) * (size_t)pb.max_faces));
-    CK(cudaMalloc(&pb.out_counts, sizeof(int)));
-    CK(cudaMalloc(&pb.out_total_kept, sizeof(int)));
-    CK(cudaMemset(pb.out_counts, 0, sizeof(int)));
-}
-
 int rf_detect_views(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, const rf_view *views, int nviews, float thr,
                     float nms, rf_face *out_faces, int *out_count, int32_t *out_view_of, float *out_view_scales) {
     if (!h || !bgr || !views || !out_count || width <= 0 || height <= 0) return fail(h, RF_ERR_INVALID_ARG, "rf_detect_views: bad arguments");
@@ -992,9 +970,10 @@ int rf_detect_views(rf_handle h, const uint8_t *bgr, int width, int height, int 
     const int rs = row_stride ? row_stride : width * 3;
     try {
         CK(cudaSetDevice(h->device));
-        switch_ctx(h, 0);
-        ensure_merge_buffers(h);
-        const uint8_t *d_src = upload_raw(h, bgr, width, height, rs);
+        Ctx &c = h->ctx[0];
+        // every view may contribute max_faces candidates to the merged list of the one image
+        if (!h->pb_merge.cand_keys) alloc_post_buffers(h->pb_merge, h->cfg.max_batch * mf, 1, mf);
+        const uint8_t *d_src = upload_raw(h, c.stream, bgr, width, height, rs);
         ViewSet vs{};
         vs.nviews = nviews;
         vs.img_w_minus1 = (float)(width - 1);
@@ -1006,14 +985,14 @@ int rf_detect_views(rf_handle h, const uint8_t *bgr, int width, int height, int 
             vs.scale[v] = letterbox_fill(lb[v], d_src, width, height, h->d_input + (size_t)v * img_bytes, bw, bh, vs.flip[v], area);
             if (out_view_scales) out_view_scales[v] = vs.scale[v];
         }
-        CK(launch_letterbox_batch(lb.data(), nviews, Wn, Hn, h->stream));     // all views of the image: one launch
-        set_params(h, thr, nms);
-        forward_graph(h, nviews);
-        launch_merge_views(h->pb, vs, h->pb_merge, h->stream);
-        launch_nms(1, h->d_params, h->pb_merge, h->stream);
-        CK(cudaMemcpyAsync(h->h_counts, h->pb_merge.out_counts, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-        CK(cudaMemcpyAsync(h->h_dets, h->pb_merge.out_dets, sizeof(rf_det) * (size_t)mf, cudaMemcpyDeviceToHost, h->stream));
-        CK(cudaStreamSynchronize(h->stream));
+        CK(launch_letterbox_batch(lb.data(), nviews, Wn, Hn, c.stream));     // all views of the image: one launch
+        set_params(h, c, thr, nms);
+        forward_graph(h, c, nviews);
+        launch_merge_views(c.pb, vs, h->pb_merge, c.stream);
+        launch_nms(1, c.d_params, h->pb_merge, c.stream);
+        CK(cudaMemcpyAsync(h->h_counts, h->pb_merge.out_counts, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
+        CK(cudaMemcpyAsync(h->h_dets, h->pb_merge.out_dets, sizeof(rf_det) * (size_t)mf, cudaMemcpyDeviceToHost, c.stream));
+        CK(cudaStreamSynchronize(c.stream));
         const int k = h->h_counts[0];
         *out_count = k;
         for (int j = 0; j < k; j++) {
@@ -1031,13 +1010,13 @@ int rf_preprocess(rf_handle h, const uint8_t *bgr, int width, int height, int ro
     const int rs = row_stride ? row_stride : width * 3;
     try {
         CK(cudaSetDevice(h->device));
-        switch_ctx(h, 0);
-        const uint8_t *d_src = upload_raw(h, bgr, width, height, rs);
+        cudaStream_t s = h->ctx[0].stream;
+        const uint8_t *d_src = upload_raw(h, s, bgr, width, height, rs);
         LbItem it;
         letterbox_fill(it, d_src, width, height, h->d_input, Wn, Hn, 0, (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0);
-        CK(launch_letterbox_batch(&it, 1, Wn, Hn, h->stream));
-        CK(cudaMemcpyAsync(h->h_input, h->d_input, (size_t)Hn * Wn * 3, cudaMemcpyDeviceToHost, h->stream));
-        CK(cudaStreamSynchronize(h->stream));
+        CK(launch_letterbox_batch(&it, 1, Wn, Hn, s));
+        CK(cudaMemcpyAsync(h->h_input, h->d_input, (size_t)Hn * Wn * 3, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
         memcpy(out, h->h_input, (size_t)Hn * Wn * 3);
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
@@ -1055,20 +1034,18 @@ int rf_forward_heads(rf_handle h, const uint8_t *bgr, int n, float *const heads_
     if (!bgr || !heads_out) return fail(h, RF_ERR_INVALID_ARG, "rf_forward_heads: NULL argument");
     try {
         CK(cudaSetDevice(h->device));
-        switch_ctx(h, 0);
+        Ctx &c = h->ctx[0];
         ensure_blobs(h);
         const size_t bytes = (size_t)n * h->cfg.net_h * h->cfg.net_w * 3;
-        CK(cudaStreamSynchronize(h->stream));
+        CK(cudaStreamSynchronize(c.stream));
         memcpy(h->h_input, bgr, bytes);
-        CK(cudaMemcpyAsync(h->d_input, h->h_input, bytes, cudaMemcpyHostToDevice, h->stream));
-        set_params(h, h->cur_thr, h->cur_nms);
-        h->blobs_in_plan = true;
-        try { run_steps(h, n, h->stream); } catch (...) { h->blobs_in_plan = false; throw; }
-        h->blobs_in_plan = false;
+        CK(cudaMemcpyAsync(h->d_input, h->h_input, bytes, cudaMemcpyHostToDevice, c.stream));
+        set_params(h, c, c.cur_thr, c.cur_nms);
+        run_steps(h, Run{c, n, c.stream, h->d_blobs});
         CK(cudaGetLastError());
         for (int i = 0; i < 9; i++)
-            CK(cudaMemcpyAsync(heads_out[i], h->d_blobs[i], sizeof(float) * h->blob_elems[i] * n, cudaMemcpyDeviceToHost, h->stream));
-        CK(cudaStreamSynchronize(h->stream));
+            CK(cudaMemcpyAsync(heads_out[i], h->d_blobs[i], sizeof(float) * h->blob_elems[i] * n, cudaMemcpyDeviceToHost, c.stream));
+        CK(cudaStreamSynchronize(c.stream));
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }
@@ -1081,16 +1058,16 @@ int rf_postprocess(rf_handle h, const float *const heads[9], int n, float thr, f
     if (!heads) return fail(h, RF_ERR_INVALID_ARG, "rf_postprocess: NULL heads");
     try {
         CK(cudaSetDevice(h->device));
-        switch_ctx(h, 0);
+        Ctx &c = h->ctx[0];
         ensure_blobs(h);
         for (int i = 0; i < 9; i++)
-            CK(cudaMemcpyAsync(h->d_blobs[i], heads[i], sizeof(float) * h->blob_elems[i] * n, cudaMemcpyHostToDevice, h->stream));
-        set_params(h, thr, nms);
-        launch_blob_decode(h->d_blobs, h->lv, n, h->cfg.net_w, h->cfg.net_h, h->d_params, h->pb, h->stream);
-        if (out_ncand) CK(cudaMemcpyAsync(h->h_counts + h->cfg.max_batch, h->pb.cand_count, sizeof(int) * n, cudaMemcpyDeviceToHost, h->stream));
-        launch_nms(n, h->d_params, h->pb, h->stream);
+            CK(cudaMemcpyAsync(h->d_blobs[i], heads[i], sizeof(float) * h->blob_elems[i] * n, cudaMemcpyHostToDevice, c.stream));
+        set_params(h, c, thr, nms);
+        launch_blob_decode(h->d_blobs, h->lv, n, h->cfg.net_w, h->cfg.net_h, c.d_params, c.pb, c.stream);
+        if (out_ncand) CK(cudaMemcpyAsync(h->h_counts + h->cfg.max_batch, c.pb.cand_count, sizeof(int) * n, cudaMemcpyDeviceToHost, c.stream));
+        launch_nms(n, c.d_params, c.pb, c.stream);
         CK(cudaGetLastError());
-        fetch_results(h, n, out_faces, out_counts, out_idx, nullptr);
+        fetch_results(h, c, n, out_faces, out_counts, out_idx);
         if (out_ncand) for (int i = 0; i < n; i++) out_ncand[i] = h->h_counts[h->cfg.max_batch + i];
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
@@ -1109,11 +1086,11 @@ int rf_debug_get_tensor(rf_handle h, const char *name, int n, float *out_nchw, i
     if (!out_nchw) return RF_OK;
     try {
         CK(cudaSetDevice(h->device));
-        switch_ctx(h, 0);
-        CK(cudaStreamSynchronize(h->stream));
+        const Ctx &x = h->ctx[0];
+        CK(cudaStreamSynchronize(x.stream));
         size_t elems = (size_t)n * t.h * t.w * t.c;
         std::vector<unsigned char> host(elems * h->elem);
-        CK(cudaMemcpy(host.data(), h->tptr(it->second), host.size(), cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(host.data(), x.arena + t.offset, host.size(), cudaMemcpyDeviceToHost));
         for (int b = 0; b < n; b++)
             for (int y = 0; y < t.h; y++)
                 for (int x = 0; x < t.w; x++)
@@ -1136,16 +1113,11 @@ int rf_debug_keep_all(rf_handle h) {
         CK(cudaSetDevice(h->device));
         for (auto &t : h->tensors) { t.first = -1; t.last = -1; }
         place_tensors(h, true);
-        for (int c = 0; c < h->nctx; c++) {
-            switch_ctx(h, c);
-            CK(cudaStreamSynchronize(h->stream));
-            for (auto &g : h->graphs) cudaGraphExecDestroy(g.second);
-            h->graphs.clear();
-            CK(cudaFree(h->arena));
-            h->arena = nullptr;
-            CK(cudaMalloc(&h->arena, h->arena_bytes));
+        for (Ctx &c : h->ctx) {
+            CK(cudaStreamSynchronize(c.stream));
+            release_ctx(c, false);
+            create_ctx(h, c, false);
         }
-        switch_ctx(h, 0);
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }
@@ -1165,37 +1137,37 @@ int rf_calibrate_int8(rf_handle h, const uint8_t *bgr_net_sized, int n_images, c
         CK(cudaSetDevice(h->device));
         int rc = rf_debug_keep_all(h);
         if (rc) return rc;
-        switch_ctx(h, 0);
+        Ctx &c = h->ctx[0];
         CK(cudaMalloc(&d_max, sizeof(float) * T));
         CK(cudaMalloc(&d_hist, sizeof(unsigned) * (size_t)T * CALIB_BINS));
-        CK(cudaMemsetAsync(d_max, 0, sizeof(float) * T, h->stream));
-        CK(cudaMemsetAsync(d_hist, 0, sizeof(unsigned) * (size_t)T * CALIB_BINS, h->stream));
+        CK(cudaMemsetAsync(d_max, 0, sizeof(float) * T, c.stream));
+        CK(cudaMemsetAsync(d_hist, 0, sizeof(unsigned) * (size_t)T * CALIB_BINS, c.stream));
         std::vector<float> hmax(T, 0.f);
         for (int pass = 0; pass < 2; pass++) {
             for (int i0 = 0; i0 < n_images; i0 += h->cfg.max_batch) {
                 const int n = std::min(h->cfg.max_batch, n_images - i0);
-                CK(cudaStreamSynchronize(h->stream));
+                CK(cudaStreamSynchronize(c.stream));
                 memcpy(h->h_input, bgr_net_sized + (size_t)i0 * img_bytes, (size_t)n * img_bytes);
-                CK(cudaMemcpyAsync(h->d_input, h->h_input, (size_t)n * img_bytes, cudaMemcpyHostToDevice, h->stream));
-                set_params(h, h->cur_thr, h->cur_nms);
-                run_steps(h, n, h->stream, false);
+                CK(cudaMemcpyAsync(h->d_input, h->h_input, (size_t)n * img_bytes, cudaMemcpyHostToDevice, c.stream));
+                set_params(h, c, c.cur_thr, c.cur_nms);
+                run_steps(h, Run{c, n, c.stream}, false);
                 for (int t = 0; t < T; t++) {
                     const TensorInfo &ti = h->tensors[t];
                     const size_t elems = (size_t)n * ti.h * ti.w * ti.c;
-                    const float *x = reinterpret_cast<const float *>(h->tptr(t));
-                    if (pass == 0) launch_absmax<float>(x, elems, d_max + t, h->stream);
-                    else if (hmax[t] > 0.f) launch_hist<float>(x, elems, (float)CALIB_BINS / hmax[t], d_hist + (size_t)t * CALIB_BINS, h->stream);
+                    const float *x = reinterpret_cast<const float *>(c.arena + ti.offset);
+                    if (pass == 0) launch_absmax<float>(x, elems, d_max + t, c.stream);
+                    else if (hmax[t] > 0.f) launch_hist<float>(x, elems, (float)CALIB_BINS / hmax[t], d_hist + (size_t)t * CALIB_BINS, c.stream);
                 }
                 CK(cudaGetLastError());
             }
             if (pass == 0) {
-                CK(cudaMemcpyAsync(hmax.data(), d_max, sizeof(float) * T, cudaMemcpyDeviceToHost, h->stream));
-                CK(cudaStreamSynchronize(h->stream));
+                CK(cudaMemcpyAsync(hmax.data(), d_max, sizeof(float) * T, cudaMemcpyDeviceToHost, c.stream));
+                CK(cudaStreamSynchronize(c.stream));
             }
         }
         std::vector<unsigned> hist((size_t)T * CALIB_BINS);
-        CK(cudaMemcpyAsync(hist.data(), d_hist, sizeof(unsigned) * hist.size(), cudaMemcpyDeviceToHost, h->stream));
-        CK(cudaStreamSynchronize(h->stream));
+        CK(cudaMemcpyAsync(hist.data(), d_hist, sizeof(unsigned) * hist.size(), cudaMemcpyDeviceToHost, c.stream));
+        CK(cudaStreamSynchronize(c.stream));
         cudaFree(d_max); cudaFree(d_hist);
         d_max = nullptr; d_hist = nullptr;
         std::vector<std::pair<std::string, float>> scales;
@@ -1294,13 +1266,7 @@ int rf_plan_describe(const rf_config *cfg, char *out, int cap) {
     if (!build_mnet_model(layers, h->model, err)) return fail(nullptr, RF_ERR_MODEL, err);
     if (cfg->int8_table_path && !read_int8_table(cfg->int8_table_path, h->int8_scales, err)) return fail(nullptr, RF_ERR_IO, err);
     try {
-        h->use_tc = cfg->precision == RF_PREC_INT8 || (cfg->precision == RF_PREC_FP16 && !(cfg->flags & RF_FLAG_NO_TENSORCORE));
-        if (cfg->precision == RF_PREC_INT8) build_plan_i8(h);
-        else if (cfg->precision == RF_PREC_FP32) build_plan<float>(h);
-        else if (h->use_tc && !(cfg->flags & RF_FLAG_LEGACY_TC)) build_plan_tiles(h);
-        else build_plan<__half>(h);
-        link_steps(h);
-        place_tensors(h, false);
+        make_plan(h, false);
     } catch (const CudaFail &f) { return fail_cuda(nullptr, f); }
     catch (const PlanFail &f) { return fail(nullptr, f.status, f.msg); }
     std::string text = fmt("%d launches per forward, activation arena %zu bytes per batch of %d\n", (int)h->steps.size(), h->arena_bytes, cfg->max_batch);
@@ -1317,53 +1283,39 @@ int rf_profile_layers(rf_handle h, int n, int iters, char (*names)[64], float *m
     int cnt = 0;
     try {
         CK(cudaSetDevice(h->device));
-        switch_ctx(h, 0);
-        set_params(h, h->cur_thr, h->cur_nms);
-        run_steps(h, n, h->stream, false);  // warm everything once (also leaves consistent inputs for every step)
-        CK(cudaStreamSynchronize(h->stream));
-        struct ProfGuard { rf_handle h; ~ProfGuard() { h->profiling = false; } } guard{h};
-        h->profiling = true;
-        for (size_t si = 0; si < h->steps.size(); si++) {
-            auto &st = h->steps[si];
-            if (cnt >= cap) break;
-            if ((int)si == h->head_step + 1) {
-                // sort+nms consumes the candidate list: give every timed launch a fresh one
-                float acc = 0;
-                for (int i = 0; i < iters; i++) {
-                    h->steps[h->head_step].launch(n, h->stream);
-                    CK(cudaEventRecord(h->ev0, h->stream));
-                    st.launch(n, h->stream);
-                    CK(cudaEventRecord(h->ev1, h->stream));
-                    CK(cudaEventSynchronize(h->ev1));
-                    float t = 0;
-                    CK(cudaEventElapsedTime(&t, h->ev0, h->ev1));
-                    acc += t;
-                }
-                snprintf(names[cnt], 64, "%s", st.name.c_str());
-                ms[cnt] = acc / iters;
-                if (bytes) bytes[cnt] = st.bytes_per_img * n;
-                if (flops) flops[cnt] = st.flops_per_img * n;
-                cnt++;
-                continue;
+        Ctx &c = h->ctx[0];
+        set_params(h, c, c.cur_thr, c.cur_nms);
+        run_steps(h, Run{c, n, c.stream}, false);  // warm everything once (also leaves consistent inputs for every step)
+        CK(cudaStreamSynchronize(c.stream));
+        const Run one{c, n, c.stream, nullptr, true};
+        for (size_t si = 0; si < h->steps.size() && cnt < cap; si++) {
+            const Step &st = h->steps[si];
+            // sort+nms consumes the candidate list: it is timed launch by launch, each behind a fresh list from the head step
+            const bool fresh = (int)si == h->head_step + 1;
+            const int rounds = fresh ? iters : 1;
+            if (!fresh) st.launch(one);
+            float acc = 0;
+            for (int r = 0; r < rounds; r++) {
+                if (fresh) h->steps[h->head_step].launch(one);
+                CK(cudaEventRecord(h->ev0, c.stream));
+                for (int i = 0; i < iters / rounds; i++) st.launch(one);
+                CK(cudaEventRecord(h->ev1, c.stream));
+                CK(cudaEventSynchronize(h->ev1));
+                float t = 0;
+                CK(cudaEventElapsedTime(&t, h->ev0, h->ev1));
+                acc += t;
             }
-            st.launch(n, h->stream);
-            CK(cudaEventRecord(h->ev0, h->stream));
-            for (int i = 0; i < iters; i++) st.launch(n, h->stream);
-            CK(cudaEventRecord(h->ev1, h->stream));
-            CK(cudaEventSynchronize(h->ev1));
-            float t = 0;
-            CK(cudaEventElapsedTime(&t, h->ev0, h->ev1));
             snprintf(names[cnt], 64, "%s", st.name.c_str());
-            ms[cnt] = t / iters;
+            ms[cnt] = acc / iters;
             if (bytes) bytes[cnt] = st.bytes_per_img * n;
             if (flops) flops[cnt] = st.flops_per_img * n;
             cnt++;
         }
         CK(cudaGetLastError());
         // single steps were launched out of their forward: leave the last-block / candidate counters as a forward expects them
-        CK(cudaMemsetAsync(h->pb.tile_done, 0, sizeof(int) * h->cfg.max_batch, h->stream));
-        CK(cudaMemsetAsync(h->pb.cand_count, 0, sizeof(int) * h->cfg.max_batch, h->stream));
-        CK(cudaStreamSynchronize(h->stream));
+        CK(cudaMemsetAsync(c.pb.tile_done, 0, sizeof(int) * h->cfg.max_batch, c.stream));
+        CK(cudaMemsetAsync(c.pb.cand_count, 0, sizeof(int) * h->cfg.max_batch, c.stream));
+        CK(cudaStreamSynchronize(c.stream));
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return cnt;
 }

@@ -61,10 +61,36 @@ struct TensorInfo {
     size_t offset = 0;  // bytes into the arena (already scaled by max_batch)
 };
 
+// One execution context: everything a forward pass writes (activation arena, candidate / output buffers, run parameters)
+// and everything it is issued on (stream, lane streams, events, captured graphs).  The asynchronous entry points rotate
+// through the handle's contexts so that consecutive batches overlap on the GPU (most kernels of one batch-8 step fill well
+// under one wave of the 132 SMs).
+struct Ctx {
+    static constexpr int kParamSlots = 1024;
+    cudaStream_t stream = nullptr, lane_stream[3] = {nullptr, nullptr, nullptr};   // [0] unused (lane 0 runs on `stream`)
+    std::vector<cudaEvent_t> step_event;
+    unsigned char *arena = nullptr;
+    PostBuffers pb{};
+    PostParams *d_params = nullptr, *h_params = nullptr;   // h_params: pinned ring of kParamSlots (set_params)
+    unsigned param_seq = 0;
+    float cur_thr = 0.5f, cur_nms = 0.4f;
+    std::map<int, cudaGraphExec_t> graphs;
+    cudaEvent_t fence = nullptr;
+};
+
+// What one step launch writes into and where it is issued.
+struct Run {
+    const Ctx &ctx;                  // arena, pb, d_params
+    int n;
+    cudaStream_t stream;
+    float *const *blobs = nullptr;   // rf_forward_heads: the head step also writes the nine raw head blobs here
+    bool single = false;             // rf_profile_layers: a step launched on its own, out of its forward (no last-block NMS)
+};
+
 struct Step {
     std::string name;
     std::vector<int> in, out;
-    std::function<void(int /*n*/, cudaStream_t)> launch;
+    std::function<void(const Run &)> launch;
     double flops_per_img = 0, bytes_per_img = 0;  // algorithmic
     int lane = 0;                 // 0 = main stream; 1, 2 = side branches of the forward graph
     std::vector<int> deps;        // producer steps in OTHER lanes this step must wait for (filled by link_steps)
@@ -100,7 +126,6 @@ struct rf_handle_s {
     int device = 0;
     int num_sms = RF_NUM_SMS;   // plan heuristics ("does this layer fill one wave") and the persistent tile-chain grid
     int elem = 4;  // bytes per activation element
-    cudaStream_t stream = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
 
     std::vector<TensorInfo> tensors;
@@ -111,12 +136,10 @@ struct rf_handle_s {
     unsigned tile_mask = 0;                           // which parts of the FP16 plan run as tile chains (RF_TILE_MASK)
     int lane_last[3] = {-1, -1, -1};                  // last step of each side lane (joined at the end of the forward)
     int cache_status = 0;                             // model.h CACHE_*: how the folded model was obtained
-    bool profiling = false;                           // rf_profile_layers is launching single steps out of their forward
     int tile_expected = 0;                            // tiles per image over the three SSH chains (last-block NMS)
     std::vector<float> tile_bias_tmp;                 // plan-time scratch
     unsigned *tile_dbg = nullptr, *tile_dbg_dev = nullptr;   // host-mapped word a timed-out hand-off of a tile chain reports into
-    unsigned char *arena = nullptr;
-    size_t arena_bytes = 0;
+    size_t arena_bytes = 0;                           // of each context's arena
 
     // weights
     std::vector<float> wstage;  // host staging of all fp32 weights
@@ -144,8 +167,6 @@ struct rf_handle_s {
     void *d_align_crops = nullptr;
     size_t align_crops_bytes = 0;
     double *d_align_mats = nullptr;
-    PostParams *d_params = nullptr, *h_params = nullptr;
-    PostBuffers pb{};
     LevelDesc lv[3];
     HeadWeights hw[3];
     int feat_tensor[3] = {-1, -1, -1};
@@ -153,7 +174,6 @@ struct rf_handle_s {
     size_t blob_elems[9] = {0};       // per image
     rf_det *h_dets = nullptr;         // pinned [max_batch][max_faces]
     int *h_counts = nullptr;          // pinned [2*max_batch]: kept, candidates
-    std::map<int, cudaGraphExec_t> graphs;
     // pipelined end-to-end path (rf_submit_batch / rf_collect_batch)
     struct Slot {
         uint8_t *d_in = nullptr, *h_in = nullptr;     // device input, pinned staging for pageable sources
@@ -165,61 +185,14 @@ struct rf_handle_s {
     } slots[RF_PIPELINE_DEPTH];
     cudaStream_t copy_stream = nullptr;
     unsigned submit_seq = 0, collect_seq = 0;
-    cudaStream_t lane_stream[3] = {nullptr, nullptr, nullptr};   // [0] unused (the caller's stream is lane 0)
-    std::vector<cudaEvent_t> step_event;
-    bool blobs_in_plan = false;       // head step writes blobs (forward_heads path)
-    static constexpr int kParamSlots = 1024;
-    unsigned param_seq = 0;
-    float cur_thr = 0.5f, cur_nms = 0.4f;
-
-    void *tptr(int id) const { return arena + tensors[id].offset; }
-
-    // Execution contexts.  Everything a forward pass writes (activation arena, candidate / output buffers,
-    // run parameters) and everything it is issued on (stream, lane streams, events, captured graphs) exists
-    // once per context; the asynchronous entry points rotate through the contexts so that consecutive batches
-    // overlap on the GPU (most kernels of one batch-8 step fill well under one wave of the 132 SMs).  The
-    // members above always hold the ACTIVE context; switch_ctx() swaps them with a saved one.
-    struct Ctx {
-        cudaStream_t stream = nullptr, lane_stream[3] = {nullptr, nullptr, nullptr};
-        std::vector<cudaEvent_t> step_event;
-        unsigned char *arena = nullptr;
-        PostBuffers pb{};
-        PostParams *d_params = nullptr, *h_params = nullptr;
-        unsigned param_seq = 0;
-        float cur_thr = 0.5f, cur_nms = 0.4f;
-        std::map<int, cudaGraphExec_t> graphs;
-        cudaEvent_t fence = nullptr;
-    };
-    std::vector<Ctx> saved;
-    int active = 0, nctx = 1;
+    // execution contexts (Ctx): the blocking entry points run on context 0, the asynchronous ones rotate through all
+    std::vector<Ctx> ctx;
     unsigned next_dev_ctx = 0;
-    cudaStream_t last_stream = nullptr;
-    cudaEvent_t fence = nullptr;
+    cudaStream_t last_stream = nullptr;   // of the last device-resident call (rf_last_stream)
     void *jpeg = nullptr;             // nvJPEG decoder state (jpeg.cu), created by the first JPEG call
 };
 
 namespace rf_eng {
-inline void switch_ctx(rf_handle h, int i) {
-    if (i == h->active) return;
-    auto xchg = [&](rf_handle_s::Ctx &c) {
-        std::swap(c.stream, h->stream);
-        for (int l = 0; l < 3; l++) std::swap(c.lane_stream[l], h->lane_stream[l]);
-        std::swap(c.step_event, h->step_event);
-        std::swap(c.arena, h->arena);
-        std::swap(c.pb, h->pb);
-        std::swap(c.d_params, h->d_params);
-        std::swap(c.h_params, h->h_params);
-        std::swap(c.param_seq, h->param_seq);
-        std::swap(c.cur_thr, h->cur_thr);
-        std::swap(c.cur_nms, h->cur_nms);
-        std::swap(c.graphs, h->graphs);
-        std::swap(c.fence, h->fence);
-    };
-    xchg(h->saved[h->active]);   // park the active state in its slot
-    xchg(h->saved[i]);           // and bring context i in
-    h->active = i;
-}
-
 inline int fail(rf_handle h, int code, const std::string &msg) {
     if (h) h->err = msg; else create_error() = msg;
     return code;
@@ -288,7 +261,7 @@ cudaError_t tile_init();
 std::string describe_chains(rf_handle h);
 // ---- exported by comm.cu --------------------------------------------------------------------------------------------
 void comm_release(rf_handle h);
-void comm_wait_in_graph(rf_handle h, int n, cudaStream_t s);   // last node of the forward once a communicator exists
+void comm_wait_in_graph(rf_handle h, const Ctx &c, int n, cudaStream_t s);   // last node of the forward once a communicator exists
 // ---- exported by jpeg.cu (f1 ingest: nvJPEG decode into device memory) ------------------------------------------------
 int jpeg_info(rf_handle h, const uint8_t *data, size_t len, int *w, int *hgt);
 int jpeg_decode(rf_handle h, const uint8_t *const *data, const size_t *len, int n, uint8_t *const *dst, const int *w, const int *hgt, cudaStream_t s);

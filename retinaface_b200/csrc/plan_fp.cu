@@ -183,7 +183,7 @@ std::vector<__half> make_stem_blob(const std::vector<float> &w0, const std::vect
 int plan_pair_legacy(Builder &B, int i, int tin, int ih, int iw) {
     rf_handle h = B.h;
     const Model &m = h->model;
-    auto T_ = [h](int id) { return reinterpret_cast<__half *>(h->tptr(id)); };
+    auto T_ = [h](const Run &r, int id) { return reinterpret_cast<__half *>(r.ctx.arena + h->tensors[id].offset); };
     auto Wd = [h](size_t off) { return h->d_weights + off; };
     const double es = h->elem;
     const FoldedConv &dw = m.conv("mobilenet0_conv" + std::to_string(i) + "_fwd");
@@ -211,23 +211,23 @@ int plan_pair_legacy(Builder &B, int i, int tin, int ih, int iw) {
     // table, vertical reuse
     const bool tiles2d = oh * ow_ > 56 * 56 && C >= 16 && C <= 64 && geo.nsplit == 1 && !(h->cfg.flags & RF_FLAG_DW_1D);
     if (tiles2d) s.name = fmt("tc2d_dw%d+pw%d_s%d_%dto%d", i, i + 1, S, C, N);
-    s.launch = [=](int n, cudaStream_t st) {
+    s.launch = [=](const Run &r) {
         if (tiles2d) {
             TcDw2dArgs a{};
-            a.in = T_(tin); a.C = C; a.nimg = n; a.IH = ih; a.IW = iw; a.OH = oh; a.OW = ow_; a.S = S; a.N = N;
+            a.in = T_(r, tin); a.C = C; a.nimg = r.n; a.IH = ih; a.IW = iw; a.OH = oh; a.OW = ow_; a.S = S; a.N = N;
             a.TH = 8;
             const int t16 = (ow_ + 15) / 16, t14 = (ow_ + 13) / 14;
             a.TW = t14 < t16 ? 14 : 16;
             tc_dw2d_finish(a);
-            a.wimg = h->d_weights_h + oimg; a.bias = Wd(obp); a.dw_w = Wd(owd); a.dw_b = Wd(obd); a.out = T_(tpw);
-            launch_tc_dwpw_2d(a, st);
+            a.wimg = h->d_weights_h + oimg; a.bias = Wd(obp); a.dw_w = Wd(owd); a.dw_b = Wd(obd); a.out = T_(r, tpw);
+            launch_tc_dwpw_2d(a, r.stream);
             return;
         }
         TcDwArgs a{};
-        a.in = T_(tin); a.C = C; a.nimg = n; a.IH = ih; a.IW = iw; a.OH = oh; a.OW = ow_; a.S = S;
+        a.in = T_(r, tin); a.C = C; a.nimg = r.n; a.IH = ih; a.IW = iw; a.OH = oh; a.OW = ow_; a.S = S;
         a.N = N / geo.nsplit; a.Ntotal = N; a.Kpad = Kpad; a.rows = geo.rows; a.Wp = iw + 2; a.Hp = ih + 1; a.Rmax = geo.Rmax;
-        a.wimg = h->d_weights_h + oimg; a.bias = Wd(obp); a.dw_w = Wd(owd); a.dw_b = Wd(obd); a.out = T_(tpw);
-        launch_tc_dwpw(a, geo.nsplit, st);
+        a.wimg = h->d_weights_h + oimg; a.bias = Wd(obp); a.dw_w = Wd(owd); a.dw_b = Wd(obd); a.out = T_(r, tpw);
+        launch_tc_dwpw(a, geo.nsplit, r.stream);
     };
     B.step(std::move(s));
     return tpw;
@@ -239,7 +239,7 @@ void plan_conv_legacy(Builder &B, const std::string &sname, std::vector<const Fo
                       int off0, int n0, int relu0, int t1, int ld1, int off1, int relu1, int lane, int tup, int up_which) {
     rf_handle h = B.h;
     const Model &m = h->model;
-    auto T_ = [h](int id) { return reinterpret_cast<__half *>(h->tptr(id)); };
+    auto T_ = [h](const Run &r, int id) { return reinterpret_cast<__half *>(r.ctx.arena + h->tensors[id].offset); };
     auto Wd = [h](size_t off) { return h->d_weights + off; };
     const double es = h->elem;
     std::vector<float> bias;
@@ -263,15 +263,15 @@ void plan_conv_legacy(Builder &B, const std::string &sname, std::vector<const Fo
     if (t1 >= 0) s.out.push_back(t1);
     s.flops_per_img = 2.0 * ih * iw * cin * ks * ks * N + (tup >= 0 ? 2.0 * ih * iw * cin * 4 : 0.0);
     s.bytes_per_img = ((double)ih * iw * cin + (double)ih * iw * N + (tup >= 0 ? (double)(ih / 2) * (iw / 2) * cin : 0.0)) * es;
-    s.launch = [=](int n, cudaStream_t st) {
+    s.launch = [=](const Run &r) {
         TcConvArgs a{};
-        a.in = T_(tin); a.Cin = cin; a.nimg = n; a.H = ih; a.W = iw; a.taps = ks * ks; a.N = N;
+        a.in = T_(r, tin); a.Cin = cin; a.nimg = r.n; a.H = ih; a.W = iw; a.taps = ks * ks; a.N = N;
         a.Wp = ks == 3 ? iw + 2 : iw; a.Hp = ks == 3 ? ih + 1 : ih;
         a.R = (ks == 3 ? 128 + 2 * (iw + 3) : 128) | 1;
         a.wimg = h->d_weights_h + oimg; a.bias = Wd(ob);
-        a.out = TcOut{T_(t0) + off0, ld0, n0, relu0, t1 >= 0 ? T_(t1) + off1 : nullptr, ld1, relu1};
-        if (tup >= 0) { a.up = T_(tup); a.up_w = Wd(oup); a.Cmax = (((a.R / a.Wp + 2) / 2 + 3) * (iw / 2)) | 1; }
-        launch_tc_conv(a, st);
+        a.out = TcOut{T_(r, t0) + off0, ld0, n0, relu0, t1 >= 0 ? T_(r, t1) + off1 : nullptr, ld1, relu1};
+        if (tup >= 0) { a.up = T_(r, tup); a.up_w = Wd(oup); a.Cmax = (((a.R / a.Wp + 2) / 2 + 3) * (iw / 2)) | 1; }
+        launch_tc_conv(a, r.stream);
     };
     B.step(std::move(s));
 }
@@ -280,7 +280,7 @@ void plan_conv_legacy(Builder &B, const std::string &sname, std::vector<const Fo
 int plan_fpn_merge_h2(Builder &B, const std::string &name, int tlat, int tup, int fh, int fw, int which) {
     rf_handle h = B.h;
     const Model &m = h->model;
-    auto T_ = [h](int id) { return reinterpret_cast<__half *>(h->tptr(id)); };
+    auto T_ = [h](const Run &r, int id) { return reinterpret_cast<__half *>(r.ctx.arena + h->tensors[id].offset); };
     const double es = h->elem;
     std::vector<__half> uwh(16 * 64);
     for (int c = 0; c < 64; c++)
@@ -292,10 +292,10 @@ int plan_fpn_merge_h2(Builder &B, const std::string &name, int tlat, int tup, in
     s.in = {tlat, tup}; s.out = {plus};
     s.flops_per_img = 2.0 * fh * fw * 64 * 4;
     s.bytes_per_img = ((double)fh * fw * 64 * 2 + (double)(fh / 2) * (fw / 2) * 64) * es;
-    s.launch = [=](int n, cudaStream_t st) {
+    s.launch = [=](const Run &r) {
         // 128 threads per block: a 56-pixel row is 448 (pixel, 8-channel) items = 3.5 blocks
-        CK(launch_k(k_fpn_merge_h2, dim3((unsigned)((fw * 8 + 127) / 128), (unsigned)fh, (unsigned)n), dim3(128), 0, st, (const __half *)T_(tlat), (const __half *)T_(tup),
-                    (__half *)T_(plus), (const __half *)(h->d_weights_h + ouw), n, fh, fw, 64));
+        CK(launch_k(k_fpn_merge_h2, dim3((unsigned)((fw * 8 + 127) / 128), (unsigned)fh, (unsigned)r.n), dim3(128), 0, r.stream, (const __half *)T_(r, tlat), (const __half *)T_(r, tup),
+                    (__half *)T_(r, plus), (const __half *)(h->d_weights_h + ouw), r.n, fh, fw, 64));
     };
     B.step(std::move(s));
     return plus;
@@ -306,7 +306,7 @@ template <typename T>
 void plan_heads_and_nms(Builder &B, bool with_heads, bool with_nms) {
     rf_handle h = B.h;
     const Model &m = h->model;
-    auto T_ = [h](int id) { return reinterpret_cast<T *>(h->tptr(id)); };
+    auto T_ = [h](const Run &r, int id) { return reinterpret_cast<T *>(r.ctx.arena + h->tensors[id].offset); };
     auto Wd = [h](size_t off) { return h->d_weights + off; };
     const double es = h->elem;
     const int H = h->cfg.net_h, W = h->cfg.net_w;
@@ -336,10 +336,10 @@ void plan_heads_and_nms(Builder &B, bool with_heads, bool with_nms) {
         s.bytes_per_img = px * 64 * es;
         int f0 = h->feat_tensor[0], f1 = h->feat_tensor[1], f2 = h->feat_tensor[2];
         size_t w0 = hw_off[0], w1 = hw_off[1], w2 = hw_off[2], b0 = hb_off[0], b1 = hb_off[1], b2 = hb_off[2];
-        s.launch = [=](int n, cudaStream_t st) {
-            const T *feat[3] = {T_(f0), T_(f1), T_(f2)};
+        s.launch = [=](const Run &r) {
+            const T *feat[3] = {T_(r, f0), T_(r, f1), T_(r, f2)};
             HeadWeights hws[3] = {{Wd(w0), Wd(b0), 1.f}, {Wd(w1), Wd(b1), 1.f}, {Wd(w2), Wd(b2), 1.f}};
-            launch_head_decode<T>(feat, hws, h->lv, n, W, H, h->d_params, h->pb, h->blobs_in_plan ? h->d_blobs : nullptr, st, with_nms);
+            launch_head_decode<T>(feat, hws, h->lv, r.n, W, H, r.ctx.d_params, r.ctx.pb, r.blobs, r.stream, with_nms);
         };
         if (with_nms) s.name = "heads_1x1+softmax+decode+nms_all_levels";     // decode -> NMS in one launch (last block per image)
         h->head_step = (int)h->steps.size();
@@ -354,7 +354,7 @@ void plan_heads_and_nms(Builder &B, bool with_heads, bool with_nms) {
         s.in = {h->feat_tensor[0], h->feat_tensor[1], h->feat_tensor[2]};
         s.flops_per_img = 0;
         s.bytes_per_img = 0;
-        s.launch = [=](int n, cudaStream_t st) { launch_nms(n, h->d_params, h->pb, st); };
+        s.launch = [=](const Run &r) { launch_nms(r.n, r.ctx.d_params, r.ctx.pb, r.stream); };
         h->nms_step = (int)h->steps.size();
         B.step(std::move(s));
     }
@@ -367,7 +367,7 @@ int plan_stem_tc(Builder &B) {
     rf_handle h = B.h;
     const Model &m = h->model;
     const int H = h->cfg.net_h, W = h->cfg.net_w;
-    auto T_ = [h](int id) { return reinterpret_cast<__half *>(h->tptr(id)); };
+    auto T_ = [h](const Run &r, int id) { return reinterpret_cast<__half *>(r.ctx.arena + h->tensors[id].offset); };
     auto Wd = [h](size_t off) { return h->d_weights + off; };
     const double es = h->elem;
     const int cur_h = H / 2, cur_w = W / 2;
@@ -391,14 +391,14 @@ int plan_stem_tc(Builder &B) {
     s.out = {out};
     s.flops_per_img = 2.0 * cur_h * cur_w * (8 * 27 + 8 * 9 + 8 * 16);
     s.bytes_per_img = (double)H * W * 3 + (double)cur_h * cur_w * 16 * es;
-    s.launch = [=](int n, cudaStream_t st) {
+    s.launch = [=](const Run &r) {
         const int tiles = ((H / 2 + 15) / 16) * ((W / 2 + 15) / 16);
         if (simt_stem) {
             StemWeights sw{Wd(ow0), Wd(ob0), Wd(owd), Wd(obd), Wd(owp), Wd(obp)};
-            CK(launch_k(k_stem<__half>, dim3((unsigned)(tiles * n)), dim3(256), 0, st, (const PostParams *)h->d_params, (__half *)T_(out), sw, n, H, W, 1.0f));
+            CK(launch_k(k_stem<__half>, dim3((unsigned)(tiles * r.n)), dim3(256), 0, r.stream, (const PostParams *)r.ctx.d_params, (__half *)T_(r, out), sw, r.n, H, W, 1.0f));
         } else {
             StemTcArgs a{reinterpret_cast<const unsigned char *>(h->d_weights_h + oblob)};
-            CK(launch_k(k_stem_tc<__half>, dim3((unsigned)((W / 2 + 15) / 16), (unsigned)((H / 2 + 15) / 16), (unsigned)n), dim3(256), 0, st, (const PostParams *)h->d_params, (__half *)T_(out), a, n, H, W, 1.0f));
+            CK(launch_k(k_stem_tc<__half>, dim3((unsigned)((W / 2 + 15) / 16), (unsigned)((H / 2 + 15) / 16), (unsigned)r.n), dim3(256), 0, r.stream, (const PostParams *)r.ctx.d_params, (__half *)T_(r, out), a, r.n, H, W, 1.0f));
         }
     };
     B.step(std::move(s));
@@ -410,7 +410,7 @@ void build_plan(rf_handle h) {
     Builder B{h, h->cfg.net_h, h->cfg.net_w};
     const Model &m = h->model;
     const int H = h->cfg.net_h, W = h->cfg.net_w;
-    auto T_ = [h](int id) { return reinterpret_cast<T *>(h->tptr(id)); };
+    auto T_ = [h](const Run &r, int id) { return reinterpret_cast<T *>(r.ctx.arena + h->tensors[id].offset); };
     auto Wd = [h](size_t off) { return h->d_weights + off; };
     const double es = h->elem;
 
@@ -444,9 +444,9 @@ void build_plan(rf_handle h) {
         s.out = {out};
         s.flops_per_img = 2.0 * cur_h * cur_w * 8 * 27;
         s.bytes_per_img = (double)H * W * 3 + (double)cur_h * cur_w * 8 * es;
-        s.launch = [=](int n, cudaStream_t st) {
-            long total = (long)n * (H / 2) * (W / 2);
-            CK_L(k_conv0<T>, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, st, (const PostParams *)h->d_params, T_(out), Wd(ow), Wd(ob), n, H, W);
+        s.launch = [=](const Run &r) {
+            long total = (long)r.n * (H / 2) * (W / 2);
+            CK_L(k_conv0<T>, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, r.stream, (const PostParams *)r.ctx.d_params, T_(r, out), Wd(ow), Wd(ob), r.n, H, W);
         };
         B.step(std::move(s));
     }
@@ -481,11 +481,11 @@ void build_plan(rf_handle h) {
             s.in = {tin}; s.out = {tdw};
             s.flops_per_img = 2.0 * oh * ow_ * C * 9;
             s.bytes_per_img = ((double)ih * iw * C + (double)oh * ow_ * C) * es;
-            s.launch = [=](int n, cudaStream_t st) {
-                long total = (long)n * oh * ow_ * (C / 8);
+            s.launch = [=](const Run &r) {
+                long total = (long)r.n * oh * ow_ * (C / 8);
                 unsigned g = (unsigned)((total + 255) / 256);
-                if (S == 1) CK_L(k_dw3x3<T, 1>, dim3(g), dim3(256), 0, st, (const T *)T_(tin), T_(tdw), Wd(owd), Wd(obd), n, ih, iw, C);
-                else CK_L(k_dw3x3<T, 2>, dim3(g), dim3(256), 0, st, (const T *)T_(tin), T_(tdw), Wd(owd), Wd(obd), n, ih, iw, C);
+                if (S == 1) CK_L(k_dw3x3<T, 1>, dim3(g), dim3(256), 0, r.stream, (const T *)T_(r, tin), T_(r, tdw), Wd(owd), Wd(obd), r.n, ih, iw, C);
+                else CK_L(k_dw3x3<T, 2>, dim3(g), dim3(256), 0, r.stream, (const T *)T_(r, tin), T_(r, tdw), Wd(owd), Wd(obd), r.n, ih, iw, C);
             };
             B.step(std::move(s));
         }
@@ -500,9 +500,9 @@ void build_plan(rf_handle h) {
             s.in = {tdw}; s.out = {tpw};
             s.flops_per_img = 2.0 * oh * ow_ * C * N;
             s.bytes_per_img = ((double)oh * ow_ * C + (double)oh * ow_ * N) * es;
-            s.launch = [=](int n, cudaStream_t st) {
-                OutSplit<T> o{T_(tpw), N, N, 1, nullptr, 0, 0};
-                launch_gemm<T>(T_(tdw), C, C, Wd(owp), Wd(obp), N, 1, o, n, oh, ow_, st);
+            s.launch = [=](const Run &r) {
+                OutSplit<T> o{T_(r, tpw), N, N, 1, nullptr, 0, 0};
+                launch_gemm<T>(T_(r, tdw), C, C, Wd(owp), Wd(obp), N, 1, o, r.n, oh, ow_, r.stream);
             };
             B.step(std::move(s));
         }
@@ -536,9 +536,9 @@ void build_plan(rf_handle h) {
         if (t1 >= 0) s.out.push_back(t1);
         s.flops_per_img = 2.0 * ih * iw * cin * ks * ks * N;
         s.bytes_per_img = ((double)ih * iw * cin + (double)ih * iw * N) * es;
-        s.launch = [=](int n, cudaStream_t st) {
-            OutSplit<T> o{T_(t0) + off0, ld0, n0, relu0, t1 >= 0 ? T_(t1) + off1 : nullptr, ld1, relu1};
-            launch_gemm<T>(T_(tin), ldin, cin, Wd(ow), Wd(ob), N, ks, o, n, ih, iw, st);
+        s.launch = [=](const Run &r) {
+            OutSplit<T> o{T_(r, t0) + off0, ld0, n0, relu0, t1 >= 0 ? T_(r, t1) + off1 : nullptr, ld1, relu1};
+            launch_gemm<T>(T_(r, tin), ldin, cin, Wd(ow), Wd(ob), N, ks, o, r.n, ih, iw, r.stream);
         };
         B.step(std::move(s));
     };
@@ -567,9 +567,9 @@ void build_plan(rf_handle h) {
         s.in = {tlat, tup}; s.out = {out};
         s.flops_per_img = 2.0 * fh * fw * 64 * 4;
         s.bytes_per_img = ((double)fh * fw * 64 * 2 + (double)(fh / 2) * (fw / 2) * 64) * es;
-        s.launch = [=](int n, cudaStream_t st) {
-            long total = (long)n * fh * fw * 8;
-            CK_L(k_upsample_add<T>, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, st, (const T *)T_(tlat), (const T *)T_(tup), T_(out), Wd(ow), n,
+        s.launch = [=](const Run &r) {
+            long total = (long)r.n * fh * fw * 8;
+            CK_L(k_upsample_add<T>, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, r.stream, (const T *)T_(r, tlat), (const T *)T_(r, tup), T_(r, out), Wd(ow), r.n,
                      fh, fw, 64, fh / 2, fw / 2);
         };
         B.step(std::move(s));

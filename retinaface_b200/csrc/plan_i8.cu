@@ -128,7 +128,7 @@ void build_plan_i8(rf_handle h) {
     Builder B{h, h->cfg.net_h, h->cfg.net_w};
     const Model &m = h->model;
     const int H = h->cfg.net_h, W = h->cfg.net_w;
-    auto Q_ = [h](int id) { return reinterpret_cast<int8_t *>(h->tptr(id)); };
+    auto Q_ = [h](const Run &r, int id) { return reinterpret_cast<int8_t *>(r.ctx.arena + h->tensors[id].offset); };
     auto Wd = [h](size_t off) { return h->d_weights + off; };
     auto scale_of = [h](const std::string &name) -> float {
         auto it = h->int8_scales.find(name);
@@ -164,15 +164,15 @@ void build_plan_i8(rf_handle h) {
         const bool simt_stem = (h->cfg.flags & (RF_FLAG_SIMT_STEM | RF_FLAG_NO_TENSORCORE)) != 0;
         size_t oblob = B.add_weights_h(make_stem_blob(w0, c0.b, wd, dw.b, wp, pw.b));
         if (!simt_stem) s.name = "tc_stem_conv0+dw1+pw2_u8_to_16ch_i8";
-        s.launch = [=](int n, cudaStream_t st) {
+        s.launch = [=](const Run &r) {
             if (simt_stem) {
                 StemWeights sw{Wd(ow0), Wd(ob0), Wd(owd), Wd(obd), Wd(owp), Wd(obp)};
                 const int tiles = ((H / 2 + 15) / 16) * ((W / 2 + 15) / 16);
-                launch_k(k_stem<int8_t>, dim3((unsigned)(tiles * n)), dim3(256), 0, st, (const PostParams *)h->d_params, Q_(out), sw, n, H, W, inv);
+                launch_k(k_stem<int8_t>, dim3((unsigned)(tiles * r.n)), dim3(256), 0, r.stream, (const PostParams *)r.ctx.d_params, Q_(r, out), sw, r.n, H, W, inv);
             } else {
                 StemTcArgs a{reinterpret_cast<const unsigned char *>(h->d_weights_h + oblob)};
-                launch_k(k_stem_tc<int8_t>, dim3((unsigned)((W / 2 + 15) / 16), (unsigned)((H / 2 + 15) / 16), (unsigned)n), dim3(256), 0, st,
-                         (const PostParams *)h->d_params, Q_(out), a, n, H, W, inv);
+                launch_k(k_stem_tc<int8_t>, dim3((unsigned)((W / 2 + 15) / 16), (unsigned)((H / 2 + 15) / 16), (unsigned)r.n), dim3(256), 0, r.stream,
+                         (const PostParams *)r.ctx.d_params, Q_(r, out), a, r.n, H, W, inv);
             }
         };
         B.step(std::move(s));
@@ -205,24 +205,24 @@ void build_plan_i8(rf_handle h) {
         s.bytes_per_img = (double)ih * iw * C + (double)oh * ow_ * N;
         const bool tiles2d = oh * ow_ > 56 * 56 && C >= 16 && C <= 64 && geo.nsplit == 1 && !(h->cfg.flags & RF_FLAG_DW_1D);   // as the FP16 plan
         if (tiles2d) s.name = fmt("i8_2d_dw%d+pw%d_s%d_%dto%d", i, i + 1, S, C, N);
-        s.launch = [=](int n, cudaStream_t st) {
+        s.launch = [=](const Run &r) {
             if (tiles2d) {
                 TcDw2dArgsI8 a{};
-                a.in = Q_(tin); a.C = C; a.nimg = n; a.IH = ih; a.IW = iw; a.OH = oh; a.OW = ow_; a.S = S; a.N = N; a.Kpad = Kpad;
+                a.in = Q_(r, tin); a.C = C; a.nimg = r.n; a.IH = ih; a.IW = iw; a.OH = oh; a.OW = ow_; a.S = S; a.N = N; a.Kpad = Kpad;
                 a.TH = 8;
                 a.TW = (ow_ + 13) / 14 < (ow_ + 15) / 16 ? 14 : 16;
                 tc_dw2d_i8_finish(a);
                 a.wimg = h->d_weights_q + oimg; a.mult = Wd(omul); a.bq = Wd(obq); a.dw_w = Wd(owd); a.dw_b = Wd(obd); a.inv_mid = inv_mid;
-                a.out = Q_(tpw);
-                launch_tc_dwpw_2d_i8(a, st);
+                a.out = Q_(r, tpw);
+                launch_tc_dwpw_2d_i8(a, r.stream);
                 return;
             }
             TcDwArgsI8 a{};
-            a.in = Q_(tin); a.C = C; a.nimg = n; a.IH = ih; a.IW = iw; a.OH = oh; a.OW = ow_; a.S = S;
+            a.in = Q_(r, tin); a.C = C; a.nimg = r.n; a.IH = ih; a.IW = iw; a.OH = oh; a.OW = ow_; a.S = S;
             a.N = N / geo.nsplit; a.Ntotal = N; a.Kpad = Kpad; a.rows = geo.rows; a.Wp = iw + 2; a.Hp = ih + 1; a.Rmax = geo.Rmax;
             a.wimg = h->d_weights_q + oimg; a.mult = Wd(omul); a.bq = Wd(obq); a.dw_w = Wd(owd); a.dw_b = Wd(obd); a.inv_mid = inv_mid;
-            a.out = Q_(tpw);
-            launch_tc_dwpw_i8(a, geo.nsplit, st);
+            a.out = Q_(r, tpw);
+            launch_tc_dwpw_i8(a, geo.nsplit, r.stream);
         };
         B.step(std::move(s));
         cur = tpw; cur_h = oh; cur_w = ow_;
@@ -262,15 +262,15 @@ void build_plan_i8(rf_handle h) {
         if (t1 >= 0) s.out.push_back(t1);
         s.flops_per_img = 2.0 * ih * iw * cin * ks * ks * N;
         s.bytes_per_img = (double)ih * iw * cin + (double)ih * iw * N + (tup >= 0 ? (double)(ih / 2) * (iw / 2) * cin : 0.0);
-        s.launch = [=](int n, cudaStream_t st) {
+        s.launch = [=](const Run &r) {
             TcConvArgsI8 a{};
-            a.in = Q_(tin); a.Cin = cin; a.nimg = n; a.H = ih; a.W = iw; a.taps = ks * ks; a.N = N;
+            a.in = Q_(r, tin); a.Cin = cin; a.nimg = r.n; a.H = ih; a.W = iw; a.taps = ks * ks; a.N = N;
             a.Wp = ks == 3 ? iw + 2 : iw; a.Hp = ks == 3 ? ih + 1 : ih;
             a.R = (ks == 3 ? 128 + 2 * (iw + 3) : 128) | 1;
             a.wimg = h->d_weights_q + oimg; a.mult = Wd(omul); a.bq = Wd(obq);
-            a.out = TcOutI8{Q_(t0) + off0, ld0, n0, relu0, t1 >= 0 ? Q_(t1) + off1 : nullptr, ld1, relu1};
-            if (tup >= 0) { a.up = Q_(tup); a.up_wq = Wd(oup); a.lat_mul = lat_mul; a.Cmax = (((a.R / a.Wp + 2) / 2 + 3) * (iw / 2)) | 1; }
-            launch_tc_conv_i8(a, st);
+            a.out = TcOutI8{Q_(r, t0) + off0, ld0, n0, relu0, t1 >= 0 ? Q_(r, t1) + off1 : nullptr, ld1, relu1};
+            if (tup >= 0) { a.up = Q_(r, tup); a.up_wq = Wd(oup); a.lat_mul = lat_mul; a.Cmax = (((a.R / a.Wp + 2) / 2 + 3) * (iw / 2)) | 1; }
+            launch_tc_conv_i8(a, r.stream);
         };
         B.step(std::move(s));
     };
@@ -325,9 +325,9 @@ void build_plan_i8(rf_handle h) {
         s.in = {lat1, aggr2}; s.out = {plus1};
         s.flops_per_img = 2.0 * h8 * w8 * 64 * 4;
         s.bytes_per_img = (double)h8 * w8 * 64 * 2 + (double)(h8 / 2) * (w8 / 2) * 64;
-        s.launch = [=](int n, cudaStream_t st) {
-            launch_k(k_fpn_merge_i8, dim3((unsigned)((w8 * 4 + 127) / 128), (unsigned)h8, (unsigned)n), dim3(128), 0, st, (const int8_t *)Q_(lat1), (const int8_t *)Q_(aggr2), Q_(plus1),
-                     Wd(owq), lat_mul, n, h8, w8, 64);
+        s.launch = [=](const Run &r) {
+            launch_k(k_fpn_merge_i8, dim3((unsigned)((w8 * 4 + 127) / 128), (unsigned)h8, (unsigned)r.n), dim3(128), 0, r.stream, (const int8_t *)Q_(r, lat1), (const int8_t *)Q_(r, aggr2), Q_(r, plus1),
+                     Wd(owq), lat_mul, r.n, h8, w8, 64);
         };
         B.step(std::move(s));
         conv_step("c1_aggr_3x3_64to64", {&m.conv("rf_c1_aggr")}, plus1, h8, w8, aggr1, 64, 0, 64, 1, -1, 0, 0, 0, 0, -1, 0, -1);
@@ -361,10 +361,10 @@ void build_plan_i8(rf_handle h) {
         int f0 = h->feat_tensor[0], f1 = h->feat_tensor[1], f2 = h->feat_tensor[2];
         size_t w0 = hw_off[0], w1 = hw_off[1], w2 = hw_off[2], b0 = hb_off[0], b1 = hb_off[1], b2 = hb_off[2];
         float s0 = hs[0], s1 = hs[1], s2 = hs[2];
-        s.launch = [=](int n, cudaStream_t st) {
-            const int8_t *feat[3] = {Q_(f0), Q_(f1), Q_(f2)};
+        s.launch = [=](const Run &r) {
+            const int8_t *feat[3] = {Q_(r, f0), Q_(r, f1), Q_(r, f2)};
             HeadWeights hws[3] = {{Wd(w0), Wd(b0), s0}, {Wd(w1), Wd(b1), s1}, {Wd(w2), Wd(b2), s2}};
-            launch_head_decode<int8_t>(feat, hws, h->lv, n, W, H, h->d_params, h->pb, h->blobs_in_plan ? h->d_blobs : nullptr, st, true);
+            launch_head_decode<int8_t>(feat, hws, h->lv, r.n, W, H, r.ctx.d_params, r.ctx.pb, r.blobs, r.stream, true);
         };
         s.name = "i8_heads_1x1+softmax+decode+nms_all_levels";      // decode -> NMS in one launch (last block per image)
         h->head_step = (int)h->steps.size();

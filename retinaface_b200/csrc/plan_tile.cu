@@ -382,7 +382,9 @@ int forced_th(const std::string &chain) {
     return 0;
 }
 
-void launch_chain(rf_handle h, const std::shared_ptr<TileChain> &cp, int n, cudaStream_t st) {
+void launch_chain(rf_handle h, const std::shared_ptr<TileChain> &cp, const Run &r) {
+    const int n = r.n;
+    cudaStream_t st = r.stream;
     TileChain &c = *cp;
     TchArgs a = c.args;
     a.nimg = n;
@@ -415,18 +417,19 @@ void launch_chain(rf_handle h, const std::shared_ptr<TileChain> &cp, int n, cuda
     memset(&maps, 0, sizeof maps);
     const TchBuf &b0 = a.buf[0];
     const int bc = std::min(c.in_C, 64);
-    if (c.in_s2) maps.in = make_map(h->tptr(c.in_tensor), c.in_C, c.in_W, c.in_H, n, bc, 2 * a.Wl, 2 * b0.nrows, 2);
-    else maps.in = make_map(h->tptr(c.in_tensor), c.in_C, c.in_W, c.in_H, n, bc, a.Wl, b0.nrows, 1);
-    if (c.merge_tensor >= 0) maps.aux = make_map(h->tptr(c.merge_tensor), 64, c.W / 2, c.H / 2, n, 64, c.W / 2 + 2, a.merge_rows, 1);
-    for (int i = 0; i < c.nstores; i++) maps.st[i] = make_map(h->tptr(c.bufs[c.store_buf_of[i]].store_tensor), c.store_C[i], c.W, c.H, n, std::min(c.store_C[i], 64), c.W, 1, 1);
+    auto T_ = [&](int id) { return r.ctx.arena + h->tensors[id].offset; };
+    if (c.in_s2) maps.in = make_map(T_(c.in_tensor), c.in_C, c.in_W, c.in_H, n, bc, 2 * a.Wl, 2 * b0.nrows, 2);
+    else maps.in = make_map(T_(c.in_tensor), c.in_C, c.in_W, c.in_H, n, bc, a.Wl, b0.nrows, 1);
+    if (c.merge_tensor >= 0) maps.aux = make_map(T_(c.merge_tensor), 64, c.W / 2, c.H / 2, n, 64, c.W / 2 + 2, a.merge_rows, 1);
+    for (int i = 0; i < c.nstores; i++) maps.st[i] = make_map(T_(c.bufs[c.store_buf_of[i]].store_tensor), c.store_C[i], c.W, c.H, n, std::min(c.store_C[i], 64), c.W, 1, 1);
     if (c.level >= 0) {
         a.head.lv = h->lv[c.level];
-        a.head.pb = h->pb;
-        a.head.params = h->d_params;
+        a.head.pb = r.ctx.pb;
+        a.head.params = r.ctx.d_params;
         a.head.net_w = h->cfg.net_w; a.head.net_h = h->cfg.net_h;
-        a.head.done = h->pb.tile_done;
-        a.head.expected = (c.fused_nms && !h->profiling) ? h->tile_expected : 0;    // rf_profile_layers launches single steps: no last-block NMS then
-        for (int k = 0; k < 3; k++) a.head.blobs[k] = h->blobs_in_plan ? h->d_blobs[3 * c.level + k] : nullptr;
+        a.head.done = r.ctx.pb.tile_done;
+        a.head.expected = (c.fused_nms && !r.single) ? h->tile_expected : 0;    // a step launched on its own: no last-block NMS
+        for (int k = 0; k < 3; k++) a.head.blobs[k] = r.blobs ? r.blobs[3 * c.level + k] : nullptr;
     }
     const int grid = std::min(a.ntiles, h->num_sms);
     CK(launch_k(k_tile_chain<0>, dim3((unsigned)grid), dim3(TCH_THREADS), (size_t)a.smem_bytes, st, maps, a));
@@ -447,7 +450,7 @@ void add_chain_step(Builder &B, std::shared_ptr<TileChain> c, int lane, double b
     for (auto &ls : c->stages) fl += ls.flops * c->W * c->H;
     s.flops_per_img = fl;
     s.bytes_per_img = bytes_per_img;
-    s.launch = [h, c](int n, cudaStream_t st) { launch_chain(h, c, n, st); };
+    s.launch = [h, c](const Run &r) { launch_chain(h, c, r); };
     B.step(std::move(s));
 }
 

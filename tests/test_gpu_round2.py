@@ -98,6 +98,28 @@ def test_tile_chains_equal_round1_kernels(mask, hw, nb, golden_image, monkeypatc
         old.close()
 
 
+def test_profile_layers_between_detections(golden_image):
+    """rf_profile_layers launches every step on its own, out of its forward: the SSH tile chains of a one-context FP16 handle
+    then skip their fused last-block NMS.  It times every step and leaves the handle as it found it: the detections before
+    and after it are bit-equal."""
+    from retinaface_b200 import RF_PREC_FP16
+    from retinaface_b200.capi import plan_describe
+    assert "tile_ssh_c1+heads+decode" in plan_describe(caffemodel("mnet25"), 448, 448, max_batch=8, streams=1)
+    inp = letterbox_bgr_u8(golden_image, 448, 448)
+    batch = [inp, np.roll(inp, 24, axis=1), s_noise_batch(1, 448, 448, seed=3)[0]]
+    eng = _engine("mnet25", 448, 448, RF_PREC_FP16, max_batch=8, streams=1)
+    try:
+        before, idx_before = eng.detect_batch(batch, 0.5, 0.4, want_index=True)
+        prof = eng.profile_layers(len(batch), iters=3)
+        after, idx_after = eng.detect_batch(batch, 0.5, 0.4, want_index=True)
+        assert [p["name"] for p in prof][-1] == "tile_ssh_c1+heads+decode" and all(p["ms"] > 0 for p in prof)
+        assert len(before[0]) >= 4
+        for i in range(len(batch)):
+            assert np.array_equal(before[i], after[i]) and np.array_equal(idx_before[i], idx_after[i]), i
+    finally:
+        eng.close()
+
+
 @pytest.mark.parametrize("mask", [511, 482])
 @pytest.mark.parametrize("model", ["mnet25", "mnet-deconv-0517"])
 def test_tile_plans_against_golden_fp32(mask, model, golden_image, monkeypatch):

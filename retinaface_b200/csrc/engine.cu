@@ -100,6 +100,7 @@ void place_tensors(rf_handle h, bool keep_all) {
 void make_plan(rf_handle h, bool init) {
     const rf_config &cfg = h->cfg;
     h->use_tc = cfg.precision == RF_PREC_INT8 || (cfg.precision == RF_PREC_FP16 && !(cfg.flags & RF_FLAG_NO_TENSORCORE));
+    h->on_device = init;
     if (init && h->use_tc) CK(tc_init());
     if (cfg.precision == RF_PREC_INT8) { if (init) CK(tc_init_i8()); build_plan_i8(h); }
     else if (cfg.precision == RF_PREC_FP32) build_plan<float>(h);

@@ -125,6 +125,7 @@ struct rf_handle_s {
     std::map<std::string, float> int8_scales;
     int device = 0;
     int num_sms = RF_NUM_SMS;   // plan heuristics ("does this layer fill one wave") and the persistent tile-chain grid
+    bool on_device = false;     // the plan is built for launches (rf_create), not only described: occupancy may be queried
     int elem = 4;  // bytes per activation element
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
 
@@ -248,6 +249,13 @@ cudaError_t tc_init();
 std::vector<__half> make_stem_blob(const std::vector<float> &w0, const std::vector<float> &b0, const std::vector<float> &wd,
                                    const std::vector<float> &bd, const std::vector<float> &wp, const std::vector<float> &bp);
 int plan_stem_tc(Builder &B);
+int resident_ctas(rf_handle h, const void *kern, int threads, size_t smem);
+// Persistent grid over `tiles` tiles: each CTA takes a run of consecutive tiles, the grid is what the device holds at once.
+struct PersistentGrid { int run, grid; };
+inline PersistentGrid persistent_grid(int tiles, int resident) {
+    const int run = std::max(1, (tiles + resident - 1) / std::max(resident, 1));
+    return {run, (tiles + run - 1) / run};
+}
 int plan_pair_legacy(Builder &B, int i, int tin, int ih, int iw);
 void plan_conv_legacy(Builder &B, const std::string &sname, std::vector<const FoldedConv *> cs, int tin, int ih, int iw, int t0, int ld0,
                       int off0, int n0, int relu0, int t1, int ld1, int off1, int relu1, int lane = 0, int tup = -1, int up_which = 0);

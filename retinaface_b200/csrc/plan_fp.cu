@@ -100,15 +100,30 @@ void launch_tc_dwpw(const TcDwArgs &a_in, int nsplit, cudaStream_t s) {
         default: CK_L(k_tc_dwpw_staged<256>, grid, dim3(TC_THREADS), smem, s, a); break;
     }
 }
-void launch_tc_dwpw_2d(const TcDw2dArgs &a, cudaStream_t s) {
-    const dim3 grid((unsigned)(a.tiles_x * a.tiles_y * a.nimg));
-    const size_t smem = tc_dw2d_smem_bytes(a);
-    switch (tc_n_bucket(a.N)) {
-        case 32: CK_L(k_tc_dwpw_2d<32>, grid, dim3(TC_THREADS), smem, s, a); break;
-        case 64: CK_L(k_tc_dwpw_2d<64>, grid, dim3(TC_THREADS), smem, s, a); break;
-        case 128: CK_L(k_tc_dwpw_2d<128>, grid, dim3(TC_THREADS), smem, s, a); break;
-        default: CK_L(k_tc_dwpw_2d<256>, grid, dim3(TC_THREADS), smem, s, a); break;
+// the k_tc_dwpw_2d instantiation of a layer with N output channels
+static void (*dw2d_kernel(int N))(TcDw2dArgs) {
+    switch (tc_n_bucket(N)) {
+        case 32: return k_tc_dwpw_2d<32>;
+        case 64: return k_tc_dwpw_2d<64>;
+        case 128: return k_tc_dwpw_2d<128>;
+        default: return k_tc_dwpw_2d<256>;
     }
+}
+// persistent: at most `resident` CTAs (resident_ctas of this layer's instantiation and shared memory), each over a run of tiles
+void launch_tc_dwpw_2d(TcDw2dArgs a, int resident, cudaStream_t s) {
+    const PersistentGrid pg = persistent_grid(a.tiles_x * a.tiles_y * a.nimg, resident);
+    a.run = pg.run;
+    CK_L(dw2d_kernel(a.N), dim3((unsigned)pg.grid), dim3(TC_THREADS), tc_dw2d_smem_bytes(a), s, a);
+}
+
+// CTAs of `kern` the whole device holds at once with `threads` threads and `smem` bytes of dynamic shared memory: the grid of
+// the persistent kernels.  Queried once, when the plan is built for launches; a plan that is only described launches nothing.
+int resident_ctas(rf_handle h, const void *kern, int threads, size_t smem) {
+    if (!h->on_device) return h->num_sms;
+    int per_sm = 0;
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem));
+    if (per_sm < 1) throw PlanFail{RF_ERR_UNSUPPORTED, fmt("a kernel with %zu bytes of dynamic shared memory does not fit an SM", smem)};
+    return per_sm * h->num_sms;
 }
 
 cudaError_t tc_init() {
@@ -210,17 +225,23 @@ int plan_pair_legacy(Builder &B, int i, int tin, int ih, int iw) {
     // large maps (> 56x56 outputs; measured: no gain below): 2-D tiles (tc_dwpw2d.cuh) -- half the staged halo, no position
     // table, vertical reuse
     const bool tiles2d = oh * ow_ > 56 * 56 && C >= 16 && C <= 64 && geo.nsplit == 1 && !(h->cfg.flags & RF_FLAG_DW_1D);
-    if (tiles2d) s.name = fmt("tc2d_dw%d+pw%d_s%d_%dto%d", i, i + 1, S, C, N);
+    TcDw2dArgs g2{};            // 2-D tile geometry (independent of the batch)
+    int resident = 0;
+    if (tiles2d) {
+        s.name = fmt("tc2d_dw%d+pw%d_s%d_%dto%d", i, i + 1, S, C, N);
+        g2.C = C; g2.IH = ih; g2.IW = iw; g2.OH = oh; g2.OW = ow_; g2.S = S; g2.N = N;
+        g2.TH = 8;
+        const int t16 = (ow_ + 15) / 16, t14 = (ow_ + 13) / 14;
+        g2.TW = t14 < t16 ? 14 : 16;
+        tc_dw2d_finish(g2);
+        resident = resident_ctas(h, (const void *)dw2d_kernel(N), TC_THREADS, tc_dw2d_smem_bytes(g2));
+    }
     s.launch = [=](const Run &r) {
         if (tiles2d) {
-            TcDw2dArgs a{};
-            a.in = T_(r, tin); a.C = C; a.nimg = r.n; a.IH = ih; a.IW = iw; a.OH = oh; a.OW = ow_; a.S = S; a.N = N;
-            a.TH = 8;
-            const int t16 = (ow_ + 15) / 16, t14 = (ow_ + 13) / 14;
-            a.TW = t14 < t16 ? 14 : 16;
-            tc_dw2d_finish(a);
+            TcDw2dArgs a = g2;
+            a.in = T_(r, tin); a.nimg = r.n;
             a.wimg = h->d_weights_h + oimg; a.bias = Wd(obp); a.dw_w = Wd(owd); a.dw_b = Wd(obd); a.out = T_(r, tpw);
-            launch_tc_dwpw_2d(a, r.stream);
+            launch_tc_dwpw_2d(a, resident, r.stream);
             return;
         }
         TcDwArgs a{};
@@ -391,14 +412,17 @@ int plan_stem_tc(Builder &B) {
     s.out = {out};
     s.flops_per_img = 2.0 * cur_h * cur_w * (8 * 27 + 8 * 9 + 8 * 16);
     s.bytes_per_img = (double)H * W * 3 + (double)cur_h * cur_w * 16 * es;
+    const int tiles = ((H / 2 + 15) / 16) * ((W / 2 + 15) / 16);
+    const int resident = simt_stem ? 0 : resident_ctas(h, (const void *)k_stem_tc<__half>, 256, 0);
     s.launch = [=](const Run &r) {
-        const int tiles = ((H / 2 + 15) / 16) * ((W / 2 + 15) / 16);
         if (simt_stem) {
             StemWeights sw{Wd(ow0), Wd(ob0), Wd(owd), Wd(obd), Wd(owp), Wd(obp)};
             CK(launch_k(k_stem<__half>, dim3((unsigned)(tiles * r.n)), dim3(256), 0, r.stream, (const PostParams *)r.ctx.d_params, (__half *)T_(r, out), sw, r.n, H, W, 1.0f));
         } else {
             StemTcArgs a{reinterpret_cast<const unsigned char *>(h->d_weights_h + oblob)};
-            CK(launch_k(k_stem_tc<__half>, dim3((unsigned)((W / 2 + 15) / 16), (unsigned)((H / 2 + 15) / 16), (unsigned)r.n), dim3(256), 0, r.stream, (const PostParams *)r.ctx.d_params, (__half *)T_(r, out), a, r.n, H, W, 1.0f));
+            const PersistentGrid pg = persistent_grid(tiles * r.n, resident);
+            stem_tc_finish(a, H, W, pg.run);
+            CK(launch_k(k_stem_tc<__half>, dim3((unsigned)pg.grid), dim3(256), 0, r.stream, (const PostParams *)r.ctx.d_params, (__half *)T_(r, out), a, r.n, H, W, 1.0f));
         }
     };
     B.step(std::move(s));

@@ -164,14 +164,17 @@ void build_plan_i8(rf_handle h) {
         const bool simt_stem = (h->cfg.flags & (RF_FLAG_SIMT_STEM | RF_FLAG_NO_TENSORCORE)) != 0;
         size_t oblob = B.add_weights_h(make_stem_blob(w0, c0.b, wd, dw.b, wp, pw.b));
         if (!simt_stem) s.name = "tc_stem_conv0+dw1+pw2_u8_to_16ch_i8";
+        const int tiles = ((H / 2 + 15) / 16) * ((W / 2 + 15) / 16);
+        const int resident = simt_stem ? 0 : resident_ctas(h, (const void *)k_stem_tc<int8_t>, 256, 0);
         s.launch = [=](const Run &r) {
             if (simt_stem) {
                 StemWeights sw{Wd(ow0), Wd(ob0), Wd(owd), Wd(obd), Wd(owp), Wd(obp)};
-                const int tiles = ((H / 2 + 15) / 16) * ((W / 2 + 15) / 16);
                 launch_k(k_stem<int8_t>, dim3((unsigned)(tiles * r.n)), dim3(256), 0, r.stream, (const PostParams *)r.ctx.d_params, Q_(r, out), sw, r.n, H, W, inv);
             } else {
                 StemTcArgs a{reinterpret_cast<const unsigned char *>(h->d_weights_h + oblob)};
-                launch_k(k_stem_tc<int8_t>, dim3((unsigned)((W / 2 + 15) / 16), (unsigned)((H / 2 + 15) / 16), (unsigned)r.n), dim3(256), 0, r.stream,
+                const PersistentGrid pg = persistent_grid(tiles * r.n, resident);
+                stem_tc_finish(a, H, W, pg.run);
+                launch_k(k_stem_tc<int8_t>, dim3((unsigned)pg.grid), dim3(256), 0, r.stream,
                          (const PostParams *)r.ctx.d_params, Q_(r, out), a, r.n, H, W, inv);
             }
         };

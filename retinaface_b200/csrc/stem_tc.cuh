@@ -4,8 +4,9 @@
 //
 // The CUDA-core stem (kernels_simt.cuh k_stem) spends two thirds of its instructions on the 216 + 128 FMAs per pixel of the
 // two dense layers.  Here they become wgmma GEMMs with the accumulator in registers and the depthwise stencil stays on CUDA cores:
-//   per CTA: a 16x16 tile of the H/2 x W/2 map (256 threads, 32 KB of shared memory, <= 64 registers: 4 CTAs per SM)
-//   1. stage the 37x37x3 u8 input patch (32-bit loads, all of a warp's rows in flight before the first store)
+//   per CTA: a run of consecutive 16x16 tiles of the H/2 x W/2 maps of all images (persistent: 256 threads, 36 KB of shared
+//   memory, <= 64 registers: 4 CTAs per SM; the constants are fetched once per CTA), per tile:
+//   1. stage the 37x37x3 u8 input patch of the NEXT tile (4-byte cp.async into the second buffer) -- it lands while 2.-7. run
 //   2. im2col of conv0 for the 18x18 ring (324 rows, padded to 3 x 128) straight into the MMA A operand: each thread turns the
 //      27 u8 taps of one position into FP16 by byte permutes (0x6400 | b = 1024 + b, minus 1024: exact) -- K = 27 padded to 32
 //   3. 6 row blocks x 2 K-steps x {hi, lo} wgmma (M=64 per warpgroup, N=16 (8 used), K=16): conv0 for the whole ring, the
@@ -33,7 +34,16 @@ constexpr int STEM_CONST_BYTES = STEM_B0_BYTES + STEM_B1_BYTES + STEM_F_FLOATS *
 static_assert(STEM_CONST_BYTES % 16 == 0, "bulk copy size");
 struct StemTcArgs {
     const unsigned char *consts;     // STEM_CONST_BYTES, 16-byte aligned
+    int tiles_per_cta;               // consecutive 16x16 tiles per CTA (numbered image-major); grid = ceil(tiles / tiles_per_cta)
+    uint32_t mul_tiles, mul_tiles_x; // fast_div multipliers of the tiles per image and per tile row (stem_tc_finish)
 };
+// tile counts of an H x W input (output map H/2 x W/2 in 16 x 16 tiles) and the multipliers that decode a tile index
+inline void stem_tc_finish(StemTcArgs &a, int H, int W, int tiles_per_cta) {
+    const int tiles_x = (W / 2 + 15) / 16, tiles = tiles_x * ((H / 2 + 15) / 16);
+    a.tiles_per_cta = tiles_per_cta;
+    a.mul_tiles = fast_div_mul((uint32_t)tiles);
+    a.mul_tiles_x = fast_div_mul((uint32_t)tiles_x);
+}
 
 constexpr int STEM_LBO0 = 384 * 16 + 16;    // A0: 3 tiles x 128 rows
 constexpr int STEM_LBO1 = 256 * 16 + 16;    // A1: 2 tiles x 128 rows
@@ -46,13 +56,13 @@ template <typename OutT>
 __global__ void __launch_bounds__(256, 4) k_stem_tc(const PostParams *__restrict__ run, OutT *__restrict__ out, StemTcArgs w,
                                                     int n, int H, int W, float out_inv_scale) {
     constexpr bool I8 = sizeof(OutT) == 1;
-    __shared__ __align__(16) uint8_t s_in[37][116];
+    __shared__ __align__(16) uint8_t s_in[2][37][116];        // two staging buffers: tile t + 1's patch lands during tile t
     __shared__ __align__(128) unsigned char s_a0[4 * STEM_LBO0];
     __shared__ __align__(128) unsigned char s_const[STEM_CONST_BYTES];
     __shared__ __align__(8) uint64_t bar_w;
 
     // conv0's operand is dead once every warpgroup's conv0 MMAs have completed: the pointwise operand (2 * STEM_LBO1 bytes) and, behind it, conv0's
-    // FP32 output ring reuse its space -- 32 KB of shared memory per CTA
+    // FP32 output ring reuse its space -- 36 KB of shared memory per CTA with the two staging buffers
     unsigned char *s_a1 = s_a0;
     constexpr int STEM_C0_OFF = (2 * STEM_LBO1 + 127) / 128 * 128;
     static_assert(STEM_C0_OFF + 18 * 18 * 8 * 4 <= 4 * STEM_LBO0, "conv0 ring must fit behind the pointwise operand");
@@ -60,8 +70,15 @@ __global__ void __launch_bounds__(256, 4) k_stem_tc(const PostParams *__restrict
     float (*s_c0)[18 * 18][4] = reinterpret_cast<float (*)[18 * 18][4]>(s_a0 + STEM_C0_OFF);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int OH = H >> 1, OW = W >> 1;
-    const int b = blockIdx.z;            // grid = (tiles_x, tiles_y, images)
-    const int oy0 = blockIdx.y << 4, ox0 = blockIdx.x << 4;
+    // tiles of 16 x 16 outputs, numbered image-major over all n images; this CTA takes [t_begin, t_end), which may cross
+    // from one image into the next
+    const int tiles_x = (OW + 15) >> 4, tiles = tiles_x * ((OH + 15) >> 4);
+    const int t_begin = (int)blockIdx.x * w.tiles_per_cta, t_end = min(t_begin + w.tiles_per_cta, tiles * n);
+    auto decode = [&](int t, int &b, int &oy0, int &ox0) {
+        b = fast_div(t, w.mul_tiles);
+        const int trem = t - b * tiles, ty = fast_div(trem, w.mul_tiles_x);
+        oy0 = ty << 4; ox0 = (trem - ty * tiles_x) << 4;
+    };
 
     const __half *s_b0 = reinterpret_cast<const __half *>(s_const), *s_b1 = reinterpret_cast<const __half *>(s_const + STEM_B0_BYTES);
     const float *s_bias0 = reinterpret_cast<const float *>(s_const + STEM_B0_BYTES + STEM_B1_BYTES);
@@ -74,227 +91,241 @@ __global__ void __launch_bounds__(256, 4) k_stem_tc(const PostParams *__restrict
     }
     pdl_trigger();
     pdl_wait();
-    // ---- 1. stage the u8 patch (see k_stem) ------------------------------------------------------------------
-    const uint8_t *__restrict__ img = run->input + (size_t)b * H * W * 3;
-    const int iy0 = 2 * oy0 - 3, cb0 = (2 * ox0 - 3) * 3;
-    const int al0 = cb0 & ~3, mis = cb0 - al0;
-    const bool aligned = ((reinterpret_cast<uintptr_t>(img) & 3) == 0);
-    const int rowbytes = W * 3;
-    {   // warp w stages rows w, w + 8, ...: lane = 32-bit word of the row; all loads in flight before the first store
-        uint32_t v[5];
-        const int gb = al0 + 4 * lane;
-        const bool fast = aligned && gb >= 0 && gb + 3 < rowbytes;
+    // ---- 1. stage tile t's u8 patch into buffer buf (see k_stem): warp w stages rows w, w + 8, ...; lane = 32-bit word of the
+    // row.  Words inside the image go by cp.async (4 bytes, in flight while the previous tile computes); words that straddle
+    // the image's left or right edge, rows outside it (zeros) and every word of an image base that is not 4-byte aligned are
+    // loaded and stored synchronously.
+    auto stage = [&](int t, int buf) {
+        int b, oy0, ox0;
+        decode(t, b, oy0, ox0);
+        const uint8_t *__restrict__ img = run->input + (size_t)b * H * W * 3;
+        const int iy0 = 2 * oy0 - 3, cb0 = (2 * ox0 - 3) * 3;
+        const int gb = (cb0 & ~3) + 4 * lane;
+        const int rowbytes = W * 3;
+        const bool fast = ((reinterpret_cast<uintptr_t>(img) & 3) == 0) && gb >= 0 && gb + 3 < rowbytes;
+        if (lane < 29) {
 #pragma unroll
-        for (int k = 0; k < 5; k++) {
-            const int r = warp + 8 * k, iy = iy0 + r;
-            v[k] = 0;
-            if (r < 37 && lane < 29 && iy >= 0 && iy < H) {
-                const uint8_t *rowp = img + (size_t)iy * rowbytes;
-                if (fast) {
-                    v[k] = __ldg(reinterpret_cast<const uint32_t *>(rowp + gb));
+            for (int k = 0; k < 5; k++) {
+                const int r = warp + 8 * k, iy = iy0 + r;
+                if (r >= 37) break;
+                uint8_t *dst = &s_in[buf][r][4 * lane];
+                const bool rowok = iy >= 0 && iy < H;
+                const uint8_t *rowp = img + (size_t)(rowok ? iy : 0) * rowbytes;
+                if (fast && rowok) {
+                    cp_async4(dst, rowp + gb);
                 } else {
+                    uint32_t v = 0;
+                    if (rowok)
 #pragma unroll
-                    for (int j = 0; j < 4; j++)
-                        if (gb + j >= 0 && gb + j < rowbytes) v[k] |= (uint32_t)rowp[gb + j] << (8 * j);
+                        for (int j = 0; j < 4; j++)
+                            if (gb + j >= 0 && gb + j < rowbytes) v |= (uint32_t)rowp[gb + j] << (8 * j);
+                    *reinterpret_cast<uint32_t *>(dst) = v;
                 }
             }
         }
+        cp_async_commit();
+    };
+    stage(t_begin, 0);
+    int buf = 0;
+    for (int t = t_begin; t < t_end; t++, buf ^= 1) {
+        cp_async_wait_all();
+        // tile t's patch has landed, and every thread is done with tile t - 1: its im2col has read the other staging buffer, its
+        // last shared reads (the pointwise wgmma after wg::wait<0>, or the INT8 pointwise stage) are complete
+        __syncthreads();
+        if (t + 1 < t_end) stage(t + 1, buf ^ 1);
+        int b, oy0, ox0;
+        decode(t, b, oy0, ox0);
+        const int mis = ((2 * ox0 - 3) * 3) & 3;
+        // ---- 2. conv0 im2col -> A0 (rows = ring positions, K = (ky, kx, c) padded to 32) -----------------------------
+        for (int p = tid; p < 384; p += 256) {
+            uint32_t h2[16];                     // 32 halfs
 #pragma unroll
-        for (int k = 0; k < 5; k++) {
-            const int r = warp + 8 * k;
-            if (r < 37 && lane < 29) *reinterpret_cast<uint32_t *>(&s_in[r][4 * lane]) = v[k];
-        }
-    }
-    __syncthreads();
-    // ---- 2. conv0 im2col -> A0 (rows = ring positions, K = (ky, kx, c) padded to 32) -----------------------------
-    for (int p = tid; p < 384; p += 256) {
-        uint32_t h2[16];                     // 32 halfs
-#pragma unroll
-        for (int i = 0; i < 16; i++) h2[i] = 0;
-        if (p < 324) {
-            const int py = p / 18, px = p - py * 18;
-            // 9 consecutive bytes per kernel row, starting at an arbitrary byte offset: three aligned words + funnel
-            // shifts; u8 -> FP16 without a convert: 0x6400 | b is the half 1024 + b, minus 1024 (exact)
-            const int off = mis + 6 * px, sh = (off & 3) * 8;
-            uint32_t bytes[3][3];
-#pragma unroll
-            for (int ky = 0; ky < 3; ky++) {
-                const uint32_t *row = reinterpret_cast<const uint32_t *>(&s_in[2 * py + ky][off & ~3]);
-                const uint32_t w0 = row[0], w1 = row[1], w2 = row[2];      // (off & 3) + 8 <= 11: three words cover the 9 bytes
-                bytes[ky][0] = __funnelshift_r(w0, w1, sh);
-                bytes[ky][1] = __funnelshift_r(w1, w2, sh);
-                bytes[ky][2] = __funnelshift_r(w2, 0u, sh);
-            }
-            const __half2 k1024 = __floats2half2_rn(1024.f, 1024.f);
-#pragma unroll
-            for (int i = 0; i < 14; i++) {                  // K index k = ky * 9 + j; halfs (2i, 2i + 1) share a register
-                const int k0 = 2 * i, k1 = 2 * i + 1 < 27 ? 2 * i + 1 : 2 * i;
-                const int ra = k0 / 9, ja = k0 % 9, rb = k1 / 9, jb = k1 % 9;
-                const uint32_t wa = bytes[ra][ja >> 2], wb = bytes[rb][jb >> 2];
-                uint32_t biased;                            // (b_k0, 0x64, b_k1, 0x64)
-                if (ra == rb && (ja >> 2) == (jb >> 2))
-                    biased = __byte_perm(wa, 0x64646464u, (ja & 3) | 0x40 | ((jb & 3) << 8) | 0x4000);
-                else
-                    biased = __byte_perm(__byte_perm(wa, wb, (ja & 3) | ((4 + (jb & 3)) << 4)), 0x64646464u, 0x4140);
-                const __half2 r = __hsub2(*reinterpret_cast<const __half2 *>(&biased), k1024);
-                h2[i] = *reinterpret_cast<const uint32_t *>(&r);
-            }
-            h2[13] &= 0xffffu;                              // k = 27 is padding
-        }
-#pragma unroll
-        for (int g = 0; g < 4; g++)
-            *reinterpret_cast<uint4 *>(s_a0 + g * STEM_LBO0 + p * 16) = make_uint4(h2[4 * g], h2[4 * g + 1], h2[4 * g + 2], h2[4 * g + 3]);
-    }
-    tc::fence_async_smem();
-    __syncthreads();
-    tc::mbar_wait(&bar_w, 0);            // B images and the FP32 constants
-    const int wgi = warp >> 2, c2 = 2 * (lane & 3);
-    const int rl = 16 * (warp & 3) + (lane >> 2);      // fragment rows rl, rl + 8 of each 64-row block (wgmma.cuh)
-    // ---- 3. conv0 GEMM: warpgroup w computes row blocks w, w + 2, w + 4 ---------------------------------------------------
-    float d0[3][8];
-    {
-        const uint32_t a0 = tc::smem_u32(s_a0), b0 = tc::smem_u32(s_b0);
-#pragma unroll
-        for (int j = 0; j < 3; j++)
-#pragma unroll
-            for (int i = 0; i < 8; i++) d0[j][i] = 0.f;
-        wg::fence();
-#pragma unroll
-        for (int j = 0; j < 3; j++)
-#pragma unroll
-            for (int part = 0; part < 2; part++)
-#pragma unroll
-                for (int ks = 0; ks < 2; ks++) {
-                    const uint64_t ad = wg::desc(a0 + (uint32_t)(2 * ks) * STEM_LBO0 + (uint32_t)(64 * (wgi + 2 * j)) * 16, STEM_LBO0, 128);
-                    const uint64_t bd = wg::desc(b0 + (uint32_t)(part * 4 + 2 * ks) * 256, 256, 128);
-                    wg::mma_ss<16>(d0[j], ad, bd, part | ks);
-                }
-        wg::commit();
-        wg::wait<0>();
-#pragma unroll
-        for (int j = 0; j < 3; j++) wg::fence_regs(d0[j]);
-    }
-    __syncthreads();                     // conv0's operand is dead: s_c0 overwrites it
-    // ---- 4. conv0 epilogue -> s_c0 (FP32), zero outside the map (columns 8..15 of the N = 16 tile are padding) ------------
-#pragma unroll
-    for (int j = 0; j < 3; j++)
-#pragma unroll
-        for (int e = 0; e < 2; e++) {
-            const int p = 64 * (wgi + 2 * j) + rl + 8 * e;
+            for (int i = 0; i < 16; i++) h2[i] = 0;
             if (p < 324) {
                 const int py = p / 18, px = p - py * 18;
-                const int cy = oy0 - 1 + py, cx = ox0 - 1 + px;
-                const bool inside = cy >= 0 && cy < OH && cx >= 0 && cx < OW;
-                const float v0 = inside ? fmaxf(d0[j][2 * e] + s_bias0[c2], 0.f) : 0.f;
-                const float v1 = inside ? fmaxf(d0[j][2 * e + 1] + s_bias0[c2 + 1], 0.f) : 0.f;
-                *reinterpret_cast<float2 *>(&s_c0[c2 >> 2][p][c2 & 3]) = make_float2(v0, v1);
-            }
-        }
-    __syncthreads();
-    // ---- 5. depthwise 3x3 + ReLU -> A1 (FP16, GEMM row = pixel ty * 16 + tx) ------------------------------------------------
-    // thread = (4-channel plane, column, PAIR of output rows): 4 ring rows x 3 columns = 12 loads feed 2 outputs, the 9
-    // weight vectors of the plane are warp-uniform (broadcast).  Per output the accumulation order is (ky, kx) ascending.
-    {
-        const int plane = tid >> 7, q = tid & 127;
-        const int tx = q & 15, ty = (q >> 4) << 1;
-        const float4 bv = *reinterpret_cast<const float4 *>(&s_wd[72 + plane * 4]);
-        float d0[4] = {bv.x, bv.y, bv.z, bv.w}, d1[4] = {bv.x, bv.y, bv.z, bv.w};
+                // 9 consecutive bytes per kernel row, starting at an arbitrary byte offset: three aligned words + funnel
+                // shifts; u8 -> FP16 without a convert: 0x6400 | b is the half 1024 + b, minus 1024 (exact)
+                const int off = mis + 6 * px, sh = (off & 3) * 8;
+                uint32_t bytes[3][3];
 #pragma unroll
-        for (int ry = 0; ry < 4; ry++)
+                for (int ky = 0; ky < 3; ky++) {
+                    const uint32_t *row = reinterpret_cast<const uint32_t *>(&s_in[buf][2 * py + ky][off & ~3]);
+                    const uint32_t w0 = row[0], w1 = row[1], w2 = row[2];      // (off & 3) + 8 <= 11: three words cover the 9 bytes
+                    bytes[ky][0] = __funnelshift_r(w0, w1, sh);
+                    bytes[ky][1] = __funnelshift_r(w1, w2, sh);
+                    bytes[ky][2] = __funnelshift_r(w2, 0u, sh);
+                }
+                const __half2 k1024 = __floats2half2_rn(1024.f, 1024.f);
 #pragma unroll
-            for (int kx = 0; kx < 3; kx++) {
-                const float4 a = *reinterpret_cast<const float4 *>(&s_c0[plane][(ty + ry) * 18 + tx + kx][0]);
-                if (ry < 3) {
-                    const float4 w = *reinterpret_cast<const float4 *>(&s_wd[(ry * 3 + kx) * 8 + plane * 4]);
-                    d0[0] = fmaf(a.x, w.x, d0[0]); d0[1] = fmaf(a.y, w.y, d0[1]); d0[2] = fmaf(a.z, w.z, d0[2]); d0[3] = fmaf(a.w, w.w, d0[3]);
+                for (int i = 0; i < 14; i++) {                  // K index k = ky * 9 + j; halfs (2i, 2i + 1) share a register
+                    const int k0 = 2 * i, k1 = 2 * i + 1 < 27 ? 2 * i + 1 : 2 * i;
+                    const int ra = k0 / 9, ja = k0 % 9, rb = k1 / 9, jb = k1 % 9;
+                    const uint32_t wa = bytes[ra][ja >> 2], wb = bytes[rb][jb >> 2];
+                    uint32_t biased;                            // (b_k0, 0x64, b_k1, 0x64)
+                    if (ra == rb && (ja >> 2) == (jb >> 2))
+                        biased = __byte_perm(wa, 0x64646464u, (ja & 3) | 0x40 | ((jb & 3) << 8) | 0x4000);
+                    else
+                        biased = __byte_perm(__byte_perm(wa, wb, (ja & 3) | ((4 + (jb & 3)) << 4)), 0x64646464u, 0x4140);
+                    const __half2 r = __hsub2(*reinterpret_cast<const __half2 *>(&biased), k1024);
+                    h2[i] = *reinterpret_cast<const uint32_t *>(&r);
                 }
-                if (ry > 0) {
-                    const float4 w = *reinterpret_cast<const float4 *>(&s_wd[((ry - 1) * 3 + kx) * 8 + plane * 4]);
-                    d1[0] = fmaf(a.x, w.x, d1[0]); d1[1] = fmaf(a.y, w.y, d1[1]); d1[2] = fmaf(a.z, w.z, d1[2]); d1[3] = fmaf(a.w, w.w, d1[3]);
-                }
+                h2[13] &= 0xffffu;                              // k = 27 is padding
             }
-        const int row = ty * 16 + tx;
-        if constexpr (I8) {
-            // FP32 depthwise output -> shared [plane][pixel][4] (the pointwise operand's place, unused here)
-            float (*s_dwo)[256][4] = reinterpret_cast<float (*)[256][4]>(s_a1);
-            *reinterpret_cast<float4 *>(&s_dwo[plane][row][0]) = make_float4(fmaxf(d0[0], 0.f), fmaxf(d0[1], 0.f), fmaxf(d0[2], 0.f), fmaxf(d0[3], 0.f));
-            *reinterpret_cast<float4 *>(&s_dwo[plane][row + 16][0]) = make_float4(fmaxf(d1[0], 0.f), fmaxf(d1[1], 0.f), fmaxf(d1[2], 0.f), fmaxf(d1[3], 0.f));
-        } else {
-            const __half2 h00 = __floats2half2_rn(fmaxf(d0[0], 0.f), fmaxf(d0[1], 0.f)), h01 = __floats2half2_rn(fmaxf(d0[2], 0.f), fmaxf(d0[3], 0.f));
-            const __half2 h10 = __floats2half2_rn(fmaxf(d1[0], 0.f), fmaxf(d1[1], 0.f)), h11 = __floats2half2_rn(fmaxf(d1[2], 0.f), fmaxf(d1[3], 0.f));
-            *reinterpret_cast<uint2 *>(s_a1 + row * 16 + plane * 8) = make_uint2(*reinterpret_cast<const uint32_t *>(&h00), *reinterpret_cast<const uint32_t *>(&h01));
-            *reinterpret_cast<uint2 *>(s_a1 + (row + 16) * 16 + plane * 8) = make_uint2(*reinterpret_cast<const uint32_t *>(&h10), *reinterpret_cast<const uint32_t *>(&h11));
-            *reinterpret_cast<uint4 *>(s_a1 + STEM_LBO1 + tid * 16) = make_uint4(0, 0, 0, 0);      // K padding (channels 8..15)
+#pragma unroll
+            for (int g = 0; g < 4; g++)
+                *reinterpret_cast<uint4 *>(s_a0 + g * STEM_LBO0 + p * 16) = make_uint4(h2[4 * g], h2[4 * g + 1], h2[4 * g + 2], h2[4 * g + 3]);
         }
-    }
-    if constexpr (I8) {
-        // ---- 6'. pointwise 8 -> 16 in FP32 (k_stem's operation order), ReLU, quantise, one 16-byte store per pixel -------
+        tc::fence_async_smem();
         __syncthreads();
-        const float (*s_dwo)[256][4] = reinterpret_cast<const float (*)[256][4]>(s_a1);
-        const float *s_wp = s_bias2 + 16;
-        const int oy = oy0 + (tid >> 4), ox = ox0 + (tid & 15);
-        if (oy < OH && ox < OW) {
-            const float4 da = *reinterpret_cast<const float4 *>(&s_dwo[0][tid][0]), db = *reinterpret_cast<const float4 *>(&s_dwo[1][tid][0]);
-            const float d[8] = {da.x, da.y, da.z, da.w, db.x, db.y, db.z, db.w};
-            float o[16];
+        tc::mbar_wait(&bar_w, 0);            // B images and the FP32 constants
+        const int wgi = warp >> 2, c2 = 2 * (lane & 3);
+        const int rl = 16 * (warp & 3) + (lane >> 2);      // fragment rows rl, rl + 8 of each 64-row block (wgmma.cuh)
+        // ---- 3. conv0 GEMM: warpgroup w computes row blocks w, w + 2, w + 4 ---------------------------------------------------
+        float d0[3][8];
+        {
+            const uint32_t a0 = tc::smem_u32(s_a0), b0 = tc::smem_u32(s_b0);
 #pragma unroll
-            for (int j = 0; j < 16; j++) o[j] = s_bias2[j];
+            for (int j = 0; j < 3; j++)
 #pragma unroll
-            for (int c = 0; c < 8; c++)
+                for (int i = 0; i < 8; i++) d0[j][i] = 0.f;
+            wg::fence();
+#pragma unroll
+            for (int j = 0; j < 3; j++)
+#pragma unroll
+                for (int part = 0; part < 2; part++)
+#pragma unroll
+                    for (int ks = 0; ks < 2; ks++) {
+                        const uint64_t ad = wg::desc(a0 + (uint32_t)(2 * ks) * STEM_LBO0 + (uint32_t)(64 * (wgi + 2 * j)) * 16, STEM_LBO0, 128);
+                        const uint64_t bd = wg::desc(b0 + (uint32_t)(part * 4 + 2 * ks) * 256, 256, 128);
+                        wg::mma_ss<16>(d0[j], ad, bd, part | ks);
+                    }
+            wg::commit();
+            wg::wait<0>();
+#pragma unroll
+            for (int j = 0; j < 3; j++) wg::fence_regs(d0[j]);
+        }
+        __syncthreads();                     // conv0's operand is dead: s_c0 overwrites it
+        // ---- 4. conv0 epilogue -> s_c0 (FP32), zero outside the map (columns 8..15 of the N = 16 tile are padding) ------------
+#pragma unroll
+        for (int j = 0; j < 3; j++)
+#pragma unroll
+            for (int e = 0; e < 2; e++) {
+                const int p = 64 * (wgi + 2 * j) + rl + 8 * e;
+                if (p < 324) {
+                    const int py = p / 18, px = p - py * 18;
+                    const int cy = oy0 - 1 + py, cx = ox0 - 1 + px;
+                    const bool inside = cy >= 0 && cy < OH && cx >= 0 && cx < OW;
+                    const float v0 = inside ? fmaxf(d0[j][2 * e] + s_bias0[c2], 0.f) : 0.f;
+                    const float v1 = inside ? fmaxf(d0[j][2 * e + 1] + s_bias0[c2 + 1], 0.f) : 0.f;
+                    *reinterpret_cast<float2 *>(&s_c0[c2 >> 2][p][c2 & 3]) = make_float2(v0, v1);
+                }
+            }
+        __syncthreads();
+        // ---- 5. depthwise 3x3 + ReLU -> A1 (FP16, GEMM row = pixel ty * 16 + tx) ------------------------------------------------
+        // thread = (4-channel plane, column, PAIR of output rows): 4 ring rows x 3 columns = 12 loads feed 2 outputs, the 9
+        // weight vectors of the plane are warp-uniform (broadcast).  Per output the accumulation order is (ky, kx) ascending.
+        {
+            const int plane = tid >> 7, q = tid & 127;
+            const int tx = q & 15, ty = (q >> 4) << 1;
+            const float4 bv = *reinterpret_cast<const float4 *>(&s_wd[72 + plane * 4]);
+            float d0[4] = {bv.x, bv.y, bv.z, bv.w}, d1[4] = {bv.x, bv.y, bv.z, bv.w};
+#pragma unroll
+            for (int ry = 0; ry < 4; ry++)
+#pragma unroll
+                for (int kx = 0; kx < 3; kx++) {
+                    const float4 a = *reinterpret_cast<const float4 *>(&s_c0[plane][(ty + ry) * 18 + tx + kx][0]);
+                    if (ry < 3) {
+                        const float4 w = *reinterpret_cast<const float4 *>(&s_wd[(ry * 3 + kx) * 8 + plane * 4]);
+                        d0[0] = fmaf(a.x, w.x, d0[0]); d0[1] = fmaf(a.y, w.y, d0[1]); d0[2] = fmaf(a.z, w.z, d0[2]); d0[3] = fmaf(a.w, w.w, d0[3]);
+                    }
+                    if (ry > 0) {
+                        const float4 w = *reinterpret_cast<const float4 *>(&s_wd[((ry - 1) * 3 + kx) * 8 + plane * 4]);
+                        d1[0] = fmaf(a.x, w.x, d1[0]); d1[1] = fmaf(a.y, w.y, d1[1]); d1[2] = fmaf(a.z, w.z, d1[2]); d1[3] = fmaf(a.w, w.w, d1[3]);
+                    }
+                }
+            const int row = ty * 16 + tx;
+            if constexpr (I8) {
+                // FP32 depthwise output -> shared [plane][pixel][4] (the pointwise operand's place, unused here)
+                float (*s_dwo)[256][4] = reinterpret_cast<float (*)[256][4]>(s_a1);
+                *reinterpret_cast<float4 *>(&s_dwo[plane][row][0]) = make_float4(fmaxf(d0[0], 0.f), fmaxf(d0[1], 0.f), fmaxf(d0[2], 0.f), fmaxf(d0[3], 0.f));
+                *reinterpret_cast<float4 *>(&s_dwo[plane][row + 16][0]) = make_float4(fmaxf(d1[0], 0.f), fmaxf(d1[1], 0.f), fmaxf(d1[2], 0.f), fmaxf(d1[3], 0.f));
+            } else {
+                const __half2 h00 = __floats2half2_rn(fmaxf(d0[0], 0.f), fmaxf(d0[1], 0.f)), h01 = __floats2half2_rn(fmaxf(d0[2], 0.f), fmaxf(d0[3], 0.f));
+                const __half2 h10 = __floats2half2_rn(fmaxf(d1[0], 0.f), fmaxf(d1[1], 0.f)), h11 = __floats2half2_rn(fmaxf(d1[2], 0.f), fmaxf(d1[3], 0.f));
+                *reinterpret_cast<uint2 *>(s_a1 + row * 16 + plane * 8) = make_uint2(*reinterpret_cast<const uint32_t *>(&h00), *reinterpret_cast<const uint32_t *>(&h01));
+                *reinterpret_cast<uint2 *>(s_a1 + (row + 16) * 16 + plane * 8) = make_uint2(*reinterpret_cast<const uint32_t *>(&h10), *reinterpret_cast<const uint32_t *>(&h11));
+                *reinterpret_cast<uint4 *>(s_a1 + STEM_LBO1 + tid * 16) = make_uint4(0, 0, 0, 0);      // K padding (channels 8..15)
+            }
+        }
+        if constexpr (I8) {
+            // ---- 6'. pointwise 8 -> 16 in FP32 (k_stem's operation order), ReLU, quantise, one 16-byte store per pixel -------
+            __syncthreads();
+            const float (*s_dwo)[256][4] = reinterpret_cast<const float (*)[256][4]>(s_a1);
+            const float *s_wp = s_bias2 + 16;
+            const int oy = oy0 + (tid >> 4), ox = ox0 + (tid & 15);
+            if (oy < OH && ox < OW) {
+                const float4 da = *reinterpret_cast<const float4 *>(&s_dwo[0][tid][0]), db = *reinterpret_cast<const float4 *>(&s_dwo[1][tid][0]);
+                const float d[8] = {da.x, da.y, da.z, da.w, db.x, db.y, db.z, db.w};
+                float o[16];
+#pragma unroll
+                for (int j = 0; j < 16; j++) o[j] = s_bias2[j];
+#pragma unroll
+                for (int c = 0; c < 8; c++)
+#pragma unroll
+                    for (int j4 = 0; j4 < 4; j4++) {
+                        const float4 wv = *reinterpret_cast<const float4 *>(&s_wp[c * 16 + j4 * 4]);
+                        o[j4 * 4 + 0] = fmaf(d[c], wv.x, o[j4 * 4 + 0]); o[j4 * 4 + 1] = fmaf(d[c], wv.y, o[j4 * 4 + 1]);
+                        o[j4 * 4 + 2] = fmaf(d[c], wv.z, o[j4 * 4 + 2]); o[j4 * 4 + 3] = fmaf(d[c], wv.w, o[j4 * 4 + 3]);
+                    }
+                uint32_t pk[4];
 #pragma unroll
                 for (int j4 = 0; j4 < 4; j4++) {
-                    const float4 wv = *reinterpret_cast<const float4 *>(&s_wp[c * 16 + j4 * 4]);
-                    o[j4 * 4 + 0] = fmaf(d[c], wv.x, o[j4 * 4 + 0]); o[j4 * 4 + 1] = fmaf(d[c], wv.y, o[j4 * 4 + 1]);
-                    o[j4 * 4 + 2] = fmaf(d[c], wv.z, o[j4 * 4 + 2]); o[j4 * 4 + 3] = fmaf(d[c], wv.w, o[j4 * 4 + 3]);
-                }
-            uint32_t pk[4];
+                    uint32_t word = 0;
 #pragma unroll
-            for (int j4 = 0; j4 < 4; j4++) {
-                uint32_t word = 0;
-#pragma unroll
-                for (int k = 0; k < 4; k++) {
-                    int q = __float2int_rn(__fmul_rn(fmaxf(o[j4 * 4 + k], 0.f), out_inv_scale));
-                    q = max(-127, min(127, q));
-                    word |= (uint32_t)(q & 0xff) << (8 * k);
+                    for (int k = 0; k < 4; k++) {
+                        int q = __float2int_rn(__fmul_rn(fmaxf(o[j4 * 4 + k], 0.f), out_inv_scale));
+                        q = max(-127, min(127, q));
+                        word |= (uint32_t)(q & 0xff) << (8 * k);
+                    }
+                    pk[j4] = word;
                 }
-                pk[j4] = word;
+                *reinterpret_cast<uint4 *>(out + (((size_t)b * OH + oy) * OW + ox) * 16) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
             }
-            *reinterpret_cast<uint4 *>(out + (((size_t)b * OH + oy) * OW + ox) * 16) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+        } else {
+        tc::fence_async_smem();
+        __syncthreads();
+        // ---- 6. pointwise GEMM: warpgroup w computes row blocks w, w + 2 ---------------------------------------------------------
+        float d1[2][8];
+        {
+            const uint32_t a1 = tc::smem_u32(s_a1), b1 = tc::smem_u32(s_b1);
+#pragma unroll
+            for (int j = 0; j < 2; j++)
+#pragma unroll
+                for (int i = 0; i < 8; i++) d1[j][i] = 0.f;
+            wg::fence();
+#pragma unroll
+            for (int j = 0; j < 2; j++)
+                wg::mma_ss<16>(d1[j], wg::desc(a1 + (uint32_t)(64 * (wgi + 2 * j)) * 16, STEM_LBO1, 128), wg::desc(b1, 256, 128), 0);
+            wg::commit();
+            wg::wait<0>();
+#pragma unroll
+            for (int j = 0; j < 2; j++) wg::fence_regs(d1[j]);
         }
-    } else {
-    tc::fence_async_smem();
-    __syncthreads();
-    // ---- 6. pointwise GEMM: warpgroup w computes row blocks w, w + 2 ---------------------------------------------------------
-    float d1[2][8];
-    {
-        const uint32_t a1 = tc::smem_u32(s_a1), b1 = tc::smem_u32(s_b1);
+        // ---- 7. epilogue: + bias, ReLU, FP16, store ----------------------------------------------------------------------------
 #pragma unroll
         for (int j = 0; j < 2; j++)
 #pragma unroll
-            for (int i = 0; i < 8; i++) d1[j][i] = 0.f;
-        wg::fence();
+            for (int e = 0; e < 2; e++) {
+                const int row = 64 * (wgi + 2 * j) + rl + 8 * e;      // pixel ty * 16 + tx of step 5
+                const int oy = oy0 + (row >> 4), ox = ox0 + (row & 15);
+                if (oy < OH && ox < OW) {
+                    __half *dst = reinterpret_cast<__half *>(out) + (((size_t)b * OH + oy) * OW + ox) * 16;
 #pragma unroll
-        for (int j = 0; j < 2; j++)
-            wg::mma_ss<16>(d1[j], wg::desc(a1 + (uint32_t)(64 * (wgi + 2 * j)) * 16, STEM_LBO1, 128), wg::desc(b1, 256, 128), 0);
-        wg::commit();
-        wg::wait<0>();
-#pragma unroll
-        for (int j = 0; j < 2; j++) wg::fence_regs(d1[j]);
-    }
-    // ---- 7. epilogue: + bias, ReLU, FP16, store ----------------------------------------------------------------------------
-#pragma unroll
-    for (int j = 0; j < 2; j++)
-#pragma unroll
-        for (int e = 0; e < 2; e++) {
-            const int row = 64 * (wgi + 2 * j) + rl + 8 * e;      // pixel ty * 16 + tx of step 5
-            const int oy = oy0 + (row >> 4), ox = ox0 + (row & 15);
-            if (oy < OH && ox < OW) {
-                __half *dst = reinterpret_cast<__half *>(out) + (((size_t)b * OH + oy) * OW + ox) * 16;
-#pragma unroll
-                for (int i = 0; i < 2; i++) {
-                    const int c = 8 * i + c2;
-                    *reinterpret_cast<__half2 *>(dst + c) = __floats2half2_rn(fmaxf(d1[j][4 * i + 2 * e] + s_bias2[c], 0.f),
-                                                                              fmaxf(d1[j][4 * i + 2 * e + 1] + s_bias2[c + 1], 0.f));
+                    for (int i = 0; i < 2; i++) {
+                        const int c = 8 * i + c2;
+                        *reinterpret_cast<__half2 *>(dst + c) = __floats2half2_rn(fmaxf(d1[j][4 * i + 2 * e] + s_bias2[c], 0.f),
+                                                                                  fmaxf(d1[j][4 * i + 2 * e + 1] + s_bias2[c + 1], 0.f));
+                    }
                 }
             }
         }

@@ -114,6 +114,10 @@ __device__ __forceinline__ void cp_async16_zfill_s(uint32_t smem_dst, const void
     const unsigned sz = valid ? 16u : 0u;
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_dst), "l"(gsrc), "r"(sz) : "memory");
 }
+__device__ __forceinline__ void cp_async4(void *smem_dst, const void *gsrc) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(tc::smem_u32(smem_dst)), "l"(gsrc) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() {
     asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 0;" ::: "memory");
 }

@@ -6,8 +6,8 @@
 // with the accumulator in registers.  What differs is the tile: TH x TW output pixels of ONE image (TH*TW <= 128) instead of
 // 128 consecutive pixels of the linearised map.  On a wide map the 1-D tile stages 128 + 2*(W+3) input positions for 128
 // outputs (2.8x at W = 112); the 2-D tile stages ((TH-1)*S+3) x ((TW-1)*S+3) (1.4x), needs no position table (a staged
-// row is a contiguous run of the NHWC input: the cp.async addresses are affine in the lane), and a 2x2 block of adjacent
-// outputs sits in one thread: each staged activation it reads is converted once for all four (dw_stencil_block).
+// row is a contiguous run of the NHWC input: the cp.async addresses are affine in the lane), and a pair of horizontally
+// adjacent outputs sits in one thread: each staged activation it reads is converted once for both (dw_stencil_block).
 #pragma once
 #include "tc_conv.cuh"
 
@@ -19,6 +19,7 @@ struct TcDw2dArgs {
     int N;                  // output channels (multiple of 16, <= 256)
     int TH, TW;             // output tile, TH * TW <= 128, TH even
     int tiles_x, tiles_y;
+    int run;                // consecutive tiles per CTA (tiles of all images numbered image-major); grid = ceil(tiles / run)
     int PH, PW;             // staged window: (TH-1)*S+3 x (TW-1)*S+3   (tc_dw2d_finish)
     uint32_t lbo_a;         // group stride of the A operand, bytes (tc_dw2d_finish)
     uint32_t mul_TW, mul_tiles_x, mul_tiles;   // fast_div multipliers (tc_dw2d_finish)
@@ -45,11 +46,11 @@ inline void tc_dw2d_finish(TcDw2dArgs &a) {
     a.mul_tiles = fast_div_mul((uint32_t)(a.tiles_x * a.tiles_y));
 }
 inline size_t tc_dw2d_smem_bytes(const TcDw2dArgs &a) {
-    return (size_t)a.PH * a.PW * a.C * 2 + (size_t)(a.C / 8) * a.lbo_a + (size_t)a.C * a.N * 2 + 128;
+    return 2 * (size_t)a.PH * a.PW * a.C * 2 + (size_t)(a.C / 8) * a.lbo_a + (size_t)a.C * a.N * 2 + 128;
 }
 
-// resident CTAs per SM the register allocation aims at (80 registers at 3: the 2x2 output block of the stencil holds 32
-// accumulators, and at 4 -- 64 registers -- it spills).  The pointwise accumulator is taken in chunks of at most 32 columns.
+// resident CTAs per SM the register allocation aims at (80 registers at 3; at 4 -- 64 registers -- the persistent loop
+// spills).  The pointwise accumulator is taken in chunks of at most 32 columns.
 #ifndef RF_DW2D_OCC
 #define RF_DW2D_OCC 3
 #endif
@@ -66,14 +67,17 @@ __global__ void __launch_bounds__(TC_THREADS, RF_DW2D_OCC) k_tc_dwpw_2d(const Tc
     const int PH = a.PH, PW = a.PW;
     const uint32_t lbo_a = a.lbo_a;
     const int pix = a.C * 2;             // bytes per staged pixel
-    unsigned char *sS = smem;
-    unsigned char *sA = smem + (size_t)PH * PW * pix;
+    const uint32_t stage_bytes = (uint32_t)(PH * PW * pix);
+    unsigned char *sA = smem + 2 * (size_t)stage_bytes;          // behind the two staging buffers
     unsigned char *sB = sA + (size_t)G * lbo_a;
     const int tiles = a.tiles_x * a.tiles_y;
-    const int b = fast_div((int)blockIdx.x, a.mul_tiles), trem = blockIdx.x - b * tiles;
-    const int ty0 = fast_div(trem, a.mul_tiles_x);
-    const int oy0 = ty0 * a.TH, ox0 = (trem - ty0 * a.tiles_x) * a.TW;
-    const int iy0 = oy0 * a.S - 1, ix0 = ox0 * a.S - 1;          // input coordinates of staged (0, 0)
+    const int t_end = min((int)blockIdx.x * a.run + a.run, tiles * a.nimg);
+    // tile t -> image b, output origin (oy0, ox0); a CTA's run of tiles may cross from one image into the next
+    auto decode = [&](int t, int &b, int &oy0, int &ox0) {
+        b = fast_div(t, a.mul_tiles);
+        const int trem = t - b * tiles, ty0 = fast_div(trem, a.mul_tiles_x);
+        oy0 = ty0 * a.TH; ox0 = (trem - ty0 * a.tiles_x) * a.TW;
+    };
 
     if (tid == 0) {
         tc::mbar_init(&bar_b, 1);
@@ -87,83 +91,98 @@ __global__ void __launch_bounds__(TC_THREADS, RF_DW2D_OCC) k_tc_dwpw_2d(const Tc
     for (int i = tid; i < 9 * a.C; i += TC_THREADS) s_dww[i] = dw_weight_f16(a.dw_w[i]);
     if (tid < a.C) s_dwb[tid] = a.dw_b[tid];
     pdl_wait();
-    // ---- stage the (PH x PW) input window: one warp per staged row, lanes over (column, channel group) -- a staged row
-    // is PW*C contiguous halfs of the input (16 B per lane, fully coalesced); outside the map: zero fill ------------------
-    {
+    // ---- stage tile t's (PH x PW) input window into buffer buf: one warp per staged row, lanes over (column, channel
+    // group) -- a staged row is PW*C contiguous halfs of the input (16 B per lane, fully coalesced); outside the map: zero fill
+    const uint32_t sS_s = tc::smem_u32(smem);
+    auto stage = [&](int t, int buf) {
+        int b, oy0, ox0;
+        decode(t, b, oy0, ox0);
+        const int iy0 = oy0 * a.S - 1, ix0 = ox0 * a.S - 1;      // input coordinates of staged (0, 0)
         // item i of a row = (column px = i / G, group g = i % G): with C = 8 G its source is src_row + 8 i halfs -- affine in i
         const int per_row = PW << lg;
         const int px_lo = max(0, -ix0), px_hi = min(PW, a.IW - ix0);       // columns inside the map
         const unsigned px_n = (unsigned)max(px_hi - px_lo, 0);
-        const uint32_t sS_s = tc::smem_u32(sS);
         for (int py = warp; py < PH; py += TC_THREADS / 32) {
             const int iy = iy0 + py;
             const bool rowok = iy >= 0 && iy < a.IH;
             const __half *src_row = a.in + (ptrdiff_t)(((b * a.IH + (rowok ? iy : 0)) * a.IW + ix0) * a.C);
-            const uint32_t dst_row = sS_s + (uint32_t)(py * PW * pix);
+            const uint32_t dst_row = sS_s + (uint32_t)buf * stage_bytes + (uint32_t)(py * PW * pix);
             const __half *zsrc = a.in;      // any valid address: zero bytes are read from it
             for (int i = lane; i < per_row; i += 32) {
                 const bool ok = rowok && (unsigned)((i >> lg) - px_lo) < px_n;
                 cp_async16_zfill_s(dst_row + (uint32_t)i * 16u, ok ? src_row + i * 8 : zsrc, ok);
             }
         }
-    }
-    cp_async_wait_all();
-    __syncthreads();
-    // ---- depthwise stencil -> A operand.  GEMM row r = ty * TW + tx ------------------------------------------------------
-    // item = (channel group, 2x2 block of outputs): at stride 1 a 4x4 window feeds 4 outputs (16 conversions for 36 taps), at
-    // stride 2 a 5x5 window (25 for 36).  TH and TW are even.
-    const int rows = a.TH * a.TW;
-    auto stencil = [&](auto s_) {
+        cp_async_commit();
+    };
+    // ---- depthwise stencil of the window at sS -> A operand.  GEMM row r = ty * TW + tx ------------------------------------
+    // item = (channel group, pair of horizontally adjacent outputs): at stride 1 a 3x4 window feeds 2 outputs (12 conversions
+    // for 18 taps), at stride 2 a 3x5 window (15 for 18).  TW is even.  A 2x2 block (16 / 25 conversions for 36 taps) has half
+    // as many items, which leaves half the threads idle at C = 32 and three quarters at C = 16 while the stencil runs.
+    auto stencil = [&](auto s_, const unsigned char *sS) {
         constexpr int S = decltype(s_)::value;
-        const int items = (a.TH >> 1) * (a.TW >> 1) << lg;
+        const int items = a.TH * (a.TW >> 1) << lg;
         for (int it = tid; it < items; it += TC_THREADS) {
             const int g = it & (G - 1), rest = it >> lg;
-            const int typ = fast_div(2 * rest, a.mul_TW), ty = 2 * typ, tx = 2 * rest - typ * a.TW;
-            float acc[2][2][8];
+            const int ty = fast_div(2 * rest, a.mul_TW), tx = 2 * rest - ty * a.TW;
+            float acc[1][2][8];
             dw_bias8(acc[0][0], &s_dwb[g * 8]);
 #pragma unroll
-            for (int i = 0; i < 8; i++) { acc[0][1][i] = acc[0][0][i]; acc[1][0][i] = acc[0][0][i]; acc[1][1][i] = acc[0][0][i]; }
-            dw_stencil_block<S, 2, 2>(acc, sS + (ty * S * PW + tx * S) * pix + g * 16, PW * pix, pix, &s_dww[g * 8], a.C);
-            const int r = ty * a.TW + tx;
-            unsigned char *dst = sA + (size_t)g * lbo_a + (size_t)r * 16;
+            for (int i = 0; i < 8; i++) acc[0][1][i] = acc[0][0][i];
+            dw_stencil_block<S, 1, 2>(acc, sS + (ty * S * PW + tx * S) * pix + g * 16, PW * pix, pix, &s_dww[g * 8], a.C);
+            unsigned char *dst = sA + (size_t)g * lbo_a + (size_t)(ty * a.TW + tx) * 16;
             *reinterpret_cast<uint4 *>(dst) = dw_relu_h8(acc[0][0]);
             *reinterpret_cast<uint4 *>(dst + 16) = dw_relu_h8(acc[0][1]);
-            *reinterpret_cast<uint4 *>(dst + a.TW * 16) = dw_relu_h8(acc[1][0]);
-            *reinterpret_cast<uint4 *>(dst + a.TW * 16 + 16) = dw_relu_h8(acc[1][1]);
         }
     };
-    if (a.S == 1) stencil(std::integral_constant<int, 1>{});
-    else stencil(std::integral_constant<int, 2>{});
-    tc::fence_async_smem();
-    __syncthreads();
-    if (64 * (warp >> 2) >= rows) return;         // the second warpgroup has no GEMM rows
-    tc::mbar_wait(&bar_b, 0);
-    long orow[2];
+    const int rows = a.TH * a.TW;
+    const bool has_gemm = 64 * (warp >> 2) < rows;      // the second warpgroup has no GEMM rows when TH * TW <= 64
+    const int t_begin = (int)blockIdx.x * a.run;
+    stage(t_begin, 0);
+    // ---- persistent loop over the CTA's run of tiles: tile t + 1's window is in flight while tile t computes -------------
+    for (int t = t_begin; t < t_end; t++) {
+        const int buf = (t - t_begin) & 1;
+        cp_async_wait_all();
+        // tile t's window has landed, and every thread is done with tile t - 1: its stencil has read the other staging
+        // buffer, its wgmma chains (wg::wait<0>) have read sA
+        __syncthreads();
+        if (t + 1 < t_end) stage(t + 1, buf ^ 1);
+        const unsigned char *sS = smem + (size_t)buf * stage_bytes;
+        if (a.S == 1) stencil(std::integral_constant<int, 1>{}, sS);
+        else stencil(std::integral_constant<int, 2>{}, sS);
+        tc::fence_async_smem();
+        __syncthreads();
+        if (!has_gemm) continue;                     // no GEMM rows, but the next tile's barriers are reached
+        tc::mbar_wait(&bar_b, 0);
+        int b, oy0, ox0;
+        decode(t, b, oy0, ox0);
+        long orow[2];
 #pragma unroll
-    for (int e = 0; e < 2; e++) {
-        const int r = tc_frag_row() + 8 * e;
-        const int ty = fast_div(r, a.mul_TW), tx = r - ty * a.TW;
-        const int oy = oy0 + ty, ox = ox0 + tx;
-        orow[e] = (r < rows && oy < a.OH && ox < a.OW) ? (long)((b * a.OH + oy) * a.OW + ox) : -1;
-    }
-    const uint32_t a_addr = tc::smem_u32(sA) + (uint32_t)(64 * (warp >> 2)) * 16u, b_addr = tc::smem_u32(sB);
-    const uint32_t lbo_b = (uint32_t)a.N * 16;
-    const TcOut o{a.out, a.N, a.N, 1, nullptr, 0, 0};
-    wg::for_chunks<(NT < 32 ? NT : 32)>(a.N, [&](auto nc, int n0) {
-        constexpr int NC = decltype(nc)::value;
-        float d[NC / 2];                 // not zeroed: the first MMA runs with scale-d = 0 (see wg::fence)
-        wg::fence();
-        wg::mma_ss<NC>(d, wg::desc(a_addr, lbo_a, 128), wg::desc(b_addr + (uint32_t)n0 * 16u, lbo_b, 128), 0);
-        for (int ks = 1; ks < (a.C >> 4); ks++) {
-            const uint64_t ad = wg::desc(a_addr + (uint32_t)(2 * ks) * lbo_a, lbo_a, 128);
-            const uint64_t bd = wg::desc(b_addr + (uint32_t)(2 * ks) * lbo_b + (uint32_t)n0 * 16u, lbo_b, 128);
-            wg::mma_ss<NC>(d, ad, bd, 1);
+        for (int e = 0; e < 2; e++) {
+            const int r = tc_frag_row() + 8 * e;
+            const int ty = fast_div(r, a.mul_TW), tx = r - ty * a.TW;
+            const int oy = oy0 + ty, ox = ox0 + tx;
+            orow[e] = (r < rows && oy < a.OH && ox < a.OW) ? (long)((b * a.OH + oy) * a.OW + ox) : -1;
         }
-        wg::commit();
-        wg::wait<0>();
-        wg::fence_regs(d);
-        tc_epilogue<NC>(d, n0, s_bias, o, orow, 0);
-    });
+        const uint32_t a_addr = tc::smem_u32(sA) + (uint32_t)(64 * (warp >> 2)) * 16u, b_addr = tc::smem_u32(sB);
+        const uint32_t lbo_b = (uint32_t)a.N * 16;
+        const TcOut o{a.out, a.N, a.N, 1, nullptr, 0, 0};
+        wg::for_chunks<(NT < 32 ? NT : 32)>(a.N, [&](auto nc, int n0) {
+            constexpr int NC = decltype(nc)::value;
+            float d[NC / 2];                 // not zeroed: the first MMA runs with scale-d = 0 (see wg::fence)
+            wg::fence();
+            wg::mma_ss<NC>(d, wg::desc(a_addr, lbo_a, 128), wg::desc(b_addr + (uint32_t)n0 * 16u, lbo_b, 128), 0);
+            for (int ks = 1; ks < (a.C >> 4); ks++) {
+                const uint64_t ad = wg::desc(a_addr + (uint32_t)(2 * ks) * lbo_a, lbo_a, 128);
+                const uint64_t bd = wg::desc(b_addr + (uint32_t)(2 * ks) * lbo_b + (uint32_t)n0 * 16u, lbo_b, 128);
+                wg::mma_ss<NC>(d, ad, bd, 1);
+            }
+            wg::commit();
+            wg::wait<0>();
+            wg::fence_regs(d);
+            tc_epilogue<NC>(d, n0, s_bias, o, orow, 0);
+        });
+    }
 }
 
 }  // namespace rf

@@ -268,6 +268,41 @@ int rf_detect_align_batch_device(rf_handle h, const uint8_t *dev_bgr, int n, flo
  * letter-boxes one host image into a host net_h*net_w*3 u8 BGR buffer using the GPU kernel. */
 int rf_preprocess(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, uint8_t *out_net_sized);
 
+/* f6 video frames: detect (and align) on 8-bit YUV 4:2:0 frames -- NVDEC's NV12 surfaces, software decoders' I420, cameras' NV21
+ * -- with the colour conversion fused into the letter-box kernel: each source tap is converted to BGR before the unchanged resize,
+ * so the network input is byte for byte the letter-box of cv2.cvtColor(frame, COLOR_YUV2BGR_<layout>) (nearest chroma, OpenCV's
+ * 20-bit fixed point), under either resize definition (RF_FLAG_NPP_RESIZE), and a crop is cv2.warpAffine(cvtColor(frame), M).
+ * One descriptor covers all four layouts: NV12 = {y, u = uv, v = uv + 1, uv_step 2}, NV21 = {v = vu, u = vu + 1, uv_step 2},
+ * I420 / YV12 = three planes, uv_step 1.  Chroma sample j of chroma row r is at u[r * uv_pitch + j * uv_step] (v likewise).
+ * Invalid descriptors (size not positive and even, a NULL plane, uv_step not 1 or 2, semi-planar u and v not adjacent bytes,
+ * y_pitch < width, uv_pitch < width / 2 * uv_step), an unknown matrix or bad align params: RF_ERR_INVALID_ARG; a frame larger
+ * than max_image or n > max_batch: RF_ERR_CAPACITY; both before anything is launched. */
+typedef struct rf_yuv_frame {
+    const uint8_t *y, *u, *v;        /* plane origins */
+    int y_pitch, uv_pitch, uv_step;  /* bytes; uv_step 2: semi-planar (NV12, NV21), 1: planar (I420, YV12) */
+    int width, height;               /* even, <= max_image */
+} rf_yuv_frame;
+#define RF_YUV_BT601 0               /* == cv2.COLOR_YUV2BGR_{NV12,NV21,I420,YV12} */
+#define RF_YUV_BT709 1               /* the same formula with round(c * 2^20) of the limited-range BT.709 matrix (NVDEC's HD output) */
+/* Host frames (pinned or pageable): the planes are uploaded as they are, 1.5 bytes per pixel, into the raw buffers, letter-boxed
+ * and detected on context 0; blocking.  out_faces [n][max_faces] / out_counts / out_anchor_index as rf_detect_batch, but in FRAME
+ * pixels (rf_detect_align_batch's map-back).  align == NULL: no crops, frames are staged a chunk of raw buffers at a time.
+ * Otherwise crops and matrices as rf_detect_align_batch (out_crops required, out_mats optional); every frame then needs its own
+ * raw buffer while the crops are cut: more frames than the handle has is RF_ERR_CAPACITY. */
+int rf_detect_yuv_batch(rf_handle h, const rf_yuv_frame *frames, int n, int matrix, float score_threshold, float nms_threshold,
+                        const rf_align_params *align, rf_face *out_faces, int *out_counts, int32_t *out_anchor_index, void *out_crops,
+                        double *out_mats);
+/* Device frames (frames: host array of descriptors of DEVICE planes), read in place and never written; the caller keeps them alive
+ * until rf_last_stream() passes this call.  Asynchronous, rotating over the execution contexts like rf_detect_batch_device, each
+ * context letter-boxing into an input tensor of its own; *dev_dets / *dev_counts as there (network-input pixels), out_scales
+ * (host, [n]) receives each frame's map-back factor.  align != NULL: crops into dev_crops (required) and dev_mats (optional) as
+ * rf_detect_align_batch_device. */
+int rf_detect_yuv_batch_device(rf_handle h, const rf_yuv_frame *frames, int n, int matrix, float score_threshold, float nms_threshold,
+                               const rf_align_params *align, void *dev_crops, double *dev_mats, const rf_det **dev_dets,
+                               const int32_t **dev_counts, float *out_scales);
+/* Preprocess parity of f6 (as rf_preprocess): one host frame letter-boxed into a host net_h*net_w*3 u8 BGR buffer. */
+int rf_preprocess_yuv(rf_handle h, const rf_yuv_frame *frame, int matrix, uint8_t *out_net_sized);
+
 /* Introspection. */
 int rf_get_net_size(rf_handle h, int *net_w, int *net_h, int *max_batch, int *max_faces);
 int rf_num_anchors(rf_handle h);            /* per image: 8,232 @448x448, 47,040 @1280x896 */

@@ -27,6 +27,7 @@ EXPORTS = [
     "rf_model_load", "rf_network_config", "rf_cache_status",
     "rf_detect_jpeg_batch", "rf_decode_jpeg", "rf_jpeg_backend",
     "rf_detect_align_batch", "rf_detect_align_batch_device",
+    "rf_detect_yuv_batch", "rf_detect_yuv_batch_device", "rf_preprocess_yuv",
 ]
 COMM_BLOB_BYTES = 128
 
@@ -60,6 +61,73 @@ def crop_shape(fmt: str, crop) -> Tuple[tuple, type]:
     _, dt, hwc = CROP_FORMATS[fmt]
     w, h = int(crop[0]) or 112, int(crop[1]) or 112
     return ((h, w, 3) if hwc else (3, h, w)), dt
+
+
+class YuvFrame(C.Structure):     # rf_yuv_frame
+    _fields_ = [("y", C.c_void_p), ("u", C.c_void_p), ("v", C.c_void_p), ("y_pitch", C.c_int), ("uv_pitch", C.c_int), ("uv_step", C.c_int),
+                ("width", C.c_int), ("height", C.c_int)]
+
+
+RF_YUV_BT601, RF_YUV_BT709 = 0, 1
+YUV_MATRICES = {"bt601": RF_YUV_BT601, "bt709": RF_YUV_BT709}
+YUV_LAYOUTS = ("nv12", "nv21", "i420", "yv12")
+
+
+def _plane(a):
+    """(address, row pitch in bytes, rows, row bytes, on the GPU) of a 2-D u8 plane: a numpy array or a torch tensor whose rows are
+    contiguous (pitch >= row bytes)."""
+    if hasattr(a, "data_ptr"):          # torch
+        if a.dtype.itemsize != 1 or a.dim() != 2 or a.stride(1) != 1:
+            raise ValueError(f"2-D uint8 plane with contiguous rows expected, got {tuple(a.shape)} {a.dtype} strides {a.stride()}")
+        return a.data_ptr(), a.stride(0), a.shape[0], a.shape[1], a.is_cuda
+    a = np.asarray(a)
+    if a.dtype != np.uint8 or a.ndim != 2 or a.strides[1] != 1:
+        raise ValueError(f"2-D uint8 plane with contiguous rows expected, got {a.shape} {a.dtype} strides {a.strides}")
+    return a.ctypes.data, a.strides[0], a.shape[0], a.shape[1], False
+
+
+def yuv_frame(frame, layout: str = "nv12") -> Tuple[YuvFrame, bool]:
+    """rf_yuv_frame of one 4:2:0 frame, and whether its planes are device memory.  `frame`: OpenCV's single buffer, a C-contiguous
+    (h * 3 / 2, w) u8 array / tensor in `layout` (nv12 | nv21 | i420 | yv12); or planes with their own pitches, (y, uv) for nv12 /
+    nv21 (uv: (h / 2, w) interleaved) or (y, u, v) in that order for i420 / yv12 (u, v: (h / 2, w / 2)).  The caller keeps the
+    memory alive."""
+    if layout not in YUV_LAYOUTS:
+        raise ValueError(f"layout {layout!r}: one of {YUV_LAYOUTS}")
+    semi = layout in ("nv12", "nv21")
+    if isinstance(frame, (tuple, list)):
+        planes = [_plane(p) for p in frame]
+        if len(planes) != (2 if semi else 3):
+            raise ValueError(f"{layout}: {'(y, uv)' if semi else '(y, u, v)'} planes expected, got {len(planes)}")
+        (y, yp, h, w, dev), rest = planes[0], planes[1:]
+        if any(p[4] != dev for p in rest):
+            raise ValueError("planes must all be host or all be device memory")
+        if semi:
+            uv, uvp = rest[0][0], rest[0][1]
+            u, v = (uv, uv + 1) if layout == "nv12" else (uv + 1, uv)
+            return YuvFrame(y, u, v, yp, uvp, 2, w, h), dev
+        if rest[0][1] != rest[1][1]:
+            raise ValueError("u and v planes must share one pitch")
+        return YuvFrame(y, rest[0][0], rest[1][0], yp, rest[0][1], 1, w, h), dev
+    p, pitch, rows, w, dev = _plane(frame)
+    contiguous = frame.is_contiguous() if hasattr(frame, "is_contiguous") else frame.flags.c_contiguous
+    if not contiguous or rows % 3 or w % 2:
+        raise ValueError(f"single-buffer 4:2:0 frame: C-contiguous (h * 3 / 2, w) with even h and w expected, got {rows}x{w}")
+    h = rows * 2 // 3
+    c = p + w * h
+    if semi:
+        u, v = (c, c + 1) if layout == "nv12" else (c + 1, c)
+        return YuvFrame(p, u, v, w, w, 2, w, h), dev
+    q = c + (w // 2) * (h // 2)
+    u, v = (c, q) if layout == "i420" else (q, c)
+    return YuvFrame(p, u, v, w, w // 2, 1, w, h), dev
+
+
+def _matrix(matrix) -> int:
+    if isinstance(matrix, str):
+        if matrix not in YUV_MATRICES:
+            raise ValueError(f"matrix {matrix!r}: one of {sorted(YUV_MATRICES)}")
+        return YUV_MATRICES[matrix]
+    return int(matrix)
 
 
 class RfError(RuntimeError):
@@ -148,6 +216,11 @@ def load_library() -> C.CDLL:
                                           C.c_float, C.c_float, C.POINTER(AlignParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.rf_detect_align_batch_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_float, C.POINTER(AlignParams), C.c_void_p,
                                                  C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
+    lib.rf_detect_yuv_batch.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_int, C.c_int, C.c_float, C.c_float, C.POINTER(AlignParams), C.c_void_p,
+                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.rf_detect_yuv_batch_device.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_int, C.c_int, C.c_float, C.c_float, C.POINTER(AlignParams),
+                                               C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_void_p]
+    lib.rf_preprocess_yuv.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_int, C.c_void_p]
     _lib = lib
     return lib
 
@@ -372,6 +445,68 @@ class Engine:
         self._check(self.lib.rf_detect_align_batch_device(self.h, dev_ptr if dev_ptr is not None else self.device_input_ptr(), n, thr, nms_thr,
                                                           C.byref(p), dev_crops_ptr, dev_mats_ptr, C.byref(d), C.byref(c)))
         return int(d.value), int(c.value)
+
+    # -- f6 video frames (YUV 4:2:0) ----------------------------------------------------------------
+    @staticmethod
+    def _frames(frames, layout: str, device: bool):
+        descs = [yuv_frame(f, layout) for f in frames]
+        if any(dev != device for _, dev in descs):
+            raise ValueError(f"{'device' if device else 'host'} frames expected")
+        return (YuvFrame * max(len(descs), 1))(*[d for d, _ in descs])
+
+    def detect_yuv(self, frames, thr: float, nms_thr: float, layout: str = "nv12", matrix="bt601", align: Optional[dict] = None,
+                   want_index: bool = False):
+        """rf_detect_yuv_batch: host 4:2:0 frames (see yuv_frame for the forms) -> faces in FRAME pixels, one (k, 15) float32 array
+        per frame.  align: detect_align's keywords (crop, template, fmt, max_faces, mean, std, want_mats) -> (faces, crops[, mats])
+        as detect_align returns them.  want_index appends the anchor-index arrays."""
+        n = len(frames)
+        arr = self._frames(frames, layout, False)
+        faces = np.empty((n, self.max_faces, FACE_FLOATS), dtype=np.float32)
+        counts = np.zeros(n, dtype=np.int32)
+        idx = np.empty((n, self.max_faces), dtype=np.int32) if want_index else None
+        p = crops = mats = None
+        if align is not None:
+            kw = dict(align)
+            want_mats = kw.pop("want_mats", False)
+            p = align_params(**{"fmt": "bgr_u8", **kw})
+            A = p.max_faces or self.max_faces
+            shape, dt = crop_shape(kw.get("fmt", "bgr_u8"), (p.crop_w, p.crop_h))
+            crops = np.empty((n, A) + shape, dtype=dt)
+            mats = np.empty((n, A, 2, 3), dtype=np.float64) if want_mats else None
+        self._check(self.lib.rf_detect_yuv_batch(self.h, arr, n, _matrix(matrix), thr, nms_thr, C.byref(p) if p is not None else None,
+                                                 faces.ctypes.data, counts.ctypes.data, idx.ctypes.data if want_index else None,
+                                                 crops.ctypes.data if crops is not None else None, mats.ctypes.data if mats is not None else None))
+        out = [faces[i, :counts[i]].copy() for i in range(n)]
+        if align is not None:
+            out = (out, [crops[i, :min(counts[i], A)].copy() for i in range(n)])
+            if mats is not None:
+                out += ([mats[i, :min(counts[i], A)].copy() for i in range(n)],)
+        else:
+            out = (out,)
+        if want_index:
+            out += ([idx[i, :counts[i]].copy() for i in range(n)],)
+        return out[0] if len(out) == 1 else out
+
+    def detect_yuv_device(self, frames, thr: float, nms_thr: float, layout: str = "nv12", matrix="bt601", align: Optional[dict] = None,
+                          dev_crops_ptr: Optional[int] = None, dev_mats_ptr: Optional[int] = None):
+        """rf_detect_yuv_batch_device: device 4:2:0 frames (torch CUDA tensors in yuv_frame's forms), asynchronous on
+        last_stream_ptr().  Returns (dets_ptr, counts_ptr, map-back scale of each frame); detections in network-input pixels.
+        align: detect_align's keywords; the crops land at dev_crops_ptr as in detect_align_device."""
+        n = len(frames)
+        arr = self._frames(frames, layout, True)
+        p = align_params(**align) if align is not None else None
+        scales = np.zeros(max(n, 1), dtype=np.float32)
+        d, c = C.c_void_p(), C.c_void_p()
+        self._check(self.lib.rf_detect_yuv_batch_device(self.h, arr, n, _matrix(matrix), thr, nms_thr, C.byref(p) if p is not None else None,
+                                                        dev_crops_ptr, dev_mats_ptr, C.byref(d), C.byref(c), scales.ctypes.data))
+        return int(d.value), int(c.value), scales[:n].copy()
+
+    def preprocess_yuv(self, frame, layout: str = "nv12", matrix="bt601") -> np.ndarray:
+        """rf_preprocess_yuv: one host frame letter-boxed into the (H, W, 3) u8 BGR network input."""
+        arr = self._frames([frame], layout, False)
+        out = np.empty((self.net_h, self.net_w, 3), dtype=np.uint8)
+        self._check(self.lib.rf_preprocess_yuv(self.h, arr, _matrix(matrix), out.ctypes.data))
+        return out
 
     def detect_jpeg(self, streams: Sequence[bytes], thr: float, nms_thr: float):
         """JPEG bitstreams (bytes) -> decoded on the GPU (nvJPEG), letter-boxed, detected.  Returns (list of (k,15) arrays in

@@ -58,7 +58,14 @@ __device__ void invert_affine(const double m[6], double im[6]) {
 
 // One output pixel of cv::warpAffine INTER_LINEAR / BORDER_CONSTANT 0 on 8UC3: X, Y in 1/32 source pixel (X0 + adelta >> 5),
 // integer weights 32 (32 - fx) (32 - fy) ... summing to 32768, taps outside the image contribute 0, (sum + 16384) >> 15.
-__device__ __forceinline__ void sample(const AlignImage &im, int X, int Y, int v[3]) {
+__device__ __forceinline__ void tap(const AlignImage &im, int x, int y, int p[3]) {
+    const uint8_t *q = im.src + (size_t)y * im.row_bytes + (size_t)x * 3;
+    p[0] = q[0]; p[1] = q[1]; p[2] = q[2];
+}
+__device__ __forceinline__ void tap(const AlignYuvImage &im, int x, int y, int p[3]) { yuv_pixel(im.p, x, y, p); }
+
+template <typename Img>
+__device__ __forceinline__ void sample(const Img &im, int X, int Y, int v[3]) {
     const int sx = min(max(X >> 5, -32768), 32767), sy = min(max(Y >> 5, -32768), 32767);   // saturate_cast<short>
     const int fx = X & 31, fy = Y & 31;
     const int wts[4] = {32 * (32 - fx) * (32 - fy), 32 * fx * (32 - fy), 32 * (32 - fx) * fy, 32 * fx * fy};
@@ -67,12 +74,30 @@ __device__ __forceinline__ void sample(const AlignImage &im, int X, int Y, int v
     for (int t = 0; t < 4; t++) {
         const int tx = sx + (t & 1), ty = sy + (t >> 1);
         if ((unsigned)tx < (unsigned)im.w && (unsigned)ty < (unsigned)im.h) {
-            const uint8_t *p = im.src + (size_t)ty * im.row_bytes + (size_t)tx * 3;
+            int p[3];
+            tap(im, tx, ty, p);
             acc[0] += wts[t] * p[0]; acc[1] += wts[t] * p[1]; acc[2] += wts[t] * p[2];
         }
     }
     v[0] = acc[0] >> 15; v[1] = acc[1] >> 15; v[2] = acc[2] >> 15;
 }
+
+// Where the kernel finds image i: the BGR table / uniform net-sized images of AlignArgs, or the frame table parameter.
+struct BgrImages {};
+struct YuvFrames { AlignYuvImage img[ALIGN_MAX_FRAMES]; };
+static_assert(sizeof(AlignArgs) + sizeof(YuvFrames) + 32 <= 4096, "align launch exceeds the classic 4 KB kernel parameter space");
+
+__device__ __forceinline__ AlignImage image_of(const AlignArgs &a, const BgrImages &, int i) {
+    AlignImage im;
+    if (a.images) {
+        im = a.images[i];
+    } else {
+        im.src = a.uniform_base + (size_t)i * a.uniform_bytes;
+        im.w = a.uniform_w; im.h = a.uniform_h; im.row_bytes = a.uniform_w * 3; im.scale = 1.f;
+    }
+    return im;
+}
+__device__ __forceinline__ AlignYuvImage image_of(const AlignArgs &, const YuvFrames &f, int i) { return f.img[i]; }
 
 // Four consecutive pixels of one crop row (x4 .. x4 + 3, those < cw valid).  Vector stores where the address allows.
 __device__ __forceinline__ void store_quad(const AlignArgs &a, unsigned char *crop, int y, int x4, const int v[4][3]) {
@@ -118,7 +143,8 @@ __device__ __forceinline__ void store_quad(const AlignArgs &a, unsigned char *cr
 // consecutive work items -- so that free slots cost nothing however large max_align is.  Per item, thread 0 fits the
 // transform in FP64, the CTA tabulates OpenCV's per-column (adelta, bdelta) and the band's per-row (X0, Y0) fixed-point
 // terms in shared memory, and every pixel costs integer arithmetic only.
-__global__ void __launch_bounds__(ALIGN_THREADS) k_align_faces(const AlignArgs a, const rf_det *__restrict__ dets,
+template <typename Src>
+__global__ void __launch_bounds__(ALIGN_THREADS) k_align_faces(const AlignArgs a, const __grid_constant__ Src src, const rf_det *__restrict__ dets,
                                                              const int *__restrict__ counts, int max_faces) {
     extern __shared__ int s_first[];     // [n]: crop ordinal of image i's first crop
     __shared__ int s_ax[ALIGN_MAX_SIDE], s_bx[ALIGN_MAX_SIDE], s_x0[ALIGN_BAND], s_y0[ALIGN_BAND];
@@ -165,13 +191,7 @@ __global__ void __launch_bounds__(ALIGN_THREADS) k_align_faces(const AlignArgs a
             if (s_first[mid] <= c) i = mid; else top = mid - 1;
         }
         const int j = c - s_first[i], slot = i * a.max_align + j;
-        AlignImage im;
-        if (a.images) {
-            im = a.images[i];
-        } else {
-            im.src = a.uniform_base + (size_t)i * a.uniform_bytes;
-            im.w = a.uniform_w; im.h = a.uniform_h; im.row_bytes = a.uniform_w * 3; im.scale = 1.f;
-        }
+        const auto im = image_of(a, src, i);
         if (threadIdx.x == 0) {
             double M[6], iM[6];
             s_zero = fit_similarity(dets[(size_t)i * max_faces + j].face, im.scale, a.tmpl, M) ? 0 : 1;
@@ -216,8 +236,27 @@ cudaError_t launch_align_faces(const AlignArgs &a, const PostBuffers &pb, int nu
     if (a.n <= 0 || a.max_align <= 0) return cudaSuccess;
     // two small CTAs per SM: the crops of a batch-8 step (about 40 faces x 14 bands) in one or two items per CTA, without
     // taking more than a quarter of any SM's registers from the forward kernels of other contexts running alongside
-    k_align_faces<<<2 * num_sms, ALIGN_THREADS, sizeof(int) * a.n, s>>>(a, pb.out_dets, pb.out_counts, pb.max_faces);
+    k_align_faces<<<2 * num_sms, ALIGN_THREADS, sizeof(int) * a.n, s>>>(a, BgrImages{}, pb.out_dets, pb.out_counts, pb.max_faces);
     return cudaGetLastError();
+}
+
+cudaError_t launch_align_faces_yuv(const AlignArgs &a, const AlignYuvImage *frames, const PostBuffers &pb, int num_sms, cudaStream_t s) {
+    if (a.n <= 0 || a.max_align <= 0) return cudaSuccess;
+    // chunk i0 is its own launch over frames [i0, i0 + m): the same kernel on offset records, counts, crops and matrices
+    for (int i0 = 0; i0 < a.n; i0 += ALIGN_MAX_FRAMES) {
+        const int m = std::min(ALIGN_MAX_FRAMES, a.n - i0);
+        AlignArgs c = a;
+        c.n = m;
+        c.crops = static_cast<unsigned char *>(a.crops) + (size_t)i0 * a.max_align * a.crop_bytes;
+        if (a.mats) c.mats = a.mats + (size_t)i0 * a.max_align * 6;
+        YuvFrames f{};
+        for (int i = 0; i < m; i++) f.img[i] = frames[i0 + i];
+        k_align_faces<<<2 * num_sms, ALIGN_THREADS, sizeof(int) * m, s>>>(c, f, pb.out_dets + (size_t)i0 * pb.max_faces, pb.out_counts + i0,
+                                                                        pb.max_faces);
+        cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
 }
 
 }  // namespace rf

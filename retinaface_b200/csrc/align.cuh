@@ -8,6 +8,7 @@
 #pragma once
 #include "common.cuh"
 #include "postproc.cuh"
+#include "yuv.cuh"
 
 namespace rf {
 
@@ -33,11 +34,22 @@ struct AlignArgs {
     double *mats;               // optional [n][max_align][6]: M, image -> crop
 };
 
-constexpr int ALIGN_MIN_SIDE = 8, ALIGN_MAX_SIDE = 512;
+// f6: one YUV 4:2:0 video frame of the batch (yuv.cuh), read in place; a.images / a.uniform_* are unused.  Each tap of the warp
+// is converted to BGR first, so a crop is cv2.warpAffine(cv2.cvtColor(frame), M) byte for byte.
+struct AlignYuvImage {
+    YuvPlanes p;
+    int w, h;
+    float scale;
+};
+
+constexpr int ALIGN_MIN_SIDE = 8, ALIGN_MAX_SIDE = 512, ALIGN_MAX_FRAMES = 32;
 
 size_t align_crop_bytes(int crop_w, int crop_h, int format);
 // One launch, the grid sized from the SM count: kept counts and landmarks are read from pb on the device, and only the crops
 // that exist are cut.  n <= max_batch (<= 4096: the per-image scan lives in 4 n bytes of shared memory).
 cudaError_t launch_align_faces(const AlignArgs &a, const PostBuffers &pb, int num_sms, cudaStream_t s);
+// The same over a.n YUV frames [n]: the frame table travels as a kernel parameter (no host table a later call could rewrite
+// before the copy ran), one launch per ALIGN_MAX_FRAMES frames.
+cudaError_t launch_align_faces_yuv(const AlignArgs &a, const AlignYuvImage *frames, const PostBuffers &pb, int num_sms, cudaStream_t s);
 
 }  // namespace rf

@@ -163,7 +163,7 @@ void release_ctx(Ctx &c, bool all) {
     cudaFree(c.arena);
     c.arena = nullptr;
     if (!all) return;
-    cudaFree(c.d_params); cudaFreeHost(c.h_params);
+    cudaFree(c.d_params); cudaFreeHost(c.h_params); cudaFree(c.d_frames_in);
     free_post_buffers(c.pb);
     for (auto e : c.step_event) if (e) cudaEventDestroy(e);
     for (int l = 1; l < 3; l++) if (c.lane_stream[l]) cudaStreamDestroy(c.lane_stream[l]);
@@ -468,9 +468,10 @@ int rf_launches_per_batch(rf_handle h, int n) {
     return h ? (int)h->steps.size() : RF_ERR_INVALID_ARG;
 }
 
-// `ran_on` (optional) receives the context the forward was issued on.
+// `ran_on` (optional) receives the context the forward was issued on.  `stage` (optional) issues work on that context's stream
+// ahead of the forward and returns the input tensor the forward reads instead of dev_bgr.
 static int detect_device_impl(rf_handle h, const uint8_t *dev_bgr, int n, float thr, float nms, const rf_det **dev_dets, const int32_t **dev_counts,
-                              bool gather, Ctx **ran_on = nullptr) {
+                              bool gather, Ctx **ran_on = nullptr, const std::function<const uint8_t *(Ctx &)> &stage = nullptr) {
     int rc = check_n(h, n);
     if (rc) return rc;
     if (gather && (!h->comm.ready || n == 0)) return fail(h, RF_ERR_INVALID_ARG, "rf_detect_batch_device_allgather: call rf_comm_init first (and n > 0)");
@@ -481,6 +482,7 @@ static int detect_device_impl(rf_handle h, const uint8_t *dev_bgr, int n, float 
         h->last_stream = c.stream;
         // the caller's device images are read in place (conv0 takes the pointer from the run parameters)
         if (c.param_seq && c.param_seq % Ctx::kParamSlots == 0) CK(cudaStreamSynchronize(c.stream));
+        if (stage) dev_bgr = stage(c);
         const unsigned seq = gather ? ++h->comm.seq : 0u;
         set_params(h, c, thr, nms, dev_bgr, seq);
         if (n > 0) forward_graph(h, c, n);
@@ -563,19 +565,25 @@ struct H2DRuns {
 // two pinned buffers: a row-band parallel host copy (host_copy.h) into one buffer overlaps the DMA out of the other; the
 // only host wait is for the DMA that last read the buffer about to be overwritten.  In both cases the stream orders the
 // copy into d_raw behind the letter-box kernel that still reads the previous image.
-static uint8_t *upload_raw(rf_handle h, cudaStream_t s, const uint8_t *src, int width, int height, int row_stride, int raw_slot = 0) {
-    uint8_t *d_dst = h->d_raw + (size_t)raw_slot * h->raw_bytes;
+// One host plane of `rows` rows of row_bytes (pitch bytes apart) -> d_dst, packed, on `s`: pinned sources straight, pageable
+// ones through the two pinned staging buffers (each plane fits one: it is at most a max_image BGR image).
+static void upload_plane(rf_handle h, cudaStream_t s, uint8_t *d_dst, const uint8_t *src, size_t row_bytes, size_t pitch, int rows) {
     if (is_pinned(src)) {
-        CK(cudaMemcpy2DAsync(d_dst, (size_t)width * 3, src, (size_t)row_stride, (size_t)width * 3, (size_t)height, cudaMemcpyHostToDevice, s));
-        return d_dst;
+        CK(cudaMemcpy2DAsync(d_dst, row_bytes, src, pitch, row_bytes, (size_t)rows, cudaMemcpyHostToDevice, s));
+        return;
     }
     if (!h->copy_pool) h->copy_pool.reset(new HostCopyPool((int)std::min(3u, std::max(1u, std::thread::hardware_concurrency()) - 1u)));
     const int slot = (int)(h->raw_seq++ & 1u);
     uint8_t *buf = h->h_raw + (size_t)slot * h->raw_bytes;
     CK(cudaEventSynchronize(h->raw_ev[slot]));      // (returns at once for an event never recorded)
-    h->copy_pool->copy_rows(buf, src, (size_t)width * 3, (size_t)row_stride, height);
-    CK(cudaMemcpyAsync(d_dst, buf, (size_t)width * height * 3, cudaMemcpyHostToDevice, s));
+    h->copy_pool->copy_rows(buf, src, row_bytes, pitch, rows);
+    CK(cudaMemcpyAsync(d_dst, buf, row_bytes * rows, cudaMemcpyHostToDevice, s));
     CK(cudaEventRecord(h->raw_ev[slot], s));
+}
+
+static uint8_t *upload_raw(rf_handle h, cudaStream_t s, const uint8_t *src, int width, int height, int row_stride, int raw_slot = 0) {
+    uint8_t *d_dst = h->d_raw + (size_t)raw_slot * h->raw_bytes;
+    upload_plane(h, s, d_dst, src, (size_t)width * 3, (size_t)row_stride, height);
     return d_dst;
 }
 
@@ -678,6 +686,51 @@ static int align_setup(rf_handle h, const char *who, const rf_align_params *p, A
     return RF_OK;
 }
 
+// Makes room for n images' crops and the matrices of the blocking align paths (context 0).
+static void ensure_align_buffers(rf_handle h, int n, const AlignArgs &a) {
+    if (!h->d_align_images) {
+        CK(cudaMalloc(&h->d_align_images, sizeof(AlignImage) * h->cfg.max_batch));
+        CK(cudaHostAlloc(&h->h_align_images, sizeof(AlignImage) * h->cfg.max_batch, cudaHostAllocDefault));
+        CK(cudaMalloc(&h->d_align_mats, sizeof(double) * 6 * h->cfg.max_batch * h->cfg.max_faces));
+    }
+    const size_t need = (size_t)n * a.max_align * a.crop_bytes;
+    if (need > h->align_crops_bytes) {
+        CK(cudaFree(h->d_align_crops));
+        h->d_align_crops = nullptr;
+        h->align_crops_bytes = 0;
+        CK(cudaMalloc(&h->d_align_crops, need));
+        h->align_crops_bytes = need;
+    }
+}
+
+// After fetch_results on context c: the kept faces of image i (h_dets) mapped back by scale(i), network-input pixels -> image
+// pixels (k_merge_views' map-back), into out_faces; with `a`, the crops (and matrices) of its first min(count, A) faces copied
+// out of the align buffers.  Blocking.
+extern "C++" {
+template <typename ScaleOf>
+static void put_mapped(rf_handle h, Ctx &c, int n, ScaleOf scale, const AlignArgs *a, rf_face *out_faces, void *out_crops, double *out_mats) {
+    const int mf = h->cfg.max_faces;
+    for (int i = 0; i < n; i++) {
+        const int k = h->h_counts[i];
+        const float s = scale(i);
+        for (int j = 0; out_faces && j < k; j++) {
+            rf_face f = h->h_dets[(size_t)i * mf + j].face;
+            f.x1 *= s; f.y1 *= s; f.x2 *= s; f.y2 *= s;
+            for (int l = 0; l < 5; l++) { f.lx[l] *= s; f.ly[l] *= s; }
+            out_faces[(size_t)i * mf + j] = f;
+        }
+        if (!a) continue;
+        const size_t first = (size_t)i * a->max_align, m = (size_t)std::min(k, a->max_align);
+        if (!m) continue;
+        CK(cudaMemcpyAsync(static_cast<uint8_t *>(out_crops) + first * a->crop_bytes, static_cast<uint8_t *>(h->d_align_crops) + first * a->crop_bytes,
+                           m * a->crop_bytes, cudaMemcpyDeviceToHost, c.stream));
+        if (out_mats)
+            CK(cudaMemcpyAsync(out_mats + first * 6, h->d_align_mats + first * 6, m * 6 * sizeof(double), cudaMemcpyDeviceToHost, c.stream));
+    }
+    CK(cudaStreamSynchronize(c.stream));
+}
+}  // extern "C++"
+
 int rf_detect_align_batch(rf_handle h, const uint8_t *const *imgs, const int *widths, const int *heights, const int *row_strides,
                           int n, float thr, float nms, const rf_align_params *params, rf_face *out_faces, int *out_counts,
                           void *out_crops, double *out_mats) {
@@ -687,7 +740,7 @@ int rf_detect_align_batch(rf_handle h, const uint8_t *const *imgs, const int *wi
     if ((rc = align_setup(h, "rf_detect_align_batch", params, a))) return rc;
     if (n == 0) return RF_OK;
     if (!imgs || !widths || !heights || !out_crops) return fail(h, RF_ERR_INVALID_ARG, "rf_detect_align_batch: NULL image arrays or out_crops");
-    const int Hn = h->cfg.net_h, Wn = h->cfg.net_w, mf = h->cfg.max_faces;
+    const int Hn = h->cfg.net_h, Wn = h->cfg.net_w;
     // the kernel samples every original after the forward: no raw buffer may be recycled within the call
     int raw = 0;
     for (int i = 0; i < n; i++) {
@@ -701,19 +754,7 @@ int rf_detect_align_batch(rf_handle h, const uint8_t *const *imgs, const int *wi
     try {
         CK(cudaSetDevice(h->device));
         Ctx &c = h->ctx[0];
-        if (!h->d_align_images) {
-            CK(cudaMalloc(&h->d_align_images, sizeof(AlignImage) * h->cfg.max_batch));
-            CK(cudaHostAlloc(&h->h_align_images, sizeof(AlignImage) * h->cfg.max_batch, cudaHostAllocDefault));
-            CK(cudaMalloc(&h->d_align_mats, sizeof(double) * 6 * h->cfg.max_batch * mf));
-        }
-        const size_t need = (size_t)n * a.max_align * a.crop_bytes;
-        if (need > h->align_crops_bytes) {
-            CK(cudaFree(h->d_align_crops));
-            h->d_align_crops = nullptr;
-            h->align_crops_bytes = 0;
-            CK(cudaMalloc(&h->d_align_crops, need));
-            h->align_crops_bytes = need;
-        }
+        ensure_align_buffers(h, n, a);
         if ((rc = stage_images(h, c.stream, "rf_detect_align_batch", imgs, widths, heights, row_strides, n, h->h_align_images))) return rc;
         CK(cudaMemcpyAsync(h->d_align_images, h->h_align_images, sizeof(AlignImage) * n, cudaMemcpyHostToDevice, c.stream));
         set_params(h, c, thr, nms);
@@ -724,23 +765,7 @@ int rf_detect_align_batch(rf_handle h, const uint8_t *const *imgs, const int *wi
         a.mats = out_mats ? h->d_align_mats : nullptr;
         CK(launch_align_faces(a, c.pb, h->num_sms, c.stream));
         fetch_results(h, c, n, nullptr, out_counts, nullptr);
-        for (int i = 0; i < n; i++) {
-            const int k = h->h_counts[i];
-            const float s = h->h_align_images[i].scale;
-            for (int j = 0; out_faces && j < k; j++) {
-                rf_face f = h->h_dets[(size_t)i * mf + j].face;      // network-input pixels -> image pixels (k_merge_views' map-back)
-                f.x1 *= s; f.y1 *= s; f.x2 *= s; f.y2 *= s;
-                for (int l = 0; l < 5; l++) { f.lx[l] *= s; f.ly[l] *= s; }
-                out_faces[(size_t)i * mf + j] = f;
-            }
-            const size_t first = (size_t)i * a.max_align, m = (size_t)std::min(k, a.max_align);
-            if (!m) continue;
-            CK(cudaMemcpyAsync(static_cast<uint8_t *>(out_crops) + first * a.crop_bytes, static_cast<uint8_t *>(h->d_align_crops) + first * a.crop_bytes,
-                               m * a.crop_bytes, cudaMemcpyDeviceToHost, c.stream));
-            if (out_mats)
-                CK(cudaMemcpyAsync(out_mats + first * 6, h->d_align_mats + first * 6, m * 6 * sizeof(double), cudaMemcpyDeviceToHost, c.stream));
-        }
-        CK(cudaStreamSynchronize(c.stream));
+        put_mapped(h, c, n, [&](int i) { return h->h_align_images[i].scale; }, &a, out_faces, out_crops, out_mats);
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }
@@ -764,6 +789,158 @@ int rf_detect_align_batch_device(rf_handle h, const uint8_t *dev_bgr, int n, flo
     a.mats = dev_mats;
     try {
         CK(launch_align_faces(a, c->pb, h->num_sms, c->stream));
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
+}
+
+// ---- f6 video frames: YUV 4:2:0 (yuv.cuh) ---------------------------------------------------------------------------------------
+// Checks n, the matrix and every frame descriptor; nothing is launched before this passes.
+static int check_frames(rf_handle h, const char *who, const rf_yuv_frame *frames, int n, int matrix) {
+    int rc = check_n(h, n);
+    if (rc) return rc;
+    if (n > 0 && !frames) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frames is NULL", who));
+    if (matrix != RF_YUV_BT601 && matrix != RF_YUV_BT709) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: unknown matrix %d", who, matrix));
+    for (int i = 0; i < n; i++) {
+        const rf_yuv_frame &f = frames[i];
+        if (f.width <= 0 || f.height <= 0 || (f.width & 1) || (f.height & 1))
+            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frame %d is %dx%d; 4:2:0 sizes must be positive and even", who, i, f.width, f.height));
+        if (!f.y || !f.u || !f.v) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frame %d has a NULL plane", who, i));
+        if (f.uv_step != 1 && f.uv_step != 2) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frame %d: uv_step %d, must be 1 or 2", who, i, f.uv_step));
+        const uintptr_t u = (uintptr_t)f.u, v = (uintptr_t)f.v;
+        if (f.uv_step == 2 && u != v + 1 && v != u + 1)
+            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frame %d: semi-planar u and v must be adjacent bytes of one plane", who, i));
+        if (f.y_pitch < f.width || f.uv_pitch < f.width / 2 * f.uv_step)
+            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frame %d: pitches %d / %d below the row bytes %d / %d", who, i, f.y_pitch, f.uv_pitch, f.width,
+                                                   f.width / 2 * f.uv_step));
+        if (f.width > h->cfg.max_image_w || f.height > h->cfg.max_image_h)
+            return fail(h, RF_ERR_CAPACITY, fmt("%s: frame %d is %dx%d, larger than max_image %dx%d", who, i, f.width, f.height, h->cfg.max_image_w,
+                                                h->cfg.max_image_h));
+    }
+    return RF_OK;
+}
+
+static YuvPlanes planes_of(const rf_yuv_frame &f, int matrix) { return YuvPlanes{f.y, f.u, f.v, f.y_pitch, f.uv_pitch, f.uv_step, matrix}; }
+
+// One host frame -> raw buffer `raw_slot` on `s`, 1.5 bytes per pixel: the luma packed, then the chroma as the frame lays it out
+// (one interleaved w x h/2 plane, or two w/2 x h/2 planes).  Returns the device planes.
+static YuvPlanes upload_frame(rf_handle h, cudaStream_t s, const rf_yuv_frame &f, int matrix, int raw_slot) {
+    uint8_t *d = h->d_raw + (size_t)raw_slot * h->raw_bytes, *dc = d + (size_t)f.width * f.height;
+    const int cw = f.width / 2, ch = f.height / 2;
+    upload_plane(h, s, d, f.y, f.width, f.y_pitch, f.height);
+    YuvPlanes p{d, dc, dc, f.width, f.width, f.uv_step, matrix};
+    if (f.uv_step == 2) {
+        const uint8_t *first = std::min(f.u, f.v);
+        upload_plane(h, s, dc, first, f.width, f.uv_pitch, ch);
+        p.u = dc + (f.u - first);
+        p.v = dc + (f.v - first);
+    } else {
+        upload_plane(h, s, dc, f.u, cw, f.uv_pitch, ch);
+        upload_plane(h, s, dc + (size_t)cw * ch, f.v, cw, f.uv_pitch, ch);
+        p.v = dc + (size_t)cw * ch;
+        p.uv_pitch = cw;
+    }
+    return p;
+}
+
+int rf_detect_yuv_batch(rf_handle h, const rf_yuv_frame *frames, int n, int matrix, float thr, float nms, const rf_align_params *align,
+                        rf_face *out_faces, int *out_counts, int32_t *out_idx, void *out_crops, double *out_mats) {
+    static const char *who = "rf_detect_yuv_batch";
+    int rc = check_frames(h, who, frames, n, matrix);
+    if (rc) return rc;
+    AlignArgs a;
+    if (align && (rc = align_setup(h, who, align, a))) return rc;
+    if (n == 0) return RF_OK;
+    if (align && !out_crops) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: align without out_crops", who));
+    // the crops are cut from the frames after the forward: each needs a raw buffer of its own for the whole call
+    if (align && n > h->raw_slots)
+        return fail(h, RF_ERR_CAPACITY, fmt("%s: %d frames to align, but the handle keeps at most %d resident (one %dx%d raw buffer each); split the batch",
+                                            who, n, h->raw_slots, h->cfg.max_image_w, h->cfg.max_image_h));
+    const int Hn = h->cfg.net_h, Wn = h->cfg.net_w;
+    const size_t img_bytes = (size_t)Hn * Wn * 3;
+    const int area = (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0;
+    try {
+        CK(cudaSetDevice(h->device));
+        Ctx &c = h->ctx[0];
+        if (align) ensure_align_buffers(h, n, a);
+        std::vector<LbYuvItem> lb;
+        std::vector<AlignYuvImage> orig(n);
+        for (int i = 0; i < n; i++) {
+            // a full chunk of raw buffers is letter-boxed before the next frame reuses the first (stream order)
+            if ((int)lb.size() == h->raw_slots) { CK(launch_letterbox_batch(lb.data(), (int)lb.size(), Wn, Hn, c.stream)); lb.clear(); }
+            const rf_yuv_frame &f = frames[i];
+            const YuvPlanes p = upload_frame(h, c.stream, f, matrix, (int)lb.size());
+            lb.emplace_back();
+            orig[i] = AlignYuvImage{p, f.width, f.height, letterbox_fill(lb.back(), p, f.width, f.height, h->d_input + i * img_bytes, Wn, Hn, 0, area)};
+        }
+        CK(launch_letterbox_batch(lb.data(), (int)lb.size(), Wn, Hn, c.stream));
+        set_params(h, c, thr, nms);
+        forward_graph(h, c, n);
+        if (align) {
+            a.n = n;
+            a.crops = h->d_align_crops;
+            a.mats = out_mats ? h->d_align_mats : nullptr;
+            CK(launch_align_faces_yuv(a, orig.data(), c.pb, h->num_sms, c.stream));
+        }
+        fetch_results(h, c, n, nullptr, out_counts, out_idx);
+        put_mapped(h, c, n, [&](int i) { return orig[i].scale; }, align ? &a : nullptr, out_faces, out_crops, out_mats);
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
+}
+
+int rf_detect_yuv_batch_device(rf_handle h, const rf_yuv_frame *frames, int n, int matrix, float thr, float nms, const rf_align_params *align,
+                               void *dev_crops, double *dev_mats, const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales) {
+    static const char *who = "rf_detect_yuv_batch_device";
+    int rc = check_frames(h, who, frames, n, matrix);
+    if (rc) return rc;
+    AlignArgs a;
+    if (align && (rc = align_setup(h, who, align, a))) return rc;
+    if (align && n > 0 && !dev_crops) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: align without dev_crops", who));
+    const int Hn = h->cfg.net_h, Wn = h->cfg.net_w;
+    const size_t img_bytes = (size_t)Hn * Wn * 3;
+    const int area = (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0;
+    std::vector<AlignYuvImage> orig(n);
+    // the frames are letter-boxed on the context the forward lands on, into that context's own input tensor
+    auto stage = [&](Ctx &c) -> const uint8_t * {
+        if (!c.d_frames_in) CK(cudaMalloc(&c.d_frames_in, (size_t)h->cfg.max_batch * img_bytes));
+        std::vector<LbYuvItem> lb(n);
+        for (int i = 0; i < n; i++) {
+            const rf_yuv_frame &f = frames[i];
+            const YuvPlanes p = planes_of(f, matrix);
+            orig[i] = AlignYuvImage{p, f.width, f.height, letterbox_fill(lb[i], p, f.width, f.height, c.d_frames_in + i * img_bytes, Wn, Hn, 0, area)};
+            if (out_scales) out_scales[i] = orig[i].scale;
+        }
+        CK(launch_letterbox_batch(lb.data(), n, Wn, Hn, c.stream));
+        return c.d_frames_in;
+    };
+    Ctx *c = nullptr;
+    if ((rc = detect_device_impl(h, nullptr, n, thr, nms, dev_dets, dev_counts, false, &c, stage))) return rc;
+    if (n == 0 || !align) return RF_OK;
+    a.n = n;
+    a.crops = dev_crops;
+    a.mats = dev_mats;
+    try {
+        CK(launch_align_faces_yuv(a, orig.data(), c->pb, h->num_sms, c->stream));
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
+}
+
+int rf_preprocess_yuv(rf_handle h, const rf_yuv_frame *frame, int matrix, uint8_t *out) {
+    static const char *who = "rf_preprocess_yuv";
+    if (!h) return RF_ERR_INVALID_ARG;
+    if (!frame || !out) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL frame or output", who));
+    int rc = check_frames(h, who, frame, 1, matrix);
+    if (rc) return rc;
+    const int Hn = h->cfg.net_h, Wn = h->cfg.net_w;
+    try {
+        CK(cudaSetDevice(h->device));
+        cudaStream_t s = h->ctx[0].stream;
+        const YuvPlanes p = upload_frame(h, s, *frame, matrix, 0);
+        LbYuvItem it;
+        letterbox_fill(it, p, frame->width, frame->height, h->d_input, Wn, Hn, 0, (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0);
+        CK(launch_letterbox_batch(&it, 1, Wn, Hn, s));
+        CK(cudaMemcpyAsync(h->h_input, h->d_input, (size_t)Hn * Wn * 3, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        memcpy(out, h->h_input, (size_t)Hn * Wn * 3);
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }

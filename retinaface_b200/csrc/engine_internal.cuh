@@ -76,6 +76,9 @@ struct Ctx {
     float cur_thr = 0.5f, cur_nms = 0.4f;
     std::map<int, cudaGraphExec_t> graphs;
     cudaEvent_t fence = nullptr;
+    // rf_detect_yuv_batch_device (lazily allocated): this context's letter-boxed frames [max_batch][H][W][3].  One tensor per
+    // context: the letter-box of a call on another context must not overwrite the input of a forward still running here.
+    uint8_t *d_frames_in = nullptr;
 };
 
 // What one step launch writes into and where it is issued.

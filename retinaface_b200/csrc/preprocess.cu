@@ -1,5 +1,6 @@
 // preprocess.cu -- see preprocess.cuh.
 #include <cmath>
+#include <type_traits>
 
 #include "preprocess.cuh"
 
@@ -47,33 +48,40 @@ __device__ __forceinline__ Tap tap_of(int d, int sn, double scale) {
     return t;
 }
 
-// One launch letter-boxes up to LB_MAX_IMAGES images: blockIdx.z = image, blockIdx.y = output row, a thread = 4 consecutive
-// output pixels = 12 bytes = three aligned 32-bit stores (net_w is a multiple of 32, so rows start 4-byte aligned).
-struct LbImage {
-    const uint8_t *src;      // packed rows, w x h x 3 u8 BGR
-    uint8_t *dst;            // net_h x net_w x 3
-    int sw, sh, dw, dh;      // source size, size of the resized image inside the output (top-left), rest = 0
-    double scale;            // source pixels per output pixel
-    int identity, flip, area;
-};
-struct LbBatch { LbImage img[LB_MAX_IMAGES]; };
+// One launch letter-boxes up to LB_MAX_IMAGES images (LB_MAX_FRAMES frames): blockIdx.z = image, blockIdx.y = output row, a
+// thread = 4 consecutive output pixels = 12 bytes = three aligned 32-bit stores (net_w is a multiple of 32, so rows start 4-byte
+// aligned).  Per image (LbItemT): the source, dst = net_h x net_w x 3, the source size, the size of the resized image inside
+// the output (top-left, the rest is 0), the source pixels per output pixel.
+template <typename Src> constexpr int lb_limit() { return std::is_same<Src, YuvPlanes>::value ? LB_MAX_FRAMES : LB_MAX_IMAGES; }
+template <typename Src>
+struct LbBatch { LbItemT<Src> img[lb_limit<Src>()]; };
+static_assert(sizeof(LbBatch<const uint8_t *>) + 8 <= 4096 && sizeof(LbBatch<YuvPlanes>) + 8 <= 4096,
+              "letter-box chunk exceeds the classic 4 KB kernel parameter space");
+
+// BGR of source pixel (x, y): packed u8 BGR rows, or a YUV 4:2:0 frame converted on the fly
+__device__ __forceinline__ void src_pixel(const uint8_t *src, int sw, int x, int y, int v[3]) {
+    const uint8_t *p = src + ((size_t)y * sw + x) * 3;
+    v[0] = p[0]; v[1] = p[1]; v[2] = p[2];
+}
+__device__ __forceinline__ void src_pixel(const YuvPlanes &src, int, int x, int y, int v[3]) { yuv_pixel(src, x, y, v); }
 
 // NPP's NPPI_INTER_SUPER as measured against nppiResizeSqrPixel_8u_C3R (tools/npp_dump.py, oracle/npp_oracle.cu):
 // output pixel (x, y) = the coverage-weighted mean of the source rectangle [x / f, (x + 1) / f) x [y / f, (y + 1) / f), the
 // resized extent is ceil(w f) x ceil(h f), source samples beyond the image count as ZERO (the last row / column is darker, not
 // renormalised), round half up.  Matches NPP byte for byte on 5 of 8 probe shapes and within 1 LSB on < 0.5 % of the bytes of
 // the others (NPP's own arithmetic is single precision).
-__device__ __forceinline__ void area_pixel(const LbImage &im, int x, int y, int out[3]) {
+template <typename Src>
+__device__ __forceinline__ void area_pixel(const LbItemT<Src> &im, int x, int y, int out[3]) {
     const double inv = im.scale;
     const double ax = x * inv, bx = (x + 1) * inv, ay = y * inv, by = (y + 1) * inv;
     const int x0 = (int)floor(ax), x1 = min((int)ceil(bx - 1e-12), im.sw), y0 = (int)floor(ay), y1 = min((int)ceil(by - 1e-12), im.sh);
     double acc[3] = {0.0, 0.0, 0.0};
     for (int sy = y0; sy < y1; sy++) {
         const double wy = fmin((double)(sy + 1), by) - fmax((double)sy, ay);
-        const uint8_t *row = im.src + (size_t)sy * im.sw * 3;
         for (int sx = x0; sx < x1; sx++) {
             const double w = wy * (fmin((double)(sx + 1), bx) - fmax((double)sx, ax));
-            const uint8_t *p = row + (im.flip ? im.sw - 1 - sx : sx) * 3;
+            int p[3];
+            src_pixel(im.src, im.sw, im.flip ? im.sw - 1 - sx : sx, sy, p);
             acc[0] += w * p[0]; acc[1] += w * p[1]; acc[2] += w * p[2];
         }
     }
@@ -82,21 +90,25 @@ __device__ __forceinline__ void area_pixel(const LbImage &im, int x, int y, int 
     for (int c = 0; c < 3; c++) out[c] = min(max((int)floor(acc[c] * norm + 0.5), 0), 255);
 }
 
-__device__ __forceinline__ void linear_pixel(const LbImage &im, int x, const Tap &ty, int out[3]) {
+template <typename Src>
+__device__ __forceinline__ void linear_pixel(const LbItemT<Src> &im, int x, const Tap &ty, int out[3]) {
     Tap tx = tap_of<true>(x, im.sw, im.scale);
     if (im.flip) { tx.s0 = im.sw - 1 - tx.s0; tx.s1 = im.sw - 1 - tx.s1; }
-    const uint8_t *r0 = im.src + (size_t)ty.s0 * im.sw * 3, *r1 = im.src + (size_t)ty.s1 * im.sw * 3;
+    int p00[3], p01[3], p10[3], p11[3];
+    src_pixel(im.src, im.sw, tx.s0, ty.s0, p00); src_pixel(im.src, im.sw, tx.s1, ty.s0, p01);
+    src_pixel(im.src, im.sw, tx.s0, ty.s1, p10); src_pixel(im.src, im.sw, tx.s1, ty.s1, p11);
 #pragma unroll
     for (int c = 0; c < 3; c++) {
-        int h0 = (int)r0[tx.s0 * 3 + c] * tx.a0 + (int)r0[tx.s1 * 3 + c] * tx.a1;   // HResizeLinear
-        int h1 = (int)r1[tx.s0 * 3 + c] * tx.a0 + (int)r1[tx.s1 * 3 + c] * tx.a1;
+        int h0 = p00[c] * tx.a0 + p01[c] * tx.a1;   // HResizeLinear
+        int h1 = p10[c] * tx.a0 + p11[c] * tx.a1;
         int v = (((ty.a0 * (h0 >> 4)) >> 16) + ((ty.a1 * (h1 >> 4)) >> 16) + 2) >> 2;  // VResizeLinear 8u
         out[c] = min(max(v, 0), 255);
     }
 }
 
-__global__ void __launch_bounds__(128) k_letterbox_batch(const __grid_constant__ LbBatch B, int net_w, int net_h) {
-    const LbImage &im = B.img[blockIdx.z];
+template <typename Src>
+__global__ void __launch_bounds__(128) k_letterbox_batch(const __grid_constant__ LbBatch<Src> B, int net_w, int net_h) {
+    const LbItemT<Src> &im = B.img[blockIdx.z];
     const int x4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
     const int y = blockIdx.y;
     if (x4 >= net_w) return;
@@ -112,8 +124,7 @@ __global__ void __launch_bounds__(128) k_letterbox_batch(const __grid_constant__
             // flip: the view is the letter-box of the horizontally mirrored image -- every source column index is mirrored, the
             // taps are those of the mirrored image (== cv::resize(cv::flip(img, 1)) bit for bit)
             if (im.identity) {
-                const uint8_t *p = im.src + ((size_t)y * im.sw + (im.flip ? im.sw - 1 - x : x)) * 3;
-                v[0] = p[0]; v[1] = p[1]; v[2] = p[2];
+                src_pixel(im.src, im.sw, im.flip ? im.sw - 1 - x : x, y, v);
             } else if (im.area) {
                 area_pixel(im, x, y, v);
             } else {
@@ -140,7 +151,8 @@ void letterbox_geometry_npp(int w, int h, int net_w, int net_h, int *dw, int *dh
     *scale = 1.0 / f;
 }
 
-float letterbox_fill(LbItem &it, const uint8_t *src, int w, int h, uint8_t *dst, int box_w, int box_h, int flip, int area) {
+template <typename Src>
+float letterbox_fill(LbItemT<Src> &it, typename LbItemT<Src>::Source src, int w, int h, uint8_t *dst, int box_w, int box_h, int flip, int area) {
     it.src = src; it.dst = dst; it.sw = w; it.sh = h; it.flip = flip; it.area = area;
     if (area) letterbox_geometry_npp(w, h, box_w, box_h, &it.dw, &it.dh, &it.scale);
     else letterbox_geometry(w, h, box_w, box_h, &it.dw, &it.dh, &it.scale);
@@ -152,21 +164,25 @@ float letterbox_fill(LbItem &it, const uint8_t *src, int w, int h, uint8_t *dst,
     return sc > 1.0f ? sc : 1.0f;
 }
 
-cudaError_t launch_letterbox_batch(const LbItem *items, int n, int net_w, int net_h, cudaStream_t s) {
-    for (int i0 = 0; i0 < n; i0 += LB_MAX_IMAGES) {
-        const int m = std::min(LB_MAX_IMAGES, n - i0);
-        LbBatch B{};
-        for (int i = 0; i < m; i++) {
-            const LbItem &it = items[i0 + i];
-            B.img[i] = LbImage{it.src, it.dst, it.sw, it.sh, it.dw, it.dh, it.scale, it.identity, it.flip, it.area};
-        }
+template <typename Src>
+cudaError_t launch_letterbox_batch(const LbItemT<Src> *items, int n, int net_w, int net_h, cudaStream_t s) {
+    constexpr int kMax = lb_limit<Src>();
+    for (int i0 = 0; i0 < n; i0 += kMax) {
+        const int m = std::min(kMax, n - i0);
+        LbBatch<Src> B{};
+        for (int i = 0; i < m; i++) B.img[i] = items[i0 + i];
         dim3 grid((net_w / 4 + 127) / 128, net_h, m);
-        k_letterbox_batch<<<grid, 128, 0, s>>>(B, net_w, net_h);
+        k_letterbox_batch<Src><<<grid, 128, 0, s>>>(B, net_w, net_h);
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
     }
     return cudaSuccess;
 }
+
+template float letterbox_fill<const uint8_t *>(LbItem &, const uint8_t *, int, int, uint8_t *, int, int, int, int);
+template float letterbox_fill<YuvPlanes>(LbYuvItem &, YuvPlanes, int, int, uint8_t *, int, int, int, int);
+template cudaError_t launch_letterbox_batch<const uint8_t *>(const LbItem *, int, int, int, cudaStream_t);
+template cudaError_t launch_letterbox_batch<YuvPlanes>(const LbYuvItem *, int, int, int, cudaStream_t);
 
 void launch_letterbox(const uint8_t *src, int w, int h, uint8_t *dst, int net_w, int net_h, cudaStream_t s) {
     launch_letterbox_view(src, w, h, dst, net_w, net_h, net_w, net_h, 0, s);

@@ -15,8 +15,13 @@
 // RF_FLAG_NPP_RESIZE selects the reference's OTHER branch instead (USE_NPP: imageROIResize8U3C -> nppiResizeSqrPixel_8u_C3R with
 // NPPI_INTER_SUPER): coverage-weighted super-sampling with NPP's measured edge rule (preprocess.cu area_pixel; checked against
 // NPP itself on a GPU box, oracle/npp_oracle.cu).
+//
+// The pixel source is a template parameter of the kernel: packed u8 BGR rows (every path above), or a YUV 4:2:0 video frame
+// (yuv.cuh), whose every tap -- identity, bilinear or super-sampling -- is converted to BGR before the unchanged resize
+// arithmetic, so the network input is byte for byte the letter-box of cv2.cvtColor(frame).
 #pragma once
 #include "common.cuh"
+#include "yuv.cuh"
 
 namespace rf {
 
@@ -35,17 +40,24 @@ void letterbox_geometry(int w, int h, int net_w, int net_h, int *dw, int *dh, do
 // ... and the way imageROIResize8U3C + NPP do (resizeconvertion.cu:296-310): extent ceil(w f) x ceil(h f)
 void letterbox_geometry_npp(int w, int h, int net_w, int net_h, int *dw, int *dh, double *inv_scale);
 
-// Batched letter-box: ONE launch for up to LB_MAX_IMAGES images per call chunk, each with its own source / destination buffer;
-// 4 pixels (three 32-bit stores) per thread.
-constexpr int LB_MAX_IMAGES = 64;
-struct LbItem {
-    const uint8_t *src; uint8_t *dst;
+// Batched letter-box: ONE launch for up to LB_MAX_IMAGES BGR images (LB_MAX_FRAMES YUV frames) per call chunk, each with its
+// own source / destination buffer; 4 pixels (three 32-bit stores) per thread.  The items travel as __grid_constant__ kernel
+// parameters: a chunk of either kind stays within the classic 4 KB parameter limit (static_assert in preprocess.cu).
+constexpr int LB_MAX_IMAGES = 64, LB_MAX_FRAMES = 32;
+template <typename Src>
+struct LbItemT {
+    using Source = Src;
+    Src src; uint8_t *dst;
     int sw, sh, dw, dh;
     double scale;
     int identity, flip, area;
 };
+using LbItem = LbItemT<const uint8_t *>;     // packed u8 BGR rows, w x h x 3
+using LbYuvItem = LbItemT<YuvPlanes>;        // a YUV 4:2:0 frame (flip unused: 0)
 // fills one item (geometry of either resize definition); returns the reference's map-back factor
-float letterbox_fill(LbItem &it, const uint8_t *src, int w, int h, uint8_t *dst, int box_w, int box_h, int flip, int area);
-cudaError_t launch_letterbox_batch(const LbItem *items, int n, int net_w, int net_h, cudaStream_t s);
+template <typename Src>
+float letterbox_fill(LbItemT<Src> &it, typename LbItemT<Src>::Source src, int w, int h, uint8_t *dst, int box_w, int box_h, int flip, int area);
+template <typename Src>
+cudaError_t launch_letterbox_batch(const LbItemT<Src> *items, int n, int net_w, int net_h, cudaStream_t s);
 
 }  // namespace rf

@@ -60,6 +60,17 @@ class RetinaFace:
         faces, crops = self.engine.detect_align(list(imgs), threshold, self.nms_threshold, **align)
         return [[(FaceDetectInfo.from_row(r), c) for r, c in zip(f, cs)] for f, cs in zip(faces, crops)]
 
+    def detectFrames(self, frames: Sequence, threshold: float = 0.5, layout: str = "nv12", matrix: str = "bt601", align: dict = None):
+        """f6 video frames: 8-bit YUV 4:2:0 host frames (OpenCV's single-buffer ``(h * 3 / 2, w)`` u8 arrays in ``layout`` nv12 |
+        nv21 | i420 | yv12, or plane tuples; ``matrix`` bt601 (== cv2.COLOR_YUV2BGR_*) | bt709), converted to BGR inside the
+        letter-box on the GPU.  Per frame, the faces in FRAME pixels; with ``align`` (``Engine.detect_align``'s keywords), a list
+        of ``(FaceDetectInfo, crop)`` as ``detectAndAlign`` returns."""
+        out = self.engine.detect_yuv(list(frames), threshold, self.nms_threshold, layout=layout, matrix=matrix, align=align)
+        if align is None:
+            return [[FaceDetectInfo.from_row(r) for r in per] for per in out]
+        faces, crops = out[0], out[1]
+        return [[(FaceDetectInfo.from_row(r), c) for r, c in zip(f, cs)] for f, cs in zip(faces, crops)]
+
     def detectInImage(self, img: np.ndarray, threshold: float = 0.5, scales: Sequence[float] = (1.0,), flip: bool = False
                       ) -> List[FaceDetectInfo]:
         """SURVEY.md 8f-2: what the reference leaves commented out / unused (RetinaFace.cpp:730-746, the `scales` argument of

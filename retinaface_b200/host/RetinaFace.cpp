@@ -97,19 +97,27 @@ void RetinaFace::detectBatchImages(vector<cv::Mat> imgs, float threshold) {
     }
 }
 
-void RetinaFace::detectAndAlign(vector<cv::Mat> imgs, float threshold, const AlignOptions &align) {
-    last_.assign(imgs.size(), vector<FaceDetectInfo>());
-    scales_.assign(imgs.size(), 1.f);
-    crops_.assign(imgs.size(), vector<Mat>());
+// rf_align_params of u8 BGR crops, and where they land: `per` crop slots per image of cw x ch
+static rf_align_params crop_params(const AlignOptions &align, int max_faces, int *per, int *cw, int *ch) {
     rf_align_params p{};
     p.crop_w = align.crop_w;
     p.crop_h = align.crop_h;
     for (int k = 0; k < 10; k++) p.template_xy[k] = align.template_xy[k];
     p.max_faces = align.max_faces;
     p.format = RF_CROP_BGR_U8;
-    const int per = align.max_faces > 0 ? align.max_faces : opt_.max_faces;
+    *per = align.max_faces > 0 ? align.max_faces : max_faces;
     const bool dflt = align.crop_w == 0 && align.crop_h == 0;    // rf_align_params: 0 x 0 -> 112 x 112
-    const int cw = dflt ? 112 : align.crop_w, ch = dflt ? 112 : align.crop_h;
+    *cw = dflt ? 112 : align.crop_w;
+    *ch = dflt ? 112 : align.crop_h;
+    return p;
+}
+
+void RetinaFace::detectAndAlign(vector<cv::Mat> imgs, float threshold, const AlignOptions &align) {
+    last_.assign(imgs.size(), vector<FaceDetectInfo>());
+    scales_.assign(imgs.size(), 1.f);
+    crops_.assign(imgs.size(), vector<Mat>());
+    int per = 0, cw = 0, ch = 0;
+    const rf_align_params p = crop_params(align, opt_.max_faces, &per, &cw, &ch);
     const size_t crop_bytes = (size_t)cw * ch * 3;
     const size_t mb = (size_t)opt_.max_batch;
     vector<unsigned char> crops(mb * per * crop_bytes);
@@ -125,16 +133,59 @@ void RetinaFace::detectAndAlign(vector<cv::Mat> imgs, float threshold, const Ali
         int rc = rf_detect_align_batch(h_, ptrs.data(), ws.data(), hs.data(), strides.data(), n, threshold, nms_threshold, &p,
                                        out_faces_.data(), out_counts_.data(), crops.data(), nullptr);
         if (rc != RF_OK) throw std::runtime_error(string("rf_detect_align_batch: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+        keepResults(start, n, crops.data(), per, cw, ch);
+    }
+}
+
+void RetinaFace::keepResults(size_t start, int n, const unsigned char *crops, int per, int cw, int ch) {
+    const size_t crop_bytes = (size_t)cw * ch * 3;
+    for (int i = 0; i < n; i++) {
+        const FaceDetectInfo *f = reinterpret_cast<const FaceDetectInfo *>(out_faces_.data() + (size_t)i * opt_.max_faces);
+        last_[start + i].assign(f, f + out_counts_[i]);
+        for (int j = 0; crops && j < std::min(out_counts_[i], per); j++) {
+            Mat c(ch, cw, CV_8UC3);
+            const unsigned char *src = crops + ((size_t)i * per + j) * crop_bytes;
+            for (int y = 0; y < ch; y++) std::memcpy(c.data + (size_t)y * c.step, src + (size_t)y * cw * 3, (size_t)cw * 3);
+            crops_[start + i].push_back(c);
+        }
+    }
+}
+
+void RetinaFace::detectYUV(const vector<Mat> &frames, int layout, float threshold, const AlignOptions *align) {
+    if (layout < YUV_NV12 || layout > YUV_YV12) throw std::runtime_error("detectYUV: unknown layout");
+    last_.assign(frames.size(), vector<FaceDetectInfo>());
+    scales_.assign(frames.size(), 1.f);
+    crops_.assign(frames.size(), vector<Mat>());
+    int per = 0, cw = 0, ch = 0;
+    const rf_align_params p = align ? crop_params(*align, opt_.max_faces, &per, &cw, &ch) : rf_align_params{};
+    const size_t mb = (size_t)opt_.max_batch;
+    vector<unsigned char> crops(align ? mb * per * cw * ch * 3 : 0);
+    for (size_t start = 0; start < frames.size(); start += mb) {
+        const int n = (int)std::min(mb, frames.size() - start);
+        vector<rf_yuv_frame> fr(n);
         for (int i = 0; i < n; i++) {
-            const FaceDetectInfo *f = reinterpret_cast<const FaceDetectInfo *>(out_faces_.data() + (size_t)i * opt_.max_faces);
-            last_[start + i].assign(f, f + out_counts_[i]);
-            for (int j = 0; j < std::min(out_counts_[i], per); j++) {
-                Mat c(ch, cw, CV_8UC3);
-                const unsigned char *src = crops.data() + ((size_t)i * per + j) * crop_bytes;
-                for (int y = 0; y < ch; y++) std::memcpy(c.data + (size_t)y * c.step, src + (size_t)y * cw * 3, (size_t)cw * 3);
-                crops_[start + i].push_back(c);
+            // OpenCV's single buffer: the luma rows, then the chroma -- interleaved rows of the same step (NV12 / NV21), or the
+            // U and V planes of w / 2 x h / 2 packed one after the other (I420: U first, YV12: V first)
+            const cv::Mat &m = frames[start + i];
+            if (m.empty() || m.rows % 3 || m.cols % 2) throw std::runtime_error("detectYUV: frames must be non-empty (h * 3 / 2) x w with even h and w");
+            const int w = m.cols, hh = m.rows / 3 * 2;
+            const unsigned char *c = m.data + m.step * hh;
+            rf_yuv_frame &f = fr[i];
+            f.y = m.data; f.y_pitch = (int)m.step; f.width = w; f.height = hh;
+            if (layout == YUV_NV12 || layout == YUV_NV21) {
+                f.uv_step = 2; f.uv_pitch = (int)m.step;
+                f.u = c + (layout == YUV_NV21); f.v = c + (layout == YUV_NV12);
+            } else {
+                if (m.step != (size_t)w) throw std::runtime_error("detectYUV: planar (I420 / YV12) frames must be continuous");
+                const unsigned char *q = c + (size_t)(w / 2) * (hh / 2);
+                f.uv_step = 1; f.uv_pitch = w / 2;
+                f.u = layout == YUV_I420 ? c : q; f.v = layout == YUV_I420 ? q : c;
             }
         }
+        int rc = rf_detect_yuv_batch(h_, fr.data(), n, RF_YUV_BT601, threshold, nms_threshold, align ? &p : nullptr, out_faces_.data(), out_counts_.data(),
+                                     nullptr, align ? crops.data() : nullptr, nullptr);
+        if (rc != RF_OK) throw std::runtime_error(string("rf_detect_yuv_batch: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+        keepResults(start, n, align ? crops.data() : nullptr, per, cw, ch);
     }
 }
 

@@ -78,12 +78,20 @@ class RetinaFace {
     // the crops of image i's first min(faces, max_faces) faces, crop_h x crop_w 8UC3 Mats
     void detectAndAlign(vector<cv::Mat> imgs, float threshold, const AlignOptions &align = AlignOptions());
     const vector<vector<Mat>> &lastCrops() const { return crops_; }
+    // f6 video frames (rf_detect_yuv_batch): 8-bit YUV 4:2:0 frames as OpenCV keeps them, CV_8UC1 Mats of (h * 3 / 2) x w in
+    // `layout` (YUV_NV12 .. YUV_YV12; semi-planar frames may have a row step, planar ones must be continuous), BT.601 as
+    // cv::cvtColor(COLOR_YUV2BGR_<layout>).  Afterwards lastBatchFaces() holds the faces in FRAME pixels (lastScale() is 1) and,
+    // with `align`, lastCrops() the crops as detectAndAlign leaves them.
+    enum YuvLayout { YUV_NV12 = 0, YUV_NV21 = 1, YUV_I420 = 2, YUV_YV12 = 3 };
+    void detectYUV(const vector<Mat> &frames, int layout, float threshold, const AlignOptions *align = nullptr);
     // the reference's visualisation (RetinaFace.cpp:730-741): red box outline (thickness 2), green landmark dots, on a clone
     static Mat draw(const Mat &img, const vector<FaceDetectInfo> &faces);
     int netWidth() const { return opt_.net_w; }
     int netHeight() const { return opt_.net_h; }
 
    private:
+    // faces (and, with crops, the u8 crops of the first min(count, per) faces) of images [start, start + n) of the last call
+    void keepResults(size_t start, int n, const unsigned char *crops, int per, int cw, int ch);
     rf_handle h_ = nullptr;
     RetinaFaceOptions opt_;
     string network;

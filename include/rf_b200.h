@@ -303,6 +303,79 @@ int rf_detect_yuv_batch_device(rf_handle h, const rf_yuv_frame *frames, int n, i
 /* Preprocess parity of f6 (as rf_preprocess): one host frame letter-boxed into a host net_h*net_w*3 u8 BGR buffer. */
 int rf_preprocess_yuv(rf_handle h, const rf_yuv_frame *frame, int matrix, uint8_t *out_net_sized);
 
+/* f7 tiled detection: small faces in large images.  The letter-box of rf_detect_batch shrinks a 3840x2160 frame 8.6x on a 448x448
+ * network, so a face narrower than ~137 pixels falls below the smallest anchor.  Here an image is resized to a pyramid of LEVELS,
+ * each cv::resize(img, Size(), s, s, INTER_LINEAR) byte for byte (s may exceed 1; optionally of the mirrored image; at s = 0.5 that
+ * is OpenCV's fast 2x INTER_AREA code, which cv::resize runs for INTER_LINEAR there), and every level is cut into
+ * overlapping network-sized TILES that run as ordinary batches through the unchanged forward.  Detections are mapped back to image
+ * pixels and merged across tiles and levels by one more greedy NMS (rf_detect_views' rule and threshold), all on the GPU.
+ *
+ * Geometry, per axis, with the level's size S = saturate_cast<int>(side * s) (round half to even), the tile size T (net_w or net_h)
+ * and the overlap o:
+ *   S <= T  one tile at origin 0, zeros beyond S, no shared sides;
+ *   S >  T  k = ceil((S - o) / (T - o)) tiles at origins min(i (T - o), S - T): the last tile is flush with the far edge.
+ * Each tile OWNS a half-open core: neighbours i, i + 1 split at floor((origin_i + origin_i+1 + T) / 2), the middle of the strip they
+ * share; the first core starts at 0, the last ends at the far edge of the last tile (S on a tiled axis).  The cores partition the
+ * level.  On an axis held by ONE tile nothing is filtered: that tile owns every detection along it, the zero padding beyond S
+ * included (its core is reported as [0, T)), as rf_detect_batch keeps them.  Scale 0 is the FITTED level: exactly the
+ * letter-box rf_detect_batch feeds the network (one tile, never up-scaled, the reference's float map-back factor).
+ * Seams: a kept detection of a tile survives only if its centre (x1 + x2) * 0.5 (likewise y, in float) lies in the tile's core, and
+ * it does not reach a SHARED side (x1 <= 0 on a shared left side, x2 >= net_w - 1 on a shared right one, likewise in y: the decode
+ * clamps exactly there, so such a box was cut by the tile edge).  A face of side d < o at a level is therefore found whole by
+ * exactly one tile; the default pyramid halves until the image fits, so every face is below o at some level until it is too small
+ * to detect.  Survivors map back as image x = (x + origin) * map_back (mirrored levels then un-mirrored, landmarks swapped) and
+ * join their image's candidate list with id tile * max_faces + rank, which is the tie order of the final NMS. */
+typedef struct rf_tile_level {
+    float scale;                   /* > 0: the level is the image resized by `scale`; 0: the fitted level */
+    int32_t flip;                  /* non-zero: the level is of the horizontally mirrored image */
+} rf_tile_level;
+typedef struct rf_tiling {
+    const rf_tile_level *levels;   /* NULL or nlevels == 0: the default pyramid -- levels 1, 1/2, 1/4, ... for as long as a level does
+                                      not fit in one tile, then the fitted level (an image that fits gets the fitted level alone) */
+    int nlevels;                   /* <= RF_MAX_TILE_LEVELS */
+    int overlap;                   /* resized-image pixels neighbouring tiles share; 0 -> 64, else in [16, min(net_w, net_h) / 2] */
+} rf_tiling;
+typedef struct rf_tile {           /* one tile, in the order candidate ids are numbered: level by level, row-major within a level */
+    int level, flip, scaled_w, scaled_h;          /* level index, mirrored, size of the resized level */
+    int x0, y0;                                   /* tile origin in the level */
+    int own_x0, own_y0, own_x1, own_y1;           /* ownership core in level pixels, half-open */
+    int shared_sides;                             /* RF_TILE_SIDE_* bits */
+    float scale, map_back;                        /* image pixel = (tile pixel + origin) * map_back, then un-mirrored */
+} rf_tile;
+#define RF_MAX_TILE_LEVELS 8
+#define RF_MAX_TILES 256           /* per image, all levels */
+#define RF_TILE_SIDE_LEFT   0x1
+#define RF_TILE_SIDE_TOP    0x2
+#define RF_TILE_SIDE_RIGHT  0x4
+#define RF_TILE_SIDE_BOTTOM 0x8
+/* Host-only (works without a GPU): the tiles of one width x height image on a net_w x net_h network (t may be NULL: the default
+ * pyramid, overlap 64).  Returns the tile count and writes the first min(count, cap) tiles to out (out may be NULL when cap is 0),
+ * or a status: RF_ERR_INVALID_ARG for a scale that is negative, NaN or infinite, whose resized side is 0 or exceeds 16384, an overlap
+ * out of range, nlevels outside [0, RF_MAX_TILE_LEVELS] or bad sizes; RF_ERR_CAPACITY for more than RF_MAX_TILES tiles. */
+int rf_tile_layout(int net_w, int net_h, int width, int height, const rf_tiling *t, rf_tile *out, int cap);
+/* Host images as rf_detect_batch (any size up to max_image, pinned or pageable, row strides; at most max_batch per call); blocking.
+ * out_faces [n][max_faces] in ORIGINAL IMAGE pixels, best first; out_counts [n]; out_tile_of (optional, [n][max_faces]): the tile
+ * each kept face came from, an index into rf_tile_layout of its image.  Besides the statuses of rf_tile_layout: an image above
+ * max_image is RF_ERR_CAPACITY, a handle created with RF_FLAG_NPP_RESIZE RF_ERR_UNSUPPORTED (NPPI_INTER_SUPER only down-samples;
+ * levels are defined by cv::resize); all before anything is launched.
+ * Execution contexts: the images are uploaded on context 0, a group of raw buffers at a time; their tiles are then letter-boxed,
+ * detected and merged in chunks of up to max_batch tiles, each chunk on the next context of the rotation rf_detect_batch_device
+ * uses (into that context's own input tensor), and the final NMS runs on context 0 once every context has finished.  Each chunk
+ * counts as one call for the rule that rf_detect_batch_device's outputs stay valid for `streams` calls. */
+int rf_detect_tiled(rf_handle h, const uint8_t *const *bgr_images, const int *widths, const int *heights, const int *row_strides,
+                    int n, const rf_tiling *t, float score_threshold, float nms_threshold,
+                    rf_face *out_faces, int *out_counts, int32_t *out_tile_of);
+/* The same on host YUV 4:2:0 frames (rf_detect_yuv_batch's descriptors and checks): the tiles of cv2.cvtColor(frame). */
+int rf_detect_yuv_tiled(rf_handle h, const rf_yuv_frame *frames, int n, int matrix, const rf_tiling *t, float score_threshold,
+                        float nms_threshold, rf_face *out_faces, int *out_counts, int32_t *out_tile_of);
+/* Preprocess parity of rf_detect_yuv_tiled (as rf_preprocess_yuv): tile `tile` of one host frame's layout, converted and resized as
+ * the network sees it, into a host net_h*net_w*3 u8 BGR buffer. */
+int rf_preprocess_yuv_tile(rf_handle h, const rf_yuv_frame *frame, int matrix, const rf_tiling *t, int tile, uint8_t *out_net_sized);
+/* Preprocess parity of f7 (as rf_preprocess): tile `tile` of one host image's layout, as the network sees it, into a host
+ * net_h*net_w*3 u8 BGR buffer. */
+int rf_preprocess_tile(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, const rf_tiling *t, int tile,
+                       uint8_t *out_net_sized);
+
 /* Introspection. */
 int rf_get_net_size(rf_handle h, int *net_w, int *net_h, int *max_batch, int *max_faces);
 int rf_num_anchors(rf_handle h);            /* per image: 8,232 @448x448, 47,040 @1280x896 */

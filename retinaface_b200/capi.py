@@ -28,6 +28,7 @@ EXPORTS = [
     "rf_detect_jpeg_batch", "rf_decode_jpeg", "rf_jpeg_backend",
     "rf_detect_align_batch", "rf_detect_align_batch_device",
     "rf_detect_yuv_batch", "rf_detect_yuv_batch_device", "rf_preprocess_yuv",
+    "rf_tile_layout", "rf_detect_tiled", "rf_detect_yuv_tiled", "rf_preprocess_tile", "rf_preprocess_yuv_tile",
 ]
 COMM_BLOB_BYTES = 128
 
@@ -130,6 +131,49 @@ def _matrix(matrix) -> int:
     return int(matrix)
 
 
+class TileLevel(C.Structure):    # rf_tile_level
+    _fields_ = [("scale", C.c_float), ("flip", C.c_int32)]
+
+
+class Tiling(C.Structure):       # rf_tiling
+    _fields_ = [("levels", C.POINTER(TileLevel)), ("nlevels", C.c_int), ("overlap", C.c_int)]
+
+
+class Tile(C.Structure):         # rf_tile
+    _fields_ = [(f, C.c_int) for f in ("level", "flip", "scaled_w", "scaled_h", "x0", "y0", "own_x0", "own_y0", "own_x1", "own_y1",
+                                       "shared_sides")] + [("scale", C.c_float), ("map_back", C.c_float)]
+
+
+MAX_TILE_LEVELS, MAX_TILES = 8, 256          # RF_MAX_TILE_LEVELS, RF_MAX_TILES
+TILE_SIDE_LEFT, TILE_SIDE_TOP, TILE_SIDE_RIGHT, TILE_SIDE_BOTTOM = 0x1, 0x2, 0x4, 0x8
+
+
+def tiling(levels=None, overlap: int = 0) -> Tiling:
+    """rf_tiling.  levels: [(scale, flip), ...] (scale 0: the fitted level), None or [] -> the default pyramid; overlap 0 -> 64.
+    The level array lives on the returned structure (keep it alive for the call)."""
+    levels = list(levels or [])
+    arr = (TileLevel * max(len(levels), 1))(*[TileLevel(float(s), int(bool(f))) for s, f in levels])
+    t = Tiling(C.cast(arr, C.POINTER(TileLevel)) if levels else None, len(levels), int(overlap))
+    t._keep = arr
+    return t
+
+
+def tile_dict(t: Tile) -> dict:
+    return {f: getattr(t, f) for f, _ in Tile._fields_}
+
+
+def tile_layout(net_w: int, net_h: int, width: int, height: int, levels=None, overlap: int = 0) -> List[dict]:
+    """rf_tile_layout (host-only): the tiles of one width x height image, each as a dict of rf_tile's fields, in candidate-id order."""
+    lib = load_library()
+    t = tiling(levels, overlap)
+    k = lib.rf_tile_layout(net_w, net_h, width, height, C.byref(t), None, 0)
+    if k < 0:
+        raise RfError(k, (lib.rf_last_error(None) or b"").decode())
+    out = (Tile * max(k, 1))()
+    k = lib.rf_tile_layout(net_w, net_h, width, height, C.byref(t), out, k)
+    return [tile_dict(out[i]) for i in range(k)]
+
+
 class RfError(RuntimeError):
     def __init__(self, status: int, msg: str):
         super().__init__(f"librf_b200 status {status}: {msg}")
@@ -221,6 +265,13 @@ def load_library() -> C.CDLL:
     lib.rf_detect_yuv_batch_device.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_int, C.c_int, C.c_float, C.c_float, C.POINTER(AlignParams),
                                                C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_void_p]
     lib.rf_preprocess_yuv.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_int, C.c_void_p]
+    lib.rf_tile_layout.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(Tiling), C.POINTER(Tile), C.c_int]
+    lib.rf_detect_tiled.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int,
+                                    C.POINTER(Tiling), C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.rf_detect_yuv_tiled.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_int, C.c_int, C.POINTER(Tiling), C.c_float, C.c_float, C.c_void_p,
+                                        C.c_void_p, C.c_void_p]
+    lib.rf_preprocess_tile.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(Tiling), C.c_int, C.c_void_p]
+    lib.rf_preprocess_yuv_tile.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_int, C.POINTER(Tiling), C.c_int, C.c_void_p]
     _lib = lib
     return lib
 
@@ -506,6 +557,63 @@ class Engine:
         arr = self._frames([frame], layout, False)
         out = np.empty((self.net_h, self.net_w, 3), dtype=np.uint8)
         self._check(self.lib.rf_preprocess_yuv(self.h, arr, _matrix(matrix), out.ctypes.data))
+        return out
+
+    # -- f7 tiled detection ----------------------------------------------------------------------------
+    @staticmethod
+    def _bgr_strided(im):
+        """The image as the C ABI takes it: u8 BGR HWC with contiguous pixels (rows may be strided)."""
+        if im.ndim != 3 or im.shape[2] != 3:
+            raise ValueError(f"u8 BGR HWC images expected, got shape {im.shape}")
+        if not (im.dtype == np.uint8 and im.strides[1:] == (3, 1) and im.strides[0] >= 3 * im.shape[1]):
+            im = np.ascontiguousarray(im, dtype=np.uint8)
+        return im
+
+    def _tiled_out(self, n):
+        return (np.empty((n, self.max_faces, FACE_FLOATS), dtype=np.float32), np.zeros(n, dtype=np.int32),
+                np.empty((n, self.max_faces), dtype=np.int32))
+
+    def detect_tiled(self, images: Sequence[np.ndarray], thr: float, nms_thr: float, levels=None, overlap: int = 0):
+        """rf_detect_tiled: u8 BGR HWC images (any size <= max_image; rows may be strided) cut into tiles of a scale pyramid
+        (levels: [(scale, flip), ...], scale 0 = the fitted level; None = the default pyramid).  Returns (faces: one (k, 15) float32
+        array per image in ORIGINAL IMAGE pixels, tile_of: one (k,) array per image, indices into tile_layout)."""
+        n = len(images)
+        keep = [self._bgr_strided(im) for im in images]
+        ptrs = (C.c_void_p * max(n, 1))(*[im.ctypes.data for im in keep])
+        ws = (C.c_int * max(n, 1))(*[im.shape[1] for im in keep])
+        hs = (C.c_int * max(n, 1))(*[im.shape[0] for im in keep])
+        rs = (C.c_int * max(n, 1))(*[im.strides[0] for im in keep])
+        t = tiling(levels, overlap)
+        faces, counts, tile_of = self._tiled_out(n)
+        self._check(self.lib.rf_detect_tiled(self.h, ptrs, ws, hs, rs, n, C.byref(t), thr, nms_thr, faces.ctypes.data, counts.ctypes.data,
+                                             tile_of.ctypes.data))
+        return [faces[i, :counts[i]].copy() for i in range(n)], [tile_of[i, :counts[i]].copy() for i in range(n)]
+
+    def detect_yuv_tiled(self, frames, thr: float, nms_thr: float, layout: str = "nv12", matrix="bt601", levels=None, overlap: int = 0):
+        """rf_detect_yuv_tiled: host 4:2:0 frames (yuv_frame's forms) -> (faces, tile_of) as detect_tiled, in FRAME pixels."""
+        n = len(frames)
+        arr = self._frames(frames, layout, False)
+        t = tiling(levels, overlap)
+        faces, counts, tile_of = self._tiled_out(n)
+        self._check(self.lib.rf_detect_yuv_tiled(self.h, arr, n, _matrix(matrix), C.byref(t), thr, nms_thr, faces.ctypes.data,
+                                                 counts.ctypes.data, tile_of.ctypes.data))
+        return [faces[i, :counts[i]].copy() for i in range(n)], [tile_of[i, :counts[i]].copy() for i in range(n)]
+
+    def preprocess_tile(self, img: np.ndarray, tile: int, levels=None, overlap: int = 0) -> np.ndarray:
+        """rf_preprocess_tile: tile `tile` of the image's layout as the network sees it, (H, W, 3) u8 BGR."""
+        img = self._bgr_strided(img)
+        out = np.empty((self.net_h, self.net_w, 3), dtype=np.uint8)
+        t = tiling(levels, overlap)
+        self._check(self.lib.rf_preprocess_tile(self.h, img.ctypes.data, img.shape[1], img.shape[0], img.strides[0], C.byref(t), int(tile),
+                                                out.ctypes.data))
+        return out
+
+    def preprocess_yuv_tile(self, frame, tile: int, layout: str = "nv12", matrix="bt601", levels=None, overlap: int = 0) -> np.ndarray:
+        """rf_preprocess_yuv_tile: tile `tile` of one host 4:2:0 frame's layout as the network sees it, (H, W, 3) u8 BGR."""
+        arr = self._frames([frame], layout, False)
+        out = np.empty((self.net_h, self.net_w, 3), dtype=np.uint8)
+        t = tiling(levels, overlap)
+        self._check(self.lib.rf_preprocess_yuv_tile(self.h, arr, _matrix(matrix), C.byref(t), int(tile), out.ctypes.data))
         return out
 
     def detect_jpeg(self, streams: Sequence[bytes], thr: float, nms_thr: float):

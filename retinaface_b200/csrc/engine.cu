@@ -238,6 +238,7 @@ void destroy(rf_handle h) {
     jpeg_release(h);
     for (Ctx &c : h->ctx) release_ctx(c, true);
     free_post_buffers(h->pb_merge);
+    free_post_buffers(h->pb_tiles);
     cudaFree(h->d_weights); cudaFree(h->d_weights_h); cudaFree(h->d_weights_q); cudaFree(h->d_input); cudaFree(h->d_raw);
     for (auto p : h->d_blobs) cudaFree(p);
     h->copy_pool.reset();
@@ -525,12 +526,15 @@ static void put_results(rf_handle h, const rf_det *dets, const int *counts, size
     }
 }
 
-// Waits for context c's results of n images and copies them out (through the pinned h_counts / h_dets).
-static void fetch_results(rf_handle h, Ctx &c, int n, rf_face *out_faces, int *out_counts, int32_t *out_idx) {
-    CK(cudaMemcpyAsync(h->h_counts, c.pb.out_counts, sizeof(int) * n, cudaMemcpyDeviceToHost, c.stream));
-    CK(cudaMemcpyAsync(h->h_dets, c.pb.out_dets, sizeof(rf_det) * (size_t)n * h->cfg.max_faces, cudaMemcpyDeviceToHost, c.stream));
-    CK(cudaStreamSynchronize(c.stream));
+// Waits for the results of n images in pb (written on stream s) and copies them out (through the pinned h_counts / h_dets).
+static void fetch_post(rf_handle h, const PostBuffers &pb, cudaStream_t s, int n, rf_face *out_faces, int *out_counts, int32_t *out_idx) {
+    CK(cudaMemcpyAsync(h->h_counts, pb.out_counts, sizeof(int) * n, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(h->h_dets, pb.out_dets, sizeof(rf_det) * (size_t)n * h->cfg.max_faces, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
     put_results(h, h->h_dets, h->h_counts, 0, n, out_faces, out_counts, out_idx);
+}
+static void fetch_results(rf_handle h, Ctx &c, int n, rf_face *out_faces, int *out_counts, int32_t *out_idx) {
+    fetch_post(h, c.pb, c.stream, n, out_faces, out_counts, out_idx);
 }
 
 // Whether `p` is page-locked host memory (cudaHostAlloc / cudaHostRegister), which an H2D copy may read in place.
@@ -945,6 +949,191 @@ int rf_preprocess_yuv(rf_handle h, const rf_yuv_frame *frame, int matrix, uint8_
     return RF_OK;
 }
 
+// ---- f7 tiled detection: a scale pyramid cut into network-sized tiles (preprocess.cuh tile_layout) ----------------------------------
+int rf_tile_layout(int net_w, int net_h, int width, int height, const rf_tiling *t, rf_tile *out, int cap) {
+    if (cap < 0 || (cap > 0 && !out)) return fail(nullptr, RF_ERR_INVALID_ARG, "rf_tile_layout: cap < 0 or out is NULL");
+    std::vector<rf_tile> tiles;
+    std::string err;
+    const int rc = tile_layout(net_w, net_h, width, height, t, tiles, &err);
+    if (rc) return fail(nullptr, rc, "rf_tile_layout: " + err);
+    std::copy_n(tiles.begin(), std::min<size_t>(tiles.size(), (size_t)cap), out);
+    return (int)tiles.size();
+}
+
+// The checks every tiled entry point shares, after its own input checks: the resize definition and each image's layout.
+static int tiled_layouts(rf_handle h, const char *who, int n, const int *widths, const int *heights, const rf_tiling *t,
+                         std::vector<std::vector<rf_tile>> &layouts) {
+    if (h->cfg.flags & RF_FLAG_NPP_RESIZE)
+        return fail(h, RF_ERR_UNSUPPORTED, fmt("%s: tiles are levels of cv::resize; the handle letter-boxes with NPPI_INTER_SUPER, which "
+                                               "only down-samples", who));
+    layouts.resize(n);
+    for (int i = 0; i < n; i++) {
+        std::string err;
+        const int rc = tile_layout(h->cfg.net_w, h->cfg.net_h, widths[i], heights[i], t, layouts[i], &err);
+        if (rc) return fail(h, rc, fmt("%s: image %d: %s", who, i, err.c_str()));
+    }
+    return RF_OK;
+}
+
+// Tiled detection of n images whose layouts are checked.  upload(s, i, slot) brings image i into raw buffer `slot` on stream s and
+// returns the letter-box source.  Context 0 uploads up to raw_slots images at a time; their tiles are letter-boxed, detected and
+// merged in chunks of up to max_batch, each chunk on the next context of the rf_detect_batch_device rotation, into that context's
+// own input tensor.  Before the next group overwrites the raw buffers -- and before the final NMS -- context 0 waits for every
+// context the group used.
+extern "C++" {
+template <typename Src, typename Upload>
+static void detect_tiled_impl(rf_handle h, int n, const int *widths, const int *heights, const std::vector<std::vector<rf_tile>> &layouts,
+                              Upload upload, float thr, float nms, rf_face *out_faces, int *out_counts, int32_t *out_tile_of) {
+    const int Hn = h->cfg.net_h, Wn = h->cfg.net_w, mf = h->cfg.max_faces, B = h->cfg.max_batch;
+    const size_t img_bytes = (size_t)Hn * Wn * 3;
+    size_t most = 0;
+    for (const auto &l : layouts) most = std::max(most, l.size());
+    // every tile of an image may contribute max_faces candidates to the image's merged list
+    if ((size_t)h->pb_tiles.anchors_per_image < most * mf) {
+        free_post_buffers(h->pb_tiles);
+        alloc_post_buffers(h->pb_tiles, (int)(most * mf), B, mf);
+    }
+    Ctx &c0 = h->ctx[0];
+    std::vector<Src> src(n);
+    struct TileRef { int image, tile; };
+    for (int g0 = 0; g0 < n; g0 += h->raw_slots) {
+        const int g1 = std::min(n, g0 + h->raw_slots);
+        for (int i = g0; i < g1; i++) src[i] = upload(c0.stream, i, i - g0);
+        CK(cudaEventRecord(c0.fence, c0.stream));     // the raw images of this group are on the device
+        std::vector<TileRef> refs;
+        for (int i = g0; i < g1; i++)
+            for (int k = 0; k < (int)layouts[i].size(); k++) refs.push_back(TileRef{i, k});
+        std::vector<char> joined(h->ctx.size(), 0);
+        for (size_t k0 = 0; k0 < refs.size(); k0 += B) {
+            const int m = (int)std::min<size_t>(B, refs.size() - k0);
+            const size_t ci = h->next_dev_ctx++ % h->ctx.size();
+            Ctx &c = h->ctx[ci];
+            if (ci != 0 && !joined[ci]) CK(cudaStreamWaitEvent(c.stream, c0.fence, 0));
+            joined[ci] = 1;
+            if (!c.d_frames_in) CK(cudaMalloc(&c.d_frames_in, (size_t)B * img_bytes));
+            if (c.param_seq && c.param_seq % Ctx::kParamSlots == 0) CK(cudaStreamSynchronize(c.stream));
+            std::vector<LbItemT<Src>> lb(m);
+            std::vector<MergeSource> ms(m);
+            for (int b = 0; b < m; b++) {
+                const TileRef r = refs[k0 + b];
+                const rf_tile &tl = layouts[r.image][r.tile];
+                tile_fill(lb[b], src[r.image], widths[r.image], heights[r.image], c.d_frames_in + b * img_bytes, Wn, Hn, tl);
+                ms[b] = tile_source(r.image, r.tile, mf, tl, widths[r.image]);
+            }
+            CK(launch_letterbox_batch(lb.data(), m, Wn, Hn, c.stream));
+            set_params(h, c, thr, nms, c.d_frames_in);
+            forward_graph(h, c, m);
+            CK(launch_merge(c.pb, ms.data(), m, Wn, Hn, h->pb_tiles, c.stream));
+        }
+        for (size_t ci = 1; ci < h->ctx.size(); ci++) {
+            if (!joined[ci]) continue;
+            CK(cudaEventRecord(h->ctx[ci].fence, h->ctx[ci].stream));
+            CK(cudaStreamWaitEvent(c0.stream, h->ctx[ci].fence, 0));
+        }
+    }
+    // the final NMS over each image's candidates from all its tiles and levels reads its threshold from context 0's parameters
+    if (c0.param_seq && c0.param_seq % Ctx::kParamSlots == 0) CK(cudaStreamSynchronize(c0.stream));
+    set_params(h, c0, thr, nms);
+    launch_nms(n, c0.d_params, h->pb_tiles, c0.stream);
+    CK(cudaGetLastError());
+    fetch_post(h, h->pb_tiles, c0.stream, n, out_faces, out_counts, out_tile_of);
+    if (out_tile_of)      // candidate id = tile * max_faces + rank
+        for (int i = 0; i < n; i++)
+            for (int j = 0; j < std::min(h->h_counts[i], mf); j++) out_tile_of[(size_t)i * mf + j] /= mf;
+}
+}  // extern "C++"
+
+int rf_detect_tiled(rf_handle h, const uint8_t *const *imgs, const int *widths, const int *heights, const int *row_strides, int n,
+                    const rf_tiling *t, float thr, float nms, rf_face *out_faces, int *out_counts, int32_t *out_tile_of) {
+    static const char *who = "rf_detect_tiled";
+    int rc = check_n(h, n);
+    if (rc) return rc;
+    if (n > 0 && (!imgs || !widths || !heights)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL image arrays", who));
+    for (int i = 0; i < n; i++) {
+        if (!imgs[i] || widths[i] <= 0 || heights[i] <= 0) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: image %d is empty", who, i));
+        if (row_strides && row_strides[i] && row_strides[i] < widths[i] * 3)
+            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: image %d: row stride %d below %d bytes", who, i, row_strides[i], widths[i] * 3));
+        if (widths[i] > h->cfg.max_image_w || heights[i] > h->cfg.max_image_h)
+            return fail(h, RF_ERR_CAPACITY, fmt("%s: image %d is %dx%d, larger than max_image %dx%d", who, i, widths[i], heights[i],
+                                                h->cfg.max_image_w, h->cfg.max_image_h));
+    }
+    std::vector<std::vector<rf_tile>> layouts;
+    if ((rc = tiled_layouts(h, who, n, widths, heights, t, layouts))) return rc;
+    if (n == 0) return RF_OK;
+    try {
+        CK(cudaSetDevice(h->device));
+        auto upload = [&](cudaStream_t s, int i, int slot) -> const uint8_t * {
+            const int rs = row_strides && row_strides[i] ? row_strides[i] : widths[i] * 3;
+            return upload_raw(h, s, imgs[i], widths[i], heights[i], rs, slot);
+        };
+        detect_tiled_impl<const uint8_t *>(h, n, widths, heights, layouts, upload, thr, nms, out_faces, out_counts, out_tile_of);
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
+}
+
+int rf_detect_yuv_tiled(rf_handle h, const rf_yuv_frame *frames, int n, int matrix, const rf_tiling *t, float thr, float nms,
+                        rf_face *out_faces, int *out_counts, int32_t *out_tile_of) {
+    static const char *who = "rf_detect_yuv_tiled";
+    int rc = check_frames(h, who, frames, n, matrix);
+    if (rc) return rc;
+    std::vector<int> widths(n), heights(n);
+    for (int i = 0; i < n; i++) { widths[i] = frames[i].width; heights[i] = frames[i].height; }
+    std::vector<std::vector<rf_tile>> layouts;
+    if ((rc = tiled_layouts(h, who, n, widths.data(), heights.data(), t, layouts))) return rc;
+    if (n == 0) return RF_OK;
+    try {
+        CK(cudaSetDevice(h->device));
+        auto upload = [&](cudaStream_t s, int i, int slot) { return upload_frame(h, s, frames[i], matrix, slot); };
+        detect_tiled_impl<YuvPlanes>(h, n, widths.data(), heights.data(), layouts, upload, thr, nms, out_faces, out_counts, out_tile_of);
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
+}
+
+// The parity hooks of the tiled paths: tile `tile` of one image's layout into `out`.  upload(s) brings the image into raw buffer 0
+// on s and returns the letter-box source.
+extern "C++" {
+template <typename Src, typename Upload>
+static int preprocess_tile_impl(rf_handle h, const char *who, int width, int height, const rf_tiling *t, int tile, uint8_t *out, Upload upload) {
+    std::vector<std::vector<rf_tile>> layouts;
+    int rc = tiled_layouts(h, who, 1, &width, &height, t, layouts);
+    if (rc) return rc;
+    if (tile < 0 || tile >= (int)layouts[0].size())
+        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: tile %d, the layout has %zu", who, tile, layouts[0].size()));
+    const int Hn = h->cfg.net_h, Wn = h->cfg.net_w;
+    try {
+        CK(cudaSetDevice(h->device));
+        cudaStream_t s = h->ctx[0].stream;
+        LbItemT<Src> it;
+        tile_fill(it, upload(s), width, height, h->d_input, Wn, Hn, layouts[0][tile]);
+        CK(launch_letterbox_batch(&it, 1, Wn, Hn, s));
+        CK(cudaMemcpyAsync(h->h_input, h->d_input, (size_t)Hn * Wn * 3, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        memcpy(out, h->h_input, (size_t)Hn * Wn * 3);
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
+}
+}  // extern "C++"
+
+int rf_preprocess_tile(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, const rf_tiling *t, int tile, uint8_t *out) {
+    static const char *who = "rf_preprocess_tile";
+    if (!h) return RF_ERR_INVALID_ARG;
+    if (!bgr || !out || width <= 0 || height <= 0) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: bad arguments", who));
+    if (width > h->cfg.max_image_w || height > h->cfg.max_image_h) return fail(h, RF_ERR_CAPACITY, fmt("%s: image larger than max_image", who));
+    const int rs = row_stride ? row_stride : width * 3;
+    return preprocess_tile_impl<const uint8_t *>(h, who, width, height, t, tile, out,
+                                                 [&](cudaStream_t s) { return (const uint8_t *)upload_raw(h, s, bgr, width, height, rs); });
+}
+
+int rf_preprocess_yuv_tile(rf_handle h, const rf_yuv_frame *frame, int matrix, const rf_tiling *t, int tile, uint8_t *out) {
+    static const char *who = "rf_preprocess_yuv_tile";
+    if (!h) return RF_ERR_INVALID_ARG;
+    if (!frame || !out) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL frame or output", who));
+    int rc = check_frames(h, who, frame, 1, matrix);
+    if (rc) return rc;
+    return preprocess_tile_impl<YuvPlanes>(h, who, frame->width, frame->height, t, tile, out,
+                                           [&](cudaStream_t s) { return upload_frame(h, s, *frame, matrix, 0); });
+}
+
 // ---- f1 ingest: compressed images (main.cpp:18-26 decodes on the host with cv::imread) ---------------------------------------
 int rf_detect_jpeg_batch(rf_handle h, const uint8_t *const *jpegs, const size_t *jpeg_bytes, int n, float thr, float nms, rf_face *out_faces,
                          int *out_counts, int32_t *out_idx, int *out_widths, int *out_heights) {
@@ -1152,21 +1341,20 @@ int rf_detect_views(rf_handle h, const uint8_t *bgr, int width, int height, int 
         // every view may contribute max_faces candidates to the merged list of the one image
         if (!h->pb_merge.cand_keys) alloc_post_buffers(h->pb_merge, h->cfg.max_batch * mf, 1, mf);
         const uint8_t *d_src = upload_raw(h, c.stream, bgr, width, height, rs);
-        ViewSet vs{};
-        vs.nviews = nviews;
-        vs.img_w_minus1 = (float)(width - 1);
         const int area = (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0;
         std::vector<LbItem> lb(nviews);
+        std::vector<MergeSource> ms(nviews);
         for (int v = 0; v < nviews; v++) {
             const int bw = std::max(1, (int)(Wn * views[v].shrink)), bh = std::max(1, (int)(Hn * views[v].shrink));
-            vs.flip[v] = views[v].flip ? 1 : 0;
-            vs.scale[v] = letterbox_fill(lb[v], d_src, width, height, h->d_input + (size_t)v * img_bytes, bw, bh, vs.flip[v], area);
-            if (out_view_scales) out_view_scales[v] = vs.scale[v];
+            const int flip = views[v].flip ? 1 : 0;
+            const float scale = letterbox_fill(lb[v], d_src, width, height, h->d_input + (size_t)v * img_bytes, bw, bh, flip, area);
+            ms[v] = view_source(v, mf, scale, flip, width);
+            if (out_view_scales) out_view_scales[v] = scale;
         }
         CK(launch_letterbox_batch(lb.data(), nviews, Wn, Hn, c.stream));     // all views of the image: one launch
         set_params(h, c, thr, nms);
         forward_graph(h, c, nviews);
-        launch_merge_views(c.pb, vs, h->pb_merge, c.stream);
+        CK(launch_merge(c.pb, ms.data(), nviews, Wn, Hn, h->pb_merge, c.stream));
         launch_nms(1, c.d_params, h->pb_merge, c.stream);
         CK(cudaMemcpyAsync(h->h_counts, h->pb_merge.out_counts, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
         CK(cudaMemcpyAsync(h->h_dets, h->pb_merge.out_dets, sizeof(rf_det) * (size_t)mf, cudaMemcpyDeviceToHost, c.stream));

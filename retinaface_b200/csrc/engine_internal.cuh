@@ -158,6 +158,7 @@ struct rf_handle_s {
     uint8_t *d_input = nullptr;       // [max_batch][H][W][3] u8 BGR
     uint8_t *h_input = nullptr;       // pinned mirror
     PostBuffers pb_merge{};           // rf_detect_views: candidates of all views of one image (lazily allocated)
+    PostBuffers pb_tiles{};           // rf_detect_tiled: candidates of all tiles of each image (lazily grown to the largest layout)
     uint8_t *d_raw = nullptr;         // one raw caller image (max_image) for the letterbox kernel
     uint8_t *h_raw = nullptr;         // pinned, TWO buffers of raw_bytes: staging of pageable caller images (upload_raw)
     size_t raw_bytes = 0;

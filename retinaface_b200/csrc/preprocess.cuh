@@ -20,6 +20,9 @@
 // (yuv.cuh), whose every tap -- identity, bilinear or super-sampling -- is converted to BGR before the unchanged resize
 // arithmetic, so the network input is byte for byte the letter-box of cv2.cvtColor(frame).
 #pragma once
+#include <string>
+#include <vector>
+
 #include "common.cuh"
 #include "yuv.cuh"
 
@@ -40,24 +43,43 @@ void letterbox_geometry(int w, int h, int net_w, int net_h, int *dw, int *dh, do
 // ... and the way imageROIResize8U3C + NPP do (resizeconvertion.cu:296-310): extent ceil(w f) x ceil(h f)
 void letterbox_geometry_npp(int w, int h, int net_w, int net_h, int *dw, int *dh, double *inv_scale);
 
+// The reference's own float `scale` of a letter-box into box_w x box_h (RetinaFace.cpp:587-591), the factor its map-back
+// multiplies by (:732-738).
+float letterbox_map_back(int w, int h, int box_w, int box_h);
+
 // Batched letter-box: ONE launch for up to LB_MAX_IMAGES BGR images (LB_MAX_FRAMES YUV frames) per call chunk, each with its
 // own source / destination buffer; 4 pixels (three 32-bit stores) per thread.  The items travel as __grid_constant__ kernel
 // parameters: a chunk of either kind stays within the classic 4 KB parameter limit (static_assert in preprocess.cu).
+// An item's output pixel (x, y) is pixel (x + x0, y + y0) of the whole resized image (dw x dh, zero beyond): origin 0 is the
+// letter-box, another origin cuts one tile out of a resized pyramid level (tile_fill below).  scale < 1 up-scales.
 constexpr int LB_MAX_IMAGES = 64, LB_MAX_FRAMES = 32;
+// cv::resize(INTER_LINEAR) at exactly 2x down-scaling runs OpenCV's fast INTER_AREA code, whose border rule differs from the
+// bilinear taps on a side of 3 mod 4.  Tile levels of scale 0.5 use it, so that they are the cv::resize the header promises; the
+// letter-box keeps its own bytes.
+constexpr int LB_HALF_AREA = 2;
 template <typename Src>
 struct LbItemT {
     using Source = Src;
     Src src; uint8_t *dst;
     int sw, sh, dw, dh;
     double scale;
-    int identity, flip, area;
+    int identity, flip, area;   // area: 0 bilinear, 1 NPP super-sampling, LB_HALF_AREA OpenCV's 2x fast area path (tiles only)
+    int16_t x0, y0;     // 16 bits keep 64 BGR items within 4 KB; origins are below the largest level side (16384)
 };
 using LbItem = LbItemT<const uint8_t *>;     // packed u8 BGR rows, w x h x 3
-using LbYuvItem = LbItemT<YuvPlanes>;        // a YUV 4:2:0 frame (flip unused: 0)
-// fills one item (geometry of either resize definition); returns the reference's map-back factor
+using LbYuvItem = LbItemT<YuvPlanes>;        // a YUV 4:2:0 frame
+// fills one item (geometry of either resize definition, origin 0); returns the reference's map-back factor
 template <typename Src>
 float letterbox_fill(LbItemT<Src> &it, typename LbItemT<Src>::Source src, int w, int h, uint8_t *dst, int box_w, int box_h, int flip, int area);
 template <typename Src>
 cudaError_t launch_letterbox_batch(const LbItemT<Src> *items, int n, int net_w, int net_h, cudaStream_t s);
+
+// ---- f7 tiles (rf_b200.h rf_tile_layout) ------------------------------------------------------------------------------------------
+// The one statement of the tile geometry: rf_tile_layout, the tiled detect paths and rf_preprocess_tile all call it.  Fills `out`
+// with every tile of a w x h image (t may be NULL) and returns RF_OK, or a status with the reason in *err.
+int tile_layout(int net_w, int net_h, int w, int h, const rf_tiling *t, std::vector<rf_tile> &out, std::string *err);
+// The letter-box item of one tile: the image's level resized, mirrored when the tile's level is, and cut at the tile's origin.
+template <typename Src>
+void tile_fill(LbItemT<Src> &it, typename LbItemT<Src>::Source src, int w, int h, uint8_t *dst, int net_w, int net_h, const rf_tile &tile);
 
 }  // namespace rf

@@ -71,6 +71,19 @@ class RetinaFace:
         faces, crops = out[0], out[1]
         return [[(FaceDetectInfo.from_row(r), c) for r, c in zip(f, cs)] for f, cs in zip(faces, crops)]
 
+    def detectTiled(self, imgs: Sequence[np.ndarray], threshold: float = 0.5, scales: Sequence[float] = None, flip: bool = False,
+                    overlap: int = 0) -> List[List[FaceDetectInfo]]:
+        """f7 small faces in large images: each image is resized to a pyramid of levels, every level cut into overlapping
+        network-sized tiles, the tiles detected as ordinary batches and the faces merged across tiles and levels on the GPU
+        (rf_detect_tiled).  Faces in ORIGINAL IMAGE pixels.  ``scales``: the levels (a scale may exceed 1; 0 is the letter-box of
+        ``detectBatchImages``), each also run mirrored with ``flip``; None: the default pyramid 1, 1/2, 1/4, ... down to the
+        letter-box; ``flip`` needs explicit ``scales`` (ValueError otherwise).  ``overlap``: pixels neighbouring tiles share (0: 64)."""
+        if flip and scales is None:
+            raise ValueError("detectTiled: flip mirrors the given scales; the default pyramid has no mirrored levels -- pass scales")
+        levels = None if scales is None else [(float(s), f) for s in scales for f in ((False, True) if flip else (False,))]
+        faces, _ = self.engine.detect_tiled(list(imgs), threshold, self.nms_threshold, levels=levels, overlap=overlap)
+        return [[FaceDetectInfo.from_row(r) for r in per] for per in faces]
+
     def detectInImage(self, img: np.ndarray, threshold: float = 0.5, scales: Sequence[float] = (1.0,), flip: bool = False
                       ) -> List[FaceDetectInfo]:
         """SURVEY.md 8f-2: what the reference leaves commented out / unused (RetinaFace.cpp:730-746, the `scales` argument of

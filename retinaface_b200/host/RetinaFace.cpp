@@ -189,6 +189,34 @@ void RetinaFace::detectYUV(const vector<Mat> &frames, int layout, float threshol
     }
 }
 
+void RetinaFace::detectTiled(const vector<Mat> &imgs, float threshold, const vector<float> &scales, bool flip, int overlap) {
+    if (flip && scales.empty()) throw std::invalid_argument("detectTiled: flip mirrors the given scales; the default pyramid has none");
+    last_.assign(imgs.size(), vector<FaceDetectInfo>());
+    scales_.assign(imgs.size(), 1.f);
+    crops_.assign(imgs.size(), vector<Mat>());
+    vector<rf_tile_level> levels;
+    for (float s : scales) {
+        levels.push_back(rf_tile_level{s, 0});
+        if (flip) levels.push_back(rf_tile_level{s, 1});
+    }
+    const rf_tiling t{levels.empty() ? nullptr : levels.data(), (int)levels.size(), overlap};
+    const size_t mb = (size_t)opt_.max_batch;
+    for (size_t start = 0; start < imgs.size(); start += mb) {
+        const int n = (int)std::min(mb, imgs.size() - start);
+        vector<const uint8_t *> ptrs(n);
+        vector<int> ws(n), hs(n), strides(n);
+        for (int i = 0; i < n; i++) {
+            const cv::Mat &m = imgs[start + i];
+            if (m.empty()) throw std::runtime_error("detectTiled: empty image");
+            ptrs[i] = m.data; ws[i] = m.cols; hs[i] = m.rows; strides[i] = (int)m.step;
+        }
+        int rc = rf_detect_tiled(h_, ptrs.data(), ws.data(), hs.data(), strides.data(), n, &t, threshold, nms_threshold, out_faces_.data(),
+                                 out_counts_.data(), nullptr);
+        if (rc != RF_OK) throw std::runtime_error(string("rf_detect_tiled: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+        keepResults(start, n, nullptr, 0, 0, 0);
+    }
+}
+
 vector<FaceDetectInfo> RetinaFace::detectInImage(const Mat &img, float threshold, const vector<float> &scales, bool flip) {
     vector<FaceDetectInfo> out;
     if (img.empty()) return out;

@@ -84,6 +84,14 @@ class RetinaFace {
     // with `align`, lastCrops() the crops as detectAndAlign leaves them.
     enum YuvLayout { YUV_NV12 = 0, YUV_NV21 = 1, YUV_I420 = 2, YUV_YV12 = 3 };
     void detectYUV(const vector<Mat> &frames, int layout, float threshold, const AlignOptions *align = nullptr);
+    // f7 small faces in large images (rf_detect_tiled): each image resized to a pyramid of levels, every level cut into overlapping
+    // network-sized tiles, merged across tiles and levels on the GPU.  `scales`: the levels (may exceed 1; 0 is the letter-box of
+    // detectBatchImages), each also mirrored with `flip`; empty: the default pyramid 1, 1/2, 1/4, ... down to the letter-box, which
+    // has no mirrored levels (`flip` with empty `scales` throws std::invalid_argument).
+    // `overlap`: pixels neighbouring tiles share (0: 64).  Afterwards lastBatchFaces() holds the faces in ORIGINAL IMAGE pixels
+    // (lastScale() is 1).
+    void detectTiled(const vector<Mat> &imgs, float threshold = 0.5, const vector<float> &scales = vector<float>(), bool flip = false,
+                     int overlap = 0);
     // the reference's visualisation (RetinaFace.cpp:730-741): red box outline (thickness 2), green landmark dots, on a clone
     static Mat draw(const Mat &img, const vector<FaceDetectInfo> &faces);
     int netWidth() const { return opt_.net_w; }

@@ -376,6 +376,40 @@ int rf_preprocess_yuv_tile(rf_handle h, const rf_yuv_frame *frame, int matrix, c
 int rf_preprocess_tile(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, const rf_tiling *t, int tile,
                        uint8_t *out_net_sized);
 
+/* f8 small faces in device-resident frames, with crops: the tiled detection of f7 on images or NVDEC surfaces already on the GPU,
+ * asynchronous, and the f5 crops of every kept face cut from the original image, so nothing leaves the GPU between the decoder and a
+ * recogniser's input tensor.  Faces are those rf_detect_tiled / rf_detect_yuv_tiled return for the same pixels, bit for bit: in
+ * ORIGINAL IMAGE (frame) pixels, best first.  Crops and matrices have the layout, formats, defaults and max_faces limit of
+ * rf_detect_align_batch(_device); each M maps image to crop and is fitted on the returned landmarks (map-back factor 1), and a u8
+ * crop is cv2.warpAffine(img, M, INTER_LINEAR, BORDER_CONSTANT) -- of cv2.cvtColor(frame) for YUV -- byte for byte.
+ * Statuses as rf_detect_tiled / rf_detect_yuv_tiled (NULL arrays, empty images, a row stride below 3 w, bad frame descriptors,
+ * rf_tile_layout's, an image above max_image, n > max_batch, RF_FLAG_NPP_RESIZE -> RF_ERR_UNSUPPORTED); bad align params, or align
+ * without out_crops / dev_crops: RF_ERR_INVALID_ARG; all before anything is launched.
+ *
+ * Host, blocking: rf_detect_tiled / rf_detect_yuv_tiled plus the crops (align required; out_crops [n][A][crop bytes], out_mats
+ * optional [n][A][6], host).  Every original stays resident in a raw buffer of its own until its crops are cut: more images than the
+ * handle has raw buffers is RF_ERR_CAPACITY (rf_detect_yuv_batch's rule). */
+int rf_detect_tiled_align(rf_handle h, const uint8_t *const *bgr_images, const int *widths, const int *heights, const int *row_strides,
+                          int n, const rf_tiling *t, float score_threshold, float nms_threshold, const rf_align_params *align,
+                          rf_face *out_faces, int *out_counts, int32_t *out_tile_of, void *out_crops, double *out_mats);
+int rf_detect_yuv_tiled_align(rf_handle h, const rf_yuv_frame *frames, int n, int matrix, const rf_tiling *t, float score_threshold,
+                              float nms_threshold, const rf_align_params *align, rf_face *out_faces, int *out_counts,
+                              int32_t *out_tile_of, void *out_crops, double *out_mats);
+/* Device, asynchronous: dev_bgr[i] (u8 BGR rows row_strides[i] bytes apart; NULL or 0: packed) or the frames' planes are DEVICE
+ * memory, read in place and never written; align may be NULL (no crops), else the crops go to dev_crops (required) and dev_mats
+ * (optional), device memory.  *dev_dets -> [max_batch][max_faces] rf_det, *dev_counts -> [max_batch] int32 (kept count, clamped to
+ * max_faces); anchor_index is the merge's candidate id, tile * max_faces + rank, so anchor_index / max_faces is the blocking paths'
+ * out_tile_of.  Detections, counts, crops and matrices are complete in stream order on rf_last_stream(); the caller keeps the frames
+ * alive and unmodified until that stream has passed the call.  The records live in a ring of `streams` output slots: the returned
+ * pointers stay valid until `streams` further tiled device calls.  Tiles run in chunks over the rf_detect_batch_device rotation as
+ * in rf_detect_tiled, each chunk counting as one call for that function's validity rule.  n = 0 launches nothing. */
+int rf_detect_tiled_device(rf_handle h, const uint8_t *const *dev_bgr, const int *widths, const int *heights, const int *row_strides,
+                           int n, const rf_tiling *t, float score_threshold, float nms_threshold, const rf_align_params *align,
+                           void *dev_crops, double *dev_mats, const rf_det **dev_dets, const int32_t **dev_counts);
+int rf_detect_yuv_tiled_device(rf_handle h, const rf_yuv_frame *frames, int n, int matrix, const rf_tiling *t, float score_threshold,
+                               float nms_threshold, const rf_align_params *align, void *dev_crops, double *dev_mats,
+                               const rf_det **dev_dets, const int32_t **dev_counts);
+
 /* Introspection. */
 int rf_get_net_size(rf_handle h, int *net_w, int *net_h, int *max_batch, int *max_faces);
 int rf_num_anchors(rf_handle h);            /* per image: 8,232 @448x448, 47,040 @1280x896 */

@@ -29,6 +29,7 @@ EXPORTS = [
     "rf_detect_align_batch", "rf_detect_align_batch_device",
     "rf_detect_yuv_batch", "rf_detect_yuv_batch_device", "rf_preprocess_yuv",
     "rf_tile_layout", "rf_detect_tiled", "rf_detect_yuv_tiled", "rf_preprocess_tile", "rf_preprocess_yuv_tile",
+    "rf_detect_tiled_align", "rf_detect_yuv_tiled_align", "rf_detect_tiled_device", "rf_detect_yuv_tiled_device",
 ]
 COMM_BLOB_BYTES = 128
 
@@ -272,6 +273,16 @@ def load_library() -> C.CDLL:
                                         C.c_void_p, C.c_void_p]
     lib.rf_preprocess_tile.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(Tiling), C.c_int, C.c_void_p]
     lib.rf_preprocess_yuv_tile.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_int, C.POINTER(Tiling), C.c_int, C.c_void_p]
+    lib.rf_detect_tiled_align.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int,
+                                          C.POINTER(Tiling), C.c_float, C.c_float, C.POINTER(AlignParams), C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_void_p]
+    lib.rf_detect_yuv_tiled_align.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_int, C.c_int, C.POINTER(Tiling), C.c_float, C.c_float,
+                                              C.POINTER(AlignParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.rf_detect_tiled_device.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int,
+                                           C.POINTER(Tiling), C.c_float, C.c_float, C.POINTER(AlignParams), C.c_void_p, C.c_void_p,
+                                           C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
+    lib.rf_detect_yuv_tiled_device.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_int, C.c_int, C.POINTER(Tiling), C.c_float, C.c_float,
+                                               C.POINTER(AlignParams), C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
     _lib = lib
     return lib
 
@@ -573,10 +584,30 @@ class Engine:
         return (np.empty((n, self.max_faces, FACE_FLOATS), dtype=np.float32), np.zeros(n, dtype=np.int32),
                 np.empty((n, self.max_faces), dtype=np.int32))
 
-    def detect_tiled(self, images: Sequence[np.ndarray], thr: float, nms_thr: float, levels=None, overlap: int = 0):
+    def _host_align(self, n: int, align: dict):
+        """rf_align_params and the host crop / matrix arrays of detect_yuv's align keywords: (params, A, crops, mats or None)."""
+        kw = dict(align)
+        want_mats = kw.pop("want_mats", False)
+        p = align_params(**{"fmt": "bgr_u8", **kw})
+        A = p.max_faces or self.max_faces
+        shape, dt = crop_shape(kw.get("fmt", "bgr_u8"), (p.crop_w, p.crop_h))
+        return p, A, np.empty((n, A) + shape, dtype=dt), (np.empty((n, A, 2, 3), dtype=np.float64) if want_mats else None)
+
+    @staticmethod
+    def _tiled_result(n, faces, counts, tile_of, A=0, crops=None, mats=None):
+        out = ([faces[i, :counts[i]].copy() for i in range(n)], [tile_of[i, :counts[i]].copy() for i in range(n)])
+        if crops is not None:
+            out += ([crops[i, :min(counts[i], A)].copy() for i in range(n)],)
+            if mats is not None:
+                out += ([mats[i, :min(counts[i], A)].copy() for i in range(n)],)
+        return out
+
+    def detect_tiled(self, images: Sequence[np.ndarray], thr: float, nms_thr: float, levels=None, overlap: int = 0, align: Optional[dict] = None):
         """rf_detect_tiled: u8 BGR HWC images (any size <= max_image; rows may be strided) cut into tiles of a scale pyramid
         (levels: [(scale, flip), ...], scale 0 = the fitted level; None = the default pyramid).  Returns (faces: one (k, 15) float32
-        array per image in ORIGINAL IMAGE pixels, tile_of: one (k,) array per image, indices into tile_layout)."""
+        array per image in ORIGINAL IMAGE pixels, tile_of: one (k,) array per image, indices into tile_layout).  align: detect_align's
+        keywords (crop, template, fmt, max_faces, mean, std, want_mats) -> rf_detect_tiled_align, and the crops (and matrices) follow:
+        (faces, tile_of, crops[, mats]) as detect_align returns them."""
         n = len(images)
         keep = [self._bgr_strided(im) for im in images]
         ptrs = (C.c_void_p * max(n, 1))(*[im.ctypes.data for im in keep])
@@ -585,19 +616,75 @@ class Engine:
         rs = (C.c_int * max(n, 1))(*[im.strides[0] for im in keep])
         t = tiling(levels, overlap)
         faces, counts, tile_of = self._tiled_out(n)
-        self._check(self.lib.rf_detect_tiled(self.h, ptrs, ws, hs, rs, n, C.byref(t), thr, nms_thr, faces.ctypes.data, counts.ctypes.data,
-                                             tile_of.ctypes.data))
-        return [faces[i, :counts[i]].copy() for i in range(n)], [tile_of[i, :counts[i]].copy() for i in range(n)]
+        if align is None:
+            self._check(self.lib.rf_detect_tiled(self.h, ptrs, ws, hs, rs, n, C.byref(t), thr, nms_thr, faces.ctypes.data, counts.ctypes.data,
+                                                 tile_of.ctypes.data))
+            return self._tiled_result(n, faces, counts, tile_of)
+        p, A, crops, mats = self._host_align(n, align)
+        self._check(self.lib.rf_detect_tiled_align(self.h, ptrs, ws, hs, rs, n, C.byref(t), thr, nms_thr, C.byref(p), faces.ctypes.data,
+                                                   counts.ctypes.data, tile_of.ctypes.data, crops.ctypes.data,
+                                                   mats.ctypes.data if mats is not None else None))
+        return self._tiled_result(n, faces, counts, tile_of, A, crops, mats)
 
-    def detect_yuv_tiled(self, frames, thr: float, nms_thr: float, layout: str = "nv12", matrix="bt601", levels=None, overlap: int = 0):
-        """rf_detect_yuv_tiled: host 4:2:0 frames (yuv_frame's forms) -> (faces, tile_of) as detect_tiled, in FRAME pixels."""
+    def detect_yuv_tiled(self, frames, thr: float, nms_thr: float, layout: str = "nv12", matrix="bt601", levels=None, overlap: int = 0,
+                         align: Optional[dict] = None):
+        """rf_detect_yuv_tiled: host 4:2:0 frames (yuv_frame's forms) -> (faces, tile_of) as detect_tiled, in FRAME pixels; with align,
+        rf_detect_yuv_tiled_align and (faces, tile_of, crops[, mats]) as detect_tiled."""
         n = len(frames)
         arr = self._frames(frames, layout, False)
         t = tiling(levels, overlap)
         faces, counts, tile_of = self._tiled_out(n)
-        self._check(self.lib.rf_detect_yuv_tiled(self.h, arr, n, _matrix(matrix), C.byref(t), thr, nms_thr, faces.ctypes.data,
-                                                 counts.ctypes.data, tile_of.ctypes.data))
-        return [faces[i, :counts[i]].copy() for i in range(n)], [tile_of[i, :counts[i]].copy() for i in range(n)]
+        if align is None:
+            self._check(self.lib.rf_detect_yuv_tiled(self.h, arr, n, _matrix(matrix), C.byref(t), thr, nms_thr, faces.ctypes.data,
+                                                     counts.ctypes.data, tile_of.ctypes.data))
+            return self._tiled_result(n, faces, counts, tile_of)
+        p, A, crops, mats = self._host_align(n, align)
+        self._check(self.lib.rf_detect_yuv_tiled_align(self.h, arr, n, _matrix(matrix), C.byref(t), thr, nms_thr, C.byref(p), faces.ctypes.data,
+                                                       counts.ctypes.data, tile_of.ctypes.data, crops.ctypes.data,
+                                                       mats.ctypes.data if mats is not None else None))
+        return self._tiled_result(n, faces, counts, tile_of, A, crops, mats)
+
+    @staticmethod
+    def _device_images(images):
+        """(pointers, widths, heights, row strides) of u8 BGR HWC torch CUDA tensors with contiguous pixels; the row stride is
+        stride(0), so a slice of a larger tensor is read in place."""
+        n = len(images)
+        for im in images:
+            if not (hasattr(im, "data_ptr") and getattr(im, "is_cuda", False)):
+                raise ValueError(f"device images must be torch CUDA tensors, got {type(im).__name__}")
+            if (str(im.dtype) != "torch.uint8" or im.dim() != 3 or im.shape[2] != 3 or im.stride(2) != 1 or im.stride(1) != 3
+                    or im.stride(0) < 3 * im.shape[1]):
+                raise ValueError(f"u8 BGR HWC tensor with contiguous pixels expected, got {tuple(im.shape)} {im.dtype} strides {im.stride()}")
+        return ((C.c_void_p * max(n, 1))(*[im.data_ptr() for im in images]), (C.c_int * max(n, 1))(*[im.shape[1] for im in images]),
+                (C.c_int * max(n, 1))(*[im.shape[0] for im in images]), (C.c_int * max(n, 1))(*[im.stride(0) for im in images]))
+
+    def detect_tiled_device(self, images, thr: float, nms_thr: float, levels=None, overlap: int = 0, align: Optional[dict] = None,
+                            dev_crops_ptr: Optional[int] = None, dev_mats_ptr: Optional[int] = None):
+        """rf_detect_tiled_device: u8 BGR HWC torch CUDA tensors (rows may be strided), tiled as detect_tiled, asynchronous on
+        last_stream_ptr().  Returns the (dets_ptr, counts_ptr) device addresses: [max_batch][max_faces] rf_det in ORIGINAL IMAGE pixels,
+        anchor_index = tile * max_faces + rank, valid for `streams` further tiled device calls.  align: detect_align's keywords; the
+        crops land at dev_crops_ptr as in detect_align_device.  Host arrays: ValueError."""
+        n = len(images)
+        ptrs, ws, hs, rs = self._device_images(images)
+        t = tiling(levels, overlap)
+        p = align_params(**align) if align is not None else None
+        d, c = C.c_void_p(), C.c_void_p()
+        self._check(self.lib.rf_detect_tiled_device(self.h, ptrs, ws, hs, rs, n, C.byref(t), thr, nms_thr, C.byref(p) if p is not None else None,
+                                                    dev_crops_ptr, dev_mats_ptr, C.byref(d), C.byref(c)))
+        return int(d.value or 0), int(c.value or 0)
+
+    def detect_yuv_tiled_device(self, frames, thr: float, nms_thr: float, layout: str = "nv12", matrix="bt601", levels=None, overlap: int = 0,
+                                align: Optional[dict] = None, dev_crops_ptr: Optional[int] = None, dev_mats_ptr: Optional[int] = None):
+        """rf_detect_yuv_tiled_device: device 4:2:0 frames (torch CUDA tensors in yuv_frame's forms), otherwise as detect_tiled_device
+        (faces in FRAME pixels).  Host frames: ValueError."""
+        n = len(frames)
+        arr = self._frames(frames, layout, True)
+        t = tiling(levels, overlap)
+        p = align_params(**align) if align is not None else None
+        d, c = C.c_void_p(), C.c_void_p()
+        self._check(self.lib.rf_detect_yuv_tiled_device(self.h, arr, n, _matrix(matrix), C.byref(t), thr, nms_thr,
+                                                        C.byref(p) if p is not None else None, dev_crops_ptr, dev_mats_ptr, C.byref(d), C.byref(c)))
+        return int(d.value or 0), int(c.value or 0)
 
     def preprocess_tile(self, img: np.ndarray, tile: int, levels=None, overlap: int = 0) -> np.ndarray:
         """rf_preprocess_tile: tile `tile` of the image's layout as the network sees it, (H, W, 3) u8 BGR."""

@@ -85,7 +85,9 @@ __device__ __forceinline__ void sample(const Img &im, int X, int Y, int v[3]) {
 // Where the kernel finds image i: the BGR table / uniform net-sized images of AlignArgs, or the frame table parameter.
 struct BgrImages {};
 struct YuvFrames { AlignYuvImage img[ALIGN_MAX_FRAMES]; };
+struct BgrTable { AlignImage img[ALIGN_MAX_FRAMES]; };     // f8: BGR images whose table travels as a kernel parameter
 static_assert(sizeof(AlignArgs) + sizeof(YuvFrames) + 32 <= 4096, "align launch exceeds the classic 4 KB kernel parameter space");
+static_assert(sizeof(AlignArgs) + sizeof(BgrTable) + 32 <= 4096, "align launch exceeds the classic 4 KB kernel parameter space");
 
 __device__ __forceinline__ AlignImage image_of(const AlignArgs &a, const BgrImages &, int i) {
     AlignImage im;
@@ -98,6 +100,7 @@ __device__ __forceinline__ AlignImage image_of(const AlignArgs &a, const BgrImag
     return im;
 }
 __device__ __forceinline__ AlignYuvImage image_of(const AlignArgs &, const YuvFrames &f, int i) { return f.img[i]; }
+__device__ __forceinline__ AlignImage image_of(const AlignArgs &, const BgrTable &t, int i) { return t.img[i]; }
 
 // Four consecutive pixels of one crop row (x4 .. x4 + 3, those < cw valid).  Vector stores where the address allows.
 __device__ __forceinline__ void store_quad(const AlignArgs &a, unsigned char *crop, int y, int x4, const int v[4][3]) {
@@ -230,6 +233,27 @@ __global__ void __launch_bounds__(ALIGN_THREADS) k_align_faces(const AlignArgs a
     }
 }
 
+// Chunk i0 is its own launch over images [i0, i0 + m), whose table (Table: YuvFrames or BgrTable) is a kernel parameter: the
+// same kernel on offset records, counts, crops and matrices.
+template <typename Table, typename Img>
+cudaError_t launch_table(const AlignArgs &a, const Img *images, const PostBuffers &pb, int num_sms, cudaStream_t s) {
+    if (a.n <= 0 || a.max_align <= 0) return cudaSuccess;
+    for (int i0 = 0; i0 < a.n; i0 += ALIGN_MAX_FRAMES) {
+        const int m = std::min(ALIGN_MAX_FRAMES, a.n - i0);
+        AlignArgs c = a;
+        c.n = m;
+        c.crops = static_cast<unsigned char *>(a.crops) + (size_t)i0 * a.max_align * a.crop_bytes;
+        if (a.mats) c.mats = a.mats + (size_t)i0 * a.max_align * 6;
+        Table t{};
+        for (int i = 0; i < m; i++) t.img[i] = images[i0 + i];
+        k_align_faces<<<2 * num_sms, ALIGN_THREADS, sizeof(int) * m, s>>>(c, t, pb.out_dets + (size_t)i0 * pb.max_faces, pb.out_counts + i0,
+                                                                        pb.max_faces);
+        cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
+}
+
 }  // namespace
 
 cudaError_t launch_align_faces(const AlignArgs &a, const PostBuffers &pb, int num_sms, cudaStream_t s) {
@@ -241,22 +265,11 @@ cudaError_t launch_align_faces(const AlignArgs &a, const PostBuffers &pb, int nu
 }
 
 cudaError_t launch_align_faces_yuv(const AlignArgs &a, const AlignYuvImage *frames, const PostBuffers &pb, int num_sms, cudaStream_t s) {
-    if (a.n <= 0 || a.max_align <= 0) return cudaSuccess;
-    // chunk i0 is its own launch over frames [i0, i0 + m): the same kernel on offset records, counts, crops and matrices
-    for (int i0 = 0; i0 < a.n; i0 += ALIGN_MAX_FRAMES) {
-        const int m = std::min(ALIGN_MAX_FRAMES, a.n - i0);
-        AlignArgs c = a;
-        c.n = m;
-        c.crops = static_cast<unsigned char *>(a.crops) + (size_t)i0 * a.max_align * a.crop_bytes;
-        if (a.mats) c.mats = a.mats + (size_t)i0 * a.max_align * 6;
-        YuvFrames f{};
-        for (int i = 0; i < m; i++) f.img[i] = frames[i0 + i];
-        k_align_faces<<<2 * num_sms, ALIGN_THREADS, sizeof(int) * m, s>>>(c, f, pb.out_dets + (size_t)i0 * pb.max_faces, pb.out_counts + i0,
-                                                                        pb.max_faces);
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return e;
-    }
-    return cudaSuccess;
+    return launch_table<YuvFrames>(a, frames, pb, num_sms, s);
+}
+
+cudaError_t launch_align_faces(const AlignArgs &a, const AlignImage *images, const PostBuffers &pb, int num_sms, cudaStream_t s) {
+    return launch_table<BgrTable>(a, images, pb, num_sms, s);
 }
 
 }  // namespace rf

@@ -51,5 +51,9 @@ cudaError_t launch_align_faces(const AlignArgs &a, const PostBuffers &pb, int nu
 // The same over a.n YUV frames [n]: the frame table travels as a kernel parameter (no host table a later call could rewrite
 // before the copy ran), one launch per ALIGN_MAX_FRAMES frames.
 cudaError_t launch_align_faces_yuv(const AlignArgs &a, const AlignYuvImage *frames, const PostBuffers &pb, int num_sms, cudaStream_t s);
+// f8: the same over a.n BGR images [n] (a.images / a.uniform_* unused), the table a kernel parameter as the frames are above: an
+// asynchronous call cannot have its table rewritten by a later one.  The tiled paths pass scale 1 (their records are already in
+// image pixels; __fmul_rn(l, 1.f) is exact).
+cudaError_t launch_align_faces(const AlignArgs &a, const AlignImage *images, const PostBuffers &pb, int num_sms, cudaStream_t s);
 
 }  // namespace rf

@@ -239,6 +239,11 @@ void destroy(rf_handle h) {
     for (Ctx &c : h->ctx) release_ctx(c, true);
     free_post_buffers(h->pb_merge);
     free_post_buffers(h->pb_tiles);
+    for (auto &s : h->tiled_slots) {
+        free_post_buffers(s.pb);
+        if (s.free) cudaEventDestroy(s.free);
+        if (s.start) cudaEventDestroy(s.start);
+    }
     cudaFree(h->d_weights); cudaFree(h->d_weights_h); cudaFree(h->d_weights_q); cudaFree(h->d_input); cudaFree(h->d_raw);
     for (auto p : h->d_blobs) cudaFree(p);
     h->copy_pool.reset();
@@ -975,31 +980,27 @@ static int tiled_layouts(rf_handle h, const char *who, int n, const int *widths,
     return RF_OK;
 }
 
-// Tiled detection of n images whose layouts are checked.  upload(s, i, slot) brings image i into raw buffer `slot` on stream s and
-// returns the letter-box source.  Context 0 uploads up to raw_slots images at a time; their tiles are letter-boxed, detected and
-// merged in chunks of up to max_batch, each chunk on the next context of the rf_detect_batch_device rotation, into that context's
-// own input tensor.  Before the next group overwrites the raw buffers -- and before the final NMS -- context 0 waits for every
-// context the group used.
+// Tiled detection of n images whose layouts are checked, into `dst` (its candidate lists empty: allocation and every k_nms leave
+// them so), the final NMS on `home`.  source(s, i, slot) returns the letter-box source of image i; the blocking paths upload it
+// into raw buffer `slot` on s, a `group` of raw buffers at a time, the device paths return the caller's memory (one group).  The
+// tiles are letter-boxed, detected and merged in chunks of up to max_batch, each chunk on the next context of the
+// rf_detect_batch_device rotation, into that context's own input tensor.  Another context waits for `ready` -- recorded on home
+// once the group's sources are on the device and `dst` may be written -- before its first letter-box of the group, or, with
+// `in_place` (the sources are the caller's device memory), only before its first merge.  Home waits for every context the group
+// used before the next group overwrites the raw buffers, and before the final NMS.
 extern "C++" {
-template <typename Src, typename Upload>
+template <typename Src, typename Source>
 static void detect_tiled_impl(rf_handle h, int n, const int *widths, const int *heights, const std::vector<std::vector<rf_tile>> &layouts,
-                              Upload upload, float thr, float nms, rf_face *out_faces, int *out_counts, int32_t *out_tile_of) {
+                              Source source, int group, bool in_place, Ctx &home, cudaEvent_t ready, PostBuffers &dst, float thr, float nms,
+                              std::vector<Src> &src) {
     const int Hn = h->cfg.net_h, Wn = h->cfg.net_w, mf = h->cfg.max_faces, B = h->cfg.max_batch;
     const size_t img_bytes = (size_t)Hn * Wn * 3;
-    size_t most = 0;
-    for (const auto &l : layouts) most = std::max(most, l.size());
-    // every tile of an image may contribute max_faces candidates to the image's merged list
-    if ((size_t)h->pb_tiles.anchors_per_image < most * mf) {
-        free_post_buffers(h->pb_tiles);
-        alloc_post_buffers(h->pb_tiles, (int)(most * mf), B, mf);
-    }
-    Ctx &c0 = h->ctx[0];
-    std::vector<Src> src(n);
+    src.resize(n);
     struct TileRef { int image, tile; };
-    for (int g0 = 0; g0 < n; g0 += h->raw_slots) {
-        const int g1 = std::min(n, g0 + h->raw_slots);
-        for (int i = g0; i < g1; i++) src[i] = upload(c0.stream, i, i - g0);
-        CK(cudaEventRecord(c0.fence, c0.stream));     // the raw images of this group are on the device
+    for (int g0 = 0; g0 < n; g0 += group) {
+        const int g1 = std::min(n, g0 + group);
+        for (int i = g0; i < g1; i++) src[i] = source(home.stream, i, i - g0);
+        CK(cudaEventRecord(ready, home.stream));
         std::vector<TileRef> refs;
         for (int i = g0; i < g1; i++)
             for (int k = 0; k < (int)layouts[i].size(); k++) refs.push_back(TileRef{i, k});
@@ -1008,7 +1009,8 @@ static void detect_tiled_impl(rf_handle h, int n, const int *widths, const int *
             const int m = (int)std::min<size_t>(B, refs.size() - k0);
             const size_t ci = h->next_dev_ctx++ % h->ctx.size();
             Ctx &c = h->ctx[ci];
-            if (ci != 0 && !joined[ci]) CK(cudaStreamWaitEvent(c.stream, c0.fence, 0));
+            const bool wait = &c != &home && !joined[ci];
+            if (wait && !in_place) CK(cudaStreamWaitEvent(c.stream, ready, 0));
             joined[ci] = 1;
             if (!c.d_frames_in) CK(cudaMalloc(&c.d_frames_in, (size_t)B * img_bytes));
             if (c.param_seq && c.param_seq % Ctx::kParamSlots == 0) CK(cudaStreamSynchronize(c.stream));
@@ -1023,29 +1025,133 @@ static void detect_tiled_impl(rf_handle h, int n, const int *widths, const int *
             CK(launch_letterbox_batch(lb.data(), m, Wn, Hn, c.stream));
             set_params(h, c, thr, nms, c.d_frames_in);
             forward_graph(h, c, m);
-            CK(launch_merge(c.pb, ms.data(), m, Wn, Hn, h->pb_tiles, c.stream));
+            if (wait && in_place) CK(cudaStreamWaitEvent(c.stream, ready, 0));
+            CK(launch_merge(c.pb, ms.data(), m, Wn, Hn, dst, c.stream));
         }
-        for (size_t ci = 1; ci < h->ctx.size(); ci++) {
-            if (!joined[ci]) continue;
+        for (size_t ci = 0; ci < h->ctx.size(); ci++) {
+            if (!joined[ci] || &h->ctx[ci] == &home) continue;
             CK(cudaEventRecord(h->ctx[ci].fence, h->ctx[ci].stream));
-            CK(cudaStreamWaitEvent(c0.stream, h->ctx[ci].fence, 0));
+            CK(cudaStreamWaitEvent(home.stream, h->ctx[ci].fence, 0));
         }
     }
-    // the final NMS over each image's candidates from all its tiles and levels reads its threshold from context 0's parameters
-    if (c0.param_seq && c0.param_seq % Ctx::kParamSlots == 0) CK(cudaStreamSynchronize(c0.stream));
-    set_params(h, c0, thr, nms);
-    launch_nms(n, c0.d_params, h->pb_tiles, c0.stream);
+    // the final NMS over each image's candidates from all its tiles and levels reads its threshold from home's parameters
+    if (home.param_seq && home.param_seq % Ctx::kParamSlots == 0) CK(cudaStreamSynchronize(home.stream));
+    set_params(h, home, thr, nms);
+    launch_nms(n, home.d_params, dst, home.stream);
     CK(cudaGetLastError());
+}
+}  // extern "C++"
+
+// Makes room in pb for the candidates of the largest layout: every tile of an image may contribute max_faces.
+static bool tiled_grow(rf_handle h, PostBuffers &pb, const std::vector<std::vector<rf_tile>> &layouts) {
+    size_t most = 0;
+    for (const auto &l : layouts) most = std::max(most, l.size());
+    const int mf = h->cfg.max_faces;
+    if ((size_t)pb.anchors_per_image >= most * mf) return false;
+    free_post_buffers(pb);
+    alloc_post_buffers(pb, (int)(most * mf), h->cfg.max_batch, mf);
+    return true;
+}
+
+// The crop source of a tiled path's image i: its original, at map-back factor 1 (the merged records are in image pixels).
+extern "C++" {
+static AlignImage align_source(const uint8_t *p, int w, int hgt) { return AlignImage{p, w, hgt, w * 3, 1.f}; }
+static AlignImage align_source(const BgrRows &r, int w, int hgt) { return AlignImage{r.p, w, hgt, r.pitch, 1.f}; }
+static AlignYuvImage align_source(const YuvPlanes &p, int w, int hgt) { return AlignYuvImage{p, w, hgt, 1.f}; }
+static cudaError_t launch_align_table(const AlignArgs &a, const std::vector<AlignImage> &im, const PostBuffers &pb, int sms, cudaStream_t s) {
+    return launch_align_faces(a, im.data(), pb, sms, s);
+}
+static cudaError_t launch_align_table(const AlignArgs &a, const std::vector<AlignYuvImage> &im, const PostBuffers &pb, int sms, cudaStream_t s) {
+    return launch_align_faces_yuv(a, im.data(), pb, sms, s);
+}
+
+
+// The crops of every kept face in pb (a.crops / a.mats set by the caller), cut on s from the originals src.
+template <typename Src>
+static void tiled_crops(rf_handle h, AlignArgs a, int n, const int *widths, const int *heights, const std::vector<Src> &src, const PostBuffers &pb,
+                        cudaStream_t s) {
+    std::vector<decltype(align_source(src[0], 0, 0))> im(n);
+    for (int i = 0; i < n; i++) im[i] = align_source(src[i], widths[i], heights[i]);
+    a.n = n;
+    CK(launch_align_table(a, im, pb, h->num_sms, s));
+}
+
+// The blocking tiled paths: sources uploaded on context 0, merged into pb_tiles, fetched.  With `a` (the call has checked that
+// every image gets a raw buffer of its own, so all originals stay resident), the crops are cut on context 0 after the NMS and
+// copied out with the faces.
+template <typename Src, typename Upload>
+static void detect_tiled_blocking(rf_handle h, int n, const int *widths, const int *heights, const std::vector<std::vector<rf_tile>> &layouts,
+                                  Upload upload, float thr, float nms, const AlignArgs *a, rf_face *out_faces, int *out_counts,
+                                  int32_t *out_tile_of, void *out_crops, double *out_mats) {
+    const int mf = h->cfg.max_faces;
+    tiled_grow(h, h->pb_tiles, layouts);
+    Ctx &c0 = h->ctx[0];
+    std::vector<Src> src;
+    detect_tiled_impl<Src>(h, n, widths, heights, layouts, upload, h->raw_slots, false, c0, c0.fence, h->pb_tiles, thr, nms, src);
+    AlignArgs aa{};
+    if (a) {
+        ensure_align_buffers(h, n, *a);
+        aa = *a;
+        aa.n = n;
+        aa.crops = h->d_align_crops;
+        aa.mats = out_mats ? h->d_align_mats : nullptr;
+        tiled_crops(h, aa, n, widths, heights, src, h->pb_tiles, c0.stream);
+    }
     fetch_post(h, h->pb_tiles, c0.stream, n, out_faces, out_counts, out_tile_of);
     if (out_tile_of)      // candidate id = tile * max_faces + rank
         for (int i = 0; i < n; i++)
             for (int j = 0; j < std::min(h->h_counts[i], mf); j++) out_tile_of[(size_t)i * mf + j] /= mf;
+    if (a) put_mapped(h, c0, n, [](int) { return 1.f; }, &aa, nullptr, out_crops, out_mats);
+}
+
+// The asynchronous tiled paths: the caller's device sources src[i] read in place, merged into the next slot of the ring, the final
+// NMS and the crops on the home stream (the context the call's first chunk lands on), which rf_last_stream returns.
+//   1. Home waits for the slot's `free` event before anything merges into it and records `start`; every other context waits for
+//      `start` before its first merge (k_nms left the slot's candidate counts at zero).
+//   2. A slot that must grow is freed only after the host has waited for `free`, and its counts are cleared on home before `start`.
+//   3. Home joins every context it used through their fence events before the NMS.
+//   4. The crops are cut on home after the NMS; then `free` is recorded.
+template <typename Src>
+static void detect_tiled_device(rf_handle h, int n, const int *widths, const int *heights, const std::vector<std::vector<rf_tile>> &layouts,
+                                const std::vector<Src> &dev_src, float thr, float nms, const AlignArgs *a, void *dev_crops, double *dev_mats,
+                                const rf_det **dev_dets, const int32_t **dev_counts) {
+    if (h->tiled_slots.empty()) {
+        h->tiled_slots.resize(h->ctx.size());
+        for (auto &s : h->tiled_slots) {
+            CK(cudaEventCreateWithFlags(&s.free, cudaEventDisableTiming));
+            CK(cudaEventCreateWithFlags(&s.start, cudaEventDisableTiming));
+        }
+    }
+    rf_handle_s::TiledSlot &slot = h->tiled_slots[h->next_tiled_slot++ % h->tiled_slots.size()];
+    Ctx &home = h->ctx[h->next_dev_ctx % h->ctx.size()];
+    size_t most = 0;
+    for (const auto &l : layouts) most = std::max(most, l.size());
+    if ((size_t)slot.pb.anchors_per_image < most * h->cfg.max_faces) {
+        CK(cudaEventSynchronize(slot.free));     // the slot's last call has finished with the buffers about to be freed
+        tiled_grow(h, slot.pb, layouts);
+        // alloc_post_buffers clears the counts on the legacy stream, which the contexts' streams do not wait for
+        CK(cudaMemsetAsync(slot.pb.cand_count, 0, sizeof(int) * slot.pb.max_batch, home.stream));
+    }
+    CK(cudaStreamWaitEvent(home.stream, slot.free, 0));
+    std::vector<Src> src;
+    detect_tiled_impl<Src>(h, n, widths, heights, layouts, [&](cudaStream_t, int i, int) { return dev_src[i]; }, n, true, home, slot.start,
+                           slot.pb, thr, nms, src);
+    if (a) {
+        AlignArgs aa = *a;
+        aa.crops = dev_crops;
+        aa.mats = dev_mats;
+        tiled_crops(h, aa, n, widths, heights, src, slot.pb, home.stream);
+    }
+    CK(cudaEventRecord(slot.free, home.stream));
+    h->last_stream = home.stream;
+    if (dev_dets) *dev_dets = slot.pb.out_dets;
+    if (dev_counts) *dev_counts = slot.pb.out_counts;
 }
 }  // extern "C++"
 
-int rf_detect_tiled(rf_handle h, const uint8_t *const *imgs, const int *widths, const int *heights, const int *row_strides, int n,
-                    const rf_tiling *t, float thr, float nms, rf_face *out_faces, int *out_counts, int32_t *out_tile_of) {
-    static const char *who = "rf_detect_tiled";
+// Checks of the BGR tiled entry points, before the layouts: NULL arrays, empty images, row strides below 3 w, images above max_image.
+static int check_tiled_images(rf_handle h, const char *who, const uint8_t *const *imgs, const int *widths, const int *heights,
+                              const int *row_strides, int n) {
     int rc = check_n(h, n);
     if (rc) return rc;
     if (n > 0 && (!imgs || !widths || !heights)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL image arrays", who));
@@ -1057,8 +1163,30 @@ int rf_detect_tiled(rf_handle h, const uint8_t *const *imgs, const int *widths, 
             return fail(h, RF_ERR_CAPACITY, fmt("%s: image %d is %dx%d, larger than max_image %dx%d", who, i, widths[i], heights[i],
                                                 h->cfg.max_image_w, h->cfg.max_image_h));
     }
+    return RF_OK;
+}
+
+// Checks of the align arguments of a tiled entry point (after its image checks): the params, somewhere for the crops to go, and --
+// for the blocking variants (`resident`) -- a raw buffer for every original until the crops are cut.
+static int check_tiled_align(rf_handle h, const char *who, const rf_align_params *align, int n, const void *crops, bool resident, AlignArgs &a) {
+    int rc = align_setup(h, who, align, a);
+    if (rc) return rc;
+    if (n > 0 && !crops) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: align without %s", who, resident ? "out_crops" : "dev_crops"));
+    if (resident && n > h->raw_slots)
+        return fail(h, RF_ERR_CAPACITY, fmt("%s: %d images to align, but the handle keeps at most %d resident (one %dx%d raw buffer each); split "
+                                            "the batch", who, n, h->raw_slots, h->cfg.max_image_w, h->cfg.max_image_h));
+    return RF_OK;
+}
+
+static int tiled_bgr(rf_handle h, const char *who, const uint8_t *const *imgs, const int *widths, const int *heights, const int *row_strides, int n,
+                     const rf_tiling *t, float thr, float nms, bool aligned, const rf_align_params *align, rf_face *out_faces, int *out_counts,
+                     int32_t *out_tile_of, void *out_crops, double *out_mats) {
+    int rc = check_tiled_images(h, who, imgs, widths, heights, row_strides, n);
+    if (rc) return rc;
     std::vector<std::vector<rf_tile>> layouts;
     if ((rc = tiled_layouts(h, who, n, widths, heights, t, layouts))) return rc;
+    AlignArgs a;
+    if (aligned && (rc = check_tiled_align(h, who, align, n, out_crops, true, a))) return rc;
     if (n == 0) return RF_OK;
     try {
         CK(cudaSetDevice(h->device));
@@ -1066,25 +1194,97 @@ int rf_detect_tiled(rf_handle h, const uint8_t *const *imgs, const int *widths, 
             const int rs = row_strides && row_strides[i] ? row_strides[i] : widths[i] * 3;
             return upload_raw(h, s, imgs[i], widths[i], heights[i], rs, slot);
         };
-        detect_tiled_impl<const uint8_t *>(h, n, widths, heights, layouts, upload, thr, nms, out_faces, out_counts, out_tile_of);
+        detect_tiled_blocking<const uint8_t *>(h, n, widths, heights, layouts, upload, thr, nms, aligned ? &a : nullptr, out_faces, out_counts,
+                                               out_tile_of, out_crops, out_mats);
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }
 
-int rf_detect_yuv_tiled(rf_handle h, const rf_yuv_frame *frames, int n, int matrix, const rf_tiling *t, float thr, float nms,
-                        rf_face *out_faces, int *out_counts, int32_t *out_tile_of) {
-    static const char *who = "rf_detect_yuv_tiled";
+static int tiled_yuv(rf_handle h, const char *who, const rf_yuv_frame *frames, int n, int matrix, const rf_tiling *t, float thr, float nms,
+                     bool aligned, const rf_align_params *align, rf_face *out_faces, int *out_counts, int32_t *out_tile_of, void *out_crops,
+                     double *out_mats) {
     int rc = check_frames(h, who, frames, n, matrix);
     if (rc) return rc;
     std::vector<int> widths(n), heights(n);
     for (int i = 0; i < n; i++) { widths[i] = frames[i].width; heights[i] = frames[i].height; }
     std::vector<std::vector<rf_tile>> layouts;
     if ((rc = tiled_layouts(h, who, n, widths.data(), heights.data(), t, layouts))) return rc;
+    AlignArgs a;
+    if (aligned && (rc = check_tiled_align(h, who, align, n, out_crops, true, a))) return rc;
     if (n == 0) return RF_OK;
     try {
         CK(cudaSetDevice(h->device));
         auto upload = [&](cudaStream_t s, int i, int slot) { return upload_frame(h, s, frames[i], matrix, slot); };
-        detect_tiled_impl<YuvPlanes>(h, n, widths.data(), heights.data(), layouts, upload, thr, nms, out_faces, out_counts, out_tile_of);
+        detect_tiled_blocking<YuvPlanes>(h, n, widths.data(), heights.data(), layouts, upload, thr, nms, aligned ? &a : nullptr, out_faces,
+                                         out_counts, out_tile_of, out_crops, out_mats);
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
+}
+
+int rf_detect_tiled(rf_handle h, const uint8_t *const *imgs, const int *widths, const int *heights, const int *row_strides, int n,
+                    const rf_tiling *t, float thr, float nms, rf_face *out_faces, int *out_counts, int32_t *out_tile_of) {
+    return tiled_bgr(h, "rf_detect_tiled", imgs, widths, heights, row_strides, n, t, thr, nms, false, nullptr, out_faces, out_counts, out_tile_of,
+                     nullptr, nullptr);
+}
+
+int rf_detect_yuv_tiled(rf_handle h, const rf_yuv_frame *frames, int n, int matrix, const rf_tiling *t, float thr, float nms,
+                        rf_face *out_faces, int *out_counts, int32_t *out_tile_of) {
+    return tiled_yuv(h, "rf_detect_yuv_tiled", frames, n, matrix, t, thr, nms, false, nullptr, out_faces, out_counts, out_tile_of, nullptr, nullptr);
+}
+
+int rf_detect_tiled_align(rf_handle h, const uint8_t *const *imgs, const int *widths, const int *heights, const int *row_strides, int n,
+                          const rf_tiling *t, float thr, float nms, const rf_align_params *align, rf_face *out_faces, int *out_counts,
+                          int32_t *out_tile_of, void *out_crops, double *out_mats) {
+    return tiled_bgr(h, "rf_detect_tiled_align", imgs, widths, heights, row_strides, n, t, thr, nms, true, align, out_faces, out_counts,
+                     out_tile_of, out_crops, out_mats);
+}
+
+int rf_detect_yuv_tiled_align(rf_handle h, const rf_yuv_frame *frames, int n, int matrix, const rf_tiling *t, float thr, float nms,
+                              const rf_align_params *align, rf_face *out_faces, int *out_counts, int32_t *out_tile_of, void *out_crops,
+                              double *out_mats) {
+    return tiled_yuv(h, "rf_detect_yuv_tiled_align", frames, n, matrix, t, thr, nms, true, align, out_faces, out_counts, out_tile_of, out_crops,
+                     out_mats);
+}
+
+int rf_detect_tiled_device(rf_handle h, const uint8_t *const *dev_bgr, const int *widths, const int *heights, const int *row_strides, int n,
+                           const rf_tiling *t, float thr, float nms, const rf_align_params *align, void *dev_crops, double *dev_mats,
+                           const rf_det **dev_dets, const int32_t **dev_counts) {
+    static const char *who = "rf_detect_tiled_device";
+    int rc = check_tiled_images(h, who, dev_bgr, widths, heights, row_strides, n);
+    if (rc) return rc;
+    std::vector<std::vector<rf_tile>> layouts;
+    if ((rc = tiled_layouts(h, who, n, widths, heights, t, layouts))) return rc;
+    AlignArgs a;
+    if (align && (rc = check_tiled_align(h, who, align, n, dev_crops, false, a))) return rc;
+    if (n == 0) return RF_OK;
+    std::vector<BgrRows> src(n);
+    for (int i = 0; i < n; i++) src[i] = BgrRows{dev_bgr[i], row_strides && row_strides[i] ? row_strides[i] : widths[i] * 3};
+    try {
+        CK(cudaSetDevice(h->device));
+        detect_tiled_device(h, n, widths, heights, layouts, src, thr, nms, align ? &a : nullptr, dev_crops, dev_mats, dev_dets, dev_counts);
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
+}
+
+int rf_detect_yuv_tiled_device(rf_handle h, const rf_yuv_frame *frames, int n, int matrix, const rf_tiling *t, float thr, float nms,
+                               const rf_align_params *align, void *dev_crops, double *dev_mats, const rf_det **dev_dets,
+                               const int32_t **dev_counts) {
+    static const char *who = "rf_detect_yuv_tiled_device";
+    int rc = check_frames(h, who, frames, n, matrix);
+    if (rc) return rc;
+    std::vector<int> widths(n), heights(n);
+    for (int i = 0; i < n; i++) { widths[i] = frames[i].width; heights[i] = frames[i].height; }
+    std::vector<std::vector<rf_tile>> layouts;
+    if ((rc = tiled_layouts(h, who, n, widths.data(), heights.data(), t, layouts))) return rc;
+    AlignArgs a;
+    if (align && (rc = check_tiled_align(h, who, align, n, dev_crops, false, a))) return rc;
+    if (n == 0) return RF_OK;
+    std::vector<YuvPlanes> src(n);
+    for (int i = 0; i < n; i++) src[i] = planes_of(frames[i], matrix);
+    try {
+        CK(cudaSetDevice(h->device));
+        detect_tiled_device(h, n, widths.data(), heights.data(), layouts, src, thr, nms, align ? &a : nullptr, dev_crops, dev_mats, dev_dets,
+                            dev_counts);
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }

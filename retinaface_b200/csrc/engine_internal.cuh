@@ -159,6 +159,15 @@ struct rf_handle_s {
     uint8_t *h_input = nullptr;       // pinned mirror
     PostBuffers pb_merge{};           // rf_detect_views: candidates of all views of one image (lazily allocated)
     PostBuffers pb_tiles{};           // rf_detect_tiled: candidates of all tiles of each image (lazily grown to the largest layout)
+    // rf_detect_tiled_device / rf_detect_yuv_tiled_device: a ring of `streams` output slots (created by the first such call).  A
+    // slot holds one call's merged candidates and final records (grown lazily like pb_tiles); `free` is recorded once the call's
+    // crops are cut, `start` once the call's home stream has waited for `free`.
+    struct TiledSlot {
+        PostBuffers pb{};
+        cudaEvent_t free = nullptr, start = nullptr;
+    };
+    std::vector<TiledSlot> tiled_slots;
+    unsigned next_tiled_slot = 0;
     uint8_t *d_raw = nullptr;         // one raw caller image (max_image) for the letterbox kernel
     uint8_t *h_raw = nullptr;         // pinned, TWO buffers of raw_bytes: staging of pageable caller images (upload_raw)
     size_t raw_bytes = 0;

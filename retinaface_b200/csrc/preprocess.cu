@@ -54,15 +54,19 @@ __device__ __forceinline__ Tap tap_of(int d, int sn, double scale) {
 // thread = 4 consecutive output pixels = 12 bytes = three aligned 32-bit stores (net_w is a multiple of 32, so rows start 4-byte
 // aligned).  Per image (LbItemT): the source, dst = net_h x net_w x 3, the source size, the size of the resized image inside
 // the output (top-left, the rest is 0), the source pixels per output pixel.
-template <typename Src> constexpr int lb_limit() { return std::is_same<Src, YuvPlanes>::value ? LB_MAX_FRAMES : LB_MAX_IMAGES; }
+template <typename Src> constexpr int lb_limit() { return std::is_same<Src, const uint8_t *>::value ? LB_MAX_IMAGES : LB_MAX_FRAMES; }
 template <typename Src>
 struct LbBatch { LbItemT<Src> img[lb_limit<Src>()]; };
-static_assert(sizeof(LbBatch<const uint8_t *>) + 8 <= 4096 && sizeof(LbBatch<YuvPlanes>) + 8 <= 4096,
+static_assert(sizeof(LbBatch<const uint8_t *>) + 8 <= 4096 && sizeof(LbBatch<YuvPlanes>) + 8 <= 4096 && sizeof(LbBatch<BgrRows>) + 8 <= 4096,
               "letter-box chunk exceeds the classic 4 KB kernel parameter space");
 
-// BGR of source pixel (x, y): packed u8 BGR rows, or a YUV 4:2:0 frame converted on the fly
+// BGR of source pixel (x, y): packed or pitched u8 BGR rows, or a YUV 4:2:0 frame converted on the fly
 __device__ __forceinline__ void src_pixel(const uint8_t *src, int sw, int x, int y, int v[3]) {
     const uint8_t *p = src + ((size_t)y * sw + x) * 3;
+    v[0] = p[0]; v[1] = p[1]; v[2] = p[2];
+}
+__device__ __forceinline__ void src_pixel(const BgrRows &src, int, int x, int y, int v[3]) {
+    const uint8_t *p = src.p + (size_t)y * src.pitch + (size_t)x * 3;
     v[0] = p[0]; v[1] = p[1]; v[2] = p[2];
 }
 __device__ __forceinline__ void src_pixel(const YuvPlanes &src, int, int x, int y, int v[3]) { yuv_pixel(src, x, y, v); }
@@ -323,6 +327,8 @@ template cudaError_t launch_letterbox_batch<const uint8_t *>(const LbItem *, int
 template cudaError_t launch_letterbox_batch<YuvPlanes>(const LbYuvItem *, int, int, int, cudaStream_t);
 template void tile_fill<const uint8_t *>(LbItem &, const uint8_t *, int, int, uint8_t *, int, int, const rf_tile &);
 template void tile_fill<YuvPlanes>(LbYuvItem &, YuvPlanes, int, int, uint8_t *, int, int, const rf_tile &);
+template cudaError_t launch_letterbox_batch<BgrRows>(const LbRowsItem *, int, int, int, cudaStream_t);
+template void tile_fill<BgrRows>(LbRowsItem &, BgrRows, int, int, uint8_t *, int, int, const rf_tile &);
 
 void launch_letterbox(const uint8_t *src, int w, int h, uint8_t *dst, int net_w, int net_h, cudaStream_t s) {
     launch_letterbox_view(src, w, h, dst, net_w, net_h, net_w, net_h, 0, s);

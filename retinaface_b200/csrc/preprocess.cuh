@@ -66,8 +66,14 @@ struct LbItemT {
     int identity, flip, area;   // area: 0 bilinear, 1 NPP super-sampling, LB_HALF_AREA OpenCV's 2x fast area path (tiles only)
     int16_t x0, y0;     // 16 bits keep 64 BGR items within 4 KB; origins are below the largest level side (16384)
 };
+// u8 BGR rows `pitch` bytes apart, read in place: a caller's device image that may be a view of a larger allocation (f8)
+struct BgrRows {
+    const uint8_t *p;
+    int pitch;
+};
 using LbItem = LbItemT<const uint8_t *>;     // packed u8 BGR rows, w x h x 3
 using LbYuvItem = LbItemT<YuvPlanes>;        // a YUV 4:2:0 frame
+using LbRowsItem = LbItemT<BgrRows>;         // pitched u8 BGR rows (up to LB_MAX_FRAMES per launch, like frames)
 // fills one item (geometry of either resize definition, origin 0); returns the reference's map-back factor
 template <typename Src>
 float letterbox_fill(LbItemT<Src> &it, typename LbItemT<Src>::Source src, int w, int h, uint8_t *dst, int box_w, int box_h, int flip, int area);

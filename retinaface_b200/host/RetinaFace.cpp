@@ -189,7 +189,8 @@ void RetinaFace::detectYUV(const vector<Mat> &frames, int layout, float threshol
     }
 }
 
-void RetinaFace::detectTiled(const vector<Mat> &imgs, float threshold, const vector<float> &scales, bool flip, int overlap) {
+void RetinaFace::detectTiled(const vector<Mat> &imgs, float threshold, const vector<float> &scales, bool flip, int overlap,
+                             const AlignOptions *align) {
     if (flip && scales.empty()) throw std::invalid_argument("detectTiled: flip mirrors the given scales; the default pyramid has none");
     last_.assign(imgs.size(), vector<FaceDetectInfo>());
     scales_.assign(imgs.size(), 1.f);
@@ -200,7 +201,10 @@ void RetinaFace::detectTiled(const vector<Mat> &imgs, float threshold, const vec
         if (flip) levels.push_back(rf_tile_level{s, 1});
     }
     const rf_tiling t{levels.empty() ? nullptr : levels.data(), (int)levels.size(), overlap};
+    int per = 0, cw = 0, ch = 0;
+    const rf_align_params p = align ? crop_params(*align, opt_.max_faces, &per, &cw, &ch) : rf_align_params{};
     const size_t mb = (size_t)opt_.max_batch;
+    vector<unsigned char> crops(align ? mb * per * cw * ch * 3 : 0);
     for (size_t start = 0; start < imgs.size(); start += mb) {
         const int n = (int)std::min(mb, imgs.size() - start);
         vector<const uint8_t *> ptrs(n);
@@ -210,10 +214,13 @@ void RetinaFace::detectTiled(const vector<Mat> &imgs, float threshold, const vec
             if (m.empty()) throw std::runtime_error("detectTiled: empty image");
             ptrs[i] = m.data; ws[i] = m.cols; hs[i] = m.rows; strides[i] = (int)m.step;
         }
-        int rc = rf_detect_tiled(h_, ptrs.data(), ws.data(), hs.data(), strides.data(), n, &t, threshold, nms_threshold, out_faces_.data(),
-                                 out_counts_.data(), nullptr);
-        if (rc != RF_OK) throw std::runtime_error(string("rf_detect_tiled: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
-        keepResults(start, n, nullptr, 0, 0, 0);
+        int rc = align ? rf_detect_tiled_align(h_, ptrs.data(), ws.data(), hs.data(), strides.data(), n, &t, threshold, nms_threshold, &p,
+                                               out_faces_.data(), out_counts_.data(), nullptr, crops.data(), nullptr)
+                       : rf_detect_tiled(h_, ptrs.data(), ws.data(), hs.data(), strides.data(), n, &t, threshold, nms_threshold, out_faces_.data(),
+                                         out_counts_.data(), nullptr);
+        if (rc != RF_OK)
+            throw std::runtime_error(string(align ? "rf_detect_tiled_align: " : "rf_detect_tiled: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+        keepResults(start, n, align ? crops.data() : nullptr, per, cw, ch);
     }
 }
 

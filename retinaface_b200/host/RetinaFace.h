@@ -89,9 +89,9 @@ class RetinaFace {
     // detectBatchImages), each also mirrored with `flip`; empty: the default pyramid 1, 1/2, 1/4, ... down to the letter-box, which
     // has no mirrored levels (`flip` with empty `scales` throws std::invalid_argument).
     // `overlap`: pixels neighbouring tiles share (0: 64).  Afterwards lastBatchFaces() holds the faces in ORIGINAL IMAGE pixels
-    // (lastScale() is 1).
+    // (lastScale() is 1) and, with `align` (rf_detect_tiled_align), lastCrops() the crops as detectAndAlign leaves them.
     void detectTiled(const vector<Mat> &imgs, float threshold = 0.5, const vector<float> &scales = vector<float>(), bool flip = false,
-                     int overlap = 0);
+                     int overlap = 0, const AlignOptions *align = nullptr);
     // the reference's visualisation (RetinaFace.cpp:730-741): red box outline (thickness 2), green landmark dots, on a clone
     static Mat draw(const Mat &img, const vector<FaceDetectInfo> &faces);
     int netWidth() const { return opt_.net_w; }

@@ -410,6 +410,46 @@ int rf_detect_yuv_tiled_device(rf_handle h, const rf_yuv_frame *frames, int n, i
                                float nms_threshold, const rf_align_params *align, void *dev_crops, double *dev_mats,
                                const rf_det **dev_dets, const int32_t **dev_counts);
 
+/* f9 rotated and mirrored images.  Orientation o in 1..8 is the EXIF tag: the DISPLAYED image is D = T_o(S), S the stored W x H
+ * image and T_o the transform cv::imread applies (1 identity, 2 flip(1), 3 rotate 180, 4 flip(0), 5 transpose, 6 rotate 90
+ * clockwise, 7 transpose + flip(-1), 8 rotate 90 counter-clockwise; 5..8 display H x W).  Displayed pixel (x, y) reads stored pixel
+ *   1 (x, y)   2 (W-1-x, y)   3 (W-1-x, H-1-y)   4 (x, H-1-y)   5 (y, x)   6 (y, H-1-x)   7 (W-1-y, H-1-x)   8 (W-1-y, x)
+ * and 2, 4, 5, 7 mirror.  The orientation moves integer tap addresses only -- tap positions, weights and rounding are those of the
+ * displayed image -- so every letter-box (either resize definition) and crop byte is the one computed on T_o(S) (on
+ * T_o(cvtColor(frame)) for YUV), and no rotated copy of the image is made.  Orientation 1 is the unoriented path.  An orientation
+ * outside 1..8 is RF_ERR_INVALID_ARG, before anything is launched; every other argument is checked as by the unoriented twin.
+ *
+ * rf_detect_align_batch on T_o(img): host images (pinned or pageable), blocking; faces in DISPLAYED image pixels.  align == NULL: no
+ * crops (out_crops / out_mats unused).  Otherwise crops and matrices as rf_detect_align_batch (M maps displayed image -> crop), with
+ * its raw-buffer rule on the stored images: every image that is not a network-sized packed image in orientation 1 needs a raw
+ * buffer of its own. */
+int rf_detect_oriented_batch(rf_handle h, const uint8_t *const *bgr_images, const int *widths, const int *heights, const int *row_strides,
+                             const int *orientations, int n, float score_threshold, float nms_threshold, const rf_align_params *align,
+                             rf_face *out_faces, int *out_counts, int32_t *out_anchor_index, void *out_crops, double *out_mats);
+/* rf_detect_yuv_batch_device on T_o(frame) (portrait NVDEC surfaces): the same context rotation, per-context input tensor and
+ * validity rule; records in network-input pixels of the displayed frame, out_scales per displayed frame. */
+int rf_detect_yuv_oriented_device(rf_handle h, const rf_yuv_frame *frames, const int *orientations, int n, int matrix, float score_threshold,
+                                  float nms_threshold, const rf_align_params *align, void *dev_crops, double *dev_mats, const rf_det **dev_dets,
+                                  const int32_t **dev_counts, float *out_scales);
+/* Preprocess parity (as rf_preprocess / rf_preprocess_yuv): the letter-box of T_o(img) / T_o(cvtColor(frame)). */
+int rf_preprocess_oriented(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, int orientation, uint8_t *out_net_sized);
+int rf_preprocess_yuv_oriented(rf_handle h, const rf_yuv_frame *frame, int matrix, int orientation, uint8_t *out_net_sized);
+/* rf_detect_views with orientations: view v is T_{o_v}(img) letter-boxed into the shrunk box.  All views run as one batch, their
+ * faces are mapped back to STORED image pixels (the table above, inverted; mirrored views swap left and right landmarks) and merged
+ * by rf_detect_views' NMS.  {1, 6, 3, 8} at shrink 1 finds faces in any of the four rotations, and the landmarks, in stored pixels,
+ * give f5 crops that come out upright.  Orientations 1 / 2 are rf_detect_views' flip 0 / 1, bit for bit. */
+typedef struct rf_oriented_view {
+    float shrink;
+    int32_t orientation;
+} rf_oriented_view;
+int rf_detect_views_oriented(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, const rf_oriented_view *views, int nviews,
+                             float score_threshold, float nms_threshold, rf_face *out_faces, int *out_count, int32_t *out_view_of,
+                             float *out_view_scales);
+/* Host-only (works without a GPU): the Exif orientation (tag 0x0112 of IFD0 in the first APP1 "Exif" segment, either TIFF byte order)
+ * of a JPEG, 1..8; 1 when it is absent or malformed.  Never reads past `bytes`.  What cv::imread applies, for callers of
+ * rf_decode_jpeg or their own decoder. */
+int rf_jpeg_exif_orientation(const uint8_t *jpeg, size_t bytes);
+
 /* Introspection. */
 int rf_get_net_size(rf_handle h, int *net_w, int *net_h, int *max_batch, int *max_faces);
 int rf_num_anchors(rf_handle h);            /* per image: 8,232 @448x448, 47,040 @1280x896 */

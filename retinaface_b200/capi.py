@@ -30,12 +30,24 @@ EXPORTS = [
     "rf_detect_yuv_batch", "rf_detect_yuv_batch_device", "rf_preprocess_yuv",
     "rf_tile_layout", "rf_detect_tiled", "rf_detect_yuv_tiled", "rf_preprocess_tile", "rf_preprocess_yuv_tile",
     "rf_detect_tiled_align", "rf_detect_yuv_tiled_align", "rf_detect_tiled_device", "rf_detect_yuv_tiled_device",
+    "rf_detect_oriented_batch", "rf_detect_yuv_oriented_device", "rf_preprocess_oriented", "rf_preprocess_yuv_oriented",
+    "rf_detect_views_oriented", "rf_jpeg_exif_orientation",
 ]
 COMM_BLOB_BYTES = 128
 
 
 class _View(C.Structure):       # rf_view
     _fields_ = [("shrink", C.c_float), ("flip", C.c_int32)]
+
+
+class _OrientedView(C.Structure):    # rf_oriented_view
+    _fields_ = [("shrink", C.c_float), ("orientation", C.c_int32)]
+
+
+# EXIF orientations (rf_b200.h f9): 1 upright, 2 mirrored, 3 rotated 180, 4 upside-down mirror, 5 transposed, 6 rotated 90 clockwise,
+# 7 transverse, 8 rotated 90 counter-clockwise; ANY_ORIENTATION are the four rotations rf_detect_views_oriented sweeps
+ORIENTATIONS = tuple(range(1, 9))
+ANY_ORIENTATION = (1, 6, 3, 8)
 
 
 RF_CROP_BGR_U8, RF_CROP_RGB_F32, RF_CROP_RGB_F16 = 0, 1, 2
@@ -283,6 +295,17 @@ def load_library() -> C.CDLL:
                                            C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
     lib.rf_detect_yuv_tiled_device.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_int, C.c_int, C.POINTER(Tiling), C.c_float, C.c_float,
                                                C.POINTER(AlignParams), C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
+    lib.rf_detect_oriented_batch.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int),
+                                             C.POINTER(C.c_int), C.c_int, C.c_float, C.c_float, C.POINTER(AlignParams), C.c_void_p, C.c_void_p,
+                                             C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.rf_detect_yuv_oriented_device.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.POINTER(C.c_int), C.c_int, C.c_int, C.c_float, C.c_float,
+                                                  C.POINTER(AlignParams), C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                                  C.c_void_p]
+    lib.rf_preprocess_oriented.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
+    lib.rf_preprocess_yuv_oriented.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_int, C.c_int, C.c_void_p]
+    lib.rf_detect_views_oriented.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(_OrientedView), C.c_int, C.c_float,
+                                             C.c_float, C.c_void_p, C.POINTER(C.c_int), C.c_void_p, C.c_void_p]
+    lib.rf_jpeg_exif_orientation.argtypes = [C.c_void_p, C.c_size_t]
     _lib = lib
     return lib
 
@@ -360,6 +383,21 @@ def nccl_unique_id() -> bytes:
     if rc != 0:
         raise RfError(rc, (lib.rf_last_error(None) or b"").decode())
     return buf.raw
+
+
+def exif_orientation(jpeg: bytes) -> int:
+    """rf_jpeg_exif_orientation (host-only): the EXIF orientation 1..8 cv::imread would apply to these JPEG bytes, 1 without one."""
+    lib = load_library()
+    buf = np.frombuffer(bytes(jpeg), dtype=np.uint8)
+    return int(lib.rf_jpeg_exif_orientation(buf.ctypes.data if buf.size else None, buf.size))
+
+
+def _orientations(orientations, n: int):
+    """The int array of n EXIF orientations the oriented entry points take (their range is checked by the library)."""
+    o = [int(v) for v in orientations]
+    if len(o) != n:
+        raise ValueError(f"{n} items but {len(o)} orientations")
+    return (C.c_int * max(n, 1))(*o)
 
 
 def kl_threshold_bins(hist: np.ndarray, levels: int = 128) -> float:
@@ -841,6 +879,85 @@ class Engine:
         self._check(self.lib.rf_detect_views(self.h, C.c_void_p(img.ctypes.data), img.shape[1], img.shape[0], 0, varr, nv, C.c_float(thr),
                                              C.c_float(nms), C.c_void_p(faces.ctypes.data), C.byref(count),
                                              C.c_void_p(view_of.ctypes.data), C.c_void_p(scales.ctypes.data)))
+        return faces[:count.value].copy(), view_of[:count.value].copy(), scales[:nv].copy()
+
+    # -- f9 rotated and mirrored images (EXIF orientations 1..8) ---------------------------------------------------------------
+    def detect_oriented(self, images: Sequence[np.ndarray], orientations: Sequence[int], thr: float, nms_thr: float, align: Optional[dict] = None,
+                        want_index: bool = False):
+        """rf_detect_oriented_batch: u8 BGR HWC images as STORED (any size <= max_image; rows may be strided), image i shown in EXIF
+        orientation orientations[i].  Returns one (k, 15) float32 array per image in DISPLAYED image pixels -- detect_align's faces
+        on T_o(img) -- without a rotated copy ever being made.  align: detect_align's keywords -> (faces, crops[, mats]), the crops
+        cut from the displayed image.  want_index appends the anchor-index arrays."""
+        n = len(images)
+        keep = [self._bgr_strided(im) for im in images]
+        arr = _orientations(orientations, n)
+        ptrs = (C.c_void_p * max(n, 1))(*[im.ctypes.data for im in keep])
+        ws = (C.c_int * max(n, 1))(*[im.shape[1] for im in keep])
+        hs = (C.c_int * max(n, 1))(*[im.shape[0] for im in keep])
+        rs = (C.c_int * max(n, 1))(*[im.strides[0] for im in keep])
+        faces = np.empty((n, self.max_faces, FACE_FLOATS), dtype=np.float32)
+        counts = np.zeros(n, dtype=np.int32)
+        idx = np.empty((n, self.max_faces), dtype=np.int32) if want_index else None
+        p = crops = mats = None
+        A = 0
+        if align is not None:
+            p, A, crops, mats = self._host_align(n, align)
+        self._check(self.lib.rf_detect_oriented_batch(self.h, ptrs, ws, hs, rs, arr, n, thr, nms_thr, C.byref(p) if p is not None else None,
+                                                      faces.ctypes.data, counts.ctypes.data, idx.ctypes.data if want_index else None,
+                                                      crops.ctypes.data if crops is not None else None,
+                                                      mats.ctypes.data if mats is not None else None))
+        out = ([faces[i, :counts[i]].copy() for i in range(n)],)
+        if align is not None:
+            out += ([crops[i, :min(counts[i], A)].copy() for i in range(n)],)
+            if mats is not None:
+                out += ([mats[i, :min(counts[i], A)].copy() for i in range(n)],)
+        if want_index:
+            out += ([idx[i, :counts[i]].copy() for i in range(n)],)
+        return out[0] if len(out) == 1 else out
+
+    def detect_yuv_oriented_device(self, frames, orientations: Sequence[int], thr: float, nms_thr: float, layout: str = "nv12", matrix="bt601",
+                                   align: Optional[dict] = None, dev_crops_ptr: Optional[int] = None, dev_mats_ptr: Optional[int] = None):
+        """rf_detect_yuv_oriented_device: detect_yuv_device on frames shown in EXIF orientation orientations[i] (portrait NVDEC surfaces).
+        Returns (dets_ptr, counts_ptr, map-back scale of each displayed frame); detections in network-input pixels of the displayed
+        frame.  Host frames: ValueError."""
+        n = len(frames)
+        arr = self._frames(frames, layout, True)
+        o = _orientations(orientations, n)
+        p = align_params(**align) if align is not None else None
+        scales = np.zeros(max(n, 1), dtype=np.float32)
+        d, c = C.c_void_p(), C.c_void_p()
+        self._check(self.lib.rf_detect_yuv_oriented_device(self.h, arr, o, n, _matrix(matrix), thr, nms_thr, C.byref(p) if p is not None else None,
+                                                           dev_crops_ptr, dev_mats_ptr, C.byref(d), C.byref(c), scales.ctypes.data))
+        return int(d.value or 0), int(c.value or 0), scales[:n].copy()
+
+    def preprocess_oriented(self, img: np.ndarray, orientation: int) -> np.ndarray:
+        """rf_preprocess_oriented: the (H, W, 3) u8 BGR letter-box of the image shown in EXIF orientation `orientation`."""
+        img = self._bgr_strided(img)
+        out = np.empty((self.net_h, self.net_w, 3), dtype=np.uint8)
+        self._check(self.lib.rf_preprocess_oriented(self.h, img.ctypes.data, img.shape[1], img.shape[0], img.strides[0], int(orientation),
+                                                    out.ctypes.data))
+        return out
+
+    def preprocess_yuv_oriented(self, frame, orientation: int, layout: str = "nv12", matrix="bt601") -> np.ndarray:
+        """rf_preprocess_yuv_oriented: the letter-box of one host frame shown in EXIF orientation `orientation`."""
+        arr = self._frames([frame], layout, False)
+        out = np.empty((self.net_h, self.net_w, 3), dtype=np.uint8)
+        self._check(self.lib.rf_preprocess_yuv_oriented(self.h, arr, _matrix(matrix), int(orientation), out.ctypes.data))
+        return out
+
+    def detect_views_oriented(self, img: np.ndarray, views, thr: float, nms: float):
+        """rf_detect_views_oriented: one image, views = [(shrink, orientation), ...] run as one batch, mapped back into STORED image
+        pixels and merged on the GPU.  Returns (faces [k, 15], view index of each face [k], map-back scale of each view)."""
+        img = self._bgr_strided(img)
+        nv = len(views)
+        varr = (_OrientedView * max(nv, 1))(*[_OrientedView(float(s), int(o)) for s, o in views])
+        faces = np.empty((self.max_faces, 15), dtype=np.float32)
+        view_of = np.empty(self.max_faces, dtype=np.int32)
+        scales = np.empty(max(nv, 1), dtype=np.float32)
+        count = C.c_int(0)
+        self._check(self.lib.rf_detect_views_oriented(self.h, C.c_void_p(img.ctypes.data), img.shape[1], img.shape[0], img.strides[0], varr, nv,
+                                                      C.c_float(thr), C.c_float(nms), C.c_void_p(faces.ctypes.data), C.byref(count),
+                                                      C.c_void_p(view_of.ctypes.data), C.c_void_p(scales.ctypes.data)))
         return faces[:count.value].copy(), view_of[:count.value].copy(), scales[:nv].copy()
 
     def calibrate_int8(self, images: np.ndarray, out_table: str):

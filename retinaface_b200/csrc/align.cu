@@ -63,8 +63,16 @@ __device__ __forceinline__ void tap(const AlignImage &im, int x, int y, int p[3]
     p[0] = q[0]; p[1] = q[1]; p[2] = q[2];
 }
 __device__ __forceinline__ void tap(const AlignYuvImage &im, int x, int y, int p[3]) { yuv_pixel(im.p, x, y, p); }
-
+// displayed pixel (x, y) of an oriented image: reflected, then transposed, as the letter-box reads it (preprocess.cu)
 template <typename Img>
+__device__ __forceinline__ void oriented_tap(const Img &im, int x, int y, int p[3]) {
+    if (im.orient & LB_FLIP_X) x = im.w - 1 - x;
+    if (im.orient & LB_FLIP_Y) y = im.h - 1 - y;
+    if (im.orient & LB_TRANSPOSE) tap(im, y, x, p);
+    else tap(im, x, y, p);
+}
+
+template <bool ORIENTED, typename Img>
 __device__ __forceinline__ void sample(const Img &im, int X, int Y, int v[3]) {
     const int sx = min(max(X >> 5, -32768), 32767), sy = min(max(Y >> 5, -32768), 32767);   // saturate_cast<short>
     const int fx = X & 31, fy = Y & 31;
@@ -75,17 +83,21 @@ __device__ __forceinline__ void sample(const Img &im, int X, int Y, int v[3]) {
         const int tx = sx + (t & 1), ty = sy + (t >> 1);
         if ((unsigned)tx < (unsigned)im.w && (unsigned)ty < (unsigned)im.h) {
             int p[3];
-            tap(im, tx, ty, p);
+            if (ORIENTED) oriented_tap(im, tx, ty, p);
+            else tap(im, tx, ty, p);
             acc[0] += wts[t] * p[0]; acc[1] += wts[t] * p[1]; acc[2] += wts[t] * p[2];
         }
     }
     v[0] = acc[0] >> 15; v[1] = acc[1] >> 15; v[2] = acc[2] >> 15;
 }
 
-// Where the kernel finds image i: the BGR table / uniform net-sized images of AlignArgs, or the frame table parameter.
-struct BgrImages {};
-struct YuvFrames { AlignYuvImage img[ALIGN_MAX_FRAMES]; };
-struct BgrTable { AlignImage img[ALIGN_MAX_FRAMES]; };     // f8: BGR images whose table travels as a kernel parameter
+// Where the kernel finds image i: the BGR table / uniform net-sized images of AlignArgs, or the frame table parameter.  Only the
+// tables of the oriented paths (f9) read `orient`: the other instantiations keep their code.
+struct BgrImages { static constexpr bool kOriented = false; };
+template <bool O> struct YuvFramesT { static constexpr bool kOriented = O; AlignYuvImage img[ALIGN_MAX_FRAMES]; };
+template <bool O> struct BgrTableT { static constexpr bool kOriented = O; AlignImage img[ALIGN_MAX_FRAMES]; };   // f8: BGR images whose table travels as a kernel parameter
+using YuvFrames = YuvFramesT<false>;
+using BgrTable = BgrTableT<false>;
 static_assert(sizeof(AlignArgs) + sizeof(YuvFrames) + 32 <= 4096, "align launch exceeds the classic 4 KB kernel parameter space");
 static_assert(sizeof(AlignArgs) + sizeof(BgrTable) + 32 <= 4096, "align launch exceeds the classic 4 KB kernel parameter space");
 
@@ -95,12 +107,12 @@ __device__ __forceinline__ AlignImage image_of(const AlignArgs &a, const BgrImag
         im = a.images[i];
     } else {
         im.src = a.uniform_base + (size_t)i * a.uniform_bytes;
-        im.w = a.uniform_w; im.h = a.uniform_h; im.row_bytes = a.uniform_w * 3; im.scale = 1.f;
+        im.w = a.uniform_w; im.h = a.uniform_h; im.row_bytes = a.uniform_w * 3; im.scale = 1.f; im.orient = 0;
     }
     return im;
 }
-__device__ __forceinline__ AlignYuvImage image_of(const AlignArgs &, const YuvFrames &f, int i) { return f.img[i]; }
-__device__ __forceinline__ AlignImage image_of(const AlignArgs &, const BgrTable &t, int i) { return t.img[i]; }
+template <bool O> __device__ __forceinline__ AlignYuvImage image_of(const AlignArgs &, const YuvFramesT<O> &f, int i) { return f.img[i]; }
+template <bool O> __device__ __forceinline__ AlignImage image_of(const AlignArgs &, const BgrTableT<O> &t, int i) { return t.img[i]; }
 
 // Four consecutive pixels of one crop row (x4 .. x4 + 3, those < cw valid).  Vector stores where the address allows.
 __device__ __forceinline__ void store_quad(const AlignArgs &a, unsigned char *crop, int y, int x4, const int v[4][3]) {
@@ -224,7 +236,7 @@ __global__ void __launch_bounds__(ALIGN_THREADS) k_align_faces(const AlignArgs a
 #pragma unroll
             for (int k = 0; k < 4; k++) {
                 const int x = x4 + k;
-                if (x < cw && !zero) sample(im, (s_x0[r] + s_ax[x]) >> 5, (s_y0[r] + s_bx[x]) >> 5, v[k]);
+                if (x < cw && !zero) sample<Src::kOriented>(im, (s_x0[r] + s_ax[x]) >> 5, (s_y0[r] + s_bx[x]) >> 5, v[k]);
                 else v[k][0] = v[k][1] = v[k][2] = 0;
             }
             store_quad(a, crop, ybase + r, x4, v);
@@ -264,12 +276,12 @@ cudaError_t launch_align_faces(const AlignArgs &a, const PostBuffers &pb, int nu
     return cudaGetLastError();
 }
 
-cudaError_t launch_align_faces_yuv(const AlignArgs &a, const AlignYuvImage *frames, const PostBuffers &pb, int num_sms, cudaStream_t s) {
-    return launch_table<YuvFrames>(a, frames, pb, num_sms, s);
+cudaError_t launch_align_faces_yuv(const AlignArgs &a, const AlignYuvImage *frames, const PostBuffers &pb, int num_sms, cudaStream_t s, bool oriented) {
+    return oriented ? launch_table<YuvFramesT<true>>(a, frames, pb, num_sms, s) : launch_table<YuvFrames>(a, frames, pb, num_sms, s);
 }
 
-cudaError_t launch_align_faces(const AlignArgs &a, const AlignImage *images, const PostBuffers &pb, int num_sms, cudaStream_t s) {
-    return launch_table<BgrTable>(a, images, pb, num_sms, s);
+cudaError_t launch_align_faces(const AlignArgs &a, const AlignImage *images, const PostBuffers &pb, int num_sms, cudaStream_t s, bool oriented) {
+    return oriented ? launch_table<BgrTableT<true>>(a, images, pb, num_sms, s) : launch_table<BgrTable>(a, images, pb, num_sms, s);
 }
 
 }  // namespace rf

@@ -8,16 +8,20 @@
 #pragma once
 #include "common.cuh"
 #include "postproc.cuh"
+#include "preprocess.cuh"
 #include "yuv.cuh"
 
 namespace rf {
 
 // One source image of the batch: u8 BGR HWC rows of row_bytes, and the factor that maps network-input coordinates to its
-// pixels (the float letterbox_fill returns; 1 for network-sized images).
+// pixels (the float letterbox_fill returns; 1 for network-sized images).  f9: `orient` (LB_* bits, preprocess.cuh) views the
+// stored rows in another orientation; w x h is then the DISPLAYED size, which the warp's bounds test uses, and displayed tap (x, y)
+// reads the stored pixel the letter-box would, so a crop is cv2.warpAffine(T_o(img), M).  0: the rows as they are.
 struct AlignImage {
     const uint8_t *src;
     int w, h, row_bytes;
     float scale;
+    int orient;
 };
 
 struct AlignArgs {
@@ -38,8 +42,9 @@ struct AlignArgs {
 // is converted to BGR first, so a crop is cv2.warpAffine(cv2.cvtColor(frame), M) byte for byte.
 struct AlignYuvImage {
     YuvPlanes p;
-    int w, h;
+    int w, h;           // displayed size
     float scale;
+    int orient;         // LB_* bits, as AlignImage
 };
 
 constexpr int ALIGN_MIN_SIDE = 8, ALIGN_MAX_SIDE = 512, ALIGN_MAX_FRAMES = 32;
@@ -50,10 +55,13 @@ size_t align_crop_bytes(int crop_w, int crop_h, int format);
 cudaError_t launch_align_faces(const AlignArgs &a, const PostBuffers &pb, int num_sms, cudaStream_t s);
 // The same over a.n YUV frames [n]: the frame table travels as a kernel parameter (no host table a later call could rewrite
 // before the copy ran), one launch per ALIGN_MAX_FRAMES frames.
-cudaError_t launch_align_faces_yuv(const AlignArgs &a, const AlignYuvImage *frames, const PostBuffers &pb, int num_sms, cudaStream_t s);
+// oriented (f9): the frames' `orient` bits apply (a separate instantiation; false reads the frames as stored).
+cudaError_t launch_align_faces_yuv(const AlignArgs &a, const AlignYuvImage *frames, const PostBuffers &pb, int num_sms, cudaStream_t s,
+                                   bool oriented = false);
 // f8: the same over a.n BGR images [n] (a.images / a.uniform_* unused), the table a kernel parameter as the frames are above: an
 // asynchronous call cannot have its table rewritten by a later one.  The tiled paths pass scale 1 (their records are already in
 // image pixels; __fmul_rn(l, 1.f) is exact).
-cudaError_t launch_align_faces(const AlignArgs &a, const AlignImage *images, const PostBuffers &pb, int num_sms, cudaStream_t s);
+cudaError_t launch_align_faces(const AlignArgs &a, const AlignImage *images, const PostBuffers &pb, int num_sms, cudaStream_t s,
+                               bool oriented = false);
 
 }  // namespace rf

@@ -599,8 +599,10 @@ static uint8_t *upload_raw(rf_handle h, cudaStream_t s, const uint8_t *src, int 
 // The n caller images of rf_detect_batch -> the input tensor, on `s`.  With `originals`
 // (rf_detect_align_batch, which has checked that every image that is not network-sized gets a raw buffer of its own),
 // originals[i] records where image i's own pixels stay resident and its map-back scale.
+// f9 `orient` (optional): image i is shown in EXIF orientation orient[i] (checked by the caller); only orientation 1 takes the
+// straight copy, and originals[i] then describes the displayed image.
 static int stage_images(rf_handle h, cudaStream_t s, const char *who, const uint8_t *const *imgs, const int *widths, const int *heights,
-                        const int *row_strides, int n, AlignImage *originals) {
+                        const int *row_strides, int n, AlignImage *originals, const int *orient = nullptr) {
     const int Hn = h->cfg.net_h, Wn = h->cfg.net_w;
     const size_t img_bytes = (size_t)Hn * Wn * 3;
     // Network-sized packed images are copied H2D straight from the caller's memory when it is
@@ -621,7 +623,8 @@ static int stage_images(rf_handle h, cudaStream_t s, const char *who, const uint
     for (int i = 0; i < n; i++) {
         if (!imgs[i] || widths[i] <= 0 || heights[i] <= 0) { return fail(h, RF_ERR_INVALID_ARG, fmt("%s: image %d is empty", who, i)); }
         const int rs = row_strides && row_strides[i] ? row_strides[i] : widths[i] * 3;
-        if (widths[i] == Wn && heights[i] == Hn && rs == Wn * 3) {
+        const int bits = orient ? lb_orientation_bits(orient[i]) : 0;
+        if (widths[i] == Wn && heights[i] == Hn && rs == Wn * 3 && bits == 0) {
             const uint8_t *src = imgs[i];
             const bool in_mirror = src >= h->h_input && src < h->h_input + (size_t)h->cfg.max_batch * img_bytes;
             if (!in_mirror && !is_pinned(src)) {
@@ -640,8 +643,10 @@ static int stage_images(rf_handle h, cudaStream_t s, const char *who, const uint
             if ((int)lb.size() == h->raw_slots) flush_lb();
             const uint8_t *d_src = upload_raw(h, s, imgs[i], widths[i], heights[i], rs, (int)lb.size());
             lb.emplace_back();
-            const float scale = letterbox_fill(lb.back(), d_src, widths[i], heights[i], h->d_input + (size_t)i * img_bytes, Wn, Hn, 0, area);
-            if (originals) originals[i] = AlignImage{d_src, widths[i], heights[i], widths[i] * 3, scale};
+            int dw = widths[i], dh = heights[i];
+            if (bits & LB_TRANSPOSE) std::swap(dw, dh);
+            const float scale = letterbox_fill(lb.back(), d_src, dw, dh, h->d_input + (size_t)i * img_bytes, Wn, Hn, bits, area);
+            if (originals) originals[i] = AlignImage{d_src, dw, dh, widths[i] * 3, scale, bits};
         }
     }
     runs.flush();
@@ -802,6 +807,62 @@ int rf_detect_align_batch_device(rf_handle h, const uint8_t *dev_bgr, int n, flo
     return RF_OK;
 }
 
+// ---- f9 oriented images (rf_b200.h rf_detect_oriented_batch) ------------------------------------------------------------------------
+static int check_orientations(rf_handle h, const char *who, const int *orientations, int n) {
+    if (n > 0 && !orientations) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: orientations is NULL", who));
+    for (int i = 0; i < n; i++)
+        if (lb_orientation_bits(orientations[i]) < 0)
+            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: item %d: orientation %d, must be in 1..8 (EXIF)", who, i, orientations[i]));
+    return RF_OK;
+}
+
+int rf_detect_oriented_batch(rf_handle h, const uint8_t *const *imgs, const int *widths, const int *heights, const int *row_strides,
+                             const int *orientations, int n, float thr, float nms, const rf_align_params *align, rf_face *out_faces,
+                             int *out_counts, int32_t *out_idx, void *out_crops, double *out_mats) {
+    static const char *who = "rf_detect_oriented_batch";
+    int rc = check_n(h, n);
+    if (rc) return rc;
+    AlignArgs a;
+    if (align && (rc = align_setup(h, who, align, a))) return rc;
+    if (n == 0) return RF_OK;
+    if (!imgs || !widths || !heights) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL image arrays", who));
+    if (align && !out_crops) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: align without out_crops", who));
+    if ((rc = check_orientations(h, who, orientations, n))) return rc;
+    const int Hn = h->cfg.net_h, Wn = h->cfg.net_w;
+    for (int i = 0; i < n; i++)
+        if (!imgs[i] || widths[i] <= 0 || heights[i] <= 0) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: image %d is empty", who, i));
+    if (align) {
+        // rf_detect_align_batch's rule, on the stored images: the crops are cut after the forward, so no raw buffer may be recycled
+        int raw = 0;
+        for (int i = 0; i < n; i++) {
+            const int rs = row_strides && row_strides[i] ? row_strides[i] : widths[i] * 3;
+            raw += !(widths[i] == Wn && heights[i] == Hn && rs == Wn * 3 && orientations[i] == 1);
+        }
+        if (raw > h->raw_slots)
+            return fail(h, RF_ERR_CAPACITY, fmt("%s: %d images need a raw buffer, but the handle keeps at most %d originals resident "
+                                                "(one %dx%d raw buffer each); split the batch", who, raw, h->raw_slots, h->cfg.max_image_w,
+                                                h->cfg.max_image_h));
+    }
+    try {
+        CK(cudaSetDevice(h->device));
+        Ctx &c = h->ctx[0];
+        if (align) ensure_align_buffers(h, n, a);
+        std::vector<AlignImage> orig(n);
+        if ((rc = stage_images(h, c.stream, who, imgs, widths, heights, row_strides, n, orig.data(), orientations))) return rc;
+        set_params(h, c, thr, nms);
+        forward_graph(h, c, n);
+        if (align) {
+            a.n = n;
+            a.crops = h->d_align_crops;
+            a.mats = out_mats ? h->d_align_mats : nullptr;
+            CK(launch_align_faces(a, orig.data(), c.pb, h->num_sms, c.stream, true));
+        }
+        fetch_results(h, c, n, nullptr, out_counts, out_idx);
+        put_mapped(h, c, n, [&](int i) { return orig[i].scale; }, align ? &a : nullptr, out_faces, out_crops, out_mats);
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
+}
+
 // ---- f6 video frames: YUV 4:2:0 (yuv.cuh) ---------------------------------------------------------------------------------------
 // Checks n, the matrix and every frame descriptor; nothing is launched before this passes.
 static int check_frames(rf_handle h, const char *who, const rf_yuv_frame *frames, int n, int matrix) {
@@ -896,14 +957,16 @@ int rf_detect_yuv_batch(rf_handle h, const rf_yuv_frame *frames, int n, int matr
     return RF_OK;
 }
 
-int rf_detect_yuv_batch_device(rf_handle h, const rf_yuv_frame *frames, int n, int matrix, float thr, float nms, const rf_align_params *align,
-                               void *dev_crops, double *dev_mats, const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales) {
-    static const char *who = "rf_detect_yuv_batch_device";
+// rf_detect_yuv_batch_device, and with `orient` (f9: frame i shown in EXIF orientation orient[i]) rf_detect_yuv_oriented_device
+static int yuv_device_impl(rf_handle h, const char *who, const rf_yuv_frame *frames, const int *orient, int n, int matrix, float thr, float nms,
+                           const rf_align_params *align, void *dev_crops, double *dev_mats, const rf_det **dev_dets, const int32_t **dev_counts,
+                           float *out_scales) {
     int rc = check_frames(h, who, frames, n, matrix);
     if (rc) return rc;
     AlignArgs a;
     if (align && (rc = align_setup(h, who, align, a))) return rc;
     if (align && n > 0 && !dev_crops) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: align without dev_crops", who));
+    if (orient && (rc = check_orientations(h, who, orient, n))) return rc;
     const int Hn = h->cfg.net_h, Wn = h->cfg.net_w;
     const size_t img_bytes = (size_t)Hn * Wn * 3;
     const int area = (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0;
@@ -915,7 +978,9 @@ int rf_detect_yuv_batch_device(rf_handle h, const rf_yuv_frame *frames, int n, i
         for (int i = 0; i < n; i++) {
             const rf_yuv_frame &f = frames[i];
             const YuvPlanes p = planes_of(f, matrix);
-            orig[i] = AlignYuvImage{p, f.width, f.height, letterbox_fill(lb[i], p, f.width, f.height, c.d_frames_in + i * img_bytes, Wn, Hn, 0, area)};
+            const int bits = orient ? lb_orientation_bits(orient[i]) : 0;
+            const int dw = (bits & LB_TRANSPOSE) ? f.height : f.width, dh = (bits & LB_TRANSPOSE) ? f.width : f.height;
+            orig[i] = AlignYuvImage{p, dw, dh, letterbox_fill(lb[i], p, dw, dh, c.d_frames_in + i * img_bytes, Wn, Hn, bits, area), bits};
             if (out_scales) out_scales[i] = orig[i].scale;
         }
         CK(launch_letterbox_batch(lb.data(), n, Wn, Hn, c.stream));
@@ -928,30 +993,55 @@ int rf_detect_yuv_batch_device(rf_handle h, const rf_yuv_frame *frames, int n, i
     a.crops = dev_crops;
     a.mats = dev_mats;
     try {
-        CK(launch_align_faces_yuv(a, orig.data(), c->pb, h->num_sms, c->stream));
+        CK(launch_align_faces_yuv(a, orig.data(), c->pb, h->num_sms, c->stream, orient != nullptr));
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }
 
-int rf_preprocess_yuv(rf_handle h, const rf_yuv_frame *frame, int matrix, uint8_t *out) {
-    static const char *who = "rf_preprocess_yuv";
+int rf_detect_yuv_batch_device(rf_handle h, const rf_yuv_frame *frames, int n, int matrix, float thr, float nms, const rf_align_params *align,
+                               void *dev_crops, double *dev_mats, const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales) {
+    return yuv_device_impl(h, "rf_detect_yuv_batch_device", frames, nullptr, n, matrix, thr, nms, align, dev_crops, dev_mats, dev_dets, dev_counts,
+                           out_scales);
+}
+
+int rf_detect_yuv_oriented_device(rf_handle h, const rf_yuv_frame *frames, const int *orientations, int n, int matrix, float thr, float nms,
+                                  const rf_align_params *align, void *dev_crops, double *dev_mats, const rf_det **dev_dets,
+                                  const int32_t **dev_counts, float *out_scales) {
+    static const char *who = "rf_detect_yuv_oriented_device";
+    if (!h) return RF_ERR_INVALID_ARG;
+    if (n > 0 && !orientations) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: orientations is NULL", who));
+    return yuv_device_impl(h, who, frames, orientations, n, matrix, thr, nms, align, dev_crops, dev_mats, dev_dets,
+                           dev_counts, out_scales);
+}
+
+static int preprocess_yuv_impl(rf_handle h, const char *who, const rf_yuv_frame *frame, int matrix, int orientation, uint8_t *out) {
     if (!h) return RF_ERR_INVALID_ARG;
     if (!frame || !out) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL frame or output", who));
     int rc = check_frames(h, who, frame, 1, matrix);
     if (rc) return rc;
+    if ((rc = check_orientations(h, who, &orientation, 1))) return rc;
+    const int bits = lb_orientation_bits(orientation);
+    const int dw = (bits & LB_TRANSPOSE) ? frame->height : frame->width, dh = (bits & LB_TRANSPOSE) ? frame->width : frame->height;
     const int Hn = h->cfg.net_h, Wn = h->cfg.net_w;
     try {
         CK(cudaSetDevice(h->device));
         cudaStream_t s = h->ctx[0].stream;
         const YuvPlanes p = upload_frame(h, s, *frame, matrix, 0);
         LbYuvItem it;
-        letterbox_fill(it, p, frame->width, frame->height, h->d_input, Wn, Hn, 0, (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0);
+        letterbox_fill(it, p, dw, dh, h->d_input, Wn, Hn, bits, (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0);
         CK(launch_letterbox_batch(&it, 1, Wn, Hn, s));
         CK(cudaMemcpyAsync(h->h_input, h->d_input, (size_t)Hn * Wn * 3, cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
         memcpy(out, h->h_input, (size_t)Hn * Wn * 3);
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
+}
+
+int rf_preprocess_yuv(rf_handle h, const rf_yuv_frame *frame, int matrix, uint8_t *out) {
+    return preprocess_yuv_impl(h, "rf_preprocess_yuv", frame, matrix, 1, out);
+}
+int rf_preprocess_yuv_oriented(rf_handle h, const rf_yuv_frame *frame, int matrix, int orientation, uint8_t *out) {
+    return preprocess_yuv_impl(h, "rf_preprocess_yuv_oriented", frame, matrix, orientation, out);
 }
 
 // ---- f7 tiled detection: a scale pyramid cut into network-sized tiles (preprocess.cuh tile_layout) ----------------------------------
@@ -1523,14 +1613,19 @@ int rf_detect_batch_allgather(rf_handle h, const uint8_t *const *imgs, int n, fl
     return rf_collect_batch_allgather(h, t, out_faces, out_counts, out_idx);
 }
 
-int rf_detect_views(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, const rf_view *views, int nviews, float thr,
-                    float nms, rf_face *out_faces, int *out_count, int32_t *out_view_of, float *out_view_scales) {
-    if (!h || !bgr || !views || !out_count || width <= 0 || height <= 0) return fail(h, RF_ERR_INVALID_ARG, "rf_detect_views: bad arguments");
+// rf_detect_views and rf_detect_views_oriented: view v is (shrink, LB_* bits); `views` only for the NULL check of either entry point
+static int views_impl(rf_handle h, const char *who, const uint8_t *bgr, int width, int height, int row_stride, const void *views, int nviews,
+                      const std::function<float(int)> &shrink_of, const std::function<int(int)> &bits_of, float thr, float nms, rf_face *out_faces,
+                      int *out_count, int32_t *out_view_of, float *out_view_scales) {
+    if (!h || !bgr || !views || !out_count || width <= 0 || height <= 0) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: bad arguments", who));
     if (nviews < 1 || nviews > RF_MAX_VIEWS || nviews > h->cfg.max_batch)
-        return fail(h, RF_ERR_CAPACITY, fmt("rf_detect_views: %d views, limit min(RF_MAX_VIEWS = %d, max_batch = %d)", nviews, RF_MAX_VIEWS, h->cfg.max_batch));
-    if (width > h->cfg.max_image_w || height > h->cfg.max_image_h) return fail(h, RF_ERR_CAPACITY, "rf_detect_views: image larger than max_image");
-    for (int v = 0; v < nviews; v++)
-        if (!(views[v].shrink > 0.f && views[v].shrink <= 1.f)) return fail(h, RF_ERR_INVALID_ARG, fmt("rf_detect_views: view %d: shrink must be in (0, 1]", v));
+        return fail(h, RF_ERR_CAPACITY, fmt("%s: %d views, limit min(RF_MAX_VIEWS = %d, max_batch = %d)", who, nviews, RF_MAX_VIEWS, h->cfg.max_batch));
+    if (width > h->cfg.max_image_w || height > h->cfg.max_image_h) return fail(h, RF_ERR_CAPACITY, fmt("%s: image larger than max_image", who));
+    for (int v = 0; v < nviews; v++) {
+        const float shrink = shrink_of(v);
+        if (!(shrink > 0.f && shrink <= 1.f)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: view %d: shrink must be in (0, 1]", who, v));
+        if (bits_of(v) < 0) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: view %d: orientation must be in 1..8 (EXIF)", who, v));
+    }
     static_assert(RF_MAX_VIEWS == RF_MAX_VIEWS_DEV, "view capacity of the merge kernel");
     const int Hn = h->cfg.net_h, Wn = h->cfg.net_w, mf = h->cfg.max_faces;
     const size_t img_bytes = (size_t)Hn * Wn * 3;
@@ -1545,10 +1640,12 @@ int rf_detect_views(rf_handle h, const uint8_t *bgr, int width, int height, int 
         std::vector<LbItem> lb(nviews);
         std::vector<MergeSource> ms(nviews);
         for (int v = 0; v < nviews; v++) {
-            const int bw = std::max(1, (int)(Wn * views[v].shrink)), bh = std::max(1, (int)(Hn * views[v].shrink));
-            const int flip = views[v].flip ? 1 : 0;
-            const float scale = letterbox_fill(lb[v], d_src, width, height, h->d_input + (size_t)v * img_bytes, bw, bh, flip, area);
-            ms[v] = view_source(v, mf, scale, flip, width);
+            const int bw = std::max(1, (int)(Wn * shrink_of(v))), bh = std::max(1, (int)(Hn * shrink_of(v)));
+            const int bits = bits_of(v);
+            // the view letter-boxes the displayed image; its faces map back into stored pixels (postproc.cuh)
+            const int dw = (bits & LB_TRANSPOSE) ? height : width, dh = (bits & LB_TRANSPOSE) ? width : height;
+            const float scale = letterbox_fill(lb[v], d_src, dw, dh, h->d_input + (size_t)v * img_bytes, bw, bh, bits, area);
+            ms[v] = (bits & ~LB_FLIP_X) ? oriented_view_source(v, mf, scale, bits, dw, dh) : view_source(v, mf, scale, bits, width);
             if (out_view_scales) out_view_scales[v] = scale;
         }
         CK(launch_letterbox_batch(lb.data(), nviews, Wn, Hn, c.stream));     // all views of the image: one launch
@@ -1569,9 +1666,26 @@ int rf_detect_views(rf_handle h, const uint8_t *bgr, int width, int height, int 
     return RF_OK;
 }
 
-int rf_preprocess(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, uint8_t *out) {
-    if (!h || !bgr || !out || width <= 0 || height <= 0) return fail(h, RF_ERR_INVALID_ARG, "rf_preprocess: bad arguments");
-    if (width > h->cfg.max_image_w || height > h->cfg.max_image_h) return fail(h, RF_ERR_CAPACITY, "rf_preprocess: image larger than max_image");
+int rf_detect_views(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, const rf_view *views, int nviews, float thr,
+                    float nms, rf_face *out_faces, int *out_count, int32_t *out_view_of, float *out_view_scales) {
+    return views_impl(h, "rf_detect_views", bgr, width, height, row_stride, views, nviews, [&](int v) { return views[v].shrink; },
+                      [&](int v) { return views[v].flip ? 1 : 0; }, thr, nms, out_faces, out_count, out_view_of, out_view_scales);
+}
+
+int rf_detect_views_oriented(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, const rf_oriented_view *views, int nviews,
+                             float thr, float nms, rf_face *out_faces, int *out_count, int32_t *out_view_of, float *out_view_scales) {
+    return views_impl(h, "rf_detect_views_oriented", bgr, width, height, row_stride, views, nviews, [&](int v) { return views[v].shrink; },
+                      [&](int v) { return lb_orientation_bits(views[v].orientation); }, thr, nms, out_faces, out_count, out_view_of,
+                      out_view_scales);
+}
+
+static int preprocess_impl(rf_handle h, const char *who, const uint8_t *bgr, int width, int height, int row_stride, int orientation, uint8_t *out) {
+    if (!h || !bgr || !out || width <= 0 || height <= 0) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: bad arguments", who));
+    if (width > h->cfg.max_image_w || height > h->cfg.max_image_h) return fail(h, RF_ERR_CAPACITY, fmt("%s: image larger than max_image", who));
+    int rc = check_orientations(h, who, &orientation, 1);
+    if (rc) return rc;
+    const int bits = lb_orientation_bits(orientation);
+    const int dw = (bits & LB_TRANSPOSE) ? height : width, dh = (bits & LB_TRANSPOSE) ? width : height;
     const int Hn = h->cfg.net_h, Wn = h->cfg.net_w;
     const int rs = row_stride ? row_stride : width * 3;
     try {
@@ -1579,13 +1693,20 @@ int rf_preprocess(rf_handle h, const uint8_t *bgr, int width, int height, int ro
         cudaStream_t s = h->ctx[0].stream;
         const uint8_t *d_src = upload_raw(h, s, bgr, width, height, rs);
         LbItem it;
-        letterbox_fill(it, d_src, width, height, h->d_input, Wn, Hn, 0, (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0);
+        letterbox_fill(it, d_src, dw, dh, h->d_input, Wn, Hn, bits, (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0);
         CK(launch_letterbox_batch(&it, 1, Wn, Hn, s));
         CK(cudaMemcpyAsync(h->h_input, h->d_input, (size_t)Hn * Wn * 3, cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
         memcpy(out, h->h_input, (size_t)Hn * Wn * 3);
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
+}
+
+int rf_preprocess(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, uint8_t *out) {
+    return preprocess_impl(h, "rf_preprocess", bgr, width, height, row_stride, 1, out);
+}
+int rf_preprocess_oriented(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, int orientation, uint8_t *out) {
+    return preprocess_impl(h, "rf_preprocess_oriented", bgr, width, height, row_stride, orientation, out);
 }
 
 static void ensure_blobs(rf_handle h) {

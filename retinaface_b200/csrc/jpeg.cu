@@ -247,3 +247,44 @@ int jpeg_decode(rf_handle h, const uint8_t *const *data, const size_t *len, int 
 }
 
 }  // namespace rf_eng
+
+// f9: the Exif orientation cv::imread applies.  Walks the marker segments up to the first scan; in the first APP1 segment that
+// starts "Exif\0\0" reads IFD0's tag 0x0112 (its first 16-bit value, as OpenCV's ExifReader does, whatever the declared type) in the
+// TIFF header's byte order.  Every read is bounds-checked against the segment, and the segment against `bytes`.
+extern "C" int rf_jpeg_exif_orientation(const uint8_t *p, size_t n) {
+    if (!p || n < 4 || p[0] != 0xFF || p[1] != 0xD8) return 1;
+    size_t i = 2;
+    while (i + 4 <= n) {
+        if (p[i] != 0xFF) return 1;
+        const uint8_t m = p[i + 1];
+        if (m == 0xFF) { i++; continue; }                                        // fill byte
+        if (m == 0x01 || (m >= 0xD0 && m <= 0xD7)) { i += 2; continue; }          // markers without a length
+        if (m == 0xDA || m == 0xD9) return 1;                                     // scan data / end of image: no Exif before it
+        const size_t len = ((size_t)p[i + 2] << 8) | p[i + 3];
+        if (len < 2 || i + 2 + len > n) return 1;
+        if (m == 0xE1 && len >= 8 && memcmp(p + i + 4, "Exif\0\0", 6) == 0) {
+            const uint8_t *t = p + i + 10;
+            const size_t tn = len - 8;
+            if (tn < 8) return 1;
+            const bool le = t[0] == 'I' && t[1] == 'I', be = t[0] == 'M' && t[1] == 'M';
+            if (!le && !be) return 1;
+            auto u16 = [&](size_t o) -> unsigned { return le ? t[o] | (t[o + 1] << 8) : (t[o] << 8) | t[o + 1]; };
+            auto u32 = [&](size_t o) -> size_t { return le ? (size_t)u16(o) | ((size_t)u16(o + 2) << 16) : ((size_t)u16(o) << 16) | u16(o + 2); };
+            if (u16(2) != 42) return 1;
+            const size_t ifd = u32(4);
+            if (ifd > tn || tn - ifd < 2) return 1;
+            const size_t cnt = u16(ifd);
+            for (size_t k = 0; k < cnt; k++) {
+                const size_t e = ifd + 2 + 12 * k;
+                if (e > tn || tn - e < 12) return 1;
+                if (u16(e) == 0x0112) {
+                    const unsigned o = u16(e + 8);
+                    return o >= 1 && o <= 8 ? (int)o : 1;
+                }
+            }
+            return 1;
+        }
+        i += 2 + len;
+    }
+    return 1;
+}

@@ -20,6 +20,7 @@
 #include <cmath>
 
 #include "postproc_dev.cuh"
+#include "preprocess.cuh"
 
 namespace rf {
 
@@ -191,12 +192,13 @@ struct MergeSet {
 };
 static_assert(sizeof(MergeSet) + 2 * sizeof(PostBuffers) + 8 <= 4096, "merge launch exceeds the classic 4 KB kernel parameter space");
 
+template <bool ORIENTED>
 __global__ void __launch_bounds__(256) k_merge(PostBuffers src, const __grid_constant__ MergeSet ms, int net_w, int net_h, PostBuffers dst) {
     const MergeSource &m = ms.src[blockIdx.x];
     const int b = ms.first + blockIdx.x;
     const int n = min(src.out_counts[b], src.max_faces);
     const float sc = m.map_back, wm1 = m.img_w_minus1;
-    const bool flip = m.flip != 0;
+    const bool flip = ORIENTED ? lb_mirrored(m.flip) : m.flip != 0;
     for (int j = threadIdx.x; j < n; j += blockDim.x) {
         const rf_face f = src.out_dets[(size_t)b * src.max_faces + j].face;
         const float cx = __fmul_rn(__fadd_rn(f.x1, f.x2), 0.5f), cy = __fmul_rn(__fadd_rn(f.y1, f.y2), 0.5f);
@@ -208,17 +210,35 @@ __global__ void __launch_bounds__(256) k_merge(PostBuffers src, const __grid_con
         rf_det d;
         d.face.score = f.score;
         const float x1 = map_back(f.x1, m.x0, sc), x2 = map_back(f.x2, m.x0, sc);    // RetinaFace.cpp:733-734: rect.x1 * scale ...
-        d.face.y1 = map_back(f.y1, m.y0, sc);
-        d.face.y2 = map_back(f.y2, m.y0, sc);
-        d.face.x1 = flip ? __fsub_rn(wm1, x2) : x1;
-        d.face.x2 = flip ? __fsub_rn(wm1, x1) : x2;
+        if (!ORIENTED) {
+            d.face.y1 = map_back(f.y1, m.y0, sc);
+            d.face.y2 = map_back(f.y2, m.y0, sc);
+            d.face.x1 = flip ? __fsub_rn(wm1, x2) : x1;
+            d.face.x2 = flip ? __fsub_rn(wm1, x1) : x2;
+        } else {
+            // displayed -> stored pixels: reflect (a reflection reverses the corners' order), then transpose
+            const float hm1 = m.img_h_minus1, y1 = map_back(f.y1, m.y0, sc), y2 = map_back(f.y2, m.y0, sc);
+            const bool fx = m.flip & LB_FLIP_X, fy = m.flip & LB_FLIP_Y, tr = m.flip & LB_TRANSPOSE;
+            const float ax1 = fx ? __fsub_rn(wm1, x2) : x1, ax2 = fx ? __fsub_rn(wm1, x1) : x2;
+            const float ay1 = fy ? __fsub_rn(hm1, y2) : y1, ay2 = fy ? __fsub_rn(hm1, y1) : y2;
+            d.face.x1 = tr ? ay1 : ax1; d.face.x2 = tr ? ay2 : ax2;
+            d.face.y1 = tr ? ax1 : ay1; d.face.y2 = tr ? ax2 : ay2;
+        }
 #pragma unroll
         for (int k = 0; k < 5; k++) {
             // mirrored source: the detector's "left eye" is the subject's right one -- swap 0<->1 and 3<->4 (2 = nose)
             const int ks = flip ? (k == 0 ? 1 : k == 1 ? 0 : k == 3 ? 4 : k == 4 ? 3 : 2) : k;
             const float x = map_back(f.lx[ks], m.x0, sc);                               // :739
-            d.face.lx[k] = flip ? __fsub_rn(wm1, x) : x;
-            d.face.ly[k] = map_back(f.ly[ks], m.y0, sc);
+            if (!ORIENTED) {
+                d.face.lx[k] = flip ? __fsub_rn(wm1, x) : x;
+                d.face.ly[k] = map_back(f.ly[ks], m.y0, sc);
+            } else {
+                const float y = map_back(f.ly[ks], m.y0, sc);
+                const float ax = (m.flip & LB_FLIP_X) ? __fsub_rn(wm1, x) : x, ay = (m.flip & LB_FLIP_Y) ? __fsub_rn(m.img_h_minus1, y) : y;
+                const bool tr = m.flip & LB_TRANSPOSE;
+                d.face.lx[k] = tr ? ay : ax;
+                d.face.ly[k] = tr ? ax : ay;
+            }
         }
         d.anchor_index = m.id_base + j;
         append_candidate(dst, m.image, d);
@@ -282,6 +302,12 @@ MergeSource view_source(int view, int max_faces, float scale, int flip, int img_
     return m;
 }
 
+MergeSource oriented_view_source(int view, int max_faces, float scale, int bits, int disp_w, int disp_h) {
+    MergeSource m = view_source(view, max_faces, scale, bits, disp_w);
+    m.img_h_minus1 = (float)(disp_h - 1);
+    return m;
+}
+
 MergeSource tile_source(int image, int tile, int max_faces, const rf_tile &t, int img_w) {
     MergeSource m{};
     m.image = image;
@@ -307,8 +333,13 @@ cudaError_t launch_merge(const PostBuffers &src, const MergeSource *src_desc, in
         MergeSet ms{};
         ms.first = b0;
         ms.nsrc = std::min(MERGE_MAX_SOURCES, n - b0);
-        for (int i = 0; i < ms.nsrc; i++) ms.src[i] = src_desc[b0 + i];
-        k_merge<<<ms.nsrc, 256, 0, s>>>(src, ms, net_w, net_h, dst);
+        bool oriented = false;
+        for (int i = 0; i < ms.nsrc; i++) {
+            ms.src[i] = src_desc[b0 + i];
+            oriented |= (ms.src[i].flip & ~LB_FLIP_X) != 0;
+        }
+        if (oriented) k_merge<true><<<ms.nsrc, 256, 0, s>>>(src, ms, net_w, net_h, dst);
+        else k_merge<false><<<ms.nsrc, 256, 0, s>>>(src, ms, net_w, net_h, dst);
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
     }

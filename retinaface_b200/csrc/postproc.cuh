@@ -69,12 +69,19 @@ void launch_nms(int n, const PostParams *params, const PostBuffers &pb, cudaStre
 // the result does not depend on which launch appended first.
 // src_desc[b] describes batch slot b, b < n.
 constexpr int RF_MAX_VIEWS_DEV = 16;
+// f9 oriented views: `flip` holds LB_* bits (preprocess.cuh) and the source is the letter-box of the DISPLAYED image T_o(img), whose
+// size is img_w x img_h (minus 1).  A kept face maps back to displayed pixels as above, then to STORED pixels: x -> img_w-1 - x under
+// LB_FLIP_X, y -> img_h-1 - y under LB_FLIP_Y (box corners swapped), then x and y trade places under LB_TRANSPOSE; left and right
+// landmarks swap when the bits mirror.  Sources with LB_FLIP_Y or LB_TRANSPOSE run in a separate instantiation of the kernel.
 struct MergeSource {
     int image, id_base, flip, shared_sides;    // shared_sides: RF_TILE_SIDE_* bits
     float x0, y0, map_back, img_w_minus1;
     float own_x0, own_y0, own_x1, own_y1;      // tile pixels; +-infinity for a view (everything owned)
+    float img_h_minus1;                        // displayed height - 1 (oriented views only)
 };
 MergeSource view_source(int view, int max_faces, float scale, int flip, int img_w);
+// a view of the image in orientation `bits`, letter-boxed from its displayed disp_w x disp_h form
+MergeSource oriented_view_source(int view, int max_faces, float scale, int bits, int disp_w, int disp_h);
 MergeSource tile_source(int image, int tile, int max_faces, const rf_tile &t, int img_w);   // tile: its index in the image's layout
 cudaError_t launch_merge(const PostBuffers &src, const MergeSource *src_desc, int n, int net_w, int net_h, const PostBuffers &dst,
                          cudaStream_t s);

@@ -71,12 +71,23 @@ __device__ __forceinline__ void src_pixel(const BgrRows &src, int, int x, int y,
 }
 __device__ __forceinline__ void src_pixel(const YuvPlanes &src, int, int x, int y, int v[3]) { yuv_pixel(src, x, y, v); }
 
+// f9: the orientation touches integer tap addresses only.  Every tap position, weight and rounding below is computed in the
+// DISPLAYED frame (sw x sh), a displayed column / row is then reflected by the item's LB_FLIP_X / LB_FLIP_Y bit, and the transposed
+// instantiation (T) reads displayed (x, y) at stored column y, stored row x -- so the bytes are those of cv::resize(T_o(img)).
+template <typename Src> __device__ __forceinline__ int col_of(const LbItemT<Src> &im, int x) { return (im.flip & LB_FLIP_X) ? im.sw - 1 - x : x; }
+template <typename Src> __device__ __forceinline__ int row_of(const LbItemT<Src> &im, int y) { return (im.flip & LB_FLIP_Y) ? im.sh - 1 - y : y; }
+template <bool T, typename Src>
+__device__ __forceinline__ void stored_pixel(const LbItemT<Src> &im, int x, int y, int v[3]) {
+    if (T) src_pixel(im.src, im.sh, y, x, v);     // packed rows of the stored image are sh (its width) pixels long
+    else src_pixel(im.src, im.sw, x, y, v);
+}
+
 // NPP's NPPI_INTER_SUPER as measured against nppiResizeSqrPixel_8u_C3R (tools/npp_dump.py, oracle/npp_oracle.cu):
 // output pixel (x, y) = the coverage-weighted mean of the source rectangle [x / f, (x + 1) / f) x [y / f, (y + 1) / f), the
 // resized extent is ceil(w f) x ceil(h f), source samples beyond the image count as ZERO (the last row / column is darker, not
 // renormalised), round half up.  Matches NPP byte for byte on 5 of 8 probe shapes and within 1 LSB on < 0.5 % of the bytes of
 // the others (NPP's own arithmetic is single precision).
-template <typename Src>
+template <bool T, typename Src>
 __device__ __forceinline__ void area_pixel(const LbItemT<Src> &im, int x, int y, int out[3]) {
     const double inv = im.scale;
     const double ax = x * inv, bx = (x + 1) * inv, ay = y * inv, by = (y + 1) * inv;
@@ -87,7 +98,7 @@ __device__ __forceinline__ void area_pixel(const LbItemT<Src> &im, int x, int y,
         for (int sx = x0; sx < x1; sx++) {
             const double w = wy * (fmin((double)(sx + 1), bx) - fmax((double)sx, ax));
             int p[3];
-            src_pixel(im.src, im.sw, im.flip ? im.sw - 1 - sx : sx, sy, p);
+            stored_pixel<T>(im, col_of(im, sx), row_of(im, sy), p);
             acc[0] += w * p[0]; acc[1] += w * p[1]; acc[2] += w * p[2];
         }
     }
@@ -96,13 +107,14 @@ __device__ __forceinline__ void area_pixel(const LbItemT<Src> &im, int x, int y,
     for (int c = 0; c < 3; c++) out[c] = min(max((int)floor(acc[c] * norm + 0.5), 0), 255);
 }
 
-template <typename Src>
-__device__ __forceinline__ void linear_pixel(const LbItemT<Src> &im, int x, const Tap &ty, int out[3]) {
+template <bool T, typename Src>
+__device__ __forceinline__ void linear_pixel(const LbItemT<Src> &im, int x, Tap ty, int out[3]) {
     Tap tx = tap_of<true>(x, im.sw, im.scale);
-    if (im.flip) { tx.s0 = im.sw - 1 - tx.s0; tx.s1 = im.sw - 1 - tx.s1; }
+    tx.s0 = col_of(im, tx.s0); tx.s1 = col_of(im, tx.s1);
+    ty.s0 = row_of(im, ty.s0); ty.s1 = row_of(im, ty.s1);
     int p00[3], p01[3], p10[3], p11[3];
-    src_pixel(im.src, im.sw, tx.s0, ty.s0, p00); src_pixel(im.src, im.sw, tx.s1, ty.s0, p01);
-    src_pixel(im.src, im.sw, tx.s0, ty.s1, p10); src_pixel(im.src, im.sw, tx.s1, ty.s1, p11);
+    stored_pixel<T>(im, tx.s0, ty.s0, p00); stored_pixel<T>(im, tx.s1, ty.s0, p01);
+    stored_pixel<T>(im, tx.s0, ty.s1, p10); stored_pixel<T>(im, tx.s1, ty.s1, p11);
 #pragma unroll
     for (int c = 0; c < 3; c++) {
         int h0 = p00[c] * tx.a0 + p01[c] * tx.a1;   // HResizeLinear
@@ -116,20 +128,33 @@ __device__ __forceinline__ void linear_pixel(const LbItemT<Src> &im, int x, cons
 // (resize.cpp: `interpolation == INTER_LINEAR && is_area_fast && iscale_x == 2 && iscale_y == 2`): output pixel (x, y) is the mean
 // of the source block [2x, 2x + 2) x [2y, 2y + 2).  A whole block rounds as the bilinear taps would, (sum + 2) >> 2; a block cut by
 // the far edge of a side of 3 mod 4 (whose halved size rounds up) averages the pixels it has, rounded half to even.
-template <typename Src>
+template <bool T, typename Src>
 __device__ __forceinline__ void half_pixel(const LbItemT<Src> &im, int x, int y, int out[3]) {
     const int nx = min(2, im.sw - 2 * x), ny = min(2, im.sh - 2 * y);
     int acc[3] = {0, 0, 0};
     for (int sy = 0; sy < ny; sy++)
         for (int sx = 0; sx < nx; sx++) {
-            const int c = 2 * x + sx;
             int p[3];
-            src_pixel(im.src, im.sw, im.flip ? im.sw - 1 - c : c, 2 * y + sy, p);
+            stored_pixel<T>(im, col_of(im, 2 * x + sx), row_of(im, 2 * y + sy), p);
             acc[0] += p[0]; acc[1] += p[1]; acc[2] += p[2];
         }
     const int cnt = nx * ny;
 #pragma unroll
     for (int c = 0; c < 3; c++) out[c] = cnt == 4 ? (acc[c] + 2) >> 2 : __float2int_rn(__fdiv_rn((float)acc[c], (float)cnt));
+}
+
+// Pixel (x, y) of the resized displayed image (inside dw x dh); ty: the vertical bilinear tap of row y (bilinear items only).
+template <bool T, typename Src>
+__device__ __forceinline__ void lb_pixel(const LbItemT<Src> &im, int x, int y, const Tap &ty, int v[3]) {
+    if (im.identity) {
+        stored_pixel<T>(im, col_of(im, x), row_of(im, y), v);
+    } else if (im.area == LB_HALF_AREA) {
+        half_pixel<T>(im, x, y, v);
+    } else if (im.area) {
+        area_pixel<T>(im, x, y, v);
+    } else {
+        linear_pixel<T>(im, x, ty, v);
+    }
 }
 
 template <typename Src>
@@ -147,25 +172,49 @@ __global__ void __launch_bounds__(128) k_letterbox_batch(const __grid_constant__
     for (int k = 0; k < 4; k++) {
         const int x = x4 + k + im.x0;
         int v[3] = {0, 0, 0};
-        if (row_in && x < im.dw) {
-            // flip: the view is the letter-box of the horizontally mirrored image -- every source column index is mirrored, the
-            // taps are those of the mirrored image (== cv::resize(cv::flip(img, 1)) bit for bit)
-            if (im.identity) {
-                src_pixel(im.src, im.sw, im.flip ? im.sw - 1 - x : x, y, v);
-            } else if (im.area == LB_HALF_AREA) {
-                half_pixel(im, x, y, v);
-            } else if (im.area) {
-                area_pixel(im, x, y, v);
-            } else {
-                linear_pixel(im, x, ty, v);
-            }
-        }
+        // flip bits: the view is the letter-box of the mirrored / upside-down image -- every source column / row index is reflected,
+        // the taps are those of the reflected image (== cv::resize(cv::flip(img, ...)) bit for bit)
+        if (row_in && x < im.dw) lb_pixel<false>(im, x, y, ty, v);
         px[3 * k] = (unsigned char)v[0]; px[3 * k + 1] = (unsigned char)v[1]; px[3 * k + 2] = (unsigned char)v[2];
     }
     uint32_t *o = reinterpret_cast<uint32_t *>(im.dst + ((size_t)blockIdx.y * net_w + x4) * 3);
     o[0] = px[0] | (px[1] << 8) | (px[2] << 16) | ((uint32_t)px[3] << 24);
     o[1] = px[4] | (px[5] << 8) | (px[6] << 16) | ((uint32_t)px[7] << 24);
     o[2] = px[8] | (px[9] << 8) | (px[10] << 16) | ((uint32_t)px[11] << 24);
+}
+
+// f9, the transposed orientations (LB_TRANSPOSE: EXIF 5..8).  Consecutive output pixels of a row read consecutive stored ROWS, so a
+// row-per-thread gather would touch one 3-byte pixel per stored row per lane.  Instead a CTA computes one 32 x 32 block of the output:
+// lane l of each warp takes output row by + l, so the 32 lanes of a warp read 32 consecutive pixels of one stored row, and the warps
+// step over the block's columns.  The block goes through shared memory (rows padded to 25 words: the lanes' byte writes fall in
+// distinct banks) and leaves as whole output rows, 24 consecutive 32-bit words each.
+constexpr int LBT_SIDE = 32, LBT_THREADS = 128, LBT_ROW_WORDS = 25;
+template <typename Src>
+__global__ void __launch_bounds__(LBT_THREADS) k_letterbox_transposed(const __grid_constant__ LbBatch<Src> B, int net_w, int net_h) {
+    __shared__ uint32_t s_blk[LBT_SIDE * LBT_ROW_WORDS];
+    const LbItemT<Src> &im = B.img[blockIdx.z];
+    unsigned char *sb = reinterpret_cast<unsigned char *>(s_blk);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int bx = blockIdx.x * LBT_SIDE, by = blockIdx.y * LBT_SIDE;
+    const int oy = by + lane, y = oy + im.y0;
+    const bool row_in = oy < net_h && y < im.dh;
+    Tap ty{};
+    if (row_in && !im.identity && !im.area) ty = tap_of<false>(y, im.sh, im.scale);
+    for (int c = warp; c < LBT_SIDE; c += LBT_THREADS / 32) {
+        const int x = bx + c + im.x0;
+        int v[3] = {0, 0, 0};
+        if (row_in && x < im.dw) lb_pixel<true>(im, x, y, ty, v);
+        unsigned char *d = sb + lane * (LBT_ROW_WORDS * 4) + 3 * c;
+        d[0] = (unsigned char)v[0]; d[1] = (unsigned char)v[1]; d[2] = (unsigned char)v[2];
+    }
+    __syncthreads();
+    constexpr int kWords = LBT_SIDE * 3 / 4;      // 24 words per output row of the block
+    for (int k = threadIdx.x; k < LBT_SIDE * kWords; k += LBT_THREADS) {
+        const int r = k / kWords, w = k - r * kWords;
+        if (by + r >= net_h) break;
+        uint32_t *o = reinterpret_cast<uint32_t *>(im.dst + ((size_t)(by + r) * net_w + bx) * 3);
+        o[w] = s_blk[r * LBT_ROW_WORDS + w];
+    }
 }
 
 }  // namespace
@@ -311,10 +360,16 @@ cudaError_t launch_letterbox_batch(const LbItemT<Src> *items, int n, int net_w, 
     constexpr int kMax = lb_limit<Src>();
     for (int i0 = 0; i0 < n; i0 += kMax) {
         const int m = std::min(kMax, n - i0);
-        LbBatch<Src> B{};
-        for (int i = 0; i < m; i++) B.img[i] = items[i0 + i];
-        dim3 grid((net_w / 4 + 127) / 128, net_h, m);
-        k_letterbox_batch<Src><<<grid, 128, 0, s>>>(B, net_w, net_h);
+        // a chunk that mixes orientations is two launches: the upright / reflected items, then the transposed ones
+        LbBatch<Src> B{}, Bt{};
+        int nb = 0, nt = 0;
+        for (int i = 0; i < m; i++) {
+            const LbItemT<Src> &it = items[i0 + i];
+            if (it.flip & LB_TRANSPOSE) Bt.img[nt++] = it;
+            else B.img[nb++] = it;
+        }
+        if (nb) k_letterbox_batch<Src><<<dim3((net_w / 4 + 127) / 128, net_h, nb), 128, 0, s>>>(B, net_w, net_h);
+        if (nt) k_letterbox_transposed<Src><<<dim3(net_w / LBT_SIDE, (net_h + LBT_SIDE - 1) / LBT_SIDE, nt), LBT_THREADS, 0, s>>>(Bt, net_w, net_h);
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
     }

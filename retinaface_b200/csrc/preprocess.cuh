@@ -57,13 +57,25 @@ constexpr int LB_MAX_IMAGES = 64, LB_MAX_FRAMES = 32;
 // bilinear taps on a side of 3 mod 4.  Tile levels of scale 0.5 use it, so that they are the cv::resize the header promises; the
 // letter-box keeps its own bytes.
 constexpr int LB_HALF_AREA = 2;
+// f9 orientations.  An item's `flip` is a set of LB_* bits over the DISPLAYED image (sw x sh, the frame the taps are computed in):
+// displayed pixel (x, y) reads stored pixel (x', y') with x' = FLIP_X ? sw-1-x : x, y' = FLIP_Y ? sh-1-y : y, swapped when
+// TRANSPOSE.  0 / LB_FLIP_X are the plain and the mirrored view.  The EXIF orientation o (rf_b200.h) is lb_orientation_bits(o).
+constexpr int LB_FLIP_X = 1, LB_FLIP_Y = 2, LB_TRANSPOSE = 4;
+// EXIF orientation 1..8 -> LB_* bits (-1 outside 1..8)
+inline int lb_orientation_bits(int o) {
+    static const int bits[9] = {-1, 0, LB_FLIP_X, LB_FLIP_X | LB_FLIP_Y, LB_FLIP_Y, LB_TRANSPOSE, LB_TRANSPOSE | LB_FLIP_X,
+                                LB_TRANSPOSE | LB_FLIP_X | LB_FLIP_Y, LB_TRANSPOSE | LB_FLIP_Y};
+    return o >= 1 && o <= 8 ? bits[o] : -1;
+}
+// whether the orientation bits mirror the image (an odd number of reflections: left and right landmarks trade places)
+__host__ __device__ inline bool lb_mirrored(int bits) { return ((bits & 1) ^ ((bits >> 1) & 1) ^ ((bits >> 2) & 1)) != 0; }
 template <typename Src>
 struct LbItemT {
     using Source = Src;
     Src src; uint8_t *dst;
-    int sw, sh, dw, dh;
+    int sw, sh, dw, dh;   // sw x sh: the DISPLAYED source size (stored h x w when LB_TRANSPOSE)
     double scale;
-    int identity, flip, area;   // area: 0 bilinear, 1 NPP super-sampling, LB_HALF_AREA OpenCV's 2x fast area path (tiles only)
+    int identity, flip, area;   // flip: LB_* bits; area: 0 bilinear, 1 NPP super-sampling, LB_HALF_AREA OpenCV's 2x fast area path (tiles only)
     int16_t x0, y0;     // 16 bits keep 64 BGR items within 4 KB; origins are below the largest level side (16384)
 };
 // u8 BGR rows `pitch` bytes apart, read in place: a caller's device image that may be a view of a larger allocation (f8)

@@ -14,7 +14,7 @@ from typing import List, Sequence
 
 import numpy as np
 
-from .capi import RF_PREC_FP16, Engine
+from .capi import ANY_ORIENTATION, RF_PREC_FP16, Engine
 
 
 @dataclass
@@ -98,6 +98,25 @@ class RetinaFace:
             return []
         views = [(float(s), f) for s in scales for f in ((False, True) if flip else (False,))]
         faces, _, _ = self.engine.detect_views(img, views, threshold, self.nms_threshold)
+        return [FaceDetectInfo.from_row(r) for r in faces]
+
+    def detectOriented(self, imgs: Sequence[np.ndarray], orientations: Sequence[int], threshold: float = 0.5, align: dict = None) -> List[list]:
+        """f9 rotated and mirrored images: image i as stored, shown in EXIF orientation ``orientations[i]`` (1..8, what cv::imread
+        applies; ``capi.exif_orientation`` reads it from JPEG bytes).  Per image, the faces in DISPLAYED image pixels, found and
+        cropped without a rotated copy (rf_detect_oriented_batch); with ``align`` (``Engine.detect_align``'s keywords), a list of
+        ``(FaceDetectInfo, crop)`` cut from the displayed image."""
+        out = self.engine.detect_oriented(list(imgs), list(orientations), threshold, self.nms_threshold, align=align)
+        if align is None:
+            return [[FaceDetectInfo.from_row(r) for r in per] for per in out]
+        return [[(FaceDetectInfo.from_row(r), c) for r, c in zip(f, cs)] for f, cs in zip(out[0], out[1])]
+
+    def detectAnyOrientation(self, img: np.ndarray, threshold: float = 0.5) -> List[FaceDetectInfo]:
+        """f9 unknown orientation: the image in its four rotations (EXIF 1, 6, 3, 8) as one batch, merged on the GPU
+        (rf_detect_views_oriented).  Faces in STORED image pixels, landmarks on the subject's sides, so an aligned crop of a
+        sideways face comes out upright."""
+        if img is None or img.size == 0:
+            return []
+        faces, _, _ = self.engine.detect_views_oriented(img, [(1.0, o) for o in ANY_ORIENTATION], threshold, self.nms_threshold)
         return [FaceDetectInfo.from_row(r) for r in faces]
 
     @staticmethod

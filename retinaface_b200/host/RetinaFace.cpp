@@ -241,6 +241,45 @@ vector<FaceDetectInfo> RetinaFace::detectInImage(const Mat &img, float threshold
     return out;
 }
 
+void RetinaFace::detectOriented(const vector<Mat> &imgs, const vector<int> &orientations, float threshold, const AlignOptions *align) {
+    if (orientations.size() != imgs.size()) throw std::invalid_argument("detectOriented: one orientation per image");
+    last_.assign(imgs.size(), vector<FaceDetectInfo>());
+    scales_.assign(imgs.size(), 1.f);
+    crops_.assign(imgs.size(), vector<Mat>());
+    int per = 0, cw = 0, ch = 0;
+    const rf_align_params p = align ? crop_params(*align, opt_.max_faces, &per, &cw, &ch) : rf_align_params{};
+    const size_t mb = (size_t)opt_.max_batch;
+    vector<unsigned char> crops(align ? mb * per * cw * ch * 3 : 0);
+    for (size_t start = 0; start < imgs.size(); start += mb) {
+        const int n = (int)std::min(mb, imgs.size() - start);
+        vector<const uint8_t *> ptrs(n);
+        vector<int> ws(n), hs(n), strides(n);
+        for (int i = 0; i < n; i++) {
+            const cv::Mat &m = imgs[start + i];
+            if (m.empty()) throw std::runtime_error("detectOriented: empty image");
+            ptrs[i] = m.data; ws[i] = m.cols; hs[i] = m.rows; strides[i] = (int)m.step;
+        }
+        int rc = rf_detect_oriented_batch(h_, ptrs.data(), ws.data(), hs.data(), strides.data(), orientations.data() + start, n, threshold,
+                                          nms_threshold, align ? &p : nullptr, out_faces_.data(), out_counts_.data(), nullptr,
+                                          align ? crops.data() : nullptr, nullptr);
+        if (rc != RF_OK) throw std::runtime_error(string("rf_detect_oriented_batch: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+        keepResults(start, n, align ? crops.data() : nullptr, per, cw, ch);
+    }
+}
+
+vector<FaceDetectInfo> RetinaFace::detectAnyOrientation(const Mat &img, float threshold) {
+    vector<FaceDetectInfo> out;
+    if (img.empty()) return out;
+    const rf_oriented_view views[4] = {{1.f, 1}, {1.f, 6}, {1.f, 3}, {1.f, 8}};
+    int count = 0;
+    int rc = rf_detect_views_oriented(h_, img.data, img.cols, img.rows, (int)img.step, views, 4, threshold, nms_threshold, out_faces_.data(),
+                                      &count, nullptr, nullptr);
+    if (rc != RF_OK) throw std::runtime_error(string("rf_detect_views_oriented: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+    const FaceDetectInfo *f = reinterpret_cast<const FaceDetectInfo *>(out_faces_.data());
+    out.assign(f, f + count);
+    return out;
+}
+
 Mat RetinaFace::draw(const Mat &img, const vector<FaceDetectInfo> &faces) {
     Mat out = img.clone();     // RetinaFace.cpp:744: drawing on the caller's image would accumulate boxes
     auto fill = [&out](int x0, int y0, int x1, int y1, unsigned char b, unsigned char g, unsigned char r) {

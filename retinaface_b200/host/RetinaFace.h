@@ -92,6 +92,13 @@ class RetinaFace {
     // (lastScale() is 1) and, with `align` (rf_detect_tiled_align), lastCrops() the crops as detectAndAlign leaves them.
     void detectTiled(const vector<Mat> &imgs, float threshold = 0.5, const vector<float> &scales = vector<float>(), bool flip = false,
                      int overlap = 0, const AlignOptions *align = nullptr);
+    // f9 rotated and mirrored images (rf_detect_oriented_batch): imgs[i] as stored, shown in EXIF orientation orientations[i] (1..8,
+    // what cv::imread applies; rf_jpeg_exif_orientation reads it from JPEG bytes).  Afterwards lastBatchFaces() holds the faces in
+    // DISPLAYED image pixels (lastScale() is 1) and, with `align`, lastCrops() the crops of the displayed image.  No rotated copy is made.
+    void detectOriented(const vector<Mat> &imgs, const vector<int> &orientations, float threshold = 0.5, const AlignOptions *align = nullptr);
+    // f9 unknown orientation (rf_detect_views_oriented): the image in its four rotations (EXIF 1, 6, 3, 8) as one batch, merged on
+    // the GPU; faces in STORED image pixels, landmarks on the subject's sides (an aligned crop of a sideways face comes out upright).
+    vector<FaceDetectInfo> detectAnyOrientation(const Mat &img, float threshold = 0.5);
     // the reference's visualisation (RetinaFace.cpp:730-741): red box outline (thickness 2), green landmark dots, on a clone
     static Mat draw(const Mat &img, const vector<FaceDetectInfo> &faces);
     int netWidth() const { return opt_.net_w; }

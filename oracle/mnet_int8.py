@@ -56,6 +56,13 @@ def quant_weights(w):
     return qw, sw
 
 
+def int_gemm(a, b):
+    """Exact integer product a @ b of int32 matrices whose entries are within [-127, 127], as int64.  Multiplied in
+    float64 so that numpy hands it to BLAS (it has no BLAS path for integers): every product and every partial sum is an
+    integer far below 2**53, so each is exact in any summation order."""
+    return (a.astype(np.float64) @ b.astype(np.float64)).astype(np.int64)
+
+
 def _im2col(q, k, pad):
     """q: (n,c,h,w) int32 -> (n, h*w, k*k*c) with K ordered (tap, channel); stride 1."""
     n, c, h, w = q.shape
@@ -85,7 +92,7 @@ class Int8Oracle:
         qw, sw = quant_weights(w)
         n, c, h, wd = q_in.shape
         cols = _im2col(q_in, k, k // 2)
-        acc = cols.astype(np.int64) @ qw.T.astype(np.int64)                               # exact integer GEMM
+        acc = int_gemm(cols, qw.T)                                                        # exact integer GEMM
         assert np.abs(acc).max() < 2 ** 24
         res, o0 = [], 0
         for (cn, s_out, relu) in outs:
@@ -141,13 +148,18 @@ class Int8Oracle:
                 full[:, :, ky:ky + 2 * uh:2, kx:kx + 2 * uw:2] += (q_up.astype(F) * wq[None, :, ky, kx, None, None]).astype(F)
         return np.clip(np.rint(full[:, :, 1:1 + h, 1:1 + wd]), -127, 127).astype(np.int32)
 
-    def ssh(self, q_in, s_in, lv):
+    def ssh(self, q_in, s_in, lv, tens=None):
+        """The SSH context head of one level -> (concat, its scale); `tens`, when given, also receives the two quantised
+        context tensors inside the head."""
         p = f"rf_{lv}_det"
         s_cat = self.t[p + "_concat_relu"]
         s_c1, s_c31 = self.t[p + "_context_conv1_relu"], self.t[p + "_context_conv3_1_relu"]
         det, ctx1 = self.gemm_conv(q_in, s_in, [p + "_conv1", p + "_context_conv1"], [(32, s_cat, True), (16, s_c1, True)])
         c2, c31 = self.gemm_conv(ctx1, s_c1, [p + "_context_conv2", p + "_context_conv3_1"], [(16, s_cat, True), (16, s_c31, True)])
         c32, = self.gemm_conv(c31, s_c31, [p + "_context_conv3_2"], [(16, s_cat, True)])
+        if tens is not None:
+            tens[p + "_context_conv1_relu"] = (ctx1, s_c1)
+            tens[p + "_context_conv3_1_relu"] = (c31, s_c31)
         return np.concatenate([det, c2, c32], axis=1), s_cat
 
     def heads(self, q_cat, s_cat, stride):
@@ -169,9 +181,10 @@ class Int8Oracle:
         """q_stem: optional int32 (n,16,h/2,w/2) stem output to continue from (lets a test separate the FP32 stem,
         whose summation order differs between implementations, from the bit-exact integer part)."""
         t = self.t
-        q, s = self.stem(img_u8_nhwc)
-        if q_stem is not None:
-            q = np.asarray(q_stem, dtype=np.int32)
+        if q_stem is None:
+            q, s = self.stem(img_u8_nhwc)
+        else:
+            q, s = np.asarray(q_stem, dtype=np.int32), t["mobilenet0_relu2_fwd"]
         tens = {"mobilenet0_relu2_fwd": (q, s)}
         feats = {}
         for i in range(3, 27, 2):
@@ -182,13 +195,13 @@ class Int8Oracle:
         lat3, = self.gemm_conv(*feats[26], ["rf_c3_lateral"], [(64, t["rf_c3_lateral_relu"], True)])
         lat2, = self.gemm_conv(*feats[22], ["rf_c2_lateral"], [(64, t["rf_c2_lateral_relu"], True)])
         lat1, = self.gemm_conv(*feats[10], ["rf_c1_red_conv"], [(64, t["rf_c1_red_conv_relu"], True)])
-        cat3, s3 = self.ssh(lat3, t["rf_c3_lateral_relu"], "c3")
+        cat3, s3 = self.ssh(lat3, t["rf_c3_lateral_relu"], "c3", tens)
         plus0 = self.merge(lat2, t["rf_c2_lateral_relu"], lat3, t["rf_c3_lateral_relu"], 0, t["_plus0"])
         aggr2, = self.gemm_conv(plus0, t["_plus0"], ["rf_c2_aggr"], [(64, t["rf_c2_aggr_relu"], True)])
-        cat2, s2 = self.ssh(aggr2, t["rf_c2_aggr_relu"], "c2")
+        cat2, s2 = self.ssh(aggr2, t["rf_c2_aggr_relu"], "c2", tens)
         plus1 = self.merge(lat1, t["rf_c1_red_conv_relu"], aggr2, t["rf_c2_aggr_relu"], 1, t["_plus1"])
         aggr1, = self.gemm_conv(plus1, t["_plus1"], ["rf_c1_aggr"], [(64, t["rf_c1_aggr_relu"], True)])
-        cat1, s1 = self.ssh(aggr1, t["rf_c1_aggr_relu"], "c1")
+        cat1, s1 = self.ssh(aggr1, t["rf_c1_aggr_relu"], "c1", tens)
         tens.update({"rf_c3_lateral_relu": (lat3, t["rf_c3_lateral_relu"]), "rf_c2_lateral_relu": (lat2, t["rf_c2_lateral_relu"]),
                      "rf_c1_red_conv_relu": (lat1, t["rf_c1_red_conv_relu"]), "_plus0": (plus0, t["_plus0"]),
                      "rf_c2_aggr_relu": (aggr2, t["rf_c2_aggr_relu"]), "_plus1": (plus1, t["_plus1"]),

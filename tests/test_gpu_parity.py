@@ -404,7 +404,7 @@ def test_int8_engine_vs_integer_oracle(golden_image, post_oracle):
     result against the FP32 golden detections of the reference's model -- the calibration's own tolerance: same
     5 faces, boxes within 2 px, scores within 0.03."""
     from oracle.mnet_int8 import Int8Oracle
-    from retinaface_b200 import RF_PREC_INT8, Engine
+    from retinaface_b200 import RF_PREC_INT8, Engine, RfError
     table = os.path.join(GOLDEN, "weights", "mnet-deconv-0517.table.int8")
     inp = letterbox_bgr_u8(golden_image, 448, 448)
     batch = np.stack([inp, np.roll(inp, 24, axis=1)])
@@ -418,11 +418,17 @@ def test_int8_engine_vs_integer_oracle(golden_image, post_oracle):
         d = np.abs(stem_gpu - stem_ref)
         assert d.max() <= 1 and (d > 0).mean() < 1e-3, (d.max(), (d > 0).mean())
         o_heads, o_t = oracle.forward(batch, want_tensors=True, q_stem=stem_gpu)
+        compared = 0
         for name, (q, s) in o_t.items():
-            if name in ("_plus0", "_plus1", "mobilenet0_relu2_fwd"):
-                continue          # the FPN sums are fused into the aggr conv's staging at this batch size
-            got = eng.debug_tensor(name, 2)
+            if name == "mobilenet0_relu2_fwd":
+                continue          # the engine's own stem output, which the oracle continued from
+            try:
+                got = eng.debug_tensor(name, 2)
+            except RfError:
+                continue          # an FPN sum the plan does not materialise
+            compared += 1
             assert np.array_equal(got, q), (name, np.abs(got - q).max(), (got != q).mean())
+        assert compared >= 26
         for k in range(9):
             assert np.abs(heads[k] - o_heads[k]).max() < 1e-4, (k, np.abs(heads[k] - o_heads[k]).max())
         faces, idx = eng.detect_batch(list(batch), 0.9, 0.4, want_index=True)

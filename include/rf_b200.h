@@ -450,6 +450,92 @@ int rf_detect_views_oriented(rf_handle h, const uint8_t *bgr, int width, int hei
  * rf_decode_jpeg or their own decoder. */
 int rf_jpeg_exif_orientation(const uint8_t *jpeg, size_t bytes);
 
+/* f10 face tracking across video frames, on the GPU: per-video tracks with stable ids, so that a recogniser runs once per new
+ * identity instead of once per face per frame, and counting / dwell time / "who entered" need no host round trip.  One tracker holds
+ * max_videos independent sequences (cameras, files), each with up to max_tracks live tracks (tentative, confirmed and lost).
+ *
+ * Definition: ByteTrack's association (Zhang et al., 2022) with SORT's constant-velocity Kalman filter, in FP64, stated exactly so
+ * that a scalar restatement reproduces every bit.  Per track and per coordinate c of (cx, cy, a = w / h, h): position m, velocity u and
+ * a 2 x 2 covariance (P00, P01, P11) -- ByteTrack's 8 x 8 filter, which decouples into these four scalar filters.  With h the track's
+ * current height m_h, sp = 1 / 20 and sv = 1 / 160:
+ *   predict  (a LOST track first has u_h = 0) q_pos = sp * h (1e-2 for a), q_vel = sv * h (1e-5 for a);
+ *            P00 = ((P00 + P01) + (P01 + P11)) + q_pos * q_pos, P01 = P01 + P11, P11 = P11 + q_vel * q_vel, m = m + u
+ *   update   r = sp * h (1e-1 for a), S = P00 + r * r, K0 = P00 / S, K1 = P01 / S, y = z - m, m += K0 * y, u += K1 * y,
+ *            P00 -= (K0 * S) * K0, P01 -= (K0 * S) * K1, P11 -= (K1 * S) * K1   (q and r use h before the step)
+ *   birth    m = z, u = 0, P00 = ((2 * sp) * h)^2 (1e-2^2 for a), P11 = ((10 * sv) * h)^2 (1e-5^2 for a), P01 = 0
+ *   z        from a record's float box in frame pixels, widened to double: w = x2 - x1, h = y2 - y1, cx = x1 + w / 2, cy = y1 + h / 2
+ *            (records with w <= 0 or h <= 0 are ignored)
+ *   box      of a mean: w = a * h, x1 = cx - w / 2, y1 = cy - h / 2, x2 = x1 + w, y2 = y1 + h
+ * The match score is the IoU, in FP64, of a track's predicted box and a record's box with the reference NMS's +1 pixel convention.
+ * Per frame of a video, after predicting every live track, with the frame's records (best score first; index = record index):
+ *   1. records with score >= high_thresh are HIGH, the others LOW;
+ *   2. CONFIRMED and LOST tracks against HIGH records, matched when IoU > iou_high;
+ *   3. tracks CONFIRMED at frame start and still unmatched against LOW records, IoU > iou_low;
+ *   4. TENTATIVE tracks against the remaining HIGH records, IoU > iou_tentative; an unmatched TENTATIVE track is removed;
+ *   5. matched tracks: Kalman update, hits + 1, lost_frames = 0, the record's face kept; LOST and TENTATIVE ones become CONFIRMED
+ *      (a LOST one keeps its id);
+ *   6. unmatched CONFIRMED tracks become LOST (lost_frames = 1), unmatched LOST ones count lost_frames + 1; a LOST track is removed
+ *      when lost_frames exceeds max_lost;
+ *   7. each remaining HIGH record with score >= new_thresh, in record order, starts a track with the video's next id (ids start at 1
+ *      and are not reused before a reset), TENTATIVE -- CONFIRMED on the video's first frame since create or reset.  Without a free
+ *      slot the birth is skipped and the video's overflow counter (rf_tracker_debug_state) counts it.
+ * Each stage is greedy by descending IoU: the highest-IoU pair whose track and record are both free is matched, and so on; ties go
+ * to the lower track id, then the lower record index.  This equals ByteTrack's optimal assignment whenever no track has two
+ * candidates above the threshold (the usual case for faces, which NMS keeps apart), and is deterministic.  ByteTrack's score fusion
+ * and duplicate-track removal are not part of it.  age counts the frames since birth, the birth frame included. */
+typedef struct rf_tracker_s *rf_tracker;
+typedef struct rf_track_config {
+    int max_videos;                 /* 1..4096 */
+    int max_tracks;                 /* per video, LOST included; 0 -> 64, at most 1024 */
+    float high_thresh, new_thresh;  /* 0 -> 0.6, 0.7; else in (0, 1] */
+    float iou_high, iou_low, iou_tentative;   /* 0 -> 0.2, 0.5, 0.3; else in (0, 1] */
+    int max_lost;                   /* frames; 0 -> 30 */
+} rf_track_config;
+#define RF_TRACK_TENTATIVE 0
+#define RF_TRACK_CONFIRMED 1
+#define RF_TRACK_LOST      2
+typedef struct rf_track {
+    int32_t id, state;              /* per-video id; RF_TRACK_* */
+    int32_t det;                    /* index of the record matched on this frame, -1 */
+    int32_t crop_slot;              /* this frame's crop j of the track, -1 */
+    int32_t hits, age, lost_frames, reserved;
+    float kx1, ky1, kx2, ky2;       /* filtered box (mean after this frame), frame pixels */
+    float vx, vy;                   /* centre velocity, pixels per frame */
+    rf_face face;                   /* last matched detection, frame pixels */
+} rf_track;
+/* Creates a tracker on the handle's device (state of every video zeroed).  Bad config: RF_ERR_INVALID_ARG. */
+int  rf_tracker_create(rf_handle h, const rf_track_config *cfg, rf_tracker *out);
+void rf_tracker_destroy(rf_tracker t);                 /* before rf_destroy of its handle; waits for the tracker's work */
+/* Restarts one video (ids from 1, first-frame rule) or all (-1).  Asynchronous, ordered after every update issued before it. */
+int  rf_tracker_reset(rf_tracker t, int video);
+/* Applies n frames of device records to the tracker: the records of any device detect call on the handle (rf_detect_batch_device,
+ * rf_detect_yuv_batch_device, the oriented and tiled device calls, the all-gather call), laid out [n][max_faces] as they return them,
+ * kept counts dev_counts [n].  Frame i belongs to video videos[i]; a video may appear more than once, its frames then apply in call
+ * order.  Coordinates map to frame pixels as __fmul_rn(x, scales[i]) (f5's map-back); scales == NULL means 1 (tiled records, already
+ * in image pixels).  Asynchronous, issued on rf_last_stream(), where the records complete; updates are ordered among themselves
+ * whatever context they land on (an event chain), forwards still overlap.  *dev_tracks -> [n][max_tracks] rf_track: frame i's list
+ * holds every live track after that frame, sorted by id, *dev_track_counts -> [n] int32 its length; crop_slot is -1.  The outputs live
+ * in a ring of `streams` slots and stay valid for `streams` further tracker calls.  n = 0 launches nothing.  A video outside
+ * [0, max_videos), n > max_batch (RF_ERR_CAPACITY), NULL arrays, a non-finite or non-positive scale: an error status before anything
+ * is launched. */
+int  rf_track_update(rf_tracker t, const int *videos, int n, const rf_det *dev_dets, const int32_t *dev_counts,
+                     const float *scales, const rf_track **dev_tracks, const int32_t **dev_track_counts);
+/* rf_detect_yuv_batch_device (same context rotation; *dev_dets, *dev_counts and out_scales as there), then rf_track_update of its
+ * records on the same context.  align != NULL: crops only for the tracks that became CONFIRMED on this frame -- new identities, not
+ * LOST tracks found again -- compacted per frame in id order into dev_crops [n][A][crop bytes] (A and formats as
+ * rf_detect_align_batch_device; dev_mats optional [n][A][6]); each such track's crop_slot says where its crop is, and crops beyond A
+ * are not cut (crop_slot -1).  A crop is the one rf_detect_yuv_batch_device cuts for the matched record, byte for byte.  Statuses of
+ * both calls, before anything is launched. */
+int  rf_detect_yuv_track_device(rf_handle h, rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, int matrix,
+                                float score_threshold, float nms_threshold, const rf_align_params *align, void *dev_crops,
+                                double *dev_mats, const rf_track **dev_tracks, const int32_t **dev_track_counts,
+                                const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales);
+/* Parity aid, blocking (waits for every issued update): video's FP64 state into out (cap doubles).  out[0..3] = live tracks, next id,
+ * frames since reset, births skipped for want of a slot; then per live track in id order RF_TRACK_DEBUG_DOUBLES values: id, state,
+ * hits, age, lost_frames, m[4], u[4], P00[4], P01[4], P11[4] (coordinates cx, cy, a, h).  Returns the live track count. */
+#define RF_TRACK_DEBUG_DOUBLES 25
+int  rf_tracker_debug_state(rf_tracker t, int video, double *out, int cap);
+
 /* Introspection. */
 int rf_get_net_size(rf_handle h, int *net_w, int *net_h, int *max_batch, int *max_faces);
 int rf_num_anchors(rf_handle h);            /* per image: 8,232 @448x448, 47,040 @1280x896 */

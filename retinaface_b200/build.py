@@ -25,6 +25,7 @@ SOURCES = [
     ("postproc.cu", ["-fmad=false"]),
     ("preprocess.cu", ["-fmad=false"]),
     ("align.cu", ["-fmad=false"]),      # cv::warpAffine's coordinates and the similarity fit: multiply and add, never fused
+    ("track.cu", ["-fmad=false"]),      # the tracker's FP64 Kalman filter and IoU: every step one rounding, as oracle/track.py states it
     ("calibrate.cu", []),
     ("model.cpp", []),
     ("frontend.cpp", []),

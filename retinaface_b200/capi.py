@@ -32,6 +32,7 @@ EXPORTS = [
     "rf_detect_tiled_align", "rf_detect_yuv_tiled_align", "rf_detect_tiled_device", "rf_detect_yuv_tiled_device",
     "rf_detect_oriented_batch", "rf_detect_yuv_oriented_device", "rf_preprocess_oriented", "rf_preprocess_yuv_oriented",
     "rf_detect_views_oriented", "rf_jpeg_exif_orientation",
+    "rf_tracker_create", "rf_tracker_destroy", "rf_tracker_reset", "rf_track_update", "rf_detect_yuv_track_device", "rf_tracker_debug_state",
 ]
 COMM_BLOB_BYTES = 128
 
@@ -187,6 +188,28 @@ def tile_layout(net_w: int, net_h: int, width: int, height: int, levels=None, ov
     return [tile_dict(out[i]) for i in range(k)]
 
 
+class TrackConfig(C.Structure):  # rf_track_config
+    _fields_ = [("max_videos", C.c_int), ("max_tracks", C.c_int), ("high_thresh", C.c_float), ("new_thresh", C.c_float),
+                ("iou_high", C.c_float), ("iou_low", C.c_float), ("iou_tentative", C.c_float), ("max_lost", C.c_int)]
+
+
+class Face(C.Structure):         # rf_face
+    _fields_ = [("score", C.c_float), ("x1", C.c_float), ("y1", C.c_float), ("x2", C.c_float), ("y2", C.c_float),
+                ("lx", C.c_float * 5), ("ly", C.c_float * 5)]
+
+
+class TrackRecord(C.Structure):  # rf_track
+    _fields_ = [(f, C.c_int32) for f in ("id", "state", "det", "crop_slot", "hits", "age", "lost_frames", "reserved")] + \
+               [(f, C.c_float) for f in ("kx1", "ky1", "kx2", "ky2", "vx", "vy")] + [("face", Face)]
+
+
+TRACK_TENTATIVE, TRACK_CONFIRMED, TRACK_LOST = 0, 1, 2      # RF_TRACK_*
+TRACK_DEBUG_DOUBLES = 25                                     # RF_TRACK_DEBUG_DOUBLES
+# one rf_track as a numpy record (the layout of TrackRecord)
+TRACK_DTYPE = np.dtype([(f, "<i4") for f in ("id", "state", "det", "crop_slot", "hits", "age", "lost_frames", "reserved")] +
+                       [(f, "<f4") for f in ("kx1", "ky1", "kx2", "ky2", "vx", "vy")] + [("face", "<f4", (FACE_FLOATS,))])
+
+
 class RfError(RuntimeError):
     def __init__(self, status: int, msg: str):
         super().__init__(f"librf_b200 status {status}: {msg}")
@@ -306,6 +329,16 @@ def load_library() -> C.CDLL:
     lib.rf_detect_views_oriented.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(_OrientedView), C.c_int, C.c_float,
                                              C.c_float, C.c_void_p, C.POINTER(C.c_int), C.c_void_p, C.c_void_p]
     lib.rf_jpeg_exif_orientation.argtypes = [C.c_void_p, C.c_size_t]
+    lib.rf_tracker_create.argtypes = [C.c_void_p, C.POINTER(TrackConfig), C.POINTER(C.c_void_p)]
+    lib.rf_tracker_destroy.argtypes = [C.c_void_p]
+    lib.rf_tracker_destroy.restype = None
+    lib.rf_tracker_reset.argtypes = [C.c_void_p, C.c_int]
+    lib.rf_track_update.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p),
+                                    C.POINTER(C.c_void_p)]
+    lib.rf_detect_yuv_track_device.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(YuvFrame), C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float,
+                                               C.POINTER(AlignParams), C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                               C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_void_p]
+    lib.rf_tracker_debug_state.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
     _lib = lib
     return lib
 
@@ -960,6 +993,12 @@ class Engine:
                                                       C.c_void_p(view_of.ctypes.data), C.c_void_p(scales.ctypes.data)))
         return faces[:count.value].copy(), view_of[:count.value].copy(), scales[:nv].copy()
 
+    # -- f10 face tracking across video frames ---------------------------------------------------------------------------------
+    def tracker(self, max_videos: int = 1, max_tracks: int = 0, high_thresh: float = 0.0, new_thresh: float = 0.0, iou_high: float = 0.0,
+                iou_low: float = 0.0, iou_tentative: float = 0.0, max_lost: int = 0) -> "Tracker":
+        """rf_tracker_create: a tracker of max_videos independent sequences on this engine (0 -> the defaults of rf_track_config)."""
+        return Tracker(self, TrackConfig(max_videos, max_tracks, high_thresh, new_thresh, iou_high, iou_low, iou_tentative, max_lost))
+
     def calibrate_int8(self, images: np.ndarray, out_table: str):
         """INT8 entropy calibration on an RF_PREC_FP32 engine; writes a TensorRT-format table."""
         images = np.ascontiguousarray(images, dtype=np.uint8)
@@ -991,3 +1030,83 @@ class Engine:
             nm = names.raw[64 * i:64 * (i + 1)].split(b"\0", 1)[0].decode()
             out.append(dict(name=nm, ms=float(ms[i]), bytes=float(by[i]), flops=float(fl[i])))
         return out
+
+
+class _DevArray:
+    def __init__(self, ptr, shape, typestr):
+        self.__cuda_array_interface__ = dict(shape=shape, typestr=typestr, data=(ptr, False), version=3)
+
+
+class Tracker:
+    """One rf_tracker of an Engine: per-video face tracks with stable ids, updated on the GPU.  Close it before its engine."""
+
+    def __init__(self, engine: Engine, cfg: TrackConfig):
+        self.engine, self.lib = engine, engine.lib
+        t = C.c_void_p()
+        engine._check(self.lib.rf_tracker_create(engine.h, C.byref(cfg), C.byref(t)))
+        self.t = t
+        self.max_videos = cfg.max_videos
+        self.max_tracks = cfg.max_tracks or 64
+
+    def close(self):
+        if getattr(self, "t", None):
+            self.lib.rf_tracker_destroy(self.t)
+            self.t = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    @staticmethod
+    def _ints(vals, n):
+        v = [int(x) for x in vals]
+        if len(v) != n:
+            raise ValueError(f"{n} frames but {len(v)} video indices")
+        return (C.c_int * max(n, 1))(*v)
+
+    def update(self, videos: Sequence[int], dets_ptr: int, counts_ptr: int, scales=None):
+        """rf_track_update on the device records of a detect call (frame i of video videos[i]; scales: the map-back factor of each
+        frame, None for records already in image pixels).  Asynchronous.  Returns the (tracks_ptr, track_counts_ptr) device addresses."""
+        n = len(videos)
+        sc = None if scales is None else np.ascontiguousarray(scales, dtype=np.float32)
+        if sc is not None and sc.size != n:
+            raise ValueError(f"{n} frames but {sc.size} scales")
+        tp, cp = C.c_void_p(), C.c_void_p()
+        self.engine._check(self.lib.rf_track_update(self.t, self._ints(videos, n), n, dets_ptr, counts_ptr, sc.ctypes.data if sc is not None else None,
+                                                    C.byref(tp), C.byref(cp)))
+        return int(tp.value or 0), int(cp.value or 0)
+
+    def detect_yuv_device(self, frames, videos: Sequence[int], thr: float, nms_thr: float, layout: str = "nv12", matrix="bt601",
+                          align: Optional[dict] = None, dev_crops_ptr: Optional[int] = None, dev_mats_ptr: Optional[int] = None):
+        """rf_detect_yuv_track_device: Engine.detect_yuv_device on device 4:2:0 frames, then the update; with align, the crops of the
+        tracks confirmed on each frame at dev_crops_ptr [n][A].  Returns (tracks_ptr, track_counts_ptr, dets_ptr, counts_ptr, scales)."""
+        n = len(frames)
+        arr = self.engine._frames(frames, layout, True)
+        p = align_params(**align) if align is not None else None
+        scales = np.zeros(max(n, 1), dtype=np.float32)
+        tp, tc, d, c = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
+        self.engine._check(self.lib.rf_detect_yuv_track_device(self.engine.h, self.t, arr, self._ints(videos, n), n, _matrix(matrix), thr, nms_thr,
+                                                               C.byref(p) if p is not None else None, dev_crops_ptr, dev_mats_ptr, C.byref(tp),
+                                                               C.byref(tc), C.byref(d), C.byref(c), scales.ctypes.data))
+        return int(tp.value or 0), int(tc.value or 0), int(d.value or 0), int(c.value or 0), scales[:n].copy()
+
+    def reset(self, video: int = -1):
+        """rf_tracker_reset: restart one video (ids from 1), or all with -1; ordered after every issued update."""
+        self.engine._check(self.lib.rf_tracker_reset(self.t, int(video)))
+
+    def debug_state(self, video: int):
+        """rf_tracker_debug_state (blocking): (header [live, next id, frames, overflow], (live, 25) float64 per-track rows in id order)."""
+        cap = 4 + TRACK_DEBUG_DOUBLES * self.max_tracks
+        out = np.zeros(cap, dtype=np.float64)
+        k = self.engine._check(self.lib.rf_tracker_debug_state(self.t, int(video), out.ctypes.data, cap))
+        return out[:4].copy(), out[4:4 + k * TRACK_DEBUG_DOUBLES].reshape(k, TRACK_DEBUG_DOUBLES).copy()
+
+    def read(self, tracks_ptr: int, counts_ptr: int, n: int) -> List[np.ndarray]:
+        """The track lists of n frames of an update's outputs (TRACK_DTYPE records), copied to the host after the last stream."""
+        import torch
+        self.engine._check(self.lib.rf_synchronize(self.engine.h))
+        raw = torch.as_tensor(_DevArray(tracks_ptr, (n, self.max_tracks * TRACK_DTYPE.itemsize), "|u1"), device="cuda").cpu().numpy()
+        counts = torch.as_tensor(_DevArray(counts_ptr, (n,), "<i4"), device="cuda").cpu().numpy()
+        return [raw[i].view(TRACK_DTYPE)[:counts[i]].copy() for i in range(n)]

@@ -9,6 +9,7 @@
 #include "engine_internal.cuh"
 #include "calibrate.cuh"
 #include "preprocess.cuh"
+#include "track.cuh"
 
 namespace rf_eng {
 
@@ -2005,6 +2006,243 @@ int rf_profile_layers(rf_handle h, int n, int iters, char (*names)[64], float *m
         CK(cudaStreamSynchronize(c.stream));
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return cnt;
+}
+
+// ---- f10 face tracking across video frames (track.cuh) ---------------------------------------------------------------------------
+// The tracker owns every video's state and a ring of output slots.  Its kernels are ordered by an event chain: each update (and
+// each reset) waits for `chain` on the stream it is issued on, which may belong to any context, and records it again, so the state
+// of a video is only ever touched by one launch at a time while the forwards of the contexts still overlap.  A slot's `free` is
+// recorded once its due faces have been cropped; the next call on that slot waits for it.
+struct rf_tracker_s {
+    rf_handle h = nullptr;
+    rf_track_config cfg{};             // defaults applied
+    TrackVideo *d_videos = nullptr;    // [max_videos]
+    TrackState *d_state = nullptr;     // [max_videos][max_tracks]
+    TrackPair *d_pairs = nullptr;      // [ctas][max_tracks * max_faces]
+    int *d_order = nullptr;
+    struct Slot {
+        rf_track *tracks = nullptr;    // [max_batch][max_tracks]
+        int *counts = nullptr;         // [max_batch]
+        rf_det *due = nullptr;         // [max_batch][max_faces]
+        int *due_counts = nullptr;     // [max_batch]
+        cudaEvent_t free = nullptr;
+    };
+    std::vector<Slot> slots;
+    unsigned next_slot = 0;
+    cudaEvent_t chain = nullptr;
+};
+
+static void tracker_release(rf_tracker t) {
+    if (t->chain) cudaEventSynchronize(t->chain);
+    for (auto &s : t->slots) {
+        if (s.free) { cudaEventSynchronize(s.free); cudaEventDestroy(s.free); }
+        cudaFree(s.tracks); cudaFree(s.counts); cudaFree(s.due); cudaFree(s.due_counts);
+    }
+    if (t->chain) cudaEventDestroy(t->chain);
+    cudaFree(t->d_videos); cudaFree(t->d_state); cudaFree(t->d_pairs); cudaFree(t->d_order);
+    delete t;
+}
+
+int rf_tracker_create(rf_handle h, const rf_track_config *cfg, rf_tracker *out) {
+    static const char *who = "rf_tracker_create";
+    if (!h) return RF_ERR_INVALID_ARG;
+    if (!cfg || !out) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL config or output", who));
+    *out = nullptr;
+    rf_track_config c = *cfg;
+    if (c.max_videos < 1 || c.max_videos > 4096) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: max_videos %d, must be in [1, 4096]", who, c.max_videos));
+    if (c.max_tracks == 0) c.max_tracks = 64;
+    if (c.max_tracks < 1 || c.max_tracks > TRACK_MAX_TRACKS)
+        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: max_tracks %d, must be in [1, %d]", who, c.max_tracks, TRACK_MAX_TRACKS));
+    if (c.max_lost == 0) c.max_lost = 30;
+    if (c.max_lost < 0) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: max_lost %d is negative", who, c.max_lost));
+    float *th[5] = {&c.high_thresh, &c.new_thresh, &c.iou_high, &c.iou_low, &c.iou_tentative};
+    const float dflt[5] = {0.6f, 0.7f, 0.2f, 0.5f, 0.3f};
+    for (int k = 0; k < 5; k++) {
+        if (*th[k] == 0.f) *th[k] = dflt[k];
+        if (!(*th[k] > 0.f && *th[k] <= 1.f))
+            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: thresholds must be in (0, 1] (0: the default), got %g", who, (double)*th[k]));
+    }
+    std::unique_ptr<rf_tracker_s, void (*)(rf_tracker)> t(new rf_tracker_s, tracker_release);
+    t->h = h;
+    t->cfg = c;
+    try {
+        CK(cudaSetDevice(h->device));
+        const size_t T = c.max_tracks, F = h->cfg.max_faces, B = h->cfg.max_batch;
+        const size_t ctas = std::min<size_t>({B, (size_t)TRACK_MAX_FRAMES, (size_t)c.max_videos});
+        CK(cudaMalloc(&t->d_videos, sizeof(TrackVideo) * c.max_videos));
+        CK(cudaMalloc(&t->d_state, sizeof(TrackState) * c.max_videos * T));
+        CK(cudaMalloc(&t->d_pairs, sizeof(TrackPair) * ctas * T * F));
+        CK(cudaMalloc(&t->d_order, sizeof(int) * ctas * T * F));
+        CK(cudaMemset(t->d_videos, 0, sizeof(TrackVideo) * c.max_videos));
+        CK(cudaMemset(t->d_state, 0, sizeof(TrackState) * c.max_videos * T));
+        t->slots.resize(h->ctx.size());
+        for (auto &s : t->slots) {
+            CK(cudaMalloc(&s.tracks, sizeof(rf_track) * B * T));
+            CK(cudaMalloc(&s.counts, sizeof(int) * B));
+            CK(cudaMalloc(&s.due, sizeof(rf_det) * B * F));
+            CK(cudaMalloc(&s.due_counts, sizeof(int) * B));
+            CK(cudaEventCreateWithFlags(&s.free, cudaEventDisableTiming));
+        }
+        CK(cudaEventCreateWithFlags(&t->chain, cudaEventDisableTiming));
+        CK(cudaDeviceSynchronize());      // the zeroed state is in place before any context's stream reads it
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    *out = t.release();
+    return RF_OK;
+}
+
+void rf_tracker_destroy(rf_tracker t) {
+    if (!t) return;
+    cudaSetDevice(t->h->device);
+    tracker_release(t);
+}
+
+int rf_tracker_reset(rf_tracker t, int video) {
+    if (!t) return RF_ERR_INVALID_ARG;
+    rf_handle h = t->h;
+    if (video < -1 || video >= t->cfg.max_videos)
+        return fail(h, RF_ERR_INVALID_ARG, fmt("rf_tracker_reset: video %d, must be -1 or in [0, %d)", video, t->cfg.max_videos));
+    try {
+        CK(cudaSetDevice(h->device));
+        cudaStream_t s = h->ctx[0].stream;
+        const size_t v0 = video < 0 ? 0 : video, nv = video < 0 ? t->cfg.max_videos : 1, T = t->cfg.max_tracks;
+        CK(cudaStreamWaitEvent(s, t->chain, 0));
+        CK(cudaMemsetAsync(t->d_videos + v0, 0, sizeof(TrackVideo) * nv, s));
+        CK(cudaMemsetAsync(t->d_state + v0 * T, 0, sizeof(TrackState) * nv * T, s));
+        CK(cudaEventRecord(t->chain, s));
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
+}
+
+// Everything rf_track_update refuses, checked before anything is launched.
+static int check_track_args(rf_tracker t, const char *who, const int *videos, int n, const float *scales) {
+    rf_handle h = t->h;
+    int rc = check_n(h, n);
+    if (rc) return rc;
+    if (n > 0 && !videos) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: videos is NULL", who));
+    for (int i = 0; i < n; i++) {
+        if (videos[i] < 0 || videos[i] >= t->cfg.max_videos)
+            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frame %d: video %d, must be in [0, %d)", who, i, videos[i], t->cfg.max_videos));
+        if (scales && !(std::isfinite(scales[i]) && scales[i] > 0.f))
+            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frame %d: scale %g, must be finite and positive", who, i, (double)scales[i]));
+    }
+    return RF_OK;
+}
+
+// Issues the update of n frames on s (the records complete there) into the next ring slot, ordered by the chain.  `a` (crops):
+// the due faces are cut on s into a's crops, then the slot's `free` is recorded.
+static void track_issue(rf_tracker t, const int *videos, int n, const rf_det *dets, const int32_t *counts, const float *scales, cudaStream_t s,
+                        const AlignArgs *a, const YuvPlanes *planes, const int *widths, const int *heights, const rf_track **dev_tracks,
+                        const int32_t **dev_track_counts) {
+    rf_handle h = t->h;
+    rf_tracker_s::Slot &slot = t->slots[t->next_slot++ % t->slots.size()];
+    CK(cudaStreamWaitEvent(s, slot.free, 0));
+    CK(cudaStreamWaitEvent(s, t->chain, 0));
+    TrackArgs ta{};
+    ta.p = TrackParams{t->cfg.max_tracks, h->cfg.max_faces, t->cfg.max_lost, t->cfg.high_thresh, t->cfg.new_thresh, t->cfg.iou_high,
+                       t->cfg.iou_low, t->cfg.iou_tentative};
+    ta.videos = t->d_videos;
+    ta.state = t->d_state;
+    ta.pairs = t->d_pairs;
+    ta.order = t->d_order;
+    ta.dets = dets;
+    ta.counts = counts;
+    ta.tracks = slot.tracks;
+    ta.track_counts = slot.counts;
+    if (a) {
+        ta.due = slot.due;
+        ta.due_counts = slot.due_counts;
+        ta.max_align = a->max_align;
+    }
+    CK(launch_track_update(ta, videos, scales, n, s));
+    CK(cudaEventRecord(t->chain, s));
+    if (a) {
+        // the due faces are already in frame pixels: scale 1, as the tiled paths crop their merged records
+        std::vector<AlignYuvImage> orig(n);
+        for (int i = 0; i < n; i++) orig[i] = AlignYuvImage{planes[i], widths[i], heights[i], 1.f, 0};
+        PostBuffers view{};
+        view.out_dets = slot.due;
+        view.out_counts = slot.due_counts;
+        view.max_faces = h->cfg.max_faces;
+        CK(launch_align_faces_yuv(*a, orig.data(), view, h->num_sms, s));
+    }
+    CK(cudaEventRecord(slot.free, s));
+    if (dev_tracks) *dev_tracks = slot.tracks;
+    if (dev_track_counts) *dev_track_counts = slot.counts;
+}
+
+int rf_track_update(rf_tracker t, const int *videos, int n, const rf_det *dev_dets, const int32_t *dev_counts, const float *scales,
+                    const rf_track **dev_tracks, const int32_t **dev_track_counts) {
+    static const char *who = "rf_track_update";
+    if (!t) return RF_ERR_INVALID_ARG;
+    rf_handle h = t->h;
+    int rc = check_track_args(t, who, videos, n, scales);
+    if (rc) return rc;
+    if (n > 0 && (!dev_dets || !dev_counts)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL records or counts", who));
+    if (n == 0) return RF_OK;
+    try {
+        CK(cudaSetDevice(h->device));
+        track_issue(t, videos, n, dev_dets, dev_counts, scales, (cudaStream_t)rf_last_stream(h), nullptr, nullptr, nullptr, nullptr, dev_tracks,
+                    dev_track_counts);
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
+}
+
+int rf_detect_yuv_track_device(rf_handle h, rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, int matrix, float thr, float nms,
+                               const rf_align_params *align, void *dev_crops, double *dev_mats, const rf_track **dev_tracks,
+                               const int32_t **dev_track_counts, const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales) {
+    static const char *who = "rf_detect_yuv_track_device";
+    if (!h) return RF_ERR_INVALID_ARG;
+    if (!t || t->h != h) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker is NULL or belongs to another handle", who));
+    int rc = check_track_args(t, who, videos, n, nullptr);
+    if (rc) return rc;
+    if ((rc = check_frames(h, who, frames, n, matrix))) return rc;
+    AlignArgs a;
+    if (align && (rc = align_setup(h, who, align, a))) return rc;
+    if (align && n > 0 && !dev_crops) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: align without dev_crops", who));
+    if (n == 0) return RF_OK;
+    std::vector<float> scales(n);
+    const rf_det *dets = nullptr;
+    const int32_t *counts = nullptr;
+    if ((rc = yuv_device_impl(h, who, frames, nullptr, n, matrix, thr, nms, nullptr, nullptr, nullptr, &dets, &counts, scales.data()))) return rc;
+    if (dev_dets) *dev_dets = dets;
+    if (dev_counts) *dev_counts = counts;
+    if (out_scales) std::copy(scales.begin(), scales.end(), out_scales);
+    try {
+        std::vector<YuvPlanes> planes(n);
+        std::vector<int> widths(n), heights(n);
+        for (int i = 0; i < n; i++) { planes[i] = planes_of(frames[i], matrix); widths[i] = frames[i].width; heights[i] = frames[i].height; }
+        if (align) { a.n = n; a.crops = dev_crops; a.mats = dev_mats; }
+        track_issue(t, videos, n, dets, counts, scales.data(), h->last_stream, align ? &a : nullptr, planes.data(), widths.data(), heights.data(),
+                    dev_tracks, dev_track_counts);
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
+}
+
+int rf_tracker_debug_state(rf_tracker t, int video, double *out, int cap) {
+    static const char *who = "rf_tracker_debug_state";
+    if (!t) return RF_ERR_INVALID_ARG;
+    rf_handle h = t->h;
+    if (video < 0 || video >= t->cfg.max_videos) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: video %d, must be in [0, %d)", who, video, t->cfg.max_videos));
+    if (cap > 0 && !out) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: out is NULL", who));
+    const int T = t->cfg.max_tracks;
+    TrackVideo hv{};
+    std::vector<TrackState> st(T);
+    try {
+        CK(cudaSetDevice(h->device));
+        CK(cudaEventSynchronize(t->chain));
+        CK(cudaMemcpy(&hv, t->d_videos + video, sizeof hv, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(st.data(), t->d_state + (size_t)video * T, sizeof(TrackState) * T, cudaMemcpyDeviceToHost));
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    std::vector<const TrackState *> live;
+    for (const TrackState &k : st) if (k.id) live.push_back(&k);
+    std::sort(live.begin(), live.end(), [](const TrackState *x, const TrackState *y) { return x->id < y->id; });
+    std::vector<double> v = {(double)live.size(), (double)(hv.issued + 1), (double)hv.frames, (double)hv.overflow};
+    for (const TrackState *k : live) {
+        for (int x : {k->id, k->state, k->hits, k->age, k->lost}) v.push_back(x);
+        for (const double *arr : {k->m, k->u, k->p00, k->p01, k->p11}) v.insert(v.end(), arr, arr + 4);
+    }
+    std::copy(v.begin(), v.begin() + std::min<size_t>(v.size(), (size_t)std::max(cap, 0)), out);
+    return (int)live.size();
 }
 
 }  // extern "C"

@@ -119,6 +119,39 @@ class RetinaFace:
         faces, _, _ = self.engine.detect_views_oriented(img, [(1.0, o) for o in ANY_ORIENTATION], threshold, self.nms_threshold)
         return [FaceDetectInfo.from_row(r) for r in faces]
 
+    def trackFrames(self, frames: Sequence, videos: Sequence[int], threshold: float = 0.5, layout: str = "nv12", matrix: str = "bt601",
+                    align: dict = None, max_videos: int = 64):
+        """f10 tracking: device 4:2:0 frames (torch CUDA tensors in ``Engine.detect_yuv_device``'s forms), frame i of video
+        ``videos[i]``, detected and associated with the tracks of earlier frames on the GPU (rf_detect_yuv_track_device).  Per frame, a
+        list of ``(id, state, FaceDetectInfo)`` over every live track (``capi.TRACK_*`` states; the face is the last matched one, in
+        FRAME pixels), and per frame a list of ``(id, crop)``: with ``align`` (``Engine.detect_align``'s keywords), one crop per track
+        confirmed on that frame -- a new identity -- as a torch CUDA tensor.  The tracker is created on the first call with
+        ``max_videos`` sequences; ``resetTracks`` restarts them."""
+        import torch
+        from .capi import crop_shape
+        if getattr(self, "_tracker", None) is None:
+            self._tracker = self.engine.tracker(max_videos=max_videos)
+        n = len(frames)
+        crops = None
+        if align is not None:
+            kw = {"fmt": "bgr_u8", **align}
+            A = kw.get("max_faces") or self.engine.max_faces
+            shape, dt = crop_shape(kw["fmt"], kw.get("crop", (112, 112)))
+            crops = torch.empty((n, A) + shape, dtype={np.uint8: torch.uint8, np.float32: torch.float32, np.float16: torch.float16}[dt],
+                                device="cuda")
+        tp, tc, _, _, _ = self._tracker.detect_yuv_device(list(frames), list(videos), threshold, self.nms_threshold, layout=layout, matrix=matrix,
+                                                          align=align, dev_crops_ptr=crops.data_ptr() if crops is not None else None)
+        recs = self._tracker.read(tp, tc, n)
+        tracks = [[(int(r["id"]), int(r["state"]), FaceDetectInfo.from_row(r["face"])) for r in per] for per in recs]
+        new = [[(int(r["id"]), crops[i, r["crop_slot"]]) for r in per if r["crop_slot"] >= 0] if crops is not None else []
+               for i, per in enumerate(recs)]
+        return tracks, new
+
+    def resetTracks(self, video: int = -1):
+        """Restart one video's tracks (ids from 1), or every video's with -1."""
+        if getattr(self, "_tracker", None) is not None:
+            self._tracker.reset(video)
+
     @staticmethod
     def draw(img: np.ndarray, faces: Sequence[FaceDetectInfo]) -> np.ndarray:
         """The reference's commented-out visualisation (RetinaFace.cpp:730-741): red box outline of thickness 2, green

@@ -37,7 +37,10 @@ RetinaFace::RetinaFace(string &model, string network_, float nms, const RetinaFa
     out_counts_.resize(opt_.max_batch);
 }
 
-RetinaFace::~RetinaFace() { rf_destroy(h_); }
+RetinaFace::~RetinaFace() {
+    rf_tracker_destroy(tracker_);   // before its handle
+    rf_destroy(h_);
+}
 
 void RetinaFace::detect(const Mat &img, float threshold, float /*scales*/) {
     if (img.empty()) {   // RetinaFace.cpp:578-580
@@ -278,6 +281,33 @@ vector<FaceDetectInfo> RetinaFace::detectAnyOrientation(const Mat &img, float th
     const FaceDetectInfo *f = reinterpret_cast<const FaceDetectInfo *>(out_faces_.data());
     out.assign(f, f + count);
     return out;
+}
+
+void RetinaFace::trackYUV(const vector<rf_yuv_frame> &device_frames, const vector<int> &videos, float threshold, const AlignOptions *align,
+                          void *dev_crops) {
+    if (videos.size() != device_frames.size()) throw std::invalid_argument("trackYUV: one video index per frame");
+    if (device_frames.size() > (size_t)opt_.max_batch) throw std::invalid_argument("trackYUV: at most max_batch frames per call");
+    if (!tracker_) {
+        rf_track_config tc{};
+        tc.max_videos = opt_.track_videos;
+        int rc = rf_tracker_create(h_, &tc, &tracker_);
+        if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_create: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+    }
+    int per = 0, cw = 0, ch = 0;
+    const rf_align_params p = align ? crop_params(*align, opt_.max_faces, &per, &cw, &ch) : rf_align_params{};
+    const int n = (int)device_frames.size();
+    tracks_ = DeviceTracks{};
+    int rc = rf_detect_yuv_track_device(h_, tracker_, device_frames.data(), videos.data(), n, RF_YUV_BT601, threshold, nms_threshold,
+                                        align ? &p : nullptr, dev_crops, nullptr, &tracks_.tracks, &tracks_.counts, nullptr, nullptr, nullptr);
+    if (rc != RF_OK) throw std::runtime_error(string("rf_detect_yuv_track_device: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+    tracks_.n = n;
+    tracks_.max_tracks = 64;      // rf_track_config's default
+}
+
+void RetinaFace::resetTracks(int video) {
+    if (!tracker_) return;
+    int rc = rf_tracker_reset(tracker_, video);
+    if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_reset: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
 }
 
 Mat RetinaFace::draw(const Mat &img, const vector<FaceDetectInfo> &faces) {

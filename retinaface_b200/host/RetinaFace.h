@@ -38,6 +38,7 @@ struct RetinaFaceOptions {
     string int8_table_file = "mnet-deconv-0517.table.int8";   // used when precision == RF_PREC_INT8 (trtnetbase.cpp:13)
     string prototxt_file;                // e.g. "mnet-deconv-0517.prototxt" (RetinaFace.cpp:276): parsed, checked, drives the weight
                                          // folding; with net_w = net_h = 0 it also sets the network size.  Empty: built-in graph
+    int track_videos = 16;               // sequences of the tracker trackYUV creates on its first call
     string cache_file;                   // folded-model cache (the reference's "retina.cache", trtnetbase.cpp:205-243, but with a
                                          // staleness check).  Empty: none
 };
@@ -99,6 +100,20 @@ class RetinaFace {
     // f9 unknown orientation (rf_detect_views_oriented): the image in its four rotations (EXIF 1, 6, 3, 8) as one batch, merged on
     // the GPU; faces in STORED image pixels, landmarks on the subject's sides (an aligned crop of a sideways face comes out upright).
     vector<FaceDetectInfo> detectAnyOrientation(const Mat &img, float threshold = 0.5);
+    // f10 tracking (rf_detect_yuv_track_device): DEVICE 4:2:0 frames (descriptors of device planes, e.g. NVDEC surfaces; at most
+    // max_batch per call), frame i of video videos[i] in [0, track_videos), detected and associated with the tracks of earlier frames
+    // on the GPU.  Asynchronous on rf_last_stream(handle()).  Afterwards lastTracks() holds the device track lists; with `align`, the
+    // crops of the tracks confirmed on each frame (new identities) land in dev_crops [n][A] u8 BGR at each such track's crop_slot.
+    struct DeviceTracks {
+        const rf_track *tracks = nullptr;   // device [n][max_tracks], each frame's live tracks sorted by id
+        const int32_t *counts = nullptr;    // device [n]
+        int n = 0, max_tracks = 0;
+    };
+    void trackYUV(const vector<rf_yuv_frame> &device_frames, const vector<int> &videos, float threshold = 0.5, const AlignOptions *align = nullptr,
+                  void *dev_crops = nullptr);
+    const DeviceTracks &lastTracks() const { return tracks_; }
+    void resetTracks(int video = -1);
+    rf_handle handle() const { return h_; }
     // the reference's visualisation (RetinaFace.cpp:730-741): red box outline (thickness 2), green landmark dots, on a clone
     static Mat draw(const Mat &img, const vector<FaceDetectInfo> &faces);
     int netWidth() const { return opt_.net_w; }
@@ -108,6 +123,8 @@ class RetinaFace {
     // faces (and, with crops, the u8 crops of the first min(count, per) faces) of images [start, start + n) of the last call
     void keepResults(size_t start, int n, const unsigned char *crops, int per, int cw, int ch);
     rf_handle h_ = nullptr;
+    rf_tracker tracker_ = nullptr;
+    DeviceTracks tracks_;
     RetinaFaceOptions opt_;
     string network;
     float nms_threshold;

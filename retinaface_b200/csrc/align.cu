@@ -58,11 +58,11 @@ __device__ void invert_affine(const double m[6], double im[6]) {
 
 // One output pixel of cv::warpAffine INTER_LINEAR / BORDER_CONSTANT 0 on 8UC3: X, Y in 1/32 source pixel (X0 + adelta >> 5),
 // integer weights 32 (32 - fx) (32 - fy) ... summing to 32768, taps outside the image contribute 0, (sum + 16384) >> 15.
-__device__ __forceinline__ void tap(const AlignImage &im, int x, int y, int p[3]) {
-    const uint8_t *q = im.src + (size_t)y * im.row_bytes + (size_t)x * 3;
+__device__ __forceinline__ void tap(const AlignImageT<BgrRows> &im, int x, int y, int p[3]) {
+    const uint8_t *q = im.src.p + (size_t)y * im.src.pitch + (size_t)x * 3;
     p[0] = q[0]; p[1] = q[1]; p[2] = q[2];
 }
-__device__ __forceinline__ void tap(const AlignYuvImage &im, int x, int y, int p[3]) { yuv_pixel(im.p, x, y, p); }
+__device__ __forceinline__ void tap(const AlignImageT<YuvPlanes> &im, int x, int y, int p[3]) { yuv_pixel(im.src, x, y, p); }
 // displayed pixel (x, y) of an oriented image: reflected, then transposed, as the letter-box reads it (preprocess.cu)
 template <typename Img>
 __device__ __forceinline__ void oriented_tap(const Img &im, int x, int y, int p[3]) {
@@ -91,28 +91,16 @@ __device__ __forceinline__ void sample(const Img &im, int X, int Y, int v[3]) {
     v[0] = acc[0] >> 15; v[1] = acc[1] >> 15; v[2] = acc[2] >> 15;
 }
 
-// Where the kernel finds image i: the BGR table / uniform net-sized images of AlignArgs, or the frame table parameter.  Only the
-// tables of the oriented paths (f9) read `orient`: the other instantiations keep their code.
-struct BgrImages { static constexpr bool kOriented = false; };
-template <bool O> struct YuvFramesT { static constexpr bool kOriented = O; AlignYuvImage img[ALIGN_MAX_FRAMES]; };
-template <bool O> struct BgrTableT { static constexpr bool kOriented = O; AlignImage img[ALIGN_MAX_FRAMES]; };   // f8: BGR images whose table travels as a kernel parameter
-using YuvFrames = YuvFramesT<false>;
-using BgrTable = BgrTableT<false>;
-static_assert(sizeof(AlignArgs) + sizeof(YuvFrames) + 32 <= 4096, "align launch exceeds the classic 4 KB kernel parameter space");
-static_assert(sizeof(AlignArgs) + sizeof(BgrTable) + 32 <= 4096, "align launch exceeds the classic 4 KB kernel parameter space");
-
-__device__ __forceinline__ AlignImage image_of(const AlignArgs &a, const BgrImages &, int i) {
-    AlignImage im;
-    if (a.images) {
-        im = a.images[i];
-    } else {
-        im.src = a.uniform_base + (size_t)i * a.uniform_bytes;
-        im.w = a.uniform_w; im.h = a.uniform_h; im.row_bytes = a.uniform_w * 3; im.scale = 1.f; im.orient = 0;
-    }
-    return im;
-}
-template <bool O> __device__ __forceinline__ AlignYuvImage image_of(const AlignArgs &, const YuvFramesT<O> &f, int i) { return f.img[i]; }
-template <bool O> __device__ __forceinline__ AlignImage image_of(const AlignArgs &, const BgrTableT<O> &t, int i) { return t.img[i]; }
+// A launch's chunk of the image table.  Only the oriented tables (f9) read `orient`: the other instantiations keep their code.
+template <typename Src, bool O>
+struct AlignTable {
+    static constexpr bool kOriented = O;
+    AlignImageT<Src> img[align_table_limit<Src>()];
+};
+static_assert(sizeof(AlignImageT<BgrRows>) == 32, "64 BGR images per launch rely on the 32-byte entry");
+static_assert(sizeof(AlignArgs) + sizeof(AlignTable<BgrRows, false>) + 32 <= 4096 &&
+              sizeof(AlignArgs) + sizeof(AlignTable<YuvPlanes, false>) + 32 <= 4096,
+              "align launch exceeds the classic 4 KB kernel parameter space");
 
 // Four consecutive pixels of one crop row (x4 .. x4 + 3, those < cw valid).  Vector stores where the address allows.
 __device__ __forceinline__ void store_quad(const AlignArgs &a, unsigned char *crop, int y, int x4, const int v[4][3]) {
@@ -158,8 +146,8 @@ __device__ __forceinline__ void store_quad(const AlignArgs &a, unsigned char *cr
 // consecutive work items -- so that free slots cost nothing however large max_align is.  Per item, thread 0 fits the
 // transform in FP64, the CTA tabulates OpenCV's per-column (adelta, bdelta) and the band's per-row (X0, Y0) fixed-point
 // terms in shared memory, and every pixel costs integer arithmetic only.
-template <typename Src>
-__global__ void __launch_bounds__(ALIGN_THREADS) k_align_faces(const AlignArgs a, const __grid_constant__ Src src, const rf_det *__restrict__ dets,
+template <typename Table>
+__global__ void __launch_bounds__(ALIGN_THREADS) k_align_faces(const AlignArgs a, const __grid_constant__ Table table, const rf_det *__restrict__ dets,
                                                              const int *__restrict__ counts, int max_faces) {
     extern __shared__ int s_first[];     // [n]: crop ordinal of image i's first crop
     __shared__ int s_ax[ALIGN_MAX_SIDE], s_bx[ALIGN_MAX_SIDE], s_x0[ALIGN_BAND], s_y0[ALIGN_BAND];
@@ -206,7 +194,7 @@ __global__ void __launch_bounds__(ALIGN_THREADS) k_align_faces(const AlignArgs a
             if (s_first[mid] <= c) i = mid; else top = mid - 1;
         }
         const int j = c - s_first[i], slot = i * a.max_align + j;
-        const auto im = image_of(a, src, i);
+        const auto im = table.img[i];
         if (threadIdx.x == 0) {
             double M[6], iM[6];
             s_zero = fit_similarity(dets[(size_t)i * max_faces + j].face, im.scale, a.tmpl, M) ? 0 : 1;
@@ -236,7 +224,7 @@ __global__ void __launch_bounds__(ALIGN_THREADS) k_align_faces(const AlignArgs a
 #pragma unroll
             for (int k = 0; k < 4; k++) {
                 const int x = x4 + k;
-                if (x < cw && !zero) sample<Src::kOriented>(im, (s_x0[r] + s_ax[x]) >> 5, (s_y0[r] + s_bx[x]) >> 5, v[k]);
+                if (x < cw && !zero) sample<Table::kOriented>(im, (s_x0[r] + s_ax[x]) >> 5, (s_y0[r] + s_bx[x]) >> 5, v[k]);
                 else v[k][0] = v[k][1] = v[k][2] = 0;
             }
             store_quad(a, crop, ybase + r, x4, v);
@@ -245,19 +233,20 @@ __global__ void __launch_bounds__(ALIGN_THREADS) k_align_faces(const AlignArgs a
     }
 }
 
-// Chunk i0 is its own launch over images [i0, i0 + m), whose table (Table: YuvFrames or BgrTable) is a kernel parameter: the
-// same kernel on offset records, counts, crops and matrices.
-template <typename Table, typename Img>
-cudaError_t launch_table(const AlignArgs &a, const Img *images, const PostBuffers &pb, int num_sms, cudaStream_t s) {
-    if (a.n <= 0 || a.max_align <= 0) return cudaSuccess;
-    for (int i0 = 0; i0 < a.n; i0 += ALIGN_MAX_FRAMES) {
-        const int m = std::min(ALIGN_MAX_FRAMES, a.n - i0);
+// Chunk i0 is its own launch over images [i0, i0 + m): the same kernel on offset records, counts, crops and matrices.  Two small
+// CTAs per SM: the crops of a batch-8 step (about 40 faces x 14 bands) in one or two items per CTA, without taking more than a
+// quarter of any SM's registers from the forward kernels of other contexts running alongside.
+template <typename Table, typename Src>
+cudaError_t launch_table(const AlignArgs &a, const AlignImageT<Src> *table, const PostBuffers &pb, int num_sms, cudaStream_t s) {
+    constexpr int kMax = align_table_limit<Src>();
+    for (int i0 = 0; i0 < a.n; i0 += kMax) {
+        const int m = std::min(kMax, a.n - i0);
         AlignArgs c = a;
         c.n = m;
         c.crops = static_cast<unsigned char *>(a.crops) + (size_t)i0 * a.max_align * a.crop_bytes;
         if (a.mats) c.mats = a.mats + (size_t)i0 * a.max_align * 6;
         Table t{};
-        for (int i = 0; i < m; i++) t.img[i] = images[i0 + i];
+        for (int i = 0; i < m; i++) t.img[i] = table[i0 + i];
         k_align_faces<<<2 * num_sms, ALIGN_THREADS, sizeof(int) * m, s>>>(c, t, pb.out_dets + (size_t)i0 * pb.max_faces, pb.out_counts + i0,
                                                                         pb.max_faces);
         cudaError_t e = cudaGetLastError();
@@ -268,20 +257,13 @@ cudaError_t launch_table(const AlignArgs &a, const Img *images, const PostBuffer
 
 }  // namespace
 
-cudaError_t launch_align_faces(const AlignArgs &a, const PostBuffers &pb, int num_sms, cudaStream_t s) {
+template <typename Src>
+cudaError_t launch_align_faces(const AlignArgs &a, const AlignImageT<Src> *table, const PostBuffers &pb, int num_sms, cudaStream_t s, bool oriented) {
     if (a.n <= 0 || a.max_align <= 0) return cudaSuccess;
-    // two small CTAs per SM: the crops of a batch-8 step (about 40 faces x 14 bands) in one or two items per CTA, without
-    // taking more than a quarter of any SM's registers from the forward kernels of other contexts running alongside
-    k_align_faces<<<2 * num_sms, ALIGN_THREADS, sizeof(int) * a.n, s>>>(a, BgrImages{}, pb.out_dets, pb.out_counts, pb.max_faces);
-    return cudaGetLastError();
+    return oriented ? launch_table<AlignTable<Src, true>>(a, table, pb, num_sms, s) : launch_table<AlignTable<Src, false>>(a, table, pb, num_sms, s);
 }
 
-cudaError_t launch_align_faces_yuv(const AlignArgs &a, const AlignYuvImage *frames, const PostBuffers &pb, int num_sms, cudaStream_t s, bool oriented) {
-    return oriented ? launch_table<YuvFramesT<true>>(a, frames, pb, num_sms, s) : launch_table<YuvFrames>(a, frames, pb, num_sms, s);
-}
-
-cudaError_t launch_align_faces(const AlignArgs &a, const AlignImage *images, const PostBuffers &pb, int num_sms, cudaStream_t s, bool oriented) {
-    return oriented ? launch_table<BgrTableT<true>>(a, images, pb, num_sms, s) : launch_table<BgrTable>(a, images, pb, num_sms, s);
-}
+template cudaError_t launch_align_faces<BgrRows>(const AlignArgs &, const AlignImageT<BgrRows> *, const PostBuffers &, int, cudaStream_t, bool);
+template cudaError_t launch_align_faces<YuvPlanes>(const AlignArgs &, const AlignImageT<YuvPlanes> *, const PostBuffers &, int, cudaStream_t, bool);
 
 }  // namespace rf

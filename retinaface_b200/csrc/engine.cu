@@ -249,7 +249,7 @@ void destroy(rf_handle h) {
     for (auto p : h->d_blobs) cudaFree(p);
     h->copy_pool.reset();
     for (auto e : h->raw_ev) if (e) cudaEventDestroy(e);
-    cudaFree(h->d_align_images); cudaFreeHost(h->h_align_images); cudaFree(h->d_align_crops); cudaFree(h->d_align_mats);
+    cudaFree(h->d_align_crops); cudaFree(h->d_align_mats);
     cudaFreeHost(h->h_input); cudaFreeHost(h->h_raw); cudaFreeHost(h->h_dets); cudaFreeHost(h->h_counts); cudaFreeHost(h->tile_dbg);
     for (auto &sl : h->slots) {
         cudaFree(sl.d_in); cudaFreeHost(sl.h_in); cudaFreeHost(sl.h_dets); cudaFreeHost(sl.h_counts);
@@ -570,13 +570,11 @@ struct H2DRuns {
     }
 };
 
-// One caller image of arbitrary size -> d_raw (packed rows) on `s`.  Pinned sources (cudaHostAlloc /
-// cudaHostRegister) are copied straight from the caller's memory, row stride and all.  Pageable sources are staged through
-// two pinned buffers: a row-band parallel host copy (host_copy.h) into one buffer overlaps the DMA out of the other; the
-// only host wait is for the DMA that last read the buffer about to be overwritten.  In both cases the stream orders the
-// copy into d_raw behind the letter-box kernel that still reads the previous image.
-// One host plane of `rows` rows of row_bytes (pitch bytes apart) -> d_dst, packed, on `s`: pinned sources straight, pageable
-// ones through the two pinned staging buffers (each plane fits one: it is at most a max_image BGR image).
+// One host plane of `rows` rows of row_bytes (pitch bytes apart) -> d_dst, packed, on `s`.  Pinned sources (cudaHostAlloc /
+// cudaHostRegister) are copied straight from the caller's memory, row stride and all.  Pageable sources are staged through the
+// two pinned buffers (each plane fits one: it is at most a max_image BGR image): a row-band parallel host copy (host_copy.h) into
+// one buffer overlaps the DMA out of the other; the only host wait is for the DMA that last read the buffer about to be
+// overwritten.  In both cases the stream orders the copy into d_raw behind the letter-box kernel that still reads the previous image.
 static void upload_plane(rf_handle h, cudaStream_t s, uint8_t *d_dst, const uint8_t *src, size_t row_bytes, size_t pitch, int rows) {
     if (is_pinned(src)) {
         CK(cudaMemcpy2DAsync(d_dst, row_bytes, src, pitch, row_bytes, (size_t)rows, cudaMemcpyHostToDevice, s));
@@ -591,86 +589,133 @@ static void upload_plane(rf_handle h, cudaStream_t s, uint8_t *d_dst, const uint
     CK(cudaEventRecord(h->raw_ev[slot], s));
 }
 
-static uint8_t *upload_raw(rf_handle h, cudaStream_t s, const uint8_t *src, int width, int height, int row_stride, int raw_slot = 0) {
-    uint8_t *d_dst = h->d_raw + (size_t)raw_slot * h->raw_bytes;
-    upload_plane(h, s, d_dst, src, (size_t)width * 3, (size_t)row_stride, height);
-    return d_dst;
-}
-
-// The n caller images of rf_detect_batch -> the input tensor, on `s`.  With `originals`
-// (rf_detect_align_batch, which has checked that every image that is not network-sized gets a raw buffer of its own),
-// originals[i] records where image i's own pixels stay resident and its map-back scale.
-// f9 `orient` (optional): image i is shown in EXIF orientation orient[i] (checked by the caller); only orientation 1 takes the
-// straight copy, and originals[i] then describes the displayed image.
-static int stage_images(rf_handle h, cudaStream_t s, const char *who, const uint8_t *const *imgs, const int *widths, const int *heights,
-                        const int *row_strides, int n, AlignImage *originals, const int *orient = nullptr) {
-    const int Hn = h->cfg.net_h, Wn = h->cfg.net_w;
-    const size_t img_bytes = (size_t)Hn * Wn * 3;
-    // Network-sized packed images are copied H2D straight from the caller's memory when it is
-    // pinned (cudaHostAlloc / cudaHostRegister / the library's own rf_pinned_input), otherwise via the
-    // library's pinned mirror; runs of adjacent sources collapse into one copy.  Other sizes are
-    // letter-boxed on the GPU one by one (preprocess.cuh).
-    H2DRuns runs{h->d_input, img_bytes, s};
-    bool staging_dirty = false;
-    // other sizes: uploaded into per-image raw buffers, then ONE letter-box launch for all of them (RF_FLAG_NPP_RESIZE: the
-    // reference's NPP super-sampling definition instead of its OpenCV bilinear one)
-    const int area = (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0;
-    std::vector<LbItem> lb;
-    auto flush_lb = [&]() {
-        if (lb.empty()) return;
-        CK(launch_letterbox_batch(lb.data(), (int)lb.size(), Wn, Hn, s));
-        lb.clear();
-    };
-    for (int i = 0; i < n; i++) {
-        if (!imgs[i] || widths[i] <= 0 || heights[i] <= 0) { return fail(h, RF_ERR_INVALID_ARG, fmt("%s: image %d is empty", who, i)); }
-        const int rs = row_strides && row_strides[i] ? row_strides[i] : widths[i] * 3;
-        const int bits = orient ? lb_orientation_bits(orient[i]) : 0;
-        if (widths[i] == Wn && heights[i] == Hn && rs == Wn * 3 && bits == 0) {
-            const uint8_t *src = imgs[i];
-            const bool in_mirror = src >= h->h_input && src < h->h_input + (size_t)h->cfg.max_batch * img_bytes;
-            if (!in_mirror && !is_pinned(src)) {
-                if (!staging_dirty) { CK(cudaStreamSynchronize(s)); staging_dirty = true; }
-                uint8_t *slot = h->h_input + (size_t)i * img_bytes;
-                memcpy(slot, src, img_bytes);
-                src = slot;
-            }
-            runs.add(i, src);
-            if (originals) originals[i] = AlignImage{h->d_input + (size_t)i * img_bytes, Wn, Hn, Wn * 3, 1.f};
-        } else {
-            runs.flush();
-            if (widths[i] > h->cfg.max_image_w || heights[i] > h->cfg.max_image_h)
-                return fail(h, RF_ERR_CAPACITY, fmt("image %d is %dx%d, larger than max_image %dx%d", i, widths[i], heights[i],
-                                                    h->cfg.max_image_w, h->cfg.max_image_h));
-            if ((int)lb.size() == h->raw_slots) flush_lb();
-            const uint8_t *d_src = upload_raw(h, s, imgs[i], widths[i], heights[i], rs, (int)lb.size());
-            lb.emplace_back();
-            int dw = widths[i], dh = heights[i];
-            if (bits & LB_TRANSPOSE) std::swap(dw, dh);
-            const float scale = letterbox_fill(lb.back(), d_src, dw, dh, h->d_input + (size_t)i * img_bytes, Wn, Hn, bits, area);
-            if (originals) originals[i] = AlignImage{d_src, dw, dh, widths[i] * 3, scale, bits};
-        }
-    }
-    runs.flush();
-    flush_lb();
+// ---- image sources ---------------------------------------------------------------------------------------------------------------
+// Every detect entry point describes the caller's pixels with one of two sources.  A source checks the caller's description (every
+// check runs before anything is copied or launched), reports image i's stored size and EXIF orientation, and hands the letter-box
+// and crop kernels its pixels: upload(s, i, slot) copies host image i into raw buffer `slot` on s (the blocking paths),
+// in_place(i) reads the caller's device memory (the asynchronous ones).  Src is what those kernels read.
+static int check_orientations(rf_handle h, const char *who, const int *orientations, int n) {
+    if (n > 0 && !orientations) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: orientations is NULL", who));
+    for (int i = 0; i < n; i++)
+        if (lb_orientation_bits(orientations[i]) < 0)
+            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: item %d: orientation %d, must be in 1..8 (EXIF)", who, i, orientations[i]));
     return RF_OK;
 }
 
-int rf_detect_batch(rf_handle h, const uint8_t *const *imgs, const int *widths, const int *heights, const int *row_strides,
-                    int n, float thr, float nms, rf_face *out_faces, int *out_counts, int32_t *out_idx) {
+// Checks n, the matrix and every frame descriptor; nothing is launched before this passes.
+static int check_frames(rf_handle h, const char *who, const rf_yuv_frame *frames, int n, int matrix) {
     int rc = check_n(h, n);
     if (rc) return rc;
-    if (n == 0) return RF_OK;
-    if (!imgs || !widths || !heights) return fail(h, RF_ERR_INVALID_ARG, "rf_detect_batch: NULL image arrays");
-    try {
-        CK(cudaSetDevice(h->device));
-        Ctx &c = h->ctx[0];
-        if ((rc = stage_images(h, c.stream, "rf_detect_batch", imgs, widths, heights, row_strides, n, nullptr))) return rc;
-        set_params(h, c, thr, nms);
-        forward_graph(h, c, n);
-        fetch_results(h, c, n, out_faces, out_counts, out_idx);
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    if (n > 0 && !frames) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frames is NULL", who));
+    if (matrix != RF_YUV_BT601 && matrix != RF_YUV_BT709) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: unknown matrix %d", who, matrix));
+    for (int i = 0; i < n; i++) {
+        const rf_yuv_frame &f = frames[i];
+        if (f.width <= 0 || f.height <= 0 || (f.width & 1) || (f.height & 1))
+            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frame %d is %dx%d; 4:2:0 sizes must be positive and even", who, i, f.width, f.height));
+        if (!f.y || !f.u || !f.v) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frame %d has a NULL plane", who, i));
+        if (f.uv_step != 1 && f.uv_step != 2) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frame %d: uv_step %d, must be 1 or 2", who, i, f.uv_step));
+        const uintptr_t u = (uintptr_t)f.u, v = (uintptr_t)f.v;
+        if (f.uv_step == 2 && u != v + 1 && v != u + 1)
+            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frame %d: semi-planar u and v must be adjacent bytes of one plane", who, i));
+        if (f.y_pitch < f.width || f.uv_pitch < f.width / 2 * f.uv_step)
+            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frame %d: pitches %d / %d below the row bytes %d / %d", who, i, f.y_pitch, f.uv_pitch, f.width,
+                                                   f.width / 2 * f.uv_step));
+        if (f.width > h->cfg.max_image_w || f.height > h->cfg.max_image_h)
+            return fail(h, RF_ERR_CAPACITY, fmt("%s: frame %d is %dx%d, larger than max_image %dx%d", who, i, f.width, f.height, h->cfg.max_image_w,
+                                                h->cfg.max_image_h));
+    }
     return RF_OK;
 }
+
+
+// BGR images: u8 BGR HWC rows row_strides[i] bytes apart (NULL or 0: packed), shown in EXIF orientation orient[i] when `oriented`.
+struct BgrImages {
+    using Src = BgrRows;
+    const uint8_t *const *imgs;
+    const int *widths, *heights, *row_strides, *orient;
+    bool oriented;
+    int width(int i) const { return widths[i]; }
+    int height(int i) const { return heights[i]; }
+    int stride(int i) const { return row_strides && row_strides[i] ? row_strides[i] : widths[i] * 3; }
+    int bits(int i) const { return oriented ? lb_orientation_bits(orient[i]) : 0; }
+    // network-sized, packed and upright: copied straight into the input tensor, without a raw buffer or a letter-box
+    bool direct(rf_handle h, int i) const {
+        return widths[i] == h->cfg.net_w && heights[i] == h->cfg.net_h && stride(i) == h->cfg.net_w * 3 && bits(i) == 0;
+    }
+    int check(rf_handle h, const char *who, int n) const {
+        int rc = check_n(h, n);
+        if (rc) return rc;
+        if (n > 0 && (!imgs || !widths || !heights)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL image arrays", who));
+        for (int i = 0; i < n; i++) {
+            if (!imgs[i] || widths[i] <= 0 || heights[i] <= 0) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: image %d is empty", who, i));
+            if (stride(i) < widths[i] * 3)
+                return fail(h, RF_ERR_INVALID_ARG, fmt("%s: image %d: row stride %d below %d bytes", who, i, stride(i), widths[i] * 3));
+            if (widths[i] > h->cfg.max_image_w || heights[i] > h->cfg.max_image_h)
+                return fail(h, RF_ERR_CAPACITY, fmt("%s: image %d is %dx%d, larger than max_image %dx%d", who, i, widths[i], heights[i],
+                                                    h->cfg.max_image_w, h->cfg.max_image_h));
+        }
+        return oriented ? check_orientations(h, who, orient, n) : RF_OK;
+    }
+    BgrRows upload(rf_handle h, cudaStream_t s, int i, int slot) const {
+        uint8_t *d = h->d_raw + (size_t)slot * h->raw_bytes;
+        upload_plane(h, s, d, imgs[i], (size_t)widths[i] * 3, (size_t)stride(i), heights[i]);
+        return BgrRows{d, widths[i] * 3};
+    }
+    BgrRows in_place(int i) const { return BgrRows{imgs[i], stride(i)}; }
+};
+
+// YUV 4:2:0 frames (yuv.cuh) in `matrix`, shown in EXIF orientation orient[i] when `oriented`.
+struct YuvFrames {
+    using Src = YuvPlanes;
+    const rf_yuv_frame *frames;
+    int matrix;
+    const int *orient;
+    bool oriented;
+    int width(int i) const { return frames[i].width; }
+    int height(int i) const { return frames[i].height; }
+    int bits(int i) const { return oriented ? lb_orientation_bits(orient[i]) : 0; }
+    bool direct(rf_handle, int) const { return false; }
+    int check(rf_handle h, const char *who, int n) const {
+        int rc = check_frames(h, who, frames, n, matrix);
+        if (rc || !oriented) return rc;
+        return check_orientations(h, who, orient, n);
+    }
+    // 1.5 bytes per pixel: the luma packed, then the chroma as the frame lays it out (one interleaved w x h/2 plane, or two
+    // w/2 x h/2 planes)
+    YuvPlanes upload(rf_handle h, cudaStream_t s, int i, int slot) const {
+        const rf_yuv_frame &f = frames[i];
+        uint8_t *d = h->d_raw + (size_t)slot * h->raw_bytes, *dc = d + (size_t)f.width * f.height;
+        const int cw = f.width / 2, ch = f.height / 2;
+        upload_plane(h, s, d, f.y, f.width, f.y_pitch, f.height);
+        YuvPlanes p{d, dc, dc, f.width, f.width, f.uv_step, matrix};
+        if (f.uv_step == 2) {
+            const uint8_t *first = std::min(f.u, f.v);
+            upload_plane(h, s, dc, first, f.width, f.uv_pitch, ch);
+            p.u = dc + (f.u - first);
+            p.v = dc + (f.v - first);
+        } else {
+            upload_plane(h, s, dc, f.u, cw, f.uv_pitch, ch);
+            upload_plane(h, s, dc + (size_t)cw * ch, f.v, cw, f.uv_pitch, ch);
+            p.v = dc + (size_t)cw * ch;
+            p.uv_pitch = cw;
+        }
+        return p;
+    }
+    YuvPlanes in_place(int i) const {
+        const rf_yuv_frame &f = frames[i];
+        return YuvPlanes{f.y, f.u, f.v, f.y_pitch, f.uv_pitch, f.uv_step, matrix};
+    }
+};
+
+extern "C++" {
+// the displayed size of image i: its stored size, transposed for EXIF orientations 5..8
+template <typename Source>
+static void displayed_size(const Source &src, int i, int &w, int &hgt) {
+    const bool t = (src.bits(i) & LB_TRANSPOSE) != 0;
+    w = t ? src.height(i) : src.width(i);
+    hgt = t ? src.width(i) : src.height(i);
+}
+}  // extern "C++"
 
 // ---- f5 face alignment (align.cuh) ----------------------------------------------------------------------------------------------
 // Checks the caller's rf_align_params and fills the image-independent kernel arguments (defaults applied).
@@ -701,13 +746,23 @@ static int align_setup(rf_handle h, const char *who, const rf_align_params *p, A
     return RF_OK;
 }
 
+
+// The align checks of every entry point that crops: the params, somewhere for the crops to go and -- the blocking paths cut the
+// crops from the originals after the forward -- a raw buffer of its own for each of the `resident` originals that need one.
+static int check_align(rf_handle h, const char *who, const rf_align_params *p, int n, const void *crops, int resident, AlignArgs &a) {
+    int rc = align_setup(h, who, p, a);
+    if (rc) return rc;
+    if (n > 0 && !crops) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: align without a crop buffer", who));
+    if (resident > h->raw_slots)
+        return fail(h, RF_ERR_CAPACITY, fmt("%s: %d images need a raw buffer until their crops are cut, but the handle keeps at most %d "
+                                            "originals resident (one %dx%d raw buffer each); split the batch", who, resident, h->raw_slots,
+                                            h->cfg.max_image_w, h->cfg.max_image_h));
+    return RF_OK;
+}
+
 // Makes room for n images' crops and the matrices of the blocking align paths (context 0).
 static void ensure_align_buffers(rf_handle h, int n, const AlignArgs &a) {
-    if (!h->d_align_images) {
-        CK(cudaMalloc(&h->d_align_images, sizeof(AlignImage) * h->cfg.max_batch));
-        CK(cudaHostAlloc(&h->h_align_images, sizeof(AlignImage) * h->cfg.max_batch, cudaHostAllocDefault));
-        CK(cudaMalloc(&h->d_align_mats, sizeof(double) * 6 * h->cfg.max_batch * h->cfg.max_faces));
-    }
+    if (!h->d_align_mats) CK(cudaMalloc(&h->d_align_mats, sizeof(double) * 6 * h->cfg.max_batch * h->cfg.max_faces));
     const size_t need = (size_t)n * a.max_align * a.crop_bytes;
     if (need > h->align_crops_bytes) {
         CK(cudaFree(h->d_align_crops));
@@ -746,242 +801,156 @@ static void put_mapped(rf_handle h, Ctx &c, int n, ScaleOf scale, const AlignArg
 }
 }  // extern "C++"
 
-int rf_detect_align_batch(rf_handle h, const uint8_t *const *imgs, const int *widths, const int *heights, const int *row_strides,
-                          int n, float thr, float nms, const rf_align_params *params, rf_face *out_faces, int *out_counts,
-                          void *out_crops, double *out_mats) {
-    int rc = check_n(h, n);
+
+// The blocking letter-box path of rf_detect_batch, rf_detect_align_batch, rf_detect_oriented_batch and rf_detect_yuv_batch, on
+// context 0.  Network-sized packed upright images are copied H2D straight from the caller's memory when it is pinned
+// (cudaHostAlloc / cudaHostRegister / the library's own rf_pinned_input), otherwise via the library's pinned mirror; runs of
+// adjacent sources collapse into one copy.  Every other image is uploaded into a raw buffer of its own, a chunk of raw_slots at a
+// time, each chunk letter-boxed by one launch (RF_FLAG_NPP_RESIZE: the reference's NPP super-sampling definition instead of its
+// OpenCV bilinear one).  With `aligned`, the check has made sure that no raw buffer is recycled within the call, and the crops are
+// cut from the originals after the forward.  `map_back`: faces in image pixels rather than network-input pixels.
+extern "C++" {
+template <typename Source>
+static int detect_blocking(rf_handle h, const char *who, const Source &src, int n, float thr, float nms, bool aligned, const rf_align_params *align,
+                           bool map_back, rf_face *out_faces, int *out_counts, int32_t *out_idx, void *out_crops, double *out_mats) {
+    using Src = typename Source::Src;
+    int rc = src.check(h, who, n);
     if (rc) return rc;
     AlignArgs a;
-    if ((rc = align_setup(h, "rf_detect_align_batch", params, a))) return rc;
-    if (n == 0) return RF_OK;
-    if (!imgs || !widths || !heights || !out_crops) return fail(h, RF_ERR_INVALID_ARG, "rf_detect_align_batch: NULL image arrays or out_crops");
-    const int Hn = h->cfg.net_h, Wn = h->cfg.net_w;
-    // the kernel samples every original after the forward: no raw buffer may be recycled within the call
-    int raw = 0;
-    for (int i = 0; i < n; i++) {
-        const int rs = row_strides && row_strides[i] ? row_strides[i] : widths[i] * 3;
-        raw += !(widths[i] == Wn && heights[i] == Hn && rs == Wn * 3);
+    if (aligned) {
+        int raw = 0;
+        for (int i = 0; i < n; i++) raw += !src.direct(h, i);
+        if ((rc = check_align(h, who, align, n, out_crops, raw, a))) return rc;
     }
-    if (raw > h->raw_slots)
-        return fail(h, RF_ERR_CAPACITY, fmt("rf_detect_align_batch: %d images are not %dx%d packed, but the handle keeps at most %d such originals "
-                                            "resident (one %dx%d raw buffer each); split the batch", raw, Wn, Hn, h->raw_slots,
-                                            h->cfg.max_image_w, h->cfg.max_image_h));
+    if (n == 0) return RF_OK;
+    const int Hn = h->cfg.net_h, Wn = h->cfg.net_w;
+    const size_t img_bytes = (size_t)Hn * Wn * 3;
+    const int area = (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0;
     try {
         CK(cudaSetDevice(h->device));
         Ctx &c = h->ctx[0];
-        ensure_align_buffers(h, n, a);
-        if ((rc = stage_images(h, c.stream, "rf_detect_align_batch", imgs, widths, heights, row_strides, n, h->h_align_images))) return rc;
-        CK(cudaMemcpyAsync(h->d_align_images, h->h_align_images, sizeof(AlignImage) * n, cudaMemcpyHostToDevice, c.stream));
+        if (aligned) ensure_align_buffers(h, n, a);
+        // where each original stays resident, and its map-back factor (only the crops and the map-back read them)
+        std::vector<AlignImageT<Src>> orig(aligned || map_back ? n : 0);
+        H2DRuns runs{h->d_input, img_bytes, c.stream};
+        bool staging_dirty = false;
+        std::vector<LbItemT<Src>> lb;
+        for (int i = 0; i < n; i++) {
+            if constexpr (std::is_same<Src, BgrRows>::value) {
+                if (src.direct(h, i)) {
+                    const uint8_t *p = src.imgs[i];
+                    const bool in_mirror = p >= h->h_input && p < h->h_input + (size_t)h->cfg.max_batch * img_bytes;
+                    if (!in_mirror && !is_pinned(p)) {
+                        if (!staging_dirty) { CK(cudaStreamSynchronize(c.stream)); staging_dirty = true; }
+                        uint8_t *slot = h->h_input + (size_t)i * img_bytes;
+                        memcpy(slot, p, img_bytes);
+                        p = slot;
+                    }
+                    runs.add(i, p);
+                    if (!orig.empty()) orig[i] = AlignImageT<Src>{BgrRows{h->d_input + (size_t)i * img_bytes, Wn * 3}, Wn, Hn, 1.f, 0};
+                    continue;
+                }
+                runs.flush();
+            }
+            // a full chunk of raw buffers is letter-boxed before the next image reuses the first (stream order)
+            if ((int)lb.size() == h->raw_slots) { CK(launch_letterbox_batch(lb.data(), (int)lb.size(), Wn, Hn, c.stream)); lb.clear(); }
+            const Src p = src.upload(h, c.stream, i, (int)lb.size());
+            const int bits = src.bits(i);
+            int dw, dh;
+            displayed_size(src, i, dw, dh);
+            lb.emplace_back();
+            const float scale = letterbox_fill(lb.back(), p, dw, dh, h->d_input + (size_t)i * img_bytes, Wn, Hn, bits, area);
+            if (!orig.empty()) orig[i] = AlignImageT<Src>{p, dw, dh, scale, bits};
+        }
+        runs.flush();
+        if (!lb.empty()) CK(launch_letterbox_batch(lb.data(), (int)lb.size(), Wn, Hn, c.stream));
         set_params(h, c, thr, nms);
         forward_graph(h, c, n);
-        a.images = h->d_align_images;
-        a.n = n;
-        a.crops = h->d_align_crops;
-        a.mats = out_mats ? h->d_align_mats : nullptr;
-        CK(launch_align_faces(a, c.pb, h->num_sms, c.stream));
-        fetch_results(h, c, n, nullptr, out_counts, nullptr);
-        put_mapped(h, c, n, [&](int i) { return h->h_align_images[i].scale; }, &a, out_faces, out_crops, out_mats);
+        if (aligned) {
+            a.n = n;
+            a.crops = h->d_align_crops;
+            a.mats = out_mats ? h->d_align_mats : nullptr;
+            CK(launch_align_faces(a, orig.data(), c.pb, h->num_sms, c.stream, src.oriented));
+        }
+        fetch_results(h, c, n, map_back ? nullptr : out_faces, out_counts, out_idx);
+        if (map_back) put_mapped(h, c, n, [&](int i) { return orig[i].scale; }, aligned ? &a : nullptr, out_faces, out_crops, out_mats);
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
+}
+}  // extern "C++"
+
+int rf_detect_batch(rf_handle h, const uint8_t *const *imgs, const int *widths, const int *heights, const int *row_strides,
+                    int n, float thr, float nms, rf_face *out_faces, int *out_counts, int32_t *out_idx) {
+    return detect_blocking(h, "rf_detect_batch", BgrImages{imgs, widths, heights, row_strides, nullptr, false}, n, thr, nms, false, nullptr,
+                           false, out_faces, out_counts, out_idx, nullptr, nullptr);
+}
+
+int rf_detect_align_batch(rf_handle h, const uint8_t *const *imgs, const int *widths, const int *heights, const int *row_strides,
+                          int n, float thr, float nms, const rf_align_params *params, rf_face *out_faces, int *out_counts,
+                          void *out_crops, double *out_mats) {
+    return detect_blocking(h, "rf_detect_align_batch", BgrImages{imgs, widths, heights, row_strides, nullptr, false}, n, thr, nms, true, params,
+                           true, out_faces, out_counts, nullptr, out_crops, out_mats);
+}
+
+// f9 oriented images (rf_b200.h rf_detect_oriented_batch)
+int rf_detect_oriented_batch(rf_handle h, const uint8_t *const *imgs, const int *widths, const int *heights, const int *row_strides,
+                             const int *orientations, int n, float thr, float nms, const rf_align_params *align, rf_face *out_faces,
+                             int *out_counts, int32_t *out_idx, void *out_crops, double *out_mats) {
+    return detect_blocking(h, "rf_detect_oriented_batch", BgrImages{imgs, widths, heights, row_strides, orientations, true}, n, thr, nms,
+                           align != nullptr, align, true, out_faces, out_counts, out_idx, out_crops, out_mats);
+}
+
+// f6 video frames: YUV 4:2:0 (yuv.cuh)
+int rf_detect_yuv_batch(rf_handle h, const rf_yuv_frame *frames, int n, int matrix, float thr, float nms, const rf_align_params *align,
+                        rf_face *out_faces, int *out_counts, int32_t *out_idx, void *out_crops, double *out_mats) {
+    return detect_blocking(h, "rf_detect_yuv_batch", YuvFrames{frames, matrix, nullptr, false}, n, thr, nms, align != nullptr, align, true,
+                           out_faces, out_counts, out_idx, out_crops, out_mats);
 }
 
 int rf_detect_align_batch_device(rf_handle h, const uint8_t *dev_bgr, int n, float thr, float nms, const rf_align_params *params,
                                  void *dev_crops, double *dev_mats, const rf_det **dev_dets, const int32_t **dev_counts) {
     if (!h) return RF_ERR_INVALID_ARG;
     AlignArgs a;
-    int rc = align_setup(h, "rf_detect_align_batch_device", params, a);
+    int rc = check_align(h, "rf_detect_align_batch_device", params, n, dev_crops, 0, a);
     if (rc) return rc;
-    if (n > 0 && !dev_crops) return fail(h, RF_ERR_INVALID_ARG, "rf_detect_align_batch_device: dev_crops is NULL");
     Ctx *c = nullptr;
     if ((rc = detect_device_impl(h, dev_bgr, n, thr, nms, dev_dets, dev_counts, false, &c))) return rc;
     if (n == 0) return RF_OK;
-    a.uniform_base = dev_bgr ? dev_bgr : h->d_input;
-    a.uniform_bytes = (size_t)h->cfg.net_h * h->cfg.net_w * 3;
-    a.uniform_w = h->cfg.net_w;
-    a.uniform_h = h->cfg.net_h;
+    // the crops are cut from the network-sized images the forward read
+    const int Hn = h->cfg.net_h, Wn = h->cfg.net_w;
+    const uint8_t *base = dev_bgr ? dev_bgr : h->d_input;
+    std::vector<AlignImageT<BgrRows>> table(n);
+    for (int i = 0; i < n; i++) table[i] = AlignImageT<BgrRows>{BgrRows{base + (size_t)i * Hn * Wn * 3, Wn * 3}, Wn, Hn, 1.f, 0};
     a.n = n;
     a.crops = dev_crops;
     a.mats = dev_mats;
     try {
-        CK(launch_align_faces(a, c->pb, h->num_sms, c->stream));
+        CK(launch_align_faces(a, table.data(), c->pb, h->num_sms, c->stream));
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }
 
-// ---- f9 oriented images (rf_b200.h rf_detect_oriented_batch) ------------------------------------------------------------------------
-static int check_orientations(rf_handle h, const char *who, const int *orientations, int n) {
-    if (n > 0 && !orientations) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: orientations is NULL", who));
-    for (int i = 0; i < n; i++)
-        if (lb_orientation_bits(orientations[i]) < 0)
-            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: item %d: orientation %d, must be in 1..8 (EXIF)", who, i, orientations[i]));
-    return RF_OK;
-}
-
-int rf_detect_oriented_batch(rf_handle h, const uint8_t *const *imgs, const int *widths, const int *heights, const int *row_strides,
-                             const int *orientations, int n, float thr, float nms, const rf_align_params *align, rf_face *out_faces,
-                             int *out_counts, int32_t *out_idx, void *out_crops, double *out_mats) {
-    static const char *who = "rf_detect_oriented_batch";
-    int rc = check_n(h, n);
+// rf_detect_yuv_batch_device, rf_detect_yuv_oriented_device and the detect half of rf_detect_yuv_track_device: the frames are
+// letter-boxed on the context the forward lands on, into that context's own input tensor, and cropped in place.
+static int yuv_device_impl(rf_handle h, const char *who, const YuvFrames &src, int n, float thr, float nms, const rf_align_params *align,
+                           void *dev_crops, double *dev_mats, const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales) {
+    int rc = src.check(h, who, n);
     if (rc) return rc;
     AlignArgs a;
-    if (align && (rc = align_setup(h, who, align, a))) return rc;
-    if (n == 0) return RF_OK;
-    if (!imgs || !widths || !heights) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL image arrays", who));
-    if (align && !out_crops) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: align without out_crops", who));
-    if ((rc = check_orientations(h, who, orientations, n))) return rc;
-    const int Hn = h->cfg.net_h, Wn = h->cfg.net_w;
-    for (int i = 0; i < n; i++)
-        if (!imgs[i] || widths[i] <= 0 || heights[i] <= 0) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: image %d is empty", who, i));
-    if (align) {
-        // rf_detect_align_batch's rule, on the stored images: the crops are cut after the forward, so no raw buffer may be recycled
-        int raw = 0;
-        for (int i = 0; i < n; i++) {
-            const int rs = row_strides && row_strides[i] ? row_strides[i] : widths[i] * 3;
-            raw += !(widths[i] == Wn && heights[i] == Hn && rs == Wn * 3 && orientations[i] == 1);
-        }
-        if (raw > h->raw_slots)
-            return fail(h, RF_ERR_CAPACITY, fmt("%s: %d images need a raw buffer, but the handle keeps at most %d originals resident "
-                                                "(one %dx%d raw buffer each); split the batch", who, raw, h->raw_slots, h->cfg.max_image_w,
-                                                h->cfg.max_image_h));
-    }
-    try {
-        CK(cudaSetDevice(h->device));
-        Ctx &c = h->ctx[0];
-        if (align) ensure_align_buffers(h, n, a);
-        std::vector<AlignImage> orig(n);
-        if ((rc = stage_images(h, c.stream, who, imgs, widths, heights, row_strides, n, orig.data(), orientations))) return rc;
-        set_params(h, c, thr, nms);
-        forward_graph(h, c, n);
-        if (align) {
-            a.n = n;
-            a.crops = h->d_align_crops;
-            a.mats = out_mats ? h->d_align_mats : nullptr;
-            CK(launch_align_faces(a, orig.data(), c.pb, h->num_sms, c.stream, true));
-        }
-        fetch_results(h, c, n, nullptr, out_counts, out_idx);
-        put_mapped(h, c, n, [&](int i) { return orig[i].scale; }, align ? &a : nullptr, out_faces, out_crops, out_mats);
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    return RF_OK;
-}
-
-// ---- f6 video frames: YUV 4:2:0 (yuv.cuh) ---------------------------------------------------------------------------------------
-// Checks n, the matrix and every frame descriptor; nothing is launched before this passes.
-static int check_frames(rf_handle h, const char *who, const rf_yuv_frame *frames, int n, int matrix) {
-    int rc = check_n(h, n);
-    if (rc) return rc;
-    if (n > 0 && !frames) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frames is NULL", who));
-    if (matrix != RF_YUV_BT601 && matrix != RF_YUV_BT709) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: unknown matrix %d", who, matrix));
-    for (int i = 0; i < n; i++) {
-        const rf_yuv_frame &f = frames[i];
-        if (f.width <= 0 || f.height <= 0 || (f.width & 1) || (f.height & 1))
-            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frame %d is %dx%d; 4:2:0 sizes must be positive and even", who, i, f.width, f.height));
-        if (!f.y || !f.u || !f.v) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frame %d has a NULL plane", who, i));
-        if (f.uv_step != 1 && f.uv_step != 2) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frame %d: uv_step %d, must be 1 or 2", who, i, f.uv_step));
-        const uintptr_t u = (uintptr_t)f.u, v = (uintptr_t)f.v;
-        if (f.uv_step == 2 && u != v + 1 && v != u + 1)
-            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frame %d: semi-planar u and v must be adjacent bytes of one plane", who, i));
-        if (f.y_pitch < f.width || f.uv_pitch < f.width / 2 * f.uv_step)
-            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frame %d: pitches %d / %d below the row bytes %d / %d", who, i, f.y_pitch, f.uv_pitch, f.width,
-                                                   f.width / 2 * f.uv_step));
-        if (f.width > h->cfg.max_image_w || f.height > h->cfg.max_image_h)
-            return fail(h, RF_ERR_CAPACITY, fmt("%s: frame %d is %dx%d, larger than max_image %dx%d", who, i, f.width, f.height, h->cfg.max_image_w,
-                                                h->cfg.max_image_h));
-    }
-    return RF_OK;
-}
-
-static YuvPlanes planes_of(const rf_yuv_frame &f, int matrix) { return YuvPlanes{f.y, f.u, f.v, f.y_pitch, f.uv_pitch, f.uv_step, matrix}; }
-
-// One host frame -> raw buffer `raw_slot` on `s`, 1.5 bytes per pixel: the luma packed, then the chroma as the frame lays it out
-// (one interleaved w x h/2 plane, or two w/2 x h/2 planes).  Returns the device planes.
-static YuvPlanes upload_frame(rf_handle h, cudaStream_t s, const rf_yuv_frame &f, int matrix, int raw_slot) {
-    uint8_t *d = h->d_raw + (size_t)raw_slot * h->raw_bytes, *dc = d + (size_t)f.width * f.height;
-    const int cw = f.width / 2, ch = f.height / 2;
-    upload_plane(h, s, d, f.y, f.width, f.y_pitch, f.height);
-    YuvPlanes p{d, dc, dc, f.width, f.width, f.uv_step, matrix};
-    if (f.uv_step == 2) {
-        const uint8_t *first = std::min(f.u, f.v);
-        upload_plane(h, s, dc, first, f.width, f.uv_pitch, ch);
-        p.u = dc + (f.u - first);
-        p.v = dc + (f.v - first);
-    } else {
-        upload_plane(h, s, dc, f.u, cw, f.uv_pitch, ch);
-        upload_plane(h, s, dc + (size_t)cw * ch, f.v, cw, f.uv_pitch, ch);
-        p.v = dc + (size_t)cw * ch;
-        p.uv_pitch = cw;
-    }
-    return p;
-}
-
-int rf_detect_yuv_batch(rf_handle h, const rf_yuv_frame *frames, int n, int matrix, float thr, float nms, const rf_align_params *align,
-                        rf_face *out_faces, int *out_counts, int32_t *out_idx, void *out_crops, double *out_mats) {
-    static const char *who = "rf_detect_yuv_batch";
-    int rc = check_frames(h, who, frames, n, matrix);
-    if (rc) return rc;
-    AlignArgs a;
-    if (align && (rc = align_setup(h, who, align, a))) return rc;
-    if (n == 0) return RF_OK;
-    if (align && !out_crops) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: align without out_crops", who));
-    // the crops are cut from the frames after the forward: each needs a raw buffer of its own for the whole call
-    if (align && n > h->raw_slots)
-        return fail(h, RF_ERR_CAPACITY, fmt("%s: %d frames to align, but the handle keeps at most %d resident (one %dx%d raw buffer each); split the batch",
-                                            who, n, h->raw_slots, h->cfg.max_image_w, h->cfg.max_image_h));
+    if (align && (rc = check_align(h, who, align, n, dev_crops, 0, a))) return rc;
     const int Hn = h->cfg.net_h, Wn = h->cfg.net_w;
     const size_t img_bytes = (size_t)Hn * Wn * 3;
     const int area = (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0;
-    try {
-        CK(cudaSetDevice(h->device));
-        Ctx &c = h->ctx[0];
-        if (align) ensure_align_buffers(h, n, a);
-        std::vector<LbYuvItem> lb;
-        std::vector<AlignYuvImage> orig(n);
-        for (int i = 0; i < n; i++) {
-            // a full chunk of raw buffers is letter-boxed before the next frame reuses the first (stream order)
-            if ((int)lb.size() == h->raw_slots) { CK(launch_letterbox_batch(lb.data(), (int)lb.size(), Wn, Hn, c.stream)); lb.clear(); }
-            const rf_yuv_frame &f = frames[i];
-            const YuvPlanes p = upload_frame(h, c.stream, f, matrix, (int)lb.size());
-            lb.emplace_back();
-            orig[i] = AlignYuvImage{p, f.width, f.height, letterbox_fill(lb.back(), p, f.width, f.height, h->d_input + i * img_bytes, Wn, Hn, 0, area)};
-        }
-        CK(launch_letterbox_batch(lb.data(), (int)lb.size(), Wn, Hn, c.stream));
-        set_params(h, c, thr, nms);
-        forward_graph(h, c, n);
-        if (align) {
-            a.n = n;
-            a.crops = h->d_align_crops;
-            a.mats = out_mats ? h->d_align_mats : nullptr;
-            CK(launch_align_faces_yuv(a, orig.data(), c.pb, h->num_sms, c.stream));
-        }
-        fetch_results(h, c, n, nullptr, out_counts, out_idx);
-        put_mapped(h, c, n, [&](int i) { return orig[i].scale; }, align ? &a : nullptr, out_faces, out_crops, out_mats);
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    return RF_OK;
-}
-
-// rf_detect_yuv_batch_device, and with `orient` (f9: frame i shown in EXIF orientation orient[i]) rf_detect_yuv_oriented_device
-static int yuv_device_impl(rf_handle h, const char *who, const rf_yuv_frame *frames, const int *orient, int n, int matrix, float thr, float nms,
-                           const rf_align_params *align, void *dev_crops, double *dev_mats, const rf_det **dev_dets, const int32_t **dev_counts,
-                           float *out_scales) {
-    int rc = check_frames(h, who, frames, n, matrix);
-    if (rc) return rc;
-    AlignArgs a;
-    if (align && (rc = align_setup(h, who, align, a))) return rc;
-    if (align && n > 0 && !dev_crops) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: align without dev_crops", who));
-    if (orient && (rc = check_orientations(h, who, orient, n))) return rc;
-    const int Hn = h->cfg.net_h, Wn = h->cfg.net_w;
-    const size_t img_bytes = (size_t)Hn * Wn * 3;
-    const int area = (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0;
-    std::vector<AlignYuvImage> orig(n);
-    // the frames are letter-boxed on the context the forward lands on, into that context's own input tensor
+    std::vector<AlignImageT<YuvPlanes>> orig(n);
     auto stage = [&](Ctx &c) -> const uint8_t * {
         if (!c.d_frames_in) CK(cudaMalloc(&c.d_frames_in, (size_t)h->cfg.max_batch * img_bytes));
         std::vector<LbYuvItem> lb(n);
         for (int i = 0; i < n; i++) {
-            const rf_yuv_frame &f = frames[i];
-            const YuvPlanes p = planes_of(f, matrix);
-            const int bits = orient ? lb_orientation_bits(orient[i]) : 0;
-            const int dw = (bits & LB_TRANSPOSE) ? f.height : f.width, dh = (bits & LB_TRANSPOSE) ? f.width : f.height;
-            orig[i] = AlignYuvImage{p, dw, dh, letterbox_fill(lb[i], p, dw, dh, c.d_frames_in + i * img_bytes, Wn, Hn, bits, area), bits};
+            const YuvPlanes p = src.in_place(i);
+            const int bits = src.bits(i);
+            int dw, dh;
+            displayed_size(src, i, dw, dh);
+            orig[i] = AlignImageT<YuvPlanes>{p, dw, dh, letterbox_fill(lb[i], p, dw, dh, c.d_frames_in + i * img_bytes, Wn, Hn, bits, area), bits};
             if (out_scales) out_scales[i] = orig[i].scale;
         }
         CK(launch_letterbox_batch(lb.data(), n, Wn, Hn, c.stream));
@@ -994,55 +963,22 @@ static int yuv_device_impl(rf_handle h, const char *who, const rf_yuv_frame *fra
     a.crops = dev_crops;
     a.mats = dev_mats;
     try {
-        CK(launch_align_faces_yuv(a, orig.data(), c->pb, h->num_sms, c->stream, orient != nullptr));
+        CK(launch_align_faces(a, orig.data(), c->pb, h->num_sms, c->stream, src.oriented));
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }
 
 int rf_detect_yuv_batch_device(rf_handle h, const rf_yuv_frame *frames, int n, int matrix, float thr, float nms, const rf_align_params *align,
                                void *dev_crops, double *dev_mats, const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales) {
-    return yuv_device_impl(h, "rf_detect_yuv_batch_device", frames, nullptr, n, matrix, thr, nms, align, dev_crops, dev_mats, dev_dets, dev_counts,
-                           out_scales);
+    return yuv_device_impl(h, "rf_detect_yuv_batch_device", YuvFrames{frames, matrix, nullptr, false}, n, thr, nms, align, dev_crops, dev_mats,
+                           dev_dets, dev_counts, out_scales);
 }
 
 int rf_detect_yuv_oriented_device(rf_handle h, const rf_yuv_frame *frames, const int *orientations, int n, int matrix, float thr, float nms,
                                   const rf_align_params *align, void *dev_crops, double *dev_mats, const rf_det **dev_dets,
                                   const int32_t **dev_counts, float *out_scales) {
-    static const char *who = "rf_detect_yuv_oriented_device";
-    if (!h) return RF_ERR_INVALID_ARG;
-    if (n > 0 && !orientations) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: orientations is NULL", who));
-    return yuv_device_impl(h, who, frames, orientations, n, matrix, thr, nms, align, dev_crops, dev_mats, dev_dets,
-                           dev_counts, out_scales);
-}
-
-static int preprocess_yuv_impl(rf_handle h, const char *who, const rf_yuv_frame *frame, int matrix, int orientation, uint8_t *out) {
-    if (!h) return RF_ERR_INVALID_ARG;
-    if (!frame || !out) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL frame or output", who));
-    int rc = check_frames(h, who, frame, 1, matrix);
-    if (rc) return rc;
-    if ((rc = check_orientations(h, who, &orientation, 1))) return rc;
-    const int bits = lb_orientation_bits(orientation);
-    const int dw = (bits & LB_TRANSPOSE) ? frame->height : frame->width, dh = (bits & LB_TRANSPOSE) ? frame->width : frame->height;
-    const int Hn = h->cfg.net_h, Wn = h->cfg.net_w;
-    try {
-        CK(cudaSetDevice(h->device));
-        cudaStream_t s = h->ctx[0].stream;
-        const YuvPlanes p = upload_frame(h, s, *frame, matrix, 0);
-        LbYuvItem it;
-        letterbox_fill(it, p, dw, dh, h->d_input, Wn, Hn, bits, (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0);
-        CK(launch_letterbox_batch(&it, 1, Wn, Hn, s));
-        CK(cudaMemcpyAsync(h->h_input, h->d_input, (size_t)Hn * Wn * 3, cudaMemcpyDeviceToHost, s));
-        CK(cudaStreamSynchronize(s));
-        memcpy(out, h->h_input, (size_t)Hn * Wn * 3);
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    return RF_OK;
-}
-
-int rf_preprocess_yuv(rf_handle h, const rf_yuv_frame *frame, int matrix, uint8_t *out) {
-    return preprocess_yuv_impl(h, "rf_preprocess_yuv", frame, matrix, 1, out);
-}
-int rf_preprocess_yuv_oriented(rf_handle h, const rf_yuv_frame *frame, int matrix, int orientation, uint8_t *out) {
-    return preprocess_yuv_impl(h, "rf_preprocess_yuv_oriented", frame, matrix, orientation, out);
+    return yuv_device_impl(h, "rf_detect_yuv_oriented_device", YuvFrames{frames, matrix, orientations, true}, n, thr, nms, align, dev_crops,
+                           dev_mats, dev_dets, dev_counts, out_scales);
 }
 
 // ---- f7 tiled detection: a scale pyramid cut into network-sized tiles (preprocess.cuh tile_layout) ----------------------------------
@@ -1056,41 +992,52 @@ int rf_tile_layout(int net_w, int net_h, int width, int height, const rf_tiling 
     return (int)tiles.size();
 }
 
-// The checks every tiled entry point shares, after its own input checks: the resize definition and each image's layout.
-static int tiled_layouts(rf_handle h, const char *who, int n, const int *widths, const int *heights, const rf_tiling *t,
-                         std::vector<std::vector<rf_tile>> &layouts) {
+
+extern "C++" {
+// The checks every tiled path shares, after its source check: the resize definition and each image's layout.
+template <typename Source>
+static int tiled_layouts(rf_handle h, const char *who, const Source &src, int n, const rf_tiling *t, std::vector<std::vector<rf_tile>> &layouts) {
     if (h->cfg.flags & RF_FLAG_NPP_RESIZE)
         return fail(h, RF_ERR_UNSUPPORTED, fmt("%s: tiles are levels of cv::resize; the handle letter-boxes with NPPI_INTER_SUPER, which "
                                                "only down-samples", who));
     layouts.resize(n);
     for (int i = 0; i < n; i++) {
         std::string err;
-        const int rc = tile_layout(h->cfg.net_w, h->cfg.net_h, widths[i], heights[i], t, layouts[i], &err);
+        const int rc = tile_layout(h->cfg.net_w, h->cfg.net_h, src.width(i), src.height(i), t, layouts[i], &err);
         if (rc) return fail(h, rc, fmt("%s: image %d: %s", who, i, err.c_str()));
     }
     return RF_OK;
 }
 
+// The front end of every tiled entry point: the source check, the layouts, then the align checks (`resident`: the blocking paths
+// keep every original in a raw buffer of its own until the crops are cut).
+template <typename Source>
+static int tiled_check(rf_handle h, const char *who, const Source &src, int n, const rf_tiling *t, bool aligned, const rf_align_params *align,
+                       const void *crops, bool resident, std::vector<std::vector<rf_tile>> &layouts, AlignArgs &a) {
+    int rc = src.check(h, who, n);
+    if (rc) return rc;
+    if ((rc = tiled_layouts(h, who, src, n, t, layouts))) return rc;
+    return aligned ? check_align(h, who, align, n, crops, resident ? n : 0, a) : RF_OK;
+}
+
 // Tiled detection of n images whose layouts are checked, into `dst` (its candidate lists empty: allocation and every k_nms leave
-// them so), the final NMS on `home`.  source(s, i, slot) returns the letter-box source of image i; the blocking paths upload it
-// into raw buffer `slot` on s, a `group` of raw buffers at a time, the device paths return the caller's memory (one group).  The
+// them so), the final NMS on `home`.  The blocking paths upload image i into raw buffer `slot` on home, a `group` of raw buffers at
+// a time; with `in_place` (one group), the device paths read the caller's memory.  The
 // tiles are letter-boxed, detected and merged in chunks of up to max_batch, each chunk on the next context of the
 // rf_detect_batch_device rotation, into that context's own input tensor.  Another context waits for `ready` -- recorded on home
 // once the group's sources are on the device and `dst` may be written -- before its first letter-box of the group, or, with
 // `in_place` (the sources are the caller's device memory), only before its first merge.  Home waits for every context the group
 // used before the next group overwrites the raw buffers, and before the final NMS.
-extern "C++" {
-template <typename Src, typename Source>
-static void detect_tiled_impl(rf_handle h, int n, const int *widths, const int *heights, const std::vector<std::vector<rf_tile>> &layouts,
-                              Source source, int group, bool in_place, Ctx &home, cudaEvent_t ready, PostBuffers &dst, float thr, float nms,
-                              std::vector<Src> &src) {
+template <typename Source>
+static void detect_tiled_impl(rf_handle h, const Source &source, int n, const std::vector<std::vector<rf_tile>> &layouts, int group, bool in_place,
+                              Ctx &home, cudaEvent_t ready, PostBuffers &dst, float thr, float nms, std::vector<typename Source::Src> &src) {
     const int Hn = h->cfg.net_h, Wn = h->cfg.net_w, mf = h->cfg.max_faces, B = h->cfg.max_batch;
     const size_t img_bytes = (size_t)Hn * Wn * 3;
     src.resize(n);
     struct TileRef { int image, tile; };
     for (int g0 = 0; g0 < n; g0 += group) {
         const int g1 = std::min(n, g0 + group);
-        for (int i = g0; i < g1; i++) src[i] = source(home.stream, i, i - g0);
+        for (int i = g0; i < g1; i++) src[i] = in_place ? source.in_place(i) : source.upload(h, home.stream, i, i - g0);
         CK(cudaEventRecord(ready, home.stream));
         std::vector<TileRef> refs;
         for (int i = g0; i < g1; i++)
@@ -1105,13 +1052,13 @@ static void detect_tiled_impl(rf_handle h, int n, const int *widths, const int *
             joined[ci] = 1;
             if (!c.d_frames_in) CK(cudaMalloc(&c.d_frames_in, (size_t)B * img_bytes));
             if (c.param_seq && c.param_seq % Ctx::kParamSlots == 0) CK(cudaStreamSynchronize(c.stream));
-            std::vector<LbItemT<Src>> lb(m);
+            std::vector<LbItemT<typename Source::Src>> lb(m);
             std::vector<MergeSource> ms(m);
             for (int b = 0; b < m; b++) {
                 const TileRef r = refs[k0 + b];
                 const rf_tile &tl = layouts[r.image][r.tile];
-                tile_fill(lb[b], src[r.image], widths[r.image], heights[r.image], c.d_frames_in + b * img_bytes, Wn, Hn, tl);
-                ms[b] = tile_source(r.image, r.tile, mf, tl, widths[r.image]);
+                tile_fill(lb[b], src[r.image], source.width(r.image), source.height(r.image), c.d_frames_in + b * img_bytes, Wn, Hn, tl);
+                ms[b] = tile_source(r.image, r.tile, mf, tl, source.width(r.image));
             }
             CK(launch_letterbox_batch(lb.data(), m, Wn, Hn, c.stream));
             set_params(h, c, thr, nms, c.d_frames_in);
@@ -1131,7 +1078,6 @@ static void detect_tiled_impl(rf_handle h, int n, const int *widths, const int *
     launch_nms(n, home.d_params, dst, home.stream);
     CK(cudaGetLastError());
 }
-}  // extern "C++"
 
 // Makes room in pb for the candidates of the largest layout: every tile of an image may contribute max_faces.
 static bool tiled_grow(rf_handle h, PostBuffers &pb, const std::vector<std::vector<rf_tile>> &layouts) {
@@ -1144,55 +1090,48 @@ static bool tiled_grow(rf_handle h, PostBuffers &pb, const std::vector<std::vect
     return true;
 }
 
-// The crop source of a tiled path's image i: its original, at map-back factor 1 (the merged records are in image pixels).
-extern "C++" {
-static AlignImage align_source(const uint8_t *p, int w, int hgt) { return AlignImage{p, w, hgt, w * 3, 1.f}; }
-static AlignImage align_source(const BgrRows &r, int w, int hgt) { return AlignImage{r.p, w, hgt, r.pitch, 1.f}; }
-static AlignYuvImage align_source(const YuvPlanes &p, int w, int hgt) { return AlignYuvImage{p, w, hgt, 1.f}; }
-static cudaError_t launch_align_table(const AlignArgs &a, const std::vector<AlignImage> &im, const PostBuffers &pb, int sms, cudaStream_t s) {
-    return launch_align_faces(a, im.data(), pb, sms, s);
-}
-static cudaError_t launch_align_table(const AlignArgs &a, const std::vector<AlignYuvImage> &im, const PostBuffers &pb, int sms, cudaStream_t s) {
-    return launch_align_faces_yuv(a, im.data(), pb, sms, s);
-}
 
-
-// The crops of every kept face in pb (a.crops / a.mats set by the caller), cut on s from the originals src.
-template <typename Src>
-static void tiled_crops(rf_handle h, AlignArgs a, int n, const int *widths, const int *heights, const std::vector<Src> &src, const PostBuffers &pb,
+// The crops of every kept face in pb (a.crops / a.mats set by the caller), cut on s from the originals srcs at map-back factor 1
+// (the merged records are in image pixels).
+template <typename Source>
+static void tiled_crops(rf_handle h, AlignArgs a, int n, const Source &source, const std::vector<typename Source::Src> &srcs, const PostBuffers &pb,
                         cudaStream_t s) {
-    std::vector<decltype(align_source(src[0], 0, 0))> im(n);
-    for (int i = 0; i < n; i++) im[i] = align_source(src[i], widths[i], heights[i]);
+    std::vector<AlignImageT<typename Source::Src>> table(n);
+    for (int i = 0; i < n; i++) table[i] = AlignImageT<typename Source::Src>{srcs[i], source.width(i), source.height(i), 1.f, 0};
     a.n = n;
-    CK(launch_align_table(a, im, pb, h->num_sms, s));
+    CK(launch_align_faces(a, table.data(), pb, h->num_sms, s));
 }
 
-// The blocking tiled paths: sources uploaded on context 0, merged into pb_tiles, fetched.  With `a` (the call has checked that
-// every image gets a raw buffer of its own, so all originals stay resident), the crops are cut on context 0 after the NMS and
-// copied out with the faces.
-template <typename Src, typename Upload>
-static void detect_tiled_blocking(rf_handle h, int n, const int *widths, const int *heights, const std::vector<std::vector<rf_tile>> &layouts,
-                                  Upload upload, float thr, float nms, const AlignArgs *a, rf_face *out_faces, int *out_counts,
-                                  int32_t *out_tile_of, void *out_crops, double *out_mats) {
-    const int mf = h->cfg.max_faces;
-    tiled_grow(h, h->pb_tiles, layouts);
-    Ctx &c0 = h->ctx[0];
-    std::vector<Src> src;
-    detect_tiled_impl<Src>(h, n, widths, heights, layouts, upload, h->raw_slots, false, c0, c0.fence, h->pb_tiles, thr, nms, src);
-    AlignArgs aa{};
-    if (a) {
-        ensure_align_buffers(h, n, *a);
-        aa = *a;
-        aa.n = n;
-        aa.crops = h->d_align_crops;
-        aa.mats = out_mats ? h->d_align_mats : nullptr;
-        tiled_crops(h, aa, n, widths, heights, src, h->pb_tiles, c0.stream);
-    }
-    fetch_post(h, h->pb_tiles, c0.stream, n, out_faces, out_counts, out_tile_of);
-    if (out_tile_of)      // candidate id = tile * max_faces + rank
-        for (int i = 0; i < n; i++)
-            for (int j = 0; j < std::min(h->h_counts[i], mf); j++) out_tile_of[(size_t)i * mf + j] /= mf;
-    if (a) put_mapped(h, c0, n, [](int) { return 1.f; }, &aa, nullptr, out_crops, out_mats);
+// The blocking tiled paths: sources uploaded on context 0, merged into pb_tiles, fetched.  With `aligned`, the crops are cut on
+// context 0 after the NMS and copied out with the faces.
+template <typename Source>
+static int detect_tiled_blocking(rf_handle h, const char *who, const Source &source, int n, const rf_tiling *t, float thr, float nms, bool aligned,
+                                 const rf_align_params *align, rf_face *out_faces, int *out_counts, int32_t *out_tile_of, void *out_crops,
+                                 double *out_mats) {
+    std::vector<std::vector<rf_tile>> layouts;
+    AlignArgs a;
+    int rc = tiled_check(h, who, source, n, t, aligned, align, out_crops, true, layouts, a);
+    if (rc || n == 0) return rc;
+    try {
+        CK(cudaSetDevice(h->device));
+        const int mf = h->cfg.max_faces;
+        tiled_grow(h, h->pb_tiles, layouts);
+        Ctx &c0 = h->ctx[0];
+        std::vector<typename Source::Src> srcs;
+        detect_tiled_impl(h, source, n, layouts, h->raw_slots, false, c0, c0.fence, h->pb_tiles, thr, nms, srcs);
+        if (aligned) {
+            ensure_align_buffers(h, n, a);
+            a.crops = h->d_align_crops;
+            a.mats = out_mats ? h->d_align_mats : nullptr;
+            tiled_crops(h, a, n, source, srcs, h->pb_tiles, c0.stream);
+        }
+        fetch_post(h, h->pb_tiles, c0.stream, n, out_faces, out_counts, out_tile_of);
+        if (out_tile_of)      // candidate id = tile * max_faces + rank
+            for (int i = 0; i < n; i++)
+                for (int j = 0; j < std::min(h->h_counts[i], mf); j++) out_tile_of[(size_t)i * mf + j] /= mf;
+        if (aligned) put_mapped(h, c0, n, [](int) { return 1.f; }, &a, nullptr, out_crops, out_mats);
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
 }
 
 // The asynchronous tiled paths: the caller's device sources src[i] read in place, merged into the next slot of the ring, the final
@@ -1202,200 +1141,116 @@ static void detect_tiled_blocking(rf_handle h, int n, const int *widths, const i
 //   2. A slot that must grow is freed only after the host has waited for `free`, and its counts are cleared on home before `start`.
 //   3. Home joins every context it used through their fence events before the NMS.
 //   4. The crops are cut on home after the NMS; then `free` is recorded.
-template <typename Src>
-static void detect_tiled_device(rf_handle h, int n, const int *widths, const int *heights, const std::vector<std::vector<rf_tile>> &layouts,
-                                const std::vector<Src> &dev_src, float thr, float nms, const AlignArgs *a, void *dev_crops, double *dev_mats,
-                                const rf_det **dev_dets, const int32_t **dev_counts) {
-    if (h->tiled_slots.empty()) {
-        h->tiled_slots.resize(h->ctx.size());
-        for (auto &s : h->tiled_slots) {
-            CK(cudaEventCreateWithFlags(&s.free, cudaEventDisableTiming));
-            CK(cudaEventCreateWithFlags(&s.start, cudaEventDisableTiming));
+template <typename Source>
+static int detect_tiled_device(rf_handle h, const char *who, const Source &source, int n, const rf_tiling *t, float thr, float nms,
+                               const rf_align_params *align, void *dev_crops, double *dev_mats, const rf_det **dev_dets, const int32_t **dev_counts) {
+    std::vector<std::vector<rf_tile>> layouts;
+    AlignArgs a;
+    int rc = tiled_check(h, who, source, n, t, align != nullptr, align, dev_crops, false, layouts, a);
+    if (rc || n == 0) return rc;
+    try {
+        CK(cudaSetDevice(h->device));
+        if (h->tiled_slots.empty()) {
+            h->tiled_slots.resize(h->ctx.size());
+            for (auto &s : h->tiled_slots) {
+                CK(cudaEventCreateWithFlags(&s.free, cudaEventDisableTiming));
+                CK(cudaEventCreateWithFlags(&s.start, cudaEventDisableTiming));
+            }
         }
-    }
-    rf_handle_s::TiledSlot &slot = h->tiled_slots[h->next_tiled_slot++ % h->tiled_slots.size()];
-    Ctx &home = h->ctx[h->next_dev_ctx % h->ctx.size()];
-    size_t most = 0;
-    for (const auto &l : layouts) most = std::max(most, l.size());
-    if ((size_t)slot.pb.anchors_per_image < most * h->cfg.max_faces) {
-        CK(cudaEventSynchronize(slot.free));     // the slot's last call has finished with the buffers about to be freed
-        tiled_grow(h, slot.pb, layouts);
-        // alloc_post_buffers clears the counts on the legacy stream, which the contexts' streams do not wait for
-        CK(cudaMemsetAsync(slot.pb.cand_count, 0, sizeof(int) * slot.pb.max_batch, home.stream));
-    }
-    CK(cudaStreamWaitEvent(home.stream, slot.free, 0));
-    std::vector<Src> src;
-    detect_tiled_impl<Src>(h, n, widths, heights, layouts, [&](cudaStream_t, int i, int) { return dev_src[i]; }, n, true, home, slot.start,
-                           slot.pb, thr, nms, src);
-    if (a) {
-        AlignArgs aa = *a;
-        aa.crops = dev_crops;
-        aa.mats = dev_mats;
-        tiled_crops(h, aa, n, widths, heights, src, slot.pb, home.stream);
-    }
-    CK(cudaEventRecord(slot.free, home.stream));
-    h->last_stream = home.stream;
-    if (dev_dets) *dev_dets = slot.pb.out_dets;
-    if (dev_counts) *dev_counts = slot.pb.out_counts;
+        rf_handle_s::TiledSlot &slot = h->tiled_slots[h->next_tiled_slot++ % h->tiled_slots.size()];
+        Ctx &home = h->ctx[h->next_dev_ctx % h->ctx.size()];
+        size_t most = 0;
+        for (const auto &l : layouts) most = std::max(most, l.size());
+        if ((size_t)slot.pb.anchors_per_image < most * h->cfg.max_faces) {
+            CK(cudaEventSynchronize(slot.free));     // the slot's last call has finished with the buffers about to be freed
+            tiled_grow(h, slot.pb, layouts);
+            // alloc_post_buffers clears the counts on the legacy stream, which the contexts' streams do not wait for
+            CK(cudaMemsetAsync(slot.pb.cand_count, 0, sizeof(int) * slot.pb.max_batch, home.stream));
+        }
+        CK(cudaStreamWaitEvent(home.stream, slot.free, 0));
+        std::vector<typename Source::Src> srcs;
+        detect_tiled_impl(h, source, n, layouts, n, true, home, slot.start, slot.pb, thr, nms, srcs);
+        if (align) {
+            a.crops = dev_crops;
+            a.mats = dev_mats;
+            tiled_crops(h, a, n, source, srcs, slot.pb, home.stream);
+        }
+        CK(cudaEventRecord(slot.free, home.stream));
+        h->last_stream = home.stream;
+        if (dev_dets) *dev_dets = slot.pb.out_dets;
+        if (dev_counts) *dev_counts = slot.pb.out_counts;
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
 }
+
 }  // extern "C++"
-
-// Checks of the BGR tiled entry points, before the layouts: NULL arrays, empty images, row strides below 3 w, images above max_image.
-static int check_tiled_images(rf_handle h, const char *who, const uint8_t *const *imgs, const int *widths, const int *heights,
-                              const int *row_strides, int n) {
-    int rc = check_n(h, n);
-    if (rc) return rc;
-    if (n > 0 && (!imgs || !widths || !heights)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL image arrays", who));
-    for (int i = 0; i < n; i++) {
-        if (!imgs[i] || widths[i] <= 0 || heights[i] <= 0) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: image %d is empty", who, i));
-        if (row_strides && row_strides[i] && row_strides[i] < widths[i] * 3)
-            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: image %d: row stride %d below %d bytes", who, i, row_strides[i], widths[i] * 3));
-        if (widths[i] > h->cfg.max_image_w || heights[i] > h->cfg.max_image_h)
-            return fail(h, RF_ERR_CAPACITY, fmt("%s: image %d is %dx%d, larger than max_image %dx%d", who, i, widths[i], heights[i],
-                                                h->cfg.max_image_w, h->cfg.max_image_h));
-    }
-    return RF_OK;
-}
-
-// Checks of the align arguments of a tiled entry point (after its image checks): the params, somewhere for the crops to go, and --
-// for the blocking variants (`resident`) -- a raw buffer for every original until the crops are cut.
-static int check_tiled_align(rf_handle h, const char *who, const rf_align_params *align, int n, const void *crops, bool resident, AlignArgs &a) {
-    int rc = align_setup(h, who, align, a);
-    if (rc) return rc;
-    if (n > 0 && !crops) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: align without %s", who, resident ? "out_crops" : "dev_crops"));
-    if (resident && n > h->raw_slots)
-        return fail(h, RF_ERR_CAPACITY, fmt("%s: %d images to align, but the handle keeps at most %d resident (one %dx%d raw buffer each); split "
-                                            "the batch", who, n, h->raw_slots, h->cfg.max_image_w, h->cfg.max_image_h));
-    return RF_OK;
-}
-
-static int tiled_bgr(rf_handle h, const char *who, const uint8_t *const *imgs, const int *widths, const int *heights, const int *row_strides, int n,
-                     const rf_tiling *t, float thr, float nms, bool aligned, const rf_align_params *align, rf_face *out_faces, int *out_counts,
-                     int32_t *out_tile_of, void *out_crops, double *out_mats) {
-    int rc = check_tiled_images(h, who, imgs, widths, heights, row_strides, n);
-    if (rc) return rc;
-    std::vector<std::vector<rf_tile>> layouts;
-    if ((rc = tiled_layouts(h, who, n, widths, heights, t, layouts))) return rc;
-    AlignArgs a;
-    if (aligned && (rc = check_tiled_align(h, who, align, n, out_crops, true, a))) return rc;
-    if (n == 0) return RF_OK;
-    try {
-        CK(cudaSetDevice(h->device));
-        auto upload = [&](cudaStream_t s, int i, int slot) -> const uint8_t * {
-            const int rs = row_strides && row_strides[i] ? row_strides[i] : widths[i] * 3;
-            return upload_raw(h, s, imgs[i], widths[i], heights[i], rs, slot);
-        };
-        detect_tiled_blocking<const uint8_t *>(h, n, widths, heights, layouts, upload, thr, nms, aligned ? &a : nullptr, out_faces, out_counts,
-                                               out_tile_of, out_crops, out_mats);
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    return RF_OK;
-}
-
-static int tiled_yuv(rf_handle h, const char *who, const rf_yuv_frame *frames, int n, int matrix, const rf_tiling *t, float thr, float nms,
-                     bool aligned, const rf_align_params *align, rf_face *out_faces, int *out_counts, int32_t *out_tile_of, void *out_crops,
-                     double *out_mats) {
-    int rc = check_frames(h, who, frames, n, matrix);
-    if (rc) return rc;
-    std::vector<int> widths(n), heights(n);
-    for (int i = 0; i < n; i++) { widths[i] = frames[i].width; heights[i] = frames[i].height; }
-    std::vector<std::vector<rf_tile>> layouts;
-    if ((rc = tiled_layouts(h, who, n, widths.data(), heights.data(), t, layouts))) return rc;
-    AlignArgs a;
-    if (aligned && (rc = check_tiled_align(h, who, align, n, out_crops, true, a))) return rc;
-    if (n == 0) return RF_OK;
-    try {
-        CK(cudaSetDevice(h->device));
-        auto upload = [&](cudaStream_t s, int i, int slot) { return upload_frame(h, s, frames[i], matrix, slot); };
-        detect_tiled_blocking<YuvPlanes>(h, n, widths.data(), heights.data(), layouts, upload, thr, nms, aligned ? &a : nullptr, out_faces,
-                                         out_counts, out_tile_of, out_crops, out_mats);
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    return RF_OK;
-}
 
 int rf_detect_tiled(rf_handle h, const uint8_t *const *imgs, const int *widths, const int *heights, const int *row_strides, int n,
                     const rf_tiling *t, float thr, float nms, rf_face *out_faces, int *out_counts, int32_t *out_tile_of) {
-    return tiled_bgr(h, "rf_detect_tiled", imgs, widths, heights, row_strides, n, t, thr, nms, false, nullptr, out_faces, out_counts, out_tile_of,
-                     nullptr, nullptr);
+    return detect_tiled_blocking(h, "rf_detect_tiled", BgrImages{imgs, widths, heights, row_strides, nullptr, false}, n, t, thr, nms, false,
+                                 nullptr, out_faces, out_counts, out_tile_of, nullptr, nullptr);
 }
 
 int rf_detect_yuv_tiled(rf_handle h, const rf_yuv_frame *frames, int n, int matrix, const rf_tiling *t, float thr, float nms,
                         rf_face *out_faces, int *out_counts, int32_t *out_tile_of) {
-    return tiled_yuv(h, "rf_detect_yuv_tiled", frames, n, matrix, t, thr, nms, false, nullptr, out_faces, out_counts, out_tile_of, nullptr, nullptr);
+    return detect_tiled_blocking(h, "rf_detect_yuv_tiled", YuvFrames{frames, matrix, nullptr, false}, n, t, thr, nms, false, nullptr, out_faces,
+                                 out_counts, out_tile_of, nullptr, nullptr);
 }
 
 int rf_detect_tiled_align(rf_handle h, const uint8_t *const *imgs, const int *widths, const int *heights, const int *row_strides, int n,
                           const rf_tiling *t, float thr, float nms, const rf_align_params *align, rf_face *out_faces, int *out_counts,
                           int32_t *out_tile_of, void *out_crops, double *out_mats) {
-    return tiled_bgr(h, "rf_detect_tiled_align", imgs, widths, heights, row_strides, n, t, thr, nms, true, align, out_faces, out_counts,
-                     out_tile_of, out_crops, out_mats);
+    return detect_tiled_blocking(h, "rf_detect_tiled_align", BgrImages{imgs, widths, heights, row_strides, nullptr, false}, n, t, thr, nms, true,
+                                 align, out_faces, out_counts, out_tile_of, out_crops, out_mats);
 }
 
 int rf_detect_yuv_tiled_align(rf_handle h, const rf_yuv_frame *frames, int n, int matrix, const rf_tiling *t, float thr, float nms,
                               const rf_align_params *align, rf_face *out_faces, int *out_counts, int32_t *out_tile_of, void *out_crops,
                               double *out_mats) {
-    return tiled_yuv(h, "rf_detect_yuv_tiled_align", frames, n, matrix, t, thr, nms, true, align, out_faces, out_counts, out_tile_of, out_crops,
-                     out_mats);
+    return detect_tiled_blocking(h, "rf_detect_yuv_tiled_align", YuvFrames{frames, matrix, nullptr, false}, n, t, thr, nms, true, align, out_faces,
+                                 out_counts, out_tile_of, out_crops, out_mats);
 }
 
 int rf_detect_tiled_device(rf_handle h, const uint8_t *const *dev_bgr, const int *widths, const int *heights, const int *row_strides, int n,
                            const rf_tiling *t, float thr, float nms, const rf_align_params *align, void *dev_crops, double *dev_mats,
                            const rf_det **dev_dets, const int32_t **dev_counts) {
-    static const char *who = "rf_detect_tiled_device";
-    int rc = check_tiled_images(h, who, dev_bgr, widths, heights, row_strides, n);
-    if (rc) return rc;
-    std::vector<std::vector<rf_tile>> layouts;
-    if ((rc = tiled_layouts(h, who, n, widths, heights, t, layouts))) return rc;
-    AlignArgs a;
-    if (align && (rc = check_tiled_align(h, who, align, n, dev_crops, false, a))) return rc;
-    if (n == 0) return RF_OK;
-    std::vector<BgrRows> src(n);
-    for (int i = 0; i < n; i++) src[i] = BgrRows{dev_bgr[i], row_strides && row_strides[i] ? row_strides[i] : widths[i] * 3};
-    try {
-        CK(cudaSetDevice(h->device));
-        detect_tiled_device(h, n, widths, heights, layouts, src, thr, nms, align ? &a : nullptr, dev_crops, dev_mats, dev_dets, dev_counts);
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    return RF_OK;
+    return detect_tiled_device(h, "rf_detect_tiled_device", BgrImages{dev_bgr, widths, heights, row_strides, nullptr, false}, n, t, thr, nms,
+                               align, dev_crops, dev_mats, dev_dets, dev_counts);
 }
 
 int rf_detect_yuv_tiled_device(rf_handle h, const rf_yuv_frame *frames, int n, int matrix, const rf_tiling *t, float thr, float nms,
                                const rf_align_params *align, void *dev_crops, double *dev_mats, const rf_det **dev_dets,
                                const int32_t **dev_counts) {
-    static const char *who = "rf_detect_yuv_tiled_device";
-    int rc = check_frames(h, who, frames, n, matrix);
-    if (rc) return rc;
-    std::vector<int> widths(n), heights(n);
-    for (int i = 0; i < n; i++) { widths[i] = frames[i].width; heights[i] = frames[i].height; }
-    std::vector<std::vector<rf_tile>> layouts;
-    if ((rc = tiled_layouts(h, who, n, widths.data(), heights.data(), t, layouts))) return rc;
-    AlignArgs a;
-    if (align && (rc = check_tiled_align(h, who, align, n, dev_crops, false, a))) return rc;
-    if (n == 0) return RF_OK;
-    std::vector<YuvPlanes> src(n);
-    for (int i = 0; i < n; i++) src[i] = planes_of(frames[i], matrix);
-    try {
-        CK(cudaSetDevice(h->device));
-        detect_tiled_device(h, n, widths.data(), heights.data(), layouts, src, thr, nms, align ? &a : nullptr, dev_crops, dev_mats, dev_dets,
-                            dev_counts);
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    return RF_OK;
+    return detect_tiled_device(h, "rf_detect_yuv_tiled_device", YuvFrames{frames, matrix, nullptr, false}, n, t, thr, nms, align, dev_crops,
+                               dev_mats, dev_dets, dev_counts);
 }
 
-// The parity hooks of the tiled paths: tile `tile` of one image's layout into `out`.  upload(s) brings the image into raw buffer 0
-// on s and returns the letter-box source.
+// ---- parity hooks: the network input of one image ---------------------------------------------------------------------------------
+// Image 0 of src uploaded into raw buffer 0 and letter-boxed (with `tiled`, tile `tile` of its layout) into `out`.
 extern "C++" {
-template <typename Src, typename Upload>
-static int preprocess_tile_impl(rf_handle h, const char *who, int width, int height, const rf_tiling *t, int tile, uint8_t *out, Upload upload) {
-    std::vector<std::vector<rf_tile>> layouts;
-    int rc = tiled_layouts(h, who, 1, &width, &height, t, layouts);
+template <typename Source>
+static int preprocess_one(rf_handle h, const char *who, const Source &src, bool tiled, const rf_tiling *t, int tile, uint8_t *out) {
+    if (!h) return RF_ERR_INVALID_ARG;
+    if (!out) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: out is NULL", who));
+    int rc = src.check(h, who, 1);
     if (rc) return rc;
-    if (tile < 0 || tile >= (int)layouts[0].size())
+    std::vector<std::vector<rf_tile>> layouts;
+    if (tiled && (rc = tiled_layouts(h, who, src, 1, t, layouts))) return rc;
+    if (tiled && (tile < 0 || tile >= (int)layouts[0].size()))
         return fail(h, RF_ERR_INVALID_ARG, fmt("%s: tile %d, the layout has %zu", who, tile, layouts[0].size()));
     const int Hn = h->cfg.net_h, Wn = h->cfg.net_w;
     try {
         CK(cudaSetDevice(h->device));
         cudaStream_t s = h->ctx[0].stream;
-        LbItemT<Src> it;
-        tile_fill(it, upload(s), width, height, h->d_input, Wn, Hn, layouts[0][tile]);
+        const typename Source::Src p = src.upload(h, s, 0, 0);
+        LbItemT<typename Source::Src> it;
+        if (tiled) {
+            tile_fill(it, p, src.width(0), src.height(0), h->d_input, Wn, Hn, layouts[0][tile]);
+        } else {
+            int dw, dh;
+            displayed_size(src, 0, dw, dh);
+            letterbox_fill(it, p, dw, dh, h->d_input, Wn, Hn, src.bits(0), (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0);
+        }
         CK(launch_letterbox_batch(&it, 1, Wn, Hn, s));
         CK(cudaMemcpyAsync(h->h_input, h->d_input, (size_t)Hn * Wn * 3, cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
@@ -1405,24 +1260,23 @@ static int preprocess_tile_impl(rf_handle h, const char *who, int width, int hei
 }
 }  // extern "C++"
 
-int rf_preprocess_tile(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, const rf_tiling *t, int tile, uint8_t *out) {
-    static const char *who = "rf_preprocess_tile";
-    if (!h) return RF_ERR_INVALID_ARG;
-    if (!bgr || !out || width <= 0 || height <= 0) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: bad arguments", who));
-    if (width > h->cfg.max_image_w || height > h->cfg.max_image_h) return fail(h, RF_ERR_CAPACITY, fmt("%s: image larger than max_image", who));
-    const int rs = row_stride ? row_stride : width * 3;
-    return preprocess_tile_impl<const uint8_t *>(h, who, width, height, t, tile, out,
-                                                 [&](cudaStream_t s) { return (const uint8_t *)upload_raw(h, s, bgr, width, height, rs); });
+int rf_preprocess(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, uint8_t *out) {
+    return preprocess_one(h, "rf_preprocess", BgrImages{&bgr, &width, &height, &row_stride, nullptr, false}, false, nullptr, 0, out);
 }
-
+int rf_preprocess_oriented(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, int orientation, uint8_t *out) {
+    return preprocess_one(h, "rf_preprocess_oriented", BgrImages{&bgr, &width, &height, &row_stride, &orientation, true}, false, nullptr, 0, out);
+}
+int rf_preprocess_yuv(rf_handle h, const rf_yuv_frame *frame, int matrix, uint8_t *out) {
+    return preprocess_one(h, "rf_preprocess_yuv", YuvFrames{frame, matrix, nullptr, false}, false, nullptr, 0, out);
+}
+int rf_preprocess_yuv_oriented(rf_handle h, const rf_yuv_frame *frame, int matrix, int orientation, uint8_t *out) {
+    return preprocess_one(h, "rf_preprocess_yuv_oriented", YuvFrames{frame, matrix, &orientation, true}, false, nullptr, 0, out);
+}
+int rf_preprocess_tile(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, const rf_tiling *t, int tile, uint8_t *out) {
+    return preprocess_one(h, "rf_preprocess_tile", BgrImages{&bgr, &width, &height, &row_stride, nullptr, false}, true, t, tile, out);
+}
 int rf_preprocess_yuv_tile(rf_handle h, const rf_yuv_frame *frame, int matrix, const rf_tiling *t, int tile, uint8_t *out) {
-    static const char *who = "rf_preprocess_yuv_tile";
-    if (!h) return RF_ERR_INVALID_ARG;
-    if (!frame || !out) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL frame or output", who));
-    int rc = check_frames(h, who, frame, 1, matrix);
-    if (rc) return rc;
-    return preprocess_tile_impl<YuvPlanes>(h, who, frame->width, frame->height, t, tile, out,
-                                           [&](cudaStream_t s) { return upload_frame(h, s, *frame, matrix, 0); });
+    return preprocess_one(h, "rf_preprocess_yuv_tile", YuvFrames{frame, matrix, nullptr, false}, true, t, tile, out);
 }
 
 // ---- f1 ingest: compressed images (main.cpp:18-26 decodes on the host with cv::imread) ---------------------------------------
@@ -1459,7 +1313,7 @@ int rf_detect_jpeg_batch(rf_handle h, const uint8_t *const *jpegs, const size_t 
                 dst.push_back(direct ? h->d_input + (size_t)i1 * img_bytes : h->d_raw + (size_t)used * h->raw_bytes);
                 if (!direct) {
                     lb.emplace_back();
-                    letterbox_fill(lb.back(), dst.back(), w[i1], hg[i1], h->d_input + (size_t)i1 * img_bytes, Wn, Hn, 0, area);
+                    letterbox_fill(lb.back(), BgrRows{dst.back(), w[i1] * 3}, w[i1], hg[i1], h->d_input + (size_t)i1 * img_bytes, Wn, Hn, 0, area);
                     used++;
                 }
             }
@@ -1621,7 +1475,9 @@ static int views_impl(rf_handle h, const char *who, const uint8_t *bgr, int widt
     if (!h || !bgr || !views || !out_count || width <= 0 || height <= 0) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: bad arguments", who));
     if (nviews < 1 || nviews > RF_MAX_VIEWS || nviews > h->cfg.max_batch)
         return fail(h, RF_ERR_CAPACITY, fmt("%s: %d views, limit min(RF_MAX_VIEWS = %d, max_batch = %d)", who, nviews, RF_MAX_VIEWS, h->cfg.max_batch));
-    if (width > h->cfg.max_image_w || height > h->cfg.max_image_h) return fail(h, RF_ERR_CAPACITY, fmt("%s: image larger than max_image", who));
+    const BgrImages src{&bgr, &width, &height, &row_stride, nullptr, false};
+    int rc = src.check(h, who, 1);
+    if (rc) return rc;
     for (int v = 0; v < nviews; v++) {
         const float shrink = shrink_of(v);
         if (!(shrink > 0.f && shrink <= 1.f)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: view %d: shrink must be in (0, 1]", who, v));
@@ -1630,13 +1486,12 @@ static int views_impl(rf_handle h, const char *who, const uint8_t *bgr, int widt
     static_assert(RF_MAX_VIEWS == RF_MAX_VIEWS_DEV, "view capacity of the merge kernel");
     const int Hn = h->cfg.net_h, Wn = h->cfg.net_w, mf = h->cfg.max_faces;
     const size_t img_bytes = (size_t)Hn * Wn * 3;
-    const int rs = row_stride ? row_stride : width * 3;
     try {
         CK(cudaSetDevice(h->device));
         Ctx &c = h->ctx[0];
         // every view may contribute max_faces candidates to the merged list of the one image
         if (!h->pb_merge.cand_keys) alloc_post_buffers(h->pb_merge, h->cfg.max_batch * mf, 1, mf);
-        const uint8_t *d_src = upload_raw(h, c.stream, bgr, width, height, rs);
+        const BgrRows d_src = src.upload(h, c.stream, 0, 0);
         const int area = (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0;
         std::vector<LbItem> lb(nviews);
         std::vector<MergeSource> ms(nviews);
@@ -1678,36 +1533,6 @@ int rf_detect_views_oriented(rf_handle h, const uint8_t *bgr, int width, int hei
     return views_impl(h, "rf_detect_views_oriented", bgr, width, height, row_stride, views, nviews, [&](int v) { return views[v].shrink; },
                       [&](int v) { return lb_orientation_bits(views[v].orientation); }, thr, nms, out_faces, out_count, out_view_of,
                       out_view_scales);
-}
-
-static int preprocess_impl(rf_handle h, const char *who, const uint8_t *bgr, int width, int height, int row_stride, int orientation, uint8_t *out) {
-    if (!h || !bgr || !out || width <= 0 || height <= 0) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: bad arguments", who));
-    if (width > h->cfg.max_image_w || height > h->cfg.max_image_h) return fail(h, RF_ERR_CAPACITY, fmt("%s: image larger than max_image", who));
-    int rc = check_orientations(h, who, &orientation, 1);
-    if (rc) return rc;
-    const int bits = lb_orientation_bits(orientation);
-    const int dw = (bits & LB_TRANSPOSE) ? height : width, dh = (bits & LB_TRANSPOSE) ? width : height;
-    const int Hn = h->cfg.net_h, Wn = h->cfg.net_w;
-    const int rs = row_stride ? row_stride : width * 3;
-    try {
-        CK(cudaSetDevice(h->device));
-        cudaStream_t s = h->ctx[0].stream;
-        const uint8_t *d_src = upload_raw(h, s, bgr, width, height, rs);
-        LbItem it;
-        letterbox_fill(it, d_src, dw, dh, h->d_input, Wn, Hn, bits, (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0);
-        CK(launch_letterbox_batch(&it, 1, Wn, Hn, s));
-        CK(cudaMemcpyAsync(h->h_input, h->d_input, (size_t)Hn * Wn * 3, cudaMemcpyDeviceToHost, s));
-        CK(cudaStreamSynchronize(s));
-        memcpy(out, h->h_input, (size_t)Hn * Wn * 3);
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    return RF_OK;
-}
-
-int rf_preprocess(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, uint8_t *out) {
-    return preprocess_impl(h, "rf_preprocess", bgr, width, height, row_stride, 1, out);
-}
-int rf_preprocess_oriented(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, int orientation, uint8_t *out) {
-    return preprocess_impl(h, "rf_preprocess_oriented", bgr, width, height, row_stride, orientation, out);
 }
 
 static void ensure_blobs(rf_handle h) {
@@ -2131,7 +1956,7 @@ static int check_track_args(rf_tracker t, const char *who, const int *videos, in
 // Issues the update of n frames on s (the records complete there) into the next ring slot, ordered by the chain.  `a` (crops):
 // the due faces are cut on s into a's crops, then the slot's `free` is recorded.
 static void track_issue(rf_tracker t, const int *videos, int n, const rf_det *dets, const int32_t *counts, const float *scales, cudaStream_t s,
-                        const AlignArgs *a, const YuvPlanes *planes, const int *widths, const int *heights, const rf_track **dev_tracks,
+                        const AlignArgs *a, const AlignImageT<YuvPlanes> *table, const rf_track **dev_tracks,
                         const int32_t **dev_track_counts) {
     rf_handle h = t->h;
     rf_tracker_s::Slot &slot = t->slots[t->next_slot++ % t->slots.size()];
@@ -2156,14 +1981,11 @@ static void track_issue(rf_tracker t, const int *videos, int n, const rf_det *de
     CK(launch_track_update(ta, videos, scales, n, s));
     CK(cudaEventRecord(t->chain, s));
     if (a) {
-        // the due faces are already in frame pixels: scale 1, as the tiled paths crop their merged records
-        std::vector<AlignYuvImage> orig(n);
-        for (int i = 0; i < n; i++) orig[i] = AlignYuvImage{planes[i], widths[i], heights[i], 1.f, 0};
         PostBuffers view{};
         view.out_dets = slot.due;
         view.out_counts = slot.due_counts;
         view.max_faces = h->cfg.max_faces;
-        CK(launch_align_faces_yuv(*a, orig.data(), view, h->num_sms, s));
+        CK(launch_align_faces(*a, table, view, h->num_sms, s));
     }
     CK(cudaEventRecord(slot.free, s));
     if (dev_tracks) *dev_tracks = slot.tracks;
@@ -2181,7 +2003,7 @@ int rf_track_update(rf_tracker t, const int *videos, int n, const rf_det *dev_de
     if (n == 0) return RF_OK;
     try {
         CK(cudaSetDevice(h->device));
-        track_issue(t, videos, n, dev_dets, dev_counts, scales, (cudaStream_t)rf_last_stream(h), nullptr, nullptr, nullptr, nullptr, dev_tracks,
+        track_issue(t, videos, n, dev_dets, dev_counts, scales, (cudaStream_t)rf_last_stream(h), nullptr, nullptr, dev_tracks,
                     dev_track_counts);
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
@@ -2195,25 +2017,24 @@ int rf_detect_yuv_track_device(rf_handle h, rf_tracker t, const rf_yuv_frame *fr
     if (!t || t->h != h) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker is NULL or belongs to another handle", who));
     int rc = check_track_args(t, who, videos, n, nullptr);
     if (rc) return rc;
-    if ((rc = check_frames(h, who, frames, n, matrix))) return rc;
+    const YuvFrames src{frames, matrix, nullptr, false};
+    if ((rc = src.check(h, who, n))) return rc;
     AlignArgs a;
-    if (align && (rc = align_setup(h, who, align, a))) return rc;
-    if (align && n > 0 && !dev_crops) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: align without dev_crops", who));
+    if (align && (rc = check_align(h, who, align, n, dev_crops, 0, a))) return rc;
     if (n == 0) return RF_OK;
     std::vector<float> scales(n);
     const rf_det *dets = nullptr;
     const int32_t *counts = nullptr;
-    if ((rc = yuv_device_impl(h, who, frames, nullptr, n, matrix, thr, nms, nullptr, nullptr, nullptr, &dets, &counts, scales.data()))) return rc;
+    if ((rc = yuv_device_impl(h, who, src, n, thr, nms, nullptr, nullptr, nullptr, &dets, &counts, scales.data()))) return rc;
     if (dev_dets) *dev_dets = dets;
     if (dev_counts) *dev_counts = counts;
     if (out_scales) std::copy(scales.begin(), scales.end(), out_scales);
     try {
-        std::vector<YuvPlanes> planes(n);
-        std::vector<int> widths(n), heights(n);
-        for (int i = 0; i < n; i++) { planes[i] = planes_of(frames[i], matrix); widths[i] = frames[i].width; heights[i] = frames[i].height; }
+        // the due faces are already in frame pixels: scale 1, as the tiled paths crop their merged records
+        std::vector<AlignImageT<YuvPlanes>> table(n);
+        for (int i = 0; i < n; i++) table[i] = AlignImageT<YuvPlanes>{src.in_place(i), src.width(i), src.height(i), 1.f, 0};
         if (align) { a.n = n; a.crops = dev_crops; a.mats = dev_mats; }
-        track_issue(t, videos, n, dets, counts, scales.data(), h->last_stream, align ? &a : nullptr, planes.data(), widths.data(), heights.data(),
-                    dev_tracks, dev_track_counts);
+        track_issue(t, videos, n, dets, counts, scales.data(), h->last_stream, align ? &a : nullptr, table.data(), dev_tracks, dev_track_counts);
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }

@@ -169,15 +169,13 @@ struct rf_handle_s {
     std::vector<TiledSlot> tiled_slots;
     unsigned next_tiled_slot = 0;
     uint8_t *d_raw = nullptr;         // one raw caller image (max_image) for the letterbox kernel
-    uint8_t *h_raw = nullptr;         // pinned, TWO buffers of raw_bytes: staging of pageable caller images (upload_raw)
+    uint8_t *h_raw = nullptr;         // pinned, TWO buffers of raw_bytes: staging of pageable caller images (upload_plane)
     size_t raw_bytes = 0;
     int raw_slots = 1;                // raw device buffers (one per batch element, capped)
     cudaEvent_t raw_ev[2] = {nullptr, nullptr};   // H2D out of staging buffer i has completed
     unsigned raw_seq = 0;
     std::unique_ptr<HostCopyPool> copy_pool;      // row-band parallel host copy into the staging buffers (lazily created)
-    // rf_detect_align_batch (lazily allocated): where each image's original pixels are resident, the crops (grown on
-    // demand) and the matrices [max_batch][max_faces][6]
-    AlignImage *d_align_images = nullptr, *h_align_images = nullptr;
+    // the blocking align paths (lazily allocated): the crops (grown on demand) and the matrices [max_batch][max_faces][6]
     void *d_align_crops = nullptr;
     size_t align_crops_bytes = 0;
     double *d_align_mats = nullptr;

@@ -54,22 +54,19 @@ __device__ __forceinline__ Tap tap_of(int d, int sn, double scale) {
 // thread = 4 consecutive output pixels = 12 bytes = three aligned 32-bit stores (net_w is a multiple of 32, so rows start 4-byte
 // aligned).  Per image (LbItemT): the source, dst = net_h x net_w x 3, the source size, the size of the resized image inside
 // the output (top-left, the rest is 0), the source pixels per output pixel.
-template <typename Src> constexpr int lb_limit() { return std::is_same<Src, const uint8_t *>::value ? LB_MAX_IMAGES : LB_MAX_FRAMES; }
+template <typename Src> constexpr int lb_limit() { return std::is_same<Src, BgrRows>::value ? LB_MAX_IMAGES : LB_MAX_FRAMES; }
 template <typename Src>
 struct LbBatch { LbItemT<Src> img[lb_limit<Src>()]; };
-static_assert(sizeof(LbBatch<const uint8_t *>) + 8 <= 4096 && sizeof(LbBatch<YuvPlanes>) + 8 <= 4096 && sizeof(LbBatch<BgrRows>) + 8 <= 4096,
+static_assert(sizeof(LbItemT<BgrRows>) == 56, "64 BGR items per launch rely on the 56-byte item");
+static_assert(sizeof(LbBatch<BgrRows>) + 8 <= 4096 && sizeof(LbBatch<YuvPlanes>) + 8 <= 4096,
               "letter-box chunk exceeds the classic 4 KB kernel parameter space");
 
-// BGR of source pixel (x, y): packed or pitched u8 BGR rows, or a YUV 4:2:0 frame converted on the fly
-__device__ __forceinline__ void src_pixel(const uint8_t *src, int sw, int x, int y, int v[3]) {
-    const uint8_t *p = src + ((size_t)y * sw + x) * 3;
-    v[0] = p[0]; v[1] = p[1]; v[2] = p[2];
-}
-__device__ __forceinline__ void src_pixel(const BgrRows &src, int, int x, int y, int v[3]) {
+// BGR of stored pixel (x, y): u8 BGR rows, or a YUV 4:2:0 frame converted on the fly
+__device__ __forceinline__ void src_pixel(const BgrRows &src, int x, int y, int v[3]) {
     const uint8_t *p = src.p + (size_t)y * src.pitch + (size_t)x * 3;
     v[0] = p[0]; v[1] = p[1]; v[2] = p[2];
 }
-__device__ __forceinline__ void src_pixel(const YuvPlanes &src, int, int x, int y, int v[3]) { yuv_pixel(src, x, y, v); }
+__device__ __forceinline__ void src_pixel(const YuvPlanes &src, int x, int y, int v[3]) { yuv_pixel(src, x, y, v); }
 
 // f9: the orientation touches integer tap addresses only.  Every tap position, weight and rounding below is computed in the
 // DISPLAYED frame (sw x sh), a displayed column / row is then reflected by the item's LB_FLIP_X / LB_FLIP_Y bit, and the transposed
@@ -78,8 +75,8 @@ template <typename Src> __device__ __forceinline__ int col_of(const LbItemT<Src>
 template <typename Src> __device__ __forceinline__ int row_of(const LbItemT<Src> &im, int y) { return (im.flip & LB_FLIP_Y) ? im.sh - 1 - y : y; }
 template <bool T, typename Src>
 __device__ __forceinline__ void stored_pixel(const LbItemT<Src> &im, int x, int y, int v[3]) {
-    if (T) src_pixel(im.src, im.sh, y, x, v);     // packed rows of the stored image are sh (its width) pixels long
-    else src_pixel(im.src, im.sw, x, y, v);
+    if (T) src_pixel(im.src, y, x, v);
+    else src_pixel(im.src, x, y, v);
 }
 
 // NPP's NPPI_INTER_SUPER as measured against nppiResizeSqrPixel_8u_C3R (tools/npp_dump.py, oracle/npp_oracle.cu):
@@ -376,25 +373,11 @@ cudaError_t launch_letterbox_batch(const LbItemT<Src> *items, int n, int net_w, 
     return cudaSuccess;
 }
 
-template float letterbox_fill<const uint8_t *>(LbItem &, const uint8_t *, int, int, uint8_t *, int, int, int, int);
+template float letterbox_fill<BgrRows>(LbItem &, BgrRows, int, int, uint8_t *, int, int, int, int);
 template float letterbox_fill<YuvPlanes>(LbYuvItem &, YuvPlanes, int, int, uint8_t *, int, int, int, int);
-template cudaError_t launch_letterbox_batch<const uint8_t *>(const LbItem *, int, int, int, cudaStream_t);
+template cudaError_t launch_letterbox_batch<BgrRows>(const LbItem *, int, int, int, cudaStream_t);
 template cudaError_t launch_letterbox_batch<YuvPlanes>(const LbYuvItem *, int, int, int, cudaStream_t);
-template void tile_fill<const uint8_t *>(LbItem &, const uint8_t *, int, int, uint8_t *, int, int, const rf_tile &);
+template void tile_fill<BgrRows>(LbItem &, BgrRows, int, int, uint8_t *, int, int, const rf_tile &);
 template void tile_fill<YuvPlanes>(LbYuvItem &, YuvPlanes, int, int, uint8_t *, int, int, const rf_tile &);
-template cudaError_t launch_letterbox_batch<BgrRows>(const LbRowsItem *, int, int, int, cudaStream_t);
-template void tile_fill<BgrRows>(LbRowsItem &, BgrRows, int, int, uint8_t *, int, int, const rf_tile &);
-
-void launch_letterbox(const uint8_t *src, int w, int h, uint8_t *dst, int net_w, int net_h, cudaStream_t s) {
-    launch_letterbox_view(src, w, h, dst, net_w, net_h, net_w, net_h, 0, s);
-}
-
-float launch_letterbox_view(const uint8_t *src, int w, int h, uint8_t *dst, int net_w, int net_h, int box_w, int box_h, int flip,
-                            cudaStream_t s) {
-    LbItem it;
-    const float sc = letterbox_fill(it, src, w, h, dst, box_w, box_h, flip, 0);
-    launch_letterbox_batch(&it, 1, net_w, net_h, s);
-    return sc;
-}
 
 }  // namespace rf

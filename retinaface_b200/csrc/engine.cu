@@ -100,13 +100,13 @@ void place_tensors(rf_handle h, bool keep_all) {
 // arena.  `init`: also set the kernels' launch attributes up on the current device (rf_plan_describe needs no GPU).
 void make_plan(rf_handle h, bool init) {
     const rf_config &cfg = h->cfg;
-    h->use_tc = cfg.precision == RF_PREC_INT8 || (cfg.precision == RF_PREC_FP16 && !(cfg.flags & RF_FLAG_NO_TENSORCORE));
+    const bool simt = cfg.precision == RF_PREC_FP32 || (cfg.precision == RF_PREC_FP16 && (cfg.flags & RF_FLAG_NO_TENSORCORE));
     h->on_device = init;
-    if (init && h->use_tc) CK(tc_init());
+    if (init && !simt) CK(tc_init());
     if (cfg.precision == RF_PREC_INT8) { if (init) CK(tc_init_i8()); build_plan_i8(h); }
     else if (cfg.precision == RF_PREC_FP32) build_plan<float>(h);
-    else if (h->use_tc && !(cfg.flags & RF_FLAG_LEGACY_TC)) { if (init) CK(tile_init()); build_plan_tiles(h); }
-    else build_plan<__half>(h);
+    else if (simt) build_plan<__half>(h);
+    else { if (init) CK(tile_init()); build_plan_tiles(h); }
     link_steps(h);
     place_tensors(h, false);
 }
@@ -1075,7 +1075,7 @@ static void detect_tiled_impl(rf_handle h, const Source &source, int n, const st
     // the final NMS over each image's candidates from all its tiles and levels reads its threshold from home's parameters
     if (home.param_seq && home.param_seq % Ctx::kParamSlots == 0) CK(cudaStreamSynchronize(home.stream));
     set_params(h, home, thr, nms);
-    launch_nms(n, home.d_params, dst, home.stream);
+    CK(launch_nms(n, home.d_params, dst, home.stream));
     CK(cudaGetLastError());
 }
 
@@ -1508,7 +1508,7 @@ static int views_impl(rf_handle h, const char *who, const uint8_t *bgr, int widt
         set_params(h, c, thr, nms);
         forward_graph(h, c, nviews);
         CK(launch_merge(c.pb, ms.data(), nviews, Wn, Hn, h->pb_merge, c.stream));
-        launch_nms(1, c.d_params, h->pb_merge, c.stream);
+        CK(launch_nms(1, c.d_params, h->pb_merge, c.stream));
         CK(cudaMemcpyAsync(h->h_counts, h->pb_merge.out_counts, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
         CK(cudaMemcpyAsync(h->h_dets, h->pb_merge.out_dets, sizeof(rf_det) * (size_t)mf, cudaMemcpyDeviceToHost, c.stream));
         CK(cudaStreamSynchronize(c.stream));
@@ -1576,9 +1576,9 @@ int rf_postprocess(rf_handle h, const float *const heads[9], int n, float thr, f
         for (int i = 0; i < 9; i++)
             CK(cudaMemcpyAsync(h->d_blobs[i], heads[i], sizeof(float) * h->blob_elems[i] * n, cudaMemcpyHostToDevice, c.stream));
         set_params(h, c, thr, nms);
-        launch_blob_decode(h->d_blobs, h->lv, n, h->cfg.net_w, h->cfg.net_h, c.d_params, c.pb, c.stream);
+        CK(launch_blob_decode(h->d_blobs, h->lv, n, h->cfg.net_w, h->cfg.net_h, c.d_params, c.pb, c.stream));
         if (out_ncand) CK(cudaMemcpyAsync(h->h_counts + h->cfg.max_batch, c.pb.cand_count, sizeof(int) * n, cudaMemcpyDeviceToHost, c.stream));
-        launch_nms(n, c.d_params, c.pb, c.stream);
+        CK(launch_nms(n, c.d_params, c.pb, c.stream));
         CK(cudaGetLastError());
         fetch_results(h, c, n, out_faces, out_counts, out_idx);
         if (out_ncand) for (int i = 0; i < n; i++) out_ncand[i] = h->h_counts[h->cfg.max_batch + i];

@@ -1,6 +1,8 @@
 // engine_internal.cuh -- what the translation units behind include/rf_b200.h share: the handle, the step / tensor records,
 // the plan builder, and the functions each unit exports to the others.
-//   plan_fp.cu   FP32 / FP16 layer plan (build_plan<T>), tensor-core launch helpers, tile geometry
+//   plan_net.cu  the walk of the network every layer plan is built from, and the leaf helpers the plans share
+//   plan_fp.cu   SIMT layer plans (FP32, FP16 without tensor cores), FP16 tensor-core per-layer operations and launch helpers
+//   plan_tile.cu FP16 tensor-core layer plan: tile chains, and the per-layer operations where a chain is off or does not fit
 //   plan_i8.cu   INT8 layer plan (build_plan_i8)
 //   engine.cu    tensor placement, CUDA-graph executor, the C-ABI entry points
 #pragma once
@@ -152,7 +154,6 @@ struct rf_handle_s {
     __half *d_weights_h = nullptr;
     std::vector<int8_t> wstage_q;  // INT8 tensor-core weight images (tc_conv_i8.cuh)
     int8_t *d_weights_q = nullptr;
-    bool use_tc = false;
 
     // io
     uint8_t *d_input = nullptr;       // [max_batch][H][W][3] u8 BGR
@@ -251,15 +252,72 @@ struct Builder {
     void step(Step s) { h->steps.push_back(std::move(s)); }
 };
 
+// ---- layer plans: one walk of the network (plan_net.cu) calls one set of operations per plan --------------------------------
+// A destination of a convolution's output channels: n channels (the first destination; the second takes the rest) at channel
+// `off` of rows of `ld` channels of tensor t (t < 0: none).
+struct ConvOut { int t = -1, ld = 0, off = 0, n = 0, relu = 0; };
+// One convolution step: convolutions sharing the input, concatenated along N.
+struct ConvNode {
+    std::string name;                       // step name without the plan's prefix
+    std::vector<const FoldedConv *> cs;
+    int in = -1, h = 0, w = 0;              // input tensor and its map size
+    ConvOut out[2];                         // out[1].t < 0: one destination
+    int lane = 0;
+    int up = -1, up_which = 0;              // up >= 0: the FPN merge in + deconv(up, up_w[up_which]) fused into the staging ...
+    std::string sum;                        // ... the name of that never materialised sum (its INT8 scale)
+};
+// Depthwise i + pointwise i+1 on an h x w input; the op creates the output tensor `out` (and, where it stores it, `mid`).
+struct PairNode { int i; const FoldedConv *dw, *pw; std::string mid, out; int h, w; };
+struct StemNode { const FoldedConv *conv0; std::string out0; PairNode pair; };   // conv0 -> out0, then pair 1 + 2
+// Backbone segment `id` (0 = A ... 5 = F): pairs, then optionally the lateral 1x1 conv `lat` on the last pair's output, into
+// a new tensor `lat_out` (lat.in and lat.out[0].t are set by the op).
+struct SegNode { std::string chain; int id; std::vector<PairNode> pairs; ConvNode lat; std::string lat_out; };
+struct SegOut { int out, lat; };
+// FPN level `level` (1 = stride 16, 2 = stride 8): lat + upsample(up) -> the tensor `sum`, then aggr 3x3; `fused` is the
+// aggr conv with the merge fused into it, `aggr` the one on the stand-alone sum (aggr.in set by the op).
+struct MergeNode { std::string lv, sum; int level, lat, up, h, w; ConvNode fused, aggr; };
+// SSH level `level` (0 = stride 32) on `in` into the concat tensor `cat`: conv1 + context conv1 (-> ctx1), context conv2 +
+// conv3_1 (-> ctx31), context conv3_2; then the level's predictors (cls, bbox, landmark).
+struct SshNode {
+    std::string lv, ctx1, ctx31;
+    int level, lane, in, h, w, cat;
+    const FoldedConv *conv1, *ctx_conv1, *ctx_conv2, *ctx_conv3_1, *ctx_conv3_2;
+    const FoldedConv *pred[3];
+};
+struct HeadsNode { const FoldedConv *pred[3][3]; };     // [level][cls, bbox, landmark]; inputs: h->feat_tensor
+
+struct PlanOps {
+    Builder B;
+    explicit PlanOps(rf_handle h) : B{h, h->cfg.net_h, h->cfg.net_w} {}
+    virtual ~PlanOps() = default;
+    virtual int stem(const StemNode &n) = 0;                // returns the output of the stem's pair
+    virtual int pair(const PairNode &p, int in) = 0;        // returns the pointwise output
+    virtual void conv(const ConvNode &c) = 0;
+    virtual int merge(const MergeNode &m) = 0;              // stand-alone FPN merge; returns the `sum` tensor
+    virtual bool fuse_merge(const MergeNode &m) = 0;        // this plan's rule: merge fused into the aggr conv
+    virtual void heads(const HeadsNode &n) = 0;             // predictors + decode + NMS of all levels
+    // defaults built from the operations above (plan_net.cu)
+    virtual SegOut segment(const SegNode &s, int in);
+    virtual void merge_aggr(const MergeNode &m);
+    virtual void ssh(const SshNode &n);
+};
+void walk_network(PlanOps &ops);                            // plan_net.cu: the graph, in step order
+// shared leaf helpers (plan_net.cu)
+struct StemPack { std::vector<float> w0, wd, wp; };         // conv0 [27][8] (k = tap*3 + BGR channel), dw1 [9][8], pw2 [8][16]
+StemPack pack_stem(const StemNode &n);
+std::vector<float> pack_dw(const FoldedConv &dw, float scale = 1.f);   // depthwise 3x3 weights [9][C], times scale
+struct DwGeom { int rows, nsplit, Rmax; };
+DwGeom dw_geometry(int C, int N, int IH, int IW, int S, const std::function<bool(int rows, int N, int R)> &fits);
+int dw2d_tile_w(rf_handle h, int C, int oh, int ow, int nsplit);     // 2-D tile width of a pair's kernel; 0: 1-D
+bool aggr_fits_one_wave(rf_handle h, int fh, int fw);
+
 // ---- exported by plan_fp.cu -----------------------------------------------------------------------------------------
 constexpr int TC_SMEM_LIMIT = 200 * 1024;   // dynamic shared memory the tensor-core kernels may opt into (they also hold ~5 KB static)
-struct DwGeom { int rows, nsplit, Rmax; };
 template <typename T>
-void build_plan(rf_handle h);               // T = float (RF_PREC_FP32) | __half (RF_PREC_FP16)
+void build_plan(rf_handle h);               // the SIMT plans: T = float (RF_PREC_FP32) | __half (RF_PREC_FP16, RF_FLAG_NO_TENSORCORE)
 cudaError_t tc_init();
-std::vector<__half> make_stem_blob(const std::vector<float> &w0, const std::vector<float> &b0, const std::vector<float> &wd,
-                                   const std::vector<float> &bd, const std::vector<float> &wp, const std::vector<float> &bp);
-int plan_stem_tc(Builder &B);
+template <typename OutT>
+int plan_stem_fused(Builder &B, const StemNode &n, const char *suffix, float out_scale);   // conv0 + dw1 + pw2 in one kernel
 int resident_ctas(rf_handle h, const void *kern, int threads, size_t smem);
 // Persistent grid over `tiles` tiles: each CTA takes a run of consecutive tiles, the grid is what the device holds at once.
 struct PersistentGrid { int run, grid; };
@@ -267,15 +325,15 @@ inline PersistentGrid persistent_grid(int tiles, int resident) {
     const int run = std::max(1, (tiles + resident - 1) / std::max(resident, 1));
     return {run, (tiles + run - 1) / run};
 }
-int plan_pair_legacy(Builder &B, int i, int tin, int ih, int iw);
-void plan_conv_legacy(Builder &B, const std::string &sname, std::vector<const FoldedConv *> cs, int tin, int ih, int iw, int t0, int ld0,
-                      int off0, int n0, int relu0, int t1, int ld1, int off1, int relu1, int lane = 0, int tup = -1, int up_which = 0);
-int plan_fpn_merge_h2(Builder &B, const std::string &name, int tlat, int tup, int fh, int fw, int which);
+// the FP16 tensor-core operations (per layer)
+int plan_pair_tc(Builder &B, const PairNode &p, int in);
+void plan_conv_tc(Builder &B, const ConvNode &c);
+int plan_fpn_merge_h2(Builder &B, const MergeNode &m);
 template <typename T>
-void plan_heads_and_nms(Builder &B, bool with_heads, bool with_nms);
+void plan_heads(Builder &B, const HeadsNode &n, const float scale[3], const char *prefix, bool with_heads);
 std::vector<__half> pack_tc_weights(const std::vector<const FoldedConv *> &cs, std::vector<float> &bias, int &Kpad, int nsplit = 1);
 // ---- exported by plan_tile.cu ---------------------------------------------------------------------------------------
-void build_plan_tiles(rf_handle h);         // RF_PREC_FP16 with tensor cores: tile chains (tile_chain.cuh) + round-1 kernels where no chain fits
+void build_plan_tiles(rf_handle h);         // RF_PREC_FP16 with tensor cores: tile chains (tile_chain.cuh) + per-layer kernels where no chain fits
 cudaError_t tile_init();
 std::string describe_chains(rf_handle h);
 // ---- exported by comm.cu --------------------------------------------------------------------------------------------

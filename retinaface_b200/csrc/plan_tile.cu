@@ -1,15 +1,16 @@
-// plan_tile.cu -- the FP16 tensor-core layer plan built from tile chains (tile_chain.cuh): which layers of the reference's graph
-// (model/mnet-deconv-0517.prototxt) run as stages of which persistent kernel, the shared-memory budget of every
-// chain, the packed weights, the TMA tensor maps.  Where a chain does not fit (wide maps, 256-channel layers) the round-1
-// per-layer kernels of plan_fp.cu take over, layer by layer.
+// plan_tile.cu -- the FP16 tensor-core layer plan: which parts of the network walk (plan_net.cu) run as stages of which
+// persistent tile-chain kernel (tile_chain.cuh), the shared-memory budget of every chain, the packed weights, the TMA tensor
+// maps.  Where the mask leaves a part out or a chain does not fit (wide maps, 256-channel layers), the per-layer tensor-core
+// kernels of plan_fp.cu take over, layer by layer.
 //
-//   stem (round-1 k_stem_tc)                          conv0 + dw1 + pw2
+//   stem (per-layer k_stem_tc)                        conv0 + dw1 + pw2
 //   chain A  @ /4    dw3+pw4 (s2) -> dw5+pw6                                        -> relu6
-//   chain B  @ /8    dw7+pw8 (s2) -> dw9+pw10 -> rf_c1_red_conv                      -> relu10 (C1), rf_c1_red_conv_relu
+//   chain B  @ /8    dw7+pw8 (s2) -> dw9+pw10 -> c1 lateral 1x1                      -> relu10 (C1), c1 lateral
 //   chain C  @ /16   dw11+pw12 (s2) -> dw13+pw14 -> dw15+pw16                        -> relu16
-//   chain D  @ /16   dw17+pw18 -> dw19+pw20 -> dw21+pw22 -> rf_c2_lateral            -> relu22 (C2), rf_c2_lateral_relu
-//   /32              dw23+pw24, dw25+pw26, rf_c3_lateral: tile chain when it fits, else round-1 kernels
-//   level kernels    [FPN merge + rf_c*_aggr]  and  [SSH det/context convs + predictors + decode (+ last-block NMS)]
+//   chain D  @ /16   dw17+pw18 -> dw19+pw20 -> dw21+pw22 -> c2 lateral 1x1           -> relu22 (C2), c2 lateral
+//   chain E  @ /32   dw23+pw24
+//   /32              dw25+pw26, c3 lateral 1x1: per-layer kernels
+//   level kernels    [FPN merge + aggr 3x3]  and  [SSH det/context convs + predictors + decode (+ last-block NMS)]
 #include <cstdlib>
 
 #include "engine_internal.cuh"
@@ -133,7 +134,7 @@ int add_conv(TileChain &c, int in_buf, const std::vector<const FoldedConv *> &cs
 }
 
 // the three predictor convs of one level as one N = 32 GEMM with hi + lo FP16 weight pieces (FP32-grade products)
-int add_head(TileChain &c, int in_buf, const FoldedConv *cs[3]) {
+int add_head(TileChain &c, int in_buf, const FoldedConv *const cs[3]) {
     TileChain::LStage s;
     s.type = TCH_HEAD; s.Cin = 64; s.N = 32; s.taps = 1; s.in_buf = in_buf;
     std::vector<__half> hi((size_t)64 * 32), lo((size_t)64 * 32);
@@ -492,224 +493,140 @@ constexpr unsigned TM_LATENCY = TM_SSH | TM_HEAD | TM_NMS;
 constexpr unsigned TM_LATENCY_SMALL = TM_AGGR | TM_SSH | TM_HEAD | TM_NMS;      // max_batch <= 2
 constexpr unsigned TM_THROUGHPUT = 0;
 
-// builds the plan for one mask; false: the predictors could not be fused at all three levels (the caller retries without)
-static bool build_tiles_with_mask(rf_handle h, unsigned mask) {
-    Builder B{h, h->cfg.net_h, h->cfg.net_w};
-    const Model &m = h->model;
-    const int H = h->cfg.net_h, W = h->cfg.net_w, mb = h->cfg.max_batch, mf = h->cfg.max_faces;
-    if (!(mask & TM_SSH)) mask &= ~(TM_HEAD | TM_NMS);
-    if (!(mask & TM_HEAD)) mask &= ~TM_NMS;
-    const double es = 2;
-    auto pair = [&](int i) -> std::pair<const FoldedConv *, const FoldedConv *> {
-        return {&m.conv("mobilenet0_conv" + std::to_string(i) + "_fwd"), &m.conv("mobilenet0_conv" + std::to_string(i + 1) + "_fwd")};
-    };
-    auto relu_name = [](int i) { return "mobilenet0_relu" + std::to_string(i) + "_fwd"; };
-
-    int cur = plan_stem_tc(B);
-    int cur_h = H / 2, cur_w = W / 2, cur_c = 16;
-
-    // a backbone chain over pairs `is` (first may be stride 2) + optionally one trailing 1x1 conv on the last pair's output;
-    // falls back to round-1 kernels pair by pair
-    int lat1 = -1, lat2 = -1, lat3 = -1;
-    auto backbone = [&](const std::string &name, std::vector<int> is, bool enabled, const char *lat_conv, int *lat_out, int lane_lat) {
-        const int S = pair(is[0]).first->stride;
-        const int oh = cur_h / S, ow = cur_w / S;
-        const int Cout = pair(is.back()).second->cout;
-        bool done = false;
-        if (enabled) {
-            auto c = std::make_shared<TileChain>();
-            c->name = "tile_" + name;
-            c->in_tensor = cur; c->in_C = cur_c; c->in_W = cur_w; c->in_H = cur_h; c->in_s2 = S == 2;
-            c->W = ow; c->H = oh;
-            int b = add_buf(*c, cur_c);
-            c->bufs[b].is_input = true;
-            int tout = -1, tlat = -1;
-            for (size_t k = 0; k < is.size(); k++) {
-                auto pr = pair(is[k]);
-                int nb = add_buf(*c, pr.second->cout, k + 1 == is.size());
-                add_dwpw(*c, b, *pr.first, *pr.second, nb);
-                b = nb;
-            }
-            if (lat_conv) {
-                int lb = add_buf(*c, 64, true);
-                add_conv(*c, b, {&m.conv(lat_conv)}, {{lb, 0, 1}});
-            }
-            // tensors are created only once the chain is known to fit (a failed chain leaves no trace in the plan)
-            if (choose_tile(h, *c, mb, mf, forced_th(name))) {
-                tout = B.tensor(relu_name(is.back() + 1), oh, ow, Cout);
-                c->bufs[(int)is.size()].store_tensor = tout;
-                if (lat_conv) { tlat = B.tensor(std::string(lat_conv) + "_relu", oh, ow, 64); c->bufs[(int)is.size() + 1].store_tensor = tlat; }
-                add_chain_step(B, c, 0, ((double)cur_h * cur_w * cur_c + (double)oh * ow * Cout + (lat_conv ? (double)oh * ow * 64 : 0.0)) * es);
-                cur = tout; cur_h = oh; cur_w = ow; cur_c = Cout;
-                if (lat_out) *lat_out = tlat;
-                done = true;
-            }
-        }
-        if (!done) {
-            for (int i : is) {
-                const int S2 = pair(i).first->stride;
-                cur = plan_pair_legacy(B, i, cur, cur_h, cur_w);
-                cur_h /= S2; cur_w /= S2; cur_c = pair(i).second->cout;
-            }
-            if (lat_conv) {
-                int tl = B.tensor(std::string(lat_conv) + "_relu", cur_h, cur_w, 64);
-                plan_conv_legacy(B, std::string(lat_conv) + "_1x1", {&m.conv(lat_conv)}, cur, cur_h, cur_w, tl, 64, 0, 64, 1, -1, 0, 0, 0, lane_lat);
-                if (lat_out) *lat_out = tl;
-            }
-        }
-    };
-    // RF_TILE_SINGLE=1: one chain per depthwise+pointwise pair (no halo recomputation between layers; more, smaller kernels)
-    const bool single = env_int("RF_TILE_SINGLE", 0) != 0;
-    if (single) {
-        backbone("A3", {3}, mask & TM_A, nullptr, nullptr, 0);
-        backbone("A5", {5}, mask & TM_A, nullptr, nullptr, 0);
-        backbone("B7", {7}, mask & TM_B, nullptr, nullptr, 0);
-        backbone("B9", {9}, mask & TM_B, "rf_c1_red_conv", &lat1, 1);
-    } else {
-        backbone("A", {3, 5}, mask & TM_A, nullptr, nullptr, 0);
-        backbone("B", {7, 9}, mask & TM_B, "rf_c1_red_conv", &lat1, 1);
+// The FP16 tensor-core plan for one mask: the backbone segments, FPN merge + aggr and SSH levels run as tile chains where the
+// mask selects them and they fit, as the per-layer kernels of plan_fp.cu otherwise (mask 0: per layer throughout).
+struct TileOps : PlanOps {
+    unsigned mask;
+    const bool single = env_int("RF_TILE_SINGLE", 0) != 0;   // one chain per depthwise+pointwise pair (no halo recomputation)
+    std::shared_ptr<TileChain> ssh_chain[3];                  // the SSH chains: the last-block NMS needs all three
+    bool split_heads = false;                                 // some level's predictors are fused, others not: no plan
+    TileOps(rf_handle h, unsigned m) : PlanOps(h), mask(m) {
+        if (!(mask & TM_SSH)) mask &= ~(TM_HEAD | TM_NMS);
+        if (!(mask & TM_HEAD)) mask &= ~TM_NMS;
     }
-    const int h8 = cur_h, w8 = cur_w;
-    if (single) {
-        backbone("C11", {11}, mask & TM_C, nullptr, nullptr, 0);
-        backbone("C13", {13}, mask & TM_C, nullptr, nullptr, 0);
-        backbone("C15", {15}, mask & TM_C, nullptr, nullptr, 0);
-        backbone("D17", {17}, mask & TM_D, nullptr, nullptr, 0);
-        backbone("D19", {19}, mask & TM_D, nullptr, nullptr, 0);
-        backbone("D21", {21}, mask & TM_D, "rf_c2_lateral", &lat2, 2);
-    } else {
-        backbone("C", {11, 13, 15}, mask & TM_C, nullptr, nullptr, 0);
-        backbone("D", {17, 19, 21}, mask & TM_D, "rf_c2_lateral", &lat2, 2);
-    }
-    const int h16 = cur_h, w16 = cur_w;
-    backbone("E", {23}, mask & TM_E, nullptr, nullptr, 0);
-    backbone("F", {25}, false, "rf_c3_lateral", &lat3, 0);
-    const int h32 = cur_h, w32 = cur_w;
+    int stem(const StemNode &n) override { return plan_stem_fused<__half>(B, n, "", 1.0f); }
+    int pair(const PairNode &p, int in) override { return plan_pair_tc(B, p, in); }
+    void conv(const ConvNode &c) override { plan_conv_tc(B, c); }
+    int merge(const MergeNode &m) override { return plan_fpn_merge_h2(B, m); }
+    bool fuse_merge(const MergeNode &m) override { return aggr_fits_one_wave(B.h, m.h, m.w); }
 
-    // ---- FPN top-down + SSH ---------------------------------------------------------------------------------------------
-    // levels: 0 = stride 32 (lat3, no merge), 1 = stride 16, 2 = stride 8
-    const char *lvn[3] = {"c3", "c2", "c1"};
-    const int fh[3] = {h32, h16, h8}, fw[3] = {w32, w16, w8};
-    int feat_in[3] = {lat3, -1, -1};
-    int lat[3] = {lat3, lat2, lat1};
-    // expected tile count per image (last-block NMS) is known only when all three SSH chains exist
-    std::shared_ptr<TileChain> ssh_chain[3];
-    auto aggr_level = [&](int l) {
-        // merged = lat[l] + upsample(feat_in[l-1]); aggr 3x3 64->64
-        const std::string an = std::string("rf_") + lvn[l] + "_aggr";
-        int taggr = -1;
-        bool done = false;
-        if (mask & TM_AGGR) {
-            auto c = std::make_shared<TileChain>();
-            c->name = std::string("tile_") + lvn[l] + "_merge+aggr";
-            c->in_tensor = lat[l]; c->in_C = 64; c->in_W = fw[l]; c->in_H = fh[l];
-            c->W = fw[l]; c->H = fh[l];
-            c->merge_tensor = feat_in[l - 1];
-            c->merge_w.resize(16 * 64);
-            for (int ch = 0; ch < 64; ch++)
-                for (int t = 0; t < 16; t++) c->merge_w[t * 64 + ch] = __float2half(m.up_w[l - 1][ch * 16 + t]);
-            int bi = add_buf(*c, 64);
-            int bm = add_buf(*c, 64);
-            c->bufs[bm].is_merge = true;
-            int bo = add_buf(*c, 64, true);
-            add_conv(*c, bi, {&m.conv(an)}, {{bo, 0, 1}});
-            if (choose_tile(h, *c, mb, mf, forced_th(std::string("aggr") + lvn[l]))) {
-                taggr = B.tensor(an + "_relu", fh[l], fw[l], 64);
-                c->bufs[bo].store_tensor = taggr;
-                add_chain_step(B, c, 0, ((double)fh[l] * fw[l] * 64 * 2 + (double)(fh[l] / 2) * (fw[l] / 2) * 64) * es);
-                done = true;
+    // a backbone chain over the segment's pairs (the first may be stride 2) + its lateral conv
+    SegOut segment(const SegNode &s, int in) override {
+        if (single && s.pairs.size() > 1) {
+            SegOut o{in, -1};
+            for (size_t k = 0; k < s.pairs.size(); k++) {
+                SegNode one{s.chain + std::to_string(s.pairs[k].i), s.id, {s.pairs[k]}, {}, {}};
+                if (k + 1 == s.pairs.size()) { one.lat = s.lat; one.lat_out = s.lat_out; }
+                o = segment(one, o.out);
             }
+            return o;
         }
-        if (!done) {
-            taggr = B.tensor(an + "_relu", fh[l], fw[l], 64);
-            const long tiles = ((long)mb * (fh[l] + 1) * (fw[l] + 2) + 127) / 128;
-            if (tiles <= h->num_sms) {
-                plan_conv_legacy(B, std::string(lvn[l]) + "_upsample+add+aggr_3x3_64to64", {&m.conv(an)}, lat[l], fh[l], fw[l], taggr, 64, 0, 64, 1, -1, 0, 0, 0, 0,
-                                 feat_in[l - 1], l - 1);
-            } else {
-                int plus = plan_fpn_merge_h2(B, l == 1 ? "_plus0" : "_plus1", lat[l], feat_in[l - 1], fh[l], fw[l], l - 1);
-                plan_conv_legacy(B, std::string(lvn[l]) + "_aggr_3x3_64to64", {&m.conv(an)}, plus, fh[l], fw[l], taggr, 64, 0, 64, 1, -1, 0, 0, 0);
-            }
+        rf_handle h = B.h;
+        const bool enabled = s.id < 5 && (mask & (TM_A << s.id));      // TM_A .. TM_E; the last segment never runs as a chain
+        const PairNode &p0 = s.pairs[0];
+        const int cin = p0.dw->cout, S = p0.dw->stride, oh = p0.h / S, ow = p0.w / S, Cout = s.pairs.back().pw->cout;
+        const bool lat = !s.lat.cs.empty();
+        if (!enabled) return PlanOps::segment(s, in);
+        auto c = std::make_shared<TileChain>();
+        c->name = "tile_" + s.chain;
+        c->in_tensor = in; c->in_C = cin; c->in_W = p0.w; c->in_H = p0.h; c->in_s2 = S == 2;
+        c->W = ow; c->H = oh;
+        int b = add_buf(*c, cin);
+        c->bufs[b].is_input = true;
+        for (size_t k = 0; k < s.pairs.size(); k++) {
+            int nb = add_buf(*c, s.pairs[k].pw->cout, k + 1 == s.pairs.size());
+            add_dwpw(*c, b, *s.pairs[k].dw, *s.pairs[k].pw, nb);
+            b = nb;
         }
-        feat_in[l] = taggr;
-    };
-    auto ssh_level = [&](int l, int lane) {
-        const std::string p = std::string("rf_") + lvn[l] + "_det";
-        const int tin = feat_in[l];
-        int cat = B.tensor(p + "_concat_relu", fh[l], fw[l], 64);
-        h->feat_tensor[l] = cat;
-        bool done = false;
-        if (mask & TM_SSH) {
-            auto c = std::make_shared<TileChain>();
-            c->name = std::string("tile_ssh_") + lvn[l] + ((mask & TM_HEAD) ? "+heads+decode" : "");
-            c->in_tensor = tin; c->in_C = 64; c->in_W = fw[l]; c->in_H = fh[l];
-            c->W = fw[l]; c->H = fh[l];
-            int bi = add_buf(*c, 64);
-            int bcat = add_buf(*c, 64, true, cat);
-            int bctx1 = add_buf(*c, 16);
-            int bctx31 = add_buf(*c, 16);
-            // branches that share an input run as ONE stage over the rows the neediest branch wants: an MMA's time is its A-operand
-            // read from shared memory (128 rows x 32 bytes whatever N), so the other branch's output columns ride along for free
-            add_conv(*c, bi, {&m.conv(p + "_conv1"), &m.conv(p + "_context_conv1")}, {{bcat, 0, 1}, {bctx1, 0, 1}});
-            add_conv(*c, bctx1, {&m.conv(p + "_context_conv2"), &m.conv(p + "_context_conv3_1")}, {{bcat, 32, 1}, {bctx31, 0, 1}});
-            add_conv(*c, bctx31, {&m.conv(p + "_context_conv3_2")}, {{bcat, 48, 1}});
-            if (mask & TM_HEAD) {
-                const int strides[3] = {32, 16, 8};
-                const std::string sn = "_stride" + std::to_string(strides[l]);
-                const FoldedConv *cs[3] = {&m.conv("face_rpn_cls_score" + sn), &m.conv("face_rpn_bbox_pred" + sn), &m.conv("face_rpn_landmark_pred" + sn)};
-                add_head(*c, bcat, cs);
-                c->level = l;
-                c->fused_nms = (mask & TM_NMS) != 0;
-            }
-            if (choose_tile(h, *c, mb, mf, forced_th(std::string("ssh") + lvn[l]))) {
-                add_chain_step(B, c, lane, ((double)fh[l] * fw[l] * 64 * 2) * es);
-                ssh_chain[l] = c;
-                done = true;
-            }
+        if (lat) add_conv(*c, b, s.lat.cs, {{add_buf(*c, 64, true), 0, 1}});
+        // tensors are created only once the chain is known to fit (a failed chain leaves no trace in the plan)
+        if (!choose_tile(h, *c, h->cfg.max_batch, h->cfg.max_faces, forced_th(s.chain))) return PlanOps::segment(s, in);
+        SegOut o{B.tensor(s.pairs.back().out, oh, ow, Cout), -1};
+        c->bufs[(int)s.pairs.size()].store_tensor = o.out;
+        if (lat) { o.lat = B.tensor(s.lat_out, oh, ow, 64); c->bufs[(int)s.pairs.size() + 1].store_tensor = o.lat; }
+        add_chain_step(B, c, 0, ((double)p0.h * p0.w * cin + (double)oh * ow * Cout + (lat ? (double)oh * ow * 64 : 0.0)) * 2);
+        return o;
+    }
+
+    // merged = lat + upsample(up); aggr 3x3 64->64
+    void merge_aggr(const MergeNode &m) override {
+        rf_handle h = B.h;
+        if (!(mask & TM_AGGR)) return PlanOps::merge_aggr(m);
+        auto c = std::make_shared<TileChain>();
+        c->name = "tile_" + m.lv + "_merge+aggr";
+        c->in_tensor = m.lat; c->in_C = 64; c->in_W = m.w; c->in_H = m.h;
+        c->W = m.w; c->H = m.h;
+        c->merge_tensor = m.up;
+        c->merge_w.resize(16 * 64);
+        for (int ch = 0; ch < 64; ch++)
+            for (int t = 0; t < 16; t++) c->merge_w[t * 64 + ch] = __float2half(h->model.up_w[m.level - 1][ch * 16 + t]);
+        int bi = add_buf(*c, 64);
+        int bm = add_buf(*c, 64);
+        c->bufs[bm].is_merge = true;
+        int bo = add_buf(*c, 64, true, m.aggr.out[0].t);
+        add_conv(*c, bi, m.aggr.cs, {{bo, 0, 1}});
+        if (!choose_tile(h, *c, h->cfg.max_batch, h->cfg.max_faces, forced_th("aggr" + m.lv))) return PlanOps::merge_aggr(m);
+        add_chain_step(B, c, 0, ((double)m.h * m.w * 64 * 2 + (double)(m.h / 2) * (m.w / 2) * 64) * 2);
+    }
+
+    void ssh(const SshNode &n) override {
+        rf_handle h = B.h;
+        if (!(mask & TM_SSH)) return PlanOps::ssh(n);
+        auto c = std::make_shared<TileChain>();
+        c->name = "tile_ssh_" + n.lv + ((mask & TM_HEAD) ? "+heads+decode" : "");
+        c->in_tensor = n.in; c->in_C = 64; c->in_W = n.w; c->in_H = n.h;
+        c->W = n.w; c->H = n.h;
+        int bi = add_buf(*c, 64);
+        int bcat = add_buf(*c, 64, true, n.cat);
+        int bctx1 = add_buf(*c, 16);
+        int bctx31 = add_buf(*c, 16);
+        // branches that share an input run as ONE stage over the rows the neediest branch wants: an MMA's time is its A-operand
+        // read from shared memory (128 rows x 32 bytes whatever N), so the other branch's output columns ride along for free
+        add_conv(*c, bi, {n.conv1, n.ctx_conv1}, {{bcat, 0, 1}, {bctx1, 0, 1}});
+        add_conv(*c, bctx1, {n.ctx_conv2, n.ctx_conv3_1}, {{bcat, 32, 1}, {bctx31, 0, 1}});
+        add_conv(*c, bctx31, {n.ctx_conv3_2}, {{bcat, 48, 1}});
+        if (mask & TM_HEAD) {
+            add_head(*c, bcat, n.pred);
+            c->level = n.level;
+            c->fused_nms = (mask & TM_NMS) != 0;
         }
-        if (!done) {
-            int ctx1 = B.tensor(p + "_context_conv1_relu", fh[l], fw[l], 16);
-            int ctx31 = B.tensor(p + "_context_conv3_1_relu", fh[l], fw[l], 16);
-            plan_conv_legacy(B, std::string("ssh_") + lvn[l] + "_conv1+ctx1_3x3_64to48", {&m.conv(p + "_conv1"), &m.conv(p + "_context_conv1")}, tin, fh[l], fw[l], cat, 64, 0, 32,
-                             1, ctx1, 16, 0, 1, lane);
-            plan_conv_legacy(B, std::string("ssh_") + lvn[l] + "_ctx2+ctx3_1_3x3_16to32", {&m.conv(p + "_context_conv2"), &m.conv(p + "_context_conv3_1")}, ctx1, fh[l], fw[l], cat,
-                             64, 32, 16, 1, ctx31, 16, 0, 1, lane);
-            plan_conv_legacy(B, std::string("ssh_") + lvn[l] + "_ctx3_2_3x3_16to16", {&m.conv(p + "_context_conv3_2")}, ctx31, fh[l], fw[l], cat, 64, 48, 16, 1, -1, 0, 0, 0, lane);
+        if (!choose_tile(h, *c, h->cfg.max_batch, h->cfg.max_faces, forced_th("ssh" + n.lv))) return PlanOps::ssh(n);
+        add_chain_step(B, c, n.lane, ((double)n.h * n.w * 64 * 2) * 2);
+        ssh_chain[n.level] = c;
+    }
+
+    void heads(const HeadsNode &n) override {
+        rf_handle h = B.h;
+        const float one[3] = {1.f, 1.f, 1.f};
+        h->tile_mask = mask;
+        if (!(ssh_chain[0] && ssh_chain[1] && ssh_chain[2] && (mask & TM_HEAD))) {
+            // some level's predictors are not fused: none may be (one decode kernel covers all levels)
+            for (auto &c : ssh_chain)
+                if (c && c->level >= 0) split_heads = true;
+            if (!split_heads) plan_heads<__half>(B, n, one, "", true);
+            return;
         }
-    };
-    ssh_level(0, 1);
-    aggr_level(1);
-    ssh_level(1, 2);
-    aggr_level(2);
-    ssh_level(2, 0);
-    const bool all_heads = ssh_chain[0] && ssh_chain[1] && ssh_chain[2] && (mask & TM_HEAD);
-    if (!all_heads) {
-        // some level's predictors are not fused: none may be (one decode kernel covers all levels)
-        for (auto &c : ssh_chain)
-            if (c && c->level >= 0) return false;
-        plan_heads_and_nms<__half>(B, true, true);
-    } else {
         h->head_step = (int)h->steps.size() - 1;          // the stride-8 SSH chain (last step) emits the last candidates
         h->tile_expected = ssh_chain[0]->args.tiles_per_img + ssh_chain[1]->args.tiles_per_img + ssh_chain[2]->args.tiles_per_img;
-        if (!(mask & TM_NMS)) plan_heads_and_nms<__half>(B, false, true);
+        if (!(mask & TM_NMS)) plan_heads<__half>(B, n, one, "", false);
     }
-    h->tile_mask = mask;
-    return true;
-}
+};
 
 void build_plan_tiles(rf_handle h) {
     // the chain plan is meant for one forward at a time AND small batches (tools/mask_sweep.py compares the selections); at
-    // large batches every per-layer kernel fills the GPU
+    // large batches every per-layer kernel fills the GPU.  RF_FLAG_LEGACY_TC: no chains.
     const bool latency_mode = h->cfg.streams == 1 && h->cfg.max_batch <= 16;
     const unsigned dflt = !latency_mode ? TM_THROUGHPUT : (h->cfg.max_batch <= 2 ? TM_LATENCY_SMALL : TM_LATENCY);
-    const unsigned mask = (unsigned)env_int("RF_TILE_MASK", (int)dflt);
+    const unsigned mask = (h->cfg.flags & RF_FLAG_LEGACY_TC) ? 0u : (unsigned)env_int("RF_TILE_MASK", (int)dflt);
     for (unsigned m : {mask, mask & ~(unsigned)(TM_HEAD | TM_NMS)}) {
         // a failed attempt leaves no trace
         h->steps.clear(); h->tensors.clear(); h->tensor_by_name.clear(); h->chains.clear();
         h->wstage.clear(); h->wstage_h.clear(); h->wstage_q.clear();
         h->head_step = h->nms_step = -1; h->tile_expected = 0;
         for (int &f : h->feat_tensor) f = -1;
-        if (build_tiles_with_mask(h, m)) return;
+        TileOps ops(h, m);
+        walk_network(ops);
+        if (!ops.split_heads) return;
     }
     throw PlanFail{RF_ERR_UNSUPPORTED, "no tile-chain plan fits this network size; create the handle with RF_FLAG_LEGACY_TC"};
 }

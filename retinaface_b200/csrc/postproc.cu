@@ -250,7 +250,7 @@ size_t nms_smem_bytes(int max_faces) { return sizeof(int) * (size_t)max_faces; }
 }  // namespace
 
 template <typename T>
-void launch_head_decode(const T *const feat[3], const HeadWeights hw[3], const LevelDesc lv[3], int n,
+cudaError_t launch_head_decode(const T *const feat[3], const HeadWeights hw[3], const LevelDesc lv[3], int n,
                         int net_w, int net_h, const PostParams *params, const PostBuffers &pb,
                         float *const blobs[9], cudaStream_t s, bool fuse_nms) {
     HeadLaunch L;
@@ -267,27 +267,27 @@ void launch_head_decode(const T *const feat[3], const HeadWeights hw[3], const L
     for (int i = 0; i < 9; i++) L.blobs[i] = write ? blobs[i] : nullptr;
     dim3 grid(blk, n);
     const size_t dyn = fuse_nms ? nms_smem_bytes(pb.max_faces) : 0;
-    if (write) launch_k(k_head_decode<T, true>, grid, dim3(128), dyn, s, L, net_w, net_h, params, pb, fuse_nms ? 1 : 0);
-    else launch_k(k_head_decode<T, false>, grid, dim3(128), dyn, s, L, net_w, net_h, params, pb, fuse_nms ? 1 : 0);
+    if (write) return launch_k(k_head_decode<T, true>, grid, dim3(128), dyn, s, L, net_w, net_h, params, pb, fuse_nms ? 1 : 0);
+    return launch_k(k_head_decode<T, false>, grid, dim3(128), dyn, s, L, net_w, net_h, params, pb, fuse_nms ? 1 : 0);
 }
-template void launch_head_decode<float>(const float *const[3], const HeadWeights[3], const LevelDesc[3], int, int, int,
+template cudaError_t launch_head_decode<float>(const float *const[3], const HeadWeights[3], const LevelDesc[3], int, int, int,
                                         const PostParams *, const PostBuffers &, float *const[9], cudaStream_t, bool);
-template void launch_head_decode<__half>(const __half *const[3], const HeadWeights[3], const LevelDesc[3], int, int, int,
+template cudaError_t launch_head_decode<__half>(const __half *const[3], const HeadWeights[3], const LevelDesc[3], int, int, int,
                                          const PostParams *, const PostBuffers &, float *const[9], cudaStream_t, bool);
-template void launch_head_decode<int8_t>(const int8_t *const[3], const HeadWeights[3], const LevelDesc[3], int, int, int,
+template cudaError_t launch_head_decode<int8_t>(const int8_t *const[3], const HeadWeights[3], const LevelDesc[3], int, int, int,
                                          const PostParams *, const PostBuffers &, float *const[9], cudaStream_t, bool);
 
-void launch_blob_decode(const float *const blobs[9], const LevelDesc lv[3], int n, int net_w, int net_h,
+cudaError_t launch_blob_decode(const float *const blobs[9], const LevelDesc lv[3], int n, int net_w, int net_h,
                         const PostParams *params, const PostBuffers &pb, cudaStream_t s) {
     BlobLaunch L;
     for (int i = 0; i < 9; i++) L.blobs[i] = blobs[i];
     for (int l = 0; l < 3; l++) L.lv[l] = lv[l];
     dim3 grid((pb.anchors_per_image + 255) / 256, n);
-    launch_k(k_blob_decode, grid, dim3(256), 0, s, L, net_w, net_h, params, pb);
+    return launch_k(k_blob_decode, grid, dim3(256), 0, s, L, net_w, net_h, params, pb);
 }
 
-void launch_nms(int n, const PostParams *params, const PostBuffers &pb, cudaStream_t s) {
-    launch_k(k_nms, dim3(n), dim3(NMS_THREADS), nms_smem_bytes(pb.max_faces), s, params, pb);
+cudaError_t launch_nms(int n, const PostParams *params, const PostBuffers &pb, cudaStream_t s) {
+    return launch_k(k_nms, dim3(n), dim3(NMS_THREADS), nms_smem_bytes(pb.max_faces), s, params, pb);
 }
 
 MergeSource view_source(int view, int max_faces, float scale, int flip, int img_w) {

@@ -45,16 +45,16 @@ struct HeadWeights {
 // feat[l]: NHWC [n][h][w][64] SSH output (post concat+ReLU) in T.  blobs (optional, may be all
 // NULL): the 9 NCHW float32 head blobs in engine order, for rf_forward_heads.
 template <typename T>
-void launch_head_decode(const T *const feat[3], const HeadWeights hw[3], const LevelDesc lv[3], int n,
+cudaError_t launch_head_decode(const T *const feat[3], const HeadWeights hw[3], const LevelDesc lv[3], int n,
                         int net_w, int net_h, const PostParams *params, const PostBuffers &pb,
                         float *const blobs[9], cudaStream_t s, bool fuse_nms = false);
 
 // Decode from caller-provided head blobs (device, NCHW f32, engine order): rf_postprocess.
-void launch_blob_decode(const float *const blobs[9], const LevelDesc lv[3], int n, int net_w, int net_h,
+cudaError_t launch_blob_decode(const float *const blobs[9], const LevelDesc lv[3], int n, int net_w, int net_h,
                         const PostParams *params, const PostBuffers &pb, cudaStream_t s);
 
 // Sort candidates by (score desc, emission index asc) and run greedy NMS; one CTA per image.
-void launch_nms(int n, const PostParams *params, const PostBuffers &pb, cudaStream_t s);
+cudaError_t launch_nms(int n, const PostParams *params, const PostBuffers &pb, cudaStream_t s);
 
 // Views (SURVEY.md 8f-2) and tiles (f7): gather the kept detections of the images of one batch (src.out_dets / out_counts, network
 // coordinates; batch slot b = source b) into candidate lists in original-image coordinates, one list per destination image.  Per

@@ -1,6 +1,7 @@
 #!/usr/bin/env python
 """Device-timed step time of the FP16 engine for several RF_TILE_MASK selections (development tool): 4 execution contexts
-(throughput mode) and 1 context (single-step latency), batch 8 and 32.  Mask 9999 = RF_FLAG_LEGACY_TC (round-1 kernels only).  One process per configuration."""
+(throughput mode) and 1 context (single-step latency), batch 8 and 32.  Mask 9999 = RF_FLAG_LEGACY_TC, the same plan as mask 0 (per-layer
+kernels only, RF_TILE_MASK ignored).  One process per configuration."""
 import argparse, json, os, subprocess, sys, time
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -12,7 +13,8 @@ def child(mask, batch, streams):
     if 10000 <= mask < 20000:
         os.environ["RF_TILE_SINGLE"] = "1"
         mask -= 10000
-    os.environ["RF_TILE_MASK"] = str(mask)
+    if mask != 9999:
+        os.environ["RF_TILE_MASK"] = str(mask)
     import cv2, torch
     from oracle.inputs import letterbox_bgr_u8
     from retinaface_b200 import RF_PREC_FP16, Engine

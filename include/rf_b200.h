@@ -536,6 +536,78 @@ int  rf_detect_yuv_track_device(rf_handle h, rf_tracker t, const rf_yuv_frame *f
 #define RF_TRACK_DEBUG_DOUBLES 25
 int  rf_tracker_debug_state(rf_tracker t, int video, double *out, int cap);
 
+/* f11 best shots: the best crop of every tracked face, kept on the GPU, and one crop per identity when its track ends -- the view a
+ * recogniser should see, instead of the track's second detection (f10's new-identity crop), which is usually a face entering the
+ * frame: at its edge, small, turned or blurred.
+ *
+ * A BEST-SHOT tracker is created by rf_tracker_create_best and fed only through rf_detect_yuv_track_best_device, which has the frame
+ * pixels.  Tracking is f10's, unchanged: the same rf_track lists, bit for bit.  On every frame where a track is matched or born (its
+ * rf_track.det >= 0 after the frame, TENTATIVE frames included), the call
+ *   1. cuts the u8 BGR crop rf_detect_yuv_track_device would cut for the track's record: M fitted on rf_track.face (frame pixels,
+ *      map-back 1) to the template, cv2.warpAffine(cv2.cvtColor(frame), M) byte for byte;
+ *   2. computes the crop's quality q (below);
+ *   3. keeps the crop, M, the quality terms, the record and the frame number if q is STRICTLY greater than the track's stored best;
+ *      a track's first frame always stores, and on a tie the earlier frame stays.
+ * A track that was ever CONFIRMED EMITS its best shot on the frame it is removed (a LOST track whose lost_frames exceeds max_lost);
+ * a TENTATIVE track that is removed never emits; a shot whose stored q < min_quality is dropped.  A frame's emissions are compacted
+ * in id order.  Within a video, a frame applies its removals (and their emissions) before its births, as f10 orders them, so a
+ * slot freed and reused on one frame emits the old track's shot.  rf_tracker_finish(video) emits the best shot of every live,
+ * ever-confirmed track of the video in id order, with the same filter, then resets the video as rf_tracker_reset does;
+ * rf_tracker_reset on a best-shot tracker discards the stored shots and emits nothing.
+ *
+ * Quality.  Every step FP64, one rounding each, in the order written; landmarks l_k are the record's floats in frame pixels, widened:
+ *   ex = lx1 - lx0, ey = ly1 - ly0, d2 = ex * ex + ey * ey   (d2 == 0 or M all zero: eye, frontal, sharpness, coverage and q are 0)
+ *   eye       = sqrt(d2)
+ *   t         = ((lx2 - (lx0 + lx1) / 2) * ex + (ly2 - (ly0 + ly1) / 2) * ey) / d2     (the nose's offset along the eye axis)
+ *   frontal   = max(0, 1 - 2 * |t|)
+ *   size      = min(1, eye / eye_ref)     eye_ref = the distance of template points 0 and 1 (35.24 px for the ArcFace 112 template)
+ *   INSIDE    a crop pixel whose four cv::warpAffine taps (sx, sy) .. (sx + 1, sy + 1) (the fixed-point tap, after its saturate) all
+ *             lie in the frame
+ *   coverage  = #INSIDE / (crop_w * crop_h)
+ *   g         = (3735 B + 19235 G + 9798 R + 16384) >> 15 per crop pixel   (cv2.cvtColor BGR2GRAY)
+ *   L(x, y)   = g(x-1, y) + g(x+1, y) + g(x, y-1) + g(x, y+1) - 4 g(x, y)    (cv2.Laplacian(g, ksize = 1) in the interior), over
+ *             1 <= x <= crop_w - 2, 1 <= y <= crop_h - 2 where (x, y) and its 4 neighbours are INSIDE: count N, S1 = sum L,
+ *             S2 = sum L^2 in int64
+ *   sharpness = N >= 2 ? (double)(N S2 - S1 S1) / ((double)N * (double)N) : 0      (the Laplacian's variance)
+ *   sharp     = sharpness / (sharpness + sharp_half)
+ *   q         = (((score * frontal) * size) * sharp) * coverage
+ *
+ * Outputs follow f10's rules: records and counts live in the tracker's ring of `streams` slots and stay valid for `streams` further
+ * tracker calls.  *dev_best -> [n][max_tracks] rf_best_shot, frame i's emissions in id order, *dev_best_counts -> [n] int32; emission k
+ * of frame i has its crop at dev_best_crops [i][k] ([n][max_tracks][crop bytes], the caller's device buffer) and, optionally, its M at
+ * dev_best_mats [i][k] ([n][max_tracks][6]).  The bound is exact: the tracks removed on a frame were live.  For rf_tracker_finish
+ * the buffers hold [max_tracks].  Float formats are the u8 crop converted as rf_detect_align_batch_device converts it, bit for bit.
+ * Calls are asynchronous on rf_last_stream() (rf_tracker_finish: context 0's stream), ordered with every other call on the tracker
+ * by its event chain. */
+typedef struct rf_best_config {
+    rf_align_params align;   /* geometry, template, format, mean / std of the EMITTED crops (max_faces must be 0); stored as u8 */
+    float min_quality;       /* in [0, 1]; a shot is emitted only if q >= min_quality */
+    float sharp_half;        /* 0 -> 50; else finite and > 0 */
+} rf_best_config;
+#define RF_BEST_EXIT   0     /* the track was removed */
+#define RF_BEST_FINISH 1     /* rf_tracker_finish */
+typedef struct rf_best_shot {
+    int32_t id, video;
+    int32_t frame;           /* the video's frame number (0: the first since create / reset) the crop was cut from */
+    int32_t end_frame;       /* the frame number it was emitted on (rf_tracker_finish: the video's last frame) */
+    int32_t hits, age, reason, reserved;   /* the track's hits / age when emitted; RF_BEST_* */
+    float quality, score, eye, frontal, sharpness, coverage;   /* q and its terms at `frame`, rounded from double */
+    rf_face face;            /* the track's record on `frame`, frame pixels */
+} rf_best_shot;
+/* A best-shot tracker.  Bad configs: RF_ERR_INVALID_ARG; a store (max_videos x max_tracks u8 crops) above 4 GiB: RF_ERR_CAPACITY. */
+int rf_tracker_create_best(rf_handle h, const rf_track_config *cfg, const rf_best_config *best, rf_tracker *out);
+/* rf_detect_yuv_track_device without new-identity crops, plus the best shots above (dev_best_crops required).  RF_ERR_INVALID_ARG
+ * on a plain tracker; every status before anything is launched.  rf_detect_yuv_track_device and rf_track_update refuse a best-shot
+ * tracker (RF_ERR_INVALID_ARG): frames the store never saw would break "the best of every frame". */
+int rf_detect_yuv_track_best_device(rf_handle h, rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, int matrix,
+                                    float score_threshold, float nms_threshold, void *dev_best_crops, double *dev_best_mats,
+                                    const rf_best_shot **dev_best, const int32_t **dev_best_counts,
+                                    const rf_track **dev_tracks, const int32_t **dev_track_counts,
+                                    const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales);
+/* Ends `video` (see above).  *dev_best -> [max_tracks] rf_best_shot, *dev_best_count -> one int32. */
+int rf_tracker_finish(rf_tracker t, int video, void *dev_best_crops, double *dev_best_mats,
+                      const rf_best_shot **dev_best, const int32_t **dev_best_count);
+
 /* Introspection. */
 int rf_get_net_size(rf_handle h, int *net_w, int *net_h, int *max_batch, int *max_faces);
 int rf_num_anchors(rf_handle h);            /* per image: 8,232 @448x448, 47,040 @1280x896 */

@@ -33,6 +33,7 @@ EXPORTS = [
     "rf_detect_oriented_batch", "rf_detect_yuv_oriented_device", "rf_preprocess_oriented", "rf_preprocess_yuv_oriented",
     "rf_detect_views_oriented", "rf_jpeg_exif_orientation",
     "rf_tracker_create", "rf_tracker_destroy", "rf_tracker_reset", "rf_track_update", "rf_detect_yuv_track_device", "rf_tracker_debug_state",
+    "rf_tracker_create_best", "rf_detect_yuv_track_best_device", "rf_tracker_finish",
 ]
 COMM_BLOB_BYTES = 128
 
@@ -210,6 +211,26 @@ TRACK_DTYPE = np.dtype([(f, "<i4") for f in ("id", "state", "det", "crop_slot", 
                        [(f, "<f4") for f in ("kx1", "ky1", "kx2", "ky2", "vx", "vy")] + [("face", "<f4", (FACE_FLOATS,))])
 
 
+class BestConfig(C.Structure):   # rf_best_config
+    _fields_ = [("align", AlignParams), ("min_quality", C.c_float), ("sharp_half", C.c_float)]
+
+
+def best_config(min_quality: float = 0.0, sharp_half: float = 0.0, **align) -> BestConfig:
+    """rf_best_config: ``align_params`` keywords (crop, template, fmt, mean, std) for the emitted crops; sharp_half 0 -> 50."""
+    return BestConfig(align_params(**align), float(min_quality), float(sharp_half))
+
+
+class BestShot(C.Structure):     # rf_best_shot
+    _fields_ = [(f, C.c_int32) for f in ("id", "video", "frame", "end_frame", "hits", "age", "reason", "reserved")] + \
+               [(f, C.c_float) for f in ("quality", "score", "eye", "frontal", "sharpness", "coverage")] + [("face", Face)]
+
+
+BEST_EXIT, BEST_FINISH = 0, 1                                # RF_BEST_*
+# one rf_best_shot as a numpy record (the layout of BestShot)
+BEST_DTYPE = np.dtype([(f, "<i4") for f in ("id", "video", "frame", "end_frame", "hits", "age", "reason", "reserved")] +
+                      [(f, "<f4") for f in ("quality", "score", "eye", "frontal", "sharpness", "coverage")] + [("face", "<f4", (FACE_FLOATS,))])
+
+
 class RfError(RuntimeError):
     def __init__(self, status: int, msg: str):
         super().__init__(f"librf_b200 status {status}: {msg}")
@@ -339,6 +360,10 @@ def load_library() -> C.CDLL:
                                                C.POINTER(AlignParams), C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
                                                C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_void_p]
     lib.rf_tracker_debug_state.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
+    lib.rf_tracker_create_best.argtypes = [C.c_void_p, C.POINTER(TrackConfig), C.POINTER(BestConfig), C.POINTER(C.c_void_p)]
+    lib.rf_detect_yuv_track_best_device.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(YuvFrame), C.c_void_p, C.c_int, C.c_int, C.c_float,
+                                                    C.c_float, C.c_void_p, C.c_void_p] + [C.POINTER(C.c_void_p)] * 6 + [C.c_void_p]
+    lib.rf_tracker_finish.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
     _lib = lib
     return lib
 
@@ -995,9 +1020,11 @@ class Engine:
 
     # -- f10 face tracking across video frames ---------------------------------------------------------------------------------
     def tracker(self, max_videos: int = 1, max_tracks: int = 0, high_thresh: float = 0.0, new_thresh: float = 0.0, iou_high: float = 0.0,
-                iou_low: float = 0.0, iou_tentative: float = 0.0, max_lost: int = 0) -> "Tracker":
-        """rf_tracker_create: a tracker of max_videos independent sequences on this engine (0 -> the defaults of rf_track_config)."""
-        return Tracker(self, TrackConfig(max_videos, max_tracks, high_thresh, new_thresh, iou_high, iou_low, iou_tentative, max_lost))
+                iou_low: float = 0.0, iou_tentative: float = 0.0, max_lost: int = 0, best: Optional[dict] = None) -> "Tracker":
+        """rf_tracker_create: a tracker of max_videos independent sequences on this engine (0 -> the defaults of rf_track_config).
+        best (``best_config`` keywords): a best-shot tracker (rf_tracker_create_best), fed through ``Tracker.detect_yuv_best_device``."""
+        return Tracker(self, TrackConfig(max_videos, max_tracks, high_thresh, new_thresh, iou_high, iou_low, iou_tentative, max_lost),
+                       best_config(**best) if best is not None else None)
 
     def calibrate_int8(self, images: np.ndarray, out_table: str):
         """INT8 entropy calibration on an RF_PREC_FP32 engine; writes a TensorRT-format table."""
@@ -1040,11 +1067,15 @@ class _DevArray:
 class Tracker:
     """One rf_tracker of an Engine: per-video face tracks with stable ids, updated on the GPU.  Close it before its engine."""
 
-    def __init__(self, engine: Engine, cfg: TrackConfig):
+    def __init__(self, engine: Engine, cfg: TrackConfig, best: Optional[BestConfig] = None):
         self.engine, self.lib = engine, engine.lib
         t = C.c_void_p()
-        engine._check(self.lib.rf_tracker_create(engine.h, C.byref(cfg), C.byref(t)))
+        if best is None:
+            engine._check(self.lib.rf_tracker_create(engine.h, C.byref(cfg), C.byref(t)))
+        else:
+            engine._check(self.lib.rf_tracker_create_best(engine.h, C.byref(cfg), C.byref(best), C.byref(t)))
         self.t = t
+        self.best = best
         self.max_videos = cfg.max_videos
         self.max_tracks = cfg.max_tracks or 64
 
@@ -1091,6 +1122,36 @@ class Tracker:
                                                                C.byref(p) if p is not None else None, dev_crops_ptr, dev_mats_ptr, C.byref(tp),
                                                                C.byref(tc), C.byref(d), C.byref(c), scales.ctypes.data))
         return int(tp.value or 0), int(tc.value or 0), int(d.value or 0), int(c.value or 0), scales[:n].copy()
+
+    def detect_yuv_best_device(self, frames, videos: Sequence[int], thr: float, nms_thr: float, dev_best_crops_ptr: int,
+                               dev_best_mats_ptr: Optional[int] = None, layout: str = "nv12", matrix="bt601"):
+        """rf_detect_yuv_track_best_device on a best-shot tracker: detect, track, and keep every track's best crop; the shots emitted
+        on frame i go to dev_best_crops_ptr [n][max_tracks] (and M to dev_best_mats_ptr [n][max_tracks][6]).  Returns (best_ptr,
+        best_counts_ptr, tracks_ptr, track_counts_ptr, dets_ptr, counts_ptr, scales)."""
+        n = len(frames)
+        arr = self.engine._frames(frames, layout, True)
+        scales = np.zeros(max(n, 1), dtype=np.float32)
+        bp, bc, tp, tc, d, c = (C.c_void_p() for _ in range(6))
+        self.engine._check(self.lib.rf_detect_yuv_track_best_device(self.engine.h, self.t, arr, self._ints(videos, n), n, _matrix(matrix), thr,
+                                                                    nms_thr, dev_best_crops_ptr, dev_best_mats_ptr, C.byref(bp), C.byref(bc),
+                                                                    C.byref(tp), C.byref(tc), C.byref(d), C.byref(c), scales.ctypes.data))
+        return (int(bp.value or 0), int(bc.value or 0), int(tp.value or 0), int(tc.value or 0), int(d.value or 0), int(c.value or 0),
+                scales[:n].copy())
+
+    def finish(self, video: int, dev_best_crops_ptr: int, dev_best_mats_ptr: Optional[int] = None):
+        """rf_tracker_finish: emit the best shot of every live, ever-confirmed track of `video` (crops at dev_best_crops_ptr
+        [max_tracks]), then restart the video.  Returns (best_ptr, count_ptr); read them with ``read_best(..., 1)``."""
+        bp, bc = C.c_void_p(), C.c_void_p()
+        self.engine._check(self.lib.rf_tracker_finish(self.t, int(video), dev_best_crops_ptr, dev_best_mats_ptr, C.byref(bp), C.byref(bc)))
+        return int(bp.value or 0), int(bc.value or 0)
+
+    def read_best(self, best_ptr: int, counts_ptr: int, n: int) -> List[np.ndarray]:
+        """The emitted shots of n frames (BEST_DTYPE records, id order), copied to the host after the last stream."""
+        import torch
+        self.engine._check(self.lib.rf_synchronize(self.engine.h))
+        raw = torch.as_tensor(_DevArray(best_ptr, (n, self.max_tracks * BEST_DTYPE.itemsize), "|u1"), device="cuda").cpu().numpy()
+        counts = torch.as_tensor(_DevArray(counts_ptr, (n,), "<i4"), device="cuda").cpu().numpy()
+        return [raw[i].view(BEST_DTYPE)[:counts[i]].copy() for i in range(n)]
 
     def reset(self, video: int = -1):
         """rf_tracker_reset: restart one video (ids from 1), or all with -1; ordered after every issued update."""

@@ -9,6 +9,7 @@
 #include "engine_internal.cuh"
 #include "calibrate.cuh"
 #include "preprocess.cuh"
+#include "best.cuh"
 #include "track.cuh"
 
 namespace rf_eng {
@@ -1855,6 +1856,12 @@ struct rf_tracker_s {
     std::vector<Slot> slots;
     unsigned next_slot = 0;
     cudaEvent_t chain = nullptr;
+    // f11 best shots (best.cuh); `best` false: a plain tracker, none of these allocated.  The chain orders every best-shot kernel
+    // of every call, so one set of per-call tables serves them all; only the emitted records live in the ring.
+    bool best = false;
+    BestArgs ba{};                     // store, per-video counters, per-call tables, formats (per-call pointers set per call)
+    rf_best_shot *d_best = nullptr;    // [slots][max_batch][max_tracks]
+    int *d_best_counts = nullptr;      // [slots][max_batch]
 };
 
 static void tracker_release(rf_tracker t) {
@@ -1865,6 +1872,9 @@ static void tracker_release(rf_tracker t) {
     }
     if (t->chain) cudaEventDestroy(t->chain);
     cudaFree(t->d_videos); cudaFree(t->d_state); cudaFree(t->d_pairs); cudaFree(t->d_order);
+    const BestArgs &b = t->ba;
+    cudaFree(b.store); cudaFree(b.store_crops); cudaFree(b.videos); cudaFree(b.acc); cudaFree((void *)b.seen); cudaFree((void *)b.gone); cudaFree(b.meas);
+    cudaFree(b.scratch); cudaFree(b.commit); cudaFree(b.src); cudaFree(t->d_best); cudaFree(t->d_best_counts);
     delete t;
 }
 
@@ -1933,6 +1943,10 @@ int rf_tracker_reset(rf_tracker t, int video) {
         CK(cudaStreamWaitEvent(s, t->chain, 0));
         CK(cudaMemsetAsync(t->d_videos + v0, 0, sizeof(TrackVideo) * nv, s));
         CK(cudaMemsetAsync(t->d_state + v0 * T, 0, sizeof(TrackState) * nv * T, s));
+        if (t->best) {        // the stored shots are discarded, nothing is emitted
+            CK(cudaMemsetAsync(t->ba.store + v0 * T, 0, sizeof(BestEntry) * nv * T, s));
+            CK(cudaMemsetAsync(t->ba.videos + v0, 0, sizeof(BestVideo) * nv, s));
+        }
         CK(cudaEventRecord(t->chain, s));
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
@@ -1997,6 +2011,7 @@ int rf_track_update(rf_tracker t, const int *videos, int n, const rf_det *dev_de
     static const char *who = "rf_track_update";
     if (!t) return RF_ERR_INVALID_ARG;
     rf_handle h = t->h;
+    if (t->best) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a best-shot tracker takes frames only through rf_detect_yuv_track_best_device", who));
     int rc = check_track_args(t, who, videos, n, scales);
     if (rc) return rc;
     if (n > 0 && (!dev_dets || !dev_counts)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL records or counts", who));
@@ -2015,6 +2030,7 @@ int rf_detect_yuv_track_device(rf_handle h, rf_tracker t, const rf_yuv_frame *fr
     static const char *who = "rf_detect_yuv_track_device";
     if (!h) return RF_ERR_INVALID_ARG;
     if (!t || t->h != h) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker is NULL or belongs to another handle", who));
+    if (t->best) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a best-shot tracker takes frames only through rf_detect_yuv_track_best_device", who));
     int rc = check_track_args(t, who, videos, n, nullptr);
     if (rc) return rc;
     const YuvFrames src{frames, matrix, nullptr, false};
@@ -2035,6 +2051,177 @@ int rf_detect_yuv_track_device(rf_handle h, rf_tracker t, const rf_yuv_frame *fr
         for (int i = 0; i < n; i++) table[i] = AlignImageT<YuvPlanes>{src.in_place(i), src.width(i), src.height(i), 1.f, 0};
         if (align) { a.n = n; a.crops = dev_crops; a.mats = dev_mats; }
         track_issue(t, videos, n, dets, counts, scales.data(), h->last_stream, align ? &a : nullptr, table.data(), dev_tracks, dev_track_counts);
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
+}
+
+// ---- f11 best shots (best.cuh) ---------------------------------------------------------------------------------------------------
+int rf_tracker_create_best(rf_handle h, const rf_track_config *cfg, const rf_best_config *best, rf_tracker *out) {
+    static const char *who = "rf_tracker_create_best";
+    if (!h) return RF_ERR_INVALID_ARG;
+    if (!cfg || !best || !out) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL config or output", who));
+    *out = nullptr;
+    AlignArgs o;
+    int rc = align_setup(h, who, &best->align, o);
+    if (rc) return rc;
+    if (best->align.max_faces != 0) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: align.max_faces %d, must be 0", who, best->align.max_faces));
+    if (!(best->min_quality >= 0.f && best->min_quality <= 1.f))
+        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: min_quality %g, must be in [0, 1]", who, (double)best->min_quality));
+    const float half = best->sharp_half == 0.f ? 50.f : best->sharp_half;
+    if (!(std::isfinite(half) && half > 0.f)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: sharp_half %g, must be finite and positive", who, (double)half));
+    const size_t u8_bytes = align_crop_bytes(o.crop_w, o.crop_h, RF_CROP_BGR_U8);
+    const int T = cfg->max_tracks == 0 ? 64 : cfg->max_tracks;
+    if (cfg->max_videos >= 1 && cfg->max_videos <= 4096 && T >= 1 && T <= TRACK_MAX_TRACKS && (size_t)cfg->max_videos * T * u8_bytes > ((size_t)4 << 30))
+        return fail(h, RF_ERR_CAPACITY, fmt("%s: a store of %d videos x %d tracks x %zu bytes exceeds 4 GiB", who, cfg->max_videos, T, u8_bytes));
+    rf_tracker t = nullptr;
+    if ((rc = rf_tracker_create(h, cfg, &t))) return rc;
+    std::unique_ptr<rf_tracker_s, void (*)(rf_tracker)> g(t, tracker_release);
+    t->best = true;
+    BestArgs &b = t->ba;
+    b.out = o;
+    b.u8 = o;
+    b.u8.format = RF_CROP_BGR_U8;
+    b.u8.crop_bytes = u8_bytes;
+    b.max_tracks = t->cfg.max_tracks;
+    b.max_faces = h->cfg.max_faces;
+    b.min_quality = (double)best->min_quality;
+    b.sharp_half = (double)half;
+    b.num_sms = h->num_sms;
+    try {
+        const size_t V = t->cfg.max_videos, TT = t->cfg.max_tracks, F = h->cfg.max_faces, B = h->cfg.max_batch;
+        const size_t M = std::min<size_t>(B, TRACK_MAX_FRAMES), R = t->slots.size();
+        CK(cudaMalloc(&b.store, sizeof(BestEntry) * V * TT));
+        CK(cudaMalloc(&b.store_crops, u8_bytes * V * TT));
+        CK(cudaMalloc(&b.videos, sizeof(BestVideo) * V));
+        TrackSeen *seen = nullptr;
+        TrackGone *gone = nullptr;
+        CK(cudaMalloc(&seen, sizeof(TrackSeen) * M * F));
+        b.seen = seen;
+        CK(cudaMalloc(&gone, sizeof(TrackGone) * M * TT));
+        b.gone = gone;
+        CK(cudaMalloc(&b.meas, sizeof(BestMeasure) * M * F));
+        CK(cudaMalloc(&b.acc, sizeof(BestAccum) * M * F));
+        CK(cudaMemset(b.acc, 0, sizeof(BestAccum) * M * F));
+        CK(cudaMalloc(&b.scratch, u8_bytes * M * F));
+        CK(cudaMalloc(&b.commit, sizeof(int) * M * F));
+        CK(cudaMalloc(&b.src, sizeof(int) * M * TT));
+        CK(cudaMalloc(&t->d_best, sizeof(rf_best_shot) * R * B * TT));
+        CK(cudaMalloc(&t->d_best_counts, sizeof(int) * R * B));
+        CK(cudaMemset(b.store, 0, sizeof(BestEntry) * V * TT));
+        CK(cudaMemset(b.videos, 0, sizeof(BestVideo) * V));
+        CK(cudaDeviceSynchronize());
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    *out = g.release();
+    return RF_OK;
+}
+
+int rf_detect_yuv_track_best_device(rf_handle h, rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, int matrix, float thr,
+                                    float nms, void *dev_best_crops, double *dev_best_mats, const rf_best_shot **dev_best,
+                                    const int32_t **dev_best_counts, const rf_track **dev_tracks, const int32_t **dev_track_counts,
+                                    const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales) {
+    static const char *who = "rf_detect_yuv_track_best_device";
+    if (!h) return RF_ERR_INVALID_ARG;
+    if (!t || t->h != h) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker is NULL or belongs to another handle", who));
+    if (!t->best) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: not a best-shot tracker (rf_tracker_create_best)", who));
+    int rc = check_track_args(t, who, videos, n, nullptr);
+    if (rc) return rc;
+    const YuvFrames src{frames, matrix, nullptr, false};
+    if ((rc = src.check(h, who, n))) return rc;
+    if (n > 0 && !dev_best_crops) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: dev_best_crops is NULL", who));
+    if (n == 0) return RF_OK;
+    std::vector<float> scales(n);
+    const rf_det *dets = nullptr;
+    const int32_t *counts = nullptr;
+    if ((rc = yuv_device_impl(h, who, src, n, thr, nms, nullptr, nullptr, nullptr, &dets, &counts, scales.data()))) return rc;
+    if (dev_dets) *dev_dets = dets;
+    if (dev_counts) *dev_counts = counts;
+    if (out_scales) std::copy(scales.begin(), scales.end(), out_scales);
+    try {
+        cudaStream_t s = h->last_stream;
+        const unsigned ring = t->next_slot++ % t->slots.size();
+        rf_tracker_s::Slot &slot = t->slots[ring];
+        const int T = t->cfg.max_tracks, F = h->cfg.max_faces, B = h->cfg.max_batch;
+        rf_best_shot *best = t->d_best + (size_t)ring * B * T;
+        int *best_counts = t->d_best_counts + (size_t)ring * B;
+        CK(cudaStreamWaitEvent(s, slot.free, 0));
+        CK(cudaStreamWaitEvent(s, t->chain, 0));
+        TrackArgs ta{};
+        ta.p = TrackParams{T, F, t->cfg.max_lost, t->cfg.high_thresh, t->cfg.new_thresh, t->cfg.iou_high, t->cfg.iou_low, t->cfg.iou_tentative};
+        ta.videos = t->d_videos;
+        ta.state = t->d_state;
+        ta.pairs = t->d_pairs;
+        ta.order = t->d_order;
+        ta.seen = const_cast<TrackSeen *>(t->ba.seen);
+        ta.gone = const_cast<TrackGone *>(t->ba.gone);
+        // the call in chunks of TRACK_MAX_FRAMES frames, each tracked then measured, selected, emitted and committed: the per-call
+        // tables hold one chunk
+        for (int i0 = 0; i0 < n; i0 += TRACK_MAX_FRAMES) {
+            const int m = std::min(TRACK_MAX_FRAMES, n - i0);
+            TrackArgs c = ta;
+            c.dets = dets + (size_t)i0 * F;
+            c.counts = counts + i0;
+            c.tracks = slot.tracks + (size_t)i0 * T;
+            c.track_counts = slot.counts + i0;
+            CK(launch_track_update(c, videos + i0, scales.data() + i0, m, s));
+            BestTable bt{};
+            bt.n = m;
+            for (int i = 0; i < m; i++) {
+                const int v = videos[i0 + i];
+                bt.video[i] = v;
+                bt.img[i] = AlignImageT<YuvPlanes>{src.in_place(i0 + i), src.width(i0 + i), src.height(i0 + i), 1.f, 0};
+                bool known = false;
+                for (int k = 0; k < bt.nvideos; k++) known |= bt.cta_video[k] == v;
+                if (!known) bt.cta_video[bt.nvideos++] = v;
+            }
+            BestArgs b = t->ba;
+            b.out.crops = static_cast<uint8_t *>(dev_best_crops) + (size_t)i0 * T * b.out.crop_bytes;
+            b.out.mats = dev_best_mats ? dev_best_mats + (size_t)i0 * T * 6 : nullptr;
+            b.best = best + (size_t)i0 * T;
+            b.best_counts = best_counts + i0;
+            b.counts = counts + i0;
+            CK(launch_best_frames(b, bt, s));
+        }
+        CK(cudaEventRecord(t->chain, s));
+        CK(cudaEventRecord(slot.free, s));
+        if (dev_tracks) *dev_tracks = slot.tracks;
+        if (dev_track_counts) *dev_track_counts = slot.counts;
+        if (dev_best) *dev_best = best;
+        if (dev_best_counts) *dev_best_counts = best_counts;
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
+}
+
+int rf_tracker_finish(rf_tracker t, int video, void *dev_best_crops, double *dev_best_mats, const rf_best_shot **dev_best,
+                      const int32_t **dev_best_count) {
+    static const char *who = "rf_tracker_finish";
+    if (!t) return RF_ERR_INVALID_ARG;
+    rf_handle h = t->h;
+    if (!t->best) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: not a best-shot tracker (rf_tracker_create_best)", who));
+    if (video < 0 || video >= t->cfg.max_videos) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: video %d, must be in [0, %d)", who, video, t->cfg.max_videos));
+    if (!dev_best_crops) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: dev_best_crops is NULL", who));
+    try {
+        CK(cudaSetDevice(h->device));
+        cudaStream_t s = h->ctx[0].stream;
+        const unsigned ring = t->next_slot++ % t->slots.size();
+        rf_tracker_s::Slot &slot = t->slots[ring];
+        const size_t T = t->cfg.max_tracks, B = h->cfg.max_batch;
+        CK(cudaStreamWaitEvent(s, slot.free, 0));
+        CK(cudaStreamWaitEvent(s, t->chain, 0));
+        BestArgs b = t->ba;
+        b.out.crops = dev_best_crops;
+        b.out.mats = dev_best_mats;
+        b.best = t->d_best + ring * B * T;
+        b.best_counts = t->d_best_counts + ring * B;
+        CK(launch_best_finish(b, video, t->d_state + (size_t)video * T, s));
+        // then the video restarts as rf_tracker_reset restarts it
+        CK(cudaMemsetAsync(t->d_videos + video, 0, sizeof(TrackVideo), s));
+        CK(cudaMemsetAsync(t->d_state + (size_t)video * T, 0, sizeof(TrackState) * T, s));
+        CK(cudaMemsetAsync(b.store + (size_t)video * T, 0, sizeof(BestEntry) * T, s));
+        CK(cudaMemsetAsync(b.videos + video, 0, sizeof(BestVideo), s));
+        CK(cudaEventRecord(t->chain, s));
+        CK(cudaEventRecord(slot.free, s));
+        if (dev_best) *dev_best = b.best;
+        if (dev_best_count) *dev_best_count = b.best_counts;
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }

@@ -184,9 +184,14 @@ __global__ void __launch_bounds__(TRACK_THREADS) k_track_update(const TrackArgs 
         const rf_det *dets = a.dets + (size_t)f * F;
         const int K = min(max(a.counts[f], 0), F);
         const float sc = t.scale[f];
+        TrackSeen *seen = a.seen ? a.seen + (size_t)f * F : nullptr;
+        TrackGone *gone = a.gone ? a.gone + (size_t)f * T : nullptr;
+        if (seen)
+            for (int j = tid; j < F; j += blockDim.x) seen[j].slot = -1;
         for (int i = tid; i < T; i += blockDim.x) {
             sm.match[i] = -1;
             sm.due[i] = 0;
+            if (gone) gone[i].id = 0;
             if (!sm.id[i]) continue;
             TrackState &k = S[i];
             sm.st0[i] = (unsigned char)k.state;
@@ -217,6 +222,7 @@ __global__ void __launch_bounds__(TRACK_THREADS) k_track_update(const TrackArgs 
                 k.det = j;
                 k.state = RF_TRACK_CONFIRMED;
                 sm.due[i] = st0 == RF_TRACK_TENTATIVE;
+                if (seen) seen[j] = TrackSeen{i, k.id, fj};
                 continue;
             }
             k.det = -1;
@@ -226,7 +232,11 @@ __global__ void __launch_bounds__(TRACK_THREADS) k_track_update(const TrackArgs 
                 else k.lost++;
                 remove = k.lost > a.p.max_lost;
             }
-            if (remove) { k.id = 0; sm.id[i] = 0; }
+            if (remove) {
+                if (gone) gone[i] = TrackGone{k.id, k.hits, k.age, st0 != RF_TRACK_TENTATIVE};
+                k.id = 0;
+                sm.id[i] = 0;
+            }
         }
         __syncthreads();
         if (tid == 0) {
@@ -249,6 +259,7 @@ __global__ void __launch_bounds__(TRACK_THREADS) k_track_update(const TrackArgs 
                 k.lost = 0;
                 k.det = j;
                 sm.due[slot] = first;
+                if (seen) seen[j] = TrackSeen{slot, k.id, fj};
             }
             s_frames++;
         }
@@ -325,6 +336,8 @@ cudaError_t launch_track_update(const TrackArgs &a, const int *videos, const flo
             c.due = a.due + (size_t)i0 * F;
             c.due_counts = a.due_counts + i0;
         }
+        if (a.seen) c.seen = a.seen + (size_t)i0 * F;
+        if (a.gone) c.gone = a.gone + (size_t)i0 * T;
         k_track_update<<<t.nvideos, TRACK_THREADS, smem, s>>>(c, t);
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;

@@ -44,6 +44,18 @@ struct TrackTable {
     int cta_video[TRACK_MAX_FRAMES];
 };
 
+// f11 (best.cuh): a track matched or born on a frame, at the index of its record (each such track holds a distinct record); slot -1:
+// the record went to no track.
+struct TrackSeen {
+    int slot, id;
+    rf_face face;                // the record in frame pixels, as the track keeps it
+};
+
+// f11: a track removed on a frame, at its slot; id 0: the slot lost no track.
+struct TrackGone {
+    int id, hits, age, confirmed;   // confirmed: the track was CONFIRMED at some point (its state at frame start was not TENTATIVE)
+};
+
 struct TrackArgs {
     TrackParams p;
     TrackVideo *videos;          // [max_videos]
@@ -57,6 +69,8 @@ struct TrackArgs {
     rf_det *due;                 // [n][max_faces] faces of the tracks confirmed on the frame, id order (crop_slot); NULL: no crops
     int *due_counts;             // [n]  min(due, max_align)
     int max_align;               // crop slots per frame (0 without crops)
+    TrackSeen *seen;             // optional [n][max_faces]: every record's track on the frame (f11)
+    TrackGone *gone;             // optional [n][max_tracks]: the tracks removed on the frame, by slot (f11)
 };
 
 // n frames (videos[i], scales[i]; scales NULL: 1), one launch per TRACK_MAX_FRAMES of them, in stream order on s.

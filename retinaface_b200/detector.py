@@ -120,18 +120,34 @@ class RetinaFace:
         return [FaceDetectInfo.from_row(r) for r in faces]
 
     def trackFrames(self, frames: Sequence, videos: Sequence[int], threshold: float = 0.5, layout: str = "nv12", matrix: str = "bt601",
-                    align: dict = None, max_videos: int = 64):
+                    align: dict = None, max_videos: int = 64, best: dict = None):
         """f10 tracking: device 4:2:0 frames (torch CUDA tensors in ``Engine.detect_yuv_device``'s forms), frame i of video
         ``videos[i]``, detected and associated with the tracks of earlier frames on the GPU (rf_detect_yuv_track_device).  Per frame, a
         list of ``(id, state, FaceDetectInfo)`` over every live track (``capi.TRACK_*`` states; the face is the last matched one, in
         FRAME pixels), and per frame a list of ``(id, crop)``: with ``align`` (``Engine.detect_align``'s keywords), one crop per track
         confirmed on that frame -- a new identity -- as a torch CUDA tensor.  The tracker is created on the first call with
-        ``max_videos`` sequences; ``resetTracks`` restarts them."""
+        ``max_videos`` sequences; ``resetTracks`` restarts them.
+
+        f11 best shots: with ``best`` (``capi.best_config``'s keywords: crop, template, fmt, mean, std, min_quality, sharp_half) the
+        tracker is a best-shot tracker (rf_detect_yuv_track_best_device; ``align`` must then be None) and the second list holds, per
+        frame, a ``(shot, crop)`` for every track that ended on that frame: ``shot`` a ``capi.BEST_DTYPE`` record (the quality terms
+        and the record of the track's best frame), ``crop`` that frame's crop as a torch CUDA tensor.  ``finishVideo`` emits the
+        shots of the tracks still live.  The first call decides which kind of tracker this detector keeps."""
         import torch
         from .capi import crop_shape
+        if best is not None and align is not None:
+            raise ValueError("best shots and new-identity crops are exclusive: pass best or align, not both")
         if getattr(self, "_tracker", None) is None:
-            self._tracker = self.engine.tracker(max_videos=max_videos)
+            self._tracker = self.engine.tracker(max_videos=max_videos, best=best)
         n = len(frames)
+        if best is not None:
+            crops = self._best_crops(n)
+            bp, bc, tp, tc, _, _, _ = self._tracker.detect_yuv_best_device(list(frames), list(videos), threshold, self.nms_threshold,
+                                                                          crops.data_ptr(), layout=layout, matrix=matrix)
+            recs = self._tracker.read(tp, tc, n)
+            tracks = [[(int(r["id"]), int(r["state"]), FaceDetectInfo.from_row(r["face"])) for r in per] for per in recs]
+            shots = self._tracker.read_best(bp, bc, n)
+            return tracks, [[(s, crops[i, k]) for k, s in enumerate(per)] for i, per in enumerate(shots)]
         crops = None
         if align is not None:
             kw = {"fmt": "bgr_u8", **align}
@@ -146,6 +162,25 @@ class RetinaFace:
         new = [[(int(r["id"]), crops[i, r["crop_slot"]]) for r in per if r["crop_slot"] >= 0] if crops is not None else []
                for i, per in enumerate(recs)]
         return tracks, new
+
+    def _best_crops(self, n: int):
+        import torch
+        from .capi import CROP_FORMATS, crop_shape
+        b = self._tracker.best
+        fmt = next(k for k, v in CROP_FORMATS.items() if v[0] == b.align.format)
+        shape, dt = crop_shape(fmt, (b.align.crop_w, b.align.crop_h))
+        return torch.empty((n, self._tracker.max_tracks) + shape, dtype={np.uint8: torch.uint8, np.float32: torch.float32,
+                                                                          np.float16: torch.float16}[dt], device="cuda")
+
+    def finishVideo(self, video: int) -> list:
+        """f11: end ``video`` on a best-shot tracker (rf_tracker_finish): a ``(shot, crop)`` for every live track that was ever
+        confirmed, in id order, then the video restarts (ids from 1)."""
+        if getattr(self, "_tracker", None) is None or self._tracker.best is None:
+            raise ValueError("finishVideo needs a best-shot tracker: call trackFrames(..., best=...) first")
+        crops = self._best_crops(1)[0]
+        bp, bc = self._tracker.finish(video, crops.data_ptr())
+        shots = self._tracker.read_best(bp, bc, 1)[0]
+        return [(s, crops[k]) for k, s in enumerate(shots)]
 
     def resetTracks(self, video: int = -1):
         """Restart one video's tracks (ids from 1), or every video's with -1."""

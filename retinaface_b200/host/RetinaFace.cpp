@@ -287,6 +287,7 @@ void RetinaFace::trackYUV(const vector<rf_yuv_frame> &device_frames, const vecto
                           void *dev_crops) {
     if (videos.size() != device_frames.size()) throw std::invalid_argument("trackYUV: one video index per frame");
     if (device_frames.size() > (size_t)opt_.max_batch) throw std::invalid_argument("trackYUV: at most max_batch frames per call");
+    if (best_tracker_) throw std::logic_error("trackYUV: this RetinaFace tracks with best shots (trackYUVBest)");
     if (!tracker_) {
         rf_track_config tc{};
         tc.max_videos = opt_.track_videos;
@@ -302,6 +303,40 @@ void RetinaFace::trackYUV(const vector<rf_yuv_frame> &device_frames, const vecto
     if (rc != RF_OK) throw std::runtime_error(string("rf_detect_yuv_track_device: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
     tracks_.n = n;
     tracks_.max_tracks = 64;      // rf_track_config's default
+}
+
+void RetinaFace::trackYUVBest(const vector<rf_yuv_frame> &device_frames, const vector<int> &videos, void *dev_best_crops, float threshold,
+                              float min_quality) {
+    if (videos.size() != device_frames.size()) throw std::invalid_argument("trackYUVBest: one video index per frame");
+    if (device_frames.size() > (size_t)opt_.max_batch) throw std::invalid_argument("trackYUVBest: at most max_batch frames per call");
+    if (tracker_ && !best_tracker_) throw std::logic_error("trackYUVBest: this RetinaFace already tracks without best shots (trackYUV)");
+    if (!tracker_) {
+        rf_track_config tc{};
+        tc.max_videos = opt_.track_videos;
+        rf_best_config bc{};
+        bc.min_quality = min_quality;
+        int rc = rf_tracker_create_best(h_, &tc, &bc, &tracker_);
+        if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_create_best: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+        best_tracker_ = true;
+    }
+    const int n = (int)device_frames.size();
+    tracks_ = DeviceTracks{};
+    best_ = DeviceBestShots{};
+    int rc = rf_detect_yuv_track_best_device(h_, tracker_, device_frames.data(), videos.data(), n, RF_YUV_BT601, threshold, nms_threshold,
+                                             dev_best_crops, nullptr, &best_.shots, &best_.counts, &tracks_.tracks, &tracks_.counts, nullptr,
+                                             nullptr, nullptr);
+    if (rc != RF_OK) throw std::runtime_error(string("rf_detect_yuv_track_best_device: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+    tracks_.n = best_.n = n;
+    tracks_.max_tracks = best_.max_tracks = 64;      // rf_track_config's default
+}
+
+void RetinaFace::finishVideo(int video, void *dev_best_crops) {
+    if (!tracker_ || !best_tracker_) throw std::logic_error("finishVideo: no best-shot tracker (trackYUVBest)");
+    best_ = DeviceBestShots{};
+    int rc = rf_tracker_finish(tracker_, video, dev_best_crops, nullptr, &best_.shots, &best_.counts);
+    if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_finish: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+    best_.n = 1;
+    best_.max_tracks = 64;
 }
 
 void RetinaFace::resetTracks(int video) {

@@ -113,6 +113,20 @@ class RetinaFace {
                   void *dev_crops = nullptr);
     const DeviceTracks &lastTracks() const { return tracks_; }
     void resetTracks(int video = -1);
+    // f11 best shots (rf_detect_yuv_track_best_device): trackYUV on a best-shot tracker (created on the first call with min_quality;
+    // one RetinaFace keeps one kind of tracker) that keeps the best 112x112 u8 crop of every track on the GPU.  Afterwards lastTracks()
+    // holds the track lists and lastBestShots() the shots emitted on each frame -- one per ever-confirmed track that ended there, in
+    // id order -- whose crops land in dev_best_crops [n][max_tracks] u8 BGR.  finishVideo emits the shots of a video's live tracks
+    // into dev_best_crops [max_tracks] (lastBestShots() then has n = 1) and restarts the video.
+    struct DeviceBestShots {
+        const rf_best_shot *shots = nullptr;  // device [n][max_tracks]
+        const int32_t *counts = nullptr;      // device [n]
+        int n = 0, max_tracks = 0;
+    };
+    void trackYUVBest(const vector<rf_yuv_frame> &device_frames, const vector<int> &videos, void *dev_best_crops, float threshold = 0.5,
+                      float min_quality = 0.f);
+    const DeviceBestShots &lastBestShots() const { return best_; }
+    void finishVideo(int video, void *dev_best_crops);
     rf_handle handle() const { return h_; }
     // the reference's visualisation (RetinaFace.cpp:730-741): red box outline (thickness 2), green landmark dots, on a clone
     static Mat draw(const Mat &img, const vector<FaceDetectInfo> &faces);
@@ -124,7 +138,9 @@ class RetinaFace {
     void keepResults(size_t start, int n, const unsigned char *crops, int per, int cw, int ch);
     rf_handle h_ = nullptr;
     rf_tracker tracker_ = nullptr;
+    bool best_tracker_ = false;
     DeviceTracks tracks_;
+    DeviceBestShots best_;
     RetinaFaceOptions opt_;
     string network;
     float nms_threshold;

@@ -608,6 +608,61 @@ int rf_detect_yuv_track_best_device(rf_handle h, rf_tracker t, const rf_yuv_fram
 int rf_tracker_finish(rf_tracker t, int video, void *dev_best_crops, double *dev_best_mats,
                       const rf_best_shot **dev_best, const int32_t **dev_best_count);
 
+/* f12 redaction: an in-place mosaic of every detected face -- and of every face the tracker still follows while the detector misses
+ * it -- written into the caller's device frames, so that footage can be stored, published or annotated without its faces and no
+ * frame leaves the GPU.  The calls WRITE the frames their descriptors point at (rf_yuv_frame's planes are declared const for the
+ * detect calls, which only read them).  Records of the oriented entry points are in displayed pixels and do not apply here.
+ *
+ * Regions.  Frame i's regions, in this order:
+ *   (a) its records j < min(counts[i], max_faces), in rank order; box = each coordinate as __fmul_rn(x, scales[i]) (f5's map-back;
+ *       scales == NULL means 1, as for tiled records);
+ *   (b) with track lists: every track of frame i's list whose state is RF_TRACK_LOST, in list (id) order, box (kx1, ky1, kx2, ky2).
+ *       Confirmed and tentative tracks with det >= 0 are already in (a); unmatched ones do not survive the frame.
+ * A box with a non-finite coordinate, or with w <= 0 or h <= 0, is skipped.  A region's index is its position among the boxes that
+ * were not skipped.
+ * Geometry.  FP64, one rounding per step, in this order:
+ *   w = x2 - x1, h = y2 - y1, mx = margin * w, my = margin * h
+ *   X0 = floor(max(x1 - mx, -65536)), X1 = floor(min(x2 + mx, 65536)) + 1   (half-open; + 1 = the reference's inclusive x2); Y0, Y1 likewise
+ *   snap outward to even: X0 = 2 floor(X0 / 2), X1 = 2 ceil(X1 / 2) (and Y)
+ *   cell side C = 2 ceil(max(X1 - X0, Y1 - Y0) / (2 blocks))   (even, >= 2; a box wholly beyond +-65536 has an empty rectangle, C = 2)
+ * Cells are C x C squares tiling the UNCLAMPED rectangle from (X0, Y0), the last cell of each axis possibly narrower: a face leaving
+ * the frame keeps its cell size and phase.
+ * Values.  Each cell's value is the mean of the ORIGINAL samples of the cell inside the frame, per plane, as (sum + cnt / 2) / cnt in integers: Y
+ * over luma cells; U and V over chroma cells of side C / 2 anchored at (X0 / 2, Y0 / 2) (snapping makes that grid exact); BGR each
+ * channel over the luma-coordinate cell.  "Original": before any region of the call was written, so overlapping regions never read
+ * each other's output.
+ * Output.  A luma (or BGR) pixel inside the frame and covered by at least one region's rectangle takes its cell value in the LOWEST-index region
+ * covering it; a chroma sample likewise with the rectangles halved.  Every other byte is not written: pixels outside all regions,
+ * pitch padding, and the bytes between NV12 chroma pairs that belong to other pixels. */
+typedef struct rf_redact_params {
+    int blocks;     /* cells across the longer side of a region; 0 -> 8; else 1..32 (1: one flat patch) */
+    float margin;   /* each side grows by margin x the box's side; 0 -> 0.25; else finite, in (0, 1] */
+} rf_redact_params;
+/* Redacts n device frames in place from the records of any device detect call on h (dev_dets [n][max_faces], dev_counts [n], scales
+ * as above) and, optionally, the track lists of a tracker of h (t, dev_tracks [n][max_tracks], dev_track_counts [n]: all three or
+ * none), as rf_track_update and rf_detect_yuv_track_device return them.  params NULL: the defaults.  Asynchronous, issued on
+ * rf_last_stream(), where those outputs complete; the caller keeps the frames alive until that stream has passed the call.
+ * Statuses, all before anything is launched (the frames stay untouched): the frame checks of rf_detect_yuv_batch_device (or, for
+ * rf_redact_device, of rf_detect_tiled_device's BGR images: dev_bgr[i], row stride NULL or 0 = packed); n > max_batch
+ * RF_ERR_CAPACITY; bad params, a tracker of another handle, tracks given only partly, NULL records, a non-positive or non-finite
+ * scale, or two frames whose plane byte ranges overlap: RF_ERR_INVALID_ARG.  n = 0 launches nothing.  Scratch is per execution
+ * context, allocated on first use and grown with the call: max_batch x (max_faces + max_tracks) regions x blocks^2 cells x 3 bytes
+ * at most. */
+int rf_redact_yuv_device(rf_handle h, const rf_yuv_frame *frames, int n, const rf_det *dev_dets, const int32_t *dev_counts,
+                         const float *scales, rf_tracker t, const rf_track *dev_tracks, const int32_t *dev_track_counts,
+                         const rf_redact_params *params);
+int rf_redact_device(rf_handle h, uint8_t *const *dev_bgr, const int *widths, const int *heights, const int *row_strides, int n,
+                     const rf_det *dev_dets, const int32_t *dev_counts, const float *scales, rf_tracker t, const rf_track *dev_tracks,
+                     const int32_t *dev_track_counts, const rf_redact_params *params);
+/* rf_detect_yuv_batch_device (t NULL) or rf_detect_yuv_track_device without crops (t a plain tracker of h; videos as there), then
+ * rf_redact_yuv_device of the frames with those records, scales and tracks, all on the forward's execution context.  Detections,
+ * tracks and the returned pointers are those of the two calls it replaces, bit for bit.  A best-shot tracker is RF_ERR_INVALID_ARG
+ * (its store must see every frame through rf_detect_yuv_track_best_device).  dev_tracks / dev_track_counts may be NULL. */
+int rf_detect_yuv_redact_device(rf_handle h, rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, int matrix,
+                                float score_threshold, float nms_threshold, const rf_redact_params *params,
+                                const rf_track **dev_tracks, const int32_t **dev_track_counts, const rf_det **dev_dets,
+                                const int32_t **dev_counts, float *out_scales);
+
 /* Introspection. */
 int rf_get_net_size(rf_handle h, int *net_w, int *net_h, int *max_batch, int *max_faces);
 int rf_num_anchors(rf_handle h);            /* per image: 8,232 @448x448, 47,040 @1280x896 */

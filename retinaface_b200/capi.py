@@ -34,6 +34,7 @@ EXPORTS = [
     "rf_detect_views_oriented", "rf_jpeg_exif_orientation",
     "rf_tracker_create", "rf_tracker_destroy", "rf_tracker_reset", "rf_track_update", "rf_detect_yuv_track_device", "rf_tracker_debug_state",
     "rf_tracker_create_best", "rf_detect_yuv_track_best_device", "rf_tracker_finish",
+    "rf_redact_yuv_device", "rf_redact_device", "rf_detect_yuv_redact_device",
 ]
 COMM_BLOB_BYTES = 128
 
@@ -231,6 +232,10 @@ BEST_DTYPE = np.dtype([(f, "<i4") for f in ("id", "video", "frame", "end_frame",
                       [(f, "<f4") for f in ("quality", "score", "eye", "frontal", "sharpness", "coverage")] + [("face", "<f4", (FACE_FLOATS,))])
 
 
+class RedactParams(C.Structure):  # rf_redact_params
+    _fields_ = [("blocks", C.c_int), ("margin", C.c_float)]
+
+
 class RfError(RuntimeError):
     def __init__(self, status: int, msg: str):
         super().__init__(f"librf_b200 status {status}: {msg}")
@@ -364,6 +369,13 @@ def load_library() -> C.CDLL:
     lib.rf_detect_yuv_track_best_device.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(YuvFrame), C.c_void_p, C.c_int, C.c_int, C.c_float,
                                                     C.c_float, C.c_void_p, C.c_void_p] + [C.POINTER(C.c_void_p)] * 6 + [C.c_void_p]
     lib.rf_tracker_finish.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
+    lib.rf_redact_yuv_device.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.POINTER(RedactParams)]
+    lib.rf_redact_device.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int,
+                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(RedactParams)]
+    lib.rf_detect_yuv_redact_device.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(YuvFrame), C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float,
+                                                C.POINTER(RedactParams), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                                C.POINTER(C.c_void_p), C.c_void_p]
     _lib = lib
     return lib
 
@@ -1026,6 +1038,52 @@ class Engine:
         return Tracker(self, TrackConfig(max_videos, max_tracks, high_thresh, new_thresh, iou_high, iou_low, iou_tentative, max_lost),
                        best_config(**best) if best is not None else None)
 
+    # -- f12 redaction ---------------------------------------------------------------------------------------------------------
+    @staticmethod
+    def _scales(scales, n):
+        if scales is None:
+            return None
+        sc = np.ascontiguousarray(scales, dtype=np.float32)
+        if sc.size != n:
+            raise ValueError(f"{n} frames but {sc.size} scales")
+        return sc
+
+    def redact_yuv_device(self, frames, dets_ptr: int, counts_ptr: int, scales=None, layout: str = "nv12", tracker: Optional["Tracker"] = None,
+                          tracks_ptr: Optional[int] = None, track_counts_ptr: Optional[int] = None, blocks: int = 0, margin: float = 0.0):
+        """rf_redact_yuv_device: mosaic, IN PLACE, every region of the device 4:2:0 frames (torch CUDA tensors in yuv_frame's forms):
+        the records at dets_ptr / counts_ptr of a device detect call (scales: each frame's map-back factor; None for records already
+        in frame pixels) and, with a tracker, the LOST tracks of its lists at tracks_ptr / track_counts_ptr.  Asynchronous on
+        last_stream_ptr()."""
+        n = len(frames)
+        arr = self._frames(frames, layout, True)
+        sc = self._scales(scales, n)
+        p = RedactParams(int(blocks), float(margin))
+        self._check(self.lib.rf_redact_yuv_device(self.h, arr, n, dets_ptr, counts_ptr, sc.ctypes.data if sc is not None else None,
+                                                  tracker.t if tracker is not None else None, tracks_ptr, track_counts_ptr, C.byref(p)))
+
+    def redact_device(self, images, dets_ptr: int, counts_ptr: int, scales=None, tracker: Optional["Tracker"] = None,
+                      tracks_ptr: Optional[int] = None, track_counts_ptr: Optional[int] = None, blocks: int = 0, margin: float = 0.0):
+        """rf_redact_device: redact_yuv_device on u8 BGR HWC torch CUDA tensors (rows may be strided), in place."""
+        n = len(images)
+        ptrs, ws, hs, rs = self._device_images(images)
+        sc = self._scales(scales, n)
+        p = RedactParams(int(blocks), float(margin))
+        self._check(self.lib.rf_redact_device(self.h, ptrs, ws, hs, rs, n, dets_ptr, counts_ptr, sc.ctypes.data if sc is not None else None,
+                                              tracker.t if tracker is not None else None, tracks_ptr, track_counts_ptr, C.byref(p)))
+
+    def detect_yuv_redact_device(self, frames, thr: float, nms_thr: float, layout: str = "nv12", matrix="bt601", blocks: int = 0,
+                                 margin: float = 0.0):
+        """rf_detect_yuv_redact_device without a tracker: detect_yuv_device, then redact_yuv_device of its records on the same
+        context.  Returns (dets_ptr, counts_ptr, scales) as detect_yuv_device; the frames are redacted in place."""
+        n = len(frames)
+        arr = self._frames(frames, layout, True)
+        p = RedactParams(int(blocks), float(margin))
+        scales = np.zeros(max(n, 1), dtype=np.float32)
+        d, c = C.c_void_p(), C.c_void_p()
+        self._check(self.lib.rf_detect_yuv_redact_device(self.h, None, arr, None, n, _matrix(matrix), thr, nms_thr, C.byref(p), None, None,
+                                                         C.byref(d), C.byref(c), scales.ctypes.data))
+        return int(d.value or 0), int(c.value or 0), scales[:n].copy()
+
     def calibrate_int8(self, images: np.ndarray, out_table: str):
         """INT8 entropy calibration on an RF_PREC_FP32 engine; writes a TensorRT-format table."""
         images = np.ascontiguousarray(images, dtype=np.uint8)
@@ -1137,6 +1195,19 @@ class Tracker:
                                                                     C.byref(tp), C.byref(tc), C.byref(d), C.byref(c), scales.ctypes.data))
         return (int(bp.value or 0), int(bc.value or 0), int(tp.value or 0), int(tc.value or 0), int(d.value or 0), int(c.value or 0),
                 scales[:n].copy())
+
+    def detect_yuv_redact_device(self, frames, videos: Sequence[int], thr: float, nms_thr: float, layout: str = "nv12", matrix="bt601",
+                                 blocks: int = 0, margin: float = 0.0):
+        """rf_detect_yuv_redact_device with this tracker: detect_yuv_device (no crops), the update, then the redaction of every record and
+        every LOST track, in place.  Returns (tracks_ptr, track_counts_ptr, dets_ptr, counts_ptr, scales) as detect_yuv_device."""
+        n = len(frames)
+        arr = self.engine._frames(frames, layout, True)
+        p = RedactParams(int(blocks), float(margin))
+        scales = np.zeros(max(n, 1), dtype=np.float32)
+        tp, tc, d, c = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
+        self.engine._check(self.lib.rf_detect_yuv_redact_device(self.engine.h, self.t, arr, self._ints(videos, n), n, _matrix(matrix), thr, nms_thr,
+                                                                C.byref(p), C.byref(tp), C.byref(tc), C.byref(d), C.byref(c), scales.ctypes.data))
+        return int(tp.value or 0), int(tc.value or 0), int(d.value or 0), int(c.value or 0), scales[:n].copy()
 
     def finish(self, video: int, dev_best_crops_ptr: int, dev_best_mats_ptr: Optional[int] = None):
         """rf_tracker_finish: emit the best shot of every live, ever-confirmed track of `video` (crops at dev_best_crops_ptr

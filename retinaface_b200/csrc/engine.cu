@@ -4,12 +4,14 @@
 // Replaces the reference's engine slot: TrtNetBase / TrtRetinaFaceNet
 // (retinaface/tensorrt/trtnetbase.cpp:199-330, trtretinafacenet.cpp:48-210) and the detect
 // orchestration of RetinaFace::detect / detectBatchImages (retinaface/RetinaFace.cpp:576-940).
+#include <array>
 #include <cmath>
 
 #include "engine_internal.cuh"
 #include "calibrate.cuh"
 #include "preprocess.cuh"
 #include "best.cuh"
+#include "redact.cuh"
 #include "track.cuh"
 
 namespace rf_eng {
@@ -165,7 +167,7 @@ void release_ctx(Ctx &c, bool all) {
     cudaFree(c.arena);
     c.arena = nullptr;
     if (!all) return;
-    cudaFree(c.d_params); cudaFreeHost(c.h_params); cudaFree(c.d_frames_in);
+    cudaFree(c.d_params); cudaFreeHost(c.h_params); cudaFree(c.d_frames_in); cudaFree(c.d_redact);
     free_post_buffers(c.pb);
     for (auto e : c.step_event) if (e) cudaEventDestroy(e);
     for (int l = 1; l < 3; l++) if (c.lane_stream[l]) cudaStreamDestroy(c.lane_stream[l]);
@@ -2251,6 +2253,202 @@ int rf_tracker_debug_state(rf_tracker t, int video, double *out, int cap) {
     }
     std::copy(v.begin(), v.begin() + std::min<size_t>(v.size(), (size_t)std::max(cap, 0)), out);
     return (int)live.size();
+}
+
+// ---- f12 redaction (redact.cuh) -------------------------------------------------------------------------------------------------
+extern "C++" {
+// params (NULL: defaults) -> blocks and margin
+static int redact_params(rf_handle h, const char *who, const rf_redact_params *p, int &blocks, double &margin) {
+    blocks = p && p->blocks ? p->blocks : 8;
+    const float m = p && p->margin != 0.f ? p->margin : 0.25f;
+    if (blocks < 1 || blocks > REDACT_MAX_BLOCKS)
+        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: blocks %d, must be 0 or in [1, %d]", who, blocks, REDACT_MAX_BLOCKS));
+    if (!(std::isfinite(m) && m > 0.f && m <= 1.f))
+        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: margin %g, must be 0 or finite in (0, 1]", who, (double)m));
+    margin = (double)m;
+    return RF_OK;
+}
+
+// The records, scales and tracks of a redaction call.
+static int check_redact_inputs(rf_handle h, const char *who, int n, const rf_det *dets, const int32_t *counts, const float *scales, rf_tracker t,
+                               const rf_track *tracks, const int32_t *track_counts) {
+    if (n > 0 && (!dets || !counts)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL records or counts", who));
+    const bool any = t || tracks || track_counts;
+    if (any && !(t && tracks && track_counts))
+        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker, its tracks and their counts go together (all three or none)", who));
+    if (t && t->h != h) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker belongs to another handle", who));
+    for (int i = 0; scales && i < n; i++)
+        if (!(std::isfinite(scales[i]) && scales[i] > 0.f))
+            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frame %d: scale %g, must be finite and positive", who, i, (double)scales[i]));
+    return RF_OK;
+}
+
+// Refuses two frames whose plane byte ranges overlap: a later chunk's measure would read pixels an earlier chunk has written, and
+// within a chunk two regions' writes could land on one byte.  ranges: (first byte, one past the last, frame).  A sweep in address
+// order that keeps the furthest end seen (and the furthest end of any other frame) finds every overlap of two frames.
+static int check_disjoint(rf_handle h, const char *who, std::vector<std::array<uintptr_t, 3>> ranges) {
+    std::sort(ranges.begin(), ranges.end());
+    uintptr_t end1 = 0, end2 = 0;
+    uintptr_t frame1 = ~(uintptr_t)0;        // end1: the furthest end, of frame1; end2: the furthest end of any other frame
+    for (const auto &r : ranges) {
+        const uintptr_t other = r[2] == frame1 ? end2 : end1;
+        if (r[0] < other) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frame %d overlaps the bytes of another frame of the call", who, (int)r[2]));
+        if (r[1] > end1) {
+            if (r[2] != frame1) { end2 = end1; frame1 = r[2]; }
+            end1 = r[1];
+        } else if (r[2] != frame1 && r[1] > end2) {
+            end2 = r[1];
+        }
+    }
+    return RF_OK;
+}
+
+static std::vector<std::array<uintptr_t, 3>> yuv_ranges(const rf_yuv_frame *frames, int n) {
+    std::vector<std::array<uintptr_t, 3>> r;
+    for (int i = 0; i < n; i++) {
+        const rf_yuv_frame &f = frames[i];
+        const uintptr_t y = (uintptr_t)f.y, u = (uintptr_t)f.u, v = (uintptr_t)f.v, ch = f.height / 2 - 1;
+        r.push_back({y, y + (uintptr_t)(f.height - 1) * f.y_pitch + f.width, (uintptr_t)i});
+        if (f.uv_step == 2) {
+            const uintptr_t lo = std::min(u, v);
+            r.push_back({lo, lo + ch * f.uv_pitch + f.width, (uintptr_t)i});
+        } else {
+            r.push_back({u, u + ch * f.uv_pitch + f.width / 2, (uintptr_t)i});
+            r.push_back({v, v + ch * f.uv_pitch + f.width / 2, (uintptr_t)i});
+        }
+    }
+    return r;
+}
+
+static Ctx &last_ctx(rf_handle h) {
+    for (Ctx &c : h->ctx)
+        if (c.stream == h->last_stream) return c;
+    return h->ctx[0];
+}
+
+// Issues the redaction of `frames` on context c's stream, into c's scratch (sized for max_batch frames of this call's region
+// capacity and blocks; a larger need waits for the context before the scratch is replaced).
+template <typename Dst>
+static void redact_issue(rf_handle h, Ctx &c, const std::vector<RedactFrameT<Dst>> &frames, const rf_det *dets, const int32_t *counts, rf_tracker t,
+                         const rf_track *tracks, const int32_t *track_counts, int blocks, double margin) {
+    RedactArgs a{};
+    a.n = (int)frames.size();
+    a.blocks = blocks;
+    a.margin = margin;
+    a.max_faces = h->cfg.max_faces;
+    a.max_tracks = t ? t->cfg.max_tracks : 0;
+    a.cap = a.max_faces + a.max_tracks;
+    a.dets = dets;
+    a.counts = counts;
+    a.tracks = tracks;
+    a.track_counts = track_counts;
+    const size_t need = redact_scratch_bytes(h->cfg.max_batch, a.cap, blocks);
+    if (need > c.redact_bytes) {
+        CK(cudaStreamSynchronize(c.stream));
+        CK(cudaFree(c.d_redact));
+        c.d_redact = nullptr;
+        c.redact_bytes = 0;
+        CK(cudaMalloc(&c.d_redact, need));
+        c.redact_bytes = need;
+    }
+    redact_carve(a, c.d_redact);
+    CK(launch_redact(a, frames.data(), h->num_sms, c.stream));
+}
+
+static std::vector<RedactFrameT<YuvPlanesW>> yuv_redact_table(const rf_yuv_frame *frames, int n, const float *scales) {
+    std::vector<RedactFrameT<YuvPlanesW>> v(n);
+    for (int i = 0; i < n; i++) {
+        const rf_yuv_frame &f = frames[i];
+        v[i] = RedactFrameT<YuvPlanesW>{YuvPlanesW{const_cast<uint8_t *>(f.y), const_cast<uint8_t *>(f.u), const_cast<uint8_t *>(f.v), f.y_pitch,
+                                                   f.uv_pitch, f.uv_step},
+                                        f.width, f.height, scales ? scales[i] : 1.f};
+    }
+    return v;
+}
+}  // extern "C++"
+
+int rf_redact_yuv_device(rf_handle h, const rf_yuv_frame *frames, int n, const rf_det *dev_dets, const int32_t *dev_counts, const float *scales,
+                         rf_tracker t, const rf_track *dev_tracks, const int32_t *dev_track_counts, const rf_redact_params *params) {
+    static const char *who = "rf_redact_yuv_device";
+    if (!h) return RF_ERR_INVALID_ARG;
+    int rc = check_frames(h, who, frames, n, RF_YUV_BT601);      // the matrix plays no part: the mosaic is per plane
+    if (rc) return rc;
+    int blocks;
+    double margin;
+    if ((rc = redact_params(h, who, params, blocks, margin))) return rc;
+    if ((rc = check_redact_inputs(h, who, n, dev_dets, dev_counts, scales, t, dev_tracks, dev_track_counts))) return rc;
+    if ((rc = check_disjoint(h, who, yuv_ranges(frames, n)))) return rc;
+    if (n == 0) return RF_OK;
+    try {
+        CK(cudaSetDevice(h->device));
+        redact_issue(h, last_ctx(h), yuv_redact_table(frames, n, scales), dev_dets, dev_counts, t, dev_tracks, dev_track_counts, blocks, margin);
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
+}
+
+int rf_redact_device(rf_handle h, uint8_t *const *dev_bgr, const int *widths, const int *heights, const int *row_strides, int n,
+                     const rf_det *dev_dets, const int32_t *dev_counts, const float *scales, rf_tracker t, const rf_track *dev_tracks,
+                     const int32_t *dev_track_counts, const rf_redact_params *params) {
+    static const char *who = "rf_redact_device";
+    if (!h) return RF_ERR_INVALID_ARG;
+    const BgrImages src{dev_bgr, widths, heights, row_strides, nullptr, false};
+    int rc = src.check(h, who, n);
+    if (rc) return rc;
+    int blocks;
+    double margin;
+    if ((rc = redact_params(h, who, params, blocks, margin))) return rc;
+    if ((rc = check_redact_inputs(h, who, n, dev_dets, dev_counts, scales, t, dev_tracks, dev_track_counts))) return rc;
+    std::vector<std::array<uintptr_t, 3>> ranges;
+    for (int i = 0; i < n; i++) {
+        const uintptr_t p = (uintptr_t)dev_bgr[i];
+        ranges.push_back({p, p + (uintptr_t)(heights[i] - 1) * src.stride(i) + 3 * (uintptr_t)widths[i], (uintptr_t)i});
+    }
+    if ((rc = check_disjoint(h, who, ranges))) return rc;
+    if (n == 0) return RF_OK;
+    try {
+        CK(cudaSetDevice(h->device));
+        std::vector<RedactFrameT<BgrRowsW>> v(n);
+        for (int i = 0; i < n; i++) v[i] = RedactFrameT<BgrRowsW>{BgrRowsW{dev_bgr[i], src.stride(i)}, widths[i], heights[i], scales ? scales[i] : 1.f};
+        redact_issue(h, last_ctx(h), v, dev_dets, dev_counts, t, dev_tracks, dev_track_counts, blocks, margin);
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
+}
+
+int rf_detect_yuv_redact_device(rf_handle h, rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, int matrix, float thr, float nms,
+                                const rf_redact_params *params, const rf_track **dev_tracks, const int32_t **dev_track_counts,
+                                const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales) {
+    static const char *who = "rf_detect_yuv_redact_device";
+    if (!h) return RF_ERR_INVALID_ARG;
+    int rc;
+    if (t) {
+        if (t->h != h) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker belongs to another handle", who));
+        if (t->best) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a best-shot tracker takes frames only through rf_detect_yuv_track_best_device", who));
+        if ((rc = check_track_args(t, who, videos, n, nullptr))) return rc;
+    }
+    const YuvFrames src{frames, matrix, nullptr, false};
+    if ((rc = src.check(h, who, n))) return rc;
+    int blocks;
+    double margin;
+    if ((rc = redact_params(h, who, params, blocks, margin))) return rc;
+    if ((rc = check_disjoint(h, who, yuv_ranges(frames, n)))) return rc;
+    if (n == 0) return RF_OK;
+    std::vector<float> scales(n);
+    const rf_det *dets = nullptr;
+    const int32_t *counts = nullptr;
+    if ((rc = yuv_device_impl(h, who, src, n, thr, nms, nullptr, nullptr, nullptr, &dets, &counts, scales.data()))) return rc;
+    if (dev_dets) *dev_dets = dets;
+    if (dev_counts) *dev_counts = counts;
+    if (out_scales) std::copy(scales.begin(), scales.end(), out_scales);
+    try {
+        Ctx &c = last_ctx(h);          // the forward's context
+        const rf_track *tracks = nullptr;
+        const int32_t *track_counts = nullptr;
+        if (t) track_issue(t, videos, n, dets, counts, scales.data(), c.stream, nullptr, nullptr, &tracks, &track_counts);
+        if (dev_tracks) *dev_tracks = tracks;
+        if (dev_track_counts) *dev_track_counts = track_counts;
+        redact_issue(h, c, yuv_redact_table(frames, n, scales.data()), dets, counts, t, tracks, track_counts, blocks, margin);
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
 }
 
 }  // extern "C"

@@ -81,6 +81,10 @@ struct Ctx {
     // rf_detect_yuv_batch_device (lazily allocated): this context's letter-boxed frames [max_batch][H][W][3].  One tensor per
     // context: the letter-box of a call on another context must not overwrite the input of a forward still running here.
     uint8_t *d_frames_in = nullptr;
+    // f12 redaction scratch (redact.cuh; lazily allocated, grown when a call needs more): region tables and cell means of the calls
+    // issued on this context's stream.  Per context: calls on two contexts' streams may run at once.
+    void *d_redact = nullptr;
+    size_t redact_bytes = 0;
 };
 
 // What one step launch writes into and where it is issued.

@@ -1,0 +1,352 @@
+// redact.cu -- see redact.cuh.  Compiled with -fmad=false: the region geometry is FP64 with one rounding per step, as rf_b200.h and
+// oracle/redact.py state it (margin * w, then the subtraction).
+#include <algorithm>
+
+#include "redact.cuh"
+
+namespace rf {
+
+namespace {
+
+// Lower-index rectangles an apply item keeps in shared memory; an item overlapped by more of them scans the region table instead.
+constexpr int REDACT_COVER = 512;
+
+template <typename D>
+struct RedactTable {
+    using Dst = D;
+    static constexpr int kMax = redact_table_limit<D>();
+    RedactFrameT<D> f[kMax];
+};
+static_assert(sizeof(RedactArgs) + sizeof(RedactTable<YuvPlanesW>) + 32 <= 4096 && sizeof(RedactArgs) + sizeof(RedactTable<BgrRowsW>) + 32 <= 4096,
+              "redact launch exceeds the classic 4 KB kernel parameter space");
+
+// Exclusive block scan of v over REDACT_THREADS threads; *total receives the sum.  Every thread of the CTA calls it.
+__device__ int block_scan(int v, int *total, int *s_w) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int incl = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int t = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += t;
+    }
+    if (lane == 31) s_w[warp] = incl;
+    __syncthreads();
+    int pre = 0, tot = 0;
+#pragma unroll
+    for (int w = 0; w < REDACT_THREADS / 32; w++) {
+        if (w < warp) pre += s_w[w];
+        tot += s_w[w];
+    }
+    __syncthreads();
+    *total = tot;
+    return pre + incl - v;
+}
+
+// The header's geometry of one box in frame pixels; false: the box is skipped.  mi / ai: the region's measure and apply items (0
+// when its rectangle misses the frame).  The clamps beyond +-65536 keep the integers in range without changing any non-empty
+// rectangle: a bound past them already makes the rectangle empty.
+__device__ bool region_geometry(float fx1, float fy1, float fx2, float fy2, double margin, int blocks, int W, int H, RedactRegion &g, int &mi,
+                                int &ai) {
+    if (!(isfinite(fx1) && isfinite(fy1) && isfinite(fx2) && isfinite(fy2))) return false;
+    const double x1 = fx1, y1 = fy1, x2 = fx2, y2 = fy2;
+    const double w = x2 - x1, h = y2 - y1;
+    if (!(w > 0.0) || !(h > 0.0)) return false;
+    const double mx = margin * w, my = margin * h;
+    g.x0 = (int)floor(fmin(fmax(x1 - mx, -65536.0), 65538.0)) & ~1;
+    g.y0 = (int)floor(fmin(fmax(y1 - my, -65536.0), 65538.0)) & ~1;
+    g.x1 = ((int)floor(fmax(fmin(x2 + mx, 65536.0), -65538.0)) + 2) & ~1;    // 2 ceil((floor(.) + 1) / 2)
+    g.y1 = ((int)floor(fmax(fmin(y2 + my, 65536.0), -65538.0)) + 2) & ~1;
+    const int D = max(g.x1 - g.x0, g.y1 - g.y0);
+    g.c = D > 0 ? 2 * ((D + 2 * blocks - 1) / (2 * blocks)) : 2;
+    g.nx = g.x1 > g.x0 ? (g.x1 - g.x0 + g.c - 1) / g.c : 0;
+    g.cr0 = 0;
+    mi = ai = 0;
+    const int cx0 = max(g.x0, 0), cx1 = min(g.x1, W), cy0 = max(g.y0, 0), cy1 = min(g.y1, H);
+    if (cx0 < cx1 && cy0 < cy1) {
+        g.cr0 = (cy0 - g.y0) / g.c;
+        mi = (cy1 - 1 - g.y0) / g.c - g.cr0 + 1;
+        ai = (cy1 - cy0 + REDACT_BAND - 1) / REDACT_BAND;
+    }
+    return true;
+}
+
+template <typename Table>
+__global__ void __launch_bounds__(REDACT_THREADS) k_redact_regions(const RedactArgs a, const __grid_constant__ Table table) {
+    __shared__ int s_w[3][REDACT_THREADS / 32];
+    const int i = blockIdx.x;
+    const auto &fr = table.f[i];
+    const int na = min(max(a.counts[i], 0), a.max_faces);
+    const int nb = a.tracks ? min(max(a.track_counts[i], 0), a.max_tracks) : 0;
+    int run_r = 0, run_m = 0, run_a = 0;
+    for (int k0 = 0; k0 < na + nb; k0 += REDACT_THREADS) {
+        const int k = k0 + threadIdx.x;
+        bool ok = false;
+        RedactRegion g{};
+        int mi = 0, ai = 0;
+        if (k < na) {
+            const rf_face &f = a.dets[(size_t)i * a.max_faces + k].face;
+            ok = region_geometry(__fmul_rn(f.x1, fr.scale), __fmul_rn(f.y1, fr.scale), __fmul_rn(f.x2, fr.scale), __fmul_rn(f.y2, fr.scale), a.margin,
+                                 a.blocks, fr.w, fr.h, g, mi, ai);
+        } else if (k < na + nb) {
+            const rf_track &t = a.tracks[(size_t)i * a.max_tracks + (k - na)];
+            ok = t.state == RF_TRACK_LOST && region_geometry(t.kx1, t.ky1, t.kx2, t.ky2, a.margin, a.blocks, fr.w, fr.h, g, mi, ai);
+        }
+        int tr, tm, ta;
+        const int pr = block_scan(ok ? 1 : 0, &tr, s_w[0]);
+        const int pm = block_scan(ok ? mi : 0, &tm, s_w[1]);
+        const int pa = block_scan(ok ? ai : 0, &ta, s_w[2]);
+        if (ok) {
+            g.m_first = run_m + pm;
+            g.a_first = run_a + pa;
+            a.regions[(size_t)i * a.cap + run_r + pr] = g;
+        }
+        run_r += tr;
+        run_m += tm;
+        run_a += ta;
+    }
+    if (threadIdx.x == 0) *reinterpret_cast<int4 *>(a.totals + 4 * i) = make_int4(run_r, run_m, run_a, 0);
+}
+
+// s_first[0..n]: the first work item of each frame (column `col` of the totals), s_first[n] the total.
+__device__ void frame_firsts(const RedactArgs &a, int col, int *s_first) {
+    if (threadIdx.x == 0) {
+        int run = 0;
+        for (int i = 0; i < a.n; i++) {
+            s_first[i] = run;
+            run += a.totals[4 * i + col];
+        }
+        s_first[a.n] = run;
+    }
+    __syncthreads();
+}
+
+// The frame of work item `item` (the last frame whose first item is <= item) and, within it, the region (the last whose first
+// item, field `first`, is <= k): regions without items share the next one's first item and are never chosen.
+__device__ void locate(const RedactArgs &a, const int *s_first, int item, int RedactRegion::*first, int &i, int &r, int &k) {
+    int lo = 0, hi = a.n - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (s_first[mid] <= item) lo = mid; else hi = mid - 1;
+    }
+    i = lo;
+    k = item - s_first[i];
+    const RedactRegion *R = a.regions + (size_t)i * a.cap;
+    lo = 0;
+    hi = a.totals[4 * i] - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (R[mid].*first <= k) lo = mid; else hi = mid - 1;
+    }
+    r = lo;
+}
+
+// Sum of the bytes q[y * pitch], y in [y0, y1): REDACT_UNROLL independent loads in flight per step, so that a column costs a few
+// memory round trips rather than one per row.
+constexpr int REDACT_UNROLL = 8;
+__device__ __forceinline__ unsigned column_sum(const uint8_t *q, int pitch, int y0, int y1) {
+    unsigned s = 0;
+    int y = y0;
+    for (; y + REDACT_UNROLL <= y1; y += REDACT_UNROLL) {
+        unsigned v[REDACT_UNROLL];
+#pragma unroll
+        for (int k = 0; k < REDACT_UNROLL; k++) v[k] = q[(size_t)(y + k) * pitch];
+#pragma unroll
+        for (int k = 0; k < REDACT_UNROLL; k++) s += v[k];
+    }
+    for (; y < y1; y++) s += q[(size_t)y * pitch];
+    return s;
+}
+
+// One cell row of one region per work item: every thread sums a column of the row's samples inside the frame and adds the sum to
+// its cell's shared accumulator; then one thread per cell writes the rounded means.
+template <typename Table>
+__global__ void __launch_bounds__(REDACT_THREADS) k_redact_measure(const RedactArgs a, const __grid_constant__ Table table) {
+    using Dst = typename Table::Dst;
+    __shared__ int s_first[Table::kMax + 1];
+    __shared__ unsigned long long s_sum[3][REDACT_MAX_BLOCKS];
+    constexpr bool kYuv = std::is_same<Dst, YuvPlanesW>::value;
+    frame_firsts(a, 1, s_first);
+    const int items = s_first[a.n], bb = a.blocks * a.blocks;
+    for (int item = blockIdx.x; item < items; item += gridDim.x) {
+        int i, r, k;
+        locate(a, s_first, item, &RedactRegion::m_first, i, r, k);
+        const auto &fr = table.f[i];
+        const RedactRegion g = a.regions[(size_t)i * a.cap + r];
+        const int c = g.c, cr = g.cr0 + (k - g.m_first);
+        for (int t = threadIdx.x; t < 3 * REDACT_MAX_BLOCKS; t += REDACT_THREADS) s_sum[t / REDACT_MAX_BLOCKS][t % REDACT_MAX_BLOCKS] = 0;
+        __syncthreads();
+        const int cx0 = max(g.x0, 0), cx1 = min(g.x1, fr.w);
+        const int ry0 = max(g.y0 + cr * c, 0), ry1 = min(min(g.y0 + (cr + 1) * c, g.y1), fr.h);
+        if constexpr (kYuv) {
+            const YuvPlanesW &p = fr.dst;
+            for (int x = cx0 + threadIdx.x; x < cx1; x += REDACT_THREADS) {
+                const unsigned s = column_sum(p.y + x, p.y_pitch, ry0, ry1);
+                atomicAdd(&s_sum[0][(x - g.x0) / c], (unsigned long long)s);
+            }
+            // chroma: the rectangle and the row halved (every bound is even), cells of side c / 2 anchored at (x0 / 2, y0 / 2)
+            for (int x = (cx0 >> 1) + threadIdx.x; x < (cx1 >> 1); x += REDACT_THREADS) {
+                const size_t o = (size_t)x * p.uv_step;
+                const unsigned su = column_sum(p.u + o, p.uv_pitch, ry0 >> 1, ry1 >> 1), sv = column_sum(p.v + o, p.uv_pitch, ry0 >> 1, ry1 >> 1);
+                const int cell = (2 * x - g.x0) / c;
+                atomicAdd(&s_sum[1][cell], (unsigned long long)su);
+                atomicAdd(&s_sum[2][cell], (unsigned long long)sv);
+            }
+        } else {
+            const BgrRowsW &p = fr.dst;
+            for (int x = cx0 + threadIdx.x; x < cx1; x += REDACT_THREADS) {
+                const uint8_t *q = p.p + 3 * (size_t)x;
+                const unsigned s0 = column_sum(q, p.pitch, ry0, ry1), s1 = column_sum(q + 1, p.pitch, ry0, ry1), s2 = column_sum(q + 2, p.pitch, ry0, ry1);
+                const int cell = (x - g.x0) / c;
+                atomicAdd(&s_sum[0][cell], (unsigned long long)s0);
+                atomicAdd(&s_sum[1][cell], (unsigned long long)s1);
+                atomicAdd(&s_sum[2][cell], (unsigned long long)s2);
+            }
+        }
+        __syncthreads();
+        uint8_t *out = a.cells + ((size_t)i * a.cap + r) * bb * 3 + (size_t)cr * g.nx * 3;
+        for (int cx = threadIdx.x; cx < g.nx; cx += REDACT_THREADS) {
+            const int xa = max(g.x0 + cx * c, 0), xb = min(min(g.x0 + (cx + 1) * c, g.x1), fr.w);
+            const unsigned long long cnt = xb > xa && ry1 > ry0 ? (unsigned long long)(xb - xa) * (ry1 - ry0) : 0;
+            const unsigned long long cc = kYuv ? cnt / 4 : cnt;      // chroma: both sides halved
+            out[3 * cx + 0] = cnt ? (uint8_t)((s_sum[0][cx] + cnt / 2) / cnt) : 0;
+            out[3 * cx + 1] = cc ? (uint8_t)((s_sum[1][cx] + cc / 2) / cc) : 0;
+            out[3 * cx + 2] = cc ? (uint8_t)((s_sum[2][cx] + cc / 2) / cc) : 0;
+        }
+        __syncthreads();     // the accumulators of the next item
+    }
+}
+
+// One band of REDACT_BAND rows of one region per work item: the lower-index rectangles that reach the band go to shared memory, then
+// every pixel of the band they do not cover takes its cell value -- luma first, then the band's chroma rows.
+template <typename Table>
+__global__ void __launch_bounds__(REDACT_THREADS) k_redact_apply(const RedactArgs a, const __grid_constant__ Table table) {
+    using Dst = typename Table::Dst;
+    __shared__ int s_first[Table::kMax + 1];
+    __shared__ int4 s_rect[REDACT_COVER];
+    __shared__ uint8_t s_cells[REDACT_MAX_BLOCKS * REDACT_MAX_BLOCKS * 3];
+    __shared__ int s_nrect;
+    constexpr bool kYuv = std::is_same<Dst, YuvPlanesW>::value;
+    frame_firsts(a, 2, s_first);
+    const int items = s_first[a.n], bb = a.blocks * a.blocks;
+    for (int item = blockIdx.x; item < items; item += gridDim.x) {
+        int i, r, k;
+        locate(a, s_first, item, &RedactRegion::a_first, i, r, k);
+        const auto &fr = table.f[i];
+        const RedactRegion *R = a.regions + (size_t)i * a.cap;
+        const RedactRegion g = R[r];
+        const int c = g.c, nx = g.nx;
+        const int cx0 = max(g.x0, 0), cx1 = min(g.x1, fr.w);
+        const int by0 = max(g.y0, 0) + (k - g.a_first) * REDACT_BAND, by1 = min(by0 + REDACT_BAND, min(g.y1, fr.h));
+        if (threadIdx.x == 0) s_nrect = 0;
+        __syncthreads();
+        for (int q = threadIdx.x; q < r; q += REDACT_THREADS) {
+            const RedactRegion o = R[q];
+            if (o.x0 < cx1 && o.x1 > cx0 && o.y0 < by1 && o.y1 > by0) {
+                const int slot = atomicAdd(&s_nrect, 1);
+                if (slot < REDACT_COVER) s_rect[slot] = make_int4(o.x0, o.y0, o.x1, o.y1);
+            }
+        }
+        // the region's cell values: one round trip here instead of one per pixel below
+        const uint8_t *cg = a.cells + ((size_t)i * a.cap + r) * bb * 3;
+        const int ny = (g.y1 - g.y0 + c - 1) / c;
+        for (int t = threadIdx.x; t < nx * ny * 3; t += REDACT_THREADS) s_cells[t] = cg[t];
+        __syncthreads();
+        const int nrect = s_nrect;
+        auto covered = [&](int x, int y) {
+            if (nrect <= REDACT_COVER) {
+                for (int j = 0; j < nrect; j++) {
+                    const int4 o = s_rect[j];
+                    if (x >= o.x && x < o.z && y >= o.y && y < o.w) return true;
+                }
+                return false;
+            }
+            for (int q = 0; q < r; q++) {
+                const RedactRegion &o = R[q];
+                if (x >= o.x0 && x < o.x1 && y >= o.y0 && y < o.y1) return true;
+            }
+            return false;
+        };
+        const uint8_t *cv = s_cells;
+        const int bw = cx1 - cx0, rows = by1 - by0;
+        if constexpr (kYuv) {
+            const YuvPlanesW &p = fr.dst;
+            for (int t = threadIdx.x; t < rows * bw; t += REDACT_THREADS) {
+                const int y = by0 + t / bw, x = cx0 + t % bw;
+                if (covered(x, y)) continue;
+                p.y[(size_t)y * p.y_pitch + x] = cv[((y - g.y0) / c * nx + (x - g.x0) / c) * 3];
+            }
+            const int hw = bw >> 1;
+            for (int t = threadIdx.x; t < (rows >> 1) * hw; t += REDACT_THREADS) {
+                const int y = (by0 >> 1) + t / hw, x = (cx0 >> 1) + t % hw;
+                if (covered(2 * x, 2 * y)) continue;
+                const uint8_t *v = cv + ((2 * y - g.y0) / c * nx + (2 * x - g.x0) / c) * 3;
+                const size_t o = (size_t)y * p.uv_pitch + (size_t)x * p.uv_step;
+                p.u[o] = v[1];
+                p.v[o] = v[2];
+            }
+        } else {
+            const BgrRowsW &p = fr.dst;
+            for (int t = threadIdx.x; t < rows * bw; t += REDACT_THREADS) {
+                const int y = by0 + t / bw, x = cx0 + t % bw;
+                if (covered(x, y)) continue;
+                const uint8_t *v = cv + ((y - g.y0) / c * nx + (x - g.x0) / c) * 3;
+                uint8_t *q = p.p + (size_t)y * p.pitch + 3 * (size_t)x;
+                q[0] = v[0];
+                q[1] = v[1];
+                q[2] = v[2];
+            }
+        }
+        __syncthreads();     // s_rect / s_nrect of the next item
+    }
+}
+
+size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
+
+}  // namespace
+
+size_t redact_scratch_bytes(int n, int cap, int blocks) {
+    return align256(sizeof(RedactRegion) * n * cap) + align256(sizeof(int) * 4 * n) + (size_t)n * cap * blocks * blocks * 3;
+}
+
+void redact_carve(RedactArgs &a, void *scratch) {
+    unsigned char *p = static_cast<unsigned char *>(scratch);
+    a.regions = reinterpret_cast<RedactRegion *>(p);
+    p += align256(sizeof(RedactRegion) * a.n * a.cap);
+    a.totals = reinterpret_cast<int *>(p);
+    p += align256(sizeof(int) * 4 * a.n);
+    a.cells = p;
+}
+
+// Two CTAs per SM for measure and apply, as k_align_faces: a batch-8 call has a few hundred items of each.
+template <typename Dst>
+cudaError_t launch_redact(const RedactArgs &a, const RedactFrameT<Dst> *frames, int num_sms, cudaStream_t s) {
+    constexpr int kMax = redact_table_limit<Dst>();
+    const size_t cells = (size_t)a.blocks * a.blocks * 3;
+    for (int i0 = 0; i0 < a.n; i0 += kMax) {
+        const int m = std::min(kMax, a.n - i0);
+        RedactArgs c = a;
+        c.n = m;
+        c.dets = a.dets + (size_t)i0 * a.max_faces;
+        c.counts = a.counts + i0;
+        if (a.tracks) {
+            c.tracks = a.tracks + (size_t)i0 * a.max_tracks;
+            c.track_counts = a.track_counts + i0;
+        }
+        c.regions = a.regions + (size_t)i0 * a.cap;
+        c.totals = a.totals + 4 * i0;
+        c.cells = a.cells + (size_t)i0 * a.cap * cells;
+        RedactTable<Dst> t{};
+        for (int i = 0; i < m; i++) t.f[i] = frames[i0 + i];
+        k_redact_regions<<<m, REDACT_THREADS, 0, s>>>(c, t);
+        k_redact_measure<<<2 * num_sms, REDACT_THREADS, 0, s>>>(c, t);
+        k_redact_apply<<<2 * num_sms, REDACT_THREADS, 0, s>>>(c, t);
+        const cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
+}
+
+template cudaError_t launch_redact<YuvPlanesW>(const RedactArgs &, const RedactFrameT<YuvPlanesW> *, int, cudaStream_t);
+template cudaError_t launch_redact<BgrRowsW>(const RedactArgs &, const RedactFrameT<BgrRowsW> *, int, cudaStream_t);
+
+}  // namespace rf

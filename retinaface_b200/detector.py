@@ -163,6 +163,23 @@ class RetinaFace:
                for i, per in enumerate(recs)]
         return tracks, new
 
+    def redactFrames(self, frames: Sequence, videos: Sequence[int] = None, threshold: float = 0.5, blocks: int = 0, margin: float = 0.0,
+                     layout: str = "nv12", matrix: str = "bt601", max_videos: int = 64):
+        """f12 redaction: detect on device 4:2:0 frames (torch CUDA tensors in ``Engine.detect_yuv_device``'s forms) and mosaic every
+        detected face IN PLACE (rf_detect_yuv_redact_device), ``blocks`` cells across a region's longer side (0: 8; 1: a flat patch),
+        each side grown by ``margin`` of the box (0: 0.25).  With ``videos`` (frame i of video ``videos[i]``) the frames are also
+        tracked, on this detector's plain tracker (created as ``trackFrames`` creates it), and the predicted box of every face the
+        tracker still follows while the detector misses it is redacted too.  Asynchronous: the frames are complete in stream order on
+        ``engine.last_stream_ptr()``."""
+        if videos is None:
+            self.engine.detect_yuv_redact_device(list(frames), threshold, self.nms_threshold, layout=layout, matrix=matrix, blocks=blocks,
+                                                 margin=margin)
+            return
+        if getattr(self, "_tracker", None) is None:
+            self._tracker = self.engine.tracker(max_videos=max_videos)
+        self._tracker.detect_yuv_redact_device(list(frames), list(videos), threshold, self.nms_threshold, layout=layout, matrix=matrix,
+                                               blocks=blocks, margin=margin)
+
     def _best_crops(self, n: int):
         import torch
         from .capi import CROP_FORMATS, crop_shape

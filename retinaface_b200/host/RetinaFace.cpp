@@ -305,6 +305,29 @@ void RetinaFace::trackYUV(const vector<rf_yuv_frame> &device_frames, const vecto
     tracks_.max_tracks = 64;      // rf_track_config's default
 }
 
+void RetinaFace::redactYUV(const vector<rf_yuv_frame> &device_frames, const vector<int> *videos, float threshold, const RedactOptions &opt) {
+    if (videos && videos->size() != device_frames.size()) throw std::invalid_argument("redactYUV: one video index per frame");
+    if (device_frames.size() > (size_t)opt_.max_batch) throw std::invalid_argument("redactYUV: at most max_batch frames per call");
+    if (videos && best_tracker_) throw std::logic_error("redactYUV: this RetinaFace tracks with best shots (trackYUVBest)");
+    if (videos && !tracker_) {
+        rf_track_config tc{};
+        tc.max_videos = opt_.track_videos;
+        int rc = rf_tracker_create(h_, &tc, &tracker_);
+        if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_create: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+    }
+    const rf_redact_params p{opt.blocks, opt.margin};
+    const int n = (int)device_frames.size();
+    DeviceTracks t{};
+    int rc = rf_detect_yuv_redact_device(h_, videos ? tracker_ : nullptr, device_frames.data(), videos ? videos->data() : nullptr, n, RF_YUV_BT601,
+                                         threshold, nms_threshold, &p, &t.tracks, &t.counts, nullptr, nullptr, nullptr);
+    if (rc != RF_OK) throw std::runtime_error(string("rf_detect_yuv_redact_device: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+    if (videos) {
+        tracks_ = t;
+        tracks_.n = n;
+        tracks_.max_tracks = 64;      // rf_track_config's default
+    }
+}
+
 void RetinaFace::trackYUVBest(const vector<rf_yuv_frame> &device_frames, const vector<int> &videos, void *dev_best_crops, float threshold,
                               float min_quality) {
     if (videos.size() != device_frames.size()) throw std::invalid_argument("trackYUVBest: one video index per frame");

@@ -51,6 +51,12 @@ struct AlignOptions {
     int max_faces = 0;                   // crops per image, best score first; 0: every kept face
 };
 
+// f12 redaction (rf_detect_yuv_redact_device): the mosaic written over every face
+struct RedactOptions {
+    int blocks = 8;                      // cells across a region's longer side, 1..32 (1: one flat patch)
+    float margin = 0.25f;                // each side of a box grows by margin x its side, (0, 1]
+};
+
 class RetinaFace {
    public:
     RetinaFace(string &model, string network = "net3", float nms = 0.4, const RetinaFaceOptions &opt = RetinaFaceOptions());
@@ -127,6 +133,12 @@ class RetinaFace {
                       float min_quality = 0.f);
     const DeviceBestShots &lastBestShots() const { return best_; }
     void finishVideo(int video, void *dev_best_crops);
+    // f12 redaction (rf_detect_yuv_redact_device): detect on DEVICE 4:2:0 frames and mosaic every detected face in place, on the
+    // GPU; asynchronous on rf_last_stream(handle()).  With `videos` (one per frame, in [0, track_videos)) the frames are also tracked on
+    // this RetinaFace's plain tracker (trackYUV's), lastTracks() holds the lists, and the predicted box of every LOST track -- a face the
+    // detector missed on this frame -- is redacted too.
+    void redactYUV(const vector<rf_yuv_frame> &device_frames, const vector<int> *videos = nullptr, float threshold = 0.5,
+                   const RedactOptions &opt = RedactOptions());
     rf_handle handle() const { return h_; }
     // the reference's visualisation (RetinaFace.cpp:730-741): red box outline (thickness 2), green landmark dots, on a clone
     static Mat draw(const Mat &img, const vector<FaceDetectInfo> &faces);

@@ -36,3 +36,14 @@ def s_real_batch(base: np.ndarray, batch: int) -> np.ndarray:
 def s_noise_batch(batch: int, net_h: int, net_w: int, seed: int = 0) -> np.ndarray:
     """S-noise (SURVEY.md 8d): uniform random u8, ~0 detections."""
     return np.random.default_rng(seed).integers(0, 256, (batch, net_h, net_w, 3), dtype=np.uint8)
+
+
+def mixed_batch(photo: np.ndarray, n: int, net_h: int, net_w: int, start: int = 0) -> np.ndarray:
+    """Neighbours as dissimilar as possible (the letter-boxed photo, noise, all-255, all-0, a rolled copy, a mirrored copy,
+    other noise, an upside-down copy, cycled from `start`): a tile that reads the wrong image or a stale buffer changes
+    bytes, and no two of any 8 consecutive images are the same."""
+    inp = letterbox_bgr_u8(photo, net_h, net_w)
+    noise = s_noise_batch(2, net_h, net_w, seed=21)
+    pool = [inp, noise[0], np.full((net_h, net_w, 3), 255, np.uint8), np.zeros((net_h, net_w, 3), np.uint8),
+            np.roll(inp, 37, axis=1), np.ascontiguousarray(inp[:, ::-1]), noise[1], np.ascontiguousarray(inp[::-1])]
+    return np.stack([pool[(start + i) % len(pool)] for i in range(n)])

@@ -75,6 +75,23 @@ class PostprocOracle:
         return dict(cand=cand[:n].copy(), cand_idx=cand_idx[:n].copy(),
                     faces=out[:kept].copy(), idx=out_idx[:kept].copy())
 
+    def check_engine(self, eng, batch, heads, thr: float, nms_thr: float, label: str = "") -> int:
+        """An engine's detections of `batch` against this post-process of the engine's own `heads`: selection (anchor
+        indices, order) exact, scores and landmarks bit-exact, box corners within 4e-6 relative (the exp() rounding noted in
+        postproc.cu).  Returns the number of faces compared."""
+        h, w = batch.shape[1:3]
+        faces, idx = eng.detect_batch(list(batch), thr, nms_thr, want_index=True)
+        for i in range(len(batch)):
+            ref = self.postprocess([x[i] for x in heads], h, w, thr, nms_thr)
+            lab = f"{label} image {i}"
+            assert idx[i].tolist() == ref["idx"].tolist(), lab
+            assert faces[i].shape == ref["faces"].shape, lab
+            if len(faces[i]):
+                assert np.array_equal(faces[i][:, 0], ref["faces"][:, 0]), lab
+                assert np.array_equal(faces[i][:, 5:], ref["faces"][:, 5:]), lab
+                assert np.allclose(faces[i][:, 1:5], ref["faces"][:, 1:5], rtol=4e-6, atol=1e-4), lab
+        return sum(len(f) for f in faces)
+
     def nms(self, cands: np.ndarray, thr: float):
         cands = np.ascontiguousarray(cands, dtype=np.float32).reshape(-1, FACE_FLOATS)
         n = cands.shape[0]

@@ -20,7 +20,7 @@ import pytest
 
 from conftest import GOLDEN, caffemodel
 from oracle import topology
-from oracle.inputs import letterbox_bgr_u8, s_noise_batch
+from oracle.inputs import letterbox_bgr_u8, mixed_batch
 from oracle.mnet_int8 import Int8Oracle, int_gemm, read_table
 from retinaface_b200.capi import RF_FLAG_DW_1D, RF_FLAG_SIMT_STEM, RF_PREC_INT8
 
@@ -64,16 +64,7 @@ SATURATION_FLOOR = {STEM: 0.15, "rf_c3_det_concat_relu": 0.04, "rf_c2_det_concat
 SATURATED_TENSORS = 24
 
 
-# ---- inputs and tables --------------------------------------------------------------------------------------------------
-def mixed_batch(photo, n, h, w, start=0):
-    """Neighbours as dissimilar as possible (the photo, noise, all-255, all-0, a rolled and a flipped copy, cycled from
-    `start`): a tile that reads the wrong image or a stale buffer changes bytes."""
-    inp = letterbox_bgr_u8(photo, h, w)
-    pool = [inp, s_noise_batch(1, h, w, seed=21)[0], np.full((h, w, 3), 255, np.uint8), np.zeros((h, w, 3), np.uint8),
-            np.roll(inp, 37, axis=1), np.ascontiguousarray(inp[:, ::-1])]
-    return np.stack([pool[(start + i) % len(pool)] for i in range(n)])
-
-
+# ---- tables -------------------------------------------------------------------------------------------------------------
 def write_table(path, scales):
     """TensorRT's EntropyCalibration2 cache format: '<tensor>: <big-endian float32 hex>' per line."""
     with open(path, "w") as f:
@@ -124,30 +115,11 @@ def _engine(case, table, keep_all):
 
 
 # ---- comparisons ------------------------------------------------------------------------------------------------------
-def compare_dets(mine, mine_idx, ref, label):
-    """Selection (anchor indices, order) exact; scores and landmarks bit-exact; box corners within 4e-6 relative (the exp()
-    rounding noted in postproc.cu)."""
-    assert mine_idx.tolist() == ref["idx"].tolist(), label
-    assert mine.shape == ref["faces"].shape, label
-    if len(mine):
-        assert np.array_equal(mine[:, 0], ref["faces"][:, 0]), label
-        assert np.array_equal(mine[:, 5:], ref["faces"][:, 5:]), label
-        assert np.allclose(mine[:, 1:5], ref["faces"][:, 1:5], rtol=4e-6, atol=1e-4), label
-
-
 def first_difference(name, got, want):
     bad = got != want
     b, c, y, x = np.argwhere(bad)[0]
     return (f"{name}: first difference at (image {b}, channel {c}, y {y}, x {x}): engine {got[b, c, y, x]:.0f}, oracle "
             f"{want[b, c, y, x]}; {bad.mean():.4%} of the bytes differ")
-
-
-def check_dets(eng, batch, heads, post, label):
-    h, w = batch.shape[1:3]
-    faces, idx = eng.detect_batch(list(batch), THR, NMS, want_index=True)
-    for i in range(len(batch)):
-        compare_dets(faces[i], idx[i], post.postprocess([x[i] for x in heads], h, w, THR, NMS), f"{label} image {i}")
-    return sum(len(f) for f in faces)
 
 
 _ATTEMPTED, _MERGE = set(), {}
@@ -206,12 +178,12 @@ def test_int8_engine_bit_exact_vs_integer_oracle(case_id, golden_image, tables, 
                 assert sum(f > 0 for f in frac.values()) >= SATURATED_TENSORS, (label, frac)
             for k in range(9):
                 assert np.abs(heads[k] - o_heads[k]).max() < 1e-4, (label, k, np.abs(heads[k] - o_heads[k]).max())
-            found = check_dets(keep, batch, heads, post_oracle, label)
+            found = post_oracle.check_engine(keep, batch, heads, THR, NMS, label)
             assert found > 0 or not case.faces, label       # the selection and order compared are not empty
             if prod is not None:
                 # production placement: tensors share memory across the three lanes; heads bit-equal, detections exact
                 heads_p = prod.forward_heads(batch)
-                faces_p = check_dets(prod, batch, heads_p, post_oracle, label + " (liveness placement)")
+                faces_p = post_oracle.check_engine(prod, batch, heads_p, THR, NMS, label + " (liveness placement)")
                 for k in range(9):
                     assert np.array_equal(heads_p[k], heads[k]), (label, "liveness placement", k)
                 assert faces_p == found, label

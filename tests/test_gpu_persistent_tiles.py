@@ -7,21 +7,11 @@ import numpy as np
 import pytest
 
 from conftest import GOLDEN, caffemodel
-from oracle.inputs import letterbox_bgr_u8, s_noise_batch
+from oracle.inputs import mixed_batch
 
 pytestmark = pytest.mark.gpu
 
 HEAD_NAMES = ("mobilenet0_relu4_fwd", "mobilenet0_relu6_fwd", "mobilenet0_relu8_fwd", "mobilenet0_relu10_fwd")
-
-
-def _mixed_batch(photo, n, h, w):
-    """Neighbouring images that differ as much as possible (noise, all-255, the photo, black), so that a tile computed from a
-    stale staging buffer -- the previous tile's, possibly the previous image's -- cannot go unnoticed."""
-    inp = letterbox_bgr_u8(photo, h, w)
-    noise = s_noise_batch(2, h, w, seed=11)
-    pool = [noise[0], np.full((h, w, 3), 255, np.uint8), inp, np.zeros((h, w, 3), np.uint8), np.roll(inp, 37, axis=1),
-            noise[1], np.ascontiguousarray(inp[::-1]), np.full((h, w, 3), 255, np.uint8)]
-    return np.stack([pool[i % len(pool)] for i in range(n)])
 
 
 def _engine(prec, h, w, batch, flags=0):
@@ -40,7 +30,7 @@ def test_persistent_2d_tiles_equal_the_1d_kernels(hw, batch, golden_image):
     dw3..dw11; 416x288 leaves partial 2-D tiles on its 104-wide map."""
     from retinaface_b200.capi import RF_FLAG_DW_1D
     h, w = hw
-    batch_u8 = _mixed_batch(golden_image, batch, h, w)
+    batch_u8 = mixed_batch(golden_image, batch, h, w)
     a, b = _engine("fp16", h, w, batch), _engine("fp16", h, w, batch, flags=RF_FLAG_DW_1D)
     try:
         a.debug_keep_all()
@@ -62,7 +52,7 @@ def test_persistent_tiles_batch_equals_each_image_alone(prec, hw, golden_image):
     what it gives forwarded alone: a CTA's run of tiles crosses image boundaries in the batch, never alone."""
     h, w = hw
     n = 8
-    batch_u8 = _mixed_batch(golden_image, n, h, w)
+    batch_u8 = mixed_batch(golden_image, n, h, w)
     names = ["mobilenet0_relu2_fwd"] + (["mobilenet0_relu6_fwd"] if prec == "fp16" else [])
     eng = _engine(prec, h, w, n)
     try:

@@ -536,6 +536,76 @@ int  rf_detect_yuv_track_device(rf_handle h, rf_tracker t, const rf_yuv_frame *f
 #define RF_TRACK_DEBUG_DOUBLES 25
 int  rf_tracker_debug_state(rf_tracker t, int video, double *out, int cap);
 
+/* f13 camera-motion compensation: a tracker that has the frames estimates each frame's global motion from the previous frame of
+ * the same video and moves every track with it before association, so that a pan, a shake or a zoom does not break the ids (BoT-SORT's
+ * global motion compensation, here deterministic and on the GPU).  Per frame the estimate is a similarity in frame pixels from the
+ * previous frame to this one, x' = a x - b y + tx, y' = b x + a y + ty, computed from luma alone (NV12, NV21, I420 and YV12 give the
+ * same result), every FP64 step one rounding in the order written (oracle/motion.py restates it):
+ *   1. thumbnail  D = ceil(max(W, H) / RF_MOTION_THUMB); tw = W / D, th = H / D (a partial last row / column of boxes is dropped);
+ *                 thumb(x, y) = (sum of the D x D luma box at (D x, D y) + D*D / 2) / (D*D), integers.
+ *   2. blocks     RF_MOTION_BLOCK-square blocks at (R + 16 i, R + 16 j) for every block that fits inside the thumbnail inset by the
+ *                 search radius R, numbered row by row.  A block is skipped when 256 sum(p^2) - (sum p)^2 < RF_MOTION_MIN_VAR * 65536
+ *                 (flat: walls, sky), or when it overlaps a record of this frame: the record's box (x1..y2 = __fmul_rn(coordinate,
+ *                 scale), widened to double; w = x2 - x1, h = y2 - y1) grown by RF_MOTION_FACE_MARGIN * w (h) on each side, against
+ *                 the block's frame rectangle [D x0, D (x0 + 16)) x [D y0, D (y0 + 16)): gx1 < X1 && gx2 > X0 && gy1 < Y1 && gy2 > Y0.
+ *   3. match      SAD(dy, dx) = sum |cur(x0 + c, y0 + r) - ref(x0 + dx + c, y0 + dy + r)| over |dx|, |dy| <= R; the minimum under
+ *                 the order (SAD, |dy| + |dx|, dy, dx).  The block is dropped when another offset has the same SAD or the minimum lies
+ *                 on the search border.  Sub-pixel: f = (S(-1) - S(+1)) / (2 (S(-1) - 2 S(0) + S(+1))) per axis (integers, one
+ *                 division).  The block gives the point pair p = (x0 + 7.5, y0 + 7.5) in this frame and q = ((px + dx) + fx,
+ *                 (py + dy) + fy) in the previous one.
+ *   4. fit        N kept blocks in block order (N < min_inliers: LOST).  Hypotheses h in [0, N + N / 2): h < N the translation
+ *                 p_h - q_h of block h alone; h = N + k the exact similarity of blocks k and k + N / 2: dq = q2 - q1, dp = p2 - p1,
+ *                 den = dqx dqx + dqy dqy (0: no inliers), a = (dpx dqx + dpy dqy) / den, b = (dpy dqx - dpx dqy) / den,
+ *                 tx = px1 - (a qx1 - b qy1), ty = py1 - (b qx1 + a qy1).  Point k is an inlier of (a, b, tx, ty) when
+ *                 ex = ((a qx - b qy) + tx) - px, ey = ((b qx + a qy) + ty) - py have ex ex + ey ey <= RF_MOTION_TOL^2.  The
+ *                 hypothesis with the most inliers wins, ties to the lower h.  Its inliers (fewer than min_inliers: LOST) are refitted
+ *                 by least squares, the centred closed form of the align fit: means m = S(v) / n, u = q - mq, v = p - mp,
+ *                 den = S(ux ux + uy uy) (0: LOST), a = S(ux vx + uy vy) / den, b = S(ux vy - uy vx) / den, tx = (mpx - a mqx) + b mqy,
+ *                 ty = (mpy - b mqx) - a mqy; then the inliers of that fit are selected once more (fewer than min_inliers: LOST) and
+ *                 refitted once more.  S sums in 32 lanes -- lane l adds the terms l, l + 32, ... of the inlier list in order -- then
+ *                 lane l += lane l + o for o = 16, 8, 4, 2, 1; the result is lane 0.
+ *   5. frame      c = (D - 1) / 2: a and b stay, tx' = ((D tx) + c) - ((a c) - (b c)), ty' = ((D ty) + c) - ((b c) + (a c)).
+ *   6. status     RF_MOTION_FIRST: no reference (the first frame since create / reset, or the frame size changed);
+ *                 RF_MOTION_LOST: too few blocks or inliers, a degenerate fit, or s = sqrt(a a + b b) outside
+ *                 [RF_MOTION_MIN_SCALE, RF_MOTION_MAX_SCALE] (scene cuts, flat frames); RF_MOTION_OK otherwise.  FIRST and LOST
+ *                 report the identity and move nothing.
+ * Compensation, after predict and before the first association stage, on every live track of an RF_MOTION_OK frame, with
+ * s = sqrt(a a + b b) and ss = s * s:  cx = ((a cx) - (b cy)) + tx;  cy = ((b cx) + (a cy)) + ty  (old cx, cy on the right);
+ * u_cx, u_cy likewise without t;  h = s h;  u_h = s u_h;  a and u_a stay;  P00, P01, P11 = ss * P for cx, cy and h.  This is
+ * A8 P A8^T of ByteTrack's 8 x 8 filter exactly: the cx and cy filters are born with the same covariance and take the same steps,
+ * so their covariances are equal bit for bit and a rotation keeps the four scalar filters decoupled.  After compensation rf_track.vx
+ * and .vy are the face's motion relative to the scene, not to the frame. */
+#define RF_MOTION_OK    0
+#define RF_MOTION_FIRST 1
+#define RF_MOTION_LOST  2
+#define RF_MOTION_THUMB 320              /* the thumbnail's longer side is at most this */
+#define RF_MOTION_BLOCK 16
+#define RF_MOTION_MIN_VAR 16             /* texture floor: the block's luma variance, thumbnail levels squared */
+#define RF_MOTION_FACE_MARGIN 0.5        /* records grow by this fraction of their size on each side */
+#define RF_MOTION_TOL 1.0                /* inlier distance, thumbnail pixels */
+#define RF_MOTION_MIN_SCALE 0.8
+#define RF_MOTION_MAX_SCALE 1.25
+typedef struct rf_motion_config {
+    int search;                      /* R, thumbnail pixels: 0 -> 12 (about 72 frame pixels per frame at 1080p), else 1..32 */
+    int min_inliers;                 /* 0 -> 12, else 3..361 */
+} rf_motion_config;
+typedef struct rf_motion {
+    int32_t status;                  /* RF_MOTION_* */
+    int32_t blocks, inliers, reserved;   /* blocks kept (step 4's N), inliers of the last selection */
+    double m[6];                     /* {a, -b, tx, b, a, ty}, frame pixels, previous frame -> this one (the align matrices' layout) */
+} rf_motion;
+/* Turns motion compensation on for a plain or best-shot tracker, before its first update (afterwards, or a bad config:
+ * RF_ERR_INVALID_ARG).  Allocates a reference store of max_videos thumbnails of RF_MOTION_THUMB^2 bytes (above 4 GiB:
+ * RF_ERR_CAPACITY).  The frames are then estimated by rf_detect_yuv_track_device, rf_detect_yuv_track_best_device and
+ * rf_detect_yuv_redact_device, on the forward's context inside the tracker's event chain: thumbnails, match, fit, the update, then
+ * each video's last thumbnail of the call becomes its reference.  Frame k of a video is matched against that video's previous
+ * frame of the same call, the first one against the reference.  rf_track_update, which has no pixels, refuses a motion tracker;
+ * rf_tracker_reset and rf_tracker_finish drop the video's reference. */
+int rf_tracker_set_motion(rf_tracker t, const rf_motion_config *cfg);
+/* *dev_motion -> the [n] rf_motion of the tracker's latest frame call (NULL before the first), in the ring slot of its track lists:
+ * valid for `streams` further tracker calls.  RF_ERR_INVALID_ARG on a tracker without motion. */
+int rf_tracker_motion(rf_tracker t, const rf_motion **dev_motion);
+
 /* f11 best shots: the best crop of every tracked face, kept on the GPU, and one crop per identity when its track ends -- the view a
  * recogniser should see, instead of the track's second detection (f10's new-identity crop), which is usually a face entering the
  * frame: at its edge, small, turned or blurred.

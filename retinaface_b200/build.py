@@ -29,6 +29,7 @@ SOURCES = [
     ("track.cu", ["-fmad=false"]),      # the tracker's FP64 Kalman filter and IoU: every step one rounding, as oracle/track.py states it
     ("best.cu", ["-fmad=false"]),       # the crop warp of align.cu and the FP64 face quality, as oracle/bestshot.py states it
     ("redact.cu", ["-fmad=false"]),     # the FP64 region geometry, as oracle/redact.py states it
+    ("motion.cu", ["-fmad=false"]),     # the FP64 sub-pixel match and similarity fit, as oracle/motion.py states it
     ("calibrate.cu", []),
     ("model.cpp", []),
     ("frontend.cpp", []),

@@ -34,6 +34,7 @@ EXPORTS = [
     "rf_detect_views_oriented", "rf_jpeg_exif_orientation",
     "rf_tracker_create", "rf_tracker_destroy", "rf_tracker_reset", "rf_track_update", "rf_detect_yuv_track_device", "rf_tracker_debug_state",
     "rf_tracker_create_best", "rf_detect_yuv_track_best_device", "rf_tracker_finish",
+    "rf_tracker_set_motion", "rf_tracker_motion",
     "rf_redact_yuv_device", "rf_redact_device", "rf_detect_yuv_redact_device",
 ]
 COMM_BLOB_BYTES = 128
@@ -232,6 +233,24 @@ BEST_DTYPE = np.dtype([(f, "<i4") for f in ("id", "video", "frame", "end_frame",
                       [(f, "<f4") for f in ("quality", "score", "eye", "frontal", "sharpness", "coverage")] + [("face", "<f4", (FACE_FLOATS,))])
 
 
+class MotionConfig(C.Structure):  # rf_motion_config
+    _fields_ = [("search", C.c_int), ("min_inliers", C.c_int)]
+
+
+def motion_config(search: int = 0, min_inliers: int = 0) -> MotionConfig:
+    """rf_motion_config: search radius R in thumbnail pixels (0 -> 12), min_inliers (0 -> 12)."""
+    return MotionConfig(int(search), int(min_inliers))
+
+
+class Motion(C.Structure):       # rf_motion
+    _fields_ = [(f, C.c_int32) for f in ("status", "blocks", "inliers", "reserved")] + [("m", C.c_double * 6)]
+
+
+MOTION_OK, MOTION_FIRST, MOTION_LOST = 0, 1, 2               # RF_MOTION_*
+# one rf_motion as a numpy record (the layout of Motion)
+MOTION_DTYPE = np.dtype([(f, "<i4") for f in ("status", "blocks", "inliers", "reserved")] + [("m", "<f8", (6,))])
+
+
 class RedactParams(C.Structure):  # rf_redact_params
     _fields_ = [("blocks", C.c_int), ("margin", C.c_float)]
 
@@ -369,6 +388,8 @@ def load_library() -> C.CDLL:
     lib.rf_detect_yuv_track_best_device.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(YuvFrame), C.c_void_p, C.c_int, C.c_int, C.c_float,
                                                     C.c_float, C.c_void_p, C.c_void_p] + [C.POINTER(C.c_void_p)] * 6 + [C.c_void_p]
     lib.rf_tracker_finish.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
+    lib.rf_tracker_set_motion.argtypes = [C.c_void_p, C.POINTER(MotionConfig)]
+    lib.rf_tracker_motion.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
     lib.rf_redact_yuv_device.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.POINTER(RedactParams)]
     lib.rf_redact_device.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int,
@@ -1032,11 +1053,21 @@ class Engine:
 
     # -- f10 face tracking across video frames ---------------------------------------------------------------------------------
     def tracker(self, max_videos: int = 1, max_tracks: int = 0, high_thresh: float = 0.0, new_thresh: float = 0.0, iou_high: float = 0.0,
-                iou_low: float = 0.0, iou_tentative: float = 0.0, max_lost: int = 0, best: Optional[dict] = None) -> "Tracker":
+                iou_low: float = 0.0, iou_tentative: float = 0.0, max_lost: int = 0, best: Optional[dict] = None,
+                motion=None) -> "Tracker":
         """rf_tracker_create: a tracker of max_videos independent sequences on this engine (0 -> the defaults of rf_track_config).
-        best (``best_config`` keywords): a best-shot tracker (rf_tracker_create_best), fed through ``Tracker.detect_yuv_best_device``."""
-        return Tracker(self, TrackConfig(max_videos, max_tracks, high_thresh, new_thresh, iou_high, iou_low, iou_tentative, max_lost),
-                       best_config(**best) if best is not None else None)
+        best (``best_config`` keywords): a best-shot tracker (rf_tracker_create_best), fed through ``Tracker.detect_yuv_best_device``.
+        motion (True or ``motion_config`` keywords): camera-motion compensation (rf_tracker_set_motion) from the frames of the
+        detect_yuv_* calls; read each call's estimates with ``Tracker.motion``."""
+        t = Tracker(self, TrackConfig(max_videos, max_tracks, high_thresh, new_thresh, iou_high, iou_low, iou_tentative, max_lost),
+                    best_config(**best) if best is not None else None)
+        if motion:
+            try:
+                t.set_motion(**(motion if isinstance(motion, dict) else {}))
+            except Exception:
+                t.close()
+                raise
+        return t
 
     # -- f12 redaction ---------------------------------------------------------------------------------------------------------
     @staticmethod
@@ -1134,6 +1165,7 @@ class Tracker:
             engine._check(self.lib.rf_tracker_create_best(engine.h, C.byref(cfg), C.byref(best), C.byref(t)))
         self.t = t
         self.best = best
+        self.motion_on = False
         self.max_videos = cfg.max_videos
         self.max_tracks = cfg.max_tracks or 64
 
@@ -1223,6 +1255,23 @@ class Tracker:
         raw = torch.as_tensor(_DevArray(best_ptr, (n, self.max_tracks * BEST_DTYPE.itemsize), "|u1"), device="cuda").cpu().numpy()
         counts = torch.as_tensor(_DevArray(counts_ptr, (n,), "<i4"), device="cuda").cpu().numpy()
         return [raw[i].view(BEST_DTYPE)[:counts[i]].copy() for i in range(n)]
+
+    def set_motion(self, search: int = 0, min_inliers: int = 0):
+        """rf_tracker_set_motion, before the first update."""
+        cfg = motion_config(search, min_inliers)
+        self.engine._check(self.lib.rf_tracker_set_motion(self.t, C.byref(cfg)))
+        self.motion_on = True
+
+    def motion(self, n: int) -> np.ndarray:
+        """rf_tracker_motion: the n rf_motion records (MOTION_DTYPE) of the latest frame call, copied after the last stream."""
+        import torch
+        p = C.c_void_p()
+        self.engine._check(self.lib.rf_tracker_motion(self.t, C.byref(p)))
+        if not p.value:
+            raise RuntimeError("no frame call has been made on this tracker")
+        self.engine._check(self.lib.rf_synchronize(self.engine.h))
+        raw = torch.as_tensor(_DevArray(int(p.value), (n * MOTION_DTYPE.itemsize,), "|u1"), device="cuda").cpu().numpy()
+        return raw.view(MOTION_DTYPE).copy()
 
     def reset(self, video: int = -1):
         """rf_tracker_reset: restart one video (ids from 1), or all with -1; ordered after every issued update."""

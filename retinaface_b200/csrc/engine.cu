@@ -13,6 +13,7 @@
 #include "best.cuh"
 #include "redact.cuh"
 #include "track.cuh"
+#include "motion.cuh"
 
 namespace rf_eng {
 
@@ -1853,6 +1854,7 @@ struct rf_tracker_s {
         int *counts = nullptr;         // [max_batch]
         rf_det *due = nullptr;         // [max_batch][max_faces]
         int *due_counts = nullptr;     // [max_batch]
+        rf_motion *motion = nullptr;   // [max_batch] f13, with motion on
         cudaEvent_t free = nullptr;
     };
     std::vector<Slot> slots;
@@ -1864,14 +1866,26 @@ struct rf_tracker_s {
     BestArgs ba{};                     // store, per-video counters, per-call tables, formats (per-call pointers set per call)
     rf_best_shot *d_best = nullptr;    // [slots][max_batch][max_tracks]
     int *d_best_counts = nullptr;      // [slots][max_batch]
+    bool updated = false;              // a frame call was issued (rf_tracker_set_motion comes before)
+    // f13 camera motion (motion.cuh); `motion` false: none of these allocated.  mref mirrors on the host what each video's
+    // reference slot holds (the frame size it came from, 0 x 0: none): calls, resets and finishes are issued in host order, so the
+    // reference of every frame is known when the call is issued.  The chain orders the per-call scratch as it orders f11's tables.
+    bool motion = false;
+    rf_motion_config mcfg{};
+    uint8_t *d_mstore = nullptr;       // [max_videos][MOTION_THUMB_BYTES]
+    uint8_t *d_mthumbs = nullptr;      // [max_batch][MOTION_THUMB_BYTES]
+    MotionBlock *d_mblocks = nullptr;  // [max_batch][MOTION_MAX_BLOCKS]
+    std::vector<std::array<int, 2>> mref;
+    int motion_slot = -1;              // the ring slot of the latest frame call
 };
 
 static void tracker_release(rf_tracker t) {
     if (t->chain) cudaEventSynchronize(t->chain);
     for (auto &s : t->slots) {
         if (s.free) { cudaEventSynchronize(s.free); cudaEventDestroy(s.free); }
-        cudaFree(s.tracks); cudaFree(s.counts); cudaFree(s.due); cudaFree(s.due_counts);
+        cudaFree(s.tracks); cudaFree(s.counts); cudaFree(s.due); cudaFree(s.due_counts); cudaFree(s.motion);
     }
+    cudaFree(t->d_mstore); cudaFree(t->d_mthumbs); cudaFree(t->d_mblocks);
     if (t->chain) cudaEventDestroy(t->chain);
     cudaFree(t->d_videos); cudaFree(t->d_state); cudaFree(t->d_pairs); cudaFree(t->d_order);
     const BestArgs &b = t->ba;
@@ -1949,6 +1963,7 @@ int rf_tracker_reset(rf_tracker t, int video) {
             CK(cudaMemsetAsync(t->ba.store + v0 * T, 0, sizeof(BestEntry) * nv * T, s));
             CK(cudaMemsetAsync(t->ba.videos + v0, 0, sizeof(BestVideo) * nv, s));
         }
+        for (size_t v = v0; t->motion && v < v0 + nv; v++) t->mref[v] = {0, 0};
         CK(cudaEventRecord(t->chain, s));
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
@@ -1969,15 +1984,90 @@ static int check_track_args(rf_tracker t, const char *who, const int *videos, in
     return RF_OK;
 }
 
+// ---- f13 camera motion (motion.cuh) ---------------------------------------------------------------------------------------------
+// Each video's last frame of a call, whose thumbnail becomes the video's reference once the update has run.
+struct MotionCommits {
+    std::vector<int> frames, videos, bytes;
+};
+
+// The estimate of the call's n frames into ring slot `ring`'s motions, on s inside the chain: each frame's reference is the
+// previous frame of its video in this call, else the video's stored thumbnail, else none (FIRST); a frame size change is none.
+static void motion_issue(rf_tracker t, unsigned ring, const rf_yuv_frame *frames, const int *videos, int n, const rf_det *dets,
+                         const int32_t *counts, const float *scales, cudaStream_t s, MotionCommits &commits) {
+    const int R = t->mcfg.search;
+    std::vector<MotionTable> tabs;
+    std::vector<std::array<int, 2>> last;          // (video, its latest frame of the call)
+    for (int i = 0; i < n; i++) {
+        if (i % TRACK_MAX_FRAMES == 0) {
+            tabs.emplace_back();
+            tabs.back().i0 = i;
+        }
+        MotionTable &tb = tabs.back();
+        MotionFrame &f = tb.f[tb.n++];
+        const rf_yuv_frame &fr = frames[i];
+        const int v = videos[i];
+        f.y = fr.y;
+        f.pitch = fr.y_pitch;
+        f.video = v;
+        f.scale = scales ? scales[i] : 1.f;
+        f.D = (std::max(fr.width, fr.height) + MOTION_THUMB - 1) / MOTION_THUMB;
+        f.tw = fr.width / f.D;
+        f.th = fr.height / f.D;
+        f.nbx = f.tw - 2 * R >= MOTION_BLOCK ? (f.tw - 2 * R) / MOTION_BLOCK : 0;
+        f.nby = f.th - 2 * R >= MOTION_BLOCK ? (f.th - 2 * R) / MOTION_BLOCK : 0;
+        auto it = std::find_if(last.begin(), last.end(), [v](const std::array<int, 2> &e) { return e[0] == v; });
+        const std::array<int, 2> size = {fr.width, fr.height};
+        if (it != last.end()) {
+            const rf_yuv_frame &p = frames[(*it)[1]];
+            f.ref = p.width == fr.width && p.height == fr.height ? (*it)[1] : MOTION_REF_FIRST;
+            (*it)[1] = i;
+        } else {
+            f.ref = t->mref[v] == size ? MOTION_REF_STORE : MOTION_REF_FIRST;
+            last.push_back({v, i});
+        }
+    }
+    for (const auto &e : last) {
+        const rf_yuv_frame &fr = frames[e[1]];
+        const MotionFrame &f = tabs[e[1] / TRACK_MAX_FRAMES].f[e[1] % TRACK_MAX_FRAMES];
+        t->mref[e[0]] = {fr.width, fr.height};
+        commits.frames.push_back(e[1]);
+        commits.videos.push_back(e[0]);
+        commits.bytes.push_back(f.tw * f.th);
+    }
+    MotionArgs a{};
+    a.thumbs = t->d_mthumbs;
+    a.store = t->d_mstore;
+    a.blocks = t->d_mblocks;
+    a.out = t->slots[ring].motion;
+    a.dets = dets;
+    a.counts = counts;
+    a.max_faces = t->h->cfg.max_faces;
+    a.search = R;
+    a.min_inliers = t->mcfg.min_inliers;
+    CK(launch_motion_estimate(a, tabs.data(), (int)tabs.size(), s));
+    t->motion_slot = (int)ring;
+}
+
+static void motion_commit(rf_tracker t, const MotionCommits &c, cudaStream_t s) {
+    MotionArgs a{};
+    a.thumbs = t->d_mthumbs;
+    a.store = t->d_mstore;
+    CK(launch_motion_commit(a, c.frames.data(), c.videos.data(), c.bytes.data(), (int)c.frames.size(), s));
+}
+
 // Issues the update of n frames on s (the records complete there) into the next ring slot, ordered by the chain.  `a` (crops):
 // the due faces are cut on s into a's crops, then the slot's `free` is recorded.
 static void track_issue(rf_tracker t, const int *videos, int n, const rf_det *dets, const int32_t *counts, const float *scales, cudaStream_t s,
                         const AlignArgs *a, const AlignImageT<YuvPlanes> *table, const rf_track **dev_tracks,
-                        const int32_t **dev_track_counts) {
+                        const int32_t **dev_track_counts, const rf_yuv_frame *frames) {
     rf_handle h = t->h;
-    rf_tracker_s::Slot &slot = t->slots[t->next_slot++ % t->slots.size()];
+    const unsigned ring = t->next_slot++ % t->slots.size();
+    rf_tracker_s::Slot &slot = t->slots[ring];
     CK(cudaStreamWaitEvent(s, slot.free, 0));
     CK(cudaStreamWaitEvent(s, t->chain, 0));
+    t->updated = true;
+    MotionCommits commits;
+    if (t->motion) motion_issue(t, ring, frames, videos, n, dets, counts, scales, s, commits);
     TrackArgs ta{};
     ta.p = TrackParams{t->cfg.max_tracks, h->cfg.max_faces, t->cfg.max_lost, t->cfg.high_thresh, t->cfg.new_thresh, t->cfg.iou_high,
                        t->cfg.iou_low, t->cfg.iou_tentative};
@@ -1994,7 +2084,9 @@ static void track_issue(rf_tracker t, const int *videos, int n, const rf_det *de
         ta.due_counts = slot.due_counts;
         ta.max_align = a->max_align;
     }
+    ta.motion = t->motion ? slot.motion : nullptr;
     CK(launch_track_update(ta, videos, scales, n, s));
+    if (t->motion) motion_commit(t, commits, s);
     CK(cudaEventRecord(t->chain, s));
     if (a) {
         PostBuffers view{};
@@ -2014,6 +2106,7 @@ int rf_track_update(rf_tracker t, const int *videos, int n, const rf_det *dev_de
     if (!t) return RF_ERR_INVALID_ARG;
     rf_handle h = t->h;
     if (t->best) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a best-shot tracker takes frames only through rf_detect_yuv_track_best_device", who));
+    if (t->motion) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a motion tracker needs the frames (rf_detect_yuv_track_device)", who));
     int rc = check_track_args(t, who, videos, n, scales);
     if (rc) return rc;
     if (n > 0 && (!dev_dets || !dev_counts)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL records or counts", who));
@@ -2021,7 +2114,7 @@ int rf_track_update(rf_tracker t, const int *videos, int n, const rf_det *dev_de
     try {
         CK(cudaSetDevice(h->device));
         track_issue(t, videos, n, dev_dets, dev_counts, scales, (cudaStream_t)rf_last_stream(h), nullptr, nullptr, dev_tracks,
-                    dev_track_counts);
+                    dev_track_counts, nullptr);
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }
@@ -2052,7 +2145,8 @@ int rf_detect_yuv_track_device(rf_handle h, rf_tracker t, const rf_yuv_frame *fr
         std::vector<AlignImageT<YuvPlanes>> table(n);
         for (int i = 0; i < n; i++) table[i] = AlignImageT<YuvPlanes>{src.in_place(i), src.width(i), src.height(i), 1.f, 0};
         if (align) { a.n = n; a.crops = dev_crops; a.mats = dev_mats; }
-        track_issue(t, videos, n, dets, counts, scales.data(), h->last_stream, align ? &a : nullptr, table.data(), dev_tracks, dev_track_counts);
+        track_issue(t, videos, n, dets, counts, scales.data(), h->last_stream, align ? &a : nullptr, table.data(), dev_tracks, dev_track_counts,
+                    frames);
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }
@@ -2147,6 +2241,9 @@ int rf_detect_yuv_track_best_device(rf_handle h, rf_tracker t, const rf_yuv_fram
         int *best_counts = t->d_best_counts + (size_t)ring * B;
         CK(cudaStreamWaitEvent(s, slot.free, 0));
         CK(cudaStreamWaitEvent(s, t->chain, 0));
+        t->updated = true;
+        MotionCommits commits;
+        if (t->motion) motion_issue(t, ring, frames, videos, n, dets, counts, scales.data(), s, commits);
         TrackArgs ta{};
         ta.p = TrackParams{T, F, t->cfg.max_lost, t->cfg.high_thresh, t->cfg.new_thresh, t->cfg.iou_high, t->cfg.iou_low, t->cfg.iou_tentative};
         ta.videos = t->d_videos;
@@ -2164,6 +2261,7 @@ int rf_detect_yuv_track_best_device(rf_handle h, rf_tracker t, const rf_yuv_fram
             c.counts = counts + i0;
             c.tracks = slot.tracks + (size_t)i0 * T;
             c.track_counts = slot.counts + i0;
+            c.motion = t->motion ? slot.motion + i0 : nullptr;
             CK(launch_track_update(c, videos + i0, scales.data() + i0, m, s));
             BestTable bt{};
             bt.n = m;
@@ -2183,6 +2281,7 @@ int rf_detect_yuv_track_best_device(rf_handle h, rf_tracker t, const rf_yuv_fram
             b.counts = counts + i0;
             CK(launch_best_frames(b, bt, s));
         }
+        if (t->motion) motion_commit(t, commits, s);
         CK(cudaEventRecord(t->chain, s));
         CK(cudaEventRecord(slot.free, s));
         if (dev_tracks) *dev_tracks = slot.tracks;
@@ -2220,11 +2319,53 @@ int rf_tracker_finish(rf_tracker t, int video, void *dev_best_crops, double *dev
         CK(cudaMemsetAsync(t->d_state + (size_t)video * T, 0, sizeof(TrackState) * T, s));
         CK(cudaMemsetAsync(b.store + (size_t)video * T, 0, sizeof(BestEntry) * T, s));
         CK(cudaMemsetAsync(b.videos + video, 0, sizeof(BestVideo), s));
+        if (t->motion) t->mref[video] = {0, 0};
         CK(cudaEventRecord(t->chain, s));
         CK(cudaEventRecord(slot.free, s));
         if (dev_best) *dev_best = b.best;
         if (dev_best_count) *dev_best_count = b.best_counts;
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
+}
+
+int rf_tracker_set_motion(rf_tracker t, const rf_motion_config *cfg) {
+    static const char *who = "rf_tracker_set_motion";
+    if (!t) return RF_ERR_INVALID_ARG;
+    rf_handle h = t->h;
+    if (!cfg) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL config", who));
+    if (t->motion) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: motion is already on", who));
+    if (t->updated) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker has already been updated", who));
+    const int R = cfg->search ? cfg->search : 12, mi = cfg->min_inliers ? cfg->min_inliers : 12;
+    if (R < 1 || R > MOTION_MAX_R) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: search %d, must be 0 or in [1, %d]", who, cfg->search, MOTION_MAX_R));
+    if (mi < 3 || mi > MOTION_MAX_BLOCKS)
+        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: min_inliers %d, must be 0 or in [3, %d]", who, cfg->min_inliers, MOTION_MAX_BLOCKS));
+    const size_t V = t->cfg.max_videos, B = h->cfg.max_batch;
+    if (V * MOTION_THUMB_BYTES > ((size_t)4 << 30))
+        return fail(h, RF_ERR_CAPACITY, fmt("%s: a store of %zu videos x %d bytes exceeds 4 GiB", who, V, MOTION_THUMB_BYTES));
+    try {
+        CK(cudaSetDevice(h->device));
+        CK(cudaMalloc(&t->d_mstore, V * MOTION_THUMB_BYTES));
+        CK(cudaMalloc(&t->d_mthumbs, B * MOTION_THUMB_BYTES));
+        CK(cudaMalloc(&t->d_mblocks, sizeof(MotionBlock) * B * MOTION_MAX_BLOCKS));
+        for (auto &s : t->slots) CK(cudaMalloc(&s.motion, sizeof(rf_motion) * B));
+    } catch (const CudaFail &f) {
+        cudaFree(t->d_mstore); cudaFree(t->d_mthumbs); cudaFree(t->d_mblocks);
+        t->d_mstore = t->d_mthumbs = nullptr;
+        t->d_mblocks = nullptr;
+        for (auto &s : t->slots) { cudaFree(s.motion); s.motion = nullptr; }
+        return fail_cuda(h, f);
+    }
+    t->motion = true;
+    t->mcfg = rf_motion_config{R, mi};
+    t->mref.assign(V, {0, 0});
+    return RF_OK;
+}
+
+int rf_tracker_motion(rf_tracker t, const rf_motion **dev_motion) {
+    if (!t) return RF_ERR_INVALID_ARG;
+    if (!dev_motion) return fail(t->h, RF_ERR_INVALID_ARG, "rf_tracker_motion: dev_motion is NULL");
+    if (!t->motion) return fail(t->h, RF_ERR_INVALID_ARG, "rf_tracker_motion: motion is off (rf_tracker_set_motion)");
+    *dev_motion = t->motion_slot < 0 ? nullptr : t->slots[t->motion_slot].motion;
     return RF_OK;
 }
 
@@ -2443,7 +2584,7 @@ int rf_detect_yuv_redact_device(rf_handle h, rf_tracker t, const rf_yuv_frame *f
         Ctx &c = last_ctx(h);          // the forward's context
         const rf_track *tracks = nullptr;
         const int32_t *track_counts = nullptr;
-        if (t) track_issue(t, videos, n, dets, counts, scales.data(), c.stream, nullptr, nullptr, &tracks, &track_counts);
+        if (t) track_issue(t, videos, n, dets, counts, scales.data(), c.stream, nullptr, nullptr, &tracks, &track_counts, frames);
         if (dev_tracks) *dev_tracks = tracks;
         if (dev_track_counts) *dev_track_counts = track_counts;
         redact_issue(h, c, yuv_redact_table(frames, n, scales.data()), dets, counts, t, tracks, track_counts, blocks, margin);

@@ -13,6 +13,9 @@
 //   box       w = a * h;  x1 = cx - w / 2;  y1 = cy - h / 2;  x2 = x1 + w;  y2 = y1 + h
 //   IoU       x = max(x1), y = max(y1);  iw = (min(x2) - x) + 1;  ih = (min(y2) - y) + 1;  0 unless both > 0;
 //             area = ((x2 - x1) + 1) * ((y2 - y1) + 1) of each;  inter = iw * ih;  IoU = inter / ((area_t + area_d) - inter)
+//   motion    (f13, after predict, RF_MOTION_OK frames only; restated by oracle/motion.py compensate)  s = sqrt(a * a + b * b),
+//             ss = s * s;  cx = ((a * cx) - (b * cy)) + tx;  cy = ((b * cx) + (a * cy)) + ty (old cx, cy);  u_cx, u_cy likewise
+//             without t;  h = s * h;  u_h = s * u_h;  P00, P01, P11 = ss * P for cx, cy, h
 #include <algorithm>
 
 #include "track.cuh"
@@ -70,6 +73,26 @@ __device__ __forceinline__ void kalman_predict(TrackState &k) {
         k.p01[c] = p01 + p11;
         k.p11[c] = p11 + qv * qv;
         k.m[c] = k.m[c] + k.u[c];
+    }
+}
+
+// m: rf_motion.m = {a, -b, tx, b, a, ty}
+__device__ __forceinline__ void kalman_motion(TrackState &k, const double m[6]) {
+    const double a = m[0], b = m[3], tx = m[2], ty = m[5];
+    const double s = sqrt(a * a + b * b), ss = s * s;
+    const double cx = k.m[0], cy = k.m[1], ux = k.u[0], uy = k.u[1];
+    k.m[0] = (a * cx - b * cy) + tx;
+    k.m[1] = (b * cx + a * cy) + ty;
+    k.u[0] = a * ux - b * uy;
+    k.u[1] = b * ux + a * uy;
+    k.m[3] = s * k.m[3];
+    k.u[3] = s * k.u[3];
+#pragma unroll
+    for (int c = 0; c < 4; c++) {
+        if (c == 2) continue;
+        k.p00[c] = ss * k.p00[c];
+        k.p01[c] = ss * k.p01[c];
+        k.p11[c] = ss * k.p11[c];
     }
 }
 
@@ -186,6 +209,7 @@ __global__ void __launch_bounds__(TRACK_THREADS) k_track_update(const TrackArgs 
         const float sc = t.scale[f];
         TrackSeen *seen = a.seen ? a.seen + (size_t)f * F : nullptr;
         TrackGone *gone = a.gone ? a.gone + (size_t)f * T : nullptr;
+        const double *motion = a.motion && a.motion[f].status == RF_MOTION_OK ? a.motion[f].m : nullptr;
         if (seen)
             for (int j = tid; j < F; j += blockDim.x) seen[j].slot = -1;
         for (int i = tid; i < T; i += blockDim.x) {
@@ -196,6 +220,7 @@ __global__ void __launch_bounds__(TRACK_THREADS) k_track_update(const TrackArgs 
             TrackState &k = S[i];
             sm.st0[i] = (unsigned char)k.state;
             kalman_predict(k);
+            if (motion) kalman_motion(k, motion);
             k.age++;
         }
         for (int j = tid; j < K; j += blockDim.x) sm.used[j] = 0;
@@ -338,6 +363,7 @@ cudaError_t launch_track_update(const TrackArgs &a, const int *videos, const flo
         }
         if (a.seen) c.seen = a.seen + (size_t)i0 * F;
         if (a.gone) c.gone = a.gone + (size_t)i0 * T;
+        if (a.motion) c.motion = a.motion + i0;
         k_track_update<<<t.nvideos, TRACK_THREADS, smem, s>>>(c, t);
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;

@@ -71,6 +71,7 @@ struct TrackArgs {
     int max_align;               // crop slots per frame (0 without crops)
     TrackSeen *seen;             // optional [n][max_faces]: every record's track on the frame (f11)
     TrackGone *gone;             // optional [n][max_tracks]: the tracks removed on the frame, by slot (f11)
+    const rf_motion *motion;     // optional [n]: each frame's camera motion (f13), applied after predict when RF_MOTION_OK
 };
 
 // n frames (videos[i], scales[i]; scales NULL: 1), one launch per TRACK_MAX_FRAMES of them, in stream order on s.

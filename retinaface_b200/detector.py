@@ -120,7 +120,7 @@ class RetinaFace:
         return [FaceDetectInfo.from_row(r) for r in faces]
 
     def trackFrames(self, frames: Sequence, videos: Sequence[int], threshold: float = 0.5, layout: str = "nv12", matrix: str = "bt601",
-                    align: dict = None, max_videos: int = 64, best: dict = None):
+                    align: dict = None, max_videos: int = 64, best: dict = None, motion=False):
         """f10 tracking: device 4:2:0 frames (torch CUDA tensors in ``Engine.detect_yuv_device``'s forms), frame i of video
         ``videos[i]``, detected and associated with the tracks of earlier frames on the GPU (rf_detect_yuv_track_device).  Per frame, a
         list of ``(id, state, FaceDetectInfo)`` over every live track (``capi.TRACK_*`` states; the face is the last matched one, in
@@ -132,13 +132,18 @@ class RetinaFace:
         tracker is a best-shot tracker (rf_detect_yuv_track_best_device; ``align`` must then be None) and the second list holds, per
         frame, a ``(shot, crop)`` for every track that ended on that frame: ``shot`` a ``capi.BEST_DTYPE`` record (the quality terms
         and the record of the track's best frame), ``crop`` that frame's crop as a torch CUDA tensor.  ``finishVideo`` emits the
-        shots of the tracks still live.  The first call decides which kind of tracker this detector keeps."""
+        shots of the tracks still live.
+
+        f13 camera motion: with ``motion`` (True, or ``capi.motion_config``'s keywords: search, min_inliers) the tracker estimates
+        each frame's global motion from the previous frame of the same video and moves the tracks with it, so that a panning or
+        shaking camera keeps the ids; ``Tracker.motion`` (``self._tracker``) reads the estimates.  The first call decides which kind
+        of tracker this detector keeps."""
         import torch
         from .capi import crop_shape
         if best is not None and align is not None:
             raise ValueError("best shots and new-identity crops are exclusive: pass best or align, not both")
         if getattr(self, "_tracker", None) is None:
-            self._tracker = self.engine.tracker(max_videos=max_videos, best=best)
+            self._tracker = self.engine.tracker(max_videos=max_videos, best=best, motion=motion)
         n = len(frames)
         if best is not None:
             crops = self._best_crops(n)
@@ -164,19 +169,20 @@ class RetinaFace:
         return tracks, new
 
     def redactFrames(self, frames: Sequence, videos: Sequence[int] = None, threshold: float = 0.5, blocks: int = 0, margin: float = 0.0,
-                     layout: str = "nv12", matrix: str = "bt601", max_videos: int = 64):
+                     layout: str = "nv12", matrix: str = "bt601", max_videos: int = 64, motion=False):
         """f12 redaction: detect on device 4:2:0 frames (torch CUDA tensors in ``Engine.detect_yuv_device``'s forms) and mosaic every
         detected face IN PLACE (rf_detect_yuv_redact_device), ``blocks`` cells across a region's longer side (0: 8; 1: a flat patch),
         each side grown by ``margin`` of the box (0: 0.25).  With ``videos`` (frame i of video ``videos[i]``) the frames are also
         tracked, on this detector's plain tracker (created as ``trackFrames`` creates it), and the predicted box of every face the
         tracker still follows while the detector misses it is redacted too.  Asynchronous: the frames are complete in stream order on
-        ``engine.last_stream_ptr()``."""
+        ``engine.last_stream_ptr()``.  ``motion`` as ``trackFrames``: the lost faces' predicted boxes then follow the camera.  The first
+        call decides the tracker."""
         if videos is None:
             self.engine.detect_yuv_redact_device(list(frames), threshold, self.nms_threshold, layout=layout, matrix=matrix, blocks=blocks,
                                                  margin=margin)
             return
         if getattr(self, "_tracker", None) is None:
-            self._tracker = self.engine.tracker(max_videos=max_videos)
+            self._tracker = self.engine.tracker(max_videos=max_videos, motion=motion)
         self._tracker.detect_yuv_redact_device(list(frames), list(videos), threshold, self.nms_threshold, layout=layout, matrix=matrix,
                                                blocks=blocks, margin=margin)
 

@@ -293,6 +293,7 @@ void RetinaFace::trackYUV(const vector<rf_yuv_frame> &device_frames, const vecto
         tc.max_videos = opt_.track_videos;
         int rc = rf_tracker_create(h_, &tc, &tracker_);
         if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_create: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+        trackerCreated();
     }
     int per = 0, cw = 0, ch = 0;
     const rf_align_params p = align ? crop_params(*align, opt_.max_faces, &per, &cw, &ch) : rf_align_params{};
@@ -303,6 +304,22 @@ void RetinaFace::trackYUV(const vector<rf_yuv_frame> &device_frames, const vecto
     if (rc != RF_OK) throw std::runtime_error(string("rf_detect_yuv_track_device: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
     tracks_.n = n;
     tracks_.max_tracks = 64;      // rf_track_config's default
+    noteMotion(n);
+}
+
+void RetinaFace::trackerCreated() {
+    if (!opt_.track_motion) return;
+    const rf_motion_config mc{};
+    int rc = rf_tracker_set_motion(tracker_, &mc);
+    if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_set_motion: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+}
+
+void RetinaFace::noteMotion(int n) {
+    motion_ = DeviceMotion{};
+    if (!opt_.track_motion) return;
+    int rc = rf_tracker_motion(tracker_, &motion_.motion);
+    if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_motion: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+    motion_.n = n;
 }
 
 void RetinaFace::redactYUV(const vector<rf_yuv_frame> &device_frames, const vector<int> *videos, float threshold, const RedactOptions &opt) {
@@ -314,6 +331,7 @@ void RetinaFace::redactYUV(const vector<rf_yuv_frame> &device_frames, const vect
         tc.max_videos = opt_.track_videos;
         int rc = rf_tracker_create(h_, &tc, &tracker_);
         if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_create: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+        trackerCreated();
     }
     const rf_redact_params p{opt.blocks, opt.margin};
     const int n = (int)device_frames.size();
@@ -325,6 +343,7 @@ void RetinaFace::redactYUV(const vector<rf_yuv_frame> &device_frames, const vect
         tracks_ = t;
         tracks_.n = n;
         tracks_.max_tracks = 64;      // rf_track_config's default
+        noteMotion(n);
     }
 }
 
@@ -341,6 +360,7 @@ void RetinaFace::trackYUVBest(const vector<rf_yuv_frame> &device_frames, const v
         int rc = rf_tracker_create_best(h_, &tc, &bc, &tracker_);
         if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_create_best: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
         best_tracker_ = true;
+        trackerCreated();
     }
     const int n = (int)device_frames.size();
     tracks_ = DeviceTracks{};
@@ -351,6 +371,7 @@ void RetinaFace::trackYUVBest(const vector<rf_yuv_frame> &device_frames, const v
     if (rc != RF_OK) throw std::runtime_error(string("rf_detect_yuv_track_best_device: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
     tracks_.n = best_.n = n;
     tracks_.max_tracks = best_.max_tracks = 64;      // rf_track_config's default
+    noteMotion(n);
 }
 
 void RetinaFace::finishVideo(int video, void *dev_best_crops) {

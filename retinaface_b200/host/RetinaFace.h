@@ -39,6 +39,7 @@ struct RetinaFaceOptions {
     string prototxt_file;                // e.g. "mnet-deconv-0517.prototxt" (RetinaFace.cpp:276): parsed, checked, drives the weight
                                          // folding; with net_w = net_h = 0 it also sets the network size.  Empty: built-in graph
     int track_videos = 16;               // sequences of the tracker trackYUV creates on its first call
+    bool track_motion = false;           // f13: that tracker follows the camera's motion (rf_tracker_set_motion, default config)
     string cache_file;                   // folded-model cache (the reference's "retina.cache", trtnetbase.cpp:205-243, but with a
                                          // staleness check).  Empty: none
 };
@@ -132,6 +133,13 @@ class RetinaFace {
     void trackYUVBest(const vector<rf_yuv_frame> &device_frames, const vector<int> &videos, void *dev_best_crops, float threshold = 0.5,
                       float min_quality = 0.f);
     const DeviceBestShots &lastBestShots() const { return best_; }
+    // f13 camera motion (options track_motion): the device rf_motion of each frame of the last trackYUV / trackYUVBest / tracked
+    // redactYUV call -- the estimated similarity from the video's previous frame, applied to its tracks.
+    struct DeviceMotion {
+        const rf_motion *motion = nullptr;  // device [n]
+        int n = 0;
+    };
+    const DeviceMotion &lastMotion() const { return motion_; }
     void finishVideo(int video, void *dev_best_crops);
     // f12 redaction (rf_detect_yuv_redact_device): detect on DEVICE 4:2:0 frames and mosaic every detected face in place, on the
     // GPU; asynchronous on rf_last_stream(handle()).  With `videos` (one per frame, in [0, track_videos)) the frames are also tracked on
@@ -148,11 +156,14 @@ class RetinaFace {
    private:
     // faces (and, with crops, the u8 crops of the first min(count, per) faces) of images [start, start + n) of the last call
     void keepResults(size_t start, int n, const unsigned char *crops, int per, int cw, int ch);
+    void trackerCreated();              // motion on a new tracker, as the options say
+    void noteMotion(int n);             // lastMotion() after a tracked call of n frames
     rf_handle h_ = nullptr;
     rf_tracker tracker_ = nullptr;
     bool best_tracker_ = false;
     DeviceTracks tracks_;
     DeviceBestShots best_;
+    DeviceMotion motion_;
     RetinaFaceOptions opt_;
     string network;
     float nms_threshold;

@@ -42,6 +42,23 @@ def _heads_ptrs(heads: Sequence[np.ndarray]):
     return arr, keep
 
 
+def compare_dets(mine, mine_idx, ref, label="", max_faces=None):
+    """Detections against a PostprocOracle.postprocess result: selection (anchor emission indices, order) exact; scores and
+    landmarks bit-exact; box corners within 4e-6 relative (the exp() rounding noted in postproc.cu).  With `max_faces`, the
+    output capacity: the count is min(kept, max_faces) and the faces are the oracle's top-scoring prefix."""
+    ridx, rfaces = ref["idx"], ref["faces"]
+    if max_faces is not None and len(ridx) > max_faces:
+        ridx, rfaces = ridx[:max_faces], rfaces[:max_faces]
+    assert mine_idx.tolist() == ridx.tolist(), label
+    a, b = mine, rfaces
+    assert a.shape == b.shape, label
+    if len(a) == 0:
+        return
+    assert np.array_equal(a[:, 0], b[:, 0]), label            # scores
+    assert np.array_equal(a[:, 5:], b[:, 5:]), label          # landmarks
+    assert np.allclose(a[:, 1:5], b[:, 1:5], rtol=4e-6, atol=1e-4), label
+
+
 class PostprocOracle:
     """The plain-C restatement (oracle/postproc.c)."""
 
@@ -75,21 +92,15 @@ class PostprocOracle:
         return dict(cand=cand[:n].copy(), cand_idx=cand_idx[:n].copy(),
                     faces=out[:kept].copy(), idx=out_idx[:kept].copy())
 
-    def check_engine(self, eng, batch, heads, thr: float, nms_thr: float, label: str = "") -> int:
-        """An engine's detections of `batch` against this post-process of the engine's own `heads`: selection (anchor
-        indices, order) exact, scores and landmarks bit-exact, box corners within 4e-6 relative (the exp() rounding noted in
-        postproc.cu).  Returns the number of faces compared."""
+    def check_engine(self, eng, batch, heads, thr: float, nms_thr: float, label: str = "", refs=None, dets=None) -> int:
+        """An engine's detections of `batch` (rf_detect_batch, or `dets` = (faces, indices) it already returned) against this
+        post-process of the engine's own `heads` (or `refs`, one postprocess() result per image), compared by compare_dets with
+        the engine's max_faces.  Returns the number of faces compared."""
         h, w = batch.shape[1:3]
-        faces, idx = eng.detect_batch(list(batch), thr, nms_thr, want_index=True)
+        faces, idx = dets if dets is not None else eng.detect_batch(list(batch), thr, nms_thr, want_index=True)
         for i in range(len(batch)):
-            ref = self.postprocess([x[i] for x in heads], h, w, thr, nms_thr)
-            lab = f"{label} image {i}"
-            assert idx[i].tolist() == ref["idx"].tolist(), lab
-            assert faces[i].shape == ref["faces"].shape, lab
-            if len(faces[i]):
-                assert np.array_equal(faces[i][:, 0], ref["faces"][:, 0]), lab
-                assert np.array_equal(faces[i][:, 5:], ref["faces"][:, 5:]), lab
-                assert np.allclose(faces[i][:, 1:5], ref["faces"][:, 1:5], rtol=4e-6, atol=1e-4), lab
+            ref = refs[i] if refs is not None else self.postprocess([x[i] for x in heads], h, w, thr, nms_thr)
+            compare_dets(faces[i], idx[i], ref, f"{label} image {i}", eng.max_faces)
         return sum(len(f) for f in faces)
 
     def nms(self, cands: np.ndarray, thr: float):

@@ -419,10 +419,12 @@ def model_inspect(caffemodel: str, layer: str):
 
 
 def plan_describe(caffemodel: str, net_h: int, net_w: int, precision: int = RF_PREC_FP16, max_batch: int = 8, flags: int = 0,
-                  int8_table: Optional[str] = None, streams: int = 0) -> str:
-    """The layer plan rf_create would build (host-only entry point: no GPU needed)."""
+                  int8_table: Optional[str] = None, streams: int = 0, max_faces: int = 0) -> str:
+    """The layer plan rf_create would build (host-only entry point: no GPU needed).  `max_faces` as in Engine (0 -> 256): the tile
+    chains reserve shared memory for the last-block NMS's kept list, so the plan depends on it."""
     lib = load_library()
-    cfg = _Config(caffemodel.encode(), int8_table.encode() if int8_table else None, precision, net_w, net_h, max_batch, 0, 0, 0, 0, flags, streams, None, None, None)
+    cfg = _Config(caffemodel.encode(), int8_table.encode() if int8_table else None, precision, net_w, net_h, max_batch, max_faces, 0, 0, 0,
+                  flags, streams, None, None, None)
     buf = C.create_string_buffer(1 << 16)
     lib.rf_plan_describe.argtypes = [C.POINTER(_Config), C.c_char_p, C.c_int]
     rc = lib.rf_plan_describe(C.byref(cfg), buf, len(buf))

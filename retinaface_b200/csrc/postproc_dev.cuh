@@ -11,6 +11,7 @@ namespace rf {
 
 constexpr int NMS_SMEM_CAP = 1024;  // candidates sorted / suppressed entirely in shared memory
 constexpr int NMS_RANK_MAX = 256;   // up to here a one-pass rank sort replaces the bitonic ladder
+constexpr int NMS_MASK_MAX = 64;    // up to here the whole IoU relation fits one 64-bit row per candidate: no barrier per kept face
 
 __device__ __forceinline__ unsigned long long make_key(float score, int emit) {
     unsigned u = __float_as_uint(score);
@@ -156,7 +157,7 @@ __device__ __forceinline__ void nms_image(int img, int tid, float thr, const Pos
         return ldbox((unsigned)(keys[i] & 0xffffffffu));
     };
     int nkept = 0;  // thread 0's running count (mirrored to S.nkept at the end)
-    if (n <= 64) {
+    if (n <= NMS_MASK_MAX) {
         // few candidates (the usual case: tens per image): the whole suppression relation at once -- thread (i, half) tests box i
         // against 32 later boxes -> one 64-bit row per candidate; then ONE thread walks the rows.  Same greedy rule (a box is
         // suppressed only by a KEPT earlier box), no barrier per kept face.

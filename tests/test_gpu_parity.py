@@ -13,6 +13,7 @@ from oracle import topology
 from oracle.inputs import letterbox_bgr_u8, s_noise_batch, s_real_batch
 from oracle.mnet_numpy import MnetOracle, preprocess_bgr_u8
 from oracle.postproc import PostprocOracle, ReferencePostproc, synth_heads
+from oracle.postproc import compare_dets as _compare_dets
 
 pytestmark = pytest.mark.gpu
 
@@ -23,22 +24,6 @@ TOL_FP32 = 2e-4
 def _engine(model, h, w, prec, **kw):
     from retinaface_b200 import Engine
     return Engine(caffemodel(model), h, w, precision=prec, **kw)
-
-
-def _compare_dets(mine, mine_idx, ref, label="", max_faces=None):
-    """Selection (anchor emission indices, order) bit-exact; scores + landmarks bit-exact; box corners
-    within 4e-6 relative (the exp() rounding noted in postproc.cu)."""
-    ridx, rfaces = ref["idx"], ref["faces"]
-    if max_faces is not None and len(ridx) > max_faces:   # output capacity clamp keeps the top-scoring prefix
-        ridx, rfaces = ridx[:max_faces], rfaces[:max_faces]
-    assert mine_idx.tolist() == ridx.tolist(), label
-    a, b = mine, rfaces
-    assert a.shape == b.shape, label
-    if len(a) == 0:
-        return
-    assert np.array_equal(a[:, 0], b[:, 0]), label            # scores
-    assert np.array_equal(a[:, 5:], b[:, 5:]), label          # landmarks
-    assert np.allclose(a[:, 1:5], b[:, 1:5], rtol=4e-6, atol=1e-4), label
 
 
 @pytest.fixture(scope="module")
@@ -53,11 +38,12 @@ def test_postprocess_kernels_vs_oracle(post_oracle, hw):
     h, w = hw
     eng = _engine("mnet25", h, w, RF_PREC_FP32, max_batch=4, max_faces=8192)
     try:
-        for ncand in (0, 1, 37, 64, 1024, 4000, 8192):
+        # both sides of nms_image's branch points (NMS_MASK_MAX 64, NMS_RANK_MAX 256, NMS_SMEM_CAP 1024)
+        for ncand in (0, 1, 37, 64, 65, 256, 257, 1024, 1025, 4000, 8192):
             batch = [synth_heads(h, w, ncand, seed=100 + ncand + i) for i in range(3)]
             heads = [np.stack([b[k] for b in batch]) for k in range(9)]
             for thr, nms in ((0.9, 0.4), (0.5, 0.4), (0.9, 0.0), (0.9, 1.0)):
-                if ncand > 1024 and (thr, nms) != (0.9, 0.4):
+                if ncand > 1025 and (thr, nms) != (0.9, 0.4):
                     continue
                 faces, idx, ncands = eng.postprocess(heads, thr, nms)
                 for i in range(3):
@@ -167,7 +153,8 @@ def test_fp32_detect_matches_golden_detections(hw, golden_image, post_oracle):
         try:
             dets = np.load(os.path.join(GOLDEN, f"dets_{model}_{h}x{w}.npz"))
             inp = letterbox_bgr_u8(golden_image, h, w)
-            for thr in (0.9, 0.5):
+            # 0.02: the WIDER evaluation threshold, 9e-4 from the nearest P(face) of the golden heads at 448^2 (FP32 error ~1e-5)
+            for thr in (0.9, 0.5, 0.02):
                 faces, idx = eng.detect_batch([inp, inp], thr, 0.4, want_index=True)
                 g = dets[f"faces_thr{thr}"]
                 for f in faces:
@@ -177,6 +164,8 @@ def test_fp32_detect_matches_golden_detections(hw, golden_image, post_oracle):
                 assert np.array_equal(faces[0], faces[1])
             # consistency: rf_forward_heads -> oracle post-process == rf_detect_batch, selection bit-exact
             heads = eng.forward_heads(inp[None])
+            margin = float(np.abs(np.concatenate([x[0, 2:4].ravel() for x in heads[0::3]]) - np.float32(0.02)).min())
+            print(f"{model} {hw}: closest P(face) to 0.02 is {margin:.2e} away")
             ref = post_oracle.postprocess([x[0] for x in heads], h, w, 0.5, 0.4)
             faces, idx = eng.detect_batch([inp], 0.5, 0.4, want_index=True)
             _compare_dets(faces[0], idx[0], ref, f"{model} {hw}")
@@ -556,17 +545,17 @@ def test_detect_views_tta_and_map_back(golden_image, post_oracle):
     bit for bit, in order.  A single (1.0, no flip) view is detect + map-back."""
     from retinaface_b200 import RF_PREC_FP32, RfError
     h_img, w_img = golden_image.shape[:2]
-    eng = _engine("mnet25", 448, 448, RF_PREC_FP32, max_batch=4, max_image=(1024, 1280))
-    try:
-        views = [(1.0, False), (1.0, True), (0.75, False), (0.6, True)]
-        faces, view_of, scales = eng.detect_views(golden_image, views, 0.9, 0.4)
+    views = [(1.0, False), (1.0, True), (0.75, False), (0.6, True)]
+
+    def check_views(eng, thr, nms):
+        faces, view_of, scales = eng.detect_views(golden_image, views, thr, nms)
         cands = []
         for v, (s, flip) in enumerate(views):
             bw, bh = int(448 * s), int(448 * s)
             src = np.ascontiguousarray(golden_image[:, ::-1]) if flip else golden_image
             canvas = np.zeros((448, 448, 3), np.uint8)
             canvas[:bh, :bw] = letterbox_bgr_u8(src, bh, bw)
-            det = eng.detect_batch([canvas], 0.9, 0.4)[0]
+            det = eng.detect_batch([canvas], thr, nms)[0]
             sc = max(np.float32(1.0 * w_img / bw), np.float32(1.0 * h_img / bh), np.float32(1.0))
             assert scales[v] == sc
             m = det.copy()
@@ -582,11 +571,28 @@ def test_detect_views_tta_and_map_back(golden_image, post_oracle):
             cands.append((v, m))
         allc = np.concatenate([m for _, m in cands])
         vids = np.concatenate([np.full(len(m), v, np.int32) for v, m in cands])
-        want, pos = post_oracle.nms(allc, 0.4)
-        assert len(want) >= 5 and len(cands[3][1]) >= 1        # the small mirrored view still finds faces
-        assert faces.shape == want.shape
-        assert np.array_equal(faces, want)
-        assert np.array_equal(view_of, vids[pos])
+        want, pos = post_oracle.nms(allc, nms)
+        want, pos = want[:eng.max_faces], pos[:eng.max_faces]          # the output capacity keeps the top-scoring prefix
+        assert faces.shape == want.shape, (thr, nms, faces.shape, want.shape)
+        assert np.array_equal(faces, want), (thr, nms)
+        assert np.array_equal(view_of, vids[pos]), (thr, nms)
+        return faces, cands
+
+    # the views' detections merged by k_nms beyond its shared-memory working set (> 1024 candidates): ids view * max_faces + rank
+    heavy = _engine("mnet25", 448, 448, RF_PREC_FP32, max_batch=4, max_image=(1024, 1280), max_faces=8192)
+    try:
+        for nms in (1.0, 0.4):
+            merged, cands = check_views(heavy, 0.001, nms)
+            total = sum(len(m) for _, m in cands)
+            print(f"views at thr 0.001, nms {nms}: {total} candidates from 4 views, {len(merged)} merged faces")
+            if nms == 1.0:
+                assert total > 1024
+    finally:
+        heavy.close()
+    eng = _engine("mnet25", 448, 448, RF_PREC_FP32, max_batch=4, max_image=(1024, 1280))
+    try:
+        faces, cands = check_views(eng, 0.9, 0.4)
+        assert len(faces) >= 5 and len(cands[3][1]) >= 1        # the small mirrored view still finds faces
         # single plain view == detect + map-back
         one, _, sc1 = eng.detect_views(golden_image, [(1.0, False)], 0.9, 0.4)
         plain = eng.detect_batch([golden_image], 0.9, 0.4)[0]

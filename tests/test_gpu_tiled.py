@@ -135,7 +135,7 @@ def letterbox_448(img):
 
 def _host_tiled(eng, img, levels, overlap, thr, nms, post_oracle):
     """The merge oracle: every tile built on the host, detected through rf_detect_batch in batches, mapped back and filtered in
-    float32 numpy, merged by the oracle NMS.  Returns (faces, tile of each face)."""
+    float32 numpy, merged by the oracle NMS.  Returns (faces, tile of each face, number of merged candidates)."""
     tiles = _layout(eng, img, levels, overlap)
     cache, ins = {}, []
     for t in tiles:
@@ -153,27 +153,43 @@ def _host_tiled(eng, img, levels, overlap, thr, nms, post_oracle):
     allc = np.concatenate(cands)
     ids = np.concatenate(tile_ids)
     want, pos = post_oracle.nms(allc, nms)
-    return want, ids[pos]
+    want, pos = want[:eng.max_faces], pos[:eng.max_faces]        # the output capacity keeps the top-scoring prefix
+    return want, ids[pos], len(allc)
 
 
 def test_merge_equals_host_tiles_detected_one_by_one(golden_image):
     """Golden photo and a 3840 x 2160 canvas, levels {1.5 mirrored, 1.0, 0.5, fitted}: faces, order and out_tile_of identical bit for
-    bit to the host merge of every tile detected through rf_detect_batch (FP32)."""
+    bit to the host merge of every tile detected through rf_detect_batch (FP32).  At thresholds 0.02 and 0.001 the canvas's 211 tiles
+    send tens of thousands of candidates (ids tile * max_faces + rank) to the final k_nms, past its shared-memory working set; a
+    handle with max_batch 48 runs 48 tiles per forward, which k_merge takes in two launches of at most 40 sources."""
     from oracle.postproc import PostprocOracle
     post_oracle = PostprocOracle()
     canvas, _, _ = _canvas(golden_image)
     levels = [(1.5, 1), (1.0, 0), (0.5, 0), (0.0, 0)]
-    eng = _engine("fp32")
+    cases = [("fp32", dict(), "golden", golden_image, 0.5), ("fp32", dict(), "canvas", canvas, 0.5), ("fp32", dict(), "canvas", canvas, 0.02),
+             ("fp32", dict(), "canvas", canvas, 0.001), ("fp32", dict(max_batch=48), "canvas", canvas, 0.5),
+             ("fp32", dict(max_batch=48), "canvas", canvas, 0.02)]
+    engines = {}
     try:
-        for name, img in (("golden", golden_image), ("canvas", canvas)):
-            want, want_tile = _host_tiled(eng, img, levels, 0, 0.5, 0.4, post_oracle)
-            faces, tile_of = eng.detect_tiled([img], 0.5, 0.4, levels=levels)
-            assert len(want) >= 5, name
-            assert faces[0].shape == want.shape, (name, faces[0].shape, want.shape)
-            assert np.array_equal(faces[0], want), name
-            assert np.array_equal(tile_of[0], want_tile), name
+        for prec, kw, name, img, thr in cases:
+            key = (prec, tuple(kw.items()))
+            if key not in engines:
+                engines[key] = _engine(prec, **kw)
+            eng = engines[key]
+            assert len(_layout(eng, img, levels)) > (40 if eng.max_batch > 40 else 0)
+            want, want_tile, ncand = _host_tiled(eng, img, levels, 0, thr, 0.4, post_oracle)
+            faces, tile_of = eng.detect_tiled([img], thr, 0.4, levels=levels)
+            label = (name, thr, eng.max_batch)
+            print(f"merge {label}: {ncand} candidates, {len(faces[0])} faces")
+            assert len(want) >= 5, label
+            if thr <= 0.001:
+                assert ncand > 1024, label
+            assert faces[0].shape == want.shape, (label, faces[0].shape, want.shape)
+            assert np.array_equal(faces[0], want), label
+            assert np.array_equal(tile_of[0], want_tile), label
     finally:
-        eng.close()
+        for eng in engines.values():
+            eng.close()
 
 
 def _iou(a, b):

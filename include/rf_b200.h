@@ -733,6 +733,52 @@ int rf_detect_yuv_redact_device(rf_handle h, rf_tracker t, const rf_yuv_frame *f
                                 const rf_track **dev_tracks, const int32_t **dev_track_counts, const rf_det **dev_dets,
                                 const int32_t **dev_counts, float *out_scales);
 
+/* f14 redaction styles: a soft elliptical blur -- what broadcast, body-camera and street-level footage is published with -- or f12's
+ * mosaic, over a rectangle or its inscribed ellipse, through the same regions.  Regions, their order, skipped boxes, the FP64
+ * rectangle [X0, X1) x [Y0, Y1) snapped to even coordinates (unclamped) and "original" are f12's, above.  With W = X1 - X0 and
+ * H = Y1 - Y0:
+ * Shape.  RECT covers the rectangle, as f12.  ELLIPSE covers a sample whose centre lies in the ellipse inscribed in the rectangle:
+ *   u = 2x + 1 - X0 - X1, v = 2y + 1 - Y0 - Y1, covered iff u^2 H^2 + v^2 W^2 <= W^2 H^2, in exact integers (W^2 H^2 reaches about
+ *   3e20 under the +-65536 clamp: 128-bit on the device).  Chroma samples use the same test on the halved rectangle.  A rectangle
+ *   empty on either axis (W <= 0 or H <= 0, only beyond the clamp) covers nothing, in either shape.  A sample takes its value from
+ *   the LOWEST-index region whose shape covers it; no other byte is written.  With the default margin 0.25 the ellipse contains the
+ *   whole detection box (a corner sits at 1 / (1 + 2 margin) <= 1 / sqrt(2) of each semi-axis); below margin ~0.207 the box's corners
+ *   fall outside it.
+ * MOSAIC.  f12's cells and cell values exactly; only the set of written samples follows the shape.
+ * BLUR.  D = max(W, H); the luma / BGR radius a = clamp(ceil(D / (2 detail)), 1, 127), the chroma radius a_c = (a + 1) >> 1.  The
+ *   filter is a box of width n = 2a + 1 applied three times per axis, as one integer kernel k = box * box * box (6a + 1 taps, sum n^3,
+ *   sigma = sqrt(a (a + 1))).  The value of sample (x, y) of a plane is
+ *     S = sum_{i,j} k[i] k[j] P[clampY(y + j)][clampX(x + i)]      (replicate borders, P the ORIGINAL plane)
+ *     out = (S + (n^6 - 1) / 2) / n^6                               (integers; n^6 is odd, so no ties)
+ *   over the plane of the frame: luma w x h, chroma w/2 x h/2, BGR per channel at w x h.  A one-axis sum is at most 255^4 < 2^32 and
+ *   S at most 255^7 < 2^63 at a = 127.  No exp(): every implementation of this definition agrees bit for bit.
+ * kind 0 is BLUR and shape 0 ELLIPSE, so a zeroed struct is a detail-4 elliptical blur at margin 0.25. */
+#define RF_REDACT_MOSAIC 1
+#define RF_REDACT_BLUR 2
+#define RF_REDACT_RECT 1
+#define RF_REDACT_ELLIPSE 2
+typedef struct rf_redact_style {
+    int kind;       /* RF_REDACT_MOSAIC or RF_REDACT_BLUR; 0 -> BLUR */
+    int shape;      /* RF_REDACT_RECT or RF_REDACT_ELLIPSE; 0 -> ELLIPSE */
+    int blocks;     /* mosaic only, as in rf_redact_params: 0 -> 8; else 1..32; must be 0 for BLUR */
+    int detail;     /* blur only: 0 -> 4; else 1..64 (a larger detail, a smaller radius); must be 0 for MOSAIC */
+    float margin;   /* as rf_redact_params: 0 -> 0.25; else finite, in (0, 1] */
+} rf_redact_style;
+/* The three f12 calls with a style (NULL: the zeroed struct's defaults).  Statuses, in the same order as the f12 call's, plus
+ * RF_ERR_INVALID_ARG for a bad style where f12 checks its params; nothing is launched on any of them.  {MOSAIC, RECT} writes the bytes
+ * the f12 call writes.  BLUR adds scratch planes per execution context, grown with the call: one frame's plane bytes per frame
+ * (w h 3 / 2 for YUV, 3 w h for BGR) beside f12's region tables. */
+int rf_redact_yuv_device_style(rf_handle h, const rf_yuv_frame *frames, int n, const rf_det *dev_dets, const int32_t *dev_counts,
+                               const float *scales, rf_tracker t, const rf_track *dev_tracks, const int32_t *dev_track_counts,
+                               const rf_redact_style *style);
+int rf_redact_device_style(rf_handle h, uint8_t *const *dev_bgr, const int *widths, const int *heights, const int *row_strides, int n,
+                           const rf_det *dev_dets, const int32_t *dev_counts, const float *scales, rf_tracker t, const rf_track *dev_tracks,
+                           const int32_t *dev_track_counts, const rf_redact_style *style);
+int rf_detect_yuv_redact_device_style(rf_handle h, rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, int matrix,
+                                      float score_threshold, float nms_threshold, const rf_redact_style *style,
+                                      const rf_track **dev_tracks, const int32_t **dev_track_counts, const rf_det **dev_dets,
+                                      const int32_t **dev_counts, float *out_scales);
+
 /* Introspection. */
 int rf_get_net_size(rf_handle h, int *net_w, int *net_h, int *max_batch, int *max_faces);
 int rf_num_anchors(rf_handle h);            /* per image: 8,232 @448x448, 47,040 @1280x896 */

@@ -36,6 +36,7 @@ EXPORTS = [
     "rf_tracker_create_best", "rf_detect_yuv_track_best_device", "rf_tracker_finish",
     "rf_tracker_set_motion", "rf_tracker_motion",
     "rf_redact_yuv_device", "rf_redact_device", "rf_detect_yuv_redact_device",
+    "rf_redact_yuv_device_style", "rf_redact_device_style", "rf_detect_yuv_redact_device_style",
 ]
 COMM_BLOB_BYTES = 128
 
@@ -255,6 +256,33 @@ class RedactParams(C.Structure):  # rf_redact_params
     _fields_ = [("blocks", C.c_int), ("margin", C.c_float)]
 
 
+RF_REDACT_MOSAIC, RF_REDACT_BLUR = 1, 2
+RF_REDACT_RECT, RF_REDACT_ELLIPSE = 1, 2
+
+
+class RedactStyle(C.Structure):  # rf_redact_style
+    _fields_ = [("kind", C.c_int), ("shape", C.c_int), ("blocks", C.c_int), ("detail", C.c_int), ("margin", C.c_float)]
+
+
+def redact_style(style: str = "mosaic", shape: str = "rect", blocks: int = 0, detail: int = 0, margin: float = 0.0) -> Optional[RedactStyle]:
+    """The rf_redact_style of the redaction keywords, or None for f12's mosaic over rectangles ({"mosaic", "rect"}, detail 0), which
+    the f12 calls draw.  style: "mosaic" or "blur"; shape: "rect" or "ellipse"; detail: the blur's 0 (4) or 1..64."""
+    kinds, shapes = {"mosaic": RF_REDACT_MOSAIC, "blur": RF_REDACT_BLUR}, {"rect": RF_REDACT_RECT, "ellipse": RF_REDACT_ELLIPSE}
+    if style not in kinds or shape not in shapes:
+        raise ValueError(f"style {style!r} / shape {shape!r}: style is one of {sorted(kinds)}, shape one of {sorted(shapes)}")
+    if style == "mosaic" and shape == "rect" and not detail:
+        return None
+    return RedactStyle(kinds[style], shapes[shape], int(blocks), int(detail), float(margin))
+
+
+def _redact_call(lib, style: str, shape: str, blocks: int, detail: int, margin: float):
+    """(rf_detect_yuv_redact_device or its _style variant, the params or style struct) of the redaction keywords."""
+    st = redact_style(style, shape, blocks, detail, margin)
+    if st is None:
+        return lib.rf_detect_yuv_redact_device, RedactParams(int(blocks), float(margin))
+    return lib.rf_detect_yuv_redact_device_style, st
+
+
 class RfError(RuntimeError):
     def __init__(self, status: int, msg: str):
         super().__init__(f"librf_b200 status {status}: {msg}")
@@ -394,9 +422,14 @@ def load_library() -> C.CDLL:
                                          C.c_void_p, C.POINTER(RedactParams)]
     lib.rf_redact_device.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int,
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(RedactParams)]
+    lib.rf_redact_yuv_device_style.argtypes = lib.rf_redact_yuv_device.argtypes[:-1] + [C.POINTER(RedactStyle)]
+    lib.rf_redact_device_style.argtypes = lib.rf_redact_device.argtypes[:-1] + [C.POINTER(RedactStyle)]
     lib.rf_detect_yuv_redact_device.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(YuvFrame), C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float,
                                                 C.POINTER(RedactParams), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
                                                 C.POINTER(C.c_void_p), C.c_void_p]
+    a = list(lib.rf_detect_yuv_redact_device.argtypes)
+    a[8] = C.POINTER(RedactStyle)
+    lib.rf_detect_yuv_redact_device_style.argtypes = a
     _lib = lib
     return lib
 
@@ -1082,39 +1115,51 @@ class Engine:
         return sc
 
     def redact_yuv_device(self, frames, dets_ptr: int, counts_ptr: int, scales=None, layout: str = "nv12", tracker: Optional["Tracker"] = None,
-                          tracks_ptr: Optional[int] = None, track_counts_ptr: Optional[int] = None, blocks: int = 0, margin: float = 0.0):
+                          tracks_ptr: Optional[int] = None, track_counts_ptr: Optional[int] = None, blocks: int = 0, margin: float = 0.0,
+                          style: str = "mosaic", shape: str = "rect", detail: int = 0):
         """rf_redact_yuv_device: mosaic, IN PLACE, every region of the device 4:2:0 frames (torch CUDA tensors in yuv_frame's forms):
         the records at dets_ptr / counts_ptr of a device detect call (scales: each frame's map-back factor; None for records already
         in frame pixels) and, with a tracker, the LOST tracks of its lists at tracks_ptr / track_counts_ptr.  Asynchronous on
-        last_stream_ptr()."""
+        last_stream_ptr().  style / shape / detail other than the defaults: rf_redact_yuv_device_style (see redact_style)."""
         n = len(frames)
         arr = self._frames(frames, layout, True)
         sc = self._scales(scales, n)
+        st = redact_style(style, shape, blocks, detail, margin)
+        args = (self.h, arr, n, dets_ptr, counts_ptr, sc.ctypes.data if sc is not None else None, tracker.t if tracker is not None else None,
+                tracks_ptr, track_counts_ptr)
+        if st is not None:
+            self._check(self.lib.rf_redact_yuv_device_style(*args, C.byref(st)))
+            return
         p = RedactParams(int(blocks), float(margin))
-        self._check(self.lib.rf_redact_yuv_device(self.h, arr, n, dets_ptr, counts_ptr, sc.ctypes.data if sc is not None else None,
-                                                  tracker.t if tracker is not None else None, tracks_ptr, track_counts_ptr, C.byref(p)))
+        self._check(self.lib.rf_redact_yuv_device(*args, C.byref(p)))
 
     def redact_device(self, images, dets_ptr: int, counts_ptr: int, scales=None, tracker: Optional["Tracker"] = None,
-                      tracks_ptr: Optional[int] = None, track_counts_ptr: Optional[int] = None, blocks: int = 0, margin: float = 0.0):
+                      tracks_ptr: Optional[int] = None, track_counts_ptr: Optional[int] = None, blocks: int = 0, margin: float = 0.0,
+                      style: str = "mosaic", shape: str = "rect", detail: int = 0):
         """rf_redact_device: redact_yuv_device on u8 BGR HWC torch CUDA tensors (rows may be strided), in place."""
         n = len(images)
         ptrs, ws, hs, rs = self._device_images(images)
         sc = self._scales(scales, n)
+        st = redact_style(style, shape, blocks, detail, margin)
+        args = (self.h, ptrs, ws, hs, rs, n, dets_ptr, counts_ptr, sc.ctypes.data if sc is not None else None,
+                tracker.t if tracker is not None else None, tracks_ptr, track_counts_ptr)
+        if st is not None:
+            self._check(self.lib.rf_redact_device_style(*args, C.byref(st)))
+            return
         p = RedactParams(int(blocks), float(margin))
-        self._check(self.lib.rf_redact_device(self.h, ptrs, ws, hs, rs, n, dets_ptr, counts_ptr, sc.ctypes.data if sc is not None else None,
-                                              tracker.t if tracker is not None else None, tracks_ptr, track_counts_ptr, C.byref(p)))
+        self._check(self.lib.rf_redact_device(*args, C.byref(p)))
 
     def detect_yuv_redact_device(self, frames, thr: float, nms_thr: float, layout: str = "nv12", matrix="bt601", blocks: int = 0,
-                                 margin: float = 0.0):
+                                 margin: float = 0.0, style: str = "mosaic", shape: str = "rect", detail: int = 0):
         """rf_detect_yuv_redact_device without a tracker: detect_yuv_device, then redact_yuv_device of its records on the same
         context.  Returns (dets_ptr, counts_ptr, scales) as detect_yuv_device; the frames are redacted in place."""
         n = len(frames)
         arr = self._frames(frames, layout, True)
-        p = RedactParams(int(blocks), float(margin))
+        fn, p = _redact_call(self.lib, style, shape, blocks, detail, margin)
         scales = np.zeros(max(n, 1), dtype=np.float32)
         d, c = C.c_void_p(), C.c_void_p()
-        self._check(self.lib.rf_detect_yuv_redact_device(self.h, None, arr, None, n, _matrix(matrix), thr, nms_thr, C.byref(p), None, None,
-                                                         C.byref(d), C.byref(c), scales.ctypes.data))
+        self._check(fn(self.h, None, arr, None, n, _matrix(matrix), thr, nms_thr, C.byref(p), None, None, C.byref(d), C.byref(c),
+                       scales.ctypes.data))
         return int(d.value or 0), int(c.value or 0), scales[:n].copy()
 
     def calibrate_int8(self, images: np.ndarray, out_table: str):
@@ -1231,16 +1276,16 @@ class Tracker:
                 scales[:n].copy())
 
     def detect_yuv_redact_device(self, frames, videos: Sequence[int], thr: float, nms_thr: float, layout: str = "nv12", matrix="bt601",
-                                 blocks: int = 0, margin: float = 0.0):
+                                 blocks: int = 0, margin: float = 0.0, style: str = "mosaic", shape: str = "rect", detail: int = 0):
         """rf_detect_yuv_redact_device with this tracker: detect_yuv_device (no crops), the update, then the redaction of every record and
         every LOST track, in place.  Returns (tracks_ptr, track_counts_ptr, dets_ptr, counts_ptr, scales) as detect_yuv_device."""
         n = len(frames)
         arr = self.engine._frames(frames, layout, True)
-        p = RedactParams(int(blocks), float(margin))
+        fn, p = _redact_call(self.lib, style, shape, blocks, detail, margin)
         scales = np.zeros(max(n, 1), dtype=np.float32)
         tp, tc, d, c = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
-        self.engine._check(self.lib.rf_detect_yuv_redact_device(self.engine.h, self.t, arr, self._ints(videos, n), n, _matrix(matrix), thr, nms_thr,
-                                                                C.byref(p), C.byref(tp), C.byref(tc), C.byref(d), C.byref(c), scales.ctypes.data))
+        self.engine._check(fn(self.engine.h, self.t, arr, self._ints(videos, n), n, _matrix(matrix), thr, nms_thr, C.byref(p), C.byref(tp),
+                              C.byref(tc), C.byref(d), C.byref(c), scales.ctypes.data))
         return int(tp.value or 0), int(tc.value or 0), int(d.value or 0), int(c.value or 0), scales[:n].copy()
 
     def finish(self, video: int, dev_best_crops_ptr: int, dev_best_mats_ptr: Optional[int] = None):

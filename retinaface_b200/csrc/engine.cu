@@ -2398,16 +2398,53 @@ int rf_tracker_debug_state(rf_tracker t, int video, double *out, int cap) {
 
 // ---- f12 redaction (redact.cuh) -------------------------------------------------------------------------------------------------
 extern "C++" {
-// params (NULL: defaults) -> blocks and margin
-static int redact_params(rf_handle h, const char *who, const rf_redact_params *p, int &blocks, double &margin) {
-    blocks = p && p->blocks ? p->blocks : 8;
-    const float m = p && p->margin != 0.f ? p->margin : 0.25f;
-    if (blocks < 1 || blocks > REDACT_MAX_BLOCKS)
-        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: blocks %d, must be 0 or in [1, %d]", who, blocks, REDACT_MAX_BLOCKS));
+// A call's resolved style: f12's params are {MOSAIC, RECT, blocks, detail 0}.
+struct RedactSpec {
+    int kind = REDACT_MOSAIC, shape = REDACT_RECT, blocks = 8, detail = 0;
+    double margin = 0.25;
+};
+
+static int redact_margin(rf_handle h, const char *who, float margin, double &out) {
+    const float m = margin != 0.f ? margin : 0.25f;
     if (!(std::isfinite(m) && m > 0.f && m <= 1.f))
         return fail(h, RF_ERR_INVALID_ARG, fmt("%s: margin %g, must be 0 or finite in (0, 1]", who, (double)m));
-    margin = (double)m;
+    out = (double)m;
     return RF_OK;
+}
+
+// params (NULL: defaults) -> blocks and margin
+static int redact_params(rf_handle h, const char *who, const rf_redact_params *p, RedactSpec &r) {
+    r = RedactSpec{};
+    r.blocks = p && p->blocks ? p->blocks : 8;
+    if (r.blocks < 1 || r.blocks > REDACT_MAX_BLOCKS)
+        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: blocks %d, must be 0 or in [1, %d]", who, r.blocks, REDACT_MAX_BLOCKS));
+    return redact_margin(h, who, p ? p->margin : 0.f, r.margin);
+}
+
+// style (NULL: the zeroed struct) -> kind, shape, blocks, detail and margin
+static int redact_style(rf_handle h, const char *who, const rf_redact_style *st, RedactSpec &r) {
+    const rf_redact_style z{};
+    if (!st) st = &z;
+    r = RedactSpec{};
+    r.kind = st->kind ? st->kind : REDACT_BLUR;
+    r.shape = st->shape ? st->shape : REDACT_ELLIPSE;
+    if (r.kind != REDACT_MOSAIC && r.kind != REDACT_BLUR)
+        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: kind %d, must be 0, RF_REDACT_MOSAIC or RF_REDACT_BLUR", who, st->kind));
+    if (r.shape != REDACT_RECT && r.shape != REDACT_ELLIPSE)
+        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: shape %d, must be 0, RF_REDACT_RECT or RF_REDACT_ELLIPSE", who, st->shape));
+    if (r.kind == REDACT_MOSAIC) {
+        if (st->detail) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: detail %d, must be 0 for the mosaic", who, st->detail));
+        r.blocks = st->blocks ? st->blocks : 8;
+        if (r.blocks < 1 || r.blocks > REDACT_MAX_BLOCKS)
+            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: blocks %d, must be 0 or in [1, %d]", who, r.blocks, REDACT_MAX_BLOCKS));
+    } else {
+        if (st->blocks) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: blocks %d, must be 0 for the blur", who, st->blocks));
+        r.blocks = 1;         // the geometry's cell side, unused by the blur
+        r.detail = st->detail ? st->detail : 4;
+        if (r.detail < 1 || r.detail > BLUR_MAX_DETAIL)
+            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: detail %d, must be 0 or in [1, %d]", who, r.detail, BLUR_MAX_DETAIL));
+    }
+    return redact_margin(h, who, st->margin, r.margin);
 }
 
 // The records, scales and tracks of a redaction call.
@@ -2468,14 +2505,17 @@ static Ctx &last_ctx(rf_handle h) {
 }
 
 // Issues the redaction of `frames` on context c's stream, into c's scratch (sized for max_batch frames of this call's region
-// capacity and blocks; a larger need waits for the context before the scratch is replaced).
+// capacity and blocks, and for BLUR the frames' scratch planes; a larger need waits for the context before the scratch is replaced).
 template <typename Dst>
-static void redact_issue(rf_handle h, Ctx &c, const std::vector<RedactFrameT<Dst>> &frames, const rf_det *dets, const int32_t *counts, rf_tracker t,
-                         const rf_track *tracks, const int32_t *track_counts, int blocks, double margin) {
+static void redact_issue(rf_handle h, Ctx &c, std::vector<RedactFrameT<Dst>> frames, const rf_det *dets, const int32_t *counts, rf_tracker t,
+                         const rf_track *tracks, const int32_t *track_counts, const RedactSpec &spec) {
     RedactArgs a{};
     a.n = (int)frames.size();
-    a.blocks = blocks;
-    a.margin = margin;
+    a.blocks = spec.blocks;
+    a.margin = spec.margin;
+    a.kind = spec.kind;
+    a.shape = spec.shape;
+    a.detail = spec.detail;
     a.max_faces = h->cfg.max_faces;
     a.max_tracks = t ? t->cfg.max_tracks : 0;
     a.cap = a.max_faces + a.max_tracks;
@@ -2483,7 +2523,10 @@ static void redact_issue(rf_handle h, Ctx &c, const std::vector<RedactFrameT<Dst
     a.counts = counts;
     a.tracks = tracks;
     a.track_counts = track_counts;
-    const size_t need = redact_scratch_bytes(h->cfg.max_batch, a.cap, blocks);
+    const size_t tables = (redact_scratch_bytes(h->cfg.max_batch, a.cap, a.blocks) + 255) & ~(size_t)255;
+    size_t need = tables;
+    if (spec.kind == REDACT_BLUR)
+        for (const auto &f : frames) need += (blur_plane_bytes(std::is_same<Dst, YuvPlanesW>::value, f.w, f.h) + 255) & ~(size_t)255;
     if (need > c.redact_bytes) {
         CK(cudaStreamSynchronize(c.stream));
         CK(cudaFree(c.d_redact));
@@ -2493,6 +2536,13 @@ static void redact_issue(rf_handle h, Ctx &c, const std::vector<RedactFrameT<Dst
         c.redact_bytes = need;
     }
     redact_carve(a, c.d_redact);
+    if (spec.kind == REDACT_BLUR) {
+        size_t off = tables;
+        for (auto &f : frames) {
+            f.blur = static_cast<uint8_t *>(c.d_redact) + off;
+            off += (blur_plane_bytes(std::is_same<Dst, YuvPlanesW>::value, f.w, f.h) + 255) & ~(size_t)255;
+        }
+    }
     CK(launch_redact(a, frames.data(), h->num_sms, c.stream));
 }
 
@@ -2502,42 +2552,42 @@ static std::vector<RedactFrameT<YuvPlanesW>> yuv_redact_table(const rf_yuv_frame
         const rf_yuv_frame &f = frames[i];
         v[i] = RedactFrameT<YuvPlanesW>{YuvPlanesW{const_cast<uint8_t *>(f.y), const_cast<uint8_t *>(f.u), const_cast<uint8_t *>(f.v), f.y_pitch,
                                                    f.uv_pitch, f.uv_step},
-                                        f.width, f.height, scales ? scales[i] : 1.f};
+                                        f.width, f.height, scales ? scales[i] : 1.f, nullptr};
     }
     return v;
 }
 }  // extern "C++"
 
-int rf_redact_yuv_device(rf_handle h, const rf_yuv_frame *frames, int n, const rf_det *dev_dets, const int32_t *dev_counts, const float *scales,
-                         rf_tracker t, const rf_track *dev_tracks, const int32_t *dev_track_counts, const rf_redact_params *params) {
-    static const char *who = "rf_redact_yuv_device";
+extern "C++" {
+// The f12 and f14 entry points share one implementation each: `resolve` checks the params or the style where f12 checks its params.
+template <typename Resolve>
+static int redact_yuv_impl(rf_handle h, const char *who, const rf_yuv_frame *frames, int n, const rf_det *dev_dets, const int32_t *dev_counts,
+                           const float *scales, rf_tracker t, const rf_track *dev_tracks, const int32_t *dev_track_counts, Resolve resolve) {
     if (!h) return RF_ERR_INVALID_ARG;
     int rc = check_frames(h, who, frames, n, RF_YUV_BT601);      // the matrix plays no part: the mosaic is per plane
     if (rc) return rc;
-    int blocks;
-    double margin;
-    if ((rc = redact_params(h, who, params, blocks, margin))) return rc;
+    RedactSpec spec;
+    if ((rc = resolve(spec))) return rc;
     if ((rc = check_redact_inputs(h, who, n, dev_dets, dev_counts, scales, t, dev_tracks, dev_track_counts))) return rc;
     if ((rc = check_disjoint(h, who, yuv_ranges(frames, n)))) return rc;
     if (n == 0) return RF_OK;
     try {
         CK(cudaSetDevice(h->device));
-        redact_issue(h, last_ctx(h), yuv_redact_table(frames, n, scales), dev_dets, dev_counts, t, dev_tracks, dev_track_counts, blocks, margin);
+        redact_issue(h, last_ctx(h), yuv_redact_table(frames, n, scales), dev_dets, dev_counts, t, dev_tracks, dev_track_counts, spec);
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }
 
-int rf_redact_device(rf_handle h, uint8_t *const *dev_bgr, const int *widths, const int *heights, const int *row_strides, int n,
-                     const rf_det *dev_dets, const int32_t *dev_counts, const float *scales, rf_tracker t, const rf_track *dev_tracks,
-                     const int32_t *dev_track_counts, const rf_redact_params *params) {
-    static const char *who = "rf_redact_device";
+template <typename Resolve>
+static int redact_bgr_impl(rf_handle h, const char *who, uint8_t *const *dev_bgr, const int *widths, const int *heights, const int *row_strides,
+                           int n, const rf_det *dev_dets, const int32_t *dev_counts, const float *scales, rf_tracker t, const rf_track *dev_tracks,
+                           const int32_t *dev_track_counts, Resolve resolve) {
     if (!h) return RF_ERR_INVALID_ARG;
     const BgrImages src{dev_bgr, widths, heights, row_strides, nullptr, false};
     int rc = src.check(h, who, n);
     if (rc) return rc;
-    int blocks;
-    double margin;
-    if ((rc = redact_params(h, who, params, blocks, margin))) return rc;
+    RedactSpec spec;
+    if ((rc = resolve(spec))) return rc;
     if ((rc = check_redact_inputs(h, who, n, dev_dets, dev_counts, scales, t, dev_tracks, dev_track_counts))) return rc;
     std::vector<std::array<uintptr_t, 3>> ranges;
     for (int i = 0; i < n; i++) {
@@ -2549,16 +2599,16 @@ int rf_redact_device(rf_handle h, uint8_t *const *dev_bgr, const int *widths, co
     try {
         CK(cudaSetDevice(h->device));
         std::vector<RedactFrameT<BgrRowsW>> v(n);
-        for (int i = 0; i < n; i++) v[i] = RedactFrameT<BgrRowsW>{BgrRowsW{dev_bgr[i], src.stride(i)}, widths[i], heights[i], scales ? scales[i] : 1.f};
-        redact_issue(h, last_ctx(h), v, dev_dets, dev_counts, t, dev_tracks, dev_track_counts, blocks, margin);
+        for (int i = 0; i < n; i++) v[i] = RedactFrameT<BgrRowsW>{BgrRowsW{dev_bgr[i], src.stride(i)}, widths[i], heights[i], scales ? scales[i] : 1.f, nullptr};
+        redact_issue(h, last_ctx(h), v, dev_dets, dev_counts, t, dev_tracks, dev_track_counts, spec);
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }
 
-int rf_detect_yuv_redact_device(rf_handle h, rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, int matrix, float thr, float nms,
-                                const rf_redact_params *params, const rf_track **dev_tracks, const int32_t **dev_track_counts,
-                                const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales) {
-    static const char *who = "rf_detect_yuv_redact_device";
+template <typename Resolve>
+static int detect_yuv_redact_impl(rf_handle h, const char *who, rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, int matrix,
+                                  float thr, float nms, Resolve resolve, const rf_track **dev_tracks, const int32_t **dev_track_counts,
+                                  const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales) {
     if (!h) return RF_ERR_INVALID_ARG;
     int rc;
     if (t) {
@@ -2568,9 +2618,8 @@ int rf_detect_yuv_redact_device(rf_handle h, rf_tracker t, const rf_yuv_frame *f
     }
     const YuvFrames src{frames, matrix, nullptr, false};
     if ((rc = src.check(h, who, n))) return rc;
-    int blocks;
-    double margin;
-    if ((rc = redact_params(h, who, params, blocks, margin))) return rc;
+    RedactSpec spec;
+    if ((rc = resolve(spec))) return rc;
     if ((rc = check_disjoint(h, who, yuv_ranges(frames, n)))) return rc;
     if (n == 0) return RF_OK;
     std::vector<float> scales(n);
@@ -2587,9 +2636,57 @@ int rf_detect_yuv_redact_device(rf_handle h, rf_tracker t, const rf_yuv_frame *f
         if (t) track_issue(t, videos, n, dets, counts, scales.data(), c.stream, nullptr, nullptr, &tracks, &track_counts, frames);
         if (dev_tracks) *dev_tracks = tracks;
         if (dev_track_counts) *dev_track_counts = track_counts;
-        redact_issue(h, c, yuv_redact_table(frames, n, scales.data()), dets, counts, t, tracks, track_counts, blocks, margin);
+        redact_issue(h, c, yuv_redact_table(frames, n, scales.data()), dets, counts, t, tracks, track_counts, spec);
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
+}
+
+}  // extern "C++"
+
+int rf_redact_yuv_device(rf_handle h, const rf_yuv_frame *frames, int n, const rf_det *dev_dets, const int32_t *dev_counts, const float *scales,
+                         rf_tracker t, const rf_track *dev_tracks, const int32_t *dev_track_counts, const rf_redact_params *params) {
+    static const char *who = "rf_redact_yuv_device";
+    return redact_yuv_impl(h, who, frames, n, dev_dets, dev_counts, scales, t, dev_tracks, dev_track_counts,
+                           [&](RedactSpec &r) { return redact_params(h, who, params, r); });
+}
+
+int rf_redact_yuv_device_style(rf_handle h, const rf_yuv_frame *frames, int n, const rf_det *dev_dets, const int32_t *dev_counts, const float *scales,
+                               rf_tracker t, const rf_track *dev_tracks, const int32_t *dev_track_counts, const rf_redact_style *style) {
+    static const char *who = "rf_redact_yuv_device_style";
+    return redact_yuv_impl(h, who, frames, n, dev_dets, dev_counts, scales, t, dev_tracks, dev_track_counts,
+                           [&](RedactSpec &r) { return redact_style(h, who, style, r); });
+}
+
+int rf_redact_device(rf_handle h, uint8_t *const *dev_bgr, const int *widths, const int *heights, const int *row_strides, int n,
+                     const rf_det *dev_dets, const int32_t *dev_counts, const float *scales, rf_tracker t, const rf_track *dev_tracks,
+                     const int32_t *dev_track_counts, const rf_redact_params *params) {
+    static const char *who = "rf_redact_device";
+    return redact_bgr_impl(h, who, dev_bgr, widths, heights, row_strides, n, dev_dets, dev_counts, scales, t, dev_tracks, dev_track_counts,
+                           [&](RedactSpec &r) { return redact_params(h, who, params, r); });
+}
+
+int rf_redact_device_style(rf_handle h, uint8_t *const *dev_bgr, const int *widths, const int *heights, const int *row_strides, int n,
+                           const rf_det *dev_dets, const int32_t *dev_counts, const float *scales, rf_tracker t, const rf_track *dev_tracks,
+                           const int32_t *dev_track_counts, const rf_redact_style *style) {
+    static const char *who = "rf_redact_device_style";
+    return redact_bgr_impl(h, who, dev_bgr, widths, heights, row_strides, n, dev_dets, dev_counts, scales, t, dev_tracks, dev_track_counts,
+                           [&](RedactSpec &r) { return redact_style(h, who, style, r); });
+}
+
+int rf_detect_yuv_redact_device(rf_handle h, rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, int matrix, float thr, float nms,
+                                const rf_redact_params *params, const rf_track **dev_tracks, const int32_t **dev_track_counts,
+                                const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales) {
+    static const char *who = "rf_detect_yuv_redact_device";
+    return detect_yuv_redact_impl(h, who, t, frames, videos, n, matrix, thr, nms, [&](RedactSpec &r) { return redact_params(h, who, params, r); },
+                                  dev_tracks, dev_track_counts, dev_dets, dev_counts, out_scales);
+}
+
+int rf_detect_yuv_redact_device_style(rf_handle h, rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, int matrix, float thr,
+                                      float nms, const rf_redact_style *style, const rf_track **dev_tracks, const int32_t **dev_track_counts,
+                                      const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales) {
+    static const char *who = "rf_detect_yuv_redact_device_style";
+    return detect_yuv_redact_impl(h, who, t, frames, videos, n, matrix, thr, nms, [&](RedactSpec &r) { return redact_style(h, who, style, r); },
+                                  dev_tracks, dev_track_counts, dev_dets, dev_counts, out_scales);
 }
 
 }  // extern "C"

@@ -42,11 +42,40 @@ __device__ int block_scan(int v, int *total, int *s_w) {
     return pre + incl - v;
 }
 
+// Blur work items: strips of BLUR_W output columns x bands of BLUR_H rows.  s_v holds a band's vertical sums for its strip and the
+// strip's 3a-column halo on each side at a <= 127; its row stride is odd, so that one thread per row reads it without bank conflicts.
+constexpr int BLUR_W = 32, BLUR_H = 32, BLUR_STRIDE = BLUR_W + 6 * BLUR_MAX_RADIUS + 1, BLUR_COVER = 128;
+constexpr size_t BLUR_SMEM = sizeof(uint32_t) * BLUR_H * BLUR_STRIDE;
+constexpr int BLUR_UNROLL = 8;
+__host__ __device__ __forceinline__ int blur_items(int cw, int ch) { return ((cw + BLUR_W - 1) / BLUR_W) * ((ch + BLUR_H - 1) / BLUR_H); }
+
+// The header's ellipse test of plane sample (x, y) in [x0, x1) x [y0, y1): u^2 H^2 + v^2 W^2 <= W^2 H^2 in exact integers.  With the
+// +-65536 clamp W^2 H^2 reaches about 3e20, so the products are 128-bit; |u| < W and |v| < H keep u^2 and v^2 in 64 bits.
+__device__ __forceinline__ bool in_ellipse(int x0, int y0, int x1, int y1, int x, int y) {
+    using u128 = unsigned __int128;
+    const long long W = x1 - x0, H = y1 - y0, u = 2LL * x + 1 - x0 - x1, v = 2LL * y + 1 - y0 - y1;
+    const unsigned long long W2 = W * W, H2 = H * H;
+    return (u128)(unsigned long long)(u * u) * H2 + (u128)(unsigned long long)(v * v) * W2 <= (u128)W2 * H2;
+}
+
+// Whether the shape of a region with luma rectangle o = (x0, y0, x1, y1) covers sample (x, y) of a plane subsampled by 2^s (the
+// rectangle halved for chroma; every bound is even).  RECT is f12's test, unchanged.
+template <bool kEllipse>
+__device__ __forceinline__ bool shape_covers(int4 o, int s, int x, int y) {
+    if constexpr (!kEllipse) {
+        const int X = x << s, Y = y << s;
+        return X >= o.x && X < o.z && Y >= o.y && Y < o.w;
+    } else {
+        const int x0 = o.x >> s, y0 = o.y >> s, x1 = o.z >> s, y1 = o.w >> s;
+        return x >= x0 && x < x1 && y >= y0 && y < y1 && in_ellipse(x0, y0, x1, y1, x, y);
+    }
+}
+
 // The header's geometry of one box in frame pixels; false: the box is skipped.  mi / ai: the region's measure and apply items (0
 // when its rectangle misses the frame).  The clamps beyond +-65536 keep the integers in range without changing any non-empty
 // rectangle: a bound past them already makes the rectangle empty.
 __device__ bool region_geometry(float fx1, float fy1, float fx2, float fy2, double margin, int blocks, int W, int H, RedactRegion &g, int &mi,
-                                int &ai) {
+                                int &ai, int kind, int detail, bool yuv) {
     if (!(isfinite(fx1) && isfinite(fy1) && isfinite(fx2) && isfinite(fy2))) return false;
     const double x1 = fx1, y1 = fy1, x2 = fx2, y2 = fy2;
     const double w = x2 - x1, h = y2 - y1;
@@ -66,13 +95,17 @@ __device__ bool region_geometry(float fx1, float fy1, float fx2, float fy2, doub
         g.cr0 = (cy0 - g.y0) / g.c;
         mi = (cy1 - 1 - g.y0) / g.c - g.cr0 + 1;
         ai = (cy1 - cy0 + REDACT_BAND - 1) / REDACT_BAND;
+        if (kind == REDACT_BLUR)      // blur items: every plane's strips x bands (YUV: luma, then U and V halved; BGR: one per channel)
+            mi = yuv ? blur_items(cx1 - cx0, cy1 - cy0) + 2 * blur_items((cx1 - cx0) >> 1, (cy1 - cy0) >> 1) : 3 * blur_items(cx1 - cx0, cy1 - cy0);
     }
+    g.rad = kind == REDACT_BLUR ? min(max(D > 0 ? (D + 2 * detail - 1) / (2 * detail) : 0, 1), BLUR_MAX_RADIUS) : 0;
     return true;
 }
 
 template <typename Table>
 __global__ void __launch_bounds__(REDACT_THREADS) k_redact_regions(const RedactArgs a, const __grid_constant__ Table table) {
     __shared__ int s_w[3][REDACT_THREADS / 32];
+    constexpr bool kYuv = std::is_same<typename Table::Dst, YuvPlanesW>::value;
     const int i = blockIdx.x;
     const auto &fr = table.f[i];
     const int na = min(max(a.counts[i], 0), a.max_faces);
@@ -86,10 +119,10 @@ __global__ void __launch_bounds__(REDACT_THREADS) k_redact_regions(const RedactA
         if (k < na) {
             const rf_face &f = a.dets[(size_t)i * a.max_faces + k].face;
             ok = region_geometry(__fmul_rn(f.x1, fr.scale), __fmul_rn(f.y1, fr.scale), __fmul_rn(f.x2, fr.scale), __fmul_rn(f.y2, fr.scale), a.margin,
-                                 a.blocks, fr.w, fr.h, g, mi, ai);
+                                 a.blocks, fr.w, fr.h, g, mi, ai, a.kind, a.detail, kYuv);
         } else if (k < na + nb) {
             const rf_track &t = a.tracks[(size_t)i * a.max_tracks + (k - na)];
-            ok = t.state == RF_TRACK_LOST && region_geometry(t.kx1, t.ky1, t.kx2, t.ky2, a.margin, a.blocks, fr.w, fr.h, g, mi, ai);
+            ok = t.state == RF_TRACK_LOST && region_geometry(t.kx1, t.ky1, t.kx2, t.ky2, a.margin, a.blocks, fr.w, fr.h, g, mi, ai, a.kind, a.detail, kYuv);
         }
         int tr, tm, ta;
         const int pr = block_scan(ok ? 1 : 0, &tr, s_w[0]);
@@ -216,14 +249,21 @@ __global__ void __launch_bounds__(REDACT_THREADS) k_redact_measure(const RedactA
     }
 }
 
+// The blur scratch planes of a YUV frame: plane p (0 Y, 1 U, 2 V), rows w >> s apart.
+__device__ __forceinline__ uint8_t *blur_yuv_plane(uint8_t *b, int w, int h, int p) {
+    return p == 0 ? b : b + (size_t)w * h + (size_t)(p - 1) * (w / 2) * (h / 2);
+}
+
 // One band of REDACT_BAND rows of one region per work item: the lower-index rectangles that reach the band go to shared memory, then
-// every pixel of the band they do not cover takes its cell value -- luma first, then the band's chroma rows.
-template <typename Table>
+// every pixel of the band they do not cover takes its cell value -- luma first, then the band's chroma rows.  kEllipse: a sample is
+// written only where the region's ellipse covers it, and only the lower-index ellipses take it away.  kBlur: the value is the
+// sample's blurred value in the frame's scratch planes instead of its cell value.
+template <typename Table, bool kEllipse = false, bool kBlur = false>
 __global__ void __launch_bounds__(REDACT_THREADS) k_redact_apply(const RedactArgs a, const __grid_constant__ Table table) {
     using Dst = typename Table::Dst;
     __shared__ int s_first[Table::kMax + 1];
     __shared__ int4 s_rect[REDACT_COVER];
-    __shared__ uint8_t s_cells[REDACT_MAX_BLOCKS * REDACT_MAX_BLOCKS * 3];
+    __shared__ uint8_t s_cells[kBlur ? 1 : REDACT_MAX_BLOCKS * REDACT_MAX_BLOCKS * 3];
     __shared__ int s_nrect;
     constexpr bool kYuv = std::is_same<Dst, YuvPlanesW>::value;
     frame_firsts(a, 2, s_first);
@@ -249,20 +289,22 @@ __global__ void __launch_bounds__(REDACT_THREADS) k_redact_apply(const RedactArg
         // the region's cell values: one round trip here instead of one per pixel below
         const uint8_t *cg = a.cells + ((size_t)i * a.cap + r) * bb * 3;
         const int ny = (g.y1 - g.y0 + c - 1) / c;
-        for (int t = threadIdx.x; t < nx * ny * 3; t += REDACT_THREADS) s_cells[t] = cg[t];
+        if constexpr (!kBlur)
+            for (int t = threadIdx.x; t < nx * ny * 3; t += REDACT_THREADS) s_cells[t] = cg[t];
         __syncthreads();
         const int nrect = s_nrect;
-        auto covered = [&](int x, int y) {
+        const int4 own = make_int4(g.x0, g.y0, g.x1, g.y1);
+        // (x, y): a sample of a plane subsampled by 2^s; true when the sample is not this region's to write
+        auto covered = [&](int x, int y, int s) {
+            if (kEllipse && !shape_covers<true>(own, s, x, y)) return true;
             if (nrect <= REDACT_COVER) {
-                for (int j = 0; j < nrect; j++) {
-                    const int4 o = s_rect[j];
-                    if (x >= o.x && x < o.z && y >= o.y && y < o.w) return true;
-                }
+                for (int j = 0; j < nrect; j++)
+                    if (shape_covers<kEllipse>(s_rect[j], s, x, y)) return true;
                 return false;
             }
             for (int q = 0; q < r; q++) {
                 const RedactRegion &o = R[q];
-                if (x >= o.x0 && x < o.x1 && y >= o.y0 && y < o.y1) return true;
+                if (shape_covers<kEllipse>(make_int4(o.x0, o.y0, o.x1, o.y1), s, x, y)) return true;
             }
             return false;
         };
@@ -272,24 +314,30 @@ __global__ void __launch_bounds__(REDACT_THREADS) k_redact_apply(const RedactArg
             const YuvPlanesW &p = fr.dst;
             for (int t = threadIdx.x; t < rows * bw; t += REDACT_THREADS) {
                 const int y = by0 + t / bw, x = cx0 + t % bw;
-                if (covered(x, y)) continue;
-                p.y[(size_t)y * p.y_pitch + x] = cv[((y - g.y0) / c * nx + (x - g.x0) / c) * 3];
+                if (covered(x, y, 0)) continue;
+                p.y[(size_t)y * p.y_pitch + x] = kBlur ? fr.blur[(size_t)y * fr.w + x] : cv[((y - g.y0) / c * nx + (x - g.x0) / c) * 3];
             }
             const int hw = bw >> 1;
             for (int t = threadIdx.x; t < (rows >> 1) * hw; t += REDACT_THREADS) {
                 const int y = (by0 >> 1) + t / hw, x = (cx0 >> 1) + t % hw;
-                if (covered(2 * x, 2 * y)) continue;
-                const uint8_t *v = cv + ((2 * y - g.y0) / c * nx + (2 * x - g.x0) / c) * 3;
+                if (covered(x, y, 1)) continue;
                 const size_t o = (size_t)y * p.uv_pitch + (size_t)x * p.uv_step;
-                p.u[o] = v[1];
-                p.v[o] = v[2];
+                if constexpr (kBlur) {
+                    const size_t b = (size_t)y * (fr.w / 2) + x;
+                    p.u[o] = blur_yuv_plane(fr.blur, fr.w, fr.h, 1)[b];
+                    p.v[o] = blur_yuv_plane(fr.blur, fr.w, fr.h, 2)[b];
+                } else {
+                    const uint8_t *v = cv + ((2 * y - g.y0) / c * nx + (2 * x - g.x0) / c) * 3;
+                    p.u[o] = v[1];
+                    p.v[o] = v[2];
+                }
             }
         } else {
             const BgrRowsW &p = fr.dst;
             for (int t = threadIdx.x; t < rows * bw; t += REDACT_THREADS) {
                 const int y = by0 + t / bw, x = cx0 + t % bw;
-                if (covered(x, y)) continue;
-                const uint8_t *v = cv + ((y - g.y0) / c * nx + (x - g.x0) / c) * 3;
+                if (covered(x, y, 0)) continue;
+                const uint8_t *v = kBlur ? fr.blur + (size_t)y * 3 * fr.w + 3 * (size_t)x : cv + ((y - g.y0) / c * nx + (x - g.x0) / c) * 3;
                 uint8_t *q = p.p + (size_t)y * p.pitch + 3 * (size_t)x;
                 q[0] = v[0];
                 q[1] = v[1];
@@ -297,6 +345,156 @@ __global__ void __launch_bounds__(REDACT_THREADS) k_redact_apply(const RedactArg
             }
         }
         __syncthreads();     // s_rect / s_nrect of the next item
+    }
+}
+
+// One (region, plane, strip, band) per work item: the blur of the strip's output columns [tx0, tx1) over the band's rows [ty0, ty1),
+// from the ORIGINAL plane, into the frame's scratch planes at every sample the region owns.  The kernel k (6a + 1 taps) is three
+// boxes of n = 2a + 1, so k = (1 - z^n)^3 / (1 - z)^3: each axis is the signed combination q(t) - 3 q(t - n) + 3 q(t - 2n) - q(t - 3n)
+// of the clamped samples, summed three times.  Modular arithmetic makes every step exact -- u32 vertically (a column sum is at most
+// 255^4 < 2^32), u64 horizontally (S is at most 255^7 < 2^63).  Vertical first, one thread per column of the strip and its 3a-column
+// halo (coalesced reads across the warp), into s_v; then one thread per row of the band along s_v.
+template <typename Table, bool kEllipse>
+__global__ void __launch_bounds__(REDACT_THREADS, 2) k_redact_blur(const RedactArgs a, const __grid_constant__ Table table) {
+    using Dst = typename Table::Dst;
+    extern __shared__ uint32_t s_v[];           // [BLUR_H][BLUR_STRIDE]
+    __shared__ int s_first[Table::kMax + 1];
+    __shared__ int4 s_rect[BLUR_COVER];
+    __shared__ int s_nrect;
+    constexpr bool kYuv = std::is_same<Dst, YuvPlanesW>::value;
+    frame_firsts(a, 1, s_first);
+    const int items = s_first[a.n];
+    for (int item = blockIdx.x; item < items; item += gridDim.x) {
+        int i, r, k;
+        locate(a, s_first, item, &RedactRegion::m_first, i, r, k);
+        const auto &fr = table.f[i];
+        const RedactRegion *R = a.regions + (size_t)i * a.cap;
+        const RedactRegion g = R[r];
+        const int cx0 = max(g.x0, 0), cx1 = min(g.x1, fr.w), cy0 = max(g.y0, 0), cy1 = min(g.y1, fr.h);
+        int j = k - g.m_first, p = 0, s = 0;
+        const int n0 = blur_items(cx1 - cx0, cy1 - cy0);
+        if (j >= n0) {
+            if constexpr (kYuv) {
+                const int n1 = blur_items((cx1 - cx0) >> 1, (cy1 - cy0) >> 1);
+                s = 1;
+                p = 1 + (j - n0) / n1;
+                j = (j - n0) % n1;
+            } else {
+                p = j / n0;
+                j %= n0;
+            }
+        }
+        const uint8_t *src;
+        uint8_t *dst;
+        int pitch, step, pw, ph, dpitch, dstep;
+        if constexpr (kYuv) {
+            const YuvPlanesW &d = fr.dst;
+            src = p == 0 ? d.y : p == 1 ? d.u : d.v;
+            pitch = p ? d.uv_pitch : d.y_pitch;
+            step = p ? d.uv_step : 1;
+            pw = fr.w >> s;
+            ph = fr.h >> s;
+            dst = blur_yuv_plane(fr.blur, fr.w, fr.h, p);
+            dpitch = pw;
+            dstep = 1;
+        } else {
+            src = fr.dst.p + p;
+            pitch = fr.dst.pitch;
+            step = 3;
+            pw = fr.w;
+            ph = fr.h;
+            dst = fr.blur + p;
+            dpitch = 3 * fr.w;
+            dstep = 3;
+        }
+        const int ra = s ? (g.rad + 1) >> 1 : g.rad, n = 2 * ra + 1, h3 = 3 * ra;
+        const int px0 = cx0 >> s, px1 = cx1 >> s, py0 = cy0 >> s, py1 = cy1 >> s;
+        const int ns = (px1 - px0 + BLUR_W - 1) / BLUR_W;
+        const int tx0 = px0 + (j % ns) * BLUR_W, tx1 = min(tx0 + BLUR_W, px1);
+        const int ty0 = py0 + (j / ns) * BLUR_H, ty1 = min(ty0 + BLUR_H, py1);
+        if (threadIdx.x == 0) s_nrect = 0;
+        __syncthreads();
+        const int lx0 = tx0 << s, lx1 = tx1 << s, ly0 = ty0 << s, ly1 = ty1 << s;
+        for (int q = threadIdx.x; q < r; q += REDACT_THREADS) {
+            const RedactRegion o = R[q];
+            if (o.x0 < lx1 && o.x1 > lx0 && o.y0 < ly1 && o.y1 > ly0) {
+                const int slot = atomicAdd(&s_nrect, 1);
+                if (slot < BLUR_COVER) s_rect[slot] = make_int4(o.x0, o.y0, o.x1, o.y1);
+            }
+        }
+        const int tw = tx1 - tx0, th = ty1 - ty0, cols = tw + 2 * h3, lv = th + 2 * h3;
+        // vertical: s_v[y][c] = sum_j k[j] P[clampY(ty0 + y + j)][clampX(tx0 - 3a + c)]
+        // BLUR_UNROLL steps' loads are issued before their sums (the row index is clamped, so every load is in the plane)
+        for (int c = threadIdx.x; c < cols; c += REDACT_THREADS) {
+            const uint8_t *col = src + (size_t)min(max(tx0 - h3 + c, 0), pw - 1) * step;
+            const int ys = ty0 - h3;
+            auto q = [&](int t) -> unsigned { return t >= 0 ? (unsigned)__ldg(col + (size_t)min(max(ys + t, 0), ph - 1) * pitch) : 0u; };
+            unsigned c1 = 0, c2 = 0, c3 = 0;
+            for (int t0 = 0; t0 < lv; t0 += BLUR_UNROLL) {
+                unsigned d[BLUR_UNROLL];
+#pragma unroll
+                for (int u = 0; u < BLUR_UNROLL; u++) d[u] = q(t0 + u) - 3u * q(t0 + u - n) + 3u * q(t0 + u - 2 * n) - q(t0 + u - 3 * n);
+#pragma unroll
+                for (int u = 0; u < BLUR_UNROLL; u++) {
+                    const int t = t0 + u;
+                    c1 += d[u];
+                    c2 += c1;
+                    c3 += c2;
+                    if (t >= 2 * h3 && t < lv) s_v[(t - 2 * h3) * BLUR_STRIDE + c] = c3;
+                }
+            }
+        }
+        __syncthreads();
+        const int nrect = s_nrect;
+        const int4 own = make_int4(g.x0, g.y0, g.x1, g.y1);
+        auto owned = [&](int x, int y) {
+            if (kEllipse && !shape_covers<true>(own, s, x, y)) return false;
+            if (nrect <= BLUR_COVER) {
+                for (int e = 0; e < nrect; e++)
+                    if (shape_covers<kEllipse>(s_rect[e], s, x, y)) return false;
+                return true;
+            }
+            for (int q = 0; q < r; q++) {
+                const RedactRegion &o = R[q];
+                if (shape_covers<kEllipse>(make_int4(o.x0, o.y0, o.x1, o.y1), s, x, y)) return false;
+            }
+            return true;
+        };
+        // horizontal: S = sum_i k[i] s_v[y][3a + x - tx0 + i], rounded
+        // The rounding (S + half) / n^6 as an FP64 estimate corrected in integers: the quotient is at most 255 and S + half < 2^63, so
+        // the estimate is within one of the exact quotient, and the two corrections make it exact.
+        const unsigned long long n2 = (unsigned long long)n * n, n6 = n2 * n2 * n2, half = (n6 - 1) / 2;
+        const double inv6 = 1.0 / (double)n6;
+        for (int yy = threadIdx.x; yy < th; yy += REDACT_THREADS) {
+            const uint32_t *row = s_v + yy * BLUR_STRIDE;
+            auto q = [&](int t) -> unsigned long long { return t >= 0 && t < cols ? (unsigned long long)row[t] : 0ull; };
+            unsigned long long c1 = 0, c2 = 0, c3 = 0;
+            const int y = ty0 + yy;
+            for (int t0 = 0; t0 < cols; t0 += BLUR_UNROLL) {
+                unsigned long long d[BLUR_UNROLL];
+#pragma unroll
+                for (int u = 0; u < BLUR_UNROLL; u++)
+                    d[u] = q(t0 + u) - 3ull * q(t0 + u - n) + 3ull * q(t0 + u - 2 * n) - q(t0 + u - 3 * n);
+#pragma unroll
+                for (int u = 0; u < BLUR_UNROLL; u++) {
+                    const int t = t0 + u;
+                    c1 += d[u];
+                    c2 += c1;
+                    c3 += c2;
+                    if (t >= 2 * h3 && t < cols) {
+                        const int x = tx0 + t - 2 * h3;
+                        if (owned(x, y)) {
+                            const unsigned long long v = c3 + half;
+                            unsigned long long r = (unsigned long long)((double)v * inv6);
+                            if (r * n6 > v) r--;
+                            if ((r + 1) * n6 <= v) r++;
+                            dst[(size_t)y * dpitch + (size_t)x * dstep] = (uint8_t)r;
+                        }
+                    }
+                }
+            }
+        }
+        __syncthreads();     // s_v, s_rect and s_nrect of the next item
     }
 }
 
@@ -322,6 +520,11 @@ template <typename Dst>
 cudaError_t launch_redact(const RedactArgs &a, const RedactFrameT<Dst> *frames, int num_sms, cudaStream_t s) {
     constexpr int kMax = redact_table_limit<Dst>();
     const size_t cells = (size_t)a.blocks * a.blocks * 3;
+    if (a.kind == REDACT_BLUR) {      // s_v: above the 48 KB default
+        cudaError_t e = cudaFuncSetAttribute(k_redact_blur<RedactTable<Dst>, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BLUR_SMEM);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(k_redact_blur<RedactTable<Dst>, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BLUR_SMEM);
+        if (e != cudaSuccess) return e;
+    }
     for (int i0 = 0; i0 < a.n; i0 += kMax) {
         const int m = std::min(kMax, a.n - i0);
         RedactArgs c = a;
@@ -338,8 +541,17 @@ cudaError_t launch_redact(const RedactArgs &a, const RedactFrameT<Dst> *frames, 
         RedactTable<Dst> t{};
         for (int i = 0; i < m; i++) t.f[i] = frames[i0 + i];
         k_redact_regions<<<m, REDACT_THREADS, 0, s>>>(c, t);
-        k_redact_measure<<<2 * num_sms, REDACT_THREADS, 0, s>>>(c, t);
-        k_redact_apply<<<2 * num_sms, REDACT_THREADS, 0, s>>>(c, t);
+        const bool ell = a.shape == REDACT_ELLIPSE;
+        if (a.kind == REDACT_BLUR) {
+            if (ell) k_redact_blur<RedactTable<Dst>, true><<<2 * num_sms, REDACT_THREADS, BLUR_SMEM, s>>>(c, t);
+            else k_redact_blur<RedactTable<Dst>, false><<<2 * num_sms, REDACT_THREADS, BLUR_SMEM, s>>>(c, t);
+            if (ell) k_redact_apply<RedactTable<Dst>, true, true><<<2 * num_sms, REDACT_THREADS, 0, s>>>(c, t);
+            else k_redact_apply<RedactTable<Dst>, false, true><<<2 * num_sms, REDACT_THREADS, 0, s>>>(c, t);
+        } else {
+            k_redact_measure<<<2 * num_sms, REDACT_THREADS, 0, s>>>(c, t);
+            if (ell) k_redact_apply<RedactTable<Dst>, true><<<2 * num_sms, REDACT_THREADS, 0, s>>>(c, t);
+            else k_redact_apply<<<2 * num_sms, REDACT_THREADS, 0, s>>>(c, t);
+        }
         const cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
     }

@@ -8,6 +8,11 @@
 //                     cell value; luma first, then chroma
 // The counts are only known on the device: every CTA of measure / apply scans the frames' totals and strides over the work that
 // exists, so unused max_faces capacity costs nothing.
+// f14 styles (rf_redact_style) keep the regions kernel and the order.  MOSAIC with ELLIPSE runs measure unchanged and an apply that
+// tests each region's ellipse.  BLUR replaces measure with
+//   k_redact_blur     grid-stride over (frame, region, plane, strip of BLUR_W columns x band of BLUR_H rows): the triple-box blur of
+//                     the ORIGINAL plane, written for every sample the region owns into the frame's scratch planes
+// and its apply copies every owned sample from the scratch planes into the frame.
 #pragma once
 #include <type_traits>
 
@@ -16,6 +21,8 @@
 namespace rf {
 
 constexpr int REDACT_MAX_BLOCKS = 32, REDACT_THREADS = 256, REDACT_BAND = 16;
+constexpr int REDACT_MOSAIC = 1, REDACT_BLUR = 2, REDACT_RECT = 1, REDACT_ELLIPSE = 2;
+constexpr int BLUR_MAX_DETAIL = 64, BLUR_MAX_RADIUS = 127;
 
 // Writable frame descriptors (the read-only YuvPlanes / BgrRows of the detect paths stay const).
 struct YuvPlanesW {
@@ -28,23 +35,26 @@ struct BgrRowsW {
 };
 
 // One frame of a call: its pixels, size, and the factor its records map back by (1 for records already in frame pixels).
+// blur: the frame's scratch planes (BLUR only; YUV: luma w x h, then U and V w/2 x h/2; BGR: 3 w x h), nullptr otherwise.
 template <typename Dst>
 struct RedactFrameT {
     Dst dst;
     int w, h;
     float scale;
+    uint8_t *blur;
 };
 // Frames per launch: the table travels as a __grid_constant__ kernel parameter within the classic 4 KB (static_assert in redact.cu).
 template <typename Dst> constexpr int redact_table_limit() { return std::is_same<Dst, BgrRowsW>::value ? 64 : 32; }
 
 // One region: the snapped rectangle [x0, x1) x [y0, y1) (unclamped), cell side c, cells across nx, the first cell row inside the
-// frame, and the region's first work item of measure / apply within its frame.
+// frame, and the region's first work item of measure (blur, for BLUR) / apply within its frame; rad: the blur radius a (0 for MOSAIC).
 struct RedactRegion {
-    int x0, y0, x1, y1, c, nx, cr0, m_first, a_first, pad;
+    int x0, y0, x1, y1, c, nx, cr0, m_first, a_first, rad;
 };
 
 struct RedactArgs {
     int n, blocks, max_faces, max_tracks, cap;   // cap: regions per frame, max_faces + max_tracks
+    int kind, shape, detail;                     // rf_redact_style resolved (f12: MOSAIC, RECT, 0)
     double margin;
     const rf_det *dets;                          // [n][max_faces]
     const int *counts;                           // [n]
@@ -55,6 +65,8 @@ struct RedactArgs {
     uint8_t *cells;                              // [n][cap][blocks^2][3]
 };
 
+// Scratch plane bytes of one w x h frame for BLUR.
+inline size_t blur_plane_bytes(bool yuv, int w, int h) { return yuv ? (size_t)w * h + 2 * (size_t)(w / 2) * (h / 2) : 3 * (size_t)w * h; }
 // Scratch bytes of a call of n frames with `cap` regions each (the layout redact_carve cuts).
 size_t redact_scratch_bytes(int n, int cap, int blocks);
 void redact_carve(RedactArgs &a, void *scratch);

@@ -169,22 +169,23 @@ class RetinaFace:
         return tracks, new
 
     def redactFrames(self, frames: Sequence, videos: Sequence[int] = None, threshold: float = 0.5, blocks: int = 0, margin: float = 0.0,
-                     layout: str = "nv12", matrix: str = "bt601", max_videos: int = 64, motion=False):
+                     layout: str = "nv12", matrix: str = "bt601", max_videos: int = 64, motion=False, style: str = "mosaic",
+                     shape: str = "rect", detail: int = 0):
         """f12 redaction: detect on device 4:2:0 frames (torch CUDA tensors in ``Engine.detect_yuv_device``'s forms) and mosaic every
         detected face IN PLACE (rf_detect_yuv_redact_device), ``blocks`` cells across a region's longer side (0: 8; 1: a flat patch),
         each side grown by ``margin`` of the box (0: 0.25).  With ``videos`` (frame i of video ``videos[i]``) the frames are also
         tracked, on this detector's plain tracker (created as ``trackFrames`` creates it), and the predicted box of every face the
         tracker still follows while the detector misses it is redacted too.  Asynchronous: the frames are complete in stream order on
         ``engine.last_stream_ptr()``.  ``motion`` as ``trackFrames``: the lost faces' predicted boxes then follow the camera.  The first
-        call decides the tracker."""
+        call decides the tracker.  f14: ``style="blur"`` blurs each region instead (``detail`` 0: 4; 1..64, a larger detail a smaller
+        radius; ``blocks`` must then stay 0), and ``shape="ellipse"`` redacts the ellipse inscribed in each region."""
+        kw = dict(layout=layout, matrix=matrix, blocks=blocks, margin=margin, style=style, shape=shape, detail=detail)
         if videos is None:
-            self.engine.detect_yuv_redact_device(list(frames), threshold, self.nms_threshold, layout=layout, matrix=matrix, blocks=blocks,
-                                                 margin=margin)
+            self.engine.detect_yuv_redact_device(list(frames), threshold, self.nms_threshold, **kw)
             return
         if getattr(self, "_tracker", None) is None:
             self._tracker = self.engine.tracker(max_videos=max_videos, motion=motion)
-        self._tracker.detect_yuv_redact_device(list(frames), list(videos), threshold, self.nms_threshold, layout=layout, matrix=matrix,
-                                               blocks=blocks, margin=margin)
+        self._tracker.detect_yuv_redact_device(list(frames), list(videos), threshold, self.nms_threshold, **kw)
 
     def _best_crops(self, n: int):
         import torch

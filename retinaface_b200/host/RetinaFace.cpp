@@ -333,12 +333,13 @@ void RetinaFace::redactYUV(const vector<rf_yuv_frame> &device_frames, const vect
         if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_create: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
         trackerCreated();
     }
-    const rf_redact_params p{opt.blocks, opt.margin};
+    const rf_redact_style st{opt.style, opt.shape, opt.style == RF_REDACT_BLUR ? 0 : opt.blocks, opt.detail, opt.margin};
     const int n = (int)device_frames.size();
     DeviceTracks t{};
-    int rc = rf_detect_yuv_redact_device(h_, videos ? tracker_ : nullptr, device_frames.data(), videos ? videos->data() : nullptr, n, RF_YUV_BT601,
-                                         threshold, nms_threshold, &p, &t.tracks, &t.counts, nullptr, nullptr, nullptr);
-    if (rc != RF_OK) throw std::runtime_error(string("rf_detect_yuv_redact_device: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+    int rc = rf_detect_yuv_redact_device_style(h_, videos ? tracker_ : nullptr, device_frames.data(), videos ? videos->data() : nullptr, n,
+                                               RF_YUV_BT601, threshold, nms_threshold, &st, &t.tracks, &t.counts, nullptr, nullptr, nullptr);
+    if (rc != RF_OK)
+        throw std::runtime_error(string("rf_detect_yuv_redact_device_style: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
     if (videos) {
         tracks_ = t;
         tracks_.n = n;

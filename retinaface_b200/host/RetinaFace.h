@@ -52,10 +52,13 @@ struct AlignOptions {
     int max_faces = 0;                   // crops per image, best score first; 0: every kept face
 };
 
-// f12 redaction (rf_detect_yuv_redact_device): the mosaic written over every face
+// f12 / f14 redaction (rf_detect_yuv_redact_device_style): the mosaic or blur written over every face
 struct RedactOptions {
-    int blocks = 8;                      // cells across a region's longer side, 1..32 (1: one flat patch)
+    int blocks = 8;                      // mosaic: cells across a region's longer side, 1..32 (1: one flat patch); the blur ignores it
     float margin = 0.25f;                // each side of a box grows by margin x its side, (0, 1]
+    int style = RF_REDACT_MOSAIC;        // RF_REDACT_MOSAIC or RF_REDACT_BLUR
+    int shape = RF_REDACT_RECT;          // RF_REDACT_RECT or RF_REDACT_ELLIPSE (the ellipse inscribed in the region)
+    int detail = 0;                      // blur: 0 (4) or 1..64, a larger detail a smaller radius; 0 for the mosaic
 };
 
 class RetinaFace {
@@ -141,7 +144,7 @@ class RetinaFace {
     };
     const DeviceMotion &lastMotion() const { return motion_; }
     void finishVideo(int video, void *dev_best_crops);
-    // f12 redaction (rf_detect_yuv_redact_device): detect on DEVICE 4:2:0 frames and mosaic every detected face in place, on the
+    // f12 / f14 redaction (rf_detect_yuv_redact_device_style): detect on DEVICE 4:2:0 frames and mosaic (or blur) every detected face in place, on the
     // GPU; asynchronous on rf_last_stream(handle()).  With `videos` (one per frame, in [0, track_videos)) the frames are also tracked on
     // this RetinaFace's plain tracker (trackYUV's), lastTracks() holds the lists, and the predicted box of every LOST track -- a face the
     // detector missed on this frame -- is redacted too.

@@ -10,9 +10,11 @@ scale, four times) through rf_detect_yuv_tiled_device, then rf_redact_yuv_device
   kernel_us   microseconds per launch of each k_redact_* kernel (and their sum per 8-frame call) in a separate torch.profiler run, the mean
               faces per frame, and the byte floor of one call: the region pixels (1.5 bytes each) read twice and written once, over
               3.35 TB/s;
-and the card's name and power limit, read in the same command.
+and the card's name and power limit, read in the same command.  --style / --shape / --detail (f14) redact with that style instead
+of f12's rectangular mosaic; the runs then add detect+mosaic (the f12 call on the same records), the style's rate against it, and
+k_redact_blur's time per launch.
 
-    python tools/redact_rate.py [--min-seconds S] [--warmup W] [--rounds R]
+    python tools/redact_rate.py [--min-seconds S] [--warmup W] [--rounds R] [--style mosaic|blur] [--shape rect|ellipse] [--detail D]
 """
 import argparse
 import json
@@ -62,7 +64,13 @@ def main():
     ap.add_argument("--min-seconds", type=float, default=0.5)
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--style", default="mosaic", choices=("mosaic", "blur"))
+    ap.add_argument("--shape", default="rect", choices=("rect", "ellipse"))
+    ap.add_argument("--detail", type=int, default=0)
     args = ap.parse_args()
+    rk = dict(style=args.style, shape=args.shape, detail=args.detail)
+    styled = (args.style, args.shape, args.detail) != ("mosaic", "rect", 0)
+    kernels = KERNELS + (("k_redact_blur",) if styled else ())
     import cv2
     import torch
     from torch.profiler import ProfilerActivity, profile
@@ -97,15 +105,19 @@ def main():
 
     def detect_redact():
         d, c, sc = eng.detect_yuv_device(nxt(), thr, nms)
+        eng.redact_yuv_device(out, d, c, sc, **rk)
+
+    def detect_mosaic():
+        d, c, sc = eng.detect_yuv_device(nxt(), thr, nms)
         eng.redact_yuv_device(out, d, c, sc)
 
     def track_redact():
         tp, tc, d, c, sc = trk.detect_yuv_device(nxt(), vids, thr, nms)
-        eng.redact_yuv_device(out, d, c, sc, tracker=trk, tracks_ptr=tp, track_counts_ptr=tc)
+        eng.redact_yuv_device(out, d, c, sc, tracker=trk, tracks_ptr=tp, track_counts_ptr=tc, **rk)
 
     def tiled_redact():
         d, c = eng4k.detect_yuv_tiled_device(tiled_in, thr, nms)
-        eng4k.redact_yuv_device(tiled_out, d, c, None)
+        eng4k.redact_yuv_device(tiled_out, d, c, None, **rk)
 
     runs = {
         "detect": (eng, lambda: eng.detect_yuv_device(nxt(), thr, nms)),
@@ -115,6 +127,8 @@ def main():
         "tiled": (eng4k, lambda: eng4k.detect_yuv_tiled_device(tiled_in, thr, nms)),
         "tiled+redact": (eng4k, tiled_redact),
     }
+    if styled:
+        runs["detect+mosaic"] = (eng, detect_mosaic)
     for e, fn in runs.values():
         for _ in range(args.warmup):
             fn()
@@ -137,23 +151,29 @@ def main():
     d, c = eng4k.detect_yuv_tiled_device(tiled_in, thr, nms)
     recs4k = _records(eng4k, d, c, B)
     kernel_us = {}
-    for name, (e, fn) in (("detect+redact", runs["detect+redact"]), ("tiled+redact", runs["tiled+redact"])):
+    for name in ("detect+redact", "tiled+redact") + (("detect+mosaic",) if styled else ()):
+        e, fn = runs[name]
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
             for _ in range(50):
                 fn()
             e.synchronize()
         per = {}
-        for k in KERNELS:
+        for k in kernels:
             ks = [ev for ev in prof.events() if k in ev.name]
             per[k] = sum(ev.device_time for ev in ks) / len(ks) if ks else None
         per["per_call"] = sum(v for v in per.values() if v is not None)
         kernel_us[name] = per
     smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
     med = {k: round(float(np.median(v)), 1) for k, v in rates.items()}
-    print(json.dumps(dict(frames_per_s=med, rounds=rates, redact_share={k: round(med[k + "+redact"] / med[k], 4) for k in ("detect", "track", "tiled")},
-                          kernel_us=kernel_us, faces_per_frame=faces, faces_per_frame_4k=float(np.mean([len(r) for r in recs4k])),
-                          floor_bytes_per_call=floor_bytes, floor_us_per_call=floor_bytes / 3.35e12 * 1e6,
-                          floor_bytes_per_call_4k=_floor_bytes(recs4k, None, 3840, 2160), gpu=smi.stdout.strip())))
+    res = dict(frames_per_s=med, rounds=rates, redact_share={k: round(med[k + "+redact"] / med[k], 4) for k in ("detect", "track", "tiled")},
+               kernel_us=kernel_us, faces_per_frame=faces, faces_per_frame_4k=float(np.mean([len(r) for r in recs4k])),
+               floor_bytes_per_call=floor_bytes, floor_us_per_call=floor_bytes / 3.35e12 * 1e6,
+               floor_bytes_per_call_4k=_floor_bytes(recs4k, None, 3840, 2160), gpu=smi.stdout.strip())
+    if styled:
+        res["style"] = rk
+        res["style_vs_mosaic"] = dict(frames=round(med["detect+redact"] / med["detect+mosaic"], 4),
+                                      kernels=round(kernel_us["detect+redact"]["per_call"] / kernel_us["detect+mosaic"]["per_call"], 4))
+    print(json.dumps(res))
     trk.close()
     eng.close()
     eng4k.close()

@@ -779,6 +779,69 @@ int rf_detect_yuv_redact_device_style(rf_handle h, rf_tracker t, const rf_yuv_fr
                                       const rf_track **dev_tracks, const int32_t **dev_track_counts, const rf_det **dev_dets,
                                       const int32_t **dev_counts, float *out_scales);
 
+/* f15 look-back redaction: a face is usually visible for a few frames before the detector first fires on it -- it walks in from the
+ * edge, turns towards the camera, comes out from behind someone, or is too small or blurred at first.  f12 / f14 redact each frame as
+ * it arrives, so those frames go out uncovered.  A LOOK-BACK tracker keeps the last L frames of each video on the GPU, emits every
+ * frame L frames late, and by then knows every track born in the L frames that followed it: the emitted frame is also covered where
+ * each of those faces already was.  oracle/lookback.py restates the definition; every FP64 step is one rounding in the order written.
+ *
+ * A look-back tracker is a plain tracker (with or without f13 motion) on which rf_tracker_set_lookback was called before its first
+ * update.  It is fed only through rf_detect_yuv_redact_lookback_device.
+ *   Frame numbers  each video counts its frames from 0 since create, reset or drain (the host knows every number when a call is issued).
+ *   Births         the births of frame f are the tracks of f's list with age == 1, in list (id) order -- TENTATIVE births included: a
+ *                  record at or above new_thresh is a confident face, and the rule errs towards covering it.
+ *   Look-back box  of a birth on frame b with record box `face` (x1, y1, x2, y2, frame pixels, widened to double), on frame e = b - k,
+ *                  1 <= k <= L, e at or after the first frame the video still buffers:
+ *                    1. w = x2 - x1, h = y2 - y1, cx = x1 + w / 2, cy = y1 + h / 2 (f10's z);
+ *                    2. with motion, for f = b, b - 1, ..., e + 1 with frame f's rf_motion {a, -B, tx, B, a, ty} of status RF_MOTION_OK
+ *                       (FIRST and LOST move nothing), the motion undone: s2 = a a + B B, dx = cx - tx, dy = cy - ty,
+ *                       cx = (a dx + B dy) / s2, cy = (a dy - B dx) / s2, s = sqrt(s2), w = w / s, h = h / s;
+ *                    3. g = 0.5 + grow k, ex = g w, ey = g h; the box is (cx - ex, cy - ey, cx + ex, cy + ey), each rounded to float.
+ *                  The face's own motion is not extrapolated (a birth's Kalman velocity is zero): the growth covers it.  At the
+ *                  default, each side moves out by 10 % of the box per frame back -- 10 px per frame for a 100 px face.
+ *   Regions        of an emitted frame e, in this order, each box through f12's geometry (margin, snap, skipped boxes):
+ *                    (a) e's records in rank order, as __fmul_rn(x, scale);  (b) e's LOST tracks in id order, (kx1, ky1, kx2, ky2)
+ *                    -- exactly what rf_redact_yuv_device_style draws on frame e --
+ *                    (c) the look-back boxes of the births on frames e + 1 .. min(e + L, the video's last frame seen), frame by
+ *                        frame, id order within a frame.
+ *                  Shapes, styles and ownership are f14's: the lowest-index region whose shape covers a sample owns it.
+ *   Output         frame e's ORIGINAL bytes (the input as it arrived) go to the caller's out frame, and the regions are redacted over
+ *                  them with the call's rf_redact_style.  The out frame's pitch padding is not written.
+ * Memory: a video's buffer is allocated on its first frame, L x w h 3 / 2 bytes packed in the frame's layout (47 MB per 1080p video
+ * at L = 15), plus a log of 2 L frames' regions and births; it is kept until the tracker is destroyed and reallocated only when a
+ * video restarts (reset, drain) at another frame size.  Each ring slot of the tracker gains max(max_batch, L) x (max_faces +
+ * max_tracks + L min(max_faces, max_tracks)) records for the regions of the emitted frames. */
+typedef struct rf_lookback_config {
+    int frames;      /* L: 0 -> 15 (half a second at 30 fps); else 1..64 */
+    float grow;      /* growth per frame back: 0 -> 0.1; else finite in (0, 1] */
+} rf_lookback_config;
+/* Makes t a look-back tracker.  Bad values, a call after the tracker's first update, a second call or a best-shot tracker:
+ * RF_ERR_INVALID_ARG.  rf_detect_yuv_track_device, rf_track_update and rf_detect_yuv_redact_device(_style) refuse a look-back
+ * tracker (RF_ERR_INVALID_ARG): the buffer must see every frame. */
+int rf_tracker_set_lookback(rf_tracker t, const rf_lookback_config *cfg);
+/* rf_detect_yuv_track_device without crops (records, scales, tracks and motion bit for bit the same), then: each frame is stored in
+ * its video's buffer, and frame i, number num_i in its video, emits frame num_i - L of that video when num_i >= L: out_frames[i]
+ * receives it, redacted as above with `style` (NULL: the zeroed struct's defaults), and out_frame_numbers[i] (host) = num_i - L;
+ * otherwise out_frame_numbers[i] = -1 and out_frames[i] is not written.  An out frame must have its input frame's size and layout
+ * (uv_step, and the chroma order for semi-planar frames; pitches are free) and be disjoint from every input and out frame of the call,
+ * or be exactly frames[i]'s descriptor: delayed output into the caller's own surface.  The input frames are disjoint too.  A video may appear at most L times in one call
+ * and its frame size and layout may not change before a drain or reset.  Statuses, all before anything is launched: those of
+ * rf_detect_yuv_redact_device_style, a tracker that is not a look-back tracker, each rule above (RF_ERR_INVALID_ARG), a failed buffer
+ * allocation (RF_ERR_CAPACITY).  Asynchronous on the forward's context; the tracker's event chain orders its state, and the caller
+ * keeps the input and out frames alive until that stream has passed the call. */
+int rf_detect_yuv_redact_lookback_device(rf_handle h, rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, int matrix,
+                                         float score_threshold, float nms_threshold, const rf_redact_style *style,
+                                         const rf_yuv_frame *out_frames, int32_t *out_frame_numbers, const rf_track **dev_tracks,
+                                         const int32_t **dev_track_counts, const rf_det **dev_dets, const int32_t **dev_counts,
+                                         float *out_scales);
+/* Ends `video`: emits its min(L, frames seen) buffered frames in frame order into out_frames[0 ..) (windows end at the last frame
+ * seen), *n_out of them with their numbers in out_frame_numbers, then restarts the video as rf_tracker_reset does.  cap below the
+ * count: RF_ERR_CAPACITY; bad out frames (as above, against the video's frames): RF_ERR_INVALID_ARG; nothing launched on either.
+ * Asynchronous on context 0's stream, inside the tracker's event chain.  rf_tracker_reset on a look-back tracker drops the buffered
+ * frames and emits nothing. */
+int rf_tracker_drain(rf_tracker t, int video, const rf_redact_style *style, const rf_yuv_frame *out_frames, int cap, int *n_out,
+                     int32_t *out_frame_numbers);
+
 /* Introspection. */
 int rf_get_net_size(rf_handle h, int *net_w, int *net_h, int *max_batch, int *max_faces);
 int rf_num_anchors(rf_handle h);            /* per image: 8,232 @448x448, 47,040 @1280x896 */

@@ -30,6 +30,7 @@ SOURCES = [
     ("best.cu", ["-fmad=false"]),       # the crop warp of align.cu and the FP64 face quality, as oracle/bestshot.py states it
     ("redact.cu", ["-fmad=false"]),     # the FP64 region geometry, as oracle/redact.py states it
     ("motion.cu", ["-fmad=false"]),     # the FP64 sub-pixel match and similarity fit, as oracle/motion.py states it
+    ("lookback.cu", ["-fmad=false"]),   # the FP64 look-back box, as oracle/lookback.py states it
     ("calibrate.cu", []),
     ("model.cpp", []),
     ("frontend.cpp", []),

@@ -37,6 +37,7 @@ EXPORTS = [
     "rf_tracker_set_motion", "rf_tracker_motion",
     "rf_redact_yuv_device", "rf_redact_device", "rf_detect_yuv_redact_device",
     "rf_redact_yuv_device_style", "rf_redact_device_style", "rf_detect_yuv_redact_device_style",
+    "rf_tracker_set_lookback", "rf_detect_yuv_redact_lookback_device", "rf_tracker_drain",
 ]
 COMM_BLOB_BYTES = 128
 
@@ -275,6 +276,16 @@ def redact_style(style: str = "mosaic", shape: str = "rect", blocks: int = 0, de
     return RedactStyle(kinds[style], shapes[shape], int(blocks), int(detail), float(margin))
 
 
+class LookbackConfig(C.Structure):  # rf_lookback_config
+    _fields_ = [("frames", C.c_int), ("grow", C.c_float)]
+
+
+def _style_struct(style: str, shape: str, blocks: int, detail: int, margin: float) -> RedactStyle:
+    """The rf_redact_style of the redaction keywords, {MOSAIC, RECT} included (the look-back calls take only a style)."""
+    st = redact_style(style, shape, blocks, detail, margin)
+    return st if st is not None else RedactStyle(RF_REDACT_MOSAIC, RF_REDACT_RECT, int(blocks), 0, float(margin))
+
+
 def _redact_call(lib, style: str, shape: str, blocks: int, detail: int, margin: float):
     """(rf_detect_yuv_redact_device or its _style variant, the params or style struct) of the redaction keywords."""
     st = redact_style(style, shape, blocks, detail, margin)
@@ -430,6 +441,9 @@ def load_library() -> C.CDLL:
     a = list(lib.rf_detect_yuv_redact_device.argtypes)
     a[8] = C.POINTER(RedactStyle)
     lib.rf_detect_yuv_redact_device_style.argtypes = a
+    lib.rf_tracker_set_lookback.argtypes = [C.c_void_p, C.POINTER(LookbackConfig)]
+    lib.rf_detect_yuv_redact_lookback_device.argtypes = a[:9] + [C.POINTER(YuvFrame), C.c_void_p] + a[9:]
+    lib.rf_tracker_drain.argtypes = [C.c_void_p, C.c_int, C.POINTER(RedactStyle), C.POINTER(YuvFrame), C.c_int, C.POINTER(C.c_int), C.c_void_p]
     _lib = lib
     return lib
 
@@ -1089,19 +1103,22 @@ class Engine:
     # -- f10 face tracking across video frames ---------------------------------------------------------------------------------
     def tracker(self, max_videos: int = 1, max_tracks: int = 0, high_thresh: float = 0.0, new_thresh: float = 0.0, iou_high: float = 0.0,
                 iou_low: float = 0.0, iou_tentative: float = 0.0, max_lost: int = 0, best: Optional[dict] = None,
-                motion=None) -> "Tracker":
+                motion=None, lookback=None) -> "Tracker":
         """rf_tracker_create: a tracker of max_videos independent sequences on this engine (0 -> the defaults of rf_track_config).
         best (``best_config`` keywords): a best-shot tracker (rf_tracker_create_best), fed through ``Tracker.detect_yuv_best_device``.
         motion (True or ``motion_config`` keywords): camera-motion compensation (rf_tracker_set_motion) from the frames of the
-        detect_yuv_* calls; read each call's estimates with ``Tracker.motion``."""
+        detect_yuv_* calls; read each call's estimates with ``Tracker.motion``.  lookback (True, L, or ``set_lookback`` keywords): a
+        look-back tracker (rf_tracker_set_lookback), fed through ``Tracker.detect_yuv_redact_lookback_device``."""
         t = Tracker(self, TrackConfig(max_videos, max_tracks, high_thresh, new_thresh, iou_high, iou_low, iou_tentative, max_lost),
                     best_config(**best) if best is not None else None)
-        if motion:
-            try:
+        try:
+            if motion:
                 t.set_motion(**(motion if isinstance(motion, dict) else {}))
-            except Exception:
-                t.close()
-                raise
+            if lookback:
+                t.set_lookback(**(lookback if isinstance(lookback, dict) else {} if lookback is True else {"frames": int(lookback)}))
+        except Exception:
+            t.close()
+            raise
         return t
 
     # -- f12 redaction ---------------------------------------------------------------------------------------------------------
@@ -1213,6 +1230,7 @@ class Tracker:
         self.t = t
         self.best = best
         self.motion_on = False
+        self.lookback = 0            # L of a look-back tracker
         self.max_videos = cfg.max_videos
         self.max_tracks = cfg.max_tracks or 64
 
@@ -1319,6 +1337,45 @@ class Tracker:
         self.engine._check(self.lib.rf_synchronize(self.engine.h))
         raw = torch.as_tensor(_DevArray(int(p.value), (n * MOTION_DTYPE.itemsize,), "|u1"), device="cuda").cpu().numpy()
         return raw.view(MOTION_DTYPE).copy()
+
+    def set_lookback(self, frames: int = 0, grow: float = 0.0):
+        """rf_tracker_set_lookback, before the first update: keep each video's last L frames (0 -> 15) on the GPU and emit every frame L
+        frames late, covered where the faces born after it already were (grow: the box growth per frame back, 0 -> 0.1)."""
+        cfg = LookbackConfig(int(frames), float(grow))
+        self.engine._check(self.lib.rf_tracker_set_lookback(self.t, C.byref(cfg)))
+        self.lookback = cfg.frames or 15
+
+    def detect_yuv_redact_lookback_device(self, frames, videos: Sequence[int], out_frames, thr: float, nms_thr: float, layout: str = "nv12",
+                                          matrix="bt601", blocks: int = 0, margin: float = 0.0, style: str = "mosaic", shape: str = "rect",
+                                          detail: int = 0):
+        """rf_detect_yuv_redact_lookback_device: detect and track the device 4:2:0 frames, store them, and write frame num - L of each
+        frame's video, redacted, into out_frames[i] (the same forms as frames, in `layout`; out_frames[i] may be frames[i] itself).
+        Returns (out frame numbers (-1: nothing emitted), tracks_ptr, track_counts_ptr, dets_ptr, counts_ptr, scales)."""
+        n = len(frames)
+        if len(out_frames) != n:
+            raise ValueError(f"{n} frames but {len(out_frames)} out frames")
+        arr = self.engine._frames(frames, layout, True)
+        outs = self.engine._frames(out_frames, layout, True)
+        st = _style_struct(style, shape, blocks, detail, margin)
+        nums = np.full(max(n, 1), -1, dtype=np.int32)
+        scales = np.zeros(max(n, 1), dtype=np.float32)
+        tp, tc, d, c = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
+        self.engine._check(self.lib.rf_detect_yuv_redact_lookback_device(self.engine.h, self.t, arr, self._ints(videos, n), n, _matrix(matrix), thr,
+                                                                         nms_thr, C.byref(st), outs, nums.ctypes.data, C.byref(tp), C.byref(tc),
+                                                                         C.byref(d), C.byref(c), scales.ctypes.data))
+        return nums[:n].copy(), int(tp.value or 0), int(tc.value or 0), int(d.value or 0), int(c.value or 0), scales[:n].copy()
+
+    def drain(self, video: int, out_frames, layout: str = "nv12", blocks: int = 0, margin: float = 0.0, style: str = "mosaic",
+              shape: str = "rect", detail: int = 0) -> np.ndarray:
+        """rf_tracker_drain: write the video's buffered frames (at most L, in frame order) into out_frames[0..), then restart the video.
+        Returns the numbers of the frames written."""
+        k = len(out_frames)
+        outs = self.engine._frames(out_frames, layout, True) if k else None
+        st = _style_struct(style, shape, blocks, detail, margin)
+        nums = np.zeros(max(k, 1), dtype=np.int32)
+        n_out = C.c_int(0)
+        self.engine._check(self.lib.rf_tracker_drain(self.t, int(video), C.byref(st), outs, k, C.byref(n_out), nums.ctypes.data))
+        return nums[:n_out.value].copy()
 
     def reset(self, video: int = -1):
         """rf_tracker_reset: restart one video (ids from 1), or all with -1; ordered after every issued update."""

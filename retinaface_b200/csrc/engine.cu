@@ -14,6 +14,7 @@
 #include "redact.cuh"
 #include "track.cuh"
 #include "motion.cuh"
+#include "lookback.cuh"
 
 namespace rf_eng {
 
@@ -1855,6 +1856,8 @@ struct rf_tracker_s {
         rf_det *due = nullptr;         // [max_batch][max_faces]
         int *due_counts = nullptr;     // [max_batch]
         rf_motion *motion = nullptr;   // [max_batch] f13, with motion on
+        rf_det *lb_boxes = nullptr;    // [max(max_batch, L)][lookback_records] f15, the regions of the emitted frames
+        int *lb_counts = nullptr;      // [max(max_batch, L)]
         cudaEvent_t free = nullptr;
     };
     std::vector<Slot> slots;
@@ -1877,6 +1880,20 @@ struct rf_tracker_s {
     MotionBlock *d_mblocks = nullptr;  // [max_batch][MOTION_MAX_BLOCKS]
     std::vector<std::array<int, 2>> mref;
     int motion_slot = -1;              // the ring slot of the latest frame call
+    // f15 look-back (lookback.cuh); `lookback` false: none of these allocated.  lbv mirrors on the host each video's frame count and
+    // layout, so that every frame's number, buffer slot and emission are known when a call is issued.  A video's device block is its
+    // frame buffer (L packed frames of frame_bytes) followed by its log (2 L slots of lookback_slot_bytes).
+    bool lookback = false;
+    int lb_frames = 0;                 // L
+    float lb_grow = 0.f;
+    struct LookbackVideo {
+        uint8_t *d = nullptr;
+        size_t frame_bytes = 0;
+        int w = 0, h = 0, step = 0;
+        bool v_first = false;          // semi-planar with V before U (NV21)
+        long long frames = 0;          // frames since create, reset or drain
+    };
+    std::vector<LookbackVideo> lbv;
 };
 
 static void tracker_release(rf_tracker t) {
@@ -1884,7 +1901,9 @@ static void tracker_release(rf_tracker t) {
     for (auto &s : t->slots) {
         if (s.free) { cudaEventSynchronize(s.free); cudaEventDestroy(s.free); }
         cudaFree(s.tracks); cudaFree(s.counts); cudaFree(s.due); cudaFree(s.due_counts); cudaFree(s.motion);
+        cudaFree(s.lb_boxes); cudaFree(s.lb_counts);
     }
+    for (auto &v : t->lbv) cudaFree(v.d);
     cudaFree(t->d_mstore); cudaFree(t->d_mthumbs); cudaFree(t->d_mblocks);
     if (t->chain) cudaEventDestroy(t->chain);
     cudaFree(t->d_videos); cudaFree(t->d_state); cudaFree(t->d_pairs); cudaFree(t->d_order);
@@ -1964,6 +1983,7 @@ int rf_tracker_reset(rf_tracker t, int video) {
             CK(cudaMemsetAsync(t->ba.videos + v0, 0, sizeof(BestVideo) * nv, s));
         }
         for (size_t v = v0; t->motion && v < v0 + nv; v++) t->mref[v] = {0, 0};
+        for (size_t v = v0; t->lookback && v < v0 + nv; v++) t->lbv[v].frames = 0;     // the buffered frames are dropped
         CK(cudaEventRecord(t->chain, s));
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
@@ -2107,6 +2127,7 @@ int rf_track_update(rf_tracker t, const int *videos, int n, const rf_det *dev_de
     rf_handle h = t->h;
     if (t->best) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a best-shot tracker takes frames only through rf_detect_yuv_track_best_device", who));
     if (t->motion) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a motion tracker needs the frames (rf_detect_yuv_track_device)", who));
+    if (t->lookback) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a look-back tracker takes frames only through rf_detect_yuv_redact_lookback_device", who));
     int rc = check_track_args(t, who, videos, n, scales);
     if (rc) return rc;
     if (n > 0 && (!dev_dets || !dev_counts)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL records or counts", who));
@@ -2126,6 +2147,7 @@ int rf_detect_yuv_track_device(rf_handle h, rf_tracker t, const rf_yuv_frame *fr
     if (!h) return RF_ERR_INVALID_ARG;
     if (!t || t->h != h) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker is NULL or belongs to another handle", who));
     if (t->best) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a best-shot tracker takes frames only through rf_detect_yuv_track_best_device", who));
+    if (t->lookback) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a look-back tracker takes frames only through rf_detect_yuv_redact_lookback_device", who));
     int rc = check_track_args(t, who, videos, n, nullptr);
     if (rc) return rc;
     const YuvFrames src{frames, matrix, nullptr, false};
@@ -2504,11 +2526,12 @@ static Ctx &last_ctx(rf_handle h) {
     return h->ctx[0];
 }
 
-// Issues the redaction of `frames` on context c's stream, into c's scratch (sized for max_batch frames of this call's region
-// capacity and blocks, and for BLUR the frames' scratch planes; a larger need waits for the context before the scratch is replaced).
+// Issues the redaction of `frames` on context c's stream, into c's scratch (sized for max_batch frames -- or more, for a drain -- of
+// this call's region capacity and blocks, and for BLUR the frames' scratch planes; a larger need waits for the context before the
+// scratch is replaced).  records: the records per frame of dets (0: max_faces; f15's look-back regions have more).
 template <typename Dst>
 static void redact_issue(rf_handle h, Ctx &c, std::vector<RedactFrameT<Dst>> frames, const rf_det *dets, const int32_t *counts, rf_tracker t,
-                         const rf_track *tracks, const int32_t *track_counts, const RedactSpec &spec) {
+                         const rf_track *tracks, const int32_t *track_counts, const RedactSpec &spec, int records = 0) {
     RedactArgs a{};
     a.n = (int)frames.size();
     a.blocks = spec.blocks;
@@ -2516,14 +2539,14 @@ static void redact_issue(rf_handle h, Ctx &c, std::vector<RedactFrameT<Dst>> fra
     a.kind = spec.kind;
     a.shape = spec.shape;
     a.detail = spec.detail;
-    a.max_faces = h->cfg.max_faces;
+    a.max_faces = records ? records : h->cfg.max_faces;
     a.max_tracks = t ? t->cfg.max_tracks : 0;
     a.cap = a.max_faces + a.max_tracks;
     a.dets = dets;
     a.counts = counts;
     a.tracks = tracks;
     a.track_counts = track_counts;
-    const size_t tables = (redact_scratch_bytes(h->cfg.max_batch, a.cap, a.blocks) + 255) & ~(size_t)255;
+    const size_t tables = (redact_scratch_bytes(std::max(h->cfg.max_batch, a.n), a.cap, a.blocks) + 255) & ~(size_t)255;
     size_t need = tables;
     if (spec.kind == REDACT_BLUR)
         for (const auto &f : frames) need += (blur_plane_bytes(std::is_same<Dst, YuvPlanesW>::value, f.w, f.h) + 255) & ~(size_t)255;
@@ -2614,6 +2637,8 @@ static int detect_yuv_redact_impl(rf_handle h, const char *who, rf_tracker t, co
     if (t) {
         if (t->h != h) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker belongs to another handle", who));
         if (t->best) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a best-shot tracker takes frames only through rf_detect_yuv_track_best_device", who));
+        if (t->lookback)
+            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a look-back tracker takes frames only through rf_detect_yuv_redact_lookback_device", who));
         if ((rc = check_track_args(t, who, videos, n, nullptr))) return rc;
     }
     const YuvFrames src{frames, matrix, nullptr, false};
@@ -2687,6 +2712,310 @@ int rf_detect_yuv_redact_device_style(rf_handle h, rf_tracker t, const rf_yuv_fr
     static const char *who = "rf_detect_yuv_redact_device_style";
     return detect_yuv_redact_impl(h, who, t, frames, videos, n, matrix, thr, nms, [&](RedactSpec &r) { return redact_style(h, who, style, r); },
                                   dev_tracks, dev_track_counts, dev_dets, dev_counts, out_scales);
+}
+
+// ---- f15 look-back redaction (lookback.cuh) --------------------------------------------------------------------------------------
+int rf_tracker_set_lookback(rf_tracker t, const rf_lookback_config *cfg) {
+    static const char *who = "rf_tracker_set_lookback";
+    if (!t) return RF_ERR_INVALID_ARG;
+    rf_handle h = t->h;
+    if (!cfg) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL config", who));
+    if (t->best) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a best-shot tracker cannot look back", who));
+    if (t->lookback) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: look-back is already on", who));
+    if (t->updated) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker has already been updated", who));
+    const int L = cfg->frames ? cfg->frames : 15;
+    const float grow = cfg->grow != 0.f ? cfg->grow : 0.1f;
+    if (L < 1 || L > LOOKBACK_MAX_L) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frames %d, must be 0 or in [1, %d]", who, cfg->frames, LOOKBACK_MAX_L));
+    if (!(std::isfinite(grow) && grow > 0.f && grow <= 1.f))
+        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: grow %g, must be 0 or finite in (0, 1]", who, (double)cfg->grow));
+    const size_t rows = std::max(h->cfg.max_batch, L), recs = lookback_records(h->cfg.max_faces, t->cfg.max_tracks, L);
+    try {
+        CK(cudaSetDevice(h->device));
+        for (auto &s : t->slots) {
+            CK(cudaMalloc(&s.lb_boxes, sizeof(rf_det) * rows * recs));
+            CK(cudaMalloc(&s.lb_counts, sizeof(int) * rows));
+        }
+    } catch (const CudaFail &f) {
+        for (auto &s : t->slots) {
+            cudaFree(s.lb_boxes); cudaFree(s.lb_counts);
+            s.lb_boxes = nullptr;
+            s.lb_counts = nullptr;
+        }
+        return fail_cuda(h, f);
+    }
+    t->lookback = true;
+    t->lb_frames = L;
+    t->lb_grow = grow;
+    t->lbv.assign(t->cfg.max_videos, {});
+    return RF_OK;
+}
+
+extern "C++" {
+// An out frame of a look-back call: a valid descriptor with the size and layout (uv_step, chroma order) of the frames it receives.
+static int check_out_frame(rf_handle h, const char *who, const rf_yuv_frame &o, int i, int w, int ht, int step, bool v_first) {
+    if (!o.y || !o.u || !o.v) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: out frame %d has a NULL plane", who, i));
+    if (o.width != w || o.height != ht || o.uv_step != step)
+        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: out frame %d is %dx%d with uv_step %d, its video's frames are %dx%d with uv_step %d", who, i,
+                                               o.width, o.height, o.uv_step, w, ht, step));
+    const uintptr_t u = (uintptr_t)o.u, v = (uintptr_t)o.v;
+    if (step == 2 && ((v + 1 != u && u + 1 != v) || (v < u) != v_first))
+        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: out frame %d: semi-planar u and v must be adjacent, in the input's order", who, i));
+    if (o.y_pitch < w || o.uv_pitch < w / 2 * step)
+        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: out frame %d: pitches %d / %d below the row bytes %d / %d", who, i, o.y_pitch, o.uv_pitch, w, w / 2 * step));
+    return RF_OK;
+}
+
+static bool same_frame(const rf_yuv_frame &a, const rf_yuv_frame &b) {
+    return a.y == b.y && a.u == b.u && a.v == b.v && a.y_pitch == b.y_pitch && a.uv_pitch == b.uv_pitch && a.uv_step == b.uv_step &&
+           a.width == b.width && a.height == b.height;
+}
+
+static uint8_t *lb_log(rf_tracker t, const rf_tracker_s::LookbackVideo &v) { return v.d + (size_t)t->lb_frames * v.frame_bytes; }
+
+// The swap entry of one frame: its planes (in: NULL for a drain; out: NULL when it emits nothing) and its buffer slot.
+static LookbackSwapFrame lb_swap_frame(const rf_yuv_frame *in, const rf_yuv_frame *out, uint8_t *slot) {
+    const rf_yuv_frame &g = in ? *in : *out;
+    LookbackSwapFrame f{};
+    f.w = g.width;
+    f.h = g.height;
+    f.planar = g.uv_step == 1;
+    f.slot = slot;
+    if (in) {
+        f.in[0] = in->y;
+        f.in[1] = f.planar ? in->u : std::min(in->u, in->v);
+        f.in_v = in->v;
+        f.in_pitch[0] = in->y_pitch;
+        f.in_pitch[1] = in->uv_pitch;
+    }
+    if (out) {
+        f.out[0] = const_cast<uint8_t *>(out->y);
+        f.out[1] = const_cast<uint8_t *>(f.planar ? out->u : std::min(out->u, out->v));
+        f.out_v = const_cast<uint8_t *>(out->v);
+        f.out_pitch[0] = out->y_pitch;
+        f.out_pitch[1] = out->uv_pitch;
+    }
+    return f;
+}
+
+static void lb_swap(const std::vector<LookbackSwapFrame> &v, cudaStream_t s) {
+    for (size_t i0 = 0; i0 < v.size(); i0 += LOOKBACK_TABLE) {
+        LookbackSwapTable tb{};
+        int rows = 0;
+        for (size_t i = i0; i < std::min(v.size(), i0 + LOOKBACK_TABLE); i++) {
+            tb.f[tb.n++] = v[i];
+            rows = std::max(rows, v[i].h + (v[i].planar ? v[i].h : v[i].h / 2));
+        }
+        CK(launch_lookback_swap(tb, rows, s));
+    }
+}
+
+// The (a) + (b) + (c) records of the emitted frames {video, e, span} into ring slot `slot`'s look-back boxes.
+static void lb_boxes(rf_tracker t, rf_tracker_s::Slot &slot, const std::vector<std::array<long long, 3>> &em, cudaStream_t s) {
+    LookbackArgs a{};
+    a.max_faces = t->h->cfg.max_faces;
+    a.max_tracks = t->cfg.max_tracks;
+    a.slot_bytes = lookback_slot_bytes(a.max_faces, a.max_tracks);
+    a.ring = 2 * t->lb_frames;
+    a.grow = (double)t->lb_grow;
+    a.out = slot.lb_boxes;
+    a.out_counts = slot.lb_counts;
+    a.records = lookback_records(a.max_faces, a.max_tracks, t->lb_frames);
+    for (size_t j0 = 0; j0 < em.size(); j0 += LOOKBACK_TABLE) {
+        LookbackBoxTable tb{};
+        tb.j0 = (int)j0;
+        for (size_t j = j0; j < std::min(em.size(), j0 + LOOKBACK_TABLE); j++, tb.n++) {
+            tb.log[tb.n] = lb_log(t, t->lbv[em[j][0]]);
+            tb.e_slot[tb.n] = (int)(em[j][1] % a.ring);
+            tb.span[tb.n] = (int)em[j][2];
+        }
+        CK(launch_lookback_boxes(a, tb, s));
+    }
+}
+
+// Allocates (or, at a new frame size, replaces) the buffer of a video that has no buffered frames.  false: the allocation failed.
+static bool lb_alloc(rf_tracker t, rf_tracker_s::LookbackVideo &v, const rf_yuv_frame &f) {
+    const size_t fb = ((size_t)f.width * f.height * 3 / 2 + 255) & ~(size_t)255;
+    const size_t bytes = (size_t)t->lb_frames * fb + 2 * (size_t)t->lb_frames * lookback_slot_bytes(t->h->cfg.max_faces, t->cfg.max_tracks);
+    if (v.d && v.frame_bytes == fb) return true;
+    if (v.d) {
+        CK(cudaEventSynchronize(t->chain));      // the last drain's swap may still read it
+        CK(cudaFree(v.d));
+        v.d = nullptr;
+    }
+    if (cudaMalloc(&v.d, bytes) != cudaSuccess) {
+        cudaGetLastError();
+        v.d = nullptr;
+        return false;
+    }
+    v.frame_bytes = fb;
+    return true;
+}
+}  // extern "C++"
+
+int rf_detect_yuv_redact_lookback_device(rf_handle h, rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, int matrix, float thr,
+                                         float nms, const rf_redact_style *style, const rf_yuv_frame *out_frames, int32_t *out_frame_numbers,
+                                         const rf_track **dev_tracks, const int32_t **dev_track_counts, const rf_det **dev_dets,
+                                         const int32_t **dev_counts, float *out_scales) {
+    static const char *who = "rf_detect_yuv_redact_lookback_device";
+    if (!h) return RF_ERR_INVALID_ARG;
+    if (!t || t->h != h) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker is NULL or belongs to another handle", who));
+    if (!t->lookback) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: not a look-back tracker (rf_tracker_set_lookback)", who));
+    int rc = check_track_args(t, who, videos, n, nullptr);
+    if (rc) return rc;
+    const YuvFrames src{frames, matrix, nullptr, false};
+    if ((rc = src.check(h, who, n))) return rc;
+    RedactSpec spec;
+    if ((rc = redact_style(h, who, style, spec))) return rc;
+    if (n > 0 && (!out_frames || !out_frame_numbers)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL out frames or frame numbers", who));
+    const int L = t->lb_frames;
+    // each frame's number; a video's size and layout are those of its buffered frames, else of its first frame in the call
+    std::vector<long long> num(n);
+    std::vector<std::array<int, 3>> seen;        // (video, first frame of the call, frames in the call)
+    auto ranges = yuv_ranges(frames, n);
+    for (int i = 0; i < n; i++) {
+        const int v = videos[i];
+        auto it = std::find_if(seen.begin(), seen.end(), [v](const std::array<int, 3> &e) { return e[0] == v; });
+        if (it == seen.end()) it = seen.insert(seen.end(), std::array<int, 3>{v, i, 0});
+        const rf_tracker_s::LookbackVideo &lv = t->lbv[v];
+        const rf_yuv_frame &f = frames[i], &g = frames[(*it)[1]];
+        const bool v_first = f.uv_step == 2 && f.v < f.u;
+        const bool same = lv.frames > 0 ? f.width == lv.w && f.height == lv.h && f.uv_step == lv.step && v_first == lv.v_first
+                                        : f.width == g.width && f.height == g.height && f.uv_step == g.uv_step && v_first == (g.uv_step == 2 && g.v < g.u);
+        if (!same)
+            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frame %d: video %d changes its frame size or layout; drain or reset it first", who, i, v));
+        if (++(*it)[2] > L) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: video %d appears more than L = %d times in one call", who, v, L));
+        num[i] = lv.frames + (*it)[2] - 1;
+        if ((rc = check_out_frame(h, who, out_frames[i], i, f.width, f.height, f.uv_step, v_first))) return rc;
+        if (!same_frame(out_frames[i], f))
+            for (auto &r : yuv_ranges(out_frames + i, 1)) ranges.push_back({r[0], r[1], (uintptr_t)(n + i)});
+    }
+    if ((rc = check_disjoint(h, who, ranges))) return rc;
+    if (n == 0) return RF_OK;
+    try {
+        CK(cudaSetDevice(h->device));
+        for (const auto &e : seen) {
+            rf_tracker_s::LookbackVideo &lv = t->lbv[e[0]];
+            if (lv.frames > 0) continue;
+            const rf_yuv_frame &f = frames[e[1]];
+            if (!lb_alloc(t, lv, f))
+                return fail(h, RF_ERR_CAPACITY, fmt("%s: video %d: no device memory for %d frames of %dx%d", who, e[0], L, f.width, f.height));
+            lv.w = f.width;
+            lv.h = f.height;
+            lv.step = f.uv_step;
+            lv.v_first = f.uv_step == 2 && f.v < f.u;
+        }
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    std::vector<float> scales(n);
+    const rf_det *dets = nullptr;
+    const int32_t *counts = nullptr;
+    if ((rc = yuv_device_impl(h, who, src, n, thr, nms, nullptr, nullptr, nullptr, &dets, &counts, scales.data()))) return rc;
+    if (dev_dets) *dev_dets = dets;
+    if (dev_counts) *dev_counts = counts;
+    if (out_scales) std::copy(scales.begin(), scales.end(), out_scales);
+    try {
+        Ctx &c = last_ctx(h);          // the forward's context
+        const rf_track *tracks = nullptr;
+        const int32_t *track_counts = nullptr;
+        track_issue(t, videos, n, dets, counts, scales.data(), c.stream, nullptr, nullptr, &tracks, &track_counts, frames);
+        rf_tracker_s::Slot &slot = t->slots[(t->next_slot - 1) % t->slots.size()];
+        if (dev_tracks) *dev_tracks = tracks;
+        if (dev_track_counts) *dev_track_counts = track_counts;
+        // the update recorded the chain; the look-back state follows it on the same stream and records it again
+        LookbackArgs a{};
+        a.dets = dets;
+        a.counts = counts;
+        a.tracks = tracks;
+        a.track_counts = track_counts;
+        a.motion = t->motion ? slot.motion : nullptr;
+        a.max_faces = h->cfg.max_faces;
+        a.max_tracks = t->cfg.max_tracks;
+        a.slot_bytes = lookback_slot_bytes(a.max_faces, a.max_tracks);
+        a.ring = 2 * L;
+        for (int i0 = 0; i0 < n; i0 += LOOKBACK_TABLE) {
+            LookbackLogTable lt{};
+            lt.i0 = i0;
+            for (int i = i0; i < std::min(n, i0 + LOOKBACK_TABLE); i++, lt.n++) {
+                lt.scale[lt.n] = scales[i];
+                lt.slot[lt.n] = lb_log(t, t->lbv[videos[i]]) + (size_t)(num[i] % a.ring) * a.slot_bytes;
+            }
+            CK(launch_lookback_log(a, lt, c.stream));
+        }
+        std::vector<LookbackSwapFrame> sw;
+        std::vector<std::array<long long, 3>> em;
+        std::vector<rf_yuv_frame> outs;
+        for (int i = 0; i < n; i++) {
+            const rf_tracker_s::LookbackVideo &lv = t->lbv[videos[i]];
+            const bool emits = num[i] >= L;
+            sw.push_back(lb_swap_frame(frames + i, emits ? out_frames + i : nullptr, lv.d + (size_t)(num[i] % L) * lv.frame_bytes));
+            if (emits) {
+                em.push_back({videos[i], num[i] - L, L});
+                outs.push_back(out_frames[i]);
+            }
+        }
+        lb_swap(sw, c.stream);
+        lb_boxes(t, slot, em, c.stream);
+        CK(cudaEventRecord(t->chain, c.stream));
+        if (!em.empty())
+            redact_issue(h, c, yuv_redact_table(outs.data(), (int)outs.size(), nullptr), slot.lb_boxes, slot.lb_counts, nullptr, nullptr, nullptr,
+                         spec, lookback_records(h->cfg.max_faces, t->cfg.max_tracks, L));
+        CK(cudaEventRecord(slot.free, c.stream));
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    for (int i = 0; i < n; i++) {
+        t->lbv[videos[i]].frames = std::max(t->lbv[videos[i]].frames, num[i] + 1);
+        out_frame_numbers[i] = num[i] >= L ? (int32_t)(num[i] - L) : -1;
+    }
+    return RF_OK;
+}
+
+int rf_tracker_drain(rf_tracker t, int video, const rf_redact_style *style, const rf_yuv_frame *out_frames, int cap, int *n_out,
+                     int32_t *out_frame_numbers) {
+    static const char *who = "rf_tracker_drain";
+    if (!t) return RF_ERR_INVALID_ARG;
+    rf_handle h = t->h;
+    if (!t->lookback) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: not a look-back tracker (rf_tracker_set_lookback)", who));
+    if (video < 0 || video >= t->cfg.max_videos) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: video %d, must be in [0, %d)", who, video, t->cfg.max_videos));
+    RedactSpec spec;
+    int rc = redact_style(h, who, style, spec);
+    if (rc) return rc;
+    if (!n_out) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: n_out is NULL", who));
+    rf_tracker_s::LookbackVideo &lv = t->lbv[video];
+    const int L = t->lb_frames, k = (int)std::min<long long>(L, lv.frames);
+    if (cap < k) return fail(h, RF_ERR_CAPACITY, fmt("%s: video %d has %d buffered frames, cap is %d", who, video, k, cap));
+    if (k > 0 && (!out_frames || !out_frame_numbers)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL out frames or frame numbers", who));
+    for (int j = 0; j < k; j++)
+        if ((rc = check_out_frame(h, who, out_frames[j], j, lv.w, lv.h, lv.step, lv.v_first))) return rc;
+    if ((rc = check_disjoint(h, who, yuv_ranges(out_frames, k)))) return rc;
+    try {
+        CK(cudaSetDevice(h->device));
+        Ctx &c = h->ctx[0];
+        const unsigned ring = t->next_slot++ % t->slots.size();
+        rf_tracker_s::Slot &slot = t->slots[ring];
+        CK(cudaStreamWaitEvent(c.stream, slot.free, 0));
+        CK(cudaStreamWaitEvent(c.stream, t->chain, 0));
+        std::vector<LookbackSwapFrame> sw;
+        std::vector<std::array<long long, 3>> em;
+        for (int j = 0; j < k; j++) {
+            const long long e = lv.frames - k + j;
+            sw.push_back(lb_swap_frame(nullptr, out_frames + j, lv.d + (size_t)(e % L) * lv.frame_bytes));
+            em.push_back({video, e, lv.frames - 1 - e});
+        }
+        lb_swap(sw, c.stream);
+        lb_boxes(t, slot, em, c.stream);
+        // then the video restarts as rf_tracker_reset restarts it
+        const size_t T = t->cfg.max_tracks;
+        CK(cudaMemsetAsync(t->d_videos + video, 0, sizeof(TrackVideo), c.stream));
+        CK(cudaMemsetAsync(t->d_state + (size_t)video * T, 0, sizeof(TrackState) * T, c.stream));
+        if (t->motion) t->mref[video] = {0, 0};
+        CK(cudaEventRecord(t->chain, c.stream));
+        if (k > 0)
+            redact_issue(h, c, yuv_redact_table(out_frames, k, nullptr), slot.lb_boxes, slot.lb_counts, nullptr, nullptr, nullptr, spec,
+                         lookback_records(h->cfg.max_faces, t->cfg.max_tracks, L));
+        CK(cudaEventRecord(slot.free, c.stream));
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    for (int j = 0; j < k; j++) out_frame_numbers[j] = (int32_t)(lv.frames - k + j);
+    lv.frames = 0;
+    *n_out = k;
+    return RF_OK;
 }
 
 }  // extern "C"

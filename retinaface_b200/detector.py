@@ -170,7 +170,7 @@ class RetinaFace:
 
     def redactFrames(self, frames: Sequence, videos: Sequence[int] = None, threshold: float = 0.5, blocks: int = 0, margin: float = 0.0,
                      layout: str = "nv12", matrix: str = "bt601", max_videos: int = 64, motion=False, style: str = "mosaic",
-                     shape: str = "rect", detail: int = 0):
+                     shape: str = "rect", detail: int = 0, lookback: int = 0, out: Sequence = None):
         """f12 redaction: detect on device 4:2:0 frames (torch CUDA tensors in ``Engine.detect_yuv_device``'s forms) and mosaic every
         detected face IN PLACE (rf_detect_yuv_redact_device), ``blocks`` cells across a region's longer side (0: 8; 1: a flat patch),
         each side grown by ``margin`` of the box (0: 0.25).  With ``videos`` (frame i of video ``videos[i]``) the frames are also
@@ -178,14 +178,30 @@ class RetinaFace:
         tracker still follows while the detector misses it is redacted too.  Asynchronous: the frames are complete in stream order on
         ``engine.last_stream_ptr()``.  ``motion`` as ``trackFrames``: the lost faces' predicted boxes then follow the camera.  The first
         call decides the tracker.  f14: ``style="blur"`` blurs each region instead (``detail`` 0: 4; 1..64, a larger detail a smaller
-        radius; ``blocks`` must then stay 0), and ``shape="ellipse"`` redacts the ellipse inscribed in each region."""
+        radius; ``blocks`` must then stay 0), and ``shape="ellipse"`` redacts the ellipse inscribed in each region.
+        f15: ``lookback=L`` (with ``videos``) makes the tracker a look-back tracker: each frame is kept on the GPU and frame num - L of
+        its video, also covered where the faces first detected in the next L frames already were, is written into ``out[i]`` (None:
+        the input frame itself, in place).  Returns the emitted frame numbers (-1: nothing emitted yet); ``drainVideo`` emits the rest."""
         kw = dict(layout=layout, matrix=matrix, blocks=blocks, margin=margin, style=style, shape=shape, detail=detail)
         if videos is None:
+            if lookback:
+                raise ValueError("lookback needs videos: the buffered frames belong to a video")
             self.engine.detect_yuv_redact_device(list(frames), threshold, self.nms_threshold, **kw)
             return
         if getattr(self, "_tracker", None) is None:
-            self._tracker = self.engine.tracker(max_videos=max_videos, motion=motion)
+            self._tracker = self.engine.tracker(max_videos=max_videos, motion=motion, lookback=lookback or None)
+        if lookback:
+            return self._tracker.detect_yuv_redact_lookback_device(list(frames), list(videos), list(frames if out is None else out), threshold,
+                                                                   self.nms_threshold, **kw)[0]
         self._tracker.detect_yuv_redact_device(list(frames), list(videos), threshold, self.nms_threshold, **kw)
+
+    def drainVideo(self, video: int, out: Sequence, layout: str = "nv12", blocks: int = 0, margin: float = 0.0, style: str = "mosaic",
+                   shape: str = "rect", detail: int = 0):
+        """f15: end ``video`` on a look-back tracker (rf_tracker_drain): its buffered frames (at most L, in frame order) go, redacted,
+        into ``out[0..)``; then the video restarts.  Returns their frame numbers."""
+        if getattr(self, "_tracker", None) is None or not self._tracker.lookback:
+            raise ValueError("drainVideo needs a look-back tracker: call redactFrames(..., lookback=L) first")
+        return self._tracker.drain(video, list(out), layout=layout, blocks=blocks, margin=margin, style=style, shape=shape, detail=detail)
 
     def _best_crops(self, n: int):
         import torch

@@ -322,8 +322,12 @@ void RetinaFace::noteMotion(int n) {
     motion_.n = n;
 }
 
-void RetinaFace::redactYUV(const vector<rf_yuv_frame> &device_frames, const vector<int> *videos, float threshold, const RedactOptions &opt) {
+void RetinaFace::redactYUV(const vector<rf_yuv_frame> &device_frames, const vector<int> *videos, float threshold, const RedactOptions &opt,
+                           const vector<rf_yuv_frame> *out_frames) {
     if (videos && videos->size() != device_frames.size()) throw std::invalid_argument("redactYUV: one video index per frame");
+    if (opt.lookback && !videos) throw std::invalid_argument("redactYUV: lookback needs videos");
+    if (out_frames && (!opt.lookback || out_frames->size() != device_frames.size()))
+        throw std::invalid_argument("redactYUV: out_frames go with lookback, one per frame");
     if (device_frames.size() > (size_t)opt_.max_batch) throw std::invalid_argument("redactYUV: at most max_batch frames per call");
     if (videos && best_tracker_) throw std::logic_error("redactYUV: this RetinaFace tracks with best shots (trackYUVBest)");
     if (videos && !tracker_) {
@@ -332,10 +336,28 @@ void RetinaFace::redactYUV(const vector<rf_yuv_frame> &device_frames, const vect
         int rc = rf_tracker_create(h_, &tc, &tracker_);
         if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_create: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
         trackerCreated();
+        if (opt.lookback) {
+            const rf_lookback_config lc{opt.lookback, 0.f};
+            rc = rf_tracker_set_lookback(tracker_, &lc);
+            if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_set_lookback: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+        }
     }
     const rf_redact_style st{opt.style, opt.shape, opt.style == RF_REDACT_BLUR ? 0 : opt.blocks, opt.detail, opt.margin};
     const int n = (int)device_frames.size();
     DeviceTracks t{};
+    if (opt.lookback) {
+        frame_numbers_.assign(n, -1);
+        int rc = rf_detect_yuv_redact_lookback_device(h_, tracker_, device_frames.data(), videos->data(), n, RF_YUV_BT601, threshold, nms_threshold,
+                                                      &st, (out_frames ? out_frames : &device_frames)->data(), frame_numbers_.data(), &t.tracks,
+                                                      &t.counts, nullptr, nullptr, nullptr);
+        if (rc != RF_OK)
+            throw std::runtime_error(string("rf_detect_yuv_redact_lookback_device: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+        tracks_ = t;
+        tracks_.n = n;
+        tracks_.max_tracks = 64;      // rf_track_config's default
+        noteMotion(n);
+        return;
+    }
     int rc = rf_detect_yuv_redact_device_style(h_, videos ? tracker_ : nullptr, device_frames.data(), videos ? videos->data() : nullptr, n,
                                                RF_YUV_BT601, threshold, nms_threshold, &st, &t.tracks, &t.counts, nullptr, nullptr, nullptr);
     if (rc != RF_OK)
@@ -412,4 +434,15 @@ Mat RetinaFace::draw(const Mat &img, const vector<FaceDetectInfo> &faces) {
         }
     }
     return out;
+}
+
+vector<int32_t> RetinaFace::drainVideo(int video, const vector<rf_yuv_frame> &out_frames, const RedactOptions &opt) {
+    if (!tracker_) throw std::logic_error("drainVideo: no look-back tracker (redactYUV with lookback first)");
+    const rf_redact_style st{opt.style, opt.shape, opt.style == RF_REDACT_BLUR ? 0 : opt.blocks, opt.detail, opt.margin};
+    vector<int32_t> nums(out_frames.size());
+    int n = 0;
+    int rc = rf_tracker_drain(tracker_, video, &st, out_frames.data(), (int)out_frames.size(), &n, nums.data());
+    if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_drain: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+    nums.resize(n);
+    return nums;
 }

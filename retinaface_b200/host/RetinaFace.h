@@ -59,6 +59,8 @@ struct RedactOptions {
     int style = RF_REDACT_MOSAIC;        // RF_REDACT_MOSAIC or RF_REDACT_BLUR
     int shape = RF_REDACT_RECT;          // RF_REDACT_RECT or RF_REDACT_ELLIPSE (the ellipse inscribed in the region)
     int detail = 0;                      // blur: 0 (4) or 1..64, a larger detail a smaller radius; 0 for the mosaic
+    int lookback = 0;                    // f15, with videos: L (1..64) frames of delay, so that faces are covered before their first
+                                         // detection (rf_detect_yuv_redact_lookback_device); 0: redact in place, undelayed
 };
 
 class RetinaFace {
@@ -148,8 +150,14 @@ class RetinaFace {
     // GPU; asynchronous on rf_last_stream(handle()).  With `videos` (one per frame, in [0, track_videos)) the frames are also tracked on
     // this RetinaFace's plain tracker (trackYUV's), lastTracks() holds the lists, and the predicted box of every LOST track -- a face the
     // detector missed on this frame -- is redacted too.
+    // f15: with opt.lookback = L the tracker (created by the first tracked call) keeps each video's last L frames on the GPU, and
+    // frame i writes frame num_i - L of its video, also covered where the faces first detected in the next L frames already were,
+    // into out_frames[i] (nullptr: device_frames[i] itself); lastFrameNumbers()[i] is num_i - L, or -1 while the video fills.
+    // drainVideo writes the video's remaining buffered frames into out_frames[0..) and restarts it; it returns their numbers.
     void redactYUV(const vector<rf_yuv_frame> &device_frames, const vector<int> *videos = nullptr, float threshold = 0.5,
-                   const RedactOptions &opt = RedactOptions());
+                   const RedactOptions &opt = RedactOptions(), const vector<rf_yuv_frame> *out_frames = nullptr);
+    const vector<int32_t> &lastFrameNumbers() const { return frame_numbers_; }
+    vector<int32_t> drainVideo(int video, const vector<rf_yuv_frame> &out_frames, const RedactOptions &opt = RedactOptions());
     rf_handle handle() const { return h_; }
     // the reference's visualisation (RetinaFace.cpp:730-741): red box outline (thickness 2), green landmark dots, on a clone
     static Mat draw(const Mat &img, const vector<FaceDetectInfo> &faces);
@@ -167,6 +175,7 @@ class RetinaFace {
     DeviceTracks tracks_;
     DeviceBestShots best_;
     DeviceMotion motion_;
+    vector<int32_t> frame_numbers_;
     RetinaFaceOptions opt_;
     string network;
     float nms_threshold;

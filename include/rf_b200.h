@@ -498,7 +498,8 @@ typedef struct rf_track {
     int32_t id, state;              /* per-video id; RF_TRACK_* */
     int32_t det;                    /* index of the record matched on this frame, -1 */
     int32_t crop_slot;              /* this frame's crop j of the track, -1 */
-    int32_t hits, age, lost_frames, reserved;
+    int32_t hits, age, lost_frames;
+    int32_t followed;               /* f16: 1 when the track was moved by template search on this frame, else 0 */
     float kx1, ky1, kx2, ky2;       /* filtered box (mean after this frame), frame pixels */
     float vx, vy;                   /* centre velocity, pixels per frame */
     rf_face face;                   /* last matched detection, frame pixels */
@@ -841,6 +842,92 @@ int rf_detect_yuv_redact_lookback_device(rf_handle h, rf_tracker t, const rf_yuv
  * frames and emits nothing. */
 int rf_tracker_drain(rf_tracker t, int video, const rf_redact_style *style, const rf_yuv_frame *out_frames, int cap, int *n_out,
                      int32_t *out_frame_numbers);
+
+/* f16 following between detections: run the detector on key frames only and move every known face on the frames in between by
+ * searching for its own pixels, the way deployed detect + track pipelines run at a detection interval.  A FOLLOW tracker
+ * (rf_tracker_set_follow) keeps, per track, a luma template cut on the track's last detection frame, and takes two kinds of frames:
+ * detect frames through rf_detect_yuv_track_device / rf_detect_yuv_redact_device(_style) -- records, track lists and redacted
+ * bytes exactly a plain tracker's, plus the cut below -- and follow frames through rf_track_follow_device, which runs no detector.
+ * Every FP64 step is one rounding in the order written; pixels are integers (oracle/follow.py restates every bit).
+ *   Grid        of a box (cx, cy, w, h) at scale c: gw = (w * G) * c, gh = (h * G) * c with G = 1 + 2 RF_FOLLOW_MARGIN;
+ *               px = gw / T, py = gh / T (T = RF_FOLLOW_TEMPLATE); ox = ((cx - gw / 2) + px / 2) - 0.5, oy likewise: template pixel
+ *               (i, j) is centred on frame point (ox + px i, oy + py j).
+ *   Sampler     cv2.warpAffine(luma, [[px, 0, X], [0, py, Y]], INTER_LINEAR | WARP_INVERSE_MAP, BORDER_CONSTANT 0), byte for byte:
+ *               Xf = (rint(X * 1024) + 16 + rint((px * i) * 1024)) >> 5, Yf = (rint((py * j + Y) * 1024) + 16) >> 5 (rint: half to
+ *               even), then f5's 1/32-pixel integer bilinear; a pixel is INSIDE when its four taps lie in the frame.
+ *   Cut         on every detect frame, for each track whose det >= 0 after the frame (births included; of several frames of one
+ *               video in a call, the track's last such frame): the T x T template at (X, Y) = (ox, oy) of its face box (x1..y2 widened
+ *               to double; w = x2 - x1, h = y2 - y1, cx = x1 + w / 2, cy = y1 + h / 2; c = 1).  The template is FLAT when
+ *               T^2 sum(p^2) - (sum p)^2 < RF_FOLLOW_MIN_VAR T^4.  NV12, NV21, I420 and YV12 give the same templates.
+ * On a follow frame every live track is predicted (f10) and, on a motion tracker, moved by the frame's camera motion (f13's
+ * compensation, when RF_MOTION_OK); then each TENTATIVE or CONFIRMED track is searched from that state m (pcx = m_cx, pcy = m_cy,
+ * pw = m_a * m_h, ph = m_h).  A state with ph or pw outside (0, 65536] or |pcx| or |pcy| above 65536 is not searched: MISMATCH.
+ *   Windows     for scale k in {0, 1, 2}, c_k = {1 / RF_FOLLOW_SCALE, 1, RF_FOLLOW_SCALE} (1 / s one rounding): the grid of the
+ *               predicted box at c_k, sampled as a (T + 2R) square at (X, Y) = (ox - R px, oy - R py) (R px one rounding).
+ *   Match       SAD(k, dy, dx) = sum |template(i, j) - window_k(R + dx + i, R + dy + j)| over |dx|, |dy| <= R; the minimum under
+ *               the order (SAD, |dx| + |dy|, k, dy, dx).  Sub-pixel per axis, when the minimum is inside the border: f =
+ *               (S(-1) - S(+1)) / (2 (S(-1) - 2 S0 + S(+1))) (integers, one division; 0 when the denominator is 0), else 0.
+ *   Box         ncx = pcx + ((double)dx + fx) * px_k, ncy likewise; nw = pw * c_k, nh = ph * c_k; x1 = ncx - nw / 2,
+ *               y1 = ncy - nh / 2, x2 = ncx + nw / 2, y2 = ncy + nh / 2, each rounded to float.  Landmarks of the previous face f:
+ *               ow = f.x2 - f.x1, ocx = f.x1 + ow / 2 (y likewise), l' = (float)(ncx + (l - ocx) * (nw / ow)); the score is kept.
+ *   Status      (searched tracks) in this order: RF_FOLLOW_FLAT (the track's template is FLAT, or it has none), RF_FOLLOW_OUTSIDE (4 x the INSIDE
+ *               pixels of the chosen candidate < 3 T^2), RF_FOLLOW_BORDER (|dx| or |dy| == R), RF_FOLLOW_MISMATCH (SAD > max_mad *
+ *               T^2, in double, or the box is empty), else RF_FOLLOW_OK.
+ *   Tracker     replaces f10's association on a follow frame: an OK track takes f10's Kalman update with z of the followed box,
+ *               lost_frames = 0, face = the followed face, followed = 1, hits and state unchanged (hits count detector matches); a
+ *               failed CONFIRMED track becomes LOST, a failed TENTATIVE track is removed; LOST tracks are predicted only and count
+ *               lost_frames as in f10.  No births, no confirmations, det = -1 and crop_slot = -1 everywhere; age and the video's
+ *               frame count advance.  Frames of one video in one call are applied in call order, each searched from the state
+ *               the previous one left.
+ *   Motion      f13 estimates a follow frame from luma as on a detect frame, except that its face mask (step 2) takes, in place of
+ *               the frame's records, the face boxes of the video's TENTATIVE and CONFIRMED tracks before the frame (scale 1).
+ *   Redaction   of a follow frame (rf_track_follow_redact_device): (a) every OK-followed track's face box, in id order, then (b) every
+ *               LOST track of the frame's list, (kx1, ky1, kx2, ky2), in id order; f12's geometry, f14's styles and ownership.
+ * Templates are cut on detect frames only, so a run of follow frames always compares against the detector-anchored appearance and
+ * its error cannot build up. */
+#define RF_FOLLOW_TEMPLATE 32
+#define RF_FOLLOW_MARGIN 0.25            /* context around the face box, a fraction of its size on each side */
+#define RF_FOLLOW_SCALE 1.05
+#define RF_FOLLOW_MIN_VAR 16             /* texture floor of a template, luma levels squared */
+#define RF_FOLLOW_MAX_SEARCH 16
+#define RF_FOLLOW_OK       0
+#define RF_FOLLOW_FLAT     1
+#define RF_FOLLOW_BORDER   2
+#define RF_FOLLOW_MISMATCH 3
+#define RF_FOLLOW_OUTSIDE  4
+#define RF_FOLLOW_LOST     5             /* a LOST track: predicted only, not searched */
+typedef struct rf_follow_config {
+    int search;          /* R, template pixels: 0 -> 8, else 1..RF_FOLLOW_MAX_SEARCH */
+    float max_mad;       /* mean absolute difference bound, luma levels: 0 -> 24, else finite in (0, 255] */
+} rf_follow_config;
+typedef struct rf_follow {
+    int32_t id, status;          /* track id; RF_FOLLOW_* */
+    int32_t dx, dy, scale, sad;  /* the minimum: offset in template pixels, scale index k, its SAD (0 for LOST tracks) */
+    float fx, fy;                /* sub-pixel fractions */
+    float x1, y1, x2, y2;        /* the followed box, frame pixels (kept by the track only when status is OK) */
+} rf_follow;
+/* Makes a plain or motion tracker a follow tracker, before its first update.  Allocates a template store of max_videos x max_tracks x
+ * RF_FOLLOW_TEMPLATE^2 bytes (above 4 GiB: RF_ERR_CAPACITY).  A best-shot or look-back tracker, a second call, a call after an
+ * update, or bad values: RF_ERR_INVALID_ARG; rf_tracker_set_lookback refuses a follow tracker, rf_tracker_set_motion may come before
+ * or after (both before the first update).
+ * rf_track_update, which has no pixels, refuses a follow tracker; rf_tracker_reset drops the video's templates. */
+int rf_tracker_set_follow(rf_tracker t, const rf_follow_config *cfg);
+/* The follow step on n device frames (frame i of video videos[i]) of a follow tracker: windows sampled from each frame's luma,
+ * then the tracker step above.  *dev_tracks / *dev_track_counts as rf_track_update's, in the same ring.  Statuses as rf_track_update
+ * (frames checked as rf_detect_yuv_batch_device checks them), a tracker that is not a follow tracker: RF_ERR_INVALID_ARG; all
+ * before anything is launched.  Asynchronous on rf_last_stream()'s stream, inside the tracker's event chain; the caller keeps the
+ * frames alive until that stream has passed the call.  n = 0 launches nothing.  On a motion tracker rf_tracker_motion then returns
+ * the call's [n] estimates. */
+int rf_track_follow_device(rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, const rf_track **dev_tracks,
+                           const int32_t **dev_track_counts);
+/* rf_track_follow_device (the same lists, bit for bit), then the frames redacted in place with `style` (NULL: the zeroed struct's
+ * defaults) over the regions above.  Statuses of rf_track_follow_device, then a bad style or frames whose plane byte ranges overlap
+ * (RF_ERR_INVALID_ARG), all before anything is launched; asynchronous on rf_last_stream()'s context. */
+int rf_track_follow_redact_device(rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, const rf_redact_style *style,
+                                  const rf_track **dev_tracks, const int32_t **dev_track_counts);
+/* *dev_follow -> [n][max_tracks] rf_follow of the tracker's latest follow call, each frame's records in its track-list order (NULL
+ * before the first); valid for `streams` further tracker calls.  RF_ERR_INVALID_ARG on a tracker that is not a follow tracker. */
+int rf_tracker_follow(rf_tracker t, const rf_follow **dev_follow);
 
 /* Introspection. */
 int rf_get_net_size(rf_handle h, int *net_w, int *net_h, int *max_batch, int *max_faces);

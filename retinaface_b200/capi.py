@@ -38,6 +38,7 @@ EXPORTS = [
     "rf_redact_yuv_device", "rf_redact_device", "rf_detect_yuv_redact_device",
     "rf_redact_yuv_device_style", "rf_redact_device_style", "rf_detect_yuv_redact_device_style",
     "rf_tracker_set_lookback", "rf_detect_yuv_redact_lookback_device", "rf_tracker_drain",
+    "rf_tracker_set_follow", "rf_track_follow_device", "rf_tracker_follow", "rf_track_follow_redact_device",
 ]
 COMM_BLOB_BYTES = 128
 
@@ -204,14 +205,14 @@ class Face(C.Structure):         # rf_face
 
 
 class TrackRecord(C.Structure):  # rf_track
-    _fields_ = [(f, C.c_int32) for f in ("id", "state", "det", "crop_slot", "hits", "age", "lost_frames", "reserved")] + \
+    _fields_ = [(f, C.c_int32) for f in ("id", "state", "det", "crop_slot", "hits", "age", "lost_frames", "followed")] + \
                [(f, C.c_float) for f in ("kx1", "ky1", "kx2", "ky2", "vx", "vy")] + [("face", Face)]
 
 
 TRACK_TENTATIVE, TRACK_CONFIRMED, TRACK_LOST = 0, 1, 2      # RF_TRACK_*
 TRACK_DEBUG_DOUBLES = 25                                     # RF_TRACK_DEBUG_DOUBLES
 # one rf_track as a numpy record (the layout of TrackRecord)
-TRACK_DTYPE = np.dtype([(f, "<i4") for f in ("id", "state", "det", "crop_slot", "hits", "age", "lost_frames", "reserved")] +
+TRACK_DTYPE = np.dtype([(f, "<i4") for f in ("id", "state", "det", "crop_slot", "hits", "age", "lost_frames", "followed")] +
                        [(f, "<f4") for f in ("kx1", "ky1", "kx2", "ky2", "vx", "vy")] + [("face", "<f4", (FACE_FLOATS,))])
 
 
@@ -251,6 +252,21 @@ class Motion(C.Structure):       # rf_motion
 MOTION_OK, MOTION_FIRST, MOTION_LOST = 0, 1, 2               # RF_MOTION_*
 # one rf_motion as a numpy record (the layout of Motion)
 MOTION_DTYPE = np.dtype([(f, "<i4") for f in ("status", "blocks", "inliers", "reserved")] + [("m", "<f8", (6,))])
+
+
+class FollowConfig(C.Structure):  # rf_follow_config
+    _fields_ = [("search", C.c_int), ("max_mad", C.c_float)]
+
+
+class FollowRecord(C.Structure):  # rf_follow
+    _fields_ = [(f, C.c_int32) for f in ("id", "status", "dx", "dy", "scale", "sad")] + \
+               [(f, C.c_float) for f in ("fx", "fy", "x1", "y1", "x2", "y2")]
+
+
+FOLLOW_OK, FOLLOW_FLAT, FOLLOW_BORDER, FOLLOW_MISMATCH, FOLLOW_OUTSIDE, FOLLOW_LOST = range(6)   # RF_FOLLOW_*
+# one rf_follow as a numpy record (the layout of FollowRecord)
+FOLLOW_DTYPE = np.dtype([(f, "<i4") for f in ("id", "status", "dx", "dy", "scale", "sad")] +
+                        [(f, "<f4") for f in ("fx", "fy", "x1", "y1", "x2", "y2")])
 
 
 class RedactParams(C.Structure):  # rf_redact_params
@@ -444,6 +460,11 @@ def load_library() -> C.CDLL:
     lib.rf_tracker_set_lookback.argtypes = [C.c_void_p, C.POINTER(LookbackConfig)]
     lib.rf_detect_yuv_redact_lookback_device.argtypes = a[:9] + [C.POINTER(YuvFrame), C.c_void_p] + a[9:]
     lib.rf_tracker_drain.argtypes = [C.c_void_p, C.c_int, C.POINTER(RedactStyle), C.POINTER(YuvFrame), C.c_int, C.POINTER(C.c_int), C.c_void_p]
+    lib.rf_tracker_set_follow.argtypes = [C.c_void_p, C.POINTER(FollowConfig)]
+    lib.rf_track_follow_device.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_void_p, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
+    lib.rf_tracker_follow.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
+    lib.rf_track_follow_redact_device.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_void_p, C.c_int, C.POINTER(RedactStyle),
+                                                  C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
     _lib = lib
     return lib
 
@@ -1103,12 +1124,14 @@ class Engine:
     # -- f10 face tracking across video frames ---------------------------------------------------------------------------------
     def tracker(self, max_videos: int = 1, max_tracks: int = 0, high_thresh: float = 0.0, new_thresh: float = 0.0, iou_high: float = 0.0,
                 iou_low: float = 0.0, iou_tentative: float = 0.0, max_lost: int = 0, best: Optional[dict] = None,
-                motion=None, lookback=None) -> "Tracker":
+                motion=None, lookback=None, follow=None) -> "Tracker":
         """rf_tracker_create: a tracker of max_videos independent sequences on this engine (0 -> the defaults of rf_track_config).
         best (``best_config`` keywords): a best-shot tracker (rf_tracker_create_best), fed through ``Tracker.detect_yuv_best_device``.
         motion (True or ``motion_config`` keywords): camera-motion compensation (rf_tracker_set_motion) from the frames of the
         detect_yuv_* calls; read each call's estimates with ``Tracker.motion``.  lookback (True, L, or ``set_lookback`` keywords): a
-        look-back tracker (rf_tracker_set_lookback), fed through ``Tracker.detect_yuv_redact_lookback_device``."""
+        look-back tracker (rf_tracker_set_lookback), fed through ``Tracker.detect_yuv_redact_lookback_device``.  follow (True or
+        ``set_follow`` keywords): a follow tracker (rf_tracker_set_follow), whose frames between detections go through
+        ``Tracker.follow_device``."""
         t = Tracker(self, TrackConfig(max_videos, max_tracks, high_thresh, new_thresh, iou_high, iou_low, iou_tentative, max_lost),
                     best_config(**best) if best is not None else None)
         try:
@@ -1116,6 +1139,8 @@ class Engine:
                 t.set_motion(**(motion if isinstance(motion, dict) else {}))
             if lookback:
                 t.set_lookback(**(lookback if isinstance(lookback, dict) else {} if lookback is True else {"frames": int(lookback)}))
+            if follow:
+                t.set_follow(**(follow if isinstance(follow, dict) else {}))
         except Exception:
             t.close()
             raise
@@ -1231,6 +1256,7 @@ class Tracker:
         self.best = best
         self.motion_on = False
         self.lookback = 0            # L of a look-back tracker
+        self.follow_on = False
         self.max_videos = cfg.max_videos
         self.max_tracks = cfg.max_tracks or 64
 
@@ -1376,6 +1402,45 @@ class Tracker:
         n_out = C.c_int(0)
         self.engine._check(self.lib.rf_tracker_drain(self.t, int(video), C.byref(st), outs, k, C.byref(n_out), nums.ctypes.data))
         return nums[:n_out.value].copy()
+
+    def set_follow(self, search: int = 0, max_mad: float = 0.0):
+        """rf_tracker_set_follow, before the first update: cut a luma template of every track on its detection frames, so that the
+        frames in between can go through ``follow_device`` (search: R in template pixels, 0 -> 8; max_mad: 0 -> 24)."""
+        cfg = FollowConfig(int(search), float(max_mad))
+        self.engine._check(self.lib.rf_tracker_set_follow(self.t, C.byref(cfg)))
+        self.follow_on = True
+
+    def follow_device(self, frames, videos: Sequence[int], layout: str = "nv12"):
+        """rf_track_follow_device: move every track of the device 4:2:0 frames' videos by template search, without the detector.
+        Asynchronous.  Returns the (tracks_ptr, track_counts_ptr) device addresses; read them with ``read``."""
+        n = len(frames)
+        arr = self.engine._frames(frames, layout, True)
+        tp, tc = C.c_void_p(), C.c_void_p()
+        self.engine._check(self.lib.rf_track_follow_device(self.t, arr, self._ints(videos, n), n, C.byref(tp), C.byref(tc)))
+        return int(tp.value or 0), int(tc.value or 0)
+
+    def follow_redact_device(self, frames, videos: Sequence[int], layout: str = "nv12", blocks: int = 0, margin: float = 0.0,
+                             style: str = "mosaic", shape: str = "rect", detail: int = 0):
+        """rf_track_follow_redact_device: follow_device, then redact the frames IN PLACE over every OK-followed face and every LOST
+        track (``redact_style``'s keywords).  Returns the (tracks_ptr, track_counts_ptr) device addresses."""
+        n = len(frames)
+        arr = self.engine._frames(frames, layout, True)
+        st = _style_struct(style, shape, blocks, detail, margin)
+        tp, tc = C.c_void_p(), C.c_void_p()
+        self.engine._check(self.lib.rf_track_follow_redact_device(self.t, arr, self._ints(videos, n), n, C.byref(st), C.byref(tp), C.byref(tc)))
+        return int(tp.value or 0), int(tc.value or 0)
+
+    def follow(self, n: int) -> np.ndarray:
+        """rf_tracker_follow: the [n][max_tracks] rf_follow records (FOLLOW_DTYPE) of the latest follow call, each frame's in its
+        track-list order, copied after the last stream."""
+        import torch
+        p = C.c_void_p()
+        self.engine._check(self.lib.rf_tracker_follow(self.t, C.byref(p)))
+        if not p.value:
+            raise RuntimeError("no follow call has been made on this tracker")
+        self.engine._check(self.lib.rf_synchronize(self.engine.h))
+        raw = torch.as_tensor(_DevArray(int(p.value), (n * self.max_tracks * FOLLOW_DTYPE.itemsize,), "|u1"), device="cuda").cpu().numpy()
+        return raw.view(FOLLOW_DTYPE).reshape(n, self.max_tracks).copy()
 
     def reset(self, video: int = -1):
         """rf_tracker_reset: restart one video (ids from 1), or all with -1; ordered after every issued update."""

@@ -15,6 +15,7 @@
 #include "track.cuh"
 #include "motion.cuh"
 #include "lookback.cuh"
+#include "follow.cuh"
 
 namespace rf_eng {
 
@@ -1894,6 +1895,19 @@ struct rf_tracker_s {
         long long frames = 0;          // frames since create, reset or drain
     };
     std::vector<LookbackVideo> lbv;
+    // f16 following (follow.cuh); `follow` false: none of these allocated.  The chain orders the per-call measurements as it orders
+    // f11's tables; the follow records live in the ring.
+    bool follow = false;
+    rf_follow_config fcfg{};
+    uint8_t *d_fstore = nullptr;         // [max_videos][max_tracks][FOLLOW_BYTES]
+    FollowEntry *d_fentries = nullptr;   // [max_videos][max_tracks]
+    FollowMeas *d_fmeas = nullptr;       // [max_batch][max_tracks]
+    rf_follow *d_follow = nullptr;       // [slots][max_batch][max_tracks]
+    rf_det *d_fregions = nullptr;        // [slots][max_batch][max_tracks] the OK-followed faces (redaction's records)
+    int *d_fregion_counts = nullptr;     // [slots][max_batch]
+    rf_det *d_fmask = nullptr;           // [max_batch][max_tracks] with motion: each follow frame's face mask
+    int *d_fmask_counts = nullptr;       // [max_batch]
+    int follow_slot = -1;                // the ring slot of the latest follow call
 };
 
 static void tracker_release(rf_tracker t) {
@@ -1905,6 +1919,8 @@ static void tracker_release(rf_tracker t) {
     }
     for (auto &v : t->lbv) cudaFree(v.d);
     cudaFree(t->d_mstore); cudaFree(t->d_mthumbs); cudaFree(t->d_mblocks);
+    cudaFree(t->d_fstore); cudaFree(t->d_fentries); cudaFree(t->d_fmeas); cudaFree(t->d_follow);
+    cudaFree(t->d_fregions); cudaFree(t->d_fregion_counts); cudaFree(t->d_fmask); cudaFree(t->d_fmask_counts);
     if (t->chain) cudaEventDestroy(t->chain);
     cudaFree(t->d_videos); cudaFree(t->d_state); cudaFree(t->d_pairs); cudaFree(t->d_order);
     const BestArgs &b = t->ba;
@@ -1984,6 +2000,7 @@ int rf_tracker_reset(rf_tracker t, int video) {
         }
         for (size_t v = v0; t->motion && v < v0 + nv; v++) t->mref[v] = {0, 0};
         for (size_t v = v0; t->lookback && v < v0 + nv; v++) t->lbv[v].frames = 0;     // the buffered frames are dropped
+        if (t->follow) CK(cudaMemsetAsync(t->d_fentries + v0 * T, 0, sizeof(FollowEntry) * nv * T, s));
         CK(cudaEventRecord(t->chain, s));
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
@@ -2075,6 +2092,35 @@ static void motion_commit(rf_tracker t, const MotionCommits &c, cudaStream_t s) 
     CK(launch_motion_commit(a, c.frames.data(), c.videos.data(), c.bytes.data(), (int)c.frames.size(), s));
 }
 
+// ---- f16 following (follow.cuh) -------------------------------------------------------------------------------------------------
+static FollowArgs follow_args(rf_tracker t) {
+    FollowArgs f{};
+    f.p = TrackParams{t->cfg.max_tracks, t->h->cfg.max_faces, t->cfg.max_lost, t->cfg.high_thresh, t->cfg.new_thresh, t->cfg.iou_high,
+                      t->cfg.iou_low, t->cfg.iou_tentative};
+    f.videos = t->d_videos;
+    f.state = t->d_state;
+    f.store = t->d_fstore;
+    f.entries = t->d_fentries;
+    f.meas = t->d_fmeas;
+    f.search = t->fcfg.search;
+    f.max_mad = t->fcfg.max_mad;
+    return f;
+}
+
+static FollowFrame follow_frame(const rf_yuv_frame &fr, int video, int i) {
+    return FollowFrame{fr.y, fr.y_pitch, fr.width, fr.height, video, i};
+}
+
+// The templates of the tracks matched on a detect call's frames, from the call's lists in `slot`, on s inside the chain.
+static void follow_cut(rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, const rf_tracker_s::Slot &slot, cudaStream_t s) {
+    FollowArgs f = follow_args(t);
+    f.lists = slot.tracks;
+    f.list_counts = slot.counts;
+    std::vector<FollowFrame> tab(n);
+    for (int i = 0; i < n; i++) tab[i] = follow_frame(frames[i], videos[i], i);
+    CK(launch_follow_cut(f, tab.data(), n, s));
+}
+
 // Issues the update of n frames on s (the records complete there) into the next ring slot, ordered by the chain.  `a` (crops):
 // the due faces are cut on s into a's crops, then the slot's `free` is recorded.
 static void track_issue(rf_tracker t, const int *videos, int n, const rf_det *dets, const int32_t *counts, const float *scales, cudaStream_t s,
@@ -2107,6 +2153,7 @@ static void track_issue(rf_tracker t, const int *videos, int n, const rf_det *de
     ta.motion = t->motion ? slot.motion : nullptr;
     CK(launch_track_update(ta, videos, scales, n, s));
     if (t->motion) motion_commit(t, commits, s);
+    if (t->follow) follow_cut(t, frames, videos, n, slot, s);
     CK(cudaEventRecord(t->chain, s));
     if (a) {
         PostBuffers view{};
@@ -2127,6 +2174,7 @@ int rf_track_update(rf_tracker t, const int *videos, int n, const rf_det *dev_de
     rf_handle h = t->h;
     if (t->best) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a best-shot tracker takes frames only through rf_detect_yuv_track_best_device", who));
     if (t->motion) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a motion tracker needs the frames (rf_detect_yuv_track_device)", who));
+    if (t->follow) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a follow tracker needs the frames (rf_detect_yuv_track_device)", who));
     if (t->lookback) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a look-back tracker takes frames only through rf_detect_yuv_redact_lookback_device", who));
     int rc = check_track_args(t, who, videos, n, scales);
     if (rc) return rc;
@@ -2388,6 +2436,194 @@ int rf_tracker_motion(rf_tracker t, const rf_motion **dev_motion) {
     if (!dev_motion) return fail(t->h, RF_ERR_INVALID_ARG, "rf_tracker_motion: dev_motion is NULL");
     if (!t->motion) return fail(t->h, RF_ERR_INVALID_ARG, "rf_tracker_motion: motion is off (rf_tracker_set_motion)");
     *dev_motion = t->motion_slot < 0 ? nullptr : t->slots[t->motion_slot].motion;
+    return RF_OK;
+}
+
+int rf_tracker_set_follow(rf_tracker t, const rf_follow_config *cfg) {
+    static const char *who = "rf_tracker_set_follow";
+    if (!t) return RF_ERR_INVALID_ARG;
+    rf_handle h = t->h;
+    if (!cfg) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL config", who));
+    if (t->best) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a best-shot tracker cannot follow", who));
+    if (t->lookback) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a look-back tracker cannot follow", who));
+    if (t->follow) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: following is already on", who));
+    if (t->updated) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker has already been updated", who));
+    const int R = cfg->search ? cfg->search : 8;
+    const float mad = cfg->max_mad != 0.f ? cfg->max_mad : 24.f;
+    if (R < 1 || R > FOLLOW_MAX_R) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: search %d, must be 0 or in [1, %d]", who, cfg->search, FOLLOW_MAX_R));
+    if (!(std::isfinite(mad) && mad > 0.f && mad <= 255.f))
+        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: max_mad %g, must be 0 or finite in (0, 255]", who, (double)cfg->max_mad));
+    const size_t V = t->cfg.max_videos, T = t->cfg.max_tracks, B = h->cfg.max_batch;
+    if (V * T * FOLLOW_BYTES > ((size_t)4 << 30))
+        return fail(h, RF_ERR_CAPACITY, fmt("%s: a store of %zu videos x %zu tracks x %d bytes exceeds 4 GiB", who, V, T, FOLLOW_BYTES));
+    try {
+        CK(cudaSetDevice(h->device));
+        CK(cudaMalloc(&t->d_fstore, V * T * FOLLOW_BYTES));
+        CK(cudaMalloc(&t->d_fentries, sizeof(FollowEntry) * V * T));
+        CK(cudaMalloc(&t->d_fmeas, sizeof(FollowMeas) * B * T));
+        CK(cudaMalloc(&t->d_follow, sizeof(rf_follow) * t->slots.size() * B * T));
+        CK(cudaMalloc(&t->d_fregions, sizeof(rf_det) * t->slots.size() * B * T));
+        CK(cudaMalloc(&t->d_fregion_counts, sizeof(int) * t->slots.size() * B));
+        CK(cudaMalloc(&t->d_fmask, sizeof(rf_det) * B * T));
+        CK(cudaMalloc(&t->d_fmask_counts, sizeof(int) * B));
+        CK(cudaMemset(t->d_fentries, 0, sizeof(FollowEntry) * V * T));
+        CK(cudaDeviceSynchronize());
+    } catch (const CudaFail &f) {
+        cudaFree(t->d_fstore); cudaFree(t->d_fentries); cudaFree(t->d_fmeas); cudaFree(t->d_follow);
+        cudaFree(t->d_fregions); cudaFree(t->d_fregion_counts); cudaFree(t->d_fmask); cudaFree(t->d_fmask_counts);
+        t->d_fstore = nullptr;
+        t->d_fentries = nullptr;
+        t->d_fmeas = nullptr;
+        t->d_follow = nullptr;
+        t->d_fregions = t->d_fmask = nullptr;
+        t->d_fregion_counts = t->d_fmask_counts = nullptr;
+        return fail_cuda(h, f);
+    }
+    t->follow = true;
+    t->fcfg = rf_follow_config{R, mad};
+    return RF_OK;
+}
+
+// Everything a follow call refuses, checked before anything is launched.
+static int check_follow(rf_tracker t, const char *who, const rf_yuv_frame *frames, const int *videos, int n) {
+    if (!t->follow) return fail(t->h, RF_ERR_INVALID_ARG, fmt("%s: not a follow tracker (rf_tracker_set_follow)", who));
+    int rc = check_track_args(t, who, videos, n, nullptr);
+    if (rc) return rc;
+    return check_frames(t->h, who, frames, n, RF_YUV_BT601);
+}
+
+// Issues the follow step of n frames on s into the next ring slot, ordered by the chain.  In rounds -- the r-th frame of every video
+// of the call, then the next -- so that each frame is searched from the state its video's previous frame left; with motion, each
+// round first masks the tracks' faces and estimates its frames' motion (the reference: the video's previous frame of the call, else
+// its stored thumbnail), and each video's last thumbnail of the call becomes its reference afterwards.  Returns the ring slot.
+static unsigned follow_issue(rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, cudaStream_t s) {
+    rf_handle h = t->h;
+    const unsigned ring = t->next_slot++ % t->slots.size();
+    rf_tracker_s::Slot &slot = t->slots[ring];
+    const size_t T = t->cfg.max_tracks, B = h->cfg.max_batch;
+    CK(cudaStreamWaitEvent(s, slot.free, 0));
+    CK(cudaStreamWaitEvent(s, t->chain, 0));
+    t->updated = true;
+    FollowArgs f = follow_args(t);
+    f.follow = t->d_follow + ring * B * T;
+    f.tracks = slot.tracks;
+    f.track_counts = slot.counts;
+    f.regions = t->d_fregions + ring * B * T;
+    f.region_counts = t->d_fregion_counts + ring * B;
+    std::vector<int> round(n);
+    int rounds = 0;
+    for (int i = 0; i < n; i++) {
+        int r = 0;
+        for (int k = 0; k < i; k++) r += videos[k] == videos[i];
+        round[i] = r;
+        rounds = std::max(rounds, r + 1);
+    }
+    // f13: one single-frame table per frame, so that a frame's thumbnail, blocks and motion sit at its index in the call
+    std::vector<MotionTable> mt(t->motion ? n : 0);
+    MotionCommits commits;
+    MotionArgs ma{};
+    if (t->motion) {
+        const int R = t->mcfg.search;
+        std::vector<int> last(t->cfg.max_videos, -1);
+        for (int i = 0; i < n; i++) {
+            const rf_yuv_frame &fr = frames[i];
+            const int v = videos[i];
+            MotionTable &tb = mt[i];
+            tb.i0 = i;
+            tb.n = 1;
+            MotionFrame &mf = tb.f[0];
+            mf.y = fr.y;
+            mf.pitch = fr.y_pitch;
+            mf.video = v;
+            mf.scale = 1.f;
+            mf.D = (std::max(fr.width, fr.height) + MOTION_THUMB - 1) / MOTION_THUMB;
+            mf.tw = fr.width / mf.D;
+            mf.th = fr.height / mf.D;
+            mf.nbx = mf.tw - 2 * R >= MOTION_BLOCK ? (mf.tw - 2 * R) / MOTION_BLOCK : 0;
+            mf.nby = mf.th - 2 * R >= MOTION_BLOCK ? (mf.th - 2 * R) / MOTION_BLOCK : 0;
+            const std::array<int, 2> size = {fr.width, fr.height};
+            if (last[v] >= 0) {
+                const rf_yuv_frame &p = frames[last[v]];
+                mf.ref = p.width == fr.width && p.height == fr.height ? last[v] : MOTION_REF_FIRST;
+            } else {
+                mf.ref = t->mref[v] == size ? MOTION_REF_STORE : MOTION_REF_FIRST;
+            }
+            last[v] = i;
+        }
+        for (int v = 0; v < t->cfg.max_videos; v++) {
+            if (last[v] < 0) continue;
+            t->mref[v] = {frames[last[v]].width, frames[last[v]].height};
+            commits.frames.push_back(last[v]);
+            commits.videos.push_back(v);
+            commits.bytes.push_back(mt[last[v]].f[0].tw * mt[last[v]].f[0].th);
+        }
+        ma.thumbs = t->d_mthumbs;
+        ma.store = t->d_mstore;
+        ma.blocks = t->d_mblocks;
+        ma.out = slot.motion;
+        ma.dets = t->d_fmask;
+        ma.counts = t->d_fmask_counts;
+        ma.max_faces = (int)T;
+        ma.search = R;
+        ma.min_inliers = t->mcfg.min_inliers;
+        f.motion = slot.motion;
+        f.mask = t->d_fmask;
+        f.mask_counts = t->d_fmask_counts;
+        t->motion_slot = (int)ring;
+    }
+    for (int r = 0; r < rounds; r++) {
+        FollowTable tab{};
+        std::vector<MotionTable> rt;
+        auto flush = [&]() {
+            if (!tab.n) return;
+            if (t->motion) {
+                CK(launch_follow_mask(f, tab, s));
+                CK(launch_motion_estimate(ma, rt.data(), (int)rt.size(), s));
+            }
+            CK(launch_follow_round(f, tab, s));
+            tab.n = 0;
+            rt.clear();
+        };
+        for (int i = 0; i < n; i++) {
+            if (round[i] != r) continue;
+            tab.f[tab.n++] = follow_frame(frames[i], videos[i], i);
+            if (t->motion) rt.push_back(mt[i]);
+            if (tab.n == TRACK_MAX_FRAMES) flush();
+        }
+        flush();
+    }
+    if (t->motion) motion_commit(t, commits, s);
+    CK(cudaEventRecord(t->chain, s));
+    t->follow_slot = (int)ring;
+    return ring;
+}
+
+int rf_track_follow_device(rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, const rf_track **dev_tracks,
+                           const int32_t **dev_track_counts) {
+    static const char *who = "rf_track_follow_device";
+    if (!t) return RF_ERR_INVALID_ARG;
+    rf_handle h = t->h;
+    int rc = check_follow(t, who, frames, videos, n);
+    if (rc) return rc;
+    if (n == 0) return RF_OK;
+    try {
+        CK(cudaSetDevice(h->device));
+        cudaStream_t s = (cudaStream_t)rf_last_stream(h);
+        const unsigned ring = follow_issue(t, frames, videos, n, s);
+        rf_tracker_s::Slot &slot = t->slots[ring];
+        CK(cudaEventRecord(slot.free, s));
+        if (dev_tracks) *dev_tracks = slot.tracks;
+        if (dev_track_counts) *dev_track_counts = slot.counts;
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
+}
+
+int rf_tracker_follow(rf_tracker t, const rf_follow **dev_follow) {
+    if (!t) return RF_ERR_INVALID_ARG;
+    if (!dev_follow) return fail(t->h, RF_ERR_INVALID_ARG, "rf_tracker_follow: dev_follow is NULL");
+    if (!t->follow) return fail(t->h, RF_ERR_INVALID_ARG, "rf_tracker_follow: not a follow tracker (rf_tracker_set_follow)");
+    const size_t T = t->cfg.max_tracks, B = t->h->cfg.max_batch;
+    *dev_follow = t->follow_slot < 0 ? nullptr : t->d_follow + (size_t)t->follow_slot * B * T;
     return RF_OK;
 }
 
@@ -2714,6 +2950,33 @@ int rf_detect_yuv_redact_device_style(rf_handle h, rf_tracker t, const rf_yuv_fr
                                   dev_tracks, dev_track_counts, dev_dets, dev_counts, out_scales);
 }
 
+int rf_track_follow_redact_device(rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, const rf_redact_style *style,
+                                  const rf_track **dev_tracks, const int32_t **dev_track_counts) {
+    static const char *who = "rf_track_follow_redact_device";
+    if (!t) return RF_ERR_INVALID_ARG;
+    rf_handle h = t->h;
+    int rc = check_follow(t, who, frames, videos, n);
+    if (rc) return rc;
+    RedactSpec spec;
+    if ((rc = redact_style(h, who, style, spec))) return rc;
+    if ((rc = check_disjoint(h, who, yuv_ranges(frames, n)))) return rc;
+    if (n == 0) return RF_OK;
+    try {
+        CK(cudaSetDevice(h->device));
+        Ctx &c = last_ctx(h);
+        const unsigned ring = follow_issue(t, frames, videos, n, c.stream);
+        rf_tracker_s::Slot &slot = t->slots[ring];
+        const size_t T = t->cfg.max_tracks, B = h->cfg.max_batch;
+        // (a) the OK-followed faces in id order, (b) the LOST tracks of the lists: f12's geometry, f14's styles and ownership
+        redact_issue(h, c, yuv_redact_table(frames, n, nullptr), t->d_fregions + ring * B * T, t->d_fregion_counts + ring * B, t, slot.tracks,
+                     slot.counts, spec, (int)T);
+        CK(cudaEventRecord(slot.free, c.stream));
+        if (dev_tracks) *dev_tracks = slot.tracks;
+        if (dev_track_counts) *dev_track_counts = slot.counts;
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
+}
+
 // ---- f15 look-back redaction (lookback.cuh) --------------------------------------------------------------------------------------
 int rf_tracker_set_lookback(rf_tracker t, const rf_lookback_config *cfg) {
     static const char *who = "rf_tracker_set_lookback";
@@ -2722,6 +2985,7 @@ int rf_tracker_set_lookback(rf_tracker t, const rf_lookback_config *cfg) {
     if (!cfg) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL config", who));
     if (t->best) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a best-shot tracker cannot look back", who));
     if (t->lookback) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: look-back is already on", who));
+    if (t->follow) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a follow tracker cannot look back", who));
     if (t->updated) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker has already been updated", who));
     const int L = cfg->frames ? cfg->frames : 15;
     const float grow = cfg->grow != 0.f ? cfg->grow : 0.1f;

@@ -119,8 +119,34 @@ class RetinaFace:
         faces, _, _ = self.engine.detect_views_oriented(img, [(1.0, o) for o in ANY_ORIENTATION], threshold, self.nms_threshold)
         return [FaceDetectInfo.from_row(r) for r in faces]
 
+    def _interval_calls(self, videos: Sequence[int], detect_every: int):
+        """f16: frame i of video v is a detect frame when v's frame number (counted over every call since the tracker's creation or
+        the video's reset) is divisible by detect_every.  Returns [(detect?, frame indices)] in issue order: each video's frames split
+        into runs of one kind, the p-th runs of every video after the (p - 1)-th, detect before follow -- so each video's frames keep
+        their order and a call of one kind stays one call."""
+        nums = self.__dict__.setdefault("_frame_no", {})
+        runs, seg = {}, {}
+        for i, v in enumerate(videos):
+            v = int(v)
+            det = nums.get(v, 0) % detect_every == 0
+            nums[v] = nums.get(v, 0) + 1
+            p, last = seg.get(v, (-1, None))
+            if det != last:
+                p += 1
+            seg[v] = (p, det)
+            runs.setdefault((p, not det), []).append(i)
+        return [(not follow, idx) for (_, follow), idx in sorted(runs.items())]
+
+    def _interval_tracker(self, detect_every: int, best=None, lookback=0):
+        if int(detect_every) < 1:
+            raise ValueError(f"detect_every {detect_every}, must be >= 1")
+        if detect_every > 1 and (best is not None or lookback):
+            raise ValueError("detect_every > 1 does not combine with best shots or look-back yet")
+        if detect_every > 1 and getattr(self, "_tracker", None) is not None and not self._tracker.follow_on:
+            raise ValueError("detect_every > 1 needs a follow tracker: this detector's tracker was created without one")
+
     def trackFrames(self, frames: Sequence, videos: Sequence[int], threshold: float = 0.5, layout: str = "nv12", matrix: str = "bt601",
-                    align: dict = None, max_videos: int = 64, best: dict = None, motion=False):
+                    align: dict = None, max_videos: int = 64, best: dict = None, motion=False, detect_every: int = 1):
         """f10 tracking: device 4:2:0 frames (torch CUDA tensors in ``Engine.detect_yuv_device``'s forms), frame i of video
         ``videos[i]``, detected and associated with the tracks of earlier frames on the GPU (rf_detect_yuv_track_device).  Per frame, a
         list of ``(id, state, FaceDetectInfo)`` over every live track (``capi.TRACK_*`` states; the face is the last matched one, in
@@ -137,13 +163,31 @@ class RetinaFace:
         f13 camera motion: with ``motion`` (True, or ``capi.motion_config``'s keywords: search, min_inliers) the tracker estimates
         each frame's global motion from the previous frame of the same video and moves the tracks with it, so that a panning or
         shaking camera keeps the ids; ``Tracker.motion`` (``self._tracker``) reads the estimates.  The first call decides which kind
-        of tracker this detector keeps."""
+        of tracker this detector keeps.
+
+        f16 detection interval: with ``detect_every=k`` > 1 the tracker is a follow tracker; each video's frames whose number is
+        divisible by k are detected, the others followed by template search without the detector (rf_track_follow_device).  A call
+        mixing both kinds is split into detect and follow calls; each video's frames keep their order.  Follow frames have no crops."""
         import torch
         from .capi import crop_shape
         if best is not None and align is not None:
             raise ValueError("best shots and new-identity crops are exclusive: pass best or align, not both")
+        self._interval_tracker(detect_every, best=best)
         if getattr(self, "_tracker", None) is None:
-            self._tracker = self.engine.tracker(max_videos=max_videos, best=best, motion=motion)
+            self._tracker = self.engine.tracker(max_videos=max_videos, best=best, motion=motion, follow=detect_every > 1)
+        if self._tracker.follow_on:
+            tracks, new = [None] * len(frames), [[] for _ in frames]
+            for det, idx in self._interval_calls(videos, detect_every):
+                fr, vi = [frames[i] for i in idx], [videos[i] for i in idx]
+                if det:
+                    t, c = self._track_call(fr, vi, threshold, layout, matrix, align)
+                else:
+                    tp, tc = self._tracker.follow_device(fr, vi, layout=layout)
+                    t = self._lists(tp, tc, len(idx))
+                    c = [[] for _ in idx]
+                for j, i in enumerate(idx):
+                    tracks[i], new[i] = t[j], c[j]
+            return tracks, new
         n = len(frames)
         if best is not None:
             crops = self._best_crops(n)
@@ -153,6 +197,16 @@ class RetinaFace:
             tracks = [[(int(r["id"]), int(r["state"]), FaceDetectInfo.from_row(r["face"])) for r in per] for per in recs]
             shots = self._tracker.read_best(bp, bc, n)
             return tracks, [[(s, crops[i, k]) for k, s in enumerate(per)] for i, per in enumerate(shots)]
+        return self._track_call(frames, videos, threshold, layout, matrix, align)
+
+    def _lists(self, tp: int, tc: int, n: int):
+        recs = self._tracker.read(tp, tc, n)
+        return [[(int(r["id"]), int(r["state"]), FaceDetectInfo.from_row(r["face"])) for r in per] for per in recs]
+
+    def _track_call(self, frames, videos, threshold, layout, matrix, align):
+        import torch
+        from .capi import crop_shape
+        n = len(frames)
         crops = None
         if align is not None:
             kw = {"fmt": "bgr_u8", **align}
@@ -170,7 +224,7 @@ class RetinaFace:
 
     def redactFrames(self, frames: Sequence, videos: Sequence[int] = None, threshold: float = 0.5, blocks: int = 0, margin: float = 0.0,
                      layout: str = "nv12", matrix: str = "bt601", max_videos: int = 64, motion=False, style: str = "mosaic",
-                     shape: str = "rect", detail: int = 0, lookback: int = 0, out: Sequence = None):
+                     shape: str = "rect", detail: int = 0, lookback: int = 0, out: Sequence = None, detect_every: int = 1):
         """f12 redaction: detect on device 4:2:0 frames (torch CUDA tensors in ``Engine.detect_yuv_device``'s forms) and mosaic every
         detected face IN PLACE (rf_detect_yuv_redact_device), ``blocks`` cells across a region's longer side (0: 8; 1: a flat patch),
         each side grown by ``margin`` of the box (0: 0.25).  With ``videos`` (frame i of video ``videos[i]``) the frames are also
@@ -181,18 +235,32 @@ class RetinaFace:
         radius; ``blocks`` must then stay 0), and ``shape="ellipse"`` redacts the ellipse inscribed in each region.
         f15: ``lookback=L`` (with ``videos``) makes the tracker a look-back tracker: each frame is kept on the GPU and frame num - L of
         its video, also covered where the faces first detected in the next L frames already were, is written into ``out[i]`` (None:
-        the input frame itself, in place).  Returns the emitted frame numbers (-1: nothing emitted yet); ``drainVideo`` emits the rest."""
+        the input frame itself, in place).  Returns the emitted frame numbers (-1: nothing emitted yet); ``drainVideo`` emits the rest.
+        f16: ``detect_every=k`` (with ``videos``) detects each video's frames whose number is divisible by k and follows the faces on
+        the others (rf_track_follow_redact_device), redacting every followed face and every LOST track, as ``trackFrames`` splits."""
         kw = dict(layout=layout, matrix=matrix, blocks=blocks, margin=margin, style=style, shape=shape, detail=detail)
+        self._interval_tracker(detect_every, lookback=lookback)
         if videos is None:
             if lookback:
                 raise ValueError("lookback needs videos: the buffered frames belong to a video")
+            if detect_every > 1:
+                raise ValueError("detect_every needs videos: the frame numbers belong to a video")
             self.engine.detect_yuv_redact_device(list(frames), threshold, self.nms_threshold, **kw)
             return
         if getattr(self, "_tracker", None) is None:
-            self._tracker = self.engine.tracker(max_videos=max_videos, motion=motion, lookback=lookback or None)
+            self._tracker = self.engine.tracker(max_videos=max_videos, motion=motion, lookback=lookback or None, follow=detect_every > 1)
         if lookback:
             return self._tracker.detect_yuv_redact_lookback_device(list(frames), list(videos), list(frames if out is None else out), threshold,
                                                                    self.nms_threshold, **kw)[0]
+        if self._tracker.follow_on:
+            fkw = {k: v for k, v in kw.items() if k != "matrix"}
+            for det, idx in self._interval_calls(videos, detect_every):
+                fr, vi = [frames[i] for i in idx], [videos[i] for i in idx]
+                if det:
+                    self._tracker.detect_yuv_redact_device(fr, vi, threshold, self.nms_threshold, **kw)
+                else:
+                    self._tracker.follow_redact_device(fr, vi, **fkw)
+            return
         self._tracker.detect_yuv_redact_device(list(frames), list(videos), threshold, self.nms_threshold, **kw)
 
     def drainVideo(self, video: int, out: Sequence, layout: str = "nv12", blocks: int = 0, margin: float = 0.0, style: str = "mosaic",
@@ -226,6 +294,9 @@ class RetinaFace:
         """Restart one video's tracks (ids from 1), or every video's with -1."""
         if getattr(self, "_tracker", None) is not None:
             self._tracker.reset(video)
+        nums = getattr(self, "_frame_no", {})
+        for v in (list(nums) if video < 0 else [video]):
+            nums.pop(v, None)
 
     @staticmethod
     def draw(img: np.ndarray, faces: Sequence[FaceDetectInfo]) -> np.ndarray:

@@ -288,13 +288,27 @@ void RetinaFace::trackYUV(const vector<rf_yuv_frame> &device_frames, const vecto
     if (videos.size() != device_frames.size()) throw std::invalid_argument("trackYUV: one video index per frame");
     if (device_frames.size() > (size_t)opt_.max_batch) throw std::invalid_argument("trackYUV: at most max_batch frames per call");
     if (best_tracker_) throw std::logic_error("trackYUV: this RetinaFace tracks with best shots (trackYUVBest)");
-    if (!tracker_) {
-        rf_track_config tc{};
-        tc.max_videos = opt_.track_videos;
-        int rc = rf_tracker_create(h_, &tc, &tracker_);
-        if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_create: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
-        trackerCreated();
+    if (!tracker_) makeTracker(0);
+    if (opt_.detect_every > 1) {
+        for (const auto &call : intervalCalls(videos)) {
+            vector<rf_yuv_frame> fr;
+            vector<int> vi;
+            for (int i : call.second) { fr.push_back(device_frames[i]); vi.push_back(videos[i]); }
+            if (call.first) {
+                // new-identity crops only when the call is one detect call: the crops' rows are the call's frames
+                const bool whole = call.second.size() == device_frames.size();
+                trackDetect(fr, vi, threshold, whole ? align : nullptr, whole ? dev_crops : nullptr);
+            } else {
+                followCall(fr, vi, nullptr);
+            }
+        }
+        return;
     }
+    trackDetect(device_frames, videos, threshold, align, dev_crops);
+}
+
+void RetinaFace::trackDetect(const vector<rf_yuv_frame> &device_frames, const vector<int> &videos, float threshold, const AlignOptions *align,
+                             void *dev_crops) {
     int per = 0, cw = 0, ch = 0;
     const rf_align_params p = align ? crop_params(*align, opt_.max_faces, &per, &cw, &ch) : rf_align_params{};
     const int n = (int)device_frames.size();
@@ -307,7 +321,62 @@ void RetinaFace::trackYUV(const vector<rf_yuv_frame> &device_frames, const vecto
     noteMotion(n);
 }
 
+rf_tracker RetinaFace::makeTracker(int lookback) {
+    rf_track_config tc{};
+    tc.max_videos = opt_.track_videos;
+    int rc = rf_tracker_create(h_, &tc, &tracker_);
+    if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_create: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+    trackerCreated();
+    if (lookback) {
+        const rf_lookback_config lc{lookback, 0.f};
+        rc = rf_tracker_set_lookback(tracker_, &lc);
+        if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_set_lookback: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+    }
+    return tracker_;
+}
+
+vector<std::pair<bool, vector<int>>> RetinaFace::intervalCalls(const vector<int> &videos) {
+    std::map<std::pair<int, bool>, vector<int>> runs;     // (run p, follow?) -> frames: sorted, p first, then detect before follow
+    std::map<int, std::pair<int, int>> seg;                // video -> (run, kind of that run: 1 detect, 0 follow)
+    for (int i = 0; i < (int)videos.size(); i++) {
+        const int v = videos[i];
+        const bool det = frame_no_[v]++ % opt_.detect_every == 0;
+        auto it = seg.find(v);
+        int p = it == seg.end() ? 0 : it->second.first;
+        if (it != seg.end() && it->second.second != (int)det) p++;
+        seg[v] = {p, (int)det};
+        runs[{p, !det}].push_back(i);
+    }
+    vector<std::pair<bool, vector<int>>> out;
+    for (auto &r : runs) out.push_back({!r.first.second, r.second});
+    return out;
+}
+
+void RetinaFace::followCall(const vector<rf_yuv_frame> &frames, const vector<int> &videos, const rf_redact_style *style) {
+    const int n = (int)frames.size();
+    DeviceTracks t{};
+    int rc = style ? rf_track_follow_redact_device(tracker_, frames.data(), videos.data(), n, style, &t.tracks, &t.counts)
+                   : rf_track_follow_device(tracker_, frames.data(), videos.data(), n, &t.tracks, &t.counts);
+    if (rc != RF_OK)
+        throw std::runtime_error(string(style ? "rf_track_follow_redact_device: " : "rf_track_follow_device: ") + rf_status_string(rc) + ": " +
+                                 rf_last_error(h_));
+    tracks_ = t;
+    tracks_.n = n;
+    tracks_.max_tracks = 64;      // rf_track_config's default
+    follow_ = DeviceFollow{};
+    rc = rf_tracker_follow(tracker_, &follow_.follow);
+    if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_follow: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+    follow_.n = n;
+    follow_.max_tracks = 64;
+    noteMotion(n);
+}
+
 void RetinaFace::trackerCreated() {
+    if (opt_.detect_every > 1) {
+        const rf_follow_config fc{};
+        int rc = rf_tracker_set_follow(tracker_, &fc);
+        if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_set_follow: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+    }
     if (!opt_.track_motion) return;
     const rf_motion_config mc{};
     int rc = rf_tracker_set_motion(tracker_, &mc);
@@ -330,19 +399,30 @@ void RetinaFace::redactYUV(const vector<rf_yuv_frame> &device_frames, const vect
         throw std::invalid_argument("redactYUV: out_frames go with lookback, one per frame");
     if (device_frames.size() > (size_t)opt_.max_batch) throw std::invalid_argument("redactYUV: at most max_batch frames per call");
     if (videos && best_tracker_) throw std::logic_error("redactYUV: this RetinaFace tracks with best shots (trackYUVBest)");
-    if (videos && !tracker_) {
-        rf_track_config tc{};
-        tc.max_videos = opt_.track_videos;
-        int rc = rf_tracker_create(h_, &tc, &tracker_);
-        if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_create: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
-        trackerCreated();
-        if (opt.lookback) {
-            const rf_lookback_config lc{opt.lookback, 0.f};
-            rc = rf_tracker_set_lookback(tracker_, &lc);
-            if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_set_lookback: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
-        }
-    }
+    if (opt.lookback && opt_.detect_every > 1) throw std::invalid_argument("redactYUV: lookback does not combine with detect_every yet");
+    if (videos && !tracker_) makeTracker(opt.lookback);
     const rf_redact_style st{opt.style, opt.shape, opt.style == RF_REDACT_BLUR ? 0 : opt.blocks, opt.detail, opt.margin};
+    if (videos && opt_.detect_every > 1) {
+        for (const auto &call : intervalCalls(*videos)) {
+            vector<rf_yuv_frame> fr;
+            vector<int> vi;
+            for (int i : call.second) { fr.push_back(device_frames[i]); vi.push_back((*videos)[i]); }
+            if (call.first) {
+                DeviceTracks t{};
+                int rc = rf_detect_yuv_redact_device_style(h_, tracker_, fr.data(), vi.data(), (int)fr.size(), RF_YUV_BT601, threshold,
+                                                           nms_threshold, &st, &t.tracks, &t.counts, nullptr, nullptr, nullptr);
+                if (rc != RF_OK)
+                    throw std::runtime_error(string("rf_detect_yuv_redact_device_style: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+                tracks_ = t;
+                tracks_.n = (int)fr.size();
+                tracks_.max_tracks = 64;      // rf_track_config's default
+                noteMotion((int)fr.size());
+            } else {
+                followCall(fr, vi, &st);
+            }
+        }
+        return;
+    }
     const int n = (int)device_frames.size();
     DeviceTracks t{};
     if (opt.lookback) {
@@ -407,6 +487,8 @@ void RetinaFace::finishVideo(int video, void *dev_best_crops) {
 }
 
 void RetinaFace::resetTracks(int video) {
+    if (video < 0) frame_no_.clear();
+    else frame_no_.erase(video);
     if (!tracker_) return;
     int rc = rf_tracker_reset(tracker_, video);
     if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_reset: ") + rf_status_string(rc) + ": " + rf_last_error(h_));

@@ -13,7 +13,9 @@
 #ifndef RF_B200_HOST_RETINAFACE_H
 #define RF_B200_HOST_RETINAFACE_H
 
+#include <map>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "cv_compat.hpp"
@@ -40,6 +42,9 @@ struct RetinaFaceOptions {
                                          // folding; with net_w = net_h = 0 it also sets the network size.  Empty: built-in graph
     int track_videos = 16;               // sequences of the tracker trackYUV creates on its first call
     bool track_motion = false;           // f13: that tracker follows the camera's motion (rf_tracker_set_motion, default config)
+    int detect_every = 1;                // f16: > 1 makes that tracker a follow tracker (rf_tracker_set_follow, default config);
+                                         // trackYUV / redactYUV then detect a video's frames whose number is divisible by it and
+                                         // follow the faces on the others (rf_track_follow_device / rf_track_follow_redact_device)
     string cache_file;                   // folded-model cache (the reference's "retina.cache", trtnetbase.cpp:205-243, but with a
                                          // staleness check).  Empty: none
 };
@@ -145,6 +150,14 @@ class RetinaFace {
         int n = 0;
     };
     const DeviceMotion &lastMotion() const { return motion_; }
+    // f16 (options detect_every > 1): a call whose frames are of both kinds is issued as detect and follow calls, each video's frames
+    // in order (the p-th run of one kind of every video after the (p - 1)-th, detect first); lastTracks() and lastMotion() then hold
+    // the last of them.  lastFollow() holds the rf_follow records of the last follow call (nullptr before one).
+    struct DeviceFollow {
+        const rf_follow *follow = nullptr;  // device [n][max_tracks], each frame's in its list order
+        int n = 0, max_tracks = 0;
+    };
+    const DeviceFollow &lastFollow() const { return follow_; }
     void finishVideo(int video, void *dev_best_crops);
     // f12 / f14 redaction (rf_detect_yuv_redact_device_style): detect on DEVICE 4:2:0 frames and mosaic (or blur) every detected face in place, on the
     // GPU; asynchronous on rf_last_stream(handle()).  With `videos` (one per frame, in [0, track_videos)) the frames are also tracked on
@@ -169,12 +182,19 @@ class RetinaFace {
     void keepResults(size_t start, int n, const unsigned char *crops, int per, int cw, int ch);
     void trackerCreated();              // motion on a new tracker, as the options say
     void noteMotion(int n);             // lastMotion() after a tracked call of n frames
+    rf_tracker makeTracker(int lookback);   // trackYUV's / redactYUV's tracker, as the options say
+    // f16: the call's frames as (detect?, frame indices) sub-calls in issue order; advances each video's frame number
+    vector<std::pair<bool, vector<int>>> intervalCalls(const vector<int> &videos);
+    void followCall(const vector<rf_yuv_frame> &frames, const vector<int> &videos, const rf_redact_style *style);
+    void trackDetect(const vector<rf_yuv_frame> &frames, const vector<int> &videos, float threshold, const AlignOptions *align, void *dev_crops);
     rf_handle h_ = nullptr;
     rf_tracker tracker_ = nullptr;
     bool best_tracker_ = false;
     DeviceTracks tracks_;
     DeviceBestShots best_;
     DeviceMotion motion_;
+    DeviceFollow follow_;
+    std::map<int, long long> frame_no_;
     vector<int32_t> frame_numbers_;
     RetinaFaceOptions opt_;
     string network;

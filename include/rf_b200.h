@@ -929,6 +929,36 @@ int rf_track_follow_redact_device(rf_tracker t, const rf_yuv_frame *frames, cons
  * before the first); valid for `streams` further tracker calls.  RF_ERR_INVALID_ARG on a tracker that is not a follow tracker. */
 int rf_tracker_follow(rf_tracker t, const rf_follow **dev_follow);
 
+/* f17 searching look-back: f15's box only covers a face that moves less than grow x its size per frame back.  A SEARCHING look-back
+ * tracker follows each birth back through the buffered frames with f16's template search (below), so the look-back regions take the
+ * face's own path.  oracle/lookback_search.py restates the definition; every FP64 step is one rounding in the order written.
+ *   Chain      of a birth (f15's births; record box `face`) on frame b:
+ *                1. Template: f16's Cut of `face` on frame b's luma (the grid at c = 1, the Sampler, the FLAT test).
+ *                2. Steps k = 1, 2, ..., K = min(L, b) (frame numbers since create, reset or drain: a chain never crosses a restart)
+ *                   on frame e = b - k, from the box (x1, y1, x2, y2) of step k - 1 (`face` at k = 1), widened to double:
+ *                   w = x2 - x1, h = y2 - y1, cx = x1 + w / 2, cy = y1 + h / 2;
+ *                3. with motion, frame e + 1's rf_motion undone when RF_MOTION_OK, by f15's step-2 formulas;
+ *                4. f16's search of the state z = (cx, cy, w / h, h) (pcx = cx, pcy = cy, pw = (w / h) h, ph = h): the bound
+ *                   (MISMATCH, not searched), Windows, Match, Box and Status exactly as f16 states them, against the birth's template
+ *                   (it is never re-cut, so error cannot build up along the chain);
+ *                5. the chain stops at its first status other than RF_FOLLOW_OK (a FLAT template stops it at k = 1).
+ *   Regions    of an emitted frame e: f15's (a), (b) and (c) unchanged and in the same order, then
+ *                (d) for the births on frames e + 1 .. min(e + L, the video's last frame seen), frame by frame, id order within a
+ *                    frame: the box of the birth's step b - e, when its chain reached that step with status OK.
+ *              Geometry, shapes, styles and ownership are f12 / f14's.  Since (d) comes last, a searching tracker's out frame differs
+ *              from a plain look-back tracker's only on samples (d) alone covers: a false match can add coverage, never remove it.
+ * Memory: each log slot grows by min(max_faces, max_tracks) x L boxes and as many chain lengths; each ring slot by the step records
+ * below; each emitted frame's region records from F + T + L min(F, T) to F + T + 2 L min(F, T). */
+/* Makes a look-back tracker (with or without motion) a searching one, after rf_tracker_set_lookback and before the first update.
+ * cfg: f16's rf_follow_config and bounds (search R 0 -> 8, max_mad 0 -> 24).  Not a look-back tracker, a second call, a call after
+ * an update, or bad values: RF_ERR_INVALID_ARG, nothing changed.  A look-back tracker that never makes this call is unchanged. */
+int rf_tracker_set_lookback_search(rf_tracker t, const rf_follow_config *cfg);
+/* Of the tracker's latest rf_detect_yuv_redact_lookback_device call (NULL before the first): *dev_steps -> [n][min(max_faces,
+ * max_tracks)][L] rf_follow, row (i, r) the r-th birth of frame i, step k - 1 its step on frame num_i - k; *dev_lengths -> [n][min(F,
+ * T)] int32 the steps taken, the failing last one included (0 past the frame's births).  Valid for `streams` further tracker calls.
+ * RF_ERR_INVALID_ARG on a tracker that is not searching. */
+int rf_tracker_lookback_search(rf_tracker t, const rf_follow **dev_steps, const int32_t **dev_lengths);
+
 /* Introspection. */
 int rf_get_net_size(rf_handle h, int *net_w, int *net_h, int *max_batch, int *max_faces);
 int rf_num_anchors(rf_handle h);            /* per image: 8,232 @448x448, 47,040 @1280x896 */

@@ -31,6 +31,7 @@ SOURCES = [
     ("redact.cu", ["-fmad=false"]),     # the FP64 region geometry, as oracle/redact.py states it
     ("motion.cu", ["-fmad=false"]),     # the FP64 sub-pixel match and similarity fit, as oracle/motion.py states it
     ("lookback.cu", ["-fmad=false"]),   # the FP64 look-back box, as oracle/lookback.py states it
+    ("lookback_search.cu", ["-fmad=false"]),   # f16's search along a birth's chain, as oracle/lookback_search.py states it
     ("follow.cu", ["-fmad=false"]),     # the FP64 template grids, sub-pixel step and Kalman update, as oracle/follow.py states it
     ("calibrate.cu", []),
     ("model.cpp", []),

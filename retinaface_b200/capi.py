@@ -39,6 +39,7 @@ EXPORTS = [
     "rf_redact_yuv_device_style", "rf_redact_device_style", "rf_detect_yuv_redact_device_style",
     "rf_tracker_set_lookback", "rf_detect_yuv_redact_lookback_device", "rf_tracker_drain",
     "rf_tracker_set_follow", "rf_track_follow_device", "rf_tracker_follow", "rf_track_follow_redact_device",
+    "rf_tracker_set_lookback_search", "rf_tracker_lookback_search",
 ]
 COMM_BLOB_BYTES = 128
 
@@ -463,6 +464,8 @@ def load_library() -> C.CDLL:
     lib.rf_tracker_set_follow.argtypes = [C.c_void_p, C.POINTER(FollowConfig)]
     lib.rf_track_follow_device.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_void_p, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
     lib.rf_tracker_follow.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
+    lib.rf_tracker_set_lookback_search.argtypes = [C.c_void_p, C.POINTER(FollowConfig)]
+    lib.rf_tracker_lookback_search.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
     lib.rf_track_follow_redact_device.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_void_p, C.c_int, C.POINTER(RedactStyle),
                                                   C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
     _lib = lib
@@ -1124,14 +1127,15 @@ class Engine:
     # -- f10 face tracking across video frames ---------------------------------------------------------------------------------
     def tracker(self, max_videos: int = 1, max_tracks: int = 0, high_thresh: float = 0.0, new_thresh: float = 0.0, iou_high: float = 0.0,
                 iou_low: float = 0.0, iou_tentative: float = 0.0, max_lost: int = 0, best: Optional[dict] = None,
-                motion=None, lookback=None, follow=None) -> "Tracker":
+                motion=None, lookback=None, follow=None, lookback_search=None) -> "Tracker":
         """rf_tracker_create: a tracker of max_videos independent sequences on this engine (0 -> the defaults of rf_track_config).
         best (``best_config`` keywords): a best-shot tracker (rf_tracker_create_best), fed through ``Tracker.detect_yuv_best_device``.
         motion (True or ``motion_config`` keywords): camera-motion compensation (rf_tracker_set_motion) from the frames of the
         detect_yuv_* calls; read each call's estimates with ``Tracker.motion``.  lookback (True, L, or ``set_lookback`` keywords): a
         look-back tracker (rf_tracker_set_lookback), fed through ``Tracker.detect_yuv_redact_lookback_device``.  follow (True or
         ``set_follow`` keywords): a follow tracker (rf_tracker_set_follow), whose frames between detections go through
-        ``Tracker.follow_device``."""
+        ``Tracker.follow_device``.  lookback_search (True or ``set_lookback_search`` keywords, with lookback): a searching look-back
+        tracker (rf_tracker_set_lookback_search)."""
         t = Tracker(self, TrackConfig(max_videos, max_tracks, high_thresh, new_thresh, iou_high, iou_low, iou_tentative, max_lost),
                     best_config(**best) if best is not None else None)
         try:
@@ -1141,6 +1145,8 @@ class Engine:
                 t.set_lookback(**(lookback if isinstance(lookback, dict) else {} if lookback is True else {"frames": int(lookback)}))
             if follow:
                 t.set_follow(**(follow if isinstance(follow, dict) else {}))
+            if lookback_search:
+                t.set_lookback_search(**(lookback_search if isinstance(lookback_search, dict) else {}))
         except Exception:
             t.close()
             raise
@@ -1257,6 +1263,7 @@ class Tracker:
         self.motion_on = False
         self.lookback = 0            # L of a look-back tracker
         self.follow_on = False
+        self.lookback_search_on = False
         self.max_videos = cfg.max_videos
         self.max_tracks = cfg.max_tracks or 64
 
@@ -1390,6 +1397,27 @@ class Tracker:
                                                                          nms_thr, C.byref(st), outs, nums.ctypes.data, C.byref(tp), C.byref(tc),
                                                                          C.byref(d), C.byref(c), scales.ctypes.data))
         return nums[:n].copy(), int(tp.value or 0), int(tc.value or 0), int(d.value or 0), int(c.value or 0), scales[:n].copy()
+
+    def set_lookback_search(self, search: int = 0, max_mad: float = 0.0):
+        """rf_tracker_set_lookback_search, after ``set_lookback`` and before the first update: follow every new face back through the
+        buffered frames by f16's template search and cover its path too (search: R in template pixels, 0 -> 8; max_mad: 0 -> 24)."""
+        cfg = FollowConfig(int(search), float(max_mad))
+        self.engine._check(self.lib.rf_tracker_set_lookback_search(self.t, C.byref(cfg)))
+        self.lookback_search_on = True
+
+    def lookback_search(self, n: int):
+        """rf_tracker_lookback_search: the latest look-back call's [n][min(max_faces, max_tracks)][L] step records (FOLLOW_DTYPE) and
+        [n][min(max_faces, max_tracks)] chain lengths, copied after the last stream."""
+        import torch
+        p, q = C.c_void_p(), C.c_void_p()
+        self.engine._check(self.lib.rf_tracker_lookback_search(self.t, C.byref(p), C.byref(q)))
+        if not p.value:
+            raise RuntimeError("no look-back call has been made on this tracker")
+        self.engine._check(self.lib.rf_synchronize(self.engine.h))
+        bcap = min(self.engine.max_faces, self.max_tracks)
+        raw = torch.as_tensor(_DevArray(int(p.value), (n * bcap * self.lookback * FOLLOW_DTYPE.itemsize,), "|u1"), device="cuda").cpu().numpy()
+        lens = torch.as_tensor(_DevArray(int(q.value), (n * bcap * 4,), "|u1"), device="cuda").cpu().numpy()
+        return raw.view(FOLLOW_DTYPE).reshape(n, bcap, self.lookback).copy(), lens.view(np.int32).reshape(n, bcap).copy()
 
     def drain(self, video: int, out_frames, layout: str = "nv12", blocks: int = 0, margin: float = 0.0, style: str = "mosaic",
               shape: str = "rect", detail: int = 0) -> np.ndarray:

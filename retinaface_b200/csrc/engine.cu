@@ -1859,6 +1859,8 @@ struct rf_tracker_s {
         rf_motion *motion = nullptr;   // [max_batch] f13, with motion on
         rf_det *lb_boxes = nullptr;    // [max(max_batch, L)][lookback_records] f15, the regions of the emitted frames
         int *lb_counts = nullptr;      // [max(max_batch, L)]
+        rf_follow *lb_steps = nullptr; // [max_batch][min(max_faces, max_tracks)][L] f17, the step records of a look-back call
+        int *lb_lengths = nullptr;     // [max_batch][min(max_faces, max_tracks)]
         cudaEvent_t free = nullptr;
     };
     std::vector<Slot> slots;
@@ -1895,6 +1897,10 @@ struct rf_tracker_s {
         long long frames = 0;          // frames since create, reset or drain
     };
     std::vector<LookbackVideo> lbv;
+    // f17 searching look-back: the step records live in the ring, the chains in the log slots.
+    bool lb_search = false;
+    rf_follow_config lscfg{};
+    int lb_search_slot = -1;           // the ring slot of the latest look-back call
     // f16 following (follow.cuh); `follow` false: none of these allocated.  The chain orders the per-call measurements as it orders
     // f11's tables; the follow records live in the ring.
     bool follow = false;
@@ -1915,7 +1921,7 @@ static void tracker_release(rf_tracker t) {
     for (auto &s : t->slots) {
         if (s.free) { cudaEventSynchronize(s.free); cudaEventDestroy(s.free); }
         cudaFree(s.tracks); cudaFree(s.counts); cudaFree(s.due); cudaFree(s.due_counts); cudaFree(s.motion);
-        cudaFree(s.lb_boxes); cudaFree(s.lb_counts);
+        cudaFree(s.lb_boxes); cudaFree(s.lb_counts); cudaFree(s.lb_steps); cudaFree(s.lb_lengths);
     }
     for (auto &v : t->lbv) cudaFree(v.d);
     cudaFree(t->d_mstore); cudaFree(t->d_mthumbs); cudaFree(t->d_mblocks);
@@ -2992,7 +2998,7 @@ int rf_tracker_set_lookback(rf_tracker t, const rf_lookback_config *cfg) {
     if (L < 1 || L > LOOKBACK_MAX_L) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frames %d, must be 0 or in [1, %d]", who, cfg->frames, LOOKBACK_MAX_L));
     if (!(std::isfinite(grow) && grow > 0.f && grow <= 1.f))
         return fail(h, RF_ERR_INVALID_ARG, fmt("%s: grow %g, must be 0 or finite in (0, 1]", who, (double)cfg->grow));
-    const size_t rows = std::max(h->cfg.max_batch, L), recs = lookback_records(h->cfg.max_faces, t->cfg.max_tracks, L);
+    const size_t rows = std::max(h->cfg.max_batch, L), recs = lookback_records(h->cfg.max_faces, t->cfg.max_tracks, L, false);
     try {
         CK(cudaSetDevice(h->device));
         for (auto &s : t->slots) {
@@ -3011,6 +3017,54 @@ int rf_tracker_set_lookback(rf_tracker t, const rf_lookback_config *cfg) {
     t->lb_frames = L;
     t->lb_grow = grow;
     t->lbv.assign(t->cfg.max_videos, {});
+    return RF_OK;
+}
+
+int rf_tracker_set_lookback_search(rf_tracker t, const rf_follow_config *cfg) {
+    static const char *who = "rf_tracker_set_lookback_search";
+    if (!t) return RF_ERR_INVALID_ARG;
+    rf_handle h = t->h;
+    if (!cfg) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL config", who));
+    if (!t->lookback) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: not a look-back tracker (rf_tracker_set_lookback)", who));
+    if (t->lb_search) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the look-back search is already on", who));
+    if (t->updated) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker has already been updated", who));
+    const int R = cfg->search ? cfg->search : 8;
+    const float mad = cfg->max_mad != 0.f ? cfg->max_mad : 24.f;
+    if (R < 1 || R > FOLLOW_MAX_R) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: search %d, must be 0 or in [1, %d]", who, cfg->search, FOLLOW_MAX_R));
+    if (!(std::isfinite(mad) && mad > 0.f && mad <= 255.f))
+        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: max_mad %g, must be 0 or finite in (0, 255]", who, (double)cfg->max_mad));
+    const int L = t->lb_frames;
+    const size_t B = h->cfg.max_batch, bcap = std::min(h->cfg.max_faces, t->cfg.max_tracks);
+    const size_t rows = std::max(h->cfg.max_batch, L), recs = lookback_records(h->cfg.max_faces, t->cfg.max_tracks, L, true);
+    std::vector<rf_tracker_s::Slot> grown(t->slots.size());
+    try {
+        CK(cudaSetDevice(h->device));
+        for (auto &s : grown) {
+            CK(cudaMalloc(&s.lb_boxes, sizeof(rf_det) * rows * recs));
+            CK(cudaMalloc(&s.lb_steps, sizeof(rf_follow) * B * bcap * L));
+            CK(cudaMalloc(&s.lb_lengths, sizeof(int) * B * bcap));
+        }
+    } catch (const CudaFail &f) {
+        for (auto &s : grown) { cudaFree(s.lb_boxes); cudaFree(s.lb_steps); cudaFree(s.lb_lengths); }
+        return fail_cuda(h, f);
+    }
+    for (size_t i = 0; i < t->slots.size(); i++) {     // no call has used the ring's region records yet
+        cudaFree(t->slots[i].lb_boxes);
+        t->slots[i].lb_boxes = grown[i].lb_boxes;
+        t->slots[i].lb_steps = grown[i].lb_steps;
+        t->slots[i].lb_lengths = grown[i].lb_lengths;
+    }
+    t->lb_search = true;
+    t->lscfg = rf_follow_config{R, mad};
+    return RF_OK;
+}
+
+int rf_tracker_lookback_search(rf_tracker t, const rf_follow **dev_steps, const int32_t **dev_lengths) {
+    if (!t) return RF_ERR_INVALID_ARG;
+    if (!t->lb_search) return fail(t->h, RF_ERR_INVALID_ARG, "rf_tracker_lookback_search: not a searching look-back tracker (rf_tracker_set_lookback_search)");
+    const bool any = t->lb_search_slot >= 0;
+    if (dev_steps) *dev_steps = any ? t->slots[t->lb_search_slot].lb_steps : nullptr;
+    if (dev_lengths) *dev_lengths = any ? t->slots[t->lb_search_slot].lb_lengths : nullptr;
     return RF_OK;
 }
 
@@ -3035,6 +3089,8 @@ static bool same_frame(const rf_yuv_frame &a, const rf_yuv_frame &b) {
 }
 
 static uint8_t *lb_log(rf_tracker t, const rf_tracker_s::LookbackVideo &v) { return v.d + (size_t)t->lb_frames * v.frame_bytes; }
+static size_t lb_slot_bytes(rf_tracker t) { return lookback_slot_bytes(t->h->cfg.max_faces, t->cfg.max_tracks, t->lb_search ? t->lb_frames : 0); }
+static int lb_records(rf_tracker t) { return lookback_records(t->h->cfg.max_faces, t->cfg.max_tracks, t->lb_frames, t->lb_search); }
 
 // The swap entry of one frame: its planes (in: NULL for a drain; out: NULL when it emits nothing) and its buffer slot.
 static LookbackSwapFrame lb_swap_frame(const rf_yuv_frame *in, const rf_yuv_frame *out, uint8_t *slot) {
@@ -3078,12 +3134,14 @@ static void lb_boxes(rf_tracker t, rf_tracker_s::Slot &slot, const std::vector<s
     LookbackArgs a{};
     a.max_faces = t->h->cfg.max_faces;
     a.max_tracks = t->cfg.max_tracks;
-    a.slot_bytes = lookback_slot_bytes(a.max_faces, a.max_tracks);
+    a.slot_bytes = lb_slot_bytes(t);
     a.ring = 2 * t->lb_frames;
     a.grow = (double)t->lb_grow;
     a.out = slot.lb_boxes;
     a.out_counts = slot.lb_counts;
-    a.records = lookback_records(a.max_faces, a.max_tracks, t->lb_frames);
+    a.records = lb_records(t);
+    a.search = t->lb_search ? t->lscfg.search : 0;
+    a.L = t->lb_frames;
     for (size_t j0 = 0; j0 < em.size(); j0 += LOOKBACK_TABLE) {
         LookbackBoxTable tb{};
         tb.j0 = (int)j0;
@@ -3096,10 +3154,46 @@ static void lb_boxes(rf_tracker t, rf_tracker_s::Slot &slot, const std::vector<s
     }
 }
 
+// f17: the chains of the call's births (k_lookback_search), after the log and before the swap.  Tables take whole videos: each video's
+// frames of the call, in number order, so that a step on an earlier frame of the call finds it in the same table.
+static void lb_search(rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, const std::vector<long long> &num, const LookbackArgs &a,
+                      cudaStream_t s) {
+    std::vector<std::vector<int>> by;            // the call's frames of each video, in first-appearance order
+    std::vector<int> vid;
+    for (int i = 0; i < n; i++) {
+        auto it = std::find(vid.begin(), vid.end(), videos[i]);
+        if (it == vid.end()) {
+            vid.push_back(videos[i]);
+            by.emplace_back();
+            it = vid.end() - 1;
+        }
+        by[it - vid.begin()].push_back(i);
+    }
+    LookbackSearchTable tb{};
+    for (size_t q = 0; q <= by.size(); q++) {
+        if (tb.n > 0 && (q == by.size() || tb.n + (int)by[q].size() > LOOKBACK_SEARCH_FRAMES || tb.nv == LOOKBACK_SEARCH_VIDEOS)) {
+            CK(launch_lookback_search(a, tb, s));
+            tb = LookbackSearchTable{};
+        }
+        if (q == by.size()) break;
+        const rf_tracker_s::LookbackVideo &lv = t->lbv[vid[q]];
+        LookbackSearchVideo &v = tb.v[tb.nv];
+        v.buf = lv.d;
+        v.log = lb_log(t, lv);
+        v.frame_bytes = lv.frame_bytes;
+        v.num0 = num[by[q][0]];
+        v.w = lv.w;
+        v.h = lv.h;
+        v.first = tb.n;
+        for (int i : by[q]) tb.f[tb.n++] = LookbackSearchFrame{frames[i].y, frames[i].y_pitch, tb.nv, i};
+        tb.nv++;
+    }
+}
+
 // Allocates (or, at a new frame size, replaces) the buffer of a video that has no buffered frames.  false: the allocation failed.
 static bool lb_alloc(rf_tracker t, rf_tracker_s::LookbackVideo &v, const rf_yuv_frame &f) {
     const size_t fb = ((size_t)f.width * f.height * 3 / 2 + 255) & ~(size_t)255;
-    const size_t bytes = (size_t)t->lb_frames * fb + 2 * (size_t)t->lb_frames * lookback_slot_bytes(t->h->cfg.max_faces, t->cfg.max_tracks);
+    const size_t bytes = (size_t)t->lb_frames * fb + 2 * (size_t)t->lb_frames * lb_slot_bytes(t);
     if (v.d && v.frame_bytes == fb) return true;
     if (v.d) {
         CK(cudaEventSynchronize(t->chain));      // the last drain's swap may still read it
@@ -3193,8 +3287,9 @@ int rf_detect_yuv_redact_lookback_device(rf_handle h, rf_tracker t, const rf_yuv
         a.motion = t->motion ? slot.motion : nullptr;
         a.max_faces = h->cfg.max_faces;
         a.max_tracks = t->cfg.max_tracks;
-        a.slot_bytes = lookback_slot_bytes(a.max_faces, a.max_tracks);
+        a.slot_bytes = lb_slot_bytes(t);
         a.ring = 2 * L;
+        a.L = L;
         for (int i0 = 0; i0 < n; i0 += LOOKBACK_TABLE) {
             LookbackLogTable lt{};
             lt.i0 = i0;
@@ -3203,6 +3298,14 @@ int rf_detect_yuv_redact_lookback_device(rf_handle h, rf_tracker t, const rf_yuv
                 lt.slot[lt.n] = lb_log(t, t->lbv[videos[i]]) + (size_t)(num[i] % a.ring) * a.slot_bytes;
             }
             CK(launch_lookback_log(a, lt, c.stream));
+        }
+        if (t->lb_search) {
+            a.search = t->lscfg.search;
+            a.max_mad = t->lscfg.max_mad;
+            a.steps = slot.lb_steps;
+            a.lengths = slot.lb_lengths;
+            lb_search(t, frames, videos, n, num, a, c.stream);
+            t->lb_search_slot = (int)((t->next_slot - 1) % t->slots.size());
         }
         std::vector<LookbackSwapFrame> sw;
         std::vector<std::array<long long, 3>> em;
@@ -3221,7 +3324,7 @@ int rf_detect_yuv_redact_lookback_device(rf_handle h, rf_tracker t, const rf_yuv
         CK(cudaEventRecord(t->chain, c.stream));
         if (!em.empty())
             redact_issue(h, c, yuv_redact_table(outs.data(), (int)outs.size(), nullptr), slot.lb_boxes, slot.lb_counts, nullptr, nullptr, nullptr,
-                         spec, lookback_records(h->cfg.max_faces, t->cfg.max_tracks, L));
+                         spec, lb_records(t));
         CK(cudaEventRecord(slot.free, c.stream));
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     for (int i = 0; i < n; i++) {
@@ -3273,7 +3376,7 @@ int rf_tracker_drain(rf_tracker t, int video, const rf_redact_style *style, cons
         CK(cudaEventRecord(t->chain, c.stream));
         if (k > 0)
             redact_issue(h, c, yuv_redact_table(out_frames, k, nullptr), slot.lb_boxes, slot.lb_counts, nullptr, nullptr, nullptr, spec,
-                         lookback_records(h->cfg.max_faces, t->cfg.max_tracks, L));
+                         lb_records(t));
         CK(cudaEventRecord(slot.free, c.stream));
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     for (int j = 0; j < k; j++) out_frame_numbers[j] = (int32_t)(lv.frames - k + j);

@@ -14,60 +14,17 @@
 
 #include "follow.cuh"
 #include "kalman.cuh"
+#include "tsearch.cuh"
 
 namespace rf {
 namespace {
-
-constexpr int WIN = FOLLOW_T + 2 * FOLLOW_MAX_R;      // window side at the largest R
-constexpr int WWORDS = WIN / 4 + 1;                    // words per window row: a candidate row may read one word past its last
-constexpr int MAX_SIDE = 2 * FOLLOW_MAX_R + 1;
-constexpr double kGrow = 1.0 + 2.0 * RF_FOLLOW_MARGIN;
-constexpr double FOLLOW_MAX_BOX = 65536.0;             // predicted centre and size bound: keeps the fixed-point coordinates in int
-
-struct Grid {
-    double px, py, ox, oy;
-};
-
-__device__ __forceinline__ Grid grid_of(double cx, double cy, double w, double h, double c) {
-    const double gw = (w * kGrow) * c, gh = (h * kGrow) * c;
-    Grid g;
-    g.px = gw / (double)FOLLOW_T;
-    g.py = gh / (double)FOLLOW_T;
-    g.ox = ((cx - gw / 2.0) + g.px / 2.0) - 0.5;
-    g.oy = ((cy - gh / 2.0) + g.py / 2.0) - 0.5;
-    return g;
-}
-
-// c_k: {1 / s, 1, s}
-__device__ __forceinline__ double scale_of(int k) { return k == 0 ? 1.0 / RF_FOLLOW_SCALE : k == 1 ? 1.0 : RF_FOLLOW_SCALE; }
-
-// Pixel (i, j) of the map [[px, 0, X], [0, py, Y]]: cv::warpAffine's fixed-point coordinate and f5's integer bilinear on the luma
-// plane (warp.cuh's sample() on one channel).  inside: all four taps lay in the frame.
-__device__ __forceinline__ int luma_at(const FollowFrame &f, double px, double py, double X, double Y, int i, int j, bool &inside) {
-    const int Xf = (__double2int_rn(X * 1024.0) + 16 + __double2int_rn((px * (double)i) * 1024.0)) >> 5;
-    const int Yf = (__double2int_rn((py * (double)j + Y) * 1024.0) + 16) >> 5;
-    const int sx = min(max(Xf >> 5, -32768), 32767), sy = min(max(Yf >> 5, -32768), 32767);
-    const int fx = Xf & 31, fy = Yf & 31;
-    const int wts[4] = {32 * (32 - fx) * (32 - fy), 32 * fx * (32 - fy), 32 * (32 - fx) * fy, 32 * fx * fy};
-    int acc = 16384, in = 0;
-#pragma unroll
-    for (int t = 0; t < 4; t++) {
-        const int tx = sx + (t & 1), ty = sy + (t >> 1);
-        if ((unsigned)tx < (unsigned)f.w && (unsigned)ty < (unsigned)f.h) {
-            acc += wts[t] * f.y[(size_t)ty * f.pitch + tx];
-            in++;
-        }
-    }
-    inside = in == 4;
-    return acc >> 15;
-}
 
 __global__ void __launch_bounds__(FOLLOW_THREADS) k_follow_cut(const FollowArgs a, const __grid_constant__ FollowTable t) {
     __shared__ int s_slot;
     __shared__ double s_g[4];
     __shared__ unsigned long long s_sum, s_sq;
     const FollowFrame &f = t.f[blockIdx.y];
-    const int T = a.p.max_tracks, tid = threadIdx.x, lane = tid & 31;
+    const int T = a.p.max_tracks, tid = threadIdx.x;
     if ((int)blockIdx.x >= a.list_counts[f.frame]) return;                     // uniform
     const rf_track &tr = a.lists[(size_t)f.frame * T + blockIdx.x];
     if (tr.det < 0) return;                                                       // uniform
@@ -85,38 +42,22 @@ __global__ void __launch_bounds__(FOLLOW_THREADS) k_follow_cut(const FollowArgs 
         s_slot = slot;
         s_sum = 0;
         s_sq = 0;
-        const double x1 = tr.face.x1, y1 = tr.face.y1, w = (double)tr.face.x2 - x1, h = (double)tr.face.y2 - y1;
-        const Grid g = grid_of(x1 + w / 2.0, y1 + h / 2.0, w, h, 1.0);
-        s_g[0] = g.px; s_g[1] = g.py; s_g[2] = g.ox; s_g[3] = g.oy;
+        cut_grid(tr.face, s_g);
     }
     __syncthreads();
     const int slot = s_slot;
     if (slot < 0) return;                                                         // uniform
     const size_t e = (size_t)f.video * T + slot;
-    uint8_t *dst = a.store + e * FOLLOW_BYTES;
-    unsigned s1 = 0, s2 = 0;
-    for (int p = tid; p < FOLLOW_BYTES; p += FOLLOW_THREADS) {
-        bool in;
-        const unsigned v = (unsigned)luma_at(f, s_g[0], s_g[1], s_g[2], s_g[3], p % FOLLOW_T, p / FOLLOW_T, in);
-        dst[p] = (uint8_t)v;
-        s1 += v;
-        s2 += v * v;
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) { s1 += __shfl_xor_sync(0xffffffffu, s1, o); s2 += __shfl_xor_sync(0xffffffffu, s2, o); }
-    if (lane == 0) { atomicAdd(&s_sum, (unsigned long long)s1); atomicAdd(&s_sq, (unsigned long long)s2); }
+    cut_template(f, s_g, a.store + e * FOLLOW_BYTES, &s_sum, &s_sq);
     __syncthreads();
-    if (tid == 0) {
-        const long long var = (long long)FOLLOW_BYTES * (long long)s_sq - (long long)s_sum * (long long)s_sum;
-        a.entries[e] = FollowEntry{tr.id, var < (long long)RF_FOLLOW_MIN_VAR * FOLLOW_BYTES * FOLLOW_BYTES};
-    }
+    if (tid == 0) a.entries[e] = FollowEntry{tr.id, template_flat(s_sum, s_sq)};
 }
 
 __global__ void __launch_bounds__(FOLLOW_THREADS) k_follow_search(const FollowArgs a, const __grid_constant__ FollowTable t) {
-    __shared__ uint32_t s_win[3][WIN][WWORDS];
-    __shared__ uint8_t s_in[3][WIN][WIN];
+    __shared__ uint32_t s_win[3][FOLLOW_WIN][FOLLOW_WWORDS];
+    __shared__ uint8_t s_in[3][FOLLOW_WIN][FOLLOW_WIN];
     __shared__ uint32_t s_tpl[FOLLOW_BYTES / 4];
-    __shared__ int s_sad[3 * MAX_SIDE * MAX_SIDE];
+    __shared__ int s_sad[3 * FOLLOW_MAX_SIDE * FOLLOW_MAX_SIDE];
     __shared__ unsigned long long s_key[FOLLOW_THREADS / 32];
     __shared__ double s_g[3][4];
     __shared__ int s_inside;
@@ -139,8 +80,7 @@ __global__ void __launch_bounds__(FOLLOW_THREADS) k_follow_search(const FollowAr
     }
     const double pw = pa * ph;
     const int R = a.search, W = FOLLOW_T + 2 * R, side = 2 * R + 1, nc = side * side;
-    const bool bounded = ph > 0.0 && ph <= FOLLOW_MAX_BOX && pw > 0.0 && pw <= FOLLOW_MAX_BOX && fabs(pcx) <= FOLLOW_MAX_BOX &&
-                         fabs(pcy) <= FOLLOW_MAX_BOX;
+    const bool bounded = FOLLOW_SEARCH_BOUNDED(pcx, pcy, pw, ph);
     if (a.entries[e].id != id || !bounded) {                                      // uniform: no template, or no search
         if (tid == 0) {
             rf_follow r{};
@@ -150,70 +90,20 @@ __global__ void __launch_bounds__(FOLLOW_THREADS) k_follow_search(const FollowAr
         }
         return;
     }
-    if (tid < 3) {
-        const Grid g = grid_of(pcx, pcy, pw, ph, scale_of(tid));
-        s_g[tid][0] = g.px;
-        s_g[tid][1] = g.py;
-        s_g[tid][2] = g.ox - (double)R * g.px;
-        s_g[tid][3] = g.oy - (double)R * g.py;
-    }
+    if (tid < 3) search_grid(s_g, tid, pcx, pcy, pw, ph, R);
     if (tid == 0) s_inside = 0;
     const uint32_t *tsrc = reinterpret_cast<const uint32_t *>(a.store + e * FOLLOW_BYTES);
     for (int w = tid; w < FOLLOW_BYTES / 4; w += FOLLOW_THREADS) s_tpl[w] = tsrc[w];
     __syncthreads();
-    for (int p = tid; p < 3 * W * W; p += FOLLOW_THREADS) {
-        const int k = p / (W * W), rem = p - k * W * W, r = rem / W, c = rem - r * W;
-        bool in;
-        const int v = luma_at(f, s_g[k][0], s_g[k][1], s_g[k][2], s_g[k][3], c, r, in);
-        reinterpret_cast<uint8_t *>(s_win[k][r])[c] = (uint8_t)v;
-        s_in[k][r][c] = in;
-    }
+    search_windows(f, s_g, W, s_win, s_in, tid);
     __syncthreads();
-    unsigned long long best = ~0ull;
-    for (int o = tid; o < 3 * nc; o += FOLLOW_THREADS) {
-        const int k = o / nc, rem = o - k * nc, wy = rem / side, wx = rem - wy * side;
-        const uint32_t *wp = &s_win[k][wy][wx >> 2];
-        const unsigned sel = 0x3210u + 0x1111u * (unsigned)(wx & 3);
-        unsigned sad = 0;
-        for (int r = 0; r < FOLLOW_T; r++, wp += WWORDS) {
-            uint32_t w0 = wp[0];
-#pragma unroll
-            for (int q = 0; q < FOLLOW_T / 4; q++) {
-                const uint32_t w1 = wp[q + 1];
-                sad = __vsadu4(s_tpl[r * (FOLLOW_T / 4) + q], __byte_perm(w0, w1, sel)) + sad;
-                w0 = w1;
-            }
-        }
-        s_sad[o] = (int)sad;
-        const int dx = wx - R, dy = wy - R;
-        const unsigned long long key = ((unsigned long long)sad << 20) | ((unsigned long long)(abs(dx) + abs(dy)) << 14) |
-                                       ((unsigned long long)k << 12) | ((unsigned long long)wy << 6) | (unsigned long long)wx;
-        best = min(best, key);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) best = min(best, __shfl_xor_sync(0xffffffffu, best, o));
-    if (lane == 0) s_key[tid >> 5] = best;
-    __syncthreads();
-    best = s_key[0];
-#pragma unroll
-    for (int w = 1; w < FOLLOW_THREADS / 32; w++) best = min(best, s_key[w]);
-    const int k = (int)(best >> 12) & 3, wy = (int)(best >> 6) & 63, wx = (int)best & 63;
-    int in = 0;
-    for (int p = tid; p < FOLLOW_BYTES; p += FOLLOW_THREADS) in += s_in[k][wy + p / FOLLOW_T][wx + p % FOLLOW_T];
-    if (in) atomicAdd(&s_inside, in);
+    const unsigned long long best = search_min(s_win, s_tpl, s_sad, s_key, R, side, nc, tid, lane);
+    const SearchPick pick = search_pick(best);
+    search_inside(s_in, pick, &s_inside, tid);
     __syncthreads();
     if (tid != 0) return;
-    const int dx = wx - R, dy = wy - R, c = k * nc + wy * side + wx, s0 = s_sad[c];
-    const bool border = abs(dx) == R || abs(dy) == R;
-    double fx = 0.0, fy = 0.0;
-    if (!border) {
-        const int xm = s_sad[c - 1], xp = s_sad[c + 1], ym = s_sad[c - side], yp = s_sad[c + side];
-        const int dnx = 2 * (xm - 2 * s0 + xp), dny = 2 * (ym - 2 * s0 + yp);
-        if (dnx != 0) fx = (double)(xm - xp) / (double)dnx;
-        if (dny != 0) fy = (double)(ym - yp) / (double)dny;
-    }
-    const double ncx = pcx + ((double)dx + fx) * s_g[k][0], ncy = pcy + ((double)dy + fy) * s_g[k][1];
-    const double nw = pw * scale_of(k), nh = ph * scale_of(k);
+    const SearchHit h = search_hit(s_sad, s_g, pick, R, side, nc, pcx, pcy, pw, ph);
+    const double ncx = h.ncx, ncy = h.ncy, nw = h.nw, nh = h.nh;
     const rf_face &o = S.face;
     rf_face nf;
     nf.score = o.score;
@@ -230,19 +120,15 @@ __global__ void __launch_bounds__(FOLLOW_THREADS) k_follow_search(const FollowAr
     }
     rf_follow r;
     r.id = id;
-    r.dx = dx;
-    r.dy = dy;
-    r.scale = k;
-    r.sad = s0;
-    r.fx = (float)fx;
-    r.fy = (float)fy;
+    r.dx = h.dx;
+    r.dy = h.dy;
+    r.scale = pick.k;
+    r.sad = h.sad;
+    r.fx = (float)h.fx;
+    r.fy = (float)h.fy;
     r.x1 = nf.x1; r.y1 = nf.y1; r.x2 = nf.x2; r.y2 = nf.y2;
     const bool empty = !((double)nf.x2 - (double)nf.x1 > 0.0) || !((double)nf.y2 - (double)nf.y1 > 0.0);
-    r.status = a.entries[e].flat                                 ? RF_FOLLOW_FLAT
-               : 4 * s_inside < 3 * FOLLOW_BYTES                 ? RF_FOLLOW_OUTSIDE
-               : border                                          ? RF_FOLLOW_BORDER
-               : (double)s0 > (double)a.max_mad * (double)FOLLOW_BYTES || empty ? RF_FOLLOW_MISMATCH
-                                                                 : RF_FOLLOW_OK;
+    r.status = search_status(a.entries[e].flat, s_inside, h, a.max_mad, empty);
     out->rec = r;
     out->face = nf;
 }

@@ -18,11 +18,6 @@ constexpr int SWAP_UNROLL = 4;                       // 16-byte chunks in flight
 
 __host__ __device__ __forceinline__ size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 
-__device__ __forceinline__ const float4 *slot_boxes(const uint8_t *slot) { return reinterpret_cast<const float4 *>(slot + sizeof(LookbackHead)); }
-__device__ __forceinline__ const LookbackBirth *slot_births(const uint8_t *slot, int max_faces, int max_tracks) {
-    return reinterpret_cast<const LookbackBirth *>(slot_boxes(slot) + max_faces + max_tracks);
-}
-
 // Exclusive block scan of a 0/1 flag over LOOKBACK_THREADS threads; *total receives the count.  Every thread of the CTA calls it.
 __device__ int flag_scan(bool v, int *total, int *s_w) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -133,7 +128,33 @@ __global__ void __launch_bounds__(LOOKBACK_THREADS) k_lookback_boxes(const Lookb
         r.anchor_index = -1;
         out[nab + q] = r;
     }
-    if (threadIdx.x == 0) a.out_counts[t.j0 + k] = nab + nb;
+    int nd = 0;
+    if (a.search) {      // f17 (d): the same births in the same order, each with its step d's box when the chain reached it OK
+        __shared__ int s_w[LOOKBACK_THREADS / 32];
+        for (int q0 = 0; q0 < nb; q0 += LOOKBACK_THREADS) {
+            const int q = q0 + threadIdx.x;
+            int d = 1;
+            while (d < span && s_first[d] <= q) d++;
+            const uint8_t *sb = slot_of(d);
+            const int rk = q - s_first[d - 1];
+            const bool ok = q < nb && d <= slot_nok(sb, a.max_faces, a.max_tracks, a.L)[rk];
+            int tot;
+            const int pos = flag_scan(ok, &tot, s_w);
+            if (ok) {
+                const float4 b = slot_chain(sb, a.max_faces, a.max_tracks)[(size_t)rk * a.L + d - 1];
+                rf_det r{};
+                r.face.score = 1.f;
+                r.face.x1 = b.x;
+                r.face.y1 = b.y;
+                r.face.x2 = b.z;
+                r.face.y2 = b.w;
+                r.anchor_index = -1;
+                out[nab + nb + nd + pos] = r;
+            }
+            nd += tot;
+        }
+    }
+    if (threadIdx.x == 0) a.out_counts[t.j0 + k] = nab + nb + nd;
 }
 
 // One warp per plane row (luma rows, then the chroma rows: one interleaved plane, or U then V).  A thread owns the same bytes of the
@@ -200,8 +221,10 @@ __global__ void __launch_bounds__(LOOKBACK_THREADS) k_lookback_swap(const __grid
 
 }  // namespace
 
-size_t lookback_slot_bytes(int max_faces, int max_tracks) {
-    return align256(sizeof(LookbackHead) + sizeof(float4) * (max_faces + max_tracks) + sizeof(LookbackBirth) * std::min(max_faces, max_tracks));
+size_t lookback_slot_bytes(int max_faces, int max_tracks, int search_L) {
+    const size_t bcap = std::min(max_faces, max_tracks);
+    if (search_L) return align256(lookback_chain_offset(max_faces, max_tracks) + bcap * search_L * sizeof(float4) + bcap * sizeof(int));
+    return align256(sizeof(LookbackHead) + sizeof(float4) * (max_faces + max_tracks) + sizeof(LookbackBirth) * bcap);
 }
 
 cudaError_t launch_lookback_log(const LookbackArgs &a, const LookbackLogTable &t, cudaStream_t s) {

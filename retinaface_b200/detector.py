@@ -224,7 +224,8 @@ class RetinaFace:
 
     def redactFrames(self, frames: Sequence, videos: Sequence[int] = None, threshold: float = 0.5, blocks: int = 0, margin: float = 0.0,
                      layout: str = "nv12", matrix: str = "bt601", max_videos: int = 64, motion=False, style: str = "mosaic",
-                     shape: str = "rect", detail: int = 0, lookback: int = 0, out: Sequence = None, detect_every: int = 1):
+                     shape: str = "rect", detail: int = 0, lookback: int = 0, out: Sequence = None, detect_every: int = 1,
+                     lookback_search=False):
         """f12 redaction: detect on device 4:2:0 frames (torch CUDA tensors in ``Engine.detect_yuv_device``'s forms) and mosaic every
         detected face IN PLACE (rf_detect_yuv_redact_device), ``blocks`` cells across a region's longer side (0: 8; 1: a flat patch),
         each side grown by ``margin`` of the box (0: 0.25).  With ``videos`` (frame i of video ``videos[i]``) the frames are also
@@ -237,8 +238,13 @@ class RetinaFace:
         its video, also covered where the faces first detected in the next L frames already were, is written into ``out[i]`` (None:
         the input frame itself, in place).  Returns the emitted frame numbers (-1: nothing emitted yet); ``drainVideo`` emits the rest.
         f16: ``detect_every=k`` (with ``videos``) detects each video's frames whose number is divisible by k and follows the faces on
-        the others (rf_track_follow_redact_device), redacting every followed face and every LOST track, as ``trackFrames`` splits."""
+        the others (rf_track_follow_redact_device), redacting every followed face and every LOST track, as ``trackFrames`` splits.
+        f17: ``lookback_search`` (True or ``Tracker.set_lookback_search`` keywords, with ``lookback``) follows every new face back
+        through the buffered frames by template search and covers its path as well; the first call decides, and asking for it on a
+        tracker created without it raises ValueError."""
         kw = dict(layout=layout, matrix=matrix, blocks=blocks, margin=margin, style=style, shape=shape, detail=detail)
+        if lookback_search and not lookback:
+            raise ValueError("lookback_search needs lookback: the search runs through the look-back buffer")
         self._interval_tracker(detect_every, lookback=lookback)
         if videos is None:
             if lookback:
@@ -248,7 +254,10 @@ class RetinaFace:
             self.engine.detect_yuv_redact_device(list(frames), threshold, self.nms_threshold, **kw)
             return
         if getattr(self, "_tracker", None) is None:
-            self._tracker = self.engine.tracker(max_videos=max_videos, motion=motion, lookback=lookback or None, follow=detect_every > 1)
+            self._tracker = self.engine.tracker(max_videos=max_videos, motion=motion, lookback=lookback or None, follow=detect_every > 1,
+                                                lookback_search=lookback_search or None)
+        elif lookback_search and not self._tracker.lookback_search_on:
+            raise ValueError("lookback_search: this detector's tracker was created without the look-back search (the first call decides)")
         if lookback:
             return self._tracker.detect_yuv_redact_lookback_device(list(frames), list(videos), list(frames if out is None else out), threshold,
                                                                    self.nms_threshold, **kw)[0]

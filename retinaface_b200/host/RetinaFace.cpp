@@ -321,7 +321,7 @@ void RetinaFace::trackDetect(const vector<rf_yuv_frame> &device_frames, const ve
     noteMotion(n);
 }
 
-rf_tracker RetinaFace::makeTracker(int lookback) {
+rf_tracker RetinaFace::makeTracker(int lookback, bool lookback_search) {
     rf_track_config tc{};
     tc.max_videos = opt_.track_videos;
     int rc = rf_tracker_create(h_, &tc, &tracker_);
@@ -331,6 +331,12 @@ rf_tracker RetinaFace::makeTracker(int lookback) {
         const rf_lookback_config lc{lookback, 0.f};
         rc = rf_tracker_set_lookback(tracker_, &lc);
         if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_set_lookback: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+        if (lookback_search) {
+            const rf_follow_config fc{0, 0.f};
+            rc = rf_tracker_set_lookback_search(tracker_, &fc);
+            if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_set_lookback_search: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+            tracker_search_ = true;
+        }
     }
     return tracker_;
 }
@@ -400,7 +406,10 @@ void RetinaFace::redactYUV(const vector<rf_yuv_frame> &device_frames, const vect
     if (device_frames.size() > (size_t)opt_.max_batch) throw std::invalid_argument("redactYUV: at most max_batch frames per call");
     if (videos && best_tracker_) throw std::logic_error("redactYUV: this RetinaFace tracks with best shots (trackYUVBest)");
     if (opt.lookback && opt_.detect_every > 1) throw std::invalid_argument("redactYUV: lookback does not combine with detect_every yet");
-    if (videos && !tracker_) makeTracker(opt.lookback);
+    if (opt.lookback_search && !opt.lookback) throw std::invalid_argument("redactYUV: lookback_search needs lookback");
+    if (videos && !tracker_) makeTracker(opt.lookback, opt.lookback_search);
+    if (videos && opt.lookback_search && !tracker_search_)
+        throw std::logic_error("redactYUV: lookback_search, but this RetinaFace's tracker was created without it (the first call decides)");
     const rf_redact_style st{opt.style, opt.shape, opt.style == RF_REDACT_BLUR ? 0 : opt.blocks, opt.detail, opt.margin};
     if (videos && opt_.detect_every > 1) {
         for (const auto &call : intervalCalls(*videos)) {

@@ -66,6 +66,10 @@ struct RedactOptions {
     int detail = 0;                      // blur: 0 (4) or 1..64, a larger detail a smaller radius; 0 for the mosaic
     int lookback = 0;                    // f15, with videos: L (1..64) frames of delay, so that faces are covered before their first
                                          // detection (rf_detect_yuv_redact_lookback_device); 0: redact in place, undelayed
+    bool lookback_search = false;        // f17, with lookback: follow each new face back through the buffered frames by template
+                                         // search (rf_tracker_set_lookback_search, default R and max_mad) and cover its path too;
+                                         // the first tracked call decides, and a later call asking for it on a tracker made
+                                         // without it throws
 };
 
 class RetinaFace {
@@ -182,13 +186,14 @@ class RetinaFace {
     void keepResults(size_t start, int n, const unsigned char *crops, int per, int cw, int ch);
     void trackerCreated();              // motion on a new tracker, as the options say
     void noteMotion(int n);             // lastMotion() after a tracked call of n frames
-    rf_tracker makeTracker(int lookback);   // trackYUV's / redactYUV's tracker, as the options say
+    rf_tracker makeTracker(int lookback, bool lookback_search = false);   // trackYUV's / redactYUV's tracker, as the options say
     // f16: the call's frames as (detect?, frame indices) sub-calls in issue order; advances each video's frame number
     vector<std::pair<bool, vector<int>>> intervalCalls(const vector<int> &videos);
     void followCall(const vector<rf_yuv_frame> &frames, const vector<int> &videos, const rf_redact_style *style);
     void trackDetect(const vector<rf_yuv_frame> &frames, const vector<int> &videos, float threshold, const AlignOptions *align, void *dev_crops);
     rf_handle h_ = nullptr;
     rf_tracker tracker_ = nullptr;
+    bool tracker_search_ = false;        // f17: tracker_ searches its look-back buffer
     bool best_tracker_ = false;
     DeviceTracks tracks_;
     DeviceBestShots best_;

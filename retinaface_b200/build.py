@@ -17,6 +17,7 @@ COMMON = ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
 # that pair of braces (bit-exact decode / IoU, see the header comment there).
 SOURCES = [
     ("engine.cu", []),
+    ("tracker.cu", []),
     ("plan_net.cu", []),
     ("plan_fp.cu", []),
     ("plan_i8.cu", []),

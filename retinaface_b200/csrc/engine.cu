@@ -1,5 +1,6 @@
-// engine.cu -- the handle behind include/rf_b200.h: model upload, activation arena, CUDA-graph executor and the C-ABI entry
-// points.  The layer plans live in plan_fp.cu (FP32 / FP16) and plan_i8.cu (INT8); shared types in engine_internal.cuh.
+// engine.cu -- the handle behind include/rf_b200.h: model upload, activation arena, CUDA-graph executor and the detect C-ABI
+// entry points.  The layer plans live in plan_fp.cu (FP32 / FP16) and plan_i8.cu (INT8), the video tracker in tracker.cu; shared
+// types in engine_internal.cuh.
 //
 // Replaces the reference's engine slot: TrtNetBase / TrtRetinaFaceNet
 // (retinaface/tensorrt/trtnetbase.cpp:199-330, trtretinafacenet.cpp:48-210) and the detect
@@ -10,12 +11,6 @@
 #include "engine_internal.cuh"
 #include "calibrate.cuh"
 #include "preprocess.cuh"
-#include "best.cuh"
-#include "redact.cuh"
-#include "track.cuh"
-#include "motion.cuh"
-#include "lookback.cuh"
-#include "follow.cuh"
 
 namespace rf_eng {
 
@@ -576,12 +571,13 @@ struct H2DRuns {
     }
 };
 
+extern "C++" {
 // One host plane of `rows` rows of row_bytes (pitch bytes apart) -> d_dst, packed, on `s`.  Pinned sources (cudaHostAlloc /
 // cudaHostRegister) are copied straight from the caller's memory, row stride and all.  Pageable sources are staged through the
 // two pinned buffers (each plane fits one: it is at most a max_image BGR image): a row-band parallel host copy (host_copy.h) into
 // one buffer overlaps the DMA out of the other; the only host wait is for the DMA that last read the buffer about to be
 // overwritten.  In both cases the stream orders the copy into d_raw behind the letter-box kernel that still reads the previous image.
-static void upload_plane(rf_handle h, cudaStream_t s, uint8_t *d_dst, const uint8_t *src, size_t row_bytes, size_t pitch, int rows) {
+void rf_eng::upload_plane(rf_handle h, cudaStream_t s, uint8_t *d_dst, const uint8_t *src, size_t row_bytes, size_t pitch, int rows) {
     if (is_pinned(src)) {
         CK(cudaMemcpy2DAsync(d_dst, row_bytes, src, pitch, row_bytes, (size_t)rows, cudaMemcpyHostToDevice, s));
         return;
@@ -595,12 +591,7 @@ static void upload_plane(rf_handle h, cudaStream_t s, uint8_t *d_dst, const uint
     CK(cudaEventRecord(h->raw_ev[slot], s));
 }
 
-// ---- image sources ---------------------------------------------------------------------------------------------------------------
-// Every detect entry point describes the caller's pixels with one of two sources.  A source checks the caller's description (every
-// check runs before anything is copied or launched), reports image i's stored size and EXIF orientation, and hands the letter-box
-// and crop kernels its pixels: upload(s, i, slot) copies host image i into raw buffer `slot` on s (the blocking paths),
-// in_place(i) reads the caller's device memory (the asynchronous ones).  Src is what those kernels read.
-static int check_orientations(rf_handle h, const char *who, const int *orientations, int n) {
+int rf_eng::check_orientations(rf_handle h, const char *who, const int *orientations, int n) {
     if (n > 0 && !orientations) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: orientations is NULL", who));
     for (int i = 0; i < n; i++)
         if (lb_orientation_bits(orientations[i]) < 0)
@@ -609,7 +600,7 @@ static int check_orientations(rf_handle h, const char *who, const int *orientati
 }
 
 // Checks n, the matrix and every frame descriptor; nothing is launched before this passes.
-static int check_frames(rf_handle h, const char *who, const rf_yuv_frame *frames, int n, int matrix) {
+int rf_eng::check_frames(rf_handle h, const char *who, const rf_yuv_frame *frames, int n, int matrix) {
     int rc = check_n(h, n);
     if (rc) return rc;
     if (n > 0 && !frames) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frames is NULL", who));
@@ -632,86 +623,8 @@ static int check_frames(rf_handle h, const char *who, const rf_yuv_frame *frames
     }
     return RF_OK;
 }
+}  // extern "C++"
 
-
-// BGR images: u8 BGR HWC rows row_strides[i] bytes apart (NULL or 0: packed), shown in EXIF orientation orient[i] when `oriented`.
-struct BgrImages {
-    using Src = BgrRows;
-    const uint8_t *const *imgs;
-    const int *widths, *heights, *row_strides, *orient;
-    bool oriented;
-    int width(int i) const { return widths[i]; }
-    int height(int i) const { return heights[i]; }
-    int stride(int i) const { return row_strides && row_strides[i] ? row_strides[i] : widths[i] * 3; }
-    int bits(int i) const { return oriented ? lb_orientation_bits(orient[i]) : 0; }
-    // network-sized, packed and upright: copied straight into the input tensor, without a raw buffer or a letter-box
-    bool direct(rf_handle h, int i) const {
-        return widths[i] == h->cfg.net_w && heights[i] == h->cfg.net_h && stride(i) == h->cfg.net_w * 3 && bits(i) == 0;
-    }
-    int check(rf_handle h, const char *who, int n) const {
-        int rc = check_n(h, n);
-        if (rc) return rc;
-        if (n > 0 && (!imgs || !widths || !heights)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL image arrays", who));
-        for (int i = 0; i < n; i++) {
-            if (!imgs[i] || widths[i] <= 0 || heights[i] <= 0) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: image %d is empty", who, i));
-            if (stride(i) < widths[i] * 3)
-                return fail(h, RF_ERR_INVALID_ARG, fmt("%s: image %d: row stride %d below %d bytes", who, i, stride(i), widths[i] * 3));
-            if (widths[i] > h->cfg.max_image_w || heights[i] > h->cfg.max_image_h)
-                return fail(h, RF_ERR_CAPACITY, fmt("%s: image %d is %dx%d, larger than max_image %dx%d", who, i, widths[i], heights[i],
-                                                    h->cfg.max_image_w, h->cfg.max_image_h));
-        }
-        return oriented ? check_orientations(h, who, orient, n) : RF_OK;
-    }
-    BgrRows upload(rf_handle h, cudaStream_t s, int i, int slot) const {
-        uint8_t *d = h->d_raw + (size_t)slot * h->raw_bytes;
-        upload_plane(h, s, d, imgs[i], (size_t)widths[i] * 3, (size_t)stride(i), heights[i]);
-        return BgrRows{d, widths[i] * 3};
-    }
-    BgrRows in_place(int i) const { return BgrRows{imgs[i], stride(i)}; }
-};
-
-// YUV 4:2:0 frames (yuv.cuh) in `matrix`, shown in EXIF orientation orient[i] when `oriented`.
-struct YuvFrames {
-    using Src = YuvPlanes;
-    const rf_yuv_frame *frames;
-    int matrix;
-    const int *orient;
-    bool oriented;
-    int width(int i) const { return frames[i].width; }
-    int height(int i) const { return frames[i].height; }
-    int bits(int i) const { return oriented ? lb_orientation_bits(orient[i]) : 0; }
-    bool direct(rf_handle, int) const { return false; }
-    int check(rf_handle h, const char *who, int n) const {
-        int rc = check_frames(h, who, frames, n, matrix);
-        if (rc || !oriented) return rc;
-        return check_orientations(h, who, orient, n);
-    }
-    // 1.5 bytes per pixel: the luma packed, then the chroma as the frame lays it out (one interleaved w x h/2 plane, or two
-    // w/2 x h/2 planes)
-    YuvPlanes upload(rf_handle h, cudaStream_t s, int i, int slot) const {
-        const rf_yuv_frame &f = frames[i];
-        uint8_t *d = h->d_raw + (size_t)slot * h->raw_bytes, *dc = d + (size_t)f.width * f.height;
-        const int cw = f.width / 2, ch = f.height / 2;
-        upload_plane(h, s, d, f.y, f.width, f.y_pitch, f.height);
-        YuvPlanes p{d, dc, dc, f.width, f.width, f.uv_step, matrix};
-        if (f.uv_step == 2) {
-            const uint8_t *first = std::min(f.u, f.v);
-            upload_plane(h, s, dc, first, f.width, f.uv_pitch, ch);
-            p.u = dc + (f.u - first);
-            p.v = dc + (f.v - first);
-        } else {
-            upload_plane(h, s, dc, f.u, cw, f.uv_pitch, ch);
-            upload_plane(h, s, dc + (size_t)cw * ch, f.v, cw, f.uv_pitch, ch);
-            p.v = dc + (size_t)cw * ch;
-            p.uv_pitch = cw;
-        }
-        return p;
-    }
-    YuvPlanes in_place(int i) const {
-        const rf_yuv_frame &f = frames[i];
-        return YuvPlanes{f.y, f.u, f.v, f.y_pitch, f.uv_pitch, f.uv_step, matrix};
-    }
-};
 
 extern "C++" {
 // the displayed size of image i: its stored size, transposed for EXIF orientations 5..8
@@ -724,8 +637,9 @@ static void displayed_size(const Source &src, int i, int &w, int &hgt) {
 }  // extern "C++"
 
 // ---- f5 face alignment (align.cuh) ----------------------------------------------------------------------------------------------
+extern "C++" {
 // Checks the caller's rf_align_params and fills the image-independent kernel arguments (defaults applied).
-static int align_setup(rf_handle h, const char *who, const rf_align_params *p, AlignArgs &a) {
+int rf_eng::align_setup(rf_handle h, const char *who, const rf_align_params *p, AlignArgs &a) {
     if (!p) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: params is NULL", who));
     a = AlignArgs{};
     a.crop_w = p->crop_w; a.crop_h = p->crop_h;
@@ -755,7 +669,7 @@ static int align_setup(rf_handle h, const char *who, const rf_align_params *p, A
 
 // The align checks of every entry point that crops: the params, somewhere for the crops to go and -- the blocking paths cut the
 // crops from the originals after the forward -- a raw buffer of its own for each of the `resident` originals that need one.
-static int check_align(rf_handle h, const char *who, const rf_align_params *p, int n, const void *crops, int resident, AlignArgs &a) {
+int rf_eng::check_align(rf_handle h, const char *who, const rf_align_params *p, int n, const void *crops, int resident, AlignArgs &a) {
     int rc = align_setup(h, who, p, a);
     if (rc) return rc;
     if (n > 0 && !crops) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: align without a crop buffer", who));
@@ -765,6 +679,7 @@ static int check_align(rf_handle h, const char *who, const rf_align_params *p, i
                                             h->cfg.max_image_w, h->cfg.max_image_h));
     return RF_OK;
 }
+}  // extern "C++"
 
 // Makes room for n images' crops and the matrices of the blocking align paths (context 0).
 static void ensure_align_buffers(rf_handle h, int n, const AlignArgs &a) {
@@ -936,10 +851,11 @@ int rf_detect_align_batch_device(rf_handle h, const uint8_t *dev_bgr, int n, flo
     return RF_OK;
 }
 
+extern "C++" {
 // rf_detect_yuv_batch_device, rf_detect_yuv_oriented_device and the detect half of rf_detect_yuv_track_device: the frames are
 // letter-boxed on the context the forward lands on, into that context's own input tensor, and cropped in place.
-static int yuv_device_impl(rf_handle h, const char *who, const YuvFrames &src, int n, float thr, float nms, const rf_align_params *align,
-                           void *dev_crops, double *dev_mats, const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales) {
+int rf_eng::yuv_device_impl(rf_handle h, const char *who, const YuvFrames &src, int n, float thr, float nms, const rf_align_params *align,
+                            void *dev_crops, double *dev_mats, const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales) {
     int rc = src.check(h, who, n);
     if (rc) return rc;
     AlignArgs a;
@@ -973,6 +889,7 @@ static int yuv_device_impl(rf_handle h, const char *who, const YuvFrames &src, i
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }
+}  // extern "C++"
 
 int rf_detect_yuv_batch_device(rf_handle h, const rf_yuv_frame *frames, int n, int matrix, float thr, float nms, const rf_align_params *align,
                                void *dev_crops, double *dev_mats, const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales) {
@@ -1837,1552 +1754,6 @@ int rf_profile_layers(rf_handle h, int n, int iters, char (*names)[64], float *m
         CK(cudaStreamSynchronize(c.stream));
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return cnt;
-}
-
-// ---- f10 face tracking across video frames (track.cuh) ---------------------------------------------------------------------------
-// The tracker owns every video's state and a ring of output slots.  Its kernels are ordered by an event chain: each update (and
-// each reset) waits for `chain` on the stream it is issued on, which may belong to any context, and records it again, so the state
-// of a video is only ever touched by one launch at a time while the forwards of the contexts still overlap.  A slot's `free` is
-// recorded once its due faces have been cropped; the next call on that slot waits for it.
-struct rf_tracker_s {
-    rf_handle h = nullptr;
-    rf_track_config cfg{};             // defaults applied
-    TrackVideo *d_videos = nullptr;    // [max_videos]
-    TrackState *d_state = nullptr;     // [max_videos][max_tracks]
-    TrackPair *d_pairs = nullptr;      // [ctas][max_tracks * max_faces]
-    int *d_order = nullptr;
-    struct Slot {
-        rf_track *tracks = nullptr;    // [max_batch][max_tracks]
-        int *counts = nullptr;         // [max_batch]
-        rf_det *due = nullptr;         // [max_batch][max_faces]
-        int *due_counts = nullptr;     // [max_batch]
-        rf_motion *motion = nullptr;   // [max_batch] f13, with motion on
-        rf_det *lb_boxes = nullptr;    // [max(max_batch, L)][lookback_records] f15, the regions of the emitted frames
-        int *lb_counts = nullptr;      // [max(max_batch, L)]
-        rf_follow *lb_steps = nullptr; // [max_batch][min(max_faces, max_tracks)][L] f17, the step records of a look-back call
-        int *lb_lengths = nullptr;     // [max_batch][min(max_faces, max_tracks)]
-        cudaEvent_t free = nullptr;
-    };
-    std::vector<Slot> slots;
-    unsigned next_slot = 0;
-    cudaEvent_t chain = nullptr;
-    // f11 best shots (best.cuh); `best` false: a plain tracker, none of these allocated.  The chain orders every best-shot kernel
-    // of every call, so one set of per-call tables serves them all; only the emitted records live in the ring.
-    bool best = false;
-    BestArgs ba{};                     // store, per-video counters, per-call tables, formats (per-call pointers set per call)
-    rf_best_shot *d_best = nullptr;    // [slots][max_batch][max_tracks]
-    int *d_best_counts = nullptr;      // [slots][max_batch]
-    bool updated = false;              // a frame call was issued (rf_tracker_set_motion comes before)
-    // f13 camera motion (motion.cuh); `motion` false: none of these allocated.  mref mirrors on the host what each video's
-    // reference slot holds (the frame size it came from, 0 x 0: none): calls, resets and finishes are issued in host order, so the
-    // reference of every frame is known when the call is issued.  The chain orders the per-call scratch as it orders f11's tables.
-    bool motion = false;
-    rf_motion_config mcfg{};
-    uint8_t *d_mstore = nullptr;       // [max_videos][MOTION_THUMB_BYTES]
-    uint8_t *d_mthumbs = nullptr;      // [max_batch][MOTION_THUMB_BYTES]
-    MotionBlock *d_mblocks = nullptr;  // [max_batch][MOTION_MAX_BLOCKS]
-    std::vector<std::array<int, 2>> mref;
-    int motion_slot = -1;              // the ring slot of the latest frame call
-    // f15 look-back (lookback.cuh); `lookback` false: none of these allocated.  lbv mirrors on the host each video's frame count and
-    // layout, so that every frame's number, buffer slot and emission are known when a call is issued.  A video's device block is its
-    // frame buffer (L packed frames of frame_bytes) followed by its log (2 L slots of lookback_slot_bytes).
-    bool lookback = false;
-    int lb_frames = 0;                 // L
-    float lb_grow = 0.f;
-    struct LookbackVideo {
-        uint8_t *d = nullptr;
-        size_t frame_bytes = 0;
-        int w = 0, h = 0, step = 0;
-        bool v_first = false;          // semi-planar with V before U (NV21)
-        long long frames = 0;          // frames since create, reset or drain
-    };
-    std::vector<LookbackVideo> lbv;
-    // f17 searching look-back: the step records live in the ring, the chains in the log slots.
-    bool lb_search = false;
-    rf_follow_config lscfg{};
-    int lb_search_slot = -1;           // the ring slot of the latest look-back call
-    // f16 following (follow.cuh); `follow` false: none of these allocated.  The chain orders the per-call measurements as it orders
-    // f11's tables; the follow records live in the ring.
-    bool follow = false;
-    rf_follow_config fcfg{};
-    uint8_t *d_fstore = nullptr;         // [max_videos][max_tracks][FOLLOW_BYTES]
-    FollowEntry *d_fentries = nullptr;   // [max_videos][max_tracks]
-    FollowMeas *d_fmeas = nullptr;       // [max_batch][max_tracks]
-    rf_follow *d_follow = nullptr;       // [slots][max_batch][max_tracks]
-    rf_det *d_fregions = nullptr;        // [slots][max_batch][max_tracks] the OK-followed faces (redaction's records)
-    int *d_fregion_counts = nullptr;     // [slots][max_batch]
-    rf_det *d_fmask = nullptr;           // [max_batch][max_tracks] with motion: each follow frame's face mask
-    int *d_fmask_counts = nullptr;       // [max_batch]
-    int follow_slot = -1;                // the ring slot of the latest follow call
-};
-
-static void tracker_release(rf_tracker t) {
-    if (t->chain) cudaEventSynchronize(t->chain);
-    for (auto &s : t->slots) {
-        if (s.free) { cudaEventSynchronize(s.free); cudaEventDestroy(s.free); }
-        cudaFree(s.tracks); cudaFree(s.counts); cudaFree(s.due); cudaFree(s.due_counts); cudaFree(s.motion);
-        cudaFree(s.lb_boxes); cudaFree(s.lb_counts); cudaFree(s.lb_steps); cudaFree(s.lb_lengths);
-    }
-    for (auto &v : t->lbv) cudaFree(v.d);
-    cudaFree(t->d_mstore); cudaFree(t->d_mthumbs); cudaFree(t->d_mblocks);
-    cudaFree(t->d_fstore); cudaFree(t->d_fentries); cudaFree(t->d_fmeas); cudaFree(t->d_follow);
-    cudaFree(t->d_fregions); cudaFree(t->d_fregion_counts); cudaFree(t->d_fmask); cudaFree(t->d_fmask_counts);
-    if (t->chain) cudaEventDestroy(t->chain);
-    cudaFree(t->d_videos); cudaFree(t->d_state); cudaFree(t->d_pairs); cudaFree(t->d_order);
-    const BestArgs &b = t->ba;
-    cudaFree(b.store); cudaFree(b.store_crops); cudaFree(b.videos); cudaFree(b.acc); cudaFree((void *)b.seen); cudaFree((void *)b.gone); cudaFree(b.meas);
-    cudaFree(b.scratch); cudaFree(b.commit); cudaFree(b.src); cudaFree(t->d_best); cudaFree(t->d_best_counts);
-    delete t;
-}
-
-int rf_tracker_create(rf_handle h, const rf_track_config *cfg, rf_tracker *out) {
-    static const char *who = "rf_tracker_create";
-    if (!h) return RF_ERR_INVALID_ARG;
-    if (!cfg || !out) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL config or output", who));
-    *out = nullptr;
-    rf_track_config c = *cfg;
-    if (c.max_videos < 1 || c.max_videos > 4096) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: max_videos %d, must be in [1, 4096]", who, c.max_videos));
-    if (c.max_tracks == 0) c.max_tracks = 64;
-    if (c.max_tracks < 1 || c.max_tracks > TRACK_MAX_TRACKS)
-        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: max_tracks %d, must be in [1, %d]", who, c.max_tracks, TRACK_MAX_TRACKS));
-    if (c.max_lost == 0) c.max_lost = 30;
-    if (c.max_lost < 0) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: max_lost %d is negative", who, c.max_lost));
-    float *th[5] = {&c.high_thresh, &c.new_thresh, &c.iou_high, &c.iou_low, &c.iou_tentative};
-    const float dflt[5] = {0.6f, 0.7f, 0.2f, 0.5f, 0.3f};
-    for (int k = 0; k < 5; k++) {
-        if (*th[k] == 0.f) *th[k] = dflt[k];
-        if (!(*th[k] > 0.f && *th[k] <= 1.f))
-            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: thresholds must be in (0, 1] (0: the default), got %g", who, (double)*th[k]));
-    }
-    std::unique_ptr<rf_tracker_s, void (*)(rf_tracker)> t(new rf_tracker_s, tracker_release);
-    t->h = h;
-    t->cfg = c;
-    try {
-        CK(cudaSetDevice(h->device));
-        const size_t T = c.max_tracks, F = h->cfg.max_faces, B = h->cfg.max_batch;
-        const size_t ctas = std::min<size_t>({B, (size_t)TRACK_MAX_FRAMES, (size_t)c.max_videos});
-        CK(cudaMalloc(&t->d_videos, sizeof(TrackVideo) * c.max_videos));
-        CK(cudaMalloc(&t->d_state, sizeof(TrackState) * c.max_videos * T));
-        CK(cudaMalloc(&t->d_pairs, sizeof(TrackPair) * ctas * T * F));
-        CK(cudaMalloc(&t->d_order, sizeof(int) * ctas * T * F));
-        CK(cudaMemset(t->d_videos, 0, sizeof(TrackVideo) * c.max_videos));
-        CK(cudaMemset(t->d_state, 0, sizeof(TrackState) * c.max_videos * T));
-        t->slots.resize(h->ctx.size());
-        for (auto &s : t->slots) {
-            CK(cudaMalloc(&s.tracks, sizeof(rf_track) * B * T));
-            CK(cudaMalloc(&s.counts, sizeof(int) * B));
-            CK(cudaMalloc(&s.due, sizeof(rf_det) * B * F));
-            CK(cudaMalloc(&s.due_counts, sizeof(int) * B));
-            CK(cudaEventCreateWithFlags(&s.free, cudaEventDisableTiming));
-        }
-        CK(cudaEventCreateWithFlags(&t->chain, cudaEventDisableTiming));
-        CK(cudaDeviceSynchronize());      // the zeroed state is in place before any context's stream reads it
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    *out = t.release();
-    return RF_OK;
-}
-
-void rf_tracker_destroy(rf_tracker t) {
-    if (!t) return;
-    cudaSetDevice(t->h->device);
-    tracker_release(t);
-}
-
-int rf_tracker_reset(rf_tracker t, int video) {
-    if (!t) return RF_ERR_INVALID_ARG;
-    rf_handle h = t->h;
-    if (video < -1 || video >= t->cfg.max_videos)
-        return fail(h, RF_ERR_INVALID_ARG, fmt("rf_tracker_reset: video %d, must be -1 or in [0, %d)", video, t->cfg.max_videos));
-    try {
-        CK(cudaSetDevice(h->device));
-        cudaStream_t s = h->ctx[0].stream;
-        const size_t v0 = video < 0 ? 0 : video, nv = video < 0 ? t->cfg.max_videos : 1, T = t->cfg.max_tracks;
-        CK(cudaStreamWaitEvent(s, t->chain, 0));
-        CK(cudaMemsetAsync(t->d_videos + v0, 0, sizeof(TrackVideo) * nv, s));
-        CK(cudaMemsetAsync(t->d_state + v0 * T, 0, sizeof(TrackState) * nv * T, s));
-        if (t->best) {        // the stored shots are discarded, nothing is emitted
-            CK(cudaMemsetAsync(t->ba.store + v0 * T, 0, sizeof(BestEntry) * nv * T, s));
-            CK(cudaMemsetAsync(t->ba.videos + v0, 0, sizeof(BestVideo) * nv, s));
-        }
-        for (size_t v = v0; t->motion && v < v0 + nv; v++) t->mref[v] = {0, 0};
-        for (size_t v = v0; t->lookback && v < v0 + nv; v++) t->lbv[v].frames = 0;     // the buffered frames are dropped
-        if (t->follow) CK(cudaMemsetAsync(t->d_fentries + v0 * T, 0, sizeof(FollowEntry) * nv * T, s));
-        CK(cudaEventRecord(t->chain, s));
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    return RF_OK;
-}
-
-// Everything rf_track_update refuses, checked before anything is launched.
-static int check_track_args(rf_tracker t, const char *who, const int *videos, int n, const float *scales) {
-    rf_handle h = t->h;
-    int rc = check_n(h, n);
-    if (rc) return rc;
-    if (n > 0 && !videos) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: videos is NULL", who));
-    for (int i = 0; i < n; i++) {
-        if (videos[i] < 0 || videos[i] >= t->cfg.max_videos)
-            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frame %d: video %d, must be in [0, %d)", who, i, videos[i], t->cfg.max_videos));
-        if (scales && !(std::isfinite(scales[i]) && scales[i] > 0.f))
-            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frame %d: scale %g, must be finite and positive", who, i, (double)scales[i]));
-    }
-    return RF_OK;
-}
-
-// ---- f13 camera motion (motion.cuh) ---------------------------------------------------------------------------------------------
-// Each video's last frame of a call, whose thumbnail becomes the video's reference once the update has run.
-struct MotionCommits {
-    std::vector<int> frames, videos, bytes;
-};
-
-// The estimate of the call's n frames into ring slot `ring`'s motions, on s inside the chain: each frame's reference is the
-// previous frame of its video in this call, else the video's stored thumbnail, else none (FIRST); a frame size change is none.
-static void motion_issue(rf_tracker t, unsigned ring, const rf_yuv_frame *frames, const int *videos, int n, const rf_det *dets,
-                         const int32_t *counts, const float *scales, cudaStream_t s, MotionCommits &commits) {
-    const int R = t->mcfg.search;
-    std::vector<MotionTable> tabs;
-    std::vector<std::array<int, 2>> last;          // (video, its latest frame of the call)
-    for (int i = 0; i < n; i++) {
-        if (i % TRACK_MAX_FRAMES == 0) {
-            tabs.emplace_back();
-            tabs.back().i0 = i;
-        }
-        MotionTable &tb = tabs.back();
-        MotionFrame &f = tb.f[tb.n++];
-        const rf_yuv_frame &fr = frames[i];
-        const int v = videos[i];
-        f.y = fr.y;
-        f.pitch = fr.y_pitch;
-        f.video = v;
-        f.scale = scales ? scales[i] : 1.f;
-        f.D = (std::max(fr.width, fr.height) + MOTION_THUMB - 1) / MOTION_THUMB;
-        f.tw = fr.width / f.D;
-        f.th = fr.height / f.D;
-        f.nbx = f.tw - 2 * R >= MOTION_BLOCK ? (f.tw - 2 * R) / MOTION_BLOCK : 0;
-        f.nby = f.th - 2 * R >= MOTION_BLOCK ? (f.th - 2 * R) / MOTION_BLOCK : 0;
-        auto it = std::find_if(last.begin(), last.end(), [v](const std::array<int, 2> &e) { return e[0] == v; });
-        const std::array<int, 2> size = {fr.width, fr.height};
-        if (it != last.end()) {
-            const rf_yuv_frame &p = frames[(*it)[1]];
-            f.ref = p.width == fr.width && p.height == fr.height ? (*it)[1] : MOTION_REF_FIRST;
-            (*it)[1] = i;
-        } else {
-            f.ref = t->mref[v] == size ? MOTION_REF_STORE : MOTION_REF_FIRST;
-            last.push_back({v, i});
-        }
-    }
-    for (const auto &e : last) {
-        const rf_yuv_frame &fr = frames[e[1]];
-        const MotionFrame &f = tabs[e[1] / TRACK_MAX_FRAMES].f[e[1] % TRACK_MAX_FRAMES];
-        t->mref[e[0]] = {fr.width, fr.height};
-        commits.frames.push_back(e[1]);
-        commits.videos.push_back(e[0]);
-        commits.bytes.push_back(f.tw * f.th);
-    }
-    MotionArgs a{};
-    a.thumbs = t->d_mthumbs;
-    a.store = t->d_mstore;
-    a.blocks = t->d_mblocks;
-    a.out = t->slots[ring].motion;
-    a.dets = dets;
-    a.counts = counts;
-    a.max_faces = t->h->cfg.max_faces;
-    a.search = R;
-    a.min_inliers = t->mcfg.min_inliers;
-    CK(launch_motion_estimate(a, tabs.data(), (int)tabs.size(), s));
-    t->motion_slot = (int)ring;
-}
-
-static void motion_commit(rf_tracker t, const MotionCommits &c, cudaStream_t s) {
-    MotionArgs a{};
-    a.thumbs = t->d_mthumbs;
-    a.store = t->d_mstore;
-    CK(launch_motion_commit(a, c.frames.data(), c.videos.data(), c.bytes.data(), (int)c.frames.size(), s));
-}
-
-// ---- f16 following (follow.cuh) -------------------------------------------------------------------------------------------------
-static FollowArgs follow_args(rf_tracker t) {
-    FollowArgs f{};
-    f.p = TrackParams{t->cfg.max_tracks, t->h->cfg.max_faces, t->cfg.max_lost, t->cfg.high_thresh, t->cfg.new_thresh, t->cfg.iou_high,
-                      t->cfg.iou_low, t->cfg.iou_tentative};
-    f.videos = t->d_videos;
-    f.state = t->d_state;
-    f.store = t->d_fstore;
-    f.entries = t->d_fentries;
-    f.meas = t->d_fmeas;
-    f.search = t->fcfg.search;
-    f.max_mad = t->fcfg.max_mad;
-    return f;
-}
-
-static FollowFrame follow_frame(const rf_yuv_frame &fr, int video, int i) {
-    return FollowFrame{fr.y, fr.y_pitch, fr.width, fr.height, video, i};
-}
-
-// The templates of the tracks matched on a detect call's frames, from the call's lists in `slot`, on s inside the chain.
-static void follow_cut(rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, const rf_tracker_s::Slot &slot, cudaStream_t s) {
-    FollowArgs f = follow_args(t);
-    f.lists = slot.tracks;
-    f.list_counts = slot.counts;
-    std::vector<FollowFrame> tab(n);
-    for (int i = 0; i < n; i++) tab[i] = follow_frame(frames[i], videos[i], i);
-    CK(launch_follow_cut(f, tab.data(), n, s));
-}
-
-// Issues the update of n frames on s (the records complete there) into the next ring slot, ordered by the chain.  `a` (crops):
-// the due faces are cut on s into a's crops, then the slot's `free` is recorded.
-static void track_issue(rf_tracker t, const int *videos, int n, const rf_det *dets, const int32_t *counts, const float *scales, cudaStream_t s,
-                        const AlignArgs *a, const AlignImageT<YuvPlanes> *table, const rf_track **dev_tracks,
-                        const int32_t **dev_track_counts, const rf_yuv_frame *frames) {
-    rf_handle h = t->h;
-    const unsigned ring = t->next_slot++ % t->slots.size();
-    rf_tracker_s::Slot &slot = t->slots[ring];
-    CK(cudaStreamWaitEvent(s, slot.free, 0));
-    CK(cudaStreamWaitEvent(s, t->chain, 0));
-    t->updated = true;
-    MotionCommits commits;
-    if (t->motion) motion_issue(t, ring, frames, videos, n, dets, counts, scales, s, commits);
-    TrackArgs ta{};
-    ta.p = TrackParams{t->cfg.max_tracks, h->cfg.max_faces, t->cfg.max_lost, t->cfg.high_thresh, t->cfg.new_thresh, t->cfg.iou_high,
-                       t->cfg.iou_low, t->cfg.iou_tentative};
-    ta.videos = t->d_videos;
-    ta.state = t->d_state;
-    ta.pairs = t->d_pairs;
-    ta.order = t->d_order;
-    ta.dets = dets;
-    ta.counts = counts;
-    ta.tracks = slot.tracks;
-    ta.track_counts = slot.counts;
-    if (a) {
-        ta.due = slot.due;
-        ta.due_counts = slot.due_counts;
-        ta.max_align = a->max_align;
-    }
-    ta.motion = t->motion ? slot.motion : nullptr;
-    CK(launch_track_update(ta, videos, scales, n, s));
-    if (t->motion) motion_commit(t, commits, s);
-    if (t->follow) follow_cut(t, frames, videos, n, slot, s);
-    CK(cudaEventRecord(t->chain, s));
-    if (a) {
-        PostBuffers view{};
-        view.out_dets = slot.due;
-        view.out_counts = slot.due_counts;
-        view.max_faces = h->cfg.max_faces;
-        CK(launch_align_faces(*a, table, view, h->num_sms, s));
-    }
-    CK(cudaEventRecord(slot.free, s));
-    if (dev_tracks) *dev_tracks = slot.tracks;
-    if (dev_track_counts) *dev_track_counts = slot.counts;
-}
-
-int rf_track_update(rf_tracker t, const int *videos, int n, const rf_det *dev_dets, const int32_t *dev_counts, const float *scales,
-                    const rf_track **dev_tracks, const int32_t **dev_track_counts) {
-    static const char *who = "rf_track_update";
-    if (!t) return RF_ERR_INVALID_ARG;
-    rf_handle h = t->h;
-    if (t->best) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a best-shot tracker takes frames only through rf_detect_yuv_track_best_device", who));
-    if (t->motion) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a motion tracker needs the frames (rf_detect_yuv_track_device)", who));
-    if (t->follow) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a follow tracker needs the frames (rf_detect_yuv_track_device)", who));
-    if (t->lookback) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a look-back tracker takes frames only through rf_detect_yuv_redact_lookback_device", who));
-    int rc = check_track_args(t, who, videos, n, scales);
-    if (rc) return rc;
-    if (n > 0 && (!dev_dets || !dev_counts)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL records or counts", who));
-    if (n == 0) return RF_OK;
-    try {
-        CK(cudaSetDevice(h->device));
-        track_issue(t, videos, n, dev_dets, dev_counts, scales, (cudaStream_t)rf_last_stream(h), nullptr, nullptr, dev_tracks,
-                    dev_track_counts, nullptr);
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    return RF_OK;
-}
-
-int rf_detect_yuv_track_device(rf_handle h, rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, int matrix, float thr, float nms,
-                               const rf_align_params *align, void *dev_crops, double *dev_mats, const rf_track **dev_tracks,
-                               const int32_t **dev_track_counts, const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales) {
-    static const char *who = "rf_detect_yuv_track_device";
-    if (!h) return RF_ERR_INVALID_ARG;
-    if (!t || t->h != h) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker is NULL or belongs to another handle", who));
-    if (t->best) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a best-shot tracker takes frames only through rf_detect_yuv_track_best_device", who));
-    if (t->lookback) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a look-back tracker takes frames only through rf_detect_yuv_redact_lookback_device", who));
-    int rc = check_track_args(t, who, videos, n, nullptr);
-    if (rc) return rc;
-    const YuvFrames src{frames, matrix, nullptr, false};
-    if ((rc = src.check(h, who, n))) return rc;
-    AlignArgs a;
-    if (align && (rc = check_align(h, who, align, n, dev_crops, 0, a))) return rc;
-    if (n == 0) return RF_OK;
-    std::vector<float> scales(n);
-    const rf_det *dets = nullptr;
-    const int32_t *counts = nullptr;
-    if ((rc = yuv_device_impl(h, who, src, n, thr, nms, nullptr, nullptr, nullptr, &dets, &counts, scales.data()))) return rc;
-    if (dev_dets) *dev_dets = dets;
-    if (dev_counts) *dev_counts = counts;
-    if (out_scales) std::copy(scales.begin(), scales.end(), out_scales);
-    try {
-        // the due faces are already in frame pixels: scale 1, as the tiled paths crop their merged records
-        std::vector<AlignImageT<YuvPlanes>> table(n);
-        for (int i = 0; i < n; i++) table[i] = AlignImageT<YuvPlanes>{src.in_place(i), src.width(i), src.height(i), 1.f, 0};
-        if (align) { a.n = n; a.crops = dev_crops; a.mats = dev_mats; }
-        track_issue(t, videos, n, dets, counts, scales.data(), h->last_stream, align ? &a : nullptr, table.data(), dev_tracks, dev_track_counts,
-                    frames);
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    return RF_OK;
-}
-
-// ---- f11 best shots (best.cuh) ---------------------------------------------------------------------------------------------------
-int rf_tracker_create_best(rf_handle h, const rf_track_config *cfg, const rf_best_config *best, rf_tracker *out) {
-    static const char *who = "rf_tracker_create_best";
-    if (!h) return RF_ERR_INVALID_ARG;
-    if (!cfg || !best || !out) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL config or output", who));
-    *out = nullptr;
-    AlignArgs o;
-    int rc = align_setup(h, who, &best->align, o);
-    if (rc) return rc;
-    if (best->align.max_faces != 0) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: align.max_faces %d, must be 0", who, best->align.max_faces));
-    if (!(best->min_quality >= 0.f && best->min_quality <= 1.f))
-        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: min_quality %g, must be in [0, 1]", who, (double)best->min_quality));
-    const float half = best->sharp_half == 0.f ? 50.f : best->sharp_half;
-    if (!(std::isfinite(half) && half > 0.f)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: sharp_half %g, must be finite and positive", who, (double)half));
-    const size_t u8_bytes = align_crop_bytes(o.crop_w, o.crop_h, RF_CROP_BGR_U8);
-    const int T = cfg->max_tracks == 0 ? 64 : cfg->max_tracks;
-    if (cfg->max_videos >= 1 && cfg->max_videos <= 4096 && T >= 1 && T <= TRACK_MAX_TRACKS && (size_t)cfg->max_videos * T * u8_bytes > ((size_t)4 << 30))
-        return fail(h, RF_ERR_CAPACITY, fmt("%s: a store of %d videos x %d tracks x %zu bytes exceeds 4 GiB", who, cfg->max_videos, T, u8_bytes));
-    rf_tracker t = nullptr;
-    if ((rc = rf_tracker_create(h, cfg, &t))) return rc;
-    std::unique_ptr<rf_tracker_s, void (*)(rf_tracker)> g(t, tracker_release);
-    t->best = true;
-    BestArgs &b = t->ba;
-    b.out = o;
-    b.u8 = o;
-    b.u8.format = RF_CROP_BGR_U8;
-    b.u8.crop_bytes = u8_bytes;
-    b.max_tracks = t->cfg.max_tracks;
-    b.max_faces = h->cfg.max_faces;
-    b.min_quality = (double)best->min_quality;
-    b.sharp_half = (double)half;
-    b.num_sms = h->num_sms;
-    try {
-        const size_t V = t->cfg.max_videos, TT = t->cfg.max_tracks, F = h->cfg.max_faces, B = h->cfg.max_batch;
-        const size_t M = std::min<size_t>(B, TRACK_MAX_FRAMES), R = t->slots.size();
-        CK(cudaMalloc(&b.store, sizeof(BestEntry) * V * TT));
-        CK(cudaMalloc(&b.store_crops, u8_bytes * V * TT));
-        CK(cudaMalloc(&b.videos, sizeof(BestVideo) * V));
-        TrackSeen *seen = nullptr;
-        TrackGone *gone = nullptr;
-        CK(cudaMalloc(&seen, sizeof(TrackSeen) * M * F));
-        b.seen = seen;
-        CK(cudaMalloc(&gone, sizeof(TrackGone) * M * TT));
-        b.gone = gone;
-        CK(cudaMalloc(&b.meas, sizeof(BestMeasure) * M * F));
-        CK(cudaMalloc(&b.acc, sizeof(BestAccum) * M * F));
-        CK(cudaMemset(b.acc, 0, sizeof(BestAccum) * M * F));
-        CK(cudaMalloc(&b.scratch, u8_bytes * M * F));
-        CK(cudaMalloc(&b.commit, sizeof(int) * M * F));
-        CK(cudaMalloc(&b.src, sizeof(int) * M * TT));
-        CK(cudaMalloc(&t->d_best, sizeof(rf_best_shot) * R * B * TT));
-        CK(cudaMalloc(&t->d_best_counts, sizeof(int) * R * B));
-        CK(cudaMemset(b.store, 0, sizeof(BestEntry) * V * TT));
-        CK(cudaMemset(b.videos, 0, sizeof(BestVideo) * V));
-        CK(cudaDeviceSynchronize());
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    *out = g.release();
-    return RF_OK;
-}
-
-int rf_detect_yuv_track_best_device(rf_handle h, rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, int matrix, float thr,
-                                    float nms, void *dev_best_crops, double *dev_best_mats, const rf_best_shot **dev_best,
-                                    const int32_t **dev_best_counts, const rf_track **dev_tracks, const int32_t **dev_track_counts,
-                                    const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales) {
-    static const char *who = "rf_detect_yuv_track_best_device";
-    if (!h) return RF_ERR_INVALID_ARG;
-    if (!t || t->h != h) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker is NULL or belongs to another handle", who));
-    if (!t->best) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: not a best-shot tracker (rf_tracker_create_best)", who));
-    int rc = check_track_args(t, who, videos, n, nullptr);
-    if (rc) return rc;
-    const YuvFrames src{frames, matrix, nullptr, false};
-    if ((rc = src.check(h, who, n))) return rc;
-    if (n > 0 && !dev_best_crops) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: dev_best_crops is NULL", who));
-    if (n == 0) return RF_OK;
-    std::vector<float> scales(n);
-    const rf_det *dets = nullptr;
-    const int32_t *counts = nullptr;
-    if ((rc = yuv_device_impl(h, who, src, n, thr, nms, nullptr, nullptr, nullptr, &dets, &counts, scales.data()))) return rc;
-    if (dev_dets) *dev_dets = dets;
-    if (dev_counts) *dev_counts = counts;
-    if (out_scales) std::copy(scales.begin(), scales.end(), out_scales);
-    try {
-        cudaStream_t s = h->last_stream;
-        const unsigned ring = t->next_slot++ % t->slots.size();
-        rf_tracker_s::Slot &slot = t->slots[ring];
-        const int T = t->cfg.max_tracks, F = h->cfg.max_faces, B = h->cfg.max_batch;
-        rf_best_shot *best = t->d_best + (size_t)ring * B * T;
-        int *best_counts = t->d_best_counts + (size_t)ring * B;
-        CK(cudaStreamWaitEvent(s, slot.free, 0));
-        CK(cudaStreamWaitEvent(s, t->chain, 0));
-        t->updated = true;
-        MotionCommits commits;
-        if (t->motion) motion_issue(t, ring, frames, videos, n, dets, counts, scales.data(), s, commits);
-        TrackArgs ta{};
-        ta.p = TrackParams{T, F, t->cfg.max_lost, t->cfg.high_thresh, t->cfg.new_thresh, t->cfg.iou_high, t->cfg.iou_low, t->cfg.iou_tentative};
-        ta.videos = t->d_videos;
-        ta.state = t->d_state;
-        ta.pairs = t->d_pairs;
-        ta.order = t->d_order;
-        ta.seen = const_cast<TrackSeen *>(t->ba.seen);
-        ta.gone = const_cast<TrackGone *>(t->ba.gone);
-        // the call in chunks of TRACK_MAX_FRAMES frames, each tracked then measured, selected, emitted and committed: the per-call
-        // tables hold one chunk
-        for (int i0 = 0; i0 < n; i0 += TRACK_MAX_FRAMES) {
-            const int m = std::min(TRACK_MAX_FRAMES, n - i0);
-            TrackArgs c = ta;
-            c.dets = dets + (size_t)i0 * F;
-            c.counts = counts + i0;
-            c.tracks = slot.tracks + (size_t)i0 * T;
-            c.track_counts = slot.counts + i0;
-            c.motion = t->motion ? slot.motion + i0 : nullptr;
-            CK(launch_track_update(c, videos + i0, scales.data() + i0, m, s));
-            BestTable bt{};
-            bt.n = m;
-            for (int i = 0; i < m; i++) {
-                const int v = videos[i0 + i];
-                bt.video[i] = v;
-                bt.img[i] = AlignImageT<YuvPlanes>{src.in_place(i0 + i), src.width(i0 + i), src.height(i0 + i), 1.f, 0};
-                bool known = false;
-                for (int k = 0; k < bt.nvideos; k++) known |= bt.cta_video[k] == v;
-                if (!known) bt.cta_video[bt.nvideos++] = v;
-            }
-            BestArgs b = t->ba;
-            b.out.crops = static_cast<uint8_t *>(dev_best_crops) + (size_t)i0 * T * b.out.crop_bytes;
-            b.out.mats = dev_best_mats ? dev_best_mats + (size_t)i0 * T * 6 : nullptr;
-            b.best = best + (size_t)i0 * T;
-            b.best_counts = best_counts + i0;
-            b.counts = counts + i0;
-            CK(launch_best_frames(b, bt, s));
-        }
-        if (t->motion) motion_commit(t, commits, s);
-        CK(cudaEventRecord(t->chain, s));
-        CK(cudaEventRecord(slot.free, s));
-        if (dev_tracks) *dev_tracks = slot.tracks;
-        if (dev_track_counts) *dev_track_counts = slot.counts;
-        if (dev_best) *dev_best = best;
-        if (dev_best_counts) *dev_best_counts = best_counts;
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    return RF_OK;
-}
-
-int rf_tracker_finish(rf_tracker t, int video, void *dev_best_crops, double *dev_best_mats, const rf_best_shot **dev_best,
-                      const int32_t **dev_best_count) {
-    static const char *who = "rf_tracker_finish";
-    if (!t) return RF_ERR_INVALID_ARG;
-    rf_handle h = t->h;
-    if (!t->best) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: not a best-shot tracker (rf_tracker_create_best)", who));
-    if (video < 0 || video >= t->cfg.max_videos) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: video %d, must be in [0, %d)", who, video, t->cfg.max_videos));
-    if (!dev_best_crops) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: dev_best_crops is NULL", who));
-    try {
-        CK(cudaSetDevice(h->device));
-        cudaStream_t s = h->ctx[0].stream;
-        const unsigned ring = t->next_slot++ % t->slots.size();
-        rf_tracker_s::Slot &slot = t->slots[ring];
-        const size_t T = t->cfg.max_tracks, B = h->cfg.max_batch;
-        CK(cudaStreamWaitEvent(s, slot.free, 0));
-        CK(cudaStreamWaitEvent(s, t->chain, 0));
-        BestArgs b = t->ba;
-        b.out.crops = dev_best_crops;
-        b.out.mats = dev_best_mats;
-        b.best = t->d_best + ring * B * T;
-        b.best_counts = t->d_best_counts + ring * B;
-        CK(launch_best_finish(b, video, t->d_state + (size_t)video * T, s));
-        // then the video restarts as rf_tracker_reset restarts it
-        CK(cudaMemsetAsync(t->d_videos + video, 0, sizeof(TrackVideo), s));
-        CK(cudaMemsetAsync(t->d_state + (size_t)video * T, 0, sizeof(TrackState) * T, s));
-        CK(cudaMemsetAsync(b.store + (size_t)video * T, 0, sizeof(BestEntry) * T, s));
-        CK(cudaMemsetAsync(b.videos + video, 0, sizeof(BestVideo), s));
-        if (t->motion) t->mref[video] = {0, 0};
-        CK(cudaEventRecord(t->chain, s));
-        CK(cudaEventRecord(slot.free, s));
-        if (dev_best) *dev_best = b.best;
-        if (dev_best_count) *dev_best_count = b.best_counts;
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    return RF_OK;
-}
-
-int rf_tracker_set_motion(rf_tracker t, const rf_motion_config *cfg) {
-    static const char *who = "rf_tracker_set_motion";
-    if (!t) return RF_ERR_INVALID_ARG;
-    rf_handle h = t->h;
-    if (!cfg) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL config", who));
-    if (t->motion) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: motion is already on", who));
-    if (t->updated) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker has already been updated", who));
-    const int R = cfg->search ? cfg->search : 12, mi = cfg->min_inliers ? cfg->min_inliers : 12;
-    if (R < 1 || R > MOTION_MAX_R) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: search %d, must be 0 or in [1, %d]", who, cfg->search, MOTION_MAX_R));
-    if (mi < 3 || mi > MOTION_MAX_BLOCKS)
-        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: min_inliers %d, must be 0 or in [3, %d]", who, cfg->min_inliers, MOTION_MAX_BLOCKS));
-    const size_t V = t->cfg.max_videos, B = h->cfg.max_batch;
-    if (V * MOTION_THUMB_BYTES > ((size_t)4 << 30))
-        return fail(h, RF_ERR_CAPACITY, fmt("%s: a store of %zu videos x %d bytes exceeds 4 GiB", who, V, MOTION_THUMB_BYTES));
-    try {
-        CK(cudaSetDevice(h->device));
-        CK(cudaMalloc(&t->d_mstore, V * MOTION_THUMB_BYTES));
-        CK(cudaMalloc(&t->d_mthumbs, B * MOTION_THUMB_BYTES));
-        CK(cudaMalloc(&t->d_mblocks, sizeof(MotionBlock) * B * MOTION_MAX_BLOCKS));
-        for (auto &s : t->slots) CK(cudaMalloc(&s.motion, sizeof(rf_motion) * B));
-    } catch (const CudaFail &f) {
-        cudaFree(t->d_mstore); cudaFree(t->d_mthumbs); cudaFree(t->d_mblocks);
-        t->d_mstore = t->d_mthumbs = nullptr;
-        t->d_mblocks = nullptr;
-        for (auto &s : t->slots) { cudaFree(s.motion); s.motion = nullptr; }
-        return fail_cuda(h, f);
-    }
-    t->motion = true;
-    t->mcfg = rf_motion_config{R, mi};
-    t->mref.assign(V, {0, 0});
-    return RF_OK;
-}
-
-int rf_tracker_motion(rf_tracker t, const rf_motion **dev_motion) {
-    if (!t) return RF_ERR_INVALID_ARG;
-    if (!dev_motion) return fail(t->h, RF_ERR_INVALID_ARG, "rf_tracker_motion: dev_motion is NULL");
-    if (!t->motion) return fail(t->h, RF_ERR_INVALID_ARG, "rf_tracker_motion: motion is off (rf_tracker_set_motion)");
-    *dev_motion = t->motion_slot < 0 ? nullptr : t->slots[t->motion_slot].motion;
-    return RF_OK;
-}
-
-int rf_tracker_set_follow(rf_tracker t, const rf_follow_config *cfg) {
-    static const char *who = "rf_tracker_set_follow";
-    if (!t) return RF_ERR_INVALID_ARG;
-    rf_handle h = t->h;
-    if (!cfg) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL config", who));
-    if (t->best) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a best-shot tracker cannot follow", who));
-    if (t->lookback) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a look-back tracker cannot follow", who));
-    if (t->follow) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: following is already on", who));
-    if (t->updated) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker has already been updated", who));
-    const int R = cfg->search ? cfg->search : 8;
-    const float mad = cfg->max_mad != 0.f ? cfg->max_mad : 24.f;
-    if (R < 1 || R > FOLLOW_MAX_R) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: search %d, must be 0 or in [1, %d]", who, cfg->search, FOLLOW_MAX_R));
-    if (!(std::isfinite(mad) && mad > 0.f && mad <= 255.f))
-        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: max_mad %g, must be 0 or finite in (0, 255]", who, (double)cfg->max_mad));
-    const size_t V = t->cfg.max_videos, T = t->cfg.max_tracks, B = h->cfg.max_batch;
-    if (V * T * FOLLOW_BYTES > ((size_t)4 << 30))
-        return fail(h, RF_ERR_CAPACITY, fmt("%s: a store of %zu videos x %zu tracks x %d bytes exceeds 4 GiB", who, V, T, FOLLOW_BYTES));
-    try {
-        CK(cudaSetDevice(h->device));
-        CK(cudaMalloc(&t->d_fstore, V * T * FOLLOW_BYTES));
-        CK(cudaMalloc(&t->d_fentries, sizeof(FollowEntry) * V * T));
-        CK(cudaMalloc(&t->d_fmeas, sizeof(FollowMeas) * B * T));
-        CK(cudaMalloc(&t->d_follow, sizeof(rf_follow) * t->slots.size() * B * T));
-        CK(cudaMalloc(&t->d_fregions, sizeof(rf_det) * t->slots.size() * B * T));
-        CK(cudaMalloc(&t->d_fregion_counts, sizeof(int) * t->slots.size() * B));
-        CK(cudaMalloc(&t->d_fmask, sizeof(rf_det) * B * T));
-        CK(cudaMalloc(&t->d_fmask_counts, sizeof(int) * B));
-        CK(cudaMemset(t->d_fentries, 0, sizeof(FollowEntry) * V * T));
-        CK(cudaDeviceSynchronize());
-    } catch (const CudaFail &f) {
-        cudaFree(t->d_fstore); cudaFree(t->d_fentries); cudaFree(t->d_fmeas); cudaFree(t->d_follow);
-        cudaFree(t->d_fregions); cudaFree(t->d_fregion_counts); cudaFree(t->d_fmask); cudaFree(t->d_fmask_counts);
-        t->d_fstore = nullptr;
-        t->d_fentries = nullptr;
-        t->d_fmeas = nullptr;
-        t->d_follow = nullptr;
-        t->d_fregions = t->d_fmask = nullptr;
-        t->d_fregion_counts = t->d_fmask_counts = nullptr;
-        return fail_cuda(h, f);
-    }
-    t->follow = true;
-    t->fcfg = rf_follow_config{R, mad};
-    return RF_OK;
-}
-
-// Everything a follow call refuses, checked before anything is launched.
-static int check_follow(rf_tracker t, const char *who, const rf_yuv_frame *frames, const int *videos, int n) {
-    if (!t->follow) return fail(t->h, RF_ERR_INVALID_ARG, fmt("%s: not a follow tracker (rf_tracker_set_follow)", who));
-    int rc = check_track_args(t, who, videos, n, nullptr);
-    if (rc) return rc;
-    return check_frames(t->h, who, frames, n, RF_YUV_BT601);
-}
-
-// Issues the follow step of n frames on s into the next ring slot, ordered by the chain.  In rounds -- the r-th frame of every video
-// of the call, then the next -- so that each frame is searched from the state its video's previous frame left; with motion, each
-// round first masks the tracks' faces and estimates its frames' motion (the reference: the video's previous frame of the call, else
-// its stored thumbnail), and each video's last thumbnail of the call becomes its reference afterwards.  Returns the ring slot.
-static unsigned follow_issue(rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, cudaStream_t s) {
-    rf_handle h = t->h;
-    const unsigned ring = t->next_slot++ % t->slots.size();
-    rf_tracker_s::Slot &slot = t->slots[ring];
-    const size_t T = t->cfg.max_tracks, B = h->cfg.max_batch;
-    CK(cudaStreamWaitEvent(s, slot.free, 0));
-    CK(cudaStreamWaitEvent(s, t->chain, 0));
-    t->updated = true;
-    FollowArgs f = follow_args(t);
-    f.follow = t->d_follow + ring * B * T;
-    f.tracks = slot.tracks;
-    f.track_counts = slot.counts;
-    f.regions = t->d_fregions + ring * B * T;
-    f.region_counts = t->d_fregion_counts + ring * B;
-    std::vector<int> round(n);
-    int rounds = 0;
-    for (int i = 0; i < n; i++) {
-        int r = 0;
-        for (int k = 0; k < i; k++) r += videos[k] == videos[i];
-        round[i] = r;
-        rounds = std::max(rounds, r + 1);
-    }
-    // f13: one single-frame table per frame, so that a frame's thumbnail, blocks and motion sit at its index in the call
-    std::vector<MotionTable> mt(t->motion ? n : 0);
-    MotionCommits commits;
-    MotionArgs ma{};
-    if (t->motion) {
-        const int R = t->mcfg.search;
-        std::vector<int> last(t->cfg.max_videos, -1);
-        for (int i = 0; i < n; i++) {
-            const rf_yuv_frame &fr = frames[i];
-            const int v = videos[i];
-            MotionTable &tb = mt[i];
-            tb.i0 = i;
-            tb.n = 1;
-            MotionFrame &mf = tb.f[0];
-            mf.y = fr.y;
-            mf.pitch = fr.y_pitch;
-            mf.video = v;
-            mf.scale = 1.f;
-            mf.D = (std::max(fr.width, fr.height) + MOTION_THUMB - 1) / MOTION_THUMB;
-            mf.tw = fr.width / mf.D;
-            mf.th = fr.height / mf.D;
-            mf.nbx = mf.tw - 2 * R >= MOTION_BLOCK ? (mf.tw - 2 * R) / MOTION_BLOCK : 0;
-            mf.nby = mf.th - 2 * R >= MOTION_BLOCK ? (mf.th - 2 * R) / MOTION_BLOCK : 0;
-            const std::array<int, 2> size = {fr.width, fr.height};
-            if (last[v] >= 0) {
-                const rf_yuv_frame &p = frames[last[v]];
-                mf.ref = p.width == fr.width && p.height == fr.height ? last[v] : MOTION_REF_FIRST;
-            } else {
-                mf.ref = t->mref[v] == size ? MOTION_REF_STORE : MOTION_REF_FIRST;
-            }
-            last[v] = i;
-        }
-        for (int v = 0; v < t->cfg.max_videos; v++) {
-            if (last[v] < 0) continue;
-            t->mref[v] = {frames[last[v]].width, frames[last[v]].height};
-            commits.frames.push_back(last[v]);
-            commits.videos.push_back(v);
-            commits.bytes.push_back(mt[last[v]].f[0].tw * mt[last[v]].f[0].th);
-        }
-        ma.thumbs = t->d_mthumbs;
-        ma.store = t->d_mstore;
-        ma.blocks = t->d_mblocks;
-        ma.out = slot.motion;
-        ma.dets = t->d_fmask;
-        ma.counts = t->d_fmask_counts;
-        ma.max_faces = (int)T;
-        ma.search = R;
-        ma.min_inliers = t->mcfg.min_inliers;
-        f.motion = slot.motion;
-        f.mask = t->d_fmask;
-        f.mask_counts = t->d_fmask_counts;
-        t->motion_slot = (int)ring;
-    }
-    for (int r = 0; r < rounds; r++) {
-        FollowTable tab{};
-        std::vector<MotionTable> rt;
-        auto flush = [&]() {
-            if (!tab.n) return;
-            if (t->motion) {
-                CK(launch_follow_mask(f, tab, s));
-                CK(launch_motion_estimate(ma, rt.data(), (int)rt.size(), s));
-            }
-            CK(launch_follow_round(f, tab, s));
-            tab.n = 0;
-            rt.clear();
-        };
-        for (int i = 0; i < n; i++) {
-            if (round[i] != r) continue;
-            tab.f[tab.n++] = follow_frame(frames[i], videos[i], i);
-            if (t->motion) rt.push_back(mt[i]);
-            if (tab.n == TRACK_MAX_FRAMES) flush();
-        }
-        flush();
-    }
-    if (t->motion) motion_commit(t, commits, s);
-    CK(cudaEventRecord(t->chain, s));
-    t->follow_slot = (int)ring;
-    return ring;
-}
-
-int rf_track_follow_device(rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, const rf_track **dev_tracks,
-                           const int32_t **dev_track_counts) {
-    static const char *who = "rf_track_follow_device";
-    if (!t) return RF_ERR_INVALID_ARG;
-    rf_handle h = t->h;
-    int rc = check_follow(t, who, frames, videos, n);
-    if (rc) return rc;
-    if (n == 0) return RF_OK;
-    try {
-        CK(cudaSetDevice(h->device));
-        cudaStream_t s = (cudaStream_t)rf_last_stream(h);
-        const unsigned ring = follow_issue(t, frames, videos, n, s);
-        rf_tracker_s::Slot &slot = t->slots[ring];
-        CK(cudaEventRecord(slot.free, s));
-        if (dev_tracks) *dev_tracks = slot.tracks;
-        if (dev_track_counts) *dev_track_counts = slot.counts;
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    return RF_OK;
-}
-
-int rf_tracker_follow(rf_tracker t, const rf_follow **dev_follow) {
-    if (!t) return RF_ERR_INVALID_ARG;
-    if (!dev_follow) return fail(t->h, RF_ERR_INVALID_ARG, "rf_tracker_follow: dev_follow is NULL");
-    if (!t->follow) return fail(t->h, RF_ERR_INVALID_ARG, "rf_tracker_follow: not a follow tracker (rf_tracker_set_follow)");
-    const size_t T = t->cfg.max_tracks, B = t->h->cfg.max_batch;
-    *dev_follow = t->follow_slot < 0 ? nullptr : t->d_follow + (size_t)t->follow_slot * B * T;
-    return RF_OK;
-}
-
-int rf_tracker_debug_state(rf_tracker t, int video, double *out, int cap) {
-    static const char *who = "rf_tracker_debug_state";
-    if (!t) return RF_ERR_INVALID_ARG;
-    rf_handle h = t->h;
-    if (video < 0 || video >= t->cfg.max_videos) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: video %d, must be in [0, %d)", who, video, t->cfg.max_videos));
-    if (cap > 0 && !out) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: out is NULL", who));
-    const int T = t->cfg.max_tracks;
-    TrackVideo hv{};
-    std::vector<TrackState> st(T);
-    try {
-        CK(cudaSetDevice(h->device));
-        CK(cudaEventSynchronize(t->chain));
-        CK(cudaMemcpy(&hv, t->d_videos + video, sizeof hv, cudaMemcpyDeviceToHost));
-        CK(cudaMemcpy(st.data(), t->d_state + (size_t)video * T, sizeof(TrackState) * T, cudaMemcpyDeviceToHost));
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    std::vector<const TrackState *> live;
-    for (const TrackState &k : st) if (k.id) live.push_back(&k);
-    std::sort(live.begin(), live.end(), [](const TrackState *x, const TrackState *y) { return x->id < y->id; });
-    std::vector<double> v = {(double)live.size(), (double)(hv.issued + 1), (double)hv.frames, (double)hv.overflow};
-    for (const TrackState *k : live) {
-        for (int x : {k->id, k->state, k->hits, k->age, k->lost}) v.push_back(x);
-        for (const double *arr : {k->m, k->u, k->p00, k->p01, k->p11}) v.insert(v.end(), arr, arr + 4);
-    }
-    std::copy(v.begin(), v.begin() + std::min<size_t>(v.size(), (size_t)std::max(cap, 0)), out);
-    return (int)live.size();
-}
-
-// ---- f12 redaction (redact.cuh) -------------------------------------------------------------------------------------------------
-extern "C++" {
-// A call's resolved style: f12's params are {MOSAIC, RECT, blocks, detail 0}.
-struct RedactSpec {
-    int kind = REDACT_MOSAIC, shape = REDACT_RECT, blocks = 8, detail = 0;
-    double margin = 0.25;
-};
-
-static int redact_margin(rf_handle h, const char *who, float margin, double &out) {
-    const float m = margin != 0.f ? margin : 0.25f;
-    if (!(std::isfinite(m) && m > 0.f && m <= 1.f))
-        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: margin %g, must be 0 or finite in (0, 1]", who, (double)m));
-    out = (double)m;
-    return RF_OK;
-}
-
-// params (NULL: defaults) -> blocks and margin
-static int redact_params(rf_handle h, const char *who, const rf_redact_params *p, RedactSpec &r) {
-    r = RedactSpec{};
-    r.blocks = p && p->blocks ? p->blocks : 8;
-    if (r.blocks < 1 || r.blocks > REDACT_MAX_BLOCKS)
-        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: blocks %d, must be 0 or in [1, %d]", who, r.blocks, REDACT_MAX_BLOCKS));
-    return redact_margin(h, who, p ? p->margin : 0.f, r.margin);
-}
-
-// style (NULL: the zeroed struct) -> kind, shape, blocks, detail and margin
-static int redact_style(rf_handle h, const char *who, const rf_redact_style *st, RedactSpec &r) {
-    const rf_redact_style z{};
-    if (!st) st = &z;
-    r = RedactSpec{};
-    r.kind = st->kind ? st->kind : REDACT_BLUR;
-    r.shape = st->shape ? st->shape : REDACT_ELLIPSE;
-    if (r.kind != REDACT_MOSAIC && r.kind != REDACT_BLUR)
-        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: kind %d, must be 0, RF_REDACT_MOSAIC or RF_REDACT_BLUR", who, st->kind));
-    if (r.shape != REDACT_RECT && r.shape != REDACT_ELLIPSE)
-        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: shape %d, must be 0, RF_REDACT_RECT or RF_REDACT_ELLIPSE", who, st->shape));
-    if (r.kind == REDACT_MOSAIC) {
-        if (st->detail) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: detail %d, must be 0 for the mosaic", who, st->detail));
-        r.blocks = st->blocks ? st->blocks : 8;
-        if (r.blocks < 1 || r.blocks > REDACT_MAX_BLOCKS)
-            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: blocks %d, must be 0 or in [1, %d]", who, r.blocks, REDACT_MAX_BLOCKS));
-    } else {
-        if (st->blocks) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: blocks %d, must be 0 for the blur", who, st->blocks));
-        r.blocks = 1;         // the geometry's cell side, unused by the blur
-        r.detail = st->detail ? st->detail : 4;
-        if (r.detail < 1 || r.detail > BLUR_MAX_DETAIL)
-            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: detail %d, must be 0 or in [1, %d]", who, r.detail, BLUR_MAX_DETAIL));
-    }
-    return redact_margin(h, who, st->margin, r.margin);
-}
-
-// The records, scales and tracks of a redaction call.
-static int check_redact_inputs(rf_handle h, const char *who, int n, const rf_det *dets, const int32_t *counts, const float *scales, rf_tracker t,
-                               const rf_track *tracks, const int32_t *track_counts) {
-    if (n > 0 && (!dets || !counts)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL records or counts", who));
-    const bool any = t || tracks || track_counts;
-    if (any && !(t && tracks && track_counts))
-        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker, its tracks and their counts go together (all three or none)", who));
-    if (t && t->h != h) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker belongs to another handle", who));
-    for (int i = 0; scales && i < n; i++)
-        if (!(std::isfinite(scales[i]) && scales[i] > 0.f))
-            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frame %d: scale %g, must be finite and positive", who, i, (double)scales[i]));
-    return RF_OK;
-}
-
-// Refuses two frames whose plane byte ranges overlap: a later chunk's measure would read pixels an earlier chunk has written, and
-// within a chunk two regions' writes could land on one byte.  ranges: (first byte, one past the last, frame).  A sweep in address
-// order that keeps the furthest end seen (and the furthest end of any other frame) finds every overlap of two frames.
-static int check_disjoint(rf_handle h, const char *who, std::vector<std::array<uintptr_t, 3>> ranges) {
-    std::sort(ranges.begin(), ranges.end());
-    uintptr_t end1 = 0, end2 = 0;
-    uintptr_t frame1 = ~(uintptr_t)0;        // end1: the furthest end, of frame1; end2: the furthest end of any other frame
-    for (const auto &r : ranges) {
-        const uintptr_t other = r[2] == frame1 ? end2 : end1;
-        if (r[0] < other) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frame %d overlaps the bytes of another frame of the call", who, (int)r[2]));
-        if (r[1] > end1) {
-            if (r[2] != frame1) { end2 = end1; frame1 = r[2]; }
-            end1 = r[1];
-        } else if (r[2] != frame1 && r[1] > end2) {
-            end2 = r[1];
-        }
-    }
-    return RF_OK;
-}
-
-static std::vector<std::array<uintptr_t, 3>> yuv_ranges(const rf_yuv_frame *frames, int n) {
-    std::vector<std::array<uintptr_t, 3>> r;
-    for (int i = 0; i < n; i++) {
-        const rf_yuv_frame &f = frames[i];
-        const uintptr_t y = (uintptr_t)f.y, u = (uintptr_t)f.u, v = (uintptr_t)f.v, ch = f.height / 2 - 1;
-        r.push_back({y, y + (uintptr_t)(f.height - 1) * f.y_pitch + f.width, (uintptr_t)i});
-        if (f.uv_step == 2) {
-            const uintptr_t lo = std::min(u, v);
-            r.push_back({lo, lo + ch * f.uv_pitch + f.width, (uintptr_t)i});
-        } else {
-            r.push_back({u, u + ch * f.uv_pitch + f.width / 2, (uintptr_t)i});
-            r.push_back({v, v + ch * f.uv_pitch + f.width / 2, (uintptr_t)i});
-        }
-    }
-    return r;
-}
-
-static Ctx &last_ctx(rf_handle h) {
-    for (Ctx &c : h->ctx)
-        if (c.stream == h->last_stream) return c;
-    return h->ctx[0];
-}
-
-// Issues the redaction of `frames` on context c's stream, into c's scratch (sized for max_batch frames -- or more, for a drain -- of
-// this call's region capacity and blocks, and for BLUR the frames' scratch planes; a larger need waits for the context before the
-// scratch is replaced).  records: the records per frame of dets (0: max_faces; f15's look-back regions have more).
-template <typename Dst>
-static void redact_issue(rf_handle h, Ctx &c, std::vector<RedactFrameT<Dst>> frames, const rf_det *dets, const int32_t *counts, rf_tracker t,
-                         const rf_track *tracks, const int32_t *track_counts, const RedactSpec &spec, int records = 0) {
-    RedactArgs a{};
-    a.n = (int)frames.size();
-    a.blocks = spec.blocks;
-    a.margin = spec.margin;
-    a.kind = spec.kind;
-    a.shape = spec.shape;
-    a.detail = spec.detail;
-    a.max_faces = records ? records : h->cfg.max_faces;
-    a.max_tracks = t ? t->cfg.max_tracks : 0;
-    a.cap = a.max_faces + a.max_tracks;
-    a.dets = dets;
-    a.counts = counts;
-    a.tracks = tracks;
-    a.track_counts = track_counts;
-    const size_t tables = (redact_scratch_bytes(std::max(h->cfg.max_batch, a.n), a.cap, a.blocks) + 255) & ~(size_t)255;
-    size_t need = tables;
-    if (spec.kind == REDACT_BLUR)
-        for (const auto &f : frames) need += (blur_plane_bytes(std::is_same<Dst, YuvPlanesW>::value, f.w, f.h) + 255) & ~(size_t)255;
-    if (need > c.redact_bytes) {
-        CK(cudaStreamSynchronize(c.stream));
-        CK(cudaFree(c.d_redact));
-        c.d_redact = nullptr;
-        c.redact_bytes = 0;
-        CK(cudaMalloc(&c.d_redact, need));
-        c.redact_bytes = need;
-    }
-    redact_carve(a, c.d_redact);
-    if (spec.kind == REDACT_BLUR) {
-        size_t off = tables;
-        for (auto &f : frames) {
-            f.blur = static_cast<uint8_t *>(c.d_redact) + off;
-            off += (blur_plane_bytes(std::is_same<Dst, YuvPlanesW>::value, f.w, f.h) + 255) & ~(size_t)255;
-        }
-    }
-    CK(launch_redact(a, frames.data(), h->num_sms, c.stream));
-}
-
-static std::vector<RedactFrameT<YuvPlanesW>> yuv_redact_table(const rf_yuv_frame *frames, int n, const float *scales) {
-    std::vector<RedactFrameT<YuvPlanesW>> v(n);
-    for (int i = 0; i < n; i++) {
-        const rf_yuv_frame &f = frames[i];
-        v[i] = RedactFrameT<YuvPlanesW>{YuvPlanesW{const_cast<uint8_t *>(f.y), const_cast<uint8_t *>(f.u), const_cast<uint8_t *>(f.v), f.y_pitch,
-                                                   f.uv_pitch, f.uv_step},
-                                        f.width, f.height, scales ? scales[i] : 1.f, nullptr};
-    }
-    return v;
-}
-}  // extern "C++"
-
-extern "C++" {
-// The f12 and f14 entry points share one implementation each: `resolve` checks the params or the style where f12 checks its params.
-template <typename Resolve>
-static int redact_yuv_impl(rf_handle h, const char *who, const rf_yuv_frame *frames, int n, const rf_det *dev_dets, const int32_t *dev_counts,
-                           const float *scales, rf_tracker t, const rf_track *dev_tracks, const int32_t *dev_track_counts, Resolve resolve) {
-    if (!h) return RF_ERR_INVALID_ARG;
-    int rc = check_frames(h, who, frames, n, RF_YUV_BT601);      // the matrix plays no part: the mosaic is per plane
-    if (rc) return rc;
-    RedactSpec spec;
-    if ((rc = resolve(spec))) return rc;
-    if ((rc = check_redact_inputs(h, who, n, dev_dets, dev_counts, scales, t, dev_tracks, dev_track_counts))) return rc;
-    if ((rc = check_disjoint(h, who, yuv_ranges(frames, n)))) return rc;
-    if (n == 0) return RF_OK;
-    try {
-        CK(cudaSetDevice(h->device));
-        redact_issue(h, last_ctx(h), yuv_redact_table(frames, n, scales), dev_dets, dev_counts, t, dev_tracks, dev_track_counts, spec);
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    return RF_OK;
-}
-
-template <typename Resolve>
-static int redact_bgr_impl(rf_handle h, const char *who, uint8_t *const *dev_bgr, const int *widths, const int *heights, const int *row_strides,
-                           int n, const rf_det *dev_dets, const int32_t *dev_counts, const float *scales, rf_tracker t, const rf_track *dev_tracks,
-                           const int32_t *dev_track_counts, Resolve resolve) {
-    if (!h) return RF_ERR_INVALID_ARG;
-    const BgrImages src{dev_bgr, widths, heights, row_strides, nullptr, false};
-    int rc = src.check(h, who, n);
-    if (rc) return rc;
-    RedactSpec spec;
-    if ((rc = resolve(spec))) return rc;
-    if ((rc = check_redact_inputs(h, who, n, dev_dets, dev_counts, scales, t, dev_tracks, dev_track_counts))) return rc;
-    std::vector<std::array<uintptr_t, 3>> ranges;
-    for (int i = 0; i < n; i++) {
-        const uintptr_t p = (uintptr_t)dev_bgr[i];
-        ranges.push_back({p, p + (uintptr_t)(heights[i] - 1) * src.stride(i) + 3 * (uintptr_t)widths[i], (uintptr_t)i});
-    }
-    if ((rc = check_disjoint(h, who, ranges))) return rc;
-    if (n == 0) return RF_OK;
-    try {
-        CK(cudaSetDevice(h->device));
-        std::vector<RedactFrameT<BgrRowsW>> v(n);
-        for (int i = 0; i < n; i++) v[i] = RedactFrameT<BgrRowsW>{BgrRowsW{dev_bgr[i], src.stride(i)}, widths[i], heights[i], scales ? scales[i] : 1.f, nullptr};
-        redact_issue(h, last_ctx(h), v, dev_dets, dev_counts, t, dev_tracks, dev_track_counts, spec);
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    return RF_OK;
-}
-
-template <typename Resolve>
-static int detect_yuv_redact_impl(rf_handle h, const char *who, rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, int matrix,
-                                  float thr, float nms, Resolve resolve, const rf_track **dev_tracks, const int32_t **dev_track_counts,
-                                  const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales) {
-    if (!h) return RF_ERR_INVALID_ARG;
-    int rc;
-    if (t) {
-        if (t->h != h) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker belongs to another handle", who));
-        if (t->best) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a best-shot tracker takes frames only through rf_detect_yuv_track_best_device", who));
-        if (t->lookback)
-            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a look-back tracker takes frames only through rf_detect_yuv_redact_lookback_device", who));
-        if ((rc = check_track_args(t, who, videos, n, nullptr))) return rc;
-    }
-    const YuvFrames src{frames, matrix, nullptr, false};
-    if ((rc = src.check(h, who, n))) return rc;
-    RedactSpec spec;
-    if ((rc = resolve(spec))) return rc;
-    if ((rc = check_disjoint(h, who, yuv_ranges(frames, n)))) return rc;
-    if (n == 0) return RF_OK;
-    std::vector<float> scales(n);
-    const rf_det *dets = nullptr;
-    const int32_t *counts = nullptr;
-    if ((rc = yuv_device_impl(h, who, src, n, thr, nms, nullptr, nullptr, nullptr, &dets, &counts, scales.data()))) return rc;
-    if (dev_dets) *dev_dets = dets;
-    if (dev_counts) *dev_counts = counts;
-    if (out_scales) std::copy(scales.begin(), scales.end(), out_scales);
-    try {
-        Ctx &c = last_ctx(h);          // the forward's context
-        const rf_track *tracks = nullptr;
-        const int32_t *track_counts = nullptr;
-        if (t) track_issue(t, videos, n, dets, counts, scales.data(), c.stream, nullptr, nullptr, &tracks, &track_counts, frames);
-        if (dev_tracks) *dev_tracks = tracks;
-        if (dev_track_counts) *dev_track_counts = track_counts;
-        redact_issue(h, c, yuv_redact_table(frames, n, scales.data()), dets, counts, t, tracks, track_counts, spec);
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    return RF_OK;
-}
-
-}  // extern "C++"
-
-int rf_redact_yuv_device(rf_handle h, const rf_yuv_frame *frames, int n, const rf_det *dev_dets, const int32_t *dev_counts, const float *scales,
-                         rf_tracker t, const rf_track *dev_tracks, const int32_t *dev_track_counts, const rf_redact_params *params) {
-    static const char *who = "rf_redact_yuv_device";
-    return redact_yuv_impl(h, who, frames, n, dev_dets, dev_counts, scales, t, dev_tracks, dev_track_counts,
-                           [&](RedactSpec &r) { return redact_params(h, who, params, r); });
-}
-
-int rf_redact_yuv_device_style(rf_handle h, const rf_yuv_frame *frames, int n, const rf_det *dev_dets, const int32_t *dev_counts, const float *scales,
-                               rf_tracker t, const rf_track *dev_tracks, const int32_t *dev_track_counts, const rf_redact_style *style) {
-    static const char *who = "rf_redact_yuv_device_style";
-    return redact_yuv_impl(h, who, frames, n, dev_dets, dev_counts, scales, t, dev_tracks, dev_track_counts,
-                           [&](RedactSpec &r) { return redact_style(h, who, style, r); });
-}
-
-int rf_redact_device(rf_handle h, uint8_t *const *dev_bgr, const int *widths, const int *heights, const int *row_strides, int n,
-                     const rf_det *dev_dets, const int32_t *dev_counts, const float *scales, rf_tracker t, const rf_track *dev_tracks,
-                     const int32_t *dev_track_counts, const rf_redact_params *params) {
-    static const char *who = "rf_redact_device";
-    return redact_bgr_impl(h, who, dev_bgr, widths, heights, row_strides, n, dev_dets, dev_counts, scales, t, dev_tracks, dev_track_counts,
-                           [&](RedactSpec &r) { return redact_params(h, who, params, r); });
-}
-
-int rf_redact_device_style(rf_handle h, uint8_t *const *dev_bgr, const int *widths, const int *heights, const int *row_strides, int n,
-                           const rf_det *dev_dets, const int32_t *dev_counts, const float *scales, rf_tracker t, const rf_track *dev_tracks,
-                           const int32_t *dev_track_counts, const rf_redact_style *style) {
-    static const char *who = "rf_redact_device_style";
-    return redact_bgr_impl(h, who, dev_bgr, widths, heights, row_strides, n, dev_dets, dev_counts, scales, t, dev_tracks, dev_track_counts,
-                           [&](RedactSpec &r) { return redact_style(h, who, style, r); });
-}
-
-int rf_detect_yuv_redact_device(rf_handle h, rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, int matrix, float thr, float nms,
-                                const rf_redact_params *params, const rf_track **dev_tracks, const int32_t **dev_track_counts,
-                                const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales) {
-    static const char *who = "rf_detect_yuv_redact_device";
-    return detect_yuv_redact_impl(h, who, t, frames, videos, n, matrix, thr, nms, [&](RedactSpec &r) { return redact_params(h, who, params, r); },
-                                  dev_tracks, dev_track_counts, dev_dets, dev_counts, out_scales);
-}
-
-int rf_detect_yuv_redact_device_style(rf_handle h, rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, int matrix, float thr,
-                                      float nms, const rf_redact_style *style, const rf_track **dev_tracks, const int32_t **dev_track_counts,
-                                      const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales) {
-    static const char *who = "rf_detect_yuv_redact_device_style";
-    return detect_yuv_redact_impl(h, who, t, frames, videos, n, matrix, thr, nms, [&](RedactSpec &r) { return redact_style(h, who, style, r); },
-                                  dev_tracks, dev_track_counts, dev_dets, dev_counts, out_scales);
-}
-
-int rf_track_follow_redact_device(rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, const rf_redact_style *style,
-                                  const rf_track **dev_tracks, const int32_t **dev_track_counts) {
-    static const char *who = "rf_track_follow_redact_device";
-    if (!t) return RF_ERR_INVALID_ARG;
-    rf_handle h = t->h;
-    int rc = check_follow(t, who, frames, videos, n);
-    if (rc) return rc;
-    RedactSpec spec;
-    if ((rc = redact_style(h, who, style, spec))) return rc;
-    if ((rc = check_disjoint(h, who, yuv_ranges(frames, n)))) return rc;
-    if (n == 0) return RF_OK;
-    try {
-        CK(cudaSetDevice(h->device));
-        Ctx &c = last_ctx(h);
-        const unsigned ring = follow_issue(t, frames, videos, n, c.stream);
-        rf_tracker_s::Slot &slot = t->slots[ring];
-        const size_t T = t->cfg.max_tracks, B = h->cfg.max_batch;
-        // (a) the OK-followed faces in id order, (b) the LOST tracks of the lists: f12's geometry, f14's styles and ownership
-        redact_issue(h, c, yuv_redact_table(frames, n, nullptr), t->d_fregions + ring * B * T, t->d_fregion_counts + ring * B, t, slot.tracks,
-                     slot.counts, spec, (int)T);
-        CK(cudaEventRecord(slot.free, c.stream));
-        if (dev_tracks) *dev_tracks = slot.tracks;
-        if (dev_track_counts) *dev_track_counts = slot.counts;
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    return RF_OK;
-}
-
-// ---- f15 look-back redaction (lookback.cuh) --------------------------------------------------------------------------------------
-int rf_tracker_set_lookback(rf_tracker t, const rf_lookback_config *cfg) {
-    static const char *who = "rf_tracker_set_lookback";
-    if (!t) return RF_ERR_INVALID_ARG;
-    rf_handle h = t->h;
-    if (!cfg) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL config", who));
-    if (t->best) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a best-shot tracker cannot look back", who));
-    if (t->lookback) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: look-back is already on", who));
-    if (t->follow) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: a follow tracker cannot look back", who));
-    if (t->updated) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker has already been updated", who));
-    const int L = cfg->frames ? cfg->frames : 15;
-    const float grow = cfg->grow != 0.f ? cfg->grow : 0.1f;
-    if (L < 1 || L > LOOKBACK_MAX_L) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frames %d, must be 0 or in [1, %d]", who, cfg->frames, LOOKBACK_MAX_L));
-    if (!(std::isfinite(grow) && grow > 0.f && grow <= 1.f))
-        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: grow %g, must be 0 or finite in (0, 1]", who, (double)cfg->grow));
-    const size_t rows = std::max(h->cfg.max_batch, L), recs = lookback_records(h->cfg.max_faces, t->cfg.max_tracks, L, false);
-    try {
-        CK(cudaSetDevice(h->device));
-        for (auto &s : t->slots) {
-            CK(cudaMalloc(&s.lb_boxes, sizeof(rf_det) * rows * recs));
-            CK(cudaMalloc(&s.lb_counts, sizeof(int) * rows));
-        }
-    } catch (const CudaFail &f) {
-        for (auto &s : t->slots) {
-            cudaFree(s.lb_boxes); cudaFree(s.lb_counts);
-            s.lb_boxes = nullptr;
-            s.lb_counts = nullptr;
-        }
-        return fail_cuda(h, f);
-    }
-    t->lookback = true;
-    t->lb_frames = L;
-    t->lb_grow = grow;
-    t->lbv.assign(t->cfg.max_videos, {});
-    return RF_OK;
-}
-
-int rf_tracker_set_lookback_search(rf_tracker t, const rf_follow_config *cfg) {
-    static const char *who = "rf_tracker_set_lookback_search";
-    if (!t) return RF_ERR_INVALID_ARG;
-    rf_handle h = t->h;
-    if (!cfg) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL config", who));
-    if (!t->lookback) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: not a look-back tracker (rf_tracker_set_lookback)", who));
-    if (t->lb_search) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the look-back search is already on", who));
-    if (t->updated) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker has already been updated", who));
-    const int R = cfg->search ? cfg->search : 8;
-    const float mad = cfg->max_mad != 0.f ? cfg->max_mad : 24.f;
-    if (R < 1 || R > FOLLOW_MAX_R) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: search %d, must be 0 or in [1, %d]", who, cfg->search, FOLLOW_MAX_R));
-    if (!(std::isfinite(mad) && mad > 0.f && mad <= 255.f))
-        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: max_mad %g, must be 0 or finite in (0, 255]", who, (double)cfg->max_mad));
-    const int L = t->lb_frames;
-    const size_t B = h->cfg.max_batch, bcap = std::min(h->cfg.max_faces, t->cfg.max_tracks);
-    const size_t rows = std::max(h->cfg.max_batch, L), recs = lookback_records(h->cfg.max_faces, t->cfg.max_tracks, L, true);
-    std::vector<rf_tracker_s::Slot> grown(t->slots.size());
-    try {
-        CK(cudaSetDevice(h->device));
-        for (auto &s : grown) {
-            CK(cudaMalloc(&s.lb_boxes, sizeof(rf_det) * rows * recs));
-            CK(cudaMalloc(&s.lb_steps, sizeof(rf_follow) * B * bcap * L));
-            CK(cudaMalloc(&s.lb_lengths, sizeof(int) * B * bcap));
-        }
-    } catch (const CudaFail &f) {
-        for (auto &s : grown) { cudaFree(s.lb_boxes); cudaFree(s.lb_steps); cudaFree(s.lb_lengths); }
-        return fail_cuda(h, f);
-    }
-    for (size_t i = 0; i < t->slots.size(); i++) {     // no call has used the ring's region records yet
-        cudaFree(t->slots[i].lb_boxes);
-        t->slots[i].lb_boxes = grown[i].lb_boxes;
-        t->slots[i].lb_steps = grown[i].lb_steps;
-        t->slots[i].lb_lengths = grown[i].lb_lengths;
-    }
-    t->lb_search = true;
-    t->lscfg = rf_follow_config{R, mad};
-    return RF_OK;
-}
-
-int rf_tracker_lookback_search(rf_tracker t, const rf_follow **dev_steps, const int32_t **dev_lengths) {
-    if (!t) return RF_ERR_INVALID_ARG;
-    if (!t->lb_search) return fail(t->h, RF_ERR_INVALID_ARG, "rf_tracker_lookback_search: not a searching look-back tracker (rf_tracker_set_lookback_search)");
-    const bool any = t->lb_search_slot >= 0;
-    if (dev_steps) *dev_steps = any ? t->slots[t->lb_search_slot].lb_steps : nullptr;
-    if (dev_lengths) *dev_lengths = any ? t->slots[t->lb_search_slot].lb_lengths : nullptr;
-    return RF_OK;
-}
-
-extern "C++" {
-// An out frame of a look-back call: a valid descriptor with the size and layout (uv_step, chroma order) of the frames it receives.
-static int check_out_frame(rf_handle h, const char *who, const rf_yuv_frame &o, int i, int w, int ht, int step, bool v_first) {
-    if (!o.y || !o.u || !o.v) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: out frame %d has a NULL plane", who, i));
-    if (o.width != w || o.height != ht || o.uv_step != step)
-        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: out frame %d is %dx%d with uv_step %d, its video's frames are %dx%d with uv_step %d", who, i,
-                                               o.width, o.height, o.uv_step, w, ht, step));
-    const uintptr_t u = (uintptr_t)o.u, v = (uintptr_t)o.v;
-    if (step == 2 && ((v + 1 != u && u + 1 != v) || (v < u) != v_first))
-        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: out frame %d: semi-planar u and v must be adjacent, in the input's order", who, i));
-    if (o.y_pitch < w || o.uv_pitch < w / 2 * step)
-        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: out frame %d: pitches %d / %d below the row bytes %d / %d", who, i, o.y_pitch, o.uv_pitch, w, w / 2 * step));
-    return RF_OK;
-}
-
-static bool same_frame(const rf_yuv_frame &a, const rf_yuv_frame &b) {
-    return a.y == b.y && a.u == b.u && a.v == b.v && a.y_pitch == b.y_pitch && a.uv_pitch == b.uv_pitch && a.uv_step == b.uv_step &&
-           a.width == b.width && a.height == b.height;
-}
-
-static uint8_t *lb_log(rf_tracker t, const rf_tracker_s::LookbackVideo &v) { return v.d + (size_t)t->lb_frames * v.frame_bytes; }
-static size_t lb_slot_bytes(rf_tracker t) { return lookback_slot_bytes(t->h->cfg.max_faces, t->cfg.max_tracks, t->lb_search ? t->lb_frames : 0); }
-static int lb_records(rf_tracker t) { return lookback_records(t->h->cfg.max_faces, t->cfg.max_tracks, t->lb_frames, t->lb_search); }
-
-// The swap entry of one frame: its planes (in: NULL for a drain; out: NULL when it emits nothing) and its buffer slot.
-static LookbackSwapFrame lb_swap_frame(const rf_yuv_frame *in, const rf_yuv_frame *out, uint8_t *slot) {
-    const rf_yuv_frame &g = in ? *in : *out;
-    LookbackSwapFrame f{};
-    f.w = g.width;
-    f.h = g.height;
-    f.planar = g.uv_step == 1;
-    f.slot = slot;
-    if (in) {
-        f.in[0] = in->y;
-        f.in[1] = f.planar ? in->u : std::min(in->u, in->v);
-        f.in_v = in->v;
-        f.in_pitch[0] = in->y_pitch;
-        f.in_pitch[1] = in->uv_pitch;
-    }
-    if (out) {
-        f.out[0] = const_cast<uint8_t *>(out->y);
-        f.out[1] = const_cast<uint8_t *>(f.planar ? out->u : std::min(out->u, out->v));
-        f.out_v = const_cast<uint8_t *>(out->v);
-        f.out_pitch[0] = out->y_pitch;
-        f.out_pitch[1] = out->uv_pitch;
-    }
-    return f;
-}
-
-static void lb_swap(const std::vector<LookbackSwapFrame> &v, cudaStream_t s) {
-    for (size_t i0 = 0; i0 < v.size(); i0 += LOOKBACK_TABLE) {
-        LookbackSwapTable tb{};
-        int rows = 0;
-        for (size_t i = i0; i < std::min(v.size(), i0 + LOOKBACK_TABLE); i++) {
-            tb.f[tb.n++] = v[i];
-            rows = std::max(rows, v[i].h + (v[i].planar ? v[i].h : v[i].h / 2));
-        }
-        CK(launch_lookback_swap(tb, rows, s));
-    }
-}
-
-// The (a) + (b) + (c) records of the emitted frames {video, e, span} into ring slot `slot`'s look-back boxes.
-static void lb_boxes(rf_tracker t, rf_tracker_s::Slot &slot, const std::vector<std::array<long long, 3>> &em, cudaStream_t s) {
-    LookbackArgs a{};
-    a.max_faces = t->h->cfg.max_faces;
-    a.max_tracks = t->cfg.max_tracks;
-    a.slot_bytes = lb_slot_bytes(t);
-    a.ring = 2 * t->lb_frames;
-    a.grow = (double)t->lb_grow;
-    a.out = slot.lb_boxes;
-    a.out_counts = slot.lb_counts;
-    a.records = lb_records(t);
-    a.search = t->lb_search ? t->lscfg.search : 0;
-    a.L = t->lb_frames;
-    for (size_t j0 = 0; j0 < em.size(); j0 += LOOKBACK_TABLE) {
-        LookbackBoxTable tb{};
-        tb.j0 = (int)j0;
-        for (size_t j = j0; j < std::min(em.size(), j0 + LOOKBACK_TABLE); j++, tb.n++) {
-            tb.log[tb.n] = lb_log(t, t->lbv[em[j][0]]);
-            tb.e_slot[tb.n] = (int)(em[j][1] % a.ring);
-            tb.span[tb.n] = (int)em[j][2];
-        }
-        CK(launch_lookback_boxes(a, tb, s));
-    }
-}
-
-// f17: the chains of the call's births (k_lookback_search), after the log and before the swap.  Tables take whole videos: each video's
-// frames of the call, in number order, so that a step on an earlier frame of the call finds it in the same table.
-static void lb_search(rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, const std::vector<long long> &num, const LookbackArgs &a,
-                      cudaStream_t s) {
-    std::vector<std::vector<int>> by;            // the call's frames of each video, in first-appearance order
-    std::vector<int> vid;
-    for (int i = 0; i < n; i++) {
-        auto it = std::find(vid.begin(), vid.end(), videos[i]);
-        if (it == vid.end()) {
-            vid.push_back(videos[i]);
-            by.emplace_back();
-            it = vid.end() - 1;
-        }
-        by[it - vid.begin()].push_back(i);
-    }
-    LookbackSearchTable tb{};
-    for (size_t q = 0; q <= by.size(); q++) {
-        if (tb.n > 0 && (q == by.size() || tb.n + (int)by[q].size() > LOOKBACK_SEARCH_FRAMES || tb.nv == LOOKBACK_SEARCH_VIDEOS)) {
-            CK(launch_lookback_search(a, tb, s));
-            tb = LookbackSearchTable{};
-        }
-        if (q == by.size()) break;
-        const rf_tracker_s::LookbackVideo &lv = t->lbv[vid[q]];
-        LookbackSearchVideo &v = tb.v[tb.nv];
-        v.buf = lv.d;
-        v.log = lb_log(t, lv);
-        v.frame_bytes = lv.frame_bytes;
-        v.num0 = num[by[q][0]];
-        v.w = lv.w;
-        v.h = lv.h;
-        v.first = tb.n;
-        for (int i : by[q]) tb.f[tb.n++] = LookbackSearchFrame{frames[i].y, frames[i].y_pitch, tb.nv, i};
-        tb.nv++;
-    }
-}
-
-// Allocates (or, at a new frame size, replaces) the buffer of a video that has no buffered frames.  false: the allocation failed.
-static bool lb_alloc(rf_tracker t, rf_tracker_s::LookbackVideo &v, const rf_yuv_frame &f) {
-    const size_t fb = ((size_t)f.width * f.height * 3 / 2 + 255) & ~(size_t)255;
-    const size_t bytes = (size_t)t->lb_frames * fb + 2 * (size_t)t->lb_frames * lb_slot_bytes(t);
-    if (v.d && v.frame_bytes == fb) return true;
-    if (v.d) {
-        CK(cudaEventSynchronize(t->chain));      // the last drain's swap may still read it
-        CK(cudaFree(v.d));
-        v.d = nullptr;
-    }
-    if (cudaMalloc(&v.d, bytes) != cudaSuccess) {
-        cudaGetLastError();
-        v.d = nullptr;
-        return false;
-    }
-    v.frame_bytes = fb;
-    return true;
-}
-}  // extern "C++"
-
-int rf_detect_yuv_redact_lookback_device(rf_handle h, rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, int matrix, float thr,
-                                         float nms, const rf_redact_style *style, const rf_yuv_frame *out_frames, int32_t *out_frame_numbers,
-                                         const rf_track **dev_tracks, const int32_t **dev_track_counts, const rf_det **dev_dets,
-                                         const int32_t **dev_counts, float *out_scales) {
-    static const char *who = "rf_detect_yuv_redact_lookback_device";
-    if (!h) return RF_ERR_INVALID_ARG;
-    if (!t || t->h != h) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker is NULL or belongs to another handle", who));
-    if (!t->lookback) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: not a look-back tracker (rf_tracker_set_lookback)", who));
-    int rc = check_track_args(t, who, videos, n, nullptr);
-    if (rc) return rc;
-    const YuvFrames src{frames, matrix, nullptr, false};
-    if ((rc = src.check(h, who, n))) return rc;
-    RedactSpec spec;
-    if ((rc = redact_style(h, who, style, spec))) return rc;
-    if (n > 0 && (!out_frames || !out_frame_numbers)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL out frames or frame numbers", who));
-    const int L = t->lb_frames;
-    // each frame's number; a video's size and layout are those of its buffered frames, else of its first frame in the call
-    std::vector<long long> num(n);
-    std::vector<std::array<int, 3>> seen;        // (video, first frame of the call, frames in the call)
-    auto ranges = yuv_ranges(frames, n);
-    for (int i = 0; i < n; i++) {
-        const int v = videos[i];
-        auto it = std::find_if(seen.begin(), seen.end(), [v](const std::array<int, 3> &e) { return e[0] == v; });
-        if (it == seen.end()) it = seen.insert(seen.end(), std::array<int, 3>{v, i, 0});
-        const rf_tracker_s::LookbackVideo &lv = t->lbv[v];
-        const rf_yuv_frame &f = frames[i], &g = frames[(*it)[1]];
-        const bool v_first = f.uv_step == 2 && f.v < f.u;
-        const bool same = lv.frames > 0 ? f.width == lv.w && f.height == lv.h && f.uv_step == lv.step && v_first == lv.v_first
-                                        : f.width == g.width && f.height == g.height && f.uv_step == g.uv_step && v_first == (g.uv_step == 2 && g.v < g.u);
-        if (!same)
-            return fail(h, RF_ERR_INVALID_ARG, fmt("%s: frame %d: video %d changes its frame size or layout; drain or reset it first", who, i, v));
-        if (++(*it)[2] > L) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: video %d appears more than L = %d times in one call", who, v, L));
-        num[i] = lv.frames + (*it)[2] - 1;
-        if ((rc = check_out_frame(h, who, out_frames[i], i, f.width, f.height, f.uv_step, v_first))) return rc;
-        if (!same_frame(out_frames[i], f))
-            for (auto &r : yuv_ranges(out_frames + i, 1)) ranges.push_back({r[0], r[1], (uintptr_t)(n + i)});
-    }
-    if ((rc = check_disjoint(h, who, ranges))) return rc;
-    if (n == 0) return RF_OK;
-    try {
-        CK(cudaSetDevice(h->device));
-        for (const auto &e : seen) {
-            rf_tracker_s::LookbackVideo &lv = t->lbv[e[0]];
-            if (lv.frames > 0) continue;
-            const rf_yuv_frame &f = frames[e[1]];
-            if (!lb_alloc(t, lv, f))
-                return fail(h, RF_ERR_CAPACITY, fmt("%s: video %d: no device memory for %d frames of %dx%d", who, e[0], L, f.width, f.height));
-            lv.w = f.width;
-            lv.h = f.height;
-            lv.step = f.uv_step;
-            lv.v_first = f.uv_step == 2 && f.v < f.u;
-        }
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    std::vector<float> scales(n);
-    const rf_det *dets = nullptr;
-    const int32_t *counts = nullptr;
-    if ((rc = yuv_device_impl(h, who, src, n, thr, nms, nullptr, nullptr, nullptr, &dets, &counts, scales.data()))) return rc;
-    if (dev_dets) *dev_dets = dets;
-    if (dev_counts) *dev_counts = counts;
-    if (out_scales) std::copy(scales.begin(), scales.end(), out_scales);
-    try {
-        Ctx &c = last_ctx(h);          // the forward's context
-        const rf_track *tracks = nullptr;
-        const int32_t *track_counts = nullptr;
-        track_issue(t, videos, n, dets, counts, scales.data(), c.stream, nullptr, nullptr, &tracks, &track_counts, frames);
-        rf_tracker_s::Slot &slot = t->slots[(t->next_slot - 1) % t->slots.size()];
-        if (dev_tracks) *dev_tracks = tracks;
-        if (dev_track_counts) *dev_track_counts = track_counts;
-        // the update recorded the chain; the look-back state follows it on the same stream and records it again
-        LookbackArgs a{};
-        a.dets = dets;
-        a.counts = counts;
-        a.tracks = tracks;
-        a.track_counts = track_counts;
-        a.motion = t->motion ? slot.motion : nullptr;
-        a.max_faces = h->cfg.max_faces;
-        a.max_tracks = t->cfg.max_tracks;
-        a.slot_bytes = lb_slot_bytes(t);
-        a.ring = 2 * L;
-        a.L = L;
-        for (int i0 = 0; i0 < n; i0 += LOOKBACK_TABLE) {
-            LookbackLogTable lt{};
-            lt.i0 = i0;
-            for (int i = i0; i < std::min(n, i0 + LOOKBACK_TABLE); i++, lt.n++) {
-                lt.scale[lt.n] = scales[i];
-                lt.slot[lt.n] = lb_log(t, t->lbv[videos[i]]) + (size_t)(num[i] % a.ring) * a.slot_bytes;
-            }
-            CK(launch_lookback_log(a, lt, c.stream));
-        }
-        if (t->lb_search) {
-            a.search = t->lscfg.search;
-            a.max_mad = t->lscfg.max_mad;
-            a.steps = slot.lb_steps;
-            a.lengths = slot.lb_lengths;
-            lb_search(t, frames, videos, n, num, a, c.stream);
-            t->lb_search_slot = (int)((t->next_slot - 1) % t->slots.size());
-        }
-        std::vector<LookbackSwapFrame> sw;
-        std::vector<std::array<long long, 3>> em;
-        std::vector<rf_yuv_frame> outs;
-        for (int i = 0; i < n; i++) {
-            const rf_tracker_s::LookbackVideo &lv = t->lbv[videos[i]];
-            const bool emits = num[i] >= L;
-            sw.push_back(lb_swap_frame(frames + i, emits ? out_frames + i : nullptr, lv.d + (size_t)(num[i] % L) * lv.frame_bytes));
-            if (emits) {
-                em.push_back({videos[i], num[i] - L, L});
-                outs.push_back(out_frames[i]);
-            }
-        }
-        lb_swap(sw, c.stream);
-        lb_boxes(t, slot, em, c.stream);
-        CK(cudaEventRecord(t->chain, c.stream));
-        if (!em.empty())
-            redact_issue(h, c, yuv_redact_table(outs.data(), (int)outs.size(), nullptr), slot.lb_boxes, slot.lb_counts, nullptr, nullptr, nullptr,
-                         spec, lb_records(t));
-        CK(cudaEventRecord(slot.free, c.stream));
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    for (int i = 0; i < n; i++) {
-        t->lbv[videos[i]].frames = std::max(t->lbv[videos[i]].frames, num[i] + 1);
-        out_frame_numbers[i] = num[i] >= L ? (int32_t)(num[i] - L) : -1;
-    }
-    return RF_OK;
-}
-
-int rf_tracker_drain(rf_tracker t, int video, const rf_redact_style *style, const rf_yuv_frame *out_frames, int cap, int *n_out,
-                     int32_t *out_frame_numbers) {
-    static const char *who = "rf_tracker_drain";
-    if (!t) return RF_ERR_INVALID_ARG;
-    rf_handle h = t->h;
-    if (!t->lookback) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: not a look-back tracker (rf_tracker_set_lookback)", who));
-    if (video < 0 || video >= t->cfg.max_videos) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: video %d, must be in [0, %d)", who, video, t->cfg.max_videos));
-    RedactSpec spec;
-    int rc = redact_style(h, who, style, spec);
-    if (rc) return rc;
-    if (!n_out) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: n_out is NULL", who));
-    rf_tracker_s::LookbackVideo &lv = t->lbv[video];
-    const int L = t->lb_frames, k = (int)std::min<long long>(L, lv.frames);
-    if (cap < k) return fail(h, RF_ERR_CAPACITY, fmt("%s: video %d has %d buffered frames, cap is %d", who, video, k, cap));
-    if (k > 0 && (!out_frames || !out_frame_numbers)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL out frames or frame numbers", who));
-    for (int j = 0; j < k; j++)
-        if ((rc = check_out_frame(h, who, out_frames[j], j, lv.w, lv.h, lv.step, lv.v_first))) return rc;
-    if ((rc = check_disjoint(h, who, yuv_ranges(out_frames, k)))) return rc;
-    try {
-        CK(cudaSetDevice(h->device));
-        Ctx &c = h->ctx[0];
-        const unsigned ring = t->next_slot++ % t->slots.size();
-        rf_tracker_s::Slot &slot = t->slots[ring];
-        CK(cudaStreamWaitEvent(c.stream, slot.free, 0));
-        CK(cudaStreamWaitEvent(c.stream, t->chain, 0));
-        std::vector<LookbackSwapFrame> sw;
-        std::vector<std::array<long long, 3>> em;
-        for (int j = 0; j < k; j++) {
-            const long long e = lv.frames - k + j;
-            sw.push_back(lb_swap_frame(nullptr, out_frames + j, lv.d + (size_t)(e % L) * lv.frame_bytes));
-            em.push_back({video, e, lv.frames - 1 - e});
-        }
-        lb_swap(sw, c.stream);
-        lb_boxes(t, slot, em, c.stream);
-        // then the video restarts as rf_tracker_reset restarts it
-        const size_t T = t->cfg.max_tracks;
-        CK(cudaMemsetAsync(t->d_videos + video, 0, sizeof(TrackVideo), c.stream));
-        CK(cudaMemsetAsync(t->d_state + (size_t)video * T, 0, sizeof(TrackState) * T, c.stream));
-        if (t->motion) t->mref[video] = {0, 0};
-        CK(cudaEventRecord(t->chain, c.stream));
-        if (k > 0)
-            redact_issue(h, c, yuv_redact_table(out_frames, k, nullptr), slot.lb_boxes, slot.lb_counts, nullptr, nullptr, nullptr, spec,
-                         lb_records(t));
-        CK(cudaEventRecord(slot.free, c.stream));
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    for (int j = 0; j < k; j++) out_frame_numbers[j] = (int32_t)(lv.frames - k + j);
-    lv.frames = 0;
-    *n_out = k;
-    return RF_OK;
 }
 
 }  // extern "C"

@@ -4,7 +4,8 @@
 //   plan_fp.cu   SIMT layer plans (FP32, FP16 without tensor cores), FP16 tensor-core per-layer operations and launch helpers
 //   plan_tile.cu FP16 tensor-core layer plan: tile chains, and the per-layer operations where a chain is off or does not fit
 //   plan_i8.cu   INT8 layer plan (build_plan_i8)
-//   engine.cu    tensor placement, CUDA-graph executor, the C-ABI entry points
+//   engine.cu    tensor placement, CUDA-graph executor, the detect C-ABI entry points
+//   tracker.cu   the video tracker's C-ABI entry points (f10 - f17) and redaction
 #pragma once
 #include <algorithm>
 #include <cstdarg>
@@ -351,5 +352,101 @@ const char *jpeg_backend(rf_handle h);
 // ---- exported by plan_i8.cu -----------------------------------------------------------------------------------------
 void build_plan_i8(rf_handle h);
 cudaError_t tc_init_i8();
+
+// ---- exported by engine.cu (the detect entry points) -----------------------------------------------------------------
+int check_n(rf_handle h, int n);
+int check_frames(rf_handle h, const char *who, const rf_yuv_frame *frames, int n, int matrix);
+int check_orientations(rf_handle h, const char *who, const int *orientations, int n);
+void upload_plane(rf_handle h, cudaStream_t s, uint8_t *d_dst, const uint8_t *src, size_t row_bytes, size_t pitch, int rows);
+int align_setup(rf_handle h, const char *who, const rf_align_params *p, AlignArgs &a);
+int check_align(rf_handle h, const char *who, const rf_align_params *p, int n, const void *crops, int resident, AlignArgs &a);
+
+// ---- image sources ---------------------------------------------------------------------------------------------------------------
+// Every detect entry point describes the caller's pixels with one of two sources.  A source checks the caller's description (every
+// check runs before anything is copied or launched), reports image i's stored size and EXIF orientation, and hands the letter-box
+// and crop kernels its pixels: upload(s, i, slot) copies host image i into raw buffer `slot` on s (the blocking paths),
+// in_place(i) reads the caller's device memory (the asynchronous ones).  Src is what those kernels read.
+
+// BGR images: u8 BGR HWC rows row_strides[i] bytes apart (NULL or 0: packed), shown in EXIF orientation orient[i] when `oriented`.
+struct BgrImages {
+    using Src = BgrRows;
+    const uint8_t *const *imgs;
+    const int *widths, *heights, *row_strides, *orient;
+    bool oriented;
+    int width(int i) const { return widths[i]; }
+    int height(int i) const { return heights[i]; }
+    int stride(int i) const { return row_strides && row_strides[i] ? row_strides[i] : widths[i] * 3; }
+    int bits(int i) const { return oriented ? lb_orientation_bits(orient[i]) : 0; }
+    // network-sized, packed and upright: copied straight into the input tensor, without a raw buffer or a letter-box
+    bool direct(rf_handle h, int i) const {
+        return widths[i] == h->cfg.net_w && heights[i] == h->cfg.net_h && stride(i) == h->cfg.net_w * 3 && bits(i) == 0;
+    }
+    int check(rf_handle h, const char *who, int n) const {
+        int rc = check_n(h, n);
+        if (rc) return rc;
+        if (n > 0 && (!imgs || !widths || !heights)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL image arrays", who));
+        for (int i = 0; i < n; i++) {
+            if (!imgs[i] || widths[i] <= 0 || heights[i] <= 0) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: image %d is empty", who, i));
+            if (stride(i) < widths[i] * 3)
+                return fail(h, RF_ERR_INVALID_ARG, fmt("%s: image %d: row stride %d below %d bytes", who, i, stride(i), widths[i] * 3));
+            if (widths[i] > h->cfg.max_image_w || heights[i] > h->cfg.max_image_h)
+                return fail(h, RF_ERR_CAPACITY, fmt("%s: image %d is %dx%d, larger than max_image %dx%d", who, i, widths[i], heights[i],
+                                                    h->cfg.max_image_w, h->cfg.max_image_h));
+        }
+        return oriented ? check_orientations(h, who, orient, n) : RF_OK;
+    }
+    BgrRows upload(rf_handle h, cudaStream_t s, int i, int slot) const {
+        uint8_t *d = h->d_raw + (size_t)slot * h->raw_bytes;
+        upload_plane(h, s, d, imgs[i], (size_t)widths[i] * 3, (size_t)stride(i), heights[i]);
+        return BgrRows{d, widths[i] * 3};
+    }
+    BgrRows in_place(int i) const { return BgrRows{imgs[i], stride(i)}; }
+};
+
+// YUV 4:2:0 frames (yuv.cuh) in `matrix`, shown in EXIF orientation orient[i] when `oriented`.
+struct YuvFrames {
+    using Src = YuvPlanes;
+    const rf_yuv_frame *frames;
+    int matrix;
+    const int *orient;
+    bool oriented;
+    int width(int i) const { return frames[i].width; }
+    int height(int i) const { return frames[i].height; }
+    int bits(int i) const { return oriented ? lb_orientation_bits(orient[i]) : 0; }
+    bool direct(rf_handle, int) const { return false; }
+    int check(rf_handle h, const char *who, int n) const {
+        int rc = check_frames(h, who, frames, n, matrix);
+        if (rc || !oriented) return rc;
+        return check_orientations(h, who, orient, n);
+    }
+    // 1.5 bytes per pixel: the luma packed, then the chroma as the frame lays it out (one interleaved w x h/2 plane, or two
+    // w/2 x h/2 planes)
+    YuvPlanes upload(rf_handle h, cudaStream_t s, int i, int slot) const {
+        const rf_yuv_frame &f = frames[i];
+        uint8_t *d = h->d_raw + (size_t)slot * h->raw_bytes, *dc = d + (size_t)f.width * f.height;
+        const int cw = f.width / 2, ch = f.height / 2;
+        upload_plane(h, s, d, f.y, f.width, f.y_pitch, f.height);
+        YuvPlanes p{d, dc, dc, f.width, f.width, f.uv_step, matrix};
+        if (f.uv_step == 2) {
+            const uint8_t *first = std::min(f.u, f.v);
+            upload_plane(h, s, dc, first, f.width, f.uv_pitch, ch);
+            p.u = dc + (f.u - first);
+            p.v = dc + (f.v - first);
+        } else {
+            upload_plane(h, s, dc, f.u, cw, f.uv_pitch, ch);
+            upload_plane(h, s, dc + (size_t)cw * ch, f.v, cw, f.uv_pitch, ch);
+            p.v = dc + (size_t)cw * ch;
+            p.uv_pitch = cw;
+        }
+        return p;
+    }
+    YuvPlanes in_place(int i) const {
+        const rf_yuv_frame &f = frames[i];
+        return YuvPlanes{f.y, f.u, f.v, f.y_pitch, f.uv_pitch, f.uv_step, matrix};
+    }
+};
+
+int yuv_device_impl(rf_handle h, const char *who, const YuvFrames &src, int n, float thr, float nms, const rf_align_params *align,
+                    void *dev_crops, double *dev_mats, const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales);
 
 }  // namespace rf_eng

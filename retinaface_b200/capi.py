@@ -4,6 +4,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import types
 from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -14,33 +15,6 @@ RF_PREC_FP32, RF_PREC_FP16, RF_PREC_INT8 = 0, 1, 2
 RF_FLAG_NO_GRAPH, RF_FLAG_NO_TENSORCORE, RF_FLAG_SIMT_STEM, RF_FLAG_DW_1D, RF_FLAG_LEGACY_TC, RF_FLAG_NPP_RESIZE = 0x1, 0x2, 0x4, 0x8, 0x10, 0x20
 FACE_FLOATS = 15
 PIPELINE_DEPTH = 6   # RF_PIPELINE_DEPTH
-
-# every symbol include/rf_b200.h declares (checked by tests/test_capi_symbols.py)
-EXPORTS = [
-    "rf_abi_version", "rf_build_info", "rf_status_string", "rf_create", "rf_destroy", "rf_last_error",
-    "rf_pinned_input", "rf_device_input", "rf_detect_batch", "rf_submit_batch", "rf_collect_batch", "rf_detect_batch_device", "rf_forward_heads",
-    "rf_postprocess", "rf_preprocess", "rf_get_net_size", "rf_num_anchors", "rf_stream", "rf_synchronize", "rf_fence", "rf_last_stream",
-    "rf_launches_per_batch", "rf_profile_layers", "rf_debug_get_tensor", "rf_debug_keep_all", "rf_model_inspect", "rf_calibrate_int8", "rf_kl_threshold_bins",
-    "rf_detect_views", "rf_plan_describe",
-    "rf_comm_export", "rf_comm_init", "rf_comm_nccl_unique_id", "rf_comm_init_nccl", "rf_comm_info", "rf_detect_batch_device_allgather",
-    "rf_submit_batch_allgather", "rf_collect_batch_allgather", "rf_detect_batch_allgather",
-    "rf_model_load", "rf_network_config", "rf_cache_status",
-    "rf_detect_jpeg_batch", "rf_decode_jpeg", "rf_jpeg_backend",
-    "rf_detect_align_batch", "rf_detect_align_batch_device",
-    "rf_detect_yuv_batch", "rf_detect_yuv_batch_device", "rf_preprocess_yuv",
-    "rf_tile_layout", "rf_detect_tiled", "rf_detect_yuv_tiled", "rf_preprocess_tile", "rf_preprocess_yuv_tile",
-    "rf_detect_tiled_align", "rf_detect_yuv_tiled_align", "rf_detect_tiled_device", "rf_detect_yuv_tiled_device",
-    "rf_detect_oriented_batch", "rf_detect_yuv_oriented_device", "rf_preprocess_oriented", "rf_preprocess_yuv_oriented",
-    "rf_detect_views_oriented", "rf_jpeg_exif_orientation",
-    "rf_tracker_create", "rf_tracker_destroy", "rf_tracker_reset", "rf_track_update", "rf_detect_yuv_track_device", "rf_tracker_debug_state",
-    "rf_tracker_create_best", "rf_detect_yuv_track_best_device", "rf_tracker_finish",
-    "rf_tracker_set_motion", "rf_tracker_motion",
-    "rf_redact_yuv_device", "rf_redact_device", "rf_detect_yuv_redact_device",
-    "rf_redact_yuv_device_style", "rf_redact_device_style", "rf_detect_yuv_redact_device_style",
-    "rf_tracker_set_lookback", "rf_detect_yuv_redact_lookback_device", "rf_tracker_drain",
-    "rf_tracker_set_follow", "rf_track_follow_device", "rf_tracker_follow", "rf_track_follow_redact_device",
-    "rf_tracker_set_lookback_search", "rf_tracker_lookback_search",
-]
 COMM_BLOB_BYTES = 128
 
 
@@ -205,6 +179,13 @@ class Face(C.Structure):         # rf_face
                 ("lx", C.c_float * 5), ("ly", C.c_float * 5)]
 
 
+def _record_dtype(struct) -> np.dtype:
+    """The numpy record of a ctypes Structure: every field at its ctypes offset, a nested Face as FACE_FLOATS floats."""
+    names = [f for f, _ in struct._fields_]
+    return np.dtype(dict(names=names, formats=[("<f4", (FACE_FLOATS,)) if t is Face else np.dtype(t) for _, t in struct._fields_],
+                         offsets=[getattr(struct, f).offset for f in names], itemsize=C.sizeof(struct)))
+
+
 class TrackRecord(C.Structure):  # rf_track
     _fields_ = [(f, C.c_int32) for f in ("id", "state", "det", "crop_slot", "hits", "age", "lost_frames", "followed")] + \
                [(f, C.c_float) for f in ("kx1", "ky1", "kx2", "ky2", "vx", "vy")] + [("face", Face)]
@@ -212,9 +193,7 @@ class TrackRecord(C.Structure):  # rf_track
 
 TRACK_TENTATIVE, TRACK_CONFIRMED, TRACK_LOST = 0, 1, 2      # RF_TRACK_*
 TRACK_DEBUG_DOUBLES = 25                                     # RF_TRACK_DEBUG_DOUBLES
-# one rf_track as a numpy record (the layout of TrackRecord)
-TRACK_DTYPE = np.dtype([(f, "<i4") for f in ("id", "state", "det", "crop_slot", "hits", "age", "lost_frames", "followed")] +
-                       [(f, "<f4") for f in ("kx1", "ky1", "kx2", "ky2", "vx", "vy")] + [("face", "<f4", (FACE_FLOATS,))])
+TRACK_DTYPE = _record_dtype(TrackRecord)                     # one rf_track as a numpy record
 
 
 class BestConfig(C.Structure):   # rf_best_config
@@ -232,9 +211,7 @@ class BestShot(C.Structure):     # rf_best_shot
 
 
 BEST_EXIT, BEST_FINISH = 0, 1                                # RF_BEST_*
-# one rf_best_shot as a numpy record (the layout of BestShot)
-BEST_DTYPE = np.dtype([(f, "<i4") for f in ("id", "video", "frame", "end_frame", "hits", "age", "reason", "reserved")] +
-                      [(f, "<f4") for f in ("quality", "score", "eye", "frontal", "sharpness", "coverage")] + [("face", "<f4", (FACE_FLOATS,))])
+BEST_DTYPE = _record_dtype(BestShot)                         # one rf_best_shot as a numpy record
 
 
 class MotionConfig(C.Structure):  # rf_motion_config
@@ -251,8 +228,7 @@ class Motion(C.Structure):       # rf_motion
 
 
 MOTION_OK, MOTION_FIRST, MOTION_LOST = 0, 1, 2               # RF_MOTION_*
-# one rf_motion as a numpy record (the layout of Motion)
-MOTION_DTYPE = np.dtype([(f, "<i4") for f in ("status", "blocks", "inliers", "reserved")] + [("m", "<f8", (6,))])
+MOTION_DTYPE = _record_dtype(Motion)                         # one rf_motion as a numpy record
 
 
 class FollowConfig(C.Structure):  # rf_follow_config
@@ -265,9 +241,7 @@ class FollowRecord(C.Structure):  # rf_follow
 
 
 FOLLOW_OK, FOLLOW_FLAT, FOLLOW_BORDER, FOLLOW_MISMATCH, FOLLOW_OUTSIDE, FOLLOW_LOST = range(6)   # RF_FOLLOW_*
-# one rf_follow as a numpy record (the layout of FollowRecord)
-FOLLOW_DTYPE = np.dtype([(f, "<i4") for f in ("id", "status", "dx", "dy", "scale", "sad")] +
-                        [(f, "<f4") for f in ("fx", "fy", "x1", "y1", "x2", "y2")])
+FOLLOW_DTYPE = _record_dtype(FollowRecord)                   # one rf_follow as a numpy record
 
 
 class RedactParams(C.Structure):  # rf_redact_params
@@ -297,18 +271,16 @@ class LookbackConfig(C.Structure):  # rf_lookback_config
     _fields_ = [("frames", C.c_int), ("grow", C.c_float)]
 
 
-def _style_struct(style: str, shape: str, blocks: int, detail: int, margin: float) -> RedactStyle:
-    """The rf_redact_style of the redaction keywords, {MOSAIC, RECT} included (the look-back calls take only a style)."""
+def _redaction(lib, name: str, style: str, shape: str, blocks: int, detail: int, margin: float):
+    """(entry point, the rf_redact_params or rf_redact_style to pass it) of the redaction keywords for the call `name`.  An f12
+    entry point draws f12's mosaic over rectangles from rf_redact_params and anything else through its `_style` variant; the
+    calls that take only a style get one for every set of keywords, {MOSAIC, RECT} included."""
     st = redact_style(style, shape, blocks, detail, margin)
-    return st if st is not None else RedactStyle(RF_REDACT_MOSAIC, RF_REDACT_RECT, int(blocks), 0, float(margin))
-
-
-def _redact_call(lib, style: str, shape: str, blocks: int, detail: int, margin: float):
-    """(rf_detect_yuv_redact_device or its _style variant, the params or style struct) of the redaction keywords."""
-    st = redact_style(style, shape, blocks, detail, margin)
+    if name + "_style" not in _SIGNATURES:
+        return getattr(lib, name), st if st is not None else RedactStyle(RF_REDACT_MOSAIC, RF_REDACT_RECT, int(blocks), 0, float(margin))
     if st is None:
-        return lib.rf_detect_yuv_redact_device, RedactParams(int(blocks), float(margin))
-    return lib.rf_detect_yuv_redact_device_style, st
+        return getattr(lib, name), RedactParams(int(blocks), float(margin))
+    return getattr(lib, name + "_style"), st
 
 
 class RfError(RuntimeError):
@@ -322,6 +294,87 @@ class _Config(C.Structure):
                 ("net_w", C.c_int), ("net_h", C.c_int), ("max_batch", C.c_int), ("max_faces", C.c_int),
                 ("device", C.c_int), ("max_image_w", C.c_int), ("max_image_h", C.c_int), ("flags", C.c_uint),
                 ("streams", C.c_int), ("prototxt_path", C.c_char_p), ("cache_path", C.c_char_p), ("network", C.c_char_p)]
+
+
+# The C signature of every function include/rf_b200.h declares: name -> (restype, argtypes), applied by load_library().
+# rf_handle, rf_tracker and output arrays are plain addresses; _PP is the address of a pointer the call writes.
+_P, _I, _F, _S = C.c_void_p, C.c_int, C.c_float, C.c_char_p
+_PP, _PI = C.POINTER(C.c_void_p), C.POINTER(C.c_int)
+_ALIGN, _FRAMES, _TILING, _STYLE = C.POINTER(AlignParams), C.POINTER(YuvFrame), C.POINTER(Tiling), C.POINTER(RedactStyle)
+_DETECT_DEVICE = [_P, _P, _I, _F, _F, _PP, _PP]                 # rf_detect_batch_device and its allgather
+_SUBMIT, _COLLECT = [_P, _PP, _I, _F, _F, _PI], [_P, _I, _P, _P, _P]
+_REDACT_YUV = [_P, _FRAMES, _I, _P, _P, _P, _P, _P, _P]         # rf_redact_yuv_device(_style) before the params or style
+_REDACT_BGR = [_P, _PP, _PI, _PI, _PI, _I, _P, _P, _P, _P, _P, _P]
+_DETECT_YUV_TRACKED = [_P, _P, _FRAMES, _P, _I, _I, _F, _F]     # (h, t, frames, videos, n, matrix, thresholds) of the tracked calls
+_TRACKED_OUT = [_PP, _PP, _PP, _PP, _P]                         # their (tracks, track counts, dets, counts, scales) outputs
+_SIGNATURES = {
+    "rf_abi_version": (_I, []), "rf_build_info": (_S, []), "rf_status_string": (_S, [_I]),
+    "rf_create": (_I, [C.POINTER(_Config), _PP]), "rf_destroy": (None, [_P]), "rf_last_error": (_S, [_P]),
+    "rf_pinned_input": (_P, [_P]), "rf_device_input": (_P, [_P]),
+    "rf_detect_batch": (_I, [_P, _PP, _PI, _PI, _PI, _I, _F, _F, _P, _P, _P]),
+    "rf_submit_batch": (_I, _SUBMIT), "rf_collect_batch": (_I, _COLLECT), "rf_detect_batch_device": (_I, _DETECT_DEVICE),
+    "rf_forward_heads": (_I, [_P, _P, _I, _PP]),
+    "rf_postprocess": (_I, [_P, _PP, _I, _F, _F, _P, _P, _P, _P]),
+    "rf_preprocess": (_I, [_P, _P, _I, _I, _I, _P]),
+    "rf_get_net_size": (_I, [_P, _PI, _PI, _PI, _PI]), "rf_num_anchors": (_I, [_P]), "rf_stream": (_P, [_P]),
+    "rf_synchronize": (_I, [_P]), "rf_fence": (_I, [_P]), "rf_last_stream": (_P, [_P]), "rf_launches_per_batch": (_I, [_P, _I]),
+    "rf_profile_layers": (_I, [_P, _I, _I, _P, _P, _P, _P, _I]),
+    "rf_debug_get_tensor": (_I, [_P, _S, _I, _P, _PI, _PI, _PI]), "rf_debug_keep_all": (_I, [_P]),
+    "rf_model_inspect": (_I, [_S, _S, _P, _I, _P, _I, _PI]),
+    "rf_calibrate_int8": (_I, [_P, _P, _I, _S]), "rf_kl_threshold_bins": (C.c_double, [_P, _I, _I]),
+    "rf_detect_views": (_I, [_P, _P, _I, _I, _I, C.POINTER(_View), _I, _F, _F, _P, _PI, _P, _P]),
+    "rf_plan_describe": (_I, [C.POINTER(_Config), _S, _I]),
+    "rf_comm_export": (_I, [_P, _I, _I, _P]), "rf_comm_init": (_I, [_P, _P]), "rf_comm_nccl_unique_id": (_I, [_P]),
+    "rf_comm_init_nccl": (_I, [_P, _P, _I, _I]), "rf_comm_info": (_I, [_P, _PI, _PI]),
+    "rf_detect_batch_device_allgather": (_I, _DETECT_DEVICE), "rf_submit_batch_allgather": (_I, _SUBMIT),
+    "rf_collect_batch_allgather": (_I, _COLLECT), "rf_detect_batch_allgather": (_I, [_P, _PP, _I, _F, _F, _P, _P, _P]),
+    "rf_model_load": (_I, [_S, _S, _S, _PI, _PI, _S, _P, _I, _P, _I, _PI]),
+    "rf_network_config": (_I, [_S, _PI, _PI, _PI, C.POINTER(C.c_float), _PI]), "rf_cache_status": (_I, [_P]),
+    "rf_detect_jpeg_batch": (_I, [_P, _P, _P, _I, _F, _F, _P, _P, _P, _P, _P]),
+    "rf_decode_jpeg": (_I, [_P, _P, C.c_size_t, _P, C.c_size_t, _P, _P]), "rf_jpeg_backend": (_S, [_P]),
+    "rf_detect_align_batch": (_I, [_P, _PP, _PI, _PI, _PI, _I, _F, _F, _ALIGN, _P, _P, _P, _P]),
+    "rf_detect_align_batch_device": (_I, [_P, _P, _I, _F, _F, _ALIGN, _P, _P, _PP, _PP]),
+    "rf_detect_yuv_batch": (_I, [_P, _FRAMES, _I, _I, _F, _F, _ALIGN, _P, _P, _P, _P, _P]),
+    "rf_detect_yuv_batch_device": (_I, [_P, _FRAMES, _I, _I, _F, _F, _ALIGN, _P, _P, _PP, _PP, _P]),
+    "rf_preprocess_yuv": (_I, [_P, _FRAMES, _I, _P]),
+    "rf_tile_layout": (_I, [_I, _I, _I, _I, _TILING, C.POINTER(Tile), _I]),
+    "rf_detect_tiled": (_I, [_P, _PP, _PI, _PI, _PI, _I, _TILING, _F, _F, _P, _P, _P]),
+    "rf_detect_yuv_tiled": (_I, [_P, _FRAMES, _I, _I, _TILING, _F, _F, _P, _P, _P]),
+    "rf_preprocess_tile": (_I, [_P, _P, _I, _I, _I, _TILING, _I, _P]),
+    "rf_preprocess_yuv_tile": (_I, [_P, _FRAMES, _I, _TILING, _I, _P]),
+    "rf_detect_tiled_align": (_I, [_P, _PP, _PI, _PI, _PI, _I, _TILING, _F, _F, _ALIGN, _P, _P, _P, _P, _P]),
+    "rf_detect_yuv_tiled_align": (_I, [_P, _FRAMES, _I, _I, _TILING, _F, _F, _ALIGN, _P, _P, _P, _P, _P]),
+    "rf_detect_tiled_device": (_I, [_P, _PP, _PI, _PI, _PI, _I, _TILING, _F, _F, _ALIGN, _P, _P, _PP, _PP]),
+    "rf_detect_yuv_tiled_device": (_I, [_P, _FRAMES, _I, _I, _TILING, _F, _F, _ALIGN, _P, _P, _PP, _PP]),
+    "rf_detect_oriented_batch": (_I, [_P, _PP, _PI, _PI, _PI, _PI, _I, _F, _F, _ALIGN, _P, _P, _P, _P, _P]),
+    "rf_detect_yuv_oriented_device": (_I, [_P, _FRAMES, _PI, _I, _I, _F, _F, _ALIGN, _P, _P, _PP, _PP, _P]),
+    "rf_preprocess_oriented": (_I, [_P, _P, _I, _I, _I, _I, _P]),
+    "rf_preprocess_yuv_oriented": (_I, [_P, _FRAMES, _I, _I, _P]),
+    "rf_detect_views_oriented": (_I, [_P, _P, _I, _I, _I, C.POINTER(_OrientedView), _I, _F, _F, _P, _PI, _P, _P]),
+    "rf_jpeg_exif_orientation": (_I, [_P, C.c_size_t]),
+    "rf_tracker_create": (_I, [_P, C.POINTER(TrackConfig), _PP]), "rf_tracker_destroy": (None, [_P]),
+    "rf_tracker_reset": (_I, [_P, _I]),
+    "rf_track_update": (_I, [_P, _P, _I, _P, _P, _P, _PP, _PP]),
+    "rf_detect_yuv_track_device": (_I, _DETECT_YUV_TRACKED + [_ALIGN, _P, _P] + _TRACKED_OUT),
+    "rf_tracker_debug_state": (_I, [_P, _I, _P, _I]),
+    "rf_tracker_create_best": (_I, [_P, C.POINTER(TrackConfig), C.POINTER(BestConfig), _PP]),
+    "rf_detect_yuv_track_best_device": (_I, _DETECT_YUV_TRACKED + [_P, _P, _PP, _PP] + _TRACKED_OUT),
+    "rf_tracker_finish": (_I, [_P, _I, _P, _P, _PP, _PP]),
+    "rf_tracker_set_motion": (_I, [_P, C.POINTER(MotionConfig)]), "rf_tracker_motion": (_I, [_P, _PP]),
+    "rf_redact_yuv_device": (_I, _REDACT_YUV + [C.POINTER(RedactParams)]),
+    "rf_redact_device": (_I, _REDACT_BGR + [C.POINTER(RedactParams)]),
+    "rf_detect_yuv_redact_device": (_I, _DETECT_YUV_TRACKED + [C.POINTER(RedactParams)] + _TRACKED_OUT),
+    "rf_redact_yuv_device_style": (_I, _REDACT_YUV + [_STYLE]), "rf_redact_device_style": (_I, _REDACT_BGR + [_STYLE]),
+    "rf_detect_yuv_redact_device_style": (_I, _DETECT_YUV_TRACKED + [_STYLE] + _TRACKED_OUT),
+    "rf_tracker_set_lookback": (_I, [_P, C.POINTER(LookbackConfig)]),
+    "rf_detect_yuv_redact_lookback_device": (_I, _DETECT_YUV_TRACKED + [_STYLE, _FRAMES, _P] + _TRACKED_OUT),
+    "rf_tracker_drain": (_I, [_P, _I, _STYLE, _FRAMES, _I, _PI, _P]),
+    "rf_tracker_set_follow": (_I, [_P, C.POINTER(FollowConfig)]),
+    "rf_track_follow_device": (_I, [_P, _FRAMES, _P, _I, _PP, _PP]), "rf_tracker_follow": (_I, [_P, _PP]),
+    "rf_track_follow_redact_device": (_I, [_P, _FRAMES, _P, _I, _STYLE, _PP, _PP]),
+    "rf_tracker_set_lookback_search": (_I, [_P, C.POINTER(FollowConfig)]), "rf_tracker_lookback_search": (_I, [_P, _PP, _PP]),
+}
+EXPORTS = list(_SIGNATURES)     # every symbol include/rf_b200.h declares (checked by tests/test_host_side.py)
 
 
 def lib_path() -> str:
@@ -341,133 +394,9 @@ def load_library() -> C.CDLL:
         raise ImportError(f"{p} not found: run `python -c 'import __graft_entry__ as g; g.build()'` "
                           "(retinaface_b200 has no CPU fallback)")
     lib = C.CDLL(p)
-    lib.rf_build_info.restype = C.c_char_p
-    lib.rf_status_string.restype = C.c_char_p
-    lib.rf_last_error.restype = C.c_char_p
-    lib.rf_last_error.argtypes = [C.c_void_p]
-    lib.rf_create.argtypes = [C.POINTER(_Config), C.POINTER(C.c_void_p)]
-    lib.rf_destroy.argtypes = [C.c_void_p]
-    lib.rf_destroy.restype = None
-    lib.rf_pinned_input.restype = C.c_void_p
-    lib.rf_pinned_input.argtypes = [C.c_void_p]
-    lib.rf_device_input.restype = C.c_void_p
-    lib.rf_device_input.argtypes = [C.c_void_p]
-    lib.rf_stream.restype = C.c_void_p
-    lib.rf_stream.argtypes = [C.c_void_p]
-    lib.rf_last_stream.restype = C.c_void_p
-    lib.rf_last_stream.argtypes = [C.c_void_p]
-    for name in ("rf_synchronize", "rf_num_anchors", "rf_fence"):
-        getattr(lib, name).argtypes = [C.c_void_p]
-    lib.rf_launches_per_batch.argtypes = [C.c_void_p, C.c_int]
-    lib.rf_get_net_size.argtypes = [C.c_void_p] + [C.POINTER(C.c_int)] * 4
-    lib.rf_detect_batch.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_int),
-                                    C.POINTER(C.c_int), C.c_int, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.rf_detect_views.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(_View), C.c_int, C.c_float, C.c_float,
-                                    C.c_void_p, C.POINTER(C.c_int), C.c_void_p, C.c_void_p]
-    lib.rf_submit_batch.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_float, C.c_float, C.POINTER(C.c_int)]
-    lib.rf_collect_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.rf_detect_batch_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_float,
-                                           C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
-    lib.rf_forward_heads.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_void_p)]
-    lib.rf_postprocess.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_float, C.c_float,
-                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.rf_preprocess.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]
-    lib.rf_profile_layers.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
-    lib.rf_debug_get_tensor.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.c_void_p] + [C.POINTER(C.c_int)] * 3
-    lib.rf_debug_keep_all.argtypes = [C.c_void_p]
-    lib.rf_calibrate_int8.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_char_p]
-    lib.rf_kl_threshold_bins.argtypes = [C.c_void_p, C.c_int, C.c_int]
-    lib.rf_kl_threshold_bins.restype = C.c_double
-    lib.rf_cache_status.argtypes = [C.c_void_p]
-    lib.rf_comm_export.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
-    lib.rf_comm_init.argtypes = [C.c_void_p, C.c_void_p]
-    lib.rf_comm_nccl_unique_id.argtypes = [C.c_void_p]
-    lib.rf_comm_init_nccl.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
-    lib.rf_comm_info.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]
-    lib.rf_detect_batch_device_allgather.argtypes = lib.rf_detect_batch_device.argtypes
-    lib.rf_submit_batch_allgather.argtypes = lib.rf_submit_batch.argtypes
-    lib.rf_collect_batch_allgather.argtypes = lib.rf_collect_batch.argtypes
-    lib.rf_detect_batch_allgather.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.rf_detect_jpeg_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p,
-                                         C.c_void_p, C.c_void_p]
-    lib.rf_decode_jpeg.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
-    lib.rf_jpeg_backend.restype = C.c_char_p
-    lib.rf_jpeg_backend.argtypes = [C.c_void_p]
-    lib.rf_detect_align_batch.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int,
-                                          C.c_float, C.c_float, C.POINTER(AlignParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.rf_detect_align_batch_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_float, C.POINTER(AlignParams), C.c_void_p,
-                                                 C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
-    lib.rf_detect_yuv_batch.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_int, C.c_int, C.c_float, C.c_float, C.POINTER(AlignParams), C.c_void_p,
-                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.rf_detect_yuv_batch_device.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_int, C.c_int, C.c_float, C.c_float, C.POINTER(AlignParams),
-                                               C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_void_p]
-    lib.rf_preprocess_yuv.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_int, C.c_void_p]
-    lib.rf_tile_layout.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(Tiling), C.POINTER(Tile), C.c_int]
-    lib.rf_detect_tiled.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int,
-                                    C.POINTER(Tiling), C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.rf_detect_yuv_tiled.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_int, C.c_int, C.POINTER(Tiling), C.c_float, C.c_float, C.c_void_p,
-                                        C.c_void_p, C.c_void_p]
-    lib.rf_preprocess_tile.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(Tiling), C.c_int, C.c_void_p]
-    lib.rf_preprocess_yuv_tile.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_int, C.POINTER(Tiling), C.c_int, C.c_void_p]
-    lib.rf_detect_tiled_align.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int,
-                                          C.POINTER(Tiling), C.c_float, C.c_float, C.POINTER(AlignParams), C.c_void_p, C.c_void_p, C.c_void_p,
-                                          C.c_void_p, C.c_void_p]
-    lib.rf_detect_yuv_tiled_align.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_int, C.c_int, C.POINTER(Tiling), C.c_float, C.c_float,
-                                              C.POINTER(AlignParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.rf_detect_tiled_device.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int,
-                                           C.POINTER(Tiling), C.c_float, C.c_float, C.POINTER(AlignParams), C.c_void_p, C.c_void_p,
-                                           C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
-    lib.rf_detect_yuv_tiled_device.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_int, C.c_int, C.POINTER(Tiling), C.c_float, C.c_float,
-                                               C.POINTER(AlignParams), C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
-    lib.rf_detect_oriented_batch.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int),
-                                             C.POINTER(C.c_int), C.c_int, C.c_float, C.c_float, C.POINTER(AlignParams), C.c_void_p, C.c_void_p,
-                                             C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.rf_detect_yuv_oriented_device.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.POINTER(C.c_int), C.c_int, C.c_int, C.c_float, C.c_float,
-                                                  C.POINTER(AlignParams), C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
-                                                  C.c_void_p]
-    lib.rf_preprocess_oriented.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
-    lib.rf_preprocess_yuv_oriented.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_int, C.c_int, C.c_void_p]
-    lib.rf_detect_views_oriented.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(_OrientedView), C.c_int, C.c_float,
-                                             C.c_float, C.c_void_p, C.POINTER(C.c_int), C.c_void_p, C.c_void_p]
-    lib.rf_jpeg_exif_orientation.argtypes = [C.c_void_p, C.c_size_t]
-    lib.rf_tracker_create.argtypes = [C.c_void_p, C.POINTER(TrackConfig), C.POINTER(C.c_void_p)]
-    lib.rf_tracker_destroy.argtypes = [C.c_void_p]
-    lib.rf_tracker_destroy.restype = None
-    lib.rf_tracker_reset.argtypes = [C.c_void_p, C.c_int]
-    lib.rf_track_update.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p),
-                                    C.POINTER(C.c_void_p)]
-    lib.rf_detect_yuv_track_device.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(YuvFrame), C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float,
-                                               C.POINTER(AlignParams), C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
-                                               C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_void_p]
-    lib.rf_tracker_debug_state.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
-    lib.rf_tracker_create_best.argtypes = [C.c_void_p, C.POINTER(TrackConfig), C.POINTER(BestConfig), C.POINTER(C.c_void_p)]
-    lib.rf_detect_yuv_track_best_device.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(YuvFrame), C.c_void_p, C.c_int, C.c_int, C.c_float,
-                                                    C.c_float, C.c_void_p, C.c_void_p] + [C.POINTER(C.c_void_p)] * 6 + [C.c_void_p]
-    lib.rf_tracker_finish.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
-    lib.rf_tracker_set_motion.argtypes = [C.c_void_p, C.POINTER(MotionConfig)]
-    lib.rf_tracker_motion.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
-    lib.rf_redact_yuv_device.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                         C.c_void_p, C.POINTER(RedactParams)]
-    lib.rf_redact_device.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int,
-                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(RedactParams)]
-    lib.rf_redact_yuv_device_style.argtypes = lib.rf_redact_yuv_device.argtypes[:-1] + [C.POINTER(RedactStyle)]
-    lib.rf_redact_device_style.argtypes = lib.rf_redact_device.argtypes[:-1] + [C.POINTER(RedactStyle)]
-    lib.rf_detect_yuv_redact_device.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(YuvFrame), C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float,
-                                                C.POINTER(RedactParams), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
-                                                C.POINTER(C.c_void_p), C.c_void_p]
-    a = list(lib.rf_detect_yuv_redact_device.argtypes)
-    a[8] = C.POINTER(RedactStyle)
-    lib.rf_detect_yuv_redact_device_style.argtypes = a
-    lib.rf_tracker_set_lookback.argtypes = [C.c_void_p, C.POINTER(LookbackConfig)]
-    lib.rf_detect_yuv_redact_lookback_device.argtypes = a[:9] + [C.POINTER(YuvFrame), C.c_void_p] + a[9:]
-    lib.rf_tracker_drain.argtypes = [C.c_void_p, C.c_int, C.POINTER(RedactStyle), C.POINTER(YuvFrame), C.c_int, C.POINTER(C.c_int), C.c_void_p]
-    lib.rf_tracker_set_follow.argtypes = [C.c_void_p, C.POINTER(FollowConfig)]
-    lib.rf_track_follow_device.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_void_p, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
-    lib.rf_tracker_follow.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
-    lib.rf_tracker_set_lookback_search.argtypes = [C.c_void_p, C.POINTER(FollowConfig)]
-    lib.rf_tracker_lookback_search.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
-    lib.rf_track_follow_redact_device.argtypes = [C.c_void_p, C.POINTER(YuvFrame), C.c_void_p, C.c_int, C.POINTER(RedactStyle),
-                                                  C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
+    for name, (restype, argtypes) in _SIGNATURES.items():
+        fn = getattr(lib, name)
+        fn.restype, fn.argtypes = restype, argtypes
     _lib = lib
     return lib
 
@@ -497,7 +426,6 @@ def plan_describe(caffemodel: str, net_h: int, net_w: int, precision: int = RF_P
     cfg = _Config(caffemodel.encode(), int8_table.encode() if int8_table else None, precision, net_w, net_h, max_batch, max_faces, 0, 0, 0,
                   flags, streams, None, None, None)
     buf = C.create_string_buffer(1 << 16)
-    lib.rf_plan_describe.argtypes = [C.POINTER(_Config), C.c_char_p, C.c_int]
     rc = lib.rf_plan_describe(C.byref(cfg), buf, len(buf))
     if rc < 0:
         raise RfError(rc, (lib.rf_last_error(None) or b"").decode())
@@ -507,8 +435,6 @@ def plan_describe(caffemodel: str, net_h: int, net_w: int, precision: int = RF_P
 def model_load(caffemodel: str, prototxt: Optional[str] = None, cache: Optional[str] = None, layer: Optional[str] = None):
     """rf_model_load (host-only): the load path of rf_create.  Returns (cache_status, input_dims, (w, b) of `layer` or None)."""
     lib = load_library()
-    lib.rf_model_load.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_char_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int,
-                                  C.POINTER(C.c_int)]
     cs = C.c_int(0)
     idims = (C.c_int * 4)()
     dims = (C.c_int * 4)()
@@ -530,7 +456,6 @@ def model_load(caffemodel: str, prototxt: Optional[str] = None, cache: Optional[
 def network_config(network: str):
     """rf_network_config: (strides, scales per level, ratios) of the reference's network-name switch; RfError(-7) where unsupported."""
     lib = load_library()
-    lib.rf_network_config.argtypes = [C.c_char_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_float), C.POINTER(C.c_int)]
     nl, nr = C.c_int(0), C.c_int(0)
     strides, scales, ratios = (C.c_int * 3)(), (C.c_int * 6)(), (C.c_float * 2)()
     rc = lib.rf_network_config(network.encode(), C.byref(nl), strides, scales, ratios, C.byref(nr))
@@ -576,6 +501,23 @@ STRIDES = (32, 16, 8)
 
 def head_shapes(net_h: int, net_w: int) -> List[Tuple[int, int, int]]:
     return [(c, net_h // s, net_w // s) for s in STRIDES for c in (4, 8, 20)]
+
+
+def device_view(ptr: int, shape, typestr: str):
+    """A torch CUDA tensor aliasing the `shape` array of numpy type `typestr` (e.g. "<f4") at device address ptr, without a copy."""
+    import torch
+    cai = dict(shape=tuple(shape), typestr=typestr, data=(int(ptr), False), version=3)
+    return torch.as_tensor(types.SimpleNamespace(__cuda_array_interface__=cai), device="cuda")
+
+
+def _addr(a: Optional[np.ndarray]):
+    """The address of an optional host output array, as the C ABI takes it (NULL for None)."""
+    return a.ctypes.data if a is not None else None
+
+
+def _ref(s: Optional[C.Structure]):
+    """An optional structure passed by reference (NULL for None)."""
+    return C.byref(s) if s is not None else None
 
 
 class Engine:
@@ -645,6 +587,20 @@ class Engine:
     def last_stream_ptr(self) -> int:
         return int(self.lib.rf_last_stream(self.h) or 0)
 
+    def _fetch(self, ptr: int, dtype, *shape) -> np.ndarray:
+        """A host copy of the `shape` array of `dtype` records at device address ptr, taken after rf_synchronize."""
+        dtype = np.dtype(dtype)
+        self._check(self.lib.rf_synchronize(self.h))
+        return device_view(ptr, (int(np.prod(shape)) * dtype.itemsize,), "|u1").cpu().numpy().view(dtype).reshape(shape)
+
+    def read_dets(self, dets_ptr: int, counts_ptr: int, n: int):
+        """The rf_det records of n images of a device detect call, copied after rf_synchronize: (faces: one (k, 15) float32 array per
+        image, anchor_index: one (k,) int32 array per image)."""
+        rec = self._fetch(dets_ptr, np.float32, n, self.max_faces, FACE_FLOATS + 1)
+        counts = self._fetch(counts_ptr, np.int32, n)
+        return ([rec[i, :counts[i], :FACE_FLOATS].copy() for i in range(n)],
+                [rec[i, :counts[i], FACE_FLOATS].view(np.int32).copy() for i in range(n)])
+
     # -- end to end ------------------------------------------------------------------------
     def detect_batch(self, images: Sequence[np.ndarray], thr: float, nms_thr: float, want_index: bool = False):
         """images: u8 BGR HWC arrays (any size <= max_image).  Returns list of (k,15) float32 arrays
@@ -668,36 +624,62 @@ class Engine:
             return out, [idx[i, :counts[i]].copy() for i in range(n)]
         return out
 
+    # -- host arguments and results of the aligning, tiled and oriented calls ---------------------------------------------------
+    @staticmethod
+    def _bgr_strided(im):
+        """The image as the C ABI takes it: u8 BGR HWC with contiguous pixels (rows may be strided)."""
+        if im.ndim != 3 or im.shape[2] != 3:
+            raise ValueError(f"u8 BGR HWC images expected, got shape {im.shape}")
+        if not (im.dtype == np.uint8 and im.strides[1:] == (3, 1) and im.strides[0] >= 3 * im.shape[1]):
+            im = np.ascontiguousarray(im, dtype=np.uint8)
+        return im
+
+    @staticmethod
+    def _host_images(images):
+        """(the arrays to keep alive, pointers, widths, heights, row strides) of host u8 BGR HWC images, each as _bgr_strided."""
+        keep = [Engine._bgr_strided(im) for im in images]
+        n = max(len(keep), 1)
+        return (keep, (C.c_void_p * n)(*[im.ctypes.data for im in keep]), (C.c_int * n)(*[im.shape[1] for im in keep]),
+                (C.c_int * n)(*[im.shape[0] for im in keep]), (C.c_int * n)(*[im.strides[0] for im in keep]))
+
+    def _outputs(self, n: int, index: bool):
+        """The host faces, counts and (with index) per-face int32 arrays a detect call on n images writes."""
+        return (np.empty((n, self.max_faces, FACE_FLOATS), dtype=np.float32), np.zeros(n, dtype=np.int32),
+                np.empty((n, self.max_faces), dtype=np.int32) if index else None)
+
+    def _host_align(self, n: int, align: dict):
+        """rf_align_params and the host crop / matrix arrays of detect_align's keywords: (params, A, crops, mats or None)."""
+        kw = dict(align)
+        want_mats = kw.pop("want_mats", False)
+        p = align_params(**{"fmt": "bgr_u8", **kw})
+        A = p.max_faces or self.max_faces
+        shape, dt = crop_shape(kw.get("fmt", "bgr_u8"), (p.crop_w, p.crop_h))
+        return p, A, np.empty((n, A) + shape, dtype=dt), (np.empty((n, A, 2, 3), dtype=np.float64) if want_mats else None)
+
+    @staticmethod
+    def _result(counts, faces, tile_of=None, A=0, crops=None, mats=None, idx=None):
+        """A host call's per-image lists (faces[, tile_of][, crops[, mats]][, idx]), each array cut to its image's count (the crops
+        and matrices to at most A); the faces alone when nothing else was asked for."""
+        n = len(counts)
+        out = [[a[i, :counts[i]].copy() for i in range(n)] for a in (faces, tile_of) if a is not None]
+        out += [[a[i, :min(counts[i], A)].copy() for i in range(n)] for a in (crops, mats) if a is not None]
+        if idx is not None:
+            out.append([idx[i, :counts[i]].copy() for i in range(n)])
+        return out[0] if len(out) == 1 else tuple(out)
+
     def detect_align(self, images: Sequence[np.ndarray], thr: float, nms_thr: float, crop=(112, 112), template=None, fmt: str = "bgr_u8",
                      max_faces: int = 0, want_mats: bool = False, mean: float = 0.0, std: float = 0.0):
         """rf_detect_align_batch: u8 BGR HWC images (any size <= max_image; rows may be strided, e.g. a slice of a larger array)
         -> (faces: list of (k, 15) float32 arrays in ORIGINAL IMAGE pixels, crops: list of (min(k, A), *crop_shape) arrays
         [, mats: list of (min(k, A), 2, 3) float64 image -> crop matrices]), A = max_faces or the engine's max_faces."""
         n = len(images)
-        keep = []
-        for im in images:
-            if im.ndim != 3 or im.shape[2] != 3:
-                raise ValueError(f"u8 BGR HWC images expected, got shape {im.shape}")
-            if not (im.dtype == np.uint8 and im.strides[1:] == (3, 1) and im.strides[0] >= 3 * im.shape[1]):
-                im = np.ascontiguousarray(im, dtype=np.uint8)
-            keep.append(im)
-        p = align_params(crop, template, fmt, max_faces, mean, std)
-        A = max_faces or self.max_faces
-        shape, dt = crop_shape(fmt, (p.crop_w, p.crop_h))
-        ptrs = (C.c_void_p * max(n, 1))(*[im.ctypes.data for im in keep])
-        ws = (C.c_int * max(n, 1))(*[im.shape[1] for im in keep])
-        hs = (C.c_int * max(n, 1))(*[im.shape[0] for im in keep])
-        rs = (C.c_int * max(n, 1))(*[im.strides[0] for im in keep])
-        faces = np.empty((n, self.max_faces, FACE_FLOATS), dtype=np.float32)
-        counts = np.zeros(n, dtype=np.int32)
-        crops = np.empty((n, A) + shape, dtype=dt)
-        mats = np.empty((n, A, 2, 3), dtype=np.float64) if want_mats else None
+        keep, ptrs, ws, hs, rs = self._host_images(images)
+        p, A, crops, mats = self._host_align(n, dict(crop=crop, template=template, fmt=fmt, max_faces=max_faces, mean=mean, std=std,
+                                                     want_mats=want_mats))
+        faces, counts, _ = self._outputs(n, False)
         self._check(self.lib.rf_detect_align_batch(self.h, ptrs, ws, hs, rs, n, thr, nms_thr, C.byref(p), faces.ctypes.data, counts.ctypes.data,
-                                                   crops.ctypes.data, mats.ctypes.data if want_mats else None))
-        out = ([faces[i, :counts[i]].copy() for i in range(n)], [crops[i, :min(counts[i], A)].copy() for i in range(n)])
-        if want_mats:
-            out += ([mats[i, :min(counts[i], A)].copy() for i in range(n)],)
-        return out
+                                                   crops.ctypes.data, _addr(mats)))
+        return self._result(counts, faces, A=A, crops=crops, mats=mats)
 
     def detect_align_device(self, n: int, thr: float, nms_thr: float, dev_crops_ptr: int, crop=(112, 112), template=None, fmt: str = "bgr_u8",
                             max_faces: int = 0, mean: float = 0.0, std: float = 0.0, dev_mats_ptr: Optional[int] = None,
@@ -725,31 +707,11 @@ class Engine:
         as detect_align returns them.  want_index appends the anchor-index arrays."""
         n = len(frames)
         arr = self._frames(frames, layout, False)
-        faces = np.empty((n, self.max_faces, FACE_FLOATS), dtype=np.float32)
-        counts = np.zeros(n, dtype=np.int32)
-        idx = np.empty((n, self.max_faces), dtype=np.int32) if want_index else None
-        p = crops = mats = None
-        if align is not None:
-            kw = dict(align)
-            want_mats = kw.pop("want_mats", False)
-            p = align_params(**{"fmt": "bgr_u8", **kw})
-            A = p.max_faces or self.max_faces
-            shape, dt = crop_shape(kw.get("fmt", "bgr_u8"), (p.crop_w, p.crop_h))
-            crops = np.empty((n, A) + shape, dtype=dt)
-            mats = np.empty((n, A, 2, 3), dtype=np.float64) if want_mats else None
-        self._check(self.lib.rf_detect_yuv_batch(self.h, arr, n, _matrix(matrix), thr, nms_thr, C.byref(p) if p is not None else None,
-                                                 faces.ctypes.data, counts.ctypes.data, idx.ctypes.data if want_index else None,
-                                                 crops.ctypes.data if crops is not None else None, mats.ctypes.data if mats is not None else None))
-        out = [faces[i, :counts[i]].copy() for i in range(n)]
-        if align is not None:
-            out = (out, [crops[i, :min(counts[i], A)].copy() for i in range(n)])
-            if mats is not None:
-                out += ([mats[i, :min(counts[i], A)].copy() for i in range(n)],)
-        else:
-            out = (out,)
-        if want_index:
-            out += ([idx[i, :counts[i]].copy() for i in range(n)],)
-        return out[0] if len(out) == 1 else out
+        faces, counts, idx = self._outputs(n, want_index)
+        p, A, crops, mats = self._host_align(n, align) if align is not None else (None, 0, None, None)
+        self._check(self.lib.rf_detect_yuv_batch(self.h, arr, n, _matrix(matrix), thr, nms_thr, _ref(p), faces.ctypes.data, counts.ctypes.data,
+                                                 _addr(idx), _addr(crops), _addr(mats)))
+        return self._result(counts, faces, A=A, crops=crops, mats=mats, idx=idx)
 
     def detect_yuv_device(self, frames, thr: float, nms_thr: float, layout: str = "nv12", matrix="bt601", align: Optional[dict] = None,
                           dev_crops_ptr: Optional[int] = None, dev_mats_ptr: Optional[int] = None):
@@ -761,7 +723,7 @@ class Engine:
         p = align_params(**align) if align is not None else None
         scales = np.zeros(max(n, 1), dtype=np.float32)
         d, c = C.c_void_p(), C.c_void_p()
-        self._check(self.lib.rf_detect_yuv_batch_device(self.h, arr, n, _matrix(matrix), thr, nms_thr, C.byref(p) if p is not None else None,
+        self._check(self.lib.rf_detect_yuv_batch_device(self.h, arr, n, _matrix(matrix), thr, nms_thr, _ref(p),
                                                         dev_crops_ptr, dev_mats_ptr, C.byref(d), C.byref(c), scales.ctypes.data))
         return int(d.value), int(c.value), scales[:n].copy()
 
@@ -773,37 +735,6 @@ class Engine:
         return out
 
     # -- f7 tiled detection ----------------------------------------------------------------------------
-    @staticmethod
-    def _bgr_strided(im):
-        """The image as the C ABI takes it: u8 BGR HWC with contiguous pixels (rows may be strided)."""
-        if im.ndim != 3 or im.shape[2] != 3:
-            raise ValueError(f"u8 BGR HWC images expected, got shape {im.shape}")
-        if not (im.dtype == np.uint8 and im.strides[1:] == (3, 1) and im.strides[0] >= 3 * im.shape[1]):
-            im = np.ascontiguousarray(im, dtype=np.uint8)
-        return im
-
-    def _tiled_out(self, n):
-        return (np.empty((n, self.max_faces, FACE_FLOATS), dtype=np.float32), np.zeros(n, dtype=np.int32),
-                np.empty((n, self.max_faces), dtype=np.int32))
-
-    def _host_align(self, n: int, align: dict):
-        """rf_align_params and the host crop / matrix arrays of detect_yuv's align keywords: (params, A, crops, mats or None)."""
-        kw = dict(align)
-        want_mats = kw.pop("want_mats", False)
-        p = align_params(**{"fmt": "bgr_u8", **kw})
-        A = p.max_faces or self.max_faces
-        shape, dt = crop_shape(kw.get("fmt", "bgr_u8"), (p.crop_w, p.crop_h))
-        return p, A, np.empty((n, A) + shape, dtype=dt), (np.empty((n, A, 2, 3), dtype=np.float64) if want_mats else None)
-
-    @staticmethod
-    def _tiled_result(n, faces, counts, tile_of, A=0, crops=None, mats=None):
-        out = ([faces[i, :counts[i]].copy() for i in range(n)], [tile_of[i, :counts[i]].copy() for i in range(n)])
-        if crops is not None:
-            out += ([crops[i, :min(counts[i], A)].copy() for i in range(n)],)
-            if mats is not None:
-                out += ([mats[i, :min(counts[i], A)].copy() for i in range(n)],)
-        return out
-
     def detect_tiled(self, images: Sequence[np.ndarray], thr: float, nms_thr: float, levels=None, overlap: int = 0, align: Optional[dict] = None):
         """rf_detect_tiled: u8 BGR HWC images (any size <= max_image; rows may be strided) cut into tiles of a scale pyramid
         (levels: [(scale, flip), ...], scale 0 = the fitted level; None = the default pyramid).  Returns (faces: one (k, 15) float32
@@ -811,22 +742,17 @@ class Engine:
         keywords (crop, template, fmt, max_faces, mean, std, want_mats) -> rf_detect_tiled_align, and the crops (and matrices) follow:
         (faces, tile_of, crops[, mats]) as detect_align returns them."""
         n = len(images)
-        keep = [self._bgr_strided(im) for im in images]
-        ptrs = (C.c_void_p * max(n, 1))(*[im.ctypes.data for im in keep])
-        ws = (C.c_int * max(n, 1))(*[im.shape[1] for im in keep])
-        hs = (C.c_int * max(n, 1))(*[im.shape[0] for im in keep])
-        rs = (C.c_int * max(n, 1))(*[im.strides[0] for im in keep])
+        keep, ptrs, ws, hs, rs = self._host_images(images)
         t = tiling(levels, overlap)
-        faces, counts, tile_of = self._tiled_out(n)
+        faces, counts, tile_of = self._outputs(n, True)
         if align is None:
             self._check(self.lib.rf_detect_tiled(self.h, ptrs, ws, hs, rs, n, C.byref(t), thr, nms_thr, faces.ctypes.data, counts.ctypes.data,
                                                  tile_of.ctypes.data))
-            return self._tiled_result(n, faces, counts, tile_of)
+            return self._result(counts, faces, tile_of)
         p, A, crops, mats = self._host_align(n, align)
         self._check(self.lib.rf_detect_tiled_align(self.h, ptrs, ws, hs, rs, n, C.byref(t), thr, nms_thr, C.byref(p), faces.ctypes.data,
-                                                   counts.ctypes.data, tile_of.ctypes.data, crops.ctypes.data,
-                                                   mats.ctypes.data if mats is not None else None))
-        return self._tiled_result(n, faces, counts, tile_of, A, crops, mats)
+                                                   counts.ctypes.data, tile_of.ctypes.data, crops.ctypes.data, _addr(mats)))
+        return self._result(counts, faces, tile_of, A, crops, mats)
 
     def detect_yuv_tiled(self, frames, thr: float, nms_thr: float, layout: str = "nv12", matrix="bt601", levels=None, overlap: int = 0,
                          align: Optional[dict] = None):
@@ -835,16 +761,15 @@ class Engine:
         n = len(frames)
         arr = self._frames(frames, layout, False)
         t = tiling(levels, overlap)
-        faces, counts, tile_of = self._tiled_out(n)
+        faces, counts, tile_of = self._outputs(n, True)
         if align is None:
             self._check(self.lib.rf_detect_yuv_tiled(self.h, arr, n, _matrix(matrix), C.byref(t), thr, nms_thr, faces.ctypes.data,
                                                      counts.ctypes.data, tile_of.ctypes.data))
-            return self._tiled_result(n, faces, counts, tile_of)
+            return self._result(counts, faces, tile_of)
         p, A, crops, mats = self._host_align(n, align)
         self._check(self.lib.rf_detect_yuv_tiled_align(self.h, arr, n, _matrix(matrix), C.byref(t), thr, nms_thr, C.byref(p), faces.ctypes.data,
-                                                       counts.ctypes.data, tile_of.ctypes.data, crops.ctypes.data,
-                                                       mats.ctypes.data if mats is not None else None))
-        return self._tiled_result(n, faces, counts, tile_of, A, crops, mats)
+                                                       counts.ctypes.data, tile_of.ctypes.data, crops.ctypes.data, _addr(mats)))
+        return self._result(counts, faces, tile_of, A, crops, mats)
 
     @staticmethod
     def _device_images(images):
@@ -871,7 +796,7 @@ class Engine:
         t = tiling(levels, overlap)
         p = align_params(**align) if align is not None else None
         d, c = C.c_void_p(), C.c_void_p()
-        self._check(self.lib.rf_detect_tiled_device(self.h, ptrs, ws, hs, rs, n, C.byref(t), thr, nms_thr, C.byref(p) if p is not None else None,
+        self._check(self.lib.rf_detect_tiled_device(self.h, ptrs, ws, hs, rs, n, C.byref(t), thr, nms_thr, _ref(p),
                                                     dev_crops_ptr, dev_mats_ptr, C.byref(d), C.byref(c)))
         return int(d.value or 0), int(c.value or 0)
 
@@ -885,7 +810,7 @@ class Engine:
         p = align_params(**align) if align is not None else None
         d, c = C.c_void_p(), C.c_void_p()
         self._check(self.lib.rf_detect_yuv_tiled_device(self.h, arr, n, _matrix(matrix), C.byref(t), thr, nms_thr,
-                                                        C.byref(p) if p is not None else None, dev_crops_ptr, dev_mats_ptr, C.byref(d), C.byref(c)))
+                                                        _ref(p), dev_crops_ptr, dev_mats_ptr, C.byref(d), C.byref(c)))
         return int(d.value or 0), int(c.value or 0)
 
     def preprocess_tile(self, img: np.ndarray, tile: int, levels=None, overlap: int = 0) -> np.ndarray:
@@ -1053,31 +978,13 @@ class Engine:
         on T_o(img) -- without a rotated copy ever being made.  align: detect_align's keywords -> (faces, crops[, mats]), the crops
         cut from the displayed image.  want_index appends the anchor-index arrays."""
         n = len(images)
-        keep = [self._bgr_strided(im) for im in images]
+        keep, ptrs, ws, hs, rs = self._host_images(images)
         arr = _orientations(orientations, n)
-        ptrs = (C.c_void_p * max(n, 1))(*[im.ctypes.data for im in keep])
-        ws = (C.c_int * max(n, 1))(*[im.shape[1] for im in keep])
-        hs = (C.c_int * max(n, 1))(*[im.shape[0] for im in keep])
-        rs = (C.c_int * max(n, 1))(*[im.strides[0] for im in keep])
-        faces = np.empty((n, self.max_faces, FACE_FLOATS), dtype=np.float32)
-        counts = np.zeros(n, dtype=np.int32)
-        idx = np.empty((n, self.max_faces), dtype=np.int32) if want_index else None
-        p = crops = mats = None
-        A = 0
-        if align is not None:
-            p, A, crops, mats = self._host_align(n, align)
-        self._check(self.lib.rf_detect_oriented_batch(self.h, ptrs, ws, hs, rs, arr, n, thr, nms_thr, C.byref(p) if p is not None else None,
-                                                      faces.ctypes.data, counts.ctypes.data, idx.ctypes.data if want_index else None,
-                                                      crops.ctypes.data if crops is not None else None,
-                                                      mats.ctypes.data if mats is not None else None))
-        out = ([faces[i, :counts[i]].copy() for i in range(n)],)
-        if align is not None:
-            out += ([crops[i, :min(counts[i], A)].copy() for i in range(n)],)
-            if mats is not None:
-                out += ([mats[i, :min(counts[i], A)].copy() for i in range(n)],)
-        if want_index:
-            out += ([idx[i, :counts[i]].copy() for i in range(n)],)
-        return out[0] if len(out) == 1 else out
+        faces, counts, idx = self._outputs(n, want_index)
+        p, A, crops, mats = self._host_align(n, align) if align is not None else (None, 0, None, None)
+        self._check(self.lib.rf_detect_oriented_batch(self.h, ptrs, ws, hs, rs, arr, n, thr, nms_thr, _ref(p), faces.ctypes.data,
+                                                      counts.ctypes.data, _addr(idx), _addr(crops), _addr(mats)))
+        return self._result(counts, faces, A=A, crops=crops, mats=mats, idx=idx)
 
     def detect_yuv_oriented_device(self, frames, orientations: Sequence[int], thr: float, nms_thr: float, layout: str = "nv12", matrix="bt601",
                                    align: Optional[dict] = None, dev_crops_ptr: Optional[int] = None, dev_mats_ptr: Optional[int] = None):
@@ -1090,7 +997,7 @@ class Engine:
         p = align_params(**align) if align is not None else None
         scales = np.zeros(max(n, 1), dtype=np.float32)
         d, c = C.c_void_p(), C.c_void_p()
-        self._check(self.lib.rf_detect_yuv_oriented_device(self.h, arr, o, n, _matrix(matrix), thr, nms_thr, C.byref(p) if p is not None else None,
+        self._check(self.lib.rf_detect_yuv_oriented_device(self.h, arr, o, n, _matrix(matrix), thr, nms_thr, _ref(p),
                                                            dev_crops_ptr, dev_mats_ptr, C.byref(d), C.byref(c), scales.ctypes.data))
         return int(d.value or 0), int(c.value or 0), scales[:n].copy()
 
@@ -1172,14 +1079,9 @@ class Engine:
         n = len(frames)
         arr = self._frames(frames, layout, True)
         sc = self._scales(scales, n)
-        st = redact_style(style, shape, blocks, detail, margin)
-        args = (self.h, arr, n, dets_ptr, counts_ptr, sc.ctypes.data if sc is not None else None, tracker.t if tracker is not None else None,
-                tracks_ptr, track_counts_ptr)
-        if st is not None:
-            self._check(self.lib.rf_redact_yuv_device_style(*args, C.byref(st)))
-            return
-        p = RedactParams(int(blocks), float(margin))
-        self._check(self.lib.rf_redact_yuv_device(*args, C.byref(p)))
+        fn, p = _redaction(self.lib, "rf_redact_yuv_device", style, shape, blocks, detail, margin)
+        self._check(fn(self.h, arr, n, dets_ptr, counts_ptr, _addr(sc), tracker.t if tracker is not None else None, tracks_ptr,
+                       track_counts_ptr, C.byref(p)))
 
     def redact_device(self, images, dets_ptr: int, counts_ptr: int, scales=None, tracker: Optional["Tracker"] = None,
                       tracks_ptr: Optional[int] = None, track_counts_ptr: Optional[int] = None, blocks: int = 0, margin: float = 0.0,
@@ -1188,14 +1090,9 @@ class Engine:
         n = len(images)
         ptrs, ws, hs, rs = self._device_images(images)
         sc = self._scales(scales, n)
-        st = redact_style(style, shape, blocks, detail, margin)
-        args = (self.h, ptrs, ws, hs, rs, n, dets_ptr, counts_ptr, sc.ctypes.data if sc is not None else None,
-                tracker.t if tracker is not None else None, tracks_ptr, track_counts_ptr)
-        if st is not None:
-            self._check(self.lib.rf_redact_device_style(*args, C.byref(st)))
-            return
-        p = RedactParams(int(blocks), float(margin))
-        self._check(self.lib.rf_redact_device(*args, C.byref(p)))
+        fn, p = _redaction(self.lib, "rf_redact_device", style, shape, blocks, detail, margin)
+        self._check(fn(self.h, ptrs, ws, hs, rs, n, dets_ptr, counts_ptr, _addr(sc), tracker.t if tracker is not None else None, tracks_ptr,
+                       track_counts_ptr, C.byref(p)))
 
     def detect_yuv_redact_device(self, frames, thr: float, nms_thr: float, layout: str = "nv12", matrix="bt601", blocks: int = 0,
                                  margin: float = 0.0, style: str = "mosaic", shape: str = "rect", detail: int = 0):
@@ -1203,7 +1100,7 @@ class Engine:
         context.  Returns (dets_ptr, counts_ptr, scales) as detect_yuv_device; the frames are redacted in place."""
         n = len(frames)
         arr = self._frames(frames, layout, True)
-        fn, p = _redact_call(self.lib, style, shape, blocks, detail, margin)
+        fn, p = _redaction(self.lib, "rf_detect_yuv_redact_device", style, shape, blocks, detail, margin)
         scales = np.zeros(max(n, 1), dtype=np.float32)
         d, c = C.c_void_p(), C.c_void_p()
         self._check(fn(self.h, None, arr, None, n, _matrix(matrix), thr, nms_thr, C.byref(p), None, None, C.byref(d), C.byref(c),
@@ -1241,11 +1138,6 @@ class Engine:
             nm = names.raw[64 * i:64 * (i + 1)].split(b"\0", 1)[0].decode()
             out.append(dict(name=nm, ms=float(ms[i]), bytes=float(by[i]), flops=float(fl[i])))
         return out
-
-
-class _DevArray:
-    def __init__(self, ptr, shape, typestr):
-        self.__cuda_array_interface__ = dict(shape=shape, typestr=typestr, data=(ptr, False), version=3)
 
 
 class Tracker:
@@ -1289,12 +1181,9 @@ class Tracker:
         """rf_track_update on the device records of a detect call (frame i of video videos[i]; scales: the map-back factor of each
         frame, None for records already in image pixels).  Asynchronous.  Returns the (tracks_ptr, track_counts_ptr) device addresses."""
         n = len(videos)
-        sc = None if scales is None else np.ascontiguousarray(scales, dtype=np.float32)
-        if sc is not None and sc.size != n:
-            raise ValueError(f"{n} frames but {sc.size} scales")
+        sc = self.engine._scales(scales, n)
         tp, cp = C.c_void_p(), C.c_void_p()
-        self.engine._check(self.lib.rf_track_update(self.t, self._ints(videos, n), n, dets_ptr, counts_ptr, sc.ctypes.data if sc is not None else None,
-                                                    C.byref(tp), C.byref(cp)))
+        self.engine._check(self.lib.rf_track_update(self.t, self._ints(videos, n), n, dets_ptr, counts_ptr, _addr(sc), C.byref(tp), C.byref(cp)))
         return int(tp.value or 0), int(cp.value or 0)
 
     def detect_yuv_device(self, frames, videos: Sequence[int], thr: float, nms_thr: float, layout: str = "nv12", matrix="bt601",
@@ -1307,7 +1196,7 @@ class Tracker:
         scales = np.zeros(max(n, 1), dtype=np.float32)
         tp, tc, d, c = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
         self.engine._check(self.lib.rf_detect_yuv_track_device(self.engine.h, self.t, arr, self._ints(videos, n), n, _matrix(matrix), thr, nms_thr,
-                                                               C.byref(p) if p is not None else None, dev_crops_ptr, dev_mats_ptr, C.byref(tp),
+                                                               _ref(p), dev_crops_ptr, dev_mats_ptr, C.byref(tp),
                                                                C.byref(tc), C.byref(d), C.byref(c), scales.ctypes.data))
         return int(tp.value or 0), int(tc.value or 0), int(d.value or 0), int(c.value or 0), scales[:n].copy()
 
@@ -1332,7 +1221,7 @@ class Tracker:
         every LOST track, in place.  Returns (tracks_ptr, track_counts_ptr, dets_ptr, counts_ptr, scales) as detect_yuv_device."""
         n = len(frames)
         arr = self.engine._frames(frames, layout, True)
-        fn, p = _redact_call(self.lib, style, shape, blocks, detail, margin)
+        fn, p = _redaction(self.lib, "rf_detect_yuv_redact_device", style, shape, blocks, detail, margin)
         scales = np.zeros(max(n, 1), dtype=np.float32)
         tp, tc, d, c = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
         self.engine._check(fn(self.engine.h, self.t, arr, self._ints(videos, n), n, _matrix(matrix), thr, nms_thr, C.byref(p), C.byref(tp),
@@ -1348,11 +1237,9 @@ class Tracker:
 
     def read_best(self, best_ptr: int, counts_ptr: int, n: int) -> List[np.ndarray]:
         """The emitted shots of n frames (BEST_DTYPE records, id order), copied to the host after the last stream."""
-        import torch
-        self.engine._check(self.lib.rf_synchronize(self.engine.h))
-        raw = torch.as_tensor(_DevArray(best_ptr, (n, self.max_tracks * BEST_DTYPE.itemsize), "|u1"), device="cuda").cpu().numpy()
-        counts = torch.as_tensor(_DevArray(counts_ptr, (n,), "<i4"), device="cuda").cpu().numpy()
-        return [raw[i].view(BEST_DTYPE)[:counts[i]].copy() for i in range(n)]
+        raw = self.engine._fetch(best_ptr, BEST_DTYPE, n, self.max_tracks)
+        counts = self.engine._fetch(counts_ptr, np.int32, n)
+        return [raw[i, :counts[i]].copy() for i in range(n)]
 
     def set_motion(self, search: int = 0, min_inliers: int = 0):
         """rf_tracker_set_motion, before the first update."""
@@ -1362,14 +1249,11 @@ class Tracker:
 
     def motion(self, n: int) -> np.ndarray:
         """rf_tracker_motion: the n rf_motion records (MOTION_DTYPE) of the latest frame call, copied after the last stream."""
-        import torch
         p = C.c_void_p()
         self.engine._check(self.lib.rf_tracker_motion(self.t, C.byref(p)))
         if not p.value:
             raise RuntimeError("no frame call has been made on this tracker")
-        self.engine._check(self.lib.rf_synchronize(self.engine.h))
-        raw = torch.as_tensor(_DevArray(int(p.value), (n * MOTION_DTYPE.itemsize,), "|u1"), device="cuda").cpu().numpy()
-        return raw.view(MOTION_DTYPE).copy()
+        return self.engine._fetch(p.value, MOTION_DTYPE, n)
 
     def set_lookback(self, frames: int = 0, grow: float = 0.0):
         """rf_tracker_set_lookback, before the first update: keep each video's last L frames (0 -> 15) on the GPU and emit every frame L
@@ -1389,13 +1273,12 @@ class Tracker:
             raise ValueError(f"{n} frames but {len(out_frames)} out frames")
         arr = self.engine._frames(frames, layout, True)
         outs = self.engine._frames(out_frames, layout, True)
-        st = _style_struct(style, shape, blocks, detail, margin)
+        fn, st = _redaction(self.lib, "rf_detect_yuv_redact_lookback_device", style, shape, blocks, detail, margin)
         nums = np.full(max(n, 1), -1, dtype=np.int32)
         scales = np.zeros(max(n, 1), dtype=np.float32)
         tp, tc, d, c = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
-        self.engine._check(self.lib.rf_detect_yuv_redact_lookback_device(self.engine.h, self.t, arr, self._ints(videos, n), n, _matrix(matrix), thr,
-                                                                         nms_thr, C.byref(st), outs, nums.ctypes.data, C.byref(tp), C.byref(tc),
-                                                                         C.byref(d), C.byref(c), scales.ctypes.data))
+        self.engine._check(fn(self.engine.h, self.t, arr, self._ints(videos, n), n, _matrix(matrix), thr, nms_thr, C.byref(st), outs,
+                              nums.ctypes.data, C.byref(tp), C.byref(tc), C.byref(d), C.byref(c), scales.ctypes.data))
         return nums[:n].copy(), int(tp.value or 0), int(tc.value or 0), int(d.value or 0), int(c.value or 0), scales[:n].copy()
 
     def set_lookback_search(self, search: int = 0, max_mad: float = 0.0):
@@ -1408,16 +1291,12 @@ class Tracker:
     def lookback_search(self, n: int):
         """rf_tracker_lookback_search: the latest look-back call's [n][min(max_faces, max_tracks)][L] step records (FOLLOW_DTYPE) and
         [n][min(max_faces, max_tracks)] chain lengths, copied after the last stream."""
-        import torch
         p, q = C.c_void_p(), C.c_void_p()
         self.engine._check(self.lib.rf_tracker_lookback_search(self.t, C.byref(p), C.byref(q)))
         if not p.value:
             raise RuntimeError("no look-back call has been made on this tracker")
-        self.engine._check(self.lib.rf_synchronize(self.engine.h))
         bcap = min(self.engine.max_faces, self.max_tracks)
-        raw = torch.as_tensor(_DevArray(int(p.value), (n * bcap * self.lookback * FOLLOW_DTYPE.itemsize,), "|u1"), device="cuda").cpu().numpy()
-        lens = torch.as_tensor(_DevArray(int(q.value), (n * bcap * 4,), "|u1"), device="cuda").cpu().numpy()
-        return raw.view(FOLLOW_DTYPE).reshape(n, bcap, self.lookback).copy(), lens.view(np.int32).reshape(n, bcap).copy()
+        return self.engine._fetch(p.value, FOLLOW_DTYPE, n, bcap, self.lookback), self.engine._fetch(q.value, np.int32, n, bcap)
 
     def drain(self, video: int, out_frames, layout: str = "nv12", blocks: int = 0, margin: float = 0.0, style: str = "mosaic",
               shape: str = "rect", detail: int = 0) -> np.ndarray:
@@ -1425,10 +1304,10 @@ class Tracker:
         Returns the numbers of the frames written."""
         k = len(out_frames)
         outs = self.engine._frames(out_frames, layout, True) if k else None
-        st = _style_struct(style, shape, blocks, detail, margin)
+        fn, st = _redaction(self.lib, "rf_tracker_drain", style, shape, blocks, detail, margin)
         nums = np.zeros(max(k, 1), dtype=np.int32)
         n_out = C.c_int(0)
-        self.engine._check(self.lib.rf_tracker_drain(self.t, int(video), C.byref(st), outs, k, C.byref(n_out), nums.ctypes.data))
+        self.engine._check(fn(self.t, int(video), C.byref(st), outs, k, C.byref(n_out), nums.ctypes.data))
         return nums[:n_out.value].copy()
 
     def set_follow(self, search: int = 0, max_mad: float = 0.0):
@@ -1453,22 +1332,19 @@ class Tracker:
         track (``redact_style``'s keywords).  Returns the (tracks_ptr, track_counts_ptr) device addresses."""
         n = len(frames)
         arr = self.engine._frames(frames, layout, True)
-        st = _style_struct(style, shape, blocks, detail, margin)
+        fn, st = _redaction(self.lib, "rf_track_follow_redact_device", style, shape, blocks, detail, margin)
         tp, tc = C.c_void_p(), C.c_void_p()
-        self.engine._check(self.lib.rf_track_follow_redact_device(self.t, arr, self._ints(videos, n), n, C.byref(st), C.byref(tp), C.byref(tc)))
+        self.engine._check(fn(self.t, arr, self._ints(videos, n), n, C.byref(st), C.byref(tp), C.byref(tc)))
         return int(tp.value or 0), int(tc.value or 0)
 
     def follow(self, n: int) -> np.ndarray:
         """rf_tracker_follow: the [n][max_tracks] rf_follow records (FOLLOW_DTYPE) of the latest follow call, each frame's in its
         track-list order, copied after the last stream."""
-        import torch
         p = C.c_void_p()
         self.engine._check(self.lib.rf_tracker_follow(self.t, C.byref(p)))
         if not p.value:
             raise RuntimeError("no follow call has been made on this tracker")
-        self.engine._check(self.lib.rf_synchronize(self.engine.h))
-        raw = torch.as_tensor(_DevArray(int(p.value), (n * self.max_tracks * FOLLOW_DTYPE.itemsize,), "|u1"), device="cuda").cpu().numpy()
-        return raw.view(FOLLOW_DTYPE).reshape(n, self.max_tracks).copy()
+        return self.engine._fetch(p.value, FOLLOW_DTYPE, n, self.max_tracks)
 
     def reset(self, video: int = -1):
         """rf_tracker_reset: restart one video (ids from 1), or all with -1; ordered after every issued update."""
@@ -1483,8 +1359,6 @@ class Tracker:
 
     def read(self, tracks_ptr: int, counts_ptr: int, n: int) -> List[np.ndarray]:
         """The track lists of n frames of an update's outputs (TRACK_DTYPE records), copied to the host after the last stream."""
-        import torch
-        self.engine._check(self.lib.rf_synchronize(self.engine.h))
-        raw = torch.as_tensor(_DevArray(tracks_ptr, (n, self.max_tracks * TRACK_DTYPE.itemsize), "|u1"), device="cuda").cpu().numpy()
-        counts = torch.as_tensor(_DevArray(counts_ptr, (n,), "<i4"), device="cuda").cpu().numpy()
-        return [raw[i].view(TRACK_DTYPE)[:counts[i]].copy() for i in range(n)]
+        raw = self.engine._fetch(tracks_ptr, TRACK_DTYPE, n, self.max_tracks)
+        counts = self.engine._fetch(counts_ptr, np.int32, n)
+        return [raw[i, :counts[i]].copy() for i in range(n)]

@@ -14,7 +14,7 @@ from typing import List, Sequence
 
 import numpy as np
 
-from .capi import ANY_ORIENTATION, RF_PREC_FP16, Engine
+from .capi import ANY_ORIENTATION, CROP_FORMATS, RF_PREC_FP16, Engine, crop_shape
 
 
 @dataclass
@@ -168,8 +168,6 @@ class RetinaFace:
         f16 detection interval: with ``detect_every=k`` > 1 the tracker is a follow tracker; each video's frames whose number is
         divisible by k are detected, the others followed by template search without the detector (rf_track_follow_device).  A call
         mixing both kinds is split into detect and follow calls; each video's frames keep their order.  Follow frames have no crops."""
-        import torch
-        from .capi import crop_shape
         if best is not None and align is not None:
             raise ValueError("best shots and new-identity crops are exclusive: pass best or align, not both")
         self._interval_tracker(detect_every, best=best)
@@ -183,7 +181,7 @@ class RetinaFace:
                     t, c = self._track_call(fr, vi, threshold, layout, matrix, align)
                 else:
                     tp, tc = self._tracker.follow_device(fr, vi, layout=layout)
-                    t = self._lists(tp, tc, len(idx))
+                    t = self._lists(self._tracker.read(tp, tc, len(idx)))
                     c = [[] for _ in idx]
                 for j, i in enumerate(idx):
                     tracks[i], new[i] = t[j], c[j]
@@ -193,31 +191,33 @@ class RetinaFace:
             crops = self._best_crops(n)
             bp, bc, tp, tc, _, _, _ = self._tracker.detect_yuv_best_device(list(frames), list(videos), threshold, self.nms_threshold,
                                                                           crops.data_ptr(), layout=layout, matrix=matrix)
-            recs = self._tracker.read(tp, tc, n)
-            tracks = [[(int(r["id"]), int(r["state"]), FaceDetectInfo.from_row(r["face"])) for r in per] for per in recs]
+            tracks = self._lists(self._tracker.read(tp, tc, n))
             shots = self._tracker.read_best(bp, bc, n)
             return tracks, [[(s, crops[i, k]) for k, s in enumerate(per)] for i, per in enumerate(shots)]
         return self._track_call(frames, videos, threshold, layout, matrix, align)
 
-    def _lists(self, tp: int, tc: int, n: int):
-        recs = self._tracker.read(tp, tc, n)
+    @staticmethod
+    def _lists(recs):
+        """(id, state, FaceDetectInfo) rows of each frame's TRACK_DTYPE records."""
         return [[(int(r["id"]), int(r["state"]), FaceDetectInfo.from_row(r["face"])) for r in per] for per in recs]
 
-    def _track_call(self, frames, videos, threshold, layout, matrix, align):
+    @staticmethod
+    def _crops(n: int, per: int, fmt: str, crop):
+        """An uninitialised (n, per, *crop_shape) torch CUDA tensor for crops in `fmt`."""
         import torch
-        from .capi import crop_shape
+        shape, dt = crop_shape(fmt, crop)
+        return torch.empty((n, per) + shape, dtype={np.uint8: torch.uint8, np.float32: torch.float32, np.float16: torch.float16}[dt],
+                           device="cuda")
+
+    def _track_call(self, frames, videos, threshold, layout, matrix, align):
         n = len(frames)
         crops = None
         if align is not None:
-            kw = {"fmt": "bgr_u8", **align}
-            A = kw.get("max_faces") or self.engine.max_faces
-            shape, dt = crop_shape(kw["fmt"], kw.get("crop", (112, 112)))
-            crops = torch.empty((n, A) + shape, dtype={np.uint8: torch.uint8, np.float32: torch.float32, np.float16: torch.float16}[dt],
-                                device="cuda")
+            crops = self._crops(n, align.get("max_faces") or self.engine.max_faces, align.get("fmt", "bgr_u8"), align.get("crop", (112, 112)))
         tp, tc, _, _, _ = self._tracker.detect_yuv_device(list(frames), list(videos), threshold, self.nms_threshold, layout=layout, matrix=matrix,
                                                           align=align, dev_crops_ptr=crops.data_ptr() if crops is not None else None)
         recs = self._tracker.read(tp, tc, n)
-        tracks = [[(int(r["id"]), int(r["state"]), FaceDetectInfo.from_row(r["face"])) for r in per] for per in recs]
+        tracks = self._lists(recs)
         new = [[(int(r["id"]), crops[i, r["crop_slot"]]) for r in per if r["crop_slot"] >= 0] if crops is not None else []
                for i, per in enumerate(recs)]
         return tracks, new
@@ -281,13 +281,9 @@ class RetinaFace:
         return self._tracker.drain(video, list(out), layout=layout, blocks=blocks, margin=margin, style=style, shape=shape, detail=detail)
 
     def _best_crops(self, n: int):
-        import torch
-        from .capi import CROP_FORMATS, crop_shape
         b = self._tracker.best
         fmt = next(k for k, v in CROP_FORMATS.items() if v[0] == b.align.format)
-        shape, dt = crop_shape(fmt, (b.align.crop_w, b.align.crop_h))
-        return torch.empty((n, self._tracker.max_tracks) + shape, dtype={np.uint8: torch.uint8, np.float32: torch.float32,
-                                                                          np.float16: torch.float16}[dt], device="cuda")
+        return self._crops(n, self._tracker.max_tracks, fmt, (b.align.crop_w, b.align.crop_h))
 
     def finishVideo(self, video: int) -> list:
         """f11: end ``video`` on a best-shot tracker (rf_tracker_finish): a ``(shot, crop)`` for every live track that was ever

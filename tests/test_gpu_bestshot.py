@@ -37,19 +37,6 @@ def _engine(prec="fp16", **kw):
     return Engine(caffemodel("mnet25"), 448, 448, precision=RF_PREC_FP32 if prec == "fp32" else RF_PREC_FP16, **kw)
 
 
-class _Dev:
-    def __init__(self, ptr, shape, typestr):
-        self.__cuda_array_interface__ = dict(shape=shape, typestr=typestr, data=(ptr, False), version=3)
-
-
-def _records(eng, dptr, cptr, n):
-    import torch
-    eng.synchronize()
-    rec = torch.as_tensor(_Dev(dptr, (n, eng.max_faces, 16), "<f4"), device="cuda").cpu().numpy()
-    counts = torch.as_tensor(_Dev(cptr, (n,), "<i4"), device="cuda").cpu().numpy()
-    return [rec[i, :counts[i], :15].copy() for i in range(n)]
-
-
 def _cuda(a):
     import torch
     return torch.from_numpy(np.ascontiguousarray(a)).cuda()
@@ -97,7 +84,7 @@ def _best_run(eng, trk, dev, per_call, crops, mats=None, videos=None):
                                                                mats[s:s + per_call].data_ptr() if mats is not None else None)
         shots = trk.read_best(bp, bc, len(chunk))
         tracks = trk.read(tp, tc, len(chunk))
-        recs = _records(eng, d, c, len(chunk))
+        recs = eng.read_dets(d, c, len(chunk))[0]
         out += [(shots[i], tracks[i], recs[i], sc[i]) for i in range(len(chunk))]
     return out
 
@@ -120,7 +107,7 @@ def _oracle_video(eng, dev, bgr, min_quality=0.0):
         crops = torch.zeros((1, mf, 112, 112, 3), dtype=torch.uint8, device="cuda")
         mats = torch.zeros((1, mf, 6), dtype=torch.float64, device="cuda")
         d, c, sc = eng.detect_yuv_device([dev[t]], THR, NMS, align=dict(), dev_crops_ptr=crops.data_ptr(), dev_mats_ptr=mats.data_ptr())
-        recs = _records(eng, d, c, 1)[0]
+        recs = eng.read_dets(d, c, 1)[0][0]
         tracks = to.update(0, recs, sc[0])
         cr, mt = crops[0].cpu().numpy(), mats[0].cpu().numpy()
         per_frame.append(bo.update(0, tracks, cr, mt, W, H))
@@ -253,7 +240,7 @@ def test_float_formats_and_unchanged_tracks(video):
     for s in range(0, NF, 8):
         chunk = dev[s:s + 8]
         tp, tc, d, c, sc = plain.detect_yuv_device(chunk, [0] * len(chunk), THR, NMS)
-        tr, recs = plain.read(tp, tc, len(chunk)), _records(eng, d, c, len(chunk))
+        tr, recs = plain.read(tp, tc, len(chunk)), eng.read_dets(d, c, len(chunk))[0]
         for i in range(len(chunk)):
             _, btr, brec, bsc = res["bgr_u8"][1][s + i]
             assert btr.tobytes() == tr[i].tobytes() and np.array_equal(brec, recs[i]) and bsc == sc[i], s + i

@@ -8,7 +8,7 @@ import pytest
 from oracle.follow import FLAT, MISMATCH, FollowTrackerOracle, luma_of
 from oracle.track import LOST
 from test_gpu_lookback import FACE, NF, PY, _in_frames, _patch, _planted, _views
-from test_gpu_motion import _records, _same, _scene
+from test_gpu_motion import _same, _scene
 from test_gpu_redact import _engine
 
 pytestmark = pytest.mark.gpu
@@ -63,7 +63,7 @@ def _drive(eng, trk, views, host, k, per_call, layout, redact=False):
             if det:
                 call = trk.detect_yuv_redact_device if redact else trk.detect_yuv_device
                 tp, tc, d, c, sc = call(chunk, [0] * m, THR, NMS, layout=layout)
-                recs = _records(eng, d, c, m)
+                recs = eng.read_dets(d, c, m)[0]
                 tr = trk.read(tp, tc, m)
                 got += [("detect", tr[i], recs[i], sc[i]) for i in range(m)]
             else:
@@ -270,7 +270,7 @@ def _drive_many(eng, trk, views, vids, k, per_call, layout, style=None, sync=Tru
         tr = trk.read(tp, tc, m)
         mo = trk.motion(m) if trk.motion_on else [None] * m
         if det:
-            recs = _records(eng, d, c, m)
+            recs = eng.read_dets(d, c, m)[0]
             for j, i in enumerate(idx):
                 got[i] = ("detect", tr[j], recs[j], sc[j], mo[j])
         else:

@@ -14,7 +14,7 @@ from oracle.redact import params
 from oracle.redact_style import redact_yuv, style
 from oracle.track import TrackerOracle
 from oracle.yuv import bgr_to_frame
-from test_gpu_motion import _records, _same, _same_motion, _scene, _shake
+from test_gpu_motion import _same, _same_motion, _scene, _shake
 from test_gpu_redact import _engine
 
 pytestmark = pytest.mark.gpu
@@ -121,7 +121,7 @@ def _run(eng, trk, dev, layout, matrix, per_call, st, outs=None, videos=None, **
         vids = [0] * m if videos is None else videos[s:s + m]
         nums, tp, tc, d, c, sc = trk.detect_yuv_redact_lookback_device(views[s:s + m], vids, oviews[s:s + m], THR, NMS, layout=layout,
                                                                        matrix=matrix, style=st[0], shape=st[1], **kw)
-        recs = _records(eng, d, c, m)
+        recs = eng.read_dets(d, c, m)[0]
         tr = trk.read(tp, tc, m)
         mo = trk.motion(m) if trk.motion_on else [None] * m
         got += [(int(nums[i]), tr[i], recs[i], sc[i], mo[i]) for i in range(m)]

@@ -15,7 +15,7 @@ from oracle.redact_style import redact_yuv, style
 from oracle.track import TrackerOracle
 from test_gpu_lookback import (FACE, H, NMS, OPITCH, PITCH, PY, STYLES, THR, W, _in_frames, _lap_var, _out_frames, _patch, _surface,
                                _views)
-from test_gpu_motion import _records, _same, _same_motion, _scene
+from test_gpu_motion import _same, _same_motion, _scene
 from test_gpu_redact import _engine
 
 pytestmark = pytest.mark.gpu
@@ -70,7 +70,7 @@ def _run(eng, trk, dev, layout, matrix, per_call, st, outs=None, videos=None, se
         vids = [0] * m if videos is None else videos[s:s + m]
         nums, tp, tc, d, c, sc = trk.detect_yuv_redact_lookback_device(views[s:s + m], vids, oviews[s:s + m], _thr(s, seen), NMS, layout=layout,
                                                                        matrix=matrix, style=st[0], shape=st[1])
-        recs = _records(eng, d, c, m)
+        recs = eng.read_dets(d, c, m)[0]
         tr = trk.read(tp, tc, m)
         mo = trk.motion(m) if trk.motion_on else [None] * m
         steps, lens = trk.lookback_search(m) if trk.lookback_search_on else ([None] * m, [None] * m)

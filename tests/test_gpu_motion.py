@@ -33,19 +33,6 @@ def _engine(prec="fp16", **kw):
     return Engine(caffemodel("mnet25"), 448, 448, precision=RF_PREC_FP32 if prec == "fp32" else RF_PREC_FP16, **kw)
 
 
-class _Dev:
-    def __init__(self, ptr, shape, typestr):
-        self.__cuda_array_interface__ = dict(shape=shape, typestr=typestr, data=(ptr, False), version=3)
-
-
-def _records(eng, dptr, cptr, n):
-    import torch
-    eng.synchronize()
-    rec = torch.as_tensor(_Dev(dptr, (n, eng.max_faces, 16), "<f4"), device="cuda").cpu().numpy()
-    counts = torch.as_tensor(_Dev(cptr, (n,), "<i4"), device="cuda").cpu().numpy()
-    return [rec[i, :counts[i], :15].copy() for i in range(n)]
-
-
 def _scene(seed=7, w=3000, h=2000):
     r = np.random.default_rng(seed)
     a = cv2.resize(r.integers(0, 256, (h // 24, w // 24, 3)).astype(np.uint8), (w, h), interpolation=cv2.INTER_CUBIC).astype(np.float32)
@@ -136,7 +123,7 @@ def _run(eng, trk, dev, per_call, layout="nv12", videos=None):
         chunk = dev[s:s + per_call]
         vids = [0] * len(chunk) if videos is None else videos[s:s + per_call]
         tp, tc, d, c, sc = trk.detect_yuv_device(chunk, vids, THR, NMS, layout=layout)
-        recs = _records(eng, d, c, len(chunk))
+        recs = eng.read_dets(d, c, len(chunk))[0]
         tr = trk.read(tp, tc, len(chunk))
         mo = trk.motion(len(chunk)) if trk.motion_on else [None] * len(chunk)
         out += [(tr[i], recs[i], sc[i], mo[i]) for i in range(len(chunk))]
@@ -239,7 +226,7 @@ def test_redaction_follows_the_camera(shake, golden_image):
     eng = _engine("fp16")
     d, c, sc = eng.detect_yuv_device([torch.from_numpy(bgr_to_frame(frames[5], "nv12")).cuda()], THR, NMS)
     torch.cuda.synchronize()
-    rec = _records(eng, d, c, 1)[0]
+    rec = eng.read_dets(d, c, 1)[0][0]
     j = int(np.argmax((rec[:, 3] - rec[:, 1]) * (rec[:, 0] > 0.8)))
     box5 = rec[j, 1:5] * sc[0]
     truth = {}
@@ -266,7 +253,7 @@ def test_redaction_follows_the_camera(shake, golden_image):
         for s in range(0, 12, 4):
             chunk = dev[s:s + 4]
             tp, tc, dd, cc, scs = trk.detect_yuv_redact_device(chunk, [0] * 4, THR, NMS)
-            recs = _records(eng, dd, cc, 4)
+            recs = eng.read_dets(dd, cc, 4)[0]
             tr = trk.read(tp, tc, 4)
             for i in range(4):
                 t = s + i

@@ -27,11 +27,6 @@ NMS = (0.4, 1.0, 0.0)
 MAX_ROUNDS = 9000
 
 
-class _Dev:
-    def __init__(self, ptr, shape, typestr):
-        self.__cuda_array_interface__ = dict(shape=shape, typestr=typestr, data=(ptr, False), version=3)
-
-
 def _engine(plan, max_faces, monkeypatch):
     from retinaface_b200 import RF_PREC_FP16, RF_PREC_FP32, RF_PREC_INT8, Engine
     from retinaface_b200.capi import plan_describe
@@ -94,12 +89,8 @@ def _threshold(ps, k, start):
 
 
 def _device_records(eng, n, thr, nms, dev):
-    import torch
     d, c = eng.detect_device(n, float(thr), nms, dev.data_ptr())
-    eng.synchronize()
-    rec = torch.as_tensor(_Dev(d, (n, eng.max_faces, 16), "<f4"), device="cuda").cpu().numpy()
-    counts = torch.as_tensor(_Dev(c, (n,), "<i4"), device="cuda").cpu().numpy()
-    return [(rec[i, :counts[i], :15].copy(), rec[i, :counts[i], 15].view(np.int32).copy()) for i in range(n)]
+    return list(zip(*eng.read_dets(d, c, n)))
 
 
 @pytest.mark.parametrize("name", list(PLANS))

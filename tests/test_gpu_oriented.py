@@ -132,18 +132,6 @@ def _cuda(a):
     return torch.from_numpy(np.ascontiguousarray(a)).cuda()
 
 
-class _Dev:
-    def __init__(self, ptr, shape, typestr):
-        self.__cuda_array_interface__ = dict(shape=shape, typestr=typestr, data=(ptr, False), version=3)
-
-
-def _records(eng, dptr, cptr, n):
-    import torch
-    rec = torch.as_tensor(_Dev(dptr, (n, eng.max_faces, 16), "<f4"), device="cuda").cpu().numpy()
-    counts = torch.as_tensor(_Dev(cptr, (n,), "<i4"), device="cuda").cpu().numpy()
-    return [rec[i, :counts[i]].copy() for i in range(n)]
-
-
 def test_device_yuv_oriented_equals_the_rotated_surfaces(eng, golden_image):
     import torch
     base = [bgr_to_frame(cv2.resize(golden_image, s), "nv12") for s in ((1920, 1080), (1282, 722), (640, 444))]
@@ -159,13 +147,13 @@ def test_device_yuv_oriented_equals_the_rotated_surfaces(eng, golden_image):
     mats_ref = torch.zeros_like(mats)
     d, c, sc = eng.detect_yuv_oriented_device(dev, os_, THR, NMS, align={}, dev_crops_ptr=crops.data_ptr(), dev_mats_ptr=mats.data_ptr())
     eng.synchronize()
-    got = _records(eng, d, c, 8)
+    got, got_idx = eng.read_dets(d, c, 8)
     d2, c2, sc2 = eng.detect_yuv_device(rot, THR, NMS, align={}, dev_crops_ptr=crops_ref.data_ptr(), dev_mats_ptr=mats_ref.data_ptr())
     eng.synchronize()
-    ref = _records(eng, d2, c2, 8)
+    ref, ref_idx = eng.read_dets(d2, c2, 8)
     assert np.array_equal(sc, sc2)
     for i in range(8):
-        assert np.array_equal(got[i], ref[i]), i
+        assert np.array_equal(got[i], ref[i]) and np.array_equal(got_idx[i], ref_idx[i]), i
         k = len(got[i])
         assert torch.equal(crops[i, :k], crops_ref[i, :k]) and torch.equal(mats[i, :k], mats_ref[i, :k]), i
     assert [int(x.sum()) for x in dev] == sums                          # the surfaces are read, never written
@@ -275,7 +263,7 @@ def test_nothing_else_changes(golden_image):
             f, idx = e.detect_batch(imgs, THR, NMS, want_index=True)
             d, c, sc = e.detect_yuv_device([dframe], THR, NMS)
             e.synchronize()
-            return f, idx, _records(e, d, c, 1), sc
+            return (f, idx, *e.read_dets(d, c, 1), sc)
         before = plain()
         e.detect_oriented(imgs, [6, 7], THR, NMS, align={})
         e.detect_yuv_oriented_device([dframe], [8], THR, NMS)

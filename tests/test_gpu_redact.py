@@ -30,19 +30,6 @@ def _engine(prec="fp16", **kw):
     return Engine(caffemodel("mnet25"), 448, 448, precision=RF_PREC_FP32 if prec == "fp32" else RF_PREC_FP16, **kw)
 
 
-class _Dev:
-    def __init__(self, ptr, shape, typestr):
-        self.__cuda_array_interface__ = dict(shape=shape, typestr=typestr, data=(ptr, False), version=3)
-
-
-def _records(eng, dptr, cptr, n):
-    import torch
-    eng.synchronize()
-    rec = torch.as_tensor(_Dev(dptr, (n, eng.max_faces, 16), "<f4"), device="cuda").cpu().numpy()
-    counts = torch.as_tensor(_Dev(cptr, (n,), "<i4"), device="cuda").cpu().numpy()
-    return [rec[i, :counts[i], :15].copy() for i in range(n)]
-
-
 def _cuda(a):
     """A device copy, complete before the library's streams (which do not wait for torch's) read it."""
     import torch
@@ -98,7 +85,7 @@ def test_redaction_equals_the_oracle(golden_image, prec):
     dev = [_cuda(s) for s in surfs]
     frames = [_planes(d) for d in dev]
     d, c, sc = eng.detect_yuv_device(frames, THR, NMS, matrix="bt601")
-    recs = _records(eng, d, c, 3)
+    recs = eng.read_dets(d, c, 3)[0]
     assert all(len(r) >= 3 for r in recs)
     eng.redact_yuv_device(frames, d, c, sc)
     eng.synchronize()
@@ -110,7 +97,7 @@ def test_redaction_equals_the_oracle(golden_image, prec):
     bufs = [bgr_to_frame(im, "i420") for im in imgs]
     devi = [_cuda(b) for b in bufs]
     d, c, sc = eng.detect_yuv_device(devi, THR, NMS, layout="i420", matrix="bt709")
-    recs = _records(eng, d, c, 3)
+    recs = eng.read_dets(d, c, 3)[0]
     for blocks in (1, 32):
         eng.redact_yuv_device(devi, d, c, sc, layout="i420", blocks=blocks, margin=0.5)
         eng.synchronize()
@@ -119,7 +106,7 @@ def test_redaction_equals_the_oracle(golden_image, prec):
             assert np.array_equal(devi[k].cpu().numpy(), bufs[k]), (prec, blocks, k)
     # BGR rows 64 bytes beyond 3 w, the NV12 records
     d, c, sc = eng.detect_yuv_device(frames, THR, NMS)
-    recs = _records(eng, d, c, 3)
+    recs = eng.read_dets(d, c, 3)[0]
     big = [np.full((H, 3 * W + 64), 0xEE, np.uint8) for _ in imgs]
     for b, im in zip(big, imgs):
         b[:, :3 * W] = im.reshape(H, 3 * W)
@@ -200,9 +187,9 @@ def test_combined_call_equals_its_parts(golden_image):
     b = _clones(a)
     for s in range(0, 12, 4):
         d1, c1, s1 = eng.detect_yuv_redact_device(a[s:s + 4], THR, NMS, blocks=12, margin=0.3)
-        r1 = _records(eng, d1, c1, 4)
+        r1 = eng.read_dets(d1, c1, 4)[0]
         d2, c2, s2 = eng.detect_yuv_device(b[s:s + 4], THR, NMS)
-        r2 = _records(eng, d2, c2, 4)
+        r2 = eng.read_dets(d2, c2, 4)[0]
         eng.redact_yuv_device(b[s:s + 4], d2, c2, s2, blocks=12, margin=0.3)
         eng.synchronize()
         assert all(np.array_equal(x, y) for x, y in zip(r1, r2)) and np.array_equal(s1, s2)
@@ -215,7 +202,7 @@ def test_combined_call_equals_its_parts(golden_image):
         tp2, tc2, d2, c2, s2 = t2.detect_yuv_device(b[s:s + 3], [0] * 3, THR, NMS)
         eng.redact_yuv_device(b[s:s + 3], d2, c2, s2, tracker=t2, tracks_ptr=tp2, track_counts_ptr=tc2)
         eng.synchronize()
-        assert all(np.array_equal(x, y) for x, y in zip(_records(eng, d1, c1, 3), _records(eng, d2, c2, 3)))
+        assert all(np.array_equal(x, y) for x, y in zip(eng.read_dets(d1, c1, 3)[0], eng.read_dets(d2, c2, 3)[0]))
         assert all(np.array_equal(x.view(np.uint8), y.view(np.uint8)) for x, y in zip(t1.read(tp1, tc1, 3), t2.read(tp2, tc2, 3)))
     assert all(torch.equal(x, y) for x, y in zip(a, b))
     t1.close()
@@ -227,6 +214,7 @@ def test_tracking_closes_the_leak(golden_image):
     """The moving photo with the best face's record deleted from the device records on frames 5-7, through rf_track_update: with tracks
     its LOST track's predicted box is redacted, equal to the oracle; without tracks its pixels are the input's."""
     import torch
+    from retinaface_b200.capi import device_view
     eng = _engine("fp16")
     trk = eng.tracker()
     imgs = _moving(golden_image, 10)
@@ -235,11 +223,11 @@ def test_tracking_closes_the_leak(golden_image):
         buf = bgr_to_frame(im, "nv12")
         f1, f2 = _cuda(buf), _cuda(buf)
         d, c, sc = eng.detect_yuv_device([f1], THR, NMS)
-        rec = _records(eng, d, c, 1)[0]
+        rec = eng.read_dets(d, c, 1)[0][0]
         if 5 <= t <= 7:             # the detector misses face 0 on these frames
-            raw = torch.as_tensor(_Dev(d, (1, eng.max_faces, 16), "<f4"), device="cuda")
+            raw = device_view(d, (1, eng.max_faces, 16), "<f4")
             raw[0, :len(rec) - 1] = raw[0, 1:len(rec)].clone()
-            torch.as_tensor(_Dev(c, (1,), "<i4"), device="cuda").sub_(1)
+            device_view(c, (1,), "<i4").sub_(1)
             torch.cuda.synchronize()
             gone, rec = rec[0], rec[1:]
         tp, tc = trk.update([0], d, c, sc)
@@ -281,7 +269,7 @@ def test_tiled_4k_records(golden_image):
     buf = bgr_to_frame(img, "nv12")
     dev = _cuda(buf)
     d, c = eng.detect_yuv_tiled_device([dev], THR, NMS)
-    rec = _records(eng, d, c, 1)[0]
+    rec = eng.read_dets(d, c, 1)[0][0]
     eng.redact_yuv_device([dev], d, c, None)
     eng.synchronize()
     out = dev.cpu().numpy()
@@ -394,7 +382,7 @@ def test_nothing_else_changes(golden_image):
     def snapshot():
         faces = eng.detect_batch([inp, inp], THR, NMS)
         d, c, sc = eng.detect_yuv_device([_cuda(buf)], THR, NMS)
-        return faces, _records(eng, d, c, 1), sc, eng.launches_per_batch(8)
+        return faces, eng.read_dets(d, c, 1)[0], sc, eng.launches_per_batch(8)
 
     a = snapshot()
     for blocks in (1, 8, 32):

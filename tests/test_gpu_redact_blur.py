@@ -11,7 +11,7 @@ import pytest
 from oracle.redact import frame_regions, params
 from oracle.redact_style import redact_bgr, redact_yuv, shape_mask, style
 from oracle.yuv import bgr_to_frame
-from test_gpu_redact import (NMS, SURF, SYNTH, THR, H, W, _canvas, _clones, _cuda, _det_array, _engine, _moving, _planes, _records,
+from test_gpu_redact import (NMS, SURF, SYNTH, THR, H, W, _canvas, _clones, _cuda, _det_array, _engine, _moving, _planes,
                              _surface)
 
 pytestmark = pytest.mark.gpu
@@ -50,7 +50,7 @@ def test_styles_equal_the_oracle(golden_image, prec):
         dev = [_cuda(s) for s in surfs]
         frames = [_planes(d) for d in dev]
         d, c, sc = eng.detect_yuv_device(frames, THR, NMS, matrix="bt601")
-        recs = _records(eng, d, c, 3)
+        recs = eng.read_dets(d, c, 3)[0]
         assert all(len(r) >= 3 for r in recs)
         eng.redact_yuv_device(frames, d, c, sc, style=kind, shape=shape)
         eng.synchronize()
@@ -67,7 +67,7 @@ def test_styles_equal_the_oracle(golden_image, prec):
         bufs = [bgr_to_frame(im, "i420") for im in imgs]
         devi = [_cuda(b) for b in bufs]
         d, c, sc = eng.detect_yuv_device(devi, THR, NMS, layout="i420", matrix="bt709")
-        recs = _records(eng, d, c, 3)
+        recs = eng.read_dets(d, c, 3)[0]
         det = 2 if kind == "blur" else 0
         eng.redact_yuv_device(devi, d, c, sc, layout="i420", margin=0.5, style=kind, shape=shape, detail=det)
         eng.synchronize()
@@ -194,7 +194,7 @@ def test_lost_tracks_stay_covered(golden_image, motion):
         buf = bgr_to_frame(im, "nv12")
         f = _cuda(buf)
         tp, tc, d, c, sc = trk.detect_yuv_redact_device([f], [0], THR, NMS, style="blur", shape="ellipse")
-        rec = _records(eng, d, c, 1)[0]
+        rec = eng.read_dets(d, c, 1)[0][0]
         tracks = trk.read(tp, tc, 1)[0]
         regs = _regions([rec], sc, tracks=[tracks])[0]
         assert np.array_equal(f.cpu().numpy(), redact_yuv(buf, "nv12", regs, _style("blur", "ellipse"))), t
@@ -218,9 +218,9 @@ def test_combined_call_equals_its_parts(golden_image):
     b = _clones(a)
     for s in range(0, 8, 4):
         d1, c1, s1 = eng.detect_yuv_redact_device(a[s:s + 4], THR, NMS, **kw)
-        r1 = _records(eng, d1, c1, 4)
+        r1 = eng.read_dets(d1, c1, 4)[0]
         d2, c2, s2 = eng.detect_yuv_device(b[s:s + 4], THR, NMS)
-        r2 = _records(eng, d2, c2, 4)
+        r2 = eng.read_dets(d2, c2, 4)[0]
         eng.redact_yuv_device(b[s:s + 4], d2, c2, s2, **kw)
         eng.synchronize()
         assert all(np.array_equal(x, y) for x, y in zip(r1, r2)) and np.array_equal(s1, s2)
@@ -250,7 +250,7 @@ def test_tiled_4k_records(golden_image):
     buf = bgr_to_frame(img, "nv12")
     dev = _cuda(buf)
     d, c = eng.detect_yuv_tiled_device([dev], THR, NMS)
-    rec = _records(eng, d, c, 1)[0]
+    rec = eng.read_dets(d, c, 1)[0][0]
     assert len(rec) >= 12
     eng.redact_yuv_device([dev], d, c, None, style="blur", shape="ellipse")
     eng.synchronize()

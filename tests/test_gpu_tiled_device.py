@@ -41,19 +41,6 @@ def _canvas(golden_image, w=3840, h=2160, xs=(32, 704, 1376, 2048, 2720), ys=(32
     return c, half, [(x, y) for y in ys for x in xs]
 
 
-class _Dev:
-    def __init__(self, ptr, shape, typestr):
-        self.__cuda_array_interface__ = dict(shape=shape, typestr=typestr, data=(ptr, False), version=3)
-
-
-def _records(eng, dptr, cptr, n):
-    """(faces, candidate ids) of the first n images of a device result, read through the returned pointers (after a synchronize)."""
-    import torch
-    rec = torch.as_tensor(_Dev(dptr, (n, eng.max_faces, 16), "<f4"), device="cuda").cpu().numpy()
-    counts = torch.as_tensor(_Dev(cptr, (n,), "<i4"), device="cuda").cpu().numpy()
-    return [rec[i, :counts[i], :15].copy() for i in range(n)], [rec[i, :counts[i], 15].view(np.int32).copy() for i in range(n)]
-
-
 def _cuda(a):
     import torch
     return torch.from_numpy(np.ascontiguousarray(a)).cuda()
@@ -112,7 +99,7 @@ def test_device_bgr_equals_host(golden_image, prec):
             want, tile_of = eng.detect_tiled(imgs, THR, NMS, levels=levels)
             d, c = eng.detect_tiled_device(dev, THR, NMS, levels=levels)
             eng.synchronize()
-            _assert_same(_records(eng, d, c, 8), want, tile_of, eng.max_faces, (prec, levels))
+            _assert_same(eng.read_dets(d, c, 8), want, tile_of, eng.max_faces, (prec, levels))
             assert sum(len(f) for f in want) >= 30
     finally:
         eng.close()
@@ -144,7 +131,7 @@ def test_device_yuv_equals_host(golden_image, prec):
                 want, tile_of = eng.detect_yuv_tiled(frames, THR, NMS, layout, matrix, levels=levels)
                 d, c = eng.detect_yuv_tiled_device(dev, THR, NMS, layout, matrix, levels=levels)
                 eng.synchronize()
-                _assert_same(_records(eng, d, c, n), want, tile_of, eng.max_faces, (prec, layout, levels))
+                _assert_same(eng.read_dets(d, c, n), want, tile_of, eng.max_faces, (prec, layout, levels))
                 assert sum(len(f) for f in want) >= 20
             del surf
     finally:
@@ -207,7 +194,7 @@ def test_crops_of_every_tiled_path(golden_image):
                         d, c = eng.detect_yuv_tiled_device([_cuda(src)], THR, NMS, align=dict(fmt=fmt), dev_crops_ptr=crops.data_ptr(),
                                                            dev_mats_ptr=dmats.data_ptr())
                     eng.synchronize()
-                    df, ids = _records(eng, d, c, 1)
+                    df, ids = eng.read_dets(d, c, 1)
                     k = len(faces[0])
                     assert np.array_equal(df[0], faces[0]) and np.array_equal(ids[0] // eng.max_faces, tile_of[0])
                     assert np.array_equal(crops[0, :k].cpu().numpy(), host) and (crops[0, k:] == 7).all(), (name, kind, fmt)
@@ -331,7 +318,7 @@ def _in_flight(eng, golden_image, streams, sizes):
             assert kk > 0 and np.array_equal(bufs[k][i, :kk].cpu().numpy(), crops[i]), (k, i)
             assert (bufs[k][i, kk:] == 7.0).all(), (k, i)
         if k >= calls - streams:
-            _assert_same(_records(eng, out[k][0], out[k][1], 2), faces, tile_of, eng.max_faces, k)
+            _assert_same(eng.read_dets(out[k][0], out[k][1], 2), faces, tile_of, eng.max_faces, k)
     assert [[int(t.to(torch.int64).sum()) for t in d] for d in dev] == sums
 
 

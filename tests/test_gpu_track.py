@@ -30,19 +30,6 @@ def _engine(prec="fp16", **kw):
     return Engine(caffemodel("mnet25"), 448, 448, precision=RF_PREC_FP32 if prec == "fp32" else RF_PREC_FP16, **kw)
 
 
-class _Dev:
-    def __init__(self, ptr, shape, typestr):
-        self.__cuda_array_interface__ = dict(shape=shape, typestr=typestr, data=(ptr, False), version=3)
-
-
-def _records(eng, dptr, cptr, n):
-    import torch
-    eng.synchronize()
-    rec = torch.as_tensor(_Dev(dptr, (n, eng.max_faces, 16), "<f4"), device="cuda").cpu().numpy()
-    counts = torch.as_tensor(_Dev(cptr, (n,), "<i4"), device="cuda").cpu().numpy()
-    return [rec[i, :counts[i], :15].copy() for i in range(n)]
-
-
 @pytest.fixture(scope="module")
 def video(golden_image):
     """40 NV12 frames: the golden photo moving (7, 3) px per frame on grey, a grey occluder over its best face on frames 12-17, and a
@@ -92,7 +79,7 @@ def _track_video(eng, trk, frames, per_call=1, align=None, crops=None):
         chunk = frames[s:s + per_call]
         tp, tc, d, c, sc = trk.detect_yuv_device(chunk, [0] * len(chunk), THR, NMS, align=align,
                                                   dev_crops_ptr=crops[s:s + per_call].data_ptr() if crops is not None else None)
-        recs = _records(eng, d, c, len(chunk))
+        recs = eng.read_dets(d, c, len(chunk))[0]
         tr = trk.read(tp, tc, len(chunk))
         out += [(tr[i], recs[i], sc[i]) for i in range(len(chunk))]
     return out
@@ -110,7 +97,7 @@ def test_tracks_equal_the_oracle(video, prec):
     got = _track_video(eng, trk, dev, per_call=8)
     for t, (tracks, recs, sc) in enumerate(got):
         d, c, sc2 = eng.detect_yuv_device([dev[t]], THR, NMS)
-        ref = _records(eng, d, c, 1)[0]
+        ref = eng.read_dets(d, c, 1)[0][0]
         assert np.array_equal(ref, recs) and sc2[0] == sc, t
         _same(tracks, o.update(0, ref, sc), f"{prec} frame {t}")
     hdr, rows = trk.debug_state(0)
@@ -263,7 +250,7 @@ def test_update_on_tiled_device_records(video):
         img = torch.from_numpy(frame_to_bgr(frames[t], "nv12")).cuda()
         d, c = eng.detect_tiled_device([img], THR, NMS)
         tp, tc = trk.update([0], d, c)
-        recs = _records(eng, d, c, 1)[0]
+        recs = eng.read_dets(d, c, 1)[0][0]
         _same(trk.read(tp, tc, 1)[0], o.update(0, recs, None), f"tiled {t}")
     trk.close()
     eng.close()
@@ -276,11 +263,11 @@ def test_nothing_else_changes_and_bad_calls_launch_nothing(video, golden_image):
     eng = _engine("fp16")
     base = eng.detect_batch([golden_image], THR, NMS)[0]
     d, c, _ = eng.detect_yuv_device(dev, THR, NMS)
-    yuv = _records(eng, d, c, 2)
+    yuv = eng.read_dets(d, c, 2)[0]
     launches = eng.launches_per_batch(2)
     trk = eng.tracker(max_videos=2)
     tp, tc, d2, c2, _ = trk.detect_yuv_device(dev, [0, 1], THR, NMS)
-    assert [np.array_equal(a, b) for a, b in zip(_records(eng, d2, c2, 2), yuv)] == [True, True]
+    assert [np.array_equal(a, b) for a, b in zip(eng.read_dets(d2, c2, 2)[0], yuv)] == [True, True]
     state = [trk.debug_state(v)[0].tobytes() for v in (0, 1)]
     lib, t = eng.lib, trk.t
     can_t, can_c = C.c_void_p(0x1234), C.c_void_p(0x5678)
@@ -310,7 +297,7 @@ def test_nothing_else_changes_and_bad_calls_launch_nothing(video, golden_image):
     assert [trk.debug_state(v)[0].tobytes() for v in (0, 1)] == state     # nothing was applied
     assert np.array_equal(eng.detect_batch([golden_image], THR, NMS)[0], base)
     d, c, _ = eng.detect_yuv_device(dev, THR, NMS)
-    assert all(np.array_equal(a, b) for a, b in zip(_records(eng, d, c, 2), yuv))
+    assert all(np.array_equal(a, b) for a, b in zip(eng.read_dets(d, c, 2)[0], yuv))
     assert eng.launches_per_batch(2) == launches
     trk.close()
     eng.close()

@@ -111,19 +111,6 @@ def test_npp_resize_equals_bgr_path(golden_image):
         eng.close()
 
 
-class _Dev:
-    def __init__(self, ptr, shape, typestr):
-        self.__cuda_array_interface__ = dict(shape=shape, typestr=typestr, data=(ptr, False), version=3)
-
-
-def _device_results(eng, dptr, cptr, n):
-    import torch
-    eng.synchronize()
-    rec = torch.as_tensor(_Dev(dptr, (n, eng.max_faces, 16), "<f4"), device="cuda").cpu().numpy()
-    counts = torch.as_tensor(_Dev(cptr, (n,), "<i4"), device="cuda").cpu().numpy()
-    return [rec[i, :counts[i], :15].copy() for i in range(n)], [rec[i, :counts[i], 15].view(np.int32).copy() for i in range(n)]
-
-
 def _mixed_frames(golden_image, n):
     g = _even(golden_image)
     pool = [bgr_to_frame(g, "nv12"), bgr_to_frame(cv2.resize(golden_image, (1920, 1080)), "nv12"),
@@ -154,7 +141,7 @@ def test_detect_host_and_device_equal_bgr_detect(golden_image, prec):
                 dev = [torch.from_numpy(f).cuda() for f in frames]
                 torch.cuda.synchronize()
                 d, c, scales = eng.detect_yuv_device(dev, THR, NMS, layout, matrix)
-                df, didx = _device_results(eng, d, c, n)
+                df, didx = eng.read_dets(d, c, n)
                 for i in range(n):
                     assert np.array_equal(faces[i], want[i]) and np.array_equal(idx[i], ref_idx[i]), (n, layout, i)
                     assert np.array_equal(pf[i], want[i]) and np.array_equal(pidx[i], ref_idx[i])
@@ -221,7 +208,7 @@ def test_device_calls_over_two_contexts_leave_frames_untouched(golden_image):
             _, want_c, want_m = eng.detect_yuv(batches[b], THR, NMS, "nv12", align=dict(fmt="rgb_f16", want_mats=True))
             # out[b]'s device records were overwritten by later calls on the same context only after 2 more calls: re-run alone
             d, c, _ = eng.detect_yuv_device(dev[b], THR, NMS, "nv12")
-            faces, _ = _device_results(eng, d, c, 4)
+            faces, _ = eng.read_dets(d, c, 4)
             for i in range(4):
                 k = len(want_c[i])
                 assert k > 0 and np.array_equal(faces[i], ref[i])

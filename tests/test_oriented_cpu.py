@@ -1,10 +1,9 @@
 """CPU: f9 orientations without a GPU -- the EXIF definition (orient() against cv2.imread of JPEGs carrying each tag in both TIFF byte
 orders), rf_jpeg_exif_orientation on those and on malformed segments, the map-back into stored pixels as the inverse of the tap
-address map A_o, the 4:2:0 plane orientation against cvtColor, and the new entry points exported with their header signatures.
+address map A_o, the 4:2:0 plane orientation against cvtColor, and the C++ shell compiling the oriented calls (the entry points'
+signatures are checked in test_signatures_cpu.py).
 orient / orient_planes / stored_points are the test oracle the GPU tests (test_gpu_oriented.py) use too."""
-import ctypes as C
 import os
-import re
 import struct
 
 import cv2
@@ -14,8 +13,6 @@ import pytest
 from conftest import GOLDEN, ROOT
 from oracle.yuv import bgr_to_frame, frame_to_bgr
 
-NEW = ("rf_detect_oriented_batch", "rf_detect_yuv_oriented_device", "rf_preprocess_oriented", "rf_preprocess_yuv_oriented",
-       "rf_detect_views_oriented", "rf_jpeg_exif_orientation")
 MIRRORED = {2, 4, 5, 7}
 
 
@@ -143,41 +140,6 @@ def test_plane_orientation_commutes_with_cvtcolor(layout, o):
     code = cv2.COLOR_YUV2BGR_NV12 if layout == "nv12" else cv2.COLOR_YUV2BGR_I420
     assert np.array_equal(orient(cv2.cvtColor(frame, code), o), cv2.cvtColor(orient_planes(frame, layout, o), code))
     assert np.array_equal(orient(frame_to_bgr(frame, layout), o), frame_to_bgr(orient_planes(frame, layout, o), layout))
-
-
-def _prototype(name):
-    text = open(os.path.join(ROOT, "include", "rf_b200.h")).read()
-    m = re.search(r"\bint " + name + r"\(([^;]*)\);", text)
-    assert m, name
-    return [re.sub(r"\s+", " ", p.strip()) for p in m.group(1).split(",")]
-
-
-def _ctype_of(param):
-    from retinaface_b200 import capi
-    t = re.sub(r"\s*\*\s*", "*", re.sub(r"\s*\w+$", "", param))
-    simple = {"rf_handle": C.c_void_p, "int": C.c_int, "float": C.c_float, "size_t": C.c_size_t}
-    if t in simple:
-        return simple[t]
-    ptrs = {"const uint8_t*const*": C.POINTER(C.c_void_p), "const int*": C.POINTER(C.c_int), "const rf_align_params*": C.POINTER(capi.AlignParams),
-            "const rf_yuv_frame*": C.POINTER(capi.YuvFrame), "const rf_det**": C.POINTER(C.c_void_p), "const int32_t**": C.POINTER(C.c_void_p),
-            "const rf_oriented_view*": C.POINTER(capi._OrientedView)}
-    if t in ptrs:
-        return ptrs[t]
-    if param == "int *out_count":                  # rf_detect_views' binding: a ctypes int by reference
-        return C.POINTER(C.c_int)
-    assert t.endswith("*"), t
-    return C.c_void_p
-
-
-def test_entry_points_and_signatures(built_lib):
-    from retinaface_b200 import capi
-    lib = capi.load_library()
-    raw = C.CDLL(built_lib)
-    for name in NEW:
-        assert name in capi.EXPORTS and hasattr(raw, name), name
-        want = [_ctype_of(p) for p in _prototype(name)]
-        got = getattr(lib, name).argtypes
-        assert list(got) == want, (name, got, want)
 
 
 def test_cpp_shell_compiles_oriented_calls(built_lib, tmp_path):

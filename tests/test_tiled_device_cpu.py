@@ -1,55 +1,12 @@
-"""CPU: the f8 surface without a GPU -- the four tiled entry points exported with the ctypes signatures their header prototypes have,
-the C++ shell compiling a detectTiled call with crops, and the Python device wrappers refusing host arrays before any call."""
-import ctypes as C
+"""CPU: the f8 surface without a GPU -- the C++ shell compiling a detectTiled call with crops, and the Python device wrappers refusing
+host arrays before any call (the four tiled entry points' signatures are checked in test_signatures_cpu.py)."""
 import os
-import re
 import subprocess
 
 import numpy as np
 import pytest
 
 from conftest import ROOT
-
-NEW = ("rf_detect_tiled_align", "rf_detect_yuv_tiled_align", "rf_detect_tiled_device", "rf_detect_yuv_tiled_device")
-
-
-def _prototype(name):
-    """The parameter types of `name` in include/rf_b200.h, whitespace-normalised."""
-    text = open(os.path.join(ROOT, "include", "rf_b200.h")).read()
-    m = re.search(r"\bint " + name + r"\(([^;]*)\);", text)
-    assert m, name
-    return [re.sub(r"\s+", " ", p.strip()) for p in m.group(1).split(",")]
-
-
-def _ctype_of(param):
-    """The ctypes type capi should declare for one C parameter."""
-    from retinaface_b200 import capi
-    t = re.sub(r"\s*\*\s*", "*", re.sub(r"\s*\w+$", "", param))      # the type without the parameter name
-    simple = {"rf_handle": C.c_void_p, "int": C.c_int, "float": C.c_float}
-    if t in simple:
-        return simple[t]
-    ptrs = {"const uint8_t*const*": C.POINTER(C.c_void_p), "const int*": C.POINTER(C.c_int), "const rf_tiling*": C.POINTER(capi.Tiling),
-            "const rf_align_params*": C.POINTER(capi.AlignParams), "const rf_yuv_frame*": C.POINTER(capi.YuvFrame),
-            "const rf_det**": C.POINTER(C.c_void_p), "const int32_t**": C.POINTER(C.c_void_p)}
-    if t in ptrs:
-        return ptrs[t]
-    assert t.endswith("*"), t                      # output arrays and buffers: plain addresses
-    return C.c_void_p
-
-
-def test_entry_points_and_signatures(built_lib):
-    from retinaface_b200 import capi
-    lib = capi.load_library()
-    raw = C.CDLL(built_lib)
-    for name in NEW:
-        assert name in capi.EXPORTS and hasattr(raw, name), name
-        params = _prototype(name)
-        want = [_ctype_of(p) for p in params]
-        got = getattr(lib, name).argtypes
-        assert len(got) == len(want), (name, len(got), len(want))
-        for p, g, w in zip(params, got, want):
-            assert g == w, (name, p, g, w)
-
 
 def test_cpp_shell_compiles_a_detect_tiled_call_with_crops(built_lib, tmp_path):
     from retinaface_b200.build import build_host

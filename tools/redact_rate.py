@@ -33,19 +33,6 @@ W, H, B, FRAMES = 1920, 1080, 8, 16
 KERNELS = ("k_redact_regions", "k_redact_measure", "k_redact_apply")
 
 
-class _Dev:
-    def __init__(self, ptr, shape, typestr):
-        self.__cuda_array_interface__ = dict(shape=shape, typestr=typestr, data=(ptr, False), version=3)
-
-
-def _records(eng, d, c, n):
-    import torch
-    eng.synchronize()
-    rec = torch.as_tensor(_Dev(d, (n, eng.max_faces, 16), "<f4"), device="cuda").cpu().numpy()
-    counts = torch.as_tensor(_Dev(c, (n,), "<i4"), device="cuda").cpu().numpy()
-    return [rec[i, :counts[i], :15] for i in range(n)]
-
-
 def _floor_bytes(recs, scales, w, h):
     """Region pixels of one call (the union of each frame's rectangles inside the frame), 1.5 bytes each, read twice, written once."""
     from oracle.redact import frame_regions, params
@@ -145,11 +132,11 @@ def main():
             e.synchronize()
             rates[k].append(B * n / (time.perf_counter() - t0))
     d, c, sc = eng.detect_yuv_device(frames[0], thr, nms)
-    recs = _records(eng, d, c, B)
+    recs = eng.read_dets(d, c, B)[0]
     faces = float(np.mean([len(r) for r in recs]))
     floor_bytes = _floor_bytes(recs, sc, W, H)
     d, c = eng4k.detect_yuv_tiled_device(tiled_in, thr, nms)
-    recs4k = _records(eng4k, d, c, B)
+    recs4k = eng4k.read_dets(d, c, B)[0]
     kernel_us = {}
     for name in ("detect+redact", "tiled+redact") + (("detect+mosaic",) if styled else ()):
         e, fn = runs[name]

@@ -926,7 +926,8 @@ int rf_track_follow_device(rf_tracker t, const rf_yuv_frame *frames, const int *
 int rf_track_follow_redact_device(rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, const rf_redact_style *style,
                                   const rf_track **dev_tracks, const int32_t **dev_track_counts);
 /* *dev_follow -> [n][max_tracks] rf_follow of the tracker's latest follow call, each frame's records in its track-list order (NULL
- * before the first); valid for `streams` further tracker calls.  RF_ERR_INVALID_ARG on a tracker that is not a follow tracker. */
+ * before the first); valid for `streams` further tracker calls.  RF_ERR_INVALID_ARG on a tracker that is not a follow tracker or a
+ * following look-back tracker (f18, below). */
 int rf_tracker_follow(rf_tracker t, const rf_follow **dev_follow);
 
 /* f17 searching look-back: f15's box only covers a face that moves less than grow x its size per frame back.  A SEARCHING look-back
@@ -958,6 +959,49 @@ int rf_tracker_set_lookback_search(rf_tracker t, const rf_follow_config *cfg);
  * T)] int32 the steps taken, the failing last one included (0 past the frame's births).  Valid for `streams` further tracker calls.
  * RF_ERR_INVALID_ARG on a tracker that is not searching. */
 int rf_tracker_lookback_search(rf_tracker t, const rf_follow **dev_steps, const int32_t **dev_lengths);
+
+/* f18 following look-back: f16 runs the detector every k-th frame only, so a face that first appears between two key frames goes out
+ * uncovered until the next key frame; f15 covers a face on the L frames before its first detection, but detects every frame.  A
+ * FOLLOWING look-back tracker does both: it is a look-back tracker (f15, with or without f13 motion and f17 search) on which
+ * rf_tracker_set_lookback_follow was called before its first update, and it takes two kinds of frames.
+ *   Detect frames  through rf_detect_yuv_redact_lookback_device, unchanged: records, scales, lists, motions, step records, out frames
+ *                  and numbers are bit for bit a plain look-back tracker's in the same state; in addition f16's Cut runs on them.
+ *   Follow frames  through rf_track_follow_redact_lookback_device: f16's follow step (lists and rf_follow records bit for bit a follow
+ *                  tracker's for the same calls, f13 motion with f16's face mask included), then each frame is buffered and emitted L
+ *                  frames late as a look-back frame is.
+ *   Frame numbers  detect and follow frames share one count per video, restarted by reset and drain.
+ *   Log            of a follow frame: (a) every OK-followed face's box in id order, at scale 1; (b) every LOST track in id order; no
+ *                  births (no track there has age == 1); its motion, the frame's f13 estimate.
+ *   Regions        of an emitted frame e: (a) and (b) of frame e -- f15's on a detect frame, the log above on a follow frame: what the
+ *                  undelayed call draws on e -- then f15's (c) for the births on frames e + 1 .. min(e + L, last) (births happen on
+ *                  detect frames only; the motion chain runs through every frame in between, follow frames included), then on a
+ *                  searching tracker f17's (d), whose steps read follow frames from the buffer like any other.  Geometry, styles,
+ *                  shapes and ownership are f12 / f14's, so an out frame differs from the undelayed redaction of e only on samples
+ *                  that (c) or (d) alone cover.
+ *   Coverage       with L >= k - 1, a face first detected on key frame b is covered on frames b - L .. b - 1 -- within f15's growth or
+ *                  f17's search, detect and follow frames alike.  A face visible only between two key frames is never detected, so
+ *                  it is never covered.
+ * Drain and reset work as on a look-back tracker and, since both restart the video, also drop its templates. */
+/* Makes a look-back tracker a following one, after rf_tracker_set_lookback and before the first update; before or after
+ * rf_tracker_set_motion and rf_tracker_set_lookback_search.  cfg: f16's rf_follow_config and bounds; allocates f16's template store
+ * (above 4 GiB: RF_ERR_CAPACITY).  Not a look-back tracker, a second call, a call after an update, or bad values: RF_ERR_INVALID_ARG,
+ * nothing changed.  A following look-back tracker takes rf_detect_yuv_redact_lookback_device, rf_track_follow_redact_lookback_device,
+ * rf_tracker_drain, rf_tracker_reset, rf_tracker_follow (the latest follow call's records) and the motion and search queries of its
+ * options; it refuses rf_track_update, rf_detect_yuv_track_device, rf_detect_yuv_redact_device(_style), rf_track_follow_device and
+ * rf_track_follow_redact_device (RF_ERR_INVALID_ARG): the buffer must see every frame. */
+int rf_tracker_set_lookback_follow(rf_tracker t, const rf_follow_config *cfg);
+/* The follow step of rf_track_follow_device on n device frames (frame i of video videos[i]), then the look-back half of
+ * rf_detect_yuv_redact_lookback_device: each frame is stored, and frame i, number num_i, emits frame num_i - L of its video into
+ * out_frames[i] with out_frame_numbers[i] = num_i - L, redacted with `style` (NULL: the zeroed struct's defaults) over the regions
+ * above; otherwise out_frame_numbers[i] = -1 and out_frames[i] is not written.  Statuses, all before anything is launched: those of
+ * rf_track_follow_device, a tracker that is not a following look-back tracker, a bad style, and the out-frame rules of
+ * rf_detect_yuv_redact_lookback_device (same size and layout or exactly frames[i], disjoint frames, at most L frames of one video per
+ * call, no size change before a drain or reset): RF_ERR_INVALID_ARG; a failed buffer allocation: RF_ERR_CAPACITY.  *dev_tracks /
+ * *dev_track_counts as rf_track_follow_device's.  Asynchronous on rf_last_stream()'s context, inside the tracker's event chain; the
+ * caller keeps the input and out frames alive until that stream has passed the call. */
+int rf_track_follow_redact_lookback_device(rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, const rf_redact_style *style,
+                                           const rf_yuv_frame *out_frames, int32_t *out_frame_numbers, const rf_track **dev_tracks,
+                                           const int32_t **dev_track_counts);
 
 /* Introspection. */
 int rf_get_net_size(rf_handle h, int *net_w, int *net_h, int *max_batch, int *max_faces);

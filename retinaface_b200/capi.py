@@ -373,6 +373,8 @@ _SIGNATURES = {
     "rf_track_follow_device": (_I, [_P, _FRAMES, _P, _I, _PP, _PP]), "rf_tracker_follow": (_I, [_P, _PP]),
     "rf_track_follow_redact_device": (_I, [_P, _FRAMES, _P, _I, _STYLE, _PP, _PP]),
     "rf_tracker_set_lookback_search": (_I, [_P, C.POINTER(FollowConfig)]), "rf_tracker_lookback_search": (_I, [_P, _PP, _PP]),
+    "rf_tracker_set_lookback_follow": (_I, [_P, C.POINTER(FollowConfig)]),
+    "rf_track_follow_redact_lookback_device": (_I, [_P, _FRAMES, _P, _I, _STYLE, _FRAMES, _P, _PP, _PP]),
 }
 EXPORTS = list(_SIGNATURES)     # every symbol include/rf_b200.h declares (checked by tests/test_host_side.py)
 
@@ -1034,7 +1036,7 @@ class Engine:
     # -- f10 face tracking across video frames ---------------------------------------------------------------------------------
     def tracker(self, max_videos: int = 1, max_tracks: int = 0, high_thresh: float = 0.0, new_thresh: float = 0.0, iou_high: float = 0.0,
                 iou_low: float = 0.0, iou_tentative: float = 0.0, max_lost: int = 0, best: Optional[dict] = None,
-                motion=None, lookback=None, follow=None, lookback_search=None) -> "Tracker":
+                motion=None, lookback=None, follow=None, lookback_search=None, lookback_follow=None) -> "Tracker":
         """rf_tracker_create: a tracker of max_videos independent sequences on this engine (0 -> the defaults of rf_track_config).
         best (``best_config`` keywords): a best-shot tracker (rf_tracker_create_best), fed through ``Tracker.detect_yuv_best_device``.
         motion (True or ``motion_config`` keywords): camera-motion compensation (rf_tracker_set_motion) from the frames of the
@@ -1042,7 +1044,9 @@ class Engine:
         look-back tracker (rf_tracker_set_lookback), fed through ``Tracker.detect_yuv_redact_lookback_device``.  follow (True or
         ``set_follow`` keywords): a follow tracker (rf_tracker_set_follow), whose frames between detections go through
         ``Tracker.follow_device``.  lookback_search (True or ``set_lookback_search`` keywords, with lookback): a searching look-back
-        tracker (rf_tracker_set_lookback_search)."""
+        tracker (rf_tracker_set_lookback_search).  lookback_follow (True or ``set_lookback_follow`` keywords, with lookback): a
+        following look-back tracker (rf_tracker_set_lookback_follow), whose frames between detections go through
+        ``Tracker.follow_redact_lookback_device``."""
         t = Tracker(self, TrackConfig(max_videos, max_tracks, high_thresh, new_thresh, iou_high, iou_low, iou_tentative, max_lost),
                     best_config(**best) if best is not None else None)
         try:
@@ -1054,6 +1058,8 @@ class Engine:
                 t.set_follow(**(follow if isinstance(follow, dict) else {}))
             if lookback_search:
                 t.set_lookback_search(**(lookback_search if isinstance(lookback_search, dict) else {}))
+            if lookback_follow:
+                t.set_lookback_follow(**(lookback_follow if isinstance(lookback_follow, dict) else {}))
         except Exception:
             t.close()
             raise
@@ -1156,6 +1162,7 @@ class Tracker:
         self.lookback = 0            # L of a look-back tracker
         self.follow_on = False
         self.lookback_search_on = False
+        self.lookback_follow_on = False
         self.max_videos = cfg.max_videos
         self.max_tracks = cfg.max_tracks or 64
 
@@ -1298,6 +1305,30 @@ class Tracker:
         bcap = min(self.engine.max_faces, self.max_tracks)
         return self.engine._fetch(p.value, FOLLOW_DTYPE, n, bcap, self.lookback), self.engine._fetch(q.value, np.int32, n, bcap)
 
+    def set_lookback_follow(self, search: int = 0, max_mad: float = 0.0):
+        """rf_tracker_set_lookback_follow, after ``set_lookback`` and before the first update: cut f16's templates on the detect frames
+        so that the frames in between can go through ``follow_redact_lookback_device`` (search: R in template pixels, 0 -> 8; max_mad:
+        0 -> 24)."""
+        cfg = FollowConfig(int(search), float(max_mad))
+        self.engine._check(self.lib.rf_tracker_set_lookback_follow(self.t, C.byref(cfg)))
+        self.lookback_follow_on = True
+
+    def follow_redact_lookback_device(self, frames, videos: Sequence[int], out_frames, layout: str = "nv12", blocks: int = 0,
+                                      margin: float = 0.0, style: str = "mosaic", shape: str = "rect", detail: int = 0):
+        """rf_track_follow_redact_lookback_device on a following look-back tracker: follow the faces of the device 4:2:0 frames by
+        template search, store the frames, and write frame num - L of each frame's video, redacted, into out_frames[i] (as
+        ``detect_yuv_redact_lookback_device``).  Returns (out frame numbers (-1: nothing emitted), tracks_ptr, track_counts_ptr)."""
+        n = len(frames)
+        if len(out_frames) != n:
+            raise ValueError(f"{n} frames but {len(out_frames)} out frames")
+        arr = self.engine._frames(frames, layout, True)
+        outs = self.engine._frames(out_frames, layout, True)
+        fn, st = _redaction(self.lib, "rf_track_follow_redact_lookback_device", style, shape, blocks, detail, margin)
+        nums = np.full(max(n, 1), -1, dtype=np.int32)
+        tp, tc = C.c_void_p(), C.c_void_p()
+        self.engine._check(fn(self.t, arr, self._ints(videos, n), n, C.byref(st), outs, nums.ctypes.data, C.byref(tp), C.byref(tc)))
+        return nums[:n].copy(), int(tp.value or 0), int(tc.value or 0)
+
     def drain(self, video: int, out_frames, layout: str = "nv12", blocks: int = 0, margin: float = 0.0, style: str = "mosaic",
               shape: str = "rect", detail: int = 0) -> np.ndarray:
         """rf_tracker_drain: write the video's buffered frames (at most L, in frame order) into out_frames[0..), then restart the video.
@@ -1338,8 +1369,8 @@ class Tracker:
         return int(tp.value or 0), int(tc.value or 0)
 
     def follow(self, n: int) -> np.ndarray:
-        """rf_tracker_follow: the [n][max_tracks] rf_follow records (FOLLOW_DTYPE) of the latest follow call, each frame's in its
-        track-list order, copied after the last stream."""
+        """rf_tracker_follow: the [n][max_tracks] rf_follow records (FOLLOW_DTYPE) of the latest follow call (of a follow or a
+        following look-back tracker), each frame's in its track-list order, copied after the last stream."""
         p = C.c_void_p()
         self.engine._check(self.lib.rf_tracker_follow(self.t, C.byref(p)))
         if not p.value:

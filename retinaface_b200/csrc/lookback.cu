@@ -42,10 +42,10 @@ __global__ void __launch_bounds__(LOOKBACK_THREADS) k_lookback_log(const Lookbac
     float4 *ab = const_cast<float4 *>(slot_boxes(slot));
     LookbackBirth *births = const_cast<LookbackBirth *>(slot_births(slot, a.max_faces, a.max_tracks));
     const int bcap = min(a.max_faces, a.max_tracks);
-    const int na = min(max(a.counts[i], 0), a.max_faces);
+    const int na = min(max(a.counts[i], 0), t.per_frame);
     const float sc = t.scale[k];
     for (int j = threadIdx.x; j < na; j += LOOKBACK_THREADS) {      // (a): f12's map-back
-        const rf_face &f = a.dets[(size_t)i * a.max_faces + j].face;
+        const rf_face &f = a.dets[(size_t)i * t.per_frame + j].face;
         ab[j] = make_float4(__fmul_rn(f.x1, sc), __fmul_rn(f.y1, sc), __fmul_rn(f.x2, sc), __fmul_rn(f.y2, sc));
     }
     const int nt = min(max(a.track_counts[i], 0), a.max_tracks);

@@ -2,6 +2,7 @@
 // device, every frame emitted L frames late and covered where the faces born in the following L frames already were.  Per call, on the
 // forward's stream inside the tracker's event chain, after the track update:
 //   k_lookback_log    one CTA per frame: the frame's (a) + (b) boxes, its births and its rf_motion into the video's log slot
+//                     (f18: also a follow frame's, whose (a) are its OK-followed faces and which has no births)
 //   k_lookback_swap   one launch over all frames: each thread moves one 16-byte chunk of a plane row -- the buffered frame out, the
 //                     input in -- so an out frame equal to its input frame is safe
 //   k_lookback_boxes  one CTA per emitted frame: its (a) + (b) + (c) boxes as rf_det records of scale 1, for f12 / f14's kernels
@@ -62,9 +63,10 @@ struct LookbackArgs {
     int *lengths;
 };
 
-// k_lookback_log: frame i0 + k of the call into log slot `slot[k]`.
+// k_lookback_log: frame i0 + k of the call into log slot `slot[k]`.  per_frame: (a)'s records per frame of a.dets and their cap --
+// max_faces on a detect call (the forward's records), max_tracks on an f18 follow call (the OK-followed faces).
 struct LookbackLogTable {
-    int n, i0;
+    int n, i0, per_frame;
     float scale[LOOKBACK_TABLE];
     uint8_t *slot[LOOKBACK_TABLE];
 };

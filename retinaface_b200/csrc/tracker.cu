@@ -1,6 +1,6 @@
 // tracker.cu -- the video tracker behind include/rf_b200.h: f10 tracking, f11 best shots, f13 camera motion, f16 following, f12 / f14
-// redaction, f15 look-back and f17 searching look-back.  Detection itself is engine.cu's (yuv_device_impl).  The entry points take
-// their C linkage from rf_b200.h.
+// redaction, f15 look-back, f17 searching look-back and f18 following look-back.  Detection itself is engine.cu's (yuv_device_impl).
+// The entry points take their C linkage from rf_b200.h.
 #include <array>
 #include <cmath>
 
@@ -20,7 +20,7 @@
 // waits for it.
 //
 // A tracker is of one kind: plain, best-shot (f11), follow (f16) or look-back (f15).  Camera motion (f13) is an option of any kind,
-// the look-back search (f17) one of a look-back tracker.  admit() decides from them which calls it takes.
+// the look-back search (f17) and following (f18) options of a look-back tracker.  admit() decides from them which calls it takes.
 enum Kind { PLAIN, BEST, FOLLOW, LOOKBACK };
 
 struct rf_tracker_s {
@@ -82,8 +82,10 @@ struct rf_tracker_s {
     bool lb_search = false;
     rf_follow_config lscfg{};
     int lb_search_slot = -1;           // the ring slot of the latest look-back call
-    // f16 following (follow.cuh); allocated on a FOLLOW tracker.  The chain orders the per-call measurements as it orders f11's
-    // tables; the follow records live in the ring.
+    // f18 following look-back: a LOOKBACK tracker that also takes follow frames, with f16's store and follow records below.
+    bool lb_follow = false;
+    // f16 following (follow.cuh); allocated on a FOLLOW tracker and on a following look-back tracker.  The chain orders the per-call
+    // measurements as it orders f11's tables; the follow records live in the ring.
     rf_follow_config fcfg{};
     uint8_t *d_fstore = nullptr;         // [max_videos][max_tracks][FOLLOW_BYTES]
     FollowEntry *d_fentries = nullptr;   // [max_videos][max_tracks]
@@ -187,7 +189,7 @@ void rf_tracker_destroy(rf_tracker t) {
 }
 
 // Restarts videos [v0, v0 + nv) on s, inside the chain: no tracks, and by the kind no stored shots (BEST, nothing is emitted), no
-// templates (FOLLOW) and no buffered frames (LOOKBACK, nothing is emitted); with motion, no reference.
+// templates (FOLLOW, and a following LOOKBACK) and no buffered frames (LOOKBACK, nothing is emitted); with motion, no reference.
 static void restart(rf_tracker t, size_t v0, size_t nv, cudaStream_t s) {
     const size_t T = t->cfg.max_tracks;
     CK(cudaMemsetAsync(t->d_videos + v0, 0, sizeof(TrackVideo) * nv, s));
@@ -196,7 +198,7 @@ static void restart(rf_tracker t, size_t v0, size_t nv, cudaStream_t s) {
         CK(cudaMemsetAsync(t->ba.store + v0 * T, 0, sizeof(BestEntry) * nv * T, s));
         CK(cudaMemsetAsync(t->ba.videos + v0, 0, sizeof(BestVideo) * nv, s));
     }
-    if (t->kind == FOLLOW) CK(cudaMemsetAsync(t->d_fentries + v0 * T, 0, sizeof(FollowEntry) * nv * T, s));
+    if (t->kind == FOLLOW || t->lb_follow) CK(cudaMemsetAsync(t->d_fentries + v0 * T, 0, sizeof(FollowEntry) * nv * T, s));
     for (size_t v = v0; t->motion && v < v0 + nv; v++) t->mref[v] = {0, 0};
     for (size_t v = v0; t->kind == LOOKBACK && v < v0 + nv; v++) t->lbv[v].frames = 0;
 }
@@ -216,11 +218,12 @@ int rf_tracker_reset(rf_tracker t, int video) {
     return RF_OK;
 }
 
-// The calls admit() decides.  DETECT: rf_detect_yuv_track_device and rf_detect_yuv_redact_device(_style) with a tracker; MOTION,
-// FOLLOWS and LOOKBACK_SEARCH: the queries rf_tracker_motion, rf_tracker_follow and rf_tracker_lookback_search.
+// The calls admit() decides.  DETECT: rf_detect_yuv_track_device and rf_detect_yuv_redact_device(_style) with a tracker; FOLLOW:
+// rf_track_follow_device and rf_track_follow_redact_device; LOOKBACK_FOLLOW: rf_track_follow_redact_lookback_device; MOTION, FOLLOWS
+// and LOOKBACK_SEARCH: the queries rf_tracker_motion, rf_tracker_follow and rf_tracker_lookback_search.
 enum class Call {
-    UPDATE, DETECT, BEST, FINISH, FOLLOW, LOOKBACK, DRAIN,
-    SET_MOTION, SET_FOLLOW, SET_LOOKBACK, SET_LOOKBACK_SEARCH,         // the setters, in this range
+    UPDATE, DETECT, BEST, FINISH, FOLLOW, LOOKBACK, DRAIN, LOOKBACK_FOLLOW,
+    SET_MOTION, SET_FOLLOW, SET_LOOKBACK, SET_LOOKBACK_SEARCH, SET_LOOKBACK_FOLLOW,      // the setters, in this range
     MOTION, FOLLOWS, LOOKBACK_SEARCH
 };
 
@@ -234,19 +237,24 @@ static int admit(rf_tracker t, const char *who, Call call) {
         if (k != need) why = fmt("not a %s tracker (%s)", name[need], made_by[need]);
     };
     auto only_through = [&]() {
+        if (t->lb_follow)
+            return std::string("a following look-back tracker takes frames only through rf_detect_yuv_redact_lookback_device and "
+                               "rf_track_follow_redact_lookback_device");
         return fmt("a %s tracker takes frames only through %s", name[k],
                    k == BEST ? "rf_detect_yuv_track_best_device" : "rf_detect_yuv_redact_lookback_device");
     };
     switch (call) {
     case Call::UPDATE:
-        if (k == BEST) why = only_through();
+        if (k == BEST || t->lb_follow) why = only_through();
         else if (t->motion || k == FOLLOW) why = fmt("a %s tracker needs the frames (rf_detect_yuv_track_device)", t->motion ? "motion" : "follow");
         else if (k == LOOKBACK) why = only_through();
         break;
     case Call::DETECT: if (k == BEST || k == LOOKBACK) why = only_through(); break;
     case Call::BEST: case Call::FINISH: only(BEST); break;
-    case Call::FOLLOW: case Call::FOLLOWS: only(FOLLOW); break;
+    case Call::FOLLOW: if (t->lb_follow) why = only_through(); else only(FOLLOW); break;
+    case Call::FOLLOWS: if (!t->lb_follow) only(FOLLOW); break;
     case Call::LOOKBACK: case Call::DRAIN: only(LOOKBACK); break;
+    case Call::LOOKBACK_FOLLOW: if (!t->lb_follow) why = "not a following look-back tracker (rf_tracker_set_lookback_follow)"; break;
     case Call::SET_MOTION: if (t->motion) why = "motion is already on"; break;
     case Call::SET_FOLLOW: if (k != PLAIN) why = k == FOLLOW ? "following is already on" : fmt("a %s tracker cannot follow", name[k]); break;
     case Call::SET_LOOKBACK: if (k != PLAIN) why = k == LOOKBACK ? "look-back is already on" : fmt("a %s tracker cannot look back", name[k]); break;
@@ -254,10 +262,14 @@ static int admit(rf_tracker t, const char *who, Call call) {
         only(LOOKBACK);
         if (why.empty() && t->lb_search) why = "the look-back search is already on";
         break;
+    case Call::SET_LOOKBACK_FOLLOW:
+        only(LOOKBACK);
+        if (why.empty() && t->lb_follow) why = "look-back following is already on";
+        break;
     case Call::MOTION: if (!t->motion) why = "motion is off (rf_tracker_set_motion)"; break;
     case Call::LOOKBACK_SEARCH: if (!t->lb_search) why = "not a searching look-back tracker (rf_tracker_set_lookback_search)"; break;
     }
-    if (why.empty() && call >= Call::SET_MOTION && call <= Call::SET_LOOKBACK_SEARCH && t->updated) why = "the tracker has already been updated";
+    if (why.empty() && call >= Call::SET_MOTION && call <= Call::SET_LOOKBACK_FOLLOW && t->updated) why = "the tracker has already been updated";
     return why.empty() ? RF_OK : fail(t->h, RF_ERR_INVALID_ARG, fmt("%s: %s", who, why.c_str()));
 }
 
@@ -450,7 +462,7 @@ static unsigned track_issue(rf_tracker t, const int *videos, int n, const rf_det
     }
     CK(launch_track_update(ta, videos, scales, n, s));
     if (t->motion) motion_commit(t, commits, s);
-    if (t->kind == FOLLOW) follow_cut(t, frames, videos, n, slot, s);
+    if (t->kind == FOLLOW || t->lb_follow) follow_cut(t, frames, videos, n, slot, s);     // before a look-back call's swap: it reads the inputs
     CK(cudaEventRecord(t->chain, s));
     if (a) {
         PostBuffers view{};
@@ -717,15 +729,10 @@ static int follow_config(rf_handle h, const char *who, const rf_follow_config *c
     return RF_OK;
 }
 
-int rf_tracker_set_follow(rf_tracker t, const rf_follow_config *cfg) {
-    static const char *who = "rf_tracker_set_follow";
-    if (!t) return RF_ERR_INVALID_ARG;
+// f16's template store, measurements and face masks, and the ring's follow records and regions, for rf_tracker_set_follow and
+// rf_tracker_set_lookback_follow (admitted, cfg checked).  On failure nothing stays allocated.
+static int follow_alloc(rf_tracker t, const char *who, const rf_follow_config &fc) {
     rf_handle h = t->h;
-    if (!cfg) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL config", who));
-    int rc = admit(t, who, Call::SET_FOLLOW);
-    if (rc) return rc;
-    rf_follow_config fc;
-    if ((rc = follow_config(h, who, cfg, fc))) return rc;
     const size_t V = t->cfg.max_videos, T = t->cfg.max_tracks, B = h->cfg.max_batch;
     if (V * T * FOLLOW_BYTES > ((size_t)4 << 30))
         return fail(h, RF_ERR_CAPACITY, fmt("%s: a store of %zu videos x %zu tracks x %d bytes exceeds 4 GiB", who, V, T, FOLLOW_BYTES));
@@ -747,14 +754,27 @@ int rf_tracker_set_follow(rf_tracker t, const rf_follow_config *cfg) {
         free_follow(t);
         return fail_cuda(h, f);
     }
-    t->kind = FOLLOW;
     t->fcfg = fc;
     return RF_OK;
 }
 
-// Everything a follow call refuses, checked before anything is launched.
-static int check_follow(rf_tracker t, const char *who, const rf_yuv_frame *frames, const int *videos, int n) {
-    int rc = check_track_args(t, who, Call::FOLLOW, videos, n, nullptr);
+int rf_tracker_set_follow(rf_tracker t, const rf_follow_config *cfg) {
+    static const char *who = "rf_tracker_set_follow";
+    if (!t) return RF_ERR_INVALID_ARG;
+    rf_handle h = t->h;
+    if (!cfg) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL config", who));
+    int rc = admit(t, who, Call::SET_FOLLOW);
+    if (rc) return rc;
+    rf_follow_config fc;
+    if ((rc = follow_config(h, who, cfg, fc)) || (rc = follow_alloc(t, who, fc))) return rc;
+    t->kind = FOLLOW;
+    return RF_OK;
+}
+
+// Everything a follow call (FOLLOW, or f18's LOOKBACK_FOLLOW) refuses in its tracker, videos and frames, checked before anything is
+// launched.
+static int check_follow(rf_tracker t, const char *who, Call call, const rf_yuv_frame *frames, const int *videos, int n) {
+    int rc = check_track_args(t, who, call, videos, n, nullptr);
     return rc ? rc : check_frames(t->h, who, frames, n, RF_YUV_BT601);
 }
 
@@ -825,7 +845,7 @@ int rf_track_follow_device(rf_tracker t, const rf_yuv_frame *frames, const int *
     static const char *who = "rf_track_follow_device";
     if (!t) return RF_ERR_INVALID_ARG;
     rf_handle h = t->h;
-    int rc = check_follow(t, who, frames, videos, n);
+    int rc = check_follow(t, who, Call::FOLLOW, frames, videos, n);
     if (rc) return rc;
     if (n == 0) return RF_OK;
     try {
@@ -1165,7 +1185,7 @@ int rf_track_follow_redact_device(rf_tracker t, const rf_yuv_frame *frames, cons
     static const char *who = "rf_track_follow_redact_device";
     if (!t) return RF_ERR_INVALID_ARG;
     rf_handle h = t->h;
-    int rc = check_follow(t, who, frames, videos, n);
+    int rc = check_follow(t, who, Call::FOLLOW, frames, videos, n);
     if (rc) return rc;
     RedactSpec spec;
     if ((rc = redact_style(h, who, style, spec))) return rc;
@@ -1401,24 +1421,16 @@ static bool lb_alloc(rf_tracker t, rf_tracker_s::LookbackVideo &v, const rf_yuv_
     return true;
 }
 
-int rf_detect_yuv_redact_lookback_device(rf_handle h, rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, int matrix, float thr,
-                                         float nms, const rf_redact_style *style, const rf_yuv_frame *out_frames, int32_t *out_frame_numbers,
-                                         const rf_track **dev_tracks, const int32_t **dev_track_counts, const rf_det **dev_dets,
-                                         const int32_t **dev_counts, float *out_scales) {
-    static const char *who = "rf_detect_yuv_redact_lookback_device";
-    if (!h) return RF_ERR_INVALID_ARG;
-    if (!t || t->h != h) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker is NULL or belongs to another handle", who));
-    int rc = check_track_args(t, who, Call::LOOKBACK, videos, n, nullptr);
-    if (rc) return rc;
-    const YuvFrames src{frames, matrix, nullptr, false};
-    if ((rc = src.check(h, who, n))) return rc;
-    RedactSpec spec;
-    if ((rc = redact_style(h, who, style, spec))) return rc;
+// The frame numbers of a look-back call's n frames (each video's count on), and every rule its frames and out frames must keep; checked
+// before anything is launched.  A video's size and layout are those of its buffered frames, else of its first frame in the call.
+// seen: (video, its first frame of the call, its frames in the call).
+static int lb_numbers(rf_tracker t, const char *who, const rf_yuv_frame *frames, const int *videos, int n, const rf_yuv_frame *out_frames,
+                      const int32_t *out_frame_numbers, std::vector<long long> &num, std::vector<std::array<int, 3>> &seen) {
+    rf_handle h = t->h;
     if (n > 0 && (!out_frames || !out_frame_numbers)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL out frames or frame numbers", who));
     const int L = t->lb_frames;
-    // each frame's number; a video's size and layout are those of its buffered frames, else of its first frame in the call
-    std::vector<long long> num(n);
-    std::vector<std::array<int, 3>> seen;        // (video, first frame of the call, frames in the call)
+    int rc;
+    num.assign(n, 0);
     auto ranges = yuv_ranges(frames, n);
     for (int i = 0; i < n; i++) {
         const int v = videos[i];
@@ -1437,83 +1449,169 @@ int rf_detect_yuv_redact_lookback_device(rf_handle h, rf_tracker t, const rf_yuv
         if (!same_frame(out_frames[i], f))
             for (auto &r : yuv_ranges(out_frames + i, 1)) ranges.push_back({r[0], r[1], (uintptr_t)(n + i)});
     }
-    if ((rc = check_disjoint(h, who, ranges))) return rc;
+    return check_disjoint(h, who, ranges);
+}
+
+// The buffers of the call's videos that have no buffered frames (lb_numbers' `seen`).
+static int lb_alloc_videos(rf_tracker t, const char *who, const rf_yuv_frame *frames, const std::vector<std::array<int, 3>> &seen) {
+    for (const auto &e : seen) {
+        rf_tracker_s::LookbackVideo &lv = t->lbv[e[0]];
+        if (lv.frames > 0) continue;
+        const rf_yuv_frame &f = frames[e[1]];
+        if (!lb_alloc(t, lv, f))
+            return fail(t->h, RF_ERR_CAPACITY, fmt("%s: video %d: no device memory for %d frames of %dx%d", who, e[0], t->lb_frames, f.width, f.height));
+        lv.w = f.width;
+        lv.h = f.height;
+        lv.step = f.uv_step;
+        lv.v_first = f.uv_step == 2 && f.v < f.u;
+    }
+    return RF_OK;
+}
+
+// The look-back half of a call whose tracking was issued on c's stream into ring slot `ring` (it recorded the chain; this follows it
+// on the same stream and records it again, then the slot's `free`).  a: the frames' (a) records, per_frame of them to a frame, and
+// counts; scales: their map-back factors (NULL: 1).  Each frame's log, f17's chains on a detect call (births: a follow frame has
+// none), then the swap -- after every kernel that reads an input frame, since an out frame may be its own input -- the regions and
+// the redaction of the emitted frames.
+static void lb_issue(rf_tracker t, Ctx &c, unsigned ring, const rf_det *dets, const int32_t *counts, int per_frame, const float *scales,
+                     bool births, const rf_yuv_frame *frames, const int *videos, int n, const std::vector<long long> &num,
+                     const rf_yuv_frame *out_frames, const RedactSpec &spec) {
+    rf_handle h = t->h;
+    rf_tracker_s::Slot &slot = t->slots[ring];
+    const int L = t->lb_frames;
+    LookbackArgs a{};
+    a.dets = dets;
+    a.counts = counts;
+    a.tracks = slot.tracks;
+    a.track_counts = slot.counts;
+    a.motion = t->motion ? slot.motion : nullptr;
+    a.max_faces = h->cfg.max_faces;
+    a.max_tracks = t->cfg.max_tracks;
+    a.slot_bytes = lb_slot_bytes(t);
+    a.ring = 2 * L;
+    a.L = L;
+    for (int i0 = 0; i0 < n; i0 += LOOKBACK_TABLE) {
+        LookbackLogTable lt{};
+        lt.i0 = i0;
+        lt.per_frame = per_frame;
+        for (int i = i0; i < std::min(n, i0 + LOOKBACK_TABLE); i++, lt.n++) {
+            lt.scale[lt.n] = scales ? scales[i] : 1.f;
+            lt.slot[lt.n] = lb_log(t, t->lbv[videos[i]]) + (size_t)(num[i] % a.ring) * a.slot_bytes;
+        }
+        CK(launch_lookback_log(a, lt, c.stream));
+    }
+    if (t->lb_search && births) {
+        a.search = t->lscfg.search;
+        a.max_mad = t->lscfg.max_mad;
+        a.steps = slot.lb_steps;
+        a.lengths = slot.lb_lengths;
+        lb_search(t, frames, videos, n, num, a, c.stream);
+        t->lb_search_slot = (int)ring;
+    }
+    std::vector<LookbackSwapFrame> sw;
+    std::vector<std::array<long long, 3>> em;
+    std::vector<rf_yuv_frame> outs;
+    for (int i = 0; i < n; i++) {
+        const rf_tracker_s::LookbackVideo &lv = t->lbv[videos[i]];
+        const bool emits = num[i] >= L;
+        sw.push_back(lb_swap_frame(frames + i, emits ? out_frames + i : nullptr, lv.d + (size_t)(num[i] % L) * lv.frame_bytes));
+        if (emits) {
+            em.push_back({videos[i], num[i] - L, L});
+            outs.push_back(out_frames[i]);
+        }
+    }
+    lb_swap(sw, c.stream);
+    lb_boxes(t, slot, em, c.stream);
+    CK(cudaEventRecord(t->chain, c.stream));
+    if (!em.empty())
+        redact_issue(h, c, yuv_redact_table(outs.data(), (int)outs.size(), nullptr), slot.lb_boxes, slot.lb_counts, nullptr, nullptr, nullptr,
+                     spec, lb_records(t));
+    CK(cudaEventRecord(slot.free, c.stream));
+}
+
+// After an issued look-back call: each video's count, and each frame's emitted number (-1: none).
+static void lb_commit(rf_tracker t, const int *videos, int n, const std::vector<long long> &num, int32_t *out_frame_numbers) {
+    const int L = t->lb_frames;
+    for (int i = 0; i < n; i++) {
+        t->lbv[videos[i]].frames = std::max(t->lbv[videos[i]].frames, num[i] + 1);
+        out_frame_numbers[i] = num[i] >= L ? (int32_t)(num[i] - L) : -1;
+    }
+}
+
+int rf_detect_yuv_redact_lookback_device(rf_handle h, rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, int matrix, float thr,
+                                         float nms, const rf_redact_style *style, const rf_yuv_frame *out_frames, int32_t *out_frame_numbers,
+                                         const rf_track **dev_tracks, const int32_t **dev_track_counts, const rf_det **dev_dets,
+                                         const int32_t **dev_counts, float *out_scales) {
+    static const char *who = "rf_detect_yuv_redact_lookback_device";
+    if (!h) return RF_ERR_INVALID_ARG;
+    if (!t || t->h != h) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker is NULL or belongs to another handle", who));
+    int rc = check_track_args(t, who, Call::LOOKBACK, videos, n, nullptr);
+    if (rc) return rc;
+    const YuvFrames src{frames, matrix, nullptr, false};
+    if ((rc = src.check(h, who, n))) return rc;
+    RedactSpec spec;
+    if ((rc = redact_style(h, who, style, spec))) return rc;
+    std::vector<long long> num;
+    std::vector<std::array<int, 3>> seen;
+    if ((rc = lb_numbers(t, who, frames, videos, n, out_frames, out_frame_numbers, num, seen))) return rc;
     if (n == 0) return RF_OK;
     try {
         CK(cudaSetDevice(h->device));
-        for (const auto &e : seen) {
-            rf_tracker_s::LookbackVideo &lv = t->lbv[e[0]];
-            if (lv.frames > 0) continue;
-            const rf_yuv_frame &f = frames[e[1]];
-            if (!lb_alloc(t, lv, f))
-                return fail(h, RF_ERR_CAPACITY, fmt("%s: video %d: no device memory for %d frames of %dx%d", who, e[0], L, f.width, f.height));
-            lv.w = f.width;
-            lv.h = f.height;
-            lv.step = f.uv_step;
-            lv.v_first = f.uv_step == 2 && f.v < f.u;
-        }
+        if ((rc = lb_alloc_videos(t, who, frames, seen))) return rc;
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     Detected d;
     if ((rc = detect_for_tracker(h, who, src, n, thr, nms, d, dev_dets, dev_counts, out_scales))) return rc;
     try {
         Ctx &c = last_ctx(h);          // the forward's context
         const unsigned ring = track_issue(t, videos, n, d.dets, d.counts, d.scales.data(), frames, c.stream);
+        if (dev_tracks) *dev_tracks = t->slots[ring].tracks;
+        if (dev_track_counts) *dev_track_counts = t->slots[ring].counts;
+        lb_issue(t, c, ring, d.dets, d.counts, h->cfg.max_faces, d.scales.data(), true, frames, videos, n, num, out_frames, spec);
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    lb_commit(t, videos, n, num, out_frame_numbers);
+    return RF_OK;
+}
+
+// ---- f18 following look-back ----------------------------------------------------------------------------------------------------
+int rf_tracker_set_lookback_follow(rf_tracker t, const rf_follow_config *cfg) {
+    static const char *who = "rf_tracker_set_lookback_follow";
+    if (!t) return RF_ERR_INVALID_ARG;
+    rf_handle h = t->h;
+    if (!cfg) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL config", who));
+    int rc = admit(t, who, Call::SET_LOOKBACK_FOLLOW);
+    if (rc) return rc;
+    rf_follow_config fc;
+    if ((rc = follow_config(h, who, cfg, fc)) || (rc = follow_alloc(t, who, fc))) return rc;
+    t->lb_follow = true;
+    return RF_OK;
+}
+
+int rf_track_follow_redact_lookback_device(rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, const rf_redact_style *style,
+                                           const rf_yuv_frame *out_frames, int32_t *out_frame_numbers, const rf_track **dev_tracks,
+                                           const int32_t **dev_track_counts) {
+    static const char *who = "rf_track_follow_redact_lookback_device";
+    if (!t) return RF_ERR_INVALID_ARG;
+    rf_handle h = t->h;
+    int rc = check_follow(t, who, Call::LOOKBACK_FOLLOW, frames, videos, n);
+    if (rc) return rc;
+    RedactSpec spec;
+    if ((rc = redact_style(h, who, style, spec))) return rc;
+    std::vector<long long> num;
+    std::vector<std::array<int, 3>> seen;
+    if ((rc = lb_numbers(t, who, frames, videos, n, out_frames, out_frame_numbers, num, seen))) return rc;
+    if (n == 0) return RF_OK;
+    try {
+        CK(cudaSetDevice(h->device));
+        if ((rc = lb_alloc_videos(t, who, frames, seen))) return rc;
+        Ctx &c = last_ctx(h);
+        const unsigned ring = follow_issue(t, frames, videos, n, c.stream);
         rf_tracker_s::Slot &slot = t->slots[ring];
         if (dev_tracks) *dev_tracks = slot.tracks;
         if (dev_track_counts) *dev_track_counts = slot.counts;
-        // the update recorded the chain; the look-back state follows it on the same stream and records it again
-        LookbackArgs a{};
-        a.dets = d.dets;
-        a.counts = d.counts;
-        a.tracks = slot.tracks;
-        a.track_counts = slot.counts;
-        a.motion = t->motion ? slot.motion : nullptr;
-        a.max_faces = h->cfg.max_faces;
-        a.max_tracks = t->cfg.max_tracks;
-        a.slot_bytes = lb_slot_bytes(t);
-        a.ring = 2 * L;
-        a.L = L;
-        for (int i0 = 0; i0 < n; i0 += LOOKBACK_TABLE) {
-            LookbackLogTable lt{};
-            lt.i0 = i0;
-            for (int i = i0; i < std::min(n, i0 + LOOKBACK_TABLE); i++, lt.n++) {
-                lt.scale[lt.n] = d.scales[i];
-                lt.slot[lt.n] = lb_log(t, t->lbv[videos[i]]) + (size_t)(num[i] % a.ring) * a.slot_bytes;
-            }
-            CK(launch_lookback_log(a, lt, c.stream));
-        }
-        if (t->lb_search) {
-            a.search = t->lscfg.search;
-            a.max_mad = t->lscfg.max_mad;
-            a.steps = slot.lb_steps;
-            a.lengths = slot.lb_lengths;
-            lb_search(t, frames, videos, n, num, a, c.stream);
-            t->lb_search_slot = (int)ring;
-        }
-        std::vector<LookbackSwapFrame> sw;
-        std::vector<std::array<long long, 3>> em;
-        std::vector<rf_yuv_frame> outs;
-        for (int i = 0; i < n; i++) {
-            const rf_tracker_s::LookbackVideo &lv = t->lbv[videos[i]];
-            const bool emits = num[i] >= L;
-            sw.push_back(lb_swap_frame(frames + i, emits ? out_frames + i : nullptr, lv.d + (size_t)(num[i] % L) * lv.frame_bytes));
-            if (emits) {
-                em.push_back({videos[i], num[i] - L, L});
-                outs.push_back(out_frames[i]);
-            }
-        }
-        lb_swap(sw, c.stream);
-        lb_boxes(t, slot, em, c.stream);
-        CK(cudaEventRecord(t->chain, c.stream));
-        if (!em.empty())
-            redact_issue(h, c, yuv_redact_table(outs.data(), (int)outs.size(), nullptr), slot.lb_boxes, slot.lb_counts, nullptr, nullptr, nullptr,
-                         spec, lb_records(t));
-        CK(cudaEventRecord(slot.free, c.stream));
+        // (a): the OK-followed faces in id order, max_tracks to a frame, at scale 1 -- what rf_track_follow_redact_device draws
+        lb_issue(t, c, ring, slot.fregions, slot.fregion_counts, t->cfg.max_tracks, nullptr, false, frames, videos, n, num, out_frames, spec);
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    for (int i = 0; i < n; i++) {
-        t->lbv[videos[i]].frames = std::max(t->lbv[videos[i]].frames, num[i] + 1);
-        out_frame_numbers[i] = num[i] >= L ? (int32_t)(num[i] - L) : -1;
-    }
+    lb_commit(t, videos, n, num, out_frame_numbers);
     return RF_OK;
 }
 

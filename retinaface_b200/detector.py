@@ -140,9 +140,13 @@ class RetinaFace:
     def _interval_tracker(self, detect_every: int, best=None, lookback=0):
         if int(detect_every) < 1:
             raise ValueError(f"detect_every {detect_every}, must be >= 1")
-        if detect_every > 1 and (best is not None or lookback):
-            raise ValueError("detect_every > 1 does not combine with best shots or look-back yet")
-        if detect_every > 1 and getattr(self, "_tracker", None) is not None and not self._tracker.follow_on:
+        if detect_every > 1 and best is not None:
+            raise ValueError("detect_every > 1 does not combine with best shots yet")
+        trk = getattr(self, "_tracker", None)
+        if detect_every > 1 and lookback and trk is not None and not trk.lookback_follow_on:
+            raise ValueError("detect_every > 1 with lookback needs a following look-back tracker: this detector's tracker was created "
+                             "without one (the first call decides the tracker)")
+        if detect_every > 1 and not lookback and trk is not None and not trk.follow_on:
             raise ValueError("detect_every > 1 needs a follow tracker: this detector's tracker was created without one")
 
     def trackFrames(self, frames: Sequence, videos: Sequence[int], threshold: float = 0.5, layout: str = "nv12", matrix: str = "bt601",
@@ -241,7 +245,11 @@ class RetinaFace:
         the others (rf_track_follow_redact_device), redacting every followed face and every LOST track, as ``trackFrames`` splits.
         f17: ``lookback_search`` (True or ``Tracker.set_lookback_search`` keywords, with ``lookback``) follows every new face back
         through the buffered frames by template search and covers its path as well; the first call decides, and asking for it on a
-        tracker created without it raises ValueError."""
+        tracker created without it raises ValueError.
+        f18: ``lookback=L`` with ``detect_every=k`` > 1 makes a following look-back tracker: the frames are split as f16 splits them,
+        key frames go through the look-back call and the others through rf_track_follow_redact_lookback_device, and every frame is
+        emitted L frames late; with L >= k - 1 a face first detected on a key frame is also covered on the follow frames before it.
+        Returns every frame's emitted number in input order.  The first call decides the tracker."""
         kw = dict(layout=layout, matrix=matrix, blocks=blocks, margin=margin, style=style, shape=shape, detail=detail)
         if lookback_search and not lookback:
             raise ValueError("lookback_search needs lookback: the search runs through the look-back buffer")
@@ -253,11 +261,24 @@ class RetinaFace:
                 raise ValueError("detect_every needs videos: the frame numbers belong to a video")
             self.engine.detect_yuv_redact_device(list(frames), threshold, self.nms_threshold, **kw)
             return
+        interval = detect_every > 1
         if getattr(self, "_tracker", None) is None:
-            self._tracker = self.engine.tracker(max_videos=max_videos, motion=motion, lookback=lookback or None, follow=detect_every > 1,
-                                                lookback_search=lookback_search or None)
+            self._tracker = self.engine.tracker(max_videos=max_videos, motion=motion, lookback=lookback or None,
+                                                follow=interval and not lookback, lookback_search=lookback_search or None,
+                                                lookback_follow=(interval and lookback) or None)
         elif lookback_search and not self._tracker.lookback_search_on:
             raise ValueError("lookback_search: this detector's tracker was created without the look-back search (the first call decides)")
+        if lookback and self._tracker.lookback_follow_on:
+            outs, fkw = list(frames if out is None else out), {k: v for k, v in kw.items() if k != "matrix"}
+            nums = np.full(len(frames), -1, np.int32)
+            for det, idx in self._interval_calls(videos, detect_every):
+                fr, vi, oo = [frames[i] for i in idx], [videos[i] for i in idx], [outs[i] for i in idx]
+                if det:
+                    got = self._tracker.detect_yuv_redact_lookback_device(fr, vi, oo, threshold, self.nms_threshold, **kw)[0]
+                else:
+                    got = self._tracker.follow_redact_lookback_device(fr, vi, oo, **fkw)[0]
+                nums[idx] = got
+            return nums
         if lookback:
             return self._tracker.detect_yuv_redact_lookback_device(list(frames), list(videos), list(frames if out is None else out), threshold,
                                                                    self.nms_threshold, **kw)[0]
@@ -278,7 +299,9 @@ class RetinaFace:
         into ``out[0..)``; then the video restarts.  Returns their frame numbers."""
         if getattr(self, "_tracker", None) is None or not self._tracker.lookback:
             raise ValueError("drainVideo needs a look-back tracker: call redactFrames(..., lookback=L) first")
-        return self._tracker.drain(video, list(out), layout=layout, blocks=blocks, margin=margin, style=style, shape=shape, detail=detail)
+        nums = self._tracker.drain(video, list(out), layout=layout, blocks=blocks, margin=margin, style=style, shape=shape, detail=detail)
+        getattr(self, "_frame_no", {}).pop(video, None)      # the drain restarts the video's numbering: key frames stay aligned
+        return nums
 
     def _best_crops(self, n: int):
         b = self._tracker.best

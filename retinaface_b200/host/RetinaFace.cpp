@@ -326,7 +326,7 @@ rf_tracker RetinaFace::makeTracker(int lookback, bool lookback_search) {
     tc.max_videos = opt_.track_videos;
     int rc = rf_tracker_create(h_, &tc, &tracker_);
     if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_create: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
-    trackerCreated();
+    trackerCreated(!lookback);
     if (lookback) {
         const rf_lookback_config lc{lookback, 0.f};
         rc = rf_tracker_set_lookback(tracker_, &lc);
@@ -336,6 +336,12 @@ rf_tracker RetinaFace::makeTracker(int lookback, bool lookback_search) {
             rc = rf_tracker_set_lookback_search(tracker_, &fc);
             if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_set_lookback_search: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
             tracker_search_ = true;
+        }
+        if (opt_.detect_every > 1) {      // f18: a following look-back tracker takes the follow frames
+            const rf_follow_config fc{0, 0.f};
+            rc = rf_tracker_set_lookback_follow(tracker_, &fc);
+            if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_set_lookback_follow: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+            tracker_lookback_follow_ = true;
         }
     }
     return tracker_;
@@ -358,14 +364,19 @@ vector<std::pair<bool, vector<int>>> RetinaFace::intervalCalls(const vector<int>
     return out;
 }
 
-void RetinaFace::followCall(const vector<rf_yuv_frame> &frames, const vector<int> &videos, const rf_redact_style *style) {
+void RetinaFace::followCall(const vector<rf_yuv_frame> &frames, const vector<int> &videos, const rf_redact_style *style,
+                            const vector<rf_yuv_frame> *out_frames, int32_t *frame_numbers) {
     const int n = (int)frames.size();
     DeviceTracks t{};
-    int rc = style ? rf_track_follow_redact_device(tracker_, frames.data(), videos.data(), n, style, &t.tracks, &t.counts)
-                   : rf_track_follow_device(tracker_, frames.data(), videos.data(), n, &t.tracks, &t.counts);
+    int rc = out_frames ? rf_track_follow_redact_lookback_device(tracker_, frames.data(), videos.data(), n, style, out_frames->data(), frame_numbers,
+                                                                 &t.tracks, &t.counts)
+             : style    ? rf_track_follow_redact_device(tracker_, frames.data(), videos.data(), n, style, &t.tracks, &t.counts)
+                        : rf_track_follow_device(tracker_, frames.data(), videos.data(), n, &t.tracks, &t.counts);
     if (rc != RF_OK)
-        throw std::runtime_error(string(style ? "rf_track_follow_redact_device: " : "rf_track_follow_device: ") + rf_status_string(rc) + ": " +
-                                 rf_last_error(h_));
+        throw std::runtime_error(string(out_frames ? "rf_track_follow_redact_lookback_device: "
+                                        : style    ? "rf_track_follow_redact_device: "
+                                                   : "rf_track_follow_device: ") +
+                                 rf_status_string(rc) + ": " + rf_last_error(h_));
     tracks_ = t;
     tracks_.n = n;
     tracks_.max_tracks = 64;      // rf_track_config's default
@@ -377,8 +388,8 @@ void RetinaFace::followCall(const vector<rf_yuv_frame> &frames, const vector<int
     noteMotion(n);
 }
 
-void RetinaFace::trackerCreated() {
-    if (opt_.detect_every > 1) {
+void RetinaFace::trackerCreated(bool follow) {
+    if (follow && opt_.detect_every > 1) {
         const rf_follow_config fc{};
         int rc = rf_tracker_set_follow(tracker_, &fc);
         if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_set_follow: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
@@ -405,18 +416,27 @@ void RetinaFace::redactYUV(const vector<rf_yuv_frame> &device_frames, const vect
         throw std::invalid_argument("redactYUV: out_frames go with lookback, one per frame");
     if (device_frames.size() > (size_t)opt_.max_batch) throw std::invalid_argument("redactYUV: at most max_batch frames per call");
     if (videos && best_tracker_) throw std::logic_error("redactYUV: this RetinaFace tracks with best shots (trackYUVBest)");
-    if (opt.lookback && opt_.detect_every > 1) throw std::invalid_argument("redactYUV: lookback does not combine with detect_every yet");
     if (opt.lookback_search && !opt.lookback) throw std::invalid_argument("redactYUV: lookback_search needs lookback");
     if (videos && !tracker_) makeTracker(opt.lookback, opt.lookback_search);
     if (videos && opt.lookback_search && !tracker_search_)
         throw std::logic_error("redactYUV: lookback_search, but this RetinaFace's tracker was created without it (the first call decides)");
+    if (videos && opt.lookback && opt_.detect_every > 1 && !tracker_lookback_follow_)
+        throw std::logic_error("redactYUV: lookback with detect_every, but this RetinaFace's tracker was created without look-back (the first "
+                               "call decides)");
     const rf_redact_style st{opt.style, opt.shape, opt.style == RF_REDACT_BLUR ? 0 : opt.blocks, opt.detail, opt.margin};
+    const vector<rf_yuv_frame> &outs = out_frames ? *out_frames : device_frames;
     if (videos && opt_.detect_every > 1) {
+        if (opt.lookback) frame_numbers_.assign(device_frames.size(), -1);
         for (const auto &call : intervalCalls(*videos)) {
-            vector<rf_yuv_frame> fr;
+            vector<rf_yuv_frame> fr, of;
             vector<int> vi;
-            for (int i : call.second) { fr.push_back(device_frames[i]); vi.push_back((*videos)[i]); }
-            if (call.first) {
+            for (int i : call.second) { fr.push_back(device_frames[i]); vi.push_back((*videos)[i]); of.push_back(outs[i]); }
+            vector<int32_t> nums(fr.size(), -1);
+            if (opt.lookback) {       // f18: key frames through the look-back call, the others through its follow call
+                if (call.first) lookbackCall(fr, vi, threshold, st, of, nums.data());
+                else followCall(fr, vi, &st, &of, nums.data());
+                for (size_t j = 0; j < call.second.size(); j++) frame_numbers_[call.second[j]] = nums[j];
+            } else if (call.first) {
                 DeviceTracks t{};
                 int rc = rf_detect_yuv_redact_device_style(h_, tracker_, fr.data(), vi.data(), (int)fr.size(), RF_YUV_BT601, threshold,
                                                            nms_threshold, &st, &t.tracks, &t.counts, nullptr, nullptr, nullptr);
@@ -436,15 +456,7 @@ void RetinaFace::redactYUV(const vector<rf_yuv_frame> &device_frames, const vect
     DeviceTracks t{};
     if (opt.lookback) {
         frame_numbers_.assign(n, -1);
-        int rc = rf_detect_yuv_redact_lookback_device(h_, tracker_, device_frames.data(), videos->data(), n, RF_YUV_BT601, threshold, nms_threshold,
-                                                      &st, (out_frames ? out_frames : &device_frames)->data(), frame_numbers_.data(), &t.tracks,
-                                                      &t.counts, nullptr, nullptr, nullptr);
-        if (rc != RF_OK)
-            throw std::runtime_error(string("rf_detect_yuv_redact_lookback_device: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
-        tracks_ = t;
-        tracks_.n = n;
-        tracks_.max_tracks = 64;      // rf_track_config's default
-        noteMotion(n);
+        lookbackCall(device_frames, *videos, threshold, st, outs, frame_numbers_.data());
         return;
     }
     int rc = rf_detect_yuv_redact_device_style(h_, videos ? tracker_ : nullptr, device_frames.data(), videos ? videos->data() : nullptr, n,
@@ -457,6 +469,19 @@ void RetinaFace::redactYUV(const vector<rf_yuv_frame> &device_frames, const vect
         tracks_.max_tracks = 64;      // rf_track_config's default
         noteMotion(n);
     }
+}
+
+void RetinaFace::lookbackCall(const vector<rf_yuv_frame> &frames, const vector<int> &videos, float threshold, const rf_redact_style &st,
+                              const vector<rf_yuv_frame> &out_frames, int32_t *frame_numbers) {
+    const int n = (int)frames.size();
+    DeviceTracks t{};
+    int rc = rf_detect_yuv_redact_lookback_device(h_, tracker_, frames.data(), videos.data(), n, RF_YUV_BT601, threshold, nms_threshold, &st,
+                                                  out_frames.data(), frame_numbers, &t.tracks, &t.counts, nullptr, nullptr, nullptr);
+    if (rc != RF_OK) throw std::runtime_error(string("rf_detect_yuv_redact_lookback_device: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+    tracks_ = t;
+    tracks_.n = n;
+    tracks_.max_tracks = 64;      // rf_track_config's default
+    noteMotion(n);
 }
 
 void RetinaFace::trackYUVBest(const vector<rf_yuv_frame> &device_frames, const vector<int> &videos, void *dev_best_crops, float threshold,
@@ -534,6 +559,7 @@ vector<int32_t> RetinaFace::drainVideo(int video, const vector<rf_yuv_frame> &ou
     int n = 0;
     int rc = rf_tracker_drain(tracker_, video, &st, out_frames.data(), (int)out_frames.size(), &n, nums.data());
     if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_drain: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+    frame_no_.erase(video);       // the drain restarts the video: its key frames count from 0 again, as the library's numbers do
     nums.resize(n);
     return nums;
 }

@@ -44,7 +44,10 @@ struct RetinaFaceOptions {
     bool track_motion = false;           // f13: that tracker follows the camera's motion (rf_tracker_set_motion, default config)
     int detect_every = 1;                // f16: > 1 makes that tracker a follow tracker (rf_tracker_set_follow, default config);
                                          // trackYUV / redactYUV then detect a video's frames whose number is divisible by it and
-                                         // follow the faces on the others (rf_track_follow_device / rf_track_follow_redact_device)
+                                         // follow the faces on the others (rf_track_follow_device / rf_track_follow_redact_device).
+                                         // f18: with RedactOptions::lookback on the first tracked call, a following look-back
+                                         // tracker instead (rf_tracker_set_lookback_follow; follow frames through
+                                         // rf_track_follow_redact_lookback_device)
     string cache_file;                   // folded-model cache (the reference's "retina.cache", trtnetbase.cpp:205-243, but with a
                                          // staleness check).  Empty: none
 };
@@ -170,7 +173,9 @@ class RetinaFace {
     // f15: with opt.lookback = L the tracker (created by the first tracked call) keeps each video's last L frames on the GPU, and
     // frame i writes frame num_i - L of its video, also covered where the faces first detected in the next L frames already were,
     // into out_frames[i] (nullptr: device_frames[i] itself); lastFrameNumbers()[i] is num_i - L, or -1 while the video fills.
-    // drainVideo writes the video's remaining buffered frames into out_frames[0..) and restarts it; it returns their numbers.
+    // drainVideo writes the video's remaining buffered frames into out_frames[0..) and restarts it (and its detect_every numbering);
+    // it returns their numbers.  f18: lookback with options detect_every > 1 splits the call as f16 does and emits every frame, key
+    // frame or not, L frames late; with L >= detect_every - 1 a face is also covered on the follow frames before its first detection.
     void redactYUV(const vector<rf_yuv_frame> &device_frames, const vector<int> *videos = nullptr, float threshold = 0.5,
                    const RedactOptions &opt = RedactOptions(), const vector<rf_yuv_frame> *out_frames = nullptr);
     const vector<int32_t> &lastFrameNumbers() const { return frame_numbers_; }
@@ -184,16 +189,21 @@ class RetinaFace {
    private:
     // faces (and, with crops, the u8 crops of the first min(count, per) faces) of images [start, start + n) of the last call
     void keepResults(size_t start, int n, const unsigned char *crops, int per, int cw, int ch);
-    void trackerCreated();              // motion on a new tracker, as the options say
+    void trackerCreated(bool follow = true);   // motion (and, with follow, f16's following) on a new tracker, as the options say
     void noteMotion(int n);             // lastMotion() after a tracked call of n frames
     rf_tracker makeTracker(int lookback, bool lookback_search = false);   // trackYUV's / redactYUV's tracker, as the options say
     // f16: the call's frames as (detect?, frame indices) sub-calls in issue order; advances each video's frame number
     vector<std::pair<bool, vector<int>>> intervalCalls(const vector<int> &videos);
-    void followCall(const vector<rf_yuv_frame> &frames, const vector<int> &videos, const rf_redact_style *style);
+    // out_frames (f18): the following look-back call, its emitted numbers into frame_numbers
+    void followCall(const vector<rf_yuv_frame> &frames, const vector<int> &videos, const rf_redact_style *style,
+                    const vector<rf_yuv_frame> *out_frames = nullptr, int32_t *frame_numbers = nullptr);
+    void lookbackCall(const vector<rf_yuv_frame> &frames, const vector<int> &videos, float threshold, const rf_redact_style &st,
+                      const vector<rf_yuv_frame> &out_frames, int32_t *frame_numbers);
     void trackDetect(const vector<rf_yuv_frame> &frames, const vector<int> &videos, float threshold, const AlignOptions *align, void *dev_crops);
     rf_handle h_ = nullptr;
     rf_tracker tracker_ = nullptr;
     bool tracker_search_ = false;        // f17: tracker_ searches its look-back buffer
+    bool tracker_lookback_follow_ = false;   // f18: tracker_ is a following look-back tracker
     bool best_tracker_ = false;
     DeviceTracks tracks_;
     DeviceBestShots best_;

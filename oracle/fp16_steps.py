@@ -48,7 +48,8 @@ Tile chains (``tile_chain.cuh``: the latency plans and ``RF_TILE_MASK``): the co
 * the predictors (``:505-528``): one N = 32 GEMM with hi + lo FP16 weight pieces issued hi, lo per K step
   (``plan_tile.cu:136-157``), then an FP32 add of the bias: every head value, deltas included, is an interval.
 
-Not restated here: the FP32 engine and FP16 with ``RF_FLAG_NO_TENSORCORE``.
+The FP32 engine and FP16 with ``RF_FLAG_NO_TENSORCORE`` (the SIMT plans, every step exact) are restated in
+``oracle/fp32_steps.py``, from the primitives and head functions of this file.
 """
 from __future__ import annotations
 

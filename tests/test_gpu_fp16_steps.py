@@ -44,6 +44,7 @@ CASES = {
     "896x1280_mb3_dw1d": Case((896, 1280), 3, (3,), flags=RF_FLAG_DW_1D),   # 1-D geometries on large maps
     "288x416_mb3": Case((288, 416), 3, (3,)),                     # partial 2-D tiles (104 wide)
     "96x160_mb3": Case((96, 160), 3, (3,)),                       # every layer 1-D, SSH taps mostly in the padding
+    "32x224_mb4": Case((32, 224), 4, (4,)),                       # 1 x 7 stride-32 map (32 x 32 does not fit the planner)
     "448_mb3_simt_stem": Case((448, 448), 3, (3,), flags=RF_FLAG_SIMT_STEM),
     "deconv_448_mb8": Case((448, 448), 8, (8,), model="mnet-deconv-0517"),
     "latency_448_mb8": Case((448, 448), 8, (8,), streams=1),        # SSH + heads + NMS chains

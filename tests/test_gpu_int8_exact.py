@@ -50,6 +50,7 @@ CASES = {
     "896x1280_mb3_dw1d": Case((896, 1280), 3, (3,), flags=RF_FLAG_DW_1D),   # 1-D row / N-split geometries on large maps
     "288x416_mb3": Case((288, 416), 3, (3,)),                     # partial 2-D tiles (104 wide), 9x13 stride-32 map
     "96x160_mb3": Case((96, 160), 3, (3,), faces=False),          # every layer 1-D, SSH taps mostly in the padding
+    "32_mb4": Case((32, 32), 4, (4,), faces=False),               # smallest network: 1 x 1 stride-32 map
     "320_mb32": Case((320, 320), 32, (3,)),                       # stand-alone merge at a second geometry
     "448_mb3_simt_stem": Case((448, 448), 3, (3,), flags=RF_FLAG_SIMT_STEM),
     "mnet25_448_mb8": Case((448, 448), 8, (8,), model="mnet25", table="absmax"),

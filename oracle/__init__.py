@@ -18,6 +18,8 @@ Pieces (each function cites the reference file:line it restates):
                          reference's calibration-table scales (TensorRT's own INT8 kernels are closed source).
 * ``calibrator_ref.py`` -- numpy restatement of the entropy-calibration threshold search of rf_calibrate_int8.
 * ``inputs.py``       -- the reference's OpenCV letter-box branch + the seeded synthetic inputs of SURVEY 8d.
+* ``letterbox.py``    -- numpy restatement of the letter-box kernels' own definition (both resize branches, the 2x
+                         area rule, orientations), checked against cv2 and held against the kernels.
 * ``postproc.c``      -- plain-C restatement of anchors / decode / clip / NMS
                          (``retinaface/RetinaFace.cpp:9-199,347-492,661-726``).
 * ``postproc.py``     -- ctypes loader for the C restatement and for ``oracle/_ref``.

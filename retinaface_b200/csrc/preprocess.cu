@@ -240,6 +240,7 @@ float letterbox_fill(LbItemT<Src> &it, typename LbItemT<Src>::Source src, int w,
     else letterbox_geometry(w, h, box_w, box_h, &it.dw, &it.dh, &it.scale);
     it.identity = it.scale == 1.0 ? 1 : 0;
     if (it.identity) it.area = 0;
+    else if (!area && it.scale == 2.0) it.area = LB_HALF_AREA;   // cv::resize's own branch at exactly 2x, as tile_fill takes it
     return letterbox_map_back(w, h, box_w, box_h);
 }
 

@@ -44,8 +44,8 @@ float letterbox_map_back(int w, int h, int box_w, int box_h);
 // letter-box, another origin cuts one tile out of a resized pyramid level (tile_fill below).  scale < 1 up-scales.
 constexpr int LB_MAX_IMAGES = 64, LB_MAX_FRAMES = 32;
 // cv::resize(INTER_LINEAR) at exactly 2x down-scaling runs OpenCV's fast INTER_AREA code, whose border rule differs from the
-// bilinear taps on a side of 3 mod 4.  Tile levels of scale 0.5 use it, so that they are the cv::resize the header promises; the
-// letter-box keeps its own bytes.
+// bilinear taps on a side of 3 mod 4.  Every item of OpenCV's definition at scale 2 uses it -- a letter-box or view whose binding
+// side is exactly twice the box, and tile levels of scale 0.5 -- so that each is the cv::resize the header promises.
 constexpr int LB_HALF_AREA = 2;
 // f9 orientations.  An item's `flip` is a set of LB_* bits over the DISPLAYED image (sw x sh, the frame the taps are computed in):
 // displayed pixel (x, y) reads stored pixel (x', y') with x' = FLIP_X ? sw-1-x : x, y' = FLIP_Y ? sh-1-y : y, swapped when
@@ -71,7 +71,7 @@ struct LbItemT {
     Src src; uint8_t *dst;
     int sw, sh, dw, dh;   // sw x sh: the DISPLAYED source size (stored h x w when LB_TRANSPOSE)
     double scale;
-    uint8_t identity, flip, area;   // flip: LB_* bits; area: 0 bilinear, 1 NPP super-sampling, LB_HALF_AREA OpenCV's 2x fast area path (tiles only)
+    uint8_t identity, flip, area;   // flip: LB_* bits; area: 0 bilinear, 1 NPP super-sampling, LB_HALF_AREA OpenCV's 2x fast area path
     int16_t x0, y0;     // 16 bits keep 64 BGR items within 4 KB; origins are below the largest level side (16384)
 };
 using LbItem = LbItemT<BgrRows>;             // u8 BGR rows

@@ -302,37 +302,54 @@ static TrackParams track_params(rf_tracker t) {
     return TrackParams{c.max_tracks, t->h->cfg.max_faces, c.max_lost, c.high_thresh, c.new_thresh, c.iou_high, c.iou_low, c.iou_tentative};
 }
 
-// The update's arguments into `slot`'s lists (and motions) but for the records.
-static TrackArgs track_args(rf_tracker t, const rf_tracker_s::Slot &slot) {
-    TrackArgs ta{};
-    ta.p = track_params(t);
-    ta.videos = t->d_videos;
-    ta.state = t->d_state;
-    ta.pairs = t->d_pairs;
-    ta.order = t->d_order;
-    ta.tracks = slot.tracks;
-    ta.track_counts = slot.counts;
-    ta.motion = t->motion ? slot.motion : nullptr;
-    return ta;
-}
-
-// The detect half of a detect-then-track call: the forward of the n frames, its records and scales also handed to the caller.
-struct Detected {
-    std::vector<float> scales;
-    const rf_det *dets = nullptr;
-    const int32_t *counts = nullptr;
+// A redaction call's resolved style: f12's params are {MOSAIC, RECT, blocks, detail 0}.
+struct RedactSpec {
+    int kind = REDACT_MOSAIC, shape = REDACT_RECT, blocks = 8, detail = 0;
+    double margin = 0.25;
 };
 
-static int detect_for_tracker(rf_handle h, const char *who, const YuvFrames &src, int n, float thr, float nms, Detected &d, const rf_det **dev_dets,
-                              const int32_t **dev_counts, float *out_scales) {
-    d.scales.resize(n);
-    int rc = yuv_device_impl(h, who, src, n, thr, nms, nullptr, nullptr, nullptr, &d.dets, &d.counts, d.scales.data());
-    if (rc) return rc;
-    if (dev_dets) *dev_dets = d.dets;
-    if (dev_counts) *dev_counts = d.counts;
-    if (out_scales) std::copy(d.scales.begin(), d.scales.end(), out_scales);
-    return RF_OK;
-}
+// One tracker frame call: where its frames' records come from, what follows the update and where its outputs go.  Every exported
+// frame call fills one and runs it through frame_call, which checks it (check_call) and issues it (issue_call).  `who` names the call
+// in every message.
+struct FrameCall {
+    enum Source { RECORDS, DETECT, FOLLOW };           // the caller's records (rf_track_update), a forward, or the follow rounds
+    enum Sink { NONE, CROPS, BEST, REDACT, LOOKBACK }; // after the update: nothing, the due faces' crops, best shots, redaction, look-back
+    const char *who;
+    Call call;
+    Source source;
+    Sink sink = NONE;
+    rf_handle h = nullptr;             // DETECT: the caller's handle, which the tracker must belong to
+    rf_tracker t;
+    const rf_yuv_frame *frames = nullptr;
+    const int *videos;
+    int n;
+    // the records the tracks move with, and the sink draws: RECORDS the caller's, DETECT the forward's, FOLLOW the OK-followed faces
+    const rf_det *dets = nullptr;
+    const int32_t *counts = nullptr;
+    const float *scales = nullptr;     // their map-back factors (NULL: 1)
+    int matrix = 0;                    // DETECT
+    float thr = 0.f, nms = 0.f;
+    const rf_align_params *align = nullptr;            // CROPS
+    void *crops = nullptr;                             // CROPS, BEST
+    double *mats = nullptr;
+    const rf_redact_style *style = nullptr;            // REDACT, LOOKBACK
+    const rf_yuv_frame *out_frames = nullptr;          // LOOKBACK
+    int32_t *out_frame_numbers = nullptr;
+    const rf_track **tracks = nullptr;                 // the outputs, each may be NULL
+    const int32_t **track_counts = nullptr;
+    const rf_det **out_dets = nullptr;
+    const int32_t **out_counts = nullptr;
+    float *out_scales = nullptr;
+    const rf_best_shot **best = nullptr;
+    const int32_t **best_counts = nullptr;
+    // set by check_call
+    AlignArgs a{};
+    RedactSpec spec;
+    std::vector<long long> num;                        // LOOKBACK: lb_numbers' frame numbers and videos
+    std::vector<std::array<int, 3>> seen;
+};
+
+static int frame_call(FrameCall &c);
 
 // ---- f13 camera motion (motion.cuh) ---------------------------------------------------------------------------------------------
 // Each video's last frame of a call, whose thumbnail becomes the video's reference once the update has run.
@@ -399,14 +416,6 @@ static MotionArgs motion_args(rf_tracker t, unsigned ring, const rf_det *dets, c
     return a;
 }
 
-// The estimate of the call's n frames into ring slot `ring`'s motions, on s inside the chain, in tables of TRACK_MAX_FRAMES frames.
-static void motion_issue(rf_tracker t, unsigned ring, const rf_yuv_frame *frames, const int *videos, int n, const rf_det *dets,
-                         const int32_t *counts, const float *scales, cudaStream_t s, MotionCommits &commits) {
-    const std::vector<MotionTable> tabs = motion_tables(t, frames, videos, scales, n, TRACK_MAX_FRAMES, commits);
-    CK(launch_motion_estimate(motion_args(t, ring, dets, counts, t->h->cfg.max_faces), tabs.data(), (int)tabs.size(), s));
-    t->motion_slot = (int)ring;
-}
-
 static void motion_commit(rf_tracker t, const MotionCommits &c, cudaStream_t s) {
     MotionArgs a{};
     a.thumbs = t->d_mthumbs;
@@ -442,85 +451,85 @@ static void follow_cut(rf_tracker t, const rf_yuv_frame *frames, const int *vide
     CK(launch_follow_cut(f, tab.data(), n, s));
 }
 
-// Issues the update of n frames on s (the records complete there) into the next ring slot, ordered by the chain.  `a` (crops):
-// the due faces are cut on s into a's crops.  Returns the ring slot; the caller records its `free`.
-static unsigned track_issue(rf_tracker t, const int *videos, int n, const rf_det *dets, const int32_t *counts, const float *scales,
-                            const rf_yuv_frame *frames, cudaStream_t s, const AlignArgs *a = nullptr, const AlignImageT<YuvPlanes> *table = nullptr) {
-    rf_handle h = t->h;
-    const unsigned ring = slot_begin(t, s);
+// The update of a records or detect call into ring slot `ring`'s lists, on s inside the chain: with motion, the estimate of its frames
+// first (in tables of TRACK_MAX_FRAMES frames) and the commit after.  A best-shot call goes in chunks of TRACK_MAX_FRAMES frames, each
+// tracked, then measured, selected, emitted and committed (the per-call tables hold one chunk); launch_track_update makes the same
+// launches on a whole call.  With crops, the due faces go to the slot.
+static void update_issue(rf_tracker t, unsigned ring, const FrameCall &c, cudaStream_t s) {
     rf_tracker_s::Slot &slot = t->slots[ring];
-    t->updated = true;
+    const int T = t->cfg.max_tracks, F = t->h->cfg.max_faces;
     MotionCommits commits;
-    if (t->motion) motion_issue(t, ring, frames, videos, n, dets, counts, scales, s, commits);
-    TrackArgs ta = track_args(t, slot);
-    ta.dets = dets;
-    ta.counts = counts;
-    if (a) {
+    if (t->motion) {
+        const std::vector<MotionTable> tabs = motion_tables(t, c.frames, c.videos, c.scales, c.n, TRACK_MAX_FRAMES, commits);
+        CK(launch_motion_estimate(motion_args(t, ring, c.dets, c.counts, F), tabs.data(), (int)tabs.size(), s));
+        t->motion_slot = (int)ring;
+    }
+    TrackArgs ta{};
+    ta.p = track_params(t);
+    ta.videos = t->d_videos;
+    ta.state = t->d_state;
+    ta.pairs = t->d_pairs;
+    ta.order = t->d_order;
+    ta.tracks = slot.tracks;
+    ta.track_counts = slot.counts;
+    ta.motion = t->motion ? slot.motion : nullptr;
+    if (c.sink == FrameCall::CROPS) {
         ta.due = slot.due;
         ta.due_counts = slot.due_counts;
-        ta.max_align = a->max_align;
+        ta.max_align = c.a.max_align;
     }
-    CK(launch_track_update(ta, videos, scales, n, s));
+    if (c.sink == FrameCall::BEST) {
+        ta.seen = const_cast<TrackSeen *>(t->ba.seen);
+        ta.gone = const_cast<TrackGone *>(t->ba.gone);
+    }
+    const YuvFrames src{c.frames, c.matrix, nullptr, false};
+    const int chunk = c.sink == FrameCall::BEST ? TRACK_MAX_FRAMES : c.n;
+    for (int i0 = 0; i0 < c.n; i0 += chunk) {
+        const int m = std::min(chunk, c.n - i0);
+        TrackArgs k = ta;
+        k.dets = c.dets + (size_t)i0 * F;
+        k.counts = c.counts + i0;
+        k.tracks += (size_t)i0 * T;
+        k.track_counts += i0;
+        if (k.motion) k.motion += i0;
+        CK(launch_track_update(k, c.videos + i0, c.scales ? c.scales + i0 : nullptr, m, s));
+        if (c.sink != FrameCall::BEST) continue;
+        BestTable bt{};
+        bt.n = m;
+        for (int i = 0; i < m; i++) {
+            const int v = c.videos[i0 + i];
+            bt.video[i] = v;
+            bt.img[i] = AlignImageT<YuvPlanes>{src.in_place(i0 + i), src.width(i0 + i), src.height(i0 + i), 1.f, 0};
+            bool known = false;
+            for (int j = 0; j < bt.nvideos; j++) known |= bt.cta_video[j] == v;
+            if (!known) bt.cta_video[bt.nvideos++] = v;
+        }
+        BestArgs b = t->ba;
+        b.out.crops = static_cast<uint8_t *>(c.crops) + (size_t)i0 * T * b.out.crop_bytes;
+        b.out.mats = c.mats ? c.mats + (size_t)i0 * T * 6 : nullptr;
+        b.best = slot.best + (size_t)i0 * T;
+        b.best_counts = slot.best_counts + i0;
+        b.counts = c.counts + i0;
+        CK(launch_best_frames(b, bt, s));
+    }
     if (t->motion) motion_commit(t, commits, s);
-    if (t->kind == FOLLOW || t->lb_follow) follow_cut(t, frames, videos, n, slot, s);     // before a look-back call's swap: it reads the inputs
-    CK(cudaEventRecord(t->chain, s));
-    if (a) {
-        PostBuffers view{};
-        view.out_dets = slot.due;
-        view.out_counts = slot.due_counts;
-        view.max_faces = h->cfg.max_faces;
-        CK(launch_align_faces(*a, table, view, h->num_sms, s));
-    }
-    return ring;
 }
 
 int rf_track_update(rf_tracker t, const int *videos, int n, const rf_det *dev_dets, const int32_t *dev_counts, const float *scales,
                     const rf_track **dev_tracks, const int32_t **dev_track_counts) {
-    static const char *who = "rf_track_update";
-    if (!t) return RF_ERR_INVALID_ARG;
-    rf_handle h = t->h;
-    int rc = check_track_args(t, who, Call::UPDATE, videos, n, scales);
-    if (rc) return rc;
-    if (n > 0 && (!dev_dets || !dev_counts)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL records or counts", who));
-    if (n == 0) return RF_OK;
-    try {
-        CK(cudaSetDevice(h->device));
-        cudaStream_t s = (cudaStream_t)rf_last_stream(h);
-        const rf_tracker_s::Slot &slot = t->slots[track_issue(t, videos, n, dev_dets, dev_counts, scales, nullptr, s)];
-        CK(cudaEventRecord(slot.free, s));
-        if (dev_tracks) *dev_tracks = slot.tracks;
-        if (dev_track_counts) *dev_track_counts = slot.counts;
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    return RF_OK;
+    FrameCall c{.who = "rf_track_update", .call = Call::UPDATE, .source = FrameCall::RECORDS, .t = t, .videos = videos, .n = n,
+                .dets = dev_dets, .counts = dev_counts, .scales = scales, .tracks = dev_tracks, .track_counts = dev_track_counts};
+    return frame_call(c);
 }
 
 int rf_detect_yuv_track_device(rf_handle h, rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, int matrix, float thr, float nms,
                                const rf_align_params *align, void *dev_crops, double *dev_mats, const rf_track **dev_tracks,
                                const int32_t **dev_track_counts, const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales) {
-    static const char *who = "rf_detect_yuv_track_device";
-    if (!h) return RF_ERR_INVALID_ARG;
-    if (!t || t->h != h) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker is NULL or belongs to another handle", who));
-    int rc = check_track_args(t, who, Call::DETECT, videos, n, nullptr);
-    if (rc) return rc;
-    const YuvFrames src{frames, matrix, nullptr, false};
-    if ((rc = src.check(h, who, n))) return rc;
-    AlignArgs a;
-    if (align && (rc = check_align(h, who, align, n, dev_crops, 0, a))) return rc;
-    if (n == 0) return RF_OK;
-    Detected d;
-    if ((rc = detect_for_tracker(h, who, src, n, thr, nms, d, dev_dets, dev_counts, out_scales))) return rc;
-    try {
-        // the due faces are already in frame pixels: scale 1, as the tiled paths crop their merged records
-        std::vector<AlignImageT<YuvPlanes>> table(n);
-        for (int i = 0; i < n; i++) table[i] = AlignImageT<YuvPlanes>{src.in_place(i), src.width(i), src.height(i), 1.f, 0};
-        if (align) { a.n = n; a.crops = dev_crops; a.mats = dev_mats; }
-        cudaStream_t s = h->last_stream;
-        const rf_tracker_s::Slot &slot = t->slots[track_issue(t, videos, n, d.dets, d.counts, d.scales.data(), frames, s, align ? &a : nullptr, table.data())];
-        CK(cudaEventRecord(slot.free, s));
-        if (dev_tracks) *dev_tracks = slot.tracks;
-        if (dev_track_counts) *dev_track_counts = slot.counts;
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    return RF_OK;
+    FrameCall c{.who = "rf_detect_yuv_track_device", .call = Call::DETECT, .source = FrameCall::DETECT,
+                .sink = align ? FrameCall::CROPS : FrameCall::NONE, .h = h, .t = t, .frames = frames, .videos = videos, .n = n,
+                .matrix = matrix, .thr = thr, .nms = nms, .align = align, .crops = dev_crops, .mats = dev_mats, .tracks = dev_tracks,
+                .track_counts = dev_track_counts, .out_dets = dev_dets, .out_counts = dev_counts, .out_scales = out_scales};
+    return frame_call(c);
 }
 
 // ---- f11 best shots (best.cuh) ---------------------------------------------------------------------------------------------------
@@ -589,66 +598,11 @@ int rf_detect_yuv_track_best_device(rf_handle h, rf_tracker t, const rf_yuv_fram
                                     float nms, void *dev_best_crops, double *dev_best_mats, const rf_best_shot **dev_best,
                                     const int32_t **dev_best_counts, const rf_track **dev_tracks, const int32_t **dev_track_counts,
                                     const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales) {
-    static const char *who = "rf_detect_yuv_track_best_device";
-    if (!h) return RF_ERR_INVALID_ARG;
-    if (!t || t->h != h) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker is NULL or belongs to another handle", who));
-    int rc = check_track_args(t, who, Call::BEST, videos, n, nullptr);
-    if (rc) return rc;
-    const YuvFrames src{frames, matrix, nullptr, false};
-    if ((rc = src.check(h, who, n))) return rc;
-    if (n > 0 && !dev_best_crops) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: dev_best_crops is NULL", who));
-    if (n == 0) return RF_OK;
-    Detected d;
-    if ((rc = detect_for_tracker(h, who, src, n, thr, nms, d, dev_dets, dev_counts, out_scales))) return rc;
-    try {
-        cudaStream_t s = h->last_stream;
-        const unsigned ring = slot_begin(t, s);
-        rf_tracker_s::Slot &slot = t->slots[ring];
-        const int T = t->cfg.max_tracks, F = h->cfg.max_faces;
-        t->updated = true;
-        MotionCommits commits;
-        if (t->motion) motion_issue(t, ring, frames, videos, n, d.dets, d.counts, d.scales.data(), s, commits);
-        TrackArgs ta = track_args(t, slot);
-        ta.seen = const_cast<TrackSeen *>(t->ba.seen);
-        ta.gone = const_cast<TrackGone *>(t->ba.gone);
-        // the call in chunks of TRACK_MAX_FRAMES frames, each tracked then measured, selected, emitted and committed: the per-call
-        // tables hold one chunk
-        for (int i0 = 0; i0 < n; i0 += TRACK_MAX_FRAMES) {
-            const int m = std::min(TRACK_MAX_FRAMES, n - i0);
-            TrackArgs c = ta;
-            c.dets = d.dets + (size_t)i0 * F;
-            c.counts = d.counts + i0;
-            c.tracks += (size_t)i0 * T;
-            c.track_counts += i0;
-            if (c.motion) c.motion += i0;
-            CK(launch_track_update(c, videos + i0, d.scales.data() + i0, m, s));
-            BestTable bt{};
-            bt.n = m;
-            for (int i = 0; i < m; i++) {
-                const int v = videos[i0 + i];
-                bt.video[i] = v;
-                bt.img[i] = AlignImageT<YuvPlanes>{src.in_place(i0 + i), src.width(i0 + i), src.height(i0 + i), 1.f, 0};
-                bool known = false;
-                for (int k = 0; k < bt.nvideos; k++) known |= bt.cta_video[k] == v;
-                if (!known) bt.cta_video[bt.nvideos++] = v;
-            }
-            BestArgs b = t->ba;
-            b.out.crops = static_cast<uint8_t *>(dev_best_crops) + (size_t)i0 * T * b.out.crop_bytes;
-            b.out.mats = dev_best_mats ? dev_best_mats + (size_t)i0 * T * 6 : nullptr;
-            b.best = slot.best + (size_t)i0 * T;
-            b.best_counts = slot.best_counts + i0;
-            b.counts = d.counts + i0;
-            CK(launch_best_frames(b, bt, s));
-        }
-        if (t->motion) motion_commit(t, commits, s);
-        CK(cudaEventRecord(t->chain, s));
-        CK(cudaEventRecord(slot.free, s));
-        if (dev_tracks) *dev_tracks = slot.tracks;
-        if (dev_track_counts) *dev_track_counts = slot.counts;
-        if (dev_best) *dev_best = slot.best;
-        if (dev_best_counts) *dev_best_counts = slot.best_counts;
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    return RF_OK;
+    FrameCall c{.who = "rf_detect_yuv_track_best_device", .call = Call::BEST, .source = FrameCall::DETECT, .sink = FrameCall::BEST, .h = h,
+                .t = t, .frames = frames, .videos = videos, .n = n, .matrix = matrix, .thr = thr, .nms = nms, .crops = dev_best_crops,
+                .mats = dev_best_mats, .tracks = dev_tracks, .track_counts = dev_track_counts, .out_dets = dev_dets, .out_counts = dev_counts,
+                .out_scales = out_scales, .best = dev_best, .best_counts = dev_best_counts};
+    return frame_call(c);
 }
 
 int rf_tracker_finish(rf_tracker t, int video, void *dev_best_crops, double *dev_best_mats, const rf_best_shot **dev_best,
@@ -771,22 +725,12 @@ int rf_tracker_set_follow(rf_tracker t, const rf_follow_config *cfg) {
     return RF_OK;
 }
 
-// Everything a follow call (FOLLOW, or f18's LOOKBACK_FOLLOW) refuses in its tracker, videos and frames, checked before anything is
-// launched.
-static int check_follow(rf_tracker t, const char *who, Call call, const rf_yuv_frame *frames, const int *videos, int n) {
-    int rc = check_track_args(t, who, call, videos, n, nullptr);
-    return rc ? rc : check_frames(t->h, who, frames, n, RF_YUV_BT601);
-}
-
-// Issues the follow step of n frames on s into the next ring slot, ordered by the chain.  In rounds -- the r-th frame of every video
-// of the call, then the next -- so that each frame is searched from the state its video's previous frame left; with motion, each
-// round first masks the tracks' faces and estimates its frames' motion (the reference: the video's previous frame of the call, else
-// its stored thumbnail), and each video's last thumbnail of the call becomes its reference afterwards.  Returns the ring slot; the
-// caller records its `free`.
-static unsigned follow_issue(rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, cudaStream_t s) {
-    const unsigned ring = slot_begin(t, s);
+// The follow step of n frames into ring slot `ring`, on s inside the chain.  In rounds -- the r-th frame of every video of the call,
+// then the next -- so that each frame is searched from the state its video's previous frame left; with motion, each round first
+// masks the tracks' faces and estimates its frames' motion (the reference: the video's previous frame of the call, else its stored
+// thumbnail), and each video's last thumbnail of the call becomes its reference afterwards.
+static void follow_rounds(rf_tracker t, unsigned ring, const rf_yuv_frame *frames, const int *videos, int n, cudaStream_t s) {
     rf_tracker_s::Slot &slot = t->slots[ring];
-    t->updated = true;
     FollowArgs f = follow_args(t);
     f.follow = slot.follow;
     f.tracks = slot.tracks;
@@ -835,28 +779,14 @@ static unsigned follow_issue(rf_tracker t, const rf_yuv_frame *frames, const int
         flush();
     }
     if (t->motion) motion_commit(t, commits, s);
-    CK(cudaEventRecord(t->chain, s));
     t->follow_slot = (int)ring;
-    return ring;
 }
 
 int rf_track_follow_device(rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, const rf_track **dev_tracks,
                            const int32_t **dev_track_counts) {
-    static const char *who = "rf_track_follow_device";
-    if (!t) return RF_ERR_INVALID_ARG;
-    rf_handle h = t->h;
-    int rc = check_follow(t, who, Call::FOLLOW, frames, videos, n);
-    if (rc) return rc;
-    if (n == 0) return RF_OK;
-    try {
-        CK(cudaSetDevice(h->device));
-        cudaStream_t s = (cudaStream_t)rf_last_stream(h);
-        const rf_tracker_s::Slot &slot = t->slots[follow_issue(t, frames, videos, n, s)];
-        CK(cudaEventRecord(slot.free, s));
-        if (dev_tracks) *dev_tracks = slot.tracks;
-        if (dev_track_counts) *dev_track_counts = slot.counts;
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    return RF_OK;
+    FrameCall c{.who = "rf_track_follow_device", .call = Call::FOLLOW, .source = FrameCall::FOLLOW, .t = t, .frames = frames, .videos = videos,
+                .n = n, .tracks = dev_tracks, .track_counts = dev_track_counts};
+    return frame_call(c);
 }
 
 int rf_tracker_follow(rf_tracker t, const rf_follow **dev_follow) {
@@ -896,12 +826,6 @@ int rf_tracker_debug_state(rf_tracker t, int video, double *out, int cap) {
 }
 
 // ---- f12 redaction (redact.cuh) -------------------------------------------------------------------------------------------------
-// A call's resolved style: f12's params are {MOSAIC, RECT, blocks, detail 0}.
-struct RedactSpec {
-    int kind = REDACT_MOSAIC, shape = REDACT_RECT, blocks = 8, detail = 0;
-    double margin = 0.25;
-};
-
 static int redact_margin(rf_handle h, const char *who, float margin, double &out) {
     const float m = margin != 0.f ? margin : 0.25f;
     if (!(std::isfinite(m) && m > 0.f && m <= 1.f))
@@ -1102,33 +1026,35 @@ static int redact_bgr_impl(rf_handle h, const char *who, uint8_t *const *dev_bgr
     return RF_OK;
 }
 
-template <typename Resolve>
+// With a tracker, the tracker's frame call; without, the detect and then the redaction of its records, on the forward's context.
 static int detect_yuv_redact_impl(rf_handle h, const char *who, rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, int matrix,
-                                  float thr, float nms, Resolve resolve, const rf_track **dev_tracks, const int32_t **dev_track_counts,
-                                  const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales) {
-    if (!h) return RF_ERR_INVALID_ARG;
-    int rc;
+                                  float thr, float nms, const rf_redact_style *style, const rf_track **dev_tracks,
+                                  const int32_t **dev_track_counts, const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales) {
     if (t) {
-        if (t->h != h) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker belongs to another handle", who));
-        if ((rc = check_track_args(t, who, Call::DETECT, videos, n, nullptr))) return rc;
+        FrameCall c{.who = who, .call = Call::DETECT, .source = FrameCall::DETECT, .sink = FrameCall::REDACT, .h = h, .t = t, .frames = frames,
+                    .videos = videos, .n = n, .matrix = matrix, .thr = thr, .nms = nms, .style = style, .tracks = dev_tracks,
+                    .track_counts = dev_track_counts, .out_dets = dev_dets, .out_counts = dev_counts, .out_scales = out_scales};
+        return frame_call(c);
     }
+    if (!h) return RF_ERR_INVALID_ARG;
     const YuvFrames src{frames, matrix, nullptr, false};
-    if ((rc = src.check(h, who, n))) return rc;
+    int rc = src.check(h, who, n);
+    if (rc) return rc;
     RedactSpec spec;
-    if ((rc = resolve(spec))) return rc;
+    if ((rc = redact_style(h, who, style, spec))) return rc;
     if ((rc = check_disjoint(h, who, yuv_ranges(frames, n)))) return rc;
     if (n == 0) return RF_OK;
-    Detected d;
-    if ((rc = detect_for_tracker(h, who, src, n, thr, nms, d, dev_dets, dev_counts, out_scales))) return rc;
+    std::vector<float> scales(n);
+    const rf_det *dets = nullptr;
+    const int32_t *counts = nullptr;
+    if ((rc = yuv_device_impl(h, who, src, n, thr, nms, nullptr, nullptr, nullptr, &dets, &counts, scales.data()))) return rc;
+    if (dev_dets) *dev_dets = dets;
+    if (dev_counts) *dev_counts = counts;
+    if (out_scales) std::copy(scales.begin(), scales.end(), out_scales);
+    if (dev_tracks) *dev_tracks = nullptr;
+    if (dev_track_counts) *dev_track_counts = nullptr;
     try {
-        Ctx &c = last_ctx(h);          // the forward's context
-        const rf_tracker_s::Slot *slot = t ? &t->slots[track_issue(t, videos, n, d.dets, d.counts, d.scales.data(), frames, c.stream)] : nullptr;
-        const rf_track *tracks = slot ? slot->tracks : nullptr;
-        const int32_t *track_counts = slot ? slot->counts : nullptr;
-        if (dev_tracks) *dev_tracks = tracks;
-        if (dev_track_counts) *dev_track_counts = track_counts;
-        redact_issue(h, c, yuv_redact_table(frames, n, d.scales.data()), d.dets, d.counts, t, tracks, track_counts, spec);
-        if (slot) CK(cudaEventRecord(slot->free, c.stream));
+        redact_issue(h, last_ctx(h), yuv_redact_table(frames, n, scales.data()), dets, counts, nullptr, nullptr, nullptr, spec);
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }
@@ -1167,42 +1093,23 @@ int rf_redact_device_style(rf_handle h, uint8_t *const *dev_bgr, const int *widt
 int rf_detect_yuv_redact_device(rf_handle h, rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, int matrix, float thr, float nms,
                                 const rf_redact_params *params, const rf_track **dev_tracks, const int32_t **dev_track_counts,
                                 const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales) {
-    static const char *who = "rf_detect_yuv_redact_device";
-    return detect_yuv_redact_impl(h, who, t, frames, videos, n, matrix, thr, nms, [&](RedactSpec &r) { return redact_params(h, who, params, r); },
-                                  dev_tracks, dev_track_counts, dev_dets, dev_counts, out_scales);
+    const rf_redact_style f12{REDACT_MOSAIC, REDACT_RECT, params ? params->blocks : 0, 0, params ? params->margin : 0.f};   // as RedactSpec
+    return detect_yuv_redact_impl(h, "rf_detect_yuv_redact_device", t, frames, videos, n, matrix, thr, nms, &f12, dev_tracks, dev_track_counts,
+                                  dev_dets, dev_counts, out_scales);
 }
 
 int rf_detect_yuv_redact_device_style(rf_handle h, rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, int matrix, float thr,
                                       float nms, const rf_redact_style *style, const rf_track **dev_tracks, const int32_t **dev_track_counts,
                                       const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales) {
-    static const char *who = "rf_detect_yuv_redact_device_style";
-    return detect_yuv_redact_impl(h, who, t, frames, videos, n, matrix, thr, nms, [&](RedactSpec &r) { return redact_style(h, who, style, r); },
-                                  dev_tracks, dev_track_counts, dev_dets, dev_counts, out_scales);
+    return detect_yuv_redact_impl(h, "rf_detect_yuv_redact_device_style", t, frames, videos, n, matrix, thr, nms, style, dev_tracks,
+                                  dev_track_counts, dev_dets, dev_counts, out_scales);
 }
 
 int rf_track_follow_redact_device(rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, const rf_redact_style *style,
                                   const rf_track **dev_tracks, const int32_t **dev_track_counts) {
-    static const char *who = "rf_track_follow_redact_device";
-    if (!t) return RF_ERR_INVALID_ARG;
-    rf_handle h = t->h;
-    int rc = check_follow(t, who, Call::FOLLOW, frames, videos, n);
-    if (rc) return rc;
-    RedactSpec spec;
-    if ((rc = redact_style(h, who, style, spec))) return rc;
-    if ((rc = check_disjoint(h, who, yuv_ranges(frames, n)))) return rc;
-    if (n == 0) return RF_OK;
-    try {
-        CK(cudaSetDevice(h->device));
-        Ctx &c = last_ctx(h);
-        const rf_tracker_s::Slot &slot = t->slots[follow_issue(t, frames, videos, n, c.stream)];
-        // (a) the OK-followed faces in id order, (b) the LOST tracks of the lists: f12's geometry, f14's styles and ownership
-        redact_issue(h, c, yuv_redact_table(frames, n, nullptr), slot.fregions, slot.fregion_counts, t, slot.tracks, slot.counts, spec,
-                     t->cfg.max_tracks);
-        CK(cudaEventRecord(slot.free, c.stream));
-        if (dev_tracks) *dev_tracks = slot.tracks;
-        if (dev_track_counts) *dev_track_counts = slot.counts;
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    return RF_OK;
+    FrameCall c{.who = "rf_track_follow_redact_device", .call = Call::FOLLOW, .source = FrameCall::FOLLOW, .sink = FrameCall::REDACT, .t = t,
+                .frames = frames, .videos = videos, .n = n, .style = style, .tracks = dev_tracks, .track_counts = dev_track_counts};
+    return frame_call(c);
 }
 
 // ---- f15 look-back redaction (lookback.cuh) --------------------------------------------------------------------------------------
@@ -1452,36 +1359,34 @@ static int lb_numbers(rf_tracker t, const char *who, const rf_yuv_frame *frames,
     return check_disjoint(h, who, ranges);
 }
 
-// The buffers of the call's videos that have no buffered frames (lb_numbers' `seen`).
-static int lb_alloc_videos(rf_tracker t, const char *who, const rf_yuv_frame *frames, const std::vector<std::array<int, 3>> &seen) {
-    for (const auto &e : seen) {
-        rf_tracker_s::LookbackVideo &lv = t->lbv[e[0]];
-        if (lv.frames > 0) continue;
-        const rf_yuv_frame &f = frames[e[1]];
-        if (!lb_alloc(t, lv, f))
-            return fail(t->h, RF_ERR_CAPACITY, fmt("%s: video %d: no device memory for %d frames of %dx%d", who, e[0], t->lb_frames, f.width, f.height));
-        lv.w = f.width;
-        lv.h = f.height;
-        lv.step = f.uv_step;
-        lv.v_first = f.uv_step == 2 && f.v < f.u;
-    }
-    return RF_OK;
+// The emission of a look-back call or a drain into `slot`, on c's stream inside the chain: the swap `sw`, the regions of the emitted
+// frames `em`, then (a drain: `drained` >= 0) that video's restart, the chain, and the redaction of the emitted frames `outs`.
+static void lb_emit(rf_tracker t, Ctx &c, rf_tracker_s::Slot &slot, const std::vector<LookbackSwapFrame> &sw,
+                    const std::vector<std::array<long long, 3>> &em, const std::vector<rf_yuv_frame> &outs, const RedactSpec &spec,
+                    int drained = -1) {
+    lb_swap(sw, c.stream);
+    lb_boxes(t, slot, em, c.stream);
+    if (drained >= 0) restart(t, drained, 1, c.stream);     // then the video restarts as rf_tracker_reset restarts it
+    CK(cudaEventRecord(t->chain, c.stream));
+    if (!outs.empty())
+        redact_issue(t->h, c, yuv_redact_table(outs.data(), (int)outs.size(), nullptr), slot.lb_boxes, slot.lb_counts, nullptr, nullptr, nullptr,
+                     spec, lb_records(t));
 }
 
-// The look-back half of a call whose tracking was issued on c's stream into ring slot `ring` (it recorded the chain; this follows it
-// on the same stream and records it again, then the slot's `free`).  a: the frames' (a) records, per_frame of them to a frame, and
-// counts; scales: their map-back factors (NULL: 1).  Each frame's log, f17's chains on a detect call (births: a follow frame has
-// none), then the swap -- after every kernel that reads an input frame, since an out frame may be its own input -- the regions and
-// the redaction of the emitted frames.
-static void lb_issue(rf_tracker t, Ctx &c, unsigned ring, const rf_det *dets, const int32_t *counts, int per_frame, const float *scales,
-                     bool births, const rf_yuv_frame *frames, const int *videos, int n, const std::vector<long long> &num,
-                     const rf_yuv_frame *out_frames, const RedactSpec &spec) {
+// The look-back half of call `fc`, whose tracking was issued on c's stream into ring slot `ring` (it recorded the chain; this follows
+// it on the same stream and records it again).  (a): the call's records, per_frame of them to a frame.  Each frame's log, f17's chains
+// on a detect call (a follow frame has no births), then the swap -- after every kernel that reads an input frame, since an out frame
+// may be its own input -- the regions and the redaction of the emitted frames.
+static void lb_issue(rf_tracker t, Ctx &c, unsigned ring, const FrameCall &fc, int per_frame) {
     rf_handle h = t->h;
+    const rf_yuv_frame *frames = fc.frames, *out_frames = fc.out_frames;
+    const int *videos = fc.videos, n = fc.n;
+    const std::vector<long long> &num = fc.num;
     rf_tracker_s::Slot &slot = t->slots[ring];
     const int L = t->lb_frames;
     LookbackArgs a{};
-    a.dets = dets;
-    a.counts = counts;
+    a.dets = fc.dets;
+    a.counts = fc.counts;
     a.tracks = slot.tracks;
     a.track_counts = slot.counts;
     a.motion = t->motion ? slot.motion : nullptr;
@@ -1495,12 +1400,12 @@ static void lb_issue(rf_tracker t, Ctx &c, unsigned ring, const rf_det *dets, co
         lt.i0 = i0;
         lt.per_frame = per_frame;
         for (int i = i0; i < std::min(n, i0 + LOOKBACK_TABLE); i++, lt.n++) {
-            lt.scale[lt.n] = scales ? scales[i] : 1.f;
+            lt.scale[lt.n] = fc.scales ? fc.scales[i] : 1.f;
             lt.slot[lt.n] = lb_log(t, t->lbv[videos[i]]) + (size_t)(num[i] % a.ring) * a.slot_bytes;
         }
         CK(launch_lookback_log(a, lt, c.stream));
     }
-    if (t->lb_search && births) {
+    if (t->lb_search && fc.source == FrameCall::DETECT) {
         a.search = t->lscfg.search;
         a.max_mad = t->lscfg.max_mad;
         a.steps = slot.lb_steps;
@@ -1520,56 +1425,18 @@ static void lb_issue(rf_tracker t, Ctx &c, unsigned ring, const rf_det *dets, co
             outs.push_back(out_frames[i]);
         }
     }
-    lb_swap(sw, c.stream);
-    lb_boxes(t, slot, em, c.stream);
-    CK(cudaEventRecord(t->chain, c.stream));
-    if (!em.empty())
-        redact_issue(h, c, yuv_redact_table(outs.data(), (int)outs.size(), nullptr), slot.lb_boxes, slot.lb_counts, nullptr, nullptr, nullptr,
-                     spec, lb_records(t));
-    CK(cudaEventRecord(slot.free, c.stream));
-}
-
-// After an issued look-back call: each video's count, and each frame's emitted number (-1: none).
-static void lb_commit(rf_tracker t, const int *videos, int n, const std::vector<long long> &num, int32_t *out_frame_numbers) {
-    const int L = t->lb_frames;
-    for (int i = 0; i < n; i++) {
-        t->lbv[videos[i]].frames = std::max(t->lbv[videos[i]].frames, num[i] + 1);
-        out_frame_numbers[i] = num[i] >= L ? (int32_t)(num[i] - L) : -1;
-    }
+    lb_emit(t, c, slot, sw, em, outs, fc.spec);
 }
 
 int rf_detect_yuv_redact_lookback_device(rf_handle h, rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, int matrix, float thr,
                                          float nms, const rf_redact_style *style, const rf_yuv_frame *out_frames, int32_t *out_frame_numbers,
                                          const rf_track **dev_tracks, const int32_t **dev_track_counts, const rf_det **dev_dets,
                                          const int32_t **dev_counts, float *out_scales) {
-    static const char *who = "rf_detect_yuv_redact_lookback_device";
-    if (!h) return RF_ERR_INVALID_ARG;
-    if (!t || t->h != h) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: the tracker is NULL or belongs to another handle", who));
-    int rc = check_track_args(t, who, Call::LOOKBACK, videos, n, nullptr);
-    if (rc) return rc;
-    const YuvFrames src{frames, matrix, nullptr, false};
-    if ((rc = src.check(h, who, n))) return rc;
-    RedactSpec spec;
-    if ((rc = redact_style(h, who, style, spec))) return rc;
-    std::vector<long long> num;
-    std::vector<std::array<int, 3>> seen;
-    if ((rc = lb_numbers(t, who, frames, videos, n, out_frames, out_frame_numbers, num, seen))) return rc;
-    if (n == 0) return RF_OK;
-    try {
-        CK(cudaSetDevice(h->device));
-        if ((rc = lb_alloc_videos(t, who, frames, seen))) return rc;
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    Detected d;
-    if ((rc = detect_for_tracker(h, who, src, n, thr, nms, d, dev_dets, dev_counts, out_scales))) return rc;
-    try {
-        Ctx &c = last_ctx(h);          // the forward's context
-        const unsigned ring = track_issue(t, videos, n, d.dets, d.counts, d.scales.data(), frames, c.stream);
-        if (dev_tracks) *dev_tracks = t->slots[ring].tracks;
-        if (dev_track_counts) *dev_track_counts = t->slots[ring].counts;
-        lb_issue(t, c, ring, d.dets, d.counts, h->cfg.max_faces, d.scales.data(), true, frames, videos, n, num, out_frames, spec);
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    lb_commit(t, videos, n, num, out_frame_numbers);
-    return RF_OK;
+    FrameCall c{.who = "rf_detect_yuv_redact_lookback_device", .call = Call::LOOKBACK, .source = FrameCall::DETECT, .sink = FrameCall::LOOKBACK,
+                .h = h, .t = t, .frames = frames, .videos = videos, .n = n, .matrix = matrix, .thr = thr, .nms = nms, .style = style,
+                .out_frames = out_frames, .out_frame_numbers = out_frame_numbers, .tracks = dev_tracks, .track_counts = dev_track_counts,
+                .out_dets = dev_dets, .out_counts = dev_counts, .out_scales = out_scales};
+    return frame_call(c);
 }
 
 // ---- f18 following look-back ----------------------------------------------------------------------------------------------------
@@ -1589,30 +1456,10 @@ int rf_tracker_set_lookback_follow(rf_tracker t, const rf_follow_config *cfg) {
 int rf_track_follow_redact_lookback_device(rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, const rf_redact_style *style,
                                            const rf_yuv_frame *out_frames, int32_t *out_frame_numbers, const rf_track **dev_tracks,
                                            const int32_t **dev_track_counts) {
-    static const char *who = "rf_track_follow_redact_lookback_device";
-    if (!t) return RF_ERR_INVALID_ARG;
-    rf_handle h = t->h;
-    int rc = check_follow(t, who, Call::LOOKBACK_FOLLOW, frames, videos, n);
-    if (rc) return rc;
-    RedactSpec spec;
-    if ((rc = redact_style(h, who, style, spec))) return rc;
-    std::vector<long long> num;
-    std::vector<std::array<int, 3>> seen;
-    if ((rc = lb_numbers(t, who, frames, videos, n, out_frames, out_frame_numbers, num, seen))) return rc;
-    if (n == 0) return RF_OK;
-    try {
-        CK(cudaSetDevice(h->device));
-        if ((rc = lb_alloc_videos(t, who, frames, seen))) return rc;
-        Ctx &c = last_ctx(h);
-        const unsigned ring = follow_issue(t, frames, videos, n, c.stream);
-        rf_tracker_s::Slot &slot = t->slots[ring];
-        if (dev_tracks) *dev_tracks = slot.tracks;
-        if (dev_track_counts) *dev_track_counts = slot.counts;
-        // (a): the OK-followed faces in id order, max_tracks to a frame, at scale 1 -- what rf_track_follow_redact_device draws
-        lb_issue(t, c, ring, slot.fregions, slot.fregion_counts, t->cfg.max_tracks, nullptr, false, frames, videos, n, num, out_frames, spec);
-    } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    lb_commit(t, videos, n, num, out_frame_numbers);
-    return RF_OK;
+    FrameCall c{.who = "rf_track_follow_redact_lookback_device", .call = Call::LOOKBACK_FOLLOW, .source = FrameCall::FOLLOW,
+                .sink = FrameCall::LOOKBACK, .t = t, .frames = frames, .videos = videos, .n = n, .style = style, .out_frames = out_frames,
+                .out_frame_numbers = out_frame_numbers, .tracks = dev_tracks, .track_counts = dev_track_counts};
+    return frame_call(c);
 }
 
 int rf_tracker_drain(rf_tracker t, int video, const rf_redact_style *style, const rf_yuv_frame *out_frames, int cap, int *n_out,
@@ -1645,16 +1492,128 @@ int rf_tracker_drain(rf_tracker t, int video, const rf_redact_style *style, cons
             sw.push_back(lb_swap_frame(nullptr, out_frames + j, lv.d + (size_t)(e % L) * lv.frame_bytes));
             em.push_back({video, e, frames - 1 - e});
         }
-        lb_swap(sw, c.stream);
-        lb_boxes(t, slot, em, c.stream);
-        restart(t, video, 1, c.stream);     // then the video restarts as rf_tracker_reset restarts it
-        CK(cudaEventRecord(t->chain, c.stream));
-        if (k > 0)
-            redact_issue(h, c, yuv_redact_table(out_frames, k, nullptr), slot.lb_boxes, slot.lb_counts, nullptr, nullptr, nullptr, spec,
-                         lb_records(t));
+        lb_emit(t, c, slot, sw, em, std::vector<rf_yuv_frame>(out_frames, out_frames + k), spec, video);
         CK(cudaEventRecord(slot.free, c.stream));
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     for (int j = 0; j < k; j++) out_frame_numbers[j] = (int32_t)(frames - k + j);
     *n_out = k;
     return RF_OK;
+}
+
+// ---- the frame call path --------------------------------------------------------------------------------------------------------
+// Everything a frame call refuses, in the order it has always refused it, before anything is launched: the handle and the tracker,
+// check_track_args, the source's frames (a detect call's YUV frames, a follow call's planes) or an update's records, then the sink's
+// arguments (align params, best-shot crops, the redaction style) and the frames' disjointness or lb_numbers.
+static int check_call(FrameCall &c) {
+    rf_tracker t = c.t;
+    const char *who = c.who;
+    if (c.source == FrameCall::DETECT) {
+        if (!c.h) return RF_ERR_INVALID_ARG;
+        if (!t || t->h != c.h)
+            return fail(c.h, RF_ERR_INVALID_ARG,
+                        fmt("%s: the tracker %sbelongs to another handle", who, c.sink == FrameCall::REDACT ? "" : "is NULL or "));
+    } else if (!t) {
+        return RF_ERR_INVALID_ARG;
+    }
+    rf_handle h = t->h;
+    const int n = c.n;
+    int rc = check_track_args(t, who, c.call, c.videos, n, c.source == FrameCall::RECORDS ? c.scales : nullptr);
+    if (rc) return rc;
+    if (c.source == FrameCall::RECORDS && n > 0 && (!c.dets || !c.counts))
+        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL records or counts", who));
+    if (c.source == FrameCall::DETECT && (rc = YuvFrames{c.frames, c.matrix, nullptr, false}.check(h, who, n))) return rc;
+    if (c.source == FrameCall::FOLLOW && (rc = check_frames(h, who, c.frames, n, RF_YUV_BT601))) return rc;
+    if (c.sink == FrameCall::CROPS && (rc = check_align(h, who, c.align, n, c.crops, 0, c.a))) return rc;
+    if (c.sink == FrameCall::BEST && n > 0 && !c.crops) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: dev_best_crops is NULL", who));
+    if ((c.sink == FrameCall::REDACT || c.sink == FrameCall::LOOKBACK) && (rc = redact_style(h, who, c.style, c.spec))) return rc;
+    if (c.sink == FrameCall::REDACT && (rc = check_disjoint(h, who, yuv_ranges(c.frames, n)))) return rc;
+    if (c.sink == FrameCall::LOOKBACK && (rc = lb_numbers(t, who, c.frames, c.videos, n, c.out_frames, c.out_frame_numbers, c.num, c.seen)))
+        return rc;
+    return RF_OK;
+}
+
+// Issues a checked frame call of n > 0 frames.  The buffers of the call's look-back videos that have none are allocated before the
+// forward, so that a refusal launches nothing.  Then, on the forward's context (a records or follow call: rf_last_stream's) inside
+// the chain and in the call's ring slot: the update or the follow rounds, the template cut, the chain, the sink -- a look-back call's
+// swap after every kernel that reads an input frame -- and, last, the slot's `free`.
+static int issue_call(FrameCall &c) {
+    rf_tracker t = c.t;
+    rf_handle h = t->h;
+    const int n = c.n;
+    int rc;
+    try {
+        CK(cudaSetDevice(h->device));
+        for (const auto &e : c.seen) {     // LOOKBACK: (video, its first frame of the call, its frames in the call)
+            rf_tracker_s::LookbackVideo &lv = t->lbv[e[0]];
+            if (lv.frames > 0) continue;
+            const rf_yuv_frame &f = c.frames[e[1]];
+            if (!lb_alloc(t, lv, f))
+                return fail(h, RF_ERR_CAPACITY,
+                            fmt("%s: video %d: no device memory for %d frames of %dx%d", c.who, e[0], t->lb_frames, f.width, f.height));
+            lv.w = f.width;
+            lv.h = f.height;
+            lv.step = f.uv_step;
+            lv.v_first = f.uv_step == 2 && f.v < f.u;
+        }
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    const YuvFrames src{c.frames, c.matrix, nullptr, false};
+    std::vector<float> scales(n);
+    if (c.source == FrameCall::DETECT) {
+        if ((rc = yuv_device_impl(h, c.who, src, n, c.thr, c.nms, nullptr, nullptr, nullptr, &c.dets, &c.counts, scales.data()))) return rc;
+        c.scales = scales.data();
+        if (c.out_dets) *c.out_dets = c.dets;
+        if (c.out_counts) *c.out_counts = c.counts;
+        if (c.out_scales) std::copy(scales.begin(), scales.end(), c.out_scales);
+    }
+    try {
+        Ctx &ctx = last_ctx(h);
+        cudaStream_t s = ctx.stream;
+        const unsigned ring = slot_begin(t, s);
+        rf_tracker_s::Slot &slot = t->slots[ring];
+        t->updated = true;
+        if (c.source == FrameCall::FOLLOW) {
+            follow_rounds(t, ring, c.frames, c.videos, n, s);
+            c.dets = slot.fregions;      // in id order, max_tracks to a frame, at scale 1
+            c.counts = slot.fregion_counts;
+        } else {
+            update_issue(t, ring, c, s);
+        }
+        // the template cut reads the input frames: before a look-back call's swap
+        if (c.source == FrameCall::DETECT && (t->kind == FOLLOW || t->lb_follow)) follow_cut(t, c.frames, c.videos, n, slot, s);
+        CK(cudaEventRecord(t->chain, s));
+        const int per_frame = c.source == FrameCall::FOLLOW ? t->cfg.max_tracks : h->cfg.max_faces;
+        if (c.sink == FrameCall::CROPS) {
+            // the due faces are already in frame pixels: scale 1, as the tiled paths crop their merged records
+            std::vector<AlignImageT<YuvPlanes>> table(n);
+            for (int i = 0; i < n; i++) table[i] = AlignImageT<YuvPlanes>{src.in_place(i), src.width(i), src.height(i), 1.f, 0};
+            c.a.n = n;
+            c.a.crops = c.crops;
+            c.a.mats = c.mats;
+            PostBuffers view{};
+            view.out_dets = slot.due;
+            view.out_counts = slot.due_counts;
+            view.max_faces = h->cfg.max_faces;
+            CK(launch_align_faces(c.a, table.data(), view, h->num_sms, s));
+        } else if (c.sink == FrameCall::REDACT) {
+            // (a) the records, (b) the LOST tracks of the lists: f12's geometry, f14's styles and ownership
+            redact_issue(h, ctx, yuv_redact_table(c.frames, n, c.scales), c.dets, c.counts, t, slot.tracks, slot.counts, c.spec, per_frame);
+        } else if (c.sink == FrameCall::LOOKBACK) {
+            lb_issue(t, ctx, ring, c, per_frame);
+        }
+        CK(cudaEventRecord(slot.free, s));
+        if (c.tracks) *c.tracks = slot.tracks;
+        if (c.track_counts) *c.track_counts = slot.counts;
+        if (c.best) *c.best = slot.best;
+        if (c.best_counts) *c.best_counts = slot.best_counts;
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    for (int i = 0; c.sink == FrameCall::LOOKBACK && i < n; i++) {     // each video's count, and each frame's emitted number (-1: none)
+        t->lbv[c.videos[i]].frames = std::max(t->lbv[c.videos[i]].frames, c.num[i] + 1);
+        c.out_frame_numbers[i] = c.num[i] >= t->lb_frames ? (int32_t)(c.num[i] - t->lb_frames) : -1;
+    }
+    return RF_OK;
+}
+
+static int frame_call(FrameCall &c) {
+    int rc = check_call(c);
+    return rc || c.n == 0 ? rc : issue_call(c);
 }

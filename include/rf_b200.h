@@ -1003,6 +1003,26 @@ int rf_track_follow_redact_lookback_device(rf_tracker t, const rf_yuv_frame *fra
                                            const rf_yuv_frame *out_frames, int32_t *out_frame_numbers, const rf_track **dev_tracks,
                                            const int32_t **dev_track_counts);
 
+/* f19 tiled detection in the tracker: on a 448x448 network the letter-box of a 3840x2160 frame hides every face narrower than ~137
+ * pixels (f7), so a tracker fed by it leaks nearly every face of 4K street footage.  A TILING tracker detects through f7 / f8's tiles
+ * instead.  Every call of it that runs the detector -- rf_detect_yuv_track_device, rf_detect_yuv_track_best_device,
+ * rf_detect_yuv_redact_device(_style) and rf_detect_yuv_redact_lookback_device -- detects its frames exactly as
+ *   rf_detect_yuv_tiled_device(h, frames, n, matrix, tiling, thr, nms, NULL, ...)
+ * does: *dev_dets / *dev_counts are those records bit for bit (frame pixels; anchor_index = tile * max_faces + rank), they live in the
+ * tiled ring (the call counts as one tiled device call for its validity rule, each of its chunks as one rf_detect_batch_device call),
+ * and out_scales are all 1.  Everything after detection is what the same call does with those records at scale 1: the update,
+ * motion, templates, crops, best shots, redaction and look-back.  The tracker's work runs on the tiled call's home context
+ * (rf_last_stream()), and the tiled ring slot is released only after the tracker's last read of its records.
+ * Statuses that depend on the frame size are the call's own, after the frame checks and before anything is launched or allocated:
+ * a level side of 0 or above 16384 (RF_ERR_INVALID_ARG) and more than RF_MAX_TILES tiles (RF_ERR_CAPACITY), as rf_tile_layout
+ * reports them.  rf_track_update, the follow calls, drain, finish and reset run no detector and are unchanged. */
+/* Makes t a tiling tracker: an option of every kind (plain, best-shot, follow, look-back, with or without motion, search or
+ * following), set before the first frame call, before or after the other setters.  tiling NULL, or levels NULL / nlevels 0: the
+ * default pyramid; overlap 0: 64; the levels are copied.  A second call or a call after an update: RF_ERR_INVALID_ARG; a handle
+ * created with RF_FLAG_NPP_RESIZE: RF_ERR_UNSUPPORTED; nlevels outside [0, RF_MAX_TILE_LEVELS], a negative, NaN or infinite scale or
+ * an overlap out of range: RF_ERR_INVALID_ARG.  Nothing changes on a refusal. */
+int rf_tracker_set_tiling(rf_tracker t, const rf_tiling *tiling);
+
 /* Introspection. */
 int rf_get_net_size(rf_handle h, int *net_w, int *net_h, int *max_batch, int *max_faces);
 int rf_num_anchors(rf_handle h);            /* per image: 8,232 @448x448, 47,040 @1280x896 */

@@ -375,6 +375,7 @@ _SIGNATURES = {
     "rf_tracker_set_lookback_search": (_I, [_P, C.POINTER(FollowConfig)]), "rf_tracker_lookback_search": (_I, [_P, _PP, _PP]),
     "rf_tracker_set_lookback_follow": (_I, [_P, C.POINTER(FollowConfig)]),
     "rf_track_follow_redact_lookback_device": (_I, [_P, _FRAMES, _P, _I, _STYLE, _FRAMES, _P, _PP, _PP]),
+    "rf_tracker_set_tiling": (_I, [_P, _TILING]),
 }
 EXPORTS = list(_SIGNATURES)     # every symbol include/rf_b200.h declares (checked by tests/test_host_side.py)
 
@@ -1036,7 +1037,7 @@ class Engine:
     # -- f10 face tracking across video frames ---------------------------------------------------------------------------------
     def tracker(self, max_videos: int = 1, max_tracks: int = 0, high_thresh: float = 0.0, new_thresh: float = 0.0, iou_high: float = 0.0,
                 iou_low: float = 0.0, iou_tentative: float = 0.0, max_lost: int = 0, best: Optional[dict] = None,
-                motion=None, lookback=None, follow=None, lookback_search=None, lookback_follow=None) -> "Tracker":
+                motion=None, lookback=None, follow=None, lookback_search=None, lookback_follow=None, tiling=None) -> "Tracker":
         """rf_tracker_create: a tracker of max_videos independent sequences on this engine (0 -> the defaults of rf_track_config).
         best (``best_config`` keywords): a best-shot tracker (rf_tracker_create_best), fed through ``Tracker.detect_yuv_best_device``.
         motion (True or ``motion_config`` keywords): camera-motion compensation (rf_tracker_set_motion) from the frames of the
@@ -1046,7 +1047,8 @@ class Engine:
         ``Tracker.follow_device``.  lookback_search (True or ``set_lookback_search`` keywords, with lookback): a searching look-back
         tracker (rf_tracker_set_lookback_search).  lookback_follow (True or ``set_lookback_follow`` keywords, with lookback): a
         following look-back tracker (rf_tracker_set_lookback_follow), whose frames between detections go through
-        ``Tracker.follow_redact_lookback_device``."""
+        ``Tracker.follow_redact_lookback_device``.  tiling (True or ``set_tiling`` keywords): a tiling tracker
+        (rf_tracker_set_tiling), whose detect calls detect through the tiles of ``detect_yuv_tiled_device``."""
         t = Tracker(self, TrackConfig(max_videos, max_tracks, high_thresh, new_thresh, iou_high, iou_low, iou_tentative, max_lost),
                     best_config(**best) if best is not None else None)
         try:
@@ -1060,6 +1062,8 @@ class Engine:
                 t.set_lookback_search(**(lookback_search if isinstance(lookback_search, dict) else {}))
             if lookback_follow:
                 t.set_lookback_follow(**(lookback_follow if isinstance(lookback_follow, dict) else {}))
+            if tiling:
+                t.set_tiling(**(tiling if isinstance(tiling, dict) else {}))
         except Exception:
             t.close()
             raise
@@ -1163,6 +1167,7 @@ class Tracker:
         self.follow_on = False
         self.lookback_search_on = False
         self.lookback_follow_on = False
+        self.tiling_on = False
         self.max_videos = cfg.max_videos
         self.max_tracks = cfg.max_tracks or 64
 
@@ -1376,6 +1381,14 @@ class Tracker:
         if not p.value:
             raise RuntimeError("no follow call has been made on this tracker")
         return self.engine._fetch(p.value, FOLLOW_DTYPE, n, self.max_tracks)
+
+    def set_tiling(self, levels=None, overlap: int = 0):
+        """rf_tracker_set_tiling, before the first update: every detect call of this tracker detects its frames through the tiles of
+        ``Engine.detect_yuv_tiled_device`` (levels: [(scale, flip), ...], None -> the default pyramid; overlap 0 -> 64).  Its records
+        are then in frame pixels, with scales all 1."""
+        t = tiling(levels, overlap)
+        self.engine._check(self.lib.rf_tracker_set_tiling(self.t, C.byref(t)))
+        self.tiling_on = True
 
     def reset(self, video: int = -1):
         """rf_tracker_reset: restart one video (ids from 1), or all with -1; ordered after every issued update."""

@@ -917,12 +917,18 @@ int rf_tile_layout(int net_w, int net_h, int width, int height, const rf_tiling 
 
 
 extern "C++" {
-// The checks every tiled path shares, after its source check: the resize definition and each image's layout.
-template <typename Source>
-static int tiled_layouts(rf_handle h, const char *who, const Source &src, int n, const rf_tiling *t, std::vector<std::vector<rf_tile>> &layouts) {
+// Whether the handle can tile: levels are cv::resize's, so not with the NPP resize definition.
+int rf_eng::tiling_supported(rf_handle h, const char *who) {
     if (h->cfg.flags & RF_FLAG_NPP_RESIZE)
         return fail(h, RF_ERR_UNSUPPORTED, fmt("%s: tiles are levels of cv::resize; the handle letter-boxes with NPPI_INTER_SUPER, which "
                                                "only down-samples", who));
+    return RF_OK;
+}
+
+// The checks every tiled path shares, after its source check: the resize definition and each image's layout.
+template <typename Source>
+static int tiled_layouts(rf_handle h, const char *who, const Source &src, int n, const rf_tiling *t, std::vector<std::vector<rf_tile>> &layouts) {
+    if (int rc = tiling_supported(h, who)) return rc;
     layouts.resize(n);
     for (int i = 0; i < n; i++) {
         std::string err;
@@ -1064,6 +1070,41 @@ static int detect_tiled_blocking(rf_handle h, const char *who, const Source &sou
 //   2. A slot that must grow is freed only after the host has waited for `free`, and its counts are cleared on home before `start`.
 //   3. Home joins every context it used through their fence events before the NMS.
 //   4. The crops are cut on home after the NMS; then `free` is recorded.
+//   5. A caller that reads the records later on home (a tracker call, f19) gets `free` back and records it again after its last read,
+//      so that a later call on this slot, whose home may be another context, waits for those reads too.
+// tiled_device_issue issues a checked call of n > 0 images (align: a.crops / a.mats set, or NULL; `free` may be NULL).
+template <typename Source>
+static void tiled_device_issue(rf_handle h, const Source &source, int n, const std::vector<std::vector<rf_tile>> &layouts, float thr, float nms,
+                               const AlignArgs *align, const rf_det **dev_dets, const int32_t **dev_counts, cudaEvent_t *free) {
+    CK(cudaSetDevice(h->device));
+    if (h->tiled_slots.empty()) {
+        h->tiled_slots.resize(h->ctx.size());
+        for (auto &s : h->tiled_slots) {
+            CK(cudaEventCreateWithFlags(&s.free, cudaEventDisableTiming));
+            CK(cudaEventCreateWithFlags(&s.start, cudaEventDisableTiming));
+        }
+    }
+    rf_handle_s::TiledSlot &slot = h->tiled_slots[h->next_tiled_slot++ % h->tiled_slots.size()];
+    Ctx &home = h->ctx[h->next_dev_ctx % h->ctx.size()];
+    size_t most = 0;
+    for (const auto &l : layouts) most = std::max(most, l.size());
+    if ((size_t)slot.pb.anchors_per_image < most * h->cfg.max_faces) {
+        CK(cudaEventSynchronize(slot.free));     // the slot's last call has finished with the buffers about to be freed
+        tiled_grow(h, slot.pb, layouts);
+        // alloc_post_buffers clears the counts on the legacy stream, which the contexts' streams do not wait for
+        CK(cudaMemsetAsync(slot.pb.cand_count, 0, sizeof(int) * slot.pb.max_batch, home.stream));
+    }
+    CK(cudaStreamWaitEvent(home.stream, slot.free, 0));
+    std::vector<typename Source::Src> srcs;
+    detect_tiled_impl(h, source, n, layouts, n, true, home, slot.start, slot.pb, thr, nms, srcs);
+    if (align) tiled_crops(h, *align, n, source, srcs, slot.pb, home.stream);
+    CK(cudaEventRecord(slot.free, home.stream));
+    h->last_stream = home.stream;
+    if (dev_dets) *dev_dets = slot.pb.out_dets;
+    if (dev_counts) *dev_counts = slot.pb.out_counts;
+    if (free) *free = slot.free;
+}
+
 template <typename Source>
 static int detect_tiled_device(rf_handle h, const char *who, const Source &source, int n, const rf_tiling *t, float thr, float nms,
                                const rf_align_params *align, void *dev_crops, double *dev_mats, const rf_det **dev_dets, const int32_t **dev_counts) {
@@ -1071,37 +1112,25 @@ static int detect_tiled_device(rf_handle h, const char *who, const Source &sourc
     AlignArgs a;
     int rc = tiled_check(h, who, source, n, t, align != nullptr, align, dev_crops, false, layouts, a);
     if (rc || n == 0) return rc;
+    a.crops = dev_crops;
+    a.mats = dev_mats;
     try {
-        CK(cudaSetDevice(h->device));
-        if (h->tiled_slots.empty()) {
-            h->tiled_slots.resize(h->ctx.size());
-            for (auto &s : h->tiled_slots) {
-                CK(cudaEventCreateWithFlags(&s.free, cudaEventDisableTiming));
-                CK(cudaEventCreateWithFlags(&s.start, cudaEventDisableTiming));
-            }
-        }
-        rf_handle_s::TiledSlot &slot = h->tiled_slots[h->next_tiled_slot++ % h->tiled_slots.size()];
-        Ctx &home = h->ctx[h->next_dev_ctx % h->ctx.size()];
-        size_t most = 0;
-        for (const auto &l : layouts) most = std::max(most, l.size());
-        if ((size_t)slot.pb.anchors_per_image < most * h->cfg.max_faces) {
-            CK(cudaEventSynchronize(slot.free));     // the slot's last call has finished with the buffers about to be freed
-            tiled_grow(h, slot.pb, layouts);
-            // alloc_post_buffers clears the counts on the legacy stream, which the contexts' streams do not wait for
-            CK(cudaMemsetAsync(slot.pb.cand_count, 0, sizeof(int) * slot.pb.max_batch, home.stream));
-        }
-        CK(cudaStreamWaitEvent(home.stream, slot.free, 0));
-        std::vector<typename Source::Src> srcs;
-        detect_tiled_impl(h, source, n, layouts, n, true, home, slot.start, slot.pb, thr, nms, srcs);
-        if (align) {
-            a.crops = dev_crops;
-            a.mats = dev_mats;
-            tiled_crops(h, a, n, source, srcs, slot.pb, home.stream);
-        }
-        CK(cudaEventRecord(slot.free, home.stream));
-        h->last_stream = home.stream;
-        if (dev_dets) *dev_dets = slot.pb.out_dets;
-        if (dev_counts) *dev_counts = slot.pb.out_counts;
+        tiled_device_issue(h, source, n, layouts, thr, nms, align ? &a : nullptr, dev_dets, dev_counts, nullptr);
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
+}
+
+// rf_detect_yuv_tiled_device's check and issue without crops, for the tracker's detect calls (tracker.cu).
+int rf_eng::yuv_tiled_check(rf_handle h, const char *who, const YuvFrames &src, int n, const rf_tiling *t,
+                            std::vector<std::vector<rf_tile>> &layouts) {
+    AlignArgs a;
+    return tiled_check(h, who, src, n, t, false, nullptr, nullptr, false, layouts, a);
+}
+
+int rf_eng::yuv_tiled_issue(rf_handle h, const YuvFrames &src, int n, const std::vector<std::vector<rf_tile>> &layouts, float thr, float nms,
+                            const rf_det **dev_dets, const int32_t **dev_counts, cudaEvent_t *free) {
+    try {
+        tiled_device_issue(h, src, n, layouts, thr, nms, nullptr, dev_dets, dev_counts, free);
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }

@@ -448,5 +448,13 @@ struct YuvFrames {
 
 int yuv_device_impl(rf_handle h, const char *who, const YuvFrames &src, int n, float thr, float nms, const rf_align_params *align,
                     void *dev_crops, double *dev_mats, const rf_det **dev_dets, const int32_t **dev_counts, float *out_scales);
+// rf_detect_yuv_tiled_device without crops, split for the tracker (f19): the check (the frames, then each frame's layout, before
+// anything is launched) and the issue into the tiled ring on its home context (rf_last_stream).  *free is the ring slot's event: a
+// caller that reads the records later on home records it again there after its last read.  tiling_supported: the handle's
+// refusal of any tiling (RF_FLAG_NPP_RESIZE), with the tiled paths' message.
+int yuv_tiled_check(rf_handle h, const char *who, const YuvFrames &src, int n, const rf_tiling *t, std::vector<std::vector<rf_tile>> &layouts);
+int yuv_tiled_issue(rf_handle h, const YuvFrames &src, int n, const std::vector<std::vector<rf_tile>> &layouts, float thr, float nms,
+                    const rf_det **dev_dets, const int32_t **dev_counts, cudaEvent_t *free);
+int tiling_supported(rf_handle h, const char *who);
 
 }  // namespace rf_eng

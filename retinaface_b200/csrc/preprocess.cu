@@ -266,25 +266,50 @@ AxisTiles axis_tiles(int S, int T, int o) {
 
 // saturate_cast<int>(side * s): cv::resize's size of a level (round half to even)
 int level_side(int side, double s) { return (int)std::nearbyint(side * s); }
+
+// The refusals of an rf_tiling that hold whatever the image size, each with its message.
+bool bad_nlevels(int nlevels, std::string &msg) {
+    if (nlevels >= 0 && nlevels <= RF_MAX_TILE_LEVELS) return false;
+    msg = "nlevels " + std::to_string(nlevels) + ", must be in [0, " + std::to_string(RF_MAX_TILE_LEVELS) + "]";
+    return true;
+}
+bool bad_overlap(int net_w, int net_h, const rf_tiling *t, std::string &msg) {
+    const int o_max = std::min(net_w, net_h) / 2;
+    const int o = t && t->overlap ? t->overlap : 64;
+    if (o >= 16 && o <= o_max) return false;
+    char buf[128];
+    snprintf(buf, sizeof buf, "overlap %d, must be 0 (64) or in [16, %d]", t ? t->overlap : 0, o_max);
+    msg = buf;
+    return true;
+}
+bool bad_scale(size_t l, float s, std::string &msg) {
+    if (s >= 0.f && std::isfinite(s)) return false;
+    char buf[128];
+    snprintf(buf, sizeof buf, "level %zu: scale %g, must be finite and >= 0", l, (double)s);
+    msg = buf;
+    return true;
+}
 }  // namespace
+
+int tiling_check(int net_w, int net_h, const rf_tiling *t, std::string *err) {
+    std::string msg;
+    bool bad = bad_nlevels(t ? t->nlevels : 0, msg) || bad_overlap(net_w, net_h, t, msg);
+    for (int l = 0; !bad && t && t->levels && l < t->nlevels; l++) bad = bad_scale(l, t->levels[l].scale, msg);
+    if (bad && err) *err = msg;
+    return bad ? RF_ERR_INVALID_ARG : RF_OK;
+}
 
 int tile_layout(int net_w, int net_h, int w, int h, const rf_tiling *t, std::vector<rf_tile> &out, std::string *err) {
     out.clear();
     auto bad = [&](int status, const std::string &msg) { if (err) *err = msg; out.clear(); return status; };
     char buf[256];
+    std::string msg;
     if (net_w <= 0 || net_h <= 0 || w <= 0 || h <= 0) return bad(RF_ERR_INVALID_ARG, "image and network sizes must be positive");
     const int nlevels = t ? t->nlevels : 0;
-    if (nlevels < 0 || nlevels > RF_MAX_TILE_LEVELS) {
-        snprintf(buf, sizeof buf, "nlevels %d, must be in [0, %d]", nlevels, RF_MAX_TILE_LEVELS);
-        return bad(RF_ERR_INVALID_ARG, buf);
-    }
+    if (bad_nlevels(nlevels, msg)) return bad(RF_ERR_INVALID_ARG, msg);
     if (nlevels > 0 && !t->levels) return bad(RF_ERR_INVALID_ARG, "levels is NULL");
-    const int o_max = std::min(net_w, net_h) / 2;
     const int o = t && t->overlap ? t->overlap : 64;
-    if (o < 16 || o > o_max) {
-        snprintf(buf, sizeof buf, "overlap %d, must be 0 (64) or in [16, %d]", t ? t->overlap : 0, o_max);
-        return bad(RF_ERR_INVALID_ARG, buf);
-    }
+    if (bad_overlap(net_w, net_h, t, msg)) return bad(RF_ERR_INVALID_ARG, msg);
     std::vector<rf_tile_level> levels;
     if (nlevels > 0) {
         levels.assign(t->levels, t->levels + nlevels);
@@ -295,10 +320,7 @@ int tile_layout(int net_w, int net_h, int w, int h, const rf_tiling *t, std::vec
     }
     for (size_t l = 0; l < levels.size(); l++) {
         const float s = levels[l].scale;
-        if (!(s >= 0.f) || !std::isfinite(s)) {
-            snprintf(buf, sizeof buf, "level %zu: scale %g, must be finite and >= 0", l, (double)s);
-            return bad(RF_ERR_INVALID_ARG, buf);
-        }
+        if (bad_scale(l, s, msg)) return bad(RF_ERR_INVALID_ARG, msg);
         int sw, sh;
         float map_back;
         if (s == 0.f) {       // the fitted level: rf_detect_batch's letter-box

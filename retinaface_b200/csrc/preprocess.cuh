@@ -86,6 +86,9 @@ cudaError_t launch_letterbox_batch(const LbItemT<Src> *items, int n, int net_w, 
 // The one statement of the tile geometry: rf_tile_layout, the tiled detect paths and rf_preprocess_tile all call it.  Fills `out`
 // with every tile of a w x h image (t may be NULL) and returns RF_OK, or a status with the reason in *err.
 int tile_layout(int net_w, int net_h, int w, int h, const rf_tiling *t, std::vector<rf_tile> &out, std::string *err);
+// tile_layout's refusals that hold whatever the image size -- nlevels, the overlap, then each given level's scale, with its messages
+// (rf_tracker_set_tiling; levels NULL is not one of them: the tracker takes it as the default pyramid).
+int tiling_check(int net_w, int net_h, const rf_tiling *t, std::string *err);
 // The letter-box item of one tile: the image's level resized, mirrored when the tile's level is, and cut at the tile's origin.
 template <typename Src>
 void tile_fill(LbItemT<Src> &it, typename LbItemT<Src>::Source src, int w, int h, uint8_t *dst, int net_w, int net_h, const rf_tile &tile);

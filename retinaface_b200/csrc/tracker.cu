@@ -93,6 +93,10 @@ struct rf_tracker_s {
     rf_det *d_fmask = nullptr;           // [max_batch][max_tracks] with motion: each follow frame's face mask
     int *d_fmask_counts = nullptr;       // [max_batch]
     int follow_slot = -1;                // the ring slot of the latest follow call
+    // f19 tiling: every detect call detects through rf_detect_yuv_tiled_device's tiles of `tiling` (its levels in tile_levels).
+    bool tiled = false;
+    rf_tiling tiling{};
+    std::vector<rf_tile_level> tile_levels;
 };
 
 template <typename... P>
@@ -223,7 +227,7 @@ int rf_tracker_reset(rf_tracker t, int video) {
 // and LOOKBACK_SEARCH: the queries rf_tracker_motion, rf_tracker_follow and rf_tracker_lookback_search.
 enum class Call {
     UPDATE, DETECT, BEST, FINISH, FOLLOW, LOOKBACK, DRAIN, LOOKBACK_FOLLOW,
-    SET_MOTION, SET_FOLLOW, SET_LOOKBACK, SET_LOOKBACK_SEARCH, SET_LOOKBACK_FOLLOW,      // the setters, in this range
+    SET_MOTION, SET_FOLLOW, SET_LOOKBACK, SET_LOOKBACK_SEARCH, SET_LOOKBACK_FOLLOW, SET_TILING,      // the setters, in this range
     MOTION, FOLLOWS, LOOKBACK_SEARCH
 };
 
@@ -266,10 +270,11 @@ static int admit(rf_tracker t, const char *who, Call call) {
         only(LOOKBACK);
         if (why.empty() && t->lb_follow) why = "look-back following is already on";
         break;
+    case Call::SET_TILING: if (t->tiled) why = "tiling is already on"; break;
     case Call::MOTION: if (!t->motion) why = "motion is off (rf_tracker_set_motion)"; break;
     case Call::LOOKBACK_SEARCH: if (!t->lb_search) why = "not a searching look-back tracker (rf_tracker_set_lookback_search)"; break;
     }
-    if (why.empty() && call >= Call::SET_MOTION && call <= Call::SET_LOOKBACK_FOLLOW && t->updated) why = "the tracker has already been updated";
+    if (why.empty() && call >= Call::SET_MOTION && call <= Call::SET_TILING && t->updated) why = "the tracker has already been updated";
     return why.empty() ? RF_OK : fail(t->h, RF_ERR_INVALID_ARG, fmt("%s: %s", who, why.c_str()));
 }
 
@@ -347,6 +352,9 @@ struct FrameCall {
     RedactSpec spec;
     std::vector<long long> num;                        // LOOKBACK: lb_numbers' frame numbers and videos
     std::vector<std::array<int, 3>> seen;
+    std::vector<std::vector<rf_tile>> layouts;         // DETECT on a tiling tracker: each frame's tiles
+    // set by issue_call: a tiled detect's ring slot event, recorded again once the call has read the records
+    cudaEvent_t tiled_free = nullptr;
 };
 
 static int frame_call(FrameCall &c);
@@ -1500,6 +1508,24 @@ int rf_tracker_drain(rf_tracker t, int video, const rf_redact_style *style, cons
     return RF_OK;
 }
 
+// ---- f19 tiled detection ------------------------------------------------------------------------------------------------------------
+// An option of any kind: each detect call then takes its records from rf_detect_yuv_tiled_device's tiles (issue_call).  The tiling is
+// copied; levels NULL or nlevels 0 is the default pyramid.  What depends on the frame size is refused by the frame calls.
+int rf_tracker_set_tiling(rf_tracker t, const rf_tiling *tiling) {
+    static const char *who = "rf_tracker_set_tiling";
+    if (!t) return RF_ERR_INVALID_ARG;
+    rf_handle h = t->h;
+    int rc = admit(t, who, Call::SET_TILING);
+    if (rc || (rc = tiling_supported(h, who))) return rc;
+    std::string err;
+    if ((rc = tiling_check(h->cfg.net_w, h->cfg.net_h, tiling, &err))) return fail(h, rc, fmt("%s: %s", who, err.c_str()));
+    const bool dflt = !tiling || !tiling->levels || tiling->nlevels == 0;
+    t->tile_levels.assign(dflt ? nullptr : tiling->levels, dflt ? nullptr : tiling->levels + tiling->nlevels);
+    t->tiling = rf_tiling{t->tile_levels.empty() ? nullptr : t->tile_levels.data(), (int)t->tile_levels.size(), tiling ? tiling->overlap : 0};
+    t->tiled = true;
+    return RF_OK;
+}
+
 // ---- the frame call path --------------------------------------------------------------------------------------------------------
 // Everything a frame call refuses, in the order it has always refused it, before anything is launched: the handle and the tracker,
 // check_track_args, the source's frames (a detect call's YUV frames, a follow call's planes) or an update's records, then the sink's
@@ -1521,7 +1547,10 @@ static int check_call(FrameCall &c) {
     if (rc) return rc;
     if (c.source == FrameCall::RECORDS && n > 0 && (!c.dets || !c.counts))
         return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL records or counts", who));
-    if (c.source == FrameCall::DETECT && (rc = YuvFrames{c.frames, c.matrix, nullptr, false}.check(h, who, n))) return rc;
+    if (c.source == FrameCall::DETECT) {
+        const YuvFrames src{c.frames, c.matrix, nullptr, false};
+        if ((rc = t->tiled ? yuv_tiled_check(h, who, src, n, &t->tiling, c.layouts) : src.check(h, who, n))) return rc;
+    }
     if (c.source == FrameCall::FOLLOW && (rc = check_frames(h, who, c.frames, n, RF_YUV_BT601))) return rc;
     if (c.sink == FrameCall::CROPS && (rc = check_align(h, who, c.align, n, c.crops, 0, c.a))) return rc;
     if (c.sink == FrameCall::BEST && n > 0 && !c.crops) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: dev_best_crops is NULL", who));
@@ -1533,9 +1562,10 @@ static int check_call(FrameCall &c) {
 }
 
 // Issues a checked frame call of n > 0 frames.  The buffers of the call's look-back videos that have none are allocated before the
-// forward, so that a refusal launches nothing.  Then, on the forward's context (a records or follow call: rf_last_stream's) inside
-// the chain and in the call's ring slot: the update or the follow rounds, the template cut, the chain, the sink -- a look-back call's
-// swap after every kernel that reads an input frame -- and, last, the slot's `free`.
+// forward, so that a refusal launches nothing.  Then, on the forward's context (a records or follow call: rf_last_stream's; a tiled
+// detect: the tiled call's home) inside the chain and in the call's ring slot: the update or the follow rounds, the template cut, the
+// chain, the sink -- a look-back call's swap after every kernel that reads an input frame -- and, last, the slot's `free` and a tiled
+// detect's ring slot `free`, recorded again after the last read of its records.
 static int issue_call(FrameCall &c) {
     rf_tracker t = c.t;
     rf_handle h = t->h;
@@ -1559,7 +1589,12 @@ static int issue_call(FrameCall &c) {
     const YuvFrames src{c.frames, c.matrix, nullptr, false};
     std::vector<float> scales(n);
     if (c.source == FrameCall::DETECT) {
-        if ((rc = yuv_device_impl(h, c.who, src, n, c.thr, c.nms, nullptr, nullptr, nullptr, &c.dets, &c.counts, scales.data()))) return rc;
+        if (t->tiled) {      // f19: the tiled ring's records, in frame pixels
+            if ((rc = yuv_tiled_issue(h, src, n, c.layouts, c.thr, c.nms, &c.dets, &c.counts, &c.tiled_free))) return rc;
+            std::fill(scales.begin(), scales.end(), 1.f);
+        } else if ((rc = yuv_device_impl(h, c.who, src, n, c.thr, c.nms, nullptr, nullptr, nullptr, &c.dets, &c.counts, scales.data()))) {
+            return rc;
+        }
         c.scales = scales.data();
         if (c.out_dets) *c.out_dets = c.dets;
         if (c.out_counts) *c.out_counts = c.counts;
@@ -1601,6 +1636,7 @@ static int issue_call(FrameCall &c) {
             lb_issue(t, ctx, ring, c, per_frame);
         }
         CK(cudaEventRecord(slot.free, s));
+        if (c.tiled_free) CK(cudaEventRecord(c.tiled_free, s));     // the tiled slot is free once the call has read its records
         if (c.tracks) *c.tracks = slot.tracks;
         if (c.track_counts) *c.track_counts = slot.counts;
         if (c.best) *c.best = slot.best;

@@ -137,7 +137,7 @@ class RetinaFace:
             runs.setdefault((p, not det), []).append(i)
         return [(not follow, idx) for (_, follow), idx in sorted(runs.items())]
 
-    def _interval_tracker(self, detect_every: int, best=None, lookback=0):
+    def _interval_tracker(self, detect_every: int, best=None, lookback=0, tiling=None):
         if int(detect_every) < 1:
             raise ValueError(f"detect_every {detect_every}, must be >= 1")
         if detect_every > 1 and best is not None:
@@ -148,9 +148,11 @@ class RetinaFace:
                              "without one (the first call decides the tracker)")
         if detect_every > 1 and not lookback and trk is not None and not trk.follow_on:
             raise ValueError("detect_every > 1 needs a follow tracker: this detector's tracker was created without one")
+        if tiling and trk is not None and not trk.tiling_on:
+            raise ValueError("tiling: this detector's tracker was created without tiling (the first call decides)")
 
     def trackFrames(self, frames: Sequence, videos: Sequence[int], threshold: float = 0.5, layout: str = "nv12", matrix: str = "bt601",
-                    align: dict = None, max_videos: int = 64, best: dict = None, motion=False, detect_every: int = 1):
+                    align: dict = None, max_videos: int = 64, best: dict = None, motion=False, detect_every: int = 1, tiling=None):
         """f10 tracking: device 4:2:0 frames (torch CUDA tensors in ``Engine.detect_yuv_device``'s forms), frame i of video
         ``videos[i]``, detected and associated with the tracks of earlier frames on the GPU (rf_detect_yuv_track_device).  Per frame, a
         list of ``(id, state, FaceDetectInfo)`` over every live track (``capi.TRACK_*`` states; the face is the last matched one, in
@@ -171,12 +173,16 @@ class RetinaFace:
 
         f16 detection interval: with ``detect_every=k`` > 1 the tracker is a follow tracker; each video's frames whose number is
         divisible by k are detected, the others followed by template search without the detector (rf_track_follow_device).  A call
-        mixing both kinds is split into detect and follow calls; each video's frames keep their order.  Follow frames have no crops."""
+        mixing both kinds is split into detect and follow calls; each video's frames keep their order.  Follow frames have no crops.
+
+        f19 small faces: with ``tiling`` (True, or ``Tracker.set_tiling``'s keywords: levels, overlap) every detect call of the tracker
+        detects through the tiles of ``detectTiled`` (rf_tracker_set_tiling), so faces far below the letter-box's smallest anchor in
+        4K frames are tracked too.  The first call decides; asking for it on a tracker created without it raises ValueError."""
         if best is not None and align is not None:
             raise ValueError("best shots and new-identity crops are exclusive: pass best or align, not both")
-        self._interval_tracker(detect_every, best=best)
+        self._interval_tracker(detect_every, best=best, tiling=tiling)
         if getattr(self, "_tracker", None) is None:
-            self._tracker = self.engine.tracker(max_videos=max_videos, best=best, motion=motion, follow=detect_every > 1)
+            self._tracker = self.engine.tracker(max_videos=max_videos, best=best, motion=motion, follow=detect_every > 1, tiling=tiling)
         if self._tracker.follow_on:
             tracks, new = [None] * len(frames), [[] for _ in frames]
             for det, idx in self._interval_calls(videos, detect_every):
@@ -229,7 +235,7 @@ class RetinaFace:
     def redactFrames(self, frames: Sequence, videos: Sequence[int] = None, threshold: float = 0.5, blocks: int = 0, margin: float = 0.0,
                      layout: str = "nv12", matrix: str = "bt601", max_videos: int = 64, motion=False, style: str = "mosaic",
                      shape: str = "rect", detail: int = 0, lookback: int = 0, out: Sequence = None, detect_every: int = 1,
-                     lookback_search=False):
+                     lookback_search=False, tiling=None):
         """f12 redaction: detect on device 4:2:0 frames (torch CUDA tensors in ``Engine.detect_yuv_device``'s forms) and mosaic every
         detected face IN PLACE (rf_detect_yuv_redact_device), ``blocks`` cells across a region's longer side (0: 8; 1: a flat patch),
         each side grown by ``margin`` of the box (0: 0.25).  With ``videos`` (frame i of video ``videos[i]``) the frames are also
@@ -249,12 +255,15 @@ class RetinaFace:
         f18: ``lookback=L`` with ``detect_every=k`` > 1 makes a following look-back tracker: the frames are split as f16 splits them,
         key frames go through the look-back call and the others through rf_track_follow_redact_lookback_device, and every frame is
         emitted L frames late; with L >= k - 1 a face first detected on a key frame is also covered on the follow frames before it.
-        Returns every frame's emitted number in input order.  The first call decides the tracker."""
+        Returns every frame's emitted number in input order.  The first call decides the tracker.
+        f19: ``tiling`` (with ``videos``) as ``trackFrames``: every detect call detects through tiles, with any of the above."""
         kw = dict(layout=layout, matrix=matrix, blocks=blocks, margin=margin, style=style, shape=shape, detail=detail)
         if lookback_search and not lookback:
             raise ValueError("lookback_search needs lookback: the search runs through the look-back buffer")
-        self._interval_tracker(detect_every, lookback=lookback)
+        self._interval_tracker(detect_every, lookback=lookback, tiling=tiling)
         if videos is None:
+            if tiling:
+                raise ValueError("tiling needs videos: it is an option of the tracker")
             if lookback:
                 raise ValueError("lookback needs videos: the buffered frames belong to a video")
             if detect_every > 1:
@@ -265,7 +274,7 @@ class RetinaFace:
         if getattr(self, "_tracker", None) is None:
             self._tracker = self.engine.tracker(max_videos=max_videos, motion=motion, lookback=lookback or None,
                                                 follow=interval and not lookback, lookback_search=lookback_search or None,
-                                                lookback_follow=(interval and lookback) or None)
+                                                lookback_follow=(interval and lookback) or None, tiling=tiling)
         elif lookback_search and not self._tracker.lookback_search_on:
             raise ValueError("lookback_search: this detector's tracker was created without the look-back search (the first call decides)")
         if lookback and self._tracker.lookback_follow_on:

@@ -389,6 +389,18 @@ void RetinaFace::followCall(const vector<rf_yuv_frame> &frames, const vector<int
 }
 
 void RetinaFace::trackerCreated(bool follow) {
+    if (opt_.track_tiling) {
+        if (opt_.track_tile_flip && opt_.track_tile_scales.empty())
+            throw std::invalid_argument("track_tile_flip mirrors track_tile_scales; the default pyramid has none");
+        vector<rf_tile_level> levels;
+        for (float s : opt_.track_tile_scales) {
+            levels.push_back(rf_tile_level{s, 0});
+            if (opt_.track_tile_flip) levels.push_back(rf_tile_level{s, 1});
+        }
+        const rf_tiling t{levels.empty() ? nullptr : levels.data(), (int)levels.size(), opt_.track_tile_overlap};
+        int rc = rf_tracker_set_tiling(tracker_, &t);
+        if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_set_tiling: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+    }
     if (follow && opt_.detect_every > 1) {
         const rf_follow_config fc{};
         int rc = rf_tracker_set_follow(tracker_, &fc);

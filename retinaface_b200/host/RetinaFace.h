@@ -48,6 +48,11 @@ struct RetinaFaceOptions {
                                          // f18: with RedactOptions::lookback on the first tracked call, a following look-back
                                          // tracker instead (rf_tracker_set_lookback_follow; follow frames through
                                          // rf_track_follow_redact_lookback_device)
+    bool track_tiling = false;           // f19: every detect call of that tracker (trackYUV, trackYUVBest, redactYUV with or without
+                                         // lookback and detect_every) detects through tiles (rf_tracker_set_tiling), as detectTiled:
+    vector<float> track_tile_scales;     //   the levels (0: the letter-box); empty: the default pyramid
+    bool track_tile_flip = false;        //   each level also mirrored (needs track_tile_scales)
+    int track_tile_overlap = 0;          //   pixels neighbouring tiles share (0: 64)
     string cache_file;                   // folded-model cache (the reference's "retina.cache", trtnetbase.cpp:205-243, but with a
                                          // staleness check).  Empty: none
 };

@@ -682,7 +682,8 @@ int rf_tracker_finish(rf_tracker t, int video, void *dev_best_crops, double *dev
 /* f12 redaction: an in-place mosaic of every detected face -- and of every face the tracker still follows while the detector misses
  * it -- written into the caller's device frames, so that footage can be stored, published or annotated without its faces and no
  * frame leaves the GPU.  The calls WRITE the frames their descriptors point at (rf_yuv_frame's planes are declared const for the
- * detect calls, which only read them).  Records of the oriented entry points are in displayed pixels and do not apply here.
+ * detect calls, which only read them).  Records of the oriented entry points are in displayed pixels: redact with them through
+ * rf_redact_yuv_oriented_device_style (f20).
  *
  * Regions.  Frame i's regions, in this order:
  *   (a) its records j < min(counts[i], max_faces), in rank order; box = each coordinate as __fmul_rn(x, scales[i]) (f5's map-back;
@@ -1022,6 +1023,35 @@ int rf_track_follow_redact_lookback_device(rf_tracker t, const rf_yuv_frame *fra
  * created with RF_FLAG_NPP_RESIZE: RF_ERR_UNSUPPORTED; nlevels outside [0, RF_MAX_TILE_LEVELS], a negative, NaN or infinite scale or
  * an overlap out of range: RF_ERR_INVALID_ARG.  Nothing changes on a refusal. */
 int rf_tracker_set_tiling(rf_tracker t, const rf_tiling *tiling);
+
+/* f20 oriented videos in tracker calls: phones store portrait video as landscape frames with a rotation flag, and the detector only
+ * finds upright faces, so a tracker fed the stored surfaces misses most faces of such a video and a redacting tracker leaves them
+ * uncovered.  A tracker keeps a display orientation o (EXIF 1..8, f9's table) per video, 1 by default.  Any tracker call that reads or
+ * writes the pixels of a frame of video v, on stored frames S, is exactly that call on the displayed frames D = T_o(S), each byte it
+ * writes into D written into S at the stored address of that sample: luma by f9's A_o, chroma by A_o on the halved planes (even
+ * sides: the 2x2 chroma blocks of D are chroma blocks of S).  As in f9 an orientation only moves integer addresses; tap positions,
+ * weights, rounding, cells, blur kernels, ellipses and ownership are those of D.  So records, out_scales, track lists and state,
+ * crops and matrices are bit for bit those of the same call on orient_planes(S, o) at orientation 1, and the written bytes are
+ * that call's, mapped back.  Records, boxes, landmarks and tracks are in DISPLAYED frame pixels; crops come out upright.  Frame
+ * descriptors, their size and layout checks, and pitch padding (never written) stay in stored geometry.  A call whose frames are
+ * all at orientation 1 issues the kernels it issued before f20.  rf_track_update has no pixels and is unchanged: fed the records of
+ * rf_detect_yuv_oriented_device it already tracks in displayed pixels.
+ * Sets the orientation of `video`, or of every video when video is -1.  The videos must not have taken a frame call since create,
+ * rf_tracker_reset, rf_tracker_drain or rf_tracker_finish (which keep the orientation: it belongs to the source, not to the run).
+ * Every tracker kind and option takes it: plain, best-shot, follow and look-back, with motion, search or following.  A bad video, an
+ * orientation outside 1..8, or a video already under way: RF_ERR_INVALID_ARG.  An orientation other than 1 on a tiling tracker, or
+ * rf_tracker_set_tiling once some video is not at orientation 1: RF_ERR_UNSUPPORTED (tiled detection has no oriented path).
+ * Nothing changes on a refusal.  Sizes that describe geometry -- motion thumbnails and references, follow and search frames,
+ * redaction frames -- are the displayed ones; sizes that describe memory -- the look-back buffer, out frames, disjointness -- the
+ * stored ones. */
+int rf_tracker_set_orientation(rf_tracker t, int video, int orientation);
+/* rf_redact_yuv_device_style over the records of rf_detect_yuv_oriented_device (with its out_scales) and, optionally, the lists of
+ * rf_track_update fed those records: the redaction of T_o(frame) for o = orientations[i], mapped back.  rf_redact_yuv_device_style's
+ * statuses, with f9's orientation check after the frame checks, all before anything is launched.  Orientation 1 writes
+ * rf_redact_yuv_device_style's bytes. */
+int rf_redact_yuv_oriented_device_style(rf_handle h, const rf_yuv_frame *frames, const int *orientations, int n, const rf_det *dev_dets,
+                                        const int32_t *dev_counts, const float *scales, rf_tracker t, const rf_track *dev_tracks,
+                                        const int32_t *dev_track_counts, const rf_redact_style *style);
 
 /* Introspection. */
 int rf_get_net_size(rf_handle h, int *net_w, int *net_h, int *max_batch, int *max_faces);

@@ -34,6 +34,7 @@ SOURCES = [
     ("lookback.cu", ["-fmad=false"]),   # the FP64 look-back box, as oracle/lookback.py states it
     ("lookback_search.cu", ["-fmad=false"]),   # f16's search along a birth's chain, as oracle/lookback_search.py states it
     ("follow.cu", ["-fmad=false"]),     # the FP64 template grids, sub-pixel step and Kalman update, as oracle/follow.py states it
+    ("oriented_search.cu", ["-fmad=false"]),   # f20: the follow and look-back searches on oriented frames, the same FP64 steps
     ("calibrate.cu", []),
     ("model.cpp", []),
     ("frontend.cpp", []),

@@ -376,6 +376,8 @@ _SIGNATURES = {
     "rf_tracker_set_lookback_follow": (_I, [_P, C.POINTER(FollowConfig)]),
     "rf_track_follow_redact_lookback_device": (_I, [_P, _FRAMES, _P, _I, _STYLE, _FRAMES, _P, _PP, _PP]),
     "rf_tracker_set_tiling": (_I, [_P, _TILING]),
+    "rf_tracker_set_orientation": (_I, [_P, _I, _I]),
+    "rf_redact_yuv_oriented_device_style": (_I, [_P, _FRAMES, _PI, _I, _P, _P, _P, _P, _P, _P, _STYLE]),
 }
 EXPORTS = list(_SIGNATURES)     # every symbol include/rf_b200.h declares (checked by tests/test_host_side.py)
 
@@ -1093,6 +1095,23 @@ class Engine:
         self._check(fn(self.h, arr, n, dets_ptr, counts_ptr, _addr(sc), tracker.t if tracker is not None else None, tracks_ptr,
                        track_counts_ptr, C.byref(p)))
 
+    def redact_yuv_oriented_device(self, frames, orientations: Sequence[int], dets_ptr: int, counts_ptr: int, scales=None, layout: str = "nv12",
+                                   tracker: Optional["Tracker"] = None, tracks_ptr: Optional[int] = None, track_counts_ptr: Optional[int] = None,
+                                   blocks: int = 0, margin: float = 0.0, style: str = "mosaic", shape: str = "rect", detail: int = 0):
+        """rf_redact_yuv_oriented_device_style: redact_yuv_device of frames shown in EXIF orientation orientations[i], from the
+        displayed-pixel records of ``detect_yuv_oriented_device`` (scales: its out_scales) and, with a tracker, the LOST tracks of
+        lists fed those records.  The frames are redacted in place as displayed; every other byte stays as it was."""
+        n = len(frames)
+        arr = self._frames(frames, layout, True)
+        o = _orientations(orientations, n)
+        sc = self._scales(scales, n)
+        st = redact_style(style, shape, blocks, detail, margin)
+        if st is None:
+            st = RedactStyle(RF_REDACT_MOSAIC, RF_REDACT_RECT, int(blocks), 0, float(margin))
+        self._check(self.lib.rf_redact_yuv_oriented_device_style(self.h, arr, o, n, dets_ptr, counts_ptr, _addr(sc),
+                                                                 tracker.t if tracker is not None else None, tracks_ptr, track_counts_ptr,
+                                                                 C.byref(st)))
+
     def redact_device(self, images, dets_ptr: int, counts_ptr: int, scales=None, tracker: Optional["Tracker"] = None,
                       tracks_ptr: Optional[int] = None, track_counts_ptr: Optional[int] = None, blocks: int = 0, margin: float = 0.0,
                       style: str = "mosaic", shape: str = "rect", detail: int = 0):
@@ -1389,6 +1408,12 @@ class Tracker:
         t = tiling(levels, overlap)
         self.engine._check(self.lib.rf_tracker_set_tiling(self.t, C.byref(t)))
         self.tiling_on = True
+
+    def set_orientation(self, video: int, orientation: int):
+        """rf_tracker_set_orientation: show video (-1: every video) in EXIF orientation 1..8 from its next frame call on, before its
+        first frame call since create, reset, drain or finish.  Every frame call then reads and writes that video's frames as displayed
+        (portrait phone video stored as landscape surfaces), with records and tracks in displayed pixels."""
+        self.engine._check(self.lib.rf_tracker_set_orientation(self.t, int(video), int(orientation)))
 
     def reset(self, video: int = -1):
         """rf_tracker_reset: restart one video (ids from 1), or all with -1; ordered after every issued update."""

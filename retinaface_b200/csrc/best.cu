@@ -36,6 +36,8 @@ __device__ __forceinline__ size_t record_of(const int *s_first, int c, int F) {
 // Grid-stride over (record, band) items; records no track holds are skipped by the whole CTA.  A band's pixels are cut exactly as
 // k_align_faces cuts them (same tables, same sample, same store); its grey values and INSIDE bits, with one halo row above and below,
 // stay in shared memory for the Laplacian.
+// f20: the ORIENTED instantiation samples each frame as displayed (warp.cuh sample<true>; im.w x im.h the displayed size).
+template <bool ORIENTED>
 __global__ void __launch_bounds__(BEST_THREADS) k_best_measure(const BestArgs a, const __grid_constant__ BestTable t) {
     constexpr int R = BEST_BAND + 2;
     __shared__ int s_first[TRACK_MAX_FRAMES + 1];
@@ -90,7 +92,7 @@ __global__ void __launch_bounds__(BEST_THREADS) k_best_measure(const BestArgs a,
             for (int k = 0; k < 4; k++) {
                 const int x = x4 + k;
                 if (x < cw && !zero) {
-                    if (sample<false>(im, (s_x0[r] + s_ax[x]) >> 5, (s_y0[r] + s_bx[x]) >> 5, v[k])) bits |= 1u << k;
+                    if (sample<ORIENTED>(im, (s_x0[r] + s_ax[x]) >> 5, (s_y0[r] + s_bx[x]) >> 5, v[k])) bits |= 1u << k;
                 } else {
                     v[k][0] = v[k][1] = v[k][2] = 0;
                 }
@@ -368,7 +370,10 @@ int select_threads(int T) { return (T + 31) / 32 * 32; }
 cudaError_t launch_best_frames(const BestArgs &a, const BestTable &t, cudaStream_t s) {
     if (t.n <= 0) return cudaSuccess;
     const int T = a.max_tracks;
-    k_best_measure<<<4 * a.num_sms, BEST_THREADS, 0, s>>>(a, t);     // one wave: ~40 faces x 14 bands of a batch-8 call
+    bool oriented = false;
+    for (int i = 0; i < t.n; i++) oriented |= t.img[i].orient != 0;
+    if (oriented) k_best_measure<true><<<4 * a.num_sms, BEST_THREADS, 0, s>>>(a, t);
+    else k_best_measure<false><<<4 * a.num_sms, BEST_THREADS, 0, s>>>(a, t);     // one wave: ~40 faces x 14 bands of a batch-8 call
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     k_best_select<<<t.nvideos, select_threads(T), sizeof(int) * 2 * T, s>>>(a, t);

@@ -21,10 +21,11 @@ struct FollowMeas {
     rf_face face;
 };
 
-// One frame of a launch: its luma plane, video and index in the call (the row of its lists, follow records and measurements).
+// One frame of a launch: its luma plane, video and index in the call (the row of its lists, follow records and measurements).  f20:
+// bits, the video's orientation (LB_* bits; w x h then the displayed size), read by the oriented launches only.
 struct FollowFrame {
     const uint8_t *y;
-    int pitch, w, h, video, frame;
+    int pitch, w, h, video, frame, bits;
 };
 
 struct FollowTable {
@@ -54,10 +55,14 @@ struct FollowArgs {
 };
 
 // The templates of every track matched on the call's detect frames (after launch_track_update), one launch per TRACK_MAX_FRAMES.
-cudaError_t launch_follow_cut(const FollowArgs &a, const FollowFrame *frames, int n, cudaStream_t s);
+// oriented (f20): some frame's bits are not 0, and the luma is read as displayed (a separate instantiation).
+cudaError_t launch_follow_cut(const FollowArgs &a, const FollowFrame *frames, int n, cudaStream_t s, bool oriented = false);
 // One round of a follow call: frames of distinct videos, searched, then stepped.
-cudaError_t launch_follow_round(const FollowArgs &a, const FollowTable &t, cudaStream_t s);
+cudaError_t launch_follow_round(const FollowArgs &a, const FollowTable &t, cudaStream_t s, bool oriented = false);
 // The motion estimate's face mask of a round's frames: every TENTATIVE or CONFIRMED track's face, before the frame.
 cudaError_t launch_follow_mask(const FollowArgs &a, const FollowTable &t, cudaStream_t s);
+// f20 (oriented_search.cu): k_follow_cut and k_follow_search on frames read as displayed, one table each.
+cudaError_t launch_follow_cut_oriented(const FollowArgs &a, const FollowTable &t, cudaStream_t s);
+cudaError_t launch_follow_search_oriented(const FollowArgs &a, const FollowTable &t, cudaStream_t s);
 
 }  // namespace rf

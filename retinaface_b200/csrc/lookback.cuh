@@ -111,7 +111,8 @@ struct LookbackSearchVideo {
     const uint8_t *log;
     size_t frame_bytes;
     long long num0;               // the number of the video's first frame in the table
-    int w, h, first, pad;
+    int w, h, first;
+    int bits;                     // f20: the video's orientation (LB_* bits; w x h the displayed size), read by the oriented launch
 };
 struct LookbackSearchTable {
     int n, nv;
@@ -136,6 +137,8 @@ cudaError_t launch_lookback_log(const LookbackArgs &a, const LookbackLogTable &t
 // max_rows: the most plane rows of a frame of the table (h + h / 2 semi-planar, 2 h planar).
 cudaError_t launch_lookback_swap(const LookbackSwapTable &t, int max_rows, cudaStream_t s);
 cudaError_t launch_lookback_boxes(const LookbackArgs &a, const LookbackBoxTable &t, cudaStream_t s);
-cudaError_t launch_lookback_search(const LookbackArgs &a, const LookbackSearchTable &t, cudaStream_t s);
+// oriented (f20): some video's bits are not 0: the frames' luma is read as displayed (a separate instantiation).
+cudaError_t launch_lookback_search(const LookbackArgs &a, const LookbackSearchTable &t, cudaStream_t s, bool oriented = false);
+cudaError_t launch_lookback_search_oriented(const LookbackArgs &a, const LookbackSearchTable &t, cudaStream_t s);     // oriented_search.cu
 
 }  // namespace rf

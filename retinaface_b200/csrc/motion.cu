@@ -24,15 +24,27 @@ constexpr int COPY_WORDS = WIN * WIN_WORDS + 8;           // the four copies sta
 constexpr int MAX_OFFSETS = (2 * MOTION_MAX_R + 1) * (2 * MOTION_MAX_R + 1);
 static_assert(FIT_THREADS >= MOTION_MAX_BLOCKS, "one thread per block");
 
+// f20: the ORIENTED instantiation sums the displayed D x D box through the frame's signed strides (the sum is order-free).  On a
+// transposed frame the displayed columns are stored rows: there a CTA takes a thumbnail column and its threads the rows, so that a
+// warp's loads stay on consecutive stored bytes, and each thread walks its stored rows innermost.
+template <bool ORIENTED>
 __global__ void __launch_bounds__(MOTION_THUMB) k_motion_thumb(const MotionArgs a, const __grid_constant__ MotionTable t) {
     const MotionFrame &f = t.f[blockIdx.y];
-    const int y = blockIdx.x, x = threadIdx.x;
+    const bool tr = ORIENTED && f.xs != 1 && f.xs != -1;
+    const int y = tr ? threadIdx.x : blockIdx.x, x = tr ? blockIdx.x : threadIdx.x;
     if (y >= f.th || x >= f.tw) return;
     const int D = f.D;
-    const uint8_t *src = f.y + (size_t)D * y * f.pitch + (size_t)D * x;
     unsigned sum = 0;
-    for (int r = 0; r < D; r++, src += f.pitch)
-        for (int c = 0; c < D; c++) sum += src[c];
+    if constexpr (ORIENTED) {
+        const long long inner = tr ? f.pitch : f.xs, outer = tr ? f.xs : f.pitch;
+        const uint8_t *src = f.y + (long long)D * y * f.pitch + (long long)D * x * f.xs;
+        for (int r = 0; r < D; r++, src += outer)
+            for (int c = 0; c < D; c++) sum += src[c * inner];
+    } else {
+        const uint8_t *src = f.y + (size_t)D * y * f.pitch + (size_t)D * x;
+        for (int r = 0; r < D; r++, src += f.pitch)
+            for (int c = 0; c < D; c++) sum += src[c];
+    }
     const unsigned DD = (unsigned)(D * D);
     a.thumbs[(size_t)(t.i0 + blockIdx.y) * MOTION_THUMB_BYTES + y * f.tw + x] = (uint8_t)((sum + DD / 2) / DD);
 }
@@ -321,8 +333,14 @@ cudaError_t launch_motion_estimate(const MotionArgs &a, const MotionTable *table
     for (int k = 0; k < ntables; k++) {
         const MotionTable &t = tables[k];
         int th = 1;
-        for (int i = 0; i < t.n; i++) th = std::max(th, t.f[i].th);
-        k_motion_thumb<<<dim3(th, t.n), MOTION_THUMB, 0, s>>>(a, t);
+        bool oriented = false;
+        for (int i = 0; i < t.n; i++) {
+            const bool tr = t.f[i].xs != 1 && t.f[i].xs != -1;        // f20: a transposed frame's CTAs take thumbnail columns
+            th = std::max(th, tr ? t.f[i].tw : t.f[i].th);
+            oriented |= t.f[i].xs != 1 || t.f[i].pitch < 0;
+        }
+        if (oriented) k_motion_thumb<true><<<dim3(th, t.n), MOTION_THUMB, 0, s>>>(a, t);
+        else k_motion_thumb<false><<<dim3(th, t.n), MOTION_THUMB, 0, s>>>(a, t);
     }
     for (int k = 0; k < ntables; k++) {
         const MotionTable &t = tables[k];

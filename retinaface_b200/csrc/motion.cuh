@@ -18,11 +18,14 @@ constexpr int MOTION_REF_FIRST = -2;      // MotionFrame.ref: no reference
 constexpr int MOTION_REF_STORE = -1;      //                  the video's stored thumbnail
 
 // One frame of a call (host-decided): its luma plane, thumbnail geometry, video and reference.
+// f20: xs != 1 or a negative pitch: the frame is read as displayed, luma sample (x, y) at y[x * xs + y * pitch] (yuv.cuh
+// plane_map applied), and the thumbnail geometry is the displayed frame's.
 struct MotionFrame {
     const uint8_t *y;
     int pitch, video, ref;        // ref: an earlier frame of the call (index), MOTION_REF_STORE or MOTION_REF_FIRST
     int D, tw, th, nbx, nby;
     float scale;                  // the records' map-back factor
+    int xs;                       // 1 on a frame read as stored
 };
 
 // The frames of one launch (up to TRACK_MAX_FRAMES): frame i of the launch is call frame i0 + i.

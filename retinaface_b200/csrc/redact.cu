@@ -17,8 +17,21 @@ struct RedactTable {
     static constexpr int kMax = redact_table_limit<D>();
     RedactFrameT<D> f[kMax];
 };
-static_assert(sizeof(RedactArgs) + sizeof(RedactTable<YuvPlanesW>) + 32 <= 4096 && sizeof(RedactArgs) + sizeof(RedactTable<BgrRowsW>) + 32 <= 4096,
+static_assert(sizeof(RedactArgs) + sizeof(RedactTable<YuvPlanesW>) + 32 <= 4096 && sizeof(RedactArgs) + sizeof(RedactTable<BgrRowsW>) + 32 <= 4096 &&
+              sizeof(RedactArgs) + sizeof(RedactTable<YuvPlanesWO>) + 32 <= 4096,
               "redact launch exceeds the classic 4 KB kernel parameter space");
+
+// f20: the oriented instantiation (YuvPlanesWO) addresses its planes with signed strides; the stored layouts keep size_t offsets.
+template <typename Dst> constexpr bool kOrientedDst = std::is_same<Dst, YuvPlanesWO>::value;
+template <typename Dst> using OffT = typename std::conditional<kOrientedDst<Dst>, long long, size_t>::type;
+// Displayed luma / chroma sample (x, y): its byte offset from the plane pointer.
+__device__ __forceinline__ size_t luma_off(const YuvPlanesW &p, int x, int y) { return (size_t)y * p.y_pitch + x; }
+__device__ __forceinline__ long long luma_off(const YuvPlanesWO &p, int x, int y) { return (long long)y * p.y_ys + (long long)x * p.y_xs; }
+__device__ __forceinline__ size_t chroma_off(const YuvPlanesW &p, int x, int y) { return (size_t)y * p.uv_pitch + (size_t)x * p.uv_step; }
+__device__ __forceinline__ long long chroma_off(const YuvPlanesWO &p, int x, int y) { return (long long)y * p.c_ys + (long long)x * p.c_xs; }
+// Whether displayed rows run down stored columns (a transposed orientation): the apply kernel then walks its bands column by column.
+__device__ __forceinline__ bool transposed(const YuvPlanesW &) { return false; }
+__device__ __forceinline__ bool transposed(const YuvPlanesWO &p) { return p.y_xs != 1 && p.y_xs != -1; }
 
 // Exclusive block scan of v over REDACT_THREADS threads; *total receives the sum.  Every thread of the CTA calls it.
 __device__ int block_scan(int v, int *total, int *s_w) {
@@ -105,7 +118,7 @@ __device__ bool region_geometry(float fx1, float fy1, float fx2, float fy2, doub
 template <typename Table>
 __global__ void __launch_bounds__(REDACT_THREADS) k_redact_regions(const RedactArgs a, const __grid_constant__ Table table) {
     __shared__ int s_w[3][REDACT_THREADS / 32];
-    constexpr bool kYuv = std::is_same<typename Table::Dst, YuvPlanesW>::value;
+    constexpr bool kYuv = kRedactYuv<typename Table::Dst>;
     const int i = blockIdx.x;
     const auto &fr = table.f[i];
     const int na = min(max(a.counts[i], 0), a.max_faces);
@@ -176,17 +189,18 @@ __device__ void locate(const RedactArgs &a, const int *s_first, int item, int Re
 // Sum of the bytes q[y * pitch], y in [y0, y1): REDACT_UNROLL independent loads in flight per step, so that a column costs a few
 // memory round trips rather than one per row.
 constexpr int REDACT_UNROLL = 8;
+template <typename Off>
 __device__ __forceinline__ unsigned column_sum(const uint8_t *q, int pitch, int y0, int y1) {
     unsigned s = 0;
     int y = y0;
     for (; y + REDACT_UNROLL <= y1; y += REDACT_UNROLL) {
         unsigned v[REDACT_UNROLL];
 #pragma unroll
-        for (int k = 0; k < REDACT_UNROLL; k++) v[k] = q[(size_t)(y + k) * pitch];
+        for (int k = 0; k < REDACT_UNROLL; k++) v[k] = q[(Off)(y + k) * pitch];
 #pragma unroll
         for (int k = 0; k < REDACT_UNROLL; k++) s += v[k];
     }
-    for (; y < y1; y++) s += q[(size_t)y * pitch];
+    for (; y < y1; y++) s += q[(Off)y * pitch];
     return s;
 }
 
@@ -197,7 +211,7 @@ __global__ void __launch_bounds__(REDACT_THREADS) k_redact_measure(const RedactA
     using Dst = typename Table::Dst;
     __shared__ int s_first[Table::kMax + 1];
     __shared__ unsigned long long s_sum[3][REDACT_MAX_BLOCKS];
-    constexpr bool kYuv = std::is_same<Dst, YuvPlanesW>::value;
+    constexpr bool kYuv = kRedactYuv<Dst>;
     frame_firsts(a, 1, s_first);
     const int items = s_first[a.n], bb = a.blocks * a.blocks;
     for (int item = blockIdx.x; item < items; item += gridDim.x) {
@@ -210,16 +224,30 @@ __global__ void __launch_bounds__(REDACT_THREADS) k_redact_measure(const RedactA
         __syncthreads();
         const int cx0 = max(g.x0, 0), cx1 = min(g.x1, fr.w);
         const int ry0 = max(g.y0 + cr * c, 0), ry1 = min(min(g.y0 + (cr + 1) * c, g.y1), fr.h);
-        if constexpr (kYuv) {
+        if constexpr (kOrientedDst<Dst>) {
+            // f20: down a displayed column by y_ys / c_ys, across by y_xs / c_xs; the sums and cells are those of the upright frame
+            const YuvPlanesWO &p = fr.dst;
+            for (int x = cx0 + threadIdx.x; x < cx1; x += REDACT_THREADS) {
+                const unsigned s = column_sum<long long>(p.y + (long long)x * p.y_xs, p.y_ys, ry0, ry1);
+                atomicAdd(&s_sum[0][(x - g.x0) / c], (unsigned long long)s);
+            }
+            for (int x = (cx0 >> 1) + threadIdx.x; x < (cx1 >> 1); x += REDACT_THREADS) {
+                const long long o = (long long)x * p.c_xs;
+                const unsigned su = column_sum<long long>(p.u + o, p.c_ys, ry0 >> 1, ry1 >> 1), sv = column_sum<long long>(p.v + o, p.c_ys, ry0 >> 1, ry1 >> 1);
+                const int cell = (2 * x - g.x0) / c;
+                atomicAdd(&s_sum[1][cell], (unsigned long long)su);
+                atomicAdd(&s_sum[2][cell], (unsigned long long)sv);
+            }
+        } else if constexpr (kYuv) {
             const YuvPlanesW &p = fr.dst;
             for (int x = cx0 + threadIdx.x; x < cx1; x += REDACT_THREADS) {
-                const unsigned s = column_sum(p.y + x, p.y_pitch, ry0, ry1);
+                const unsigned s = column_sum<size_t>(p.y + x, p.y_pitch, ry0, ry1);
                 atomicAdd(&s_sum[0][(x - g.x0) / c], (unsigned long long)s);
             }
             // chroma: the rectangle and the row halved (every bound is even), cells of side c / 2 anchored at (x0 / 2, y0 / 2)
             for (int x = (cx0 >> 1) + threadIdx.x; x < (cx1 >> 1); x += REDACT_THREADS) {
                 const size_t o = (size_t)x * p.uv_step;
-                const unsigned su = column_sum(p.u + o, p.uv_pitch, ry0 >> 1, ry1 >> 1), sv = column_sum(p.v + o, p.uv_pitch, ry0 >> 1, ry1 >> 1);
+                const unsigned su = column_sum<size_t>(p.u + o, p.uv_pitch, ry0 >> 1, ry1 >> 1), sv = column_sum<size_t>(p.v + o, p.uv_pitch, ry0 >> 1, ry1 >> 1);
                 const int cell = (2 * x - g.x0) / c;
                 atomicAdd(&s_sum[1][cell], (unsigned long long)su);
                 atomicAdd(&s_sum[2][cell], (unsigned long long)sv);
@@ -228,7 +256,8 @@ __global__ void __launch_bounds__(REDACT_THREADS) k_redact_measure(const RedactA
             const BgrRowsW &p = fr.dst;
             for (int x = cx0 + threadIdx.x; x < cx1; x += REDACT_THREADS) {
                 const uint8_t *q = p.p + 3 * (size_t)x;
-                const unsigned s0 = column_sum(q, p.pitch, ry0, ry1), s1 = column_sum(q + 1, p.pitch, ry0, ry1), s2 = column_sum(q + 2, p.pitch, ry0, ry1);
+                const unsigned s0 = column_sum<size_t>(q, p.pitch, ry0, ry1), s1 = column_sum<size_t>(q + 1, p.pitch, ry0, ry1),
+                               s2 = column_sum<size_t>(q + 2, p.pitch, ry0, ry1);
                 const int cell = (x - g.x0) / c;
                 atomicAdd(&s_sum[0][cell], (unsigned long long)s0);
                 atomicAdd(&s_sum[1][cell], (unsigned long long)s1);
@@ -265,7 +294,7 @@ __global__ void __launch_bounds__(REDACT_THREADS) k_redact_apply(const RedactArg
     __shared__ int4 s_rect[REDACT_COVER];
     __shared__ uint8_t s_cells[kBlur ? 1 : REDACT_MAX_BLOCKS * REDACT_MAX_BLOCKS * 3];
     __shared__ int s_nrect;
-    constexpr bool kYuv = std::is_same<Dst, YuvPlanesW>::value;
+    constexpr bool kYuv = kRedactYuv<Dst>;
     frame_firsts(a, 2, s_first);
     const int items = s_first[a.n], bb = a.blocks * a.blocks;
     for (int item = blockIdx.x; item < items; item += gridDim.x) {
@@ -311,17 +340,19 @@ __global__ void __launch_bounds__(REDACT_THREADS) k_redact_apply(const RedactArg
         const uint8_t *cv = s_cells;
         const int bw = cx1 - cx0, rows = by1 - by0;
         if constexpr (kYuv) {
-            const YuvPlanesW &p = fr.dst;
+            const Dst &p = fr.dst;
+            // f20: down the band's columns when they are stored rows, so that consecutive threads write consecutive bytes
+            const bool down = transposed(p);
             for (int t = threadIdx.x; t < rows * bw; t += REDACT_THREADS) {
-                const int y = by0 + t / bw, x = cx0 + t % bw;
+                const int y = down ? by0 + t % rows : by0 + t / bw, x = down ? cx0 + t / rows : cx0 + t % bw;
                 if (covered(x, y, 0)) continue;
-                p.y[(size_t)y * p.y_pitch + x] = kBlur ? fr.blur[(size_t)y * fr.w + x] : cv[((y - g.y0) / c * nx + (x - g.x0) / c) * 3];
+                p.y[luma_off(p, x, y)] = kBlur ? fr.blur[(size_t)y * fr.w + x] : cv[((y - g.y0) / c * nx + (x - g.x0) / c) * 3];
             }
-            const int hw = bw >> 1;
-            for (int t = threadIdx.x; t < (rows >> 1) * hw; t += REDACT_THREADS) {
-                const int y = (by0 >> 1) + t / hw, x = (cx0 >> 1) + t % hw;
+            const int hw = bw >> 1, hr = rows >> 1;
+            for (int t = threadIdx.x; t < hr * hw; t += REDACT_THREADS) {
+                const int y = (by0 >> 1) + (down ? t % hr : t / hw), x = (cx0 >> 1) + (down ? t / hr : t % hw);
                 if (covered(x, y, 1)) continue;
-                const size_t o = (size_t)y * p.uv_pitch + (size_t)x * p.uv_step;
+                const auto o = chroma_off(p, x, y);
                 if constexpr (kBlur) {
                     const size_t b = (size_t)y * (fr.w / 2) + x;
                     p.u[o] = blur_yuv_plane(fr.blur, fr.w, fr.h, 1)[b];
@@ -361,7 +392,7 @@ __global__ void __launch_bounds__(REDACT_THREADS, 2) k_redact_blur(const RedactA
     __shared__ int s_first[Table::kMax + 1];
     __shared__ int4 s_rect[BLUR_COVER];
     __shared__ int s_nrect;
-    constexpr bool kYuv = std::is_same<Dst, YuvPlanesW>::value;
+    constexpr bool kYuv = kRedactYuv<Dst>;
     frame_firsts(a, 1, s_first);
     const int items = s_first[a.n];
     for (int item = blockIdx.x; item < items; item += gridDim.x) {
@@ -388,10 +419,15 @@ __global__ void __launch_bounds__(REDACT_THREADS, 2) k_redact_blur(const RedactA
         uint8_t *dst;
         int pitch, step, pw, ph, dpitch, dstep;
         if constexpr (kYuv) {
-            const YuvPlanesW &d = fr.dst;
+            const Dst &d = fr.dst;
             src = p == 0 ? d.y : p == 1 ? d.u : d.v;
-            pitch = p ? d.uv_pitch : d.y_pitch;
-            step = p ? d.uv_step : 1;
+            if constexpr (kOrientedDst<Dst>) {
+                pitch = p ? d.c_ys : d.y_ys;
+                step = p ? d.c_xs : d.y_xs;
+            } else {
+                pitch = p ? d.uv_pitch : d.y_pitch;
+                step = p ? d.uv_step : 1;
+            }
             pw = fr.w >> s;
             ph = fr.h >> s;
             dst = blur_yuv_plane(fr.blur, fr.w, fr.h, p);
@@ -426,9 +462,10 @@ __global__ void __launch_bounds__(REDACT_THREADS, 2) k_redact_blur(const RedactA
         // vertical: s_v[y][c] = sum_j k[j] P[clampY(ty0 + y + j)][clampX(tx0 - 3a + c)]
         // BLUR_UNROLL steps' loads are issued before their sums (the row index is clamped, so every load is in the plane)
         for (int c = threadIdx.x; c < cols; c += REDACT_THREADS) {
-            const uint8_t *col = src + (size_t)min(max(tx0 - h3 + c, 0), pw - 1) * step;
+            using Off = OffT<Dst>;
+            const uint8_t *col = src + (Off)min(max(tx0 - h3 + c, 0), pw - 1) * step;
             const int ys = ty0 - h3;
-            auto q = [&](int t) -> unsigned { return t >= 0 ? (unsigned)__ldg(col + (size_t)min(max(ys + t, 0), ph - 1) * pitch) : 0u; };
+            auto q = [&](int t) -> unsigned { return t >= 0 ? (unsigned)__ldg(col + (Off)min(max(ys + t, 0), ph - 1) * pitch) : 0u; };
             unsigned c1 = 0, c2 = 0, c3 = 0;
             for (int t0 = 0; t0 < lv; t0 += BLUR_UNROLL) {
                 unsigned d[BLUR_UNROLL];
@@ -560,5 +597,6 @@ cudaError_t launch_redact(const RedactArgs &a, const RedactFrameT<Dst> *frames, 
 
 template cudaError_t launch_redact<YuvPlanesW>(const RedactArgs &, const RedactFrameT<YuvPlanesW> *, int, cudaStream_t);
 template cudaError_t launch_redact<BgrRowsW>(const RedactArgs &, const RedactFrameT<BgrRowsW> *, int, cudaStream_t);
+template cudaError_t launch_redact<YuvPlanesWO>(const RedactArgs &, const RedactFrameT<YuvPlanesWO> *, int, cudaStream_t);
 
 }  // namespace rf

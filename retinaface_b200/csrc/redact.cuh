@@ -8,6 +8,8 @@
 //                     cell value; luma first, then chroma
 // The counts are only known on the device: every CTA of measure / apply scans the frames' totals and strides over the work that
 // exists, so unused max_faces capacity costs nothing.
+// f20 oriented frames (YuvPlanesWO) run one more instantiation of each kernel: every position, cell, ellipse and blur tap is that of
+// the displayed frame, and only the byte each sample is read from or written to moves.
 // f14 styles (rf_redact_style) keep the regions kernel and the order.  MOSAIC with ELLIPSE runs measure unchanged and an apply that
 // tests each region's ellipse.  BLUR replaces measure with
 //   k_redact_blur     grid-stride over (frame, region, plane, strip of BLUR_W columns x band of BLUR_H rows): the triple-box blur of
@@ -33,6 +35,14 @@ struct BgrRowsW {
     uint8_t *p;
     int pitch;
 };
+// f20: a YUV frame redacted as it is displayed.  y, u, v point at displayed sample (0, 0) of each plane (yuv.cuh plane_map's off
+// applied), and displayed luma sample (x, y) is y[x * y_xs + y * y_ys], chroma u / v[x * c_xs + y * c_ys].  The kernels take it as
+// their ORIENTED instantiation; RedactFrameT's w x h is then the displayed size.
+struct YuvPlanesWO {
+    uint8_t *y, *u, *v;
+    int y_xs, y_ys, c_xs, c_ys;
+};
+template <typename Dst> constexpr bool kRedactYuv = !std::is_same<Dst, BgrRowsW>::value;
 
 // One frame of a call: its pixels, size, and the factor its records map back by (1 for records already in frame pixels).
 // blur: the frame's scratch planes (BLUR only; YUV: luma w x h, then U and V w/2 x h/2; BGR: 3 w x h), nullptr otherwise.

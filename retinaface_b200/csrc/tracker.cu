@@ -1,5 +1,6 @@
 // tracker.cu -- the video tracker behind include/rf_b200.h: f10 tracking, f11 best shots, f13 camera motion, f16 following, f12 / f14
-// redaction, f15 look-back, f17 searching look-back and f18 following look-back.  Detection itself is engine.cu's (yuv_device_impl).
+// redaction, f15 look-back, f17 searching look-back, f18 following look-back, f19 tiling and f20 oriented videos.  Detection itself is
+// engine.cu's (yuv_device_impl).
 // The entry points take their C linkage from rf_b200.h.
 #include <array>
 #include <cmath>
@@ -97,7 +98,22 @@ struct rf_tracker_s {
     bool tiled = false;
     rf_tiling tiling{};
     std::vector<rf_tile_level> tile_levels;
+    // f20 display orientations: each video's EXIF orientation (1: upright), kept across restarts, and whether the video has taken a
+    // frame call since its last restart (create, reset, drain, finish), which fixes its orientation until the next one.
+    std::vector<int> orient;
+    std::vector<char> started;
 };
+
+// Whether some video of t is shown in an orientation other than 1.
+static bool any_oriented(rf_tracker t) {
+    return std::any_of(t->orient.begin(), t->orient.end(), [](int o) { return o != 1; });
+}
+
+// f20: video v's orientation as LB_* bits, and the displayed size of its stored w x h frames.
+static int video_bits(rf_tracker t, int v) { return lb_orientation_bits(t->orient[v]); }
+static std::array<int, 2> shown_size(rf_tracker t, int v, int w, int h) {
+    return video_bits(t, v) & LB_TRANSPOSE ? std::array<int, 2>{h, w} : std::array<int, 2>{w, h};
+}
 
 template <typename... P>
 static void free_null(P *&...p) {
@@ -161,6 +177,8 @@ int rf_tracker_create(rf_handle h, const rf_track_config *cfg, rf_tracker *out) 
     std::unique_ptr<rf_tracker_s, void (*)(rf_tracker)> t(new rf_tracker_s, tracker_release);
     t->h = h;
     t->cfg = c;
+    t->orient.assign(c.max_videos, 1);
+    t->started.assign(c.max_videos, 0);
     try {
         CK(cudaSetDevice(h->device));
         const size_t T = c.max_tracks, F = h->cfg.max_faces, B = h->cfg.max_batch;
@@ -205,6 +223,7 @@ static void restart(rf_tracker t, size_t v0, size_t nv, cudaStream_t s) {
     if (t->kind == FOLLOW || t->lb_follow) CK(cudaMemsetAsync(t->d_fentries + v0 * T, 0, sizeof(FollowEntry) * nv * T, s));
     for (size_t v = v0; t->motion && v < v0 + nv; v++) t->mref[v] = {0, 0};
     for (size_t v = v0; t->kind == LOOKBACK && v < v0 + nv; v++) t->lbv[v].frames = 0;
+    std::fill(t->started.begin() + v0, t->started.begin() + v0 + nv, 0);
 }
 
 int rf_tracker_reset(rf_tracker t, int video) {
@@ -353,11 +372,17 @@ struct FrameCall {
     std::vector<long long> num;                        // LOOKBACK: lb_numbers' frame numbers and videos
     std::vector<std::array<int, 3>> seen;
     std::vector<std::vector<rf_tile>> layouts;         // DETECT on a tiling tracker: each frame's tiles
+    std::vector<int> orients;                          // f20: each frame's video's orientation, when `oriented`
+    bool oriented = false;                             // some frame of the call is not at orientation 1
     // set by issue_call: a tiled detect's ring slot event, recorded again once the call has read the records
     cudaEvent_t tiled_free = nullptr;
 };
 
 static int frame_call(FrameCall &c);
+
+
+// The YUV source of a detect call: each frame in its video's orientation when some frame is oriented, else the upright source.
+static YuvFrames detect_source(const FrameCall &c) { return YuvFrames{c.frames, c.matrix, c.oriented ? c.orients.data() : nullptr, c.oriented}; }
 
 // ---- f13 camera motion (motion.cuh) ---------------------------------------------------------------------------------------------
 // Each video's last frame of a call, whose thumbnail becomes the video's reference once the update has run.
@@ -379,17 +404,19 @@ static std::vector<MotionTable> motion_tables(rf_tracker t, const rf_yuv_frame *
         MotionFrame &f = tb.f[tb.n++];
         const rf_yuv_frame &fr = frames[i];
         const int v = videos[i];
-        f.y = fr.y;
-        f.pitch = fr.y_pitch;
+        const std::array<int, 2> size = shown_size(t, v, fr.width, fr.height);      // f20: the displayed frame's thumbnail
+        const PlaneMap m = plane_map(video_bits(t, v), size[0], size[1], fr.y_pitch, 1);
+        f.y = fr.y + m.off;
+        f.pitch = m.ys;
+        f.xs = m.xs;
         f.video = v;
         f.scale = scales ? scales[i] : 1.f;
-        f.D = (std::max(fr.width, fr.height) + MOTION_THUMB - 1) / MOTION_THUMB;
-        f.tw = fr.width / f.D;
-        f.th = fr.height / f.D;
+        f.D = (std::max(size[0], size[1]) + MOTION_THUMB - 1) / MOTION_THUMB;
+        f.tw = size[0] / f.D;
+        f.th = size[1] / f.D;
         f.nbx = f.tw - 2 * R >= MOTION_BLOCK ? (f.tw - 2 * R) / MOTION_BLOCK : 0;
         f.nby = f.th - 2 * R >= MOTION_BLOCK ? (f.th - 2 * R) / MOTION_BLOCK : 0;
         auto it = std::find_if(last.begin(), last.end(), [v](const std::array<int, 2> &e) { return e[0] == v; });
-        const std::array<int, 2> size = {fr.width, fr.height};
         if (it != last.end()) {
             const rf_yuv_frame &p = frames[(*it)[1]];
             f.ref = p.width == fr.width && p.height == fr.height ? (*it)[1] : MOTION_REF_FIRST;
@@ -400,7 +427,7 @@ static std::vector<MotionTable> motion_tables(rf_tracker t, const rf_yuv_frame *
         }
     }
     for (const auto &e : last) {
-        t->mref[e[0]] = {frames[e[1]].width, frames[e[1]].height};
+        t->mref[e[0]] = shown_size(t, e[0], frames[e[1]].width, frames[e[1]].height);
         commits.frames.push_back(e[1]);
         commits.videos.push_back(e[0]);
         const MotionFrame &f = tabs[e[1] / per].f[e[1] % per];
@@ -445,8 +472,10 @@ static FollowArgs follow_args(rf_tracker t) {
     return f;
 }
 
-static FollowFrame follow_frame(const rf_yuv_frame &fr, int video, int i) {
-    return FollowFrame{fr.y, fr.y_pitch, fr.width, fr.height, video, i};
+// f20: w x h the displayed size, and the video's orientation bits for the oriented launches.
+static FollowFrame follow_frame(rf_tracker t, const rf_yuv_frame &fr, int video, int i) {
+    const std::array<int, 2> size = shown_size(t, video, fr.width, fr.height);
+    return FollowFrame{fr.y, fr.y_pitch, size[0], size[1], video, i, video_bits(t, video)};
 }
 
 // The templates of the tracks matched on a detect call's frames, from the call's lists in `slot`, on s inside the chain.
@@ -455,8 +484,12 @@ static void follow_cut(rf_tracker t, const rf_yuv_frame *frames, const int *vide
     f.lists = slot.tracks;
     f.list_counts = slot.counts;
     std::vector<FollowFrame> tab(n);
-    for (int i = 0; i < n; i++) tab[i] = follow_frame(frames[i], videos[i], i);
-    CK(launch_follow_cut(f, tab.data(), n, s));
+    bool oriented = false;
+    for (int i = 0; i < n; i++) {
+        tab[i] = follow_frame(t, frames[i], videos[i], i);
+        oriented |= tab[i].bits != 0;
+    }
+    CK(launch_follow_cut(f, tab.data(), n, s, oriented));
 }
 
 // The update of a records or detect call into ring slot `ring`'s lists, on s inside the chain: with motion, the estimate of its frames
@@ -490,7 +523,7 @@ static void update_issue(rf_tracker t, unsigned ring, const FrameCall &c, cudaSt
         ta.seen = const_cast<TrackSeen *>(t->ba.seen);
         ta.gone = const_cast<TrackGone *>(t->ba.gone);
     }
-    const YuvFrames src{c.frames, c.matrix, nullptr, false};
+    const YuvFrames src = detect_source(c);
     const int chunk = c.sink == FrameCall::BEST ? TRACK_MAX_FRAMES : c.n;
     for (int i0 = 0; i0 < c.n; i0 += chunk) {
         const int m = std::min(chunk, c.n - i0);
@@ -507,7 +540,8 @@ static void update_issue(rf_tracker t, unsigned ring, const FrameCall &c, cudaSt
         for (int i = 0; i < m; i++) {
             const int v = c.videos[i0 + i];
             bt.video[i] = v;
-            bt.img[i] = AlignImageT<YuvPlanes>{src.in_place(i0 + i), src.width(i0 + i), src.height(i0 + i), 1.f, 0};
+            const std::array<int, 2> size = shown_size(t, v, src.width(i0 + i), src.height(i0 + i));    // f20: as displayed
+            bt.img[i] = AlignImageT<YuvPlanes>{src.in_place(i0 + i), size[0], size[1], 1.f, video_bits(t, v)};
             bool known = false;
             for (int j = 0; j < bt.nvideos; j++) known |= bt.cta_video[j] == v;
             if (!known) bt.cta_video[bt.nvideos++] = v;
@@ -768,19 +802,22 @@ static void follow_rounds(rf_tracker t, unsigned ring, const rf_yuv_frame *frame
     for (int r = 0; r < rounds; r++) {
         FollowTable tab{};
         std::vector<MotionTable> rt;
+        bool oriented = false;
         auto flush = [&]() {
             if (!tab.n) return;
             if (t->motion) {
                 CK(launch_follow_mask(f, tab, s));
                 CK(launch_motion_estimate(ma, rt.data(), (int)rt.size(), s));
             }
-            CK(launch_follow_round(f, tab, s));
+            CK(launch_follow_round(f, tab, s, oriented));
             tab.n = 0;
+            oriented = false;
             rt.clear();
         };
         for (int i = 0; i < n; i++) {
             if (round[i] != r) continue;
-            tab.f[tab.n++] = follow_frame(frames[i], videos[i], i);
+            tab.f[tab.n] = follow_frame(t, frames[i], videos[i], i);
+            oriented |= tab.f[tab.n++].bits != 0;
             if (t->motion) rt.push_back(mt[i]);
             if (tab.n == TRACK_MAX_FRAMES) flush();
         }
@@ -957,7 +994,7 @@ static void redact_issue(rf_handle h, Ctx &c, std::vector<RedactFrameT<Dst>> fra
     const size_t tables = (redact_scratch_bytes(std::max(h->cfg.max_batch, a.n), a.cap, a.blocks) + 255) & ~(size_t)255;
     size_t need = tables;
     if (spec.kind == REDACT_BLUR)
-        for (const auto &f : frames) need += (blur_plane_bytes(std::is_same<Dst, YuvPlanesW>::value, f.w, f.h) + 255) & ~(size_t)255;
+        for (const auto &f : frames) need += (blur_plane_bytes(kRedactYuv<Dst>, f.w, f.h) + 255) & ~(size_t)255;
     if (need > c.redact_bytes) {
         CK(cudaStreamSynchronize(c.stream));
         CK(cudaFree(c.d_redact));
@@ -971,7 +1008,7 @@ static void redact_issue(rf_handle h, Ctx &c, std::vector<RedactFrameT<Dst>> fra
         size_t off = tables;
         for (auto &f : frames) {
             f.blur = static_cast<uint8_t *>(c.d_redact) + off;
-            off += (blur_plane_bytes(std::is_same<Dst, YuvPlanesW>::value, f.w, f.h) + 255) & ~(size_t)255;
+            off += (blur_plane_bytes(kRedactYuv<Dst>, f.w, f.h) + 255) & ~(size_t)255;
         }
     }
     CK(launch_redact(a, frames.data(), h->num_sms, c.stream));
@@ -986,6 +1023,34 @@ static std::vector<RedactFrameT<YuvPlanesW>> yuv_redact_table(const rf_yuv_frame
                                         f.width, f.height, scales ? scales[i] : 1.f, nullptr};
     }
     return v;
+}
+
+// f20: the frames shown in orientations orients[i] (EXIF), as the oriented redaction kernels address them: each plane's displayed
+// sample (0, 0) and strides (yuv.cuh plane_map), and the displayed size.
+static std::vector<RedactFrameT<YuvPlanesWO>> yuv_redact_table_oriented(const rf_yuv_frame *frames, const int *orients, int n, const float *scales) {
+    std::vector<RedactFrameT<YuvPlanesWO>> v(n);
+    for (int i = 0; i < n; i++) {
+        const rf_yuv_frame &f = frames[i];
+        const int bits = lb_orientation_bits(orients[i]);
+        const bool tr = bits & LB_TRANSPOSE;
+        const int dw = tr ? f.height : f.width, dh = tr ? f.width : f.height;
+        const PlaneMap y = plane_map(bits, dw, dh, f.y_pitch, 1), c = plane_map(bits, dw / 2, dh / 2, f.uv_pitch, f.uv_step);
+        v[i] = RedactFrameT<YuvPlanesWO>{YuvPlanesWO{const_cast<uint8_t *>(f.y) + y.off, const_cast<uint8_t *>(f.u) + c.off,
+                                                     const_cast<uint8_t *>(f.v) + c.off, y.xs, y.ys, c.xs, c.ys},
+                                         dw, dh, scales ? scales[i] : 1.f, nullptr};
+    }
+    return v;
+}
+
+// redact_issue on YUV frames, frame i shown in EXIF orientation orients[i] (NULL: every frame upright): the oriented kernels when some
+// frame is not at orientation 1, else the upright ones.
+static void redact_yuv_issue(rf_handle h, Ctx &c, const rf_yuv_frame *frames, const int *orients, int n, const float *scales, const rf_det *dets,
+                             const int32_t *counts, rf_tracker t, const rf_track *tracks, const int32_t *track_counts, const RedactSpec &spec,
+                             int records = 0) {
+    if (orients && std::any_of(orients, orients + n, [](int o) { return o != 1; }))
+        redact_issue(h, c, yuv_redact_table_oriented(frames, orients, n, scales), dets, counts, t, tracks, track_counts, spec, records);
+    else
+        redact_issue(h, c, yuv_redact_table(frames, n, scales), dets, counts, t, tracks, track_counts, spec, records);
 }
 
 // The f12 and f14 entry points share one implementation each: `resolve` checks the params or the style where f12 checks its params.
@@ -1080,6 +1145,26 @@ int rf_redact_yuv_device_style(rf_handle h, const rf_yuv_frame *frames, int n, c
     static const char *who = "rf_redact_yuv_device_style";
     return redact_yuv_impl(h, who, frames, n, dev_dets, dev_counts, scales, t, dev_tracks, dev_track_counts,
                            [&](RedactSpec &r) { return redact_style(h, who, style, r); });
+}
+
+// f20: rf_redact_yuv_device_style on T_o(frame), mapped back.  A call whose frames are all at orientation 1 issues the upright kernels.
+int rf_redact_yuv_oriented_device_style(rf_handle h, const rf_yuv_frame *frames, const int *orientations, int n, const rf_det *dev_dets,
+                                        const int32_t *dev_counts, const float *scales, rf_tracker t, const rf_track *dev_tracks,
+                                        const int32_t *dev_track_counts, const rf_redact_style *style) {
+    static const char *who = "rf_redact_yuv_oriented_device_style";
+    if (!h) return RF_ERR_INVALID_ARG;
+    int rc = check_frames(h, who, frames, n, RF_YUV_BT601);
+    if (rc || (rc = check_orientations(h, who, orientations, n))) return rc;
+    RedactSpec spec;
+    if ((rc = redact_style(h, who, style, spec))) return rc;
+    if ((rc = check_redact_inputs(h, who, n, dev_dets, dev_counts, scales, t, dev_tracks, dev_track_counts))) return rc;
+    if ((rc = check_disjoint(h, who, yuv_ranges(frames, n)))) return rc;
+    if (n == 0) return RF_OK;
+    try {
+        CK(cudaSetDevice(h->device));
+        redact_yuv_issue(h, last_ctx(h), frames, orientations, n, scales, dev_dets, dev_counts, t, dev_tracks, dev_track_counts, spec);
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
 }
 
 int rf_redact_device(rf_handle h, uint8_t *const *dev_bgr, const int *widths, const int *heights, const int *row_strides, int n,
@@ -1297,10 +1382,12 @@ static void lb_search(rf_tracker t, const rf_yuv_frame *frames, const int *video
         by[it - vid.begin()].push_back(i);
     }
     LookbackSearchTable tb{};
+    bool oriented = false;
     for (size_t q = 0; q <= by.size(); q++) {
         if (tb.n > 0 && (q == by.size() || tb.n + (int)by[q].size() > LOOKBACK_SEARCH_FRAMES || tb.nv == LOOKBACK_SEARCH_VIDEOS)) {
-            CK(launch_lookback_search(a, tb, s));
+            CK(launch_lookback_search(a, tb, s, oriented));
             tb = LookbackSearchTable{};
+            oriented = false;
         }
         if (q == by.size()) break;
         const rf_tracker_s::LookbackVideo &lv = t->lbv[vid[q]];
@@ -1309,8 +1396,11 @@ static void lb_search(rf_tracker t, const rf_yuv_frame *frames, const int *video
         v.log = lb_log(t, lv);
         v.frame_bytes = lv.frame_bytes;
         v.num0 = num[by[q][0]];
-        v.w = lv.w;
-        v.h = lv.h;
+        const std::array<int, 2> size = shown_size(t, vid[q], lv.w, lv.h);      // f20: searched as displayed
+        v.w = size[0];
+        v.h = size[1];
+        v.bits = video_bits(t, vid[q]);
+        oriented |= v.bits != 0;
         v.first = tb.n;
         for (int i : by[q]) tb.f[tb.n++] = LookbackSearchFrame{frames[i].y, frames[i].y_pitch, tb.nv, i};
         tb.nv++;
@@ -1369,16 +1459,19 @@ static int lb_numbers(rf_tracker t, const char *who, const rf_yuv_frame *frames,
 
 // The emission of a look-back call or a drain into `slot`, on c's stream inside the chain: the swap `sw`, the regions of the emitted
 // frames `em`, then (a drain: `drained` >= 0) that video's restart, the chain, and the redaction of the emitted frames `outs`.
+// f20: out frame j is redacted as its video `out_videos[j]` displays it.
 static void lb_emit(rf_tracker t, Ctx &c, rf_tracker_s::Slot &slot, const std::vector<LookbackSwapFrame> &sw,
-                    const std::vector<std::array<long long, 3>> &em, const std::vector<rf_yuv_frame> &outs, const RedactSpec &spec,
-                    int drained = -1) {
+                    const std::vector<std::array<long long, 3>> &em, const std::vector<rf_yuv_frame> &outs, const std::vector<int> &out_videos,
+                    const RedactSpec &spec, int drained = -1) {
     lb_swap(sw, c.stream);
     lb_boxes(t, slot, em, c.stream);
     if (drained >= 0) restart(t, drained, 1, c.stream);     // then the video restarts as rf_tracker_reset restarts it
     CK(cudaEventRecord(t->chain, c.stream));
-    if (!outs.empty())
-        redact_issue(t->h, c, yuv_redact_table(outs.data(), (int)outs.size(), nullptr), slot.lb_boxes, slot.lb_counts, nullptr, nullptr, nullptr,
-                     spec, lb_records(t));
+    if (outs.empty()) return;
+    std::vector<int> oo;
+    for (int v : out_videos) oo.push_back(t->orient[v]);
+    redact_yuv_issue(t->h, c, outs.data(), oo.data(), (int)outs.size(), nullptr, slot.lb_boxes, slot.lb_counts, nullptr, nullptr, nullptr, spec,
+                     lb_records(t));
 }
 
 // The look-back half of call `fc`, whose tracking was issued on c's stream into ring slot `ring` (it recorded the chain; this follows
@@ -1424,6 +1517,7 @@ static void lb_issue(rf_tracker t, Ctx &c, unsigned ring, const FrameCall &fc, i
     std::vector<LookbackSwapFrame> sw;
     std::vector<std::array<long long, 3>> em;
     std::vector<rf_yuv_frame> outs;
+    std::vector<int> out_videos;
     for (int i = 0; i < n; i++) {
         const rf_tracker_s::LookbackVideo &lv = t->lbv[videos[i]];
         const bool emits = num[i] >= L;
@@ -1431,9 +1525,10 @@ static void lb_issue(rf_tracker t, Ctx &c, unsigned ring, const FrameCall &fc, i
         if (emits) {
             em.push_back({videos[i], num[i] - L, L});
             outs.push_back(out_frames[i]);
+            out_videos.push_back(videos[i]);
         }
     }
-    lb_emit(t, c, slot, sw, em, outs, fc.spec);
+    lb_emit(t, c, slot, sw, em, outs, out_videos, fc.spec);
 }
 
 int rf_detect_yuv_redact_lookback_device(rf_handle h, rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, int matrix, float thr,
@@ -1500,7 +1595,7 @@ int rf_tracker_drain(rf_tracker t, int video, const rf_redact_style *style, cons
             sw.push_back(lb_swap_frame(nullptr, out_frames + j, lv.d + (size_t)(e % L) * lv.frame_bytes));
             em.push_back({video, e, frames - 1 - e});
         }
-        lb_emit(t, c, slot, sw, em, std::vector<rf_yuv_frame>(out_frames, out_frames + k), spec, video);
+        lb_emit(t, c, slot, sw, em, std::vector<rf_yuv_frame>(out_frames, out_frames + k), std::vector<int>(k, video), spec, video);
         CK(cudaEventRecord(slot.free, c.stream));
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     for (int j = 0; j < k; j++) out_frame_numbers[j] = (int32_t)(frames - k + j);
@@ -1517,12 +1612,37 @@ int rf_tracker_set_tiling(rf_tracker t, const rf_tiling *tiling) {
     rf_handle h = t->h;
     int rc = admit(t, who, Call::SET_TILING);
     if (rc || (rc = tiling_supported(h, who))) return rc;
+    if (any_oriented(t))      // f20, in either order: tiled detection has no oriented path
+        return fail(h, RF_ERR_UNSUPPORTED, fmt("%s: a video of this tracker is shown in an orientation other than 1 (rf_tracker_set_orientation), "
+                                               "and tiled detection has no oriented path", who));
     std::string err;
     if ((rc = tiling_check(h->cfg.net_w, h->cfg.net_h, tiling, &err))) return fail(h, rc, fmt("%s: %s", who, err.c_str()));
     const bool dflt = !tiling || !tiling->levels || tiling->nlevels == 0;
     t->tile_levels.assign(dflt ? nullptr : tiling->levels, dflt ? nullptr : tiling->levels + tiling->nlevels);
     t->tiling = rf_tiling{t->tile_levels.empty() ? nullptr : t->tile_levels.data(), (int)t->tile_levels.size(), tiling ? tiling->overlap : 0};
     t->tiled = true;
+    return RF_OK;
+}
+
+// ---- f20 oriented videos -----------------------------------------------------------------------------------------------------------
+// Each video's display orientation, fixed from its first frame call to its next restart: a call reads and writes every frame as it is
+// displayed (issue_call, redact_issue), while descriptors, out frames and every size or layout check stay in stored geometry.
+int rf_tracker_set_orientation(rf_tracker t, int video, int orientation) {
+    static const char *who = "rf_tracker_set_orientation";
+    if (!t) return RF_ERR_INVALID_ARG;
+    rf_handle h = t->h;
+    const int V = t->cfg.max_videos;
+    if (video < -1 || video >= V) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: video %d, must be -1 or in [0, %d)", who, video, V));
+    if (lb_orientation_bits(orientation) < 0)
+        return fail(h, RF_ERR_INVALID_ARG, fmt("%s: orientation %d, must be in 1..8 (EXIF)", who, orientation));
+    const int v0 = video < 0 ? 0 : video, v1 = video < 0 ? V : video + 1;
+    for (int v = v0; v < v1; v++)
+        if (t->started[v])
+            return fail(h, RF_ERR_INVALID_ARG,
+                        fmt("%s: video %d has taken a frame call since its last create, reset, drain or finish", who, v));
+    if (orientation != 1 && t->tiled)
+        return fail(h, RF_ERR_UNSUPPORTED, fmt("%s: a tiling tracker has no oriented detection (rf_tracker_set_tiling)", who));
+    std::fill(t->orient.begin() + v0, t->orient.begin() + v1, orientation);
     return RF_OK;
 }
 
@@ -1545,10 +1665,12 @@ static int check_call(FrameCall &c) {
     const int n = c.n;
     int rc = check_track_args(t, who, c.call, c.videos, n, c.source == FrameCall::RECORDS ? c.scales : nullptr);
     if (rc) return rc;
+    for (int i = 0; i < n; i++) c.oriented |= t->orient[c.videos[i]] != 1;
+    for (int i = 0; c.oriented && i < n; i++) c.orients.push_back(t->orient[c.videos[i]]);
     if (c.source == FrameCall::RECORDS && n > 0 && (!c.dets || !c.counts))
         return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL records or counts", who));
     if (c.source == FrameCall::DETECT) {
-        const YuvFrames src{c.frames, c.matrix, nullptr, false};
+        const YuvFrames src = detect_source(c);
         if ((rc = t->tiled ? yuv_tiled_check(h, who, src, n, &t->tiling, c.layouts) : src.check(h, who, n))) return rc;
     }
     if (c.source == FrameCall::FOLLOW && (rc = check_frames(h, who, c.frames, n, RF_YUV_BT601))) return rc;
@@ -1586,7 +1708,7 @@ static int issue_call(FrameCall &c) {
             lv.v_first = f.uv_step == 2 && f.v < f.u;
         }
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
-    const YuvFrames src{c.frames, c.matrix, nullptr, false};
+    const YuvFrames src = detect_source(c);
     std::vector<float> scales(n);
     if (c.source == FrameCall::DETECT) {
         if (t->tiled) {      // f19: the tiled ring's records, in frame pixels
@@ -1606,6 +1728,7 @@ static int issue_call(FrameCall &c) {
         const unsigned ring = slot_begin(t, s);
         rf_tracker_s::Slot &slot = t->slots[ring];
         t->updated = true;
+        for (int i = 0; i < n; i++) t->started[c.videos[i]] = 1;
         if (c.source == FrameCall::FOLLOW) {
             follow_rounds(t, ring, c.frames, c.videos, n, s);
             c.dets = slot.fregions;      // in id order, max_tracks to a frame, at scale 1
@@ -1618,9 +1741,14 @@ static int issue_call(FrameCall &c) {
         CK(cudaEventRecord(t->chain, s));
         const int per_frame = c.source == FrameCall::FOLLOW ? t->cfg.max_tracks : h->cfg.max_faces;
         if (c.sink == FrameCall::CROPS) {
-            // the due faces are already in frame pixels: scale 1, as the tiled paths crop their merged records
+            // the due faces are already in frame pixels: scale 1, as the tiled paths crop their merged records.  f20: displayed pixels
+            // of an oriented frame, whose crops f9's oriented warp cuts upright
             std::vector<AlignImageT<YuvPlanes>> table(n);
-            for (int i = 0; i < n; i++) table[i] = AlignImageT<YuvPlanes>{src.in_place(i), src.width(i), src.height(i), 1.f, 0};
+            for (int i = 0; i < n; i++) {
+                const int bits = src.bits(i);
+                const bool tr = bits & LB_TRANSPOSE;
+                table[i] = AlignImageT<YuvPlanes>{src.in_place(i), tr ? src.height(i) : src.width(i), tr ? src.width(i) : src.height(i), 1.f, bits};
+            }
             c.a.n = n;
             c.a.crops = c.crops;
             c.a.mats = c.mats;
@@ -1628,10 +1756,11 @@ static int issue_call(FrameCall &c) {
             view.out_dets = slot.due;
             view.out_counts = slot.due_counts;
             view.max_faces = h->cfg.max_faces;
-            CK(launch_align_faces(c.a, table.data(), view, h->num_sms, s));
+            CK(launch_align_faces(c.a, table.data(), view, h->num_sms, s, c.oriented));
         } else if (c.sink == FrameCall::REDACT) {
             // (a) the records, (b) the LOST tracks of the lists: f12's geometry, f14's styles and ownership
-            redact_issue(h, ctx, yuv_redact_table(c.frames, n, c.scales), c.dets, c.counts, t, slot.tracks, slot.counts, c.spec, per_frame);
+            redact_yuv_issue(h, ctx, c.frames, c.oriented ? c.orients.data() : nullptr, n, c.scales, c.dets, c.counts, t, slot.tracks,
+                             slot.counts, c.spec, per_frame);
         } else if (c.sink == FrameCall::LOOKBACK) {
             lb_issue(t, ctx, ring, c, per_frame);
         }

@@ -4,6 +4,7 @@
 // thread" are called by all of them, the shared arrays are the caller's.
 #pragma once
 #include "follow.cuh"
+#include "yuv.cuh"
 
 namespace rf {
 
@@ -30,8 +31,28 @@ __device__ __forceinline__ Grid grid_of(double cx, double cy, double w, double h
 // c_k: {1 / s, 1, s}
 __device__ __forceinline__ double scale_of(int k) { return k == 0 ? 1.0 / RF_FOLLOW_SCALE : k == 1 ? 1.0 : RF_FOLLOW_SCALE; }
 
+// A luma plane as the search reads it: sample (x, y) at y[y * pitch + x], w x h.
+struct PitchedLuma {
+    const uint8_t *y;
+    int pitch, w, h;
+};
+// f20: a luma plane read as it is displayed: sample (x, y) at y[x * xs + y * ys] (yuv.cuh plane_map), w x h the displayed size.
+struct OrientedLuma {
+    const uint8_t *y;
+    int xs, ys, w, h;
+};
+// A stored luma plane (pitch bytes a row) of a frame shown in orientation `bits` as w x h.
+__device__ __forceinline__ OrientedLuma oriented_luma(const uint8_t *y, int pitch, int bits, int w, int h) {
+    const PlaneMap m = plane_map(bits, w, h, pitch, 1);
+    return OrientedLuma{y + m.off, m.xs, m.ys, w, h};
+}
+template <class P>
+__device__ __forceinline__ int luma_px(const P &f, int x, int y) { return f.y[(size_t)y * f.pitch + x]; }
+__device__ __forceinline__ int luma_px(const OrientedLuma &f, int x, int y) { return f.y[(long long)y * f.ys + (long long)x * f.xs]; }
+
 // Pixel (i, j) of the map [[px, 0, X], [0, py, Y]]: cv::warpAffine's fixed-point coordinate and f5's integer bilinear on the luma
-// plane (warp.cuh's sample() on one channel).  inside: all four taps lay in the frame.  P: a luma plane with y, pitch, w and h.
+// plane (warp.cuh's sample() on one channel).  inside: all four taps lay in the frame.  P: a luma plane with y, w and h, read by
+// luma_px (PitchedLuma, FollowFrame, or an OrientedLuma).
 template <class P>
 __device__ __forceinline__ int luma_at(const P &f, double px, double py, double X, double Y, int i, int j, bool &inside) {
     const int Xf = (__double2int_rn(X * 1024.0) + 16 + __double2int_rn((px * (double)i) * 1024.0)) >> 5;
@@ -44,7 +65,7 @@ __device__ __forceinline__ int luma_at(const P &f, double px, double py, double 
     for (int t = 0; t < 4; t++) {
         const int tx = sx + (t & 1), ty = sy + (t >> 1);
         if ((unsigned)tx < (unsigned)f.w && (unsigned)ty < (unsigned)f.h) {
-            acc += wts[t] * f.y[(size_t)ty * f.pitch + tx];
+            acc += wts[t] * luma_px(f, tx, ty);
             in++;
         }
     }

@@ -38,4 +38,19 @@ __device__ __forceinline__ void yuv_pixel(const YuvPlanes &p, int x, int y, int 
     yuv_to_bgr(Y, p.u[c], p.v[c], p.matrix, out);
 }
 
+// f20: the stored address of a displayed plane sample.  A plane whose stored sample (c, r) lies at r * pitch + c * step, shown in
+// orientation `bits` (preprocess.cuh's LB_* bits of f9's A_o) as a dw x dh plane, holds displayed sample (x, y) at
+// off + x * xs + y * ys: A_o reflects then transposes integer addresses, so the map is affine with strides of +-step and +-pitch.
+// Luma uses the displayed frame's size; chroma the halved size (even sides: the 2x2 blocks of the displayed frame are blocks of the
+// stored one).  Bits 0 give off 0, xs step, ys pitch: the stored layout.
+struct PlaneMap {
+    long long off;
+    int xs, ys;
+};
+__host__ __device__ inline PlaneMap plane_map(int bits, int dw, int dh, int pitch, int step) {
+    const bool fx = bits & 1, fy = bits & 2, tr = bits & 4;      // LB_FLIP_X, LB_FLIP_Y, LB_TRANSPOSE
+    const int a = tr ? pitch : step, b = tr ? step : pitch;      // the strides of the reflected x and y
+    return PlaneMap{(fx ? (long long)a * (dw - 1) : 0) + (fy ? (long long)b * (dh - 1) : 0), fx ? -a : a, fy ? -b : b};
+}
+
 }  // namespace rf

@@ -119,6 +119,27 @@ class RetinaFace:
         faces, _, _ = self.engine.detect_views_oriented(img, [(1.0, o) for o in ANY_ORIENTATION], threshold, self.nms_threshold)
         return [FaceDetectInfo.from_row(r) for r in faces]
 
+    def setVideoOrientation(self, video: int, orientation: int):
+        """f20 oriented video (rf_tracker_set_orientation): ``video`` (-1: every video) is shown in EXIF orientation 1..8 -- portrait
+        phone video stored as landscape surfaces -- and ``trackFrames`` / ``redactFrames`` read and write its frames as displayed, with
+        tracks in displayed pixels.  Applied when this detector's tracker is created, or at once when it exists; before the video's
+        first tracked frame since creation or a reset."""
+        trk = getattr(self, "_tracker", None)
+        if trk is not None:
+            trk.set_orientation(video, orientation)
+        self._orientations = getattr(self, "_orientations", []) + [(int(video), int(orientation))]
+
+    def _new_tracker(self, **kw):
+        """Engine.tracker with this detector's video orientations applied."""
+        trk = self.engine.tracker(**kw)
+        try:
+            for v, o in getattr(self, "_orientations", []):
+                trk.set_orientation(v, o)
+        except Exception:
+            trk.close()
+            raise
+        return trk
+
     def _interval_calls(self, videos: Sequence[int], detect_every: int):
         """f16: frame i of video v is a detect frame when v's frame number (counted over every call since the tracker's creation or
         the video's reset) is divisible by detect_every.  Returns [(detect?, frame indices)] in issue order: each video's frames split
@@ -182,7 +203,7 @@ class RetinaFace:
             raise ValueError("best shots and new-identity crops are exclusive: pass best or align, not both")
         self._interval_tracker(detect_every, best=best, tiling=tiling)
         if getattr(self, "_tracker", None) is None:
-            self._tracker = self.engine.tracker(max_videos=max_videos, best=best, motion=motion, follow=detect_every > 1, tiling=tiling)
+            self._tracker = self._new_tracker(max_videos=max_videos, best=best, motion=motion, follow=detect_every > 1, tiling=tiling)
         if self._tracker.follow_on:
             tracks, new = [None] * len(frames), [[] for _ in frames]
             for det, idx in self._interval_calls(videos, detect_every):
@@ -272,7 +293,7 @@ class RetinaFace:
             return
         interval = detect_every > 1
         if getattr(self, "_tracker", None) is None:
-            self._tracker = self.engine.tracker(max_videos=max_videos, motion=motion, lookback=lookback or None,
+            self._tracker = self._new_tracker(max_videos=max_videos, motion=motion, lookback=lookback or None,
                                                 follow=interval and not lookback, lookback_search=lookback_search or None,
                                                 lookback_follow=(interval and lookback) or None, tiling=tiling)
         elif lookback_search and not self._tracker.lookback_search_on:

@@ -388,6 +388,14 @@ void RetinaFace::followCall(const vector<rf_yuv_frame> &frames, const vector<int
     noteMotion(n);
 }
 
+void RetinaFace::setVideoOrientation(int video, int orientation) {
+    if (tracker_) {
+        int rc = rf_tracker_set_orientation(tracker_, video, orientation);
+        if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_set_orientation: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+    }
+    orientations_.push_back({video, orientation});
+}
+
 void RetinaFace::trackerCreated(bool follow) {
     if (opt_.track_tiling) {
         if (opt_.track_tile_flip && opt_.track_tile_scales.empty())
@@ -406,10 +414,15 @@ void RetinaFace::trackerCreated(bool follow) {
         int rc = rf_tracker_set_follow(tracker_, &fc);
         if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_set_follow: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
     }
-    if (!opt_.track_motion) return;
-    const rf_motion_config mc{};
-    int rc = rf_tracker_set_motion(tracker_, &mc);
-    if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_set_motion: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+    if (opt_.track_motion) {
+        const rf_motion_config mc{};
+        int rc = rf_tracker_set_motion(tracker_, &mc);
+        if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_set_motion: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+    }
+    for (const auto &o : orientations_) {
+        int rc = rf_tracker_set_orientation(tracker_, o.first, o.second);
+        if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_set_orientation: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+    }
 }
 
 void RetinaFace::noteMotion(int n) {

@@ -142,6 +142,11 @@ class RetinaFace {
                   void *dev_crops = nullptr);
     const DeviceTracks &lastTracks() const { return tracks_; }
     void resetTracks(int video = -1);
+    // f20 oriented video (rf_tracker_set_orientation): video (-1: every video) is shown in EXIF orientation 1..8 -- portrait phone
+    // video stored as landscape surfaces -- and trackYUV, trackYUVBest and redactYUV read and write its frames as displayed, with
+    // tracks in displayed pixels.  Applied when this RetinaFace's tracker is created, or at once when it exists; before the video's
+    // first tracked frame since creation or resetTracks.
+    void setVideoOrientation(int video, int orientation);
     // f11 best shots (rf_detect_yuv_track_best_device): trackYUV on a best-shot tracker (created on the first call with min_quality;
     // one RetinaFace keeps one kind of tracker) that keeps the best 112x112 u8 crop of every track on the GPU.  Afterwards lastTracks()
     // holds the track lists and lastBestShots() the shots emitted on each frame -- one per ever-confirmed track that ended there, in
@@ -215,6 +220,7 @@ class RetinaFace {
     DeviceMotion motion_;
     DeviceFollow follow_;
     std::map<int, long long> frame_no_;
+    vector<std::pair<int, int>> orientations_;   // f20: setVideoOrientation's (video, orientation), replayed on a new tracker
     vector<int32_t> frame_numbers_;
     RetinaFaceOptions opt_;
     string network;

@@ -1040,7 +1040,8 @@ int rf_tracker_set_tiling(rf_tracker t, const rf_tiling *tiling);
  * rf_tracker_reset, rf_tracker_drain or rf_tracker_finish (which keep the orientation: it belongs to the source, not to the run).
  * Every tracker kind and option takes it: plain, best-shot, follow and look-back, with motion, search or following.  A bad video, an
  * orientation outside 1..8, or a video already under way: RF_ERR_INVALID_ARG.  An orientation other than 1 on a tiling tracker, or
- * rf_tracker_set_tiling once some video is not at orientation 1: RF_ERR_UNSUPPORTED (tiled detection has no oriented path).
+ * rf_tracker_set_tiling once some video is not at orientation 1: RF_ERR_UNSUPPORTED (a tiling tracker detects upright frames only;
+ * f21's oriented tiled calls feed rf_track_update and rf_redact_yuv_oriented_device_style instead).
  * Nothing changes on a refusal.  Sizes that describe geometry -- motion thumbnails and references, follow and search frames,
  * redaction frames -- are the displayed ones; sizes that describe memory -- the look-back buffer, out frames, disjointness -- the
  * stored ones. */
@@ -1052,6 +1053,39 @@ int rf_tracker_set_orientation(rf_tracker t, int video, int orientation);
 int rf_redact_yuv_oriented_device_style(rf_handle h, const rf_yuv_frame *frames, const int *orientations, int n, const rf_det *dev_dets,
                                         const int32_t *dev_counts, const float *scales, rf_tracker t, const rf_track *dev_tracks,
                                         const int32_t *dev_track_counts, const rf_redact_style *style);
+
+/* f21 small faces in rotated and mirrored images and video: f7 / f8's tiled detection of the DISPLAYED image D = T_o(S) (f9's table;
+ * D = T_o(cvtColor(frame)) for YUV), without a rotated copy.  An oriented tiled call is exactly the unoriented tiled call on D: the
+ * layout is rf_tile_layout(net_w, net_h, Dw, Dh, t) of the displayed size (H x W for 5..8), a level is cv::resize(D) (of
+ * cv::flip(D, 1) when mirrored), and faces, out_tile_of and anchor_index / max_faces are in DISPLAYED pixels and index the displayed
+ * layout, as rf_detect_oriented_batch returns them (not mapped to stored pixels as rf_detect_views_oriented does).  Crops are cut
+ * from D and M maps displayed image -> crop.  As in f9 the orientation moves integer addresses only, so every tile byte, record,
+ * crop and matrix is that of the unoriented call on T_o(S), bit for bit; orientation 1 is the unoriented call.  Statuses are the
+ * unoriented twin's, in its order: the source checks with f9's orientation check inside them (an orientation outside 1..8 or a NULL
+ * orientations array with n > 0: RF_ERR_INVALID_ARG), then the layouts of the displayed sizes (level sides, RF_MAX_TILES,
+ * the overlap), then the align checks, all before anything is launched; RF_FLAG_NPP_RESIZE: RF_ERR_UNSUPPORTED.
+ *
+ * Host BGR images, blocking: rf_detect_tiled with orientations; align == NULL: no crops (out_crops / out_mats unused), otherwise
+ * rf_detect_tiled_align's crops and its raw-buffer rule (every original stays resident: more images than raw buffers is
+ * RF_ERR_CAPACITY). */
+int rf_detect_tiled_oriented(rf_handle h, const uint8_t *const *bgr_images, const int *widths, const int *heights, const int *row_strides,
+                             const int *orientations, int n, const rf_tiling *t, float score_threshold, float nms_threshold,
+                             const rf_align_params *align, rf_face *out_faces, int *out_counts, int32_t *out_tile_of, void *out_crops,
+                             double *out_mats);
+/* Device, asynchronous: rf_detect_tiled_device / rf_detect_yuv_tiled_device with orientations -- the same ring of output slots, home
+ * context, rf_last_stream and validity rule.  A 4K portrait phone video (3840x2160 NV12 surfaces shown at 6) is tiled as 2160x3840. */
+int rf_detect_tiled_oriented_device(rf_handle h, const uint8_t *const *dev_bgr, const int *widths, const int *heights, const int *row_strides,
+                                    const int *orientations, int n, const rf_tiling *t, float score_threshold, float nms_threshold,
+                                    const rf_align_params *align, void *dev_crops, double *dev_mats, const rf_det **dev_dets,
+                                    const int32_t **dev_counts);
+int rf_detect_yuv_tiled_oriented_device(rf_handle h, const rf_yuv_frame *frames, const int *orientations, int n, int matrix, const rf_tiling *t,
+                                        float score_threshold, float nms_threshold, const rf_align_params *align, void *dev_crops,
+                                        double *dev_mats, const rf_det **dev_dets, const int32_t **dev_counts);
+/* Preprocess parity (as rf_preprocess_tile / rf_preprocess_yuv_tile): tile `tile` of the displayed image's layout. */
+int rf_preprocess_tile_oriented(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, int orientation, const rf_tiling *t,
+                                int tile, uint8_t *out_net_sized);
+int rf_preprocess_yuv_tile_oriented(rf_handle h, const rf_yuv_frame *frame, int matrix, int orientation, const rf_tiling *t, int tile,
+                                    uint8_t *out_net_sized);
 
 /* Introspection. */
 int rf_get_net_size(rf_handle h, int *net_w, int *net_h, int *max_batch, int *max_faces);

@@ -378,6 +378,11 @@ _SIGNATURES = {
     "rf_tracker_set_tiling": (_I, [_P, _TILING]),
     "rf_tracker_set_orientation": (_I, [_P, _I, _I]),
     "rf_redact_yuv_oriented_device_style": (_I, [_P, _FRAMES, _PI, _I, _P, _P, _P, _P, _P, _P, _STYLE]),
+    "rf_detect_tiled_oriented": (_I, [_P, _PP, _PI, _PI, _PI, _PI, _I, _TILING, _F, _F, _ALIGN, _P, _P, _P, _P, _P]),
+    "rf_detect_tiled_oriented_device": (_I, [_P, _PP, _PI, _PI, _PI, _PI, _I, _TILING, _F, _F, _ALIGN, _P, _P, _PP, _PP]),
+    "rf_detect_yuv_tiled_oriented_device": (_I, [_P, _FRAMES, _PI, _I, _I, _TILING, _F, _F, _ALIGN, _P, _P, _PP, _PP]),
+    "rf_preprocess_tile_oriented": (_I, [_P, _P, _I, _I, _I, _I, _TILING, _I, _P]),
+    "rf_preprocess_yuv_tile_oriented": (_I, [_P, _FRAMES, _I, _I, _TILING, _I, _P]),
 }
 EXPORTS = list(_SIGNATURES)     # every symbol include/rf_b200.h declares (checked by tests/test_host_side.py)
 
@@ -1035,6 +1040,69 @@ class Engine:
                                                       C.c_float(thr), C.c_float(nms), C.c_void_p(faces.ctypes.data), C.byref(count),
                                                       C.c_void_p(view_of.ctypes.data), C.c_void_p(scales.ctypes.data)))
         return faces[:count.value].copy(), view_of[:count.value].copy(), scales[:nv].copy()
+
+    # -- f21 tiled detection of rotated and mirrored images ---------------------------------------------------------------------
+    def detect_tiled_oriented(self, images: Sequence[np.ndarray], orientations: Sequence[int], thr: float, nms_thr: float, levels=None,
+                              overlap: int = 0, align: Optional[dict] = None):
+        """rf_detect_tiled_oriented: detect_tiled on the images shown in EXIF orientation orientations[i] -- the layout, tiles,
+        faces, tile_of and crops of the DISPLAYED image, without a rotated copy.  Returns what detect_tiled returns."""
+        n = len(images)
+        keep, ptrs, ws, hs, rs = self._host_images(images)
+        o = _orientations(orientations, n)
+        t = tiling(levels, overlap)
+        faces, counts, tile_of = self._outputs(n, True)
+        p, A, crops, mats = self._host_align(n, align) if align is not None else (None, 0, None, None)
+        self._check(self.lib.rf_detect_tiled_oriented(self.h, ptrs, ws, hs, rs, o, n, C.byref(t), thr, nms_thr, _ref(p), faces.ctypes.data,
+                                                      counts.ctypes.data, tile_of.ctypes.data, _addr(crops), _addr(mats)))
+        return self._result(counts, faces, tile_of, A, crops, mats)
+
+    def detect_tiled_oriented_device(self, images, orientations: Sequence[int], thr: float, nms_thr: float, levels=None, overlap: int = 0,
+                                     align: Optional[dict] = None, dev_crops_ptr: Optional[int] = None, dev_mats_ptr: Optional[int] = None):
+        """rf_detect_tiled_oriented_device: detect_tiled_device on images shown in EXIF orientation orientations[i]; records in
+        DISPLAYED image pixels.  Returns (dets_ptr, counts_ptr)."""
+        n = len(images)
+        ptrs, ws, hs, rs = self._device_images(images)
+        o = _orientations(orientations, n)
+        t = tiling(levels, overlap)
+        p = align_params(**align) if align is not None else None
+        d, c = C.c_void_p(), C.c_void_p()
+        self._check(self.lib.rf_detect_tiled_oriented_device(self.h, ptrs, ws, hs, rs, o, n, C.byref(t), thr, nms_thr, _ref(p),
+                                                             dev_crops_ptr, dev_mats_ptr, C.byref(d), C.byref(c)))
+        return int(d.value or 0), int(c.value or 0)
+
+    def detect_yuv_tiled_oriented_device(self, frames, orientations: Sequence[int], thr: float, nms_thr: float, layout: str = "nv12",
+                                         matrix="bt601", levels=None, overlap: int = 0, align: Optional[dict] = None,
+                                         dev_crops_ptr: Optional[int] = None, dev_mats_ptr: Optional[int] = None):
+        """rf_detect_yuv_tiled_oriented_device: detect_yuv_tiled_device on frames shown in EXIF orientation orientations[i] (portrait
+        4K NVDEC surfaces); records in DISPLAYED frame pixels.  Returns (dets_ptr, counts_ptr)."""
+        n = len(frames)
+        arr = self._frames(frames, layout, True)
+        o = _orientations(orientations, n)
+        t = tiling(levels, overlap)
+        p = align_params(**align) if align is not None else None
+        d, c = C.c_void_p(), C.c_void_p()
+        self._check(self.lib.rf_detect_yuv_tiled_oriented_device(self.h, arr, o, n, _matrix(matrix), C.byref(t), thr, nms_thr, _ref(p),
+                                                                 dev_crops_ptr, dev_mats_ptr, C.byref(d), C.byref(c)))
+        return int(d.value or 0), int(c.value or 0)
+
+    def preprocess_tile_oriented(self, img: np.ndarray, orientation: int, tile: int, levels=None, overlap: int = 0) -> np.ndarray:
+        """rf_preprocess_tile_oriented: tile `tile` of the displayed image's layout as the network sees it, (H, W, 3) u8 BGR."""
+        img = self._bgr_strided(img)
+        out = np.empty((self.net_h, self.net_w, 3), dtype=np.uint8)
+        t = tiling(levels, overlap)
+        self._check(self.lib.rf_preprocess_tile_oriented(self.h, img.ctypes.data, img.shape[1], img.shape[0], img.strides[0], int(orientation),
+                                                         C.byref(t), int(tile), out.ctypes.data))
+        return out
+
+    def preprocess_yuv_tile_oriented(self, frame, orientation: int, tile: int, layout: str = "nv12", matrix="bt601", levels=None,
+                                     overlap: int = 0) -> np.ndarray:
+        """rf_preprocess_yuv_tile_oriented: tile `tile` of the displayed frame's layout as the network sees it, (H, W, 3) u8 BGR."""
+        arr = self._frames([frame], layout, False)
+        out = np.empty((self.net_h, self.net_w, 3), dtype=np.uint8)
+        t = tiling(levels, overlap)
+        self._check(self.lib.rf_preprocess_yuv_tile_oriented(self.h, arr, _matrix(matrix), int(orientation), C.byref(t), int(tile),
+                                                             out.ctypes.data))
+        return out
 
     # -- f10 face tracking across video frames ---------------------------------------------------------------------------------
     def tracker(self, max_videos: int = 1, max_tracks: int = 0, high_thresh: float = 0.0, new_thresh: float = 0.0, iou_high: float = 0.0,

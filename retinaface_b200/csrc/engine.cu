@@ -925,14 +925,17 @@ int rf_eng::tiling_supported(rf_handle h, const char *who) {
     return RF_OK;
 }
 
-// The checks every tiled path shares, after its source check: the resize definition and each image's layout.
+// The checks every tiled path shares, after its source check: the resize definition and each image's layout, of its displayed size
+// (f21: an oriented image is tiled as the displayed image D = T_o(S)).
 template <typename Source>
 static int tiled_layouts(rf_handle h, const char *who, const Source &src, int n, const rf_tiling *t, std::vector<std::vector<rf_tile>> &layouts) {
     if (int rc = tiling_supported(h, who)) return rc;
     layouts.resize(n);
     for (int i = 0; i < n; i++) {
         std::string err;
-        const int rc = tile_layout(h->cfg.net_w, h->cfg.net_h, src.width(i), src.height(i), t, layouts[i], &err);
+        int dw, dh;
+        displayed_size(src, i, dw, dh);
+        const int rc = tile_layout(h->cfg.net_w, h->cfg.net_h, dw, dh, t, layouts[i], &err);
         if (rc) return fail(h, rc, fmt("%s: image %d: %s", who, i, err.c_str()));
     }
     return RF_OK;
@@ -986,8 +989,11 @@ static void detect_tiled_impl(rf_handle h, const Source &source, int n, const st
             for (int b = 0; b < m; b++) {
                 const TileRef r = refs[k0 + b];
                 const rf_tile &tl = layouts[r.image][r.tile];
-                tile_fill(lb[b], src[r.image], source.width(r.image), source.height(r.image), c.d_frames_in + b * img_bytes, Wn, Hn, tl);
-                ms[b] = tile_source(r.image, r.tile, mf, tl, source.width(r.image));
+                int dw, dh;
+                displayed_size(source, r.image, dw, dh);
+                tile_fill(lb[b], src[r.image], dw, dh, source.bits(r.image), c.d_frames_in + b * img_bytes, Wn, Hn, tl);
+                // records stay in displayed pixels: a mirrored level is un-mirrored with the displayed width (k_merge<false>)
+                ms[b] = tile_source(r.image, r.tile, mf, tl, dw);
             }
             CK(launch_letterbox_batch(lb.data(), m, Wn, Hn, c.stream));
             set_params(h, c, thr, nms, c.d_frames_in);
@@ -1021,14 +1027,18 @@ static bool tiled_grow(rf_handle h, PostBuffers &pb, const std::vector<std::vect
 
 
 // The crops of every kept face in pb (a.crops / a.mats set by the caller), cut on s from the originals srcs at map-back factor 1
-// (the merged records are in image pixels).
+// (the merged records are in displayed image pixels; an oriented source reads its stored pixels through f9's oriented table).
 template <typename Source>
 static void tiled_crops(rf_handle h, AlignArgs a, int n, const Source &source, const std::vector<typename Source::Src> &srcs, const PostBuffers &pb,
                         cudaStream_t s) {
     std::vector<AlignImageT<typename Source::Src>> table(n);
-    for (int i = 0; i < n; i++) table[i] = AlignImageT<typename Source::Src>{srcs[i], source.width(i), source.height(i), 1.f, 0};
+    for (int i = 0; i < n; i++) {
+        int dw, dh;
+        displayed_size(source, i, dw, dh);
+        table[i] = AlignImageT<typename Source::Src>{srcs[i], dw, dh, 1.f, source.bits(i)};
+    }
     a.n = n;
-    CK(launch_align_faces(a, table.data(), pb, h->num_sms, s));
+    CK(launch_align_faces(a, table.data(), pb, h->num_sms, s, source.oriented));
 }
 
 // The blocking tiled paths: sources uploaded on context 0, merged into pb_tiles, fetched.  With `aligned`, the crops are cut on
@@ -1177,6 +1187,28 @@ int rf_detect_yuv_tiled_device(rf_handle h, const rf_yuv_frame *frames, int n, i
                                dev_mats, dev_dets, dev_counts);
 }
 
+// f21 oriented tiled detection (rf_b200.h): the tiled paths on the displayed images, through the same checks and issue
+int rf_detect_tiled_oriented(rf_handle h, const uint8_t *const *imgs, const int *widths, const int *heights, const int *row_strides,
+                             const int *orientations, int n, const rf_tiling *t, float thr, float nms, const rf_align_params *align,
+                             rf_face *out_faces, int *out_counts, int32_t *out_tile_of, void *out_crops, double *out_mats) {
+    return detect_tiled_blocking(h, "rf_detect_tiled_oriented", BgrImages{imgs, widths, heights, row_strides, orientations, true}, n, t, thr,
+                                 nms, align != nullptr, align, out_faces, out_counts, out_tile_of, out_crops, out_mats);
+}
+
+int rf_detect_tiled_oriented_device(rf_handle h, const uint8_t *const *dev_bgr, const int *widths, const int *heights, const int *row_strides,
+                                    const int *orientations, int n, const rf_tiling *t, float thr, float nms, const rf_align_params *align,
+                                    void *dev_crops, double *dev_mats, const rf_det **dev_dets, const int32_t **dev_counts) {
+    return detect_tiled_device(h, "rf_detect_tiled_oriented_device", BgrImages{dev_bgr, widths, heights, row_strides, orientations, true}, n, t,
+                               thr, nms, align, dev_crops, dev_mats, dev_dets, dev_counts);
+}
+
+int rf_detect_yuv_tiled_oriented_device(rf_handle h, const rf_yuv_frame *frames, const int *orientations, int n, int matrix, const rf_tiling *t,
+                                        float thr, float nms, const rf_align_params *align, void *dev_crops, double *dev_mats,
+                                        const rf_det **dev_dets, const int32_t **dev_counts) {
+    return detect_tiled_device(h, "rf_detect_yuv_tiled_oriented_device", YuvFrames{frames, matrix, orientations, true}, n, t, thr, nms, align,
+                               dev_crops, dev_mats, dev_dets, dev_counts);
+}
+
 // ---- parity hooks: the network input of one image ---------------------------------------------------------------------------------
 // Image 0 of src uploaded into raw buffer 0 and letter-boxed (with `tiled`, tile `tile` of its layout) into `out`.
 extern "C++" {
@@ -1196,13 +1228,10 @@ static int preprocess_one(rf_handle h, const char *who, const Source &src, bool 
         cudaStream_t s = h->ctx[0].stream;
         const typename Source::Src p = src.upload(h, s, 0, 0);
         LbItemT<typename Source::Src> it;
-        if (tiled) {
-            tile_fill(it, p, src.width(0), src.height(0), h->d_input, Wn, Hn, layouts[0][tile]);
-        } else {
-            int dw, dh;
-            displayed_size(src, 0, dw, dh);
-            letterbox_fill(it, p, dw, dh, h->d_input, Wn, Hn, src.bits(0), (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0);
-        }
+        int dw, dh;
+        displayed_size(src, 0, dw, dh);
+        if (tiled) tile_fill(it, p, dw, dh, src.bits(0), h->d_input, Wn, Hn, layouts[0][tile]);
+        else letterbox_fill(it, p, dw, dh, h->d_input, Wn, Hn, src.bits(0), (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0);
         CK(launch_letterbox_batch(&it, 1, Wn, Hn, s));
         CK(cudaMemcpyAsync(h->h_input, h->d_input, (size_t)Hn * Wn * 3, cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
@@ -1229,6 +1258,14 @@ int rf_preprocess_tile(rf_handle h, const uint8_t *bgr, int width, int height, i
 }
 int rf_preprocess_yuv_tile(rf_handle h, const rf_yuv_frame *frame, int matrix, const rf_tiling *t, int tile, uint8_t *out) {
     return preprocess_one(h, "rf_preprocess_yuv_tile", YuvFrames{frame, matrix, nullptr, false}, true, t, tile, out);
+}
+int rf_preprocess_tile_oriented(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, int orientation, const rf_tiling *t,
+                                int tile, uint8_t *out) {
+    return preprocess_one(h, "rf_preprocess_tile_oriented", BgrImages{&bgr, &width, &height, &row_stride, &orientation, true}, true, t, tile, out);
+}
+int rf_preprocess_yuv_tile_oriented(rf_handle h, const rf_yuv_frame *frame, int matrix, int orientation, const rf_tiling *t, int tile,
+                                    uint8_t *out) {
+    return preprocess_one(h, "rf_preprocess_yuv_tile_oriented", YuvFrames{frame, matrix, &orientation, true}, true, t, tile, out);
 }
 
 // ---- f1 ingest: compressed images (main.cpp:18-26 decodes on the host with cv::imread) ---------------------------------------

@@ -362,12 +362,15 @@ int tile_layout(int net_w, int net_h, int w, int h, const rf_tiling *t, std::vec
 }
 
 template <typename Src>
-void tile_fill(LbItemT<Src> &it, typename LbItemT<Src>::Source src, int w, int h, uint8_t *dst, int net_w, int net_h, const rf_tile &tile) {
+void tile_fill(LbItemT<Src> &it, typename LbItemT<Src>::Source src, int w, int h, int bits, uint8_t *dst, int net_w, int net_h,
+               const rf_tile &tile) {
+    // the LB bits act on displayed coordinates before the transpose: mirroring the displayed image flips displayed x
+    const int flip = bits ^ (tile.flip ? LB_FLIP_X : 0);
     if (tile.scale == 0.f) {          // the fitted level: the letter-box itself
-        letterbox_fill(it, src, w, h, dst, net_w, net_h, tile.flip, 0);
+        letterbox_fill(it, src, w, h, dst, net_w, net_h, flip, 0);
         return;
     }
-    it.src = src; it.dst = dst; it.sw = w; it.sh = h; it.flip = tile.flip;
+    it.src = src; it.dst = dst; it.sw = w; it.sh = h; it.flip = flip;
     it.dw = tile.scaled_w; it.dh = tile.scaled_h;
     it.scale = 1.0 / (double)tile.scale;     // cv::resize: scale_x = 1. / inv_scale_x
     it.identity = it.scale == 1.0 ? 1 : 0;
@@ -400,7 +403,7 @@ template float letterbox_fill<BgrRows>(LbItem &, BgrRows, int, int, uint8_t *, i
 template float letterbox_fill<YuvPlanes>(LbYuvItem &, YuvPlanes, int, int, uint8_t *, int, int, int, int);
 template cudaError_t launch_letterbox_batch<BgrRows>(const LbItem *, int, int, int, cudaStream_t);
 template cudaError_t launch_letterbox_batch<YuvPlanes>(const LbYuvItem *, int, int, int, cudaStream_t);
-template void tile_fill<BgrRows>(LbItem &, BgrRows, int, int, uint8_t *, int, int, const rf_tile &);
-template void tile_fill<YuvPlanes>(LbYuvItem &, YuvPlanes, int, int, uint8_t *, int, int, const rf_tile &);
+template void tile_fill<BgrRows>(LbItem &, BgrRows, int, int, int, uint8_t *, int, int, const rf_tile &);
+template void tile_fill<YuvPlanes>(LbYuvItem &, YuvPlanes, int, int, int, uint8_t *, int, int, const rf_tile &);
 
 }  // namespace rf

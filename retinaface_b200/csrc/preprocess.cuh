@@ -90,7 +90,9 @@ int tile_layout(int net_w, int net_h, int w, int h, const rf_tiling *t, std::vec
 // (rf_tracker_set_tiling; levels NULL is not one of them: the tracker takes it as the default pyramid).
 int tiling_check(int net_w, int net_h, const rf_tiling *t, std::string *err);
 // The letter-box item of one tile: the image's level resized, mirrored when the tile's level is, and cut at the tile's origin.
+// w x h is the DISPLAYED size and `bits` the image's own LB_* orientation bits (0: upright, f21); the tile's layout is that of w x h.
 template <typename Src>
-void tile_fill(LbItemT<Src> &it, typename LbItemT<Src>::Source src, int w, int h, uint8_t *dst, int net_w, int net_h, const rf_tile &tile);
+void tile_fill(LbItemT<Src> &it, typename LbItemT<Src>::Source src, int w, int h, int bits, uint8_t *dst, int net_w, int net_h,
+               const rf_tile &tile);
 
 }  // namespace rf

@@ -72,18 +72,24 @@ class RetinaFace:
         return [[(FaceDetectInfo.from_row(r), c) for r, c in zip(f, cs)] for f, cs in zip(faces, crops)]
 
     def detectTiled(self, imgs: Sequence[np.ndarray], threshold: float = 0.5, scales: Sequence[float] = None, flip: bool = False,
-                    overlap: int = 0, align: dict = None) -> List[list]:
+                    overlap: int = 0, align: dict = None, orientations: Sequence[int] = None) -> List[list]:
         """f7 small faces in large images: each image is resized to a pyramid of levels, every level cut into overlapping
         network-sized tiles, the tiles detected as ordinary batches and the faces merged across tiles and levels on the GPU
         (rf_detect_tiled).  Faces in ORIGINAL IMAGE pixels.  ``scales``: the levels (a scale may exceed 1; 0 is the letter-box of
         ``detectBatchImages``), each also run mirrored with ``flip``; None: the default pyramid 1, 1/2, 1/4, ... down to the
         letter-box; ``flip`` needs explicit ``scales`` (ValueError otherwise).  ``overlap``: pixels neighbouring tiles share (0: 64).
         With ``align`` (``Engine.detect_align``'s keywords), per image a list of ``(FaceDetectInfo, crop)`` as ``detectAndAlign``
-        returns, the crops cut from the original image (rf_detect_tiled_align)."""
+        returns, the crops cut from the original image (rf_detect_tiled_align).  ``orientations`` (f21): image i is shown in EXIF
+        orientation ``orientations[i]`` and tiled as displayed, faces and crops in DISPLAYED image pixels (rf_detect_tiled_oriented);
+        None: the images as stored."""
         if flip and scales is None:
             raise ValueError("detectTiled: flip mirrors the given scales; the default pyramid has no mirrored levels -- pass scales")
         levels = None if scales is None else [(float(s), f) for s in scales for f in ((False, True) if flip else (False,))]
-        out = self.engine.detect_tiled(list(imgs), threshold, self.nms_threshold, levels=levels, overlap=overlap, align=align)
+        if orientations is None:
+            out = self.engine.detect_tiled(list(imgs), threshold, self.nms_threshold, levels=levels, overlap=overlap, align=align)
+        else:
+            out = self.engine.detect_tiled_oriented(list(imgs), list(orientations), threshold, self.nms_threshold, levels=levels,
+                                                    overlap=overlap, align=align)
         if align is None:
             return [[FaceDetectInfo.from_row(r) for r in per] for per in out[0]]
         return [[(FaceDetectInfo.from_row(r), c) for r, c in zip(f, cs)] for f, cs in zip(out[0], out[2])]

@@ -194,6 +194,17 @@ void RetinaFace::detectYUV(const vector<Mat> &frames, int layout, float threshol
 
 void RetinaFace::detectTiled(const vector<Mat> &imgs, float threshold, const vector<float> &scales, bool flip, int overlap,
                              const AlignOptions *align) {
+    tiled(imgs, nullptr, threshold, scales, flip, overlap, align);
+}
+
+void RetinaFace::detectTiled(const vector<Mat> &imgs, const vector<int> &orientations, float threshold, const vector<float> &scales, bool flip,
+                             int overlap, const AlignOptions *align) {
+    if (orientations.size() != imgs.size()) throw std::invalid_argument("detectTiled: one orientation per image");
+    tiled(imgs, &orientations, threshold, scales, flip, overlap, align);
+}
+
+void RetinaFace::tiled(const vector<Mat> &imgs, const vector<int> *orientations, float threshold, const vector<float> &scales, bool flip,
+                       int overlap, const AlignOptions *align) {
     if (flip && scales.empty()) throw std::invalid_argument("detectTiled: flip mirrors the given scales; the default pyramid has none");
     last_.assign(imgs.size(), vector<FaceDetectInfo>());
     scales_.assign(imgs.size(), 1.f);
@@ -217,12 +228,15 @@ void RetinaFace::detectTiled(const vector<Mat> &imgs, float threshold, const vec
             if (m.empty()) throw std::runtime_error("detectTiled: empty image");
             ptrs[i] = m.data; ws[i] = m.cols; hs[i] = m.rows; strides[i] = (int)m.step;
         }
-        int rc = align ? rf_detect_tiled_align(h_, ptrs.data(), ws.data(), hs.data(), strides.data(), n, &t, threshold, nms_threshold, &p,
+        const char *who = orientations ? "rf_detect_tiled_oriented: " : align ? "rf_detect_tiled_align: " : "rf_detect_tiled: ";
+        int rc = orientations ? rf_detect_tiled_oriented(h_, ptrs.data(), ws.data(), hs.data(), strides.data(), orientations->data() + start, n, &t,
+                                                         threshold, nms_threshold, align ? &p : nullptr, out_faces_.data(), out_counts_.data(),
+                                                         nullptr, align ? crops.data() : nullptr, nullptr)
+               : align ? rf_detect_tiled_align(h_, ptrs.data(), ws.data(), hs.data(), strides.data(), n, &t, threshold, nms_threshold, &p,
                                                out_faces_.data(), out_counts_.data(), nullptr, crops.data(), nullptr)
                        : rf_detect_tiled(h_, ptrs.data(), ws.data(), hs.data(), strides.data(), n, &t, threshold, nms_threshold, out_faces_.data(),
                                          out_counts_.data(), nullptr);
-        if (rc != RF_OK)
-            throw std::runtime_error(string(align ? "rf_detect_tiled_align: " : "rf_detect_tiled: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+        if (rc != RF_OK) throw std::runtime_error(string(who) + rf_status_string(rc) + ": " + rf_last_error(h_));
         keepResults(start, n, align ? crops.data() : nullptr, per, cw, ch);
     }
 }

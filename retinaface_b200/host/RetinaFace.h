@@ -122,6 +122,11 @@ class RetinaFace {
     // (lastScale() is 1) and, with `align` (rf_detect_tiled_align), lastCrops() the crops as detectAndAlign leaves them.
     void detectTiled(const vector<Mat> &imgs, float threshold = 0.5, const vector<float> &scales = vector<float>(), bool flip = false,
                      int overlap = 0, const AlignOptions *align = nullptr);
+    // f21 small faces in rotated and mirrored images (rf_detect_tiled_oriented): detectTiled on imgs[i] shown in EXIF orientation
+    // orientations[i] (1..8), tiled as the displayed image without a rotated copy.  Afterwards lastBatchFaces() holds the faces in
+    // DISPLAYED image pixels and, with `align`, lastCrops() the crops of the displayed image.
+    void detectTiled(const vector<Mat> &imgs, const vector<int> &orientations, float threshold = 0.5, const vector<float> &scales = vector<float>(),
+                     bool flip = false, int overlap = 0, const AlignOptions *align = nullptr);
     // f9 rotated and mirrored images (rf_detect_oriented_batch): imgs[i] as stored, shown in EXIF orientation orientations[i] (1..8,
     // what cv::imread applies; rf_jpeg_exif_orientation reads it from JPEG bytes).  Afterwards lastBatchFaces() holds the faces in
     // DISPLAYED image pixels (lastScale() is 1) and, with `align`, lastCrops() the crops of the displayed image.  No rotated copy is made.
@@ -199,6 +204,9 @@ class RetinaFace {
    private:
     // faces (and, with crops, the u8 crops of the first min(count, per) faces) of images [start, start + n) of the last call
     void keepResults(size_t start, int n, const unsigned char *crops, int per, int cw, int ch);
+    // both detectTiled overloads; orientations NULL: upright images (rf_detect_tiled / rf_detect_tiled_align)
+    void tiled(const vector<Mat> &imgs, const vector<int> *orientations, float threshold, const vector<float> &scales, bool flip, int overlap,
+               const AlignOptions *align);
     void trackerCreated(bool follow = true);   // motion (and, with follow, f16's following) on a new tracker, as the options say
     void noteMotion(int n);             // lastMotion() after a tracked call of n frames
     rf_tracker makeTracker(int lookback, bool lookback_search = false);   // trackYUV's / redactYUV's tracker, as the options say

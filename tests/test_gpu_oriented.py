@@ -1,5 +1,5 @@
 """GPU (-m gpu): f9 rotated and mirrored images -- every oriented entry point against its unoriented twin run on the rotated copy
-(orient() of test_oriented_cpu.py), bit for bit: letter-box bytes, faces, anchor indices, matrices and crops; the device YUV path on
+(orient() of oracle/orient.py), bit for bit: letter-box bytes, faces, anchor indices, matrices and crops; the device YUV path on
 oriented surfaces; oriented views against host map-back; the any-orientation sweep finding the upright photo's faces on a photo
 stored sideways; invalid orientations refused with nothing written; and that nothing else changes.  Everything goes through the C ABI."""
 import ctypes as C
@@ -13,7 +13,8 @@ import pytest
 from conftest import GOLDEN, caffemodel
 from oracle.inputs import letterbox_bgr_u8
 from oracle.yuv import bgr_to_frame, frame_to_bgr
-from test_oriented_cpu import orient, orient_planes, stored_faces
+from oracle.orient import orient, orient_planes
+from test_oriented_cpu import stored_faces
 
 pytestmark = pytest.mark.gpu
 

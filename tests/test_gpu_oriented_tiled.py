@@ -1,5 +1,5 @@
 """GPU (-m gpu): f21 oriented tiled detection.  Every case runs an oriented tiled call on stored images S against the unoriented tiled
-twin on the materialised displayed copies orient(S, o) / orient_planes(S, o) (test_oriented_cpu.py's oracle) and holds them equal bit
+twin on the materialised displayed copies orient(S, o) / orient_planes(S, o) (oracle/orient.py) and holds them equal bit
 for bit: tile bytes, records, out_tile_of / anchor_index, crops and matrices.  Also: the small faces of a portrait 4K canvas that
 neither the stored-frame tiles nor the oriented letter-box find, tracking and redaction of a portrait 4K video from these records,
 calls in flight, every refusal with nothing changed, that nothing else changes, and the Python and C++ drivers."""
@@ -11,9 +11,8 @@ import numpy as np
 import pytest
 
 from conftest import GOLDEN, caffemodel
+from oracle.orient import INVERSE, orient, orient_planes, unorient_planes
 from oracle.yuv import bgr_to_frame, frame_to_bgr
-from test_oriented_cpu import orient, orient_planes
-from test_oriented_track_cpu import INVERSE, unorient_planes
 from tile_oracle import level_image, tile_bytes
 
 pytestmark = pytest.mark.gpu

@@ -1,5 +1,5 @@
 """GPU (-m gpu): f20 oriented videos in tracker calls.  Every case runs a tracker on stored frames S with a video at orientation o against
-a twin tracker at orientation 1 on the materialised displayed frames orient_planes(S, o) (test_oriented_cpu.py's oracle), and holds
+a twin tracker at orientation 1 on the materialised displayed frames orient_planes(S, o) (oracle/orient.py), and holds
 them equal bit for bit: records, out_scales, track lists, rf_tracker_debug_state, crops and matrices, and the written frames as
 orient_planes(S_out, o) == twin_out.  Also: rf_redact_yuv_oriented_device_style against rf_redact_yuv_device_style on the rotated
 copies, a portrait phone video whose faces a tracker without the orientation leaves uncovered, pitched surfaces whose padding stays
@@ -12,9 +12,8 @@ import numpy as np
 import pytest
 
 from conftest import GOLDEN, caffemodel
+from oracle.orient import orient_planes, unorient_planes
 from oracle.yuv import bgr_to_frame
-from test_oriented_cpu import orient_planes
-from test_oriented_track_cpu import unorient_planes
 
 pytestmark = pytest.mark.gpu
 

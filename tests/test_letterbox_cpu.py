@@ -9,7 +9,7 @@ import pytest
 
 from oracle import letterbox as lb
 from oracle.inputs import letterbox_bgr_u8
-from test_oriented_cpu import orient
+from oracle.orient import orient
 
 NETS = [(448, 448), (1280, 896), (416, 288), (160, 96)]      # (net_w, net_h)
 SHRINKS = (0.5, 0.25)

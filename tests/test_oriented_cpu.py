@@ -2,7 +2,8 @@
 orders), rf_jpeg_exif_orientation on those and on malformed segments, the map-back into stored pixels as the inverse of the tap
 address map A_o, the 4:2:0 plane orientation against cvtColor, and the C++ shell compiling the oriented calls (the entry points'
 signatures are checked in test_signatures_cpu.py).
-orient / orient_planes / stored_points are the test oracle the GPU tests (test_gpu_oriented.py) use too."""
+stored_points / stored_faces are the map-back oracle the GPU tests (test_gpu_oriented.py) use too; orient and orient_planes are
+oracle/orient.py's."""
 import os
 import struct
 
@@ -11,16 +12,10 @@ import numpy as np
 import pytest
 
 from conftest import GOLDEN, ROOT
+from oracle.orient import orient, orient_planes
 from oracle.yuv import bgr_to_frame, frame_to_bgr
 
 MIRRORED = {2, 4, 5, 7}
-
-
-def orient(img, o):
-    """T_o(img): the displayed image of a stored one under EXIF orientation o (what cv2.imread applies)."""
-    return np.ascontiguousarray({1: lambda a: a, 2: lambda a: a[:, ::-1], 3: lambda a: a[::-1, ::-1], 4: lambda a: a[::-1],
-                                 5: lambda a: a.swapaxes(0, 1), 6: lambda a: np.rot90(a, -1), 7: lambda a: a.swapaxes(0, 1)[::-1, ::-1],
-                                 8: lambda a: np.rot90(a, 1)}[o](img))
 
 
 def stored_of(o, x, y, w, h):
@@ -53,20 +48,6 @@ def stored_faces(o, faces, w, h):
     lx, ly = stored_points(o, faces[:, 5:10][:, perm], faces[:, 10:15][:, perm], w, h)
     out[:, 5:10], out[:, 10:15] = lx, ly
     return out
-
-
-def orient_planes(frame, layout, o):
-    """The single-buffer 4:2:0 frame of T_o applied to each plane (chroma blocks of an even-sided frame map onto chroma blocks)."""
-    rows, w = frame.shape
-    h = rows * 2 // 3
-    y = orient(frame[:h], o)
-    if layout == "nv12":
-        uv = orient(frame[h:].reshape(h // 2, w // 2, 2), o)
-        return np.ascontiguousarray(np.concatenate([y, uv.reshape(uv.shape[0], -1)], axis=0))
-    q = (h // 2) * (w // 2)
-    flat = frame[h:].reshape(-1)
-    u, v = orient(flat[:q].reshape(h // 2, w // 2), o), orient(flat[q:].reshape(h // 2, w // 2), o)
-    return np.ascontiguousarray(np.concatenate([y.reshape(-1), u.reshape(-1), v.reshape(-1)]).reshape(-1, y.shape[1]))
 
 
 def with_exif(jpeg: bytes, o: int, little: bool = True) -> bytes:

@@ -10,7 +10,7 @@ import numpy as np
 import pytest
 
 from conftest import ROOT
-from test_oriented_cpu import orient
+from oracle.orient import orient
 from test_signatures_cpu import _exact_types, _prototypes, _squash
 
 LB_FLIP_X, LB_FLIP_Y, LB_TRANSPOSE = 1, 2, 4

@@ -2,23 +2,17 @@
 orient_planes) for every orientation and layout, pitched planes included; the stored-address map the redaction kernels use (yuv.cuh
 plane_map, restated here as the header states it) against orient_planes at luma and chroma granularity; the new entry points in the
 built library and the binding's signature table; and the C++ shell compiling setVideoOrientation.
-unorient_planes is the test oracle test_gpu_oriented_track.py uses too."""
+unorient_planes and orient_planes are oracle/orient.py's."""
 import os
 
 import numpy as np
 import pytest
 
 from conftest import ROOT
-from test_oriented_cpu import orient, orient_planes
+from oracle.orient import orient, orient_planes, unorient_planes
 
 ALL = list(range(1, 9))
-INVERSE = {6: 8, 8: 6}          # every other orientation is its own inverse
 BITS = {1: 0, 2: 1, 3: 3, 4: 2, 5: 4, 6: 5, 7: 7, 8: 6}      # EXIF -> LB_FLIP_X 1 | LB_FLIP_Y 2 | LB_TRANSPOSE 4
-
-
-def unorient_planes(frame, layout, o):
-    """The stored single-buffer 4:2:0 frame S whose orient_planes(S, layout, o) is `frame` (a displayed frame)."""
-    return orient_planes(frame, layout, INVERSE.get(o, o))
 
 
 def plane_map(bits, dw, dh, pitch, step):

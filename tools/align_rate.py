@@ -9,14 +9,11 @@ rf_fence) of K steps, the same K for both, after W warm-up steps and one warm-up
 import argparse
 import json
 import os
-import subprocess
-import sys
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-import bench  # noqa: E402
+import rates
+from rates import bench
 
 
 def main():
@@ -40,22 +37,17 @@ def main():
     # one crop tensor per execution context: consecutive (overlapping) steps never write the same buffer
     crops = [torch.empty((B, eng.max_faces, 3, 112, 112), dtype=torch.float16, device="cuda") for _ in range(nctx)]
     pos = [0]
-    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+
+    def step(align):
+        s = pos[0] % ring
+        if align:
+            eng.detect_align_device(B, bench.SCORE_THR, bench.NMS_THR, crops[pos[0] % nctx].data_ptr(), fmt="rgb_f16", dev_ptr=dev[s].data_ptr())
+        else:
+            eng.detect_device(B, bench.SCORE_THR, bench.NMS_THR, dev[s].data_ptr())
+        pos[0] += 1
 
     def block(k, align):
-        torch.cuda.synchronize()
-        ev0.record(stream)
-        for _ in range(k):
-            s = pos[0] % ring
-            if align:
-                eng.detect_align_device(B, bench.SCORE_THR, bench.NMS_THR, crops[pos[0] % nctx].data_ptr(), fmt="rgb_f16", dev_ptr=dev[s].data_ptr())
-            else:
-                eng.detect_device(B, bench.SCORE_THR, bench.NMS_THR, dev[s].data_ptr())
-            pos[0] += 1
-        eng.fence()
-        ev1.record(stream)
-        torch.cuda.synchronize()
-        return ev0.elapsed_time(ev1)
+        return rates.device_ms(lambda: step(align), k, stream, eng.fence, torch.cuda.synchronize)
 
     for _ in range(args.warmup):
         block(1, True)
@@ -70,10 +62,8 @@ def main():
     d_ms = block(K, False)
     crops_step = float(np.mean([crops_per_slot[i % ring] for i in range(K)]))
     eng.close()
-    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                         capture_output=True, text=True).stdout.strip()
     print(json.dumps(dict(workload=bench.DEFAULT_WORKLOAD, crop="112x112 RGB float16 (ArcFace template), written to a torch device tensor",
-                          gpu=gpu, steps=K, images_per_s=K * B / (a_ms * 1e-3), crops_per_s=crops_step * K / (a_ms * 1e-3),
+                          gpu=rates.card(), steps=K, images_per_s=K * B / (a_ms * 1e-3), crops_per_s=crops_step * K / (a_ms * 1e-3),
                           ms_per_step=a_ms / K, detect_only=dict(images_per_s=K * B / (d_ms * 1e-3), ms_per_step=d_ms / K),
                           align_us_per_step=(a_ms - d_ms) / K * 1e3,
                           timing="device-timed (CUDA events, rf_fence), rf_detect_align_batch_device vs rf_detect_batch_device, same inputs and K")))

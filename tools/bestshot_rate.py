@@ -8,46 +8,31 @@ the golden photo resized to 1080p, video i rolled by 8 i columns and moved 7 px 
               by rf_synchronize;
   kernel_us   microseconds per launch of k_track_update and of each k_best_* kernel, in a separate torch.profiler run (CUPTI's
               device timestamps), and the mean faces per frame;
-and the card's name and power limit, read in the same command.  The videos loop over 16 frames, so tracks live on and the best-shot
-store is exercised on every frame; best_cost is 1 - (detect + track + best) / (detect + track).
+and the card's name, power limit and maximum SM clock, read in the same command.  The videos loop over 16 frames, so tracks live on
+and the best-shot store is exercised on every frame; best_cost is 1 - (detect + track + best) / (detect + track).
 
     python tools/bestshot_rate.py [--min-seconds S] [--warmup W] [--rounds R]
 """
-import argparse
 import json
 import os
-import subprocess
-import sys
-import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-import bench  # noqa: E402
+import rates
+from rates import bench
 
-W, H, B, FRAMES = 1920, 1080, 8, 16
+B, FRAMES = 8, 16
+KERNELS = ("k_track_update", "k_best_measure", "k_best_select", "k_best_emit", "k_best_commit")
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--min-seconds", type=float, default=0.5)
-    ap.add_argument("--warmup", type=int, default=10)
-    ap.add_argument("--rounds", type=int, default=3)
-    args = ap.parse_args()
-    import cv2
+    args = rates.args(warmup=10).parse_args()
     import torch
     from torch.profiler import ProfilerActivity, profile
-    from oracle.yuv import bgr_to_frame
     from retinaface_b200 import RF_PREC_FP16, Engine
-    base = cv2.resize(cv2.imread(os.path.join(bench.GOLD, "data", "img.jpg")), (W - 7 * FRAMES, H))
-    frames = []
-    for t in range(FRAMES):
-        img = np.full((H, W, 3), 128, np.uint8)
-        img[:, 7 * t:7 * t + base.shape[1]] = base
-        frames.append([torch.from_numpy(bgr_to_frame(np.roll(img, 8 * i, axis=1), "nv12")).cuda() for i in range(B)])
+    frames = [[torch.from_numpy(f).cuda() for f in fr] for fr in rates.videos_1080p(B, FRAMES)]
     eng = Engine(os.path.join(bench.GOLD, "weights", "mnet25.caffemodel"), 448, 448, precision=RF_PREC_FP16, max_batch=B, max_faces=256,
-                 max_image=(H, W))
+                 max_image=(1080, 1920))
     trk = eng.tracker(max_videos=B)
     best = eng.tracker(max_videos=B, best=dict())
     crops = torch.empty((B, 8, 112, 112, 3), dtype=torch.uint8, device="cuda")
@@ -65,36 +50,17 @@ def main():
         "detect+track+crops": lambda: trk.detect_yuv_device(nxt(), vids, thr, nms, align=dict(max_faces=8), dev_crops_ptr=crops.data_ptr()),
         "detect+track+best": lambda: best.detect_yuv_best_device(nxt(), vids, thr, nms, shots.data_ptr()),
     }
-    for fn in runs.values():
-        for _ in range(args.warmup):
-            fn()
-    eng.synchronize()
-    rates = {k: [] for k in runs}
-    for _ in range(args.rounds):
-        for k, fn in runs.items():
-            n, t0 = 0, time.perf_counter()
-            while True:
-                fn()
-                n += 1
-                if time.perf_counter() - t0 >= args.min_seconds:
-                    break
-            eng.synchronize()
-            rates[k].append(B * n / (time.perf_counter() - t0))
+    med, per_round, _ = rates.alternate(runs, args.rounds, lambda fn: rates.host_rate(fn, eng.synchronize, args.min_seconds, args.warmup, B))
     d, c, _ = eng.detect_yuv_device(frames[0], thr, nms)
     faces = float(np.mean([len(f) for f in eng.read_dets(d, c, B)[0]]))
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         for _ in range(50):
             runs["detect+track+best"]()
         eng.synchronize()
-    kernel_us, launches = {}, {}
-    for name in ("k_track_update", "k_best_measure", "k_best_select", "k_best_emit", "k_best_commit"):
-        ks = [e for e in prof.events() if name in e.name]
-        kernel_us[name] = round(sum(e.device_time for e in ks) / len(ks), 2) if ks else None
-        launches[name] = len(ks)
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
-    med = {k: round(float(np.median(v)), 1) for k, v in rates.items()}
-    print(json.dumps(dict(frames_per_s=med, rounds=rates, best_cost=round(1 - med["detect+track+best"] / med["detect+track"], 4),
-                          kernel_us=kernel_us, launches=launches, faces_per_frame=faces, gpu=smi.stdout.strip())))
+    us, launches = rates.kernel_us(prof, KERNELS)
+    med = {k: round(v, 1) for k, v in med.items()}
+    print(json.dumps(dict(frames_per_s=med, rounds=per_round, best_cost=round(1 - med["detect+track+best"] / med["detect+track"], 4),
+                          kernel_us={k: None if t is None else round(t, 2) for k, t in us.items()}, launches=launches, faces_per_frame=faces, gpu=rates.card())))
     best.close()
     trk.close()
     eng.close()

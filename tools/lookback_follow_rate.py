@@ -11,53 +11,38 @@ into separate out surfaces.  Prints one JSON line with
   kernel_us     mean microseconds per launch, on follow calls and on detect calls apart, of k_lookback_log, k_lookback_swap,
                 k_lookback_boxes and the redaction kernels, and of f16's k_follow_search / k_follow_update / k_follow_cut, at k = 3 in a
                 separate torch.profiler run (one k_lookback_log launch per call: the j-th is call j's);
-and the card's name and power limit, read in the same command.
+and the card's name, power limit and maximum SM clock, read in the same command.
 
     python tools/lookback_follow_rate.py [--min-seconds S] [--warmup W] [--rounds R] [--frames L] [--every 1,3,5]
 """
-import argparse
 import json
 import os
-import subprocess
-import sys
-import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-import bench  # noqa: E402
+import rates
+from rates import bench
 
-W, H, B, FRAMES = 1920, 1080, 8, 16
+B, FRAMES = 8, 16
 KERNELS = ("k_lookback_log", "k_lookback_swap", "k_lookback_boxes", "k_redact", "k_follow_search", "k_follow_update", "k_follow_cut",
            "k_track_update")
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--min-seconds", type=float, default=0.5)
-    ap.add_argument("--warmup", type=int, default=20)
-    ap.add_argument("--rounds", type=int, default=3)
+    ap = rates.args(warmup=20)
     ap.add_argument("--frames", type=int, default=15)
     ap.add_argument("--every", default="1,3,5")
     args = ap.parse_args()
     every = [int(k) for k in args.every.split(",")]
-    import cv2
     import torch
     from torch.profiler import ProfilerActivity, profile
-    from oracle.yuv import bgr_to_frame
     from retinaface_b200 import RF_PREC_FP16, Engine
-    base = cv2.resize(cv2.imread(os.path.join(bench.GOLD, "data", "img.jpg")), (W - 7 * FRAMES, H))
-    frames = []
-    for t in range(FRAMES):
-        img = np.full((H, W, 3), 128, np.uint8)
-        img[:, 7 * t:7 * t + base.shape[1]] = base
-        frames.append([torch.from_numpy(bgr_to_frame(np.roll(img, 8 * i, axis=1), "nv12")).cuda() for i in range(B)])
+    frames = [[torch.from_numpy(f).cuda() for f in fr] for fr in rates.videos_1080p(B, FRAMES)]
     out = [f.clone() for f in frames[0]]
     work = [f.clone() for f in frames[0]]
     torch.cuda.synchronize()
     eng = Engine(os.path.join(bench.GOLD, "weights", "mnet25.caffemodel"), 448, 448, precision=RF_PREC_FP16, max_batch=B, max_faces=256,
-                 max_image=(H, W))
+                 max_image=(1080, 1920))
     L = args.frames
     modes = [("lookback", 1)] + [(kind, k) for k in every for kind in ("lbfollow", "f16")]
     trackers = {}
@@ -85,21 +70,10 @@ def main():
             trk.detect_yuv_redact_lookback_device(f, vids, out, thr, nms)
         else:
             trk.follow_redact_lookback_device(f, vids, out)
-    for m in modes:
-        for _ in range(max(args.warmup, L + 2)):
-            call(m)
-    eng.synchronize()
-    rates = {m: [] for m in modes}
-    for _ in range(args.rounds):
-        for m in modes:
-            n, t0 = 0, time.perf_counter()
-            while True:
-                call(m)
-                n += 1
-                if time.perf_counter() - t0 >= args.min_seconds:
-                    break
-            eng.synchronize()
-            rates[m].append(B * n / (time.perf_counter() - t0))
+    label = {m: m[0] if m[0] == "lookback" else f"{m[0]} {m[1]}" for m in modes}
+    warmup = max(args.warmup, L + 2)
+    med, per_round, _ = rates.alternate({label[m]: lambda m=m: call(m) for m in modes}, args.rounds,
+                                        lambda fn: rates.host_rate(fn, eng.synchronize, args.min_seconds, warmup, B))
     kp = ("lbfollow", 3 if 3 in every else every[-1])
     step[kp] += -step[kp] % kp[1]          # the profiled run starts on a detect call
     ncalls = 20 * kp[1]
@@ -124,12 +98,10 @@ def main():
             j = min(max(j, 0), ncalls - 1)
             per["detect" if j % kp[1] == 0 else "follow"].append(e.device_time)
         kernel_us[name] = {c: dict(mean_us=round(float(np.mean(v)), 2), launches=len(v)) for c, v in per.items() if v}
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
-    name = {m: m[0] if m[0] == "lookback" else f"{m[0]} {m[1]}" for m in modes}
-    med = {name[m]: round(float(np.median(v)), 1) for m, v in rates.items()}
-    speed = {name[m]: round(med[name[m]] / med["lookback"], 3) for m in modes if m[0] == "lbfollow"}
-    print(json.dumps(dict(frames_per_s=med, speedup_over_lookback=speed, rounds={name[m]: v for m, v in rates.items()}, L=L,
-                          profiled_every=kp[1], kernel_us=kernel_us, gpu=smi.stdout.strip())))
+    med = {k: round(v, 1) for k, v in med.items()}
+    speed = {label[m]: round(med[label[m]] / med["lookback"], 3) for m in modes if m[0] == "lbfollow"}
+    print(json.dumps(dict(frames_per_s=med, speedup_over_lookback=speed, rounds=per_round, L=L,
+                          profiled_every=kp[1], kernel_us=kernel_us, gpu=rates.card())))
     for t in trackers.values():
         t.close()
     eng.close()

@@ -12,22 +12,17 @@ mnet25 FP16 handle, mosaic + rect, L = --frames.  Prints one JSON line with
               step of that chain is OK (these frames jump back every 16 calls, so chains stop early); one_chain_us is the launch of
               a call on one video whose faces are born after L frames of 3 px steps, with at least one chain of L OK steps (its
               chains run side by side, so this bounds one such chain from above), against L x k_follow_search;
-and the card's name and power limit, read in the same command.
+and the card's name, power limit and maximum SM clock, read in the same command.
 
     python tools/lookback_search_rate.py [--min-seconds S] [--warmup W] [--rounds R] [--frames L]
 """
-import argparse
 import json
 import os
-import subprocess
-import sys
-import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-import bench  # noqa: E402
+import rates
+from rates import bench
 
 W, H, B, FRAMES = 1920, 1080, 8, 16
 KERNELS = ("k_lookback_search", "k_lookback_log", "k_lookback_swap", "k_lookback_boxes", "k_follow_search")
@@ -36,10 +31,7 @@ REPEATS = 5
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--min-seconds", type=float, default=0.5)
-    ap.add_argument("--warmup", type=int, default=20)
-    ap.add_argument("--rounds", type=int, default=3)
+    ap = rates.args(warmup=20)
     ap.add_argument("--frames", type=int, default=15)
     args = ap.parse_args()
     import cv2
@@ -47,13 +39,7 @@ def main():
     from torch.profiler import ProfilerActivity, profile
     from oracle.yuv import bgr_to_frame
     from retinaface_b200 import RF_PREC_FP16, Engine
-    photo = cv2.imread(os.path.join(bench.GOLD, "data", "img.jpg"))
-    base = cv2.resize(photo, (W - 7 * FRAMES, H))
-    frames = []
-    for t in range(FRAMES):
-        img = np.full((H, W, 3), 128, np.uint8)
-        img[:, 7 * t:7 * t + base.shape[1]] = base
-        frames.append([torch.from_numpy(bgr_to_frame(np.roll(img, 8 * i, axis=1), "nv12")).cuda() for i in range(B)])
+    frames = [[torch.from_numpy(f).cuda() for f in fr] for fr in rates.videos_1080p(B, FRAMES)]
     out = [f.clone() for f in frames[0]]
     torch.cuda.synchronize()
     weights = os.path.join(bench.GOLD, "weights", "mnet25.caffemodel")
@@ -72,21 +58,12 @@ def main():
         t = thr if key[0] == "steady" else (1.0 if (s // SPAN) % 2 == 0 else 0.5)
         trackers[key].detect_yuv_redact_lookback_device(frames[s % FRAMES], vids, out, t, nms)
 
-    for key in trackers:
-        for _ in range(max(args.warmup, L + 2 * SPAN + 2)):
+    def cycle(key):         # the timed unit is one threshold cycle of 2 SPAN calls, so every rate spans whole cycles
+        for _ in range(2 * SPAN):
             call(key)
-        eng.synchronize()
-    rates = {f"{w}/{k}": [] for w, k in trackers}
-    for _ in range(args.rounds):
-        for key in trackers:
-            n, t0 = 0, time.perf_counter()
-            while True:
-                call(key)
-                n += 1
-                if time.perf_counter() - t0 >= args.min_seconds and n % (2 * SPAN) == 0:
-                    break
-            eng.synchronize()
-            rates[f"{key[0]}/{key[1]}"].append(B * n / (time.perf_counter() - t0))
+    warmup = -(-max(args.warmup, L + 2 * SPAN + 2) // (2 * SPAN))
+    med, per_round, _ = rates.alternate({f"{w}/{k}": lambda key=(w, k): cycle(key) for w, k in trackers}, args.rounds,
+                                        lambda fn: rates.host_rate(fn, eng.synchronize, args.min_seconds, warmup, 2 * SPAN * B))
     fol = eng.tracker(max_videos=B, follow=True)
     fol.detect_yuv_device(frames[0], vids, thr, nms)
     key = ("birth_heavy", "search")
@@ -101,10 +78,7 @@ def main():
         for s in range(4 * SPAN):
             fol.follow_device(frames[(s + 1) % FRAMES], vids)
         eng.synchronize()
-    kernel_us = {}
-    for k in KERNELS:
-        ks = [ev for ev in prof.events() if k in ev.name]
-        kernel_us[k] = sum(ev.device_time for ev in ks) / len(ks) if ks else None
+    kernel_us, _ = rates.kernel_us(prof, KERNELS)
     # one k_lookback_search launch per call (8 frames <= LOOKBACK_SEARCH_FRAMES), in issue order
     search = sorted((ev for ev in prof.events() if "k_lookback_search" in ev.name), key=lambda ev: ev.time_range.start)
     assert len(search) == len(calls), (len(search), len(calls))
@@ -112,7 +86,7 @@ def main():
     with_births = [x["us"] for x in launches if x["chains"]]
     # one video whose faces move 3 px per frame, records withheld on its first L frames: each face is born on frame L and its
     # chain has L steps; the launch of that call, repeated after a reset, is the one-chain measurement
-    lin_base = cv2.resize(photo, (W - 3 * (L + 1), H))
+    lin_base = cv2.resize(cv2.imread(os.path.join(bench.GOLD, "data", "img.jpg")), (W - 3 * (L + 1), H))
     lin = []
     for t in range(L + 1):
         img = np.full((H, W, 3), 128, np.uint8)
@@ -135,15 +109,14 @@ def main():
             single.append(dict(us=ev[0].device_time, chains=int((lens > 0).sum()), full_ok_chains=len(full)))
     one.close()
     full_us = [x["us"] for x in single if x["full_ok_chains"]]
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
-    med = {k: round(float(np.median(v)), 1) for k, v in rates.items()}
+    med = {k: round(v, 1) for k, v in med.items()}
     share = {w: round(med[f"{w}/search"] / med[f"{w}/plain"], 4) for w in ("steady", "birth_heavy")}
     follow_L = L * kernel_us["k_follow_search"] if kernel_us["k_follow_search"] else None
-    print(json.dumps(dict(frames_per_s=med, rounds=rates, search_share=share, L=L, kernel_us=kernel_us, search_launches=launches,
+    print(json.dumps(dict(frames_per_s=med, rounds=per_round, search_share=share, L=L, kernel_us=kernel_us, search_launches=launches,
                           search_us_with_births=float(np.mean(with_births)) if with_births else None, one_chain_launches=single,
                           one_chain_us=float(np.mean(full_us)) if full_us else None, L_x_follow_search_us=follow_L,
                           one_chain_over_L_follow=float(np.mean(full_us)) / follow_L if full_us and follow_L else None,
-                          gpu=smi.stdout.strip())))
+                          gpu=rates.card())))
     for t in list(trackers.values()) + [fol]:
         t.close()
     eng.close()

@@ -8,33 +8,24 @@ one JSON line with
               rf_synchronize;
   kernel_us   microseconds per launch of k_motion_thumb, k_motion_match, k_motion_fit and k_motion_commit (and k_track_update) in a
               separate torch.profiler run, and their sum per 8-frame call;
-and the card's name and power limit, read in the same command.
+and the card's name, power limit and maximum SM clock, read in the same command.
 
     python tools/motion_rate.py [--min-seconds S] [--warmup W] [--rounds R]
 """
-import argparse
 import json
 import os
-import subprocess
-import sys
-import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-import bench  # noqa: E402
+import rates
+from rates import bench
 
 W, H, B, FRAMES = 1920, 1080, 8, 16
 KERNELS = ("k_motion_thumb", "k_motion_match", "k_motion_fit", "k_motion_commit", "k_track_update")
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--min-seconds", type=float, default=0.5)
-    ap.add_argument("--warmup", type=int, default=10)
-    ap.add_argument("--rounds", type=int, default=3)
-    args = ap.parse_args()
+    args = rates.args(warmup=10).parse_args()
     import cv2
     import torch
     from torch.profiler import ProfilerActivity, profile
@@ -67,37 +58,18 @@ def main():
         "detect+track": lambda: plain.detect_yuv_device(nxt(), vids, thr, nms),
         "detect+track+motion": lambda: moving.detect_yuv_device(nxt(), vids, thr, nms),
     }
-    for fn in runs.values():
-        for _ in range(args.warmup):
-            fn()
-    eng.synchronize()
-    rates = {k: [] for k in runs}
-    for _ in range(args.rounds):
-        for k, fn in runs.items():
-            n, t0 = 0, time.perf_counter()
-            while True:
-                fn()
-                n += 1
-                if time.perf_counter() - t0 >= args.min_seconds:
-                    break
-            eng.synchronize()
-            rates[k].append(B * n / (time.perf_counter() - t0))
+    med, per_round, _ = rates.alternate(runs, args.rounds, lambda fn: rates.host_rate(fn, eng.synchronize, args.min_seconds, args.warmup, B))
     calls = 50
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         for _ in range(calls):
             runs["detect+track+motion"]()
         eng.synchronize()
-    us, launches = {}, {}
-    for k in KERNELS:
-        ev = [e for e in prof.events() if k in e.name]
-        launches[k] = len(ev)
-        us[k] = sum(e.device_time for e in ev) / max(len(ev), 1) if ev else None
+    us, launches = rates.kernel_us(prof, KERNELS)
     per_call = sum(us[k] * launches[k] for k in KERNELS[:4] if us[k]) / calls
     status = moving.motion(B)["status"].tolist()
-    med = {k: round(float(np.median(v)), 1) for k, v in rates.items()}
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
-    print(json.dumps(dict(frames_per_s=med, rounds=rates, motion_cost=round(1 - med["detect+track+motion"] / med["detect+track"], 4),
-                          kernel_us=us, launches=launches, motion_us_per_call=per_call, last_status=status, gpu=smi.stdout.strip())))
+    med = {k: round(v, 1) for k, v in med.items()}
+    print(json.dumps(dict(frames_per_s=med, rounds=per_round, motion_cost=round(1 - med["detect+track+motion"] / med["detect+track"], 4),
+                          kernel_us=us, launches=launches, motion_us_per_call=per_call, last_status=status, gpu=rates.card())))
     plain.close()
     moving.close()
     eng.close()

@@ -11,43 +11,22 @@ alternated) of
   motion         a motion tracker's rf_detect_yuv_track_device;
   lookback15     rf_detect_yuv_redact_lookback_device at L = 15 (mosaic) into separate out frames;
   follow_k3      a follow tracker detecting every 3rd call and following the others (rf_track_follow_device);
-each mode's oriented / portrait ratio, the card's name and power limit read in the same command, and, from a separate torch.profiler
+each mode's oriented / portrait ratio, the card's name, power limit and maximum SM clock read in the same command, and, from a separate torch.profiler
 run, the device time per launch of the redaction apply and blur, motion thumbnail and follow search kernels in their oriented and
 upright instantiations.
 
     python tools/oriented_track_rate.py [--min-seconds S] [--warmup W] [--rounds R]
 """
-import argparse
 import json
 import os
-import subprocess
-import sys
-import time
 from collections import defaultdict
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-import bench  # noqa: E402
+import rates
+from rates import bench
 
 W, H, B, O = 1920, 1080, 8, 6
-
-
-def rate(fn, sync, min_s, warmup):
-    """Frames per second of fn() (one call = B frames), host clock over >= min_s of calls ended by sync()."""
-    for _ in range(warmup):
-        fn()
-    sync()
-    k, t0 = 0, time.perf_counter()
-    while True:
-        fn()
-        k += 1
-        if time.perf_counter() - t0 >= min_s:
-            break
-    sync()
-    return B * k / (time.perf_counter() - t0)
 
 
 def cycle(k, detect, follow):
@@ -61,17 +40,13 @@ def cycle(k, detect, follow):
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--min-seconds", type=float, default=0.5)
-    ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--rounds", type=int, default=3)
-    args = ap.parse_args()
+    args = rates.args().parse_args()
     import cv2
     import torch
     from torch.profiler import ProfilerActivity, profile
     from oracle.yuv import bgr_to_frame
+    from oracle.orient import unorient_planes
     from retinaface_b200 import RF_PREC_FP16, Engine
-    from test_oriented_track_cpu import unorient_planes
     canvas = np.full((W, H, 3), 128, np.uint8)          # displayed: H wide, W tall
     g = cv2.resize(cv2.imread(os.path.join(bench.GOLD, "data", "img.jpg")), None, fx=0.8, fy=0.8)
     canvas[200:200 + g.shape[0], :g.shape[1]] = g[:, :H]
@@ -106,7 +81,7 @@ def main():
     for r in range(args.rounds):              # alternated: every round runs each mode on both sides, the side order swapped per round
         for mode in kinds:
             for side in (("oriented", "portrait") if r % 2 == 0 else ("portrait", "oriented")):
-                got[(mode, side)].append(rate(runs[(mode, side)], eng.synchronize, args.min_seconds, args.warmup))
+                got[(mode, side)].append(rates.host_rate(runs[(mode, side)], eng.synchronize, args.min_seconds, args.warmup, B)[0])
     eng.synchronize()
     # a separate profiled run: device time per launch of the kernels whose addressing differs
     per_launch = defaultdict(lambda: [0.0, 0])
@@ -130,15 +105,13 @@ def main():
     for t in trackers:
         t.close()
     eng.close()
-    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True,
-                         text=True).stdout.strip()
     med = {k: float(np.median(v)) for k, v in got.items()}
     out = {mode: dict(oriented_frames_per_s=round(med[(mode, "oriented")], 1), portrait_frames_per_s=round(med[(mode, "portrait")], 1),
                       ratio=round(med[(mode, "oriented")] / med[(mode, "portrait")], 4),
                       oriented_runs=[round(x, 1) for x in got[(mode, "oriented")]], portrait_runs=[round(x, 1) for x in got[(mode, "portrait")]])
            for mode in kinds}
     print(json.dumps(dict(frames=f"{B} videos x {W}x{H} NV12 BT.601 stored, shown at orientation {O}, vs {H}x{W} portrait surfaces at 1; "
-                                 "one frame of each per call", model="mnet25 FP16 448x448, default contexts", gpu=gpu, modes=out,
+                                 "one frame of each per call", model="mnet25 FP16 448x448, default contexts", gpu=rates.card(), modes=out,
                           profiled_us_per_launch={k: round(v[0] / v[1], 2) for k, v in sorted(per_launch.items())},
                           profiled_launches={k: v[1] for k, v in sorted(per_launch.items())})))
 

@@ -10,24 +10,19 @@ scale, four times) through rf_detect_yuv_tiled_device, then rf_redact_yuv_device
   kernel_us   microseconds per launch of each k_redact_* kernel (and their sum per 8-frame call) in a separate torch.profiler run, the mean
               faces per frame, and the byte floor of one call: the region pixels (1.5 bytes each) read twice and written once, over
               3.35 TB/s;
-and the card's name and power limit, read in the same command.  --style / --shape / --detail (f14) redact with that style instead
+and the card's name, power limit and maximum SM clock, read in the same command.  --style / --shape / --detail (f14) redact with that style instead
 of f12's rectangular mosaic; the runs then add detect+mosaic (the f12 call on the same records), the style's rate against it, and
 k_redact_blur's time per launch.
 
     python tools/redact_rate.py [--min-seconds S] [--warmup W] [--rounds R] [--style mosaic|blur] [--shape rect|ellipse] [--detail D]
 """
-import argparse
 import json
 import os
-import subprocess
-import sys
-import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-import bench  # noqa: E402
+import rates
+from rates import bench
 
 W, H, B, FRAMES = 1920, 1080, 8, 16
 KERNELS = ("k_redact_regions", "k_redact_measure", "k_redact_apply")
@@ -47,10 +42,7 @@ def _floor_bytes(recs, scales, w, h):
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--min-seconds", type=float, default=0.5)
-    ap.add_argument("--warmup", type=int, default=10)
-    ap.add_argument("--rounds", type=int, default=3)
+    ap = rates.args(warmup=10)
     ap.add_argument("--style", default="mosaic", choices=("mosaic", "blur"))
     ap.add_argument("--shape", default="rect", choices=("rect", "ellipse"))
     ap.add_argument("--detail", type=int, default=0)
@@ -64,12 +56,7 @@ def main():
     from oracle.yuv import bgr_to_frame
     from retinaface_b200 import RF_PREC_FP16, Engine
     photo = cv2.imread(os.path.join(bench.GOLD, "data", "img.jpg"))
-    base = cv2.resize(photo, (W - 7 * FRAMES, H))
-    frames = []
-    for t in range(FRAMES):
-        img = np.full((H, W, 3), 128, np.uint8)
-        img[:, 7 * t:7 * t + base.shape[1]] = base
-        frames.append([torch.from_numpy(bgr_to_frame(np.roll(img, 8 * i, axis=1), "nv12")).cuda() for i in range(B)])
+    frames = [[torch.from_numpy(f).cuda() for f in fr] for fr in rates.videos_1080p(B, FRAMES)]
     out = [f.clone() for f in frames[0]]
     half = cv2.resize(photo, None, fx=0.5, fy=0.5)
     big = np.full((2160, 3840, 3), 128, np.uint8)
@@ -116,21 +103,8 @@ def main():
     }
     if styled:
         runs["detect+mosaic"] = (eng, detect_mosaic)
-    for e, fn in runs.values():
-        for _ in range(args.warmup):
-            fn()
-        e.synchronize()
-    rates = {k: [] for k in runs}
-    for _ in range(args.rounds):
-        for k, (e, fn) in runs.items():
-            n, t0 = 0, time.perf_counter()
-            while True:
-                fn()
-                n += 1
-                if time.perf_counter() - t0 >= args.min_seconds:
-                    break
-            e.synchronize()
-            rates[k].append(B * n / (time.perf_counter() - t0))
+    med, per_round, _ = rates.alternate(runs, args.rounds,
+                                        lambda run: rates.host_rate(run[1], run[0].synchronize, args.min_seconds, args.warmup, B))
     d, c, sc = eng.detect_yuv_device(frames[0], thr, nms)
     recs = eng.read_dets(d, c, B)[0]
     faces = float(np.mean([len(r) for r in recs]))
@@ -144,18 +118,14 @@ def main():
             for _ in range(50):
                 fn()
             e.synchronize()
-        per = {}
-        for k in kernels:
-            ks = [ev for ev in prof.events() if k in ev.name]
-            per[k] = sum(ev.device_time for ev in ks) / len(ks) if ks else None
+        per, _ = rates.kernel_us(prof, kernels)
         per["per_call"] = sum(v for v in per.values() if v is not None)
         kernel_us[name] = per
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
-    med = {k: round(float(np.median(v)), 1) for k, v in rates.items()}
-    res = dict(frames_per_s=med, rounds=rates, redact_share={k: round(med[k + "+redact"] / med[k], 4) for k in ("detect", "track", "tiled")},
+    med = {k: round(v, 1) for k, v in med.items()}
+    res = dict(frames_per_s=med, rounds=per_round, redact_share={k: round(med[k + "+redact"] / med[k], 4) for k in ("detect", "track", "tiled")},
                kernel_us=kernel_us, faces_per_frame=faces, faces_per_frame_4k=float(np.mean([len(r) for r in recs4k])),
                floor_bytes_per_call=floor_bytes, floor_us_per_call=floor_bytes / 3.35e12 * 1e6,
-               floor_bytes_per_call_4k=_floor_bytes(recs4k, None, 3840, 2160), gpu=smi.stdout.strip())
+               floor_bytes_per_call_4k=_floor_bytes(recs4k, None, 3840, 2160), gpu=rates.card())
     if styled:
         res["style"] = rk
         res["style_vs_mosaic"] = dict(frames=round(med["detect+redact"] / med["detect+mosaic"], 4),

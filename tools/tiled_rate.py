@@ -5,7 +5,7 @@ columns), the default pyramid (overlap 64), through rf_detect_tiled on
   - the same with streams = 1 (one context, the latency plan),
   - a 1280x896 mnet25 FP16 handle.
 Prints one JSON line with, per handle:
-  tiled       blocking calls timed with the host clock after warm-up, enough calls for about 0.5 s: images/s and tiles/s;
+  tiled       blocking calls timed with the host clock after warm-up, at least --min-seconds of calls: images/s and tiles/s;
   batch       the same images through rf_detect_batch (one letter-box each), and the cost ratio tiled / batch;
   kernels     in a separate torch.profiler run: microseconds per launch of the tile letter-box and of the merge kernel;
 and the card's name, power limit and maximum SM clock, read in the same command.
@@ -15,30 +15,13 @@ and the card's name, power limit and maximum SM clock, read in the same command.
 import argparse
 import json
 import os
-import subprocess
-import sys
-import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-import bench  # noqa: E402
+import rates
+from rates import bench
 
 W4K, H4K, B = 3840, 2160, 8
-
-
-def timed(fn, min_s, warmup):
-    for _ in range(warmup):
-        fn()
-    t = time.perf_counter()
-    fn()
-    one = time.perf_counter() - t
-    k = max(3, int(np.ceil(min_s / max(one, 1e-6))))
-    t = time.perf_counter()
-    for _ in range(k):
-        fn()
-    return (time.perf_counter() - t) / k, k
 
 
 def main():
@@ -46,19 +29,21 @@ def main():
     ap.add_argument("--min-seconds", type=float, default=0.5)
     ap.add_argument("--warmup", type=int, default=3)
     args = ap.parse_args()
-    import cv2
     import torch
     from torch.profiler import ProfilerActivity, profile
     from retinaface_b200 import RF_PREC_FP16, Engine, capi
-    base = cv2.resize(cv2.imread(os.path.join(bench.GOLD, "data", "img.jpg")), (W4K, H4K))
-    imgs = [np.roll(base, 8 * i, axis=1) for i in range(B)]
+    imgs = rates.golden_4k(B)
     model = os.path.join(bench.GOLD, "weights", "mnet25.caffemodel")
     out = {}
     for name, (nw, nh, streams) in {"448x448": (448, 448, 0), "448x448_streams1": (448, 448, 1), "1280x896": (1280, 896, 0)}.items():
         eng = Engine(model, nh, nw, precision=RF_PREC_FP16, max_batch=B, max_faces=256, max_image=(H4K, W4K), streams=streams)
         tiles = len(capi.tile_layout(nw, nh, W4K, H4K))
-        s_tiled, k_tiled = timed(lambda: eng.detect_tiled(imgs, bench.SCORE_THR, bench.NMS_THR), args.min_seconds, args.warmup)
-        s_batch, k_batch = timed(lambda: eng.detect_batch(imgs, bench.SCORE_THR, bench.NMS_THR), args.min_seconds, args.warmup)
+        # blocking calls: seconds per call is the inverse of host_rate's calls per second
+        r_tiled, k_tiled = rates.host_rate(lambda: eng.detect_tiled(imgs, bench.SCORE_THR, bench.NMS_THR), eng.synchronize, args.min_seconds,
+                                           args.warmup, 1)
+        r_batch, k_batch = rates.host_rate(lambda: eng.detect_batch(imgs, bench.SCORE_THR, bench.NMS_THR), eng.synchronize, args.min_seconds,
+                                           args.warmup, 1)
+        s_tiled, s_batch = 1 / r_tiled, 1 / r_batch
         faces, _ = eng.detect_tiled(imgs, bench.SCORE_THR, bench.NMS_THR)
         plain = eng.detect_batch(imgs, bench.SCORE_THR, bench.NMS_THR)
         torch.cuda.synchronize()
@@ -66,8 +51,7 @@ def main():
             for _ in range(3):
                 eng.detect_tiled(imgs, bench.SCORE_THR, bench.NMS_THR)
             eng.synchronize()
-        lb = [e.device_time for e in prof.events() if "k_letterbox_batch" in e.name]
-        mg = [e.device_time for e in prof.events() if "k_merge" in e.name]
+        us, launches = rates.kernel_us(prof, ["k_letterbox_batch", "k_merge"])
         out[name] = dict(
             net=f"{nw}x{nh}", streams=streams, tiles_per_image=tiles,
             tiled=dict(calls=k_tiled, ms_per_call=s_tiled * 1e3, images_per_s=B / s_tiled, tiles_per_s=B * tiles / s_tiled,
@@ -75,12 +59,10 @@ def main():
             batch=dict(calls=k_batch, ms_per_call=s_batch * 1e3, images_per_s=B / s_batch,
                        faces_per_image=float(np.mean([len(f) for f in plain]))),
             cost_ratio_tiled_over_batch=s_tiled / s_batch,
-            kernels=dict(tile_letterbox_us_per_launch=float(np.mean(lb)) if lb else None, letterbox_launches=len(lb),
-                         merge_us_per_launch=float(np.mean(mg)) if mg else None, merge_launches=len(mg)))
+            kernels=dict(tile_letterbox_us_per_launch=us["k_letterbox_batch"], letterbox_launches=launches["k_letterbox_batch"],
+                         merge_us_per_launch=us["k_merge"], merge_launches=launches["k_merge"]))
         eng.close()
-    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                         capture_output=True, text=True).stdout.strip()
-    print(json.dumps(dict(images=f"{B} x {W4K}x{H4K} S-real BGR, pageable", pyramid="default, overlap 64", model="mnet25 FP16", gpu=gpu,
+    print(json.dumps(dict(images=f"{B} x {W4K}x{H4K} S-real BGR, pageable", pyramid="default, overlap 64", model="mnet25 FP16", gpu=rates.card(),
                           **out)))
 
 

@@ -6,25 +6,23 @@ larger than twice the H100's L2, as bench.py.  Prints one JSON line:
   device      one device-timed block (CUDA events, rf_fence) of K steps each, the same K, calibrated as align_rate.py:
               rf_detect_yuv_batch_device on NV12 without and with 112x112 RGB F16 crops, and rf_detect_batch_device on the same
               frames pre-letter-boxed to BGR; the difference is the conversion + letter-box per step.
-  host        blocking calls, host clock: I420 host frames through rf_detect_yuv_batch vs 1080p BGR host images through
-              rf_detect_batch (pinned and pageable), and the CPU cv2.cvtColor a BGR caller pays first, timed on its own.
+  host        blocking calls, host clock over at least --host-seconds of calls: I420 host frames through rf_detect_yuv_batch vs 1080p
+              BGR host images through rf_detect_batch (pinned and pageable), and the CPU cv2.cvtColor a BGR caller pays first, timed
+              on its own.
   kernel      in a separate torch.profiler run: the YUV letter-box kernel's microseconds per launch (batch 8) against its byte
               floor -- the luma / chroma rows its taps touch plus the output, at the data-sheet 3.35 TB/s (not measured).
 
-    python tools/yuv_rate.py [--steps K] [--warmup W] [--host-steps H]
+    python tools/yuv_rate.py [--steps K] [--warmup W] [--host-seconds S]
 """
 import argparse
+import itertools
 import json
 import os
-import subprocess
-import sys
-import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-import bench  # noqa: E402
+import rates
+from rates import bench
 
 FW, FH = 1920, 1080
 
@@ -54,7 +52,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=0, help="timed device steps (0: calibrate to about 0.5 s)")
     ap.add_argument("--warmup", type=int, default=20)
-    ap.add_argument("--host-steps", type=int, default=20)
+    ap.add_argument("--host-seconds", type=float, default=0.5)
     args = ap.parse_args()
     import cv2
     import torch
@@ -77,25 +75,20 @@ def main():
     nctx = 8
     crops = [torch.empty((B, eng.max_faces, 3, 112, 112), dtype=torch.float16, device="cuda") for _ in range(nctx)]
     pos = [0]
-    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+
+    def step(mode):
+        s = pos[0] % ring
+        if mode == "yuv":
+            eng.detect_yuv_device(dev[s], bench.SCORE_THR, bench.NMS_THR, "nv12")
+        elif mode == "yuv_align":
+            eng.detect_yuv_device(dev[s], bench.SCORE_THR, bench.NMS_THR, "nv12", align=dict(fmt="rgb_f16"),
+                                  dev_crops_ptr=crops[pos[0] % nctx].data_ptr())
+        else:
+            eng.detect_device(B, bench.SCORE_THR, bench.NMS_THR, net[s].data_ptr())
+        pos[0] += 1
 
     def block(k, mode):
-        torch.cuda.synchronize()
-        ev0.record(stream)
-        for _ in range(k):
-            s = pos[0] % ring
-            if mode == "yuv":
-                eng.detect_yuv_device(dev[s], bench.SCORE_THR, bench.NMS_THR, "nv12")
-            elif mode == "yuv_align":
-                eng.detect_yuv_device(dev[s], bench.SCORE_THR, bench.NMS_THR, "nv12", align=dict(fmt="rgb_f16"),
-                                      dev_crops_ptr=crops[pos[0] % nctx].data_ptr())
-            else:
-                eng.detect_device(B, bench.SCORE_THR, bench.NMS_THR, net[s].data_ptr())
-            pos[0] += 1
-        eng.fence()
-        ev1.record(stream)
-        torch.cuda.synchronize()
-        return ev0.elapsed_time(ev1)
+        return rates.device_ms(lambda: step(mode), k, stream, eng.fence, torch.cuda.synchronize)
 
     modes = ("yuv", "yuv_align", "bgr_net")
     for _ in range(args.warmup):
@@ -112,23 +105,20 @@ def main():
     device = {m: dict(ms_per_step=ms[m] / K, frames_per_s=K * B / (ms[m] * 1e-3)) for m in modes}
     device["convert_letterbox_us_per_step"] = (ms["yuv"] - ms["bgr_net"]) / K * 1e3
 
-    # host ingest: blocking calls, wall clock
-    def host_rate(fn, batches):
-        fn(batches[0])
-        t = time.perf_counter()
-        for i in range(args.host_steps):
-            fn(batches[i % len(batches)])
-        return (time.perf_counter() - t) / args.host_steps
+    # host ingest: blocking calls, so seconds per call is the inverse of host_rate's calls per second
+    def host_s(fn, batches):
+        it = itertools.cycle(batches)
+        return 1 / rates.host_rate(lambda: fn(next(it)), eng.synchronize, args.host_seconds, 1, 1)[0]
 
     pin = lambda b: [torch.from_numpy(x).pin_memory().numpy() for x in b]  # noqa: E731
     hb = bgr[:2]
     hy = i420[:2]
     host = dict(
-        i420_pageable_ms=host_rate(lambda b: eng.detect_yuv(b, bench.SCORE_THR, bench.NMS_THR, "i420"), hy) * 1e3,
-        i420_pinned_ms=host_rate(lambda b: eng.detect_yuv(b, bench.SCORE_THR, bench.NMS_THR, "i420"), [pin(b) for b in hy]) * 1e3,
-        bgr_pageable_ms=host_rate(lambda b: eng.detect_batch(b, bench.SCORE_THR, bench.NMS_THR), hb) * 1e3,
-        bgr_pinned_ms=host_rate(lambda b: eng.detect_batch(b, bench.SCORE_THR, bench.NMS_THR), [pin(b) for b in hb]) * 1e3,
-        cpu_cvtcolor_i420_to_bgr_ms_per_batch=host_rate(lambda b: [cv2.cvtColor(f, cv2.COLOR_YUV2BGR_I420) for f in b], hy) * 1e3)
+        i420_pageable_ms=host_s(lambda b: eng.detect_yuv(b, bench.SCORE_THR, bench.NMS_THR, "i420"), hy) * 1e3,
+        i420_pinned_ms=host_s(lambda b: eng.detect_yuv(b, bench.SCORE_THR, bench.NMS_THR, "i420"), [pin(b) for b in hy]) * 1e3,
+        bgr_pageable_ms=host_s(lambda b: eng.detect_batch(b, bench.SCORE_THR, bench.NMS_THR), hb) * 1e3,
+        bgr_pinned_ms=host_s(lambda b: eng.detect_batch(b, bench.SCORE_THR, bench.NMS_THR), [pin(b) for b in hb]) * 1e3,
+        cpu_cvtcolor_i420_to_bgr_ms_per_batch=host_s(lambda b: [cv2.cvtColor(f, cv2.COLOR_YUV2BGR_I420) for f in b], hy) * 1e3)
 
     # kernel time, profiler on, its own run
     from torch.profiler import ProfilerActivity, profile
@@ -137,17 +127,16 @@ def main():
         for i in range(50):
             eng.detect_yuv_device(dev[i % ring], bench.SCORE_THR, bench.NMS_THR, "nv12")
         eng.synchronize()
-    ev = [e for e in prof.events() if "k_letterbox_batch" in e.name and "YuvPlanes" in e.name]
-    us = float(np.mean([e.device_time for e in ev])) if ev else float("nan")
+    kernel = "k_letterbox_batch<.*YuvPlanes"          # the letter-box instantiated for YUV planes
+    us, launches = rates.kernel_us(prof, [kernel])
+    us, launches = us[kernel], launches[kernel]
     rd, wr = letterbox_floor_bytes(H, Wd)
     floor_us = B * (rd + wr) / 3.35e12 * 1e6
     eng.close()
-    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                         capture_output=True, text=True).stdout.strip()
-    print(json.dumps(dict(workload=bench.DEFAULT_WORKLOAD, frames=f"{FW}x{FH} S-real, NV12 device / I420 host", gpu=gpu, steps=K, ring=ring,
+    print(json.dumps(dict(workload=bench.DEFAULT_WORKLOAD, frames=f"{FW}x{FH} S-real, NV12 device / I420 host", gpu=rates.card(), steps=K, ring=ring,
                           device=device, host=host,
-                          kernel=dict(yuv_letterbox_us_per_launch=us, launches=len(ev), batch=B, read_bytes_per_frame=rd, write_bytes_per_frame=wr,
-                                      floor_us_at_3_35_TBps=floor_us, share_of_floor=floor_us / us if ev else None))))
+                          kernel=dict(yuv_letterbox_us_per_launch=us, launches=launches, batch=B, read_bytes_per_frame=rd, write_bytes_per_frame=wr,
+                                      floor_us_at_3_35_TBps=floor_us, share_of_floor=floor_us / us if us else None))))
 
 
 if __name__ == "__main__":

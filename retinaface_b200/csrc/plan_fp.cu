@@ -113,6 +113,7 @@ static void (*dw2d_kernel(int N))(TcDw2dArgs) {
 void launch_tc_dwpw_2d(TcDw2dArgs a, int resident, cudaStream_t s) {
     const PersistentGrid pg = persistent_grid(a.tiles_x * a.tiles_y * a.nimg, resident);
     a.run = pg.run;
+    a.stages = std::min(a.stages, a.run + 1);       // a run of one tile has no use for a third window's shared memory
     CK_L(dw2d_kernel(a.N), dim3((unsigned)pg.grid), dim3(TC_THREADS), tc_dw2d_smem_bytes(a), s, a);
 }
 
@@ -191,16 +192,24 @@ int plan_pair_tc(Builder &B, const PairNode &p, int tin) {
     s.in = {tin}; s.out = {tpw};
     s.flops_per_img = 2.0 * oh * ow_ * C * 9 + 2.0 * oh * ow_ * C * N;
     s.bytes_per_img = ((double)ih * iw * C + (double)oh * ow_ * N) * es;
-    const int tw = dw2d_tile_w(h, C, oh, ow_, geo.nsplit);
+    int tw = dw2d_tile_w(h, C, oh, ow_, geo.nsplit);
     TcDw2dArgs g2{};            // 2-D tile geometry (independent of the batch)
     int resident = 0;
     if (tw) {
-        s.name = fmt("tc2d_dw%d+pw%d_s%d_%dto%d", i, i + 1, S, C, N);
         g2.C = C; g2.IH = ih; g2.IW = iw; g2.OH = oh; g2.OW = ow_; g2.S = S; g2.N = N;
         g2.TH = 8; g2.TW = tw;
         tc_dw2d_finish(g2);
+        // a ring of three staged windows where they fit, else two.  With several execution contexts, one CTA per SM, each
+        // over a run of ceil(tiles / SMs): the SM's other slots stay free for the other contexts' kernels (DESIGN §3: faster
+        // on the flagship than three CTAs per SM with runs a third as long, though slower as a kernel alone, so a
+        // one-context handle keeps every slot)
+        g2.stages = 3;
+        if (tc_dw2d_smem_bytes(g2) > (size_t)TC_SMEM_LIMIT) g2.stages = 2;
         resident = resident_ctas(h, (const void *)dw2d_kernel(N), TC_THREADS, tc_dw2d_smem_bytes(g2));
+        if (h->cfg.streams != 1) resident = std::min(resident, h->num_sms);
+        if (!tc_dw2d_out_fits(g2)) tw = 0;      // the output tile does not fit a consumed window: the 1-D kernel
     }
+    if (tw) s.name = fmt("tc2d_dw%d+pw%d_s%d_%dto%d", i, i + 1, S, C, N);
     s.launch = [=](const Run &r) {
         if (tw) {
             TcDw2dArgs a = g2;

@@ -20,9 +20,10 @@ struct TcDw2dArgs {
     int TH, TW;             // output tile, TH * TW <= 128, TH even
     int tiles_x, tiles_y;
     int run;                // consecutive tiles per CTA (tiles of all images numbered image-major); grid = ceil(tiles / run)
+    int stages;             // staged windows in the ring: 2 or 3 (plan_pair_tc)
     int PH, PW;             // staged window: (TH-1)*S+3 x (TW-1)*S+3   (tc_dw2d_finish)
     uint32_t lbo_a;         // group stride of the A operand, bytes (tc_dw2d_finish)
-    uint32_t mul_TW, mul_tiles_x, mul_tiles;   // fast_div multipliers (tc_dw2d_finish)
+    uint32_t mul_TW, mul_tiles_x, mul_tiles, mul_cpp;   // fast_div multipliers (tc_dw2d_finish)
     const __half *wimg;     // [C/8][N][8]
     const float *bias;      // [N]
     const float *dw_w, *dw_b;   // [9][C], [C]
@@ -44,12 +45,18 @@ inline void tc_dw2d_finish(TcDw2dArgs &a) {
     a.mul_TW = fast_div_mul((uint32_t)a.TW);
     a.mul_tiles_x = fast_div_mul((uint32_t)a.tiles_x);
     a.mul_tiles = fast_div_mul((uint32_t)(a.tiles_x * a.tiles_y));
+    a.mul_cpp = fast_div_mul((uint32_t)(a.N >> 3));
 }
+inline size_t tc_dw2d_stage_bytes(const TcDw2dArgs &a) { return (size_t)a.PH * a.PW * a.C * 2; }
+// The output tile, [128 rows][N + 8 halfs]: the 16-byte pad per row puts the 8 rows of an accumulator fragment's store in 8
+// different bank groups.  It is written into the staged window the tile has just consumed.
+inline size_t tc_dw2d_out_bytes(const TcDw2dArgs &a) { return (size_t)128 * (a.N * 2 + 16); }
+inline bool tc_dw2d_out_fits(const TcDw2dArgs &a) { return tc_dw2d_out_bytes(a) <= tc_dw2d_stage_bytes(a); }
 inline size_t tc_dw2d_smem_bytes(const TcDw2dArgs &a) {
-    return 2 * (size_t)a.PH * a.PW * a.C * 2 + (size_t)(a.C / 8) * a.lbo_a + (size_t)a.C * a.N * 2 + 128;
+    return (size_t)a.stages * tc_dw2d_stage_bytes(a) + (size_t)(a.C / 8) * a.lbo_a + (size_t)a.C * a.N * 2 + 128;
 }
 
-// resident CTAs per SM the register allocation aims at (80 registers at 3; at 4 -- 64 registers -- the persistent loop
+// resident CTAs per SM the register allocation aims at (75 registers at 3; at 4 -- 64 registers -- the persistent loop
 // spills).  The pointwise accumulator is taken in chunks of at most 32 columns.
 #ifndef RF_DW2D_OCC
 #define RF_DW2D_OCC 3
@@ -64,14 +71,15 @@ __global__ void __launch_bounds__(TC_THREADS, RF_DW2D_OCC) k_tc_dwpw_2d(const Tc
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int G = a.C >> 3, lg = 31 - __clz(G);
-    const int PH = a.PH, PW = a.PW;
+    const int PH = a.PH, PW = a.PW, ns = a.stages;
     const uint32_t lbo_a = a.lbo_a;
     const int pix = a.C * 2;             // bytes per staged pixel
     const uint32_t stage_bytes = (uint32_t)(PH * PW * pix);
-    unsigned char *sA = smem + 2 * (size_t)stage_bytes;          // behind the two staging buffers
+    unsigned char *sA = smem + (size_t)ns * stage_bytes;         // behind the staging ring
     unsigned char *sB = sA + (size_t)G * lbo_a;
     const int tiles = a.tiles_x * a.tiles_y;
-    const int t_end = min((int)blockIdx.x * a.run + a.run, tiles * a.nimg);
+    const int t_begin = (int)blockIdx.x * a.run;
+    const int t_end = min(t_begin + a.run, tiles * a.nimg);
     // tile t -> image b, output origin (oy0, ox0); a CTA's run of tiles may cross from one image into the next
     auto decode = [&](int t, int &b, int &oy0, int &ox0) {
         b = fast_div(t, a.mul_tiles);
@@ -92,96 +100,127 @@ __global__ void __launch_bounds__(TC_THREADS, RF_DW2D_OCC) k_tc_dwpw_2d(const Tc
     if (tid < a.C) s_dwb[tid] = a.dw_b[tid];
     pdl_wait();
     // ---- stage tile t's (PH x PW) input window into buffer buf: one warp per staged row, lanes over (column, channel
-    // group) -- a staged row is PW*C contiguous halfs of the input (16 B per lane, fully coalesced); outside the map: zero fill
+    // group) -- a staged row is PW*C contiguous halfs of the input (16 B per lane, fully coalesced); outside the map: zero
+    // fill.  Every call commits one cp.async group, an empty one past the end of the run, so that the window of tile t is
+    // always the group issued ns - 1 calls before the latest
     const uint32_t sS_s = tc::smem_u32(smem);
     auto stage = [&](int t, int buf) {
-        int b, oy0, ox0;
-        decode(t, b, oy0, ox0);
-        const int iy0 = oy0 * a.S - 1, ix0 = ox0 * a.S - 1;      // input coordinates of staged (0, 0)
-        // item i of a row = (column px = i / G, group g = i % G): with C = 8 G its source is src_row + 8 i halfs -- affine in i
-        const int per_row = PW << lg;
-        const int px_lo = max(0, -ix0), px_hi = min(PW, a.IW - ix0);       // columns inside the map
-        const unsigned px_n = (unsigned)max(px_hi - px_lo, 0);
-        for (int py = warp; py < PH; py += TC_THREADS / 32) {
-            const int iy = iy0 + py;
-            const bool rowok = iy >= 0 && iy < a.IH;
-            const __half *src_row = a.in + (ptrdiff_t)(((b * a.IH + (rowok ? iy : 0)) * a.IW + ix0) * a.C);
-            const uint32_t dst_row = sS_s + (uint32_t)buf * stage_bytes + (uint32_t)(py * PW * pix);
-            const __half *zsrc = a.in;      // any valid address: zero bytes are read from it
-            for (int i = lane; i < per_row; i += 32) {
-                const bool ok = rowok && (unsigned)((i >> lg) - px_lo) < px_n;
-                cp_async16_zfill_s(dst_row + (uint32_t)i * 16u, ok ? src_row + i * 8 : zsrc, ok);
+        if (t < t_end) {
+            int b, oy0, ox0;
+            decode(t, b, oy0, ox0);
+            const int iy0 = oy0 * a.S - 1, ix0 = ox0 * a.S - 1;      // input coordinates of staged (0, 0)
+            // item i of a row = (column px = i / G, group g = i % G): with C = 8 G its source is src_row + 8 i halfs -- affine in i
+            const int per_row = PW << lg;
+            const int px_lo = max(0, -ix0), px_hi = min(PW, a.IW - ix0);       // columns inside the map
+            const unsigned px_n = (unsigned)max(px_hi - px_lo, 0);
+            for (int py = warp; py < PH; py += TC_THREADS / 32) {
+                const int iy = iy0 + py;
+                const bool rowok = iy >= 0 && iy < a.IH;
+                const __half *src_row = a.in + (ptrdiff_t)(((b * a.IH + (rowok ? iy : 0)) * a.IW + ix0) * a.C);
+                const uint32_t dst_row = sS_s + (uint32_t)buf * stage_bytes + (uint32_t)(py * PW * pix);
+                const __half *zsrc = a.in;      // any valid address: zero bytes are read from it
+                for (int i = lane; i < per_row; i += 32) {
+                    const bool ok = rowok && (unsigned)((i >> lg) - px_lo) < px_n;
+                    cp_async16_zfill_s(dst_row + (uint32_t)i * 16u, ok ? src_row + i * 8 : zsrc, ok);
+                }
             }
         }
         cp_async_commit();
     };
     // ---- depthwise stencil of the window at sS -> A operand.  GEMM row r = ty * TW + tx ------------------------------------
-    // item = (channel group, pair of horizontally adjacent outputs): at stride 1 a 3x4 window feeds 2 outputs (12 conversions
-    // for 18 taps), at stride 2 a 3x5 window (15 for 18).  TW is even.  A 2x2 block (16 / 25 conversions for 36 taps) has half
-    // as many items, which leaves half the threads idle at C = 32 and three quarters at C = 16 while the stencil runs.
-    auto stencil = [&](auto s_, const unsigned char *sS) {
-        constexpr int S = decltype(s_)::value;
-        const int items = a.TH * (a.TW >> 1) << lg;
+    // item = (channel group, NX horizontally adjacent outputs).  A pair (NX = 2) at stride 1 reads a 3x4 window for 2 outputs
+    // (12 conversions for 18 taps), at stride 2 a 3x5 window (15 for 18); TW is even.  Where pairs are fewer than the threads
+    // (C = 16: 64 pairs x 2 groups) every thread takes one output instead (9 conversions for 9 taps), so that none waits at
+    // the barrier while the others compute.  A 2x2 block (16 / 25 conversions for 36 taps) has half as many items again.
+    auto stencil = [&](auto s_, auto nx_, const unsigned char *sS) {
+        constexpr int S = decltype(s_)::value, NX = decltype(nx_)::value;
+        const int items = (a.TH * a.TW / NX) << lg;
         for (int it = tid; it < items; it += TC_THREADS) {
             const int g = it & (G - 1), rest = it >> lg;
-            const int ty = fast_div(2 * rest, a.mul_TW), tx = 2 * rest - ty * a.TW;
-            float acc[1][2][8];
+            const int ty = fast_div(NX * rest, a.mul_TW), tx = NX * rest - ty * a.TW;
+            float acc[1][NX][8];
             dw_bias8(acc[0][0], &s_dwb[g * 8]);
 #pragma unroll
-            for (int i = 0; i < 8; i++) acc[0][1][i] = acc[0][0][i];
-            dw_stencil_block<S, 1, 2>(acc, sS + (ty * S * PW + tx * S) * pix + g * 16, PW * pix, pix, &s_dww[g * 8], a.C);
+            for (int q = 1; q < NX; q++)
+#pragma unroll
+                for (int i = 0; i < 8; i++) acc[0][q][i] = acc[0][0][i];
+            dw_stencil_block<S, 1, NX>(acc, sS + (ty * S * PW + tx * S) * pix + g * 16, PW * pix, pix, &s_dww[g * 8], a.C);
             unsigned char *dst = sA + (size_t)g * lbo_a + (size_t)(ty * a.TW + tx) * 16;
-            *reinterpret_cast<uint4 *>(dst) = dw_relu_h8(acc[0][0]);
-            *reinterpret_cast<uint4 *>(dst + 16) = dw_relu_h8(acc[0][1]);
+#pragma unroll
+            for (int q = 0; q < NX; q++) *reinterpret_cast<uint4 *>(dst + 16 * q) = dw_relu_h8(acc[0][q]);
         }
     };
+    const bool singles = ((a.TH * a.TW / 2) << lg) < TC_THREADS;
     const int rows = a.TH * a.TW;
     const bool has_gemm = 64 * (warp >> 2) < rows;      // the second warpgroup has no GEMM rows when TH * TW <= 64
-    const int t_begin = (int)blockIdx.x * a.run;
-    stage(t_begin, 0);
-    // ---- persistent loop over the CTA's run of tiles: tile t + 1's window is in flight while tile t computes -------------
-    for (int t = t_begin; t < t_end; t++) {
-        const int buf = (t - t_begin) & 1;
-        cp_async_wait_all();
-        // tile t's window has landed, and every thread is done with tile t - 1: its stencil has read the other staging
-        // buffer, its wgmma chains (wg::wait<0>) have read sA
+    const uint32_t ostride = (uint32_t)a.N * 2 + 16;     // bytes per row of the output tile (tc_dw2d_out_bytes)
+    const int cpp = a.N >> 3;                             // 16-byte pieces per output pixel
+    for (int j = 0; j < ns - 1; j++) stage(t_begin + j, j);
+    // ---- persistent loop over the CTA's run of tiles: the windows of tiles t + 1 .. t + ns - 1 are in flight while tile t
+    // computes.  Three barriers per tile: X (window t landed; tile t - 1's output tile read), Y (A operand written), Z
+    // (output tile written)
+    for (int t = t_begin, buf = 0; t < t_end; t++, buf = buf + 1 == ns ? 0 : buf + 1) {
+        if (ns == 3) asm volatile("cp.async.wait_group 1;" ::: "memory");
+        else asm volatile("cp.async.wait_group 0;" ::: "memory");
+        // X: every thread's pieces of window t have landed, and every thread is done with tile t - 1: its stencil read the
+        // buffer the next window goes into, its stores read that buffer's output tile
         __syncthreads();
-        if (t + 1 < t_end) stage(t + 1, buf ^ 1);
-        const unsigned char *sS = smem + (size_t)buf * stage_bytes;
-        if (a.S == 1) stencil(std::integral_constant<int, 1>{}, sS);
-        else stencil(std::integral_constant<int, 2>{}, sS);
+        stage(t + ns - 1, buf == 0 ? ns - 1 : buf - 1);
+        unsigned char *sS = smem + (size_t)buf * stage_bytes;
+        if (a.S == 1) {
+            if (singles) stencil(std::integral_constant<int, 1>{}, std::integral_constant<int, 1>{}, sS);
+            else stencil(std::integral_constant<int, 1>{}, std::integral_constant<int, 2>{}, sS);
+        } else {
+            if (singles) stencil(std::integral_constant<int, 2>{}, std::integral_constant<int, 1>{}, sS);
+            else stencil(std::integral_constant<int, 2>{}, std::integral_constant<int, 2>{}, sS);
+        }
         tc::fence_async_smem();
-        __syncthreads();
-        if (!has_gemm) continue;                     // no GEMM rows, but the next tile's barriers are reached
-        tc::mbar_wait(&bar_b, 0);
+        __syncthreads();                             // Y: the A operand is complete; window t has been read
+        if (has_gemm) {
+            tc::mbar_wait(&bar_b, 0);
+            const uint32_t a_addr = tc::smem_u32(sA) + (uint32_t)(64 * (warp >> 2)) * 16u, b_addr = tc::smem_u32(sB);
+            const uint32_t lbo_b = (uint32_t)a.N * 16;
+            // rows of this thread's fragment in the output tile, which takes the place of window t
+            unsigned char *orow0 = sS + (uint32_t)tc_frag_row() * ostride + 4 * (lane & 3);
+            wg::for_chunks<(NT < 32 ? NT : 32)>(a.N, [&](auto nc, int n0) {
+                constexpr int NC = decltype(nc)::value;
+                float d[NC / 2];                 // not zeroed: the first MMA runs with scale-d = 0 (see wg::fence)
+                wg::fence();
+                wg::mma_ss<NC>(d, wg::desc(a_addr, lbo_a, 128), wg::desc(b_addr + (uint32_t)n0 * 16u, lbo_b, 128), 0);
+                for (int ks = 1; ks < (a.C >> 4); ks++) {
+                    const uint64_t ad = wg::desc(a_addr + (uint32_t)(2 * ks) * lbo_a, lbo_a, 128);
+                    const uint64_t bd = wg::desc(b_addr + (uint32_t)(2 * ks) * lbo_b + (uint32_t)n0 * 16u, lbo_b, 128);
+                    wg::mma_ss<NC>(d, ad, bd, 1);
+                }
+                wg::commit();
+                wg::wait<0>();
+                wg::fence_regs(d);
+                // bias, ReLU and FP16 round as tc_epilogue, into the output tile
+                const int c2 = 2 * (lane & 3);
+#pragma unroll
+                for (int e = 0; e < 2; e++) {
+#pragma unroll
+                    for (int i = 0; i < NC / 8; i++) {
+                        const int n = n0 + 8 * i + c2;
+                        const float f0 = fmaxf(d[4 * i + 2 * e] + s_bias[n], 0.f), f1 = fmaxf(d[4 * i + 2 * e + 1] + s_bias[n + 1], 0.f);
+                        *reinterpret_cast<__half2 *>(orow0 + 8 * e * ostride + (n0 + 8 * i) * 2) = __floats2half2_rn(f0, f1);
+                    }
+                }
+            });
+        }
+        __syncthreads();                             // Z: the output tile is complete
+        // ---- the output tile -> global memory: an output row of the tile is TW * N contiguous halfs of the NHWC output,
+        // stored as 16-byte pieces, consecutive lanes on consecutive pieces; pixels outside the map are not stored
         int b, oy0, ox0;
         decode(t, b, oy0, ox0);
-        long orow[2];
-#pragma unroll
-        for (int e = 0; e < 2; e++) {
-            const int r = tc_frag_row() + 8 * e;
+        for (int it = tid; it < rows * cpp; it += TC_THREADS) {
+            const int r = fast_div(it, a.mul_cpp), j = it - r * cpp;
             const int ty = fast_div(r, a.mul_TW), tx = r - ty * a.TW;
             const int oy = oy0 + ty, ox = ox0 + tx;
-            orow[e] = (r < rows && oy < a.OH && ox < a.OW) ? (long)((b * a.OH + oy) * a.OW + ox) : -1;
+            if (oy >= a.OH || ox >= a.OW) continue;
+            const uint4 v = *reinterpret_cast<const uint4 *>(sS + (uint32_t)r * ostride + 16 * j);
+            *reinterpret_cast<uint4 *>(a.out + (size_t)((b * a.OH + oy) * a.OW + ox) * a.N + 8 * j) = v;
         }
-        const uint32_t a_addr = tc::smem_u32(sA) + (uint32_t)(64 * (warp >> 2)) * 16u, b_addr = tc::smem_u32(sB);
-        const uint32_t lbo_b = (uint32_t)a.N * 16;
-        const TcOut o{a.out, a.N, a.N, 1, nullptr, 0, 0};
-        wg::for_chunks<(NT < 32 ? NT : 32)>(a.N, [&](auto nc, int n0) {
-            constexpr int NC = decltype(nc)::value;
-            float d[NC / 2];                 // not zeroed: the first MMA runs with scale-d = 0 (see wg::fence)
-            wg::fence();
-            wg::mma_ss<NC>(d, wg::desc(a_addr, lbo_a, 128), wg::desc(b_addr + (uint32_t)n0 * 16u, lbo_b, 128), 0);
-            for (int ks = 1; ks < (a.C >> 4); ks++) {
-                const uint64_t ad = wg::desc(a_addr + (uint32_t)(2 * ks) * lbo_a, lbo_a, 128);
-                const uint64_t bd = wg::desc(b_addr + (uint32_t)(2 * ks) * lbo_b + (uint32_t)n0 * 16u, lbo_b, 128);
-                wg::mma_ss<NC>(d, ad, bd, 1);
-            }
-            wg::commit();
-            wg::wait<0>();
-            wg::fence_regs(d);
-            tc_epilogue<NC>(d, n0, s_bias, o, orow, 0);
-        });
     }
 }
 

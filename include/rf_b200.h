@@ -679,6 +679,44 @@ int rf_detect_yuv_track_best_device(rf_handle h, rf_tracker t, const rf_yuv_fram
 int rf_tracker_finish(rf_tracker t, int video, void *dev_best_crops, double *dev_best_mats,
                       const rf_best_shot **dev_best, const int32_t **dev_best_count);
 
+/* f22 best shots for live cameras.  A live stream has no end, so f11's shot -- emitted when the track ends -- comes too late for
+ * access control or a watch list; and f11 needs every frame detected.  Two options of a best-shot tracker, each set before its first
+ * frame call, in either order and with rf_tracker_set_motion, rf_tracker_set_tiling and rf_tracker_set_orientation.
+ *
+ * LIVE shots (rf_tracker_set_best_live).  Per frame of a video, after f11's removals and store updates, every track that is CONFIRMED
+ * after the frame and matched on it (rf_track.det >= 0; a track born CONFIRMED on a video's first frame included) is considered, with its
+ * stored best (q, frame s) and its live state: n live shots so far, the last one's q_l and the frame number e_l it was emitted on.
+ *   n == 0   the track emits when  q >= (double)first_quality && q >= (double)min_quality
+ *   n > 0    the track emits when  frame - e_l >= min_gap && q > q_l * (1.0 + (double)improve)   (the sum and the product FP64, one
+ *            rounding each)
+ * An emission is the stored shot as an EXIT shot would carry it: frame = s, end_frame = this frame, the track's hits and age after this
+ * frame, reason RF_BEST_LIVE; its crop and M go to the same buffers in the same format.  It then sets q_l = q, e_l = frame, n = n + 1.
+ * A frame's EXIT shots (removed tracks) and LIVE shots (matched tracks) are compacted together in id order.  EXIT and FINISH are
+ * unchanged: every ever-confirmed track still ends with exactly one EXIT or FINISH shot when its q clears min_quality, which may repeat
+ * its last live crop (the same id and frame), so live shots are strictly additive.  LOST and TENTATIVE tracks never emit live; an
+ * improvement held back by min_gap goes out on the track's next matched frame after the gap, or with its EXIT shot.  rf_tracker_reset
+ * and rf_tracker_finish drop the live state with the store.
+ * Bounds: at most one shot per slot per frame (removals come before births, and a birth is TENTATIVE except on a video's first frame,
+ * where nothing can be removed), so the [n][max_tracks] buffers of f11 hold every frame; and, q being at most 1, at most
+ * 1 + floor(ln(1 / first_quality) / ln(1 + improve)) live shots per track (7 with the defaults).
+ *
+ * Following (rf_tracker_set_best_follow).  f16's interval on a best-shot tracker: detect frames go through
+ * rf_detect_yuv_track_best_device exactly as on a best-shot tracker (records, lists, quality, store and shots), and f16's Cut runs on
+ * them; follow frames go through rf_track_follow_best_device: f16's follow step (lists and rf_follow records bit for bit a follow
+ * tracker's), then f11's selection with no records -- the tracks removed on the frame emit their EXIT shots as on a detect frame, and
+ * nothing is measured or stored.  Follow frames count in the frame numbers of rf_best_shot; live shots occur on detect frames only
+ * (follow frames match no records).  rf_tracker_follow returns the latest follow call's records; motion, tiling and orientation work as
+ * on the f16, f19 and f20 paths; reset and finish also drop the templates. */
+#define RF_BEST_LIVE   2     /* f22: emitted while the track lives */
+typedef struct rf_best_live_config {
+    float first_quality;     /* 0 -> 0.3; else in (0, 1] */
+    float improve;           /* 0 -> 0.2; else finite and > 0 */
+    int   min_gap;           /* frames between two live shots of one track: 0 -> 30; else 1 .. 1 << 20 */
+} rf_best_live_config;
+/* Turns live shots on.  Not a best-shot tracker, a second call, a call after the first frame call, or bad values (NaN, out of
+ * range): RF_ERR_INVALID_ARG, nothing changed. */
+int rf_tracker_set_best_live(rf_tracker t, const rf_best_live_config *cfg);
+
 /* f12 redaction: an in-place mosaic of every detected face -- and of every face the tracker still follows while the detector misses
  * it -- written into the caller's device frames, so that footage can be stored, published or annotated without its faces and no
  * frame leaves the GPU.  The calls WRITE the frames their descriptors point at (rf_yuv_frame's planes are declared const for the
@@ -1003,6 +1041,22 @@ int rf_tracker_set_lookback_follow(rf_tracker t, const rf_follow_config *cfg);
 int rf_track_follow_redact_lookback_device(rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, const rf_redact_style *style,
                                            const rf_yuv_frame *out_frames, int32_t *out_frame_numbers, const rf_track **dev_tracks,
                                            const int32_t **dev_track_counts);
+
+/* f22 following best-shot trackers (the f22 block above; here, after f16's rf_follow_config). */
+/* Makes a best-shot tracker a following one: cfg, its bounds and its template store (above 4 GiB: RF_ERR_CAPACITY) are
+ * rf_tracker_set_follow's.  Not a best-shot tracker, a second call, a call after the first frame call, or bad values:
+ * RF_ERR_INVALID_ARG, nothing changed.  rf_tracker_set_follow keeps refusing a best-shot tracker.  A following best-shot tracker takes
+ * rf_detect_yuv_track_best_device, rf_track_follow_best_device, rf_tracker_finish, rf_tracker_reset, rf_tracker_follow and its options'
+ * queries; rf_track_update, rf_detect_yuv_track_device, rf_track_follow_device and rf_track_follow_redact_device refuse it
+ * (RF_ERR_INVALID_ARG). */
+int rf_tracker_set_best_follow(rf_tracker t, const rf_follow_config *cfg);
+/* The follow step of rf_track_follow_device on n device frames (frame i of video videos[i]), then the frames' EXIT shots as above, in
+ * rf_detect_yuv_track_best_device's outputs and buffers (dev_best_crops required when n > 0).  Statuses, all before anything is
+ * launched: those of rf_track_follow_device, a tracker that is not a following best-shot tracker, a NULL dev_best_crops:
+ * RF_ERR_INVALID_ARG.  Asynchronous on rf_last_stream()'s context, inside the tracker's event chain. */
+int rf_track_follow_best_device(rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, void *dev_best_crops,
+                                double *dev_best_mats, const rf_best_shot **dev_best, const int32_t **dev_best_counts,
+                                const rf_track **dev_tracks, const int32_t **dev_track_counts);
 
 /* f19 tiled detection in the tracker: on a 448x448 network the letter-box of a 3840x2160 frame hides every face narrower than ~137
  * pixels (f7), so a tracker fed by it leaks nearly every face of 4K street footage.  A TILING tracker detects through f7 / f8's tiles

@@ -210,7 +210,11 @@ class BestShot(C.Structure):     # rf_best_shot
                [(f, C.c_float) for f in ("quality", "score", "eye", "frontal", "sharpness", "coverage")] + [("face", Face)]
 
 
-BEST_EXIT, BEST_FINISH = 0, 1                                # RF_BEST_*
+BEST_EXIT, BEST_FINISH, BEST_LIVE = 0, 1, 2                  # RF_BEST_*
+
+
+class BestLiveConfig(C.Structure):   # rf_best_live_config (f22)
+    _fields_ = [("first_quality", C.c_float), ("improve", C.c_float), ("min_gap", C.c_int)]
 BEST_DTYPE = _record_dtype(BestShot)                         # one rf_best_shot as a numpy record
 
 
@@ -376,6 +380,9 @@ _SIGNATURES = {
     "rf_tracker_set_lookback_follow": (_I, [_P, C.POINTER(FollowConfig)]),
     "rf_track_follow_redact_lookback_device": (_I, [_P, _FRAMES, _P, _I, _STYLE, _FRAMES, _P, _PP, _PP]),
     "rf_tracker_set_tiling": (_I, [_P, _TILING]),
+    "rf_tracker_set_best_live": (_I, [_P, C.POINTER(BestLiveConfig)]),
+    "rf_tracker_set_best_follow": (_I, [_P, C.POINTER(FollowConfig)]),
+    "rf_track_follow_best_device": (_I, [_P, _FRAMES, _P, _I, _P, _P, _PP, _PP, _PP, _PP]),
     "rf_tracker_set_orientation": (_I, [_P, _I, _I]),
     "rf_redact_yuv_oriented_device_style": (_I, [_P, _FRAMES, _PI, _I, _P, _P, _P, _P, _P, _P, _STYLE]),
     "rf_detect_tiled_oriented": (_I, [_P, _PP, _PI, _PI, _PI, _PI, _I, _TILING, _F, _F, _ALIGN, _P, _P, _P, _P, _P]),
@@ -1107,7 +1114,8 @@ class Engine:
     # -- f10 face tracking across video frames ---------------------------------------------------------------------------------
     def tracker(self, max_videos: int = 1, max_tracks: int = 0, high_thresh: float = 0.0, new_thresh: float = 0.0, iou_high: float = 0.0,
                 iou_low: float = 0.0, iou_tentative: float = 0.0, max_lost: int = 0, best: Optional[dict] = None,
-                motion=None, lookback=None, follow=None, lookback_search=None, lookback_follow=None, tiling=None) -> "Tracker":
+                motion=None, lookback=None, follow=None, lookback_search=None, lookback_follow=None, tiling=None, best_live=None,
+                best_follow=None) -> "Tracker":
         """rf_tracker_create: a tracker of max_videos independent sequences on this engine (0 -> the defaults of rf_track_config).
         best (``best_config`` keywords): a best-shot tracker (rf_tracker_create_best), fed through ``Tracker.detect_yuv_best_device``.
         motion (True or ``motion_config`` keywords): camera-motion compensation (rf_tracker_set_motion) from the frames of the
@@ -1118,7 +1126,10 @@ class Engine:
         tracker (rf_tracker_set_lookback_search).  lookback_follow (True or ``set_lookback_follow`` keywords, with lookback): a
         following look-back tracker (rf_tracker_set_lookback_follow), whose frames between detections go through
         ``Tracker.follow_redact_lookback_device``.  tiling (True or ``set_tiling`` keywords): a tiling tracker
-        (rf_tracker_set_tiling), whose detect calls detect through the tiles of ``detect_yuv_tiled_device``."""
+        (rf_tracker_set_tiling), whose detect calls detect through the tiles of ``detect_yuv_tiled_device``.  best_live (True or
+        ``set_best_live`` keywords, with best): live shots while tracks live (rf_tracker_set_best_live).  best_follow (True or
+        ``set_best_follow`` keywords, with best): a following best-shot tracker (rf_tracker_set_best_follow), whose frames between
+        detections go through ``Tracker.follow_best_device``."""
         t = Tracker(self, TrackConfig(max_videos, max_tracks, high_thresh, new_thresh, iou_high, iou_low, iou_tentative, max_lost),
                     best_config(**best) if best is not None else None)
         try:
@@ -1134,6 +1145,10 @@ class Engine:
                 t.set_lookback_follow(**(lookback_follow if isinstance(lookback_follow, dict) else {}))
             if tiling:
                 t.set_tiling(**(tiling if isinstance(tiling, dict) else {}))
+            if best_live:
+                t.set_best_live(**(best_live if isinstance(best_live, dict) else {}))
+            if best_follow:
+                t.set_best_follow(**(best_follow if isinstance(best_follow, dict) else {}))
         except Exception:
             t.close()
             raise
@@ -1255,6 +1270,8 @@ class Tracker:
         self.lookback_search_on = False
         self.lookback_follow_on = False
         self.tiling_on = False
+        self.best_live_on = False
+        self.best_follow_on = False
         self.max_videos = cfg.max_videos
         self.max_tracks = cfg.max_tracks or 64
 
@@ -1339,6 +1356,33 @@ class Tracker:
         raw = self.engine._fetch(best_ptr, BEST_DTYPE, n, self.max_tracks)
         counts = self.engine._fetch(counts_ptr, np.int32, n)
         return [raw[i, :counts[i]].copy() for i in range(n)]
+
+    def set_best_live(self, first_quality: float = 0.0, improve: float = 0.0, min_gap: int = 0):
+        """rf_tracker_set_best_live, on a best-shot tracker before the first frame call: emit a track's stored shot while it lives
+        (RF_BEST_LIVE) once q >= first_quality (0 -> 0.3), then whenever q beats the last live shot's by the factor 1 + improve (0 ->
+        0.2) at least min_gap (0 -> 30) frames later."""
+        cfg = BestLiveConfig(float(first_quality), float(improve), int(min_gap))
+        self.engine._check(self.lib.rf_tracker_set_best_live(self.t, C.byref(cfg)))
+        self.best_live_on = True
+
+    def set_best_follow(self, search: int = 0, max_mad: float = 0.0):
+        """rf_tracker_set_best_follow, on a best-shot tracker before the first frame call: cut f16's templates on the detect frames so
+        that the frames in between can go through ``follow_best_device`` (search: R in template pixels, 0 -> 8; max_mad: 0 -> 24)."""
+        cfg = FollowConfig(int(search), float(max_mad))
+        self.engine._check(self.lib.rf_tracker_set_best_follow(self.t, C.byref(cfg)))
+        self.best_follow_on = True
+
+    def follow_best_device(self, frames, videos: Sequence[int], dev_best_crops_ptr: int, dev_best_mats_ptr: Optional[int] = None,
+                           layout: str = "nv12"):
+        """rf_track_follow_best_device on a following best-shot tracker: follow the faces of the device 4:2:0 frames by template
+        search, then emit the EXIT shots of the tracks removed on them into dev_best_crops_ptr [n][max_tracks] (as
+        ``detect_yuv_best_device``).  Returns (best_ptr, best_counts_ptr, tracks_ptr, track_counts_ptr)."""
+        n = len(frames)
+        arr = self.engine._frames(frames, layout, True)
+        bp, bc, tp, tc = (C.c_void_p() for _ in range(4))
+        self.engine._check(self.lib.rf_track_follow_best_device(self.t, arr, self._ints(videos, n), n, dev_best_crops_ptr, dev_best_mats_ptr,
+                                                                C.byref(bp), C.byref(bc), C.byref(tp), C.byref(tc)))
+        return int(bp.value or 0), int(bc.value or 0), int(tp.value or 0), int(tc.value or 0)
 
     def set_motion(self, search: int = 0, min_inliers: int = 0):
         """rf_tracker_set_motion, before the first update."""

@@ -215,7 +215,10 @@ __device__ __forceinline__ int id_rank(const int *s_emit, int T, int id) {
 
 // One CTA per video of the call, thread i = track slot i (blockDim >= max_tracks).  Thread i carries the slot's best through the
 // call's frames: id (0: none), q, source (>= 0: the store entry as it was before the call; < 0: a scratch crop of the call) and frame.
-__global__ void k_best_select(const BestArgs a, const __grid_constant__ BestTable t) {
+// f22: LIVE adds the live policy (rf_b200.h rf_tracker_set_best_live) after each frame's store step, and emits the frame's EXIT and
+// LIVE shots together (a slot has at most one of them on a frame); SEEN false is a follow frame's launch: no records, removals only.
+template <bool LIVE, bool SEEN>
+__global__ void k_best_select(const BestArgs a, const __grid_constant__ BestTable t, const BestLiveArgs l) {
     extern __shared__ int s_dyn[];
     __shared__ int s_frame, s_count;
     const int T = a.max_tracks, F = a.max_faces, i = threadIdx.x, v = t.cta_video[blockIdx.x];
@@ -224,24 +227,28 @@ __global__ void k_best_select(const BestArgs a, const __grid_constant__ BestTabl
     const int si = v * T + i;
     int bid = 0, bsrc = si, bframe = 0;
     double bq = 0.0;
+    BestLive lv{};
     if (mine) {
         const BestEntry &e = a.store[si];
         bid = e.id;
         bq = e.m.q;
         bframe = e.frame;
+        if constexpr (LIVE) lv = l.live[si];
     }
     if (i == 0) s_frame = a.videos[v].frames;
     for (int f = 0; f < t.n; f++) {
         if (t.video[f] != v) continue;       // uniform over the CTA
         if (mine) { s_j[i] = -1; s_emit[i] = 0; }
-        for (int j = i; j < F; j += blockDim.x) a.commit[(size_t)f * F + j] = -1;
+        if constexpr (SEEN)
+            for (int j = i; j < F; j += blockDim.x) a.commit[(size_t)f * F + j] = -1;
         if (i == 0) s_count = 0;
         __syncthreads();
         const int frame = s_frame;
-        for (int j = i; j < F; j += blockDim.x) {
-            const int sl = a.seen[(size_t)f * F + j].slot;
-            if (sl >= 0) s_j[sl] = j;
-        }
+        if constexpr (SEEN)
+            for (int j = i; j < F; j += blockDim.x) {
+                const int sl = a.seen[(size_t)f * F + j].slot;
+                if (sl >= 0) s_j[sl] = j;
+            }
         // removals first: an ever-confirmed track's best is emitted if it clears min_quality
         TrackGone g{};
         int esrc = 0, eframe = 0;
@@ -259,10 +266,11 @@ __global__ void k_best_select(const BestArgs a, const __grid_constant__ BestTabl
             }
         }
         __syncthreads();
-        if (mine && s_emit[i])
-            put_emission(a, f, id_rank(s_emit, T, g.id), esrc, g.id, v, eframe, frame, g.hits, g.age, RF_BEST_EXIT);
+        if constexpr (!LIVE)
+            if (mine && s_emit[i])
+                put_emission(a, f, id_rank(s_emit, T, g.id), esrc, g.id, v, eframe, frame, g.hits, g.age, RF_BEST_EXIT);
         // then the tracks matched or born on the frame: a new track always stores, a known one only on a strictly better q
-        if (mine && s_j[i] >= 0) {
+        if (SEEN && mine && s_j[i] >= 0) {
             const size_t fj = (size_t)f * F + s_j[i];
             const int id = a.seen[fj].id;
             const double q = a.meas[fj].q;
@@ -272,6 +280,27 @@ __global__ void k_best_select(const BestArgs a, const __grid_constant__ BestTabl
                 bsrc = -1 - (int)fj;
                 bframe = frame;
             }
+        }
+        if constexpr (LIVE) {
+            // a track CONFIRMED after the frame and matched on it: its first live shot once q clears first_quality and min_quality, a
+            // further one once min_gap frames have passed and q beats the last one's by the factor 1 + improve
+            TrackLife k{};
+            bool live = false;
+            if (mine && s_j[i] >= 0) {
+                k = l.life[(size_t)f * F + s_j[i]];
+                if (k.state == RF_TRACK_CONFIRMED) {
+                    const int n = lv.id == bid ? lv.n : 0;
+                    live = n == 0 ? bq >= l.first_quality && bq >= a.min_quality : frame - lv.e >= l.min_gap && bq > lv.q * l.ratio;
+                    if (live) {
+                        lv = BestLive{bid, n + 1, frame, 0, bq};
+                        s_emit[i] = bid;
+                        atomicAdd(&s_count, 1);
+                    }
+                }
+            }
+            __syncthreads();
+            if (live) put_emission(a, f, id_rank(s_emit, T, bid), bsrc, bid, v, bframe, frame, k.hits, k.age, RF_BEST_LIVE);
+            else if (mine && s_emit[i]) put_emission(a, f, id_rank(s_emit, T, g.id), esrc, g.id, v, eframe, frame, g.hits, g.age, RF_BEST_EXIT);
         }
         __syncthreads();
         if (i == 0) {
@@ -290,6 +319,7 @@ __global__ void k_best_select(const BestArgs a, const __grid_constant__ BestTabl
         } else if (!bid) {
             a.store[si].id = 0;
         }
+        if constexpr (LIVE) l.live[si] = lv;
     }
     if (i == 0) a.videos[v].frames = s_frame;
 }
@@ -367,7 +397,8 @@ int select_threads(int T) { return (T + 31) / 32 * 32; }
 
 }  // namespace
 
-cudaError_t launch_best_frames(const BestArgs &a, const BestTable &t, cudaStream_t s) {
+// The four kernels of a detect chunk; k_best_select's instantiation from `l` (NULL: f11's).
+static cudaError_t best_frames(const BestArgs &a, const BestTable &t, const BestLiveArgs *l, cudaStream_t s) {
     if (t.n <= 0) return cudaSuccess;
     const int T = a.max_tracks;
     bool oriented = false;
@@ -376,11 +407,26 @@ cudaError_t launch_best_frames(const BestArgs &a, const BestTable &t, cudaStream
     else k_best_measure<false><<<4 * a.num_sms, BEST_THREADS, 0, s>>>(a, t);     // one wave: ~40 faces x 14 bands of a batch-8 call
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
-    k_best_select<<<t.nvideos, select_threads(T), sizeof(int) * 2 * T, s>>>(a, t);
+    if (l) k_best_select<true, true><<<t.nvideos, select_threads(T), sizeof(int) * 2 * T, s>>>(a, t, *l);
+    else k_best_select<false, true><<<t.nvideos, select_threads(T), sizeof(int) * 2 * T, s>>>(a, t, BestLiveArgs{});
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     k_best_emit<<<dim3(T, t.n), EMIT_THREADS, 0, s>>>(a);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     k_best_commit<<<a.num_sms, BEST_THREADS, 0, s>>>(a, t.n);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_best_frames(const BestArgs &a, const BestTable &t, cudaStream_t s) { return best_frames(a, t, nullptr, s); }
+
+cudaError_t launch_best_frames_live(const BestArgs &a, const BestTable &t, const BestLiveArgs &l, cudaStream_t s) { return best_frames(a, t, &l, s); }
+
+cudaError_t launch_best_follow(const BestArgs &a, const BestTable &t, cudaStream_t s) {
+    if (t.n <= 0) return cudaSuccess;
+    const int T = a.max_tracks;
+    k_best_select<false, false><<<t.nvideos, select_threads(T), sizeof(int) * 2 * T, s>>>(a, t, BestLiveArgs{});
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    k_best_emit<<<dim3(T, t.n), EMIT_THREADS, 0, s>>>(a);
     return cudaGetLastError();
 }
 

@@ -9,6 +9,8 @@
 //                   new best
 //   k_best_emit     emissions: source -> the caller's buffer, with the format conversion
 //   k_best_commit   the winning scratch crops -> the store (after the emissions read it: a slot freed and reused in one call is right)
+// f22: a live tracker's k_best_select also emits LIVE shots of the matched CONFIRMED tracks (rf_tracker_set_best_live); the follow frames
+// of a following best-shot tracker (rf_tracker_set_best_follow) run k_best_select on their removals and k_best_emit only.
 #pragma once
 #include "align.cuh"
 #include "track.cuh"
@@ -65,6 +67,22 @@ struct BestArgs {
     int *best_counts;             // [n]
 };
 
+// f22: the live state of one (video, slot): the track it belongs to (id 0 or another id: no live shot yet), its live shots so far, the
+// frame number and q of the last one.  Kept apart from BestEntry so that the store's layout is f11's.
+struct BestLive {
+    int id, n, e, pad;
+    double q;
+};
+
+// f22: the live policy's arguments, read by the live instantiation of k_best_select only.
+struct BestLiveArgs {
+    BestLive *live;               // [max_videos][max_tracks]
+    const TrackLife *life;        // [n][max_faces]
+    double first_quality;         // (double)first_quality
+    double ratio;                 // 1.0 + (double)improve, one rounding
+    int min_gap;
+};
+
 // The call's host tables: frame i belongs to video[i]; CTA b of k_best_select runs the frames of cta_video[b].
 struct BestTable {
     int n, nvideos;
@@ -75,6 +93,10 @@ struct BestTable {
 
 // The four kernels of one call of t.n <= TRACK_MAX_FRAMES frames, in order on s.
 cudaError_t launch_best_frames(const BestArgs &a, const BestTable &t, cudaStream_t s);
+// f22: launch_best_frames with the live policy of `l`.
+cudaError_t launch_best_frames_live(const BestArgs &a, const BestTable &t, const BestLiveArgs &l, cudaStream_t s);
+// f22: the t.n follow frames of a call (a.gone their removals): select and emit only -- the EXIT shots, and each video's frame count.
+cudaError_t launch_best_follow(const BestArgs &a, const BestTable &t, cudaStream_t s);
 // rf_tracker_finish: the emissions of every live, ever-confirmed track of `video` (state: its [max_tracks] slots) into a.best[0],
 // a.best_counts[0] and the caller's buffers.
 cudaError_t launch_best_finish(const BestArgs &a, int video, const TrackState *state, cudaStream_t s);

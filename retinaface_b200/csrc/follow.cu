@@ -8,7 +8,7 @@
 //                    from shared memory and each window row read as aligned words re-cut by __byte_perm for __vsadu4), the ordered
 //                    minimum as one 64-bit key, then the parabola, the box and the status on one thread.
 //   k_follow_update  one CTA per frame of the round (distinct videos): f10's predict (and f13's motion step), the follow rules, the
-//                    list, the rf_follow records and the redaction regions in id order.
+//                    list, the rf_follow records and the redaction regions in id order; f22, optionally, the removed tracks.
 //   k_follow_mask    one CTA per frame of the round, with motion: the faces the estimate must not take for the scene.
 // The bodies of k_follow_cut and k_follow_search live in search_kernels.cuh, shared with their f20 oriented twins (oriented_search.cu).
 #include <algorithm>
@@ -36,9 +36,11 @@ __global__ void __launch_bounds__(TRACK_THREADS) k_follow_update(const FollowArg
     TrackState *S = a.state + (size_t)f.video * T;
     const FollowMeas *meas = a.meas + (size_t)f.frame * T;
     const double *motion = a.motion && a.motion[f.frame].status == RF_MOTION_OK ? a.motion[f.frame].m : nullptr;
+    TrackGone *gone = a.gone ? a.gone + (size_t)f.frame * T : nullptr;
     if (tid == 0) { s_live = 0; s_regions = 0; }
     for (int i = tid; i < T; i += blockDim.x) {
         s_ok[i] = 0;
+        if (gone) gone[i].id = 0;
         s_id[i] = S[i].id;
         if (!s_id[i]) continue;
         TrackState &k = S[i];
@@ -64,6 +66,7 @@ __global__ void __launch_bounds__(TRACK_THREADS) k_follow_update(const FollowArg
             remove = k.lost > a.p.max_lost;
         }
         if (remove) {
+            if (gone) gone[i] = TrackGone{k.id, k.hits, k.age, st0 != RF_TRACK_TENTATIVE};
             k.id = 0;
             s_id[i] = 0;
         }

@@ -52,6 +52,8 @@ struct FollowArgs {
     int *mask_counts;
     int search;
     float max_mad;
+    TrackGone *gone;             // follow, optional: [n][max_tracks] the tracks removed on each frame, by slot (f22, a following best-shot
+                                 // tracker; age after the frame's increment)
 };
 
 // The templates of every track matched on the call's detect frames (after launch_track_update), one launch per TRACK_MAX_FRAMES.

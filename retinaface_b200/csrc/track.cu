@@ -249,6 +249,7 @@ __global__ void __launch_bounds__(TRACK_THREADS) k_track_update(const TrackArgs 
             r.age = k.age;
             r.lost_frames = k.lost;
             r.followed = 0;
+            if (a.life && k.det >= 0) a.life[(size_t)f * F + k.det] = TrackLife{k.hits, k.age, k.state, 0};
             double b[4];
             box_of(k.m, b);
             r.kx1 = (float)b[0]; r.ky1 = (float)b[1]; r.kx2 = (float)b[2]; r.ky2 = (float)b[3];
@@ -293,6 +294,7 @@ cudaError_t launch_track_update(const TrackArgs &a, const int *videos, const flo
         }
         if (a.seen) c.seen = a.seen + (size_t)i0 * F;
         if (a.gone) c.gone = a.gone + (size_t)i0 * T;
+        if (a.life) c.life = a.life + (size_t)i0 * F;
         if (a.motion) c.motion = a.motion + i0;
         k_track_update<<<t.nvideos, TRACK_THREADS, smem, s>>>(c, t);
         cudaError_t e = cudaGetLastError();

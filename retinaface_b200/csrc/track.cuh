@@ -51,6 +51,11 @@ struct TrackSeen {
     rf_face face;                // the record in frame pixels, as the track keeps it
 };
 
+// f22: a track matched or born on a frame, after the frame, at the index of its record (where TrackSeen has it).
+struct TrackLife {
+    int hits, age, state, pad;
+};
+
 // f11: a track removed on a frame, at its slot; id 0: the slot lost no track.
 struct TrackGone {
     int id, hits, age, confirmed;   // confirmed: the track was CONFIRMED at some point (its state at frame start was not TENTATIVE)
@@ -72,6 +77,7 @@ struct TrackArgs {
     TrackSeen *seen;             // optional [n][max_faces]: every record's track on the frame (f11)
     TrackGone *gone;             // optional [n][max_tracks]: the tracks removed on the frame, by slot (f11)
     const rf_motion *motion;     // optional [n]: each frame's camera motion (f13), applied after predict when RF_MOTION_OK
+    TrackLife *life;             // optional [n][max_faces]: with seen, each seen record's track after the frame (f22 live shots)
 };
 
 // n frames (videos[i], scales[i]; scales NULL: 1), one launch per TRACK_MAX_FRAMES of them, in stream order on s.

@@ -1,5 +1,6 @@
 // tracker.cu -- the video tracker behind include/rf_b200.h: f10 tracking, f11 best shots, f13 camera motion, f16 following, f12 / f14
-// redaction, f15 look-back, f17 searching look-back, f18 following look-back, f19 tiling and f20 oriented videos.  Detection itself is
+// redaction, f15 look-back, f17 searching look-back, f18 following look-back, f19 tiling, f20 oriented videos and f22 live and following
+// best shots.  Detection itself is
 // engine.cu's (yuv_device_impl).
 // The entry points take their C linkage from rf_b200.h.
 #include <array>
@@ -21,7 +22,8 @@
 // waits for it.
 //
 // A tracker is of one kind: plain, best-shot (f11), follow (f16) or look-back (f15).  Camera motion (f13) is an option of any kind,
-// the look-back search (f17) and following (f18) options of a look-back tracker.  admit() decides from them which calls it takes.
+// the look-back search (f17) and following (f18) options of a look-back tracker, live shots and following (f22) options of a best-shot
+// tracker.  admit() decides from them which calls it takes.
 enum Kind { PLAIN, BEST, FOLLOW, LOOKBACK };
 
 struct rf_tracker_s {
@@ -56,6 +58,11 @@ struct rf_tracker_s {
     // per-call tables serves them all; only the emitted records live in the ring.
     BestArgs ba{};                     // store, per-video counters, per-call tables, formats (per-call pointers set per call)
     bool updated = false;              // a frame call was issued (rf_tracker_set_motion comes before)
+    // f22 options of a BEST tracker: live shots (bl: the live state and the per-call track table, allocated with the option) and
+    // following (f16's store below, and the follow frames' removals d_fgone [max_batch][max_tracks]).
+    bool best_live = false, best_follow = false;
+    BestLiveArgs bl{};
+    TrackGone *d_fgone = nullptr;
     // f13 camera motion (motion.cuh); `motion` false: none of these allocated.  mref mirrors on the host what each video's
     // reference slot holds (the frame size it came from, 0 x 0: none): calls, resets and finishes are issued in host order, so the
     // reference of every frame is known when the call is issued.  The chain orders the per-call scratch as it orders f11's tables.
@@ -129,7 +136,7 @@ static void free_motion(rf_tracker t) {
 }
 
 static void free_follow(rf_tracker t) {
-    free_null(t->d_fstore, t->d_fentries, t->d_fmeas, t->d_fmask, t->d_fmask_counts);
+    free_null(t->d_fstore, t->d_fentries, t->d_fmeas, t->d_fmask, t->d_fmask_counts, t->d_fgone);
     for (auto &s : t->slots) free_null(s.follow, s.fregions, s.fregion_counts);
 }
 
@@ -152,6 +159,7 @@ static void tracker_release(rf_tracker t) {
     const BestArgs &b = t->ba;
     cudaFree(b.store); cudaFree(b.store_crops); cudaFree(b.videos); cudaFree(b.acc); cudaFree((void *)b.seen); cudaFree((void *)b.gone); cudaFree(b.meas);
     cudaFree(b.scratch); cudaFree(b.commit); cudaFree(b.src);
+    cudaFree(t->bl.live); cudaFree((void *)t->bl.life);
     delete t;
 }
 
@@ -210,8 +218,9 @@ void rf_tracker_destroy(rf_tracker t) {
     tracker_release(t);
 }
 
-// Restarts videos [v0, v0 + nv) on s, inside the chain: no tracks, and by the kind no stored shots (BEST, nothing is emitted), no
-// templates (FOLLOW, and a following LOOKBACK) and no buffered frames (LOOKBACK, nothing is emitted); with motion, no reference.
+// Restarts videos [v0, v0 + nv) on s, inside the chain: no tracks, and by the kind no stored shots and no live state (BEST, nothing is
+// emitted), no templates (FOLLOW, a following LOOKBACK and a following BEST) and no buffered frames (LOOKBACK, nothing is emitted); with
+// motion, no reference.
 static void restart(rf_tracker t, size_t v0, size_t nv, cudaStream_t s) {
     const size_t T = t->cfg.max_tracks;
     CK(cudaMemsetAsync(t->d_videos + v0, 0, sizeof(TrackVideo) * nv, s));
@@ -219,8 +228,9 @@ static void restart(rf_tracker t, size_t v0, size_t nv, cudaStream_t s) {
     if (t->kind == BEST) {
         CK(cudaMemsetAsync(t->ba.store + v0 * T, 0, sizeof(BestEntry) * nv * T, s));
         CK(cudaMemsetAsync(t->ba.videos + v0, 0, sizeof(BestVideo) * nv, s));
+        if (t->best_live) CK(cudaMemsetAsync(t->bl.live + v0 * T, 0, sizeof(BestLive) * nv * T, s));
     }
-    if (t->kind == FOLLOW || t->lb_follow) CK(cudaMemsetAsync(t->d_fentries + v0 * T, 0, sizeof(FollowEntry) * nv * T, s));
+    if (t->kind == FOLLOW || t->lb_follow || t->best_follow) CK(cudaMemsetAsync(t->d_fentries + v0 * T, 0, sizeof(FollowEntry) * nv * T, s));
     for (size_t v = v0; t->motion && v < v0 + nv; v++) t->mref[v] = {0, 0};
     for (size_t v = v0; t->kind == LOOKBACK && v < v0 + nv; v++) t->lbv[v].frames = 0;
     std::fill(t->started.begin() + v0, t->started.begin() + v0 + nv, 0);
@@ -242,11 +252,13 @@ int rf_tracker_reset(rf_tracker t, int video) {
 }
 
 // The calls admit() decides.  DETECT: rf_detect_yuv_track_device and rf_detect_yuv_redact_device(_style) with a tracker; FOLLOW:
-// rf_track_follow_device and rf_track_follow_redact_device; LOOKBACK_FOLLOW: rf_track_follow_redact_lookback_device; MOTION, FOLLOWS
-// and LOOKBACK_SEARCH: the queries rf_tracker_motion, rf_tracker_follow and rf_tracker_lookback_search.
+// rf_track_follow_device and rf_track_follow_redact_device; LOOKBACK_FOLLOW: rf_track_follow_redact_lookback_device; BEST_FOLLOW:
+// rf_track_follow_best_device; MOTION, FOLLOWS and LOOKBACK_SEARCH: the queries rf_tracker_motion, rf_tracker_follow and
+// rf_tracker_lookback_search.
 enum class Call {
-    UPDATE, DETECT, BEST, FINISH, FOLLOW, LOOKBACK, DRAIN, LOOKBACK_FOLLOW,
-    SET_MOTION, SET_FOLLOW, SET_LOOKBACK, SET_LOOKBACK_SEARCH, SET_LOOKBACK_FOLLOW, SET_TILING,      // the setters, in this range
+    UPDATE, DETECT, BEST, FINISH, FOLLOW, LOOKBACK, DRAIN, LOOKBACK_FOLLOW, BEST_FOLLOW,
+    SET_MOTION, SET_FOLLOW, SET_LOOKBACK, SET_LOOKBACK_SEARCH, SET_LOOKBACK_FOLLOW, SET_BEST_LIVE, SET_BEST_FOLLOW,
+    SET_TILING,                                                                                        // the setters, SET_MOTION .. here
     MOTION, FOLLOWS, LOOKBACK_SEARCH
 };
 
@@ -260,6 +272,8 @@ static int admit(rf_tracker t, const char *who, Call call) {
         if (k != need) why = fmt("not a %s tracker (%s)", name[need], made_by[need]);
     };
     auto only_through = [&]() {
+        if (t->best_follow)
+            return std::string("a best-shot tracker takes frames only through rf_detect_yuv_track_best_device and rf_track_follow_best_device");
         if (t->lb_follow)
             return std::string("a following look-back tracker takes frames only through rf_detect_yuv_redact_lookback_device and "
                                "rf_track_follow_redact_lookback_device");
@@ -274,10 +288,11 @@ static int admit(rf_tracker t, const char *who, Call call) {
         break;
     case Call::DETECT: if (k == BEST || k == LOOKBACK) why = only_through(); break;
     case Call::BEST: case Call::FINISH: only(BEST); break;
-    case Call::FOLLOW: if (t->lb_follow) why = only_through(); else only(FOLLOW); break;
-    case Call::FOLLOWS: if (!t->lb_follow) only(FOLLOW); break;
+    case Call::FOLLOW: if (t->lb_follow || t->best_follow) why = only_through(); else only(FOLLOW); break;
+    case Call::FOLLOWS: if (!t->lb_follow && !t->best_follow) only(FOLLOW); break;
     case Call::LOOKBACK: case Call::DRAIN: only(LOOKBACK); break;
     case Call::LOOKBACK_FOLLOW: if (!t->lb_follow) why = "not a following look-back tracker (rf_tracker_set_lookback_follow)"; break;
+    case Call::BEST_FOLLOW: if (!t->best_follow) why = "not a following best-shot tracker (rf_tracker_set_best_follow)"; break;
     case Call::SET_MOTION: if (t->motion) why = "motion is already on"; break;
     case Call::SET_FOLLOW: if (k != PLAIN) why = k == FOLLOW ? "following is already on" : fmt("a %s tracker cannot follow", name[k]); break;
     case Call::SET_LOOKBACK: if (k != PLAIN) why = k == LOOKBACK ? "look-back is already on" : fmt("a %s tracker cannot look back", name[k]); break;
@@ -288,6 +303,14 @@ static int admit(rf_tracker t, const char *who, Call call) {
     case Call::SET_LOOKBACK_FOLLOW:
         only(LOOKBACK);
         if (why.empty() && t->lb_follow) why = "look-back following is already on";
+        break;
+    case Call::SET_BEST_LIVE:
+        only(BEST);
+        if (why.empty() && t->best_live) why = "live shots are already on";
+        break;
+    case Call::SET_BEST_FOLLOW:
+        only(BEST);
+        if (why.empty() && t->best_follow) why = "best-shot following is already on";
         break;
     case Call::SET_TILING: if (t->tiled) why = "tiling is already on"; break;
     case Call::MOTION: if (!t->motion) why = "motion is off (rf_tracker_set_motion)"; break;
@@ -492,6 +515,31 @@ static void follow_cut(rf_tracker t, const rf_yuv_frame *frames, const int *vide
     CK(launch_follow_cut(f, tab.data(), n, s, oriented));
 }
 
+// The best-shot table of m frames of videos[]: each frame's video, and the videos in first-appearance order (one select CTA each).
+static BestTable best_table(const int *videos, int m) {
+    BestTable bt{};
+    bt.n = m;
+    for (int i = 0; i < m; i++) {
+        const int v = videos[i];
+        bt.video[i] = v;
+        bool known = false;
+        for (int j = 0; j < bt.nvideos; j++) known |= bt.cta_video[j] == v;
+        if (!known) bt.cta_video[bt.nvideos++] = v;
+    }
+    return bt;
+}
+
+// The best-shot arguments of the chunk of call c from frame i0: the caller's crops and matrices, the slot's shot records.
+static BestArgs best_args(rf_tracker t, const rf_tracker_s::Slot &slot, const FrameCall &c, int i0) {
+    const int T = t->cfg.max_tracks;
+    BestArgs b = t->ba;
+    b.out.crops = static_cast<uint8_t *>(c.crops) + (size_t)i0 * T * b.out.crop_bytes;
+    b.out.mats = c.mats ? c.mats + (size_t)i0 * T * 6 : nullptr;
+    b.best = slot.best + (size_t)i0 * T;
+    b.best_counts = slot.best_counts + i0;
+    return b;
+}
+
 // The update of a records or detect call into ring slot `ring`'s lists, on s inside the chain: with motion, the estimate of its frames
 // first (in tables of TRACK_MAX_FRAMES frames) and the commit after.  A best-shot call goes in chunks of TRACK_MAX_FRAMES frames, each
 // tracked, then measured, selected, emitted and committed (the per-call tables hold one chunk); launch_track_update makes the same
@@ -522,6 +570,7 @@ static void update_issue(rf_tracker t, unsigned ring, const FrameCall &c, cudaSt
     if (c.sink == FrameCall::BEST) {
         ta.seen = const_cast<TrackSeen *>(t->ba.seen);
         ta.gone = const_cast<TrackGone *>(t->ba.gone);
+        if (t->best_live) ta.life = const_cast<TrackLife *>(t->bl.life);
     }
     const YuvFrames src = detect_source(c);
     const int chunk = c.sink == FrameCall::BEST ? TRACK_MAX_FRAMES : c.n;
@@ -535,24 +584,15 @@ static void update_issue(rf_tracker t, unsigned ring, const FrameCall &c, cudaSt
         if (k.motion) k.motion += i0;
         CK(launch_track_update(k, c.videos + i0, c.scales ? c.scales + i0 : nullptr, m, s));
         if (c.sink != FrameCall::BEST) continue;
-        BestTable bt{};
-        bt.n = m;
+        BestTable bt = best_table(c.videos + i0, m);
         for (int i = 0; i < m; i++) {
             const int v = c.videos[i0 + i];
-            bt.video[i] = v;
             const std::array<int, 2> size = shown_size(t, v, src.width(i0 + i), src.height(i0 + i));    // f20: as displayed
             bt.img[i] = AlignImageT<YuvPlanes>{src.in_place(i0 + i), size[0], size[1], 1.f, video_bits(t, v)};
-            bool known = false;
-            for (int j = 0; j < bt.nvideos; j++) known |= bt.cta_video[j] == v;
-            if (!known) bt.cta_video[bt.nvideos++] = v;
         }
-        BestArgs b = t->ba;
-        b.out.crops = static_cast<uint8_t *>(c.crops) + (size_t)i0 * T * b.out.crop_bytes;
-        b.out.mats = c.mats ? c.mats + (size_t)i0 * T * 6 : nullptr;
-        b.best = slot.best + (size_t)i0 * T;
-        b.best_counts = slot.best_counts + i0;
+        BestArgs b = best_args(t, slot, c, i0);
         b.counts = c.counts + i0;
-        CK(launch_best_frames(b, bt, s));
+        CK(t->best_live ? launch_best_frames_live(b, bt, t->bl, s) : launch_best_frames(b, bt, s));
     }
     if (t->motion) motion_commit(t, commits, s);
 }
@@ -779,6 +819,7 @@ static void follow_rounds(rf_tracker t, unsigned ring, const rf_yuv_frame *frame
     f.track_counts = slot.counts;
     f.regions = slot.fregions;
     f.region_counts = slot.fregion_counts;
+    f.gone = t->kind == BEST ? t->d_fgone : nullptr;      // f22: a following best-shot tracker's removals, by the frame's call index
     std::vector<int> round(n);
     int rounds = 0;
     for (int i = 0; i < n; i++) {
@@ -827,6 +868,18 @@ static void follow_rounds(rf_tracker t, unsigned ring, const rf_yuv_frame *frame
     t->follow_slot = (int)ring;
 }
 
+// f22: the best-shot half of a follow call of a following best-shot tracker, after follow_rounds on s: each chunk of TRACK_MAX_FRAMES
+// frames selects its removals' EXIT shots (no records: nothing is measured or stored) and emits them.
+static void best_follow_issue(rf_tracker t, const rf_tracker_s::Slot &slot, const FrameCall &c, cudaStream_t s) {
+    const int T = t->cfg.max_tracks;
+    for (int i0 = 0; i0 < c.n; i0 += TRACK_MAX_FRAMES) {
+        const int m = std::min(TRACK_MAX_FRAMES, c.n - i0);
+        BestArgs b = best_args(t, slot, c, i0);
+        b.gone = t->d_fgone + (size_t)i0 * T;
+        CK(launch_best_follow(b, best_table(c.videos + i0, m), s));
+    }
+}
+
 int rf_track_follow_device(rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, const rf_track **dev_tracks,
                            const int32_t **dev_track_counts) {
     FrameCall c{.who = "rf_track_follow_device", .call = Call::FOLLOW, .source = FrameCall::FOLLOW, .t = t, .frames = frames, .videos = videos,
@@ -868,6 +921,70 @@ int rf_tracker_debug_state(rf_tracker t, int video, double *out, int cap) {
     }
     std::copy(v.begin(), v.begin() + std::min<size_t>(v.size(), (size_t)std::max(cap, 0)), out);
     return (int)live.size();
+}
+
+// ---- f22 live and following best shots ---------------------------------------------------------------------------------------
+int rf_tracker_set_best_live(rf_tracker t, const rf_best_live_config *cfg) {
+    static const char *who = "rf_tracker_set_best_live";
+    if (!t) return RF_ERR_INVALID_ARG;
+    rf_handle h = t->h;
+    if (!cfg) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL config", who));
+    int rc = admit(t, who, Call::SET_BEST_LIVE);
+    if (rc) return rc;
+    const float fq = cfg->first_quality == 0.f ? 0.3f : cfg->first_quality, imp = cfg->improve == 0.f ? 0.2f : cfg->improve;
+    const int gap = cfg->min_gap == 0 ? 30 : cfg->min_gap;
+    if (!(fq > 0.f && fq <= 1.f)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: first_quality %g, must be 0 or in (0, 1]", who, (double)cfg->first_quality));
+    if (!(std::isfinite(imp) && imp > 0.f)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: improve %g, must be 0 or finite and positive", who, (double)cfg->improve));
+    if (gap < 1 || gap > (1 << 20)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: min_gap %d, must be 0 or in [1, %d]", who, cfg->min_gap, 1 << 20));
+    BestLiveArgs l{};
+    const size_t V = t->cfg.max_videos, T = t->cfg.max_tracks, F = h->cfg.max_faces, M = std::min<size_t>(h->cfg.max_batch, TRACK_MAX_FRAMES);
+    try {
+        CK(cudaSetDevice(h->device));
+        CK(cudaMalloc(&l.live, sizeof(BestLive) * V * T));
+        TrackLife *life = nullptr;
+        CK(cudaMalloc(&life, sizeof(TrackLife) * M * F));
+        l.life = life;
+        CK(cudaMemset(l.live, 0, sizeof(BestLive) * V * T));
+        CK(cudaDeviceSynchronize());
+    } catch (const CudaFail &f) {
+        cudaFree(l.live);
+        cudaFree((void *)l.life);
+        return fail_cuda(h, f);
+    }
+    l.first_quality = (double)fq;
+    l.ratio = 1.0 + (double)imp;
+    l.min_gap = gap;
+    t->bl = l;
+    t->best_live = true;
+    return RF_OK;
+}
+
+int rf_tracker_set_best_follow(rf_tracker t, const rf_follow_config *cfg) {
+    static const char *who = "rf_tracker_set_best_follow";
+    if (!t) return RF_ERR_INVALID_ARG;
+    rf_handle h = t->h;
+    if (!cfg) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL config", who));
+    int rc = admit(t, who, Call::SET_BEST_FOLLOW);
+    if (rc) return rc;
+    rf_follow_config fc;
+    if ((rc = follow_config(h, who, cfg, fc)) || (rc = follow_alloc(t, who, fc))) return rc;
+    try {
+        CK(cudaMalloc(&t->d_fgone, sizeof(TrackGone) * h->cfg.max_batch * t->cfg.max_tracks));
+    } catch (const CudaFail &f) {
+        free_follow(t);
+        return fail_cuda(h, f);
+    }
+    t->best_follow = true;
+    return RF_OK;
+}
+
+int rf_track_follow_best_device(rf_tracker t, const rf_yuv_frame *frames, const int *videos, int n, void *dev_best_crops, double *dev_best_mats,
+                                const rf_best_shot **dev_best, const int32_t **dev_best_counts, const rf_track **dev_tracks,
+                                const int32_t **dev_track_counts) {
+    FrameCall c{.who = "rf_track_follow_best_device", .call = Call::BEST_FOLLOW, .source = FrameCall::FOLLOW, .sink = FrameCall::BEST, .t = t,
+                .frames = frames, .videos = videos, .n = n, .crops = dev_best_crops, .mats = dev_best_mats, .tracks = dev_tracks,
+                .track_counts = dev_track_counts, .best = dev_best, .best_counts = dev_best_counts};
+    return frame_call(c);
 }
 
 // ---- f12 redaction (redact.cuh) -------------------------------------------------------------------------------------------------
@@ -1733,11 +1850,12 @@ static int issue_call(FrameCall &c) {
             follow_rounds(t, ring, c.frames, c.videos, n, s);
             c.dets = slot.fregions;      // in id order, max_tracks to a frame, at scale 1
             c.counts = slot.fregion_counts;
+            if (c.sink == FrameCall::BEST) best_follow_issue(t, slot, c, s);
         } else {
             update_issue(t, ring, c, s);
         }
         // the template cut reads the input frames: before a look-back call's swap
-        if (c.source == FrameCall::DETECT && (t->kind == FOLLOW || t->lb_follow)) follow_cut(t, c.frames, c.videos, n, slot, s);
+        if (c.source == FrameCall::DETECT && (t->kind == FOLLOW || t->lb_follow || t->best_follow)) follow_cut(t, c.frames, c.videos, n, slot, s);
         CK(cudaEventRecord(t->chain, s));
         const int per_frame = c.source == FrameCall::FOLLOW ? t->cfg.max_tracks : h->cfg.max_faces;
         if (c.sink == FrameCall::CROPS) {

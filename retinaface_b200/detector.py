@@ -164,22 +164,28 @@ class RetinaFace:
             runs.setdefault((p, not det), []).append(i)
         return [(not follow, idx) for (_, follow), idx in sorted(runs.items())]
 
-    def _interval_tracker(self, detect_every: int, best=None, lookback=0, tiling=None):
+    def _interval_tracker(self, detect_every: int, best=None, lookback=0, tiling=None, live=None):
         if int(detect_every) < 1:
             raise ValueError(f"detect_every {detect_every}, must be >= 1")
-        if detect_every > 1 and best is not None:
-            raise ValueError("detect_every > 1 does not combine with best shots yet")
+        if live is not None and best is None:
+            raise ValueError("live shots need best shots: pass best as well")
         trk = getattr(self, "_tracker", None)
+        if live is not None and trk is not None and not trk.best_live_on:
+            raise ValueError("live: this detector's tracker was created without live shots (the first call decides)")
+        if detect_every > 1 and best is not None and trk is not None and not trk.best_follow_on:
+            raise ValueError("detect_every > 1 with best shots needs a following best-shot tracker: this detector's tracker was created "
+                             "without one (the first call decides the tracker)")
         if detect_every > 1 and lookback and trk is not None and not trk.lookback_follow_on:
             raise ValueError("detect_every > 1 with lookback needs a following look-back tracker: this detector's tracker was created "
                              "without one (the first call decides the tracker)")
-        if detect_every > 1 and not lookback and trk is not None and not trk.follow_on:
+        if detect_every > 1 and best is None and not lookback and trk is not None and not trk.follow_on:
             raise ValueError("detect_every > 1 needs a follow tracker: this detector's tracker was created without one")
         if tiling and trk is not None and not trk.tiling_on:
             raise ValueError("tiling: this detector's tracker was created without tiling (the first call decides)")
 
     def trackFrames(self, frames: Sequence, videos: Sequence[int], threshold: float = 0.5, layout: str = "nv12", matrix: str = "bt601",
-                    align: dict = None, max_videos: int = 64, best: dict = None, motion=False, detect_every: int = 1, tiling=None):
+                    align: dict = None, max_videos: int = 64, best: dict = None, motion=False, detect_every: int = 1, tiling=None,
+                    live=None):
         """f10 tracking: device 4:2:0 frames (torch CUDA tensors in ``Engine.detect_yuv_device``'s forms), frame i of video
         ``videos[i]``, detected and associated with the tracks of earlier frames on the GPU (rf_detect_yuv_track_device).  Per frame, a
         list of ``(id, state, FaceDetectInfo)`` over every live track (``capi.TRACK_*`` states; the face is the last matched one, in
@@ -204,12 +210,28 @@ class RetinaFace:
 
         f19 small faces: with ``tiling`` (True, or ``Tracker.set_tiling``'s keywords: levels, overlap) every detect call of the tracker
         detects through the tiles of ``detectTiled`` (rf_tracker_set_tiling), so faces far below the letter-box's smallest anchor in
-        4K frames are tracked too.  The first call decides; asking for it on a tracker created without it raises ValueError."""
+        4K frames are tracked too.  The first call decides; asking for it on a tracker created without it raises ValueError.
+
+        f22 live cameras: with ``best`` and ``live`` (True, or ``Tracker.set_best_live``'s keywords: first_quality, improve, min_gap)
+        the second list also holds the LIVE shots (reason ``capi.BEST_LIVE``) of tracks that are still live: a first good shot, then
+        markedly better ones.  With ``best`` and ``detect_every=k`` > 1 the tracker is a following best-shot tracker: detect frames go
+        through rf_detect_yuv_track_best_device, follow frames through rf_track_follow_best_device, whose shots (the EXIT shots of the
+        tracks removed there) are returned as well."""
         if best is not None and align is not None:
             raise ValueError("best shots and new-identity crops are exclusive: pass best or align, not both")
-        self._interval_tracker(detect_every, best=best, tiling=tiling)
+        self._interval_tracker(detect_every, best=best, tiling=tiling, live=live)
         if getattr(self, "_tracker", None) is None:
-            self._tracker = self._new_tracker(max_videos=max_videos, best=best, motion=motion, follow=detect_every > 1, tiling=tiling)
+            following = detect_every > 1
+            self._tracker = self._new_tracker(max_videos=max_videos, best=best, motion=motion, follow=following and best is None, tiling=tiling,
+                                              best_live=live, best_follow=following and best is not None)
+        if self._tracker.best_follow_on and best is not None:
+            tracks, shots = [None] * len(frames), [None] * len(frames)
+            for det, idx in self._interval_calls(videos, detect_every):
+                fr, vi = [frames[i] for i in idx], [videos[i] for i in idx]
+                t, c = self._best_call(fr, vi, threshold, layout, matrix, det)
+                for j, i in enumerate(idx):
+                    tracks[i], shots[i] = t[j], c[j]
+            return tracks, shots
         if self._tracker.follow_on:
             tracks, new = [None] * len(frames), [[] for _ in frames]
             for det, idx in self._interval_calls(videos, detect_every):
@@ -223,15 +245,23 @@ class RetinaFace:
                 for j, i in enumerate(idx):
                     tracks[i], new[i] = t[j], c[j]
             return tracks, new
-        n = len(frames)
         if best is not None:
-            crops = self._best_crops(n)
+            return self._best_call(frames, videos, threshold, layout, matrix, True)
+        return self._track_call(frames, videos, threshold, layout, matrix, align)
+
+    def _best_call(self, frames, videos, threshold, layout, matrix, detect: bool):
+        """One best-shot call -- a detect call, or (f22) a follow call of a following best-shot tracker: the lists and the
+        (shot, crop) pairs of each frame."""
+        n = len(frames)
+        crops = self._best_crops(n)
+        if detect:
             bp, bc, tp, tc, _, _, _ = self._tracker.detect_yuv_best_device(list(frames), list(videos), threshold, self.nms_threshold,
                                                                           crops.data_ptr(), layout=layout, matrix=matrix)
-            tracks = self._lists(self._tracker.read(tp, tc, n))
-            shots = self._tracker.read_best(bp, bc, n)
-            return tracks, [[(s, crops[i, k]) for k, s in enumerate(per)] for i, per in enumerate(shots)]
-        return self._track_call(frames, videos, threshold, layout, matrix, align)
+        else:
+            bp, bc, tp, tc = self._tracker.follow_best_device(list(frames), list(videos), crops.data_ptr(), layout=layout)
+        tracks = self._lists(self._tracker.read(tp, tc, n))
+        shots = self._tracker.read_best(bp, bc, n)
+        return tracks, [[(s, crops[i, k]) for k, s in enumerate(per)] for i, per in enumerate(shots)]
 
     @staticmethod
     def _lists(recs):
@@ -351,6 +381,7 @@ class RetinaFace:
             raise ValueError("finishVideo needs a best-shot tracker: call trackFrames(..., best=...) first")
         crops = self._best_crops(1)[0]
         bp, bc = self._tracker.finish(video, crops.data_ptr())
+        self.__dict__.get("_frame_no", {}).pop(int(video), None)      # the video restarts: its next frame is a detect frame
         shots = self._tracker.read_best(bp, bc, 1)[0]
         return [(s, crops[k]) for k, s in enumerate(shots)]
 

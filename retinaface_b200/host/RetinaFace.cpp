@@ -550,8 +550,68 @@ void RetinaFace::trackYUVBest(const vector<rf_yuv_frame> &device_frames, const v
     noteMotion(n);
 }
 
+void RetinaFace::trackYUVBest(const vector<rf_yuv_frame> &device_frames, const vector<int> &videos, void *dev_best_crops, float threshold,
+                              const BestOptions &bo) {
+    if (videos.size() != device_frames.size()) throw std::invalid_argument("trackYUVBest: one video index per frame");
+    if (device_frames.size() > (size_t)opt_.max_batch) throw std::invalid_argument("trackYUVBest: at most max_batch frames per call");
+    if (bo.detect_every < 1) throw std::invalid_argument("trackYUVBest: detect_every must be >= 1");
+    if (tracker_ && !best_tracker_) throw std::logic_error("trackYUVBest: this RetinaFace already tracks without best shots (trackYUV)");
+    if (tracker_ && bo.detect_every > 1 && !best_follow_)
+        throw std::logic_error("trackYUVBest: detect_every > 1, but this RetinaFace's best-shot tracker was created without it (the first call decides)");
+    bool detect = true;
+    if (bo.detect_every > 1) {
+        std::map<int, long long> nums = frame_no_;
+        int kinds = 0;       // 1: a detect frame, 2: a follow frame
+        for (int v : videos) kinds |= nums[v]++ % bo.detect_every == 0 ? 1 : 2;
+        if (kinds == 3)
+            throw std::invalid_argument("trackYUVBest: with detect_every > 1 a call takes detect frames only or follow frames only (its videos' frame "
+                                        "numbers must agree modulo detect_every)");
+        detect = kinds != 2;
+        frame_no_ = nums;
+    }
+    if (!tracker_) {
+        rf_track_config tc{};
+        tc.max_videos = opt_.track_videos;
+        rf_best_config bc{};
+        bc.min_quality = bo.min_quality;
+        int rc = rf_tracker_create_best(h_, &tc, &bc, &tracker_);
+        if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_create_best: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+        best_tracker_ = true;
+        if (bo.live && (rc = rf_tracker_set_best_live(tracker_, &bo.live_config)) != RF_OK)
+            throw std::runtime_error(string("rf_tracker_set_best_live: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+        if (bo.detect_every > 1) {
+            const rf_follow_config fc{};
+            if ((rc = rf_tracker_set_best_follow(tracker_, &fc)) != RF_OK)
+                throw std::runtime_error(string("rf_tracker_set_best_follow: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+            best_follow_ = true;
+        }
+        trackerCreated(false);
+    }
+    const int n = (int)device_frames.size();
+    tracks_ = DeviceTracks{};
+    best_ = DeviceBestShots{};
+    int rc = detect ? rf_detect_yuv_track_best_device(h_, tracker_, device_frames.data(), videos.data(), n, RF_YUV_BT601, threshold, nms_threshold,
+                                                      dev_best_crops, nullptr, &best_.shots, &best_.counts, &tracks_.tracks, &tracks_.counts,
+                                                      nullptr, nullptr, nullptr)
+                    : rf_track_follow_best_device(tracker_, device_frames.data(), videos.data(), n, dev_best_crops, nullptr, &best_.shots,
+                                                  &best_.counts, &tracks_.tracks, &tracks_.counts);
+    if (rc != RF_OK)
+        throw std::runtime_error(string(detect ? "rf_detect_yuv_track_best_device: " : "rf_track_follow_best_device: ") + rf_status_string(rc) + ": " +
+                                 rf_last_error(h_));
+    tracks_.n = best_.n = n;
+    tracks_.max_tracks = best_.max_tracks = 64;      // rf_track_config's default
+    if (!detect) {
+        const rf_follow *f = nullptr;
+        if ((rc = rf_tracker_follow(tracker_, &f)) != RF_OK)
+            throw std::runtime_error(string("rf_tracker_follow: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+        follow_ = DeviceFollow{f, n, 64};
+    }
+    noteMotion(n);
+}
+
 void RetinaFace::finishVideo(int video, void *dev_best_crops) {
     if (!tracker_ || !best_tracker_) throw std::logic_error("finishVideo: no best-shot tracker (trackYUVBest)");
+    frame_no_.erase(video);      // the video restarts: with detect_every, its next frame is a detect frame
     best_ = DeviceBestShots{};
     int rc = rf_tracker_finish(tracker_, video, dev_best_crops, nullptr, &best_.shots, &best_.counts);
     if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_finish: ") + rf_status_string(rc) + ": " + rf_last_error(h_));

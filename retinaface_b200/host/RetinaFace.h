@@ -66,6 +66,15 @@ struct AlignOptions {
 };
 
 // f12 / f14 redaction (rf_detect_yuv_redact_device_style): the mosaic or blur written over every face
+// f22 best shots for live cameras, the opt-in trackYUVBest overload's options (the first call creates the tracker with them).
+struct BestOptions {
+    int detect_every = 1;                // > 1: a following best-shot tracker (rf_tracker_set_best_follow); each video's frames whose
+                                         // number is divisible by it are detected, the others followed
+    bool live = false;                   // live shots (rf_tracker_set_best_live) with live_config (zeros: its defaults)
+    rf_best_live_config live_config{};
+    float min_quality = 0.f;
+};
+
 struct RedactOptions {
     int blocks = 8;                      // mosaic: cells across a region's longer side, 1..32 (1: one flat patch); the blur ignores it
     float margin = 0.25f;                // each side of a box grows by margin x its side, (0, 1]
@@ -164,6 +173,13 @@ class RetinaFace {
     };
     void trackYUVBest(const vector<rf_yuv_frame> &device_frames, const vector<int> &videos, void *dev_best_crops, float threshold = 0.5,
                       float min_quality = 0.f);
+    // f22: the same with BestOptions: live shots (reason RF_BEST_LIVE) while tracks live, and a detection interval.  With
+    // detect_every > 1 one call takes detect frames only or follow frames only (its videos' frame numbers agree modulo detect_every, as
+    // when each call takes the next frame of every camera); a call mixing both is std::invalid_argument before anything is issued.
+    // lastBestShots() and lastTracks() hold the call's records either way (a follow call's shots: the tracks removed on it), and
+    // lastFollow() the follow records of the last follow call.
+    void trackYUVBest(const vector<rf_yuv_frame> &device_frames, const vector<int> &videos, void *dev_best_crops, float threshold,
+                      const BestOptions &opt);
     const DeviceBestShots &lastBestShots() const { return best_; }
     // f13 camera motion (options track_motion): the device rf_motion of each frame of the last trackYUV / trackYUVBest / tracked
     // redactYUV call -- the estimated similarity from the video's previous frame, applied to its tracks.
@@ -223,6 +239,7 @@ class RetinaFace {
     bool tracker_search_ = false;        // f17: tracker_ searches its look-back buffer
     bool tracker_lookback_follow_ = false;   // f18: tracker_ is a following look-back tracker
     bool best_tracker_ = false;
+    bool best_follow_ = false;           // f22: tracker_ is a following best-shot tracker
     DeviceTracks tracks_;
     DeviceBestShots best_;
     DeviceMotion motion_;

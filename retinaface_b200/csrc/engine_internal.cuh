@@ -142,9 +142,7 @@ struct rf_handle_s {
     std::vector<TensorInfo> tensors;
     std::map<std::string, int> tensor_by_name;
     std::vector<Step> steps;
-    int head_step = -1, nms_step = -1;
     std::vector<std::shared_ptr<TileChain>> chains;   // tile-chain launches of the FP16 plan (plan_tile.cu)
-    unsigned tile_mask = 0;                           // which parts of the FP16 plan run as tile chains (RF_TILE_MASK)
     int lane_last[3] = {-1, -1, -1};                  // last step of each side lane (joined at the end of the forward)
     int cache_status = 0;                             // model.h CACHE_*: how the folded model was obtained
     int tile_expected = 0;                            // tiles per image over the three SSH chains (last-block NMS)
@@ -274,9 +272,9 @@ struct ConvNode {
 // Depthwise i + pointwise i+1 on an h x w input; the op creates the output tensor `out` (and, where it stores it, `mid`).
 struct PairNode { int i; const FoldedConv *dw, *pw; std::string mid, out; int h, w; };
 struct StemNode { const FoldedConv *conv0; std::string out0; PairNode pair; };   // conv0 -> out0, then pair 1 + 2
-// Backbone segment `id` (0 = A ... 5 = F): pairs, then optionally the lateral 1x1 conv `lat` on the last pair's output, into
-// a new tensor `lat_out` (lat.in and lat.out[0].t are set by the op).
-struct SegNode { std::string chain; int id; std::vector<PairNode> pairs; ConvNode lat; std::string lat_out; };
+// Backbone segment: pairs, then optionally the lateral 1x1 conv `lat` on the last pair's output, into a new tensor `lat_out`
+// (lat.in and lat.out[0].t are set by the op).
+struct SegNode { std::vector<PairNode> pairs; ConvNode lat; std::string lat_out; };
 struct SegOut { int out, lat; };
 // FPN level `level` (1 = stride 16, 2 = stride 8): lat + upsample(up) -> the tensor `sum`, then aggr 3x3; `fused` is the
 // aggr conv with the merge fused into it, `aggr` the one on the stand-alone sum (aggr.in set by the op).
@@ -302,7 +300,7 @@ struct PlanOps {
     virtual bool fuse_merge(const MergeNode &m) = 0;        // this plan's rule: merge fused into the aggr conv
     virtual void heads(const HeadsNode &n) = 0;             // predictors + decode + NMS of all levels
     // defaults built from the operations above (plan_net.cu)
-    virtual SegOut segment(const SegNode &s, int in);
+    SegOut segment(const SegNode &s, int in);
     virtual void merge_aggr(const MergeNode &m);
     virtual void ssh(const SshNode &n);
 };
@@ -335,10 +333,10 @@ int plan_pair_tc(Builder &B, const PairNode &p, int in);
 void plan_conv_tc(Builder &B, const ConvNode &c);
 int plan_fpn_merge_h2(Builder &B, const MergeNode &m);
 template <typename T>
-void plan_heads(Builder &B, const HeadsNode &n, const float scale[3], const char *prefix, bool with_heads);
+void plan_heads(Builder &B, const HeadsNode &n, const float scale[3], const char *prefix);
 std::vector<__half> pack_tc_weights(const std::vector<const FoldedConv *> &cs, std::vector<float> &bias, int &Kpad, int nsplit = 1);
 // ---- exported by plan_tile.cu ---------------------------------------------------------------------------------------
-void build_plan_tiles(rf_handle h);         // RF_PREC_FP16 with tensor cores: tile chains (tile_chain.cuh) + per-layer kernels where no chain fits
+void build_plan_tiles(rf_handle h);         // RF_PREC_FP16 with tensor cores: per-layer kernels + (latency mode) tile chains (tile_chain.cuh)
 cudaError_t tile_init();
 std::string describe_chains(rf_handle h);
 // ---- exported by comm.cu --------------------------------------------------------------------------------------------

@@ -296,62 +296,47 @@ int plan_fpn_merge_h2(Builder &B, const MergeNode &mn) {
     return plus;
 }
 
-// With heads: the three predictor 1x1 convs of every level + softmax + decode, then sort + NMS by the last block of each image,
-// in one launch (k_head_decode); feature level l is dequantised by scale[l].  Without (tile chains compute the predictors):
-// sort + NMS alone (k_nms).
+// The three predictor 1x1 convs of every level + softmax + decode, then sort + NMS by the last block of each image, in one
+// launch (k_head_decode); feature level l is dequantised by scale[l].
 template <typename T>
-void plan_heads(Builder &B, const HeadsNode &n, const float scale[3], const char *prefix, bool with_heads) {
+void plan_heads(Builder &B, const HeadsNode &n, const float scale[3], const char *prefix) {
     rf_handle h = B.h;
     auto T_ = [h](const Run &r, int id) { return reinterpret_cast<T *>(r.ctx.arena + h->tensors[id].offset); };
     auto Wd = [h](size_t off) { return h->d_weights + off; };
     const double es = h->elem;
     const int H = h->cfg.net_h, W = h->cfg.net_w;
     const int h32 = H / 32, w32 = W / 32, h16 = H / 16, w16 = W / 16, h8 = H / 8, w8 = W / 8;
-    if (with_heads) {
-        size_t hw_off[3], hb_off[3];
-        for (int l = 0; l < 3; l++) {
-            std::vector<float> w(32 * 64), b(32);
-            int r = 0;
-            for (auto c : n.pred[l])
-                for (int o = 0; o < c->cout; o++, r++) {
-                    b[r] = c->b[o];
-                    for (int ci = 0; ci < 64; ci++) w[r * 64 + ci] = c->w[(size_t)o * 64 + ci];
-                }
-            hw_off[l] = B.add_weights(w);
-            hb_off[l] = B.add_weights(b);
-        }
-        Step s;
-        s.name = std::string(prefix) + "heads_1x1+softmax+decode+nms_all_levels";   // decode -> NMS in one launch (last block per image)
-        s.in = {h->feat_tensor[0], h->feat_tensor[1], h->feat_tensor[2]};
-        double px = (double)h32 * w32 + (double)h16 * w16 + (double)h8 * w8;
-        s.flops_per_img = 2.0 * px * 64 * 4;   // threshold-first: only cls logits are computed for every pixel
-        s.bytes_per_img = px * 64 * es;
-        int f0 = h->feat_tensor[0], f1 = h->feat_tensor[1], f2 = h->feat_tensor[2];
-        size_t w0 = hw_off[0], w1 = hw_off[1], w2 = hw_off[2], b0 = hb_off[0], b1 = hb_off[1], b2 = hb_off[2];
-        float s0 = scale[0], s1 = scale[1], s2 = scale[2];
-        s.launch = [=](const Run &r) {
-            const T *feat[3] = {T_(r, f0), T_(r, f1), T_(r, f2)};
-            HeadWeights hws[3] = {{Wd(w0), Wd(b0), s0}, {Wd(w1), Wd(b1), s1}, {Wd(w2), Wd(b2), s2}};
-            CK(launch_head_decode<T>(feat, hws, h->lv, r.n, W, H, r.ctx.d_params, r.ctx.pb, r.blobs, r.stream, true));
-        };
-        h->head_step = (int)h->steps.size();
-        B.step(std::move(s));
-        return;
+    size_t hw_off[3], hb_off[3];
+    for (int l = 0; l < 3; l++) {
+        std::vector<float> w(32 * 64), b(32);
+        int r = 0;
+        for (auto c : n.pred[l])
+            for (int o = 0; o < c->cout; o++, r++) {
+                b[r] = c->b[o];
+                for (int ci = 0; ci < 64; ci++) w[r * 64 + ci] = c->w[(size_t)o * 64 + ci];
+            }
+        hw_off[l] = B.add_weights(w);
+        hb_off[l] = B.add_weights(b);
     }
     Step s;
-    s.name = "sort+nms";
-    // the candidates come from the steps that produce the three SSH outputs (tile chains with fused predictors, possibly on
-    // other lanes): naming those tensors as inputs makes the NMS wait for every one of them
+    s.name = std::string(prefix) + "heads_1x1+softmax+decode+nms_all_levels";   // decode -> NMS in one launch (last block per image)
     s.in = {h->feat_tensor[0], h->feat_tensor[1], h->feat_tensor[2]};
-    s.flops_per_img = 0;
-    s.bytes_per_img = 0;
-    s.launch = [=](const Run &r) { CK(launch_nms(r.n, r.ctx.d_params, r.ctx.pb, r.stream)); };
-    h->nms_step = (int)h->steps.size();
+    double px = (double)h32 * w32 + (double)h16 * w16 + (double)h8 * w8;
+    s.flops_per_img = 2.0 * px * 64 * 4;   // threshold-first: only cls logits are computed for every pixel
+    s.bytes_per_img = px * 64 * es;
+    int f0 = h->feat_tensor[0], f1 = h->feat_tensor[1], f2 = h->feat_tensor[2];
+    size_t w0 = hw_off[0], w1 = hw_off[1], w2 = hw_off[2], b0 = hb_off[0], b1 = hb_off[1], b2 = hb_off[2];
+    float s0 = scale[0], s1 = scale[1], s2 = scale[2];
+    s.launch = [=](const Run &r) {
+        const T *feat[3] = {T_(r, f0), T_(r, f1), T_(r, f2)};
+        HeadWeights hws[3] = {{Wd(w0), Wd(b0), s0}, {Wd(w1), Wd(b1), s1}, {Wd(w2), Wd(b2), s2}};
+        CK(launch_head_decode<T>(feat, hws, h->lv, r.n, W, H, r.ctx.d_params, r.ctx.pb, r.blobs, r.stream, true));
+    };
     B.step(std::move(s));
 }
-template void plan_heads<float>(Builder &, const HeadsNode &, const float[3], const char *, bool);
-template void plan_heads<__half>(Builder &, const HeadsNode &, const float[3], const char *, bool);
-template void plan_heads<int8_t>(Builder &, const HeadsNode &, const float[3], const char *, bool);
+template void plan_heads<float>(Builder &, const HeadsNode &, const float[3], const char *);
+template void plan_heads<__half>(Builder &, const HeadsNode &, const float[3], const char *);
+template void plan_heads<int8_t>(Builder &, const HeadsNode &, const float[3], const char *);
 
 // conv0 + dw1 + pw2 in one kernel: the two dense layers on tensor cores (stem_tc.cuh k_stem_tc), or all three on CUDA cores
 // (kernels_simt.cuh k_stem) with RF_FLAG_SIMT_STEM; the output is scaled by out_scale (INT8: 1 / its table scale)
@@ -500,7 +485,7 @@ struct SimtOps : PlanOps {
 
     void heads(const HeadsNode &n) override {
         const float one[3] = {1.f, 1.f, 1.f};
-        plan_heads<T>(B, n, one, "", true);
+        plan_heads<T>(B, n, one, "");
     }
 };
 

@@ -236,7 +236,7 @@ struct I8Ops : PlanOps {
     // FP32 predictors + decode on the dequantised concat tensors, and NMS
     void heads(const HeadsNode &n) override {
         const float s[3] = {tscale(B.h->feat_tensor[0]), tscale(B.h->feat_tensor[1]), tscale(B.h->feat_tensor[2])};
-        plan_heads<int8_t>(B, n, s, "i8_", true);
+        plan_heads<int8_t>(B, n, s, "i8_");
     }
 };
 

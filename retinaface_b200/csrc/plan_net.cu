@@ -23,16 +23,16 @@ void walk_network(PlanOps &ops) {
     int cur = ops.stem(StemNode{conv("mobilenet0_conv0_fwd"), "mobilenet0_relu0_fwd", pair_node(1, fh, fw)});
 
     // ---- 12 x (depthwise 3x3, pointwise 1x1) in six segments, C1 / C2 / C3 and their lateral convs (prototxt:55-1192) --------
-    struct Seg { const char *chain; std::vector<int> pairs; const char *lat, *step; int lane; };
-    const Seg segs[6] = {{"A", {3, 5}, nullptr, nullptr, 0},
-                         {"B", {7, 9}, "rf_c1_red_conv", "c1_red_1x1_64to64", 1},
-                         {"C", {11, 13, 15}, nullptr, nullptr, 0},
-                         {"D", {17, 19, 21}, "rf_c2_lateral", "c2_lateral_1x1_128to64", 2},
-                         {"E", {23}, nullptr, nullptr, 0},
-                         {"F", {25}, "rf_c3_lateral", "c3_lateral_1x1_256to64", 0}};
+    struct Seg { std::vector<int> pairs; const char *lat, *step; int lane; };
+    const Seg segs[6] = {{{3, 5}, nullptr, nullptr, 0},
+                         {{7, 9}, "rf_c1_red_conv", "c1_red_1x1_64to64", 1},
+                         {{11, 13, 15}, nullptr, nullptr, 0},
+                         {{17, 19, 21}, "rf_c2_lateral", "c2_lateral_1x1_128to64", 2},
+                         {{23}, nullptr, nullptr, 0},
+                         {{25}, "rf_c3_lateral", "c3_lateral_1x1_256to64", 0}};
     int lat[3] = {-1, -1, -1}, lh[3] = {0, 0, 0}, lw[3] = {0, 0, 0};     // per FPN level, 0 = stride 32
     for (int k = 0; k < 6; k++) {
-        SegNode s{segs[k].chain, k, {}, {}, {}};
+        SegNode s;
         for (int i : segs[k].pairs) {
             s.pairs.push_back(pair_node(i, fh, fw));
             fh /= s.pairs.back().dw->stride; fw /= s.pairs.back().dw->stride;

@@ -1,18 +1,11 @@
 // plan_tile.cu -- the FP16 tensor-core layer plan: which parts of the network walk (plan_net.cu) run as stages of which
 // persistent tile-chain kernel (tile_chain.cuh), the shared-memory budget of every chain, the packed weights, the TMA tensor
-// maps.  Where the mask leaves a part out or a chain does not fit (wide maps, 256-channel layers), the per-layer tensor-core
-// kernels of plan_fp.cu take over, layer by layer.
+// maps.  Chains run only on a handle with one execution context (TileOps); everything else, and every chain that does not
+// fit (wide maps), runs on the per-layer tensor-core kernels of plan_fp.cu, layer by layer.
 //
-//   stem (per-layer k_stem_tc)                        conv0 + dw1 + pw2
-//   chain A  @ /4    dw3+pw4 (s2) -> dw5+pw6                                        -> relu6
-//   chain B  @ /8    dw7+pw8 (s2) -> dw9+pw10 -> c1 lateral 1x1                      -> relu10 (C1), c1 lateral
-//   chain C  @ /16   dw11+pw12 (s2) -> dw13+pw14 -> dw15+pw16                        -> relu16
-//   chain D  @ /16   dw17+pw18 -> dw19+pw20 -> dw21+pw22 -> c2 lateral 1x1           -> relu22 (C2), c2 lateral
-//   chain E  @ /32   dw23+pw24
-//   /32              dw25+pw26, c3 lateral 1x1: per-layer kernels
-//   level kernels    [FPN merge + aggr 3x3]  and  [SSH det/context convs + predictors + decode (+ last-block NMS)]
-#include <cstdlib>
-
+//   stem, backbone, laterals        per-layer kernels (k_stem_tc, k_tc_dwpw_staged / k_tc_dwpw_2d, k_tc_conv_staged)
+//   tile_<lv>_merge+aggr            FPN merge (lateral + upsampled coarser level) + aggr 3x3          (c2, c1; max_batch <= 2)
+//   tile_ssh_<lv>[+heads+decode]    SSH det/context convs [+ predictors + decode + last-block NMS]     (c3, c2, c1)
 #include "engine_internal.cuh"
 #include "tile_chain.cuh"
 
@@ -54,13 +47,13 @@ struct TileChain {
         bool stored = false;          // the owned rows are TMA-stored into an arena tensor ...
         int store_tensor = -1;        // ... this one (assigned once the chain is known to fit)
         int first = 1 << 30, last = -1;   // stage indices (input: first = -1)
-        bool is_input = false, is_merge = false;
+        bool is_merge = false;
     };
     struct LStage {
-        int type = TCH_CONV, Cin = 0, N = 0, taps = 1, stride = 1, in_buf = 0;
+        int type = TCH_CONV, Cin = 0, N = 0, taps = 1, in_buf = 0;
         std::vector<int> ob_buf, ob_c16, ob_relu;
-        std::vector<__half> wd_img, wp_img;
-        std::vector<float> bd, bp;
+        std::vector<__half> wp_img;
+        std::vector<float> bp;
         int hs = 0;
         int store_buf = -1;
         double flops = 0;             // per output position
@@ -68,12 +61,11 @@ struct TileChain {
     std::string name;
     std::vector<LBuf> bufs;
     std::vector<LStage> stages;
-    int in_tensor = -1, in_C = 0, in_W = 0, in_H = 0, in_s2 = 0;   // chain input (arena tensor) and its map size
+    int in_tensor = -1, in_C = 0, in_W = 0, in_H = 0;   // chain input (arena tensor) and its map size
     int W = 0, H = 0;                 // resolution the chain works at
     int merge_tensor = -1;            // FPN merge: coarser level (64 channels, W/2 x H/2)
     std::vector<__half> merge_w;      // [16 taps][64]
-    int level = -1;                   // TCH_HEAD: FPN level (0: stride 32)
-    bool fused_nms = false;
+    int level = -1;                   // TCH_HEAD (predictors + decode + last-block NMS): FPN level (0: stride 32)
     // finalised
     TchArgs args{};
     size_t bias_off = 0;              // float offset into d_weights
@@ -92,30 +84,6 @@ int add_buf(TileChain &c, int C, bool stored = false, int store_tensor = -1) {
     b.store_tensor = store_tensor;
     c.bufs.push_back(b);
     return (int)c.bufs.size() - 1;
-}
-
-// depthwise diagonal B tiles: tap t, 16-channel slab k -> 16x16 K-major no-swizzle tile [k/8][n][8] with w on the diagonal
-std::vector<__half> pack_dw_tiles(const FoldedConv &dw) {
-    const int C = dw.cout, nk = C / 16;
-    std::vector<__half> img((size_t)9 * nk * 256, __float2half(0.f));
-    for (int t = 0; t < 9; t++)
-        for (int k = 0; k < nk; k++)
-            for (int i = 0; i < 16; i++)
-                img[((size_t)(t * nk + k)) * 256 + ((size_t)(i / 8) * 16 + i) * 8 + i % 8] = __float2half(dw.w[(size_t)(k * 16 + i) * 9 + t]);
-    return img;
-}
-
-int add_dwpw(TileChain &c, int in_buf, const FoldedConv &dw, const FoldedConv &pw, int out_buf) {
-    TileChain::LStage s;
-    s.type = TCH_DWPW; s.Cin = dw.cout; s.N = pw.cout; s.taps = 9; s.stride = dw.stride; s.in_buf = in_buf;
-    s.wd_img = pack_dw_tiles(dw);
-    s.bd = dw.b;
-    int Kpad = 0;
-    s.wp_img = pack_tc_weights({&pw}, s.bp, Kpad);
-    for (int j = 0; j < s.N / 16; j++) { s.ob_buf.push_back(out_buf); s.ob_c16.push_back(j); s.ob_relu.push_back(1); }
-    s.flops = 2.0 * s.Cin * 9 + 2.0 * s.Cin * s.N;
-    c.stages.push_back(std::move(s));
-    return (int)c.stages.size() - 1;
 }
 
 // convolution (all `cs` share the input and are concatenated along N); per conv: destination buffer, channel offset, ReLU
@@ -162,7 +130,7 @@ bool finalize_chain(rf_handle h, TileChain &c, int TH, int max_faces, bool resid
     const int ns = (int)c.stages.size(), nb = (int)c.bufs.size();
     if (ns > TCH_MAX_STAGES || nb > TCH_MAX_BUFS) return false;
     const int Wl = c.W + 2;
-    if (Wl > 256 || (c.in_s2 && 2 * Wl > 256)) return false;
+    if (Wl > 256) return false;
     // halos (reverse stage order: all consumers of a buffer come after its producers)
     for (auto &b : c.bufs) { b.halo = 0; b.first = 1 << 30; b.last = -1; }
     for (int s = ns - 1; s >= 0; s--) {
@@ -170,8 +138,7 @@ bool finalize_chain(rf_handle h, TileChain &c, int TH, int max_faces, bool resid
         int hs = 0;
         for (int b : st.ob_buf) hs = std::max(hs, c.bufs[b].halo);
         st.hs = hs;
-        const bool k3 = st.type == TCH_DWPW || st.taps == 9;
-        c.bufs[st.in_buf].halo = std::max(c.bufs[st.in_buf].halo, hs + (k3 ? 1 : 0));
+        c.bufs[st.in_buf].halo = std::max(c.bufs[st.in_buf].halo, hs + (st.taps == 9 ? 1 : 0));
     }
     const int HT = c.bufs[0].halo;       // buffer 0 is the chain input
     // lifetimes
@@ -191,7 +158,7 @@ bool finalize_chain(rf_handle h, TileChain &c, int TH, int max_faces, bool resid
     a.Wl = Wl; a.HT = HT; a.TH = TH;
     a.W = c.W; a.H = c.H;
     a.tiles_per_img = (c.H + TH - 1) / TH;
-    a.in_s2 = c.in_s2; a.in_C = c.in_C;
+    a.in_C = c.in_C;
     // buffers
     std::vector<int> bytes(nb);
     for (int b = 0; b < nb; b++) {
@@ -209,16 +176,6 @@ bool finalize_chain(rf_handle h, TileChain &c, int TH, int max_faces, bool resid
             tb.rows_lo = 0; tb.nrows = a.merge_rows;
             tb.slab_stride = round_up(a.merge_rows * (c.W / 2 + 2) * 128, 1024);
             bytes[b] = tb.slab_stride;
-            continue;
-        }
-        if (b == 0 && c.in_s2) {
-            const int Hp = TH + 2 * c.stages[0].hs + 1;           // rows of each parity plane
-            if (2 * Hp > 256) return false;
-            tb.rows_lo = HT - c.stages[0].hs - 1; tb.nrows = Hp;
-            tb.slab_stride = round_up((tb.slack + Hp * Wl + 8) * tb.row, 1024);
-            a.plane_stride = tb.slabs * tb.slab_stride;
-            bytes[b] = 4 * a.plane_stride;
-            a.in_bytes = 4u * (unsigned)tb.slabs * (unsigned)(std::min(lb.C, 64) * 2 * Wl * Hp);
             continue;
         }
         tb.slab_stride = round_up((tb.slack + tb.nrows * Wl + 8) * tb.row, 1024);
@@ -248,30 +205,26 @@ bool finalize_chain(rf_handle h, TileChain &c, int TH, int max_faces, bool resid
         placed.push_back(id);
     }
     // stages
-    int wd_max = 0, wp_max = 0, read_end = 0, mt = 0;
+    int wp_max = 0, read_end = 0, mt = 0;
     std::vector<float> bias;
     for (int s = 0; s < ns; s++) {
         auto &ls = c.stages[s];
         TchStage &st = a.st[s];
-        st.type = ls.type; st.Cin = ls.Cin; st.N = ls.N; st.taps = ls.taps; st.stride = ls.stride; st.in_buf = ls.in_buf;
-        if (ls.stride == 2 && (s != 0 || !c.in_s2)) return false;
+        st.type = ls.type; st.Cin = ls.Cin; st.N = ls.N; st.taps = ls.taps; st.in_buf = ls.in_buf;
         st.rows_lo = HT - ls.hs; st.nrows = TH + 2 * ls.hs;
         if ((int)ls.ob_buf.size() > 16 || ls.N % 16 || ls.Cin % 16 || ls.N > 256) return false;
         for (size_t j = 0; j < ls.ob_buf.size(); j++) { st.ob_buf[j] = (unsigned char)ls.ob_buf[j]; st.ob_c16[j] = (unsigned char)ls.ob_c16[j]; st.ob_relu[j] = (unsigned char)ls.ob_relu[j]; }
-        st.wd_bytes = (int)ls.wd_img.size() * 2; st.wp_bytes = (int)ls.wp_img.size() * 2;
-        wd_max = std::max(wd_max, st.wd_bytes); wp_max = std::max(wp_max, st.wp_bytes);
-        st.bias_dw = (int)bias.size(); bias.insert(bias.end(), ls.bd.begin(), ls.bd.end());
-        while (bias.size() % 4) bias.push_back(0.f);
+        st.wp_bytes = (int)ls.wp_img.size() * 2;
+        wp_max = std::max(wp_max, st.wp_bytes);
         st.bias_pw = (int)bias.size(); bias.insert(bias.end(), ls.bp.begin(), ls.bp.end());
         while (bias.size() % 4) bias.push_back(0.f);
         st.store_buf = -1; st.store_map = -1;
         // furthest byte a (partial) MMA tile of this stage may read: rows past the range + one tap
         const TchBuf &bi = a.buf[ls.in_buf];
         const int ntile = (st.nrows * Wl + 127) / 128;
-        mt += ntile * (ls.type == TCH_DWPW ? 2 : 1);
-        const int pos0 = (ls.type == TCH_DWPW && ls.stride == 2) ? bi.slack : bi.slack + (st.rows_lo - bi.rows_lo) * Wl;
-        const int last_plane = (ls.type == TCH_DWPW && ls.stride == 2) ? 3 * a.plane_stride : 0;
-        read_end = std::max(read_end, bi.off + last_plane + (bi.slabs - 1) * bi.slab_stride + (pos0 + ntile * 128 + Wl + 2) * bi.row);
+        mt += ntile;
+        const int pos0 = bi.slack + (st.rows_lo - bi.rows_lo) * Wl;
+        read_end = std::max(read_end, bi.off + (bi.slabs - 1) * bi.slab_stride + (pos0 + ntile * 128 + Wl + 2) * bi.row);
     }
     c.mtiles = mt;
     // a stage's outputs are stored once the LAST stage writing the buffer is complete
@@ -296,21 +249,17 @@ bool finalize_chain(rf_handle h, TileChain &c, int TH, int max_faces, bool resid
         bias.insert(bias.end(), mw, mw + c.merge_w.size() / 2);
     }
     // weights, bias arena, NMS scratch behind the buffers
-    const int nms_need = c.fused_nms ? (int)((sizeof(NmsSmem) + 15) / 16 * 16 + sizeof(int) * (size_t)max_faces) : 0;
+    const int nms_need = c.level >= 0 ? (int)((sizeof(NmsSmem) + 15) / 16 * 16 + sizeof(int) * (size_t)max_faces) : 0;
     a.resident = resident ? 1 : 0;
     int cursor = round_up(top, 1024);
     if (resident) {
-        // every stage keeps its own weight regions for the CTA's lifetime
-        for (int s = 0; s < ns; s++) {
-            a.st[s].wd_smem = cursor; cursor += round_up(a.st[s].wd_bytes, 128);
-            a.st[s].wp_smem = cursor; cursor += round_up(a.st[s].wp_bytes, 128);
-        }
-        a.wd_smem = a.wp_smem = cursor;
+        // every stage keeps its own weight region for the CTA's lifetime
+        for (int s = 0; s < ns; s++) { a.st[s].wp_smem = cursor; cursor += round_up(a.st[s].wp_bytes, 128); }
+        a.wp_smem = cursor;
         // NMS scratch: the input tile's region (dead by then, never TMA-stored) when large enough
         if (nms_need && bytes[0] >= nms_need) a.head.nms_smem = a.buf[0].off;
         else { a.head.nms_smem = cursor; cursor += round_up(nms_need, 128); }
     } else {
-        a.wd_smem = cursor; cursor += round_up(wd_max, 128);
         a.wp_smem = cursor; cursor += std::max(round_up(wp_max, 128), round_up(nms_need, 128));
         a.head.nms_smem = a.wp_smem;
     }
@@ -330,28 +279,17 @@ bool finalize_chain(rf_handle h, TileChain &c, int TH, int max_faces, bool resid
 // copies the packed weights + bias arena of a finalised chain into the handle's upload staging
 void commit_chain(Builder &B, TileChain &c) {
     rf_handle h = B.h;
-    for (size_t s = 0; s < c.stages.size(); s++) {
-        auto &ls = c.stages[s];
-        if (!ls.wd_img.empty()) c.args.st[s].wd_off = (int)(B.add_weights_h(ls.wd_img) * 2);
-        c.args.st[s].wp_off = (int)(B.add_weights_h(ls.wp_img) * 2);
-    }
+    for (size_t s = 0; s < c.stages.size(); s++) c.args.st[s].wp_off = (int)(B.add_weights_h(c.stages[s].wp_img) * 2);
     c.bias_off = B.add_weights(h->tile_bias_tmp);
 }
 
-int env_int(const char *name, int dflt) {
-    const char *v = getenv(name);
-    return v && *v ? atoi(v) : dflt;
-}
-
 // picks the tile height: among the heights that fit, the one with the least (waves x MMA tiles per CTA), ties to the taller
-bool choose_tile(rf_handle h, TileChain &c, int max_batch, int max_faces, int force_th) {
+bool choose_tile(rf_handle h, TileChain &c, int max_batch, int max_faces) {
     double best = 1e30;
     int best_th = 0;
     bool best_res = false;
-    const bool allow_res = env_int("RF_TILE_RESIDENT", 1) != 0;
     for (int th = 1; th <= std::min(c.H, 32); th++) {
-        if (force_th > 0 && th != force_th) continue;
-        for (int res = allow_res ? 1 : 0; res >= 0; res--) {
+        for (int res = 1; res >= 0; res--) {
             if (!finalize_chain(h, c, th, max_faces, res != 0)) continue;
             const long tiles = (long)max_batch * c.args.tiles_per_img;
             // k_tile_chain's register budget allows one CTA per SM, and its grid is one CTA per SM
@@ -364,23 +302,6 @@ bool choose_tile(rf_handle h, TileChain &c, int max_batch, int max_faces, int fo
     }
     if (!best_th) return false;
     return finalize_chain(h, c, best_th, max_faces, best_res);
-}
-
-int forced_th(const std::string &chain) {
-    // RF_TILE_TH="A=4,B=2,ssh2=7": per-chain tile heights for experiments
-    const char *v = getenv("RF_TILE_TH");
-    if (!v) return 0;
-    std::string s(v);
-    size_t p = 0;
-    while (p < s.size()) {
-        size_t e = s.find(',', p);
-        if (e == std::string::npos) e = s.size();
-        const std::string item = s.substr(p, e - p);
-        const size_t eq = item.find('=');
-        if (eq != std::string::npos && item.substr(0, eq) == chain) return atoi(item.c_str() + eq + 1);
-        p = e + 1;
-    }
-    return 0;
 }
 
 void launch_chain(rf_handle h, const std::shared_ptr<TileChain> &cp, const Run &r) {
@@ -419,8 +340,7 @@ void launch_chain(rf_handle h, const std::shared_ptr<TileChain> &cp, const Run &
     const TchBuf &b0 = a.buf[0];
     const int bc = std::min(c.in_C, 64);
     auto T_ = [&](int id) { return r.ctx.arena + h->tensors[id].offset; };
-    if (c.in_s2) maps.in = make_map(T_(c.in_tensor), c.in_C, c.in_W, c.in_H, n, bc, 2 * a.Wl, 2 * b0.nrows, 2);
-    else maps.in = make_map(T_(c.in_tensor), c.in_C, c.in_W, c.in_H, n, bc, a.Wl, b0.nrows, 1);
+    maps.in = make_map(T_(c.in_tensor), c.in_C, c.in_W, c.in_H, n, bc, a.Wl, b0.nrows, 1);
     if (c.merge_tensor >= 0) maps.aux = make_map(T_(c.merge_tensor), 64, c.W / 2, c.H / 2, n, 64, c.W / 2 + 2, a.merge_rows, 1);
     for (int i = 0; i < c.nstores; i++) maps.st[i] = make_map(T_(c.bufs[c.store_buf_of[i]].store_tensor), c.store_C[i], c.W, c.H, n, std::min(c.store_C[i], 64), c.W, 1, 1);
     if (c.level >= 0) {
@@ -429,7 +349,7 @@ void launch_chain(rf_handle h, const std::shared_ptr<TileChain> &cp, const Run &
         a.head.params = r.ctx.d_params;
         a.head.net_w = h->cfg.net_w; a.head.net_h = h->cfg.net_h;
         a.head.done = r.ctx.pb.tile_done;
-        a.head.expected = (c.fused_nms && !r.single) ? h->tile_expected : 0;    // a step launched on its own: no last-block NMS
+        a.head.expected = r.single ? 0 : h->tile_expected;    // a step launched on its own: no last-block NMS
         for (int k = 0; k < 3; k++) a.head.blobs[k] = r.blobs ? r.blobs[3 * c.level + k] : nullptr;
     }
     const int grid = std::min(a.ntiles, h->num_sms);
@@ -482,76 +402,27 @@ cudaError_t tile_init() {
     return cudaFuncSetAttribute(k_tile_chain<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, TCH_SMEM_LIMIT);
 }
 
-// RF_TILE_MASK bits: which parts of the FP16 plan run as tile chains; the others use the round-1 kernels.
-enum { TM_A = 1, TM_B = 2, TM_C = 4, TM_D = 8, TM_E = 16, TM_AGGR = 32, TM_SSH = 64, TM_HEAD = 128, TM_NMS = 256, TM_ALL = 511 };
-// Selection per mode (tools/mask_sweep.py measures the alternatives): with ONE execution context (a single forward at a
-// time: the blocking / latency mode) the SSH + predictor + NMS chains (and, at batch 1-2, the merge+aggr chains) save
-// launches and round trips through memory; with several contexts overlapping batches (throughput mode) what counts is SM
-// time per step, where the per-layer kernels win -- there only the fused decode + NMS tail is taken over.  The backbone
-// chains (depthwise on tensor cores) do more tensor-core work than the per-layer kernels' CUDA-core stencils.
-constexpr unsigned TM_LATENCY = TM_SSH | TM_HEAD | TM_NMS;
-constexpr unsigned TM_LATENCY_SMALL = TM_AGGR | TM_SSH | TM_HEAD | TM_NMS;      // max_batch <= 2
-constexpr unsigned TM_THROUGHPUT = 0;
-
-// The FP16 tensor-core plan for one mask: the backbone segments, FPN merge + aggr and SSH levels run as tile chains where the
-// mask selects them and they fit, as the per-layer kernels of plan_fp.cu otherwise (mask 0: per layer throughout).
+// The FP16 tensor-core plan.  With ONE execution context (a single forward at a time: the blocking / latency mode) the SSH
+// chains with the predictors, decode and last-block NMS fused in (and, at batch 1-2, the merge + aggr chains) save launches
+// and round trips through memory (tools/plan_sweep.py measures them against the per-layer kernels); with several contexts
+// overlapping batches (throughput mode) what counts is SM time per step, where the per-layer kernels win -- there only the
+// fused decode + NMS tail is taken over.  Every part without a chain, or whose chain does not fit, runs per layer.
 struct TileOps : PlanOps {
-    unsigned mask;
-    const bool single = env_int("RF_TILE_SINGLE", 0) != 0;   // one chain per depthwise+pointwise pair (no halo recomputation)
+    const bool ssh_chains, chain_heads, aggr_chains;
     std::shared_ptr<TileChain> ssh_chain[3];                  // the SSH chains: the last-block NMS needs all three
     bool split_heads = false;                                 // some level's predictors are fused, others not: no plan
-    TileOps(rf_handle h, unsigned m) : PlanOps(h), mask(m) {
-        if (!(mask & TM_SSH)) mask &= ~(TM_HEAD | TM_NMS);
-        if (!(mask & TM_HEAD)) mask &= ~TM_NMS;
-    }
+    TileOps(rf_handle h, bool chains, bool with_heads)
+        : PlanOps(h), ssh_chains(chains), chain_heads(chains && with_heads), aggr_chains(chains && h->cfg.max_batch <= 2) {}
     int stem(const StemNode &n) override { return plan_stem_fused<__half>(B, n, "", 1.0f); }
     int pair(const PairNode &p, int in) override { return plan_pair_tc(B, p, in); }
     void conv(const ConvNode &c) override { plan_conv_tc(B, c); }
     int merge(const MergeNode &m) override { return plan_fpn_merge_h2(B, m); }
     bool fuse_merge(const MergeNode &m) override { return aggr_fits_one_wave(B.h, m.h, m.w); }
 
-    // a backbone chain over the segment's pairs (the first may be stride 2) + its lateral conv
-    SegOut segment(const SegNode &s, int in) override {
-        if (single && s.pairs.size() > 1) {
-            SegOut o{in, -1};
-            for (size_t k = 0; k < s.pairs.size(); k++) {
-                SegNode one{s.chain + std::to_string(s.pairs[k].i), s.id, {s.pairs[k]}, {}, {}};
-                if (k + 1 == s.pairs.size()) { one.lat = s.lat; one.lat_out = s.lat_out; }
-                o = segment(one, o.out);
-            }
-            return o;
-        }
-        rf_handle h = B.h;
-        const bool enabled = s.id < 5 && (mask & (TM_A << s.id));      // TM_A .. TM_E; the last segment never runs as a chain
-        const PairNode &p0 = s.pairs[0];
-        const int cin = p0.dw->cout, S = p0.dw->stride, oh = p0.h / S, ow = p0.w / S, Cout = s.pairs.back().pw->cout;
-        const bool lat = !s.lat.cs.empty();
-        if (!enabled) return PlanOps::segment(s, in);
-        auto c = std::make_shared<TileChain>();
-        c->name = "tile_" + s.chain;
-        c->in_tensor = in; c->in_C = cin; c->in_W = p0.w; c->in_H = p0.h; c->in_s2 = S == 2;
-        c->W = ow; c->H = oh;
-        int b = add_buf(*c, cin);
-        c->bufs[b].is_input = true;
-        for (size_t k = 0; k < s.pairs.size(); k++) {
-            int nb = add_buf(*c, s.pairs[k].pw->cout, k + 1 == s.pairs.size());
-            add_dwpw(*c, b, *s.pairs[k].dw, *s.pairs[k].pw, nb);
-            b = nb;
-        }
-        if (lat) add_conv(*c, b, s.lat.cs, {{add_buf(*c, 64, true), 0, 1}});
-        // tensors are created only once the chain is known to fit (a failed chain leaves no trace in the plan)
-        if (!choose_tile(h, *c, h->cfg.max_batch, h->cfg.max_faces, forced_th(s.chain))) return PlanOps::segment(s, in);
-        SegOut o{B.tensor(s.pairs.back().out, oh, ow, Cout), -1};
-        c->bufs[(int)s.pairs.size()].store_tensor = o.out;
-        if (lat) { o.lat = B.tensor(s.lat_out, oh, ow, 64); c->bufs[(int)s.pairs.size() + 1].store_tensor = o.lat; }
-        add_chain_step(B, c, 0, ((double)p0.h * p0.w * cin + (double)oh * ow * Cout + (lat ? (double)oh * ow * 64 : 0.0)) * 2);
-        return o;
-    }
-
     // merged = lat + upsample(up); aggr 3x3 64->64
     void merge_aggr(const MergeNode &m) override {
         rf_handle h = B.h;
-        if (!(mask & TM_AGGR)) return PlanOps::merge_aggr(m);
+        if (!aggr_chains) return PlanOps::merge_aggr(m);
         auto c = std::make_shared<TileChain>();
         c->name = "tile_" + m.lv + "_merge+aggr";
         c->in_tensor = m.lat; c->in_C = 64; c->in_W = m.w; c->in_H = m.h;
@@ -565,15 +436,15 @@ struct TileOps : PlanOps {
         c->bufs[bm].is_merge = true;
         int bo = add_buf(*c, 64, true, m.aggr.out[0].t);
         add_conv(*c, bi, m.aggr.cs, {{bo, 0, 1}});
-        if (!choose_tile(h, *c, h->cfg.max_batch, h->cfg.max_faces, forced_th("aggr" + m.lv))) return PlanOps::merge_aggr(m);
+        if (!choose_tile(h, *c, h->cfg.max_batch, h->cfg.max_faces)) return PlanOps::merge_aggr(m);
         add_chain_step(B, c, 0, ((double)m.h * m.w * 64 * 2 + (double)(m.h / 2) * (m.w / 2) * 64) * 2);
     }
 
     void ssh(const SshNode &n) override {
         rf_handle h = B.h;
-        if (!(mask & TM_SSH)) return PlanOps::ssh(n);
+        if (!ssh_chains) return PlanOps::ssh(n);
         auto c = std::make_shared<TileChain>();
-        c->name = "tile_ssh_" + n.lv + ((mask & TM_HEAD) ? "+heads+decode" : "");
+        c->name = "tile_ssh_" + n.lv + (chain_heads ? "+heads+decode" : "");
         c->in_tensor = n.in; c->in_C = 64; c->in_W = n.w; c->in_H = n.h;
         c->W = n.w; c->H = n.h;
         int bi = add_buf(*c, 64);
@@ -585,12 +456,11 @@ struct TileOps : PlanOps {
         add_conv(*c, bi, {n.conv1, n.ctx_conv1}, {{bcat, 0, 1}, {bctx1, 0, 1}});
         add_conv(*c, bctx1, {n.ctx_conv2, n.ctx_conv3_1}, {{bcat, 32, 1}, {bctx31, 0, 1}});
         add_conv(*c, bctx31, {n.ctx_conv3_2}, {{bcat, 48, 1}});
-        if (mask & TM_HEAD) {
+        if (chain_heads) {
             add_head(*c, bcat, n.pred);
             c->level = n.level;
-            c->fused_nms = (mask & TM_NMS) != 0;
         }
-        if (!choose_tile(h, *c, h->cfg.max_batch, h->cfg.max_faces, forced_th("ssh" + n.lv))) return PlanOps::ssh(n);
+        if (!choose_tile(h, *c, h->cfg.max_batch, h->cfg.max_faces)) return PlanOps::ssh(n);
         add_chain_step(B, c, n.lane, ((double)n.h * n.w * 64 * 2) * 2);
         ssh_chain[n.level] = c;
     }
@@ -598,33 +468,28 @@ struct TileOps : PlanOps {
     void heads(const HeadsNode &n) override {
         rf_handle h = B.h;
         const float one[3] = {1.f, 1.f, 1.f};
-        h->tile_mask = mask;
-        if (!(ssh_chain[0] && ssh_chain[1] && ssh_chain[2] && (mask & TM_HEAD))) {
+        if (!(ssh_chain[0] && ssh_chain[1] && ssh_chain[2] && chain_heads)) {
             // some level's predictors are not fused: none may be (one decode kernel covers all levels)
             for (auto &c : ssh_chain)
                 if (c && c->level >= 0) split_heads = true;
-            if (!split_heads) plan_heads<__half>(B, n, one, "", true);
+            if (!split_heads) plan_heads<__half>(B, n, one, "");
             return;
         }
-        h->head_step = (int)h->steps.size() - 1;          // the stride-8 SSH chain (last step) emits the last candidates
         h->tile_expected = ssh_chain[0]->args.tiles_per_img + ssh_chain[1]->args.tiles_per_img + ssh_chain[2]->args.tiles_per_img;
-        if (!(mask & TM_NMS)) plan_heads<__half>(B, n, one, "", false);
     }
 };
 
 void build_plan_tiles(rf_handle h) {
-    // the chain plan is meant for one forward at a time AND small batches (tools/mask_sweep.py compares the selections); at
-    // large batches every per-layer kernel fills the GPU.  RF_FLAG_LEGACY_TC: no chains.
-    const bool latency_mode = h->cfg.streams == 1 && h->cfg.max_batch <= 16;
-    const unsigned dflt = !latency_mode ? TM_THROUGHPUT : (h->cfg.max_batch <= 2 ? TM_LATENCY_SMALL : TM_LATENCY);
-    const unsigned mask = (h->cfg.flags & RF_FLAG_LEGACY_TC) ? 0u : (unsigned)env_int("RF_TILE_MASK", (int)dflt);
-    for (unsigned m : {mask, mask & ~(unsigned)(TM_HEAD | TM_NMS)}) {
+    // the chains are meant for one forward at a time AND small batches; at large batches every per-layer kernel fills the GPU.
+    // RF_FLAG_LEGACY_TC: no chains.
+    const bool chains = h->cfg.streams == 1 && h->cfg.max_batch <= 16 && !(h->cfg.flags & RF_FLAG_LEGACY_TC);
+    for (bool with_heads : {true, false}) {        // predictors fused into some SSH chains but not all: again without
         // a failed attempt leaves no trace
         h->steps.clear(); h->tensors.clear(); h->tensor_by_name.clear(); h->chains.clear();
         h->wstage.clear(); h->wstage_h.clear(); h->wstage_q.clear();
-        h->head_step = h->nms_step = -1; h->tile_expected = 0;
+        h->tile_expected = 0;
         for (int &f : h->feat_tensor) f = -1;
-        TileOps ops(h, m);
+        TileOps ops(h, chains, with_heads);
         walk_network(ops);
         if (!ops.split_heads) return;
     }

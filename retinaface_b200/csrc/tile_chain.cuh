@@ -3,11 +3,10 @@
 // griddepcontrol.
 //
 // One CTA owns a tile = TH full-width rows of one image and runs a CHAIN of layers on it without leaving the SM:
-// every intermediate activation stays in shared memory (or registers), only the tensors other kernels need are written
+// every intermediate activation stays in shared memory, only the tensors other kernels need are written
 // back, by TMA stores.  Layers the reference's graph (model/mnet-deconv-0517.prototxt) runs one by one inside TensorRT
 // (retinaface/tensorrt/trtretinafacenet.cpp:60) become STAGES of one launch:
-//   TCH_DWPW : depthwise 3x3 (stride 1 | 2) + BN + ReLU  ->  pointwise 1x1 + BN + ReLU   (mobilenet0_conv3 .. conv24)
-//   TCH_CONV : 1x1 or 3x3 (pad 1) convolution + BN (+ ReLU)                                (laterals, rf_c*_aggr, SSH convs)
+//   TCH_CONV : 1x1 or 3x3 (pad 1) convolution + BN (+ ReLU)                                (rf_c*_aggr, SSH convs)
 //   TCH_HEAD : the three predictor 1x1 convs of a level as ONE N = 32 GEMM (FP32-grade: hi + lo FP16 weight pieces) whose
 //              epilogue is the post-process: 2-way softmax, threshold, anchor decode, clip, candidate append
 //              (RetinaFace.cpp:666-723) -- and, in the last CTA that finishes an image, sort + greedy NMS (:434-492).
@@ -22,13 +21,7 @@
 //
 // Data movement.  Activations enter by TMA tiled loads (4-D NHWC tensor map, box {<=64 channels, Wl, rows}, out-of-bounds
 // fill = the zero padding) in SWIZZLE_128B / 64B / 32B mode (64 / 32 / 16 channels per row), which is exactly the wgmma
-// K-major swizzled operand layout; stride-2 depthwise inputs arrive as four parity planes (tensor-map element strides 2).
-// Epilogue threads write stage outputs into shared memory in the same swizzled layout.
-//
-// Depthwise on tensor cores.  out[p][c] = sum_t in[p + shift_t][c] * w_t[c] is 9 * C/16 MMAs with M = 64, N = K = 16 and
-// B = diag(w_t[16 channels]): no CUDA-core instruction per tap.  The accumulator of one 16-channel slab, + bias, ReLU and
-// packed to FP16, is in registers exactly the A fragment of the pointwise GEMM's K step over those channels
-// (wgmma.cuh), so the pointwise GEMM takes its A operand from registers.
+// K-major swizzled operand layout.  Epilogue threads write stage outputs into shared memory in the same swizzled layout.
 //
 // Roles (288 threads): warps 0-3 / 4-7 = two compute warpgroups that take the MMA tiles of a stage in turn, each issuing
 // its own MMAs and running the epilogue from its accumulators; warp 8 = TMA producer (tiles, per-stage weights, TMA
@@ -47,7 +40,7 @@ constexpr int TCH_THREADS = 288;
 constexpr int TCH_MAX_STAGES = 8;
 constexpr int TCH_MAX_BUFS = 8;
 constexpr int TCH_EPI_THREADS = 256;
-enum { TCH_CONV = 0, TCH_DWPW = 1, TCH_HEAD = 2 };
+enum { TCH_CONV = 0, TCH_HEAD = 1 };
 
 struct TchBuf {
     int off;            // byte offset in dynamic shared memory (1024-aligned); position index 0 lives here
@@ -61,14 +54,13 @@ struct TchBuf {
 
 struct TchStage {
     int type;
-    int Cin, N;               // DWPW: depthwise channels / pointwise outputs; CONV, HEAD: input / output channels
-    int taps, stride;         // CONV: 1 | 9;  DWPW: stride 1 | 2 (2: stage 0 only, input = parity planes)
+    int Cin, N;               // input / output channels
+    int taps;                 // CONV: 1 | 9;  HEAD: 1
     int in_buf;
     int rows_lo, nrows;       // local rows this stage computes
-    int wd_off, wd_bytes;     // depthwise diagonal B tiles in the weight arena
     int wp_off, wp_bytes;     // B image [K/8][N][8] (HEAD: hi image then lo image)
-    int wd_smem, wp_smem;     // resident weights: this stage's own regions in shared memory
-    int bias_dw, bias_pw;     // float offsets into the bias arena
+    int wp_smem;              // resident weights: this stage's own region in shared memory
+    int bias_pw;              // float offset into the bias arena
     int store_buf, store_map; // -1 | buffer whose owned rows [HT, HT + TH) are TMA-stored once the stage is complete
     unsigned char ob_buf[16], ob_c16[16], ob_relu[16];   // per 16-column output block: buffer, channel offset / 16, ReLU
 };
@@ -90,15 +82,15 @@ struct TchArgs {
     TchBuf buf[TCH_MAX_BUFS];
     int Wl, HT, TH;
     int W, H, nimg, tiles_per_img, ntiles;
-    int wd_smem, wp_smem, bias_smem, smem_bytes;     // byte offsets in dynamic shared memory / total
+    int wp_smem, bias_smem, smem_bytes;              // byte offsets in dynamic shared memory / total
     int resident;             // 1: the weights of ALL stages stay in shared memory for the CTA's lifetime (loaded once, before
-                              // griddepcontrol.wait); 0: streamed per stage through the wd / wp buffers
+                              // griddepcontrol.wait); 0: streamed per stage through the wp buffer
     unsigned *dbg;            // host-mapped word: code of the hand-off a timed-out wait was stuck on (0: none)
     unsigned long long *trace;   // -DRF_TCH_TRACE builds: timeline of CTA 0 (count, then (code, ns) pairs)
     const unsigned char *warena;
     const float *bias;
     int bias_floats;
-    int in_s2, plane_stride, in_C;
+    int in_C;
     unsigned in_bytes;
     // FPN merge pre-stage (merge_C > 0): buffer 0 += crop(deconv(coarse)); coarse tile in buffer `merge_buf`
     int merge_C, merge_buf, merge_rows, merge_w_bias;   // merge_w_bias: float offset of the [16 taps][C] FP16 weights in the bias arena
@@ -107,7 +99,7 @@ struct TchArgs {
 };
 
 struct TchMaps {
-    CUtensorMap in;           // chain input (stride 2: element strides {1, 2, 2, 1})
+    CUtensorMap in;           // chain input
     CUtensorMap aux;          // FPN merge: the coarser level
     CUtensorMap st[3];        // TMA stores
 };
@@ -148,7 +140,8 @@ __device__ __forceinline__ void wait_warp(uint64_t *bar, unsigned parity, unsign
     wait(bar, parity, dbg, code);
     __syncwarp();
 }
-// Optional timeline of CTA 0 (build with -DRF_TCH_TRACE; tools/tile_bringup.py --trace): (event code, globaltimer ns) pairs
+// Optional timeline of CTA 0 (build with -DRF_TCH_TRACE; launch_chain prints the last launch's events of each chain to stderr):
+// (event code, globaltimer ns) pairs
 #ifdef RF_TCH_TRACE
 __device__ __forceinline__ void trace(unsigned long long *t, unsigned code) {
     if (t && blockIdx.x == 0) {
@@ -195,7 +188,7 @@ struct BlkGeo {
     uint32_t abase;           // A operand: position q0 of the stage, tap (0, 0), K step 0
     uint32_t row, slab;       // input buffer: bytes per position per slab, bytes between slabs
     int lkpr, kpr;
-    uint32_t wd, wp;          // weight images
+    uint32_t wp;              // weight image
     int q0, npos, Y0;
 };
 
@@ -258,56 +251,12 @@ __device__ __forceinline__ void conv_chunk(float (&d)[NC / 2], int n0, const Tch
     wg::fence_regs(d);
 }
 
-// depthwise (diagonal B tiles, tap-major image: tile (t, k) at (t * NK + k) * 512 bytes) -> + bias, ReLU, FP16 in registers ->
-// pointwise GEMM with A from registers -> stage output
-template <int NK>
-__device__ __forceinline__ void dwpw_block(const TchArgs &a, const TchStage &st, unsigned char *smem, const float *s_bias, const uint32_t (&tapb)[9],
-                                           const BlkGeo &k) {
-    const int t4 = threadIdx.x & 3;
-    const float *bd = s_bias + st.bias_dw;
-    uint32_t af[NK][4];
-#pragma unroll
-    for (int kk = 0; kk < NK; kk++) {
-        float d[8];
-#pragma unroll
-        for (int i = 0; i < 8; i++) d[i] = 0.f;
-        const uint32_t ak = k.abase + k_off(kk, k.lkpr, k.kpr, k.slab);
-        wg::fence();
-#pragma unroll
-        for (int t = 0; t < 9; t++) wg::mma_ss<16>(d, wg::desc_sw(ak + tapb[t], k.row), wg::desc(k.wd + (uint32_t)(t * NK + kk) * 512u, 256, 128), t > 0);
-        wg::commit();
-        wg::wait<0>();
-        wg::fence_regs(d);
-#pragma unroll
-        for (int h = 0; h < 2; h++) {       // columns 8 h + 2 t4, + 1 of rows r, r + 8 -> A fragment registers 2 h, 2 h + 1
-            const float2 bb = *reinterpret_cast<const float2 *>(bd + 16 * kk + 8 * h + 2 * t4);
-            af[kk][2 * h] = pack_h2(fmaxf(d[4 * h] + bb.x, 0.f), fmaxf(d[4 * h + 1] + bb.y, 0.f));
-            af[kk][2 * h + 1] = pack_h2(fmaxf(d[4 * h + 2] + bb.x, 0.f), fmaxf(d[4 * h + 3] + bb.y, 0.f));
-        }
-    }
-    const float *bp = s_bias + st.bias_pw;
-    const uint32_t lbo = (uint32_t)st.N * 16;
-    wg::for_chunks<(NK >= 16 ? 32 : 64)>(st.N, [&](auto nc, int n0) {
-        constexpr int NC = decltype(nc)::value;
-        float acc[NC / 2];
-#pragma unroll
-        for (int i = 0; i < NC / 2; i++) acc[i] = 0.f;
-        wg::fence();
-#pragma unroll
-        for (int kk = 0; kk < NK; kk++) wg::mma_rs<NC>(acc, af[kk], wg::desc(k.wp + (uint32_t)kk * 2u * lbo + (uint32_t)n0 * 16u, lbo, 128), kk > 0);
-        wg::commit();
-        wg::wait<0>();
-        wg::fence_regs(acc);
-        store_chunk<NC>(acc, n0, a, st, smem, bp, k);
-    });
-}
-
 }  // namespace tch
 
 template <int UNUSED>
 __global__ void __launch_bounds__(TCH_THREADS, 1) k_tile_chain(const __grid_constant__ TchMaps maps, const __grid_constant__ TchArgs a) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
-    __shared__ __align__(8) uint64_t bar_in, bar_bias, bar_stage, bar_tile, bar_wd_full, bar_wp_full;
+    __shared__ __align__(8) uint64_t bar_in, bar_bias, bar_stage, bar_tile, bar_wp_full;
     __shared__ int s_last;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -317,7 +266,7 @@ __global__ void __launch_bounds__(TCH_THREADS, 1) k_tile_chain(const __grid_cons
 
     if (tid == 0) {
         tc::mbar_init(&bar_in, 1); tc::mbar_init(&bar_bias, 1); tc::mbar_init(&bar_stage, 8); tc::mbar_init(&bar_tile, 8);
-        tc::mbar_init(&bar_wd_full, 1); tc::mbar_init(&bar_wp_full, 1);
+        tc::mbar_init(&bar_wp_full, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     pdl_trigger();
@@ -329,14 +278,12 @@ __global__ void __launch_bounds__(TCH_THREADS, 1) k_tile_chain(const __grid_cons
         if (lane == 0) {
             const unsigned bias_bytes = (unsigned)a.bias_floats * 4u;
             unsigned const_bytes = bias_bytes;
-            if (a.resident) for (int s = 0; s < a.nstages; s++) const_bytes += (unsigned)(a.st[s].wd_bytes + a.st[s].wp_bytes);
+            if (a.resident) for (int s = 0; s < a.nstages; s++) const_bytes += (unsigned)a.st[s].wp_bytes;
             tc::mbar_expect_tx(&bar_bias, const_bytes);
             tch::bulk_g2s_u32(sbase + a.bias_smem, a.bias, bias_bytes, &bar_bias);       // constants: independent of earlier kernels
             if (a.resident)
-                for (int s = 0; s < a.nstages; s++) {
-                    if (a.st[s].wd_bytes) tch::bulk_g2s_u32(sbase + a.st[s].wd_smem, a.warena + a.st[s].wd_off, (unsigned)a.st[s].wd_bytes, &bar_bias);
+                for (int s = 0; s < a.nstages; s++)
                     tch::bulk_g2s_u32(sbase + a.st[s].wp_smem, a.warena + a.st[s].wp_off, (unsigned)a.st[s].wp_bytes, &bar_bias);
-                }
             tch::prefetch_map(&maps.in);
             pdl_wait();                                                                   // activations of earlier kernels from here on
             unsigned sc = 0;
@@ -358,16 +305,8 @@ __global__ void __launch_bounds__(TCH_THREADS, 1) k_tile_chain(const __grid_cons
                 if (it > 0) { tch::wait(&bar_tile, (it - 1) & 1, a.dbg, __LINE__); tch::bulk_wait_read0(); }   // buffers free, stores have read them
                 tc::mbar_expect_tx(&bar_in, a.in_bytes + a.merge_bytes);
                 const int in_slabs = (a.in_C + 63) >> 6;
-                if (!a.in_s2) {
-                    for (int s = 0; s < in_slabs; s++)
-                        tch::tma_load_4d(sbase + B0.off + s * B0.slab_stride + B0.slack * B0.row, &maps.in, &bar_in, s * 64, -1, Y0 + B0.rows_lo, b);
-                } else {
-                    // plane (py, px) element (pr, lx) = input(2 * (Y0 + rows_lo0 - 1 + pr) + py, 2 * (lx - 1) + px)
-                    for (int k = 0; k < 4; k++)
-                        for (int s = 0; s < in_slabs; s++)
-                            tch::tma_load_4d(sbase + B0.off + k * a.plane_stride + s * B0.slab_stride + B0.slack * B0.row, &maps.in, &bar_in, s * 64,
-                                             -2 + (k & 1), 2 * (Y0 + a.st[0].rows_lo - 1) + (k >> 1), b);
-                }
+                for (int s = 0; s < in_slabs; s++)
+                    tch::tma_load_4d(sbase + B0.off + s * B0.slab_stride + B0.slack * B0.row, &maps.in, &bar_in, s * 64, -1, Y0 + B0.rows_lo, b);
                 if (a.merge_C) {
                     const TchBuf &BM = a.buf[a.merge_buf];
                     // coarse rows ((Y0 + rows_lo + 1) >> 1) - 1 ..., coarse columns -1 .. W/2
@@ -377,17 +316,13 @@ __global__ void __launch_bounds__(TCH_THREADS, 1) k_tile_chain(const __grid_cons
                 for (int s = 0; s < a.nstages; s++, sc++) {
                     const TchStage &st = a.st[s];
                     // every phase of bar_stage is observed in order; stage s-1 is complete -> its TMA store, and (streamed
-                    // weights) the single weight buffers are free for stage s
+                    // weights) the single weight buffer is free for stage s
                     if (s > 0) {
                         tch::wait(&bar_stage, (sc - 1) & 1, a.dbg, __LINE__);
                         const TchStage &sp = a.st[s - 1];
                         if (sp.store_buf >= 0) store_rows(a.buf[sp.store_buf], sp.store_map, ty, b);
                     }
                     if (!a.resident) {
-                        if (st.wd_bytes) {
-                            tc::mbar_expect_tx(&bar_wd_full, (unsigned)st.wd_bytes);
-                            tch::bulk_g2s_u32(sbase + a.wd_smem, a.warena + st.wd_off, (unsigned)st.wd_bytes, &bar_wd_full);
-                        }
                         tc::mbar_expect_tx(&bar_wp_full, (unsigned)st.wp_bytes);
                         tch::bulk_g2s_u32(sbase + a.wp_smem, a.warena + st.wp_off, (unsigned)st.wp_bytes, &bar_wp_full);
                     }
@@ -408,7 +343,7 @@ __global__ void __launch_bounds__(TCH_THREADS, 1) k_tile_chain(const __grid_cons
         const float *s_bias = reinterpret_cast<const float *>(smem + a.bias_smem);
         tch::wait_warp(&bar_bias, 0, a.dbg, __LINE__);
         pdl_wait();
-        unsigned g = 0, sc = 0, wdc = 0, wpc = 0;
+        unsigned g = 0, sc = 0, wpc = 0;
         for (int tile = blockIdx.x, it = 0; tile < a.ntiles; tile += gridDim.x, it++) {
             const int b = tile / a.tiles_per_img, ty = tile - b * a.tiles_per_img;
             const int Y0 = ty * a.TH - a.HT;
@@ -456,30 +391,21 @@ __global__ void __launch_bounds__(TCH_THREADS, 1) k_tile_chain(const __grid_cons
                 const TchStage &st = a.st[s];
                 const TchBuf &BI = a.buf[st.in_buf];
                 if (sc > 0) tch::wait_warp(&bar_stage, (sc - 1) & 1, a.dbg, __LINE__);      // inputs of this stage are in shared memory
-                if (!a.resident) {
-                    if (st.wd_bytes) { tch::wait_warp(&bar_wd_full, wdc & 1, a.dbg, __LINE__); wdc++; }
-                    tch::wait_warp(&bar_wp_full, wpc & 1, a.dbg, __LINE__); wpc++;
-                }
+                if (!a.resident) { tch::wait_warp(&bar_wp_full, wpc & 1, a.dbg, __LINE__); wpc++; }
                 if (lane == 0) TCH_TRACE(100 + s);
                 const int npos = st.nrows * Wl, ntile = (npos + 127) >> 7;
                 const int kpr = BI.row >> 5;                             // 16-channel K steps per row: 1 | 2 | 4
                 // position index (in the input buffer) of this stage's position 0
-                const int pos0 = st.type == TCH_DWPW && st.stride == 2 ? BI.slack : BI.slack + (st.rows_lo - BI.rows_lo) * Wl;
+                const int pos0 = BI.slack + (st.rows_lo - BI.rows_lo) * Wl;
                 tch::BlkGeo k;
                 k.row = (uint32_t)BI.row; k.slab = (uint32_t)BI.slab_stride;
                 k.kpr = kpr; k.lkpr = kpr == 4 ? 2 : (kpr == 2 ? 1 : 0);
-                k.wp = sbase + (a.resident ? st.wp_smem : a.wp_smem); k.wd = sbase + (a.resident ? st.wd_smem : a.wd_smem);
+                k.wp = sbase + (a.resident ? st.wp_smem : a.wp_smem);
                 k.npos = npos; k.Y0 = Y0;
-                // per tap: operand shift (+ parity plane for stride 2), bytes
+                // per tap: operand shift, bytes
                 uint32_t tapb[9];
 #pragma unroll
-                for (int t = 0; t < 9; t++) {
-                    const int dy = t / 3 - 1, dx = t % 3 - 1;
-                    int shift, plane = 0;
-                    if (st.type == TCH_DWPW && st.stride == 2) { plane = ((dy & 1) << 1) | (dx & 1); shift = (dy >= 0 ? Wl : 0) + (dx < 0 ? -1 : 0); }
-                    else shift = dy * Wl + dx;
-                    tapb[t] = (uint32_t)(shift * BI.row + plane * a.plane_stride);
-                }
+                for (int t = 0; t < 9; t++) tapb[t] = (uint32_t)(((t / 3 - 1) * Wl + t % 3 - 1) * BI.row);
                 const float *bp = s_bias + st.bias_pw;
                 for (int m = 0; m < ntile; m++) {
                     if ((int)((g + m) & 1) != wgi) continue;             // the warpgroups take the MMA tiles in turn
@@ -487,15 +413,7 @@ __global__ void __launch_bounds__(TCH_THREADS, 1) k_tile_chain(const __grid_cons
                         k.q0 = m * 128 + hb * 64;
                         if (k.q0 >= npos) break;
                         k.abase = sbase + BI.off + (uint32_t)(pos0 + k.q0) * (uint32_t)BI.row;
-                        if (st.type == TCH_DWPW) {
-                            switch (st.Cin >> 4) {
-                                case 1: tch::dwpw_block<1>(a, st, smem, s_bias, tapb, k); break;
-                                case 2: tch::dwpw_block<2>(a, st, smem, s_bias, tapb, k); break;
-                                case 4: tch::dwpw_block<4>(a, st, smem, s_bias, tapb, k); break;
-                                case 8: tch::dwpw_block<8>(a, st, smem, s_bias, tapb, k); break;
-                                default: tch::dwpw_block<16>(a, st, smem, s_bias, tapb, k); break;
-                            }
-                        } else if (st.type == TCH_CONV) {
+                        if (st.type == TCH_CONV) {
                             wg::for_chunks<64>(st.N, [&](auto nc, int n0) {
                                 constexpr int NC = decltype(nc)::value;
                                 float d[NC / 2];

@@ -73,9 +73,8 @@ class Plan:
     prec: str                # fp32 | fp16 | int8
     max_batch: int
     streams: int = 0
-    tile_mask: str = ""      # RF_TILE_MASK ("" unset)
-    nms: str = "fused"       # which NMS instantiation the plan holds: fused (k_head_decode's last block), chain (the SSH tile chains'
-                             # last CTA) or kernel (k_nms behind a stand-alone decode)
+    nms: str = "fused"       # which NMS instantiation the plan holds: fused (k_head_decode's last block) or chain (the SSH tile
+                             # chains' last CTA)
 
     @property
     def model(self):
@@ -89,9 +88,8 @@ class Plan:
 PLANS = {
     "fp32_448": Plan((448, 448), "fp32", 4),
     "fp16_448_b8": Plan((448, 448), "fp16", 8),                                        # the benchmarked FP16 plan
-    "fp16_448_latency_b8": Plan((448, 448), "fp16", 8, streams=1, nms="chain"),        # TM_LATENCY
-    "fp16_448_latency_b2": Plan((448, 448), "fp16", 2, streams=1, nms="chain"),        # TM_LATENCY_SMALL
-    "fp16_448_latency_mask255": Plan((448, 448), "fp16", 8, streams=1, tile_mask="255", nms="kernel"),
+    "fp16_448_latency_b8": Plan((448, 448), "fp16", 8, streams=1, nms="chain"),        # SSH + predictor + NMS chains
+    "fp16_448_latency_b2": Plan((448, 448), "fp16", 2, streams=1, nms="chain"),        # + merge + aggr chains
     "int8_448_b32": Plan((448, 448), "int8", 32),                                      # the benchmarked INT8 plan
     "fp16_1280x896_b3": Plan((896, 1280), "fp16", 3),
     "fp16_1280x896_latency_b3": Plan((896, 1280), "fp16", 3, streams=1),             # the SSH chains do not fit this size
@@ -105,11 +103,8 @@ def nms_variant(plan_text: str) -> str:
     steps = [ln.split(": ", 1)[1] for ln in plan_text.splitlines() if ln.startswith("step lane")]
     fused = [s for s in steps if s.endswith("heads_1x1+softmax+decode+nms_all_levels")]
     chain = [s for s in steps if re.fullmatch(r"tile_ssh_c\d\+heads\+decode", s)]
-    kernel = [s for s in steps if s == "sort+nms" or s.endswith("_sort+nms")]
-    if len(fused) == 1 and not chain and not kernel:
+    if len(fused) == 1 and not chain:
         return "fused"
-    if len(chain) == 3 and not fused and not kernel:
+    if len(chain) == 3 and not fused:
         return "chain"
-    if len(kernel) == 1 and not fused:
-        return "kernel"
     return "unknown: " + ", ".join(steps[-4:])

@@ -32,7 +32,6 @@ class Case(NamedTuple):
     placement: bool = False  # also run a handle with the production (liveness) buffer placement
     mutate: bool = False     # also apply the mutations of oracle.fp16_steps to one step's engine output
     streams: int = 0         # 1: the latency plans (tile chains for SSH + heads + NMS, and merge + aggr at max_batch <= 2)
-    tile_mask: str = ""      # RF_TILE_MASK ("511": every chain, backbone segments A .. E included)
 
 
 CASES = {
@@ -49,20 +48,13 @@ CASES = {
     "deconv_448_mb8": Case((448, 448), 8, (8,), model="mnet-deconv-0517"),
     "latency_448_mb8": Case((448, 448), 8, (8,), streams=1),        # SSH + heads + NMS chains
     "latency_448_mb2": Case((448, 448), 2, (2,), streams=1),        # + merge + aggr chains
-    "chains_448_mb5": Case((448, 448), 5, (5,), streams=1, tile_mask="511"),     # backbone chains tile_A .. tile_E
-    "chains_288x416_mb3": Case((288, 416), 3, (3,), streams=1, tile_mask="511"),
+    "latency_896x1280_mb8": Case((896, 1280), 8, (3,), streams=1),   # SSH chains without the predictors, streamed weights
 }
-# the depthwise layers of the backbone chains (plan_net.cu walk_network segments A .. E)
-CHAIN_PAIRS = {"A": (3, 5), "B": (7, 9), "C": (11, 13, 15), "D": (17, 19, 21), "E": (23,)}
 
 
-def plan_steps(case, monkeypatch):
+def plan_steps(case):
     """The case's plan (rf_plan_describe, host-only): its step names and the tile-chain lines."""
     from retinaface_b200.capi import plan_describe
-    if case.tile_mask:
-        monkeypatch.setenv("RF_TILE_MASK", case.tile_mask)
-    else:
-        monkeypatch.delenv("RF_TILE_MASK", raising=False)
     text = plan_describe(caffemodel(case.model), case.hw[0], case.hw[1], max_batch=case.max_batch, flags=case.flags,
                          streams=case.streams)
     steps = [ln.split(": ", 1)[1] for ln in text.splitlines() if ln.startswith("step lane")]
@@ -71,18 +63,14 @@ def plan_steps(case, monkeypatch):
 
 
 def walk_options(steps):
-    """What the walk must know of a plan: the depthwise layers on tensor cores, whether the predictors run in the SSH chains,
-    and the tensors the chains keep in shared memory."""
-    tc_dw, inner = set(), {"_plus0", "_plus1"}
-    for seg, pairs in CHAIN_PAIRS.items():
-        if f"tile_{seg}" in steps:
-            tc_dw.update(pairs)
-            inner.update(f"mobilenet0_relu{i + 1}_fwd" for i in pairs[:-1])
+    """What the walk must know of a plan: whether the predictors run in the SSH chains, and the tensors the chains keep in
+    shared memory."""
+    inner = {"_plus0", "_plus1"}
     for lv in ("c3", "c2", "c1"):
         if any(s.startswith(f"tile_ssh_{lv}") for s in steps):
             inner.update({f"rf_{lv}_det_context_conv1_relu", f"rf_{lv}_det_context_conv3_1_relu"})
     heads = [s.endswith("+heads+decode") for s in steps if s.startswith("tile_ssh_")]
-    return tc_dw, len(heads) == 3 and all(heads), inner
+    return len(heads) == 3 and all(heads), inner
 
 
 def _engine(case, keep_all):
@@ -118,9 +106,9 @@ def check_case(case_id, eng, batch, steps, post, label, options):
     heads = eng.forward_heads(batch)
     compared, missing, diffs, report = [], [], [], []
     case = CASES[case_id]
-    tc_dw, chain_heads, inner = options
+    chain_heads, inner = options
     for name, step, iv, got in steps.walk(batch, _fetcher(eng, n), simt_stem=bool(case.flags & RF_FLAG_SIMT_STEM),
-                                          tc_dw=tc_dw, chain_heads=chain_heads):
+                                          chain_heads=chain_heads):
         if name.startswith("heads"):
             cls, bbox, lm = iv
             l = {"heads_stride32": 0, "heads_stride16": 1, "heads_stride8": 2}[name]
@@ -159,10 +147,10 @@ def post_oracle():
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("case_id", list(CASES))
-def test_fp16_engine_inside_its_rounding_intervals(case_id, golden_image, post_oracle, monkeypatch):
+def test_fp16_engine_inside_its_rounding_intervals(case_id, golden_image, post_oracle):
     case = CASES[case_id]
     h, w = case.hw
-    options = walk_options(plan_steps(case, monkeypatch)[0])      # also sets RF_TILE_MASK for the handles below
+    options = walk_options(plan_steps(case)[0])
     steps = fs.Fp16Steps(caffemodel(case.model))
     keep = _engine(case, keep_all=True)
     prod = _engine(case, keep_all=False) if case.placement else None
@@ -205,18 +193,18 @@ def _mutations_rejected(eng, batch, steps, n):
 
 
 # ---- host side ----------------------------------------------------------------------------------------------------------
-def test_fp16_sweep_covers_every_planner_branch(monkeypatch):
+def test_fp16_sweep_covers_every_planner_branch():
     """rf_plan_describe (host-only, 132 SMs assumed) for every case of the sweep: together they must run the tensor-core and
     the CUDA-core stem, the 2-D depthwise+pointwise kernel at stride 2 on C = 16, 32 and 64 and at stride 1, a 1-D depthwise
-    step on a map above 56x56, a fused and a stand-alone FPN merge, the fused heads, the SSH chains with their predictors,
-    the merge + aggr chains, and the backbone chains tile_A .. tile_E with both resident and streamed weights.  A planner
-    change that moves a branch out of the sweep fails here, without a GPU."""
+    step on a map above 56x56, a fused and a stand-alone FPN merge, the fused heads, the SSH chains with and without their
+    predictors, and the merge + aggr chains, with both resident and streamed chain weights.  A planner change that moves a
+    branch out of the sweep fails here, without a GPU."""
     import re
     stems, s2_channels, s1_2d, big_1d, fused, alone, heads = set(), set(), [], [], [], [], []
-    ssh_heads, merge_chain, backbone = [], [], {}
+    ssh_heads, ssh_alone, merge_chain, weights = [], [], [], set()
     for case_id, case in CASES.items():
         h, w = case.hw
-        steps, chains = plan_steps(case, monkeypatch)
+        steps, chains = plan_steps(case)
         for s in steps:
             if "stem_conv0" in s:
                 stems.add(s.split("stem")[0])
@@ -228,6 +216,8 @@ def test_fp16_sweep_covers_every_planner_branch(monkeypatch):
                 heads.append(case_id)
             if re.fullmatch(r"tile_ssh_c\d\+heads\+decode", s):
                 ssh_heads.append(case_id)
+            if re.fullmatch(r"tile_ssh_c\d", s):
+                ssh_alone.append(case_id)
             if re.fullmatch(r"tile_c\d_merge\+aggr", s):
                 merge_chain.append(case_id)
             m = re.fullmatch(r"tc(2d)?_dw(\d+)\+pw\d+_s(\d)_(\d+)to\d+", s)
@@ -241,12 +231,11 @@ def test_fp16_sweep_covers_every_planner_branch(monkeypatch):
                 if (h // down) * (w // down) > 56 * 56:
                     big_1d.append(case_id)
         for ln in chains:
-            m = re.match(r"tile_([A-E]):.*\((resident|streamed) weights\)", ln)
+            m = re.match(r"tile_(ssh_c\d|c\d_merge\+aggr)\S*:.*\((resident|streamed) weights\)", ln)
             if m:
-                backbone.setdefault(m.group(1), set()).add(m.group(2))
+                weights.add(m.group(2))
     assert stems == {"tc_", ""}, stems
     assert {16, 32, 64} <= s2_channels, s2_channels
     assert s1_2d and big_1d and fused and alone and heads, (s1_2d, big_1d, fused, alone, heads)
-    assert ssh_heads and merge_chain, (ssh_heads, merge_chain)
-    assert set(backbone) == set("ABCDE"), backbone
-    assert {"resident", "streamed"} <= set().union(*backbone.values()), backbone
+    assert ssh_heads and ssh_alone and merge_chain, (ssh_heads, ssh_alone, merge_chain)
+    assert weights == {"resident", "streamed"}, weights

@@ -1,7 +1,8 @@
 """GPU (-m gpu): the post-process's sort + greedy NMS under load, in each of its three instantiations (the last block of
-k_head_decode for float, half and int8 features; the last CTA of the SSH tile chains; stand-alone k_nms), on every branch of
-nms_image (tests/nms_load.py).  The score threshold of each call is derived from the engine's own heads so that a target image
-has exactly a chosen number of candidates, on both sides of every branch boundary and at every anchor; the NMS threshold is 0.4
+k_head_decode for float, half and int8 features; the last CTA of the SSH tile chains; stand-alone k_nms behind
+rf_postprocess), on every branch of nms_image (tests/nms_load.py).  The score threshold of each call is derived from the
+engine's own heads so that a target image has exactly a chosen number of candidates, on both sides of every branch boundary
+and at every anchor; the NMS threshold is 0.4
 (production), 1.0 (nothing suppressed: every candidate record is compared, and at every anchor each anchor is appended exactly
 once) and 0.0 (any overlap suppresses); max_faces is the default 256, 4 and 8192.  Every image of every call must equal the C
 oracle's post-process of the same heads (PostprocOracle.check_engine); so must rf_postprocess on those heads, and
@@ -27,18 +28,13 @@ NMS = (0.4, 1.0, 0.0)
 MAX_ROUNDS = 9000
 
 
-def _engine(plan, max_faces, monkeypatch):
+def _engine(plan, max_faces):
     from retinaface_b200 import RF_PREC_FP16, RF_PREC_FP32, RF_PREC_INT8, Engine
     from retinaface_b200.capi import plan_describe
     prec = {"fp32": RF_PREC_FP32, "fp16": RF_PREC_FP16, "int8": RF_PREC_INT8}[plan.prec]
     kw = dict(precision=prec, max_batch=plan.max_batch, int8_table=TABLE if plan.prec == "int8" else None, streams=plan.streams)
-    if plan.tile_mask:
-        monkeypatch.setenv("RF_TILE_MASK", plan.tile_mask)
-    try:
-        variant = nms_variant(plan_describe(caffemodel(plan.model), plan.hw[0], plan.hw[1], max_faces=max_faces, **kw))
-        eng = Engine(caffemodel(plan.model), plan.hw[0], plan.hw[1], max_faces=max_faces, **kw)
-    finally:
-        monkeypatch.delenv("RF_TILE_MASK", raising=False)
+    variant = nms_variant(plan_describe(caffemodel(plan.model), plan.hw[0], plan.hw[1], max_faces=max_faces, **kw))
+    eng = Engine(caffemodel(plan.model), plan.hw[0], plan.hw[1], max_faces=max_faces, **kw)
     assert variant == plan.nms, (plan, max_faces, variant)
     assert eng.max_faces == max_faces and eng.num_anchors == plan.anchors
     return eng
@@ -94,7 +90,7 @@ def _device_records(eng, n, thr, nms, dev):
 
 
 @pytest.mark.parametrize("name", list(PLANS))
-def test_nms_under_load_equals_the_oracle(name, golden_image, monkeypatch):
+def test_nms_under_load_equals_the_oracle(name, golden_image):
     import torch
     plan = PLANS[name]
     refs = _Refs(plan)
@@ -105,7 +101,7 @@ def test_nms_under_load_equals_the_oracle(name, golden_image, monkeypatch):
     reached = set()
     t_plan = time.perf_counter()
     for mf in MAX_FACES:
-        eng = _engine(plan, mf, monkeypatch)
+        eng = _engine(plan, mf)
         try:
             label = f"{name} max_faces={mf} ({plan.nms} NMS)"
             heads = eng.forward_heads(batch)

@@ -44,22 +44,19 @@ def _match(mine, ref, iou_min=0.7):
     return pairs, len(mine) - len(pairs), len(ref) - len(pairs)
 
 
-@pytest.mark.parametrize("hw,nb", [((448, 448), 5), ((896, 1280), 2), ((288, 416), 3)])
-@pytest.mark.parametrize("mask", [511, 490, 255, 127, 63])
-def test_tile_chains_equal_round1_kernels(mask, hw, nb, golden_image, monkeypatch):
-    """The tile-chain plan (RF_TILE_MASK: 511 every chain; 490 the default selection; 255 stand-alone NMS; 127 stand-alone predictors
-    + NMS; 63 round-1 SSH)
-    against one round-1 kernel per layer (RF_FLAG_LEGACY_TC): every tensor both plans materialise within 2e-2 of its max
-    (depthwise weights are FP16 diagonal tiles in the chains, FP32 in the round-1 stencil), head blobs within 1e-2, and the
-    SAME faces (anchor indices) within 0.25 px / 5e-3 score -- on the photo, on noise and on shifted copies."""
+@pytest.mark.parametrize("hw,nb", [((448, 448), 5), ((448, 448), 2), ((288, 416), 3), ((896, 1280), 2), ((896, 1280), 8)])
+def test_tile_chains_equal_round1_kernels(hw, nb, golden_image):
+    """The latency plan of a one-context handle (448^2: SSH + predictor + NMS chains, at batch 2 the merge + aggr chains too;
+    288x416: partial tiles; 1280x896: SSH chains without the predictors, streamed weights at batch 8) against one round-1
+    kernel per layer (RF_FLAG_LEGACY_TC): every tensor both plans materialise within 2e-2 of its max, head blobs within
+    1e-2, and the SAME faces (anchor indices) within 0.25 px / 5e-3 score -- on the photo, on noise and on shifted copies."""
     from retinaface_b200 import RF_PREC_FP16
     from retinaface_b200.capi import RF_FLAG_LEGACY_TC, RfError
     h, w = hw
     inp = letterbox_bgr_u8(golden_image, h, w)
     batch = np.stack([inp, s_noise_batch(1, h, w, seed=1)[0]] + [np.roll(inp, 24 * k, axis=1) for k in range(1, nb - 1)])
-    monkeypatch.setenv("RF_TILE_MASK", str(mask))
-    new = _engine("mnet25", h, w, RF_PREC_FP16, max_batch=nb)
-    old = _engine("mnet25", h, w, RF_PREC_FP16, max_batch=nb, flags=RF_FLAG_LEGACY_TC)
+    new = _engine("mnet25", h, w, RF_PREC_FP16, max_batch=nb, streams=1)
+    old = _engine("mnet25", h, w, RF_PREC_FP16, max_batch=nb, streams=1, flags=RF_FLAG_LEGACY_TC)
     try:
         new.debug_keep_all()
         old.debug_keep_all()
@@ -120,20 +117,20 @@ def test_profile_layers_between_detections(golden_image):
         eng.close()
 
 
-@pytest.mark.parametrize("mask", [511, 482])
+@pytest.mark.parametrize("max_batch", [8, 2])
 @pytest.mark.parametrize("model", ["mnet25", "mnet-deconv-0517"])
-def test_tile_plans_against_golden_fp32(mask, model, golden_image, monkeypatch):
-    """The tile-chain plans held to the same bars as the round-1 FP16 engine (tests/test_gpu_parity.py::test_fp16_forward_and_detect):
+def test_tile_plans_against_golden_fp32(max_batch, model, golden_image):
+    """The latency plans of a one-context handle (SSH + predictor + NMS chains; at batch 2 the merge + aggr chains too) held
+    to the same bars as the round-1 FP16 engine (tests/test_gpu_parity.py::test_fp16_forward_and_detect):
     head blobs vs the golden FP32 heads (cls_prob 5e-3, deltas 2e-2 over ALL anchors), detections on the golden photo vs the
     golden FP32 detections (scores 1e-3, coordinates 0.1 px: north_star's FP16 tolerance), and -- decode + NMS running inside
     the SSH chain -- its own heads through the oracle post-process == its own detections, selection bit-exact."""
     from oracle.postproc import PostprocOracle
     from retinaface_b200 import RF_PREC_FP16
-    monkeypatch.setenv("RF_TILE_MASK", str(mask))
-    eng = _engine(model, 448, 448, RF_PREC_FP16, max_batch=8)
+    eng = _engine(model, 448, 448, RF_PREC_FP16, max_batch=max_batch, streams=1)
     try:
         inp = letterbox_bgr_u8(golden_image, 448, 448)
-        batch = s_real_batch(inp, 8)
+        batch = s_real_batch(inp, max_batch)
         heads = eng.forward_heads(batch)
         gold = np.load(os.path.join(GOLDEN, f"heads_{model}_448.npz"))
         for k, name in enumerate(topology.OUTPUT_BLOBS):
@@ -145,7 +142,7 @@ def test_tile_plans_against_golden_fp32(mask, model, golden_image, monkeypatch):
         assert np.abs(faces[0][:, 0] - dets[:, 0]).max() < 1e-3
         assert np.abs(faces[0][:, 1:] - dets[:, 1:]).max() < 0.1
         post = PostprocOracle()
-        for i in range(8):
+        for i in range(max_batch):
             ref = post.postprocess([x[i] for x in heads], 448, 448, 0.9, 0.4)
             assert idx[i].tolist() == ref["idx"].tolist(), i
             assert np.array_equal(faces[i][:, 0], ref["faces"][:, 0]) and np.array_equal(faces[i][:, 5:], ref["faces"][:, 5:]), i

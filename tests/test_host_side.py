@@ -172,34 +172,28 @@ def test_capacity_guard_for_32bit_activation_offsets(built_lib):
     assert e.value.status == -6
 
 
-def test_tile_plan_of_the_headline_config(built_lib, monkeypatch):
-    """rf_plan_describe (host-only): the FP16 plans of BASELINE configs[1].  Every chain enabled (RF_TILE_MASK=511): at most 15
-    kernel launches per forward, each chain within the 227 KB shared-memory budget of a CTA.  Defaults:
-    one execution context (latency mode) -> the convolution chains (FPN merge + aggr, SSH + predictors + decode + NMS) and
-    chain B; several contexts (throughput mode) -> the round-1 kernels with decode + NMS fused into one launch.  Chains
-    fall back to the round-1 kernels layer by layer where they cannot fit (wide maps); RF_FLAG_LEGACY_TC = one kernel per layer."""
+def test_tile_plan_of_the_headline_config(built_lib):
+    """rf_plan_describe (host-only): the FP16 plans of BASELINE configs[1].  One execution context (latency mode) -> the SSH +
+    predictor + NMS chains, and at batch <= 2 the FPN merge + aggr chains too, each within the 227 KB shared-memory budget
+    of a CTA; several contexts (throughput mode) -> the per-layer kernels with decode + NMS fused into one launch.  Wide
+    maps and other sizes stay within their launch counts; RF_FLAG_LEGACY_TC = one kernel per layer."""
     from retinaface_b200.capi import RF_FLAG_LEGACY_TC, plan_describe
-    monkeypatch.setenv("RF_TILE_MASK", "511")
-    text = plan_describe(caffemodel("mnet25"), 448, 448, max_batch=8)
-    assert int(text.split()[0]) <= 15, text
-    chains = [ln for ln in text.splitlines() if ln.startswith("tile_")]
-    assert len(chains) >= 8
-    assert any("heads+decode" in ln for ln in chains) and any("merge+aggr" in ln for ln in chains)
-    for ln in chains:
-        smem = int(re.search(r"smem (\d+) B", ln).group(1))
-        assert smem <= 227 * 1024, ln
     big = plan_describe(caffemodel("mnet25"), 896, 1280, max_batch=8)
     assert int(big.split()[0]) <= 30 and "tc2d_dw3" in big          # the 640-wide level does not fit a chain
     for hw in ((288, 416), (320, 320), (96, 160)):
         assert int(plan_describe(caffemodel("mnet-deconv-0517"), hw[0], hw[1], max_batch=3).split()[0]) <= 30
-    monkeypatch.delenv("RF_TILE_MASK")
     # latency mode (one execution context): SSH + predictor + NMS chains; at batch <= 2 the merge+aggr chains too
     lat = plan_describe(caffemodel("mnet25"), 448, 448, max_batch=8, streams=1)
     assert "tile_ssh_c1+heads+decode" in lat and "tile_c1_merge+aggr" not in lat and int(lat.split()[0]) == 22
     lat1 = plan_describe(caffemodel("mnet25"), 448, 448, max_batch=1, streams=1)
     assert "tile_ssh_c1+heads+decode" in lat1 and "tile_c1_merge+aggr" in lat1 and int(lat1.split()[0]) <= 21
+    chains = [ln for text in (lat, lat1) for ln in text.splitlines() if ln.startswith("tile_")]
+    assert len(chains) == 3 + 5
+    for ln in chains:
+        smem = int(re.search(r"smem (\d+) B", ln).group(1))
+        assert smem <= 227 * 1024, ln
     thr = plan_describe(caffemodel("mnet25"), 448, 448, max_batch=8)
-    assert int(thr.split()[0]) == 29 and "heads_1x1+softmax+decode+nms_all_levels" in thr and "sort+nms" not in thr
+    assert int(thr.split()[0]) == 29 and "heads_1x1+softmax+decode+nms_all_levels" in thr and "tile_" not in thr
     legacy = plan_describe(caffemodel("mnet25"), 448, 448, max_batch=8, flags=RF_FLAG_LEGACY_TC)
     assert int(legacy.split()[0]) == 29 and "tile_" not in legacy
 

@@ -1,5 +1,5 @@
 """Host-only guards of the NMS load sweep (tests/test_gpu_nms_load.py): its candidate-count targets straddle every branch
-boundary of nms_image as compiled, its plans still hold each of the three NMS instantiations (rf_plan_describe), and the threshold
+boundary of nms_image as compiled, its plans still hold each NMS instantiation they are there for (rf_plan_describe), and the threshold
 picker lands on exact counts through ties."""
 import os
 
@@ -28,55 +28,46 @@ def test_targets_straddle_every_branch_boundary():
         assert regime(p.anchors) == "bitonic-global", name
 
 
-def _describe(plan, max_faces, monkeypatch):
+def _describe(plan, max_faces):
     from retinaface_b200 import RF_PREC_FP16, RF_PREC_FP32, RF_PREC_INT8
     from retinaface_b200.capi import plan_describe
     prec = {"fp32": RF_PREC_FP32, "fp16": RF_PREC_FP16, "int8": RF_PREC_INT8}[plan.prec]
-    if plan.tile_mask:
-        monkeypatch.setenv("RF_TILE_MASK", plan.tile_mask)
-    else:
-        monkeypatch.delenv("RF_TILE_MASK", raising=False)
-    try:
-        return plan_describe(caffemodel(plan.model), plan.hw[0], plan.hw[1], precision=prec, max_batch=plan.max_batch,
-                             int8_table=TABLE if plan.prec == "int8" else None, streams=plan.streams, max_faces=max_faces)
-    finally:
-        monkeypatch.delenv("RF_TILE_MASK", raising=False)
+    return plan_describe(caffemodel(plan.model), plan.hw[0], plan.hw[1], precision=prec, max_batch=plan.max_batch,
+                         int8_table=TABLE if plan.prec == "int8" else None, streams=plan.streams, max_faces=max_faces)
 
 
 @pytest.mark.parametrize("name", list(PLANS))
-def test_sweep_plans_hold_their_nms_instantiation(name, monkeypatch):
+def test_sweep_plans_hold_their_nms_instantiation(name):
     """Each plan of the sweep holds the NMS instantiation it is there for, at the default max_faces and the small one.  The sweep
     also runs max_faces 8192: there a latency plan's SSH chains may no longer have room for the last-block NMS's kept list; the
     GPU test asserts whatever this reports."""
     plan = PLANS[name]
-    text = _describe(plan, 256, monkeypatch)
+    text = _describe(plan, 256)
     assert nms_variant(text) == plan.nms, (name, text)
     steps = [ln.split(": ", 1)[1] for ln in text.splitlines() if ln.startswith("step lane")]
     if plan.nms == "fused":
         tail = steps[-1]
         assert tail == ("i8_" if plan.prec == "int8" else "") + "heads_1x1+softmax+decode+nms_all_levels", steps
-    if plan.nms == "kernel":
-        assert any(s.startswith("tile_ssh_") for s in steps) and "sort+nms" in steps, steps
-    assert nms_variant(_describe(plan, 4, monkeypatch)) == plan.nms, name
-    print(f"{name}: max_faces 8192 -> {nms_variant(_describe(plan, 8192, monkeypatch))}")
+    assert nms_variant(_describe(plan, 4)) == plan.nms, name
+    print(f"{name}: max_faces 8192 -> {nms_variant(_describe(plan, 8192))}")
 
 
 def test_sweep_covers_the_three_instantiations():
-    """k_nms (rf_postprocess, the merges and the mask-255 plan), the last block of k_head_decode for float, half and int8 features,
-    and the last CTA of the SSH tile chains, at 448^2 and at a size with partial chain tiles and the global scratch."""
+    """k_nms (rf_postprocess, which every plan of the sweep runs), the last block of k_head_decode for float, half and int8
+    features, and the last CTA of the SSH tile chains, at 448^2 and at a size with partial chain tiles and the global scratch."""
     kinds = {(p.nms, p.prec) for p in PLANS.values()}
-    assert {("fused", "fp32"), ("fused", "fp16"), ("fused", "int8"), ("chain", "fp16"), ("kernel", "fp16")} <= kinds
+    assert {("fused", "fp32"), ("fused", "fp16"), ("fused", "int8"), ("chain", "fp16")} <= kinds
     assert {p.hw for p in PLANS.values() if p.nms == "chain"} >= {(448, 448), (416, 288)}
     assert {p.hw for p in PLANS.values() if p.nms == "fused" and p.prec == "fp16"} >= {(448, 448), (896, 1280)}
     assert {p.max_batch for p in PLANS.values() if p.nms == "chain" and p.hw == (448, 448)} == {2, 8}
 
 
-def test_latency_plan_keeps_its_fused_nms_up_to(monkeypatch):
+def test_latency_plan_keeps_its_fused_nms_up_to():
     """The largest max_faces (powers of two up to 8192) at which the 448^2 latency plan still runs its NMS in the SSH chains:
     the chains reserve sizeof(NmsSmem) + 4 max_faces bytes of shared memory for it.  Recorded here so that a change to the
     chains' shared-memory layout that moves it shows up."""
     plan = PLANS["fp16_448_latency_b8"]
-    fused = [mf for mf in (256, 512, 1024, 2048, 4096, 8192) if nms_variant(_describe(plan, mf, monkeypatch)) == "chain"]
+    fused = [mf for mf in (256, 512, 1024, 2048, 4096, 8192) if nms_variant(_describe(plan, mf)) == "chain"]
     print(f"448^2 latency plan: NMS in the SSH chains up to max_faces {max(fused)}")
     assert fused and fused == [256, 512, 1024, 2048, 4096, 8192][:len(fused)]
     assert max(fused) >= 256

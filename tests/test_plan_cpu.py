@@ -5,10 +5,12 @@ activation-arena size and tile-chain line must stay as it was, except for the ch
 - the per-layer fallback of the FP16 tile-chain plan names its lateral convolutions as the other per-layer plans do;
 - the SIMT plans (FP32, FP16 with RF_FLAG_NO_TENSORCORE) run rf_c1_red_conv and rf_c2_lateral right after the pointwise layer
   that produces their input (pw10, pw22) instead of after the backbone;
-- RF_FLAG_LEGACY_TC builds the FP16 plan with no tile chains: the RF_TILE_MASK=0 plan, whatever RF_TILE_MASK says.
+- RF_FLAG_LEGACY_TC builds the FP16 plan with no tile chains.
 
 The fixture was written by running this module as a script against a library built from commit 23f7863, the last one with
-a builder per precision: RF_B200_LIB=<that library> python tests/test_plan_cpu.py --write."""
+a builder per precision: RF_B200_LIB=<that library> python tests/test_plan_cpu.py --write.  Its grid then also held the
+plans selected by the RF_TILE_* environment variables, which no longer exist; a one-off filter has since dropped those
+configurations (and the texts only they referenced) and the key suffix that named the variables' values."""
 import gzip
 import json
 import os
@@ -27,41 +29,29 @@ NO_TC, SIMT_STEM, DW_1D, LEGACY_TC = 0x2, 0x4, 0x8, 0x10
 MODELS = ("mnet25", "mnet-deconv-0517")
 SIZES = ((448, 448), (896, 1280), (288, 416), (320, 320), (96, 160))      # (net_h, net_w)
 BATCHES = (1, 3, 8, 32)
-TILE_ENVS = ("", "511", "255", "127", "63", "0", "511+single")      # RF_TILE_MASK ("" unset); +single: RF_TILE_SINGLE=1
 
 
 def grid():
-    """(key, model, precision, h, w, batch, flags, streams, tile env).  Streams and RF_TILE_* matter only to the FP16
-    tensor-core plan; the flags only where a plan reads them."""
+    """(key, model, precision, h, w, batch, flags, streams).  Streams matter only to the FP16 tensor-core plan; the flags
+    only where a plan reads them."""
     for model in MODELS:
         for h, w in SIZES:
             for b in BATCHES:
-                cases = [(FP32, 0, 0, "")]
-                cases += [(FP16, f, 0, "") for f in (NO_TC, SIMT_STEM, DW_1D)]
-                cases += [(FP16, 0, s, "") for s in (1, 0)]
-                cases += [(FP16, 0, 0, env) for env in TILE_ENVS[1:]]
-                cases += [(INT8, f, 0, "") for f in (0, SIMT_STEM, DW_1D)]
-                for prec, flags, streams, env in cases:
-                    key = f"{model} p{prec} {h}x{w} b{b} f{flags} s{streams} m{env or '-'}"
-                    yield key, model, prec, h, w, b, flags, streams, env
+                cases = [(FP32, 0, 0)]
+                cases += [(FP16, f, 0) for f in (NO_TC, SIMT_STEM, DW_1D)]
+                cases += [(FP16, 0, s) for s in (1, 0)]
+                cases += [(INT8, f, 0) for f in (0, SIMT_STEM, DW_1D)]
+                for prec, flags, streams in cases:
+                    yield f"{model} p{prec} {h}x{w} b{b} f{flags} s{streams}", model, prec, h, w, b, flags, streams
 
 
-def describe(model, prec, h, w, b, flags, streams, env):
+def describe(model, prec, h, w, b, flags, streams):
     from retinaface_b200.capi import RfError, plan_describe
-    mask, single = (env.split("+") + [""])[:2] if env else ("", "")
-    for var, val in (("RF_TILE_MASK", mask), ("RF_TILE_SINGLE", "1" if single else "")):
-        if val:
-            os.environ[var] = val
-        else:
-            os.environ.pop(var, None)
     try:
         return plan_describe(os.path.join(WEIGHTS, model + ".caffemodel"), h, w, precision=prec, max_batch=b, flags=flags,
                              int8_table=TABLE if prec == INT8 else None, streams=streams)
     except RfError as e:
         return f"error {e.status}"
-    finally:
-        os.environ.pop("RF_TILE_MASK", None)
-        os.environ.pop("RF_TILE_SINGLE", None)
 
 
 def move_after(lines, name, producer):
@@ -94,24 +84,23 @@ def fixture(built_lib):
 def test_plans_equal_the_parent_builders_but_for_the_intended_changes(fixture):
     texts, plans = fixture["texts"], fixture["plans"]
     assert len(plans) == sum(1 for _ in grid())
-    for key, model, prec, h, w, b, flags, streams, env in grid():
-        got = describe(model, prec, h, w, b, flags, streams, env)
+    for key, model, prec, h, w, b, flags, streams in grid():
+        got = describe(model, prec, h, w, b, flags, streams)
         assert got == expected(texts[plans[key]], prec, flags), key
     # the grid reaches every builder and every merge rule
-    joined = "\n".join(texts)
+    joined = "\n".join(texts[plans[key]] for key, *_ in grid())
     for step in ("upsample_add_plus1", "tc_c1_upsample+add+aggr", "fpn_merge_plus1_upsample+add_h2", "fpn_merge_plus0_upsample+add_h2",
-                 "i8_c1_upsample+add+aggr", "i8_fpn_merge_c1_upsample+add", "tile_c1_merge+aggr", "tile_ssh_c1+heads+decode", "tile_B9",
+                 "i8_c1_upsample+add+aggr", "i8_fpn_merge_c1_upsample+add", "tile_c1_merge+aggr", "tile_ssh_c1+heads+decode",
                  "i8_2d_dw3", "tc2d_dw3", "stem_conv0+dw1+pw2_u8_to_16ch_i8", "tc_rf_c1_red_conv_1x1"):
         assert step in joined, step
 
 
 def test_legacy_tc_is_the_fp16_plan_without_tile_chains(built_lib):
+    """RF_FLAG_LEGACY_TC on a one-context handle (where the chains would run) builds the several-context plan."""
     for model in MODELS:
         for h, w in SIZES:
             for b in BATCHES:
-                plain = describe(model, FP16, h, w, b, 0, 0, "0")
-                for env in ("", "511"):
-                    assert describe(model, FP16, h, w, b, LEGACY_TC, 1, env) == plain, (model, h, w, b, env)
+                assert describe(model, FP16, h, w, b, LEGACY_TC, 1) == describe(model, FP16, h, w, b, 0, 0), (model, h, w, b)
 
 
 if __name__ == "__main__" and "--write" in sys.argv:

@@ -450,6 +450,44 @@ int rf_detect_views_oriented(rf_handle h, const uint8_t *bgr, int width, int hei
  * rf_decode_jpeg or their own decoder. */
 int rf_jpeg_exif_orientation(const uint8_t *jpeg, size_t bytes);
 
+/* f23 faces at any in-plane angle: rotated views.  View v shows the image (W x H, as stored) rotated counter-clockwise by
+ * views[v].angle degrees -- the sign convention of cv2.getRotationMatrix2D -- fitted into the shrink box bw x bh of rf_detect_views
+ * (bw = max(1, (int)(net_w * shrink)), likewise bh; shrink in (0, 1]).  In FP64, every operation rounded once (no FMA contraction):
+ *   a = fmod(angle, 360), plus 360 when negative; a = 360 (a tiny negative angle) is 0.  A non-finite angle is RF_ERR_INVALID_ARG.
+ *   a in {0, 90, 180, 270}: rf_detect_views_oriented's view (shrink, o) with o = 1, 8, 3, 6, bit for bit (letter-box, records and
+ *   map-back).  Any other a is a WARP view:
+ *     r = a * (M_PI / 180), c = cos(r), s = sin(r) (the C library's);  Wr = |c| * W + |s| * H,  Hr = |s| * W + |c| * H;
+ *     f = min(1, bw / Wr, bh / Hr) (never up-scaled, like the letter-box);
+ *     M = [[f * c, f * s, tx], [-(f * s), f * c, ty]] with
+ *       tx = (f * Wr - 1) / 2 - (M00 * ((W - 1) / 2) + M01 * ((H - 1) / 2)),  ty = (f * Hr - 1) / 2 - (M10 * ((W - 1) / 2) + M11 * ((H - 1) / 2)),
+ *     so the image centre lands on the centre of the rotated image's f Wr x f Hr bounding box, which sits at the input's top-left.
+ *     The network input is cv2.warpAffine(img, M, (net_w, net_h), INTER_LINEAR, BORDER_CONSTANT, 0) byte for byte: zero outside the
+ *     rotated image, like the letter-box padding.
+ *     A kept face of a warp view maps back through iM = cv::invertAffineTransform(M): its box centre ((x1 + x2) / 2, (y1 + y2) / 2)
+ *     goes through iM, the half sizes are (x2 - x1) * (1 / (2 f)) and (y2 - y1) * (1 / (2 f)), and the box is centre -/+ half size,
+ *     each rounded to float once -- axis-aligned in image pixels, with the face's own size; the face's roll is the view's angle
+ *     (out_view_of).  Each landmark is iM (lx, ly), rounded to float; a rotation does not mirror, so landmark sides are kept.
+ * The faces of all views are merged by rf_detect_views' NMS, candidate id v * max_faces + rank.  Landmarks in image pixels carry the
+ * face's roll, so f5 crops fitted on them come out upright. */
+typedef struct rf_rotated_view {
+    float angle;     /* degrees, counter-clockwise */
+    float shrink;    /* (0, 1] */
+} rf_rotated_view;
+/* One host image (pinned or pageable, row_stride 0: packed), 1..RF_MAX_VIEWS views (else RF_ERR_CAPACITY); views beyond max_batch run
+ * in consecutive batches on context 0.  Blocking.  out_faces [max_faces] in image pixels, *out_count; out_view_of (optional,
+ * [max_faces]) the view of each face; out_view_scales (optional, [nviews]) the oriented views' map-back factor and (float)(1 / f) for
+ * warp views; out_view_mats (optional, [nviews][6]) M of each warp view, all zero for the views that take the oriented path.
+ * align != NULL: the crops of the merged faces, cut from the original image, in rf_detect_align_batch's layout for one image
+ * (out_crops [A][crop bytes] required, out_mats [A][6] optional).  A non-finite angle, a shrink outside (0, 1], NULL views or bad align
+ * params: RF_ERR_INVALID_ARG; the image is checked as by rf_detect_views; all before anything is launched or written. */
+int rf_detect_views_rotated(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, const rf_rotated_view *views, int nviews,
+                            float score_threshold, float nms_threshold, const rf_align_params *align, rf_face *out_faces, int *out_count,
+                            int32_t *out_view_of, float *out_view_scales, double *out_view_mats, void *out_crops, double *out_mats);
+/* Preprocess parity of f23 (as rf_preprocess): the network input of the view (angle, shrink) of one host image, either kind, into a
+ * host net_h*net_w*3 u8 BGR buffer, and (out_mat optional, [6]) its M, all zero for a quarter turn. */
+int rf_preprocess_rotated(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, float angle, float shrink,
+                          uint8_t *out_net_sized, double *out_mat);
+
 /* f10 face tracking across video frames, on the GPU: per-video tracks with stable ids, so that a recogniser runs once per new
  * identity instead of once per face per frame, and counting / dwell time / "who entered" need no host round trip.  One tracker holds
  * max_videos independent sequences (cameras, files), each with up to max_tracks live tracks (tentative, confirmed and lost).

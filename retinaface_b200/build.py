@@ -25,7 +25,7 @@ SOURCES = [
     ("comm.cu", []),
     ("jpeg.cu", []),
     ("postproc.cu", ["-fmad=false"]),
-    ("preprocess.cu", ["-fmad=false"]),
+    ("preprocess.cu", ["-fmad=false", "-Xcompiler", "-ffp-contract=off"]),   # and f23's host-side M, one rounding per operation
     ("align.cu", ["-fmad=false"]),      # cv::warpAffine's coordinates and the similarity fit: multiply and add, never fused
     ("track.cu", ["-fmad=false"]),      # the tracker's FP64 Kalman filter and IoU: every step one rounding, as oracle/track.py states it
     ("best.cu", ["-fmad=false"]),       # the crop warp of align.cu and the FP64 face quality, as oracle/bestshot.py states it

@@ -26,6 +26,10 @@ class _OrientedView(C.Structure):    # rf_oriented_view
     _fields_ = [("shrink", C.c_float), ("orientation", C.c_int32)]
 
 
+class _RotatedView(C.Structure):     # rf_rotated_view
+    _fields_ = [("angle", C.c_float), ("shrink", C.c_float)]
+
+
 # EXIF orientations (rf_b200.h f9): 1 upright, 2 mirrored, 3 rotated 180, 4 upside-down mirror, 5 transposed, 6 rotated 90 clockwise,
 # 7 transverse, 8 rotated 90 counter-clockwise; ANY_ORIENTATION are the four rotations rf_detect_views_oriented sweeps
 ORIENTATIONS = tuple(range(1, 9))
@@ -356,6 +360,8 @@ _SIGNATURES = {
     "rf_preprocess_yuv_oriented": (_I, [_P, _FRAMES, _I, _I, _P]),
     "rf_detect_views_oriented": (_I, [_P, _P, _I, _I, _I, C.POINTER(_OrientedView), _I, _F, _F, _P, _PI, _P, _P]),
     "rf_jpeg_exif_orientation": (_I, [_P, C.c_size_t]),
+    "rf_detect_views_rotated": (_I, [_P, _P, _I, _I, _I, C.POINTER(_RotatedView), _I, _F, _F, _ALIGN, _P, _PI, _P, _P, _P, _P, _P]),
+    "rf_preprocess_rotated": (_I, [_P, _P, _I, _I, _I, _F, _F, _P, _P]),
     "rf_tracker_create": (_I, [_P, C.POINTER(TrackConfig), _PP]), "rf_tracker_destroy": (None, [_P]),
     "rf_tracker_reset": (_I, [_P, _I]),
     "rf_track_update": (_I, [_P, _P, _I, _P, _P, _P, _PP, _PP]),
@@ -1047,6 +1053,40 @@ class Engine:
                                                       C.c_float(thr), C.c_float(nms), C.c_void_p(faces.ctypes.data), C.byref(count),
                                                       C.c_void_p(view_of.ctypes.data), C.c_void_p(scales.ctypes.data)))
         return faces[:count.value].copy(), view_of[:count.value].copy(), scales[:nv].copy()
+
+    # -- f23 faces at any in-plane angle ---------------------------------------------------------------------------------------
+    def detect_views_rotated(self, img: np.ndarray, views, thr: float, nms: float, align: Optional[dict] = None):
+        """rf_detect_views_rotated: one image, views = [(angle, shrink), ...] (degrees counter-clockwise), run in batches of up to
+        max_batch and merged on the GPU.  Returns (faces [k, 15] in image pixels, view index of each face [k], map-back scale of each
+        view, M of each view [nviews, 2, 3], zeros for quarter turns); align: detect_align's keywords -> crops [min(k, A), ...]
+        [and mats [min(k, A), 2, 3]] appended, cut from the image."""
+        img = self._bgr_strided(img)
+        nv = len(views)
+        varr = (_RotatedView * max(nv, 1))(*[_RotatedView(float(a), float(s)) for a, s in views])
+        faces = np.empty((self.max_faces, 15), dtype=np.float32)
+        view_of = np.empty(self.max_faces, dtype=np.int32)
+        scales = np.empty(max(nv, 1), dtype=np.float32)
+        mats = np.empty((max(nv, 1), 2, 3), dtype=np.float64)
+        p, A, crops, cmats = self._host_align(1, align) if align is not None else (None, 0, None, None)
+        count = C.c_int(0)
+        self._check(self.lib.rf_detect_views_rotated(self.h, img.ctypes.data, img.shape[1], img.shape[0], img.strides[0], varr, nv, C.c_float(thr),
+                                                     C.c_float(nms), _ref(p), faces.ctypes.data, C.byref(count), view_of.ctypes.data,
+                                                     scales.ctypes.data, mats.ctypes.data, _addr(crops), _addr(cmats)))
+        k = count.value
+        out = (faces[:k].copy(), view_of[:k].copy(), scales[:nv].copy(), mats[:nv].copy())
+        if align is None:
+            return out
+        out += (crops[0, :min(k, A)].copy(),)
+        return out + (cmats[0, :min(k, A)].copy(),) if cmats is not None else out
+
+    def preprocess_rotated(self, img: np.ndarray, angle: float, shrink: float = 1.0):
+        """rf_preprocess_rotated: (the (H, W, 3) u8 BGR network input of the view (angle, shrink), its M [2, 3], zeros for a quarter turn)."""
+        img = self._bgr_strided(img)
+        out = np.empty((self.net_h, self.net_w, 3), dtype=np.uint8)
+        mat = np.empty((2, 3), dtype=np.float64)
+        self._check(self.lib.rf_preprocess_rotated(self.h, img.ctypes.data, img.shape[1], img.shape[0], img.strides[0], C.c_float(angle),
+                                                   C.c_float(shrink), out.ctypes.data, mat.ctypes.data))
+        return out, mat
 
     # -- f21 tiled detection of rotated and mirrored images ---------------------------------------------------------------------
     def detect_tiled_oriented(self, images: Sequence[np.ndarray], orientations: Sequence[int], thr: float, nms_thr: float, levels=None,

@@ -1524,6 +1524,159 @@ int rf_detect_views_oriented(rf_handle h, const uint8_t *bgr, int width, int hei
                       out_view_scales);
 }
 
+// ---- f23 rotated views (rf_b200.h rf_rotated_view) -------------------------------------------------------------------------------
+static int check_rotated(rf_handle h, const char *who, float angle, float shrink, int v) {
+    if (!std::isfinite(angle)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: view %d: the angle must be finite", who, v));
+    if (!(shrink > 0.f && shrink <= 1.f)) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: view %d: shrink must be in (0, 1]", who, v));
+    return RF_OK;
+}
+
+// The shrink box of a view, as views_impl computes it
+static void shrink_box(rf_handle h, float shrink, int &bw, int &bh) {
+    bw = std::max(1, (int)(h->cfg.net_w * shrink));
+    bh = std::max(1, (int)(h->cfg.net_h * shrink));
+}
+
+int rf_detect_views_rotated(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, const rf_rotated_view *views, int nviews,
+                            float thr, float nms, const rf_align_params *align, rf_face *out_faces, int *out_count, int32_t *out_view_of,
+                            float *out_view_scales, double *out_view_mats, void *out_crops, double *out_mats) {
+    const char *who = "rf_detect_views_rotated";
+    if (!h || !bgr || !views || !out_count || width <= 0 || height <= 0) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: bad arguments", who));
+    if (nviews < 1 || nviews > RF_MAX_VIEWS)
+        return fail(h, RF_ERR_CAPACITY, fmt("%s: %d views, limit RF_MAX_VIEWS = %d", who, nviews, RF_MAX_VIEWS));
+    const BgrImages src{&bgr, &width, &height, &row_stride, nullptr, false};
+    int rc = src.check(h, who, 1);
+    if (rc) return rc;
+    for (int v = 0; v < nviews; v++)
+        if ((rc = check_rotated(h, who, views[v].angle, views[v].shrink, v))) return rc;
+    AlignArgs a;
+    if (align && (rc = check_align(h, who, align, 1, out_crops, 1, a))) return rc;
+    static_assert(RF_MAX_VIEWS == RF_MAX_VIEWS_DEV && RF_MAX_VIEWS == WARP_MAX_VIEWS, "view capacity of the warp and merge kernels");
+    const int Hn = h->cfg.net_h, Wn = h->cfg.net_w, mf = h->cfg.max_faces, B = h->cfg.max_batch;
+    const size_t img_bytes = (size_t)Hn * Wn * 3;
+    const int area = (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0;
+    // the quarter turns first: within a batch they take slots 0 .. k-1, as launch_merge reads them; ids keep the caller's order
+    std::vector<RotatedGeometry> geo(nviews);
+    std::vector<int> order;
+    for (int v = 0; v < nviews; v++) {
+        int bw, bh;
+        shrink_box(h, views[v].shrink, bw, bh);
+        geo[v] = rotated_geometry(views[v].angle, width, height, bw, bh);
+        if (geo[v].orientation) order.push_back(v);
+    }
+    for (int v = 0; v < nviews; v++)
+        if (!geo[v].orientation) order.push_back(v);
+    try {
+        CK(cudaSetDevice(h->device));
+        Ctx &c = h->ctx[0];
+        // every view may contribute max_faces candidates to the merged list of the one image
+        if (h->pb_merge.anchors_per_image < RF_MAX_VIEWS * mf) {
+            free_post_buffers(h->pb_merge);
+            alloc_post_buffers(h->pb_merge, RF_MAX_VIEWS * mf, 1, mf);
+        }
+        const BgrRows d_src = src.upload(h, c.stream, 0, 0);
+        set_params(h, c, thr, nms);
+        for (int v0 = 0; v0 < nviews; v0 += B) {
+            const int m = std::min(B, nviews - v0);
+            std::vector<LbItem> lb;
+            std::vector<MergeSource> ms;
+            std::vector<WarpItem> wp;
+            std::vector<RotatedSource> rs;
+            for (int b = 0; b < m; b++) {
+                const int v = order[v0 + b];
+                const RotatedGeometry &g = geo[v];
+                uint8_t *dst = h->d_input + (size_t)b * img_bytes;
+                float scale;
+                if (g.orientation) {      // rf_detect_views_oriented's view, slot b < k
+                    int bw, bh;
+                    shrink_box(h, views[v].shrink, bw, bh);
+                    const int bits = lb_orientation_bits(g.orientation);
+                    const int dw = (bits & LB_TRANSPOSE) ? height : width, dh = (bits & LB_TRANSPOSE) ? width : height;
+                    lb.emplace_back();
+                    scale = letterbox_fill(lb.back(), d_src, dw, dh, dst, bw, bh, bits, area);
+                    ms.push_back((bits & ~LB_FLIP_X) ? oriented_view_source(v, mf, scale, bits, dw, dh) : view_source(v, mf, scale, bits, width));
+                } else {
+                    WarpItem w{d_src, width, height, dst, {}};
+                    std::copy(g.iM, g.iM + 6, w.im);
+                    wp.push_back(w);
+                    RotatedSource r{b, v * mf, {}, 1.0 / (2.0 * g.f)};
+                    std::copy(g.iM, g.iM + 6, r.im);
+                    rs.push_back(r);
+                    scale = (float)(1.0 / g.f);
+                }
+                if (out_view_scales) out_view_scales[v] = scale;
+                if (out_view_mats)
+                    for (int k = 0; k < 6; k++) out_view_mats[(size_t)v * 6 + k] = g.orientation ? 0.0 : g.M[k];
+            }
+            CK(launch_letterbox_batch(lb.data(), (int)lb.size(), Wn, Hn, c.stream));
+            CK(launch_letterbox_warp(wp.data(), (int)wp.size(), Wn, Hn, c.stream));
+            forward_graph(h, c, m);
+            CK(launch_merge(c.pb, ms.data(), (int)ms.size(), Wn, Hn, h->pb_merge, c.stream));
+            CK(launch_merge_rotated(c.pb, rs.data(), (int)rs.size(), h->pb_merge, c.stream));
+        }
+        CK(launch_nms(1, c.d_params, h->pb_merge, c.stream));
+        if (align) {
+            ensure_align_buffers(h, 1, a);
+            a.n = 1;
+            a.crops = h->d_align_crops;
+            a.mats = out_mats ? h->d_align_mats : nullptr;
+            const AlignImageT<BgrRows> orig{d_src, width, height, 1.f, 0};     // the merged records are in image pixels
+            CK(launch_align_faces(a, &orig, h->pb_merge, h->num_sms, c.stream));
+        }
+        CK(cudaMemcpyAsync(h->h_counts, h->pb_merge.out_counts, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
+        CK(cudaMemcpyAsync(h->h_dets, h->pb_merge.out_dets, sizeof(rf_det) * (size_t)mf, cudaMemcpyDeviceToHost, c.stream));
+        CK(cudaStreamSynchronize(c.stream));
+        const int k = h->h_counts[0];
+        *out_count = k;
+        for (int j = 0; j < k; j++) {
+            if (out_faces) out_faces[j] = h->h_dets[j].face;
+            if (out_view_of) out_view_of[j] = h->h_dets[j].anchor_index / mf;
+        }
+        const size_t nc = (size_t)std::min(k, align ? a.max_align : 0);
+        if (nc) {
+            CK(cudaMemcpy(out_crops, h->d_align_crops, nc * a.crop_bytes, cudaMemcpyDeviceToHost));
+            if (out_mats) CK(cudaMemcpy(out_mats, h->d_align_mats, nc * 6 * sizeof(double), cudaMemcpyDeviceToHost));
+        }
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
+}
+
+int rf_preprocess_rotated(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, float angle, float shrink, uint8_t *out,
+                          double *out_mat) {
+    const char *who = "rf_preprocess_rotated";
+    if (!h) return RF_ERR_INVALID_ARG;
+    if (!out) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: out is NULL", who));
+    const BgrImages src{&bgr, &width, &height, &row_stride, nullptr, false};
+    int rc = src.check(h, who, 1);
+    if (rc || (rc = check_rotated(h, who, angle, shrink, 0))) return rc;
+    const int Hn = h->cfg.net_h, Wn = h->cfg.net_w;
+    int bw, bh;
+    shrink_box(h, shrink, bw, bh);
+    const RotatedGeometry g = rotated_geometry(angle, width, height, bw, bh);
+    try {
+        CK(cudaSetDevice(h->device));
+        cudaStream_t s = h->ctx[0].stream;
+        const BgrRows p = src.upload(h, s, 0, 0);
+        if (g.orientation) {
+            const int bits = lb_orientation_bits(g.orientation);
+            const int dw = (bits & LB_TRANSPOSE) ? height : width, dh = (bits & LB_TRANSPOSE) ? width : height;
+            LbItem it;
+            letterbox_fill(it, p, dw, dh, h->d_input, bw, bh, bits, (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0);
+            CK(launch_letterbox_batch(&it, 1, Wn, Hn, s));
+        } else {
+            WarpItem w{p, width, height, h->d_input, {}};
+            std::copy(g.iM, g.iM + 6, w.im);
+            CK(launch_letterbox_warp(&w, 1, Wn, Hn, s));
+        }
+        CK(cudaMemcpyAsync(h->h_input, h->d_input, (size_t)Hn * Wn * 3, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        memcpy(out, h->h_input, (size_t)Hn * Wn * 3);
+        if (out_mat)
+            for (int k = 0; k < 6; k++) out_mat[k] = g.orientation ? 0.0 : g.M[k];
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
+}
+
 static void ensure_blobs(rf_handle h) {
     if (h->d_blobs[0]) return;
     for (int i = 0; i < 9; i++) CK(cudaMalloc(&h->d_blobs[i], sizeof(float) * h->blob_elems[i] * h->cfg.max_batch));

@@ -245,6 +245,40 @@ __global__ void __launch_bounds__(256) k_merge(PostBuffers src, const __grid_con
     }
 }
 
+// f23: one launch merges every warp view of a batch (postproc.cuh RotatedSource)
+struct RotatedSet {
+    RotatedSource src[RF_MAX_VIEWS_DEV];
+};
+static_assert(sizeof(RotatedSet) + 2 * sizeof(PostBuffers) <= 4096, "rotated merge launch exceeds the classic 4 KB kernel parameter space");
+
+__device__ __forceinline__ double affine_row(double a, double b, double c, double x, double y) {
+    return __dadd_rn(__dadd_rn(__dmul_rn(a, x), __dmul_rn(b, y)), c);
+}
+
+__global__ void __launch_bounds__(256) k_merge_rotated(PostBuffers src, const __grid_constant__ RotatedSet rs, PostBuffers dst) {
+    const RotatedSource &m = rs.src[blockIdx.x];
+    const int b = m.slot;
+    const int n = min(src.out_counts[b], src.max_faces);
+    const double *im = m.im;
+    for (int j = threadIdx.x; j < n; j += blockDim.x) {
+        const rf_face f = src.out_dets[(size_t)b * src.max_faces + j].face;
+        const double cx = __dmul_rn(__dadd_rn((double)f.x1, (double)f.x2), 0.5), cy = __dmul_rn(__dadd_rn((double)f.y1, (double)f.y2), 0.5);
+        const double X = affine_row(im[0], im[1], im[2], cx, cy), Y = affine_row(im[3], im[4], im[5], cx, cy);
+        const double hw = __dmul_rn(__dsub_rn((double)f.x2, (double)f.x1), m.half_inv), hh = __dmul_rn(__dsub_rn((double)f.y2, (double)f.y1), m.half_inv);
+        rf_det d;
+        d.face.score = f.score;
+        d.face.x1 = (float)__dsub_rn(X, hw); d.face.x2 = (float)__dadd_rn(X, hw);
+        d.face.y1 = (float)__dsub_rn(Y, hh); d.face.y2 = (float)__dadd_rn(Y, hh);
+#pragma unroll
+        for (int k = 0; k < 5; k++) {
+            d.face.lx[k] = (float)affine_row(im[0], im[1], im[2], (double)f.lx[k], (double)f.ly[k]);
+            d.face.ly[k] = (float)affine_row(im[3], im[4], im[5], (double)f.lx[k], (double)f.ly[k]);
+        }
+        d.anchor_index = m.id_base + j;
+        append_candidate(dst, 0, d);
+    }
+}
+
 size_t nms_smem_bytes(int max_faces) { return sizeof(int) * (size_t)max_faces; }
 
 }  // namespace
@@ -344,6 +378,15 @@ cudaError_t launch_merge(const PostBuffers &src, const MergeSource *src_desc, in
         if (e != cudaSuccess) return e;
     }
     return cudaSuccess;
+}
+
+cudaError_t launch_merge_rotated(const PostBuffers &src, const RotatedSource *src_desc, int n, const PostBuffers &dst, cudaStream_t s) {
+    if (n <= 0) return cudaSuccess;
+    if (n > RF_MAX_VIEWS_DEV) return cudaErrorInvalidValue;
+    RotatedSet rs{};
+    for (int i = 0; i < n; i++) rs.src[i] = src_desc[i];
+    k_merge_rotated<<<n, 256, 0, s>>>(src, rs, dst);
+    return cudaGetLastError();
 }
 
 cudaError_t postproc_init() {

@@ -85,6 +85,15 @@ MergeSource oriented_view_source(int view, int max_faces, float scale, int bits,
 MergeSource tile_source(int image, int tile, int max_faces, const rf_tile &t, int img_w);   // tile: its index in the image's layout
 cudaError_t launch_merge(const PostBuffers &src, const MergeSource *src_desc, int n, int net_w, int net_h, const PostBuffers &dst,
                          cudaStream_t s);
+// f23 warp views (rf_b200.h rf_rotated_view): batch slot `slot`'s kept faces mapped back through iM in FP64 -- the box centre through
+// iM, half sizes (x2 - x1) * half_inv and (y2 - y1) * half_inv (half_inv = 1 / (2 f)), each corner and landmark rounded to float once
+// -- and appended to image 0 of dst with candidate id id_base + rank.  A table of its own, so that MergeSource keeps its size.
+struct RotatedSource {
+    int slot, id_base;
+    double im[6];
+    double half_inv;
+};
+cudaError_t launch_merge_rotated(const PostBuffers &src, const RotatedSource *src_desc, int n, const PostBuffers &dst, cudaStream_t s);
 
 // dynamic shared memory the NMS kernel wants (set once at init)
 cudaError_t postproc_init();

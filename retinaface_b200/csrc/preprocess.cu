@@ -5,6 +5,7 @@
 #include <type_traits>
 
 #include "preprocess.cuh"
+#include "warp.cuh"
 
 namespace rf {
 
@@ -398,6 +399,119 @@ cudaError_t launch_letterbox_batch(const LbItemT<Src> *items, int n, int net_w, 
     }
     return cudaSuccess;
 }
+
+// ---- f23 rotated views ------------------------------------------------------------------------------------------------------------
+RotatedGeometry rotated_geometry(float angle, int w, int h, int box_w, int box_h) {
+    RotatedGeometry g{};
+    double a = std::fmod((double)angle, 360.0);
+    if (a < 0.0) a += 360.0;
+    if (a == 360.0) a = 0.0;      // a negative angle above -2^-45 rounds up to a whole turn
+    if (a == 0.0 || a == 90.0 || a == 180.0 || a == 270.0) {
+        g.orientation = a == 0.0 ? 1 : a == 90.0 ? 8 : a == 180.0 ? 3 : 6;
+        return g;
+    }
+    const double r = a * (M_PI / 180.0), c = std::cos(r), s = std::sin(r);
+    const double W = w, H = h;
+    const double wr = std::fabs(c) * W + std::fabs(s) * H, hr = std::fabs(s) * W + std::fabs(c) * H;
+    double f = 1.0;
+    f = std::min(f, box_w / wr);
+    f = std::min(f, box_h / hr);
+    g.f = f;
+    g.M[0] = f * c; g.M[1] = f * s; g.M[3] = -(f * s); g.M[4] = f * c;
+    const double cx = (W - 1.0) / 2.0, cy = (H - 1.0) / 2.0;
+    g.M[2] = (f * wr - 1.0) / 2.0 - (g.M[0] * cx + g.M[1] * cy);
+    g.M[5] = (f * hr - 1.0) / 2.0 - (g.M[3] * cx + g.M[4] * cy);
+    invert_affine(g.M, g.iM);
+    return g;
+}
+
+namespace {
+// A CTA computes WARP_BAND rows of WARP_SPAN columns of one view (short bands: many CTAs, so that the gathers' latency overlaps): it tabulates OpenCV's per-column (adelta, bdelta) and per-row
+// (X0, Y0) fixed-point terms in shared memory as k_align_faces does, so every pixel costs integer arithmetic only, and each thread
+// makes 4 consecutive pixels of a row, stored as three aligned 32-bit words (net_w is a multiple of 32).  Per row the CTA also bounds
+// the columns whose taps can reach the image; the quads outside that span are zero and gather nothing.
+constexpr int WARP_THREADS = 128, WARP_BAND = 2, WARP_SPAN = WARP_THREADS * 4;
+template <typename Src>
+struct WarpBatch { WarpItemT<Src> v[WARP_MAX_VIEWS]; };
+static_assert(sizeof(WarpBatch<BgrRows>) + 8 <= 4096, "warp launch exceeds the classic 4 KB kernel parameter space");
+
+// [lo, hi] of the x with a x + b in [-2, n + 1]: the fixed-point source coordinate is within 1/16 pixel of a x + b, and a pixel has a
+// tap in [0, n) only if that coordinate is in [-1, n), so the bound keeps a pixel of margin
+__device__ __forceinline__ void footprint(double a, double b, int n, double &lo, double &hi) {
+    if (fabs(a) < 1e-12) {
+        const bool in = b >= -2.0 && b <= n + 1.0;
+        lo = in ? -INFINITY : INFINITY;
+        hi = in ? INFINITY : -INFINITY;
+        return;
+    }
+    const double t0 = (-2.0 - b) / a, t1 = (n + 1.0 - b) / a;
+    lo = fmin(t0, t1);
+    hi = fmax(t0, t1);
+}
+
+template <typename Src>
+__global__ void __launch_bounds__(WARP_THREADS) k_letterbox_warp(const __grid_constant__ WarpBatch<Src> B, int net_w, int net_h) {
+    __shared__ int s_ax[WARP_SPAN], s_bx[WARP_SPAN], s_x0[WARP_BAND], s_y0[WARP_BAND], s_lo[WARP_BAND], s_hi[WARP_BAND];
+    const WarpItemT<Src> &it = B.v[blockIdx.z];
+    const int xb = blockIdx.x * WARP_SPAN, yb = blockIdx.y * WARP_BAND;
+    const double i0 = it.im[0], i1 = it.im[1], i2 = it.im[2], i3 = it.im[3], i4 = it.im[4], i5 = it.im[5];
+    for (int k = threadIdx.x; k < WARP_SPAN; k += WARP_THREADS) {
+        const int x = xb + k;
+        s_ax[k] = __double2int_rn(i0 * x * 1024.0);
+        s_bx[k] = __double2int_rn(i3 * x * 1024.0);
+    }
+    if (threadIdx.x < WARP_BAND) {
+        const int y = yb + threadIdx.x;
+        const double bu = i1 * y + i2, bv = i4 * y + i5;
+        s_x0[threadIdx.x] = __double2int_rn(bu * 1024.0) + 16;
+        s_y0[threadIdx.x] = __double2int_rn(bv * 1024.0) + 16;
+        double ulo, uhi, vlo, vhi;
+        footprint(i0, bu, it.w, ulo, uhi);
+        footprint(i3, bv, it.h, vlo, vhi);
+        const double lo = fmax(ulo, vlo), hi = fmin(uhi, vhi);
+        const bool any = lo <= hi;
+        const double edge = net_w + 1.0;
+        s_lo[threadIdx.x] = any ? (int)floor(fmin(fmax(lo, -2.0), edge)) - 1 : net_w + 8;
+        s_hi[threadIdx.x] = any ? (int)ceil(fmin(fmax(hi, -2.0), edge)) + 1 : -8;
+    }
+    __syncthreads();
+    const int x4 = xb + threadIdx.x * 4;
+    if (x4 >= net_w) return;
+    const AlignImageT<Src> img{it.src, it.w, it.h, 1.f, 0};
+    // every gather of the band before any store: a store may alias the source for all the compiler knows, so interleaving them would
+    // serialise the rows' gathers
+    int v[WARP_BAND][4][3] = {};
+#pragma unroll
+    for (int r = 0; r < WARP_BAND; r++) {
+        if (yb + r >= net_h || x4 + 3 < s_lo[r] || x4 > s_hi[r]) continue;
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            const int c = threadIdx.x * 4 + k;
+            sample<false>(img, (s_x0[r] + s_ax[c]) >> 5, (s_y0[r] + s_bx[c]) >> 5, v[r][k]);
+        }
+    }
+#pragma unroll
+    for (int r = 0; r < WARP_BAND; r++) {
+        if (yb + r >= net_h) break;
+        const int(*q)[3] = v[r];
+        uint32_t *o = reinterpret_cast<uint32_t *>(it.dst + ((size_t)(yb + r) * net_w + x4) * 3);
+        o[0] = q[0][0] | (q[0][1] << 8) | (q[0][2] << 16) | ((uint32_t)q[1][0] << 24);
+        o[1] = q[1][1] | (q[1][2] << 8) | (q[2][0] << 16) | ((uint32_t)q[2][1] << 24);
+        o[2] = q[2][2] | (q[3][0] << 8) | (q[3][1] << 16) | ((uint32_t)q[3][2] << 24);
+    }
+}
+}  // namespace
+
+template <typename Src>
+cudaError_t launch_letterbox_warp(const WarpItemT<Src> *items, int n, int net_w, int net_h, cudaStream_t s) {
+    if (n <= 0) return cudaSuccess;
+    if (n > WARP_MAX_VIEWS) return cudaErrorInvalidValue;
+    WarpBatch<Src> B{};
+    for (int i = 0; i < n; i++) B.v[i] = items[i];
+    k_letterbox_warp<Src><<<dim3((net_w + WARP_SPAN - 1) / WARP_SPAN, (net_h + WARP_BAND - 1) / WARP_BAND, n), WARP_THREADS, 0, s>>>(B, net_w, net_h);
+    return cudaGetLastError();
+}
+template cudaError_t launch_letterbox_warp<BgrRows>(const WarpItem *, int, int, int, cudaStream_t);
 
 template float letterbox_fill<BgrRows>(LbItem &, BgrRows, int, int, uint8_t *, int, int, int, int);
 template float letterbox_fill<YuvPlanes>(LbYuvItem &, YuvPlanes, int, int, uint8_t *, int, int, int, int);

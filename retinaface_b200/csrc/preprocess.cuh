@@ -95,4 +95,26 @@ template <typename Src>
 void tile_fill(LbItemT<Src> &it, typename LbItemT<Src>::Source src, int w, int h, int bits, uint8_t *dst, int net_w, int net_h,
                const rf_tile &tile);
 
+// ---- f23 rotated views (rf_b200.h rf_rotated_view) -------------------------------------------------------------------------------
+// The one statement of a view's geometry: the angle reduced, then either the EXIF orientation of a quarter turn (1, 8, 3, 6), or 0 and
+// the warp view's fit f, M and iM = cv::invertAffineTransform(M).  Host, FP64, no FMA contraction (preprocess.cu is built so).
+struct RotatedGeometry {
+    int orientation;
+    double f, M[6], iM[6];
+};
+RotatedGeometry rotated_geometry(float angle, int w, int h, int box_w, int box_h);
+// One warp view: the image w x h (stored) read through iM into dst (net_h x net_w x 3), cv2.warpAffine's fixed point.
+template <typename Src>
+struct WarpItemT {
+    Src src;
+    int w, h;
+    uint8_t *dst;
+    double im[6];
+};
+using WarpItem = WarpItemT<BgrRows>;
+constexpr int WARP_MAX_VIEWS = 16;     // RF_MAX_VIEWS: every warp view of a batch in one launch
+// k_letterbox_warp: n <= WARP_MAX_VIEWS items, one launch (none for n = 0)
+template <typename Src>
+cudaError_t launch_letterbox_warp(const WarpItemT<Src> *items, int n, int net_w, int net_h, cudaStream_t s);
+
 }  // namespace rf

@@ -38,8 +38,8 @@ __device__ inline bool fit_similarity(const rf_face &f, float scale, const doubl
     return true;
 }
 
-// cv::invertAffineTransform (double)
-__device__ inline void invert_affine(const double m[6], double im[6]) {
+// cv::invertAffineTransform (double); on the host for f23's rotated views
+__host__ __device__ inline void invert_affine(const double m[6], double im[6]) {
     double D = m[0] * m[4] - m[1] * m[3];
     D = D != 0.0 ? 1.0 / D : 0.0;
     const double a11 = m[4] * D, a22 = m[0] * D, a12 = -m[1] * D, a21 = -m[3] * D;

@@ -125,6 +125,25 @@ class RetinaFace:
         faces, _, _ = self.engine.detect_views_oriented(img, [(1.0, o) for o in ANY_ORIENTATION], threshold, self.nms_threshold)
         return [FaceDetectInfo.from_row(r) for r in faces]
 
+    def detectAnyAngle(self, img: np.ndarray, threshold: float = 0.5, step: float = 30.0, align: dict = None) -> list:
+        """f23 faces at any in-plane angle: the image rotated counter-clockwise by 0, step, 2 step ... below 360 degrees, each view fitted
+        into the network input (rf_detect_views_rotated; quarter turns take detectAnyOrientation's views), merged on the GPU.  Faces in
+        image pixels, axis-aligned boxes, landmarks carrying each face's roll.  With ``align`` (``Engine.detect_align``'s keywords), a list
+        of ``(FaceDetectInfo, crop)``, the crops upright.  More than 16 views (RF_MAX_VIEWS) is a ValueError."""
+        if not step > 0:
+            raise ValueError(f"step {step}: must be positive")
+        angles = [0.0]
+        while len(angles) <= 16 and len(angles) * float(step) < 360.0:
+            angles.append(len(angles) * float(step))
+        if len(angles) > 16:
+            raise ValueError(f"step {step} makes more than RF_MAX_VIEWS = 16 views")
+        if img is None or img.size == 0:
+            return []
+        out = self.engine.detect_views_rotated(img, [(a, 1.0) for a in angles], threshold, self.nms_threshold, align=align)
+        if align is None:
+            return [FaceDetectInfo.from_row(r) for r in out[0]]
+        return [(FaceDetectInfo.from_row(r), c) for r, c in zip(out[0], out[4])]
+
     def setVideoOrientation(self, video: int, orientation: int):
         """f20 oriented video (rf_tracker_set_orientation): ``video`` (-1: every video) is shown in EXIF orientation 1..8 -- portrait
         phone video stored as landscape surfaces -- and ``trackFrames`` / ``redactFrames`` read and write its frames as displayed, with

@@ -297,6 +297,30 @@ vector<FaceDetectInfo> RetinaFace::detectAnyOrientation(const Mat &img, float th
     return out;
 }
 
+vector<FaceDetectInfo> RetinaFace::detectAnyAngle(const Mat &img, float threshold, float step_deg, const AlignOptions *align) {
+    if (!(step_deg > 0.f)) throw std::invalid_argument("detectAnyAngle: step_deg must be positive");
+    vector<rf_rotated_view> views;
+    for (int k = 0; k * step_deg < 360.f; k++) {
+        if (views.size() == RF_MAX_VIEWS) throw std::invalid_argument("detectAnyAngle: more than RF_MAX_VIEWS views");
+        views.push_back(rf_rotated_view{k * step_deg, 1.f});
+    }
+    last_.assign(1, vector<FaceDetectInfo>());
+    scales_.assign(1, 1.f);
+    crops_.assign(1, vector<Mat>());
+    if (img.empty()) return last_[0];
+    int per = 0, cw = 0, ch = 0;
+    const rf_align_params p = align ? crop_params(*align, opt_.max_faces, &per, &cw, &ch) : rf_align_params{};
+    vector<unsigned char> crops(align ? (size_t)per * cw * ch * 3 : 0);
+    int count = 0;
+    int rc = rf_detect_views_rotated(h_, img.data, img.cols, img.rows, (int)img.step, views.data(), (int)views.size(), threshold, nms_threshold,
+                                     align ? &p : nullptr, out_faces_.data(), &count, nullptr, nullptr, nullptr, align ? crops.data() : nullptr,
+                                     nullptr);
+    if (rc != RF_OK) throw std::runtime_error(string("rf_detect_views_rotated: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+    out_counts_[0] = count;
+    keepResults(0, 1, align ? crops.data() : nullptr, per, cw, ch);
+    return last_[0];
+}
+
 void RetinaFace::trackYUV(const vector<rf_yuv_frame> &device_frames, const vector<int> &videos, float threshold, const AlignOptions *align,
                           void *dev_crops) {
     if (videos.size() != device_frames.size()) throw std::invalid_argument("trackYUV: one video index per frame");

@@ -143,6 +143,11 @@ class RetinaFace {
     // f9 unknown orientation (rf_detect_views_oriented): the image in its four rotations (EXIF 1, 6, 3, 8) as one batch, merged on
     // the GPU; faces in STORED image pixels, landmarks on the subject's sides (an aligned crop of a sideways face comes out upright).
     vector<FaceDetectInfo> detectAnyOrientation(const Mat &img, float threshold = 0.5);
+    // f23 faces at any in-plane angle (rf_detect_views_rotated): the image rotated counter-clockwise by 0, step_deg, 2 step_deg ... below
+    // 360 (at most RF_MAX_VIEWS views, else std::invalid_argument), merged on the GPU; faces in image pixels, landmarks carrying each
+    // face's roll.  With `align`, lastCrops()[0] holds the upright crops of the first min(faces, max_faces) faces (lastBatchFaces() and
+    // lastCrops() hold the one image).
+    vector<FaceDetectInfo> detectAnyAngle(const Mat &img, float threshold = 0.5, float step_deg = 30, const AlignOptions *align = nullptr);
     // f10 tracking (rf_detect_yuv_track_device): DEVICE 4:2:0 frames (descriptors of device planes, e.g. NVDEC surfaces; at most
     // max_batch per call), frame i of video videos[i] in [0, track_videos), detected and associated with the tracks of earlier frames
     // on the GPU.  Asynchronous on rf_last_stream(handle()).  Afterwards lastTracks() holds the device track lists; with `align`, the

@@ -488,6 +488,44 @@ int rf_detect_views_rotated(rf_handle h, const uint8_t *bgr, int width, int heig
 int rf_preprocess_rotated(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, float angle, float shrink,
                           uint8_t *out_net_sized, double *out_mat);
 
+/* f24 faces at any in-plane angle in device frames and video: f23's rotated views of device BGR images or NVDEC surfaces, n frames a
+ * call.  For each frame i the call returns exactly what rf_detect_views_rotated returns for that frame's pixels (for YUV,
+ * cv2.cvtColor(frame)) with the same views, bit for bit: records, kept count, the view of each face (anchor_index / max_faces, the
+ * candidate id v * max_faces + rank), crops and matrices.  A YUV warp view is cv2.warpAffine(cvtColor(frame), M) byte for byte (each
+ * tap converted as f6's letter-box converts it) and a YUV crop is f6's crop.  RF_FLAG_NPP_RESIZE changes only the quarter turns'
+ * letter-boxes, as in f23.
+ * The call is rf_detect_tiled_device / rf_detect_yuv_tiled_device (f8) with views in place of tiles: the same views apply to all
+ * n <= max_batch frames (more: RF_ERR_CAPACITY), frames are DEVICE memory read in place and never written, and the n * nviews network
+ * inputs run in chunks of max_batch over the rf_detect_batch_device rotation, each chunk counting as one call for that function's
+ * validity rule.  The final per-frame NMS and the crops run on the home stream, which rf_last_stream() returns.  *dev_dets ->
+ * [max_batch][max_faces] rf_det in FRAME pixels, *dev_dets / *dev_counts complete in stream order there; with scales NULL they feed
+ * rf_track_update, rf_redact_yuv_device_style and rf_redact_device_style.  The records live in a ring of `streams` output slots of
+ * their own: the returned pointers stay valid for `streams` further rotated device calls, and tiled device calls keep their own ring.
+ * out_view_scales (optional, host, [n][nviews]) and out_view_mats (optional, host, [n][nviews][6]) hold f23's values per frame -- a
+ * quarter turn's map-back factor and zero M, a warp view's (float)(1 / f) and M -- filled before return.  align != NULL: crops into
+ * dev_crops (required) and dev_mats (optional) as rf_detect_tiled_device's.  Checks, in this order and all before anything is launched
+ * or written: the frames as by the f8 twin (n included), views NULL (RF_ERR_INVALID_ARG), 1..RF_MAX_VIEWS views (else
+ * RF_ERR_CAPACITY), each view as by rf_detect_views_rotated, then the align params (align without dev_crops: RF_ERR_INVALID_ARG).
+ * n = 0 launches nothing. */
+int rf_detect_views_rotated_device(rf_handle h, const uint8_t *const *dev_bgr, const int *widths, const int *heights, const int *row_strides,
+                                   int n, const rf_rotated_view *views, int nviews, float score_threshold, float nms_threshold,
+                                   const rf_align_params *align, void *dev_crops, double *dev_mats, const rf_det **dev_dets,
+                                   const int32_t **dev_counts, float *out_view_scales, double *out_view_mats);
+int rf_detect_yuv_views_rotated_device(rf_handle h, const rf_yuv_frame *frames, int n, int matrix, const rf_rotated_view *views, int nviews,
+                                       float score_threshold, float nms_threshold, const rf_align_params *align, void *dev_crops,
+                                       double *dev_mats, const rf_det **dev_dets, const int32_t **dev_counts, float *out_view_scales,
+                                       double *out_view_mats);
+/* Preprocess parity of f24 (as rf_preprocess_rotated): the network input of the view (angle, shrink) of one HOST 4:2:0 frame, i.e.
+ * of cv2.cvtColor(frame), into a host net_h*net_w*3 u8 BGR buffer, and (out_mat optional, [6]) its M, all zero for a quarter turn. */
+int rf_preprocess_yuv_rotated(rf_handle h, const rf_yuv_frame *frame, int matrix, float angle, float shrink, uint8_t *out_net_sized,
+                              double *out_mat);
+/* The records of a device detect call (*dev_dets / *dev_counts of n <= max_batch images, while they are valid) on the host, for callers
+ * without a CUDA runtime of their own such as the C++ shell.  Blocking: waits for every execution context, then copies them into
+ * out_faces [n][max_faces] / out_counts [n] and, optional, their anchor_index into out_anchor_index [n][max_faces], rf_detect_batch's
+ * layout.  n = 0 copies nothing. */
+int rf_fetch_dets(rf_handle h, const rf_det *dev_dets, const int32_t *dev_counts, int n, rf_face *out_faces, int *out_counts,
+                  int32_t *out_anchor_index);
+
 /* f10 face tracking across video frames, on the GPU: per-video tracks with stable ids, so that a recogniser runs once per new
  * identity instead of once per face per frame, and counting / dwell time / "who entered" need no host round trip.  One tracker holds
  * max_videos independent sequences (cameras, files), each with up to max_tracks live tracks (tentative, confirmed and lost).

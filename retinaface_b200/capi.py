@@ -362,6 +362,10 @@ _SIGNATURES = {
     "rf_jpeg_exif_orientation": (_I, [_P, C.c_size_t]),
     "rf_detect_views_rotated": (_I, [_P, _P, _I, _I, _I, C.POINTER(_RotatedView), _I, _F, _F, _ALIGN, _P, _PI, _P, _P, _P, _P, _P]),
     "rf_preprocess_rotated": (_I, [_P, _P, _I, _I, _I, _F, _F, _P, _P]),
+    "rf_detect_views_rotated_device": (_I, [_P, _PP, _PI, _PI, _PI, _I, C.POINTER(_RotatedView), _I, _F, _F, _ALIGN, _P, _P, _PP, _PP, _P, _P]),
+    "rf_detect_yuv_views_rotated_device": (_I, [_P, _FRAMES, _I, _I, C.POINTER(_RotatedView), _I, _F, _F, _ALIGN, _P, _P, _PP, _PP, _P, _P]),
+    "rf_preprocess_yuv_rotated": (_I, [_P, _FRAMES, _I, _F, _F, _P, _P]),
+    "rf_fetch_dets": (_I, [_P, _P, _P, _I, _P, _P, _P]),
     "rf_tracker_create": (_I, [_P, C.POINTER(TrackConfig), _PP]), "rf_tracker_destroy": (None, [_P]),
     "rf_tracker_reset": (_I, [_P, _I]),
     "rf_track_update": (_I, [_P, _P, _I, _P, _P, _P, _PP, _PP]),
@@ -1086,6 +1090,49 @@ class Engine:
         mat = np.empty((2, 3), dtype=np.float64)
         self._check(self.lib.rf_preprocess_rotated(self.h, img.ctypes.data, img.shape[1], img.shape[0], img.strides[0], C.c_float(angle),
                                                    C.c_float(shrink), out.ctypes.data, mat.ctypes.data))
+        return out, mat
+
+    # -- f24 faces at any in-plane angle in device frames ------------------------------------------------------------------------
+    def _rotated_device(self, fn, sources, n: int, views, thr: float, nms: float, align: Optional[dict], dev_crops_ptr, dev_mats_ptr):
+        """One rotated device call: fn(sources..., views, nviews, thr, nms, align, crops, mats, &dets, &counts, scales, mats) ->
+        (dets_ptr, counts_ptr, view scales [n, nviews], view M [n, nviews, 2, 3])."""
+        nv = len(views)
+        varr = (_RotatedView * max(nv, 1))(*[_RotatedView(float(a), float(s)) for a, s in views])
+        p = align_params(**align) if align is not None else None
+        scales = np.zeros((max(n, 1), max(nv, 1)), dtype=np.float32)
+        mats = np.zeros((max(n, 1), max(nv, 1), 2, 3), dtype=np.float64)
+        d, c = C.c_void_p(), C.c_void_p()
+        self._check(fn(self.h, *sources, varr, nv, C.c_float(thr), C.c_float(nms), _ref(p), dev_crops_ptr, dev_mats_ptr, C.byref(d), C.byref(c),
+                       scales.ctypes.data, mats.ctypes.data))
+        return int(d.value or 0), int(c.value or 0), scales[:n, :nv].copy(), mats[:n, :nv].copy()
+
+    def detect_views_rotated_device(self, images, views, thr: float, nms: float, align: Optional[dict] = None,
+                                    dev_crops_ptr: Optional[int] = None, dev_mats_ptr: Optional[int] = None):
+        """rf_detect_views_rotated_device: u8 BGR HWC torch CUDA tensors (rows may be strided), each run through the views
+        [(angle, shrink), ...] of detect_views_rotated, asynchronous on last_stream_ptr().  Returns (dets_ptr, counts_ptr, map-back
+        scale of each view [n, nviews], M of each view [n, nviews, 2, 3], zeros for quarter turns): [max_batch][max_faces] rf_det in
+        IMAGE pixels, anchor_index = view * max_faces + rank, valid for `streams` further rotated device calls.  align:
+        detect_align's keywords; the crops land at dev_crops_ptr as in detect_align_device.  Host arrays: ValueError."""
+        ptrs, ws, hs, rs = self._device_images(images)
+        return self._rotated_device(self.lib.rf_detect_views_rotated_device, (ptrs, ws, hs, rs, len(images)), len(images), views, thr, nms,
+                                    align, dev_crops_ptr, dev_mats_ptr)
+
+    def detect_yuv_views_rotated_device(self, frames, views, thr: float, nms: float, layout: str = "nv12", matrix="bt601",
+                                        align: Optional[dict] = None, dev_crops_ptr: Optional[int] = None, dev_mats_ptr: Optional[int] = None):
+        """rf_detect_yuv_views_rotated_device: device 4:2:0 frames (torch CUDA tensors in yuv_frame's forms), otherwise as
+        detect_views_rotated_device (faces in FRAME pixels).  Host frames: ValueError."""
+        arr = self._frames(frames, layout, True)
+        return self._rotated_device(self.lib.rf_detect_yuv_views_rotated_device, (arr, len(frames), _matrix(matrix)), len(frames), views, thr,
+                                    nms, align, dev_crops_ptr, dev_mats_ptr)
+
+    def preprocess_yuv_rotated(self, frame, angle: float, shrink: float = 1.0, layout: str = "nv12", matrix="bt601"):
+        """rf_preprocess_yuv_rotated: (the (H, W, 3) u8 BGR network input of the view (angle, shrink) of one host frame, its M [2, 3],
+        zeros for a quarter turn)."""
+        arr = self._frames([frame], layout, False)
+        out = np.empty((self.net_h, self.net_w, 3), dtype=np.uint8)
+        mat = np.empty((2, 3), dtype=np.float64)
+        self._check(self.lib.rf_preprocess_yuv_rotated(self.h, arr, _matrix(matrix), C.c_float(angle), C.c_float(shrink), out.ctypes.data,
+                                                       mat.ctypes.data))
         return out, mat
 
     # -- f21 tiled detection of rotated and mirrored images ---------------------------------------------------------------------

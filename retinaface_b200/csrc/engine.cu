@@ -241,11 +241,12 @@ void destroy(rf_handle h) {
     for (Ctx &c : h->ctx) release_ctx(c, true);
     free_post_buffers(h->pb_merge);
     free_post_buffers(h->pb_tiles);
-    for (auto &s : h->tiled_slots) {
-        free_post_buffers(s.pb);
-        if (s.free) cudaEventDestroy(s.free);
-        if (s.start) cudaEventDestroy(s.start);
-    }
+    for (auto *ring : {&h->tiled_slots, &h->rotated_slots})
+        for (auto &s : *ring) {
+            free_post_buffers(s.pb);
+            if (s.free) cudaEventDestroy(s.free);
+            if (s.start) cudaEventDestroy(s.start);
+        }
     cudaFree(h->d_weights); cudaFree(h->d_weights_h); cudaFree(h->d_weights_q); cudaFree(h->d_input); cudaFree(h->d_raw);
     for (auto p : h->d_blobs) cudaFree(p);
     h->copy_pool.reset();
@@ -952,28 +953,64 @@ static int tiled_check(rf_handle h, const char *who, const Source &src, int n, c
     return aligned ? check_align(h, who, align, n, crops, resident ? n : 0, a) : RF_OK;
 }
 
-// Tiled detection of n images whose layouts are checked, into `dst` (its candidate lists empty: allocation and every k_nms leave
-// them so), the final NMS on `home`.  The blocking paths upload image i into raw buffer `slot` on home, a `group` of raw buffers at
-// a time; with `in_place` (one group), the device paths read the caller's memory.  The
-// tiles are letter-boxed, detected and merged in chunks of up to max_batch, each chunk on the next context of the
-// rf_detect_batch_device rotation, into that context's own input tensor.  Another context waits for `ready` -- recorded on home
-// once the group's sources are on the device and `dst` may be written -- before its first letter-box of the group, or, with
-// `in_place` (the sources are the caller's device memory), only before its first merge.  Home waits for every context the group
-// used before the next group overwrites the raw buffers, and before the final NMS.
+// The network inputs of one chunk: letter-box items with their merge sources in batch slots 0 .. lb.size() - 1 (launch_merge reads
+// contiguous slots from 0), then f24's warp views with their rotated merge sources in the slots after them.
+template <typename Src>
+struct ChunkWork {
+    std::vector<LbItemT<Src>> lb;
+    std::vector<MergeSource> ms;
+    std::vector<WarpItemT<Src>> wp;
+    std::vector<RotatedSource> rs;
+};
+// One network input of a chunked call: tile `item` of image `image`'s layout, or view `item` of it (f24).
+struct Job { int image, item; };
+
+// The jobs of the tiled paths: every tile of each image's layout.
 template <typename Source>
-static void detect_tiled_impl(rf_handle h, const Source &source, int n, const std::vector<std::vector<rf_tile>> &layouts, int group, bool in_place,
-                              Ctx &home, cudaEvent_t ready, PostBuffers &dst, float thr, float nms, std::vector<typename Source::Src> &src) {
-    const int Hn = h->cfg.net_h, Wn = h->cfg.net_w, mf = h->cfg.max_faces, B = h->cfg.max_batch;
+struct TileJobs {
+    rf_handle h;
+    const Source &source;
+    const std::vector<std::vector<rf_tile>> &layouts;
+    int count(int i) const { return (int)layouts[i].size(); }
+    void fill(const Job *jobs, int m, const std::vector<typename Source::Src> &src, uint8_t *input, ChunkWork<typename Source::Src> &w) const {
+        const int Hn = h->cfg.net_h, Wn = h->cfg.net_w;
+        const size_t img_bytes = (size_t)Hn * Wn * 3;
+        w.lb.resize(m);
+        w.ms.resize(m);
+        for (int b = 0; b < m; b++) {
+            const Job r = jobs[b];
+            const rf_tile &tl = layouts[r.image][r.item];
+            int dw, dh;
+            displayed_size(source, r.image, dw, dh);
+            tile_fill(w.lb[b], src[r.image], dw, dh, source.bits(r.image), input + b * img_bytes, Wn, Hn, tl);
+            // records stay in displayed pixels: a mirrored level is un-mirrored with the displayed width (k_merge<false>)
+            w.ms[b] = tile_source(r.image, r.item, h->cfg.max_faces, tl, dw);
+        }
+    }
+};
+
+// Chunked detection of n checked images, into `dst` (its candidate lists empty: allocation and every k_nms leave them so), the final
+// NMS on `home`.  Image i contributes jobs.count(i) network inputs (tiles, or f24's views), which jobs.fill turns into a chunk's
+// letter-box / warp items and merge sources.  The blocking paths upload image i into raw buffer `slot` on home, a `group` of raw
+// buffers at a time; with `in_place` (one group), the device paths read the caller's memory.  The network inputs are made, detected
+// and merged in chunks of up to max_batch, each chunk on the next context of the rf_detect_batch_device rotation, into that context's
+// own input tensor.  Another context waits for `ready` -- recorded on home once the group's sources are on the device and `dst` may be
+// written -- before its first letter-box of the group, or, with `in_place` (the sources are the caller's device memory), only before
+// its first merge.  Home waits for every context the group used before the next group overwrites the raw buffers, and before the
+// final NMS.
+template <typename Source, typename Jobs>
+static void detect_chunked(rf_handle h, const Source &source, int n, const Jobs &jobs, int group, bool in_place, Ctx &home, cudaEvent_t ready,
+                           PostBuffers &dst, float thr, float nms, std::vector<typename Source::Src> &src) {
+    const int Hn = h->cfg.net_h, Wn = h->cfg.net_w, B = h->cfg.max_batch;
     const size_t img_bytes = (size_t)Hn * Wn * 3;
     src.resize(n);
-    struct TileRef { int image, tile; };
     for (int g0 = 0; g0 < n; g0 += group) {
         const int g1 = std::min(n, g0 + group);
         for (int i = g0; i < g1; i++) src[i] = in_place ? source.in_place(i) : source.upload(h, home.stream, i, i - g0);
         CK(cudaEventRecord(ready, home.stream));
-        std::vector<TileRef> refs;
+        std::vector<Job> refs;
         for (int i = g0; i < g1; i++)
-            for (int k = 0; k < (int)layouts[i].size(); k++) refs.push_back(TileRef{i, k});
+            for (int k = 0; k < jobs.count(i); k++) refs.push_back(Job{i, k});
         std::vector<char> joined(h->ctx.size(), 0);
         for (size_t k0 = 0; k0 < refs.size(); k0 += B) {
             const int m = (int)std::min<size_t>(B, refs.size() - k0);
@@ -984,22 +1021,15 @@ static void detect_tiled_impl(rf_handle h, const Source &source, int n, const st
             joined[ci] = 1;
             if (!c.d_frames_in) CK(cudaMalloc(&c.d_frames_in, (size_t)B * img_bytes));
             if (c.param_seq && c.param_seq % Ctx::kParamSlots == 0) CK(cudaStreamSynchronize(c.stream));
-            std::vector<LbItemT<typename Source::Src>> lb(m);
-            std::vector<MergeSource> ms(m);
-            for (int b = 0; b < m; b++) {
-                const TileRef r = refs[k0 + b];
-                const rf_tile &tl = layouts[r.image][r.tile];
-                int dw, dh;
-                displayed_size(source, r.image, dw, dh);
-                tile_fill(lb[b], src[r.image], dw, dh, source.bits(r.image), c.d_frames_in + b * img_bytes, Wn, Hn, tl);
-                // records stay in displayed pixels: a mirrored level is un-mirrored with the displayed width (k_merge<false>)
-                ms[b] = tile_source(r.image, r.tile, mf, tl, dw);
-            }
-            CK(launch_letterbox_batch(lb.data(), m, Wn, Hn, c.stream));
+            ChunkWork<typename Source::Src> w;
+            jobs.fill(&refs[k0], m, src, c.d_frames_in, w);
+            CK(launch_letterbox_batch(w.lb.data(), (int)w.lb.size(), Wn, Hn, c.stream));
+            CK(launch_letterbox_warp(w.wp.data(), (int)w.wp.size(), Wn, Hn, c.stream));
             set_params(h, c, thr, nms, c.d_frames_in);
             forward_graph(h, c, m);
             if (wait && in_place) CK(cudaStreamWaitEvent(c.stream, ready, 0));
-            CK(launch_merge(c.pb, ms.data(), m, Wn, Hn, dst, c.stream));
+            CK(launch_merge(c.pb, w.ms.data(), (int)w.ms.size(), Wn, Hn, dst, c.stream));
+            CK(launch_merge_rotated(c.pb, w.rs.data(), (int)w.rs.size(), dst, c.stream));
         }
         for (size_t ci = 0; ci < h->ctx.size(); ci++) {
             if (!joined[ci] || &h->ctx[ci] == &home) continue;
@@ -1007,17 +1037,23 @@ static void detect_tiled_impl(rf_handle h, const Source &source, int n, const st
             CK(cudaStreamWaitEvent(home.stream, h->ctx[ci].fence, 0));
         }
     }
-    // the final NMS over each image's candidates from all its tiles and levels reads its threshold from home's parameters
+    // the final NMS over each image's candidates from all its network inputs reads its threshold from home's parameters
     if (home.param_seq && home.param_seq % Ctx::kParamSlots == 0) CK(cudaStreamSynchronize(home.stream));
     set_params(h, home, thr, nms);
     CK(launch_nms(n, home.d_params, dst, home.stream));
     CK(cudaGetLastError());
 }
 
-// Makes room in pb for the candidates of the largest layout: every tile of an image may contribute max_faces.
-static bool tiled_grow(rf_handle h, PostBuffers &pb, const std::vector<std::vector<rf_tile>> &layouts) {
-    size_t most = 0;
-    for (const auto &l : layouts) most = std::max(most, l.size());
+// The most network inputs any of the n images contributes: every one may contribute max_faces candidates.
+template <typename Jobs>
+static size_t most_jobs(const Jobs &jobs, int n) {
+    int most = 0;
+    for (int i = 0; i < n; i++) most = std::max(most, jobs.count(i));
+    return (size_t)most;
+}
+
+// Makes room in pb for `most` * max_faces candidates per image.
+static bool chunked_grow(rf_handle h, PostBuffers &pb, size_t most) {
     const int mf = h->cfg.max_faces;
     if ((size_t)pb.anchors_per_image >= most * mf) return false;
     free_post_buffers(pb);
@@ -1054,10 +1090,11 @@ static int detect_tiled_blocking(rf_handle h, const char *who, const Source &sou
     try {
         CK(cudaSetDevice(h->device));
         const int mf = h->cfg.max_faces;
-        tiled_grow(h, h->pb_tiles, layouts);
+        const TileJobs<Source> jobs{h, source, layouts};
+        chunked_grow(h, h->pb_tiles, most_jobs(jobs, n));
         Ctx &c0 = h->ctx[0];
         std::vector<typename Source::Src> srcs;
-        detect_tiled_impl(h, source, n, layouts, h->raw_slots, false, c0, c0.fence, h->pb_tiles, thr, nms, srcs);
+        detect_chunked(h, source, n, jobs, h->raw_slots, false, c0, c0.fence, h->pb_tiles, thr, nms, srcs);
         if (aligned) {
             ensure_align_buffers(h, n, a);
             a.crops = h->d_align_crops;
@@ -1073,8 +1110,9 @@ static int detect_tiled_blocking(rf_handle h, const char *who, const Source &sou
     return RF_OK;
 }
 
-// The asynchronous tiled paths: the caller's device sources src[i] read in place, merged into the next slot of the ring, the final
-// NMS and the crops on the home stream (the context the call's first chunk lands on), which rf_last_stream returns.
+// The asynchronous chunked paths (tiles, and f24's rotated views): the caller's device sources src[i] read in place, merged into the
+// next slot of `ring` (the tiled and the rotated calls each have their own), the final NMS and the crops on the home stream (the
+// context the call's first chunk lands on), which rf_last_stream returns.
 //   1. Home waits for the slot's `free` event before anything merges into it and records `start`; every other context waits for
 //      `start` before its first merge (k_nms left the slot's candidate counts at zero).
 //   2. A slot that must grow is freed only after the host has waited for `free`, and its counts are cleared on home before `start`.
@@ -1082,31 +1120,31 @@ static int detect_tiled_blocking(rf_handle h, const char *who, const Source &sou
 //   4. The crops are cut on home after the NMS; then `free` is recorded.
 //   5. A caller that reads the records later on home (a tracker call, f19) gets `free` back and records it again after its last read,
 //      so that a later call on this slot, whose home may be another context, waits for those reads too.
-// tiled_device_issue issues a checked call of n > 0 images (align: a.crops / a.mats set, or NULL; `free` may be NULL).
-template <typename Source>
-static void tiled_device_issue(rf_handle h, const Source &source, int n, const std::vector<std::vector<rf_tile>> &layouts, float thr, float nms,
-                               const AlignArgs *align, const rf_det **dev_dets, const int32_t **dev_counts, cudaEvent_t *free) {
+// device_issue issues a checked call of n > 0 images (align: a.crops / a.mats set, or NULL; `free` may be NULL).
+template <typename Source, typename Jobs>
+static void device_issue(rf_handle h, std::vector<rf_handle_s::TiledSlot> &ring, unsigned &next_slot, const Source &source, int n,
+                         const Jobs &jobs, float thr, float nms, const AlignArgs *align, const rf_det **dev_dets, const int32_t **dev_counts,
+                         cudaEvent_t *free) {
     CK(cudaSetDevice(h->device));
-    if (h->tiled_slots.empty()) {
-        h->tiled_slots.resize(h->ctx.size());
-        for (auto &s : h->tiled_slots) {
+    if (ring.empty()) {
+        ring.resize(h->ctx.size());
+        for (auto &s : ring) {
             CK(cudaEventCreateWithFlags(&s.free, cudaEventDisableTiming));
             CK(cudaEventCreateWithFlags(&s.start, cudaEventDisableTiming));
         }
     }
-    rf_handle_s::TiledSlot &slot = h->tiled_slots[h->next_tiled_slot++ % h->tiled_slots.size()];
+    rf_handle_s::TiledSlot &slot = ring[next_slot++ % ring.size()];
     Ctx &home = h->ctx[h->next_dev_ctx % h->ctx.size()];
-    size_t most = 0;
-    for (const auto &l : layouts) most = std::max(most, l.size());
+    const size_t most = most_jobs(jobs, n);
     if ((size_t)slot.pb.anchors_per_image < most * h->cfg.max_faces) {
         CK(cudaEventSynchronize(slot.free));     // the slot's last call has finished with the buffers about to be freed
-        tiled_grow(h, slot.pb, layouts);
+        chunked_grow(h, slot.pb, most);
         // alloc_post_buffers clears the counts on the legacy stream, which the contexts' streams do not wait for
         CK(cudaMemsetAsync(slot.pb.cand_count, 0, sizeof(int) * slot.pb.max_batch, home.stream));
     }
     CK(cudaStreamWaitEvent(home.stream, slot.free, 0));
     std::vector<typename Source::Src> srcs;
-    detect_tiled_impl(h, source, n, layouts, n, true, home, slot.start, slot.pb, thr, nms, srcs);
+    detect_chunked(h, source, n, jobs, n, true, home, slot.start, slot.pb, thr, nms, srcs);
     if (align) tiled_crops(h, *align, n, source, srcs, slot.pb, home.stream);
     CK(cudaEventRecord(slot.free, home.stream));
     h->last_stream = home.stream;
@@ -1125,7 +1163,8 @@ static int detect_tiled_device(rf_handle h, const char *who, const Source &sourc
     a.crops = dev_crops;
     a.mats = dev_mats;
     try {
-        tiled_device_issue(h, source, n, layouts, thr, nms, align ? &a : nullptr, dev_dets, dev_counts, nullptr);
+        device_issue(h, h->tiled_slots, h->next_tiled_slot, source, n, TileJobs<Source>{h, source, layouts}, thr, nms, align ? &a : nullptr,
+                     dev_dets, dev_counts, nullptr);
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }
@@ -1140,7 +1179,8 @@ int rf_eng::yuv_tiled_check(rf_handle h, const char *who, const YuvFrames &src, 
 int rf_eng::yuv_tiled_issue(rf_handle h, const YuvFrames &src, int n, const std::vector<std::vector<rf_tile>> &layouts, float thr, float nms,
                             const rf_det **dev_dets, const int32_t **dev_counts, cudaEvent_t *free) {
     try {
-        tiled_device_issue(h, src, n, layouts, thr, nms, nullptr, dev_dets, dev_counts, free);
+        device_issue(h, h->tiled_slots, h->next_tiled_slot, src, n, TileJobs<YuvFrames>{h, src, layouts}, thr, nms, nullptr, dev_dets,
+                     dev_counts, free);
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }
@@ -1537,6 +1577,48 @@ static void shrink_box(rf_handle h, float shrink, int &bw, int &bh) {
     bh = std::max(1, (int)(h->cfg.net_h * shrink));
 }
 
+// The geometry of view (angle, shrink) of a width x height image
+static RotatedGeometry view_geometry(rf_handle h, const rf_rotated_view &view, int width, int height) {
+    int bw, bh;
+    shrink_box(h, view.shrink, bw, bh);
+    return rotated_geometry(view.angle, width, height, bw, bh);
+}
+
+// M of a view as the calls report it: all zero for a quarter turn
+static void put_view_mat(const RotatedGeometry &g, double *out) {
+    for (int k = 0; k < 6; k++) out[k] = g.orientation ? 0.0 : g.M[k];
+}
+
+extern "C++" {
+// View v of image `image` (width x height, stored) into batch slot b, whose input is dst: a quarter turn appends
+// rf_detect_views_oriented's letter-box item and merge source (its slot is b = w.lb.size()), a warp view a warp item and its rotated
+// merge source.  Returns the view's map-back scale: the letter-box's factor, or (float)(1 / f).
+template <typename Src>
+static float rotated_item(rf_handle h, const RotatedGeometry &g, float shrink, int v, int image, Src src, int width, int height, int b,
+                          uint8_t *dst, ChunkWork<Src> &w) {
+    const int mf = h->cfg.max_faces;
+    if (g.orientation) {
+        int bw, bh;
+        shrink_box(h, shrink, bw, bh);
+        const int bits = lb_orientation_bits(g.orientation);
+        const int dw = (bits & LB_TRANSPOSE) ? height : width, dh = (bits & LB_TRANSPOSE) ? width : height;
+        w.lb.emplace_back();
+        const float scale = letterbox_fill(w.lb.back(), src, dw, dh, dst, bw, bh, bits, (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0);
+        MergeSource m = (bits & ~LB_FLIP_X) ? oriented_view_source(v, mf, scale, bits, dw, dh) : view_source(v, mf, scale, bits, width);
+        m.image = image;
+        w.ms.push_back(m);
+        return scale;
+    }
+    WarpItemT<Src> it{src, width, height, dst, {}};
+    std::copy(g.iM, g.iM + 6, it.im);
+    w.wp.push_back(it);
+    RotatedSource r{b, v * mf, image, {}, 1.0 / (2.0 * g.f)};
+    std::copy(g.iM, g.iM + 6, r.im);
+    w.rs.push_back(r);
+    return (float)(1.0 / g.f);
+}
+}  // extern "C++"
+
 int rf_detect_views_rotated(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, const rf_rotated_view *views, int nviews,
                             float thr, float nms, const rf_align_params *align, rf_face *out_faces, int *out_count, int32_t *out_view_of,
                             float *out_view_scales, double *out_view_mats, void *out_crops, double *out_mats) {
@@ -1554,14 +1636,11 @@ int rf_detect_views_rotated(rf_handle h, const uint8_t *bgr, int width, int heig
     static_assert(RF_MAX_VIEWS == RF_MAX_VIEWS_DEV && RF_MAX_VIEWS == WARP_MAX_VIEWS, "view capacity of the warp and merge kernels");
     const int Hn = h->cfg.net_h, Wn = h->cfg.net_w, mf = h->cfg.max_faces, B = h->cfg.max_batch;
     const size_t img_bytes = (size_t)Hn * Wn * 3;
-    const int area = (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0;
     // the quarter turns first: within a batch they take slots 0 .. k-1, as launch_merge reads them; ids keep the caller's order
     std::vector<RotatedGeometry> geo(nviews);
     std::vector<int> order;
     for (int v = 0; v < nviews; v++) {
-        int bw, bh;
-        shrink_box(h, views[v].shrink, bw, bh);
-        geo[v] = rotated_geometry(views[v].angle, width, height, bw, bh);
+        geo[v] = view_geometry(h, views[v], width, height);
         if (geo[v].orientation) order.push_back(v);
     }
     for (int v = 0; v < nviews; v++)
@@ -1578,41 +1657,18 @@ int rf_detect_views_rotated(rf_handle h, const uint8_t *bgr, int width, int heig
         set_params(h, c, thr, nms);
         for (int v0 = 0; v0 < nviews; v0 += B) {
             const int m = std::min(B, nviews - v0);
-            std::vector<LbItem> lb;
-            std::vector<MergeSource> ms;
-            std::vector<WarpItem> wp;
-            std::vector<RotatedSource> rs;
+            ChunkWork<BgrRows> w;
             for (int b = 0; b < m; b++) {
                 const int v = order[v0 + b];
-                const RotatedGeometry &g = geo[v];
-                uint8_t *dst = h->d_input + (size_t)b * img_bytes;
-                float scale;
-                if (g.orientation) {      // rf_detect_views_oriented's view, slot b < k
-                    int bw, bh;
-                    shrink_box(h, views[v].shrink, bw, bh);
-                    const int bits = lb_orientation_bits(g.orientation);
-                    const int dw = (bits & LB_TRANSPOSE) ? height : width, dh = (bits & LB_TRANSPOSE) ? width : height;
-                    lb.emplace_back();
-                    scale = letterbox_fill(lb.back(), d_src, dw, dh, dst, bw, bh, bits, area);
-                    ms.push_back((bits & ~LB_FLIP_X) ? oriented_view_source(v, mf, scale, bits, dw, dh) : view_source(v, mf, scale, bits, width));
-                } else {
-                    WarpItem w{d_src, width, height, dst, {}};
-                    std::copy(g.iM, g.iM + 6, w.im);
-                    wp.push_back(w);
-                    RotatedSource r{b, v * mf, {}, 1.0 / (2.0 * g.f)};
-                    std::copy(g.iM, g.iM + 6, r.im);
-                    rs.push_back(r);
-                    scale = (float)(1.0 / g.f);
-                }
+                const float scale = rotated_item(h, geo[v], views[v].shrink, v, 0, d_src, width, height, b, h->d_input + (size_t)b * img_bytes, w);
                 if (out_view_scales) out_view_scales[v] = scale;
-                if (out_view_mats)
-                    for (int k = 0; k < 6; k++) out_view_mats[(size_t)v * 6 + k] = g.orientation ? 0.0 : g.M[k];
+                if (out_view_mats) put_view_mat(geo[v], out_view_mats + (size_t)v * 6);
             }
-            CK(launch_letterbox_batch(lb.data(), (int)lb.size(), Wn, Hn, c.stream));
-            CK(launch_letterbox_warp(wp.data(), (int)wp.size(), Wn, Hn, c.stream));
+            CK(launch_letterbox_batch(w.lb.data(), (int)w.lb.size(), Wn, Hn, c.stream));
+            CK(launch_letterbox_warp(w.wp.data(), (int)w.wp.size(), Wn, Hn, c.stream));
             forward_graph(h, c, m);
-            CK(launch_merge(c.pb, ms.data(), (int)ms.size(), Wn, Hn, h->pb_merge, c.stream));
-            CK(launch_merge_rotated(c.pb, rs.data(), (int)rs.size(), h->pb_merge, c.stream));
+            CK(launch_merge(c.pb, w.ms.data(), (int)w.ms.size(), Wn, Hn, h->pb_merge, c.stream));
+            CK(launch_merge_rotated(c.pb, w.rs.data(), (int)w.rs.size(), h->pb_merge, c.stream));
         }
         CK(launch_nms(1, c.d_params, h->pb_merge, c.stream));
         if (align) {
@@ -1641,38 +1697,131 @@ int rf_detect_views_rotated(rf_handle h, const uint8_t *bgr, int width, int heig
     return RF_OK;
 }
 
-int rf_preprocess_rotated(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, float angle, float shrink, uint8_t *out,
-                          double *out_mat) {
-    const char *who = "rf_preprocess_rotated";
+extern "C++" {
+// The network input of one view of image 0 of src, either kind, into `out`, and its M (f23 / f24's parity hooks).
+template <typename Source>
+static int preprocess_rotated(rf_handle h, const char *who, const Source &src, float angle, float shrink, uint8_t *out, double *out_mat) {
     if (!h) return RF_ERR_INVALID_ARG;
     if (!out) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: out is NULL", who));
-    const BgrImages src{&bgr, &width, &height, &row_stride, nullptr, false};
     int rc = src.check(h, who, 1);
     if (rc || (rc = check_rotated(h, who, angle, shrink, 0))) return rc;
     const int Hn = h->cfg.net_h, Wn = h->cfg.net_w;
-    int bw, bh;
-    shrink_box(h, shrink, bw, bh);
-    const RotatedGeometry g = rotated_geometry(angle, width, height, bw, bh);
+    const RotatedGeometry g = view_geometry(h, rf_rotated_view{angle, shrink}, src.width(0), src.height(0));
     try {
         CK(cudaSetDevice(h->device));
         cudaStream_t s = h->ctx[0].stream;
-        const BgrRows p = src.upload(h, s, 0, 0);
-        if (g.orientation) {
-            const int bits = lb_orientation_bits(g.orientation);
-            const int dw = (bits & LB_TRANSPOSE) ? height : width, dh = (bits & LB_TRANSPOSE) ? width : height;
-            LbItem it;
-            letterbox_fill(it, p, dw, dh, h->d_input, bw, bh, bits, (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0);
-            CK(launch_letterbox_batch(&it, 1, Wn, Hn, s));
-        } else {
-            WarpItem w{p, width, height, h->d_input, {}};
-            std::copy(g.iM, g.iM + 6, w.im);
-            CK(launch_letterbox_warp(&w, 1, Wn, Hn, s));
-        }
+        ChunkWork<typename Source::Src> w;
+        rotated_item(h, g, shrink, 0, 0, src.upload(h, s, 0, 0), src.width(0), src.height(0), 0, h->d_input, w);
+        CK(launch_letterbox_batch(w.lb.data(), (int)w.lb.size(), Wn, Hn, s));
+        CK(launch_letterbox_warp(w.wp.data(), (int)w.wp.size(), Wn, Hn, s));
         CK(cudaMemcpyAsync(h->h_input, h->d_input, (size_t)Hn * Wn * 3, cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
         memcpy(out, h->h_input, (size_t)Hn * Wn * 3);
-        if (out_mat)
-            for (int k = 0; k < 6; k++) out_mat[k] = g.orientation ? 0.0 : g.M[k];
+        if (out_mat) put_view_mat(g, out_mat);
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
+}
+}  // extern "C++"
+
+int rf_preprocess_rotated(rf_handle h, const uint8_t *bgr, int width, int height, int row_stride, float angle, float shrink, uint8_t *out,
+                          double *out_mat) {
+    return preprocess_rotated(h, "rf_preprocess_rotated", BgrImages{&bgr, &width, &height, &row_stride, nullptr, false}, angle, shrink, out,
+                              out_mat);
+}
+
+// ---- f24 rotated views of device frames (rf_b200.h) -----------------------------------------------------------------------------
+extern "C++" {
+// The jobs of a rotated device call: every view of each frame, geometry geo[i * nviews + v] of frame i's size.  Within a chunk the
+// quarter turns take the first slots (launch_merge reads contiguous slots from 0); ids carry the caller's view index, so the slot
+// order does not change a result.  Each job's map-back scale goes to scales[i * nviews + v].
+template <typename Source>
+struct RotatedJobs {
+    rf_handle h;
+    const Source &source;
+    const rf_rotated_view *views;
+    int nviews;
+    const std::vector<RotatedGeometry> &geo;
+    float *scales;
+    int count(int) const { return nviews; }
+    void fill(const Job *jobs, int m, const std::vector<typename Source::Src> &src, uint8_t *input, ChunkWork<typename Source::Src> &w) const {
+        const size_t img_bytes = (size_t)h->cfg.net_h * h->cfg.net_w * 3;
+        int b = 0;
+        for (int warp = 0; warp < 2; warp++)
+            for (int j = 0; j < m; j++) {
+                const Job r = jobs[j];
+                const size_t k = (size_t)r.image * nviews + r.item;
+                if ((geo[k].orientation == 0) != (warp == 1)) continue;
+                scales[k] = rotated_item(h, geo[k], views[r.item].shrink, r.item, r.image, src[r.image], source.width(r.image),
+                                         source.height(r.image), b, input + (size_t)b * img_bytes, w);
+                b++;
+            }
+    }
+};
+
+// rf_detect_views_rotated_device / rf_detect_yuv_views_rotated_device: the checks (the source, the views, then align), then the issue
+// into the rotated ring.
+template <typename Source>
+static int detect_rotated_device(rf_handle h, const char *who, const Source &source, int n, const rf_rotated_view *views, int nviews, float thr,
+                                 float nms, const rf_align_params *align, void *dev_crops, double *dev_mats, const rf_det **dev_dets,
+                                 const int32_t **dev_counts, float *out_view_scales, double *out_view_mats) {
+    int rc = source.check(h, who, n);
+    if (rc) return rc;
+    if (!views) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: views is NULL", who));
+    if (nviews < 1 || nviews > RF_MAX_VIEWS)
+        return fail(h, RF_ERR_CAPACITY, fmt("%s: %d views, limit RF_MAX_VIEWS = %d", who, nviews, RF_MAX_VIEWS));
+    for (int v = 0; v < nviews; v++)
+        if ((rc = check_rotated(h, who, views[v].angle, views[v].shrink, v))) return rc;
+    AlignArgs a;
+    if (align && (rc = check_align(h, who, align, n, dev_crops, 0, a))) return rc;
+    if (n == 0) return RF_OK;
+    std::vector<RotatedGeometry> geo((size_t)n * nviews);
+    for (int i = 0; i < n; i++)
+        for (int v = 0; v < nviews; v++) geo[(size_t)i * nviews + v] = view_geometry(h, views[v], source.width(i), source.height(i));
+    std::vector<float> scales(geo.size());
+    a.crops = dev_crops;
+    a.mats = dev_mats;
+    try {
+        device_issue(h, h->rotated_slots, h->next_rotated_slot, source, n, RotatedJobs<Source>{h, source, views, nviews, geo, scales.data()},
+                     thr, nms, align ? &a : nullptr, dev_dets, dev_counts, nullptr);
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    if (out_view_scales) std::copy(scales.begin(), scales.end(), out_view_scales);
+    if (out_view_mats)
+        for (size_t k = 0; k < geo.size(); k++) put_view_mat(geo[k], out_view_mats + k * 6);
+    return RF_OK;
+}
+}  // extern "C++"
+
+int rf_detect_views_rotated_device(rf_handle h, const uint8_t *const *dev_bgr, const int *widths, const int *heights, const int *row_strides,
+                                   int n, const rf_rotated_view *views, int nviews, float thr, float nms, const rf_align_params *align,
+                                   void *dev_crops, double *dev_mats, const rf_det **dev_dets, const int32_t **dev_counts, float *out_view_scales,
+                                   double *out_view_mats) {
+    return detect_rotated_device(h, "rf_detect_views_rotated_device", BgrImages{dev_bgr, widths, heights, row_strides, nullptr, false}, n,
+                                 views, nviews, thr, nms, align, dev_crops, dev_mats, dev_dets, dev_counts, out_view_scales, out_view_mats);
+}
+
+int rf_detect_yuv_views_rotated_device(rf_handle h, const rf_yuv_frame *frames, int n, int matrix, const rf_rotated_view *views, int nviews,
+                                       float thr, float nms, const rf_align_params *align, void *dev_crops, double *dev_mats,
+                                       const rf_det **dev_dets, const int32_t **dev_counts, float *out_view_scales, double *out_view_mats) {
+    return detect_rotated_device(h, "rf_detect_yuv_views_rotated_device", YuvFrames{frames, matrix, nullptr, false}, n, views, nviews, thr,
+                                 nms, align, dev_crops, dev_mats, dev_dets, dev_counts, out_view_scales, out_view_mats);
+}
+
+int rf_preprocess_yuv_rotated(rf_handle h, const rf_yuv_frame *frame, int matrix, float angle, float shrink, uint8_t *out, double *out_mat) {
+    return preprocess_rotated(h, "rf_preprocess_yuv_rotated", YuvFrames{frame, matrix, nullptr, false}, angle, shrink, out, out_mat);
+}
+
+int rf_fetch_dets(rf_handle h, const rf_det *dev_dets, const int32_t *dev_counts, int n, rf_face *out_faces, int *out_counts,
+                  int32_t *out_anchor_index) {
+    int rc = check_n(h, n);
+    if (rc || n == 0) return rc;
+    if (!dev_dets || !dev_counts || !out_faces || !out_counts) return fail(h, RF_ERR_INVALID_ARG, "rf_fetch_dets: NULL records or outputs");
+    try {
+        CK(cudaSetDevice(h->device));
+        for (Ctx &c : h->ctx) CK(cudaStreamSynchronize(c.stream));
+        PostBuffers pb{};
+        pb.out_dets = const_cast<rf_det *>(dev_dets);
+        pb.out_counts = const_cast<int32_t *>(dev_counts);
+        fetch_post(h, pb, h->ctx[0].stream, n, out_faces, out_counts, out_anchor_index);
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     return RF_OK;
 }

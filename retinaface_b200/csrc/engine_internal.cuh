@@ -172,6 +172,10 @@ struct rf_handle_s {
     };
     std::vector<TiledSlot> tiled_slots;
     unsigned next_tiled_slot = 0;
+    // rf_detect_views_rotated_device / rf_detect_yuv_views_rotated_device (f24): a ring of their own, so that tiled records keep
+    // their validity rule across rotated calls
+    std::vector<TiledSlot> rotated_slots;
+    unsigned next_rotated_slot = 0;
     uint8_t *d_raw = nullptr;         // one raw caller image (max_image) for the letterbox kernel
     uint8_t *h_raw = nullptr;         // pinned, TWO buffers of raw_bytes: staging of pageable caller images (upload_plane)
     size_t raw_bytes = 0;

@@ -245,7 +245,7 @@ __global__ void __launch_bounds__(256) k_merge(PostBuffers src, const __grid_con
     }
 }
 
-// f23: one launch merges every warp view of a batch (postproc.cuh RotatedSource)
+// f23: one launch merges up to RF_MAX_VIEWS_DEV warp views (postproc.cuh RotatedSource)
 struct RotatedSet {
     RotatedSource src[RF_MAX_VIEWS_DEV];
 };
@@ -275,7 +275,7 @@ __global__ void __launch_bounds__(256) k_merge_rotated(PostBuffers src, const __
             d.face.ly[k] = (float)affine_row(im[3], im[4], im[5], (double)f.lx[k], (double)f.ly[k]);
         }
         d.anchor_index = m.id_base + j;
-        append_candidate(dst, 0, d);
+        append_candidate(dst, m.image, d);
     }
 }
 
@@ -381,12 +381,15 @@ cudaError_t launch_merge(const PostBuffers &src, const MergeSource *src_desc, in
 }
 
 cudaError_t launch_merge_rotated(const PostBuffers &src, const RotatedSource *src_desc, int n, const PostBuffers &dst, cudaStream_t s) {
-    if (n <= 0) return cudaSuccess;
-    if (n > RF_MAX_VIEWS_DEV) return cudaErrorInvalidValue;
-    RotatedSet rs{};
-    for (int i = 0; i < n; i++) rs.src[i] = src_desc[i];
-    k_merge_rotated<<<n, 256, 0, s>>>(src, rs, dst);
-    return cudaGetLastError();
+    for (int i0 = 0; i0 < n; i0 += RF_MAX_VIEWS_DEV) {
+        const int m = std::min(RF_MAX_VIEWS_DEV, n - i0);
+        RotatedSet rs{};
+        for (int i = 0; i < m; i++) rs.src[i] = src_desc[i0 + i];
+        k_merge_rotated<<<m, 256, 0, s>>>(src, rs, dst);
+        cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
 }
 
 cudaError_t postproc_init() {

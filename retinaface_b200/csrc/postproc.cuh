@@ -87,9 +87,10 @@ cudaError_t launch_merge(const PostBuffers &src, const MergeSource *src_desc, in
                          cudaStream_t s);
 // f23 warp views (rf_b200.h rf_rotated_view): batch slot `slot`'s kept faces mapped back through iM in FP64 -- the box centre through
 // iM, half sizes (x2 - x1) * half_inv and (y2 - y1) * half_inv (half_inv = 1 / (2 f)), each corner and landmark rounded to float once
-// -- and appended to image 0 of dst with candidate id id_base + rank.  A table of its own, so that MergeSource keeps its size.
+// -- and appended to image `image` of dst with candidate id id_base + rank.  A table of its own, so that MergeSource keeps its size.
+// One launch per RF_MAX_VIEWS_DEV sources (none for n = 0).
 struct RotatedSource {
-    int slot, id_base;
+    int slot, id_base, image;
     double im[6];
     double half_inv;
 };

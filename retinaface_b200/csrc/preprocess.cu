@@ -434,6 +434,8 @@ constexpr int WARP_THREADS = 128, WARP_BAND = 2, WARP_SPAN = WARP_THREADS * 4;
 template <typename Src>
 struct WarpBatch { WarpItemT<Src> v[WARP_MAX_VIEWS]; };
 static_assert(sizeof(WarpBatch<BgrRows>) + 8 <= 4096, "warp launch exceeds the classic 4 KB kernel parameter space");
+static_assert(sizeof(WarpItemT<YuvPlanes>) == 104 && sizeof(WarpBatch<YuvPlanes>) + 8 <= 4096,
+              "YUV warp launch exceeds the classic 4 KB kernel parameter space");
 
 // [lo, hi] of the x with a x + b in [-2, n + 1]: the fixed-point source coordinate is within 1/16 pixel of a x + b, and a pixel has a
 // tap in [0, n) only if that coordinate is in [-1, n), so the bound keeps a pixel of margin
@@ -504,14 +506,18 @@ __global__ void __launch_bounds__(WARP_THREADS) k_letterbox_warp(const __grid_co
 
 template <typename Src>
 cudaError_t launch_letterbox_warp(const WarpItemT<Src> *items, int n, int net_w, int net_h, cudaStream_t s) {
-    if (n <= 0) return cudaSuccess;
-    if (n > WARP_MAX_VIEWS) return cudaErrorInvalidValue;
-    WarpBatch<Src> B{};
-    for (int i = 0; i < n; i++) B.v[i] = items[i];
-    k_letterbox_warp<Src><<<dim3((net_w + WARP_SPAN - 1) / WARP_SPAN, (net_h + WARP_BAND - 1) / WARP_BAND, n), WARP_THREADS, 0, s>>>(B, net_w, net_h);
-    return cudaGetLastError();
+    for (int i0 = 0; i0 < n; i0 += WARP_MAX_VIEWS) {
+        const int m = std::min(WARP_MAX_VIEWS, n - i0);
+        WarpBatch<Src> B{};
+        for (int i = 0; i < m; i++) B.v[i] = items[i0 + i];
+        k_letterbox_warp<Src><<<dim3((net_w + WARP_SPAN - 1) / WARP_SPAN, (net_h + WARP_BAND - 1) / WARP_BAND, m), WARP_THREADS, 0, s>>>(B, net_w, net_h);
+        cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
 }
 template cudaError_t launch_letterbox_warp<BgrRows>(const WarpItem *, int, int, int, cudaStream_t);
+template cudaError_t launch_letterbox_warp<YuvPlanes>(const WarpYuvItem *, int, int, int, cudaStream_t);
 
 template float letterbox_fill<BgrRows>(LbItem &, BgrRows, int, int, uint8_t *, int, int, int, int);
 template float letterbox_fill<YuvPlanes>(LbYuvItem &, YuvPlanes, int, int, uint8_t *, int, int, int, int);

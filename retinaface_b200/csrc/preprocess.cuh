@@ -112,8 +112,9 @@ struct WarpItemT {
     double im[6];
 };
 using WarpItem = WarpItemT<BgrRows>;
-constexpr int WARP_MAX_VIEWS = 16;     // RF_MAX_VIEWS: every warp view of a batch in one launch
-// k_letterbox_warp: n <= WARP_MAX_VIEWS items, one launch (none for n = 0)
+using WarpYuvItem = WarpItemT<YuvPlanes>;     // f24: each tap converted as the letter-box converts it
+constexpr int WARP_MAX_VIEWS = 16;     // items of one k_letterbox_warp launch
+// k_letterbox_warp: one launch per WARP_MAX_VIEWS items (none for n = 0)
 template <typename Src>
 cudaError_t launch_letterbox_warp(const WarpItemT<Src> *items, int n, int net_w, int net_h, cudaStream_t s);
 

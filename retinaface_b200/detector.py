@@ -29,6 +29,19 @@ class FaceDetectInfo:  # RetinaFace.h:37-42
         return FaceDetectInfo(float(r[0]), tuple(map(float, r[1:5])), tuple(map(float, r[5:10])), tuple(map(float, r[10:15])))
 
 
+def angle_sweep(step: float) -> list:
+    """The rotated views of ``detectAnyAngle`` and ``detectAnyAngleFrames``: (angle, shrink 1) for the angles 0, step, 2 step ... below
+    360 degrees.  A step that is not positive, or one that makes more than RF_MAX_VIEWS = 16 views, is a ValueError."""
+    if not step > 0:
+        raise ValueError(f"step {step}: must be positive")
+    angles = [0.0]
+    while len(angles) <= 16 and len(angles) * float(step) < 360.0:
+        angles.append(len(angles) * float(step))
+    if len(angles) > 16:
+        raise ValueError(f"step {step} makes more than RF_MAX_VIEWS = 16 views")
+    return [(a, 1.0) for a in angles]
+
+
 class RetinaFace:
     MODEL_FILE = "mnet-deconv-0517.caffemodel"  # the file the reference always loads, RetinaFace.cpp:276
 
@@ -130,19 +143,26 @@ class RetinaFace:
         into the network input (rf_detect_views_rotated; quarter turns take detectAnyOrientation's views), merged on the GPU.  Faces in
         image pixels, axis-aligned boxes, landmarks carrying each face's roll.  With ``align`` (``Engine.detect_align``'s keywords), a list
         of ``(FaceDetectInfo, crop)``, the crops upright.  More than 16 views (RF_MAX_VIEWS) is a ValueError."""
-        if not step > 0:
-            raise ValueError(f"step {step}: must be positive")
-        angles = [0.0]
-        while len(angles) <= 16 and len(angles) * float(step) < 360.0:
-            angles.append(len(angles) * float(step))
-        if len(angles) > 16:
-            raise ValueError(f"step {step} makes more than RF_MAX_VIEWS = 16 views")
+        views = angle_sweep(step)
         if img is None or img.size == 0:
             return []
-        out = self.engine.detect_views_rotated(img, [(a, 1.0) for a in angles], threshold, self.nms_threshold, align=align)
+        out = self.engine.detect_views_rotated(img, views, threshold, self.nms_threshold, align=align)
         if align is None:
             return [FaceDetectInfo.from_row(r) for r in out[0]]
         return [(FaceDetectInfo.from_row(r), c) for r, c in zip(out[0], out[4])]
+
+    def detectAnyAngleFrames(self, device_frames: Sequence, threshold: float = 0.5, step: float = 30.0, layout: str = "nv12",
+                             matrix: str = "bt601") -> List[List[FaceDetectInfo]]:
+        """f24 faces at any in-plane angle in video: ``detectAnyAngle``'s sweep on device 4:2:0 frames (torch CUDA tensors in
+        ``Engine.detect_yuv_device``'s forms, at most max_batch), all frames in one asynchronous call
+        (rf_detect_yuv_views_rotated_device).  Per frame, the faces in FRAME pixels.  More than 16 views is a ValueError."""
+        views = angle_sweep(step)
+        frames = list(device_frames)
+        if not frames:
+            return []
+        d, c, _, _ = self.engine.detect_yuv_views_rotated_device(frames, views, threshold, self.nms_threshold, layout=layout, matrix=matrix)
+        faces, _ = self.engine.read_dets(d, c, len(frames))
+        return [[FaceDetectInfo.from_row(r) for r in per] for per in faces]
 
     def setVideoOrientation(self, video: int, orientation: int):
         """f20 oriented video (rf_tracker_set_orientation): ``video`` (-1: every video) is shown in EXIF orientation 1..8 -- portrait

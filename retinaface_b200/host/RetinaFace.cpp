@@ -297,13 +297,18 @@ vector<FaceDetectInfo> RetinaFace::detectAnyOrientation(const Mat &img, float th
     return out;
 }
 
-vector<FaceDetectInfo> RetinaFace::detectAnyAngle(const Mat &img, float threshold, float step_deg, const AlignOptions *align) {
-    if (!(step_deg > 0.f)) throw std::invalid_argument("detectAnyAngle: step_deg must be positive");
+vector<rf_rotated_view> RetinaFace::angleSweep(const char *who, float step_deg) {
+    if (!(step_deg > 0.f)) throw std::invalid_argument(string(who) + ": step_deg must be positive");
     vector<rf_rotated_view> views;
     for (int k = 0; k * step_deg < 360.f; k++) {
-        if (views.size() == RF_MAX_VIEWS) throw std::invalid_argument("detectAnyAngle: more than RF_MAX_VIEWS views");
+        if (views.size() == RF_MAX_VIEWS) throw std::invalid_argument(string(who) + ": more than RF_MAX_VIEWS views");
         views.push_back(rf_rotated_view{k * step_deg, 1.f});
     }
+    return views;
+}
+
+vector<FaceDetectInfo> RetinaFace::detectAnyAngle(const Mat &img, float threshold, float step_deg, const AlignOptions *align) {
+    const vector<rf_rotated_view> views = angleSweep("detectAnyAngle", step_deg);
     last_.assign(1, vector<FaceDetectInfo>());
     scales_.assign(1, 1.f);
     crops_.assign(1, vector<Mat>());
@@ -319,6 +324,24 @@ vector<FaceDetectInfo> RetinaFace::detectAnyAngle(const Mat &img, float threshol
     out_counts_[0] = count;
     keepResults(0, 1, align ? crops.data() : nullptr, per, cw, ch);
     return last_[0];
+}
+
+void RetinaFace::detectAnyAngleYUV(const vector<rf_yuv_frame> &device_frames, float threshold, float step_deg) {
+    const vector<rf_rotated_view> views = angleSweep("detectAnyAngleYUV", step_deg);
+    const int n = (int)device_frames.size();
+    if (n > opt_.max_batch) throw std::invalid_argument("detectAnyAngleYUV: at most max_batch frames per call");
+    last_.assign(n, vector<FaceDetectInfo>());
+    scales_.assign(n, 1.f);
+    crops_.assign(n, vector<Mat>());
+    if (n == 0) return;
+    const rf_det *dets = nullptr;
+    const int32_t *counts = nullptr;
+    int rc = rf_detect_yuv_views_rotated_device(h_, device_frames.data(), n, RF_YUV_BT601, views.data(), (int)views.size(), threshold,
+                                                nms_threshold, nullptr, nullptr, nullptr, &dets, &counts, nullptr, nullptr);
+    if (rc != RF_OK) throw std::runtime_error(string("rf_detect_yuv_views_rotated_device: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+    rc = rf_fetch_dets(h_, dets, counts, n, out_faces_.data(), out_counts_.data(), nullptr);
+    if (rc != RF_OK) throw std::runtime_error(string("rf_fetch_dets: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+    keepResults(0, n, nullptr, 0, 0, 0);
 }
 
 void RetinaFace::trackYUV(const vector<rf_yuv_frame> &device_frames, const vector<int> &videos, float threshold, const AlignOptions *align,

@@ -148,6 +148,13 @@ class RetinaFace {
     // face's roll.  With `align`, lastCrops()[0] holds the upright crops of the first min(faces, max_faces) faces (lastBatchFaces() and
     // lastCrops() hold the one image).
     vector<FaceDetectInfo> detectAnyAngle(const Mat &img, float threshold = 0.5, float step_deg = 30, const AlignOptions *align = nullptr);
+    // f24 faces at any in-plane angle in video (rf_detect_yuv_views_rotated_device, BT.601): detectAnyAngle's sweep on DEVICE 4:2:0
+    // frames (descriptors of device planes, e.g. NVDEC surfaces; at most max_batch), all frames in one call.  Blocking: afterwards
+    // lastBatchFaces()[i] holds frame i's faces in FRAME pixels (lastScale() is 1).
+    void detectAnyAngleYUV(const vector<rf_yuv_frame> &device_frames, float threshold = 0.5, float step_deg = 30);
+    // The views detectAnyAngle and detectAnyAngleYUV sweep: (0, 1), (step_deg, 1), (2 step_deg, 1) ... below 360 degrees; a step_deg
+    // that is not positive, or that makes more than RF_MAX_VIEWS views, throws std::invalid_argument naming `who`.
+    static vector<rf_rotated_view> angleSweep(const char *who, float step_deg);
     // f10 tracking (rf_detect_yuv_track_device): DEVICE 4:2:0 frames (descriptors of device planes, e.g. NVDEC surfaces; at most
     // max_batch per call), frame i of video videos[i] in [0, track_videos), detected and associated with the tracks of earlier frames
     // on the GPU.  Asynchronous on rf_last_stream(handle()).  Afterwards lastTracks() holds the device track lists; with `align`, the

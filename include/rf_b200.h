@@ -1243,7 +1243,9 @@ int rf_calibrate_int8(rf_handle h, const uint8_t *bgr_net_sized, int n_images, c
 double rf_kl_threshold_bins(const unsigned *hist, int bins, int levels);
 
 /* Host-only (works without a GPU): the layer plan rf_create would build for `cfg`, one text line per kernel launch of a
- * forward plus the geometry / shared-memory budget of every persistent tile chain.  Returns the launch count. */
+ * forward plus the geometry / shared-memory budget of every persistent tile chain.  A launch's line is "step lane <lane>:
+ * <name>", followed for a tiled launch by " | " and its tile geometry as space-separated key=value words.  Returns the launch
+ * count. */
 int rf_plan_describe(const rf_config *cfg, char *out, int cap);
 
 /* Debug / parity aids (not part of the drop-in surface): fetch a materialised activation by its

@@ -446,9 +446,11 @@ def model_inspect(caffemodel: str, layer: str):
 
 
 def plan_describe(caffemodel: str, net_h: int, net_w: int, precision: int = RF_PREC_FP16, max_batch: int = 8, flags: int = 0,
-                  int8_table: Optional[str] = None, streams: int = 0, max_faces: int = 0) -> str:
+                  int8_table: Optional[str] = None, streams: int = 0, max_faces: int = 0, geometry: bool = False) -> str:
     """The layer plan rf_create would build (host-only entry point: no GPU needed).  `max_faces` as in Engine (0 -> 256): the tile
-    chains reserve shared memory for the last-block NMS's kept list, so the plan depends on it."""
+    chains reserve shared memory for the last-block NMS's kept list, so the plan depends on it.  Each launch is a line
+    "step lane <lane>: <name>"; with `geometry`, a tiled launch's line goes on with " | " and its tile geometry (key=value
+    words)."""
     lib = load_library()
     cfg = _Config(caffemodel.encode(), int8_table.encode() if int8_table else None, precision, net_w, net_h, max_batch, max_faces, 0, 0, 0,
                   flags, streams, None, None, None)
@@ -456,7 +458,10 @@ def plan_describe(caffemodel: str, net_h: int, net_w: int, precision: int = RF_P
     rc = lib.rf_plan_describe(C.byref(cfg), buf, len(buf))
     if rc < 0:
         raise RfError(rc, (lib.rf_last_error(None) or b"").decode())
-    return buf.value.decode()
+    text = buf.value.decode()
+    if geometry:
+        return text
+    return "".join(ln.split(" | ", 1)[0] + "\n" if ln.startswith("step lane ") else ln + "\n" for ln in text.splitlines())
 
 
 def model_load(caffemodel: str, prototxt: Optional[str] = None, cache: Optional[str] = None, layer: Optional[str] = None):

@@ -2053,7 +2053,8 @@ int rf_model_inspect(const char *caffemodel_path, const char *layer, float *w, i
 }
 
 // Host-only (works without a GPU): builds the layer plan rf_create would build for `cfg` and writes one line per kernel
-// launch of a forward (and, for tile chains, their geometry and shared-memory budget) into `out`.
+// launch of a forward, "step lane <lane>: <name>" and, where the launch is tiled, " | " and its tile geometry (and, for tile
+// chains, their geometry and shared-memory budget) into `out`.
 int rf_plan_describe(const rf_config *cfg, char *out, int cap) {
     if (!cfg || !cfg->caffemodel_path || !out || cap <= 0) return fail(nullptr, RF_ERR_INVALID_ARG, "rf_plan_describe: bad arguments");
     if (cfg->net_w <= 0 || cfg->net_h <= 0 || cfg->net_w % 32 || cfg->net_h % 32 || cfg->max_batch <= 0)
@@ -2074,7 +2075,7 @@ int rf_plan_describe(const rf_config *cfg, char *out, int cap) {
     } catch (const CudaFail &f) { return fail_cuda(nullptr, f); }
     catch (const PlanFail &f) { return fail(nullptr, f.status, f.msg); }
     std::string text = fmt("%d launches per forward, activation arena %zu bytes per batch of %d\n", (int)h->steps.size(), h->arena_bytes, cfg->max_batch);
-    for (auto &st : h->steps) text += fmt("step lane %d: %s\n", st.lane, st.name.c_str());
+    for (auto &st : h->steps) text += fmt("step lane %d: %s%s%s\n", st.lane, st.name.c_str(), st.geom.empty() ? "" : " | ", st.geom.c_str());
     text += describe_chains(h);
     snprintf(out, (size_t)cap, "%s", text.c_str());
     return (int)h->steps.size();

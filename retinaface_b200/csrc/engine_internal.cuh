@@ -105,6 +105,7 @@ struct Step {
     int lane = 0;                 // 0 = main stream; 1, 2 = side branches of the forward graph
     std::vector<int> deps;        // producer steps in OTHER lanes this step must wait for (filled by link_steps)
     bool signals = false;         // some step in another lane waits for this one
+    std::string geom;             // the tiles its launch arguments fix, "key=value ..." (rf_plan_describe; empty: none)
 };
 
 }  // namespace rf_eng

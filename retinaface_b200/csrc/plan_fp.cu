@@ -31,11 +31,15 @@ std::vector<float> pack_gemm(const std::vector<const FoldedConv *> &cs, std::vec
     return w;
 }
 
+// k_conv_gemm's N tile: the widest of 64, 32, 16 that divides N.  M tiles: 64 positions of the n x H x W map.
+static int gemm_bn(int N) { return (N % 64 == 0) ? 64 : (N % 32 == 0 ? 32 : 16); }
+static std::string gemm_geom(int N, int H, int W) { return fmt("BM=64 bn=%d H=%d W=%d", gemm_bn(N), H, W); }
+
 template <typename T>
 void launch_gemm(const T *in, int ldin, int cin, const float *wk, const float *bias, int N, int ks, OutSplit<T> outs,
                  int n, int H, int W, cudaStream_t s) {
     long M = (long)n * H * W;
-    int bn = (N % 64 == 0) ? 64 : (N % 32 == 0 ? 32 : 16);
+    int bn = gemm_bn(N);
     dim3 grid((unsigned)((M + 63) / 64), (N + bn - 1) / bn);
 #define RF_GEMM(BN_, KS_) CK_L(k_conv_gemm<T, BN_, KS_>, grid, dim3(256), 0, s, in, ldin, cin, wk, bias, N, outs, n, H, W)
     if (ks == 1) { if (bn == 64) RF_GEMM(64, 1); else if (bn == 32) RF_GEMM(32, 1); else RF_GEMM(16, 1); }
@@ -209,7 +213,12 @@ int plan_pair_tc(Builder &B, const PairNode &p, int tin) {
         if (h->cfg.streams != 1) resident = std::min(resident, h->num_sms);
         if (!tc_dw2d_out_fits(g2)) tw = 0;      // the output tile does not fit a consumed window: the 1-D kernel
     }
-    if (tw) s.name = fmt("tc2d_dw%d+pw%d_s%d_%dto%d", i, i + 1, S, C, N);
+    if (tw) {
+        s.name = fmt("tc2d_dw%d+pw%d_s%d_%dto%d", i, i + 1, S, C, N);
+        s.geom = fmt("TH=%d TW=%d OH=%d OW=%d tiles_x=%d tiles_y=%d stages=%d", g2.TH, g2.TW, oh, ow_, g2.tiles_x, g2.tiles_y, g2.stages);
+    } else {
+        s.geom = fmt("rows=%d nsplit=%d Rmax=%d OH=%d OW=%d", geo.rows, geo.nsplit, geo.Rmax, oh, ow_);
+    }
     s.launch = [=](const Run &r) {
         if (tw) {
             TcDw2dArgs a = g2;
@@ -257,6 +266,8 @@ void plan_conv_tc(Builder &B, const ConvNode &c) {
     if (o1.t >= 0) s.out.push_back(o1.t);
     s.flops_per_img = 2.0 * ih * iw * cin * ks * ks * N + (tup >= 0 ? 2.0 * ih * iw * cin * 4 : 0.0);
     s.bytes_per_img = ((double)ih * iw * cin + (double)ih * iw * N + (tup >= 0 ? (double)(ih / 2) * (iw / 2) * cin : 0.0)) * es;
+    s.geom = fmt("NT=%d BM=128 H=%d W=%d Hp=%d Wp=%d merge=%s", tc_n_bucket(N), ih, iw, ks == 3 ? ih + 1 : ih, ks == 3 ? iw + 2 : iw,
+                 tup >= 0 ? "fused" : "none");
     s.launch = [=](const Run &r) {
         TcConvArgs a{};
         a.in = T_(r, tin); a.Cin = cin; a.nimg = r.n; a.H = ih; a.W = iw; a.taps = ks * ks; a.N = N;
@@ -360,6 +371,7 @@ int plan_stem_fused(Builder &B, const StemNode &n, const char *suffix, float out
     s.flops_per_img = 2.0 * cur_h * cur_w * (8 * 27 + 8 * 9 + 8 * 16);
     s.bytes_per_img = (double)H * W * 3 + (double)cur_h * cur_w * 16 * es;
     const int tiles = ((H / 2 + 15) / 16) * ((W / 2 + 15) / 16);
+    s.geom = fmt("TH=16 TW=16 OH=%d OW=%d tiles_x=%d tiles_y=%d", cur_h, cur_w, (cur_w + 15) / 16, (cur_h + 15) / 16);
     const int resident = simt_stem ? 0 : resident_ctas(h, (const void *)k_stem_tc<OutT>, 256, 0);
     s.launch = [=](const Run &r) {
         if (simt_stem) {
@@ -432,6 +444,7 @@ struct SimtOps : PlanOps {
         s2.in = {tdw}; s2.out = {tpw};
         s2.flops_per_img = 2.0 * oh * ow_ * C * N;
         s2.bytes_per_img = ((double)oh * ow_ * C + (double)oh * ow_ * N) * es;
+        s2.geom = gemm_geom(N, oh, ow_);
         s2.launch = [=](const Run &r) {
             OutSplit<T> o{t(h, r, tpw), N, N, 1, nullptr, 0, 0};
             launch_gemm<T>(t(h, r, tdw), C, C, h->d_weights + owp, h->d_weights + obp, N, 1, o, r.n, oh, ow_, r.stream);
@@ -455,6 +468,7 @@ struct SimtOps : PlanOps {
         if (o1.t >= 0) s.out.push_back(o1.t);
         s.flops_per_img = 2.0 * ih * iw * cin * ks * ks * N;
         s.bytes_per_img = ((double)ih * iw * cin + (double)ih * iw * N) * h->elem;
+        s.geom = gemm_geom(N, ih, iw);
         s.launch = [=](const Run &r) {
             OutSplit<T> o{t(h, r, o0.t) + o0.off, o0.ld, o0.n, o0.relu, o1.t >= 0 ? t(h, r, o1.t) + o1.off : nullptr, o1.ld, o1.relu};
             launch_gemm<T>(t(h, r, tin), ldin, cin, h->d_weights + ow, h->d_weights + ob, N, ks, o, r.n, ih, iw, r.stream);

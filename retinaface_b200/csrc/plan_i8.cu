@@ -139,7 +139,15 @@ struct I8Ops : PlanOps {
         s.flops_per_img = 2.0 * oh * ow_ * C * 9 + 2.0 * oh * ow_ * C * N;
         s.bytes_per_img = (double)ih * iw * C + (double)oh * ow_ * N;
         const int tw = dw2d_tile_w(h, C, oh, ow_, geo.nsplit);
-        if (tw) s.name = fmt("i8_2d_dw%d+pw%d_s%d_%dto%d", i, i + 1, S, C, N);
+        if (tw) {
+            s.name = fmt("i8_2d_dw%d+pw%d_s%d_%dto%d", i, i + 1, S, C, N);
+            TcDw2dArgsI8 g{};
+            g.OH = oh; g.OW = ow_; g.S = S; g.TH = 8; g.TW = tw;
+            tc_dw2d_i8_finish(g);
+            s.geom = fmt("TH=%d TW=%d OH=%d OW=%d tiles_x=%d tiles_y=%d", g.TH, g.TW, oh, ow_, g.tiles_x, g.tiles_y);
+        } else {
+            s.geom = fmt("rows=%d nsplit=%d Rmax=%d OH=%d OW=%d", geo.rows, geo.nsplit, geo.Rmax, oh, ow_);
+        }
         s.launch = [=](const Run &r) {
             if (tw) {
                 TcDw2dArgsI8 a{};
@@ -194,6 +202,8 @@ struct I8Ops : PlanOps {
         if (o1.t >= 0) s.out.push_back(o1.t);
         s.flops_per_img = 2.0 * ih * iw * cin * ks * ks * N;
         s.bytes_per_img = (double)ih * iw * cin + (double)ih * iw * N + (tup >= 0 ? (double)(ih / 2) * (iw / 2) * cin : 0.0);
+        s.geom = fmt("NT=%d BM=128 H=%d W=%d Hp=%d Wp=%d merge=%s", tc_n_bucket(N), ih, iw, ks == 3 ? ih + 1 : ih, ks == 3 ? iw + 2 : iw,
+                     tup >= 0 ? "fused" : "none");
         s.launch = [=](const Run &r) {
             TcConvArgsI8 a{};
             a.in = q(h, r, tin); a.Cin = cin; a.nimg = r.n; a.H = ih; a.W = iw; a.taps = ks * ks; a.N = N;

@@ -371,6 +371,7 @@ void add_chain_step(Builder &B, std::shared_ptr<TileChain> c, int lane, double b
     for (auto &ls : c->stages) fl += ls.flops * c->W * c->H;
     s.flops_per_img = fl;
     s.bytes_per_img = bytes_per_img;
+    s.geom = fmt("TH=%d H=%d W=%d tiles_per_img=%d weights=%s", c->TH, c->H, c->W, c->args.tiles_per_img, c->args.resident ? "resident" : "streamed");
     s.launch = [h, c](const Run &r) { launch_chain(h, c, r); };
     B.step(std::move(s));
 }

@@ -100,12 +100,11 @@ def _fetcher(eng, n):
     return fetch
 
 
-def check_case(case_id, eng, batch, steps, post, label, options):
+def check_case(case, eng, batch, steps, post, label, options):
     """Every step of one forward inside its interval; returns the per-tensor report lines and the engine's heads."""
     n = len(batch)
     heads = eng.forward_heads(batch)
     compared, missing, diffs, report = [], [], [], []
-    case = CASES[case_id]
     chain_heads, inner = options
     for name, step, iv, got in steps.walk(batch, _fetcher(eng, n), simt_stem=bool(case.flags & RF_FLAG_SIMT_STEM),
                                           chain_heads=chain_heads):
@@ -159,7 +158,7 @@ def test_fp16_engine_inside_its_rounding_intervals(case_id, golden_image, post_o
             label = f"{case_id} n={n}"
             t0 = time.perf_counter()
             batch = mixed_batch(golden_image, n, h, w, start=3 * run)
-            report, compared, heads, found = check_case(case_id, keep, batch, steps, post_oracle, label, options)
+            report, compared, heads, found = check_case(case, keep, batch, steps, post_oracle, label, options)
             merges = ", ".join(f"_plus{k} {'stand-alone' if f'_plus{k}' in compared else 'fused'}" for k in (0, 1))
             print(f"\n{label}: {len(compared)} tensors inside their intervals ({merges}), {found} faces, "
                   f"{time.perf_counter() - t0:.1f} s")

@@ -132,6 +132,41 @@ def post_oracle():
     return PostprocOracle()
 
 
+def check_forward(keep, oracle, batch, post, label):
+    """One forward of `batch` on the keep-all handle against the integer oracle: the FP32 stem within 1 LSB, every
+    materialised int8 tensor bit-identical (continued from the engine's own stem), the heads within 1e-4 and the detections
+    equal to the oracle post-process of the engine's own heads.  Returns (heads, oracle tensors, tensors compared, faces)."""
+    from retinaface_b200 import RfError
+    n = len(batch)
+    heads = keep.forward_heads(batch)
+    # FP32 stem: within 1 LSB of the oracle's quantised stem (summation order), on fewer than 1e-3 of the elements
+    stem = keep.debug_tensor(STEM, n)
+    d = np.abs(stem - oracle.stem(batch)[0])
+    assert d.max() <= 1 and (d > 0).mean() < 1e-3, (label, d.max(), (d > 0).mean())
+    # the integer part, continued from the engine's own stem: every materialised int8 tensor bit-identical
+    o_heads, o_t = oracle.forward(batch, want_tensors=True, q_stem=stem)
+    compared, missing, diffs = [], [], []
+    for name, (q, _) in o_t.items():
+        if name == STEM:
+            continue
+        try:
+            got = keep.debug_tensor(name, n)
+        except RfError:
+            missing.append(name)
+            continue
+        compared.append(name)
+        if not np.array_equal(got, q):
+            diffs.append(first_difference(name, got, q))
+    assert not diffs, (label, diffs)
+    # only the FPN sums may be left unmaterialised (fused into the aggr conv's staging)
+    assert set(missing) <= {"_plus0", "_plus1"}, (label, missing)
+    assert len(compared) >= 26, (label, compared)
+    for k in range(9):
+        assert np.abs(heads[k] - o_heads[k]).max() < 1e-4, (label, k, np.abs(heads[k] - o_heads[k]).max())
+    found = post.check_engine(keep, batch, heads, THR, NMS, label)
+    return heads, o_t, compared, found
+
+
 @pytest.mark.gpu
 @pytest.mark.parametrize("case_id", list(CASES))
 def test_int8_engine_bit_exact_vs_integer_oracle(case_id, golden_image, tables, post_oracle):
@@ -142,44 +177,18 @@ def test_int8_engine_bit_exact_vs_integer_oracle(case_id, golden_image, tables, 
     oracle = Int8Oracle(caffemodel(case.model), table)
     keep = _engine(case, table, keep_all=True)
     prod = _engine(case, table, keep_all=False) if case.placement else None
-    from retinaface_b200 import RfError
     try:
         for run, n in enumerate(case.runs):
             label = f"{case_id} n={n}"
             t0 = time.perf_counter()
             batch = mixed_batch(golden_image, n, h, w, start=3 * run)
-            heads = keep.forward_heads(batch)
-            # FP32 stem: within 1 LSB of the oracle's quantised stem (summation order), on fewer than 1e-3 of the elements
-            stem = keep.debug_tensor(STEM, n)
-            d = np.abs(stem - oracle.stem(batch)[0])
-            assert d.max() <= 1 and (d > 0).mean() < 1e-3, (label, d.max(), (d > 0).mean())
-            # the integer part, continued from the engine's own stem: every materialised int8 tensor bit-identical
-            o_heads, o_t = oracle.forward(batch, want_tensors=True, q_stem=stem)
-            compared, missing, diffs = [], [], []
-            for name, (q, _) in o_t.items():
-                if name == STEM:
-                    continue
-                try:
-                    got = keep.debug_tensor(name, n)
-                except RfError:
-                    missing.append(name)
-                    continue
-                compared.append(name)
-                if not np.array_equal(got, q):
-                    diffs.append(first_difference(name, got, q))
-            assert not diffs, (label, diffs)
-            # only the FPN sums may be left unmaterialised (fused into the aggr conv's staging)
-            assert set(missing) <= {"_plus0", "_plus1"}, (label, missing)
-            assert len(compared) >= 26, (label, compared)
+            heads, o_t, compared, found = check_forward(keep, oracle, batch, post_oracle, label)
             _MERGE[case_id] = "stand-alone" if "_plus1" in compared else "fused"
             if case.table == "saturating":
                 frac = {name: float((q == 127).mean()) for name, (q, _) in o_t.items()}
                 for name, floor in SATURATION_FLOOR.items():
                     assert frac[name] >= floor, (label, name, frac[name])
                 assert sum(f > 0 for f in frac.values()) >= SATURATED_TENSORS, (label, frac)
-            for k in range(9):
-                assert np.abs(heads[k] - o_heads[k]).max() < 1e-4, (label, k, np.abs(heads[k] - o_heads[k]).max())
-            found = post_oracle.check_engine(keep, batch, heads, THR, NMS, label)
             assert found > 0 or not case.faces, label       # the selection and order compared are not empty
             if prod is not None:
                 # production placement: tensors share memory across the three lanes; heads bit-equal, detections exact

@@ -1217,6 +1217,29 @@ int rf_preprocess_tile_oriented(rf_handle h, const uint8_t *bgr, int width, int 
 int rf_preprocess_yuv_tile_oriented(rf_handle h, const rf_yuv_frame *frame, int matrix, int orientation, const rf_tiling *t, int tile,
                                     uint8_t *out_net_sized);
 
+/* f25 rotated views in the tracker: f23 / f24's views find the faces of a tilted camera (a body-worn camera, a camera over a bed, a
+ * phone held at an angle), but a tracker fed by the upright letter-box leaks exactly those faces.  A VIEWS tracker detects through
+ * rotated views instead.  Every call of it that runs the detector -- rf_detect_yuv_track_device, rf_detect_yuv_track_best_device,
+ * rf_detect_yuv_redact_device(_style), rf_detect_yuv_redact_lookback_device, and so the key frames of follow, best-follow and
+ * look-back-follow trackers -- detects its frames exactly as
+ *   rf_detect_yuv_views_rotated_device(h, frames, n, matrix, views, nviews, thr, nms, NULL, NULL, NULL, dev_dets, dev_counts, NULL, NULL)
+ * does: *dev_dets / *dev_counts are those records bit for bit (frame pixels; anchor_index / max_faces = the view), they live in the
+ * rotated ring (the call counts as one rotated device call for its validity rule, each of its chunks as one rf_detect_batch_device
+ * call), and out_scales are all 1.  Everything after detection is what the same call does with those records at scale 1: the update,
+ * motion, templates, crops, best shots, redaction and look-back.  The tracker's work runs on the rotated call's home context
+ * (rf_last_stream()), and the rotated ring slot is released only after the tracker's last read of its records.  rf_track_update, the
+ * follow calls, drain, finish and reset run no detector and are unchanged.
+ * Display orientations (f20) apply: the views of a video at orientation o rotate its displayed frames D = T_o(S), so records, tracks,
+ * crops and shots are bit for bit those of the same views tracker on orient_planes(S, o) at orientation 1, and written bytes are that
+ * tracker's, mapped back.  A quarter-turn view of D reads S through one composed EXIF orientation; a warp view reads D through f9's map.
+ * Makes t a views tracker: an option of every kind (plain, best-shot with live shots or following, follow, look-back with search or
+ * following, with or without motion), set before the first frame call, before or after the other setters.  The views are copied.
+ * Statuses, in this order, nothing changed and nothing launched on a refusal: a second call or a call after a frame call
+ * (RF_ERR_INVALID_ARG), views NULL (RF_ERR_INVALID_ARG), nviews outside 1..RF_MAX_VIEWS (RF_ERR_CAPACITY), a non-finite angle or a
+ * shrink outside (0, 1] (RF_ERR_INVALID_ARG, f23's messages), a tiling tracker (RF_ERR_UNSUPPORTED; rf_tracker_set_tiling on a views
+ * tracker is refused so too: tiling a rotated view is not supported). */
+int rf_tracker_set_views(rf_tracker t, const rf_rotated_view *views, int nviews);
+
 /* Introspection. */
 int rf_get_net_size(rf_handle h, int *net_w, int *net_h, int *max_batch, int *max_faces);
 int rf_num_anchors(rf_handle h);            /* per image: 8,232 @448x448, 47,040 @1280x896 */

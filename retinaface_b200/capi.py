@@ -398,6 +398,7 @@ _SIGNATURES = {
     "rf_detect_tiled_oriented": (_I, [_P, _PP, _PI, _PI, _PI, _PI, _I, _TILING, _F, _F, _ALIGN, _P, _P, _P, _P, _P]),
     "rf_detect_tiled_oriented_device": (_I, [_P, _PP, _PI, _PI, _PI, _PI, _I, _TILING, _F, _F, _ALIGN, _P, _P, _PP, _PP]),
     "rf_detect_yuv_tiled_oriented_device": (_I, [_P, _FRAMES, _PI, _I, _I, _TILING, _F, _F, _ALIGN, _P, _P, _PP, _PP]),
+    "rf_tracker_set_views": (_I, [_P, C.POINTER(_RotatedView), _I]),
     "rf_preprocess_tile_oriented": (_I, [_P, _P, _I, _I, _I, _I, _TILING, _I, _P]),
     "rf_preprocess_yuv_tile_oriented": (_I, [_P, _FRAMES, _I, _I, _TILING, _I, _P]),
 }
@@ -1207,7 +1208,7 @@ class Engine:
     def tracker(self, max_videos: int = 1, max_tracks: int = 0, high_thresh: float = 0.0, new_thresh: float = 0.0, iou_high: float = 0.0,
                 iou_low: float = 0.0, iou_tentative: float = 0.0, max_lost: int = 0, best: Optional[dict] = None,
                 motion=None, lookback=None, follow=None, lookback_search=None, lookback_follow=None, tiling=None, best_live=None,
-                best_follow=None) -> "Tracker":
+                best_follow=None, views=None) -> "Tracker":
         """rf_tracker_create: a tracker of max_videos independent sequences on this engine (0 -> the defaults of rf_track_config).
         best (``best_config`` keywords): a best-shot tracker (rf_tracker_create_best), fed through ``Tracker.detect_yuv_best_device``.
         motion (True or ``motion_config`` keywords): camera-motion compensation (rf_tracker_set_motion) from the frames of the
@@ -1221,7 +1222,8 @@ class Engine:
         (rf_tracker_set_tiling), whose detect calls detect through the tiles of ``detect_yuv_tiled_device``.  best_live (True or
         ``set_best_live`` keywords, with best): live shots while tracks live (rf_tracker_set_best_live).  best_follow (True or
         ``set_best_follow`` keywords, with best): a following best-shot tracker (rf_tracker_set_best_follow), whose frames between
-        detections go through ``Tracker.follow_best_device``."""
+        detections go through ``Tracker.follow_best_device``.  views ([(angle, shrink), ...]): a views tracker
+        (rf_tracker_set_views), whose detect calls detect through the rotated views of ``detect_yuv_views_rotated_device``."""
         t = Tracker(self, TrackConfig(max_videos, max_tracks, high_thresh, new_thresh, iou_high, iou_low, iou_tentative, max_lost),
                     best_config(**best) if best is not None else None)
         try:
@@ -1241,6 +1243,8 @@ class Engine:
                 t.set_best_live(**(best_live if isinstance(best_live, dict) else {}))
             if best_follow:
                 t.set_best_follow(**(best_follow if isinstance(best_follow, dict) else {}))
+            if views is not None:
+                t.set_views(views)
         except Exception:
             t.close()
             raise
@@ -1362,6 +1366,7 @@ class Tracker:
         self.lookback_search_on = False
         self.lookback_follow_on = False
         self.tiling_on = False
+        self.views_on = False
         self.best_live_on = False
         self.best_follow_on = False
         self.max_videos = cfg.max_videos
@@ -1612,6 +1617,15 @@ class Tracker:
         t = tiling(levels, overlap)
         self.engine._check(self.lib.rf_tracker_set_tiling(self.t, C.byref(t)))
         self.tiling_on = True
+
+    def set_views(self, views):
+        """rf_tracker_set_views, before the first update: every detect call of this tracker detects its frames through the rotated views
+        [(angle, shrink), ...] of ``Engine.detect_yuv_views_rotated_device`` (the views are copied).  Its records are then in frame
+        pixels (an oriented video's: displayed pixels), anchor_index // max_faces the view, with scales all 1."""
+        views = list(views)
+        varr = (_RotatedView * max(len(views), 1))(*[_RotatedView(float(a), float(s)) for a, s in views])
+        self.engine._check(self.lib.rf_tracker_set_views(self.t, varr, len(views)))
+        self.views_on = True
 
     def set_orientation(self, video: int, orientation: int):
         """rf_tracker_set_orientation: show video (-1: every video) in EXIF orientation 1..8 from its next frame call on, before its

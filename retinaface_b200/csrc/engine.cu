@@ -960,6 +960,7 @@ struct ChunkWork {
     std::vector<LbItemT<Src>> lb;
     std::vector<MergeSource> ms;
     std::vector<WarpItemT<Src>> wp;
+    std::vector<int> wp_bits;          // f25: each warp item's LB_* orientation bits (0: an upright frame)
     std::vector<RotatedSource> rs;
 };
 // One network input of a chunked call: tile `item` of image `image`'s layout, or view `item` of it (f24).
@@ -1024,7 +1025,7 @@ static void detect_chunked(rf_handle h, const Source &source, int n, const Jobs 
             ChunkWork<typename Source::Src> w;
             jobs.fill(&refs[k0], m, src, c.d_frames_in, w);
             CK(launch_letterbox_batch(w.lb.data(), (int)w.lb.size(), Wn, Hn, c.stream));
-            CK(launch_letterbox_warp(w.wp.data(), (int)w.wp.size(), Wn, Hn, c.stream));
+            CK(launch_letterbox_warp(w.wp.data(), (int)w.wp.size(), Wn, Hn, c.stream, w.wp_bits.data()));
             set_params(h, c, thr, nms, c.d_frames_in);
             forward_graph(h, c, m);
             if (wait && in_place) CK(cudaStreamWaitEvent(c.stream, ready, 0));
@@ -1590,20 +1591,23 @@ static void put_view_mat(const RotatedGeometry &g, double *out) {
 }
 
 extern "C++" {
-// View v of image `image` (width x height, stored) into batch slot b, whose input is dst: a quarter turn appends
-// rf_detect_views_oriented's letter-box item and merge source (its slot is b = w.lb.size()), a warp view a warp item and its rotated
-// merge source.  Returns the view's map-back scale: the letter-box's factor, or (float)(1 / f).
+// View v of image `image` into batch slot b, whose input is dst: a quarter turn appends rf_detect_views_oriented's letter-box item and
+// merge source (its slot is b = w.lb.size()), a warp view a warp item and its rotated merge source.  width x height is the image's
+// DISPLAYED size and `orient` its own LB_* bits (0: upright, the stored image; f25: the displayed frame D = T_o(S) of an oriented video):
+// a quarter turn of D reads S through the composed orientation, a warp view reads D through f9's map, and either maps its faces back
+// into D's pixels.  Returns the view's map-back scale: the letter-box's factor, or (float)(1 / f).
 template <typename Src>
-static float rotated_item(rf_handle h, const RotatedGeometry &g, float shrink, int v, int image, Src src, int width, int height, int b,
-                          uint8_t *dst, ChunkWork<Src> &w) {
+static float rotated_item(rf_handle h, const RotatedGeometry &g, float shrink, int v, int image, Src src, int width, int height, int orient,
+                          int b, uint8_t *dst, ChunkWork<Src> &w) {
     const int mf = h->cfg.max_faces;
     if (g.orientation) {
         int bw, bh;
         shrink_box(h, shrink, bw, bh);
         const int bits = lb_orientation_bits(g.orientation);
         const int dw = (bits & LB_TRANSPOSE) ? height : width, dh = (bits & LB_TRANSPOSE) ? width : height;
+        const int read = orient ? lb_orientation_bits(exif_compose(lb_exif(orient), g.orientation)) : bits;
         w.lb.emplace_back();
-        const float scale = letterbox_fill(w.lb.back(), src, dw, dh, dst, bw, bh, bits, (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0);
+        const float scale = letterbox_fill(w.lb.back(), src, dw, dh, dst, bw, bh, read, (h->cfg.flags & RF_FLAG_NPP_RESIZE) ? 1 : 0);
         MergeSource m = (bits & ~LB_FLIP_X) ? oriented_view_source(v, mf, scale, bits, dw, dh) : view_source(v, mf, scale, bits, width);
         m.image = image;
         w.ms.push_back(m);
@@ -1612,6 +1616,7 @@ static float rotated_item(rf_handle h, const RotatedGeometry &g, float shrink, i
     WarpItemT<Src> it{src, width, height, dst, {}};
     std::copy(g.iM, g.iM + 6, it.im);
     w.wp.push_back(it);
+    w.wp_bits.push_back(orient);
     RotatedSource r{b, v * mf, image, {}, 1.0 / (2.0 * g.f)};
     std::copy(g.iM, g.iM + 6, r.im);
     w.rs.push_back(r);
@@ -1660,7 +1665,7 @@ int rf_detect_views_rotated(rf_handle h, const uint8_t *bgr, int width, int heig
             ChunkWork<BgrRows> w;
             for (int b = 0; b < m; b++) {
                 const int v = order[v0 + b];
-                const float scale = rotated_item(h, geo[v], views[v].shrink, v, 0, d_src, width, height, b, h->d_input + (size_t)b * img_bytes, w);
+                const float scale = rotated_item(h, geo[v], views[v].shrink, v, 0, d_src, width, height, 0, b, h->d_input + (size_t)b * img_bytes, w);
                 if (out_view_scales) out_view_scales[v] = scale;
                 if (out_view_mats) put_view_mat(geo[v], out_view_mats + (size_t)v * 6);
             }
@@ -1711,7 +1716,7 @@ static int preprocess_rotated(rf_handle h, const char *who, const Source &src, f
         CK(cudaSetDevice(h->device));
         cudaStream_t s = h->ctx[0].stream;
         ChunkWork<typename Source::Src> w;
-        rotated_item(h, g, shrink, 0, 0, src.upload(h, s, 0, 0), src.width(0), src.height(0), 0, h->d_input, w);
+        rotated_item(h, g, shrink, 0, 0, src.upload(h, s, 0, 0), src.width(0), src.height(0), 0, 0, h->d_input, w);
         CK(launch_letterbox_batch(w.lb.data(), (int)w.lb.size(), Wn, Hn, s));
         CK(launch_letterbox_warp(w.wp.data(), (int)w.wp.size(), Wn, Hn, s));
         CK(cudaMemcpyAsync(h->h_input, h->d_input, (size_t)Hn * Wn * 3, cudaMemcpyDeviceToHost, s));
@@ -1731,7 +1736,8 @@ int rf_preprocess_rotated(rf_handle h, const uint8_t *bgr, int width, int height
 
 // ---- f24 rotated views of device frames (rf_b200.h) -----------------------------------------------------------------------------
 extern "C++" {
-// The jobs of a rotated device call: every view of each frame, geometry geo[i * nviews + v] of frame i's size.  Within a chunk the
+// The jobs of a rotated device call: every view of each frame, geometry geo[i * nviews + v] of frame i's displayed size (f25: an
+// oriented frame's views rotate D = T_o(S)).  Within a chunk the
 // quarter turns take the first slots (launch_merge reads contiguous slots from 0); ids carry the caller's view index, so the slot
 // order does not change a result.  Each job's map-back scale goes to scales[i * nviews + v].
 template <typename Source>
@@ -1751,12 +1757,31 @@ struct RotatedJobs {
                 const Job r = jobs[j];
                 const size_t k = (size_t)r.image * nviews + r.item;
                 if ((geo[k].orientation == 0) != (warp == 1)) continue;
-                scales[k] = rotated_item(h, geo[k], views[r.item].shrink, r.item, r.image, src[r.image], source.width(r.image),
-                                         source.height(r.image), b, input + (size_t)b * img_bytes, w);
+                int dw, dh;
+                displayed_size(source, r.image, dw, dh);
+                scales[k] = rotated_item(h, geo[k], views[r.item].shrink, r.item, r.image, src[r.image], dw, dh, source.bits(r.image), b,
+                                         input + (size_t)b * img_bytes, w);
                 b++;
             }
     }
 };
+
+// The issue of a checked rotated device call of n > 0 frames into the rotated ring: each view's geometry of each frame's displayed
+// size into geo, the map-back scales into scales.
+template <typename Source>
+static void rotated_issue(rf_handle h, const Source &source, int n, const rf_rotated_view *views, int nviews, float thr, float nms,
+                          const AlignArgs *align, const rf_det **dev_dets, const int32_t **dev_counts, cudaEvent_t *free,
+                          std::vector<RotatedGeometry> &geo, std::vector<float> &scales) {
+    geo.resize((size_t)n * nviews);
+    for (int i = 0; i < n; i++) {
+        int dw, dh;
+        displayed_size(source, i, dw, dh);
+        for (int v = 0; v < nviews; v++) geo[(size_t)i * nviews + v] = view_geometry(h, views[v], dw, dh);
+    }
+    scales.resize(geo.size());
+    device_issue(h, h->rotated_slots, h->next_rotated_slot, source, n, RotatedJobs<Source>{h, source, views, nviews, geo, scales.data()}, thr,
+                 nms, align, dev_dets, dev_counts, free);
+}
 
 // rf_detect_views_rotated_device / rf_detect_yuv_views_rotated_device: the checks (the source, the views, then align), then the issue
 // into the rotated ring.
@@ -1765,30 +1790,51 @@ static int detect_rotated_device(rf_handle h, const char *who, const Source &sou
                                  float nms, const rf_align_params *align, void *dev_crops, double *dev_mats, const rf_det **dev_dets,
                                  const int32_t **dev_counts, float *out_view_scales, double *out_view_mats) {
     int rc = source.check(h, who, n);
-    if (rc) return rc;
-    if (!views) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: views is NULL", who));
-    if (nviews < 1 || nviews > RF_MAX_VIEWS)
-        return fail(h, RF_ERR_CAPACITY, fmt("%s: %d views, limit RF_MAX_VIEWS = %d", who, nviews, RF_MAX_VIEWS));
-    for (int v = 0; v < nviews; v++)
-        if ((rc = check_rotated(h, who, views[v].angle, views[v].shrink, v))) return rc;
+    if (rc || (rc = rf_eng::rotated_views_check(h, who, views, nviews))) return rc;
     AlignArgs a;
     if (align && (rc = check_align(h, who, align, n, dev_crops, 0, a))) return rc;
     if (n == 0) return RF_OK;
-    std::vector<RotatedGeometry> geo((size_t)n * nviews);
-    for (int i = 0; i < n; i++)
-        for (int v = 0; v < nviews; v++) geo[(size_t)i * nviews + v] = view_geometry(h, views[v], source.width(i), source.height(i));
-    std::vector<float> scales(geo.size());
+    std::vector<RotatedGeometry> geo;
+    std::vector<float> scales;
     a.crops = dev_crops;
     a.mats = dev_mats;
     try {
-        device_issue(h, h->rotated_slots, h->next_rotated_slot, source, n, RotatedJobs<Source>{h, source, views, nviews, geo, scales.data()},
-                     thr, nms, align ? &a : nullptr, dev_dets, dev_counts, nullptr);
+        rotated_issue(h, source, n, views, nviews, thr, nms, align ? &a : nullptr, dev_dets, dev_counts, nullptr, geo, scales);
     } catch (const CudaFail &f) { return fail_cuda(h, f); }
     if (out_view_scales) std::copy(scales.begin(), scales.end(), out_view_scales);
     if (out_view_mats)
         for (size_t k = 0; k < geo.size(); k++) put_view_mat(geo[k], out_view_mats + k * 6);
     return RF_OK;
 }
+
+// The views of a rotated device call or a views tracker (f25), with f23 / f24's statuses and messages.
+int rf_eng::rotated_views_check(rf_handle h, const char *who, const rf_rotated_view *views, int nviews) {
+    if (!views) return fail(h, RF_ERR_INVALID_ARG, fmt("%s: views is NULL", who));
+    if (nviews < 1 || nviews > RF_MAX_VIEWS)
+        return fail(h, RF_ERR_CAPACITY, fmt("%s: %d views, limit RF_MAX_VIEWS = %d", who, nviews, RF_MAX_VIEWS));
+    for (int v = 0; v < nviews; v++) {
+        const int rc = check_rotated(h, who, views[v].angle, views[v].shrink, v);
+        if (rc) return rc;
+    }
+    return RF_OK;
+}
+
+// rf_detect_yuv_views_rotated_device's check and issue without crops, for the tracker's detect calls (tracker.cu, f25).
+int rf_eng::yuv_rotated_check(rf_handle h, const char *who, const YuvFrames &src, int n, const rf_rotated_view *views, int nviews) {
+    const int rc = src.check(h, who, n);
+    return rc ? rc : rotated_views_check(h, who, views, nviews);
+}
+
+int rf_eng::yuv_rotated_issue(rf_handle h, const YuvFrames &src, int n, const rf_rotated_view *views, int nviews, float thr, float nms,
+                              const rf_det **dev_dets, const int32_t **dev_counts, cudaEvent_t *free) {
+    std::vector<RotatedGeometry> geo;
+    std::vector<float> scales;
+    try {
+        rotated_issue(h, src, n, views, nviews, thr, nms, nullptr, dev_dets, dev_counts, free, geo, scales);
+    } catch (const CudaFail &f) { return fail_cuda(h, f); }
+    return RF_OK;
+}
+
 }  // extern "C++"
 
 int rf_detect_views_rotated_device(rf_handle h, const uint8_t *const *dev_bgr, const int *widths, const int *heights, const int *row_strides,

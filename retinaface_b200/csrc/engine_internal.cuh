@@ -459,5 +459,13 @@ int yuv_tiled_check(rf_handle h, const char *who, const YuvFrames &src, int n, c
 int yuv_tiled_issue(rf_handle h, const YuvFrames &src, int n, const std::vector<std::vector<rf_tile>> &layouts, float thr, float nms,
                     const rf_det **dev_dets, const int32_t **dev_counts, cudaEvent_t *free);
 int tiling_supported(rf_handle h, const char *who);
+// rf_detect_yuv_views_rotated_device without crops, split for the tracker as the tiled call is (f25): the views' own checks (NULL,
+// 1..RF_MAX_VIEWS, each angle and shrink, with f23 / f24's statuses and messages), the check (the frames, then the views) and the issue
+// into the rotated ring on its home context.  A frame of an oriented source (src.oriented) is rotated as it is displayed: its views are
+// those of D = T_o(S), their records in displayed pixels.  *free is the ring slot's event, as yuv_tiled_issue's.
+int rotated_views_check(rf_handle h, const char *who, const rf_rotated_view *views, int nviews);
+int yuv_rotated_check(rf_handle h, const char *who, const YuvFrames &src, int n, const rf_rotated_view *views, int nviews);
+int yuv_rotated_issue(rf_handle h, const YuvFrames &src, int n, const rf_rotated_view *views, int nviews, float thr, float nms,
+                      const rf_det **dev_dets, const int32_t **dev_counts, cudaEvent_t *free);
 
 }  // namespace rf_eng

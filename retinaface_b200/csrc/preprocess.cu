@@ -433,9 +433,14 @@ namespace {
 constexpr int WARP_THREADS = 128, WARP_BAND = 2, WARP_SPAN = WARP_THREADS * 4;
 template <typename Src>
 struct WarpBatch { WarpItemT<Src> v[WARP_MAX_VIEWS]; };
+// f25: the oriented launch's items and their LB_* bits
+template <typename Src>
+struct WarpBatchO { WarpItemT<Src> v[WARP_MAX_VIEWS]; int bits[WARP_MAX_VIEWS]; };
+template <typename Src, bool ORIENTED> using WarpBatchT = typename std::conditional<ORIENTED, WarpBatchO<Src>, WarpBatch<Src>>::type;
 static_assert(sizeof(WarpBatch<BgrRows>) + 8 <= 4096, "warp launch exceeds the classic 4 KB kernel parameter space");
 static_assert(sizeof(WarpItemT<YuvPlanes>) == 104 && sizeof(WarpBatch<YuvPlanes>) + 8 <= 4096,
               "YUV warp launch exceeds the classic 4 KB kernel parameter space");
+static_assert(sizeof(WarpBatchO<YuvPlanes>) + 8 <= 4096, "oriented YUV warp launch exceeds the classic 4 KB kernel parameter space");
 
 // [lo, hi] of the x with a x + b in [-2, n + 1]: the fixed-point source coordinate is within 1/16 pixel of a x + b, and a pixel has a
 // tap in [0, n) only if that coordinate is in [-1, n), so the bound keeps a pixel of margin
@@ -451,8 +456,9 @@ __device__ __forceinline__ void footprint(double a, double b, int n, double &lo,
     hi = fmax(t0, t1);
 }
 
-template <typename Src>
-__global__ void __launch_bounds__(WARP_THREADS) k_letterbox_warp(const __grid_constant__ WarpBatch<Src> B, int net_w, int net_h) {
+// ORIENTED (f25): item z reads the displayed image of its stored source under bits[z] (its w x h displayed), f9's oriented taps.
+template <typename Src, bool ORIENTED>
+__global__ void __launch_bounds__(WARP_THREADS) k_letterbox_warp(const __grid_constant__ WarpBatchT<Src, ORIENTED> B, int net_w, int net_h) {
     __shared__ int s_ax[WARP_SPAN], s_bx[WARP_SPAN], s_x0[WARP_BAND], s_y0[WARP_BAND], s_lo[WARP_BAND], s_hi[WARP_BAND];
     const WarpItemT<Src> &it = B.v[blockIdx.z];
     const int xb = blockIdx.x * WARP_SPAN, yb = blockIdx.y * WARP_BAND;
@@ -479,7 +485,9 @@ __global__ void __launch_bounds__(WARP_THREADS) k_letterbox_warp(const __grid_co
     __syncthreads();
     const int x4 = xb + threadIdx.x * 4;
     if (x4 >= net_w) return;
-    const AlignImageT<Src> img{it.src, it.w, it.h, 1.f, 0};
+    int orient = 0;
+    if constexpr (ORIENTED) orient = B.bits[blockIdx.z];
+    const AlignImageT<Src> img{it.src, it.w, it.h, 1.f, orient};
     // every gather of the band before any store: a store may alias the source for all the compiler knows, so interleaving them would
     // serialise the rows' gathers
     int v[WARP_BAND][4][3] = {};
@@ -489,7 +497,7 @@ __global__ void __launch_bounds__(WARP_THREADS) k_letterbox_warp(const __grid_co
 #pragma unroll
         for (int k = 0; k < 4; k++) {
             const int c = threadIdx.x * 4 + k;
-            sample<false>(img, (s_x0[r] + s_ax[c]) >> 5, (s_y0[r] + s_bx[c]) >> 5, v[r][k]);
+            sample<ORIENTED>(img, (s_x0[r] + s_ax[c]) >> 5, (s_y0[r] + s_bx[c]) >> 5, v[r][k]);
         }
     }
 #pragma unroll
@@ -505,19 +513,35 @@ __global__ void __launch_bounds__(WARP_THREADS) k_letterbox_warp(const __grid_co
 }  // namespace
 
 template <typename Src>
-cudaError_t launch_letterbox_warp(const WarpItemT<Src> *items, int n, int net_w, int net_h, cudaStream_t s) {
+cudaError_t launch_letterbox_warp(const WarpItemT<Src> *items, int n, int net_w, int net_h, cudaStream_t s, const int *bits) {
+    const dim3 block(WARP_THREADS);
     for (int i0 = 0; i0 < n; i0 += WARP_MAX_VIEWS) {
         const int m = std::min(WARP_MAX_VIEWS, n - i0);
-        WarpBatch<Src> B{};
-        for (int i = 0; i < m; i++) B.v[i] = items[i0 + i];
-        k_letterbox_warp<Src><<<dim3((net_w + WARP_SPAN - 1) / WARP_SPAN, (net_h + WARP_BAND - 1) / WARP_BAND, m), WARP_THREADS, 0, s>>>(B, net_w, net_h);
+        const dim3 grid((net_w + WARP_SPAN - 1) / WARP_SPAN, (net_h + WARP_BAND - 1) / WARP_BAND, m);
+        if (bits && std::any_of(bits + i0, bits + i0 + m, [](int b) { return b != 0; })) {
+            // only the tracker's YUV frames are oriented: no BGR path passes bits, and none is compiled
+            if constexpr (std::is_same<Src, YuvPlanes>::value) {
+                WarpBatchO<Src> B{};
+                for (int i = 0; i < m; i++) {
+                    B.v[i] = items[i0 + i];
+                    B.bits[i] = bits[i0 + i];
+                }
+                k_letterbox_warp<Src, true><<<grid, block, 0, s>>>(B, net_w, net_h);
+            } else {
+                return cudaErrorNotSupported;
+            }
+        } else {
+            WarpBatch<Src> B{};
+            for (int i = 0; i < m; i++) B.v[i] = items[i0 + i];
+            k_letterbox_warp<Src, false><<<grid, block, 0, s>>>(B, net_w, net_h);
+        }
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
     }
     return cudaSuccess;
 }
-template cudaError_t launch_letterbox_warp<BgrRows>(const WarpItem *, int, int, int, cudaStream_t);
-template cudaError_t launch_letterbox_warp<YuvPlanes>(const WarpYuvItem *, int, int, int, cudaStream_t);
+template cudaError_t launch_letterbox_warp<BgrRows>(const WarpItem *, int, int, int, cudaStream_t, const int *);
+template cudaError_t launch_letterbox_warp<YuvPlanes>(const WarpYuvItem *, int, int, int, cudaStream_t, const int *);
 
 template float letterbox_fill<BgrRows>(LbItem &, BgrRows, int, int, uint8_t *, int, int, int, int);
 template float letterbox_fill<YuvPlanes>(LbYuvItem &, YuvPlanes, int, int, uint8_t *, int, int, int, int);

@@ -57,6 +57,19 @@ inline int lb_orientation_bits(int o) {
                                 LB_TRANSPOSE | LB_FLIP_X | LB_FLIP_Y, LB_TRANSPOSE | LB_FLIP_Y};
     return o >= 1 && o <= 8 ? bits[o] : -1;
 }
+// LB_* bits -> EXIF orientation 1..8, the inverse of lb_orientation_bits
+inline int lb_exif(int bits) {
+    static const int exif[8] = {1, 2, 4, 3, 5, 6, 8, 7};
+    return exif[bits & 7];
+}
+// f25: the composition of two EXIF transforms, another EXIF transform: T_{exif_compose(inner, outer)}(S) = T_outer(T_inner(S)), so a
+// view in orientation `outer` of a frame displayed in orientation `inner` reads the stored frame through one orientation.  Row
+// inner - 1, column outer - 1 (tests/test_rotated_track_cpu.py checks all 64 pairs against oracle/orient.py).
+constexpr int kExifCompose[8][8] = {
+    {1, 2, 3, 4, 5, 6, 7, 8}, {2, 1, 4, 3, 8, 7, 6, 5}, {3, 4, 1, 2, 7, 8, 5, 6}, {4, 3, 2, 1, 6, 5, 8, 7},
+    {5, 6, 7, 8, 1, 2, 3, 4}, {6, 5, 8, 7, 4, 3, 2, 1}, {7, 8, 5, 6, 3, 4, 1, 2}, {8, 7, 6, 5, 2, 1, 4, 3},
+};
+inline int exif_compose(int inner, int outer) { return kExifCompose[inner - 1][outer - 1]; }
 // whether the orientation bits mirror the image (an odd number of reflections: left and right landmarks trade places)
 __host__ __device__ inline bool lb_mirrored(int bits) { return ((bits & 1) ^ ((bits >> 1) & 1) ^ ((bits >> 2) & 1)) != 0; }
 // u8 BGR rows `pitch` bytes apart, read in place: an upload into a raw buffer (pitch 3 w), a JPEG decode, or a caller's device
@@ -114,8 +127,11 @@ struct WarpItemT {
 using WarpItem = WarpItemT<BgrRows>;
 using WarpYuvItem = WarpItemT<YuvPlanes>;     // f24: each tap converted as the letter-box converts it
 constexpr int WARP_MAX_VIEWS = 16;     // items of one k_letterbox_warp launch
-// k_letterbox_warp: one launch per WARP_MAX_VIEWS items (none for n = 0)
+// k_letterbox_warp: one launch per WARP_MAX_VIEWS items (none for n = 0).  f25: bits (NULL: all 0) gives each item's LB_* orientation;
+// an item with bits reads the DISPLAYED image D = T_o(src) -- its w x h the displayed size, iM of D -- through f9's map, as
+// launch_align_faces(..., oriented) reads it.  A launch with some item oriented runs the oriented instantiation, else the upright one.
+// Only YUV sources have one: BGR items with bits return cudaErrorNotSupported.
 template <typename Src>
-cudaError_t launch_letterbox_warp(const WarpItemT<Src> *items, int n, int net_w, int net_h, cudaStream_t s);
+cudaError_t launch_letterbox_warp(const WarpItemT<Src> *items, int n, int net_w, int net_h, cudaStream_t s, const int *bits = nullptr);
 
 }  // namespace rf

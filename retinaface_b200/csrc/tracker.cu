@@ -1,6 +1,6 @@
 // tracker.cu -- the video tracker behind include/rf_b200.h: f10 tracking, f11 best shots, f13 camera motion, f16 following, f12 / f14
-// redaction, f15 look-back, f17 searching look-back, f18 following look-back, f19 tiling, f20 oriented videos and f22 live and following
-// best shots.  Detection itself is
+// redaction, f15 look-back, f17 searching look-back, f18 following look-back, f19 tiling, f20 oriented videos, f22 live and following
+// best shots and f25 rotated views.  Detection itself is
 // engine.cu's (yuv_device_impl).
 // The entry points take their C linkage from rf_b200.h.
 #include <array>
@@ -109,6 +109,8 @@ struct rf_tracker_s {
     // frame call since its last restart (create, reset, drain, finish), which fixes its orientation until the next one.
     std::vector<int> orient;
     std::vector<char> started;
+    // f25 rotated views: every detect call detects through rf_detect_yuv_views_rotated_device's views (copied).  Empty: off.
+    std::vector<rf_rotated_view> views;
 };
 
 // Whether some video of t is shown in an orientation other than 1.
@@ -258,7 +260,7 @@ int rf_tracker_reset(rf_tracker t, int video) {
 enum class Call {
     UPDATE, DETECT, BEST, FINISH, FOLLOW, LOOKBACK, DRAIN, LOOKBACK_FOLLOW, BEST_FOLLOW,
     SET_MOTION, SET_FOLLOW, SET_LOOKBACK, SET_LOOKBACK_SEARCH, SET_LOOKBACK_FOLLOW, SET_BEST_LIVE, SET_BEST_FOLLOW,
-    SET_TILING,                                                                                        // the setters, SET_MOTION .. here
+    SET_TILING, SET_VIEWS,                                                                             // the setters, SET_MOTION .. here
     MOTION, FOLLOWS, LOOKBACK_SEARCH
 };
 
@@ -313,10 +315,11 @@ static int admit(rf_tracker t, const char *who, Call call) {
         if (why.empty() && t->best_follow) why = "best-shot following is already on";
         break;
     case Call::SET_TILING: if (t->tiled) why = "tiling is already on"; break;
+    case Call::SET_VIEWS: if (!t->views.empty()) why = "rotated views are already on"; break;
     case Call::MOTION: if (!t->motion) why = "motion is off (rf_tracker_set_motion)"; break;
     case Call::LOOKBACK_SEARCH: if (!t->lb_search) why = "not a searching look-back tracker (rf_tracker_set_lookback_search)"; break;
     }
-    if (why.empty() && call >= Call::SET_MOTION && call <= Call::SET_TILING && t->updated) why = "the tracker has already been updated";
+    if (why.empty() && call >= Call::SET_MOTION && call <= Call::SET_VIEWS && t->updated) why = "the tracker has already been updated";
     return why.empty() ? RF_OK : fail(t->h, RF_ERR_INVALID_ARG, fmt("%s: %s", who, why.c_str()));
 }
 
@@ -397,8 +400,8 @@ struct FrameCall {
     std::vector<std::vector<rf_tile>> layouts;         // DETECT on a tiling tracker: each frame's tiles
     std::vector<int> orients;                          // f20: each frame's video's orientation, when `oriented`
     bool oriented = false;                             // some frame of the call is not at orientation 1
-    // set by issue_call: a tiled detect's ring slot event, recorded again once the call has read the records
-    cudaEvent_t tiled_free = nullptr;
+    // set by issue_call: a tiled or rotated detect's ring slot event, recorded again once the call has read the records
+    cudaEvent_t detector_free = nullptr;
 };
 
 static int frame_call(FrameCall &c);
@@ -1733,11 +1736,28 @@ int rf_tracker_set_tiling(rf_tracker t, const rf_tiling *tiling) {
         return fail(h, RF_ERR_UNSUPPORTED, fmt("%s: a video of this tracker is shown in an orientation other than 1 (rf_tracker_set_orientation), "
                                                "and tiled detection has no oriented path", who));
     std::string err;
+    if (!t->views.empty())    // f25, in either order: a rotated view is not tiled
+        return fail(h, RF_ERR_UNSUPPORTED, fmt("%s: this tracker detects through rotated views (rf_tracker_set_views), which are not tiled", who));
     if ((rc = tiling_check(h->cfg.net_w, h->cfg.net_h, tiling, &err))) return fail(h, rc, fmt("%s: %s", who, err.c_str()));
     const bool dflt = !tiling || !tiling->levels || tiling->nlevels == 0;
     t->tile_levels.assign(dflt ? nullptr : tiling->levels, dflt ? nullptr : tiling->levels + tiling->nlevels);
     t->tiling = rf_tiling{t->tile_levels.empty() ? nullptr : t->tile_levels.data(), (int)t->tile_levels.size(), tiling ? tiling->overlap : 0};
     t->tiled = true;
+    return RF_OK;
+}
+
+// ---- f25 rotated views ----------------------------------------------------------------------------------------------------------------
+// An option of any kind: each detect call then takes its records from rf_detect_yuv_views_rotated_device's views (issue_call).  The
+// views are copied; an oriented video's views rotate its displayed frames.
+int rf_tracker_set_views(rf_tracker t, const rf_rotated_view *views, int nviews) {
+    static const char *who = "rf_tracker_set_views";
+    if (!t) return RF_ERR_INVALID_ARG;
+    rf_handle h = t->h;
+    int rc = admit(t, who, Call::SET_VIEWS);
+    if (rc || (rc = rotated_views_check(h, who, views, nviews))) return rc;
+    if (t->tiled)             // in either order: a rotated view is not tiled
+        return fail(h, RF_ERR_UNSUPPORTED, fmt("%s: a tiling tracker (rf_tracker_set_tiling) cannot detect through rotated views", who));
+    t->views.assign(views, views + nviews);
     return RF_OK;
 }
 
@@ -1757,7 +1777,7 @@ int rf_tracker_set_orientation(rf_tracker t, int video, int orientation) {
         if (t->started[v])
             return fail(h, RF_ERR_INVALID_ARG,
                         fmt("%s: video %d has taken a frame call since its last create, reset, drain or finish", who, v));
-    if (orientation != 1 && t->tiled)
+    if (orientation != 1 && t->tiled)      // f25: a views tracker rotates the displayed frames
         return fail(h, RF_ERR_UNSUPPORTED, fmt("%s: a tiling tracker has no oriented detection (rf_tracker_set_tiling)", who));
     std::fill(t->orient.begin() + v0, t->orient.begin() + v1, orientation);
     return RF_OK;
@@ -1788,7 +1808,10 @@ static int check_call(FrameCall &c) {
         return fail(h, RF_ERR_INVALID_ARG, fmt("%s: NULL records or counts", who));
     if (c.source == FrameCall::DETECT) {
         const YuvFrames src = detect_source(c);
-        if ((rc = t->tiled ? yuv_tiled_check(h, who, src, n, &t->tiling, c.layouts) : src.check(h, who, n))) return rc;
+        if (t->tiled) rc = yuv_tiled_check(h, who, src, n, &t->tiling, c.layouts);
+        else if (!t->views.empty()) rc = yuv_rotated_check(h, who, src, n, t->views.data(), (int)t->views.size());
+        else rc = src.check(h, who, n);
+        if (rc) return rc;
     }
     if (c.source == FrameCall::FOLLOW && (rc = check_frames(h, who, c.frames, n, RF_YUV_BT601))) return rc;
     if (c.sink == FrameCall::CROPS && (rc = check_align(h, who, c.align, n, c.crops, 0, c.a))) return rc;
@@ -1802,9 +1825,9 @@ static int check_call(FrameCall &c) {
 
 // Issues a checked frame call of n > 0 frames.  The buffers of the call's look-back videos that have none are allocated before the
 // forward, so that a refusal launches nothing.  Then, on the forward's context (a records or follow call: rf_last_stream's; a tiled
-// detect: the tiled call's home) inside the chain and in the call's ring slot: the update or the follow rounds, the template cut, the
-// chain, the sink -- a look-back call's swap after every kernel that reads an input frame -- and, last, the slot's `free` and a tiled
-// detect's ring slot `free`, recorded again after the last read of its records.
+// or rotated detect: that call's home) inside the chain and in the call's ring slot: the update or the follow rounds, the template cut,
+// the chain, the sink -- a look-back call's swap after every kernel that reads an input frame -- and, last, the slot's `free` and a
+// tiled or rotated detect's detector ring slot `free`, recorded again after the last read of its records.
 static int issue_call(FrameCall &c) {
     rf_tracker t = c.t;
     rf_handle h = t->h;
@@ -1829,7 +1852,11 @@ static int issue_call(FrameCall &c) {
     std::vector<float> scales(n);
     if (c.source == FrameCall::DETECT) {
         if (t->tiled) {      // f19: the tiled ring's records, in frame pixels
-            if ((rc = yuv_tiled_issue(h, src, n, c.layouts, c.thr, c.nms, &c.dets, &c.counts, &c.tiled_free))) return rc;
+            if ((rc = yuv_tiled_issue(h, src, n, c.layouts, c.thr, c.nms, &c.dets, &c.counts, &c.detector_free))) return rc;
+            std::fill(scales.begin(), scales.end(), 1.f);
+        } else if (!t->views.empty()) {      // f25: the rotated ring's records, in (displayed) frame pixels
+            if ((rc = yuv_rotated_issue(h, src, n, t->views.data(), (int)t->views.size(), c.thr, c.nms, &c.dets, &c.counts, &c.detector_free)))
+                return rc;
             std::fill(scales.begin(), scales.end(), 1.f);
         } else if ((rc = yuv_device_impl(h, c.who, src, n, c.thr, c.nms, nullptr, nullptr, nullptr, &c.dets, &c.counts, scales.data()))) {
             return rc;
@@ -1883,7 +1910,7 @@ static int issue_call(FrameCall &c) {
             lb_issue(t, ctx, ring, c, per_frame);
         }
         CK(cudaEventRecord(slot.free, s));
-        if (c.tiled_free) CK(cudaEventRecord(c.tiled_free, s));     // the tiled slot is free once the call has read its records
+        if (c.detector_free) CK(cudaEventRecord(c.detector_free, s));     // the detector's slot is free once the call has read its records
         if (c.tracks) *c.tracks = slot.tracks;
         if (c.track_counts) *c.track_counts = slot.counts;
         if (c.best) *c.best = slot.best;

@@ -203,9 +203,11 @@ class RetinaFace:
             runs.setdefault((p, not det), []).append(i)
         return [(not follow, idx) for (_, follow), idx in sorted(runs.items())]
 
-    def _interval_tracker(self, detect_every: int, best=None, lookback=0, tiling=None, live=None):
+    def _interval_tracker(self, detect_every: int, best=None, lookback=0, tiling=None, live=None, any_angle=None):
         if int(detect_every) < 1:
             raise ValueError(f"detect_every {detect_every}, must be >= 1")
+        if any_angle is not None and tiling:
+            raise ValueError("any_angle and tiling are exclusive: a rotated view is not tiled")
         if live is not None and best is None:
             raise ValueError("live shots need best shots: pass best as well")
         trk = getattr(self, "_tracker", None)
@@ -221,10 +223,17 @@ class RetinaFace:
             raise ValueError("detect_every > 1 needs a follow tracker: this detector's tracker was created without one")
         if tiling and trk is not None and not trk.tiling_on:
             raise ValueError("tiling: this detector's tracker was created without tiling (the first call decides)")
+        if any_angle is not None and trk is not None and not trk.views_on:
+            raise ValueError("any_angle: this detector's tracker was created without rotated views (the first call decides)")
+
+    @staticmethod
+    def _views(any_angle):
+        """The tracker's rotated views of ``any_angle`` (None: none), ``detectAnyAngleFrames``' sweep."""
+        return None if any_angle is None else angle_sweep(any_angle)
 
     def trackFrames(self, frames: Sequence, videos: Sequence[int], threshold: float = 0.5, layout: str = "nv12", matrix: str = "bt601",
                     align: dict = None, max_videos: int = 64, best: dict = None, motion=False, detect_every: int = 1, tiling=None,
-                    live=None):
+                    live=None, any_angle=None):
         """f10 tracking: device 4:2:0 frames (torch CUDA tensors in ``Engine.detect_yuv_device``'s forms), frame i of video
         ``videos[i]``, detected and associated with the tracks of earlier frames on the GPU (rf_detect_yuv_track_device).  Per frame, a
         list of ``(id, state, FaceDetectInfo)`` over every live track (``capi.TRACK_*`` states; the face is the last matched one, in
@@ -255,14 +264,18 @@ class RetinaFace:
         the second list also holds the LIVE shots (reason ``capi.BEST_LIVE``) of tracks that are still live: a first good shot, then
         markedly better ones.  With ``best`` and ``detect_every=k`` > 1 the tracker is a following best-shot tracker: detect frames go
         through rf_detect_yuv_track_best_device, follow frames through rf_track_follow_best_device, whose shots (the EXIT shots of the
-        tracks removed there) are returned as well."""
+        tracks removed there) are returned as well.
+
+        f25 tilted cameras: with ``any_angle=step`` every detect call of the tracker detects through ``detectAnyAngleFrames``' sweep of
+        rotated views (rf_tracker_set_views), so the faces of a tilted body-worn or overhead camera are tracked, with any of the above
+        but ``tiling`` (ValueError).  The first call decides; asking for it on a tracker created without it raises ValueError."""
         if best is not None and align is not None:
             raise ValueError("best shots and new-identity crops are exclusive: pass best or align, not both")
-        self._interval_tracker(detect_every, best=best, tiling=tiling, live=live)
+        self._interval_tracker(detect_every, best=best, tiling=tiling, live=live, any_angle=any_angle)
         if getattr(self, "_tracker", None) is None:
             following = detect_every > 1
             self._tracker = self._new_tracker(max_videos=max_videos, best=best, motion=motion, follow=following and best is None, tiling=tiling,
-                                              best_live=live, best_follow=following and best is not None)
+                                              best_live=live, best_follow=following and best is not None, views=self._views(any_angle))
         if self._tracker.best_follow_on and best is not None:
             tracks, shots = [None] * len(frames), [None] * len(frames)
             for det, idx in self._interval_calls(videos, detect_every):
@@ -331,7 +344,7 @@ class RetinaFace:
     def redactFrames(self, frames: Sequence, videos: Sequence[int] = None, threshold: float = 0.5, blocks: int = 0, margin: float = 0.0,
                      layout: str = "nv12", matrix: str = "bt601", max_videos: int = 64, motion=False, style: str = "mosaic",
                      shape: str = "rect", detail: int = 0, lookback: int = 0, out: Sequence = None, detect_every: int = 1,
-                     lookback_search=False, tiling=None):
+                     lookback_search=False, tiling=None, any_angle=None):
         """f12 redaction: detect on device 4:2:0 frames (torch CUDA tensors in ``Engine.detect_yuv_device``'s forms) and mosaic every
         detected face IN PLACE (rf_detect_yuv_redact_device), ``blocks`` cells across a region's longer side (0: 8; 1: a flat patch),
         each side grown by ``margin`` of the box (0: 0.25).  With ``videos`` (frame i of video ``videos[i]``) the frames are also
@@ -352,14 +365,18 @@ class RetinaFace:
         key frames go through the look-back call and the others through rf_track_follow_redact_lookback_device, and every frame is
         emitted L frames late; with L >= k - 1 a face first detected on a key frame is also covered on the follow frames before it.
         Returns every frame's emitted number in input order.  The first call decides the tracker.
-        f19: ``tiling`` (with ``videos``) as ``trackFrames``: every detect call detects through tiles, with any of the above."""
+        f19: ``tiling`` (with ``videos``) as ``trackFrames``: every detect call detects through tiles, with any of the above.
+        f25: ``any_angle=step`` (with ``videos``) as ``trackFrames``: every detect call detects through rotated views, with any of the
+        above but ``tiling``."""
         kw = dict(layout=layout, matrix=matrix, blocks=blocks, margin=margin, style=style, shape=shape, detail=detail)
         if lookback_search and not lookback:
             raise ValueError("lookback_search needs lookback: the search runs through the look-back buffer")
-        self._interval_tracker(detect_every, lookback=lookback, tiling=tiling)
+        self._interval_tracker(detect_every, lookback=lookback, tiling=tiling, any_angle=any_angle)
         if videos is None:
             if tiling:
                 raise ValueError("tiling needs videos: it is an option of the tracker")
+            if any_angle is not None:
+                raise ValueError("any_angle needs videos: it is an option of the tracker")
             if lookback:
                 raise ValueError("lookback needs videos: the buffered frames belong to a video")
             if detect_every > 1:
@@ -370,7 +387,8 @@ class RetinaFace:
         if getattr(self, "_tracker", None) is None:
             self._tracker = self._new_tracker(max_videos=max_videos, motion=motion, lookback=lookback or None,
                                                 follow=interval and not lookback, lookback_search=lookback_search or None,
-                                                lookback_follow=(interval and lookback) or None, tiling=tiling)
+                                                lookback_follow=(interval and lookback) or None, tiling=tiling,
+                                                views=self._views(any_angle))
         elif lookback_search and not self._tracker.lookback_search_on:
             raise ValueError("lookback_search: this detector's tracker was created without the look-back search (the first call decides)")
         if lookback and self._tracker.lookback_follow_on:

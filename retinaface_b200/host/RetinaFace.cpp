@@ -470,6 +470,11 @@ void RetinaFace::trackerCreated(bool follow) {
         int rc = rf_tracker_set_tiling(tracker_, &t);
         if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_set_tiling: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
     }
+    if (opt_.track_any_angle_step != 0.f) {
+        const vector<rf_rotated_view> views = angleSweep("track_any_angle_step", opt_.track_any_angle_step);
+        int rc = rf_tracker_set_views(tracker_, views.data(), (int)views.size());
+        if (rc != RF_OK) throw std::runtime_error(string("rf_tracker_set_views: ") + rf_status_string(rc) + ": " + rf_last_error(h_));
+    }
     if (follow && opt_.detect_every > 1) {
         const rf_follow_config fc{};
         int rc = rf_tracker_set_follow(tracker_, &fc);

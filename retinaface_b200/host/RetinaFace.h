@@ -53,6 +53,9 @@ struct RetinaFaceOptions {
     vector<float> track_tile_scales;     //   the levels (0: the letter-box); empty: the default pyramid
     bool track_tile_flip = false;        //   each level also mirrored (needs track_tile_scales)
     int track_tile_overlap = 0;          //   pixels neighbouring tiles share (0: 64)
+    float track_any_angle_step = 0.f;    // f25: > 0 makes every detect call of that tracker detect through detectAnyAngleYUV's sweep of
+                                         // rotated views at this step (rf_tracker_set_views), for tilted cameras; 0: off.  Not with
+                                         // track_tiling (rf_tracker_set_views refuses a tiling tracker)
     string cache_file;                   // folded-model cache (the reference's "retina.cache", trtnetbase.cpp:205-243, but with a
                                          // staleness check).  Empty: none
 };
